@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- RGB-D pair frames/sec of the se(3)-TrackNet per-frame hot path on B200.
+"""bench.py -- RGB-D pair frames/sec of the se(3)-TrackNet per-frame hot path on an H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 64] [--precision tf32]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 64] [--precision tf32] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one batch of synthetic input: `batch` (default 64)
@@ -21,6 +21,9 @@ Prints ONE JSON line (rank 0).  Keys beyond the base contract:
   cpu_baseline  the oracle's on_track path (torch CPU + numpy/cv2) timed on this box's host cores
   e2e           same metric through Tracker.on_track_batch with pinned HOST buffers: H2D of the frame,
                 poses, rendered views and D2H of the poses inside every timed step
+--dump-outputs DIR: after the timed steps, the poses the last timed step returned (rank 0's tracks; with N > 1 also every
+                rank's, gathered) as DIR/poses.npy (float64 [batch, 4, 4]) and DIR/poses_all.npy.  The inputs and weights are
+                seeded, so two builds run with the same arguments can be compared output for output.
 --impl reference: the reference's own CPU implementation of the path (oracle restatement: the
 reference code itself cannot travel to the GPU box) on all host threads, bounded sample per step.
 """
@@ -49,6 +52,7 @@ def parse():
     ap.add_argument('--no-render', action='store_true', help='skip the step-with-rendered-input-A measurement')
     ap.add_argument('--no-g21', action='store_true', help='skip the 21-weight-set leg')
     ap.add_argument('--cpu-seconds', type=float, default=12.0)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the last timed step\'s output poses to DIR/*.npy')
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 20 if args.impl == 'reference' else 500
@@ -66,7 +70,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, 'MEASURED_PEAKS.json'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback (B200_PROFILING.md)'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'H100 SXM data sheet (dense bf16, 700 W part; not measured)'
 
 
 class ClockSampler(threading.Thread):
@@ -248,7 +252,7 @@ def main():
     ow = torch.full((nb,), 200.0, dtype=torch.float64, device=dev)
     all_wids = np.tile((np.arange(nb) * G // nb).astype(np.int32), world)       # grouped by id within every rank's slice
     tracker = dist_mod.ShardedTracker(eng, all_wids, synth.CAMERA_K, 200.0, TN, RN, rank, world, args.precision)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     def step(k, gather=True):
         d = sets[k % N_INPUT_SETS][1]
@@ -271,16 +275,22 @@ def main():
     for k in range(max(args.warmup, 3)):
         step(k)
     sync_all()
+    last = None
     for k in range(args.steps):
         flush.zero_()                                   # evict the previous step's lines from L2 (untimed)
         ev[k][0].record()
-        step(k)
+        last = step(k)
         ev[k][1].record()
         launches += eng.last_launch_count()
     # the last step's pose all-gather runs on the side stream: its completion belongs to the timed region too
     tail = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
     tail[0].record(); tracker.wait_gather(); tail[1].record()
     sync_all()
+    if args.dump_outputs and rank == 0 and last is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'poses.npy'), last[0].cpu().numpy().astype(np.float64))
+        if last[1] is not None:
+            np.save(os.path.join(args.dump_outputs, 'poses_all.npy'), last[1].cpu().numpy().astype(np.float64))
     ms_steps = np.array([a.elapsed_time(b) for a, b in ev])
     total_ms = torch.tensor([float(ms_steps.sum()) + tail[0].elapsed_time(tail[1])], device=dev)
     if world > 1:
@@ -309,15 +319,15 @@ def main():
         achieved = nb * FLOP_PER_PAIR / (conv_ms * 1e-3) / 1e12
         if prec == 'tf32':
             peak, executed = (pk['bf16_tflops_sustained'] if (total_ms >= 250.0 and pk.get('bf16_tflops_sustained')) else pk['bf16_tflops']) / 2.0, 1.0
-            note = 'tf32 dense = measured bf16 cuBLAS burst (%s: %.1f TF/s) / 2 (kind::tf32 issues at half the bf16 rate; no tf32 line in the file)' % (pk_src, pk['bf16_tflops'])
+            note = 'tf32 dense = bf16 peak (%s: %.1f TF/s) / 2 (tf32 MMAs issue at half the bf16 rate)' % (pk_src, pk['bf16_tflops'])
         elif prec in ('bf16x3', 'bf16'):
             # burst peak for a short timed region, the sustained (power-capped) one when the kernels run inside a long step loop
             sustained = total_ms >= 250.0 and pk.get('bf16_tflops_sustained')
             peak, executed = (pk['bf16_tflops_sustained'] if sustained else pk['bf16_tflops']), (3.0 if prec == 'bf16x3' else 1.0)
-            note = 'measured bf16 cuBLAS %s (%s; burst %.1f, sustained %.1f; timed region %.0f ms).  bf16x3 executes 3 bf16 products per algorithmic MAC, so the tensor pipe does executed_mult x the algorithmic work' % (
-                'SUSTAINED throughput' if sustained else 'burst', pk_src, pk['bf16_tflops'], pk.get('bf16_tflops_sustained', 0), total_ms)
+            note = 'bf16 %s peak (%s; burst %.1f, sustained %.1f; timed region %.0f ms).  bf16x3 executes 3 bf16 products per algorithmic MAC, so the tensor pipe does executed_mult x the algorithmic work' % (
+                'SUSTAINED' if sustained else 'burst', pk_src, pk['bf16_tflops'], pk.get('bf16_tflops_sustained') or 0.0, total_ms)
         else:
-            peak, executed, note = 75.0, 1.0, 'nominal fp32 FFMA peak (no tensor cores in this mode)'
+            peak, executed, note = 67.0, 1.0, 'H100 SXM data-sheet fp32 FFMA peak (no tensor cores in this mode)'
         return {'bound': 'tensor', 'kernel': 'conv_resident_kernel x8 + conv_trunk_kernel x1 (17 convs, 9 launches/step)' if prec != 'fp32' else 'conv_direct_kernel',
                 'precision': prec, 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak,
                 'executed_mult': executed, 'tensor_pipe_frac': achieved * executed / peak, 'traffic': None,
@@ -328,11 +338,6 @@ def main():
 
     cms, slots = conv_stack_profile(args.precision, min(args.steps, 20))
     roofline = roofline_of(args.precision, cms, slots)
-    tj = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if os.path.exists(tj):            # dram__bytes_read+write per launch from the committed `ncu --set full` capture
-        tr = json.load(open(tj))
-        roofline['traffic'] = tr['dram_bytes_per_launch']
-        roofline['traffic_note'] = 'NOT measured in this run: dram__bytes_read+write per launch from the committed `ncu --set full` capture of this build (%s; %s)' % (tr['kernel'], tr['source'])
 
     # ---- (2b) the other tensor-core modes on the same workload (secondary numbers) -------------------
     alt = {}

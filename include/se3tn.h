@@ -1,4 +1,4 @@
-/* libse3tn -- C ABI of the B200-native se(3)-TrackNet inference hot path.
+/* libse3tn -- C ABI of the H100-native (sm_90a) se(3)-TrackNet inference hot path.
  *
  * The upstream reference (wenbowen123/iros20-6d-pose-tracking @ 18dc5bac) is pure Python and has
  * no FFI of its own; its boundary is the Python class surface (SURVEY.md section 8b).  Each entry
@@ -27,17 +27,17 @@ enum {
     SE3TN_ERR_CUDA = -2,         /* a CUDA runtime / driver call failed               */
     SE3TN_ERR_NOMEM = -3,
     SE3TN_ERR_STATE = -4,        /* e.g. forward before load_weights                  */
-    SE3TN_ERR_UNSUPPORTED = -5   /* device is not sm_100                              */
+    SE3TN_ERR_UNSUPPORTED = -5   /* device is not sm_90                               */
 };
 
 /* Arithmetic of the 17 convolutions (accumulation is always fp32). */
 enum {
-    SE3TN_PREC_TF32 = 0,    /* tcgen05 kind::tf32; operands rounded to tf32 (rna): 10-bit mantissas.  Fastest;
+    SE3TN_PREC_TF32 = 0,    /* wgmma tf32; operands rounded to tf32 (rna): 10-bit mantissas.  Fastest;
                                meets the 1e-3/1e-4 gate only for well-conditioned weights/inputs              */
     SE3TN_PREC_FP32 = 1,    /* plain FFMA direct convolution, no operand rounding (cross-check mode)         */
-    SE3TN_PREC_BF16X3 = 2,  /* tcgen05 kind::f16 on bf16 hi/lo splits, 3 products per MAC: ~2^-16 relative
+    SE3TN_PREC_BF16X3 = 2,  /* wgmma bf16 on bf16 hi/lo splits, 3 products per MAC: ~2^-16 relative
                                error (fp32-faithful for the gate) at 1.5x the tensor time of TF32            */
-    SE3TN_PREC_BF16 = 3     /* tcgen05 kind::f16, bf16 operands, 1 product per MAC (BASELINE configs[2])     */
+    SE3TN_PREC_BF16 = 3     /* wgmma bf16, bf16 operands, 1 product per MAC (BASELINE configs[2])     */
 };
 
 #define SE3TN_IMAGE_SIZE 176           /* reference dataset_info.yml:15 `resolution`          */

@@ -1,11 +1,11 @@
-"""B200-native se(3)-TrackNet inference hot path (Tracker.on_track of
-wenbowen123/iros20-6d-pose-tracking): hand-written sm_100a CUDA behind a C ABI (libse3tn.so),
+"""H100-native se(3)-TrackNet inference hot path (Tracker.on_track of
+wenbowen123/iros20-6d-pose-tracking): hand-written sm_90a CUDA behind a C ABI (libse3tn.so),
 with a Python host layer that mirrors the reference's class surface.
 
     from <this package> import Se3TrackNet, Tracker, TrackDataset, Engine
 
 Importing the package does not touch CUDA; constructing an Engine (directly or through the
-drop-in classes) requires a B200 and the built library -- there is no fallback path.
+drop-in classes) requires an H100 and the built library -- there is no fallback path.
 """
 from .engine import Engine            # noqa: F401
 from . import synth                   # noqa: F401

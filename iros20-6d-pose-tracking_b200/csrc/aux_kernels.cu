@@ -3,6 +3,7 @@
 // R^3 x so(3) pose update / label (K6 / K5).  Each replaces numpy/cv2 CPU code in the reference;
 // the file:line each follows is cited at the kernel.
 #include "aux_kernels.h"
+#include "conv_common.h"
 #include "bbox.cuh"
 #include "ptx.cuh"
 #include <cfloat>
@@ -447,7 +448,7 @@ __device__ __forceinline__ void pose_update_one(const double* A, const float tr[
     for (int k = 0; k < 16; ++k) B[k] = out[k];
 }
 
-// Head on the fused average pool (conv_umma2.cu writes pool_part[image][4 row quadrants][1024] column sums): mean -> Linear -> tanh for
+// Head on the fused average pool (conv_wgmma.cu writes pool_part[image][kPoolSlices][1024] column sums): mean -> Linear -> tanh for
 // BOTH heads of one image per CTA (threads 0-127 translation, 128-255 rotation), and -- when poses_in is given -- the pose update of that
 // track by thread 0 (K4 + K6 in one launch: the update is a 650-instruction fp64 chain per track, pure latency as its own kernel).
 // `zero_words` (nullable): scheduler / dependency counters of the step that just finished, cleared for the next one by block 0.
@@ -465,11 +466,19 @@ head_pooled_kernel(const float4* __restrict__ part, const float* __restrict__ fc
     ptx::grid_dep_wait();
     if (zero_words && blockIdx.x == 0) for (int i = threadIdx.x; i < n_zero; i += blockDim.x) zero_words[i] = 0u;
     if (img_wid) { fcw = fc_table[img_wid[n]]; fcb = fcw + 6 * 512; }
-    const float4* pp = part + static_cast<size_t>(n) * 4 * 256 + head * 128 + t;
-    const float4 a0 = pp[0], a1 = pp[256], a2 = pp[512], a3 = pp[768];
+    static_assert(se3tn::kPoolSlices == 8, "pairwise sum below");
+    const float4* pp = part + static_cast<size_t>(n) * se3tn::kPoolSlices * 256 + head * 128 + t;
+    float4 a[se3tn::kPoolSlices];
+#pragma unroll
+    for (int i = 0; i < se3tn::kPoolSlices; ++i) a[i] = pp[i * 256];
     const float inv = 1.0f / static_cast<float>(npix);
-    const float mx = ((a0.x + a1.x) + (a2.x + a3.x)) * inv, my = ((a0.y + a1.y) + (a2.y + a3.y)) * inv;
-    const float mz = ((a0.z + a1.z) + (a2.z + a3.z)) * inv, mw = ((a0.w + a1.w) + (a2.w + a3.w)) * inv;
+    auto sum8 = [&](float a0, float a1, float a2, float a3, float a4, float a5, float a6, float a7) {
+        return (((a0 + a1) + (a2 + a3)) + ((a4 + a5) + (a6 + a7))) * inv;
+    };
+    const float mx = sum8(a[0].x, a[1].x, a[2].x, a[3].x, a[4].x, a[5].x, a[6].x, a[7].x);
+    const float my = sum8(a[0].y, a[1].y, a[2].y, a[3].y, a[4].y, a[5].y, a[6].y, a[7].y);
+    const float mz = sum8(a[0].z, a[1].z, a[2].z, a[3].z, a[4].z, a[5].z, a[6].z, a[7].z);
+    const float mw = sum8(a[0].w, a[1].w, a[2].w, a[3].w, a[4].w, a[5].w, a[6].w, a[7].w);
     float acc[3];
 #pragma unroll
     for (int o = 0; o < 3; ++o) {
@@ -548,7 +557,7 @@ cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, i
 }
 
 // =============================================================================================
-// Weight preparation for the bf16 modes (conv_umma2.cu PREC_BF16X3 / PREC_BF16).
+// Weight preparation for the bf16 modes (conv_wgmma.cu PREC_BF16X3 / PREC_BF16).
 // Trunk layers, PREC_BF16X3: every 32-word K chunk of a weight row becomes [32 x bf16 hi | 32 x bf16 lo].
 // =============================================================================================
 __global__ void split_weights_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, size_t words)
@@ -578,7 +587,7 @@ cudaError_t launch_to_bf16(const float* src, void* dst, size_t n, cudaStream_t s
     return cudaGetLastError();
 }
 
-// STACK layouts for the resident-weight kernels (conv_umma2.cu): 128 rows, rows 0-63 carry the hi parts, rows 64-127 the lo parts.
+// STACK layouts for the resident-weight kernels (conv_wgmma.cu): 128 rows, rows 0-63 carry the hi parts, rows 64-127 the lo parts.
 // 64-channel 3x3 layers: src [64][9*64] (K-major, tap*64 + c) -> dst [128][9*32 words]; a tap's 128 bytes = 64 bf16 = both chunks.
 __global__ void split_stack_weights_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst)
 {
@@ -606,7 +615,7 @@ __global__ void split_stem_stack_kernel(const float* __restrict__ src, uint8_t* 
         d1[c] = __float2bfloat16_rn(w[c] - __bfloat162float(h)); d1[4 + c] = __float2bfloat16_rn(0.f);
     }
 }
-// Resident 64-channel layers (conv_umma2.cu, 16x256b epilogue): accumulator column 8j + 2m + e of every 32-column block
+// Resident 64-channel layers (conv_wgmma.cu, register-fragment epilogue): accumulator column 8j + 2m + e of every 32-column block
 // must carry output channel 8m + 2j + e, so the weight ROWS are stored in that order.
 __global__ void permute_rows64_kernel(const float* __restrict__ src, float* __restrict__ dst, int ktot)
 {

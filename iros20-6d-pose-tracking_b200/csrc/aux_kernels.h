@@ -40,7 +40,7 @@ cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, i
 cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int round_tf32, cudaStream_t s);
 cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int Win, int C, cudaStream_t s);
 // poses_in non-null: also the pose update of every track (K6 fused into K4); zero_words: n_zero 32-bit counters cleared for the next step
-cudaError_t launch_head_pooled(const float* part /*[n][4][1024]*/, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
+cudaError_t launch_head_pooled(const float* part /*[n][kPoolSlices][1024]*/, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                                int n_img, int npix, const int* img_wid, const float* const* fc_table,
                                const double* poses_in, double* poses_out, float tn, float rn, unsigned* zero_words, int n_zero, cudaStream_t s);
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,

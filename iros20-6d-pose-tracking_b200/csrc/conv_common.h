@@ -9,7 +9,7 @@
 //  * stem: 7 taps (one per filter ROW r), k_per_tap = 32 = 8 pixels x 4 channels of the
 //          zero-padded NHWC4 input starting at x = 2*ox (7 real filter columns + 1 zero column)
 //
-// Two tcgen05 kernels (conv_umma2.cu) cover the 14 launches' worth of layers:
+// Two wgmma kernels (conv_wgmma.cu) cover the 14 launches' worth of layers:
 //  * conv_resident_kernel: Cout = 64 layers (the two stems, the six 64-channel 3x3 convs); the whole weight
 //    matrix lives in shared memory; one launch per layer, static tile ranges.
 //  * conv_trunk_kernel: the Cout >= 256 layers (convAB1, convAB2.*, {trans,rot}_conv1, {trans,rot}_conv2.*) as ONE
@@ -23,12 +23,12 @@
 namespace se3tn {
 
 constexpr int kMaxTaps = 9;
-constexpr int kBlockM = 128;          // UMMA M (TMEM lanes)
+constexpr int kBlockM = 128;          // M tile: two warpgroups x wgmma M = 64
 constexpr int kChunkBytes = 128;      // one SWIZZLE_128B row of K: 32 tf32 words / 32 x [bf16 hi, bf16 lo] / 64 bf16
 
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SELU = 2 };
-enum { KIND_S1 = 0, KIND_S2 = 1, KIND_STEM = 2 };            // conv kinds (compile-time unit tables in conv_umma2.cu)
-enum { PREC_TF32 = 0, PREC_BF16X3 = 1, PREC_BF16 = 2 };      // arithmetic / storage of the tcgen05 kernels
+enum { KIND_S1 = 0, KIND_S2 = 1, KIND_STEM = 2 };            // conv kinds (compile-time unit tables in conv_wgmma.cu)
+enum { PREC_TF32 = 0, PREC_BF16X3 = 1, PREC_BF16 = 2 };      // arithmetic / storage of the wgmma kernels
 // Activation storage per precision: PREC_TF32 fp32 words (tf32-rounded); PREC_BF16X3 the same 4 bytes per channel as
 // [32 x bf16 hi | 32 x bf16 lo] per 32-channel chunk; PREC_BF16 2 bytes per channel, 64 channels per 128-byte chunk
 // (the stem INPUT stays 16 bytes per pixel [4 x hi | 4 x lo] in both bf16 modes).
@@ -61,10 +61,10 @@ struct ConvPtrs {
     float* out;
 };
 
-constexpr int kLayersPerSet = 20;     // stride of the per-set device tables: rows 0..13 the 14 conv layers, rows 14..19 the trunk layers'
-                                      // maps again with 128-row boxes (small-batch trunk tiles; same biases)
+constexpr int kLayersPerSet = 14;     // stride of the per-set device tables: one row per conv layer
+constexpr int kPoolSlices = 8;        // fused average pool: column sums per 16-row slice of the last layer's 11x11 tile (one per consumer warp)
 
-// ---- tcgen05 kernels ----------------------------------------------------------------------------------------
+// ---- wgmma kernels ----------------------------------------------------------------------------------------
 // One layer as the device sees it.  Channel counts are in CHANNELS; byte strides follow from the precision.
 struct LayerDesc {
     CUtensorMap amap[4];   // activation views: S1 one map; S2 four parity views (py*2+px); stem two (even / odd input rows)
@@ -72,7 +72,7 @@ struct LayerDesc {
     const float* bias;     // [groups*cout] fp32 (single-set)
     uint8_t* out;          // NHWC output buffer (image 0)
     const uint8_t* res;    // residual input (nullable), same storage format as out
-    float* pool_part;      // non-null: fused AdaptiveAvgPool2d(1): column sums [image][4 row quadrants][out_c] instead of the activation
+    float* pool_part;      // non-null: fused AdaptiveAvgPool2d(1): column sums [image][kPoolSlices][out_c] instead of the activation
     int kind;              // KIND_*
     int chunks;            // 128-byte K chunks per pixel per group (cin * bytes / 128)
     int cin_words;         // 32-bit words of K per tap per group (weight-matrix K offset of a tap = tap * cin_words)
@@ -86,13 +86,13 @@ struct LayerDesc {
     int act;
     int out_c, out_coff;   // channels per pixel of the output buffer, channel offset of this layer's channel 0
     int res_c;             // channels per pixel of the residual buffer
-    int li;                // row of the per-set tables (layer index; trunk layers with 128-row weight boxes: 14 + layer - 8)
+    int li;                // row of the per-set tables (layer index)
     // trunk scheduling
     int unit_base;         // first global work-unit index of this layer (units are K-split pieces when TrunkParams::ksplit > 1)
     int base_unit0;        // index of this layer's first UNSPLIT unit among all unsplit units of the launch (split-K scratch / counters)
     int units_per_image;   // tiles_x * tiles_y * n_tiles * groups (unsplit)
     int dep_layer;         // index (within the launch) of the layer whose per-image completion this layer waits for; -1: none
-    unsigned dep_target;   // value done[dep_layer][image] reaches when that image is complete (one signal per epilogue warp that finishes part of a unit: 8 x units per image; 16 x in 4-piece latency mode)
+    unsigned dep_target;   // value done[dep_layer][image] reaches when that image is complete (one signal per consumer warp and K piece: 8 x ksplit x units per image)
 };
 
 constexpr int kTrunkMaxLayers = 6;
@@ -112,7 +112,7 @@ struct TrunkParams {
     // round robin so that they are); each piece dumps its fp32 accumulator to `partial`, then finishes ITS share of the unit's
     // 32-column blocks: it waits for the other pieces' dumps, sums all pieces in a fixed order and runs the normal epilogue.  1 = off.
     int ksplit;
-    float* partial;                // [unsplit unit][piece][8 warp slices][32-column block][float4 0..7][row]
+    float* partial;                // [unsplit unit][piece][8 warp slices][32-column block][float4 0..3][lane]
     unsigned* slice_cnt;           // [unsplit unit][8 warp slices] number of pieces that have dumped the slice (zeroed before the launch)
 };
 
@@ -128,9 +128,7 @@ struct ResidentParams {
 };
 
 cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, int num_sms, bool pdl, cudaStream_t stream);
-cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int block_n /*256 | 128*/, int num_sms, bool pdl, cudaStream_t stream);
-// weights-stationary stem (conv_stem_t.cu): bf16 modes, single weight set; wstack = the stem's stacked weight matrix [128][224 words]
-cudaError_t launch_conv_stem_ws(const ResidentParams& p, const void* wstack, int prec, int debug_flags, int num_sms, bool pdl, cudaStream_t stream);
+cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int num_sms, bool pdl, cudaStream_t stream);
 // latency mode: at most kSplitMaxImages images, ksplit = kSplitK pieces, 128-channel units (at most 8 per image and layer)
 constexpr int kSplitMaxImages = 4, kSplitK = 4, kSplitMaxUnits = kSplitMaxImages * 8 * kTrunkMaxLayers;
 // 32-bit words of scheduler state a trunk launch needs: next-unit counter + done[layers][max_batch] + split-K slice counters

@@ -1,7 +1,7 @@
 // Plain fp32 FFMA direct convolution over the same NHWC tensors / packed weights as the
-// tcgen05 path.  Two jobs: (1) the `precision = fp32` mode of se3tn_forward (no operand
+// wgmma path.  Two jobs: (1) the `precision = fp32` mode of se3tn_forward (no operand
 // rounding at all, bit-for-bit independent of the tensor-core path), and (2) an on-device
-// cross-check for the tcgen05 kernel at sizes where a CPU oracle run is slow.
+// cross-check for the wgmma kernels at sizes where a CPU oracle run is slow.
 // 64 pixels x 64 output channels per CTA, 4x4 outputs per thread, K stepped 16 floats at a time.
 #include "conv_common.h"
 #include "ptx.cuh"

@@ -62,12 +62,12 @@ const LayerSpec kLayers[14] = {
     {K_S1,   B_T2,  B_U,   B_P1B,  44,  44,  64,   64,   64, 1,    64,   0, ACT_RELU,  64},   // convB2.conv2 (+id)
     {K_S1,   B_U,   B_T2,  NONE,   44,  44,  64,   64,   64, 1,    64,   0, ACT_RELU,  64},   // convB3.conv1
     {K_S1,   B_T2,  B_CAT, B_U,    44,  44,  64,   64,   64, 1,   128,  64, ACT_RELU,  64},   // convB3.conv2 (+id) -> cat[64:128]
-    {K_S2,   B_CAT, B_F1,  NONE,   44,  44, 128,  128,  256, 1,   256,   0, ACT_SELU, 256},   // convAB1
-    {K_S1,   B_F1,  B_T4,  NONE,   22,  22, 256,  256,  256, 1,   256,   0, ACT_RELU, 256},   // convAB2.conv1
-    {K_S1,   B_T4,  B_F2,  B_F1,   22,  22, 256,  256,  256, 1,   256,   0, ACT_RELU, 256},   // convAB2.conv2 (+id) = 'feature'
-    {K_S2,   B_F2,  B_H1,  NONE,   22,  22, 256,  256, 1024, 1,  1024,   0, ACT_SELU, 256},   // trans_conv1 ++ rot_conv1
-    {K_S1,   B_H1,  B_H2,  NONE,   11,  11, 1024, 512,  512, 2,  1024,   0, ACT_RELU, 256},   // {trans,rot}_conv2.conv1
-    {K_S1,   B_H2,  B_H3,  B_H1,   11,  11, 1024, 512,  512, 2,  1024,   0, ACT_RELU, 256},   // {trans,rot}_conv2.conv2 (+id)
+    {K_S2,   B_CAT, B_F1,  NONE,   44,  44, 128,  128,  256, 1,   256,   0, ACT_SELU, 128},   // convAB1
+    {K_S1,   B_F1,  B_T4,  NONE,   22,  22, 256,  256,  256, 1,   256,   0, ACT_RELU, 128},   // convAB2.conv1
+    {K_S1,   B_T4,  B_F2,  B_F1,   22,  22, 256,  256,  256, 1,   256,   0, ACT_RELU, 128},   // convAB2.conv2 (+id) = 'feature'
+    {K_S2,   B_F2,  B_H1,  NONE,   22,  22, 256,  256, 1024, 1,  1024,   0, ACT_SELU, 128},   // trans_conv1 ++ rot_conv1
+    {K_S1,   B_H1,  B_H2,  NONE,   11,  11, 1024, 512,  512, 2,  1024,   0, ACT_RELU, 128},   // {trans,rot}_conv2.conv1
+    {K_S1,   B_H2,  B_H3,  B_H1,   11,  11, 1024, 512,  512, 2,  1024,   0, ACT_RELU, 128},   // {trans,rot}_conv2.conv2 (+id)
 };
 constexpr int kFirstTrunkLayer = 8;
 
@@ -90,12 +90,12 @@ struct WeightSet {
     float* dev_tf32 = nullptr;      // same layout, conv weights rounded to tf32
     uint8_t* dev_bf16 = nullptr;    // blob-sized: conv weights as [32 bf16 hi | 32 bf16 lo] per 32-word K chunk (PREC_BF16X3 ring layers)
     uint8_t* dev_h = nullptr;       // half-blob-sized: conv weights as plain bf16, K-major (PREC_BF16; layers 2..7 with permuted rows)
-    uint8_t* dev_stack = nullptr;   // 8 x [128][288 words]: resident layers with hi / lo rows stacked along N (conv_umma2.cu STACK)
-    float* dev_perm = nullptr; float* dev_perm_tmp = nullptr;   // 64-channel layers: rows in the 16x256b epilogue's channel order, tf32 words
+    uint8_t* dev_stack = nullptr;   // 8 x [128][288 words]: resident layers with hi / lo rows stacked along N (conv_wgmma.cu STACK)
+    float* dev_perm = nullptr; float* dev_perm_tmp = nullptr;   // 64-channel layers: rows in the accumulator fragment's channel order, tf32 words
     size_t w_off[14], b_off[14];
     size_t fc_off;
     // weight tensor maps per precision: [li] -> the map the kernel of that layer wants
-    CUtensorMap bmap_tf32[kLayersPerSet], bmap_x3[kLayersPerSet], bmap_h[kLayersPerSet];   // rows 14..19: trunk layers with 128-row boxes
+    CUtensorMap bmap_tf32[kLayersPerSet], bmap_x3[kLayersPerSet], bmap_h[kLayersPerSet];
     float mean32[8], std32[8];
     double mean64[8], std64[8];
     int stats_f64 = 0;
@@ -120,16 +120,15 @@ struct se3tn_ctx {
     CUtensorMap amap4[14][4];        // activation views, 4 bytes per channel (TF32 / BF16X3; also the stems' input in every mode)
     CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16, layers 2..13)
     int pdl = 1;                     // SE3TN_PDL=0 disables programmatic dependent launch between the kernels of a step
-    int stem_ws = 0;                 // SE3TN_STEM_WS=1: weights-stationary stem (conv_stem_t.cu); 3 = timing experiment without the pooling epilogue
     std::map<int, MeshDev> meshes;   // CAD models of the rasteriser (device copies), keyed by mesh id
     MeshDev* d_meshes = nullptr; int mesh_rows = 0; bool meshes_dirty = false;
     uint8_t* render_proj = nullptr; uint8_t* render_unif = nullptr; int render_max_nv = 0, render_proj_nv = 0;   // rasteriser workspace
     FillScratch fill = {nullptr, nullptr, nullptr, nullptr}; size_t fill_pixels = 0;   // depth hole-filling scratch (grows on demand)
-    float* pool_part = nullptr;      // [max_batch][4][1024] column sums from the last conv's epilogue
+    float* pool_part = nullptr;      // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     unsigned* sched = nullptr;       // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     float* partial = nullptr;        // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
     bool sched_dirty = false;        // a step failed between the trunk launch and the head launch: clear before the next one
-    unsigned long long* trace = nullptr;   // SE3TN_TRACE=1: [14 slots][256 CTAs][8] globaltimer stamps of the last forward (conv_umma2.cu trace_stamp)
+    unsigned long long* trace = nullptr;   // SE3TN_TRACE=1: [14 slots][256 CTAs][8] globaltimer stamps of the last forward (conv_wgmma.cu trace_stamp)
     EncodeTiledFn encode = nullptr;
     std::map<int, WeightSet> weights;
     // device copies of per-set stats, rebuilt when a set changes: [max_id+1][8]
@@ -238,7 +237,7 @@ int make_map2(se3tn_ctx* c, CUtensorMap* m, const void* base, cuuint64_t inner, 
 
 // Activation-side tensor maps: built once per context (they depend only on the workspace layout).  Boxes are extended
 // by the vertical filter extent so the vertical taps become descriptor row shifts inside one shared-memory tile
-// (conv_umma2.cu).  bpc = bytes per channel of the storage format (stems: always their 16-byte-per-pixel input).
+// (conv_wgmma.cu).  bpc = bytes per channel of the storage format (stems: always their 16-byte-per-pixel input).
 int build_activation_maps(se3tn_ctx* c, int bpc, CUtensorMap (*out)[4]) {
     const cuuint64_t N = static_cast<cuuint64_t>(c->max_batch);
     for (int li = 0; li < 14; ++li) {
@@ -306,11 +305,10 @@ void fill_geom(const LayerSpec& L, int n, ConvGeom& g) {
     g.act = L.act;
 }
 
-// one layer as the tcgen05 kernels see it (conv_common.h LayerDesc)
-void fill_layer_desc(const se3tn_ctx* c, const WeightSet& ws, int li, int kprec, LayerDesc& d, int block_n = 0) {
+// one layer as the wgmma kernels see it (conv_common.h LayerDesc)
+void fill_layer_desc(const se3tn_ctx* c, const WeightSet& ws, int li, int kprec, LayerDesc& d) {
     const LayerSpec& L = kLayers[li];
-    if (!block_n) block_n = L.block_n;
-    const int row = (block_n == L.block_n) ? li : 14 + li - kFirstTrunkLayer;      // table row / weight map with the matching box height
+    const int row = li;                            // row of the per-set tables
     memset(&d, 0, sizeof d);
     const int bpc = prec_bytes_per_channel(kprec);
     const bool stem = (L.kind == K_STEM);
@@ -332,7 +330,7 @@ void fill_layer_desc(const se3tn_ctx* c, const WeightSet& ws, int li, int kprec,
     }
     d.res = (L.res != NONE) ? reinterpret_cast<const uint8_t*>(c->buf[L.res]) : nullptr;
     d.res_c = (L.res != NONE) ? res_channels(L) : 0;
-    d.cout = L.cout; d.groups = L.groups; d.n_tiles = L.cout / block_n;
+    d.cout = L.cout; d.groups = L.groups; d.n_tiles = L.cout / L.block_n;
     d.act = L.act; d.li = row;
     d.units_per_image = d.tiles_x * d.tiles_y * d.n_tiles * d.groups;
     d.dep_layer = -1; d.dep_target = 0; d.unit_base = 0;
@@ -403,7 +401,7 @@ int sync_tables(se3tn_ctx* c, cudaStream_t s) {
             m1[kv.first * kLayersPerSet + li] = kv.second.bmap_tf32[li];
             m2[kv.first * kLayersPerSet + li] = kv.second.bmap_h[li];
             m3[kv.first * kLayersPerSet + li] = kv.second.bmap_x3[li];
-            bias[kv.first * kLayersPerSet + li] = kv.second.dev + kv.second.b_off[li < 14 ? li : kFirstTrunkLayer + li - 14];
+            bias[kv.first * kLayersPerSet + li] = kv.second.dev + kv.second.b_off[li];
         }
         fc[kv.first] = kv.second.dev + kv.second.fc_off;
     }
@@ -473,24 +471,18 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         else { rp.step_x = rp.step_y = 11; rp.off_x = rp.off_y = 0; }
         rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias;
         rp.trace = c->trace ? c->trace + static_cast<size_t>(li) * 256 * 8 : nullptr;
-        if (kLayers[li].kind == K_STEM && c->stem_ws && !img_wid && kprec != PREC_TF32) {
-            ProfScope ps(c, li, s);
-            CU_TRY(c, launch_conv_stem_ws(rp, ws.dev_stack + static_cast<size_t>(li) * 128 * 288 * sizeof(float), kprec, c->stem_ws >> 1, c->num_sms, c->pdl != 0, s));
-        } else { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, kprec, c->num_sms, c->pdl != 0, s)); }
+        { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, kprec, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
         TrunkParams tp;
         memset(&tp, 0, sizeof tp);
-        // work units of 256 output channels; small batches (at most half of the SMs busy per layer otherwise) use 128:
-        // twice the units per layer and half the latency of each -- the layers of one image are a serial chain
-        const int bn = (n * 4 * 2 <= c->num_sms) ? 128 : 256;
         // latency mode: a handful of tracks keep only 8 CTAs per layer busy, and the six layers of an image are a serial chain:
         // cut every unit's K loop into kSplitK pieces (conv_trunk_kernel).  Its fp32 sums are grouped differently, so results agree
         // with the throughput mode to rounding, not bit for bit; within the mode (n = 1..4) they do not depend on n.
         int ksplit = (n <= kSplitMaxImages) ? kSplitK : 1;
         for (int l = 0; l < 14 - kFirstTrunkLayer; ++l) {
-            fill_layer_desc(c, ws, kFirstTrunkLayer + l, kprec, tp.layer[l], bn);
+            fill_layer_desc(c, ws, kFirstTrunkLayer + l, kprec, tp.layer[l]);
             while (tp.layer[l].chunks % ksplit) ksplit /= 2;       // 2-byte storage: convAB1 has only two 128-byte chunks per pixel
         }
         int base = 0, base0 = 0;
@@ -498,8 +490,8 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
             LayerDesc& d = tp.layer[l];
             d.unit_base = base; base += n * d.units_per_image * ksplit;
             d.base_unit0 = base0; base0 += n * d.units_per_image;
-            // completion signals per unit: one per epilogue warp that finishes part of it (8; in 4-piece latency mode 4 warps of each piece finish one block each)
-            if (l > 0) { d.dep_layer = l - 1; d.dep_target = (ksplit == 4 ? 16u : 8u) * static_cast<unsigned>(tp.layer[l - 1].units_per_image); }
+            // completion signals per unit: one per consumer warp of every K piece (each piece finishes 4 / ksplit of every warp's 32-column blocks)
+            if (l > 0) { d.dep_layer = l - 1; d.dep_target = 8u * static_cast<unsigned>(ksplit) * static_cast<unsigned>(tp.layer[l - 1].units_per_image); }
         }
         if (ksplit > 1 && base0 > kSplitMaxUnits) return fail(c, SE3TN_ERR_STATE, "split-K scratch too small");
         tp.ksplit = ksplit; tp.partial = c->partial;
@@ -510,12 +502,12 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         tp.sched = c->sched; tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias;
         tp.trace = c->trace ? c->trace + static_cast<size_t>(kFirstTrunkLayer) * 256 * 8 : nullptr;
         c->sched_dirty = true;                     // cleared again by the head kernel below
-        { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, kprec, bn, c->num_sms, c->pdl != 0, s)); }
+        { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, kprec, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
         ProfScope ps(c, 16, s);
-        CU_TRY(c, launch_head_pooled(c->pool_part + static_cast<size_t>(first) * 4 * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
+        CU_TRY(c, launch_head_pooled(c->pool_part + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
                                      img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc : nullptr,
                                      pose ? pose->in : nullptr, pose ? pose->out : nullptr, pose ? pose->tn : 0.f, pose ? pose->rn : 0.f,
                                      c->sched, static_cast<int>(trunk_sched_words(c->max_batch)), s));
@@ -551,15 +543,14 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
         return fail(nullptr, SE3TN_ERR_CUDA, std::string("se3tn_create: no such CUDA device: ") + cudaGetErrorString(e));
     cudaDeviceProp prop;
     CU_TRY(nullptr, cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
         return fail(nullptr, SE3TN_ERR_UNSUPPORTED, "se3tn_create: device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
-                                                    ", this library is sm_100a only (no fallback path)");
+                                                    ", this library is sm_90a only (no fallback path)");
     DeviceGuard guard(device);
     se3tn_ctx* c = new se3tn_ctx();
     c->device = device; c->max_batch = max_batch; c->num_sms = prop.multiProcessorCount;
     if (const char* ov = getenv("SE3TN_PDL")) c->pdl = atoi(ov) != 0;
     if (const char* ov = getenv("SE3TN_GRAPH")) c->use_graphs = atoi(ov) != 0;
-    if (const char* ov = getenv("SE3TN_STEM_WS")) c->stem_ws = atoi(ov);
     if (const char* ov = getenv("SE3TN_TRACE")) {
         if (atoi(ov) != 0 && cudaMalloc(&c->trace, SE3TN_TRACE_WORDS * sizeof(unsigned long long)) == cudaSuccess) cudaMemset(c->trace, 0, SE3TN_TRACE_WORDS * sizeof(unsigned long long));
     }
@@ -580,7 +571,7 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
         if (e != cudaSuccess) { delete c; return fail(nullptr, SE3TN_ERR_NOMEM, std::string("se3tn_create: cudaMalloc(workspace): ") + cudaGetErrorString(e)); }
         c->own_workspace = true;
     }
-    e = cudaMalloc(&c->pool_part, static_cast<size_t>(max_batch) * 4 * 1024 * sizeof(float));
+    e = cudaMalloc(&c->pool_part, static_cast<size_t>(max_batch) * kPoolSlices * 1024 * sizeof(float));
     if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); se3tn_destroy(c); return fail(nullptr, SE3TN_ERR_NOMEM, "se3tn_create: pool buffer: " + m); }
     e = cudaMalloc(&c->partial, trunk_partial_floats() * sizeof(float));
     if (e == cudaSuccess) e = cudaMalloc(&c->sched, trunk_sched_words(max_batch) * sizeof(unsigned));
@@ -653,23 +644,18 @@ int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_
         char what[64];
         int rc = SE3TN_OK;
         if (li >= kFirstTrunkLayer) {
-            // trunk layers: natural row order, tiles of {32 words, 256 rows} streamed through the weight ring
+            // trunk layers: natural row order, tiles of {32 words, block_n rows} streamed through the weight ring
             snprintf(what, sizeof what, "layer %d weights", li);
-            rc = make_map2(c, &ws.bmap_tf32[li], ws.dev_tf32 + ws.w_off[li], layer_ktot(L), layer_rows(L), 256, what);
+            rc = make_map2(c, &ws.bmap_tf32[li], ws.dev_tf32 + ws.w_off[li], layer_ktot(L), layer_rows(L), L.block_n, what);
             uint8_t* d3 = ws.dev_bf16 + ws.w_off[li] * sizeof(float);
             CU_TRY(c, launch_split_weights(wsrc, d3, words, 0));                          // [32 hi | 32 lo] per 32-word K chunk
-            if (!rc) rc = make_map2(c, &ws.bmap_x3[li], d3, layer_ktot(L), layer_rows(L), 256, what);
+            if (!rc) rc = make_map2(c, &ws.bmap_x3[li], d3, layer_ktot(L), layer_rows(L), L.block_n, what);
             uint8_t* dh = ws.dev_h + ws.w_off[li] * sizeof(uint16_t);
             CU_TRY(c, launch_to_bf16(wsrc, dh, words, 0));                                // plain bf16, 64 channels per 128-byte chunk
-            if (!rc) rc = make_map2(c, &ws.bmap_h[li], dh, layer_ktot(L) / 2, layer_rows(L), 256, what);
-            // the same matrices in 128-row boxes: small batches run the trunk with 128-channel work units (twice the units per layer)
-            const int ls = 14 + li - kFirstTrunkLayer;
-            if (!rc) rc = make_map2(c, &ws.bmap_tf32[ls], ws.dev_tf32 + ws.w_off[li], layer_ktot(L), layer_rows(L), 128, what);
-            if (!rc) rc = make_map2(c, &ws.bmap_x3[ls], d3, layer_ktot(L), layer_rows(L), 128, what);
-            if (!rc) rc = make_map2(c, &ws.bmap_h[ls], dh, layer_ktot(L) / 2, layer_rows(L), 128, what);
+            if (!rc) rc = make_map2(c, &ws.bmap_h[li], dh, layer_ktot(L) / 2, layer_rows(L), L.block_n, what);
         } else {
             // resident-weight layers.  Stems keep the natural row order; the 64-channel 3x3 layers use the row order of the
-            // 16x256b epilogue (all precisions).  bf16 modes: hi / lo rows stacked along N, except the 64-channel layers in PREC_BF16.
+            // accumulator fragment (all precisions).  bf16 modes: hi / lo rows stacked along N, except the 64-channel layers in PREC_BF16.
             const bool stem = (L.kind == K_STEM);
             const float* w_tf32 = ws.dev_tf32 + ws.w_off[li];
             if (!stem) {

@@ -26,7 +26,7 @@ def _stream(device):
 class Engine:
     def __init__(self, max_batch=64, device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError('se3tn Engine needs a CUDA device (sm_100a); there is no CPU fallback')
+            raise RuntimeError('se3tn Engine needs a CUDA device (sm_90a); there is no CPU fallback')
         self.lib = _lib.load()
         self.device = torch.device('cuda', torch.cuda.current_device() if device is None else
                                    (device.index if isinstance(device, torch.device) else int(device)))

@@ -1,5 +1,5 @@
 """Drop-in for the reference's se3_tracknet.py: same class name, constructor, load_state_dict /
-cuda / eval / __call__ surface and output dict -- but forward() runs the hand-written sm_100a
+cuda / eval / __call__ surface and output dict -- but forward() runs the hand-written sm_90a
 kernels of libse3tn through the C ABI instead of torch.nn -> cuDNN.
 
 Reference: se3_tracknet.py:52-112 (Se3TrackNet), network_modules.py:59-66,86-120.
@@ -47,7 +47,7 @@ class Se3TrackNet(torch.nn.Module):
         dev = args[0] if args else kwargs.get('device')
         if dev is not None and torch.device(dev).type == 'cuda':
             return self.cuda(torch.device(dev).index)
-        raise RuntimeError('Se3TrackNet (B200) only lives on a CUDA device; there is no CPU path')
+        raise RuntimeError('Se3TrackNet (H100) only lives on a CUDA device; there is no CPU path')
 
     def train(self, mode=True):
         if mode:

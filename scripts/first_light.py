@@ -11,7 +11,7 @@ import se3_oracle as O
 
 BUFS = ['X0A','X0B','Y1A','Y1B','P1A','P1B','T1','T2','U','CAT','F1','T4','F2','H1','H2','H3']
 N = int(sys.argv[1]) if len(sys.argv) > 1 else 2
-MODE = sys.argv[2] if len(sys.argv) > 2 else 'all'   # 'base' = everything but tcgen05, 'tc' = tcgen05 only
+MODE = sys.argv[2] if len(sys.argv) > 2 else 'all'   # 'base' = everything but the tensor-core convs, 'tc' = tensor-core convs only
 dev = torch.device('cuda:0')
 print(torch.cuda.get_device_name(0), torch.cuda.get_device_capability(0))
 eng = pkg.Engine(max_batch=max(N, 64))
@@ -54,7 +54,7 @@ try:
     if MODE == 'base': raise SystemExit
     t, r, f = eng.forward(Ad, Bd, precision='tf32', want_feature=True)
     torch.cuda.synchronize()
-    report('tf32 tcgen05 path vs oracle', t, r)
+    report('tf32 wgmma path vs oracle', t, r)
     for i, name in enumerate(BUFS):
         cur = eng.debug_buffer(i, N)
         if name in snap:
