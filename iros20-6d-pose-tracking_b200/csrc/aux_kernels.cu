@@ -6,8 +6,8 @@
 #include "conv_common.h"
 #include "bbox.cuh"
 #include "ptx.cuh"
+#include "storage.cuh"
 #include <cfloat>
-#include <cuda_bf16.h>
 
 namespace se3tn {
 
@@ -24,21 +24,6 @@ namespace se3tn {
 //         mean/std are float32 arrays (what train.py:121-125 saves), float64 otherwise.
 // pack:   reference data_augmentation.py:179-189 builds CHW float32; here the result goes straight
 //         into the stem conv's zero-padded NHWC4 layout (and optionally to NCHW for the drop-in API).
-
-// conv-input storage modes: 0 raw fp32, 1 fp32 words rounded to tf32, 2 per pixel [4 x bf16 hi | 4 x bf16 lo]
-__device__ __forceinline__ float4 pack_stem_pixel(float4 v, int mode) {
-    if (mode == 1) return make_float4(ptx::to_tf32(v.x), ptx::to_tf32(v.y), ptx::to_tf32(v.z), ptx::to_tf32(v.w));
-    if (mode == 2) {
-        const __nv_bfloat162 h01 = __floats2bfloat162_rn(v.x, v.y), h23 = __floats2bfloat162_rn(v.z, v.w);
-        const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
-        const __nv_bfloat162 l01 = __floats2bfloat162_rn(v.x - f01.x, v.y - f01.y), l23 = __floats2bfloat162_rn(v.z - f23.x, v.w - f23.y);
-        float4 o;
-        o.x = __uint_as_float(*reinterpret_cast<const uint32_t*>(&h01)); o.y = __uint_as_float(*reinterpret_cast<const uint32_t*>(&h23));
-        o.z = __uint_as_float(*reinterpret_cast<const uint32_t*>(&l01)); o.w = __uint_as_float(*reinterpret_cast<const uint32_t*>(&l23));
-        return o;
-    }
-    return v;
-}
 
 __device__ __forceinline__ float norm_f32(float x, float m, float s) { return __fdiv_rn(__fsub_rn(x, m), s); }
 __device__ __forceinline__ float norm_f64(float x, double m, double s) { return static_cast<float>(__ddiv_rn(__dsub_rn(static_cast<double>(x), m), s)); }
@@ -173,8 +158,8 @@ preprocess_kernel(PreprocessArgs a, int rows_per_cta)
             }
             if (a.stemA) {
                 const size_t so = (static_cast<size_t>(n) * kStemH + (y + 3)) * kStemW + (x + 3);
-                reinterpret_cast<float4*>(a.stemA)[so] = pack_stem_pixel(vA, a.round_tf32);
-                reinterpret_cast<float4*>(a.stemB)[so] = pack_stem_pixel(vB, a.round_tf32);
+                reinterpret_cast<float4*>(a.stemA)[so] = encode_stem_pixel(vA, a.precision);
+                reinterpret_cast<float4*>(a.stemB)[so] = encode_stem_pixel(vB, a.precision);
             }
         }
     }
@@ -275,7 +260,7 @@ cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, i
 // NCHW float32 (N,4,176,176) -> zero-padded NHWC4 stem input (for Se3TrackNet.forward(A, B))
 // =============================================================================================
 __global__ void __launch_bounds__(256)
-nchw_to_stem_kernel(const float* __restrict__ src, float* __restrict__ dst, int round_tf32)
+nchw_to_stem_kernel(const float* __restrict__ src, float* __restrict__ dst, int precision)
 {
     const int n = blockIdx.y;
     const int pix = blockIdx.x * blockDim.x + threadIdx.x;
@@ -283,14 +268,14 @@ nchw_to_stem_kernel(const float* __restrict__ src, float* __restrict__ dst, int 
     const int y = pix / kImg, x = pix - y * kImg;
     const float* s = src + static_cast<size_t>(n) * 4 * kImg * kImg + pix;
     float4 v = make_float4(s[0], s[kImg * kImg], s[2 * kImg * kImg], s[3 * kImg * kImg]);
-    v = pack_stem_pixel(v, round_tf32);
+    v = encode_stem_pixel(v, precision);
     reinterpret_cast<float4*>(dst)[(static_cast<size_t>(n) * kStemH + (y + 3)) * kStemW + (x + 3)] = v;
 }
 
-cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int round_tf32, cudaStream_t s) {
+cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     dim3 grid((kImg * kImg + 255) / 256, n);
-    nchw_to_stem_kernel<<<grid, 256, 0, s>>>(src, dst, round_tf32);
+    nchw_to_stem_kernel<<<grid, 256, 0, s>>>(src, dst, precision);
     return cudaGetLastError();
 }
 
@@ -335,14 +320,13 @@ cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int 
 }
 
 // =============================================================================================
-// K4 head: AdaptiveAvgPool2d(1) + Linear(512,3) + Tanh for both heads
-// (reference se3_tracknet.py:100-102, 107-109).  x: NHWC (N, 11*11, 1024): channels [0,512) are
-// the translation head, [512,1024) the rotation head.  One CTA (256 threads x 4 channels) per image.
+// K4 head of the fp32 FFMA mode: AdaptiveAvgPool2d(1) + Linear(512,3) + Tanh for both heads
+// (reference se3_tracknet.py:100-102, 107-109).  x: fp32 NHWC (N, 11*11, 1024): channels [0,512) are
+// the translation head, [512,1024) the rotation head.
 // =============================================================================================
 __global__ void __launch_bounds__(512)
 head_kernel(const float4* __restrict__ x, const float* __restrict__ fcw /*[6][512]*/, const float* __restrict__ fcb /*[6]*/,
-            float* __restrict__ out_trans, float* __restrict__ out_rot, int npix, int split_bf16,
-            const int* __restrict__ img_wid, const float* const* __restrict__ fc_table)
+            float* __restrict__ out_trans, float* __restrict__ out_rot, int npix)
 {
     // grid (n, 2): blockIdx.y = head (0 trans: channels 0..511, 1 rot: 512..1023).  512 threads =
     // 4 pixel groups x 128 threads, each thread 4 channels.
@@ -353,24 +337,11 @@ head_kernel(const float4* __restrict__ x, const float* __restrict__ fcw /*[6][51
     const int cq = t & 127, pg = t >> 7;
     const int c = head * 512 + cq * 4;                 // first of this thread's 4 channels
     ptx::grid_dep_wait();
-    if (img_wid) { fcw = fc_table[img_wid[n]]; fcb = fcw + 6 * 512; }    // per-object head weights
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!split_bf16) {
-        const float4* xp = x + static_cast<size_t>(n) * npix * 256 + (c >> 2);
-        for (int p = pg; p < npix; p += 4) {
-            const float4 v = __ldg(xp + static_cast<size_t>(p) * 256);
-            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-        }
-    } else {
-        // channels c..c+3 live in chunk c/32 as bf16 hi at byte (c%32)*2 and lo 64 bytes further
-        const uint8_t* xb = reinterpret_cast<const uint8_t*>(x) + static_cast<size_t>(n) * npix * 4096 + (c >> 5) * 128 + (c & 31) * 2;
-        for (int p = pg; p < npix; p += 4) {
-            const uint2 h = __ldg(reinterpret_cast<const uint2*>(xb + static_cast<size_t>(p) * 4096));
-            const uint2 l = __ldg(reinterpret_cast<const uint2*>(xb + static_cast<size_t>(p) * 4096 + 64));
-            const float2 h0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&h.x)), h1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&h.y));
-            const float2 l0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&l.x)), l1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&l.y));
-            s.x += h0.x + l0.x; s.y += h0.y + l0.y; s.z += h1.x + l1.x; s.w += h1.y + l1.y;
-        }
+    const float4* xp = x + static_cast<size_t>(n) * npix * 256 + (c >> 2);
+    for (int p = pg; p < npix; p += 4) {
+        const float4 v = __ldg(xp + static_cast<size_t>(p) * 256);
+        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
     }
     part4[pg][cq] = s;
     __syncthreads();
@@ -511,109 +482,117 @@ cudaError_t launch_head_pooled(const float* part, const float* fcw, const float*
 }
 
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
-                        int n_img, int npix, int split_bf16, const int* img_wid, const float* const* fc_table, cudaStream_t s) {
+                        int n_img, int npix, cudaStream_t s) {
     if (n_img <= 0) return cudaSuccess;
     const float4* x4 = reinterpret_cast<const float4*>(x);
-    void* args[] = {&x4, &fcw, &fcb, &out_trans, &out_rot, &npix, &split_bf16, &img_wid, &fc_table};
+    void* args[] = {&x4, &fcw, &fcb, &out_trans, &out_rot, &npix};
     return launch_pdl(reinterpret_cast<const void*>(head_kernel), dim3(n_img, 2), dim3(512), args, s);
 }
 
 // =============================================================================================
 // NHWC -> NCHW (the 'feature' entry of the reference's output dict, se3_tracknet.py:96)
 // =============================================================================================
-// storage: 0 fp32 words, 1 [32 x bf16 hi | 32 x bf16 lo] per 32-channel chunk, 2 plain bf16 (conv_common.h)
+// in: the storage format of PREC (storage.cuh), C % 4 == 0.  One CTA transposes 32 pixels x 32 channels.
+template <int PREC>
 __global__ void __launch_bounds__(256)
-nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int HW, int C, int storage)
+nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int HW, int C)
 {
+    using R = Raw<PREC, 4>;
     __shared__ float tile[32][33];
     const int n = blockIdx.z;
     const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;    // 32 x 8
-    for (int j = ty; j < 32; j += 8) {
-        const int p = p0 + j, c = c0 + tx;
-        float val = 0.f;
+    {
+        const int j = threadIdx.x >> 3, g = threadIdx.x & 7;    // pixel p0 + j, channels c0 + 4g .. + 3
+        const int p = p0 + j, c = c0 + 4 * g;
+        float v[4] = {0.f, 0.f, 0.f, 0.f};
         if (p < HW && c < C) {
-            const size_t pix = static_cast<size_t>(n) * HW + p;
-            if (storage == 0) val = reinterpret_cast<const float*>(in)[pix * C + c];
-            else if (storage == 1) {
-                const uint8_t* cb = in + (pix * C + (c & ~31)) * 4 + (c & 31) * 2;
-                val = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(cb)) + __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(cb + 64));
-            } else val = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(in)[pix * C + c]);
+            const uint8_t* src = in + Storage<PREC>::addr(static_cast<size_t>(n) * HW + p, C, c);
+            R r;
+#pragma unroll
+            for (int q = 0; q < R::kPieces; ++q) r.set(q, *R::at(src, q));
+            Storage<PREC>::decode(r, v);
         }
-        tile[j][tx] = val;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) tile[j][4 * g + e] = v[e];
     }
     __syncthreads();
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;    // 32 x 8
     for (int j = ty; j < 32; j += 8) {
         const int c = c0 + j, p = p0 + tx;
         if (p < HW && c < C) out[(static_cast<size_t>(n) * C + c) * HW + p] = tile[tx][j];
     }
 }
 
-cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int storage, cudaStream_t s) {
+cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s) {
     if (n_img <= 0) return cudaSuccess;
+    if (C % 4) return cudaErrorInvalidValue;
     dim3 grid((HW + 31) / 32, (C + 31) / 32, n_img);
-    nhwc_to_nchw_kernel<<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(in), out, HW, C, storage);
-    return cudaGetLastError();
-}
-
-// =============================================================================================
-// Weight preparation for the bf16 modes (conv_wgmma.cu PREC_BF16X3 / PREC_BF16).
-// Trunk layers, PREC_BF16X3: every 32-word K chunk of a weight row becomes [32 x bf16 hi | 32 x bf16 lo].
-// =============================================================================================
-__global__ void split_weights_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, size_t words)
-{
-    size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (; i < words; i += stride) {
-        const float v = src[i];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
-        const size_t chunk = i >> 5, j = i & 31;
-        *reinterpret_cast<__nv_bfloat16*>(dst + chunk * 128 + j * 2) = h;
-        *reinterpret_cast<__nv_bfloat16*>(dst + chunk * 128 + 64 + j * 2) = l;
+    const uint8_t* src = static_cast<const uint8_t*>(in);
+    switch (precision) {
+        case SE3TN_PREC_FP32:            // plain fp32 words decode like tf32 ones
+        case SE3TN_PREC_TF32:   nhwc_to_nchw_kernel<SE3TN_PREC_TF32><<<grid, 256, 0, s>>>(src, out, HW, C); break;
+        case SE3TN_PREC_BF16X3: nhwc_to_nchw_kernel<SE3TN_PREC_BF16X3><<<grid, 256, 0, s>>>(src, out, HW, C); break;
+        case SE3TN_PREC_BF16:   nhwc_to_nchw_kernel<SE3TN_PREC_BF16><<<grid, 256, 0, s>>>(src, out, HW, C); break;
+        default: return cudaErrorInvalidValue;
     }
-}
-
-// plain bf16 copy of a K-major weight matrix (PREC_BF16: 64 channels per 128-byte K chunk)
-__global__ void to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, size_t n)
-{
-    size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (; i < n; i += stride) dst[i] = __float2bfloat16_rn(src[i]);
-}
-cudaError_t launch_to_bf16(const float* src, void* dst, size_t n, cudaStream_t s) {
-    if (!n) return cudaSuccess;
-    to_bf16_kernel<<<1024, 256, 0, s>>>(src, static_cast<__nv_bfloat16*>(dst), n);
     return cudaGetLastError();
 }
 
-// STACK layouts for the resident-weight kernels (conv_wgmma.cu): 128 rows, rows 0-63 carry the hi parts, rows 64-127 the lo parts.
+// =============================================================================================
+// Weight preparation for the tensor-core modes (conv_wgmma.cu): the fp32 K-major matrices in the storage formats of
+// storage.cuh, a weight row being a "pixel" of ktot channels.
+// =============================================================================================
+template <int PREC>
+__global__ void encode_weights_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, int rows, int ktot)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;      // one thread per 4 K words of a row
+    if (i >= rows * (ktot / 4)) return;
+    const int row = i / (ktot / 4), k = (i - row * (ktot / 4)) * 4;
+    const float* w = src + static_cast<size_t>(row) * ktot + k;
+    const float v[4] = {w[0], w[1], w[2], w[3]};
+    Storage<PREC>::encode(v).store(dst + Storage<PREC>::addr(row, ktot, k));
+}
+cudaError_t launch_encode_weights(int precision, const float* src, void* dst, int rows, int ktot, cudaStream_t s) {
+    if (rows <= 0 || ktot <= 0 || ktot % 32) return cudaErrorInvalidValue;
+    const int blocks = (rows * (ktot / 4) + 255) / 256;
+    uint8_t* d = static_cast<uint8_t*>(dst);
+    switch (precision) {
+        case SE3TN_PREC_TF32:   encode_weights_kernel<SE3TN_PREC_TF32><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
+        case SE3TN_PREC_BF16X3: encode_weights_kernel<SE3TN_PREC_BF16X3><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
+        case SE3TN_PREC_BF16:   encode_weights_kernel<SE3TN_PREC_BF16><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+// STACK layouts for the resident-weight kernels (conv_wgmma.cu): the bf16x3 split as 128 rows, rows 0-63 the hi parts, rows 64-127
+// the lo parts, each row plain bf16.
 // 64-channel 3x3 layers: src [64][9*64] (K-major, tap*64 + c) -> dst [128][9*32 words]; a tap's 128 bytes = 64 bf16 = both chunks.
 __global__ void split_stack_weights_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 64 * 576) return;
-    const int co = i / 576, k = i - co * 576;
-    const float v = src[i];
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
-    *reinterpret_cast<__nv_bfloat16*>(dst + (static_cast<size_t>(co) * 288) * 4 + k * 2) = h;
-    *reinterpret_cast<__nv_bfloat16*>(dst + (static_cast<size_t>(64 + co) * 288) * 4 + k * 2) = l;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;      // one thread per 4 K words of a row
+    if (i >= 64 * 144) return;
+    const int co = i / 144, k = (i - co * 144) * 4;
+    const float* w = src + co * 576 + k;
+    const float v[4] = {w[0], w[1], w[2], w[3]};
+    const auto x = Storage<SE3TN_PREC_BF16X3>::encode(v);
+    using B = Storage<SE3TN_PREC_BF16>;
+    *reinterpret_cast<uint2*>(dst + B::addr(co, 576, k)) = x.get(0);
+    *reinterpret_cast<uint2*>(dst + B::addr(64 + co, 576, k)) = x.get(1);
 }
 // stem: src [64][7*32] -> dst [128][7*32 words]; pixel slot p of filter row r: rows 0-63 [h0..h3 h0..h3], rows 64-127 [l0..l3 0 0 0 0]
+// (against the stem input's [4 x hi | 4 x lo] pixels, storage.cuh stem_input_prec)
 __global__ void split_stem_stack_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;      // one thread per (co, r, p): 4 channels
     if (i >= 64 * 7 * 8) return;
     const int p = i & 7, r = (i >> 3) % 7, co = i / 56;
     const float* w = src + co * 224 + r * 32 + p * 4;
-    __nv_bfloat16* d0 = reinterpret_cast<__nv_bfloat16*>(dst + (static_cast<size_t>(co) * 224 + r * 32 + p * 4) * 4);
-    __nv_bfloat16* d1 = reinterpret_cast<__nv_bfloat16*>(dst + (static_cast<size_t>(64 + co) * 224 + r * 32 + p * 4) * 4);
-    for (int c = 0; c < 4; ++c) {
-        const __nv_bfloat16 h = __float2bfloat16_rn(w[c]);
-        d0[c] = h; d0[4 + c] = h;
-        d1[c] = __float2bfloat16_rn(w[c] - __bfloat162float(h)); d1[4 + c] = __float2bfloat16_rn(0.f);
-    }
+    const float v[4] = {w[0], w[1], w[2], w[3]};
+    const auto x = Storage<SE3TN_PREC_BF16X3>::encode(v);
+    const uint2 h = x.get(0), l = x.get(1);
+    *reinterpret_cast<uint4*>(dst + (static_cast<size_t>(co) * 224 + r * 32 + p * 4) * 4) = make_uint4(h.x, h.y, h.x, h.y);
+    *reinterpret_cast<uint4*>(dst + (static_cast<size_t>(64 + co) * 224 + r * 32 + p * 4) * 4) = make_uint4(l.x, l.y, 0u, 0u);
 }
 // Resident 64-channel layers (conv_wgmma.cu, register-fragment epilogue): accumulator column 8j + 2m + e of every 32-column block
 // must carry output channel 8m + 2j + e, so the weight ROWS are stored in that order.
@@ -631,15 +610,10 @@ cudaError_t launch_permute_rows64(const float* src, float* dst, int ktot, cudaSt
 }
 cudaError_t launch_split_stack_weights(const float* src, void* dst, bool stem, cudaStream_t s) {
     if (stem) split_stem_stack_kernel<<<(64 * 7 * 8 + 127) / 128, 128, 0, s>>>(src, static_cast<uint8_t*>(dst));
-    else split_stack_weights_kernel<<<(64 * 576 + 255) / 256, 256, 0, s>>>(src, static_cast<uint8_t*>(dst));
+    else split_stack_weights_kernel<<<(64 * 144 + 255) / 256, 256, 0, s>>>(src, static_cast<uint8_t*>(dst));
     return cudaGetLastError();
 }
 
-cudaError_t launch_split_weights(const float* src, void* dst, size_t words, cudaStream_t s) {
-    if (!words) return cudaSuccess;
-    split_weights_kernel<<<1024, 256, 0, s>>>(src, static_cast<uint8_t*>(dst), words);
-    return cudaGetLastError();
-}
 // stand-alone K6 (se3tn_pose_update; the batched path runs it inside head_pooled_kernel)
 __global__ void pose_update_kernel(const double* poses_in, const float* __restrict__ trans,
                                    const float* __restrict__ rot, float tn, float rn,

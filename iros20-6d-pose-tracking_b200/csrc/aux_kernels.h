@@ -24,7 +24,7 @@ struct PreprocessArgs {
     const double* mean64; const double* std64;    // [sets][8] when stats_f64
     int stats_f64;
     int stats_rows;                // rows of the mean/std tables (weight ids are clamped to it)
-    int round_tf32;                // conv-input storage: 0 raw fp32, 1 tf32-rounded words, 2 per pixel [4 bf16 hi | 4 bf16 lo]
+    int precision;                 // SE3TN_PREC_*: selects the stem-input format of stemA / stemB (storage.cuh)
     int b_precropped;              // frame_rgb/frame_depth are n ready-made 176x176 crops (processData inputs)
     float* stemA; float* stemB;    // N x 182 x 184 x 4 (nullable)
     float* nchwA; float* nchwB;    // N x 4 x 176 x 176 (nullable)
@@ -37,18 +37,18 @@ cudaError_t launch_bbox(const double* poses, const double* K4, const double* wid
                         int* out, int n, cudaStream_t s);
 cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const int* bbox, int n,
                         int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth, cudaStream_t s);
-cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int round_tf32, cudaStream_t s);
+cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s);
 cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int Win, int C, cudaStream_t s);
 // poses_in non-null: also the pose update of every track (K6 fused into K4); zero_words: n_zero 32-bit counters cleared for the next step
 cudaError_t launch_head_pooled(const float* part /*[n][kPoolSlices][1024]*/, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                                int n_img, int npix, const int* img_wid, const float* const* fc_table,
                                const double* poses_in, double* poses_out, float tn, float rn, unsigned* zero_words, int n_zero, cudaStream_t s);
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
-                        int n_img, int npix, int split_bf16, const int* img_wid, const float* const* fc_table, cudaStream_t s);
-// `in` points at the first image; storage: 0 fp32, 1 bf16 hi/lo chunks, 2 plain bf16
-cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int storage, cudaStream_t s);
-cudaError_t launch_to_bf16(const float* src, void* dst, size_t n, cudaStream_t s);
-cudaError_t launch_split_weights(const float* src, void* dst, size_t words, cudaStream_t s);
+                        int n_img, int npix, cudaStream_t s);
+// `in` points at the first image, in the activation format of `precision` (SE3TN_PREC_*)
+cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s);
+// fp32 weight matrix [rows][ktot] -> the weight format of a tensor-core precision (storage.cuh)
+cudaError_t launch_encode_weights(int precision, const float* src, void* dst, int rows, int ktot, cudaStream_t s);
 cudaError_t launch_permute_rows64(const float* src /*[64][ktot]*/, float* dst, int ktot, cudaStream_t s);
 cudaError_t launch_split_stack_weights(const float* src, void* dst /*[128][9*32 | 7*32 words]*/, bool stem, cudaStream_t s);
 cudaError_t launch_pose_update(const double* poses_in, const float* trans, const float* rot, float tn, float rn,

@@ -28,11 +28,8 @@ constexpr int kChunkBytes = 128;      // one SWIZZLE_128B row of K: 32 tf32 word
 
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SELU = 2 };
 enum { KIND_S1 = 0, KIND_S2 = 1, KIND_STEM = 2 };            // conv kinds (compile-time unit tables in conv_wgmma.cu)
-enum { PREC_TF32 = 0, PREC_BF16X3 = 1, PREC_BF16 = 2 };      // arithmetic / storage of the wgmma kernels
-// Activation storage per precision: PREC_TF32 fp32 words (tf32-rounded); PREC_BF16X3 the same 4 bytes per channel as
-// [32 x bf16 hi | 32 x bf16 lo] per 32-channel chunk; PREC_BF16 2 bytes per channel, 64 channels per 128-byte chunk
-// (the stem INPUT stays 16 bytes per pixel [4 x hi | 4 x lo] in both bf16 modes).
-__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == PREC_BF16 ? 2 : 4; }
+// The wgmma kernels take their precision as an SE3TN_PREC_* value (include/se3tn.h); the byte layout of each mode's
+// activations and weights is defined in storage.cuh.
 
 struct Tap {
     int16_t dy, dx;      // input-pixel displacement of this tap relative to (oy*stride, ox*stride)
@@ -76,7 +73,6 @@ struct LayerDesc {
     int kind;              // KIND_*
     int chunks;            // 128-byte K chunks per pixel per group (cin * bytes / 128)
     int cin_words;         // 32-bit words of K per tap per group (weight-matrix K offset of a tap = tap * cin_words)
-    int in_cbase_words;    // word offset of group 0's channels inside a pixel of the input buffer
     int in_gstride_words;  // word offset between groups
     int cout;              // per group
     int groups;

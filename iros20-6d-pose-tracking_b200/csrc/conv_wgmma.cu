@@ -15,8 +15,8 @@
 //     warp 1 weight TMA producer, warps 2-3 idle; warpgroups 1 and 2 issue the MMAs and run the epilogue from registers.
 //     Each consumer warpgroup keeps one MMA group in flight and hands an operand stage back once the group after it
 //     has been issued (wgmma.wait_group 1).
-//   * PREC selects arithmetic and storage (conv_common.h): TF32 (4 x k8 tf32 MMAs per chunk-tap), BF16X3 (x = hi + lo as
-//     two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 64 channels per chunk, 1 product).
+//   * PREC (an SE3TN_PREC_* value) selects arithmetic and storage (storage.cuh): TF32 (4 x k8 tf32 MMAs per chunk-tap),
+//     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product).
 //   * programmatic dependent launch: every CTA signals launch_dependents at entry; only the threads that touch
 //     activations execute griddepcontrol.wait, so barrier init and the weight TMA run under the previous kernel's tail.
 //   * per-object weights (reference README.md:132: one checkpoint per object class): with img_wid every work unit takes
@@ -51,7 +51,7 @@
 //     sums instead (AdaptiveAvgPool2d(1) fused; fixed order -> deterministic).
 #include "conv_common.h"
 #include "ptx.cuh"
-#include <cuda_bf16.h>
+#include "storage.cuh"
 #include <algorithm>
 
 namespace se3tn {
@@ -117,34 +117,8 @@ __device__ __forceinline__ void trace_exit(unsigned long long* tr) {
     tr[blockIdx.x * 8 + 7] = (gtimer() & ~0xffull) | (smid & 0xff);
 }
 
-// fp32 -> (bf16 hi, bf16 lo) with x ~= hi + lo; packs two values per 32-bit word (element 0 in the low half)
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    const float2 hf = __bfloat1622float2(h);
-    const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack2(uint32_t w) {
-    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
-}
 using ptx::desc_lo;
 using ptx::mk_desc;
-
-// Byte address of 4 consecutive channels (c % 4 == 0) of pixel `pix` in an NHWC buffer of C channels per pixel:
-//   TF32   : fp32 words                       -> 16 bytes at (pix*C + c) * 4
-//   BF16X3 : chunk [32 x hi | 32 x lo]        -> 8 bytes (hi) at (pix*C + (c & ~31)) * 4 + (c & 31) * 2, lo 64 bytes further
-//   BF16   : 2 bytes per channel              -> 8 bytes at (pix*C + c) * 2
-template <int PREC>
-__device__ __forceinline__ size_t chan_byte(size_t pix, int C, int c) {
-    if (PREC == PREC_TF32) return (pix * C + c) * 4;
-    if (PREC == PREC_BF16X3) return (pix * C + (c & ~31)) * 4 + (c & 31) * 2;
-    return (pix * C + c) * 2;
-}
 
 // The first 32 accumulator registers (columns 0..63) of a 64-register (N = 128) accumulator
 __device__ __forceinline__ float (&acc_lo32(float (&d)[64]))[32] { return *reinterpret_cast<float (*)[32]>(&d[0]); }
@@ -166,14 +140,14 @@ struct Consumer {
 template <int KIND, int PREC> struct RCfg {
     static constexpr bool POOL = (KIND == KIND_STEM);
     static constexpr int BN = 64;
-    // STACK: hi / lo weight rows stacked along N (header comment).  The stem input is [4 hi | 4 lo] per pixel in both bf16 modes.
-    static constexpr int kStack = (PREC == PREC_BF16X3 || (PREC == PREC_BF16 && POOL)) ? 2 : 1;
+    // STACK: hi / lo weight rows stacked along N (header comment) for layers whose input is in the bf16x3 format
+    static constexpr int kStack = ((POOL ? stem_input_prec(PREC) : PREC) == SE3TN_PREC_BF16X3) ? 2 : 1;
     static constexpr int kBTile = BN * kStack * kChunkBytes;
     static constexpr int kAUnit = POOL ? kAUnitStem : kAUnit3;
-    static constexpr int kAStages = POOL ? (PREC == PREC_TF32 ? 4 : 3) : (PREC == PREC_BF16 ? 6 : 4);
-    static constexpr int kPoolBufs = POOL ? (PREC == PREC_TF32 ? 2 : 1) : 0;
+    static constexpr int kAStages = POOL ? (PREC == SE3TN_PREC_TF32 ? 4 : 3) : (PREC == SE3TN_PREC_BF16 ? 6 : 4);
+    static constexpr int kPoolBufs = POOL ? (PREC == SE3TN_PREC_TF32 ? 2 : 1) : 0;
     static constexpr int kAcc = BN * kStack / 2;                    // accumulator registers per thread (N / 2)
-    static constexpr int kMaxWTiles = POOL ? 7 : ((PREC == PREC_TF32) ? 18 : 9);
+    static constexpr int kMaxWTiles = POOL ? 7 : ((PREC == SE3TN_PREC_TF32) ? 18 : 9);
     static constexpr int kSmem = kAStages * kAUnit + kMaxWTiles * kBTile + kPoolBufs * kPoolStageAlloc + 1024 + 512;
     static_assert(kSmem <= 232448, "shared memory budget");
 };
@@ -193,7 +167,7 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
         uint32_t b_lo;
         if (C::kStack == 2) b_lo = desc_lo(sB + KT::wtap(u, k) * C::kBTile) + ch * 4;   // chunk ch sits 64 bytes (4 x 16 B) further along K
         else                b_lo = desc_lo(sB + (KT::wtap(u, k) * tiles_per_tap + ch) * C::kBTile);
-        if constexpr (PREC == PREC_TF32) {
+        if constexpr (PREC == SE3TN_PREC_TF32) {
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) ptx::wgmma_tf32_n64(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
         } else if constexpr (C::POOL) {
@@ -208,7 +182,7 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
                 ptx::wgmma_bf16_n64(acc_lo32(acc), mk_desc(a_lo + 4 + 2 * sl), mk_desc(b_lo + 2 * sl), 1u);
             }
         } else {
-            // PREC_BF16: chunk = 64 bf16 channels: four K = 16 steps
+            // SE3TN_PREC_BF16: chunk = 64 bf16 channels: four K = 16 steps
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) ptx::wgmma_bf16_n64(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
         }
@@ -274,7 +248,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                         ptx::mbar_wait(&a_empty[stage], phase ^ 1);
                         ptx::mbar_arrive_expect_tx(&a_full[stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
                         ptx::tma_load_4d(sA + stage * C::kAUnit, &L.amap[KT::amap(u)], &a_full[stage],
-                                         L.in_cbase_words + ch * 32, ox + KT::c1(u), oy + KT::c2(u), n0);
+                                         ch * 32, ox + KT::c1(u), oy + KT::c2(u), n0);
                         if (++stage == C::kAStages) { stage = 0; phase ^= 1; }
                     }
                 }
@@ -318,7 +292,8 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
 
             // 64-channel layers: this thread's pixels and their residual pieces are known before the accumulator is: issue the
             // residual loads now so their latency hides behind the MMAs.  Piece (h, b): row cs.row(h), channels 32b + 8m .. + 7.
-            size_t rpix[2]; bool rvalid[2]; uint4 rres[2][2][2];
+            using S = Storage<PREC>;
+            size_t rpix[2]; bool rvalid[2]; Raw<PREC, 8> rres[2][2];
             if constexpr (!POOL) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -329,12 +304,11 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                     rpix[h] = (static_cast<size_t>(n0) * L.Ho + y) * L.Wo + x;
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        rres[h][b][0] = make_uint4(0u, 0u, 0u, 0u); rres[h][b][1] = make_uint4(0u, 0u, 0u, 0u);
+                        rres[h][b] = Raw<PREC, 8>{};
                         if (L.res && rvalid[h]) {
-                            const uint8_t* rp = L.res + chan_byte<PREC>(rpix[h], L.res_c, 32 * b + 8 * cs.m);
-                            if (PREC == PREC_TF32)        { rres[h][b][0] = __ldg(reinterpret_cast<const uint4*>(rp)); rres[h][b][1] = __ldg(reinterpret_cast<const uint4*>(rp + 16)); }   // 8 fp32 words
-                            else if (PREC == PREC_BF16X3) { rres[h][b][0] = __ldg(reinterpret_cast<const uint4*>(rp)); rres[h][b][1] = __ldg(reinterpret_cast<const uint4*>(rp + 64)); }   // hi piece, lo piece
-                            else                          { rres[h][b][0] = __ldg(reinterpret_cast<const uint4*>(rp)); }                                                                   // 8 bf16
+                            const uint8_t* rp = L.res + S::addr(rpix[h], L.res_c, 32 * b + 8 * cs.m);
+#pragma unroll
+                            for (int q = 0; q < rres[h][b].kPieces; ++q) rres[h][b].set(q, __ldg(rres[h][b].at(rp, q)));
                         }
                     }
                 }
@@ -397,35 +371,14 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                                 v[2 * jj + e] = a + bias8[2 * jj + e];
                             }
                         if (L.res) {
-                            if (PREC == PREC_TF32) {
-                                const uint4 r0 = rres[h][b][0], r1 = rres[h][b][1];
-                                v[0] += __uint_as_float(r0.x); v[1] += __uint_as_float(r0.y); v[2] += __uint_as_float(r0.z); v[3] += __uint_as_float(r0.w);
-                                v[4] += __uint_as_float(r1.x); v[5] += __uint_as_float(r1.y); v[6] += __uint_as_float(r1.z); v[7] += __uint_as_float(r1.w);
-                            } else {
-                                const uint4 h4 = rres[h][b][0], l4 = rres[h][b][1];       // l4 = 0 in PREC_BF16
-                                const uint32_t hw[4] = {h4.x, h4.y, h4.z, h4.w}, lw[4] = {l4.x, l4.y, l4.z, l4.w};
+                            float r[8];
+                            S::decode(rres[h][b], r);
 #pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    const float2 hf = unpack2(hw[e]), lf = unpack2(lw[e]);
-                                    v[2 * e] += hf.x + lf.x; v[2 * e + 1] += hf.y + lf.y;
-                                }
-                            }
+                            for (int e = 0; e < 8; ++e) v[e] += r[e];
                         }
 #pragma unroll
                         for (int e = 0; e < 8; ++e) v[e] = act_apply(v[e], L.act);
-                        uint8_t* outp = L.out + chan_byte<PREC>(rpix[h], L.out_c, L.out_coff + ch0);
-                        if (PREC == PREC_TF32) {
-                            *reinterpret_cast<float4*>(outp) = make_float4(ptx::to_tf32(v[0]), ptx::to_tf32(v[1]), ptx::to_tf32(v[2]), ptx::to_tf32(v[3]));
-                            *reinterpret_cast<float4*>(outp + 16) = make_float4(ptx::to_tf32(v[4]), ptx::to_tf32(v[5]), ptx::to_tf32(v[6]), ptx::to_tf32(v[7]));
-                        } else if (PREC == PREC_BF16X3) {
-                            uint32_t hw[4], lw[4];
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
-                            *reinterpret_cast<uint4*>(outp) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                            *reinterpret_cast<uint4*>(outp + 64) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                        } else {
-                            *reinterpret_cast<uint4*>(outp) = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
-                        }
+                        S::encode(v).store(L.out + S::addr(rpix[h], L.out_c, L.out_coff + ch0));
                     }
                 }
             } else {
@@ -465,18 +418,8 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                             mx.x = fmaxf(mx.x, s4.x); mx.y = fmaxf(mx.y, s4.y); mx.z = fmaxf(mx.z, s4.z); mx.w = fmaxf(mx.w, s4.w);
                         }
                     const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + c4));
-                    const float v0 = selu_fast(mx.x + b4.x), v1 = selu_fast(mx.y + b4.y), v2 = selu_fast(mx.z + b4.z), v3 = selu_fast(mx.w + b4.w);
-                    uint8_t* po = L.out + chan_byte<PREC>((static_cast<size_t>(n0) * L.Ho + oy) * L.Wo + ox, L.out_c, L.out_coff + c4);
-                    if (PREC == PREC_TF32) {
-                        *reinterpret_cast<float4*>(po) = make_float4(ptx::to_tf32(v0), ptx::to_tf32(v1), ptx::to_tf32(v2), ptx::to_tf32(v3));
-                    } else if (PREC == PREC_BF16X3) {
-                        uint32_t h0, l0, h1, l1;
-                        split2(v0, v1, h0, l0); split2(v2, v3, h1, l1);
-                        *reinterpret_cast<uint2*>(po) = make_uint2(h0, h1);
-                        *reinterpret_cast<uint2*>(po + 64) = make_uint2(l0, l1);
-                    } else {
-                        *reinterpret_cast<uint2*>(po) = make_uint2(pack_bf16(v0, v1), pack_bf16(v2, v3));
-                    }
+                    const float v4[4] = {selu_fast(mx.x + b4.x), selu_fast(mx.y + b4.y), selu_fast(mx.z + b4.z), selu_fast(mx.w + b4.w)};
+                    S::encode(v4).store(L.out + S::addr((static_cast<size_t>(n0) * L.Ho + oy) * L.Wo + ox, L.out_c, L.out_coff + c4));
                 }
                 if (C::kPoolBufs == 1) asm volatile("bar.sync 1, 256;" ::: "memory");   // single staging buffer: readers done before the next tile writes
             }
@@ -546,7 +489,7 @@ __device__ __forceinline__ void trunk_load_unit(const LayerDesc& L, const UnitCo
                                                 int& stage, uint32_t& phase, int n_stages)
 {
     using KT = KTab<KIND>;
-    const int cbase = L.in_cbase_words + c.grp * L.in_gstride_words;
+    const int cbase = c.grp * L.in_gstride_words;
     const int ox = c.tx * 11, oy = c.ty * 11;
     for (int ch = c.c0; ch < c.c1; ++ch) {
 #pragma unroll
@@ -608,11 +551,11 @@ __device__ __forceinline__ void trunk_mma_unit(float (&acc)[TCfg<PREC>::kAcc], c
                 const uint32_t b_lo = desc_lo(sB + bstage * C::kBTile);
                 const uint32_t a_lo = a_unit_lo + k * kRowShift * (kChunkBytes >> 4);
                 ptx::wgmma_fence();
-                if constexpr (PREC == PREC_TF32) {
+                if constexpr (PREC == SE3TN_PREC_TF32) {
 #pragma unroll
                     for (int kk = 0; kk < 4; ++kk)
                         ptx::wgmma_tf32_n128(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
-                } else if constexpr (PREC == PREC_BF16X3) {
+                } else if constexpr (PREC == SE3TN_PREC_BF16X3) {
                     // chunk = [32 hi | 32 lo] bf16 (A) x [32 w_hi | 32 w_lo] (B); offsets in 16-byte units
                     constexpr int AO[6] = {0, 2, 4, 6, 0, 2};      // hi, hi, lo, lo, hi, hi
                     constexpr int BO[6] = {0, 2, 0, 2, 4, 6};      // w_hi x4,        w_lo x2
@@ -750,6 +693,8 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
         }
     } else if (warp >= 4) {
         // ============================== MMA + epilogue (two warpgroups, 8 warps) ==========================
+        using S = Storage<PREC>;
+        using R4 = Raw<PREC, 4>;
         ptx::grid_dep_wait();
         const Consumer cs;
         const int ew = cs.ew;                       // consumer warp 0..7 = tile rows 16 ew .. 16 ew + 15
@@ -849,16 +794,15 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 const int chan = ch0 + 32 * bi;                   // first channel of this 32-channel block
                 // bias and residual pieces first: their L2 latency overlaps the staging round trip below
                 const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias_base + chan + grp * 4));
-                float4 r4[4];                                    // TF32: 4 fp32 words
-                uint2 rh[4], rl[4];                              // bf16: 4 channels hi (and lo, BF16X3)
+                R4 rr[4];                                        // residual: this lane's 4 pixels, 4 channels each
                 if (L.res) {
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
-                        r4[k] = make_float4(0.f, 0.f, 0.f, 0.f); rh[k] = make_uint2(0u, 0u); rl[k] = make_uint2(0u, 0u);
+                        rr[k] = R4{};
                         if (pix[k] >= 0) {
-                            const uint8_t* rp = L.res + chan_byte<PREC>(static_cast<size_t>(pix[k]), L.res_c, chan + grp * 4);
-                            if (PREC == PREC_TF32) r4[k] = __ldcg(reinterpret_cast<const float4*>(rp));
-                            else { rh[k] = __ldcg(reinterpret_cast<const uint2*>(rp)); if (PREC == PREC_BF16X3) rl[k] = __ldcg(reinterpret_cast<const uint2*>(rp + 64)); }
+                            const uint8_t* rp = L.res + S::addr(pix[k], L.res_c, chan + grp * 4);
+#pragma unroll
+                            for (int q = 0; q < R4::kPieces; ++q) rr[k].set(q, __ldcg(R4::at(rp, q)));
                         }
                     }
                 }
@@ -877,15 +821,11 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                     a4[k].x += b4.x; a4[k].y += b4.y; a4[k].z += b4.z; a4[k].w += b4.w;
                 }
                 if (L.res) {
-                    if (PREC == PREC_TF32) {
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) { a4[k].x += r4[k].x; a4[k].y += r4[k].y; a4[k].z += r4[k].z; a4[k].w += r4[k].w; }
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const float2 h0 = unpack2(rh[k].x), h1 = unpack2(rh[k].y), l0 = unpack2(rl[k].x), l1 = unpack2(rl[k].y);
-                            a4[k].x += h0.x + l0.x; a4[k].y += h0.y + l0.y; a4[k].z += h1.x + l1.x; a4[k].w += h1.y + l1.y;
-                        }
+                    for (int k = 0; k < 4; ++k) {
+                        float r[4];
+                        S::decode(rr[k], r);
+                        a4[k].x += r[0]; a4[k].y += r[1]; a4[k].z += r[2]; a4[k].w += r[3];
                     }
                 }
                 float4 psum = make_float4(0.f, 0.f, 0.f, 0.f);   // fused average pool: this lane's rows, 4 channels
@@ -895,17 +835,8 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                     o.x = act_apply(o.x, L.act); o.y = act_apply(o.y, L.act); o.z = act_apply(o.z, L.act); o.w = act_apply(o.w, L.act);
                     if (pix[k] < 0) continue;
                     if (L.pool_part) { psum.x += o.x; psum.y += o.y; psum.z += o.z; psum.w += o.w; continue; }
-                    uint8_t* po = L.out + chan_byte<PREC>(static_cast<size_t>(pix[k]), L.out_c, L.out_coff + chan + grp * 4);
-                    if (PREC == PREC_TF32) {
-                        *reinterpret_cast<float4*>(po) = make_float4(ptx::to_tf32(o.x), ptx::to_tf32(o.y), ptx::to_tf32(o.z), ptx::to_tf32(o.w));
-                    } else if (PREC == PREC_BF16X3) {
-                        uint32_t h0, l0, h1, l1;
-                        split2(o.x, o.y, h0, l0); split2(o.z, o.w, h1, l1);
-                        *reinterpret_cast<uint2*>(po) = make_uint2(h0, h1);
-                        *reinterpret_cast<uint2*>(po + 64) = make_uint2(l0, l1);
-                    } else {
-                        *reinterpret_cast<uint2*>(po) = make_uint2(pack_bf16(o.x, o.y), pack_bf16(o.z, o.w));
-                    }
+                    const float o4[4] = {o.x, o.y, o.z, o.w};
+                    S::encode(o4).store(L.out + S::addr(pix[k], L.out_c, L.out_coff + chan + grp * 4));
                 }
                 if (L.pool_part) {                                // rows 4k + sub summed above; fold the four `sub` groups (fixed order: deterministic)
 #pragma unroll
@@ -993,15 +924,15 @@ cudaError_t launch_trunk_t(const TrunkParams& p, int num_sms, bool pdl, cudaStre
 cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, int num_sms, bool pdl, cudaStream_t stream) {
     if (kind == KIND_STEM) {
         switch (prec) {
-            case PREC_TF32:   return launch_resident_t<KIND_STEM, PREC_TF32>(p, num_sms, pdl, stream);
-            case PREC_BF16X3: return launch_resident_t<KIND_STEM, PREC_BF16X3>(p, num_sms, pdl, stream);
-            case PREC_BF16:   return launch_resident_t<KIND_STEM, PREC_BF16>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_TF32:   return launch_resident_t<KIND_STEM, SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_BF16X3: return launch_resident_t<KIND_STEM, SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_BF16:   return launch_resident_t<KIND_STEM, SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
         }
     } else if (kind == KIND_S1) {
         switch (prec) {
-            case PREC_TF32:   return launch_resident_t<KIND_S1, PREC_TF32>(p, num_sms, pdl, stream);
-            case PREC_BF16X3: return launch_resident_t<KIND_S1, PREC_BF16X3>(p, num_sms, pdl, stream);
-            case PREC_BF16:   return launch_resident_t<KIND_S1, PREC_BF16>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_TF32:   return launch_resident_t<KIND_S1, SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_BF16X3: return launch_resident_t<KIND_S1, SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_BF16:   return launch_resident_t<KIND_S1, SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
         }
     }
     return cudaErrorInvalidValue;
@@ -1009,9 +940,9 @@ cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, in
 
 cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int num_sms, bool pdl, cudaStream_t stream) {
     switch (prec) {
-        case PREC_TF32:   return launch_trunk_t<PREC_TF32>(p, num_sms, pdl, stream);
-        case PREC_BF16X3: return launch_trunk_t<PREC_BF16X3>(p, num_sms, pdl, stream);
-        case PREC_BF16:   return launch_trunk_t<PREC_BF16>(p, num_sms, pdl, stream);
+        case SE3TN_PREC_TF32:   return launch_trunk_t<SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
+        case SE3TN_PREC_BF16X3: return launch_trunk_t<SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
+        case SE3TN_PREC_BF16:   return launch_trunk_t<SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
     }
     return cudaErrorInvalidValue;
 }

@@ -7,7 +7,7 @@
 #include "render.h"
 #include <dlfcn.h>
 #include "depth_fill.h"
-#include "ptx.cuh"
+#include "storage.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -85,17 +86,33 @@ size_t blob_floats() {
     return n + kFcFloats;
 }
 
-struct WeightSet {
-    float* dev = nullptr;           // exact fp32 blob (biases, fc and the fp32 mode's conv weights)
-    float* dev_tf32 = nullptr;      // same layout, conv weights rounded to tf32
-    uint8_t* dev_bf16 = nullptr;    // blob-sized: conv weights as [32 bf16 hi | 32 bf16 lo] per 32-word K chunk (PREC_BF16X3 ring layers)
-    uint8_t* dev_h = nullptr;       // half-blob-sized: conv weights as plain bf16, K-major (PREC_BF16; layers 2..7 with permuted rows)
-    uint8_t* dev_stack = nullptr;   // 8 x [128][288 words]: resident layers with hi / lo rows stacked along N (conv_wgmma.cu STACK)
-    float* dev_perm = nullptr; float* dev_perm_tmp = nullptr;   // 64-channel layers: rows in the accumulator fragment's channel order, tf32 words
+// Per-precision state is indexed by the SE3TN_PREC_* value; the fp32 FFMA mode has no entry of its own there.
+constexpr int kNumPrecs = 4;
+constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16};
+
+// An owned device allocation, freed with its owner (every entry point makes the context's device current first).
+struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
+template <typename T> using DevBuf = std::unique_ptr<T[], CudaFree>;
+template <typename T> cudaError_t dev_alloc(DevBuf<T>& b, size_t n) {
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) b.reset(static_cast<T*>(p));
+    return e;
+}
+
+// Every form of one weight set that the kernels read.
+struct DeviceWeights {
+    DevBuf<float> blob;             // exact fp32 blob (biases, fc and the fp32 mode's conv weights)
+    DevBuf<uint8_t> conv[kNumPrecs];   // tensor-core modes: conv weights in that mode's format (storage.cuh) at w_off * bytes per channel
+    DevBuf<uint8_t> stack;          // 8 x [128][288 words]: resident layers with hi / lo rows stacked along N (conv_wgmma.cu STACK)
+    DevBuf<float> perm;             // 64-channel layers: rows in the accumulator fragment's channel order, tf32 words
     size_t w_off[14], b_off[14];
     size_t fc_off;
-    // weight tensor maps per precision: [li] -> the map the kernel of that layer wants
-    CUtensorMap bmap_tf32[kLayersPerSet], bmap_x3[kLayersPerSet], bmap_h[kLayersPerSet];
+    CUtensorMap bmap[kNumPrecs][kLayersPerSet];   // the weight map the kernel of each layer wants, per precision
+};
+
+struct WeightSet {
+    std::unique_ptr<DeviceWeights> dev;   // null: not loaded
     float mean32[8], std32[8];
     double mean64[8], std64[8];
     int stats_f64 = 0;
@@ -132,11 +149,11 @@ struct se3tn_ctx {
     EncodeTiledFn encode = nullptr;
     std::map<int, WeightSet> weights;
     // device copies of per-set stats, rebuilt when a set changes: [max_id+1][8]
-    float* d_mean32 = nullptr; float* d_std32 = nullptr; double* d_mean64 = nullptr; double* d_std64 = nullptr;
+    DevBuf<float> d_mean32, d_std32; DevBuf<double> d_mean64, d_std64;
     int stats_rows = 0; bool stats_dirty = true; int stats_f64 = 0;
     // per-weight-set device tables for multi-set launches, rebuilt when a set is (re)loaded: entry [wid*14 + layer]
-    CUtensorMap* d_bmaps_tf32 = nullptr; CUtensorMap* d_bmaps_bf16 = nullptr; CUtensorMap* d_bmaps_x3 = nullptr;
-    const float** d_bias = nullptr; const float** d_fc = nullptr;   // d_fc[wid] -> [6][512] weights then [6] biases
+    DevBuf<CUtensorMap> d_bmaps[kNumPrecs];   // per tensor-core precision
+    DevBuf<const float*> d_bias, d_fc;        // d_fc[wid] -> [6][512] weights then [6] biases
     int table_rows = 0; bool tables_dirty = true;
     int launches = 0;
     bool profiling = false;
@@ -158,15 +175,6 @@ struct se3tn_ctx {
 };
 
 namespace {
-
-// conv-input storage mode of the packers for a precision: 0 raw fp32, 1 tf32 words, 2 bf16 hi/lo per pixel
-inline int store_mode_of(int precision) {
-    return precision == SE3TN_PREC_TF32 ? 1 : (precision == SE3TN_PREC_BF16X3 || precision == SE3TN_PREC_BF16) ? 2 : 0;
-}
-// kernel-side precision of a public one (-1: the fp32 FFMA mode)
-inline int kprec_of(int precision) {
-    return precision == SE3TN_PREC_TF32 ? PREC_TF32 : precision == SE3TN_PREC_BF16X3 ? PREC_BF16X3 : precision == SE3TN_PREC_BF16 ? PREC_BF16 : -1;
-}
 
 int fail(se3tn_ctx* c, int code, const std::string& msg) {
     if (c) c->err = msg; else g_create_error = msg;
@@ -306,24 +314,23 @@ void fill_geom(const LayerSpec& L, int n, ConvGeom& g) {
 }
 
 // one layer as the wgmma kernels see it (conv_common.h LayerDesc)
-void fill_layer_desc(const se3tn_ctx* c, const WeightSet& ws, int li, int kprec, LayerDesc& d) {
+void fill_layer_desc(const se3tn_ctx* c, const DeviceWeights& w, int li, int precision, LayerDesc& d) {
     const LayerSpec& L = kLayers[li];
     const int row = li;                            // row of the per-set tables
     memset(&d, 0, sizeof d);
-    const int bpc = prec_bytes_per_channel(kprec);
     const bool stem = (L.kind == K_STEM);
-    const CUtensorMap (*amaps)[4] = (bpc == 2 && !stem) ? c->amap2 : c->amap4;
+    const int bpc = prec_bytes_per_channel(stem ? stem_input_prec(precision) : precision);   // of this layer's input
+    const CUtensorMap (*amaps)[4] = bpc == 2 ? c->amap2 : c->amap4;
     for (int m = 0; m < 4; ++m) d.amap[m] = amaps[li][m];
-    d.bmap = (kprec == PREC_TF32) ? ws.bmap_tf32[row] : (kprec == PREC_BF16X3 ? ws.bmap_x3[row] : ws.bmap_h[row]);
-    d.bias = ws.dev + ws.b_off[li];
+    d.bmap = w.bmap[precision][row];
+    d.bias = w.blob.get() + w.b_off[li];
     d.kind = stem ? KIND_STEM : (L.kind == K_S2 ? KIND_S2 : KIND_S1);
-    if (stem) {                                    // K = 8 pixels x 4 channels x 4 bytes per filter row in every mode
-        d.chunks = 1; d.cin_words = 32; d.in_cbase_words = 0; d.in_gstride_words = 0;
+    d.chunks = L.cin * bpc / kChunkBytes; d.cin_words = L.cin * bpc / 4; d.in_gstride_words = d.cin_words;
+    if (stem) {
         d.out = reinterpret_cast<uint8_t*>(c->buf[li == 0 ? B_P1A : B_P1B]);   // fused MaxPool2d(3,2,1): the pooled tensor is written directly
         d.out_c = 64; d.out_coff = 0; d.Ho = d.Wo = 44;
         d.tiles_x = d.tiles_y = 9;                 // pooled 5x5 blocks
     } else {
-        d.chunks = L.cin * bpc / kChunkBytes; d.cin_words = L.cin * bpc / 4; d.in_cbase_words = 0; d.in_gstride_words = L.cin * bpc / 4;
         d.out = reinterpret_cast<uint8_t*>(c->buf[L.out]);
         d.out_c = L.out_c; d.out_coff = L.out_coff; d.Ho = d.Wo = layer_Ho(L);
         d.tiles_x = d.tiles_y = d.Ho / 11;
@@ -336,12 +343,6 @@ void fill_layer_desc(const se3tn_ctx* c, const WeightSet& ws, int li, int kprec,
     d.dep_layer = -1; d.dep_target = 0; d.unit_base = 0;
 }
 
-__global__ void round_tf32_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t n) {
-    size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (; i < n; i += stride) dst[i] = ptx::to_tf32(src[i]);
-}
-
 int sync_stats(se3tn_ctx* c, cudaStream_t s) {
     if (!c->stats_dirty) return SE3TN_OK;
     int max_id = -1, f64 = -1;
@@ -352,12 +353,11 @@ int sync_stats(se3tn_ctx* c, cudaStream_t s) {
     }
     if (max_id < 0) return fail(c, SE3TN_ERR_STATE, "se3tn_set_stats has not been called");
     const int rows = max_id + 1;
-    if (rows > c->stats_rows) {
-        cudaFree(c->d_mean32); cudaFree(c->d_std32); cudaFree(c->d_mean64); cudaFree(c->d_std64);
-        CU_TRY(c, cudaMalloc(&c->d_mean32, rows * 8 * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&c->d_std32, rows * 8 * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&c->d_mean64, rows * 8 * sizeof(double)));
-        CU_TRY(c, cudaMalloc(&c->d_std64, rows * 8 * sizeof(double)));
+    if (rows > c->stats_rows) {                    // grow: the old tables stay in place until all new ones exist
+        DevBuf<float> m32, s32; DevBuf<double> m64, s64;
+        CU_TRY(c, dev_alloc(m32, rows * 8)); CU_TRY(c, dev_alloc(s32, rows * 8));
+        CU_TRY(c, dev_alloc(m64, rows * 8)); CU_TRY(c, dev_alloc(s64, rows * 8));
+        c->d_mean32 = std::move(m32); c->d_std32 = std::move(s32); c->d_mean64 = std::move(m64); c->d_std64 = std::move(s64);
         c->stats_rows = rows;
     }
     std::vector<float> m32(rows * 8, 0.f), s32(rows * 8, 1.f);
@@ -368,10 +368,10 @@ int sync_stats(se3tn_ctx* c, cudaStream_t s) {
     }
     // synchronous copies from stack-lifetime host vectors (rare: only when stats change)
     CU_TRY(c, cudaStreamSynchronize(s));
-    CU_TRY(c, cudaMemcpy(c->d_mean32, m32.data(), rows * 8 * sizeof(float), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_std32, s32.data(), rows * 8 * sizeof(float), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_mean64, m64.data(), rows * 8 * sizeof(double), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_std64, s64.data(), rows * 8 * sizeof(double), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_mean32.get(), m32.data(), rows * 8 * sizeof(float), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_std32.get(), s32.data(), rows * 8 * sizeof(float), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_mean64.get(), m64.data(), rows * 8 * sizeof(double), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_std64.get(), s64.data(), rows * 8 * sizeof(double), cudaMemcpyHostToDevice));
     c->stats_f64 = f64; c->stats_dirty = false;
     return SE3TN_OK;
 }
@@ -383,33 +383,32 @@ int sync_tables(se3tn_ctx* c, cudaStream_t s) {
     if (max_id < 0) return fail(c, SE3TN_ERR_STATE, "no weight set loaded");
     const int rows = max_id + 1;
     CU_TRY(c, cudaStreamSynchronize(s));
-    if (rows > c->table_rows) {
-        cudaFree(c->d_bmaps_tf32); cudaFree(c->d_bmaps_bf16); cudaFree(c->d_bmaps_x3); cudaFree(c->d_bias); cudaFree(c->d_fc);
-        CU_TRY(c, cudaMalloc(&c->d_bmaps_x3, sizeof(CUtensorMap) * rows * kLayersPerSet));
-        CU_TRY(c, cudaMalloc(&c->d_bmaps_tf32, sizeof(CUtensorMap) * rows * kLayersPerSet));
-        CU_TRY(c, cudaMalloc(&c->d_bmaps_bf16, sizeof(CUtensorMap) * rows * kLayersPerSet));
-        CU_TRY(c, cudaMalloc(&c->d_bias, sizeof(float*) * rows * kLayersPerSet));
-        CU_TRY(c, cudaMalloc(&c->d_fc, sizeof(float*) * rows));
+    if (rows > c->table_rows) {                    // grow: the old tables stay in place until all new ones exist
+        DevBuf<CUtensorMap> maps[kNumPrecs]; DevBuf<const float*> bias, fc;
+        for (int p : kTensorPrecs) CU_TRY(c, dev_alloc(maps[p], rows * kLayersPerSet));
+        CU_TRY(c, dev_alloc(bias, rows * kLayersPerSet));
+        CU_TRY(c, dev_alloc(fc, rows));
+        for (int p : kTensorPrecs) c->d_bmaps[p] = std::move(maps[p]);
+        c->d_bias = std::move(bias); c->d_fc = std::move(fc);
         c->table_rows = rows;
     }
-    std::vector<CUtensorMap> m1(rows * kLayersPerSet), m2(rows * kLayersPerSet), m3(rows * kLayersPerSet);
-    memset(m1.data(), 0, m1.size() * sizeof(CUtensorMap)); memset(m2.data(), 0, m2.size() * sizeof(CUtensorMap)); memset(m3.data(), 0, m3.size() * sizeof(CUtensorMap));
-    std::vector<const float*> bias(rows * kLayersPerSet, nullptr), fc(rows, nullptr);
+    const size_t entries = static_cast<size_t>(rows) * kLayersPerSet;
+    std::vector<CUtensorMap> maps(kNumPrecs * entries);    // [precision][entry], zeroed for ids without weights
+    std::vector<const float*> bias(entries, nullptr), fc(rows, nullptr);
     for (auto& kv : c->weights) {
         if (!kv.second.dev || kv.first < 0) continue;
+        const DeviceWeights& w = *kv.second.dev;
         for (int li = 0; li < kLayersPerSet; ++li) {
-            m1[kv.first * kLayersPerSet + li] = kv.second.bmap_tf32[li];
-            m2[kv.first * kLayersPerSet + li] = kv.second.bmap_h[li];
-            m3[kv.first * kLayersPerSet + li] = kv.second.bmap_x3[li];
-            bias[kv.first * kLayersPerSet + li] = kv.second.dev + kv.second.b_off[li];
+            const size_t e = static_cast<size_t>(kv.first) * kLayersPerSet + li;
+            for (int p : kTensorPrecs) maps[p * entries + e] = w.bmap[p][li];
+            bias[e] = w.blob.get() + w.b_off[li];
         }
-        fc[kv.first] = kv.second.dev + kv.second.fc_off;
+        fc[kv.first] = w.blob.get() + w.fc_off;
     }
-    CU_TRY(c, cudaMemcpy(c->d_bmaps_tf32, m1.data(), m1.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_bmaps_bf16, m2.data(), m2.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_bmaps_x3, m3.data(), m3.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_bias, bias.data(), bias.size() * sizeof(float*), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(c->d_fc, fc.data(), fc.size() * sizeof(float*), cudaMemcpyHostToDevice));
+    for (int p : kTensorPrecs)
+        CU_TRY(c, cudaMemcpy(c->d_bmaps[p].get(), &maps[p * entries], entries * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_bias.get(), bias.data(), bias.size() * sizeof(float*), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_fc.get(), fc.data(), fc.size() * sizeof(float*), cudaMemcpyHostToDevice));
     c->tables_dirty = false;
     return SE3TN_OK;
 }
@@ -432,12 +431,11 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     if (pose_done) *pose_done = false;
     auto it = c->weights.find(weight_id);
     if (it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(weight_id) + " not loaded");
-    const WeightSet& ws = it->second;
-    const int kprec = kprec_of(precision);
-    const bool tensor = kprec >= 0;
-    if (!tensor && precision != SE3TN_PREC_FP32) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
+    const DeviceWeights& w = *it->second.dev;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
+    const bool tensor = precision != SE3TN_PREC_FP32;
     auto bufp = [&](Buf b) { return c->buf[b] + kBufFloats[b] * static_cast<size_t>(first); };
-    const float* fcw = ws.dev + ws.fc_off;
+    const float* fcw = w.blob.get() + w.fc_off;
     if (!tensor) {
         // ---- fp32 FFMA cross-check mode: 14 direct convs + 2 max-pools + head ----
         if (img_wid) return fail(c, SE3TN_ERR_INVALID, "multi-weight-set launches need a tensor-core precision");
@@ -446,32 +444,32 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
             ConvGeom g; fill_geom(L, n, g);
             ConvPtrs p;
             p.in = bufp(L.in); p.out = bufp(L.out); p.res = (L.res != NONE) ? bufp(L.res) : nullptr;
-            p.w = ws.dev + ws.w_off[li]; p.bias = ws.dev + ws.b_off[li];
+            p.w = w.blob.get() + w.w_off[li]; p.bias = w.blob.get() + w.b_off[li];
             { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_direct(g, p, s)); }
             ++c->launches;
             if (li == 0) { ProfScope ps(c, 14, s); CU_TRY(c, launch_maxpool(bufp(B_Y1A), bufp(B_P1A), n, 88, 88, 64, s)); ++c->launches; }
             if (li == 1) { ProfScope ps(c, 15, s); CU_TRY(c, launch_maxpool(bufp(B_Y1B), bufp(B_P1B), n, 88, 88, 64, s)); ++c->launches; }
         }
-        { ProfScope ps(c, 16, s); CU_TRY(c, launch_head(bufp(B_H3), fcw, fcw + 6 * 512, out_trans, out_rot, n, 121, 0, nullptr, nullptr, s)); }
+        { ProfScope ps(c, 16, s); CU_TRY(c, launch_head(bufp(B_H3), fcw, fcw + 6 * 512, out_trans, out_rot, n, 121, s)); }
         ++c->launches;
-        if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(bufp(B_F2), out_feature, n, 22 * 22, 256, 0, s)); ++c->launches; }
+        if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(bufp(B_F2), out_feature, n, 22 * 22, 256, precision, s)); ++c->launches; }
         return SE3TN_OK;
     }
     // ---- tensor-core modes: 8 resident-weight launches + 1 trunk launch + head ----
     if (img_wid) { int rc = sync_tables(c, s); if (rc) return rc; }
-    const CUtensorMap* gbmaps = img_wid ? (kprec == PREC_BF16X3 ? c->d_bmaps_x3 : (kprec == PREC_BF16 ? c->d_bmaps_bf16 : c->d_bmaps_tf32)) : nullptr;
-    const float* const* gbias = img_wid ? c->d_bias : nullptr;
+    const CUtensorMap* gbmaps = img_wid ? c->d_bmaps[precision].get() : nullptr;
+    const float* const* gbias = img_wid ? c->d_bias.get() : nullptr;
     if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched, 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
     for (int li = 0; li < kFirstTrunkLayer; ++li) {
         ResidentParams rp;
-        fill_layer_desc(c, ws, li, kprec, rp.L);
+        fill_layer_desc(c, w, li, precision, rp.L);
         rp.img_first = first; rp.n_img = n;
         rp.m_tiles = n * rp.L.tiles_x * rp.L.tiles_y;
         if (kLayers[li].kind == K_STEM) { rp.step_x = rp.step_y = 10; rp.off_x = rp.off_y = -1; }   // 11x11 conv outputs from (10*t - 1): the 5x5 pooled block's window
         else { rp.step_x = rp.step_y = 11; rp.off_x = rp.off_y = 0; }
         rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias;
         rp.trace = c->trace ? c->trace + static_cast<size_t>(li) * 256 * 8 : nullptr;
-        { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, kprec, c->num_sms, c->pdl != 0, s)); }
+        { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, precision, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
@@ -482,7 +480,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         // with the throughput mode to rounding, not bit for bit; within the mode (n = 1..4) they do not depend on n.
         int ksplit = (n <= kSplitMaxImages) ? kSplitK : 1;
         for (int l = 0; l < 14 - kFirstTrunkLayer; ++l) {
-            fill_layer_desc(c, ws, kFirstTrunkLayer + l, kprec, tp.layer[l]);
+            fill_layer_desc(c, w, kFirstTrunkLayer + l, precision, tp.layer[l]);
             while (tp.layer[l].chunks % ksplit) ksplit /= 2;       // 2-byte storage: convAB1 has only two 128-byte chunks per pixel
         }
         int base = 0, base0 = 0;
@@ -502,21 +500,78 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         tp.sched = c->sched; tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias;
         tp.trace = c->trace ? c->trace + static_cast<size_t>(kFirstTrunkLayer) * 256 * 8 : nullptr;
         c->sched_dirty = true;                     // cleared again by the head kernel below
-        { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, kprec, c->num_sms, c->pdl != 0, s)); }
+        { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, precision, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
         ProfScope ps(c, 16, s);
         CU_TRY(c, launch_head_pooled(c->pool_part + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
-                                     img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc : nullptr,
+                                     img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc.get() : nullptr,
                                      pose ? pose->in : nullptr, pose ? pose->out : nullptr, pose ? pose->tn : 0.f, pose ? pose->rn : 0.f,
                                      c->sched, static_cast<int>(trunk_sched_words(c->max_batch)), s));
         c->sched_dirty = false;
         if (pose && pose_done) *pose_done = true;
     }
     ++c->launches;
-    if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(reinterpret_cast<const uint8_t*>(c->buf[B_F2]) + static_cast<size_t>(first) * 22 * 22 * 256 * prec_bytes_per_channel(kprec), out_feature, n, 22 * 22, 256,
-                                                       kprec == PREC_BF16X3 ? 1 : (kprec == PREC_BF16 ? 2 : 0), s)); ++c->launches; }
+    if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(reinterpret_cast<const uint8_t*>(c->buf[B_F2]) + static_cast<size_t>(first) * 22 * 22 * 256 * prec_bytes_per_channel(precision), out_feature, n, 22 * 22, 256,
+                                                       precision, s)); ++c->launches; }
+    return SE3TN_OK;
+}
+
+// Every form of a weight blob the kernels read, built into `w` (which owns all of it, so a failure leaves nothing behind).
+int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
+    const size_t floats = blob_floats();
+    CU_TRY(c, dev_alloc(w.blob, floats));
+    for (int p : kTensorPrecs) CU_TRY(c, dev_alloc(w.conv[p], floats * prec_bytes_per_channel(p)));
+    CU_TRY(c, dev_alloc(w.stack, 8 * 128 * 288 * sizeof(float)));
+    CU_TRY(c, dev_alloc(w.perm, 6 * 64 * 576));
+    DevBuf<float> perm_tmp;                        // one 64-channel layer's fp32 weights with permuted rows
+    CU_TRY(c, dev_alloc(perm_tmp, 64 * 576));
+    CU_TRY(c, cudaDeviceSynchronize());
+    CU_TRY(c, cudaMemcpy(w.blob.get(), blob, floats * sizeof(float), cudaMemcpyHostToDevice));
+    size_t off = 0;
+    for (int li = 0; li < 14; ++li) {
+        const LayerSpec& L = kLayers[li];
+        const int rows = layer_rows(L), ktot = layer_ktot(L);
+        w.w_off[li] = off; off += static_cast<size_t>(rows) * ktot;
+        w.b_off[li] = off; off += rows;
+        const float* wsrc = w.blob.get() + w.w_off[li];
+        auto conv_dst = [&](int p) { return w.conv[p].get() + w.w_off[li] * prec_bytes_per_channel(p); };
+        char what[64];
+        int rc = SE3TN_OK;
+        if (li >= kFirstTrunkLayer) {
+            // trunk layers: natural row order, tiles of {32 words, block_n rows} streamed through the weight ring
+            snprintf(what, sizeof what, "layer %d weights", li);
+            for (int p : kTensorPrecs) {
+                CU_TRY(c, launch_encode_weights(p, wsrc, conv_dst(p), rows, ktot, 0));
+                if (!rc) rc = make_map2(c, &w.bmap[p][li], conv_dst(p), ktot * prec_bytes_per_channel(p) / 4, rows, L.block_n, what);
+            }
+        } else {
+            // resident-weight layers.  Stems keep the natural row order; the 64-channel 3x3 layers use the row order of the
+            // accumulator fragment (all precisions).  BF16X3: hi / lo rows stacked along N.
+            const bool stem = (L.kind == K_STEM);
+            void* w_tf32 = conv_dst(SE3TN_PREC_TF32);
+            if (!stem) {
+                if (ktot != 576 || rows != 64) return fail(c, SE3TN_ERR_STATE, "resident layer shape");
+                CU_TRY(c, launch_permute_rows64(wsrc, perm_tmp.get(), 576, 0));
+                wsrc = perm_tmp.get(); w_tf32 = w.perm.get() + static_cast<size_t>(li - 2) * 64 * 576;
+            }
+            snprintf(what, sizeof what, "layer %d resident weights", li);
+            CU_TRY(c, launch_encode_weights(SE3TN_PREC_TF32, wsrc, w_tf32, 64, ktot, 0));
+            rc = make_map2(c, &w.bmap[SE3TN_PREC_TF32][li], w_tf32, ktot, 64, 64, what);
+            uint8_t* sdst = w.stack.get() + static_cast<size_t>(li) * 128 * 288 * sizeof(float);
+            CU_TRY(c, launch_split_stack_weights(wsrc, sdst, stem, 0));
+            if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_BF16X3][li], sdst, stem ? 224 : 288, 128, 128, what);
+            if (stem) w.bmap[SE3TN_PREC_BF16][li] = w.bmap[stem_input_prec(SE3TN_PREC_BF16)][li];   // the stem's input format decides
+            else {
+                CU_TRY(c, launch_encode_weights(SE3TN_PREC_BF16, wsrc, conv_dst(SE3TN_PREC_BF16), 64, ktot, 0));   // permuted rows
+                if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_BF16][li], conv_dst(SE3TN_PREC_BF16), 288, 64, 64, what);
+            }
+        }
+        if (rc) return rc;
+    }
+    w.fc_off = off;
+    CU_TRY(c, cudaDeviceSynchronize());            // a kernel that failed above fails the load
     return SE3TN_OK;
 }
 
@@ -598,9 +653,6 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
 void se3tn_destroy(se3tn_ctx* c) {
     if (!c) return;
     DeviceGuard guard(c->device);
-    for (auto& kv : c->weights) { cudaFree(kv.second.dev); cudaFree(kv.second.dev_tf32); cudaFree(kv.second.dev_bf16); cudaFree(kv.second.dev_h); cudaFree(kv.second.dev_stack); cudaFree(kv.second.dev_perm); cudaFree(kv.second.dev_perm_tmp); }
-    cudaFree(c->d_mean32); cudaFree(c->d_std32); cudaFree(c->d_mean64); cudaFree(c->d_std64);
-    cudaFree(c->d_bmaps_tf32); cudaFree(c->d_bmaps_bf16); cudaFree(c->d_bmaps_x3); cudaFree(c->d_bias); cudaFree(c->d_fc);
     for (int i = 0; i < SE3TN_PROFILE_SLOTS; ++i) { if (c->ev0[i]) cudaEventDestroy(c->ev0[i]); if (c->ev1[i]) cudaEventDestroy(c->ev1[i]); }
     drop_graphs(c);
     if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
@@ -610,7 +662,7 @@ void se3tn_destroy(se3tn_ctx* c) {
     cudaFree(c->fill.a); cudaFree(c->fill.b); cudaFree(c->fill.lut); cudaFree(c->fill.minmax);
     cudaFree(c->hio.dev); if (c->hio.pin) cudaFreeHost(c->hio.pin);
     if (c->own_workspace) cudaFree(c->workspace);
-    delete c;
+    delete c;                                      // frees the weight sets and per-set tables it owns
 }
 
 int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_floats) {
@@ -620,71 +672,15 @@ int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_
     if (n_floats != expect || expect != SE3TN_WEIGHT_BLOB_FLOATS)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_load_weights: blob has " + std::to_string(n_floats) + " floats, expected " + std::to_string(expect));
     DeviceGuard guard(c->device);
+    // the id counts as loaded only once every form of the new weights is ready: a failed load leaves it not loaded
     WeightSet& ws = c->weights[weight_id];
-    if (!ws.dev) {
-        CU_TRY(c, cudaMalloc(&ws.dev, expect * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&ws.dev_tf32, expect * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&ws.dev_bf16, expect * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&ws.dev_h, expect * sizeof(uint16_t)));
-        CU_TRY(c, cudaMalloc(&ws.dev_stack, 8 * 128 * 288 * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&ws.dev_perm, 6 * 64 * 576 * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&ws.dev_perm_tmp, 64 * 576 * sizeof(float)));
-    }
-    CU_TRY(c, cudaDeviceSynchronize());
-    CU_TRY(c, cudaMemcpy(ws.dev, blob, expect * sizeof(float), cudaMemcpyHostToDevice));
-    round_tf32_kernel<<<1024, 256>>>(ws.dev, ws.dev_tf32, expect);
-    CU_TRY(c, cudaGetLastError());
-    size_t off = 0;
-    for (int li = 0; li < 14; ++li) {
-        const LayerSpec& L = kLayers[li];
-        const size_t words = static_cast<size_t>(layer_rows(L)) * layer_ktot(L);
-        ws.w_off[li] = off; off += words;
-        ws.b_off[li] = off; off += layer_rows(L);
-        const float* wsrc = ws.dev + ws.w_off[li];
-        char what[64];
-        int rc = SE3TN_OK;
-        if (li >= kFirstTrunkLayer) {
-            // trunk layers: natural row order, tiles of {32 words, block_n rows} streamed through the weight ring
-            snprintf(what, sizeof what, "layer %d weights", li);
-            rc = make_map2(c, &ws.bmap_tf32[li], ws.dev_tf32 + ws.w_off[li], layer_ktot(L), layer_rows(L), L.block_n, what);
-            uint8_t* d3 = ws.dev_bf16 + ws.w_off[li] * sizeof(float);
-            CU_TRY(c, launch_split_weights(wsrc, d3, words, 0));                          // [32 hi | 32 lo] per 32-word K chunk
-            if (!rc) rc = make_map2(c, &ws.bmap_x3[li], d3, layer_ktot(L), layer_rows(L), L.block_n, what);
-            uint8_t* dh = ws.dev_h + ws.w_off[li] * sizeof(uint16_t);
-            CU_TRY(c, launch_to_bf16(wsrc, dh, words, 0));                                // plain bf16, 64 channels per 128-byte chunk
-            if (!rc) rc = make_map2(c, &ws.bmap_h[li], dh, layer_ktot(L) / 2, layer_rows(L), L.block_n, what);
-        } else {
-            // resident-weight layers.  Stems keep the natural row order; the 64-channel 3x3 layers use the row order of the
-            // accumulator fragment (all precisions).  bf16 modes: hi / lo rows stacked along N, except the 64-channel layers in PREC_BF16.
-            const bool stem = (L.kind == K_STEM);
-            const float* w_tf32 = ws.dev_tf32 + ws.w_off[li];
-            if (!stem) {
-                if (layer_ktot(L) != 576 || layer_rows(L) != 64) return fail(c, SE3TN_ERR_STATE, "resident layer shape");
-                float* pt = ws.dev_perm + static_cast<size_t>(li - 2) * 64 * 576;
-                CU_TRY(c, launch_permute_rows64(wsrc, ws.dev_perm_tmp, 576, 0));
-                round_tf32_kernel<<<144, 256>>>(ws.dev_perm_tmp, pt, 64 * 576);
-                CU_TRY(c, cudaGetLastError());
-                wsrc = ws.dev_perm_tmp; w_tf32 = pt;
-            }
-            snprintf(what, sizeof what, "layer %d resident weights", li);
-            rc = make_map2(c, &ws.bmap_tf32[li], w_tf32, layer_ktot(L), 64, 64, what);
-            uint8_t* sdst = ws.dev_stack + static_cast<size_t>(li) * 128 * 288 * sizeof(float);
-            CU_TRY(c, launch_split_stack_weights(wsrc, sdst, stem, 0));
-            if (!rc) rc = make_map2(c, &ws.bmap_x3[li], sdst, stem ? 224 : 288, 128, 128, what);
-            if (stem) ws.bmap_h[li] = ws.bmap_x3[li];                                      // the stem input is [4 hi | 4 lo] per pixel in both bf16 modes
-            else {
-                uint8_t* dh = ws.dev_h + ws.w_off[li] * sizeof(uint16_t);
-                CU_TRY(c, launch_to_bf16(wsrc, dh, words, 0));                            // permuted rows, plain bf16
-                if (!rc) rc = make_map2(c, &ws.bmap_h[li], dh, 288, 64, 64, what);
-            }
-            CU_TRY(c, cudaDeviceSynchronize());                                           // dev_perm_tmp is reused by the next layer
-        }
-        if (rc) return rc;
-    }
-    CU_TRY(c, cudaDeviceSynchronize());
-    ws.fc_off = off;
+    ws.dev.reset();
     c->tables_dirty = true;
     drop_graphs(c);                                // captured steps hold the old tensor maps / table pointers
+    std::unique_ptr<DeviceWeights> w(new DeviceWeights());
+    const int rc = prepare_weights(c, *w, blob);
+    if (rc) return rc;
+    ws.dev = std::move(w);
     return SE3TN_OK;
 }
 
@@ -723,8 +719,8 @@ int se3tn_preprocess(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     a.frame_rgb = frame_rgb; a.frame_depth = frame_depth; a.H = H; a.W = W;
     a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
     a.poses = poses; a.object_width = object_width; a.rgbA = rgbA; a.depthA = depthA; a.weight_ids = weight_ids;
-    a.mean32 = c->d_mean32; a.std32 = c->d_std32; a.mean64 = c->d_mean64; a.std64 = c->d_std64;
-    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.round_tf32 = store_mode_of(precision); a.b_precropped = 0;
+    a.mean32 = c->d_mean32.get(); a.std32 = c->d_std32.get(); a.mean64 = c->d_mean64.get(); a.std64 = c->d_std64.get();
+    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.precision = precision; a.b_precropped = 0;
     a.stemA = c->buf[B_X0A]; a.stemB = c->buf[B_X0B]; a.nchwA = out_A; a.nchwB = out_B;
     a.crop_rgb = crop_rgb; a.crop_depth = crop_depth;
     { ProfScope ps(c, 17, s); CU_TRY(c, launch_preprocess(a, n, s)); }
@@ -745,8 +741,8 @@ int se3tn_normalize(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, c
     memset(&a, 0, sizeof a);
     a.frame_rgb = rgbB; a.frame_depth = depthB; a.H = kImg; a.W = kImg; a.b_precropped = 1;
     a.poses = poses; a.rgbA = rgbA; a.depthA = depthA; a.weight_ids = weight_ids;
-    a.mean32 = c->d_mean32; a.std32 = c->d_std32; a.mean64 = c->d_mean64; a.std64 = c->d_std64;
-    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.round_tf32 = store_mode_of(precision);
+    a.mean32 = c->d_mean32.get(); a.std32 = c->d_std32.get(); a.mean64 = c->d_mean64.get(); a.std64 = c->d_std64.get();
+    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.precision = precision;
     a.stemA = c->buf[B_X0A]; a.stemB = c->buf[B_X0B]; a.nchwA = out_A; a.nchwB = out_B;
     { ProfScope ps(c, 17, s); CU_TRY(c, launch_preprocess(a, n, s)); }
     ++c->launches;
@@ -781,10 +777,9 @@ int se3tn_forward(se3tn_ctx* c, int weight_id, const float* A, const float* B, i
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     c->launches = 0;
-    const int round = store_mode_of(precision);
     { ProfScope ps(c, 19, s);
-      CU_TRY(c, launch_nchw_to_stem(A, c->buf[B_X0A], n, round, s));
-      CU_TRY(c, launch_nchw_to_stem(B, c->buf[B_X0B], n, round, s)); }
+      CU_TRY(c, launch_nchw_to_stem(A, c->buf[B_X0A], n, precision, s));
+      CU_TRY(c, launch_nchw_to_stem(B, c->buf[B_X0B], n, precision, s)); }
     c->launches += 2;
     return run_network(c, weight_id, 0, n, precision, out_trans, out_rot, out_feature, s);
 }

@@ -1,0 +1,123 @@
+// Storage formats of the tensor-core precisions (SE3TN_PREC_* of include/se3tn.h): how an activation or weight value of
+// each mode is laid out in bytes.  Every kernel that reads or writes these formats goes through this header.
+//
+//   SE3TN_PREC_TF32   : 4 bytes per channel, fp32 words rounded to tf32 (rna).
+//   SE3TN_PREC_BF16X3 : 4 bytes per channel, x = hi + lo as two bf16; per 32-channel (128-byte) chunk [32 x hi | 32 x lo],
+//                       so channel c's lo half sits 64 bytes behind its hi half.
+//   SE3TN_PREC_BF16   : 2 bytes per channel, plain bf16, 64 channels per 128-byte chunk.
+// Weight matrices use the same formats with a K-major row as the "pixel" and K as the channel.
+//
+// The helpers below are conversions, adds and address arithmetic only (no multiply-add), so they compile to the same
+// instructions in files built with and without -fmad=false.  They never load: a call site loads the raw words with the
+// cache policy it needs and hands them to decode().
+#pragma once
+#include "se3tn.h"
+#include "ptx.cuh"
+#include <cstdint>
+#include <cstring>
+#include <type_traits>
+#include <cuda_bf16.h>
+
+namespace se3tn {
+
+__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == SE3TN_PREC_BF16 ? 2 : 4; }
+
+// The stem INPUT (4 channels, 16 bytes per pixel in every mode) has a format of its own: tf32 words in SE3TN_PREC_TF32, and in
+// both bf16 modes the bf16x3 split of the 4 channels as [2 words hi | 2 words lo] (no 64-byte gap), raw fp32 in SE3TN_PREC_FP32.
+// So the stems of both bf16 modes run the bf16x3 arithmetic: stacked hi / lo weight rows (conv_wgmma.cu RCfg::kStack).
+__host__ __device__ constexpr int stem_input_prec(int prec) { return prec == SE3TN_PREC_BF16 ? SE3TN_PREC_BF16X3 : prec; }
+
+// The one hi / lo split: fp32 -> (bf16 hi, bf16 lo) with x ~= hi + lo, two values per 32-bit word (element 0 in the low half)
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    const float2 hf = __bfloat1622float2(h);
+    const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+__device__ __forceinline__ float2 unpack2(uint32_t w) {
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
+}
+
+// N consecutive channels (N = 4 or 8) of format PREC as the raw words they occupy: kPieces vector pieces of kPieceWords
+// words, piece q at byte offset q * kStride from Storage<PREC>::addr() (BF16X3: hi piece, lo piece).
+template <int PREC, int N> struct Raw {
+    static constexpr bool kHiLo = PREC == SE3TN_PREC_BF16X3;
+    static constexpr int kWords = N * prec_bytes_per_channel(PREC) / 4;
+    static constexpr int kPieces = kHiLo ? 2 : (kWords > 4 ? kWords / 4 : 1);
+    static constexpr int kPieceWords = kWords / kPieces;
+    static constexpr int kStride = kHiLo ? 64 : 16;
+    using Piece = std::conditional_t<kPieceWords == 4, uint4, uint2>;
+    uint32_t w[kWords];
+    __device__ __forceinline__ static const Piece* at(const uint8_t* p, int q) { return reinterpret_cast<const Piece*>(p + q * kStride); }
+    __device__ __forceinline__ Piece get(int q) const { Piece v; memcpy(&v, w + q * kPieceWords, sizeof v); return v; }
+    __device__ __forceinline__ void set(int q, Piece v) { memcpy(w + q * kPieceWords, &v, sizeof v); }
+    __device__ __forceinline__ void store(uint8_t* p) const {
+#pragma unroll
+        for (int q = 0; q < kPieces; ++q) *reinterpret_cast<Piece*>(p + q * kStride) = get(q);
+    }
+};
+
+template <int PREC> struct Storage {
+    static_assert(PREC == SE3TN_PREC_TF32 || PREC == SE3TN_PREC_BF16X3 || PREC == SE3TN_PREC_BF16, "tensor-core precision");
+    static constexpr int kBytes = prec_bytes_per_channel(PREC);     // per channel
+    static constexpr bool kHiLo = PREC == SE3TN_PREC_BF16X3;
+
+    // Byte address of channel c (c % 4 == 0 for a group of 4 or 8) of pixel `pix` in an NHWC buffer of C channels per pixel.
+    // In BF16X3 this is the hi half; the lo half is 64 bytes further.
+    __host__ __device__ __forceinline__ static size_t addr(size_t pix, int C, int c) {
+        if (kHiLo) return (pix * C + (c & ~31)) * 4 + (c & 31) * 2;
+        return (pix * C + c) * kBytes;
+    }
+
+    template <int N> __device__ __forceinline__ static Raw<PREC, N> encode(const float (&v)[N]) {
+        Raw<PREC, N> r;
+        if constexpr (PREC == SE3TN_PREC_TF32) {
+#pragma unroll
+            for (int i = 0; i < N; ++i) r.w[i] = __float_as_uint(ptx::to_tf32(v[i]));
+        } else if constexpr (kHiLo) {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) split2(v[2 * i], v[2 * i + 1], r.w[i], r.w[N / 2 + i]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) r.w[i] = pack_bf16(v[2 * i], v[2 * i + 1]);
+        }
+        return r;
+    }
+
+    template <int N> __device__ __forceinline__ static void decode(const Raw<PREC, N>& r, float (&v)[N]) {
+        if constexpr (PREC == SE3TN_PREC_TF32) {
+#pragma unroll
+            for (int i = 0; i < N; ++i) v[i] = __uint_as_float(r.w[i]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) {
+                const float2 h = unpack2(r.w[i]);
+                if constexpr (kHiLo) {
+                    const float2 l = unpack2(r.w[N / 2 + i]);
+                    v[2 * i] = h.x + l.x; v[2 * i + 1] = h.y + l.y;
+                } else {
+                    v[2 * i] = h.x; v[2 * i + 1] = h.y;
+                }
+            }
+        }
+    }
+};
+
+// One stem-input pixel (stem_input_prec above), as the 16 bytes stored
+__device__ __forceinline__ float4 encode_stem_pixel(float4 v, int prec) {
+    const float f[4] = {v.x, v.y, v.z, v.w};
+    uint4 w;
+    switch (stem_input_prec(prec)) {
+        case SE3TN_PREC_TF32: w = Storage<SE3TN_PREC_TF32>::encode(f).get(0); break;
+        case SE3TN_PREC_BF16X3: { const auto r = Storage<SE3TN_PREC_BF16X3>::encode(f); w = make_uint4(r.w[0], r.w[1], r.w[2], r.w[3]); break; }
+        default: return v;
+    }
+    return make_float4(__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w));
+}
+
+}  // namespace se3tn
