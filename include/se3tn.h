@@ -192,7 +192,8 @@ int se3tn_vocap(se3tn_ctx* ctx, const double* errs, int n, double* out_ap, void*
 
 /* The CAD model the renderer draws: what VispyRenderer.__init__ uploads as vertex / index buffers (reference
  * vispy_renderer.py:108-129).  HOST arrays, copied: pos float32 (nv,3) metres in the object frame, nrm float32 (nv,3)
- * unit normals, col uint8 (nv,3), faces int32 (nf,3).  mesh_id >= 0; a later call with the same id replaces the model. */
+ * unit normals, col uint8 (nv,3), faces int32 (nf,3).  mesh_id >= 0; a later call with the same id replaces the model;
+ * on failure the id keeps its previous model. */
 int se3tn_set_mesh(se3tn_ctx* ctx, int mesh_id, const float* pos, const float* nrm, const uint8_t* col,
                    const int32_t* faces, int nv, int nf);
 

@@ -17,6 +17,7 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 using namespace se3tn;
@@ -90,13 +91,35 @@ size_t blob_floats() {
 constexpr int kNumPrecs = 4;
 constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16};
 
-// An owned device allocation, freed with its owner (every entry point makes the context's device current first).
-struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
-template <typename T> using DevBuf = std::unique_ptr<T[], CudaFree>;
+// Owned CUDA resources, released with their owner (every entry point makes the context's device current first).
+struct CudaRelease {
+    void operator()(void* p) const { cudaFree(p); }                  // device memory
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+    void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); }
+};
+struct CudaFreeHost { void operator()(uint8_t* p) const { cudaFreeHost(p); } };   // pinned host memory
+template <typename T> using DevBuf = std::unique_ptr<T[], CudaRelease>;
+using PinBuf = std::unique_ptr<uint8_t[], CudaFreeHost>;
+template <typename H> using Handle = std::unique_ptr<std::remove_pointer_t<H>, CudaRelease>;
+
 template <typename T> cudaError_t dev_alloc(DevBuf<T>& b, size_t n) {
     void* p = nullptr;
     const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
     if (e == cudaSuccess) b.reset(static_cast<T*>(p));
+    return e;
+}
+
+// Makes b hold at least n elements (a PinBuf holds bytes).  A larger buffer replaces b, and cap (how many b holds) changes,
+// only once it exists; the caller makes sure no queued work still uses the old buffer.
+template <typename B, typename N> cudaError_t grow(B& b, N& cap, N n) {
+    if (n <= cap) return cudaSuccess;
+    cudaError_t e;
+    if constexpr (std::is_same_v<B, PinBuf>) {
+        void* p = nullptr;
+        if ((e = cudaHostAlloc(&p, n, cudaHostAllocDefault)) == cudaSuccess) b.reset(static_cast<uint8_t*>(p));
+    } else e = dev_alloc(b, n);
+    if (e == cudaSuccess) cap = n;
     return e;
 }
 
@@ -119,6 +142,12 @@ struct WeightSet {
     bool has_stats = false;
 };
 
+// One CAD model of the rasteriser in device memory; view() is the kernels' non-owning MeshDev.
+struct Mesh {
+    DevBuf<float> pos, nrm; DevBuf<uint8_t> col; DevBuf<int> faces; int nv = 0, nf = 0;
+    MeshDev view() const { return {pos.get(), nrm.get(), col.get(), faces.get(), nv, nf}; }
+};
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -131,21 +160,21 @@ struct se3tn_ctx {
     int device = 0;
     int max_batch = 0;
     int num_sms = 0;
-    bool own_workspace = false;
-    uint8_t* workspace = nullptr;
+    uint8_t* workspace = nullptr;    // the caller's, or own_workspace
+    DevBuf<uint8_t> own_workspace;   // set only when the library allocated the workspace
     float* buf[B_COUNT] = {};
     CUtensorMap amap4[14][4];        // activation views, 4 bytes per channel (TF32 / BF16X3; also the stems' input in every mode)
     CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16, layers 2..13)
     int pdl = 1;                     // SE3TN_PDL=0 disables programmatic dependent launch between the kernels of a step
-    std::map<int, MeshDev> meshes;   // CAD models of the rasteriser (device copies), keyed by mesh id
-    MeshDev* d_meshes = nullptr; int mesh_rows = 0; bool meshes_dirty = false;
-    uint8_t* render_proj = nullptr; uint8_t* render_unif = nullptr; int render_max_nv = 0, render_proj_nv = 0;   // rasteriser workspace
-    FillScratch fill = {nullptr, nullptr, nullptr, nullptr}; size_t fill_pixels = 0;   // depth hole-filling scratch (grows on demand)
-    float* pool_part = nullptr;      // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
-    unsigned* sched = nullptr;       // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
-    float* partial = nullptr;        // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
+    std::map<int, Mesh> meshes;      // CAD models of the rasteriser, keyed by mesh id
+    DevBuf<MeshDev> d_meshes; int mesh_rows = 0; bool meshes_dirty = false;   // device table of their views, rebuilt when a model changes
+    DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
+    DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, so all four exist or none (grows on demand)
+    DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
+    DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
+    DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
     bool sched_dirty = false;        // a step failed between the trunk launch and the head launch: clear before the next one
-    unsigned long long* trace = nullptr;   // SE3TN_TRACE=1: [14 slots][256 CTAs][8] globaltimer stamps of the last forward (conv_wgmma.cu trace_stamp)
+    DevBuf<unsigned long long> trace;   // SE3TN_TRACE=1: [14 slots][256 CTAs][8] globaltimer stamps of the last forward (conv_wgmma.cu trace_stamp)
     EncodeTiledFn encode = nullptr;
     std::map<int, WeightSet> weights;
     // device copies of per-set stats, rebuilt when a set changes: [max_id+1][8]
@@ -160,15 +189,15 @@ struct se3tn_ctx {
     // CUDA graphs of whole track_batch steps (preprocess -> 8 resident convs -> trunk -> head + pose update), keyed by every baked-in argument
     int use_graphs = 1;              // SE3TN_GRAPH=0: plain stream launches; set to 0 at run time if capture is not possible
     bool last_was_graph = false;
-    struct StepGraph { std::vector<unsigned long long> key; cudaGraphExec_t exec; int launches; unsigned long long last_use; };
+    struct StepGraph { std::vector<unsigned long long> key; Handle<cudaGraphExec_t> exec; int launches; unsigned long long last_use; };
     std::vector<StepGraph> graphs; unsigned long long graph_clock = 0;
-    cudaStream_t cap_stream = nullptr;   // steps are captured on this private stream (the caller's may be the legacy default stream, which cannot be captured) and replayed on the caller's
-    cudaEvent_t ev0[SE3TN_PROFILE_SLOTS] = {}, ev1[SE3TN_PROFILE_SLOTS] = {};
+    Handle<cudaStream_t> cap_stream;   // steps are captured on this private stream (the caller's may be the legacy default stream, which cannot be captured) and replayed on the caller's
+    Handle<cudaEvent_t> ev[2][SE3TN_PROFILE_SLOTS];   // start, end of each profiling slot
     bool ev_used[SE3TN_PROFILE_SLOTS] = {};
     // se3tn_track_host: context-owned pinned staging and device-side inputs / outputs (stable addresses -> the step's graph is reused)
     struct HostIO {
-        uint8_t* pin = nullptr; size_t pin_bytes = 0;          // pinned host staging: inputs, then outputs
-        uint8_t* dev = nullptr; size_t dev_bytes = 0;          // device: frame rgb | frame depth | poses | widths | rgbA | depthA | ids | out poses | out trans | out rot
+        PinBuf pin; size_t pin_bytes = 0;                      // pinned host staging: inputs, then outputs
+        DevBuf<uint8_t> dev; size_t dev_bytes = 0;             // device: frame rgb | frame depth | poses | widths | rgbA | depthA | ids | out poses | out trans | out rot
         int H = 0, W = 0, n_cap = 0;
     } hio;
     std::string err;
@@ -194,9 +223,9 @@ struct DeviceGuard {
 struct ProfScope {
     se3tn_ctx* c; int slot; cudaStream_t s;
     ProfScope(se3tn_ctx* c_, int slot_, cudaStream_t s_) : c(c_), slot(slot_), s(s_) {
-        if (c->profiling) { cudaEventRecord(c->ev0[slot], s); }
+        if (c->profiling) { cudaEventRecord(c->ev[0][slot].get(), s); }
     }
-    ~ProfScope() { if (c->profiling) { cudaEventRecord(c->ev1[slot], s); c->ev_used[slot] = true; } }
+    ~ProfScope() { if (c->profiling) { cudaEventRecord(c->ev[1][slot].get(), s); c->ev_used[slot] = true; } }
 };
 
 size_t workspace_floats(int max_batch) {
@@ -413,11 +442,6 @@ int sync_tables(se3tn_ctx* c, cudaStream_t s) {
     return SE3TN_OK;
 }
 
-void drop_graphs(se3tn_ctx* c) {
-    for (auto& g : c->graphs) cudaGraphExecDestroy(g.exec);
-    c->graphs.clear();
-}
-
 // optional pose update fused into the head kernel (tensor-core modes): K6 for the same n tracks
 struct PoseArgs { const double* in = nullptr; double* out = nullptr; float tn = 0.f, rn = 0.f; };
 
@@ -459,7 +483,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     if (img_wid) { int rc = sync_tables(c, s); if (rc) return rc; }
     const CUtensorMap* gbmaps = img_wid ? c->d_bmaps[precision].get() : nullptr;
     const float* const* gbias = img_wid ? c->d_bias.get() : nullptr;
-    if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched, 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
+    if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
     for (int li = 0; li < kFirstTrunkLayer; ++li) {
         ResidentParams rp;
         fill_layer_desc(c, w, li, precision, rp.L);
@@ -468,7 +492,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         if (kLayers[li].kind == K_STEM) { rp.step_x = rp.step_y = 10; rp.off_x = rp.off_y = -1; }   // 11x11 conv outputs from (10*t - 1): the 5x5 pooled block's window
         else { rp.step_x = rp.step_y = 11; rp.off_x = rp.off_y = 0; }
         rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias;
-        rp.trace = c->trace ? c->trace + static_cast<size_t>(li) * 256 * 8 : nullptr;
+        rp.trace = c->trace ? c->trace.get() + static_cast<size_t>(li) * 256 * 8 : nullptr;
         { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, precision, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
@@ -492,23 +516,23 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
             if (l > 0) { d.dep_layer = l - 1; d.dep_target = 8u * static_cast<unsigned>(ksplit) * static_cast<unsigned>(tp.layer[l - 1].units_per_image); }
         }
         if (ksplit > 1 && base0 > kSplitMaxUnits) return fail(c, SE3TN_ERR_STATE, "split-K scratch too small");
-        tp.ksplit = ksplit; tp.partial = c->partial;
-        tp.slice_cnt = c->sched + 1 + static_cast<size_t>(kTrunkMaxLayers) * c->max_batch;
-        tp.layer[5].pool_part = c->pool_part;      // AdaptiveAvgPool2d(1) fused into the last conv's epilogue (indexed by absolute image)
+        tp.ksplit = ksplit; tp.partial = c->partial.get();
+        tp.slice_cnt = c->sched.get() + 1 + static_cast<size_t>(kTrunkMaxLayers) * c->max_batch;
+        tp.layer[5].pool_part = c->pool_part.get();   // AdaptiveAvgPool2d(1) fused into the last conv's epilogue (indexed by absolute image)
         tp.n_layers = 6; tp.total_units = base;
         tp.img_first = first; tp.n_img = n; tp.max_batch = c->max_batch;
-        tp.sched = c->sched; tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias;
-        tp.trace = c->trace ? c->trace + static_cast<size_t>(kFirstTrunkLayer) * 256 * 8 : nullptr;
+        tp.sched = c->sched.get(); tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias;
+        tp.trace = c->trace ? c->trace.get() + static_cast<size_t>(kFirstTrunkLayer) * 256 * 8 : nullptr;
         c->sched_dirty = true;                     // cleared again by the head kernel below
         { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, precision, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
         ProfScope ps(c, 16, s);
-        CU_TRY(c, launch_head_pooled(c->pool_part + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
+        CU_TRY(c, launch_head_pooled(c->pool_part.get() + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
                                      img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc.get() : nullptr,
                                      pose ? pose->in : nullptr, pose ? pose->out : nullptr, pose ? pose->tn : 0.f, pose ? pose->rn : 0.f,
-                                     c->sched, static_cast<int>(trunk_sched_words(c->max_batch)), s));
+                                     c->sched.get(), static_cast<int>(trunk_sched_words(c->max_batch)), s));
         c->sched_dirty = false;
         if (pose && pose_done) *pose_done = true;
     }
@@ -602,39 +626,38 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
         return fail(nullptr, SE3TN_ERR_UNSUPPORTED, "se3tn_create: device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
                                                     ", this library is sm_90a only (no fallback path)");
     DeviceGuard guard(device);
-    se3tn_ctx* c = new se3tn_ctx();
+    std::unique_ptr<se3tn_ctx> ctx(new se3tn_ctx());   // released by any early return below, while the device is still current
+    se3tn_ctx* c = ctx.get();
     c->device = device; c->max_batch = max_batch; c->num_sms = prop.multiProcessorCount;
     if (const char* ov = getenv("SE3TN_PDL")) c->pdl = atoi(ov) != 0;
     if (const char* ov = getenv("SE3TN_GRAPH")) c->use_graphs = atoi(ov) != 0;
-    if (const char* ov = getenv("SE3TN_TRACE")) {
-        if (atoi(ov) != 0 && cudaMalloc(&c->trace, SE3TN_TRACE_WORDS * sizeof(unsigned long long)) == cudaSuccess) cudaMemset(c->trace, 0, SE3TN_TRACE_WORDS * sizeof(unsigned long long));
-    }
+    if (const char* ov = getenv("SE3TN_TRACE"); ov && atoi(ov) != 0 && dev_alloc(c->trace, SE3TN_TRACE_WORDS) == cudaSuccess)
+        cudaMemset(c->trace.get(), 0, SE3TN_TRACE_WORDS * sizeof(unsigned long long));
 
     void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
     e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) {
-        delete c; return fail(nullptr, SE3TN_ERR_CUDA, "se3tn_create: cuTensorMapEncodeTiled entry point unavailable");
-    }
+    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn)
+        return fail(nullptr, SE3TN_ERR_CUDA, "se3tn_create: cuTensorMapEncodeTiled entry point unavailable");
     c->encode = reinterpret_cast<EncodeTiledFn>(fn);
 
     const size_t bytes = se3tn_workspace_bytes(max_batch);
     if (workspace) {
-        if (reinterpret_cast<uintptr_t>(workspace) % 1024) { delete c; return fail(nullptr, SE3TN_ERR_INVALID, "se3tn_create: workspace must be 1024-byte aligned"); }
+        if (reinterpret_cast<uintptr_t>(workspace) % 1024) return fail(nullptr, SE3TN_ERR_INVALID, "se3tn_create: workspace must be 1024-byte aligned");
         c->workspace = static_cast<uint8_t*>(workspace);
     } else {
-        e = cudaMalloc(&c->workspace, bytes);
-        if (e != cudaSuccess) { delete c; return fail(nullptr, SE3TN_ERR_NOMEM, std::string("se3tn_create: cudaMalloc(workspace): ") + cudaGetErrorString(e)); }
-        c->own_workspace = true;
+        e = dev_alloc(c->own_workspace, bytes);
+        if (e != cudaSuccess) return fail(nullptr, SE3TN_ERR_NOMEM, std::string("se3tn_create: cudaMalloc(workspace): ") + cudaGetErrorString(e));
+        c->workspace = c->own_workspace.get();
     }
-    e = cudaMalloc(&c->pool_part, static_cast<size_t>(max_batch) * kPoolSlices * 1024 * sizeof(float));
-    if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); se3tn_destroy(c); return fail(nullptr, SE3TN_ERR_NOMEM, "se3tn_create: pool buffer: " + m); }
-    e = cudaMalloc(&c->partial, trunk_partial_floats() * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&c->sched, trunk_sched_words(max_batch) * sizeof(unsigned));
-    if (e == cudaSuccess) e = cudaMemset(c->sched, 0, trunk_sched_words(max_batch) * sizeof(unsigned));
-    if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); se3tn_destroy(c); return fail(nullptr, SE3TN_ERR_NOMEM, "se3tn_create: scheduler state: " + m); }
+    e = dev_alloc(c->pool_part, static_cast<size_t>(max_batch) * kPoolSlices * 1024);
+    if (e != cudaSuccess) return fail(nullptr, SE3TN_ERR_NOMEM, std::string("se3tn_create: pool buffer: ") + cudaGetErrorString(e));
+    e = dev_alloc(c->partial, trunk_partial_floats());
+    if (e == cudaSuccess) e = dev_alloc(c->sched, trunk_sched_words(max_batch));
+    if (e == cudaSuccess) e = cudaMemset(c->sched.get(), 0, trunk_sched_words(max_batch) * sizeof(unsigned));
+    if (e != cudaSuccess) return fail(nullptr, SE3TN_ERR_NOMEM, std::string("se3tn_create: scheduler state: ") + cudaGetErrorString(e));
     // zero once: the stem buffers' 3-pixel halo is the conv padding and is never written again
     e = cudaMemset(c->workspace, 0, bytes);
-    if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); se3tn_destroy(c); return fail(nullptr, SE3TN_ERR_CUDA, "se3tn_create: cudaMemset: " + m); }
+    if (e != cudaSuccess) return fail(nullptr, SE3TN_ERR_CUDA, std::string("se3tn_create: cudaMemset: ") + cudaGetErrorString(e));
     float* p = reinterpret_cast<float*>(c->workspace);
     for (int b = 0; b < B_COUNT; ++b) {
         c->buf[b] = p;
@@ -642,27 +665,18 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
     }
     int rc = build_activation_maps(c, 4, c->amap4);
     if (!rc) rc = build_activation_maps(c, 2, c->amap2);
-    if (rc) { g_create_error = c->err; se3tn_destroy(c); return rc; }
+    if (rc) return fail(nullptr, rc, c->err);
     // the memsets above ran on the NULL stream: later launches may use non-blocking streams, which do not wait for it
     e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); se3tn_destroy(c); return fail(nullptr, SE3TN_ERR_CUDA, "se3tn_create: " + m); }
-    *out = c;
+    if (e != cudaSuccess) return fail(nullptr, SE3TN_ERR_CUDA, std::string("se3tn_create: ") + cudaGetErrorString(e));
+    *out = ctx.release();
     return SE3TN_OK;
 }
 
 void se3tn_destroy(se3tn_ctx* c) {
     if (!c) return;
     DeviceGuard guard(c->device);
-    for (int i = 0; i < SE3TN_PROFILE_SLOTS; ++i) { if (c->ev0[i]) cudaEventDestroy(c->ev0[i]); if (c->ev1[i]) cudaEventDestroy(c->ev1[i]); }
-    drop_graphs(c);
-    if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
-    cudaFree(c->sched); cudaFree(c->partial); cudaFree(c->pool_part); cudaFree(c->trace);
-    for (auto& kv : c->meshes) { cudaFree(const_cast<float*>(kv.second.pos)); cudaFree(const_cast<float*>(kv.second.nrm)); cudaFree(const_cast<uint8_t*>(kv.second.col)); cudaFree(const_cast<int*>(kv.second.faces)); }
-    cudaFree(c->d_meshes); cudaFree(c->render_proj); cudaFree(c->render_unif);
-    cudaFree(c->fill.a); cudaFree(c->fill.b); cudaFree(c->fill.lut); cudaFree(c->fill.minmax);
-    cudaFree(c->hio.dev); if (c->hio.pin) cudaFreeHost(c->hio.pin);
-    if (c->own_workspace) cudaFree(c->workspace);
-    delete c;                                      // frees the weight sets and per-set tables it owns
+    delete c;                                      // the context owns every resource it holds
 }
 
 int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_floats) {
@@ -676,7 +690,7 @@ int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_
     WeightSet& ws = c->weights[weight_id];
     ws.dev.reset();
     c->tables_dirty = true;
-    drop_graphs(c);                                // captured steps hold the old tensor maps / table pointers
+    c->graphs.clear();                             // captured steps hold the old tensor maps / table pointers
     std::unique_ptr<DeviceWeights> w(new DeviceWeights());
     const int rc = prepare_weights(c, *w, blob);
     if (rc) return rc;
@@ -699,7 +713,7 @@ int se3tn_set_stats(se3tn_ctx* c, int weight_id, const void* mean8, const void* 
     }
     ws.stats_f64 = is_f64 ? 1 : 0; ws.has_stats = true;
     c->stats_dirty = true;
-    drop_graphs(c);
+    c->graphs.clear();
     return SE3TN_OK;
 }
 
@@ -860,22 +874,24 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         key.push_back(bits(tn)); key.push_back(bits(rn));
         for (auto& g : c->graphs)
             if (g.key == key) {
-                CU_TRY(c, cudaGraphLaunch(g.exec, s));
+                CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
                 g.last_use = ++c->graph_clock; c->launches = g.launches; c->last_was_graph = true;
                 return SE3TN_OK;
             }
         // a new step shape: host-side table refreshes (synchronous copies) must not happen inside the capture
         int rc0 = sync_stats(c, s); if (rc0) return rc0;
         if (multi) { rc0 = sync_tables(c, s); if (rc0) return rc0; }
-        if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched, 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
-        if (!c->cap_stream && cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); c->cap_stream = nullptr; c->use_graphs = 0; key.clear(); }
-        if (!key.empty() && cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeRelaxed) != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
+        if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
+        cudaStream_t cs = nullptr;
+        if (!c->cap_stream && cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess) c->cap_stream.reset(cs);
+        if (!c->cap_stream) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
+        if (!key.empty() && cudaStreamBeginCapture(c->cap_stream.get(), cudaStreamCaptureModeRelaxed) != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
     }
     const bool capturing = graphable && !key.empty();
     auto end_capture = [&](int rc_launch) -> int {
         // turn what was recorded into an executable graph and run it; any failure falls back to plain stream launches for good
         cudaGraph_t graph = nullptr;
-        cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
+        cudaError_t e = cudaStreamEndCapture(c->cap_stream.get(), &graph);
         if (rc_launch != SE3TN_OK || e != cudaSuccess || !graph) {
             if (graph) cudaGraphDestroy(graph);
             cudaGetLastError(); c->use_graphs = 0; c->sched_dirty = true;
@@ -885,19 +901,16 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         e = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
         if (e != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; return 1; }
-        if (c->graphs.size() >= 64) {                          // evict the least recently used step
-            size_t lru = 0;
-            for (size_t i = 1; i < c->graphs.size(); ++i) if (c->graphs[i].last_use < c->graphs[lru].last_use) lru = i;
-            cudaGraphExecDestroy(c->graphs[lru].exec); c->graphs.erase(c->graphs.begin() + lru);
-        }
-        c->graphs.push_back({key, exec, c->launches, ++c->graph_clock});
+        if (c->graphs.size() >= 64)                            // evict the least recently used step
+            c->graphs.erase(std::min_element(c->graphs.begin(), c->graphs.end(), [](const auto& a, const auto& b) { return a.last_use < b.last_use; }));
+        c->graphs.push_back({key, Handle<cudaGraphExec_t>(exec), c->launches, ++c->graph_clock});
         CU_TRY(c, cudaGraphLaunch(exec, s));
         c->last_was_graph = true;
         return SE3TN_OK;
     };
     if (capturing) {
         const int rc = track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_host, weight_ids_dev, n,
-                                            tn, rn, precision, out_trans, out_rot, poses_out, multi, c->cap_stream);
+                                            tn, rn, precision, out_trans, out_rot, poses_out, multi, c->cap_stream.get());
         const int grc = end_capture(rc);
         if (grc == SE3TN_OK) return SE3TN_OK;
         if (grc != 1) return grc;                              // a real launch error
@@ -1008,16 +1021,13 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
         CU_TRY(c, cudaStreamSynchronize(s));
         const int cap = std::max(n, io.n_cap);
         const size_t per = 128 + 8 + img * 3 + img * 2 + 4 + 128 + 12 + 12;
-        const size_t dev_bytes = align256(px * 3) + align256(px * 2) + align256(per * cap) + 8 * 256;
-        cudaFree(io.dev); io.dev = nullptr; if (io.pin) { cudaFreeHost(io.pin); io.pin = nullptr; }
-        io.H = io.W = io.n_cap = 0;
-        CU_TRY(c, cudaMalloc(&io.dev, dev_bytes));
-        CU_TRY(c, cudaMemsetAsync(io.dev, 0, dev_bytes, s));    // on the caller's stream, ahead of the copies below; frame pixels outside the uploaded windows are never read, keep them defined
-        CU_TRY(c, cudaHostAlloc(&io.pin, px * 5 + per * cap + 4096, cudaHostAllocDefault));
-        io.dev_bytes = dev_bytes; io.pin_bytes = px * 5 + per * cap + 4096; io.H = H; io.W = W; io.n_cap = cap;
-        drop_graphs(c);                                          // steps captured against the old addresses
+        c->graphs.clear();                                       // before the buffers are replaced: captured steps hold their addresses
+        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 8 * 256));
+        CU_TRY(c, grow(io.pin, io.pin_bytes, px * 5 + per * cap + 4096));
+        CU_TRY(c, cudaMemsetAsync(io.dev.get(), 0, io.dev_bytes, s));   // on the caller's stream, ahead of the copies below; frame pixels outside the uploaded windows are never read, keep them defined
+        io.H = H; io.W = W; io.n_cap = cap;
     }
-    uint8_t* d = io.dev;
+    uint8_t* d = io.dev.get();
     uint8_t* d_rgb = d; d += align256(px * 3);
     uint16_t* d_depth = reinterpret_cast<uint16_t*>(d); d += align256(px * 2);
     // the per-track arrays are packed by THIS call's n (a step's graph is keyed by n anyway), inputs first, outputs behind them:
@@ -1048,7 +1058,7 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     if (y1 <= y0 || x1 <= x0) { y0 = y1 = x0 = x1 = 0; }         // every window misses the frame: nothing of it is read
     if (static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
-    uint8_t* hp = io.pin;
+    uint8_t* hp = io.pin.get();
     const int wh = y1 - y0, ww = x1 - x0;
     if (wh > 0 && ww > 0) {
         uint8_t* st_rgb = hp; hp += static_cast<size_t>(wh) * ww * 3;
@@ -1061,7 +1071,7 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
         CU_TRY(c, cudaMemcpy2DAsync(d_rgb + off * 3, static_cast<size_t>(W) * 3, st_rgb, static_cast<size_t>(ww) * 3, static_cast<size_t>(ww) * 3, wh, cudaMemcpyHostToDevice, s));
         CU_TRY(c, cudaMemcpy2DAsync(d_depth + off, static_cast<size_t>(W) * 2, st_dep, static_cast<size_t>(ww) * 2, static_cast<size_t>(ww) * 2, wh, cudaMemcpyHostToDevice, s));
     }
-    hp = io.pin + align256(static_cast<size_t>(hp - io.pin));
+    hp = io.pin.get() + align256(static_cast<size_t>(hp - io.pin.get()));
     memcpy(hp, poses, nn * 128);
     memcpy(hp + o_ow, object_width, nn * 8);
     memcpy(hp + o_rgbA, rgbA, nn * img * 3);
@@ -1109,19 +1119,13 @@ int se3tn_fill_depth_ex(se3tn_ctx* c, const uint16_t* depth_mm, int H, int W, do
         return fail(c, SE3TN_ERR_INVALID, "se3tn_fill_depth: bad arguments");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
-    const size_t px = static_cast<size_t>(H) * W;
-    if (px > c->fill_pixels) {
-        CU_TRY(c, cudaStreamSynchronize(s));
-        cudaFree(c->fill.a); cudaFree(c->fill.b); c->fill.a = c->fill.b = nullptr; c->fill_pixels = 0;
-        CU_TRY(c, cudaMalloc(&c->fill.a, px * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&c->fill.b, px * sizeof(float)));
-        c->fill_pixels = px;
-    }
-    if (!c->fill.lut) {
-        CU_TRY(c, cudaMalloc(&c->fill.lut, (kFillLutEntries + 1) * sizeof(float)));
-        CU_TRY(c, cudaMalloc(&c->fill.minmax, 2 * sizeof(unsigned)));
-    }
-    CU_TRY(c, launch_fill_depth(depth_mm, H, W, static_cast<float>(max_depth), extrapolate != 0, blur_type == SE3TN_BLUR_GAUSSIAN, c->fill, out_mm, out_m, s));
+    const size_t plane = align256(static_cast<size_t>(H) * W * sizeof(float)), lut = align256((kFillLutEntries + 1) * sizeof(float)), bytes = 2 * plane + lut + 2 * sizeof(unsigned);
+    if (bytes > c->fill_bytes) CU_TRY(c, cudaStreamSynchronize(s));   // the block is about to be replaced
+    CU_TRY(c, grow(c->fill, c->fill_bytes, bytes));
+    uint8_t* f = c->fill.get();
+    const FillScratch sc = {reinterpret_cast<float*>(f), reinterpret_cast<float*>(f + plane), reinterpret_cast<float*>(f + 2 * plane),
+                            reinterpret_cast<unsigned*>(f + 2 * plane + lut)};
+    CU_TRY(c, launch_fill_depth(depth_mm, H, W, static_cast<float>(max_depth), extrapolate != 0, blur_type == SE3TN_BLUR_GAUSSIAN, sc, out_mm, out_m, s));
     c->launches += 8;
     return SE3TN_OK;
 }
@@ -1140,19 +1144,16 @@ int se3tn_set_mesh(se3tn_ctx* c, int mesh_id, const float* pos, const float* nrm
         if (faces[i] < 0 || faces[i] >= nv) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_mesh: face index out of range");
     DeviceGuard guard(c->device);
     CU_TRY(c, cudaDeviceSynchronize());
-    MeshDev& m = c->meshes[mesh_id];
-    cudaFree(const_cast<float*>(m.pos)); cudaFree(const_cast<float*>(m.nrm)); cudaFree(const_cast<uint8_t*>(m.col)); cudaFree(const_cast<int*>(m.faces));
-    m = MeshDev{};
-    float* dpos; float* dnrm; uint8_t* dcol; int* dfaces;
-    CU_TRY(c, cudaMalloc(&dpos, sizeof(float) * 3 * nv)); m.pos = dpos;
-    CU_TRY(c, cudaMalloc(&dnrm, sizeof(float) * 3 * nv)); m.nrm = dnrm;
-    CU_TRY(c, cudaMalloc(&dcol, 3 * static_cast<size_t>(nv))); m.col = dcol;
-    CU_TRY(c, cudaMalloc(&dfaces, sizeof(int) * 3 * nf)); m.faces = dfaces;
-    CU_TRY(c, cudaMemcpy(dpos, pos, sizeof(float) * 3 * nv, cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(dnrm, nrm, sizeof(float) * 3 * nv, cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(dcol, col, 3 * static_cast<size_t>(nv), cudaMemcpyHostToDevice));
-    CU_TRY(c, cudaMemcpy(dfaces, faces, sizeof(int) * 3 * nf, cudaMemcpyHostToDevice));
-    m.nv = nv; m.nf = nf;
+    Mesh m; m.nv = nv; m.nf = nf;                  // the id's previous model stays in place until this one is complete
+    CU_TRY(c, dev_alloc(m.pos, 3 * static_cast<size_t>(nv)));
+    CU_TRY(c, dev_alloc(m.nrm, 3 * static_cast<size_t>(nv)));
+    CU_TRY(c, dev_alloc(m.col, 3 * static_cast<size_t>(nv)));
+    CU_TRY(c, dev_alloc(m.faces, 3 * static_cast<size_t>(nf)));
+    CU_TRY(c, cudaMemcpy(m.pos.get(), pos, sizeof(float) * 3 * nv, cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(m.nrm.get(), nrm, sizeof(float) * 3 * nv, cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(m.col.get(), col, 3 * static_cast<size_t>(nv), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(m.faces.get(), faces, sizeof(int) * 3 * nf, cudaMemcpyHostToDevice));
+    c->meshes[mesh_id] = std::move(m);             // frees the previous model: the device table is rebuilt before the next render
     c->meshes_dirty = true;
     return SE3TN_OK;
 }
@@ -1177,26 +1178,22 @@ int se3tn_render_ex(se3tn_ctx* c, const double* K, const double* poses, const do
     if (c->meshes_dirty) {
         const int rows = c->meshes.rbegin()->first + 1;
         CU_TRY(c, cudaStreamSynchronize(s));
-        if (rows > c->mesh_rows) { cudaFree(c->d_meshes); CU_TRY(c, cudaMalloc(&c->d_meshes, sizeof(MeshDev) * rows)); c->mesh_rows = rows; }
-        std::vector<MeshDev> tab(rows, c->meshes.begin()->second);      // unused ids alias the first model
-        for (auto& kv : c->meshes) tab[kv.first] = kv.second;
-        CU_TRY(c, cudaMemcpy(c->d_meshes, tab.data(), sizeof(MeshDev) * rows, cudaMemcpyHostToDevice));
-        c->render_max_nv = 0;
-        for (auto& kv : c->meshes) c->render_max_nv = std::max(c->render_max_nv, kv.second.nv);
-        if (c->render_max_nv > c->render_proj_nv) {          // projected-vertex workspace: max_batch x largest model
-            cudaFree(c->render_proj); c->render_proj = nullptr;
-            CU_TRY(c, cudaMalloc(&c->render_proj, static_cast<size_t>(c->max_batch) * c->render_max_nv * render_projected_bytes_per_vertex()));
-            c->render_proj_nv = c->render_max_nv;
-        }
-        if (!c->render_unif) CU_TRY(c, cudaMalloc(&c->render_unif, static_cast<size_t>(c->max_batch) * render_uniform_bytes()));
+        CU_TRY(c, grow(c->d_meshes, c->mesh_rows, rows));
+        std::vector<MeshDev> tab(rows, c->meshes.begin()->second.view());   // unused ids alias the first model
+        int max_nv = 0;
+        for (auto& kv : c->meshes) { tab[kv.first] = kv.second.view(); max_nv = std::max(max_nv, kv.second.nv); }
+        CU_TRY(c, cudaMemcpy(c->d_meshes.get(), tab.data(), sizeof(MeshDev) * rows, cudaMemcpyHostToDevice));
+        CU_TRY(c, grow(c->render_proj, c->render_proj_bytes, static_cast<size_t>(c->max_batch) * max_nv * render_projected_bytes_per_vertex()));   // max_batch x largest model
+        if (!c->render_unif) CU_TRY(c, dev_alloc(c->render_unif, static_cast<size_t>(c->max_batch) * render_uniform_bytes()));
+        c->render_max_nv = max_nv;
         c->meshes_dirty = false;
     }
     RenderArgs a;
-    a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes; a.n_meshes = c->mesh_rows;
+    a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
     a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
     a.rgb = rgbA; a.depth = depthA;
     a.mode = mode == SE3TN_RENDER_PYRENDER ? 1 : 0; a.vw = W; a.vh = H;
-    a.projected = c->render_proj; a.uniforms = c->render_unif; a.max_nv = c->render_max_nv;
+    a.projected = c->render_proj.get(); a.uniforms = c->render_unif.get(); a.max_nv = c->render_max_nv;
     { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s)); }
     c->launches += 2;
     return SE3TN_OK;
@@ -1218,15 +1215,17 @@ int se3tn_get_trace(se3tn_ctx* c, unsigned long long* out) {
     if (!c->trace) return fail(c, SE3TN_ERR_STATE, "se3tn_get_trace: the context was created without SE3TN_TRACE=1");
     DeviceGuard guard(c->device);
     CU_TRY(c, cudaDeviceSynchronize());
-    CU_TRY(c, cudaMemcpy(out, c->trace, SE3TN_TRACE_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    CU_TRY(c, cudaMemcpy(out, c->trace.get(), SE3TN_TRACE_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return SE3TN_OK;
 }
 
 int se3tn_set_profiling(se3tn_ctx* c, int enable) {
     if (!c) return SE3TN_ERR_INVALID;
     DeviceGuard guard(c->device);
-    if (enable && !c->ev0[0]) {
-        for (int i = 0; i < SE3TN_PROFILE_SLOTS; ++i) { CU_TRY(c, cudaEventCreate(&c->ev0[i])); CU_TRY(c, cudaEventCreate(&c->ev1[i])); }
+    if (enable && !c->ev[0][0]) {
+        Handle<cudaEvent_t> ev[2][SE3TN_PROFILE_SLOTS];   // installed only once every event exists
+        for (auto& row : ev) for (auto& h : row) { cudaEvent_t e = nullptr; CU_TRY(c, cudaEventCreate(&e)); h.reset(e); }
+        std::swap(c->ev, ev);
     }
     c->profiling = enable != 0;
     for (int i = 0; i < SE3TN_PROFILE_SLOTS; ++i) c->ev_used[i] = false;
@@ -1236,12 +1235,12 @@ int se3tn_set_profiling(se3tn_ctx* c, int enable) {
 int se3tn_get_profile(se3tn_ctx* c, float* ms) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!ms) return fail(c, SE3TN_ERR_INVALID, "se3tn_get_profile: null argument");
-    if (!c->ev0[0]) return fail(c, SE3TN_ERR_STATE, "se3tn_get_profile: profiling was never enabled");
+    if (!c->ev[0][0]) return fail(c, SE3TN_ERR_STATE, "se3tn_get_profile: profiling was never enabled");
     for (int i = 0; i < SE3TN_PROFILE_SLOTS; ++i) {
         ms[i] = 0.f;
         if (!c->ev_used[i]) continue;
-        CU_TRY(c, cudaEventSynchronize(c->ev1[i]));
-        CU_TRY(c, cudaEventElapsedTime(&ms[i], c->ev0[i], c->ev1[i]));
+        CU_TRY(c, cudaEventSynchronize(c->ev[1][i].get()));
+        CU_TRY(c, cudaEventElapsedTime(&ms[i], c->ev[0][i].get(), c->ev[1][i].get()));
         c->ev_used[i] = false;
     }
     return SE3TN_OK;
