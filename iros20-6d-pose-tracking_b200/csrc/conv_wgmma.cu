@@ -665,7 +665,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                         const long long t0 = clock64();
                         while (static_cast<unsigned>(ptx::ld_acquire_gpu(flag)) < L.dep_target) {
                             __nanosleep(64);
-                            if (clock64() - t0 > (1ll << 34)) __trap();     // ~10 s: a scheduling bug becomes an error, not a hung GPU
+                            if (clock64() - t0 > (1ll << 34)) ptx::timeout_trap();     // ~10 s: a scheduling bug becomes an error, not a hung GPU
                         }
                     }
                     ptx::fence_proxy_async_all();   // the TMA (async proxy) reads below must observe what the acquire made visible
@@ -765,7 +765,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                     const long long t0 = clock64();
                     while (ptx::ld_acquire_gpu(cnt) < p.ksplit) {
                         __nanosleep(32);
-                        if (clock64() - t0 > (1ll << 34)) __trap();
+                        if (clock64() - t0 > (1ll << 34)) ptx::timeout_trap();
                     }
                 }
                 __syncwarp();
