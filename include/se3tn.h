@@ -193,7 +193,8 @@ int se3tn_vocap(se3tn_ctx* ctx, const double* errs, int n, double* out_ap, void*
 /* The CAD model the renderer draws: what VispyRenderer.__init__ uploads as vertex / index buffers (reference
  * vispy_renderer.py:108-129).  HOST arrays, copied: pos float32 (nv,3) metres in the object frame, nrm float32 (nv,3)
  * unit normals, col uint8 (nv,3), faces int32 (nf,3).  mesh_id >= 0; a later call with the same id replaces the model;
- * on failure the id keeps its previous model. */
+ * on failure the id keeps its previous model.  A new model drops the context's captured steps: each is captured again on
+ * its next call. */
 int se3tn_set_mesh(se3tn_ctx* ctx, int mesh_id, const float* pos, const float* nrm, const uint8_t* col,
                    const int32_t* faces, int nv, int nf);
 
@@ -248,6 +249,35 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
                      const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
                      double* poses_out, float* out_trans, float* out_rot, void* stream);
 
+/* ---- tracking from the previous poses and the frame alone: input A rendered inside the step ------------------------- */
+
+/* Tracker.on_track for n tracks of one frame as the reference runs it (predict.py:217-296 with render_window at :246): the
+ * models are rendered at poses_in, then K0 -> conv stack -> K6, all on `stream`.  Arguments as se3tn_track_batch without
+ * rgbA / depthA; render_mode, render_H, render_W as mode, H, W of se3tn_render_ex (ignored in SE3TN_RENDER_VISPY).  Track i
+ * draws mesh weight_ids[i] (mesh 0 when the ids are NULL): one network and one CAD model per object, both under one id.
+ * Input A lands in context-owned device scratch (max_batch x 176 x 176 x 5 bytes, allocated by the first call).  One step
+ * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph under se3tn_track_batch's rules,
+ * with the render mode and camera image size part of the key; SE3TN_PREC_FP32 renders and then runs its FFMA forwards
+ * without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
+ * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
+ * camera image size out of range is SE3TN_ERR_INVALID. */
+int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                       const double* K, const double* poses_in, const double* object_width,
+                       int render_mode, int render_H, int render_W,
+                       const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                       double trans_normalizer, double rot_normalizer, int precision,
+                       float* out_trans, float* out_rot, double* poses_out, void* stream);
+
+/* se3tn_track_render with every pointer in HOST memory, the reference's own calling pattern with rendering included: the
+ * frame's crop-window rectangle, the poses, widths and ids go through se3tn_track_host's pinned staging (one copy in, one
+ * copy out, stable device addresses so the step's graph is replayed); input A is rendered on the device and never crosses
+ * the bus.  Synchronises `stream`.  Arguments as se3tn_track_host without rgbA / depthA, plus the render arguments of
+ * se3tn_track_render; weight_ids int32 (n) or NULL (all tracks use set 0 and mesh 0).  Errors as se3tn_track_render. */
+int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                            const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                            const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
+                            double* poses_out, float* out_trans, float* out_rot, void* stream);
+
 /* ---- introspection (tests / profiling) -------------------------------------------------------- */
 
 /* Device pointer + per-image float count of an internal NHWC activation buffer.
@@ -270,11 +300,11 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 #define SE3TN_TRACE_WORDS (14 * 256 * 8)
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
-/* Number of kernels the last forward / track_batch call on this context launched (for a replayed CUDA graph: the kernels
- * inside it).  se3tn_track_batch captures each distinct step (same pointers, sizes and precision) into a CUDA graph the
- * first time it sees it and replays it afterwards -- one graph launch per step; SE3TN_GRAPH=0 in the environment, an
- * enabled profiler or SE3TN_PREC_FP32 use plain stream launches.  se3tn_last_step_was_graph: 1 if the last track_batch
- * call was a graph launch. */
+/* Number of kernels the last forward / track_batch / track_render call on this context launched (for a replayed CUDA graph:
+ * the kernels inside it).  se3tn_track_batch and se3tn_track_render capture each distinct step (same pointers, sizes and
+ * precision) into a CUDA graph the first time they see it and replay it afterwards -- one graph launch per step;
+ * SE3TN_GRAPH=0 in the environment, an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
+ * se3tn_last_step_was_graph: 1 if the last track_batch / track_render call was a graph launch. */
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);
 

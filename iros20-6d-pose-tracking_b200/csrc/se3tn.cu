@@ -123,6 +123,8 @@ template <typename B, typename N> cudaError_t grow(B& b, N& cap, N n) {
     return e;
 }
 
+inline size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
+
 // Every form of one weight set that the kernels read.
 struct DeviceWeights {
     DevBuf<float> blob;             // exact fp32 blob (biases, fc and the fp32 mode's conv weights)
@@ -169,6 +171,7 @@ struct se3tn_ctx {
     std::map<int, Mesh> meshes;      // CAD models of the rasteriser, keyed by mesh id
     DevBuf<MeshDev> d_meshes; int mesh_rows = 0; bool meshes_dirty = false;   // device table of their views, rebuilt when a model changes
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
+    DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, so all four exist or none (grows on demand)
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
@@ -439,6 +442,24 @@ int sync_tables(se3tn_ctx* c, cudaStream_t s) {
     CU_TRY(c, cudaMemcpy(c->d_bias.get(), bias.data(), bias.size() * sizeof(float*), cudaMemcpyHostToDevice));
     CU_TRY(c, cudaMemcpy(c->d_fc.get(), fc.data(), fc.size() * sizeof(float*), cudaMemcpyHostToDevice));
     c->tables_dirty = false;
+    return SE3TN_OK;
+}
+
+// Rebuilds the device table of mesh views and the rasteriser workspace after se3tn_set_mesh.  Synchronous copies and
+// allocations: like sync_stats / sync_tables it runs before a step is captured, never inside the capture.
+int sync_meshes(se3tn_ctx* c, cudaStream_t s) {
+    if (!c->meshes_dirty) return SE3TN_OK;
+    const int rows = c->meshes.rbegin()->first + 1;
+    CU_TRY(c, cudaStreamSynchronize(s));
+    CU_TRY(c, grow(c->d_meshes, c->mesh_rows, rows));
+    std::vector<MeshDev> tab(rows, c->meshes.begin()->second.view());   // unused ids alias the first model
+    int max_nv = 0;
+    for (auto& kv : c->meshes) { tab[kv.first] = kv.second.view(); max_nv = std::max(max_nv, kv.second.nv); }
+    CU_TRY(c, cudaMemcpy(c->d_meshes.get(), tab.data(), sizeof(MeshDev) * rows, cudaMemcpyHostToDevice));
+    CU_TRY(c, grow(c->render_proj, c->render_proj_bytes, static_cast<size_t>(c->max_batch) * max_nv * render_projected_bytes_per_vertex()));   // max_batch x largest model
+    if (!c->render_unif) CU_TRY(c, dev_alloc(c->render_unif, static_cast<size_t>(c->max_batch) * render_uniform_bytes()));
+    c->render_max_nv = max_nv;
+    c->meshes_dirty = false;
     return SE3TN_OK;
 }
 
@@ -827,38 +848,58 @@ int se3tn_so3_log(se3tn_ctx* c, const double* poses_a, const double* poses_b, do
     return SE3TN_OK;
 }
 
-static int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                                const double* K, const double* poses_in, const double* object_width,
-                                const uint8_t* rgbA, const uint16_t* depthA,
-                                const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                                double tn, double rn, int precision,
-                                float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s);
+} // extern "C"
 
-int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                      const double* K, const double* poses_in, const double* object_width,
-                      const uint8_t* rgbA, const uint16_t* depthA,
-                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                      double tn, double rn, int precision,
-                      float* out_trans, float* out_rot, double* poses_out, void* stream) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
-    if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: weight_ids_host and weight_ids_dev must both be given or both NULL");
-    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: n exceeds max_batch");
-    // every id a track uses needs weights AND channel statistics (se3tn_set_stats is per weight id): checked here, where the
-    // ids are visible on the host, so that the preprocess kernel never normalises with another set's (or no) statistics
-    bool multi = false;
+namespace {
+
+// Input A drawn inside the step (se3tn_track_render): se3tn_render_ex's mode and camera image size (0 x 0 in the vispy mode,
+// which ignores them).
+struct RenderSpec { int mode, H, W; };
+
+int render_spec(se3tn_ctx* c, const char* fn, int mode, int H, int W, RenderSpec& r) {
+    if (mode != SE3TN_RENDER_VISPY && mode != SE3TN_RENDER_PYRENDER) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown render mode");
+    const bool pyr = mode == SE3TN_RENDER_PYRENDER;
+    if (pyr && (H <= 0 || W <= 0 || H > 65536 || W > 65536)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": render_H / render_W out of range");
+    r = {mode, pyr ? H : 0, pyr ? W : 0};
+    return SE3TN_OK;
+}
+
+// Host-side checks of one step, before anything is queued.  Every id a track uses needs weights AND channel statistics
+// (se3tn_set_stats is per weight id), so that the preprocess kernel never normalises with another set's (or no) statistics.
+// A step that renders input A also needs a model for every id: the rasteriser would otherwise draw model 0 in its place.
+// *multi: the tracks use more than one weight set.
+int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int32_t* wid_dev, int n, bool render, bool* multi) {
+    if ((wid_host == nullptr) != (wid_dev == nullptr))
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": n exceeds max_batch");
+    *multi = false;
     for (int i = 0; i < n; ++i) {
-        const int wid = weight_ids_host ? weight_ids_host[i] : 0;
+        const int wid = wid_host ? wid_host[i] : 0;
         auto it = c->weights.find(wid);
         if (wid < 0 || it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(wid) + " not loaded");
         if (!it->second.has_stats) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(wid) + " has no mean/std (se3tn_set_stats)");
-        if (wid != (weight_ids_host ? weight_ids_host[0] : 0)) multi = true;
-        if (!weight_ids_host) break;                // all tracks use set 0
+        if (render && !c->meshes.count(wid))
+            return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": id " + std::to_string(wid) + " (track " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
+        if (wid != (wid_host ? wid_host[0] : 0)) *multi = true;
+        if (!wid_host) break;                       // all tracks use set 0
     }
-    if (n == 0) return SE3TN_OK;
-    DeviceGuard guard(c->device);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    return SE3TN_OK;
+}
+
+int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                         const double* K, const double* poses_in, const double* object_width,
+                         const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
+                         const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                         double tn, double rn, int precision,
+                         float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s);
+
+// One checked step of n tracks (render, if `render` is set: input A is drawn into rgbA / depthA) -> K0 -> conv stack -> K6.
+int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+               const double* K, const double* poses_in, const double* object_width,
+               const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
+               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+               double tn, double rn, int precision,
+               float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
     // ---- one CUDA graph per distinct step: every argument that ends up inside a kernel parameter is part of the key ----
     const bool graphable = c->use_graphs && !c->profiling && precision != SE3TN_PREC_FP32;
     std::vector<unsigned long long> key;
@@ -872,6 +913,8 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
         for (int i = 0; i < 4; ++i) key.push_back(bits(K[i]));
         key.push_back(bits(tn)); key.push_back(bits(rn));
+        key.push_back(static_cast<unsigned long long>(render ? render->mode : -1));
+        key.push_back(static_cast<unsigned long long>(render ? render->H : 0)); key.push_back(static_cast<unsigned long long>(render ? render->W : 0));
         for (auto& g : c->graphs)
             if (g.key == key) {
                 CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
@@ -881,6 +924,7 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         // a new step shape: host-side table refreshes (synchronous copies) must not happen inside the capture
         int rc0 = sync_stats(c, s); if (rc0) return rc0;
         if (multi) { rc0 = sync_tables(c, s); if (rc0) return rc0; }
+        if (render) { rc0 = sync_meshes(c, s); if (rc0) return rc0; }
         if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
         cudaStream_t cs = nullptr;
         if (!c->cap_stream && cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess) c->cap_stream.reset(cs);
@@ -909,28 +953,37 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         return SE3TN_OK;
     };
     if (capturing) {
-        const int rc = track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_host, weight_ids_dev, n,
+        const int rc = track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
                                             tn, rn, precision, out_trans, out_rot, poses_out, multi, c->cap_stream.get());
         const int grc = end_capture(rc);
         if (grc == SE3TN_OK) return SE3TN_OK;
         if (grc != 1) return grc;                              // a real launch error
         // capture was not possible on this stream / driver: plain launches from here on
     }
-    return track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_host, weight_ids_dev, n,
+    return track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
                                 tn, rn, precision, out_trans, out_rot, poses_out, multi, s);
 }
 
 // the launches of one step, on stream s (being captured or not)
-static int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                                const double* K, const double* poses_in, const double* object_width,
-                                const uint8_t* rgbA, const uint16_t* depthA,
-                                const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                                double tn, double rn, int precision,
-                                float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
+int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                         const double* K, const double* poses_in, const double* object_width,
+                         const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
+                         const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                         double tn, double rn, int precision,
+                         float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
     void* stream = s;
     c->launches = 0;
-    int rc = se3tn_preprocess(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_dev, n,
-                              precision, nullptr, nullptr, nullptr, nullptr, stream);
+    int rc;
+    if (render) {                                  // track i draws mesh weight_ids[i] (0 without ids): one network and one model per object
+        rc = se3tn_render_ex(c, K, poses_in, object_width, weight_ids_dev, n, render->mode, render->H, render->W,
+                             const_cast<uint8_t*>(rgbA), const_cast<uint16_t*>(depthA), stream);
+        if (rc) return rc;
+    }
+    // preprocess_kernel is launched with programmatic stream serialization, so with a render in front of it it may start while
+    // render_kernel is still running.  It reads rgbA / depthA only after griddepcontrol.wait (aux_kernels.cu, grid_dep_wait()),
+    // which returns once render_kernel has completed and its writes are visible: keep every read of input A behind that wait.
+    rc = se3tn_preprocess(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_dev, n,
+                          precision, nullptr, nullptr, nullptr, nullptr, stream);
     if (rc) return rc;
     PoseArgs pose; pose.in = poses_in; pose.out = poses_out; pose.tn = static_cast<float>(tn); pose.rn = static_cast<float>(rn);
     bool pose_done = false;
@@ -952,6 +1005,52 @@ static int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const ui
     }
     if (pose_done) return SE3TN_OK;
     return se3tn_pose_update(c, poses_in, out_trans, out_rot, tn, rn, poses_out, n, stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                      const double* K, const double* poses_in, const double* object_width,
+                      const uint8_t* rgbA, const uint16_t* depthA,
+                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                      double tn, double rn, int precision,
+                      float* out_trans, float* out_rot, double* poses_out, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
+    bool multi = false;
+    const int rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    return track_step(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, nullptr, weight_ids_host, weight_ids_dev, n,
+                      tn, rn, precision, out_trans, out_rot, poses_out, multi, static_cast<cudaStream_t>(stream));
+}
+
+int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                       const double* K, const double* poses_in, const double* object_width,
+                       int render_mode, int render_H, int render_W,
+                       const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                       double tn, double rn, int precision,
+                       float* out_trans, float* out_rot, double* poses_out, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: null argument or empty frame");
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: null output");
+    RenderSpec r;
+    int rc = render_spec(c, "se3tn_track_render", render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    bool multi = false;
+    rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    // input A for max_batch tracks, allocated once: its address never changes, so captured steps stay valid
+    const size_t img = static_cast<size_t>(kImg) * kImg, rgb_bytes = align256(static_cast<size_t>(c->max_batch) * img * 3);
+    CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
+    return track_step(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, c->in_a.get(), reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes), &r,
+                      weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, multi, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_add_adi(se3tn_ctx* c, const double* model_pts, int m, const double* pred, const double* gt, int n,
@@ -1000,17 +1099,19 @@ inline void host_crop_window(const double* pose, const double* K, double width, 
     left = static_cast<int>(std::fmax(-lim, std::fmin(lim, umin))); top = static_cast<int>(std::fmax(-lim, std::fmin(lim, vmin)));
     cw = static_cast<int>(std::fmax(-lim, std::fmin(lim, umax))) - left; ch = static_cast<int>(std::fmax(-lim, std::fmin(lim, vmax))) - top;
 }
-inline size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-}  // namespace
 
-int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
-                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA,
-                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !rgbA || !depthA || !poses_out || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_host: null argument or empty frame");
-    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_host: n exceeds max_batch");
+// se3tn_track_host and se3tn_track_render_host: every pointer is HOST memory.  The crop-window rectangle of the frame and the
+// per-track inputs are staged through the context's pinned block into its device buffers (one copy for the per-track
+// inputs), one step runs on them -- with input A from the caller (render == NULL) or rendered inside the step, in which case
+// nothing of input A crosses the bus -- and one copy brings the outputs back before the stream is synchronised.
+int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                    const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
+                    const int32_t* weight_ids, int n, double tn, double rn, int precision,
+                    double* poses_out, float* out_trans, float* out_rot, void* stream) {
+    // the step checks the ids again; checking them here as well means an error stages and copies nothing
+    bool multi = false;
+    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi);
+    if (rc) return rc;
     if (n == 0) return SE3TN_OK;
     DeviceGuard guard(c->device);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1031,10 +1132,10 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     uint8_t* d_rgb = d; d += align256(px * 3);
     uint16_t* d_depth = reinterpret_cast<uint16_t*>(d); d += align256(px * 2);
     // the per-track arrays are packed by THIS call's n (a step's graph is keyed by n anyway), inputs first, outputs behind them:
-    // one host -> device copy carries all inputs, one device -> host copy all outputs
-    const size_t nn = static_cast<size_t>(n);
-    const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * img * 3),
-                 o_wid = o_depthA + align256(nn * img * 2), in_bytes = o_wid + align256(nn * 4);
+    // one host -> device copy carries all inputs, one device -> host copy all outputs; input A takes no room when it is rendered
+    const size_t nn = static_cast<size_t>(n), a_img = render ? 0 : img;
+    const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * a_img * 3),
+                 o_wid = o_depthA + align256(nn * a_img * 2), in_bytes = o_wid + align256(nn * 4);
     const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), out_bytes = o_ro + align256(nn * 12);
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
@@ -1074,13 +1175,17 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     hp = io.pin.get() + align256(static_cast<size_t>(hp - io.pin.get()));
     memcpy(hp, poses, nn * 128);
     memcpy(hp + o_ow, object_width, nn * 8);
-    memcpy(hp + o_rgbA, rgbA, nn * img * 3);
-    memcpy(hp + o_depthA, depthA, nn * img * 2);
+    if (!render) {
+        memcpy(hp + o_rgbA, rgbA, nn * img * 3);
+        memcpy(hp + o_depthA, depthA, nn * img * 2);
+    }
     if (weight_ids) memcpy(hp + o_wid, weight_ids, nn * 4);
     CU_TRY(c, cudaMemcpyAsync(d_in, hp, weight_ids ? in_bytes : o_wid, cudaMemcpyHostToDevice, s));
     hp += in_bytes;
-    const int rc = se3tn_track_batch(c, d_rgb, d_depth, H, W, K, d_poses, d_ow, d_rgbA, d_depthA, weight_ids, weight_ids ? d_wid : nullptr, n,
-                                     tn, rn, precision, d_tr, d_ro, d_out, stream);
+    rc = render ? se3tn_track_render(c, d_rgb, d_depth, H, W, K, d_poses, d_ow, render->mode, render->H, render->W, weight_ids, weight_ids ? d_wid : nullptr, n,
+                                     tn, rn, precision, d_tr, d_ro, d_out, stream)
+                : se3tn_track_batch(c, d_rgb, d_depth, H, W, K, d_poses, d_ow, d_rgbA, d_depthA, weight_ids, weight_ids ? d_wid : nullptr, n,
+                                    tn, rn, precision, d_tr, d_ro, d_out, stream);
     if (rc != SE3TN_OK) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
     CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
@@ -1089,6 +1194,32 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
     return SE3TN_OK;
+}
+}  // namespace
+
+int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA,
+                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
+                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !rgbA || !depthA || !poses_out || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_host: null argument or empty frame");
+    return track_host_step(c, "se3tn_track_host", frame_rgb, frame_depth, H, W, K, poses, object_width, rgbA, depthA, nullptr,
+                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, stream);
+}
+
+int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                            const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                            const int32_t* weight_ids, int n, double tn, double rn, int precision,
+                            double* poses_out, float* out_trans, float* out_rot, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render_host: null argument or empty frame");
+    RenderSpec r;
+    const int rc = render_spec(c, "se3tn_track_render_host", render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    return track_host_step(c, "se3tn_track_render_host", frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r,
+                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, stream);
 }
 
 int se3tn_allgather_poses(se3tn_ctx* c, void* nccl_comm, const double* local_poses, double* all_poses, int n_local, void* stream) {
@@ -1155,6 +1286,7 @@ int se3tn_set_mesh(se3tn_ctx* c, int mesh_id, const float* pos, const float* nrm
     CU_TRY(c, cudaMemcpy(m.faces.get(), faces, sizeof(int) * 3 * nf, cudaMemcpyHostToDevice));
     c->meshes[mesh_id] = std::move(m);             // frees the previous model: the device table is rebuilt before the next render
     c->meshes_dirty = true;
+    c->graphs.clear();                             // captured track_render steps hold the old table, workspace and largest vertex count
     return SE3TN_OK;
 }
 
@@ -1175,19 +1307,7 @@ int se3tn_render_ex(se3tn_ctx* c, const double* K, const double* poses, const do
     if (c->meshes.empty()) return fail(c, SE3TN_ERR_STATE, "se3tn_render: no mesh loaded (se3tn_set_mesh)");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
-    if (c->meshes_dirty) {
-        const int rows = c->meshes.rbegin()->first + 1;
-        CU_TRY(c, cudaStreamSynchronize(s));
-        CU_TRY(c, grow(c->d_meshes, c->mesh_rows, rows));
-        std::vector<MeshDev> tab(rows, c->meshes.begin()->second.view());   // unused ids alias the first model
-        int max_nv = 0;
-        for (auto& kv : c->meshes) { tab[kv.first] = kv.second.view(); max_nv = std::max(max_nv, kv.second.nv); }
-        CU_TRY(c, cudaMemcpy(c->d_meshes.get(), tab.data(), sizeof(MeshDev) * rows, cudaMemcpyHostToDevice));
-        CU_TRY(c, grow(c->render_proj, c->render_proj_bytes, static_cast<size_t>(c->max_batch) * max_nv * render_projected_bytes_per_vertex()));   // max_batch x largest model
-        if (!c->render_unif) CU_TRY(c, dev_alloc(c->render_unif, static_cast<size_t>(c->max_batch) * render_uniform_bytes()));
-        c->render_max_nv = max_nv;
-        c->meshes_dirty = false;
-    }
+    const int rc = sync_meshes(c, s); if (rc) return rc;
     RenderArgs a;
     a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
     a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];

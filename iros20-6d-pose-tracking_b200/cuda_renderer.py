@@ -1,7 +1,8 @@
 """Input A without OpenGL: the reference's VispyRenderer (vispy_renderer.py) or its pyrender Renderer
 (offscreen_renderer.py) + Tracker.render_window (predict.py:193-215) as one CUDA launch for all tracks (csrc/render.cu).  `CudaRenderer` plugs into
 `Tracker(renderer=...)`: it exposes render_window(ob2cam) -> (rgb uint8 (176,176,3), depth uint16 (176,176)),
-the contract of the reference method, and render_batch() for device-resident loops."""
+the contract of the reference method, and render_batch() for device-resident loops.  `mode`, `image_hw` and `mesh_id` are
+what the Tracker passes to the tracking step when it renders input A itself (Engine.track_render[_host])."""
 import numpy as np
 import torch
 

@@ -189,26 +189,43 @@ class Engine:
                                               _stream(self.device)), self._ctx)
         return out_poses, out_trans, out_rot
 
+    def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
+                     weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
+                     out_poses=None, out_trans=None, out_rot=None):
+        """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
+        K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
+        mode / image_hw as in render().  CUDA tensors in and out; nothing is synchronised."""
+        n = poses.shape[0]
+        self._check_frame(frame_rgb, frame_depth, None, None, poses, object_width, n)
+        H, W = frame_depth.shape
+        Kh = self._k4(K)
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        out_poses = torch.empty_like(poses) if out_poses is None else out_poses
+        out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
+        out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
+        wh = None
+        if weight_ids_host is not None:
+            wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
+            if weight_ids_dev is None:
+                weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        _lib.check(self.lib.se3tn_track_render(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W,
+                                               Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width), rmode, rH, rW,
+                                               wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0),
+                                               _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer),
+                                               PREC[precision], _ptr(out_trans), _ptr(out_rot), _ptr(out_poses),
+                                               _stream(self.device)), self._ctx)
+        return out_poses, out_trans, out_rot
+
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
                    weight_ids=None, precision='bf16x3', want_residuals=False):
         """The reference's calling pattern as one library call: numpy arrays in, numpy poses out, synchronous (se3tn_track_host).
         frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), poses float64 (n,4,4), object_width float64 (n), rgbA uint8
         (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous."""
         n = int(poses.shape[0])
-        for name, a, dt, shape in (('frame_rgb', frame_rgb, np.uint8, frame_depth.shape + (3,)), ('frame_depth', frame_depth, np.uint16, frame_depth.shape),
-                                   ('poses', poses, np.float64, (n, 4, 4)), ('object_width', object_width, np.float64, (n,)),
-                                   ('rgbA', rgbA, np.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', depthA, np.uint16, (n, IMAGE_SIZE, IMAGE_SIZE))):
-            if not (isinstance(a, np.ndarray) and a.dtype == dt and tuple(a.shape) == tuple(shape) and a.flags['C_CONTIGUOUS']):
-                raise ValueError('track_host: %s must be a C-contiguous %s array of shape %s' % (name, np.dtype(dt).name, tuple(shape)))
-        if frame_depth.ndim != 2:
-            raise ValueError('track_host: frame_depth must be (H, W)')
+        wid = self._check_host('track_host', frame_rgb, frame_depth, poses, object_width, weight_ids, n,
+                               (('rgbA', rgbA, np.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', depthA, np.uint16, (n, IMAGE_SIZE, IMAGE_SIZE))))
         H, W = frame_depth.shape
         Kh = self._k4(K)
-        wid = None
-        if weight_ids is not None:
-            wid = np.ascontiguousarray(weight_ids, dtype=np.int32)
-            if wid.shape != (n,):
-                raise ValueError('track_host: weight_ids must have one entry per track')
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
@@ -216,6 +233,25 @@ class Engine:
         _lib.check(self.lib.se3tn_track_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
                                              vp(rgbA), vp(depthA), vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
                                              vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
+        return (out, tr, ro) if want_residuals else out
+
+    def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
+                          weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False):
+        """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
+        the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
+        without ids); mode / image_hw as in render()."""
+        n = int(poses.shape[0])
+        wid = self._check_host('track_render_host', frame_rgb, frame_depth, poses, object_width, weight_ids, n, ())
+        H, W = frame_depth.shape
+        Kh = self._k4(K)
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        out = np.empty((n, 4, 4), dtype=np.float64)
+        tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
+        ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
+        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
+        _lib.check(self.lib.se3tn_track_render_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
+                                                    rmode, rH, rW, vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
+                                                    vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
         return (out, tr, ro) if want_residuals else out
 
     def upload_frame_window(self, rgb_host, depth_host, rgb_dev, depth_dev, y0, y1, x0, x1):
@@ -260,15 +296,20 @@ class Engine:
         rgb = out_rgb if out_rgb is not None else torch.empty((n, 176, 176, 3), dtype=torch.uint8, device=self.device)
         dep = out_depth if out_depth is not None else torch.empty((n, 176, 176), dtype=torch.uint16, device=self.device)
         Kh = self._k4(K)
+        rmode, H, W = self._render_mode(mode, image_hw)
+        _lib.check(self.lib.se3tn_render_ex(self._ctx, Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width), _ptr(mesh_ids), n,
+                                            rmode, H, W, _ptr(rgb), _ptr(dep), _stream(self.device)), self._ctx)
+        return rgb, dep
+
+    @staticmethod
+    def _render_mode(mode, image_hw):
+        """(SE3TN_RENDER_* value, H, W) of a render mode name and the camera image size it needs."""
         if mode not in ('vispy', 'pyrender'):
             raise ValueError("render mode must be 'vispy' or 'pyrender'")
         if mode == 'pyrender' and image_hw is None:
             raise ValueError("render(mode='pyrender') needs image_hw=(H, W), the camera image pyrender draws")
         H, W = (int(image_hw[0]), int(image_hw[1])) if image_hw is not None else (0, 0)
-        _lib.check(self.lib.se3tn_render_ex(self._ctx, Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width), _ptr(mesh_ids), n,
-                                            _lib.RENDER_PYRENDER if mode == 'pyrender' else _lib.RENDER_VISPY, H, W, _ptr(rgb), _ptr(dep),
-                                            _stream(self.device)), self._ctx)
-        return rgb, dep
+        return (_lib.RENDER_PYRENDER if mode == 'pyrender' else _lib.RENDER_VISPY), H, W
 
     # ------------------------------------------------------------------ pose exchange over a raw NCCL communicator (SURVEY 8e)
     def allgather_poses_nccl(self, nccl_comm, local_poses, out=None, world_size=None):
@@ -325,7 +366,7 @@ class Engine:
         return self.lib.se3tn_last_launch_count(self._ctx)
 
     def last_step_was_graph(self):
-        """True when the last track_batch call replayed (or just captured and launched) a CUDA graph of the whole step."""
+        """True when the last track_batch / track_render call replayed (or just captured and launched) a CUDA graph of the whole step."""
         return bool(self.lib.se3tn_last_step_was_graph(self._ctx))
 
     # ------------------------------------------------------------------ checks
@@ -335,10 +376,11 @@ class Engine:
             raise ValueError('expected a contiguous float32 CUDA tensor of shape (n,4,176,176), got %s %s' % (t.dtype, tuple(t.shape)))
 
     def _check_frame(self, rgb, depth, rgbA, depthA, poses, ow, n):
+        """rgbA / depthA None: input A is rendered by the call, only the frame and the per-track arrays are checked."""
         ok = (rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.is_contiguous() and rgb.dim() == 3 and rgb.shape[2] == 3 and
               depth.is_cuda and depth.dtype == torch.uint16 and depth.is_contiguous() and depth.shape == rgb.shape[:2] and
-              rgbA.is_cuda and rgbA.dtype == torch.uint8 and rgbA.is_contiguous() and tuple(rgbA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE, 3) and
-              depthA.is_cuda and depthA.dtype == torch.uint16 and depthA.is_contiguous() and tuple(depthA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE) and
+              (rgbA is None or (rgbA.is_cuda and rgbA.dtype == torch.uint8 and rgbA.is_contiguous() and tuple(rgbA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE, 3))) and
+              (depthA is None or (depthA.is_cuda and depthA.dtype == torch.uint16 and depthA.is_contiguous() and tuple(depthA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE))) and
               poses.is_cuda and poses.dtype == torch.float64 and poses.is_contiguous() and tuple(poses.shape) == (n, 4, 4) and
               ow.is_cuda and ow.dtype == torch.float64 and ow.is_contiguous() and tuple(ow.shape) == (n,))
         if not ok:
@@ -346,6 +388,22 @@ class Engine:
                              'float64 (n,4,4), float64 (n,), all contiguous CUDA tensors')
         if n > self.max_batch:
             raise ValueError('n=%d exceeds max_batch=%d' % (n, self.max_batch))
+
+    @staticmethod
+    def _check_host(fn, frame_rgb, frame_depth, poses, object_width, weight_ids, n, extra):
+        """Checks of the host-array entry points; returns weight_ids as a C-contiguous int32 array (or None)."""
+        for name, a, dt, shape in (('frame_rgb', frame_rgb, np.uint8, frame_depth.shape + (3,)), ('frame_depth', frame_depth, np.uint16, frame_depth.shape),
+                                   ('poses', poses, np.float64, (n, 4, 4)), ('object_width', object_width, np.float64, (n,))) + tuple(extra):
+            if not (isinstance(a, np.ndarray) and a.dtype == dt and tuple(a.shape) == tuple(shape) and a.flags['C_CONTIGUOUS']):
+                raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, np.dtype(dt).name, tuple(shape)))
+        if frame_depth.ndim != 2:
+            raise ValueError('%s: frame_depth must be (H, W)' % fn)
+        if weight_ids is None:
+            return None
+        wid = np.ascontiguousarray(weight_ids, dtype=np.int32)
+        if wid.shape != (n,):
+            raise ValueError('%s: weight_ids must have one entry per track' % fn)
+        return wid
 
     @staticmethod
     def _k4(K):

@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from .engine import Engine
+from .cuda_renderer import CudaRenderer
 from .se3_tracknet import Se3TrackNet
 from .datasets import TrackDataset
 from . import Utils as U
@@ -166,7 +167,6 @@ class Tracker:
         # unlit full-camera-image mode followed by crop_bbox; anything else its vispy producer.
         pyr = dataset_info.get('renderer') == 'pyrenderer'
         if renderer == 'cuda' or (renderer is None and model_path is not None and str(model_path).lower().endswith(('.ply', '.obj') if pyr else '.ply')):
-            from .cuda_renderer import CudaRenderer
             try:
                 renderer = CudaRenderer(model_path, self.K, self.engine, self.object_width, mesh_id=weight_id,
                                         mode='pyrender' if pyr else 'vispy', image_hw=(cam_cfg['height'], cam_cfg['width']) if pyr else None)
@@ -224,16 +224,34 @@ class Tracker:
         rgb, depth = r.render([ob2cam])
         return U.crop_bbox(rgb, (depth * 1000).astype(np.uint16), bbox, self.image_size)
 
+    def _fused_renderer(self, weight_ids=None, renderer_width=False):
+        """The CudaRenderer when the tracking step can render input A itself and draw exactly what rendering it first would,
+        else None.  The step draws with the Tracker's engine, camera and widths, and track i draws the model of its weight id.
+        A renderer on another engine, with another K, drawing another model without per-track ids, or (renderer_width:
+        Tracker.render_window draws at the renderer's own width) with another width renders input A first, as before."""
+        r = self.renderer
+        if not isinstance(r, CudaRenderer) or r.engine is not self.engine or not np.array_equal(r.K, self.K):
+            return None
+        if weight_ids is None and r.mesh_id != self.weight_id:
+            return None
+        if renderer_width and r.object_width != float(self.object_width):
+            return None
+        return r
+
     # ------------------------------------------------------------------ the hot path
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
                  rgbA=None, depthA=None, show=False):
-        """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose."""
+        """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose.  Without rgbA / depthA and with the
+        CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host)."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
-        if rgbA is None or depthA is None:
-            rgbA, depthA = self.render_window(A_in_cam)
-        out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth,
-                                  np.ascontiguousarray(rgbA, dtype=np.uint8)[None],
-                                  np.ascontiguousarray(depthA).astype(np.uint16)[None])
+        if (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None:
+            out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
+        else:
+            if rgbA is None or depthA is None:
+                rgbA, depthA = self.render_window(A_in_cam)
+            out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth,
+                                      np.ascontiguousarray(rgbA, dtype=np.uint8)[None],
+                                      np.ascontiguousarray(depthA).astype(np.uint16)[None])
         final_estimate = out[0]
         self.prev_rgb = current_rgb
         self.prev_depth = current_depth
@@ -247,7 +265,8 @@ class Tracker:
 
     def on_track_batch(self, prev_poses, current_rgb, current_depth, rgbA=None, depthA=None, weight_ids=None, object_width=None):
         """N independent tracks of ONE frame -> (N,4,4) float64.  rgbA / depthA None: rendered on the device by the CUDA
-        rasteriser (needs a CudaRenderer; per-track models follow weight_ids).
+        rasteriser (needs a CudaRenderer; per-track models follow weight_ids), inside the tracking step when the renderer
+        allows it (_fused_renderer).
 
         numpy inputs   -> numpy result (synchronous, like the reference's on_track).
         CUDA tensors   -> CUDA tensor, nothing is synchronised.
@@ -259,10 +278,14 @@ class Tracker:
         render = rgbA is None or depthA is None
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
-        if (not render and all(isinstance(x, np.ndarray) for x in (current_rgb, current_depth, rgbA, depthA)) and not torch.is_tensor(prev_poses)
-                and not torch.is_tensor(weight_ids) and not torch.is_tensor(object_width) and os.environ.get('SE3TN_HOST_CALL', '1') != '0'):
+        renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
+        if ((renderer is not None or (not render and all(isinstance(x, np.ndarray) for x in (rgbA, depthA))))
+                and all(isinstance(x, np.ndarray) for x in (current_rgb, current_depth))
+                and not torch.is_tensor(prev_poses) and not torch.is_tensor(weight_ids) and not torch.is_tensor(object_width)
+                and os.environ.get('SE3TN_HOST_CALL', '1') != '0'):
             # numpy in, numpy out -- the reference's own calling pattern: ONE library call stages the crop-window rectangle of the
-            # frame, the poses and input A through pinned memory, replays the step's graph and hands the poses back
+            # frame, the poses and input A (unless the step renders it) through pinned memory, replays the step's graph and hands
+            # the poses back
             c = lambda a, dt: a if (a.dtype == dt and a.flags['C_CONTIGUOUS']) else np.ascontiguousarray(a).astype(dt, copy=False)
             poses_h = np.ascontiguousarray(prev_poses, dtype=np.float64).reshape(-1, 4, 4)
             n = len(poses_h)
@@ -272,6 +295,10 @@ class Tracker:
                 wh = np.ascontiguousarray(weight_ids, dtype=np.int32)
             elif self.weight_id != 0:
                 wh = np.full(n, self.weight_id, dtype=np.int32)
+            if renderer is not None:
+                return self.engine.track_render_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h,
+                                                     self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision,
+                                                     mode=renderer.mode, image_hw=renderer.image_hw)
             return self.engine.track_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h, c(rgbA, np.uint8), c(depthA, np.uint16),
                                           self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision)
         staged = not render and all(torch.is_tensor(x) and not x.is_cuda for x in (prev_poses, current_rgb, current_depth, rgbA, depthA))
@@ -338,7 +365,7 @@ class Tracker:
                 ow = self._np_bufs[('ow', n)] = torch.full((n,), float(self.object_width), dtype=torch.float64, device=dev)
         else:
             ow = up(object_width, torch.float64, 'ow_arg')
-        if render:
+        if render and renderer is None:              # a renderer the step cannot stand in for draws input A first
             mids = None
             if weight_ids is not None:
                 mids = (weight_ids if torch.is_tensor(weight_ids) else torch.as_tensor(np.asarray(weight_ids))).to(dev, torch.int32)
@@ -361,9 +388,14 @@ class Tracker:
             wd = self._np_bufs.get(wk)
             if wd is None:
                 wd = self._np_bufs[wk] = torch.from_numpy(wh).to(dev)
-        out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
-                                            self.trans_normalizer, self.rot_normalizer,
-                                            weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, **outs)
+        if renderer is not None:                      # input A is drawn inside the step, with the weight ids as mesh ids
+            out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
+                                                 weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision,
+                                                 mode=renderer.mode, image_hw=renderer.image_hw, **outs)
+        else:
+            out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
+                                                self.trans_normalizer, self.rot_normalizer,
+                                                weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, **outs)
         if staged:
             self._stage_done[self._stage_slot].record(torch.cuda.current_stream(dev))
         return out.cpu().numpy() if as_numpy else out

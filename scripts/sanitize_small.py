@@ -19,6 +19,10 @@ R, D = torch.from_numpy(rgb).cuda(), torch.from_numpy(depth).cuda()
 for prec in ('bf16x3', 'tf32', 'bf16', 'fp32'):
     out, _, _ = eng.track_batch(R, D, K, poses, ow, rgbA, depA, 0.03, 5 * np.pi / 180, weight_ids_host=np.array([0, 1, 0], np.int32) if prec != 'fp32' else None, precision=prec)
 host = eng.track_host(rgb, depth, K, poses.cpu().numpy(), ow.cpu().numpy(), rgbA.cpu().numpy(), depA.cpu().numpy(), 0.03, 5 * np.pi / 180, weight_ids=np.array([0, 1, 0], np.int32))
+for mode, hw in (('vispy', None), ('pyrender', (480, 640))):
+    for prec in ('bf16x3', 'fp32'):
+        eng.track_render(R, D, K, poses, ow, 0.03, 5 * np.pi / 180, weight_ids_host=np.array([0, 1, 0], np.int32), precision=prec, mode=mode, image_hw=hw)
+    eng.track_render_host(rgb, depth, K, poses.cpu().numpy(), ow.cpu().numpy(), 0.03, 5 * np.pi / 180, weight_ids=np.array([0, 1, 0], np.int32), mode=mode, image_hw=hw)
 filled = eng.fill_depth(D[:96, :128].contiguous())
 m = torch.from_numpy(synth.model_points(500, 0)).cuda(); pr, gt = synth.pose_pairs(4, 0)
 add, adi = eng.add_adi(m, torch.from_numpy(pr).cuda(), torch.from_numpy(gt).cuda()); ap = eng.vocap(adi)
