@@ -59,7 +59,7 @@ struct ConvPtrs {
 };
 
 constexpr int kLayersPerSet = 14;     // stride of the per-set device tables: one row per conv layer
-constexpr int kPoolSlices = 8;        // fused average pool: column sums per 16-row slice of the last layer's 11x11 tile (one per consumer warp)
+constexpr int kPoolSlices = 8;        // fused average pool: column sums per 16-row slice of the last layer's 11x11 tile
 
 // ---- wgmma kernels ----------------------------------------------------------------------------------------
 // One layer as the device sees it.  Channel counts are in CHANNELS; byte strides follow from the precision.
@@ -88,7 +88,7 @@ struct LayerDesc {
     int base_unit0;        // index of this layer's first UNSPLIT unit among all unsplit units of the launch (split-K scratch / counters)
     int units_per_image;   // tiles_x * tiles_y * n_tiles * groups (unsplit)
     int dep_layer;         // index (within the launch) of the layer whose per-image completion this layer waits for; -1: none
-    unsigned dep_target;   // value done[dep_layer][image] reaches when that image is complete (one signal per consumer warp and K piece: 8 x ksplit x units per image)
+    unsigned dep_target;   // value done[dep_layer][image] reaches when that image is complete (one signal per warp of the owning consumer warpgroup and K piece: 4 x ksplit x units per image)
 };
 
 constexpr int kTrunkMaxLayers = 6;
@@ -108,8 +108,8 @@ struct TrunkParams {
     // round robin so that they are); each piece dumps its fp32 accumulator to `partial`, then finishes ITS share of the unit's
     // 32-column blocks: it waits for the other pieces' dumps, sums all pieces in a fixed order and runs the normal epilogue.  1 = off.
     int ksplit;
-    float* partial;                // [unsplit unit][piece][8 warp slices][32-column block][float4 0..3][lane]
-    unsigned* slice_cnt;           // [unsplit unit][8 warp slices] number of pieces that have dumped the slice (zeroed before the launch)
+    float* partial;                // [unsplit unit][piece][4 warp slices][64-row half][32-column block][float4 0..3][lane]
+    unsigned* slice_cnt;           // [unsplit unit][4 warp slices] number of pieces that have dumped the slice (zeroed before the launch)
 };
 
 struct ResidentParams {
@@ -128,7 +128,7 @@ cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int num_sms, bool 
 // latency mode: at most kSplitMaxImages images, ksplit = kSplitK pieces, 128-channel units (at most 8 per image and layer)
 constexpr int kSplitMaxImages = 4, kSplitK = 4, kSplitMaxUnits = kSplitMaxImages * 8 * kTrunkMaxLayers;
 // 32-bit words of scheduler state a trunk launch needs: next-unit counter + done[layers][max_batch] + split-K slice counters
-inline size_t trunk_sched_words(int max_batch) { return 1 + static_cast<size_t>(kTrunkMaxLayers) * max_batch + static_cast<size_t>(kSplitMaxUnits) * 8; }
+inline size_t trunk_sched_words(int max_batch) { return 1 + static_cast<size_t>(kTrunkMaxLayers) * max_batch + static_cast<size_t>(kSplitMaxUnits) * 4; }
 inline size_t trunk_partial_floats() { return static_cast<size_t>(kSplitMaxUnits) * kSplitK * 128 * 128; }
 
 cudaError_t launch_conv_direct(const ConvGeom& g, const ConvPtrs& p, cudaStream_t stream);

@@ -2,8 +2,9 @@
 // network_modules.py:59-66,86-120), im2col-free: D[pixels, Cout] = sum_tap sum_c A_tap[pixel, c] * W[Cout, tap*Cin + c].
 //
 // Common to both kernels
-//   * M tile = an 11x11 pixel box of one image (121 of 128 rows; 44, 22 and 11 are multiples of 11).  Two consumer
-//     warpgroups each own 64 of the 128 rows (wgmma M = 64) and keep their accumulator in registers.
+//   * M tile = an 11x11 pixel box of one image (121 of 128 rows; 44, 22 and 11 are multiples of 11), as two wgmma M = 64
+//     halves.  In the resident kernel each consumer warpgroup owns one half of every tile; in the trunk one warpgroup owns
+//     both halves of a work unit.  Accumulators stay in registers.
 //   * A operand by TMA "units": one cp.async.bulk.tensor.4d per (128-byte channel chunk, filter COLUMN) whose box is
 //     two rows taller than the tile.  It lands as 143 rows x 128 B in the SWIZZLE_128B K-major layout wgmma reads, and
 //     the three vertical taps of that column are the SAME tile read through descriptors whose start address is advanced
@@ -13,8 +14,8 @@
 //     view; the 7 filter rows are row shifts 0/11/22/33.
 //   * warp roles (384 threads = 3 warpgroups): warp 0 activation TMA producer (+ work scheduler in the trunk kernel),
 //     warp 1 weight TMA producer, warps 2-3 idle; warpgroups 1 and 2 issue the MMAs and run the epilogue from registers.
-//     Each consumer warpgroup keeps one MMA group in flight and hands an operand stage back once the group after it
-//     has been issued (wgmma.wait_group 1).
+//     A consumer warpgroup keeps one MMA group in flight and hands an operand stage back once the group after it has been
+//     issued (wgmma.wait_group 1).
 //   * PREC (an SE3TN_PREC_* value) selects arithmetic and storage (storage.cuh): TF32 (4 x k8 tf32 MMAs per chunk-tap),
 //     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product).
 //   * programmatic dependent launch: every CTA signals launch_dependents at entry; only the threads that touch
@@ -43,12 +44,18 @@
 //     loads of the current one, and a unit of layer l first waits until done[l-1][image] says that image's previous-layer
 //     output is complete (release/acquire at gpu scope; the waits point backwards in the pull order and all CTAs are
 //     co-resident, so the schedule cannot deadlock).
-//   * 128 output channels per unit: a 64 x 128 fp32 accumulator is 64 registers per thread, which leaves room for the
-//     epilogue's residual and bias loads without spilling (256 channels would need 128).
+//   * ping-pong: consumer warpgroup g owns every other unit the CTA pulls (both warpgroups walk the unit ring; the other
+//     one only steps its operand ring positions past the unit's stages).  A pair of named barriers passes the turn to issue
+//     MMAs: a warpgroup starts its unit's MMAs once the other has ISSUED all of its previous unit's, so one warpgroup's
+//     epilogue runs under the other's MMAs.  Each MMA step is issued once per 64-row half, in the same K order as with one
+//     warpgroup per half: bit-identical results.
+//   * registers: the 128 x 128 fp32 accumulator is 128 registers per consumer thread.  setmaxnreg moves them from the
+//     producer warpgroup (168 at launch -> 40) to the consumers (-> 232).
 //   * weights stream through a 6-stage ring of {32 words, 128 rows} tiles fed by their own producer warp.
-//   * epilogue: each warp's 16-row x 32-column accumulator block is transposed through a per-warp shared-memory tile so
-//     every global load / store instruction covers whole lines; the last layer reduces its 121 rows to per-warp column
-//     sums instead (AdaptiveAvgPool2d(1) fused; fixed order -> deterministic).
+//   * epilogue: each warp post-processes 32 rows (a 16-row slice of each half, one after the other); every 16-row x 32-column
+//     accumulator block is transposed through a per-warp shared-memory tile so every global load / store instruction covers
+//     whole lines; the last layer reduces its 121 rows to per-slice column sums instead (AdaptiveAvgPool2d(1) fused; eight
+//     16-row slices, fixed order -> deterministic).
 #include "conv_common.h"
 #include "ptx.cuh"
 #include "storage.cuh"
@@ -63,7 +70,7 @@ constexpr int kPoolStageBytes = 121 * kPoolPitch * 4;
 constexpr int kPoolStageAlloc = (kPoolStageBytes + 1023) & ~1023;
 constexpr int kAUnit3 = 19 * 1024;             // 3x3: (22 + 128) rows * 128 B = 19,200
 constexpr int kAUnitStem = 21 * 1024;          // stem: (33 + 128) rows * 128 B = 20,608
-constexpr int kWgRowBytes = 64 * kChunkBytes;  // the second consumer warpgroup's rows start 64 rows into a unit
+constexpr int kWgRowBytes = 64 * kChunkBytes;  // the second 64-row half of a tile starts 64 rows into an A unit
 
 // Compile-time unit / tap structure per conv kind, so the MMA issue loop is straight-line code with immediate row
 // shifts / weight-tile indices, and the TMA producer's box coordinates are immediates too.
@@ -436,24 +443,38 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
 // ================================================================================================================
 template <int PREC> struct TCfg {
     static constexpr int BN = 128;                                      // output channels per work unit
-    static constexpr int kAcc = BN / 2;                                 // accumulator registers per thread
+    static constexpr int kAcc = BN / 2;                                 // accumulator registers per thread and 64-row half of the tile
     static constexpr int kAStages = 3;
     static constexpr int kBStages = 6;
     static constexpr int kBTile = BN * kChunkBytes;                     // 16 KB
     static constexpr int kEpiPitch = 36;                                // words per staged row (32 + 4: conflict-free 16 B accesses)
-    static constexpr int kEpiWarpBytes = 16 * kEpiPitch * 4 + 64;       // 16 rows + 16-entry pixel-index table
+    static constexpr int kEpiWarpBytes = 16 * kEpiPitch * 4 + 128;      // 16 rows + 32-entry pixel-index table
     static constexpr int kEpiBytes = 8 * kEpiWarpBytes;
     static constexpr int kSched = 4;                                    // work-unit ring between the scheduler (A producer) and the other roles
     static constexpr int kSmem = kAStages * kAUnit3 + kBStages * kBTile + ((kEpiBytes + 1023) & ~1023) + 1024 + 512;
     static_assert(kSmem <= 232448, "shared memory budget");
 };
+// registers per thread after setmaxnreg: the producer warpgroup gives up what the consumers' 128 accumulators need
+// (launch: 168 x 384 threads; after: 40 x 128 + 232 x 256 = the same 64,512)
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+constexpr int kTurnBar = 1;                    // named barrier kTurnBar + g: consumer warpgroup g may issue its unit's MMAs
+constexpr int kTaps3 = 9;                      // weight tiles per K chunk of a 3x3 conv (one per filter tap, both strides)
+
+// move a ring position (stage, phase) on by n stages
+__device__ __forceinline__ void ring_skip(int& stage, uint32_t& phase, int n, int stages) {
+    stage += n;
+    phase ^= static_cast<uint32_t>(stage / stages) & 1u;
+    stage %= stages;
+}
 
 struct UnitCoord { int l, img, tx, ty, n_tile, grp, c0, c1, piece, gidx; };
 // per-unit timeline (SE3TN_TRACE, small launches only): 5 stamps per work unit behind the trunk's per-CTA stamps:
-// 0 dependency satisfied (producer), 1 first A unit landed (first consumer), 2 last MMA completed, 3 accumulator handed to the
-// epilogue, 4 first consumer warp finished (stores + completion signal)
+// 0 dependency satisfied (producer), 1 first A unit landed (owning consumer warpgroup, after its MMA turn came), 2 last MMA
+// completed, 3 accumulator handed to the epilogue, 4 the owning warpgroup's first warp finished (stores + completion signal; low
+// 8 bits: CTA index).  Stamps 1-4 are written by the first thread of the owning warpgroup.
 __device__ __forceinline__ void unit_stamp(const TrunkParams& p, int u, int k) {
-    if (p.trace && u < 2048) p.trace[256 * 8 + u * 5 + k] = gtimer();
+    if (p.trace && u < 2048) p.trace[256 * 8 + u * 5 + k] = k == 4 ? (gtimer() & ~0xffull) | (blockIdx.x & 0xff) : gtimer();
 }   // [c0, c1): K chunks of this piece; gidx: unsplit unit index in the launch
 
 __device__ __forceinline__ int unit_layer(const TrunkParams& p, int u) {
@@ -524,48 +545,55 @@ __device__ __forceinline__ void trunk_load_weights(const LayerDesc& L, const CUt
     }
 }
 
-// MMAs of one work unit (one consumer warpgroup, its 64 rows).  One MMA group per weight tile; a group's weight stage (and, after
-// the last tap of a filter column, its A stage) is handed back once the next group has been issued and the group has completed.
+// MMAs of one work unit (one consumer warpgroup, all 128 rows: each MMA step is issued once per 64-row half, into that half's
+// accumulator).  The warpgroup first waits for its turn: the other consumer warpgroup has issued every MMA of the CTA's previous
+// unit; once this unit's last MMA is issued it passes the turn back, and its MMAs run while the other warpgroup's epilogue does.
+// One MMA group per weight tile; a group's weight stage (and, after the last tap of a filter column, its A stage) is handed back
+// once the next group has been issued and the group has completed.
 template <int KIND, int PREC>
-__device__ __forceinline__ void trunk_mma_unit(float (&acc)[TCfg<PREC>::kAcc], const Consumer& cs, int chunks, uint8_t* sA, uint8_t* sB,
+__device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc], const Consumer& cs, int chunks, uint8_t* sA, uint8_t* sB,
                                                uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty,
                                                int& astage, uint32_t& aphase, int& bstage, uint32_t& bphase,
                                                unsigned long long* trace, bool first_unit, unsigned long long* ustamp)
 {
     using KT = KTab<KIND>;
     using C = TCfg<PREC>;
-    const bool stamp = threadIdx.x == 128;
+    const bool stamp = cs.leader();
     uint32_t fresh = 0;
     int pend_b = -1, pend_a = -1;
+    ptx::bar_sync(kTurnBar + cs.cg, 256);
     for (int ch = 0; ch < chunks; ++ch) {
 #pragma unroll
         for (int u = 0; u < KT::NU; ++u) {
             ptx::mbar_wait(&a_full[astage], aphase);
             if (first_unit && ch == 0 && u == 0 && stamp) trace_stamp(trace, 3);
             if (ustamp && ch == 0 && u == 0 && stamp) *ustamp = gtimer();
-            const uint32_t a_unit_lo = desc_lo(sA + astage * kAUnit3 + cs.cg * kWgRowBytes);
+            const uint32_t a_unit_lo = desc_lo(sA + astage * kAUnit3);
 #pragma unroll
             for (int k = 0; k < KT::ntaps(u); ++k) {
                 ptx::mbar_wait(&b_full[bstage], bphase);
                 if (first_unit && ch == 0 && u == 0 && k == 0 && stamp) trace_stamp(trace, 2);
                 const uint32_t b_lo = desc_lo(sB + bstage * C::kBTile);
-                const uint32_t a_lo = a_unit_lo + k * kRowShift * (kChunkBytes >> 4);
                 ptx::wgmma_fence();
-                if constexpr (PREC == SE3TN_PREC_TF32) {
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-                        ptx::wgmma_tf32_n128(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
-                } else if constexpr (PREC == SE3TN_PREC_BF16X3) {
-                    // chunk = [32 hi | 32 lo] bf16 (A) x [32 w_hi | 32 w_lo] (B); offsets in 16-byte units
-                    constexpr int AO[6] = {0, 2, 4, 6, 0, 2};      // hi, hi, lo, lo, hi, hi
-                    constexpr int BO[6] = {0, 2, 0, 2, 4, 6};      // w_hi x4,        w_lo x2
+                for (int hf = 0; hf < 2; ++hf) {
+                    const uint32_t a_lo = a_unit_lo + hf * (kWgRowBytes >> 4) + k * kRowShift * (kChunkBytes >> 4);
+                    if constexpr (PREC == SE3TN_PREC_TF32) {
 #pragma unroll
-                    for (int i = 0; i < 6; ++i)
-                        ptx::wgmma_bf16_n128(acc, mk_desc(a_lo + AO[i]), mk_desc(b_lo + BO[i]), fresh | (i ? 1u : 0u));
-                } else {
+                        for (int kk = 0; kk < 4; ++kk)
+                            ptx::wgmma_tf32_n128(acc[hf], mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
+                    } else if constexpr (PREC == SE3TN_PREC_BF16X3) {
+                        // chunk = [32 hi | 32 lo] bf16 (A) x [32 w_hi | 32 w_lo] (B); offsets in 16-byte units
+                        constexpr int AO[6] = {0, 2, 4, 6, 0, 2};      // hi, hi, lo, lo, hi, hi
+                        constexpr int BO[6] = {0, 2, 0, 2, 4, 6};      // w_hi x4,        w_lo x2
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-                        ptx::wgmma_bf16_n128(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
+                        for (int i = 0; i < 6; ++i)
+                            ptx::wgmma_bf16_n128(acc[hf], mk_desc(a_lo + AO[i]), mk_desc(b_lo + BO[i]), fresh | (i ? 1u : 0u));
+                    } else {
+#pragma unroll
+                        for (int kk = 0; kk < 4; ++kk)
+                            ptx::wgmma_bf16_n128(acc[hf], mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
+                    }
                 }
                 ptx::wgmma_commit();
                 ptx::wgmma_wait<1>();
@@ -581,8 +609,10 @@ __device__ __forceinline__ void trunk_mma_unit(float (&acc)[TCfg<PREC>::kAcc], c
             if (++astage == C::kAStages) { astage = 0; aphase ^= 1; }
         }
     }
+    ptx::bar_arrive(kTurnBar + (cs.cg ^ 1), 256);
     ptx::wgmma_wait<0>();
-    ptx::wgmma_reg_fence(acc);
+    ptx::wgmma_reg_fence(acc[0]);
+    ptx::wgmma_reg_fence(acc[1]);
     if (cs.leader()) {
         if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
         if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
@@ -602,7 +632,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
     uint8_t* sT = sB + C::kBStages * C::kBTile;                         // epilogue transpose tiles
     uint64_t* bars = reinterpret_cast<uint64_t*>(sT + ((C::kEpiBytes + 1023) & ~1023));
     uint64_t* a_full = bars;                       // [kAStages]
-    uint64_t* a_empty = a_full + C::kAStages;      // one arrival per consumer warpgroup
+    uint64_t* a_empty = a_full + C::kAStages;
     uint64_t* b_full = a_empty + C::kAStages;      // [kBStages]
     uint64_t* b_empty = b_full + C::kBStages;
     uint64_t* sched_full = b_empty + C::kBStages;  // [kSched]
@@ -616,8 +646,9 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
     unsigned* done = p.sched + 1;                  // done[layer * max_batch + image]
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < C::kAStages; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], 2); }
-        for (int s = 0; s < C::kBStages; ++s) { ptx::mbar_init(&b_full[s], 1); ptx::mbar_init(&b_empty[s], 2); }
+        // an operand stage is read by the one consumer warpgroup that owns its unit
+        for (int s = 0; s < C::kAStages; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], 1); }
+        for (int s = 0; s < C::kBStages; ++s) { ptx::mbar_init(&b_full[s], 1); ptx::mbar_init(&b_empty[s], 1); }
         for (int s = 0; s < C::kSched; ++s) { ptx::mbar_init(&sched_full[s], 1); ptx::mbar_init(&sched_empty[s], 9); }   // B producer + 8 consumer warps
         ptx::fence_barrier_init();
         ptx::fence_proxy_async();
@@ -637,102 +668,125 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
         return u;
     };
 
-    if (warp == 0) {
-        // ============================== scheduler + A producer ================================
-        if (lane == 0) {
-            for (int l = 0; l < p.n_layers; ++l)    // every layer brings its own tensor maps: fetch the descriptors now, not at each layer's first load
-                for (int m = 0; m < (p.layer[l].kind == KIND_S2 ? 4 : 1); ++m) ptx::prefetch_tmap(&p.layer[l].amap[m]);
-            ptx::grid_dep_wait();                   // the first layer's input comes from the previous kernel
-            int stage = 0; uint32_t phase = 0;
-            int ps = 0; uint32_t pph = 0;
-            // latency mode: the pieces of a unit (consecutive indices) must sit on DIFFERENT CTAs, because a piece's epilogue waits for
-            // the others' partial sums -- units are dealt round robin (index i goes to CTA i mod grid; every wait then points at a
-            // smaller index or at a piece whose CTA only has smaller indices left to finish: no cycle).  Throughput mode: first come, first served.
-            const bool dealt = p.ksplit > 1;
-            int u = dealt ? static_cast<int>(blockIdx.x) : static_cast<int>(atomicAdd(p.sched, 1u));
-            for (;;) {
-                ptx::mbar_wait(&sched_empty[ps], pph ^ 1);
-                sched_slot[ps] = u;
-                ptx::mbar_arrive(&sched_full[ps]);  // release: the slot write is visible to the waiters
-                if (++ps == C::kSched) { ps = 0; pph ^= 1; }
-                if (u >= p.total_units) break;
-                const UnitCoord c = decode_unit(p, u);
-                const LayerDesc& L = p.layer[c.l];
-                if (L.dep_layer >= 0) {
-                    // this image's previous-layer output is complete once all its units' epilogue warps have signalled
-                    const int* flag = reinterpret_cast<const int*>(done + L.dep_layer * p.max_batch + c.img);
-                    if (static_cast<unsigned>(ptx::ld_acquire_gpu(flag)) < L.dep_target) {
-                        const long long t0 = clock64();
-                        while (static_cast<unsigned>(ptx::ld_acquire_gpu(flag)) < L.dep_target) {
-                            __nanosleep(64);
-                            if (clock64() - t0 > (1ll << 34)) ptx::timeout_trap();     // ~10 s: a scheduling bug becomes an error, not a hung GPU
+    if (warp < 4) {
+        ptx::setmaxnreg_dec<kProducerRegs>();       // the whole producer warpgroup, idle warps 2-3 included
+        if (warp == 0) {
+            // ============================== scheduler + A producer ================================
+            if (lane == 0) {
+                for (int l = 0; l < p.n_layers; ++l)    // every layer brings its own tensor maps: fetch the descriptors now, not at each layer's first load
+                    for (int m = 0; m < (p.layer[l].kind == KIND_S2 ? 4 : 1); ++m) ptx::prefetch_tmap(&p.layer[l].amap[m]);
+                ptx::grid_dep_wait();                   // the first layer's input comes from the previous kernel
+                int stage = 0; uint32_t phase = 0;
+                int ps = 0; uint32_t pph = 0;
+                // latency mode: the pieces of a unit (consecutive indices) must sit on DIFFERENT CTAs, because a piece's epilogue waits for
+                // the others' partial sums -- units are dealt round robin (index i goes to CTA i mod grid; every wait then points at a
+                // smaller index or at a piece whose CTA only has smaller indices left to finish: no cycle).  Throughput mode: first come, first served.
+                const bool dealt = p.ksplit > 1;
+                int u = dealt ? static_cast<int>(blockIdx.x) : static_cast<int>(atomicAdd(p.sched, 1u));
+                for (;;) {
+                    ptx::mbar_wait(&sched_empty[ps], pph ^ 1);
+                    sched_slot[ps] = u;
+                    ptx::mbar_arrive(&sched_full[ps]);  // release: the slot write is visible to the waiters
+                    if (++ps == C::kSched) { ps = 0; pph ^= 1; }
+                    if (u >= p.total_units) break;
+                    const UnitCoord c = decode_unit(p, u);
+                    const LayerDesc& L = p.layer[c.l];
+                    if (L.dep_layer >= 0) {
+                        // this image's previous-layer output is complete once all its units' epilogue warps have signalled
+                        const int* flag = reinterpret_cast<const int*>(done + L.dep_layer * p.max_batch + c.img);
+                        if (static_cast<unsigned>(ptx::ld_acquire_gpu(flag)) < L.dep_target) {
+                            const long long t0 = clock64();
+                            while (static_cast<unsigned>(ptx::ld_acquire_gpu(flag)) < L.dep_target) {
+                                __nanosleep(64);
+                                if (clock64() - t0 > (1ll << 34)) ptx::timeout_trap();     // ~10 s: a scheduling bug becomes an error, not a hung GPU
+                            }
                         }
+                        ptx::fence_proxy_async_all();   // the TMA (async proxy) reads below must observe what the acquire made visible
                     }
-                    ptx::fence_proxy_async_all();   // the TMA (async proxy) reads below must observe what the acquire made visible
+                    unit_stamp(p, u, 0);
+                    if (L.kind == KIND_S1) trunk_load_unit<KIND_S1>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
+                    else                   trunk_load_unit<KIND_S2>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
+                    u = dealt ? u + static_cast<int>(gridDim.x) : static_cast<int>(atomicAdd(p.sched, 1u));   // pull the next unit only now: look-ahead = the A pipeline depth
                 }
-                unit_stamp(p, u, 0);
-                if (L.kind == KIND_S1) trunk_load_unit<KIND_S1>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
-                else                   trunk_load_unit<KIND_S2>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
-                u = dealt ? u + static_cast<int>(gridDim.x) : static_cast<int>(atomicAdd(p.sched, 1u));   // pull the next unit only now: look-ahead = the A pipeline depth
+            }
+        } else if (warp == 1) {
+            // ============================== B producer ================================
+            if (lane == 0) {
+                if (!p.img_wid) for (int l = 0; l < p.n_layers; ++l) ptx::prefetch_tmap(&p.layer[l].bmap);
+                int stage = 0; uint32_t phase = 0;
+                for (;;) {
+                    const int u = next_unit(false);
+                    if (u >= p.total_units) break;
+                    const UnitCoord c = decode_unit(p, u);
+                    const LayerDesc& L = p.layer[c.l];
+                    const CUtensorMap* bm = p.img_wid ? p.gbmaps + p.img_wid[c.img] * kLayersPerSet + L.li : &L.bmap;
+                    if (L.kind == KIND_S1) trunk_load_weights<KIND_S1, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
+                    else                   trunk_load_weights<KIND_S2, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
+                }
             }
         }
-    } else if (warp == 1) {
-        // ============================== B producer ================================
-        if (lane == 0) {
-            if (!p.img_wid) for (int l = 0; l < p.n_layers; ++l) ptx::prefetch_tmap(&p.layer[l].bmap);
-            int stage = 0; uint32_t phase = 0;
-            for (;;) {
-                const int u = next_unit(false);
-                if (u >= p.total_units) break;
-                const UnitCoord c = decode_unit(p, u);
-                const LayerDesc& L = p.layer[c.l];
-                const CUtensorMap* bm = p.img_wid ? p.gbmaps + p.img_wid[c.img] * kLayersPerSet + L.li : &L.bmap;
-                if (L.kind == KIND_S1) trunk_load_weights<KIND_S1, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
-                else                   trunk_load_weights<KIND_S2, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
-            }
-        }
-    } else if (warp >= 4) {
-        // ============================== MMA + epilogue (two warpgroups, 8 warps) ==========================
+    } else {
+        // ============================== MMA + epilogue (two warpgroups, alternate units) ==========================
+        ptx::setmaxnreg_inc<kConsumerRegs>();
         using S = Storage<PREC>;
         using R4 = Raw<PREC, 4>;
         ptx::grid_dep_wait();
         const Consumer cs;
-        const int ew = cs.ew;                       // consumer warp 0..7 = tile rows 16 ew .. 16 ew + 15
-        float (*stg)[C::kEpiPitch] = reinterpret_cast<float (*)[C::kEpiPitch]>(sT + ew * C::kEpiWarpBytes);
-        int* rowtab = reinterpret_cast<int*>(sT + ew * C::kEpiWarpBytes + 16 * C::kEpiPitch * 4);
+        const int cw = cs.cw;                       // warp cw of a warpgroup = tile rows 16 cw + [0, 16) and 64 + 16 cw + [0, 16) of its units
+        float (*stg)[C::kEpiPitch] = reinterpret_cast<float (*)[C::kEpiPitch]>(sT + cs.ew * C::kEpiWarpBytes);
+        int* rowtab = reinterpret_cast<int*>(sT + cs.ew * C::kEpiWarpBytes + 16 * C::kEpiPitch * 4);
         const int grp = lane & 7, sub = lane >> 3;  // lane = (16-byte column group, pixel within a group of 4)
         int astage = 0; uint32_t aphase = 0;
         int bstage = 0; uint32_t bphase = 0;
-        int it = 0;
-        for (;; ++it) {
+        // Ping-pong: warpgroup it % 2 owns the CTA's it-th unit, and the two take turns issuing MMAs (trunk_mma_unit), so one
+        // warpgroup's epilogue runs under the other's MMAs.  The first turn is warpgroup 0's.
+        if (cs.cg == 1) ptx::bar_arrive(kTurnBar, 256);
+        for (int it = 0;; ++it) {
             const int u = next_unit(true);
-            if (u >= p.total_units) break;
+            const bool mine = (it & 1) == cs.cg;
+            if (u >= p.total_units) {
+                // no unit left to pass the turn on to: the warpgroup whose turn it is takes it, so both barriers end balanced
+                if (mine) ptx::bar_sync(kTurnBar + cs.cg, 256);
+                break;
+            }
             const UnitCoord c = decode_unit(p, u);
             const LayerDesc& L = p.layer[c.l];
             const int chunks = L.chunks / p.ksplit;          // K chunks of this piece (the host makes chunks divisible)
+            if (!mine) {
+                // the other warpgroup's unit: step this warpgroup's operand ring positions past the stages it occupies
+                ring_skip(astage, aphase, chunks * (L.kind == KIND_S1 ? KTab<KIND_S1>::NU : KTab<KIND_S2>::NU), C::kAStages);
+                ring_skip(bstage, bphase, chunks * kTaps3, C::kBStages);
+                continue;
+            }
             {
-                const int rw = 16 * ew + (lane & 15);
+                // lane < 16: tile row 16 cw + lane; lane >= 16: tile row 64 + 16 cw + lane - 16
+                const int rw = 64 * (lane >> 4) + 16 * cw + (lane & 15);
                 const int py = rw / 11, px = rw - py * 11;
                 const int y = c.ty * 11 + py, x = c.tx * 11 + px;
                 const bool valid = (rw < 121) && (y < L.Ho) && (x < L.Wo);
                 __syncwarp();
-                if (lane < 16) rowtab[lane] = valid ? (c.img * L.Ho + y) * L.Wo + x : -1;   // pixel index of tile row 16 ew + lane
+                rowtab[lane] = valid ? (c.img * L.Ho + y) * L.Wo + x : -1;
                 __syncwarp();
             }
-            int pix[4];                                          // pixels this lane post-processes: warp rows 4k + sub (same for every block)
+            const int ch0 = c.grp * L.cout + c.n_tile * BN;      // first output channel of this unit
+            const float* bias_base = p.img_wid ? p.gbias[p.img_wid[c.img] * kLayersPerSet + L.li] : L.bias;
+            float4 b4[BN / 32];                                  // bias of the four 32-column blocks: loads in flight during the MMAs
 #pragma unroll
-            for (int k = 0; k < 4; ++k) pix[k] = rowtab[4 * k + sub];
+            for (int bi = 0; bi < BN / 32; ++bi) b4[bi] = __ldg(reinterpret_cast<const float4*>(bias_base + ch0 + 32 * bi + grp * 4));
 
-            float acc[C::kAcc];
+            float acc[2][C::kAcc];                               // tile rows [0, 64) and [64, 128)
 #pragma unroll
-            for (int i = 0; i < C::kAcc; ++i) acc[i] = 0.f;
+            for (int i = 0; i < C::kAcc; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
             unsigned long long* ust = (p.trace && u < 2048) ? p.trace + 256 * 8 + u * 5 + 1 : nullptr;
             if (L.kind == KIND_S1) trunk_mma_unit<KIND_S1, PREC>(acc, cs, chunks, sA, sB, a_full, a_empty, b_full, b_empty, astage, aphase, bstage, bphase, p.trace, it == 0, ust);
             else                   trunk_mma_unit<KIND_S2, PREC>(acc, cs, chunks, sA, sB, a_full, a_empty, b_full, b_empty, astage, aphase, bstage, bphase, p.trace, it == 0, ust);
-            if (threadIdx.x == 128) { unit_stamp(p, u, 2); unit_stamp(p, u, 3); if (it == 0) trace_stamp(p.trace, 5); }
+            if (cs.leader()) { unit_stamp(p, u, 2); unit_stamp(p, u, 3); if (it == 0) trace_stamp(p.trace, 5); }
+            int pix[2][4];                                       // pixels this lane post-processes: rows 4k + sub of each 16-row slice
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+                for (int k = 0; k < 4; ++k) pix[hf][k] = rowtab[16 * hf + 4 * k + sub];
 
-            const int ch0 = c.grp * L.cout + c.n_tile * BN;      // first output channel of this unit
-            const float* bias_base = p.img_wid ? p.gbias[p.img_wid[c.img] * kLayersPerSet + L.li] : L.bias;
             if (L.res && L.dep_layer >= 0) {
                 // the residual was written earlier in THIS launch by other CTAs (an ancestor layer of this unit): order this
                 // warp's loads after the completion counter the producer thread already observed
@@ -740,10 +794,10 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 __syncwarp();
             }
             const bool split = p.ksplit > 1;
-            // this warp's slice (16 rows x 128 columns) of piece `pc` of this unit in the split-K scratch: per 32-column block the
-            // fragment's 16 registers as 4 float4, [block][float4 jj][lane]
+            // this warp's slice (its 32 rows x 128 columns) of piece `pc` of this unit in the split-K scratch: per 64-row half and
+            // 32-column block the fragment's 16 registers as 4 float4, [half][block][float4 jj][lane]
             auto slice_of = [&](int pc) -> float* {
-                return p.partial + ((static_cast<size_t>(c.gidx) * p.ksplit + pc) * 8 + ew) * (16 * BN);
+                return p.partial + ((static_cast<size_t>(c.gidx) * p.ksplit + pc) * 4 + cw) * (32 * BN);
             };
             unsigned own = 0xFu;                                 // which of the unit's four 32-column blocks this warp post-processes
             if (split) {
@@ -752,16 +806,19 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 // them in piece order 0..ksplit-1 (the result does not depend on arrival order).
                 float4* d4 = reinterpret_cast<float4*>(slice_of(c.piece)) + lane;
 #pragma unroll
-                for (int q = 0; q < C::kAcc / 4; ++q) d4[q * 32] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+                for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+                    for (int q = 0; q < C::kAcc / 4; ++q)
+                        d4[(hf * C::kAcc / 4 + q) * 32] = make_float4(acc[hf][4 * q], acc[hf][4 * q + 1], acc[hf][4 * q + 2], acc[hf][4 * q + 3]);
                 __threadfence();
                 __syncwarp();
-                if (lane == 0) atomicAdd(p.slice_cnt + c.gidx * 8 + ew, 1u);
+                if (lane == 0) atomicAdd(p.slice_cnt + c.gidx * 4 + cw, 1u);
                 own = 0u;
 #pragma unroll
                 for (int bi = 0; bi < BN / 32; ++bi)
                     if (bi * p.ksplit / (BN / 32) == c.piece) own |= 1u << bi;
                 if (lane == 0) {
-                    const int* cnt = reinterpret_cast<const int*>(p.slice_cnt + c.gidx * 8 + ew);
+                    const int* cnt = reinterpret_cast<const int*>(p.slice_cnt + c.gidx * 4 + cw);
                     const long long t0 = clock64();
                     while (ptx::ld_acquire_gpu(cnt) < p.ksplit) {
                         __nanosleep(32);
@@ -772,80 +829,86 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 __threadfence();                                                     // order the reads below after the other pieces' dumps
                 // the owned blocks' sums of all pieces, in piece order, back into the fragment registers
 #pragma unroll
-                for (int bi = 0; bi < BN / 32; ++bi) {
-                    if (!((own >> bi) & 1u)) continue;
+                for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        float4 v[kSplitK];                       // all pieces' loads in flight before the first add
+                    for (int bi = 0; bi < BN / 32; ++bi) {
+                        if (!((own >> bi) & 1u)) continue;
 #pragma unroll
-                        for (int pc = 0; pc < kSplitK; ++pc)
-                            if (pc < p.ksplit) v[pc] = __ldcg(reinterpret_cast<const float4*>(slice_of(pc)) + lane + bi * 128 + jj * 32);
-                        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+                        for (int jj = 0; jj < 4; ++jj) {
+                            float4 v[kSplitK];                       // all pieces' loads in flight before the first add
 #pragma unroll
-                        for (int pc = 0; pc < kSplitK; ++pc)
-                            if (pc < p.ksplit) { a.x += v[pc].x; a.y += v[pc].y; a.z += v[pc].z; a.w += v[pc].w; }
-                        acc[16 * bi + 4 * jj] = a.x; acc[16 * bi + 4 * jj + 1] = a.y; acc[16 * bi + 4 * jj + 2] = a.z; acc[16 * bi + 4 * jj + 3] = a.w;
-                    }
-                }
-            }
+                            for (int pc = 0; pc < kSplitK; ++pc)
+                                if (pc < p.ksplit) v[pc] = __ldcg(reinterpret_cast<const float4*>(slice_of(pc)) + lane + (hf * C::kAcc / 4 + 4 * bi + jj) * 32);
+                            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-            for (int bi = 0; bi < BN / 32; ++bi) {
-                if (!((own >> bi) & 1u)) continue;
-                const int chan = ch0 + 32 * bi;                   // first channel of this 32-channel block
-                // bias and residual pieces first: their L2 latency overlaps the staging round trip below
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias_base + chan + grp * 4));
-                R4 rr[4];                                        // residual: this lane's 4 pixels, 4 channels each
-                if (L.res) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        rr[k] = R4{};
-                        if (pix[k] >= 0) {
-                            const uint8_t* rp = L.res + S::addr(pix[k], L.res_c, chan + grp * 4);
-#pragma unroll
-                            for (int q = 0; q < R4::kPieces; ++q) rr[k].set(q, __ldcg(R4::at(rp, q)));
+                            for (int pc = 0; pc < kSplitK; ++pc)
+                                if (pc < p.ksplit) { a.x += v[pc].x; a.y += v[pc].y; a.z += v[pc].z; a.w += v[pc].w; }
+                            acc[hf][16 * bi + 4 * jj] = a.x; acc[hf][16 * bi + 4 * jj + 1] = a.y; acc[hf][16 * bi + 4 * jj + 2] = a.z; acc[hf][16 * bi + 4 * jj + 3] = a.w;
                         }
                     }
-                }
-                // fragment -> rows of the staging tile: register 16 bi + 4 jj + 2 h + e = warp row R + 8h, block column 8 jj + 2m + e
-                __syncwarp();                                    // previous block's readers are done with stg
+            }
+            // the two 16-row slices of this warp one after the other through its staging tile: slice 4 hf + cw = tile rows 16 (4 hf + cw) + [0, 16)
 #pragma unroll
-                for (int jj = 0; jj < 4; ++jj)
+            for (int hf = 0; hf < 2; ++hf) {
+                const int slice = 4 * hf + cw;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        *reinterpret_cast<float2*>(&stg[cs.R + 8 * h][8 * jj + 2 * cs.m]) = make_float2(acc[16 * bi + 4 * jj + 2 * h], acc[16 * bi + 4 * jj + 2 * h + 1]);
-                __syncwarp();
-                float4 a4[4];
+                for (int bi = 0; bi < BN / 32; ++bi) {
+                    if (!((own >> bi) & 1u)) continue;
+                    const int chan = ch0 + 32 * bi;                   // first channel of this 32-channel block
+                    // residual pieces first: their L2 latency overlaps the staging round trip below
+                    R4 rr[4];                                        // residual: this lane's 4 pixels, 4 channels each
+                    if (L.res) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    a4[k] = *reinterpret_cast<const float4*>(&stg[4 * k + sub][grp * 4]);
-                    a4[k].x += b4.x; a4[k].y += b4.y; a4[k].z += b4.z; a4[k].w += b4.w;
-                }
-                if (L.res) {
+                        for (int k = 0; k < 4; ++k) {
+                            rr[k] = R4{};
+                            if (pix[hf][k] >= 0) {
+                                const uint8_t* rp = L.res + S::addr(pix[hf][k], L.res_c, chan + grp * 4);
+#pragma unroll
+                                for (int q = 0; q < R4::kPieces; ++q) rr[k].set(q, __ldcg(R4::at(rp, q)));
+                            }
+                        }
+                    }
+                    // fragment -> rows of the staging tile: register 16 bi + 4 jj + 2 h + e = slice row R + 8h, block column 8 jj + 2m + e
+                    __syncwarp();                                    // previous block's readers are done with stg
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            *reinterpret_cast<float2*>(&stg[cs.R + 8 * h][8 * jj + 2 * cs.m]) = make_float2(acc[hf][16 * bi + 4 * jj + 2 * h], acc[hf][16 * bi + 4 * jj + 2 * h + 1]);
+                    __syncwarp();
+                    float4 a4[4];
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
-                        float r[4];
-                        S::decode(rr[k], r);
-                        a4[k].x += r[0]; a4[k].y += r[1]; a4[k].z += r[2]; a4[k].w += r[3];
+                        a4[k] = *reinterpret_cast<const float4*>(&stg[4 * k + sub][grp * 4]);
+                        a4[k].x += b4[bi].x; a4[k].y += b4[bi].y; a4[k].z += b4[bi].z; a4[k].w += b4[bi].w;
                     }
-                }
-                float4 psum = make_float4(0.f, 0.f, 0.f, 0.f);   // fused average pool: this lane's rows, 4 channels
+                    if (L.res) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    float4 o = a4[k];
-                    o.x = act_apply(o.x, L.act); o.y = act_apply(o.y, L.act); o.z = act_apply(o.z, L.act); o.w = act_apply(o.w, L.act);
-                    if (pix[k] < 0) continue;
-                    if (L.pool_part) { psum.x += o.x; psum.y += o.y; psum.z += o.z; psum.w += o.w; continue; }
-                    const float o4[4] = {o.x, o.y, o.z, o.w};
-                    S::encode(o4).store(L.out + S::addr(pix[k], L.out_c, L.out_coff + chan + grp * 4));
-                }
-                if (L.pool_part) {                                // rows 4k + sub summed above; fold the four `sub` groups (fixed order: deterministic)
-#pragma unroll
-                    for (int off = 8; off <= 16; off <<= 1) {
-                        psum.x += __shfl_xor_sync(0xffffffffu, psum.x, off); psum.y += __shfl_xor_sync(0xffffffffu, psum.y, off);
-                        psum.z += __shfl_xor_sync(0xffffffffu, psum.z, off); psum.w += __shfl_xor_sync(0xffffffffu, psum.w, off);
+                        for (int k = 0; k < 4; ++k) {
+                            float r[4];
+                            S::decode(rr[k], r);
+                            a4[k].x += r[0]; a4[k].y += r[1]; a4[k].z += r[2]; a4[k].w += r[3];
+                        }
                     }
-                    if (sub == 0)
-                        *reinterpret_cast<float4*>(L.pool_part + (static_cast<size_t>(c.img) * kPoolSlices + ew) * L.out_c + L.out_coff + chan + grp * 4) = psum;
+                    float4 psum = make_float4(0.f, 0.f, 0.f, 0.f);   // fused average pool: this lane's rows, 4 channels
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        float4 o = a4[k];
+                        o.x = act_apply(o.x, L.act); o.y = act_apply(o.y, L.act); o.z = act_apply(o.z, L.act); o.w = act_apply(o.w, L.act);
+                        if (pix[hf][k] < 0) continue;
+                        if (L.pool_part) { psum.x += o.x; psum.y += o.y; psum.z += o.z; psum.w += o.w; continue; }
+                        const float o4[4] = {o.x, o.y, o.z, o.w};
+                        S::encode(o4).store(L.out + S::addr(pix[hf][k], L.out_c, L.out_coff + chan + grp * 4));
+                    }
+                    if (L.pool_part) {                                // rows 4k + sub summed above; fold the four `sub` groups (fixed order: deterministic)
+#pragma unroll
+                        for (int off = 8; off <= 16; off <<= 1) {
+                            psum.x += __shfl_xor_sync(0xffffffffu, psum.x, off); psum.y += __shfl_xor_sync(0xffffffffu, psum.y, off);
+                            psum.z += __shfl_xor_sync(0xffffffffu, psum.z, off); psum.w += __shfl_xor_sync(0xffffffffu, psum.w, off);
+                        }
+                        if (sub == 0)
+                            *reinterpret_cast<float4*>(L.pool_part + (static_cast<size_t>(c.img) * kPoolSlices + slice) * L.out_c + L.out_coff + chan + grp * 4) = psum;
+                    }
                 }
             }
             // this warp's part of the unit is in memory: publish it to the units of the next layer that wait for this image
@@ -855,7 +918,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 __syncwarp();
                 if (lane == 0) atomicAdd(done + c.l * p.max_batch + c.img, 1u);
             }
-            if (threadIdx.x == 128) unit_stamp(p, u, 4);
+            if (cs.leader()) unit_stamp(p, u, 4);
         }
         if (threadIdx.x == 128) { trace_stamp(p.trace, 4); trace_stamp(p.trace, 6); }
     }

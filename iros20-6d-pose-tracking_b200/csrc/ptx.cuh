@@ -34,6 +34,15 @@ __device__ __forceinline__ void st_release_gpu(int* p, int v) {
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_wait()   { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ------------------------------------------------------ warpgroup register budget, named barriers
+// setmaxnreg: every thread of the warpgroup executes the same instruction; a raised limit waits until another warpgroup
+// has released enough registers to the CTA's pool.
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// named barrier `id` over `n` threads: bar_sync waits for the count, bar_arrive adds to it without waiting
+__device__ __forceinline__ void bar_sync(int id, int n)   { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));

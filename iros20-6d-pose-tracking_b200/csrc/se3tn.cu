@@ -533,8 +533,9 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
             LayerDesc& d = tp.layer[l];
             d.unit_base = base; base += n * d.units_per_image * ksplit;
             d.base_unit0 = base0; base0 += n * d.units_per_image;
-            // completion signals per unit: one per consumer warp of every K piece (each piece finishes 4 / ksplit of every warp's 32-column blocks)
-            if (l > 0) { d.dep_layer = l - 1; d.dep_target = 8u * static_cast<unsigned>(ksplit) * static_cast<unsigned>(tp.layer[l - 1].units_per_image); }
+            // completion signals per unit: one per warp of the owning consumer warpgroup in every K piece (each piece finishes
+            // 4 / ksplit of every warp's 32-column blocks)
+            if (l > 0) { d.dep_layer = l - 1; d.dep_target = 4u * static_cast<unsigned>(ksplit) * static_cast<unsigned>(tp.layer[l - 1].units_per_image); }
         }
         if (ksplit > 1 && base0 > kSplitMaxUnits) return fail(c, SE3TN_ERR_STATE, "split-K scratch too small");
         tp.ksplit = ksplit; tp.partial = c->partial.get();

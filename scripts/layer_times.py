@@ -1,4 +1,4 @@
-"""Per-layer conv times for a precision / env configuration (timing experiments)."""
+"""Per-layer conv times (ms) for a precision and batch size.   python scripts/layer_times.py [precision] [n]"""
 import importlib, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
@@ -12,5 +12,4 @@ eng.set_profiling(True); acc = []
 for _ in range(10):
     eng.forward(A, B, precision=prec); acc.append(eng.get_profile())
 m = np.mean(np.stack(acc), 0)
-print('%s n=%d env{DUAL_M=%s,SKIP=%s}: conv %s sum %.4f' % (prec, nb, os.environ.get('SE3TN_DUAL_M', '-'), os.environ.get('SE3TN_DEBUG_SKIP', '-'),
-      ' '.join('%.4f' % x for x in m[:14]), m[:14].sum()))
+print('%s n=%d: conv %s sum %.4f' % (prec, nb, ' '.join('%.4f' % x for x in m[:14]), m[:14].sum()))

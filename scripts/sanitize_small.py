@@ -24,6 +24,11 @@ for mode, hw in (('vispy', None), ('pyrender', (480, 640))):
         eng.track_render(R, D, K, poses, ow, 0.03, 5 * np.pi / 180, weight_ids_host=np.array([0, 1, 0], np.int32), precision=prec, mode=mode, image_hw=hw)
     eng.track_render_host(rgb, depth, K, poses.cpu().numpy(), ow.cpu().numpy(), 0.03, 5 * np.pi / 180, weight_ids=np.array([0, 1, 0], np.int32), mode=mode, image_hw=hw)
 filled = eng.fill_depth(D[:96, :128].contiguous())
+# the calls above (n = 3) run the trunk's split-K latency mode; n = 6 runs its throughput mode
+eng6 = pkg.Engine(max_batch=6); eng6.load_state_dict(synth.make_state_dict(0), 0)
+A6, B6 = synth.tensor_pairs(6, seed=2); A6 = A6.cuda(); B6 = B6.cuda()
+for prec in ('bf16x3', 'tf32', 'bf16'):
+    eng6.forward(A6, B6, precision=prec)
 m = torch.from_numpy(synth.model_points(500, 0)).cuda(); pr, gt = synth.pose_pairs(4, 0)
 add, adi = eng.add_adi(m, torch.from_numpy(pr).cuda(), torch.from_numpy(gt).cuda()); ap = eng.vocap(adi)
 torch.cuda.synchronize()
