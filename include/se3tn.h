@@ -237,6 +237,20 @@ enum { SE3TN_BLUR_BILATERAL = 0, SE3TN_BLUR_GAUSSIAN = 1 };
 int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, double max_depth, int extrapolate, int blur_type,
                         uint16_t* out_mm, float* out_m, void* stream);
 
+/* Fill the observed depth inside every following track step on this context (se3tn_track_batch, _render, _host,
+ * _render_host): fill_depth(frame_depth) exactly as se3tn_fill_depth_ex computes it, with the same kernels, into context-owned
+ * scratch, then K0 reads the filled frame.  A live sensor's raw depth image goes straight into the step, as the reference's
+ * ROS node does with fill_depth before on_track (predict_ros.py:38-41: max_depth 2.0, extrapolate 0, bilateral).
+ * enable = 0 (the default) restores the plain behaviour; the other arguments are then ignored.  The caller's frame_depth is
+ * never written.  The fill adds its launches to the step (8 bilateral, 6 gaussian, 3 more with extrapolate; see
+ * se3tn_last_launch_count) and its four arguments to the step's graph key; no profiling slot times it.  The host variants
+ * upload the whole depth frame instead of the crop-window rectangle, since the fill reads every pixel.  The scratch holds
+ * 2 x H x W floats plus the filled H x W uint16 frame and grows with the frame; growing it, here or in se3tn_fill_depth[_ex],
+ * drops the context's captured steps.  SE3TN_ERR_INVALID for an unknown blur_type or a max_depth that is not finite and > 0
+ * (as a float); the setting is then unchanged.  A context is single-threaded: a caller that shares one between trackers
+ * sets the mode it wants before each track call. */
+int se3tn_set_depth_fill(se3tn_ctx* ctx, int enable, double max_depth, int extrapolate, int blur_type);
+
 /* The reference's own calling pattern as ONE call (Tracker.on_track, predict.py:217-296: numpy arrays in, numpy pose out):
  * every pointer is HOST memory.  The frame's crop-window rectangle, the poses, widths, input A and the ids are staged
  * through context-owned pinned memory into context-owned device buffers (stable addresses, so the step's CUDA graph is
@@ -301,7 +315,7 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
 /* Number of kernels the last forward / track_batch / track_render call on this context launched (for a replayed CUDA graph:
- * the kernels inside it).  se3tn_track_batch and se3tn_track_render capture each distinct step (same pointers, sizes and
+ * the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill).  se3tn_track_batch and se3tn_track_render capture each distinct step (same pointers, sizes and
  * precision) into a CUDA graph the first time they see it and replay it afterwards -- one graph launch per step;
  * SE3TN_GRAPH=0 in the environment, an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
  * se3tn_last_step_was_graph: 1 if the last track_batch / track_render call was a graph launch. */

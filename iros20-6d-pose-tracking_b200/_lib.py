@@ -38,6 +38,7 @@ SIGNATURES = {
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
+    'se3tn_set_depth_fill': (_i, [_vp, _i, _d, _i, _i]),
     'se3tn_set_mesh': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i]),
     'se3tn_render': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),

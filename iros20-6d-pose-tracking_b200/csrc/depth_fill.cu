@@ -11,6 +11,10 @@
 // accumulation whose order OpenCV's SIMD code does not expose, so the final metres agree to ~5e-7 and the uint16 millimetres
 // to +-1 on the rare pixel that sits on a truncation boundary (tests state both tolerances).
 // One thread per pixel, seven small launches per frame (1.2 MB images, L2 resident); latency matters here, not bandwidth.
+// Every kernel executes griddepcontrol.launch_dependents at entry: inside a track step that fills the frame (se3tn_set_depth_fill)
+// the next launch is preprocess_kernel, launched with programmatic dependent launch, which then becomes resident under the
+// last fill kernel's tail and reads the filled frame only after its griddepcontrol.wait.  No fill kernel is itself launched
+// with that attribute, so each one starts after the previous launch in the stream has completed.
 // The two optional branches of the reference (never used by its ROS node) are here too:
 //   extrapolate=True   every column's first valid value is extended to the top of the image, then the remaining empty pixels
 //                      take the 31x31 dilation (separable row / column maxima; exact)
@@ -32,6 +36,7 @@ __device__ __forceinline__ float inverted(const uint16_t* __restrict__ in, int i
 __global__ void __launch_bounds__(kBX * kBY)
 invert_dilate_kernel(const uint16_t* __restrict__ in, float* __restrict__ out, int H, int W, float max_depth)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     float m = -FLT_MAX;
@@ -51,6 +56,7 @@ template <int R, bool ERODE>
 __global__ void __launch_bounds__(kBX * kBY)
 box_morph_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     float m = ERODE ? FLT_MAX : -FLT_MAX;
@@ -72,6 +78,7 @@ box_morph_kernel(const float* __restrict__ in, float* __restrict__ out, int H, i
 __global__ void __launch_bounds__(kBX * kBY)
 fill_empty_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     float v = in[y * W + x];
@@ -104,6 +111,7 @@ __device__ __forceinline__ float from_key(unsigned k) {
 __global__ void __launch_bounds__(kBX * kBY)
 median5_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W, unsigned* __restrict__ minmax)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     float med = 0.f;
     const bool live = x < W && y < H;
@@ -137,11 +145,12 @@ median5_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int
     if (threadIdx.x == 0) { atomicMin(&minmax[0], kmin); atomicMax(&minmax[1], kmax); }
 }
 
-__global__ void init_minmax_kernel(unsigned* minmax) { minmax[0] = 0xFFFFFFFFu; minmax[1] = 0u; }
+__global__ void init_minmax_kernel(unsigned* minmax) { ptx::grid_dep_launch(); minmax[0] = 0xFFFFFFFFu; minmax[1] = 0u; }
 
 // OpenCV's range LUT: expLUT[i] = exp((i / scale)^2 * gauss_color_coeff), scale = 4096 / float(max - min); zero after underflow
 __global__ void lut_kernel(const unsigned* __restrict__ minmax, float* __restrict__ lut, float sigma_color)
 {
+    ptx::grid_dep_launch();
     const float mn = from_key(minmax[0]), mx = from_key(minmax[1]);
     const float len = static_cast<float>(static_cast<double>(mx) - static_cast<double>(mn));
     const float scale = static_cast<float>(1 << 12) / len;
@@ -157,6 +166,7 @@ __global__ void __launch_bounds__(kBX * kBY)
 bilateral_finish_kernel(const float* __restrict__ in, const float* __restrict__ lut, const unsigned* __restrict__ minmax,
                         int H, int W, float sigma_space, float max_depth, uint16_t* __restrict__ out_mm, float* __restrict__ out_m)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     const float mn = from_key(minmax[0]), mx = from_key(minmax[1]);
@@ -194,6 +204,7 @@ bilateral_finish_kernel(const float* __restrict__ in, const float* __restrict__ 
 // extrapolate: depth[0:top, col] = depth[top, col], top = first row with depth > 0.1 (np.argmax of an all-False column = 0: nothing to do)
 __global__ void extrapolate_top_kernel(float* __restrict__ d, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x >= W) return;
     int top = 0;
@@ -206,6 +217,7 @@ __global__ void extrapolate_top_kernel(float* __restrict__ d, int H, int W)
 __global__ void __launch_bounds__(kBX * kBY)
 rowmax31_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     float m = -FLT_MAX;
@@ -216,6 +228,7 @@ rowmax31_kernel(const float* __restrict__ in, float* __restrict__ out, int H, in
 __global__ void __launch_bounds__(kBX * kBY)
 large_fill_kernel(const float* __restrict__ rowmax, float* __restrict__ d, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     if (!(d[y * W + x] < 0.1f)) return;
@@ -227,6 +240,7 @@ large_fill_kernel(const float* __restrict__ rowmax, float* __restrict__ d, int H
 __global__ void __launch_bounds__(kBX * kBY)
 median5_plain_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     float v[25];
@@ -253,6 +267,7 @@ __device__ __forceinline__ int reflect101(int i, int n) {
 __global__ void __launch_bounds__(kBX * kBY)
 gaussian_finish_kernel(const float* __restrict__ in, int H, int W, float max_depth, uint16_t* __restrict__ out_mm, float* __restrict__ out_m)
 {
+    ptx::grid_dep_launch();
     const int x = blockIdx.x * kBX + threadIdx.x, y = blockIdx.y * kBY + threadIdx.y;
     if (x >= W || y >= H) return;
     const float k0 = 0.375f, k1 = 0.25f, k2 = 0.0625f;

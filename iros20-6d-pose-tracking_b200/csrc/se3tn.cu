@@ -172,7 +172,9 @@ struct se3tn_ctx {
     DevBuf<MeshDev> d_meshes; int mesh_rows = 0; bool meshes_dirty = false;   // device table of their views, rebuilt when a model changes
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
     DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
-    DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, so all four exist or none (grows on demand)
+    DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
+    // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
+    struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -894,6 +896,31 @@ int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t*
                          double tn, double rn, int precision,
                          float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s);
 
+// The depth-fill block for an H x W frame: scratch a | b | lut | minmax, then, when a track step fills the frame, the filled
+// uint16 frame.  Captured steps hold the block's addresses, so they are dropped, once the stream has drained, before the block
+// is replaced; grow installs the new block only once it exists.
+size_t fill_plane_bytes(int H, int W) { return align256(static_cast<size_t>(H) * W * sizeof(float)); }
+size_t fill_lut_bytes() { return align256((kFillLutEntries + 1) * sizeof(float)); }
+size_t fill_scratch_bytes(int H, int W) { return 2 * fill_plane_bytes(H, W) + fill_lut_bytes() + 2 * sizeof(unsigned); }
+
+int reserve_fill(se3tn_ctx* c, int H, int W, bool filled_frame, cudaStream_t s) {
+    const size_t bytes = filled_frame ? align256(fill_scratch_bytes(H, W)) + static_cast<size_t>(H) * W * sizeof(uint16_t) : fill_scratch_bytes(H, W);
+    if (bytes <= c->fill_bytes) return SE3TN_OK;
+    CU_TRY(c, cudaStreamSynchronize(s));
+    c->graphs.clear();
+    CU_TRY(c, grow(c->fill, c->fill_bytes, bytes));
+    return SE3TN_OK;
+}
+
+FillScratch fill_scratch(se3tn_ctx* c, int H, int W) {
+    uint8_t* f = c->fill.get();
+    const size_t plane = fill_plane_bytes(H, W), lut = fill_lut_bytes();
+    return {reinterpret_cast<float*>(f), reinterpret_cast<float*>(f + plane), reinterpret_cast<float*>(f + 2 * plane),
+            reinterpret_cast<unsigned*>(f + 2 * plane + lut)};
+}
+
+uint16_t* filled_frame(se3tn_ctx* c, int H, int W) { return reinterpret_cast<uint16_t*>(c->fill.get() + align256(fill_scratch_bytes(H, W))); }
+
 // One checked step of n tracks (render, if `render` is set: input A is drawn into rgbA / depthA) -> K0 -> conv stack -> K6.
 int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                const double* K, const double* poses_in, const double* object_width,
@@ -901,6 +928,8 @@ int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_dep
                const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                double tn, double rn, int precision,
                float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
+    const auto& fill = c->depth_fill;
+    if (fill.on) { const int rc = reserve_fill(c, H, W, true, s); if (rc) return rc; }   // before any graph lookup: a new block drops them all
     // ---- one CUDA graph per distinct step: every argument that ends up inside a kernel parameter is part of the key ----
     const bool graphable = c->use_graphs && !c->profiling && precision != SE3TN_PREC_FP32;
     std::vector<unsigned long long> key;
@@ -916,6 +945,8 @@ int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_dep
         key.push_back(bits(tn)); key.push_back(bits(rn));
         key.push_back(static_cast<unsigned long long>(render ? render->mode : -1));
         key.push_back(static_cast<unsigned long long>(render ? render->H : 0)); key.push_back(static_cast<unsigned long long>(render ? render->W : 0));
+        key.push_back(fill.on ? 1ull : 0ull); key.push_back(fill.on ? bits(fill.max_depth) : 0ull);
+        key.push_back(static_cast<unsigned long long>(fill.on ? fill.extrapolate : 0)); key.push_back(static_cast<unsigned long long>(fill.on ? fill.blur_type : 0));
         for (auto& g : c->graphs)
             if (g.key == key) {
                 CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
@@ -980,10 +1011,21 @@ int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t*
                              const_cast<uint8_t*>(rgbA), const_cast<uint16_t*>(depthA), stream);
         if (rc) return rc;
     }
-    // preprocess_kernel is launched with programmatic stream serialization, so with a render in front of it it may start while
-    // render_kernel is still running.  It reads rgbA / depthA only after griddepcontrol.wait (aux_kernels.cu, grid_dep_wait()),
-    // which returns once render_kernel has completed and its writes are visible: keep every read of input A behind that wait.
-    rc = se3tn_preprocess(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_dev, n,
+    const uint16_t* depth = frame_depth;
+    if (c->depth_fill.on) {                        // fill_depth(frame_depth) into the block track_step sized; the caller's frame is only read
+        const auto& f = c->depth_fill;
+        uint16_t* filled = filled_frame(c, H, W);
+        CU_TRY(c, launch_fill_depth(frame_depth, H, W, static_cast<float>(f.max_depth), f.extrapolate != 0, f.blur_type == SE3TN_BLUR_GAUSSIAN,
+                                    fill_scratch(c, H, W), filled, nullptr, s));
+        c->launches += fill_depth_launches(f.extrapolate != 0, f.blur_type == SE3TN_BLUR_GAUSSIAN);
+        depth = filled;
+    }
+    // preprocess_kernel is launched with programmatic stream serialization, so it may start while the launch in front of it
+    // (render_kernel, or the last fill kernel, both of which execute griddepcontrol.launch_dependents) is still running.  It
+    // reads rgbA / depthA and the frame only after griddepcontrol.wait (aux_kernels.cu, grid_dep_wait()), which returns once
+    // that launch has completed and its writes are visible: keep every read of input A and of the frame behind that wait.
+    // The fill kernels themselves are plain launches, so the first one starts after the render has completed.
+    rc = se3tn_preprocess(c, frame_rgb, depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_dev, n,
                           precision, nullptr, nullptr, nullptr, nullptr, stream);
     if (rc) return rc;
     PoseArgs pose; pose.in = poses_in; pose.out = poses_out; pose.tn = static_cast<float>(tn); pose.rn = static_cast<float>(rn);
@@ -1160,18 +1202,27 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (y1 <= y0 || x1 <= x0) { y0 = y1 = x0 = x1 = 0; }         // every window misses the frame: nothing of it is read
     if (static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
+    // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
+    // median-filtered image, and extrapolate scans whole columns.  Then the whole depth frame goes up; rgb stays windowed.
+    const bool whole_depth = c->depth_fill.on;
     uint8_t* hp = io.pin.get();
     const int wh = y1 - y0, ww = x1 - x0;
     if (wh > 0 && ww > 0) {
         uint8_t* st_rgb = hp; hp += static_cast<size_t>(wh) * ww * 3;
-        uint8_t* st_dep = hp; hp += align256(static_cast<size_t>(wh) * ww * 2);
+        uint8_t* st_dep = hp; if (!whole_depth) hp += align256(static_cast<size_t>(wh) * ww * 2);
         for (int y = 0; y < wh; ++y) {
             memcpy(st_rgb + static_cast<size_t>(y) * ww * 3, frame_rgb + (static_cast<size_t>(y0 + y) * W + x0) * 3, static_cast<size_t>(ww) * 3);
-            memcpy(st_dep + static_cast<size_t>(y) * ww * 2, frame_depth + static_cast<size_t>(y0 + y) * W + x0, static_cast<size_t>(ww) * 2);
+            if (!whole_depth) memcpy(st_dep + static_cast<size_t>(y) * ww * 2, frame_depth + static_cast<size_t>(y0 + y) * W + x0, static_cast<size_t>(ww) * 2);
         }
         const size_t off = static_cast<size_t>(y0) * W + x0;
         CU_TRY(c, cudaMemcpy2DAsync(d_rgb + off * 3, static_cast<size_t>(W) * 3, st_rgb, static_cast<size_t>(ww) * 3, static_cast<size_t>(ww) * 3, wh, cudaMemcpyHostToDevice, s));
-        CU_TRY(c, cudaMemcpy2DAsync(d_depth + off, static_cast<size_t>(W) * 2, st_dep, static_cast<size_t>(ww) * 2, static_cast<size_t>(ww) * 2, wh, cudaMemcpyHostToDevice, s));
+        if (!whole_depth)
+            CU_TRY(c, cudaMemcpy2DAsync(d_depth + off, static_cast<size_t>(W) * 2, st_dep, static_cast<size_t>(ww) * 2, static_cast<size_t>(ww) * 2, wh, cudaMemcpyHostToDevice, s));
+    }
+    if (whole_depth) {
+        memcpy(hp, frame_depth, px * 2);
+        CU_TRY(c, cudaMemcpyAsync(d_depth, hp, px * 2, cudaMemcpyHostToDevice, s));
+        hp += px * 2;
     }
     hp = io.pin.get() + align256(static_cast<size_t>(hp - io.pin.get()));
     memcpy(hp, poses, nn * 128);
@@ -1251,20 +1302,26 @@ int se3tn_fill_depth_ex(se3tn_ctx* c, const uint16_t* depth_mm, int H, int W, do
         return fail(c, SE3TN_ERR_INVALID, "se3tn_fill_depth: bad arguments");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
-    const size_t plane = align256(static_cast<size_t>(H) * W * sizeof(float)), lut = align256((kFillLutEntries + 1) * sizeof(float)), bytes = 2 * plane + lut + 2 * sizeof(unsigned);
-    if (bytes > c->fill_bytes) CU_TRY(c, cudaStreamSynchronize(s));   // the block is about to be replaced
-    CU_TRY(c, grow(c->fill, c->fill_bytes, bytes));
-    uint8_t* f = c->fill.get();
-    const FillScratch sc = {reinterpret_cast<float*>(f), reinterpret_cast<float*>(f + plane), reinterpret_cast<float*>(f + 2 * plane),
-                            reinterpret_cast<unsigned*>(f + 2 * plane + lut)};
-    CU_TRY(c, launch_fill_depth(depth_mm, H, W, static_cast<float>(max_depth), extrapolate != 0, blur_type == SE3TN_BLUR_GAUSSIAN, sc, out_mm, out_m, s));
-    c->launches += 8;
+    const int rc = reserve_fill(c, H, W, false, s);   // a larger frame replaces the block, and drops the steps that captured it
+    if (rc) return rc;
+    CU_TRY(c, launch_fill_depth(depth_mm, H, W, static_cast<float>(max_depth), extrapolate != 0, blur_type == SE3TN_BLUR_GAUSSIAN, fill_scratch(c, H, W), out_mm, out_m, s));
+    c->launches += fill_depth_launches(extrapolate != 0, blur_type == SE3TN_BLUR_GAUSSIAN);
     return SE3TN_OK;
 }
 
 int se3tn_fill_depth(se3tn_ctx* c, const uint16_t* depth_mm, int H, int W, double max_depth,
                      uint16_t* out_mm, float* out_m, void* stream) {
     return se3tn_fill_depth_ex(c, depth_mm, H, W, max_depth, 0, SE3TN_BLUR_BILATERAL, out_mm, out_m, stream);
+}
+
+int se3tn_set_depth_fill(se3tn_ctx* c, int enable, double max_depth, int extrapolate, int blur_type) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!enable) { c->depth_fill = {}; return SE3TN_OK; }
+    if (blur_type != SE3TN_BLUR_BILATERAL && blur_type != SE3TN_BLUR_GAUSSIAN) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_depth_fill: unknown blur_type");
+    const float md = static_cast<float>(max_depth);                // what the kernels compute with
+    if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_depth_fill: max_depth must be finite and > 0");
+    c->depth_fill = {true, max_depth, extrapolate != 0 ? 1 : 0, blur_type};
+    return SE3TN_OK;
 }
 
 int se3tn_set_mesh(se3tn_ctx* c, int mesh_id, const float* pos, const float* nrm, const uint8_t* col,

@@ -5,6 +5,7 @@ torch.distributed -- all arithmetic happens inside libse3tn.so.  There is no CPU
 fallback: without a CUDA device and the built library every call raises.
 """
 import ctypes as C
+import math
 import numpy as np
 import torch
 
@@ -166,10 +167,12 @@ class Engine:
 
     def track_batch(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA,
                     trans_normalizer, rot_normalizer, weight_ids_host=None, weight_ids_dev=None,
-                    precision='bf16x3', out_poses=None, out_trans=None, out_rot=None):
-        """n independent tracks of one frame: K0 -> conv stack -> K6, all enqueued on the current stream."""
+                    precision='bf16x3', out_poses=None, out_trans=None, out_rot=None, fill_depth=None):
+        """n independent tracks of one frame: K0 -> conv stack -> K6, all enqueued on the current stream.  fill_depth: the
+        observed depth is hole-filled inside the step first (depth_fill_spec); frame_depth itself is never written."""
         n = poses.shape[0]
         self._check_frame(frame_rgb, frame_depth, rgbA, depthA, poses, object_width, n)
+        fill = self.depth_fill_spec(fill_depth)
         H, W = frame_depth.shape
         Kh = self._k4(K)
         out_poses = torch.empty_like(poses) if out_poses is None else out_poses
@@ -180,6 +183,7 @@ class Engine:
             wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
             if weight_ids_dev is None:
                 weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        self._set_depth_fill(fill)
         _lib.check(self.lib.se3tn_track_batch(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W,
                                               Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width),
                                               _ptr(rgbA), _ptr(depthA),
@@ -191,15 +195,16 @@ class Engine:
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
-                     out_poses=None, out_trans=None, out_rot=None):
+                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
-        mode / image_hw as in render().  CUDA tensors in and out; nothing is synchronised."""
+        mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised."""
         n = poses.shape[0]
         self._check_frame(frame_rgb, frame_depth, None, None, poses, object_width, n)
         H, W = frame_depth.shape
         Kh = self._k4(K)
         rmode, rH, rW = self._render_mode(mode, image_hw)
+        fill = self.depth_fill_spec(fill_depth)
         out_poses = torch.empty_like(poses) if out_poses is None else out_poses
         out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
         out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
@@ -208,6 +213,7 @@ class Engine:
             wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
             if weight_ids_dev is None:
                 weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        self._set_depth_fill(fill)
         _lib.check(self.lib.se3tn_track_render(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W,
                                                Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width), rmode, rH, rW,
                                                wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0),
@@ -217,26 +223,29 @@ class Engine:
         return out_poses, out_trans, out_rot
 
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
-                   weight_ids=None, precision='bf16x3', want_residuals=False):
+                   weight_ids=None, precision='bf16x3', want_residuals=False, fill_depth=None):
         """The reference's calling pattern as one library call: numpy arrays in, numpy poses out, synchronous (se3tn_track_host).
         frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), poses float64 (n,4,4), object_width float64 (n), rgbA uint8
-        (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous."""
+        (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous.  fill_depth as in
+        track_batch: a live sensor's raw depth frame goes in as it is (the whole frame is uploaded then)."""
         n = int(poses.shape[0])
         wid = self._check_host('track_host', frame_rgb, frame_depth, poses, object_width, weight_ids, n,
                                (('rgbA', rgbA, np.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', depthA, np.uint16, (n, IMAGE_SIZE, IMAGE_SIZE))))
+        fill = self.depth_fill_spec(fill_depth)
         H, W = frame_depth.shape
         Kh = self._k4(K)
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
+        self._set_depth_fill(fill)
         _lib.check(self.lib.se3tn_track_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
                                              vp(rgbA), vp(depthA), vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
                                              vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
         return (out, tr, ro) if want_residuals else out
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
-                          weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False):
+                          weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None):
         """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
         without ids); mode / image_hw as in render()."""
@@ -245,20 +254,23 @@ class Engine:
         H, W = frame_depth.shape
         Kh = self._k4(K)
         rmode, rH, rW = self._render_mode(mode, image_hw)
+        fill = self.depth_fill_spec(fill_depth)
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
+        self._set_depth_fill(fill)
         _lib.check(self.lib.se3tn_track_render_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
                                                     rmode, rH, rW, vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
                                                     vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
         return (out, tr, ro) if want_residuals else out
 
     def upload_frame_window(self, rgb_host, depth_host, rgb_dev, depth_dev, y0, y1, x0, x1):
-        """Copy rows [y0,y1) x columns [x0,x1) of contiguous numpy frames (uint8 (H,W,3), uint16 (H,W)) into full-size device frame
-        buffers: K0 only reads a frame inside the tracks' crop windows."""
-        H, W = depth_host.shape
-        _lib.check(self.lib.se3tn_upload_frame_window(self._ctx, rgb_host.ctypes.data_as(C.c_void_p), depth_host.ctypes.data_as(C.c_void_p), int(H), int(W),
+        """Copy rows [y0,y1) x columns [x0,x1) of contiguous numpy frames (uint8 (H,W,3), uint16 (H,W); either may be None) into
+        full-size device frame buffers: K0 only reads a frame inside the tracks' crop windows."""
+        H, W = (depth_host if depth_host is not None else rgb_host).shape[:2]
+        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
+        _lib.check(self.lib.se3tn_upload_frame_window(self._ctx, vp(rgb_host), vp(depth_host), int(H), int(W),
                                                       int(y0), int(y1), int(x0), int(x1), _ptr(rgb_dev), _ptr(depth_dev), _stream(self.device)), self._ctx)
 
     # ------------------------------------------------------------------ metrics (SURVEY 8f row 1)
@@ -337,6 +349,28 @@ class Engine:
         _lib.check(self.lib.se3tn_fill_depth_ex(self._ctx, _ptr(depth_mm), int(H), int(W), float(max_depth), int(bool(extrapolate)),
                                                 1 if blur_type == 'gaussian' else 0, _ptr(out), _ptr(out_m), _stream(self.device)), self._ctx)
         return (out, out_m) if want_metres else out
+
+    @staticmethod
+    def depth_fill_spec(fill_depth):
+        """(enable, max_depth, extrapolate, blur_type) for se3tn_set_depth_fill from the tracking calls' fill_depth argument:
+        None / False: the frame's depth is used as it is.  True: fill_depth as the reference's ROS node calls it before every
+        on_track (predict_ros.py:38-41: max_depth 2.0 m, no extrapolation, bilateral).  A dict with any of max_depth /
+        extrapolate / blur_type: those arguments of fill_depth, the rest as with True."""
+        if fill_depth is None or isinstance(fill_depth, (bool, np.bool_)):
+            return (1, 2.0, 0, 0) if fill_depth else (0, 0.0, 0, 0)
+        if not isinstance(fill_depth, dict) or not set(fill_depth) <= {'max_depth', 'extrapolate', 'blur_type'}:
+            raise ValueError('fill_depth must be None, a bool or a dict with max_depth / extrapolate / blur_type')
+        blur_type = fill_depth.get('blur_type', 'bilateral')
+        if blur_type not in ('bilateral', 'gaussian'):
+            raise ValueError("blur_type must be 'bilateral' or 'gaussian'")
+        max_depth = float(fill_depth.get('max_depth', 2.0))
+        if not (math.isfinite(max_depth) and max_depth > 0):
+            raise ValueError('max_depth must be finite and > 0')
+        return (1, max_depth, int(bool(fill_depth.get('extrapolate', False))), 1 if blur_type == 'gaussian' else 0)
+
+    def _set_depth_fill(self, spec):
+        """Every tracking call sets the context's fill mode it wants: Trackers that share an Engine keep their own."""
+        _lib.check(self.lib.se3tn_set_depth_fill(self._ctx, int(spec[0]), float(spec[1]), int(spec[2]), int(spec[3])), self._ctx)
 
     # ------------------------------------------------------------------ introspection
     def debug_buffer(self, buf_id, n):

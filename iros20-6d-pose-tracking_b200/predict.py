@@ -13,6 +13,9 @@ Differences, all additive:
     show=True.
   * on_track_batch(): N independent tracks of one frame in one batched launch sequence (the
     reference is batch 1, F15).
+  * Tracker(..., fill_depth=True): on_track takes a live sensor's raw depth frame and hole-fills it
+    inside the tracking step, as the reference's ROS node does with Utils.fill_depth before every
+    on_track (predict_ros.py:38-41).
 """
 import os
 import numpy as np
@@ -126,7 +129,13 @@ def crop_windows_union(poses, K, object_width, H, W, margin=2):
 
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
-                 rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64):
+                 rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
+                 fill_depth=False):
+        """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
+        tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
+        / blur_type (Engine.depth_fill_spec)."""
+        Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
+        self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
         if self.image_size[0] != 176:
@@ -298,9 +307,10 @@ class Tracker:
             if renderer is not None:
                 return self.engine.track_render_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h,
                                                      self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw)
+                                                     mode=renderer.mode, image_hw=renderer.image_hw, fill_depth=self.fill_depth)
             return self.engine.track_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h, c(rgbA, np.uint8), c(depthA, np.uint16),
-                                          self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision)
+                                          self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision,
+                                          fill_depth=self.fill_depth)
         staged = not render and all(torch.is_tensor(x) and not x.is_cuda for x in (prev_poses, current_rgb, current_depth, rgbA, depthA))
 
         def up(x, dt, slot=None):
@@ -337,11 +347,18 @@ class Tracker:
                     if k2 not in self._np_bufs:
                         self._np_bufs[k2] = torch.zeros(k2[1], dtype=dt, device=dev)
                 rgb_d, depth_d = self._np_bufs[rk], self._np_bufs[dk]
+                # the fill reads the whole depth frame (the bilateral's range table is scaled by the whole image's min and max,
+                # extrapolate scans whole columns): then only rgb is windowed
+                dwin = (0, current_depth.shape[0], 0, current_depth.shape[1]) if Engine.depth_fill_spec(self.fill_depth)[0] else win
                 # through pinned staging (same geometry): a 2-D copy from pageable memory is staged row by row by the driver,
                 # from pinned memory it is one strided DMA
                 pk = ('pin', tuple(current_rgb.shape))
                 if os.environ.get('SE3TN_WINDOW_UPLOAD', 'pinned') == 'pageable':
-                    self.engine.upload_frame_window(current_rgb, current_depth, rgb_d, depth_d, *win)
+                    if dwin == win:
+                        self.engine.upload_frame_window(current_rgb, current_depth, rgb_d, depth_d, *win)
+                    else:
+                        self.engine.upload_frame_window(current_rgb, None, rgb_d, None, *win)
+                        self.engine.upload_frame_window(None, current_depth, None, depth_d, *dwin)
                     pk = None
                 elif pk not in self._np_bufs:
                     self._np_bufs[pk] = (torch.empty(current_rgb.shape, dtype=torch.uint8).pin_memory().numpy(),
@@ -349,10 +366,15 @@ class Tracker:
                 if pk is not None:
                     pin_rgb, pin_depth = self._np_bufs[pk]
                     y0, y1, x0, x1 = win
+                    dy0, dy1, dx0, dx1 = dwin
                     if self._pin_busy:
                         torch.cuda.current_stream(dev).synchronize()          # the previous call's DMA may still be reading the staging
-                    np.copyto(pin_rgb[y0:y1, x0:x1], current_rgb[y0:y1, x0:x1]); np.copyto(pin_depth[y0:y1, x0:x1], current_depth[y0:y1, x0:x1])
-                    self.engine.upload_frame_window(pin_rgb, pin_depth, rgb_d, depth_d, *win)
+                    np.copyto(pin_rgb[y0:y1, x0:x1], current_rgb[y0:y1, x0:x1]); np.copyto(pin_depth[dy0:dy1, dx0:dx1], current_depth[dy0:dy1, dx0:dx1])
+                    if dwin == win:
+                        self.engine.upload_frame_window(pin_rgb, pin_depth, rgb_d, depth_d, *win)
+                    else:
+                        self.engine.upload_frame_window(pin_rgb, None, rgb_d, None, *win)
+                        self.engine.upload_frame_window(None, pin_depth, None, depth_d, *dwin)
                     self._pin_busy = not as_numpy
             else:
                 rgb_d, depth_d = up(current_rgb, torch.uint8, 'rgb'), up(current_depth, torch.uint16, 'depth')
@@ -391,11 +413,12 @@ class Tracker:
         if renderer is not None:                      # input A is drawn inside the step, with the weight ids as mesh ids
             out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                  weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision,
-                                                 mode=renderer.mode, image_hw=renderer.image_hw, **outs)
+                                                 mode=renderer.mode, image_hw=renderer.image_hw, fill_depth=self.fill_depth, **outs)
         else:
             out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
                                                 self.trans_normalizer, self.rot_normalizer,
-                                                weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, **outs)
+                                                weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision,
+                                                fill_depth=self.fill_depth, **outs)
         if staged:
             self._stage_done[self._stage_slot].record(torch.cuda.current_stream(dev))
         return out.cpu().numpy() if as_numpy else out
