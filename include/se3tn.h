@@ -292,6 +292,37 @@ int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint
                             const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
                             double* poses_out, float* out_trans, float* out_rot, void* stream);
 
+/* ---- checkpoint validation: the loss of ready-made training pairs ---------------------------------------------------- */
+
+/* Problem.validate's per-batch work (reference problems.py:106-132) as ONE step: for n pairs as TrackDataset.__getitem__ reads
+ * them (datasets.py:70-112, crops already at 176 x 176), processData's post-transforms (datasets.py:136-137, se3tn_normalize),
+ * Se3TrackNet.forward in eval mode and Se3TrackNet.loss (se3_tracknet.py:114-121) on the labels of datasets.py:141-150.
+ *   rgbA, rgbB uint8 (n,176,176,3), depthA, depthB uint16 (n,176,176) mm, A_in_cam, B_in_cam double (n,16) row-major, device
+ *   weight_ids_host / weight_ids_dev as in se3tn_track_batch (both NULL: every pair uses set 0)
+ *   out_trans, out_rot float (n,3) device: the network's outputs
+ *   out_sq float (n,6) device or NULL: per pair (pred - float(label))^2 in fp32, translation then rotation, as nn.MSELoss forms them
+ *   out_labels double (n,6) device or NULL: trans_label then rot_label, bit-identical to se3tn_so3_log
+ *   out_sums float (2) device: the sums of the n x 3 translation terms and of the n x 3 rotation terms, added in a fixed order that
+ *     depends on n alone (thread t of one CTA adds pairs t, t+256, ... in order, then a tree); MSE = sum / (3 n).
+ * In the tensor-core modes the loss terms are formed in the head kernel (labels in fp64 by the same device function as
+ * se3tn_so3_log) and one more launch adds them: normalize + 8 resident convs + trunk + head + reduction = 12 launches, captured as
+ * one CUDA graph under se3tn_track_batch's rules (every pointer, n, precision, the ids' mix and the normalizers are the key).
+ * SE3TN_PREC_FP32 runs one FFMA forward per contiguous run of equal ids and then one stand-alone loss launch, without a graph:
+ * 1 + 17 per run + 1 launches.  Every id is checked on the host before anything is queued: an id without weights or statistics
+ * is SE3TN_ERR_STATE (the id is named); n == 0 or n > max_batch is SE3TN_ERR_INVALID.  Without out_sq the terms go to a
+ * context-owned max_batch x 6 float buffer, allocated by the first such call. */
+int se3tn_eval_pairs(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                     const double* A_in_cam, const double* B_in_cam,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                     double trans_normalizer, double rot_normalizer, int precision,
+                     float* out_trans, float* out_rot, float* out_sq, double* out_labels, float* out_sums, void* stream);
+
+/* Se3TrackNet.loss (reference se3_tracknet.py:114-121) on predictions that already exist: trans, rot float (n,3), trans_label,
+ * rot_label double (n,3), all device -> out_sums float (2) device, with the same loss terms and the same order of additions as
+ * se3tn_eval_pairs (one launch, any n > 0): the two callers agree bit for bit.  MSE = sum / (3 n). */
+int se3tn_pair_loss(se3tn_ctx* ctx, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,
+                    float* out_sums, void* stream);
+
 /* ---- introspection (tests / profiling) -------------------------------------------------------- */
 
 /* Device pointer + per-image float count of an internal NHWC activation buffer.
@@ -302,8 +333,9 @@ int se3tn_debug_buffer(se3tn_ctx* ctx, int id, float** ptr, size_t* floats_per_i
  * is bracketed by CUDA events on the caller's stream.  se3tn_get_profile synchronises those events
  * and writes SE3TN_PROFILE_SLOTS durations (ms) of the LAST call: [0..13] the 14 conv launches in
  * schedule order, [14],[15] the two max-pools, [16] head, [17] preprocess/normalize, [18] pose update,
- * [19] input repack (se3tn_forward only), [20] render.  Slots that did not run read 0. */
-#define SE3TN_PROFILE_SLOTS 21
+ * [19] input repack (se3tn_forward only), [20] render, [21] loss (se3tn_eval_pairs: the reduction of the head's loss terms, or
+ * the stand-alone loss launch in SE3TN_PREC_FP32; se3tn_pair_loss).  Slots that did not run read 0. */
+#define SE3TN_PROFILE_SLOTS 22
 int se3tn_set_profiling(se3tn_ctx* ctx, int enable);
 int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 
@@ -314,11 +346,12 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 #define SE3TN_TRACE_WORDS (14 * 256 * 8)
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
-/* Number of kernels the last forward / track_batch / track_render call on this context launched (for a replayed CUDA graph:
- * the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill).  se3tn_track_batch and se3tn_track_render capture each distinct step (same pointers, sizes and
+/* Number of kernels the last forward / track_batch / track_render / eval_pairs / pair_loss call on this context launched (for a
+ * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill).
+ * se3tn_track_batch, se3tn_track_render and se3tn_eval_pairs capture each distinct step (same pointers, sizes and
  * precision) into a CUDA graph the first time they see it and replay it afterwards -- one graph launch per step;
  * SE3TN_GRAPH=0 in the environment, an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
- * se3tn_last_step_was_graph: 1 if the last track_batch / track_render call was a graph launch. */
+ * se3tn_last_step_was_graph: 1 if the last track_batch / track_render / eval_pairs call was a graph launch. */
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);
 

@@ -9,6 +9,7 @@ OK, ERR_INVALID, ERR_CUDA, ERR_NOMEM, ERR_STATE, ERR_UNSUPPORTED = 0, -1, -2, -3
 PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16 = 0, 1, 2, 3
 RENDER_VISPY, RENDER_PYRENDER = 0, 1
 WEIGHT_BLOB_FLOATS = 13528326
+PROFILE_SLOTS = 22
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -42,6 +43,8 @@ SIGNATURES = {
     'se3tn_set_mesh': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i]),
     'se3tn_render': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    'se3tn_eval_pairs': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_pair_loss': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
     'se3tn_debug_buffer': (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_sz)]),
     'se3tn_last_launch_count': (_i, [_vp]),
     'se3tn_get_trace': (_i, [_vp, _vp]),

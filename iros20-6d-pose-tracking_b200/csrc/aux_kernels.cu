@@ -419,23 +419,36 @@ __device__ __forceinline__ void pose_update_one(const double* A, const float tr[
     for (int k = 0; k < 16; ++k) B[k] = out[k];
 }
 
+// K5 label of one pair (defined with so3_log_kernel below); the outputs may be global or shared memory
+__device__ __noinline__ void so3_label(const double* A, const double* B, double tn, double rn, double* trans_label, double* rot_label);
+
+// One squared error of the reference's loss: nn.MSELoss on pred.float() and target.float() (se3_tracknet.py:114-121) forms
+// (pred - float32(label))^2 in fp32 before it averages.
+__device__ __forceinline__ float loss_term(float pred, double label) {
+    const float d = __fsub_rn(pred, __double2float_rn(label));
+    return __fmul_rn(d, d);
+}
+
 // Head on the fused average pool (conv_wgmma.cu writes pool_part[image][kPoolSlices][1024] column sums): mean -> Linear -> tanh for
 // BOTH heads of one image per CTA (threads 0-127 translation, 128-255 rotation), and -- when poses_in is given -- the pose update of that
 // track by thread 0 (K4 + K6 in one launch: the update is a 650-instruction fp64 chain per track, pure latency as its own kernel).
+// loss.poses_a given: the pair's label (thread 0, alongside the others' FC work) and its six loss terms (LossArgs).
 // `zero_words` (nullable): scheduler / dependency counters of the step that just finished, cleared for the next one by block 0.
 __global__ void __launch_bounds__(256)
 head_pooled_kernel(const float4* __restrict__ part, const float* __restrict__ fcw, const float* __restrict__ fcb,
                    float* __restrict__ out_trans, float* __restrict__ out_rot, int npix,
                    const int* __restrict__ img_wid, const float* const* __restrict__ fc_table,
-                   const double* poses_in, double* poses_out /* may alias */, float tn, float rn,
+                   const double* poses_in, double* poses_out /* may alias */, float tn, float rn, LossArgs loss,
                    unsigned* __restrict__ zero_words, int n_zero)
 {
     ptx::grid_dep_launch();
     __shared__ float red[8][3];
     __shared__ float six[6];
+    __shared__ double label[6];
     const int n = blockIdx.x, head = threadIdx.x >> 7, t = threadIdx.x & 127;
     ptx::grid_dep_wait();
     if (zero_words && blockIdx.x == 0) for (int i = threadIdx.x; i < n_zero; i += blockDim.x) zero_words[i] = 0u;
+    if (loss.poses_a && threadIdx.x == 0) so3_label(loss.poses_a + n * 16, loss.poses_b + n * 16, loss.tn, loss.rn, label, label + 3);
     if (img_wid) { fcw = fc_table[img_wid[n]]; fcb = fcw + 6 * 512; }
     static_assert(se3tn::kPoolSlices == 8, "pairwise sum below");
     const float4* pp = part + static_cast<size_t>(n) * se3tn::kPoolSlices * 256 + head * 128 + t;
@@ -467,6 +480,10 @@ head_pooled_kernel(const float4* __restrict__ part, const float* __restrict__ fc
         const float v = tanhf(red[4 * h + 0][o] + red[4 * h + 1][o] + red[4 * h + 2][o] + red[4 * h + 3][o] + fcb[h * 3 + o]);
         (h == 0 ? out_trans : out_rot)[n * 3 + o] = v;
         six[threadIdx.x] = v;
+        if (loss.poses_a) {                                      // label[] was written by thread 0 before the barrier above
+            loss.sq[n * 6 + threadIdx.x] = loss_term(v, label[threadIdx.x]);
+            if (loss.labels) loss.labels[n * 6 + threadIdx.x] = label[threadIdx.x];
+        }
     }
     if (!poses_in) return;
     __syncthreads();
@@ -474,11 +491,89 @@ head_pooled_kernel(const float4* __restrict__ part, const float* __restrict__ fc
 }
 cudaError_t launch_head_pooled(const float* part, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                                int n_img, int npix, const int* img_wid, const float* const* fc_table,
-                               const double* poses_in, double* poses_out, float tn, float rn, unsigned* zero_words, int n_zero, cudaStream_t s) {
+                               const double* poses_in, double* poses_out, float tn, float rn, const LossArgs& loss,
+                               unsigned* zero_words, int n_zero, cudaStream_t s) {
     if (n_img <= 0) return cudaSuccess;
+    if (loss.poses_a && (!loss.poses_b || !loss.sq)) return cudaErrorInvalidValue;
     const float4* p4 = reinterpret_cast<const float4*>(part);
-    void* args[] = {&p4, &fcw, &fcb, &out_trans, &out_rot, &npix, &img_wid, &fc_table, &poses_in, &poses_out, &tn, &rn, &zero_words, &n_zero};
+    LossArgs la = loss;
+    void* args[] = {&p4, &fcw, &fcb, &out_trans, &out_rot, &npix, &img_wid, &fc_table, &poses_in, &poses_out, &tn, &rn, &la, &zero_words, &n_zero};
     return launch_pdl(reinterpret_cast<const void*>(head_pooled_kernel), dim3(n_img), dim3(256), args, s);
+}
+
+// =============================================================================================
+// The reduction of the loss terms (reference se3_tracknet.py:114-121: one nn.MSELoss per head).  Thread t adds the terms of pairs
+// t, t + 256, ... in index order, each pair's three as (x + y) + z, and a shared-memory tree adds the 256 partial sums: the order
+// depends on n alone, never on scheduling.  Both launches below use it, so the validation step and se3tn_pair_loss agree bit for
+// bit on equal terms.
+// =============================================================================================
+constexpr int kLossThreads = 256;
+
+template <class Terms>   // terms(i, float t[6]) yields pair i's six terms
+__device__ __forceinline__ void reduce_loss_terms(int n, Terms terms, float* sums)
+{
+    __shared__ float s_tr[kLossThreads], s_ro[kLossThreads];
+    float a = 0.f, b = 0.f;
+    for (int i = threadIdx.x; i < n; i += kLossThreads) {
+        float q[6];
+        terms(i, q);
+        a = __fadd_rn(a, __fadd_rn(__fadd_rn(q[0], q[1]), q[2]));
+        b = __fadd_rn(b, __fadd_rn(__fadd_rn(q[3], q[4]), q[5]));
+    }
+    s_tr[threadIdx.x] = a; s_ro[threadIdx.x] = b;
+    __syncthreads();
+#pragma unroll
+    for (int w = kLossThreads / 2; w > 0; w >>= 1) {
+        if (threadIdx.x < w) {
+            s_tr[threadIdx.x] = __fadd_rn(s_tr[threadIdx.x], s_tr[threadIdx.x + w]);
+            s_ro[threadIdx.x] = __fadd_rn(s_ro[threadIdx.x], s_ro[threadIdx.x + w]);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { sums[0] = s_tr[0]; sums[1] = s_ro[0]; }
+}
+
+__global__ void __launch_bounds__(kLossThreads) loss_reduce_kernel(const float* __restrict__ sq, int n, float* __restrict__ sums)
+{
+    reduce_loss_terms(n, [&](int i, float q[6]) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) q[k] = sq[i * 6 + k];
+    }, sums);
+}
+
+cudaError_t launch_loss_reduce(const float* sq, int n, float* sums, cudaStream_t s) {
+    if (n <= 0) return cudaErrorInvalidValue;
+    loss_reduce_kernel<<<1, kLossThreads, 0, s>>>(sq, n, sums);
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(kLossThreads)
+pair_loss_kernel(const float* __restrict__ trans, const float* __restrict__ rot, const double* __restrict__ trans_label,
+                 const double* __restrict__ rot_label, LossArgs loss, int n, float* __restrict__ sums)
+{
+    reduce_loss_terms(n, [&](int i, float q[6]) {
+        double lab[6];
+        if (trans_label) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { lab[k] = trans_label[i * 3 + k]; lab[3 + k] = rot_label[i * 3 + k]; }
+        } else {
+            so3_label(loss.poses_a + i * 16, loss.poses_b + i * 16, loss.tn, loss.rn, lab, lab + 3);
+        }
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            q[k] = loss_term(k < 3 ? trans[i * 3 + k] : rot[i * 3 + k - 3], lab[k]);
+            if (loss.sq) loss.sq[i * 6 + k] = q[k];
+            if (loss.labels) loss.labels[i * 6 + k] = lab[k];
+        }
+    }, sums);
+}
+
+cudaError_t launch_pair_loss(const float* trans, const float* rot, const double* trans_label, const double* rot_label,
+                             const LossArgs& loss, int n, float* sums, cudaStream_t s) {
+    if (n <= 0 || !trans || !rot || !sums || (!trans_label != !rot_label) || (!trans_label && (!loss.poses_a || !loss.poses_b)))
+        return cudaErrorInvalidValue;
+    pair_loss_kernel<<<1, kLossThreads, 0, s>>>(trans, rot, trans_label, rot_label, loss, n, sums);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
@@ -651,15 +746,13 @@ __device__ __forceinline__ void inv_transpose3(const double* m, double* o) {
     o[6] = (m[1] * m[5] - m[2] * m[4]) * id; o[7] = (m[2] * m[3] - m[0] * m[5]) * id; o[8] = (m[0] * m[4] - m[1] * m[3]) * id;
 }
 
-__global__ void so3_log_kernel(const double* __restrict__ poses_a, const double* __restrict__ poses_b,
-                               double tn, double rn, double* __restrict__ trans_label, double* __restrict__ rot_label, int n)
+// One pair.  so3_log_kernel, the validation head and pair_loss_kernel all call this one (not inlined) function, so their labels are
+// the same bits.
+__device__ __noinline__ void so3_label(const double* A, const double* B, double tn, double rn, double* trans_label, double* rot_label)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const double* A = poses_a + i * 16; const double* B = poses_b + i * 16;
-    trans_label[i * 3 + 0] = (B[3] - A[3]) / tn;
-    trans_label[i * 3 + 1] = (B[7] - A[7]) / tn;
-    trans_label[i * 3 + 2] = (B[11] - A[11]) / tn;
+    trans_label[0] = (B[3] - A[3]) / tn;
+    trans_label[1] = (B[7] - A[7]) / tn;
+    trans_label[2] = (B[11] - A[11]) / tn;
     double R[9];
 #pragma unroll
     for (int r = 0; r < 3; ++r)
@@ -698,7 +791,15 @@ __global__ void so3_log_kernel(const double* __restrict__ poses_a, const double*
         const double vth = theta / (2 * s);
         rx *= vth; ry *= vth; rz *= vth;
     }
-    rot_label[i * 3 + 0] = rx / rn; rot_label[i * 3 + 1] = ry / rn; rot_label[i * 3 + 2] = rz / rn;
+    rot_label[0] = rx / rn; rot_label[1] = ry / rn; rot_label[2] = rz / rn;
+}
+
+__global__ void so3_log_kernel(const double* __restrict__ poses_a, const double* __restrict__ poses_b,
+                               double tn, double rn, double* __restrict__ trans_label, double* __restrict__ rot_label, int n)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    so3_label(poses_a + i * 16, poses_b + i * 16, tn, rn, trans_label + i * 3, rot_label + i * 3);
 }
 
 cudaError_t launch_so3_log(const double* poses_a, const double* poses_b, double tn, double rn,

@@ -32,6 +32,17 @@ struct PreprocessArgs {
     uint16_t* crop_depth;          // N x 176 x 176 (nullable)
 };
 
+// The training loss of a validation step (reference se3_tracknet.py:114-121 on the labels of datasets.py:141-150), fused into
+// head_pooled_kernel: poses_a non-null turns it on.  For pair i it forms the label exactly as so3_log_kernel does and the six
+// squared errors (pred - float(label))^2 in fp32, trans then rot.
+struct LossArgs {
+    const double* poses_a = nullptr;   // (n,16) A_in_cam
+    const double* poses_b = nullptr;   // (n,16) B_in_cam
+    double tn = 0.0, rn = 0.0;         // trans / rot normalizer
+    float* sq = nullptr;               // (n,6) squared errors (required when poses_a is set)
+    double* labels = nullptr;          // (n,6) labels, nullable
+};
+
 cudaError_t launch_preprocess(const PreprocessArgs& a, int n, cudaStream_t s);
 cudaError_t launch_bbox(const double* poses, const double* K4, const double* widths, const double* scale3,
                         int* out, int n, cudaStream_t s);
@@ -39,10 +50,18 @@ cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, i
                         int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth, cudaStream_t s);
 cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s);
 cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int Win, int C, cudaStream_t s);
-// poses_in non-null: also the pose update of every track (K6 fused into K4); zero_words: n_zero 32-bit counters cleared for the next step
+// poses_in non-null: also the pose update of every track (K6 fused into K4); loss.poses_a non-null: also the loss terms of every pair;
+// zero_words: n_zero 32-bit counters cleared for the next step
 cudaError_t launch_head_pooled(const float* part /*[n][kPoolSlices][1024]*/, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                                int n_img, int npix, const int* img_wid, const float* const* fc_table,
-                               const double* poses_in, double* poses_out, float tn, float rn, unsigned* zero_words, int n_zero, cudaStream_t s);
+                               const double* poses_in, double* poses_out, float tn, float rn, const LossArgs& loss,
+                               unsigned* zero_words, int n_zero, cudaStream_t s);
+// sums[0] / sums[1]: the sums of the n x 3 translation / rotation terms of sq (n,6), in the fixed order of reduce_loss_terms
+cudaError_t launch_loss_reduce(const float* sq, int n, float* sums, cudaStream_t s);
+// The loss of n predictions on their own: labels from trans_label / rot_label (n,3) when given, else from loss.poses_a / poses_b;
+// the terms go to loss.sq / loss.labels when those are non-null, and their sums to `sums`, as launch_loss_reduce adds them.
+cudaError_t launch_pair_loss(const float* trans, const float* rot, const double* trans_label, const double* rot_label,
+                             const LossArgs& loss, int n, float* sums, cudaStream_t s);
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                         int n_img, int npix, cudaStream_t s);
 // `in` points at the first image, in the activation format of `precision` (SE3TN_PREC_*)

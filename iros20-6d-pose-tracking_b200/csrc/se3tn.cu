@@ -172,6 +172,7 @@ struct se3tn_ctx {
     DevBuf<MeshDev> d_meshes; int mesh_rows = 0; bool meshes_dirty = false;   // device table of their views, rebuilt when a model changes
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
     DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
+    DevBuf<float> loss_sq; size_t loss_sq_floats = 0;   // se3tn_eval_pairs' loss terms when the caller wants none back: max_batch x 6 (allocated on first use)
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
     // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
     struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
@@ -472,9 +473,10 @@ struct PoseArgs { const double* in = nullptr; double* out = nullptr; float tn = 
 // index) non-null: every image uses its own weight set in the same launches (tensor-core modes);
 // `weight_id` is then only a representative loaded set.  *pose_done tells the caller whether `pose` was applied
 // (the fp32 FFMA mode leaves it to a separate pose_update_kernel launch).
+// `loss` (tensor-core modes only; the fp32 mode leaves it to a stand-alone loss launch): the head also forms the loss terms.
 int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
                 float* out_trans, float* out_rot, float* out_feature, cudaStream_t s, const int* img_wid = nullptr,
-                const PoseArgs* pose = nullptr, bool* pose_done = nullptr) {
+                const PoseArgs* pose = nullptr, bool* pose_done = nullptr, const LossArgs* loss = nullptr) {
     if (pose_done) *pose_done = false;
     auto it = c->weights.find(weight_id);
     if (it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(weight_id) + " not loaded");
@@ -556,7 +558,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         CU_TRY(c, launch_head_pooled(c->pool_part.get() + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
                                      img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc.get() : nullptr,
                                      pose ? pose->in : nullptr, pose ? pose->out : nullptr, pose ? pose->tn : 0.f, pose ? pose->rn : 0.f,
-                                     c->sched.get(), static_cast<int>(trunk_sched_words(c->max_batch)), s));
+                                     loss ? *loss : LossArgs{}, c->sched.get(), static_cast<int>(trunk_sched_words(c->max_batch)), s));
         c->sched_dirty = false;
         if (pose && pose_done) *pose_done = true;
     }
@@ -921,49 +923,29 @@ FillScratch fill_scratch(se3tn_ctx* c, int H, int W) {
 
 uint16_t* filled_frame(se3tn_ctx* c, int H, int W) { return reinterpret_cast<uint16_t*>(c->fill.get() + align256(fill_scratch_bytes(H, W))); }
 
-// One checked step of n tracks (render, if `render` is set: input A is drawn into rgbA / depthA) -> K0 -> conv stack -> K6.
-int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-               const double* K, const double* poses_in, const double* object_width,
-               const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
-               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-               double tn, double rn, int precision,
-               float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
-    const auto& fill = c->depth_fill;
-    if (fill.on) { const int rc = reserve_fill(c, H, W, true, s); if (rc) return rc; }   // before any graph lookup: a new block drops them all
-    // ---- one CUDA graph per distinct step: every argument that ends up inside a kernel parameter is part of the key ----
-    const bool graphable = c->use_graphs && !c->profiling && precision != SE3TN_PREC_FP32;
-    std::vector<unsigned long long> key;
+inline unsigned long long key_bits(double d) { unsigned long long u; memcpy(&u, &d, 8); return u; }
+
+// One step through the context's CUDA graphs.  `key` holds every argument that ends up inside a kernel parameter (empty: the step
+// is not graphable, plain launches).  A step seen before is one graph launch; a new one runs prepare() -- host-side table refreshes,
+// synchronous copies that must not happen inside a capture -- and is captured from launch(stream) on the private capture stream.
+template <class Prepare, class Launch>
+int graph_step(se3tn_ctx* c, std::vector<unsigned long long>& key, Prepare prepare, Launch launch, cudaStream_t s) {
     c->last_was_graph = false;
-    if (graphable) {
-        auto bits = [](double d) { unsigned long long u; memcpy(&u, &d, 8); return u; };
-        const void* ptrs[] = {frame_rgb, frame_depth, poses_in, object_width, rgbA, depthA, weight_ids_dev, out_trans, out_rot, poses_out};
-        for (const void* p : ptrs) key.push_back(reinterpret_cast<unsigned long long>(p));
-        key.push_back(static_cast<unsigned long long>(H)); key.push_back(static_cast<unsigned long long>(W));
-        key.push_back(static_cast<unsigned long long>(n)); key.push_back(static_cast<unsigned long long>(precision));
-        key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
-        for (int i = 0; i < 4; ++i) key.push_back(bits(K[i]));
-        key.push_back(bits(tn)); key.push_back(bits(rn));
-        key.push_back(static_cast<unsigned long long>(render ? render->mode : -1));
-        key.push_back(static_cast<unsigned long long>(render ? render->H : 0)); key.push_back(static_cast<unsigned long long>(render ? render->W : 0));
-        key.push_back(fill.on ? 1ull : 0ull); key.push_back(fill.on ? bits(fill.max_depth) : 0ull);
-        key.push_back(static_cast<unsigned long long>(fill.on ? fill.extrapolate : 0)); key.push_back(static_cast<unsigned long long>(fill.on ? fill.blur_type : 0));
+    if (!key.empty()) {
         for (auto& g : c->graphs)
             if (g.key == key) {
                 CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
                 g.last_use = ++c->graph_clock; c->launches = g.launches; c->last_was_graph = true;
                 return SE3TN_OK;
             }
-        // a new step shape: host-side table refreshes (synchronous copies) must not happen inside the capture
-        int rc0 = sync_stats(c, s); if (rc0) return rc0;
-        if (multi) { rc0 = sync_tables(c, s); if (rc0) return rc0; }
-        if (render) { rc0 = sync_meshes(c, s); if (rc0) return rc0; }
+        const int rc0 = prepare(); if (rc0) return rc0;
         if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
         cudaStream_t cs = nullptr;
         if (!c->cap_stream && cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess) c->cap_stream.reset(cs);
         if (!c->cap_stream) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
         if (!key.empty() && cudaStreamBeginCapture(c->cap_stream.get(), cudaStreamCaptureModeRelaxed) != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
     }
-    const bool capturing = graphable && !key.empty();
+    const bool capturing = !key.empty();
     auto end_capture = [&](int rc_launch) -> int {
         // turn what was recorded into an executable graph and run it; any failure falls back to plain stream launches for good
         cudaGraph_t graph = nullptr;
@@ -985,15 +967,48 @@ int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_dep
         return SE3TN_OK;
     };
     if (capturing) {
-        const int rc = track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
-                                            tn, rn, precision, out_trans, out_rot, poses_out, multi, c->cap_stream.get());
-        const int grc = end_capture(rc);
+        const int grc = end_capture(launch(c->cap_stream.get()));
         if (grc == SE3TN_OK) return SE3TN_OK;
         if (grc != 1) return grc;                              // a real launch error
         // capture was not possible on this stream / driver: plain launches from here on
     }
-    return track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
-                                tn, rn, precision, out_trans, out_rot, poses_out, multi, s);
+    return launch(s);
+}
+
+// One checked step of n tracks (render, if `render` is set: input A is drawn into rgbA / depthA) -> K0 -> conv stack -> K6.
+int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+               const double* K, const double* poses_in, const double* object_width,
+               const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
+               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+               double tn, double rn, int precision,
+               float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
+    const auto& fill = c->depth_fill;
+    if (fill.on) { const int rc = reserve_fill(c, H, W, true, s); if (rc) return rc; }   // before any graph lookup: a new block drops them all
+    // ---- one CUDA graph per distinct step: every argument that ends up inside a kernel parameter is part of the key ----
+    std::vector<unsigned long long> key;
+    if (c->use_graphs && !c->profiling && precision != SE3TN_PREC_FP32) {
+        const void* ptrs[] = {frame_rgb, frame_depth, poses_in, object_width, rgbA, depthA, weight_ids_dev, out_trans, out_rot, poses_out};
+        for (const void* p : ptrs) key.push_back(reinterpret_cast<unsigned long long>(p));
+        key.push_back(static_cast<unsigned long long>(H)); key.push_back(static_cast<unsigned long long>(W));
+        key.push_back(static_cast<unsigned long long>(n)); key.push_back(static_cast<unsigned long long>(precision));
+        key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
+        for (int i = 0; i < 4; ++i) key.push_back(key_bits(K[i]));
+        key.push_back(key_bits(tn)); key.push_back(key_bits(rn));
+        key.push_back(static_cast<unsigned long long>(render ? render->mode : -1));
+        key.push_back(static_cast<unsigned long long>(render ? render->H : 0)); key.push_back(static_cast<unsigned long long>(render ? render->W : 0));
+        key.push_back(fill.on ? 1ull : 0ull); key.push_back(fill.on ? key_bits(fill.max_depth) : 0ull);
+        key.push_back(static_cast<unsigned long long>(fill.on ? fill.extrapolate : 0)); key.push_back(static_cast<unsigned long long>(fill.on ? fill.blur_type : 0));
+    }
+    auto prepare = [&]() -> int {
+        int rc = sync_stats(c, s); if (rc) return rc;
+        if (multi) { rc = sync_tables(c, s); if (rc) return rc; }
+        if (render) { rc = sync_meshes(c, s); if (rc) return rc; }
+        return SE3TN_OK;
+    };
+    return graph_step(c, key, prepare, [&](cudaStream_t ls) {
+        return track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
+                                    tn, rn, precision, out_trans, out_rot, poses_out, multi, ls);
+    }, s);
 }
 
 // the launches of one step, on stream s (being captured or not)
@@ -1050,6 +1065,39 @@ int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t*
     return se3tn_pose_update(c, poses_in, out_trans, out_rot, tn, rn, poses_out, n, stream);
 }
 
+// The launches of one validation step (se3tn_eval_pairs) on stream s: normalize -> conv stack -> head with the loss terms ->
+// their reduction; in SE3TN_PREC_FP32 one FFMA forward per run of equal ids, then one stand-alone loss launch.
+int eval_launches(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                  const double* A_in_cam, const double* B_in_cam, const int32_t* wid_host, const int32_t* wid_dev, int n,
+                  double tn, double rn, int precision, float* out_trans, float* out_rot, float* sq, double* out_labels,
+                  float* out_sums, bool multi, cudaStream_t s) {
+    c->launches = 0;
+    // both depths are offset by A's z (reference datasets.py:136 -> data_augmentation.py:134-144)
+    int rc = se3tn_normalize(c, rgbA, depthA, rgbB, depthB, A_in_cam, wid_dev, n, precision, nullptr, nullptr, s);
+    if (rc) return rc;
+    LossArgs loss; loss.poses_a = A_in_cam; loss.poses_b = B_in_cam; loss.tn = tn; loss.rn = rn; loss.sq = sq; loss.labels = out_labels;
+    if (precision != SE3TN_PREC_FP32) {
+        rc = run_network(c, wid_host ? wid_host[0] : 0, 0, n, precision, out_trans, out_rot, nullptr, s, multi ? wid_dev : nullptr,
+                         nullptr, nullptr, &loss);
+        if (rc) return rc;
+        ProfScope ps(c, 21, s);
+        CU_TRY(c, launch_loss_reduce(sq, n, out_sums, s));
+    } else {
+        for (int first = 0; first < n;) {
+            const int wid = wid_host ? wid_host[first] : 0;
+            int last = first + 1;
+            while (last < n && (wid_host ? wid_host[last] : 0) == wid) ++last;
+            rc = run_network(c, wid, first, last - first, precision, out_trans + first * 3, out_rot + first * 3, nullptr, s);
+            if (rc) return rc;
+            first = last;
+        }
+        ProfScope ps(c, 21, s);
+        CU_TRY(c, launch_pair_loss(out_trans, out_rot, nullptr, nullptr, loss, n, out_sums, s));
+    }
+    ++c->launches;
+    return SE3TN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1094,6 +1142,56 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
     CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
     return track_step(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, c->in_a.get(), reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes), &r,
                       weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, multi, static_cast<cudaStream_t>(stream));
+}
+
+int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                     const double* A_in_cam, const double* B_in_cam,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                     double tn, double rn, int precision,
+                     float* out_trans, float* out_rot, float* out_sq, double* out_labels, float* out_sums, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!rgbA || !depthA || !rgbB || !depthB || !A_in_cam || !B_in_cam) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null input");
+    if (!out_trans || !out_rot || !out_sums) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null output");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
+    bool multi = false;
+    int rc = check_step(c, "se3tn_eval_pairs", weight_ids_host, weight_ids_dev, n, false, &multi);
+    if (rc) return rc;
+    if (n == 0) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: n == 0 (the loss of no pairs is undefined)");
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const bool tensor = precision != SE3TN_PREC_FP32;
+    // allocated once, at max_batch pairs: nothing queued uses it before, and captured steps keep its address after
+    if (tensor && !out_sq) CU_TRY(c, grow(c->loss_sq, c->loss_sq_floats, static_cast<size_t>(c->max_batch) * 6));
+    float* sq = out_sq ? out_sq : (tensor ? c->loss_sq.get() : nullptr);
+    std::vector<unsigned long long> key;
+    if (c->use_graphs && !c->profiling && tensor) {
+        const void* ptrs[] = {rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_dev, out_trans, out_rot, sq, out_labels, out_sums};
+        key.push_back(~0ull);                                  // an evaluation step (no track step key starts with this word)
+        for (const void* p : ptrs) key.push_back(reinterpret_cast<unsigned long long>(p));
+        key.push_back(static_cast<unsigned long long>(n)); key.push_back(static_cast<unsigned long long>(precision));
+        key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
+        key.push_back(key_bits(tn)); key.push_back(key_bits(rn));
+    }
+    auto prepare = [&]() -> int {
+        int rc0 = sync_stats(c, s); if (rc0) return rc0;
+        return multi ? sync_tables(c, s) : SE3TN_OK;
+    };
+    return graph_step(c, key, prepare, [&](cudaStream_t ls) {
+        return eval_launches(c, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_host, weight_ids_dev, n, tn, rn, precision,
+                             out_trans, out_rot, sq, out_labels, out_sums, multi, ls);
+    }, s);
+}
+
+int se3tn_pair_loss(se3tn_ctx* c, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,
+                    float* out_sums, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!trans || !rot || !trans_label || !rot_label || !out_sums || n <= 0) return fail(c, SE3TN_ERR_INVALID, "se3tn_pair_loss: null/invalid argument");
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    c->launches = 0;
+    { ProfScope ps(c, 21, s); CU_TRY(c, launch_pair_loss(trans, rot, trans_label, rot_label, LossArgs{}, n, out_sums, s)); }
+    ++c->launches;
+    return SE3TN_OK;
 }
 
 int se3tn_add_adi(se3tn_ctx* c, const double* model_pts, int m, const double* pred, const double* gt, int n,

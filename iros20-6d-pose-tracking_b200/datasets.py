@@ -1,10 +1,18 @@
-"""Drop-in for the inference half of the reference's datasets.py: TrackDataset.processData and
-.processPredict (reference datasets.py:115-175) with the same signatures and return structure,
-executed by libse3tn kernels (K0 normalisation, K5 so(3) log, K6 pose update).
+"""Drop-in for the reference's datasets.py: TrackDataset's file list, __len__ / __getitem__ (reference datasets.py:50-112),
+processData and processPredict (datasets.py:115-175) with the same signatures and return structure, executed by libse3tn
+kernels (K0 normalisation, K5 so(3) log, K6 pose update, the crop kernel's nearest-neighbour resize).
 
-The training half (__getitem__, file lists, augmentations; datasets.py:50-112) is out of scope;
-pretransforms / augmentations must be None exactly as Tracker passes them (predict.py:191).
+Train-time transforms are out of scope: pretransforms / augmentations must be None, as Tracker passes them (predict.py:191).
+The reference's validation set is built WITH its random augmentations (train.py:132), so its validation loss is a random
+variable; here the loss is that of the clean pairs.
+
+One deliberate difference: the reference derives a pair's other file names by str.replace on the WHOLE path of its rgbA file
+(``path.replace('A', 'B')`` for rgbB, datasets.py:76), which also rewrites every 'A' in the directory names.  Here every
+replacement applies to the file's basename only, so a folder such as /data/A_set/ works.
 """
+import os
+import glob
+import cv2
 import numpy as np
 import torch
 
@@ -34,9 +42,31 @@ class TrackDataset:
         self.precision = precision
         self._engine = engine
         self._stats_set = False
+        self.rgbA_files = sorted(glob.glob(self.root + '/*rgbA.png')) if root else []
 
     def __len__(self):
-        return 0
+        return len(self.rgbA_files)
+
+    def __getitem__(self, index):
+        """-> (data=[dataA, dataB], target=[trans_label, rot_label], A_in_cam, B_in_cam, rgbA, rgbB, maskA, maskB), reference
+        datasets.py:70-112.  Crops that are not `resolution` x `resolution` are resized with cv2.INTER_NEAREST's mapping by the
+        crop kernel on the device.  One pair at a time, as a DataLoader would ask for it; Problem.validate reads the same files
+        and runs whole batches in one step instead."""
+        if torch.utils.data.get_worker_info() is not None:
+            raise RuntimeError('TrackDataset.__getitem__ runs CUDA kernels and cannot be called in a DataLoader worker process '
+                               '(CUDA does not survive fork): use num_workers=0, or Problem.validate / Engine.eval_pairs, which '
+                               'decode the pairs in threads and evaluate whole batches on the device')
+        p = read_pair(self.rgbA_files[index])
+        res = int(self.dataset_info['resolution'])
+        rgbA, depthA, rgbB, depthB, maskB = p['rgbA'], p['depthA'], p['rgbB'], p['depthB'], p['segB']
+        if rgbB.shape[0] != res:
+            rs = [t.cpu().numpy() if t is not None else None for t in resize_pair(self.engine, p, res)]
+            rgbA, depthA, rgbB, depthB, maskB = rs
+        if maskB is None:
+            maskB = (depthB > 100).astype(np.uint8)
+        assert np.sum(maskB) > 0, 'index={}'.format(index)
+        data, target, rgbA, rgbB, maskA, maskB = self.processData(rgbA, depthA, p['A_in_cam'], rgbB, depthB, p['B_in_cam'], maskB)
+        return data, target, p['A_in_cam'], p['B_in_cam'], rgbA, rgbB, maskA, maskB
 
     @property
     def engine(self):
@@ -85,3 +115,69 @@ class TrackDataset:
     @staticmethod
     def _u16(a, dev):
         return torch.from_numpy(np.ascontiguousarray(a).astype(np.uint16)[None]).to(dev)
+
+
+def pair_paths(rgbA_path):
+    """The files of one training pair (reference datasets.py:76-82), named from its rgbA file; the replacements touch the basename
+    only (see the module docstring)."""
+    d, b = os.path.split(rgbA_path)
+    j = lambda name: os.path.join(d, name)
+    return dict(rgbA=rgbA_path, rgbB=j(b.replace('A', 'B')), depthA=j(b.replace('rgbA', 'depthA')), depthB=j(b.replace('rgbA', 'depthB')),
+                segB=j(b.replace('rgbA', 'segB')), meta=j(b.replace('rgbA.png', 'meta.npz')))
+
+
+def read_pair(rgbA_path):
+    """Decode one pair from disk: rgb uint8 (h,w,3) in RGB order (what PIL gives the reference), depth uint16 mm, segB as stored or
+    None when the file is missing, A_in_cam / B_in_cam float64 (4,4) from meta.npz.  Host only (cv2 releases the GIL), so it may
+    run in threads.  The rgb crops must be 8-bit three-channel images, what the reference's data generator writes and what
+    processData takes: an RGBA, grayscale or 16-bit rgb file is an error (PIL would hand the reference an array of another
+    shape or depth, which its pipeline does not handle either)."""
+    f = pair_paths(rgbA_path)
+
+    def rgb(path):
+        im = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+        if im is None:
+            raise FileNotFoundError(path)
+        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+            raise ValueError('%s: rgb crops must be 8-bit three-channel images, got %s %s' % (path, im.dtype, im.shape))
+        return cv2.cvtColor(im, cv2.COLOR_BGR2RGB)
+
+    def raw(path, required=True):
+        if not required and not os.path.exists(path):
+            return None
+        im = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+        if im is None:
+            raise FileNotFoundError(path)
+        return im
+
+    meta = np.load(f['meta'])
+    return dict(rgbA=rgb(f['rgbA']), rgbB=rgb(f['rgbB']), depthA=raw(f['depthA']), depthB=raw(f['depthB']), segB=raw(f['segB'], False),
+                A_in_cam=np.asarray(meta['A_in_cam'], dtype=np.float64), B_in_cam=np.asarray(meta['B_in_cam'], dtype=np.float64))
+
+
+def resize_nearest(engine, rgb, depth, size):
+    """cv2.resize(..., (size, size), interpolation=cv2.INTER_NEAREST) of an rgb uint8 (h,w,3) and a uint16 (h,w) image, on the
+    device: the crop kernel over a window that is the whole image uses the same floor(dst * src / dst_size) source index.
+    Host or CUDA arrays in, CUDA tensors (size,size,3), (size,size) out."""
+    dev = engine.device
+    rgb = torch.as_tensor(np.ascontiguousarray(rgb) if isinstance(rgb, np.ndarray) else rgb).to(dev).contiguous()
+    depth = torch.as_tensor(np.ascontiguousarray(depth) if isinstance(depth, np.ndarray) else depth).to(dev).contiguous()
+    h, w = depth.shape
+    window = torch.tensor([[[0, 0], [h, 0], [0, w], [h, w]]], dtype=torch.int32, device=dev)   # rows (v, u): the whole image
+    r, d = engine.crop_bbox(rgb, depth, window, (size, size))
+    return r[0], d[0]
+
+
+def resize_pair(engine, pair, size):
+    """datasets.py:95-101 on the device: rgbA / depthA, rgbB / depthB and segB (when present) resized to size x size.
+    -> CUDA tensors rgbA, depthA, rgbB, depthB, segB (segB None when the pair has none)."""
+    rgbA, depthA = resize_nearest(engine, pair['rgbA'], pair['depthA'], size)
+    rgbB, depthB = resize_nearest(engine, pair['rgbB'], pair['depthB'], size)
+    segB = None
+    if pair['segB'] is not None:
+        seg = pair['segB']
+        if seg.ndim != 2 or seg.dtype not in (np.uint8, np.uint16):
+            raise ValueError('segB must be a single-channel 8- or 16-bit image')
+        _, s16 = resize_nearest(engine, pair['rgbB'], seg.astype(np.uint16), size)   # the mask rides in the depth plane
+        segB = s16.to(torch.uint8) if seg.dtype == np.uint8 else s16
+    return rgbA, depthA, rgbB, depthB, segB

@@ -43,6 +43,7 @@ class Engine:
         _lib.check(rc, None)
         self._ctx = ctx
         self._weight_ids = set()
+        self._stats = {}                  # weight id -> the (dtype, mean, std) bytes last set on the context
 
     def close(self):
         if getattr(self, '_ctx', None):
@@ -63,14 +64,20 @@ class Engine:
         self._weight_ids.add(int(weight_id))
 
     def set_stats(self, mean, std, weight_id=0):
+        """A weight set's channel statistics.  New values drop the context's captured steps (se3tn_set_stats), so the values a
+        set already has are not set again: a validation pass or a Tracker that restates them keeps every step's CUDA graph."""
         mean = np.ascontiguousarray(mean); std = np.ascontiguousarray(std)
         if mean.shape != (8,) or std.shape != (8,):
             raise ValueError('mean/std must be 8-vectors (A channels then B channels)')
         f64 = (mean.dtype == np.float64) or (std.dtype == np.float64)
         dt = np.float64 if f64 else np.float32
         mean = mean.astype(dt); std = std.astype(dt)
+        key = (bool(f64), mean.tobytes(), std.tobytes())
+        if self._stats.get(int(weight_id)) == key:
+            return
         _lib.check(self.lib.se3tn_set_stats(self._ctx, int(weight_id), mean.ctypes.data_as(C.c_void_p),
                                             std.ctypes.data_as(C.c_void_p), int(f64)), self._ctx)
+        self._stats[int(weight_id)] = key
 
     # ------------------------------------------------------------------ hot path
     def forward(self, A, B, weight_id=0, precision='bf16x3', want_feature=False):
@@ -265,6 +272,60 @@ class Engine:
                                                     vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
         return (out, tr, ro) if want_residuals else out
 
+    # ------------------------------------------------------------------ checkpoint validation
+    def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
+                   weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', want_terms=False, want_labels=False,
+                   out_trans=None, out_rot=None, out_sums=None, out_sq=None, out_labels=None):
+        """The loss of n ready-made pairs in one step (se3tn_eval_pairs): processData's post-transforms, the network in eval mode
+        and Se3TrackNet.loss's terms, enqueued on the current stream.  rgbA / rgbB uint8 (n,176,176,3), depthA / depthB uint16
+        (n,176,176), A_in_cam / B_in_cam float64 (n,4,4), all contiguous CUDA tensors.  -> (trans (n,3), rot (n,3), sums (2,)
+        float32: the summed translation / rotation squared errors, sq (n,6) float32 or None, labels (n,6) float64 or None).
+        MSE = sums / (3 n).  Pass out_* tensors to keep the step's addresses, and so its CUDA graph, across calls."""
+        n = int(A_in_cam.shape[0])
+        for name, t, dt, shape in (('rgbA', rgbA, torch.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('rgbB', rgbB, torch.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)),
+                                   ('depthA', depthA, torch.uint16, (n, IMAGE_SIZE, IMAGE_SIZE)), ('depthB', depthB, torch.uint16, (n, IMAGE_SIZE, IMAGE_SIZE)),
+                                   ('A_in_cam', A_in_cam, torch.float64, (n, 4, 4)), ('B_in_cam', B_in_cam, torch.float64, (n, 4, 4))):
+            self._check_dev(name, t, dt, shape)
+        out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
+        out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
+        out_sums = torch.empty(2, dtype=torch.float32, device=self.device) if out_sums is None else out_sums
+        if out_sq is None and want_terms:
+            out_sq = torch.empty(n, 6, dtype=torch.float32, device=self.device)
+        if out_labels is None and want_labels:
+            out_labels = torch.empty(n, 6, dtype=torch.float64, device=self.device)
+        for name, t, dt, shape in (('out_trans', out_trans, torch.float32, (n, 3)), ('out_rot', out_rot, torch.float32, (n, 3)),
+                                   ('out_sums', out_sums, torch.float32, (2,)), ('out_sq', out_sq, torch.float32, (n, 6)),
+                                   ('out_labels', out_labels, torch.float64, (n, 6))):
+            if t is not None:
+                self._check_dev(name, t, dt, shape)
+        wh = None
+        if weight_ids_host is not None:
+            wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
+            if wh.shape != (n,):
+                raise ValueError('eval_pairs: weight_ids_host must have one entry per pair')
+            if weight_ids_dev is None:
+                weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        _lib.check(self.lib.se3tn_eval_pairs(self._ctx, _ptr(rgbA), _ptr(depthA), _ptr(rgbB), _ptr(depthB), _ptr(A_in_cam), _ptr(B_in_cam),
+                                             wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0), _ptr(weight_ids_dev), n,
+                                             float(trans_normalizer), float(rot_normalizer), PREC[precision],
+                                             _ptr(out_trans), _ptr(out_rot), _ptr(out_sq), _ptr(out_labels), _ptr(out_sums),
+                                             _stream(self.device)), self._ctx)
+        return out_trans, out_rot, out_sums, out_sq, out_labels
+
+    def pair_loss(self, trans, rot, trans_label, rot_label, out_sums=None):
+        """Se3TrackNet.loss's sums on existing predictions (se3tn_pair_loss): float32 (n,3) predictions, float64 (n,3) labels,
+        contiguous CUDA tensors -> float32 (2,) CUDA tensor of the summed translation / rotation squared errors, added exactly as
+        eval_pairs adds them."""
+        n = int(trans.shape[0])
+        for name, t, dt in (('trans', trans, torch.float32), ('rot', rot, torch.float32),
+                            ('trans_label', trans_label, torch.float64), ('rot_label', rot_label, torch.float64)):
+            self._check_dev(name, t, dt, (n, 3))
+        out_sums = torch.empty(2, dtype=torch.float32, device=self.device) if out_sums is None else out_sums
+        self._check_dev('out_sums', out_sums, torch.float32, (2,))
+        _lib.check(self.lib.se3tn_pair_loss(self._ctx, _ptr(trans), _ptr(rot), _ptr(trans_label), _ptr(rot_label), n, _ptr(out_sums),
+                                            _stream(self.device)), self._ctx)
+        return out_sums
+
     def upload_frame_window(self, rgb_host, depth_host, rgb_dev, depth_dev, y0, y1, x0, x1):
         """Copy rows [y0,y1) x columns [x0,x1) of contiguous numpy frames (uint8 (H,W,3), uint16 (H,W); either may be None) into
         full-size device frame buffers: K0 only reads a frame inside the tracks' crop windows."""
@@ -385,8 +446,8 @@ class Engine:
         _lib.check(self.lib.se3tn_set_profiling(self._ctx, int(bool(enable))), self._ctx)
 
     def get_profile(self):
-        """Device ms of each kernel of the last call (21 slots, see include/se3tn.h)."""
-        ms = (C.c_float * 21)()
+        """Device ms of each kernel of the last call (PROFILE_SLOTS slots, see include/se3tn.h)."""
+        ms = (C.c_float * _lib.PROFILE_SLOTS)()
         _lib.check(self.lib.se3tn_get_profile(self._ctx, ms), self._ctx)
         return np.array(ms[:], dtype=np.float64)
 
@@ -408,6 +469,11 @@ class Engine:
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 4 and
                 tuple(t.shape[1:]) == (4, IMAGE_SIZE, IMAGE_SIZE)):
             raise ValueError('expected a contiguous float32 CUDA tensor of shape (n,4,176,176), got %s %s' % (t.dtype, tuple(t.shape)))
+
+    def _check_dev(self, name, t, dtype, shape):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == self.device and t.dtype == dtype and t.is_contiguous()
+                and tuple(t.shape) == tuple(shape)):
+            raise ValueError('%s must be a contiguous %s CUDA tensor of shape %s on %s' % (name, dtype, tuple(shape), self.device))
 
     def _check_frame(self, rgb, depth, rgbA, depthA, poses, ow, n):
         """rgbA / depthA None: input A is rendered by the call, only the frame and the per-track arrays are checked."""

@@ -2,9 +2,9 @@
 cuda / eval / __call__ surface and output dict -- but forward() runs the hand-written sm_90a
 kernels of libse3tn through the C ABI instead of torch.nn -> cuDNN.
 
-Reference: se3_tracknet.py:52-112 (Se3TrackNet), network_modules.py:59-66,86-120.
-Inference only: the training loss (se3_tracknet.py:114-121) and autograd are out of scope, so
-train(True) raises.
+Reference: se3_tracknet.py:52-121 (Se3TrackNet, its loss), network_modules.py:59-66,86-120.
+Inference only: loss() evaluates the training loss without gradients (Problem.validate's use);
+autograd and training are out of scope, so train(True) raises.
 """
 import torch
 from .engine import Engine
@@ -80,3 +80,21 @@ class Se3TrackNet(torch.nn.Module):
         if return_feature:
             out['feature'] = feat
         return out
+
+    # -- se3_tracknet.py:114-121 ------------------------------------------------------------------
+    @torch.no_grad()
+    def loss(self, predictions, targets):
+        """{'trans', 'rot'}: nn.MSELoss of (predictions[k].float(), targets[k].float()) as float32 device scalars, summed by
+        se3tn_pair_loss in the order the validation step uses (Engine.eval_pairs) and divided by the element count."""
+        eng = self.engine
+        trans = predictions[0].to(eng.device, torch.float32).contiguous()
+        rot = predictions[1].to(eng.device, torch.float32).contiguous()
+        # float64 holds any float32 target exactly, and the kernel rounds every label to float32 as .float() does
+        tl = targets[0].to(eng.device, torch.float64).contiguous()
+        rl = targets[1].to(eng.device, torch.float64).contiguous()
+        for name, p, t in (('trans', trans, tl), ('rot', rot, rl)):
+            if p.dim() != 2 or p.shape[1] != 3 or p.shape != t.shape:
+                raise ValueError('loss: %s predictions and targets must both be (n,3), got %s and %s' % (name, tuple(p.shape), tuple(t.shape)))
+        sums = eng.pair_loss(trans, rot, tl, rl)
+        denom = float(3 * trans.shape[0])
+        return {'trans': sums[0] / denom, 'rot': sums[1] / denom}
