@@ -243,8 +243,8 @@ int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, 
  * ROS node does with fill_depth before on_track (predict_ros.py:38-41: max_depth 2.0, extrapolate 0, bilateral).
  * enable = 0 (the default) restores the plain behaviour; the other arguments are then ignored.  The caller's frame_depth is
  * never written.  The fill adds its launches to the step (8 bilateral, 6 gaussian, 3 more with extrapolate; see
- * se3tn_last_launch_count) and its four arguments to the step's graph key; no profiling slot times it.  The host variants
- * upload the whole depth frame instead of the crop-window rectangle, since the fill reads every pixel.  The scratch holds
+ * se3tn_last_launch_count), and its setting is part of what makes two steps the same (se3tn_last_step_was_graph); no
+ * profiling slot times it.  The host variants upload the whole depth frame instead of the crop-window rectangle, since the fill reads every pixel.  The scratch holds
  * 2 x H x W floats plus the filled H x W uint16 frame and grows with the frame; growing it, here or in se3tn_fill_depth[_ex],
  * drops the context's captured steps.  SE3TN_ERR_INVALID for an unknown blur_type or a max_depth that is not finite and > 0
  * (as a float); the setting is then unchanged.  A context is single-threaded: a caller that shares one between trackers
@@ -270,9 +270,8 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
  * rgbA / depthA; render_mode, render_H, render_W as mode, H, W of se3tn_render_ex (ignored in SE3TN_RENDER_VISPY).  Track i
  * draws mesh weight_ids[i] (mesh 0 when the ids are NULL): one network and one CAD model per object, both under one id.
  * Input A lands in context-owned device scratch (max_batch x 176 x 176 x 5 bytes, allocated by the first call).  One step
- * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph under se3tn_track_batch's rules,
- * with the render mode and camera image size part of the key; SE3TN_PREC_FP32 renders and then runs its FFMA forwards
- * without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
+ * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph (se3tn_last_step_was_graph);
+ * SE3TN_PREC_FP32 renders and then runs its FFMA forwards without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
  * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
  * camera image size out of range is SE3TN_ERR_INVALID. */
 int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
@@ -306,7 +305,7 @@ int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint
  *     depends on n alone (thread t of one CTA adds pairs t, t+256, ... in order, then a tree); MSE = sum / (3 n).
  * In the tensor-core modes the loss terms are formed in the head kernel (labels in fp64 by the same device function as
  * se3tn_so3_log) and one more launch adds them: normalize + 8 resident convs + trunk + head + reduction = 12 launches, captured as
- * one CUDA graph under se3tn_track_batch's rules (every pointer, n, precision, the ids' mix and the normalizers are the key).
+ * one CUDA graph (se3tn_last_step_was_graph).
  * SE3TN_PREC_FP32 runs one FFMA forward per contiguous run of equal ids and then one stand-alone loss launch, without a graph:
  * 1 + 17 per run + 1 launches.  Every id is checked on the host before anything is queued: an id without weights or statistics
  * is SE3TN_ERR_STATE (the id is named); n == 0 or n > max_batch is SE3TN_ERR_INVALID.  Without out_sq the terms go to a
@@ -348,9 +347,13 @@ int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
 /* Number of kernels the last forward / track_batch / track_render / eval_pairs / pair_loss call on this context launched (for a
  * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill).
- * se3tn_track_batch, se3tn_track_render and se3tn_eval_pairs capture each distinct step (same pointers, sizes and
- * precision) into a CUDA graph the first time they see it and replay it afterwards -- one graph launch per step;
- * SE3TN_GRAPH=0 in the environment, an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
+ * se3tn_track_batch, se3tn_track_render, their _host variants and se3tn_eval_pairs capture each distinct step into a CUDA
+ * graph the first time they see it and replay it afterwards -- one graph launch per step.  Two calls are the same step when
+ * every value their kernels are given is the same: tracking or validation, n, precision, the frame's H and W, K, the two
+ * normalizers, the first weight id and whether the ids use more than one set, the render mode and camera image size, the
+ * depth-fill setting (se3tn_set_depth_fill), and the address of every device array, in or out.  A replay reads what those
+ * arrays hold at the time, and a call's host ids only decide the first id and the mix.  SE3TN_GRAPH=0 in the environment,
+ * an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
  * se3tn_last_step_was_graph: 1 if the last track_batch / track_render / eval_pairs call was a graph launch. */
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);

@@ -156,6 +156,31 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 std::string g_create_error;
 
+struct F64Bits {   // a double held as its bits: a double member would make StepKey's bytes ambiguous (0.0 == -0.0)
+    uint64_t bits = 0;
+    F64Bits() = default;
+    F64Bits(double d) { memcpy(&bits, &d, sizeof d); }
+    operator double() const { double d; memcpy(&d, &bits, sizeof d); return d; }
+};
+
+// Everything the kernels of one track or validation step are given that can differ from one call to the next.  Its bytes,
+// compared with memcmp, are the key of the step's CUDA graph (run_step), and step_launches takes its arguments from nowhere
+// else: an argument missing here could not be read by the launches, so a replayed graph never runs on stale ones.
+struct StepKey {
+    uint8_t eval, mixed;                       // a validation step (se3tn_eval_pairs); the tracks use more than one weight set
+    uint8_t fill, fill_extrapolate;            // c->depth_fill when a track step is built (zero in a validation step)
+    int32_t fill_blur, n, precision, first_wid;      // first_wid: the first track's weight set
+    int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
+    F64Bits K[4], tn, rn, fill_max_depth;
+    const uint8_t* frame_rgb; const uint16_t* frame_depth; const double* object_width;   // track step
+    const double* poses_in;                    // track step: the previous poses; validation step: A_in_cam
+    const double* B_in_cam; const uint8_t* rgbB; const uint16_t* depthB;                 // validation step
+    const uint8_t* rgbA; const uint16_t* depthA; const int32_t* wid_dev;                  // wid_dev NULL: every track uses set 0
+    float* out_trans; float* out_rot; double* poses_out;                                  // poses_out: track step
+    float* sq; double* labels; float* sums;                                               // validation step
+};
+static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
+
 }  // namespace
 
 struct se3tn_ctx {
@@ -192,10 +217,13 @@ struct se3tn_ctx {
     int table_rows = 0; bool tables_dirty = true;
     int launches = 0;
     bool profiling = false;
-    // CUDA graphs of whole track_batch steps (preprocess -> 8 resident convs -> trunk -> head + pose update), keyed by every baked-in argument
+    // CUDA graphs of whole steps (step_launches), keyed by their StepKey.  Besides the key, a step's launches read only context
+    // state whose every change drops these graphs (or that is fixed for the context's life: workspace, scheduler, activation
+    // tensor maps): the weight sets and their device tables (se3tn_load_weights), the statistics (se3tn_set_stats), the meshes
+    // and rasteriser workspace (se3tn_set_mesh), the depth-fill block (reserve_fill) and the host-IO buffers (track_host_step).
     int use_graphs = 1;              // SE3TN_GRAPH=0: plain stream launches; set to 0 at run time if capture is not possible
     bool last_was_graph = false;
-    struct StepGraph { std::vector<unsigned long long> key; Handle<cudaGraphExec_t> exec; int launches; unsigned long long last_use; };
+    struct StepGraph { StepKey key; Handle<cudaGraphExec_t> exec; int launches; unsigned long long last_use; };
     std::vector<StepGraph> graphs; unsigned long long graph_clock = 0;
     Handle<cudaStream_t> cap_stream;   // steps are captured on this private stream (the caller's may be the legacy default stream, which cannot be captured) and replayed on the caller's
     Handle<cudaEvent_t> ev[2][SE3TN_PROFILE_SLOTS];   // start, end of each profiling slot
@@ -466,18 +494,16 @@ int sync_meshes(se3tn_ctx* c, cudaStream_t s) {
     return SE3TN_OK;
 }
 
-// optional pose update fused into the head kernel (tensor-core modes): K6 for the same n tracks
-struct PoseArgs { const double* in = nullptr; double* out = nullptr; float tn = 0.f, rn = 0.f; };
+// What the head kernel does besides trans / rot, in the tensor-core modes: the pose update (K6) of the same n tracks and / or
+// the loss terms of a validation step.  The fp32 FFMA mode's head does neither; its caller launches them on their own.
+struct HeadArgs { const double* pose_in = nullptr; double* pose_out = nullptr; float tn = 0.f, rn = 0.f; LossArgs loss; };
 
 // The conv stack on images [first, first+n) of the context buffers.  img_wid (device, indexed by absolute image
-// index) non-null: every image uses its own weight set in the same launches (tensor-core modes);
-// `weight_id` is then only a representative loaded set.  *pose_done tells the caller whether `pose` was applied
-// (the fp32 FFMA mode leaves it to a separate pose_update_kernel launch).
-// `loss` (tensor-core modes only; the fp32 mode leaves it to a stand-alone loss launch): the head also forms the loss terms.
+// index) non-null: every image uses its own weight set in the same launches (tensor-core modes; the caller has run
+// sync_tables); `weight_id` is then only a representative loaded set.
 int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
                 float* out_trans, float* out_rot, float* out_feature, cudaStream_t s, const int* img_wid = nullptr,
-                const PoseArgs* pose = nullptr, bool* pose_done = nullptr, const LossArgs* loss = nullptr) {
-    if (pose_done) *pose_done = false;
+                const HeadArgs& head = HeadArgs()) {
     auto it = c->weights.find(weight_id);
     if (it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(weight_id) + " not loaded");
     const DeviceWeights& w = *it->second.dev;
@@ -505,7 +531,6 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         return SE3TN_OK;
     }
     // ---- tensor-core modes: 8 resident-weight launches + 1 trunk launch + head ----
-    if (img_wid) { int rc = sync_tables(c, s); if (rc) return rc; }
     const CUtensorMap* gbmaps = img_wid ? c->d_bmaps[precision].get() : nullptr;
     const float* const* gbias = img_wid ? c->d_bias.get() : nullptr;
     if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
@@ -557,14 +582,38 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         ProfScope ps(c, 16, s);
         CU_TRY(c, launch_head_pooled(c->pool_part.get() + static_cast<size_t>(first) * kPoolSlices * 1024, fcw, fcw + 6 * 512, out_trans, out_rot, n, 121,
                                      img_wid ? img_wid + first : nullptr, img_wid ? c->d_fc.get() : nullptr,
-                                     pose ? pose->in : nullptr, pose ? pose->out : nullptr, pose ? pose->tn : 0.f, pose ? pose->rn : 0.f,
-                                     loss ? *loss : LossArgs{}, c->sched.get(), static_cast<int>(trunk_sched_words(c->max_batch)), s));
+                                     head.pose_in, head.pose_out, head.tn, head.rn, head.loss,
+                                     c->sched.get(), static_cast<int>(trunk_sched_words(c->max_batch)), s));
         c->sched_dirty = false;
-        if (pose && pose_done) *pose_done = true;
     }
     ++c->launches;
     if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(reinterpret_cast<const uint8_t*>(c->buf[B_F2]) + static_cast<size_t>(first) * 22 * 22 * 256 * prec_bytes_per_channel(precision), out_feature, n, 22 * 22, 256,
                                                        precision, s)); ++c->launches; }
+    return SE3TN_OK;
+}
+
+// Launches shared by the public entry points and step_launches.  They check and sync nothing: their callers have checked the
+// arguments and brought the statistics / meshes up to date, outside any capture.
+// K0: preprocess (a frame and input A) or normalize (ready-made crops), with the context's statistics, into the stem buffers
+int queue_preprocess(se3tn_ctx* c, PreprocessArgs a, int n, cudaStream_t s) {
+    a.mean32 = c->d_mean32.get(); a.std32 = c->d_std32.get(); a.mean64 = c->d_mean64.get(); a.std64 = c->d_std64.get();
+    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows;
+    a.stemA = c->buf[B_X0A]; a.stemB = c->buf[B_X0B];
+    { ProfScope ps(c, 17, s); CU_TRY(c, launch_preprocess(a, n, s)); }
+    ++c->launches;
+    return SE3TN_OK;
+}
+
+int queue_render(se3tn_ctx* c, const double* K, const double* poses, const double* object_width, const int32_t* mesh_ids, int n,
+                 int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA, cudaStream_t s) {
+    RenderArgs a;
+    a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
+    a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
+    a.rgb = rgbA; a.depth = depthA;
+    a.mode = mode == SE3TN_RENDER_PYRENDER ? 1 : 0; a.vw = W; a.vh = H;
+    a.projected = c->render_proj.get(); a.uniforms = c->render_unif.get(); a.max_nv = c->render_max_nv;
+    { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s)); }
+    c->launches += 2;
     return SE3TN_OK;
 }
 
@@ -755,17 +804,12 @@ int se3tn_preprocess(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     int rc = sync_stats(c, s); if (rc) return rc;
-    PreprocessArgs a;
+    PreprocessArgs a{};
     a.frame_rgb = frame_rgb; a.frame_depth = frame_depth; a.H = H; a.W = W;
     a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
     a.poses = poses; a.object_width = object_width; a.rgbA = rgbA; a.depthA = depthA; a.weight_ids = weight_ids;
-    a.mean32 = c->d_mean32.get(); a.std32 = c->d_std32.get(); a.mean64 = c->d_mean64.get(); a.std64 = c->d_std64.get();
-    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.precision = precision; a.b_precropped = 0;
-    a.stemA = c->buf[B_X0A]; a.stemB = c->buf[B_X0B]; a.nchwA = out_A; a.nchwB = out_B;
-    a.crop_rgb = crop_rgb; a.crop_depth = crop_depth;
-    { ProfScope ps(c, 17, s); CU_TRY(c, launch_preprocess(a, n, s)); }
-    ++c->launches;
-    return SE3TN_OK;
+    a.precision = precision; a.nchwA = out_A; a.nchwB = out_B; a.crop_rgb = crop_rgb; a.crop_depth = crop_depth;
+    return queue_preprocess(c, a, n, s);
 }
 
 int se3tn_normalize(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
@@ -777,16 +821,11 @@ int se3tn_normalize(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, c
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     int rc = sync_stats(c, s); if (rc) return rc;
-    PreprocessArgs a;
-    memset(&a, 0, sizeof a);
+    PreprocessArgs a{};
     a.frame_rgb = rgbB; a.frame_depth = depthB; a.H = kImg; a.W = kImg; a.b_precropped = 1;
     a.poses = poses; a.rgbA = rgbA; a.depthA = depthA; a.weight_ids = weight_ids;
-    a.mean32 = c->d_mean32.get(); a.std32 = c->d_std32.get(); a.mean64 = c->d_mean64.get(); a.std64 = c->d_std64.get();
-    a.stats_f64 = c->stats_f64; a.stats_rows = c->stats_rows; a.precision = precision;
-    a.stemA = c->buf[B_X0A]; a.stemB = c->buf[B_X0B]; a.nchwA = out_A; a.nchwB = out_B;
-    { ProfScope ps(c, 17, s); CU_TRY(c, launch_preprocess(a, n, s)); }
-    ++c->launches;
-    return SE3TN_OK;
+    a.precision = precision; a.nchwA = out_A; a.nchwB = out_B;
+    return queue_preprocess(c, a, n, s);
 }
 
 int se3tn_compute_bbox(se3tn_ctx* c, const double* poses, const double* K, const double* widths, const double* scale,
@@ -891,13 +930,6 @@ int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int3
     return SE3TN_OK;
 }
 
-int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                         const double* K, const double* poses_in, const double* object_width,
-                         const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
-                         const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                         double tn, double rn, int precision,
-                         float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s);
-
 // The depth-fill block for an H x W frame: scratch a | b | lut | minmax, then, when a track step fills the frame, the filled
 // uint16 frame.  Captured steps hold the block's addresses, so they are dropped, once the stream has drained, before the block
 // is replaced; grow installs the new block only once it exists.
@@ -923,116 +955,71 @@ FillScratch fill_scratch(se3tn_ctx* c, int H, int W) {
 
 uint16_t* filled_frame(se3tn_ctx* c, int H, int W) { return reinterpret_cast<uint16_t*>(c->fill.get() + align256(fill_scratch_bytes(H, W))); }
 
-inline unsigned long long key_bits(double d) { unsigned long long u; memcpy(&u, &d, 8); return u; }
+// A step as run_step takes it: the key, and the ids on the host.  Only host code reads those: check_step, first_wid / mixed,
+// and the fp32 mode's runs of equal ids, which are never captured.
+struct Step : StepKey { const int32_t* wid_host; };
 
-// One step through the context's CUDA graphs.  `key` holds every argument that ends up inside a kernel parameter (empty: the step
-// is not graphable, plain launches).  A step seen before is one graph launch; a new one runs prepare() -- host-side table refreshes,
-// synchronous copies that must not happen inside a capture -- and is captured from launch(stream) on the private capture stream.
-template <class Prepare, class Launch>
-int graph_step(se3tn_ctx* c, std::vector<unsigned long long>& key, Prepare prepare, Launch launch, cudaStream_t s) {
-    c->last_was_graph = false;
-    if (!key.empty()) {
-        for (auto& g : c->graphs)
-            if (g.key == key) {
-                CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
-                g.last_use = ++c->graph_clock; c->launches = g.launches; c->last_was_graph = true;
-                return SE3TN_OK;
-            }
-        const int rc0 = prepare(); if (rc0) return rc0;
-        if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
-        cudaStream_t cs = nullptr;
-        if (!c->cap_stream && cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess) c->cap_stream.reset(cs);
-        if (!c->cap_stream) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
-        if (!key.empty() && cudaStreamBeginCapture(c->cap_stream.get(), cudaStreamCaptureModeRelaxed) != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; key.clear(); }
-    }
-    const bool capturing = !key.empty();
-    auto end_capture = [&](int rc_launch) -> int {
-        // turn what was recorded into an executable graph and run it; any failure falls back to plain stream launches for good
-        cudaGraph_t graph = nullptr;
-        cudaError_t e = cudaStreamEndCapture(c->cap_stream.get(), &graph);
-        if (rc_launch != SE3TN_OK || e != cudaSuccess || !graph) {
-            if (graph) cudaGraphDestroy(graph);
-            cudaGetLastError(); c->use_graphs = 0; c->sched_dirty = true;
-            return rc_launch != SE3TN_OK ? rc_launch : 1;      // 1: capture failed, caller relaunches directly
-        }
-        cudaGraphExec_t exec = nullptr;
-        e = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (e != cudaSuccess) { cudaGetLastError(); c->use_graphs = 0; return 1; }
-        if (c->graphs.size() >= 64)                            // evict the least recently used step
-            c->graphs.erase(std::min_element(c->graphs.begin(), c->graphs.end(), [](const auto& a, const auto& b) { return a.last_use < b.last_use; }));
-        c->graphs.push_back({key, Handle<cudaGraphExec_t>(exec), c->launches, ++c->graph_clock});
-        CU_TRY(c, cudaGraphLaunch(exec, s));
-        c->last_was_graph = true;
-        return SE3TN_OK;
-    };
-    if (capturing) {
-        const int grc = end_capture(launch(c->cap_stream.get()));
-        if (grc == SE3TN_OK) return SE3TN_OK;
-        if (grc != 1) return grc;                              // a real launch error
-        // capture was not possible on this stream / driver: plain launches from here on
-    }
-    return launch(s);
+// What every track step takes from its scalar arguments, its ids (checked by check_step: `mixed`) and the context's depth-fill
+// setting; the caller adds the device pointers.
+Step track_step(const se3tn_ctx* c, int H, int W, const double* K, const int32_t* wid_host, bool mixed, int n,
+                double tn, double rn, int precision) {
+    Step st{};
+    st.n = n; st.precision = precision; st.H = H; st.W = W;
+    for (int i = 0; i < 4; ++i) st.K[i] = K[i];
+    st.tn = tn; st.rn = rn;
+    st.wid_host = wid_host; st.first_wid = wid_host ? wid_host[0] : 0; st.mixed = mixed;
+    st.render_mode = -1;
+    const auto& f = c->depth_fill;                 // all zero when the fill is off (se3tn_set_depth_fill)
+    st.fill = f.on; st.fill_max_depth = f.max_depth; st.fill_extrapolate = f.extrapolate != 0; st.fill_blur = f.blur_type;
+    return st;
 }
 
-// One checked step of n tracks (render, if `render` is set: input A is drawn into rgbA / depthA) -> K0 -> conv stack -> K6.
-int track_step(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-               const double* K, const double* poses_in, const double* object_width,
-               const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
-               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-               double tn, double rn, int precision,
-               float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
-    const auto& fill = c->depth_fill;
-    if (fill.on) { const int rc = reserve_fill(c, H, W, true, s); if (rc) return rc; }   // before any graph lookup: a new block drops them all
-    // ---- one CUDA graph per distinct step: every argument that ends up inside a kernel parameter is part of the key ----
-    std::vector<unsigned long long> key;
-    if (c->use_graphs && !c->profiling && precision != SE3TN_PREC_FP32) {
-        const void* ptrs[] = {frame_rgb, frame_depth, poses_in, object_width, rgbA, depthA, weight_ids_dev, out_trans, out_rot, poses_out};
-        for (const void* p : ptrs) key.push_back(reinterpret_cast<unsigned long long>(p));
-        key.push_back(static_cast<unsigned long long>(H)); key.push_back(static_cast<unsigned long long>(W));
-        key.push_back(static_cast<unsigned long long>(n)); key.push_back(static_cast<unsigned long long>(precision));
-        key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
-        for (int i = 0; i < 4; ++i) key.push_back(key_bits(K[i]));
-        key.push_back(key_bits(tn)); key.push_back(key_bits(rn));
-        key.push_back(static_cast<unsigned long long>(render ? render->mode : -1));
-        key.push_back(static_cast<unsigned long long>(render ? render->H : 0)); key.push_back(static_cast<unsigned long long>(render ? render->W : 0));
-        key.push_back(fill.on ? 1ull : 0ull); key.push_back(fill.on ? key_bits(fill.max_depth) : 0ull);
-        key.push_back(static_cast<unsigned long long>(fill.on ? fill.extrapolate : 0)); key.push_back(static_cast<unsigned long long>(fill.on ? fill.blur_type : 0));
-    }
-    auto prepare = [&]() -> int {
-        int rc = sync_stats(c, s); if (rc) return rc;
-        if (multi) { rc = sync_tables(c, s); if (rc) return rc; }
-        if (render) { rc = sync_meshes(c, s); if (rc) return rc; }
-        return SE3TN_OK;
-    };
-    return graph_step(c, key, prepare, [&](cudaStream_t ls) {
-        return track_batch_launches(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, render, weight_ids_host, weight_ids_dev, n,
-                                    tn, rn, precision, out_trans, out_rot, poses_out, multi, ls);
-    }, s);
+// A track step that draws input A first.  It lands in context scratch for max_batch tracks, allocated by the first such step:
+// its address never changes after, so captured steps stay valid.
+int render_into_scratch(se3tn_ctx* c, const RenderSpec& r, Step& st) {
+    const size_t img = static_cast<size_t>(kImg) * kImg, rgb_bytes = align256(static_cast<size_t>(c->max_batch) * img * 3);
+    CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
+    st.render_mode = r.mode; st.render_H = r.H; st.render_W = r.W;
+    st.rgbA = c->in_a.get(); st.depthA = reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes);
+    return SE3TN_OK;
 }
 
-// the launches of one step, on stream s (being captured or not)
-int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                         const double* K, const double* poses_in, const double* object_width,
-                         const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
-                         const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                         double tn, double rn, int precision,
-                         float* out_trans, float* out_rot, double* poses_out, bool multi, cudaStream_t s) {
-    void* stream = s;
+// The conv stack over a step's n tracks.  Tensor-core modes: one forward in which every track picks its own weight set when the
+// ids are mixed, its head doing `head` too.  fp32: one FFMA forward per run of equal ids, `head` left to the caller.
+int run_tracks(se3tn_ctx* c, const Step& st, const HeadArgs& head, cudaStream_t s) {
+    if (st.precision != SE3TN_PREC_FP32)
+        return run_network(c, st.first_wid, 0, st.n, st.precision, st.out_trans, st.out_rot, nullptr, s, st.mixed ? st.wid_dev : nullptr, head);
+    for (int first = 0; first < st.n;) {
+        const int wid = st.wid_host ? st.wid_host[first] : 0;
+        int last = first + 1;
+        while (last < st.n && (st.wid_host ? st.wid_host[last] : 0) == wid) ++last;
+        const int rc = run_network(c, wid, first, last - first, st.precision, st.out_trans + first * 3, st.out_rot + first * 3, nullptr, s);
+        if (rc) return rc;
+        first = last;
+    }
+    return SE3TN_OK;
+}
+
+// The launches of one step on stream s, captured or not: render (if set) -> fill (if on) -> preprocess (track) or normalize
+// (validation) -> conv stack -> the fp32 pose update (track) or the loss (validation: pair_loss in fp32, the reduction of the
+// head's terms otherwise).  Arguments come from `st` alone, context state only as the graph cache's comment in se3tn_ctx lists.
+int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     c->launches = 0;
+    const double K[4] = {st.K[0], st.K[1], st.K[2], st.K[3]};
+    const bool fp32 = st.precision == SE3TN_PREC_FP32;
     int rc;
-    if (render) {                                  // track i draws mesh weight_ids[i] (0 without ids): one network and one model per object
-        rc = se3tn_render_ex(c, K, poses_in, object_width, weight_ids_dev, n, render->mode, render->H, render->W,
-                             const_cast<uint8_t*>(rgbA), const_cast<uint16_t*>(depthA), stream);
+    if (st.render_mode >= 0) {                     // track i draws mesh weight_ids[i] (0 without ids): one network and one model per object
+        rc = queue_render(c, K, st.poses_in, st.object_width, st.wid_dev, st.n, st.render_mode, st.render_H, st.render_W,
+                          const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s);
         if (rc) return rc;
     }
-    const uint16_t* depth = frame_depth;
-    if (c->depth_fill.on) {                        // fill_depth(frame_depth) into the block track_step sized; the caller's frame is only read
-        const auto& f = c->depth_fill;
-        uint16_t* filled = filled_frame(c, H, W);
-        CU_TRY(c, launch_fill_depth(frame_depth, H, W, static_cast<float>(f.max_depth), f.extrapolate != 0, f.blur_type == SE3TN_BLUR_GAUSSIAN,
-                                    fill_scratch(c, H, W), filled, nullptr, s));
-        c->launches += fill_depth_launches(f.extrapolate != 0, f.blur_type == SE3TN_BLUR_GAUSSIAN);
+    const uint16_t* depth = st.frame_depth;
+    if (st.fill) {                                 // fill_depth(frame_depth) into the block run_step sized; the caller's frame is only read
+        const bool gaussian = st.fill_blur == SE3TN_BLUR_GAUSSIAN;
+        uint16_t* filled = filled_frame(c, st.H, st.W);
+        CU_TRY(c, launch_fill_depth(st.frame_depth, st.H, st.W, static_cast<float>(st.fill_max_depth), st.fill_extrapolate != 0, gaussian,
+                                    fill_scratch(c, st.H, st.W), filled, nullptr, s));
+        c->launches += fill_depth_launches(st.fill_extrapolate != 0, gaussian);
         depth = filled;
     }
     // preprocess_kernel is launched with programmatic stream serialization, so it may start while the launch in front of it
@@ -1040,62 +1027,81 @@ int track_batch_launches(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t*
     // reads rgbA / depthA and the frame only after griddepcontrol.wait (aux_kernels.cu, grid_dep_wait()), which returns once
     // that launch has completed and its writes are visible: keep every read of input A and of the frame behind that wait.
     // The fill kernels themselves are plain launches, so the first one starts after the render has completed.
-    rc = se3tn_preprocess(c, frame_rgb, depth, H, W, K, poses_in, object_width, rgbA, depthA, weight_ids_dev, n,
-                          precision, nullptr, nullptr, nullptr, nullptr, stream);
-    if (rc) return rc;
-    PoseArgs pose; pose.in = poses_in; pose.out = poses_out; pose.tn = static_cast<float>(tn); pose.rn = static_cast<float>(rn);
-    bool pose_done = false;
-    if (precision != SE3TN_PREC_FP32) {
-        // every track picks its own weight set inside the same launches; K6 runs inside the head kernel
-        rc = run_network(c, weight_ids_host ? weight_ids_host[0] : 0, 0, n, precision, out_trans, out_rot, nullptr, s,
-                         multi ? weight_ids_dev : nullptr, &pose, &pose_done);
-        if (rc) return rc;
-    } else {
-        int first = 0;
-        while (first < n) {
-            const int wid = weight_ids_host ? weight_ids_host[first] : 0;
-            int last = first + 1;
-            while (last < n && (weight_ids_host ? weight_ids_host[last] : 0) == wid) ++last;
-            rc = run_network(c, wid, first, last - first, precision, out_trans + first * 3, out_rot + first * 3, nullptr, s);
-            if (rc) return rc;
-            first = last;
-        }
+    PreprocessArgs a{};
+    a.poses = st.poses_in; a.rgbA = st.rgbA; a.depthA = st.depthA; a.weight_ids = st.wid_dev; a.precision = st.precision;
+    HeadArgs head;
+    if (!st.eval) {
+        a.frame_rgb = st.frame_rgb; a.frame_depth = depth; a.H = st.H; a.W = st.W; a.object_width = st.object_width;
+        a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
+        head.pose_in = st.poses_in; head.pose_out = st.poses_out;
+        head.tn = static_cast<float>(st.tn); head.rn = static_cast<float>(st.rn);
+    } else {                                       // both depths are offset by A's z (reference datasets.py:136 -> data_augmentation.py:134-144)
+        a.frame_rgb = st.rgbB; a.frame_depth = st.depthB; a.H = kImg; a.W = kImg; a.b_precropped = 1;
+        head.loss.poses_a = st.poses_in; head.loss.poses_b = st.B_in_cam; head.loss.tn = st.tn; head.loss.rn = st.rn;
+        head.loss.sq = st.sq; head.loss.labels = st.labels;
     }
-    if (pose_done) return SE3TN_OK;
-    return se3tn_pose_update(c, poses_in, out_trans, out_rot, tn, rn, poses_out, n, stream);
-}
-
-// The launches of one validation step (se3tn_eval_pairs) on stream s: normalize -> conv stack -> head with the loss terms ->
-// their reduction; in SE3TN_PREC_FP32 one FFMA forward per run of equal ids, then one stand-alone loss launch.
-int eval_launches(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
-                  const double* A_in_cam, const double* B_in_cam, const int32_t* wid_host, const int32_t* wid_dev, int n,
-                  double tn, double rn, int precision, float* out_trans, float* out_rot, float* sq, double* out_labels,
-                  float* out_sums, bool multi, cudaStream_t s) {
-    c->launches = 0;
-    // both depths are offset by A's z (reference datasets.py:136 -> data_augmentation.py:134-144)
-    int rc = se3tn_normalize(c, rgbA, depthA, rgbB, depthB, A_in_cam, wid_dev, n, precision, nullptr, nullptr, s);
-    if (rc) return rc;
-    LossArgs loss; loss.poses_a = A_in_cam; loss.poses_b = B_in_cam; loss.tn = tn; loss.rn = rn; loss.sq = sq; loss.labels = out_labels;
-    if (precision != SE3TN_PREC_FP32) {
-        rc = run_network(c, wid_host ? wid_host[0] : 0, 0, n, precision, out_trans, out_rot, nullptr, s, multi ? wid_dev : nullptr,
-                         nullptr, nullptr, &loss);
-        if (rc) return rc;
-        ProfScope ps(c, 21, s);
-        CU_TRY(c, launch_loss_reduce(sq, n, out_sums, s));
+    if ((rc = queue_preprocess(c, a, st.n, s))) return rc;
+    if ((rc = run_tracks(c, st, head, s))) return rc;
+    if (!st.eval) {
+        if (!fp32) return SE3TN_OK;                // the head kernel has updated the poses
+        ProfScope ps(c, 18, s);
+        CU_TRY(c, launch_pose_update(st.poses_in, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
     } else {
-        for (int first = 0; first < n;) {
-            const int wid = wid_host ? wid_host[first] : 0;
-            int last = first + 1;
-            while (last < n && (wid_host ? wid_host[last] : 0) == wid) ++last;
-            rc = run_network(c, wid, first, last - first, precision, out_trans + first * 3, out_rot + first * 3, nullptr, s);
-            if (rc) return rc;
-            first = last;
-        }
         ProfScope ps(c, 21, s);
-        CU_TRY(c, launch_pair_loss(out_trans, out_rot, nullptr, nullptr, loss, n, out_sums, s));
+        if (fp32) CU_TRY(c, launch_pair_loss(st.out_trans, st.out_rot, nullptr, nullptr, head.loss, st.n, st.sums, s));
+        else CU_TRY(c, launch_loss_reduce(st.sq, st.n, st.sums, s));
     }
     ++c->launches;
     return SE3TN_OK;
+}
+
+// One step through the context's CUDA graphs (not with SE3TN_GRAPH=0, profiling or SE3TN_PREC_FP32): a step whose key was seen
+// before is one graph launch; a new one is captured from step_launches on the private capture stream, then launched.  Otherwise,
+// or when capture turns out not to be possible (plain launches from then on), step_launches runs on s.
+int run_step(se3tn_ctx* c, const Step& st, cudaStream_t s) {
+    int rc;
+    if (st.fill && (rc = reserve_fill(c, st.H, st.W, true, s))) return rc;   // before the lookup: a new block drops every graph
+    c->last_was_graph = false;
+    const StepKey& key = st;
+    bool capture = c->use_graphs && !c->profiling && st.precision != SE3TN_PREC_FP32;
+    if (capture)
+        for (auto& g : c->graphs)
+            if (memcmp(&g.key, &key, sizeof key) == 0) {
+                CU_TRY(c, cudaGraphLaunch(g.exec.get(), s));
+                g.last_use = ++c->graph_clock; c->launches = g.launches; c->last_was_graph = true;
+                return SE3TN_OK;
+            }
+    // host-side refreshes: synchronous copies, which must not happen inside a capture
+    if ((rc = sync_stats(c, s))) return rc;
+    if (st.mixed && (rc = sync_tables(c, s))) return rc;
+    if (st.render_mode >= 0 && (rc = sync_meshes(c, s))) return rc;
+    if (capture) {
+        if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
+        cudaStream_t cs = nullptr;
+        if (!c->cap_stream && cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess) c->cap_stream.reset(cs);
+        capture = c->cap_stream && cudaStreamBeginCapture(c->cap_stream.get(), cudaStreamCaptureModeRelaxed) == cudaSuccess;
+        if (!capture) { cudaGetLastError(); c->use_graphs = 0; }
+    }
+    if (capture) {
+        // turn what was recorded into an executable graph and run it; any failure falls back to plain stream launches for good
+        rc = step_launches(c, st, c->cap_stream.get());
+        cudaGraph_t graph = nullptr;
+        cudaGraphExec_t exec = nullptr;
+        const bool ok = cudaStreamEndCapture(c->cap_stream.get(), &graph) == cudaSuccess && rc == SE3TN_OK && graph &&
+                        cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
+        if (graph) cudaGraphDestroy(graph);
+        if (ok) {
+            if (c->graphs.size() >= 64)                        // evict the least recently used step
+                c->graphs.erase(std::min_element(c->graphs.begin(), c->graphs.end(), [](const auto& a, const auto& b) { return a.last_use < b.last_use; }));
+            c->graphs.push_back({key, Handle<cudaGraphExec_t>(exec), c->launches, ++c->graph_clock});
+            CU_TRY(c, cudaGraphLaunch(exec, s));
+            c->last_was_graph = true;
+            return SE3TN_OK;
+        }
+        cudaGetLastError(); c->use_graphs = 0; c->sched_dirty = true;
+        if (rc) return rc;                                     // a real launch error
+    }
+    return step_launches(c, st, s);
 }
 
 }  // namespace
@@ -1114,9 +1120,15 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
     const int rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || !rgbA || !depthA || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null argument or empty frame");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
     DeviceGuard guard(c->device);
-    return track_step(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, rgbA, depthA, nullptr, weight_ids_host, weight_ids_dev, n,
-                      tn, rn, precision, out_trans, out_rot, poses_out, multi, static_cast<cudaStream_t>(stream));
+    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.rgbA = rgbA; st.depthA = depthA; st.wid_dev = weight_ids_dev;
+    st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
@@ -1136,12 +1148,13 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
     rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
     DeviceGuard guard(c->device);
-    // input A for max_batch tracks, allocated once: its address never changes, so captured steps stay valid
-    const size_t img = static_cast<size_t>(kImg) * kImg, rgb_bytes = align256(static_cast<size_t>(c->max_batch) * img * 3);
-    CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
-    return track_step(c, frame_rgb, frame_depth, H, W, K, poses_in, object_width, c->in_a.get(), reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes), &r,
-                      weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, multi, static_cast<cudaStream_t>(stream));
+    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
@@ -1158,28 +1171,16 @@ int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, 
     if (rc) return rc;
     if (n == 0) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: n == 0 (the loss of no pairs is undefined)");
     DeviceGuard guard(c->device);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bool tensor = precision != SE3TN_PREC_FP32;
     // allocated once, at max_batch pairs: nothing queued uses it before, and captured steps keep its address after
     if (tensor && !out_sq) CU_TRY(c, grow(c->loss_sq, c->loss_sq_floats, static_cast<size_t>(c->max_batch) * 6));
-    float* sq = out_sq ? out_sq : (tensor ? c->loss_sq.get() : nullptr);
-    std::vector<unsigned long long> key;
-    if (c->use_graphs && !c->profiling && tensor) {
-        const void* ptrs[] = {rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_dev, out_trans, out_rot, sq, out_labels, out_sums};
-        key.push_back(~0ull);                                  // an evaluation step (no track step key starts with this word)
-        for (const void* p : ptrs) key.push_back(reinterpret_cast<unsigned long long>(p));
-        key.push_back(static_cast<unsigned long long>(n)); key.push_back(static_cast<unsigned long long>(precision));
-        key.push_back(multi ? 1ull : 0ull); key.push_back(static_cast<unsigned long long>(weight_ids_host ? weight_ids_host[0] : 0));
-        key.push_back(key_bits(tn)); key.push_back(key_bits(rn));
-    }
-    auto prepare = [&]() -> int {
-        int rc0 = sync_stats(c, s); if (rc0) return rc0;
-        return multi ? sync_tables(c, s) : SE3TN_OK;
-    };
-    return graph_step(c, key, prepare, [&](cudaStream_t ls) {
-        return eval_launches(c, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_host, weight_ids_dev, n, tn, rn, precision,
-                             out_trans, out_rot, sq, out_labels, out_sums, multi, ls);
-    }, s);
+    Step st{};
+    st.eval = 1; st.n = n; st.precision = precision; st.tn = tn; st.rn = rn; st.render_mode = -1;
+    st.wid_host = weight_ids_host; st.first_wid = weight_ids_host ? weight_ids_host[0] : 0; st.mixed = multi;
+    st.rgbA = rgbA; st.depthA = depthA; st.rgbB = rgbB; st.depthB = depthB; st.poses_in = A_in_cam; st.B_in_cam = B_in_cam;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot;
+    st.sq = out_sq ? out_sq : (tensor ? c->loss_sq.get() : nullptr); st.labels = out_labels; st.sums = out_sums;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_pair_loss(se3tn_ctx* c, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,
@@ -1249,11 +1250,11 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
-    // the step checks the ids again; checking them here as well means an error stages and copies nothing
     bool multi = false;
-    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi);
+    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi);   // before anything is staged or copied
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
     DeviceGuard guard(c->device);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     auto& io = c->hio;
@@ -1332,11 +1333,12 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (weight_ids) memcpy(hp + o_wid, weight_ids, nn * 4);
     CU_TRY(c, cudaMemcpyAsync(d_in, hp, weight_ids ? in_bytes : o_wid, cudaMemcpyHostToDevice, s));
     hp += in_bytes;
-    rc = render ? se3tn_track_render(c, d_rgb, d_depth, H, W, K, d_poses, d_ow, render->mode, render->H, render->W, weight_ids, weight_ids ? d_wid : nullptr, n,
-                                     tn, rn, precision, d_tr, d_ro, d_out, stream)
-                : se3tn_track_batch(c, d_rgb, d_depth, H, W, K, d_poses, d_ow, d_rgbA, d_depthA, weight_ids, weight_ids ? d_wid : nullptr, n,
-                                    tn, rn, precision, d_tr, d_ro, d_out, stream);
-    if (rc != SE3TN_OK) return rc;
+    Step st = track_step(c, H, W, K, weight_ids, multi, n, tn, rn, precision);
+    st.frame_rgb = d_rgb; st.frame_depth = d_depth; st.poses_in = d_poses; st.object_width = d_ow;
+    st.rgbA = d_rgbA; st.depthA = d_depthA; st.wid_dev = weight_ids ? d_wid : nullptr;
+    st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
+    if (render && (rc = render_into_scratch(c, *render, st))) return rc;
+    if ((rc = run_step(c, st, s))) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
     CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
@@ -1464,15 +1466,7 @@ int se3tn_render_ex(se3tn_ctx* c, const double* K, const double* poses, const do
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     const int rc = sync_meshes(c, s); if (rc) return rc;
-    RenderArgs a;
-    a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
-    a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
-    a.rgb = rgbA; a.depth = depthA;
-    a.mode = mode == SE3TN_RENDER_PYRENDER ? 1 : 0; a.vw = W; a.vh = H;
-    a.projected = c->render_proj.get(); a.uniforms = c->render_unif.get(); a.max_nv = c->render_max_nv;
-    { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s)); }
-    c->launches += 2;
-    return SE3TN_OK;
+    return queue_render(c, K, poses, object_width, mesh_ids, n, mode, H, W, rgbA, depthA, s);
 }
 
 int se3tn_debug_buffer(se3tn_ctx* c, int id, float** ptr, size_t* floats_per_image) {
