@@ -341,8 +341,12 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 /* Device-side timeline of the conv kernels (contexts created with SE3TN_TRACE=1 in the environment): synchronises the
  * device and copies 14 x 256 x 8 uint64 to the HOST: for conv launch l and CTA b, 8 %globaltimer (ns) stamps of the LAST
  * forward -- 0 entry, 1 setup done, 2 first weights in shared memory, 3 first activation unit, 4 last MMA committed,
- * 5 first accumulator ready, 6 last epilogue done, 7 exit (low 8 bits replaced by the SM id).  Profiling tool only. */
-#define SE3TN_TRACE_WORDS (14 * 256 * 8)
+ * 5 first accumulator ready, 6 last epilogue done, 7 exit (low 8 bits replaced by the SM id); launch 8 (the trunk) is followed by
+ * its per-unit stamps in 9-13.  Then, for the 8 resident-weight launches, SE3TN_TRACE_TILES x 4 per-tile stamps each (enough
+ * for the stems at 64 images) -- 0 first activation unit, 1 last MMA completed, 2 accumulator handed to the epilogue, 3 epilogue
+ * done (low 8 bits replaced by the CTA index); tiles that did not run read 0.  Profiling tool only. */
+#define SE3TN_TRACE_TILES 5184
+#define SE3TN_TRACE_WORDS (14 * 256 * 8 + 8 * SE3TN_TRACE_TILES * 4)
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
 /* Number of kernels the last forward / track_batch / track_render / eval_pairs / pair_loss call on this context launched (for a

@@ -10,6 +10,7 @@ PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16 = 0, 1, 2, 3
 RENDER_VISPY, RENDER_PYRENDER = 0, 1
 WEIGHT_BLOB_FLOATS = 13528326
 PROFILE_SLOTS = 22
+TRACE_TILES = 5184
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 

@@ -121,6 +121,7 @@ struct ResidentParams {
     const CUtensorMap* gbmaps;
     const float* const* gbias;
     unsigned long long* trace;
+    unsigned long long* tile_trace;    // SE3TN_TRACE: this launch's [SE3TN_TRACE_TILES][4] per-tile stamps (include/se3tn.h)
 };
 
 cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, int num_sms, bool pdl, cudaStream_t stream);

@@ -3,8 +3,9 @@
 //
 // Common to both kernels
 //   * M tile = an 11x11 pixel box of one image (121 of 128 rows; 44, 22 and 11 are multiples of 11), as two wgmma M = 64
-//     halves.  In the resident kernel each consumer warpgroup owns one half of every tile; in the trunk one warpgroup owns
-//     both halves of a work unit.  Accumulators stay in registers.
+//     halves.  Ping-pong (both kernels): one consumer warpgroup owns both halves of a tile / work unit, the two warpgroups take
+//     alternate ones.  The resident kernel keeps the halves schedule (each consumer warpgroup one half of every tile) for
+//     launches where no CTA has a second tile.  Accumulators stay in registers.
 //   * A operand by TMA "units": one cp.async.bulk.tensor.4d per (128-byte channel chunk, filter COLUMN) whose box is
 //     two rows taller than the tile.  It lands as 143 rows x 128 B in the SWIZZLE_128B K-major layout wgmma reads, and
 //     the three vertical taps of that column are the SAME tile read through descriptors whose start address is advanced
@@ -23,7 +24,7 @@
 //   * per-object weights (reference README.md:132: one checkpoint per object class): with img_wid every work unit takes
 //     its weight tensor map and bias from per-set device tables, so all tracks of a frame share the launches.
 //
-// conv_resident_kernel<KIND, PREC>  (Cout = 64: stems, 64-channel 3x3 convs)
+// conv_resident_kernel<KIND, PREC, PP>  (Cout = 64: stems, 64-channel 3x3 convs)
 //   * the whole K-major weight matrix (<= 147 KB) is TMA-loaded into shared memory once per CTA (again only when the
 //     weight-set id changes between consecutive tiles of the CTA's contiguous range), one mbarrier per filter-column
 //     unit so the first MMAs start when the first third has landed.
@@ -36,7 +37,18 @@
 //     16-byte pieces, no staging.
 //   * stem: fused MaxPool2d(3,2,1): the M tile is the 11x11 block of conv outputs that feeds a 5x5 block of pooled
 //     outputs; max -> +bias -> SELU (monotone, so they commute) on 1/4.84 of the values; the 88x88x64 conv output never
-//     reaches HBM.
+//     reaches HBM.  The fp32 sums are staged in shared memory for the 3x3 max.
+//   * ping-pong (launches with more tiles than SMs): consumer warpgroup g owns the tiles it % 2 == g of the CTA's range and
+//     issues each MMA step once per 64-row half into acc[2][kAcc], in the same K order as the halves schedule: bit-identical.
+//     A named-barrier pair passes the MMA turn as in the trunk; the warpgroup that does not own a tile steps its A ring
+//     position past the tile's chunks x NU stages (a_empty: one arrival).  Both warpgroups track the weight generation, and
+//     at a weight-set switch each arrives on b_empty once its own MMAs on the old weights have retired.  The stem's epilogue
+//     runs on the owning 128 threads (warpgroup-local named barriers); in bf16 / bf16x3 its one staging buffer (a second
+//     does not fit next to the resident weights) is handed between the warpgroups by a second named-barrier pair, in tf32
+//     warpgroup g keeps buffer g.  The stem's bias is loaded before the MMAs.
+//   * registers: the whole-tile accumulator is 128 registers (bf16x3, the stems' stacked bf16) or 64; setmaxnreg moves them
+//     from the producer warpgroup (168 at launch -> 40) to the consumers (-> 232), as in the trunk.  In the 64-channel bf16x3
+//     layers the second half's residual loads wait until the first half's epilogue has freed its accumulator registers.
 //
 // conv_trunk_kernel<PREC>  (Cout >= 256: convAB1, convAB2.{conv1,conv2}, {trans,rot}_conv1, {trans,rot}_conv2.{conv1,conv2})
 //   * ONE launch for all six layers.  A work unit = (layer, image, 11x11 tile, 128 output channels).  A persistent CTA per
@@ -123,6 +135,12 @@ __device__ __forceinline__ void trace_exit(unsigned long long* tr) {
     unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
     tr[blockIdx.x * 8 + 7] = (gtimer() & ~0xffull) | (smid & 0xff);
 }
+// per-tile timeline of a resident launch (SE3TN_TRACE, tiles < SE3TN_TRACE_TILES): 4 stamps per tile, written by the first thread
+// of the warpgroup that owns the tile (of warpgroup 0 in the halves schedule): 0 first A unit landed (after the MMA turn came),
+// 1 last MMA completed, 2 accumulator handed to the epilogue, 3 that thread finished its epilogue (low 8 bits: CTA index)
+__device__ __forceinline__ void tile_stamp(unsigned long long* tt, int tile, int k) {
+    if (tt && tile < SE3TN_TRACE_TILES) tt[tile * 4 + k] = k == 3 ? (gtimer() & ~0xffull) | (blockIdx.x & 0xff) : gtimer();
+}
 
 using ptx::desc_lo;
 using ptx::mk_desc;
@@ -138,8 +156,24 @@ struct Consumer {
         ct = static_cast<int>(threadIdx.x) - 128; cg = ct >> 7; ew = ct >> 5; cw = ew & 3; lane = ct & 31; R = lane >> 2; m = lane & 3;
     }
     __device__ __forceinline__ bool leader() const { return (ct & 127) == 0; }   // arrives on the operand-release barriers
-    __device__ __forceinline__ int row(int h) const { return 64 * cg + 16 * cw + R + 8 * h; }
+    __device__ __forceinline__ int row(int half, int h) const { return 64 * half + 16 * cw + R + 8 * h; }   // in 64-row half `half`
 };
+
+// registers per thread after setmaxnreg: the producer warpgroup gives up what the consumers' 128 accumulators need
+// (launch: 168 x 384 threads; after: 40 x 128 + 232 x 256 = the same 64,512)
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+// named barriers (0 is __syncthreads): ping-pong MMA turn, the resident stem's staging-buffer hand-over, warpgroup-local epilogue
+constexpr int kTurnBar = 1;                    // kTurnBar + g: consumer warpgroup g may issue its tile's / unit's MMAs
+constexpr int kStageBar = 3;                   // kStageBar + g: consumer warpgroup g may write the stem's single staging buffer
+constexpr int kEpiBar = 5;                     // kEpiBar + g: the 128 threads of warpgroup g (halves schedule: kEpiBar, all 256)
+
+// move a ring position (stage, phase) on by n stages
+__device__ __forceinline__ void ring_skip(int& stage, uint32_t& phase, int n, int stages) {
+    stage += n;
+    phase ^= static_cast<uint32_t>(stage / stages) & 1u;
+    stage %= stages;
+}
 
 // ================================================================================================================
 // conv_resident_kernel
@@ -197,13 +231,17 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
     }
 }
 
-template <int KIND, int PREC>
+// PP: ping-pong schedule (consumer warpgroup g owns the CTA's tiles it % 2 == g, both 64-row halves); otherwise the halves
+// schedule (each consumer warpgroup owns one half of every tile), for launches where no CTA has a second tile to overlap with.
+template <int KIND, int PREC, bool PP>
 __global__ void __launch_bounds__(kThreads2, 1)
 conv_resident_kernel(const __grid_constant__ ResidentParams p)
 {
     using C = RCfg<KIND, PREC>;
     using KT = KTab<KIND>;
     constexpr bool POOL = C::POOL;
+    constexpr int NH = PP ? 2 : 1;                                      // 64-row halves of a tile one consumer warpgroup computes
+    constexpr bool kShareStage = PP && C::kPoolBufs == 1;               // both warpgroups' stem epilogues use the one staging buffer
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const LayerDesc& L = p.L;
@@ -215,9 +253,10 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
     uint8_t* sP = sB + C::kMaxWTiles * C::kBTile;                       // pool staging (stem only)
     uint64_t* bars = reinterpret_cast<uint64_t*>(sP + C::kPoolBufs * kPoolStageAlloc);
     uint64_t* a_full = bars;                       // [kAStages]
-    uint64_t* a_empty = a_full + C::kAStages;      // [kAStages]: one arrival per consumer warpgroup
+    uint64_t* a_empty = a_full + C::kAStages;      // [kAStages]: one arrival per consumer warpgroup that reads the stage
     uint64_t* b_full = a_empty + C::kAStages;      // [NU]: weights of filter-column unit u have landed
-    uint64_t* b_empty = b_full + KT::NU;           // [1]: MMAs that read the current weights have retired (multi-set reload)
+    uint64_t* b_empty = b_full + KT::NU;           // [1]: MMAs that read the current weights have retired (multi-set reload):
+                                                   // one arrival per consumer warpgroup at each weight switch
 
     ptx::grid_dep_launch();
     if (threadIdx.x == 0) trace_stamp(p.trace, 0);
@@ -231,7 +270,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
     auto wid_of = [&](int tile) -> int { return p.img_wid ? p.img_wid[img_of(tile)] : -1; };   // -1: single-set launch
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < C::kAStages; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], 2); }
+        for (int s = 0; s < C::kAStages; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], PP ? 1 : 2); }
         for (int u = 0; u < KT::NU; ++u) ptx::mbar_init(&b_full[u], 1);
         ptx::mbar_init(&b_empty[0], 2);
         ptx::fence_barrier_init();
@@ -240,90 +279,132 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
     __syncthreads();
     if (threadIdx.x == 0) trace_stamp(p.trace, 1);
 
-    if (warp == 0) {
-        // ============================== A producer ================================
-        if (lane == 0) {
-            ptx::grid_dep_wait();                   // activations come from the previous kernel
-            int stage = 0; uint32_t phase = 0;
-            for (int tile = w_begin; tile < w_end; ++tile) {
-                const int n0 = img_of(tile), r = tile % tiles_img;
-                const int ty = r / L.tiles_x, tx = r - ty * L.tiles_x;
-                const int ox = tx * p.step_x + p.off_x, oy = ty * p.step_y + p.off_y;
-                for (int ch = 0; ch < chunks; ++ch) {
+    if (warp < 4) {
+        ptx::setmaxnreg_dec<kProducerRegs>();       // the whole producer warpgroup, idle warps 2-3 included
+        if (warp == 0) {
+            // ============================== A producer ================================
+            if (lane == 0) {
+                ptx::grid_dep_wait();                   // activations come from the previous kernel
+                int stage = 0; uint32_t phase = 0;
+                for (int tile = w_begin; tile < w_end; ++tile) {
+                    const int n0 = img_of(tile), r = tile % tiles_img;
+                    const int ty = r / L.tiles_x, tx = r - ty * L.tiles_x;
+                    const int ox = tx * p.step_x + p.off_x, oy = ty * p.step_y + p.off_y;
+                    for (int ch = 0; ch < chunks; ++ch) {
 #pragma unroll
-                    for (int u = 0; u < KT::NU; ++u) {
-                        ptx::mbar_wait(&a_empty[stage], phase ^ 1);
-                        ptx::mbar_arrive_expect_tx(&a_full[stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
-                        ptx::tma_load_4d(sA + stage * C::kAUnit, &L.amap[KT::amap(u)], &a_full[stage],
-                                         ch * 32, ox + KT::c1(u), oy + KT::c2(u), n0);
-                        if (++stage == C::kAStages) { stage = 0; phase ^= 1; }
+                        for (int u = 0; u < KT::NU; ++u) {
+                            ptx::mbar_wait(&a_empty[stage], phase ^ 1);
+                            ptx::mbar_arrive_expect_tx(&a_full[stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
+                            ptx::tma_load_4d(sA + stage * C::kAUnit, &L.amap[KT::amap(u)], &a_full[stage],
+                                             ch * 32, ox + KT::c1(u), oy + KT::c2(u), n0);
+                            if (++stage == C::kAStages) { stage = 0; phase ^= 1; }
+                        }
                     }
                 }
             }
-        }
-    } else if (warp == 1) {
-        // ============================== weight loader ================================
-        if (lane == 0) {
-            int cur = -2; uint32_t gen = 0;
-            for (int tile = w_begin; tile < w_end; ++tile) {
-                const int wid = wid_of(tile);
-                if (wid == cur) continue;
-                if (gen) ptx::mbar_wait(&b_empty[0], (gen - 1) & 1);       // MMAs that read the previous weights have retired
-                const CUtensorMap* bm = wid < 0 ? &L.bmap : p.gbmaps + wid * kLayersPerSet + L.li;
+        } else if (warp == 1) {
+            // ============================== weight loader ================================
+            if (lane == 0) {
+                int cur = -2; uint32_t gen = 0;
+                for (int tile = w_begin; tile < w_end; ++tile) {
+                    const int wid = wid_of(tile);
+                    if (wid == cur) continue;
+                    if (gen) ptx::mbar_wait(&b_empty[0], (gen - 1) & 1);       // MMAs that read the previous weights have retired
+                    const CUtensorMap* bm = wid < 0 ? &L.bmap : p.gbmaps + wid * kLayersPerSet + L.li;
 #pragma unroll
-                for (int u = 0; u < KT::NU; ++u) {                          // in the order the MMAs need them: unit by unit
-                    ptx::mbar_arrive_expect_tx(&b_full[u], static_cast<uint32_t>(KT::ntaps(u) * tiles_per_tap) * C::kBTile);
+                    for (int u = 0; u < KT::NU; ++u) {                          // in the order the MMAs need them: unit by unit
+                        ptx::mbar_arrive_expect_tx(&b_full[u], static_cast<uint32_t>(KT::ntaps(u) * tiles_per_tap) * C::kBTile);
 #pragma unroll
-                    for (int k = 0; k < KT::ntaps(u); ++k)
-                        for (int c = 0; c < tiles_per_tap; ++c) {
-                            const int wt = KT::wtap(u, k) * tiles_per_tap + c;   // tile wt covers K words [wt*32, wt*32 + 32)
-                            ptx::tma_load_2d(sB + wt * C::kBTile, bm, &b_full[u], wt * 32, 0);
-                        }
+                        for (int k = 0; k < KT::ntaps(u); ++k)
+                            for (int c = 0; c < tiles_per_tap; ++c) {
+                                const int wt = KT::wtap(u, k) * tiles_per_tap + c;   // tile wt covers K words [wt*32, wt*32 + 32)
+                                ptx::tma_load_2d(sB + wt * C::kBTile, bm, &b_full[u], wt * 32, 0);
+                            }
+                    }
+                    cur = wid; ++gen;
                 }
-                cur = wid; ++gen;
             }
         }
-    } else if (warp >= 4) {
+    } else {
         // ============================== MMA + epilogue (two warpgroups) ==========================
+        ptx::setmaxnreg_inc<kConsumerRegs>();
         ptx::grid_dep_wait();                       // residual reads / output writes must follow the previous kernel
+        using S = Storage<PREC>;
         const Consumer cs;
         const bool stamp = threadIdx.x == 128;
+        const bool tstamp = cs.leader() && (PP || cs.cg == 0);     // per-tile stamps (tile_stamp)
+        constexpr int kEpiThreads = PP ? 128 : 256;                 // threads that run one tile's epilogue
+        const int et = PP ? (cs.ct & 127) : cs.ct;                  // this thread's index among them
+        auto half_of = [&](int hf) { return PP ? hf : cs.cg; };     // 64-row half of the tile in accumulator acc[hf]
         int astage = 0; uint32_t aphase = 0;
         int w_cur = -2; uint32_t w_gen = 0;        // weight set currently in shared memory
+        if constexpr (PP) {
+            // the first MMA turn (and the stem's staging buffer) is warpgroup 0's
+            if (cs.cg == 1) { ptx::bar_arrive(kTurnBar, 256); if constexpr (kShareStage) ptx::bar_arrive(kStageBar, 256); }
+        }
         int it = 0;
         for (int tile = w_begin; tile < w_end; ++tile, ++it) {
             const int wid = wid_of(tile);
             const bool new_w = (wid != w_cur);     // wait for each unit's weights at its first use below
+            const bool w_last = tile + 1 < w_end && wid_of(tile + 1) != wid;   // the loader replaces these weights after this tile
+            if (PP && (it & 1) != cs.cg) {
+                // the other warpgroup's tile: step this warpgroup's A ring position past its stages.  Keep the weight generation
+                // in step, and take part in the hand-back of the weights as below: this warpgroup's MMAs on them retired with its
+                // previous tile.  Waiting for a new generation first keeps this warpgroup's arrival for the next switch after
+                // the loader has seen both arrivals for this one.
+                ring_skip(astage, aphase, chunks * KT::NU, C::kAStages);
+                if (new_w) {
+#pragma unroll
+                    for (int u = 0; u < KT::NU; ++u) ptx::mbar_wait(&b_full[u], w_gen & 1);
+                    w_cur = wid; ++w_gen;
+                }
+                if (w_last && cs.leader()) ptx::mbar_arrive(&b_empty[0]);
+                continue;
+            }
             const int n0 = img_of(tile), r = tile % tiles_img;
             const int ty = r / L.tiles_x, tx = r - ty * L.tiles_x;
 
             // 64-channel layers: this thread's pixels and their residual pieces are known before the accumulator is: issue the
-            // residual loads now so their latency hides behind the MMAs.  Piece (h, b): row cs.row(h), channels 32b + 8m .. + 7.
-            using S = Storage<PREC>;
-            size_t rpix[2]; bool rvalid[2]; Raw<PREC, 8> rres[2][2];
-            if constexpr (!POOL) {
+            // residual loads now so their latency hides behind the MMAs.  Piece (hf, h, b): row cs.row(half_of(hf), h),
+            // channels 32b + 8m .. + 7.  Ping-pong with the 128-register bf16x3 accumulator: only the first half's pieces here,
+            // the second half's once the first half's accumulator registers are free (0 spills; their latency then overlaps
+            // the first half's epilogue and the other warpgroup's MMAs).
+            constexpr int kPreRes = (PP && C::kStack == 2) ? 1 : NH;
+            size_t rpix[NH][2]; bool rvalid[NH][2]; Raw<PREC, 8> rres[NH][2][2];
+            auto load_res = [&](int hf) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    const int rw = cs.row(h);
+                    const int rw = cs.row(half_of(hf), h);
                     const int py = rw / 11, px = rw - py * 11;
                     const int y = ty * 11 + py, x = tx * 11 + px;
-                    rvalid[h] = (rw < 121) && (y < L.Ho) && (x < L.Wo);
-                    rpix[h] = (static_cast<size_t>(n0) * L.Ho + y) * L.Wo + x;
+                    rvalid[hf][h] = (rw < 121) && (y < L.Ho) && (x < L.Wo);
+                    rpix[hf][h] = (static_cast<size_t>(n0) * L.Ho + y) * L.Wo + x;
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        rres[h][b] = Raw<PREC, 8>{};
-                        if (L.res && rvalid[h]) {
-                            const uint8_t* rp = L.res + S::addr(rpix[h], L.res_c, 32 * b + 8 * cs.m);
+                        rres[hf][h][b] = Raw<PREC, 8>{};
+                        if (L.res && rvalid[hf][h]) {
+                            const uint8_t* rp = L.res + S::addr(rpix[hf][h], L.res_c, 32 * b + 8 * cs.m);
 #pragma unroll
-                            for (int q = 0; q < rres[h][b].kPieces; ++q) rres[h][b].set(q, __ldg(rres[h][b].at(rp, q)));
+                            for (int q = 0; q < Raw<PREC, 8>::kPieces; ++q) rres[hf][h][b].set(q, __ldg(Raw<PREC, 8>::at(rp, q)));
                         }
                     }
                 }
-            }
-
-            float acc[C::kAcc];
+            };
+            if constexpr (!POOL) {
 #pragma unroll
-            for (int i = 0; i < C::kAcc; ++i) acc[i] = 0.f;
+                for (int hf = 0; hf < kPreRes; ++hf) load_res(hf);
+            }
+            // stem: every pooled vector this thread finishes has channels c4 = (et % 16) * 4 (the thread stride is a multiple
+            // of 16): its bias is loaded under the MMAs too
+            float4 pb4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if constexpr (POOL) pb4 = __ldg(reinterpret_cast<const float4*>((p.img_wid ? p.gbias[p.img_wid[n0] * kLayersPerSet + L.li] : L.bias) + (et & 15) * 4));
+
+            float acc[NH][C::kAcc];
+#pragma unroll
+            for (int hf = 0; hf < NH; ++hf)
+#pragma unroll
+                for (int i = 0; i < C::kAcc; ++i) acc[hf][i] = 0.f;
+            if constexpr (PP) ptx::bar_sync(kTurnBar + cs.cg, 256);    // the other warpgroup has issued all MMAs of its previous tile
             uint32_t fresh = 0;                     // 0 until the first MMA of this tile has been issued
             int pend = -1;                          // A stage of the previous MMA group, released once that group has completed
             for (int ch = 0; ch < chunks; ++ch) {
@@ -334,9 +415,19 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                         if (it == 0 && u == 0 && stamp) trace_stamp(p.trace, 2);
                     }
                     ptx::mbar_wait(&a_full[astage], aphase);
-                    if (it == 0 && ch == 0 && u == 0 && stamp) trace_stamp(p.trace, 3);
+                    if (ch == 0 && u == 0) {
+                        if (it == 0 && stamp) trace_stamp(p.trace, 3);
+                        if (tstamp) tile_stamp(p.tile_trace, tile, 0);
+                    }
                     ptx::wgmma_fence();
-                    resident_mma_unit<KIND, PREC>(acc, desc_lo(sA + astage * C::kAUnit + cs.cg * kWgRowBytes), sB, u, ch, tiles_per_tap, fresh);
+                    // each MMA step once per 64-row half, every half's accumulator in the same K order
+                    const uint32_t a_unit_lo = desc_lo(sA + astage * C::kAUnit);
+#pragma unroll
+                    for (int hf = 0; hf < NH; ++hf) {
+                        uint32_t f = fresh;
+                        resident_mma_unit<KIND, PREC>(acc[hf], a_unit_lo + half_of(hf) * (kWgRowBytes >> 4), sB, u, ch, tiles_per_tap, f);
+                    }
+                    fresh = 1u;
                     ptx::wgmma_commit();
                     ptx::wgmma_wait<1>();
                     if (pend >= 0 && cs.leader()) ptx::mbar_arrive(&a_empty[pend]);
@@ -344,74 +435,88 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                     if (++astage == C::kAStages) { astage = 0; aphase ^= 1; }
                 }
             }
+            if constexpr (PP) ptx::bar_arrive(kTurnBar + (cs.cg ^ 1), 256);   // all of this tile's MMAs are issued: the other's turn
             ptx::wgmma_wait<0>();
-            ptx::wgmma_reg_fence(acc);
+#pragma unroll
+            for (int hf = 0; hf < NH; ++hf) ptx::wgmma_reg_fence(acc[hf]);
+            if (tstamp) tile_stamp(p.tile_trace, tile, 1);
             if (cs.leader()) {
                 ptx::mbar_arrive(&a_empty[pend]);
                 // the next tile uses other weights -> tell the loader that these MMAs have retired
-                if (tile + 1 < w_end && wid_of(tile + 1) != wid) ptx::mbar_arrive(&b_empty[0]);
+                if (w_last) ptx::mbar_arrive(&b_empty[0]);
             }
             if (new_w) { w_cur = wid; ++w_gen; }
             if (it == 0 && stamp) trace_stamp(p.trace, 5);
+            if (tstamp) tile_stamp(p.tile_trace, tile, 2);
 
             if constexpr (!POOL) {
                 // ---------------- 64-channel layers ----------------
-                // Fragment register 16b + 4jj + 2h + e = row cs.row(h), column 32b + 8jj + 2m + e, which carries channel 32b + 8m + 2jj + e
-                // (permuted weight rows): the thread owns 8 CONSECUTIVE channels of each of its pixels per 32-column block.
+                // Fragment register 16b + 4jj + 2h + e = row cs.row(half, h), column 32b + 8jj + 2m + e, which carries channel
+                // 32b + 8m + 2jj + e (permuted weight rows): the thread owns 8 CONSECUTIVE channels of each of its pixels per
+                // 32-column block.
 #pragma unroll
-                for (int b = 0; b < 2; ++b) {
-                    const int ch0 = 32 * b + 8 * cs.m;
-                    const float* bias_base = (p.img_wid ? p.gbias[p.img_wid[n0] * kLayersPerSet + L.li] : L.bias) + ch0;
-                    const float4 bA = __ldg(reinterpret_cast<const float4*>(bias_base)), bB = __ldg(reinterpret_cast<const float4*>(bias_base + 4));
-                    const float bias8[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
+                for (int hf = 0; hf < NH; ++hf) {
+                    if (hf >= kPreRes) load_res(hf);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (!rvalid[h]) continue;
-                        float v[8];
+                    for (int b = 0; b < 2; ++b) {
+                        const int ch0 = 32 * b + 8 * cs.m;
+                        const float* bias_base = (p.img_wid ? p.gbias[p.img_wid[n0] * kLayersPerSet + L.li] : L.bias) + ch0;
+                        const float4 bA = __ldg(reinterpret_cast<const float4*>(bias_base)), bB = __ldg(reinterpret_cast<const float4*>(bias_base + 4));
+                        const float bias8[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
 #pragma unroll
-                        for (int jj = 0; jj < 4; ++jj)
+                        for (int h = 0; h < 2; ++h) {
+                            if (!rvalid[hf][h]) continue;
+                            float v[8];
 #pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int ri = 16 * b + 4 * jj + 2 * h + e;
-                                float a = acc[ri];
-                                if constexpr (C::kStack == 2) a += acc[32 + ri];
-                                v[2 * jj + e] = a + bias8[2 * jj + e];
+                            for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const int ri = 16 * b + 4 * jj + 2 * h + e;
+                                    float a = acc[hf][ri];
+                                    if constexpr (C::kStack == 2) a += acc[hf][32 + ri];
+                                    v[2 * jj + e] = a + bias8[2 * jj + e];
+                                }
+                            if (L.res) {
+                                float r[8];
+                                S::decode(rres[hf][h][b], r);
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) v[e] += r[e];
                             }
-                        if (L.res) {
-                            float r[8];
-                            S::decode(rres[h][b], r);
 #pragma unroll
-                            for (int e = 0; e < 8; ++e) v[e] += r[e];
+                            for (int e = 0; e < 8; ++e) v[e] = act_apply(v[e], L.act);
+                            S::encode(v).store(L.out + S::addr(rpix[hf][h], L.out_c, L.out_coff + ch0));
                         }
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) v[e] = act_apply(v[e], L.act);
-                        S::encode(v).store(L.out + S::addr(rpix[h], L.out_c, L.out_coff + ch0));
                     }
                 }
             } else {
                 // ---- stem: conv tile 11x11 -> 5x5 max-pooled outputs (MaxPool2d(3,2,1), -inf padding) ----
+                // Ping-pong: with one staging buffer the two warpgroups' epilogues take turns on it (kStageBar); with two, tile
+                // it % 2 == g always uses buffer g, and this warpgroup's readers of two tiles ago must be done before it writes.
                 float* stage = reinterpret_cast<float*>(sP + (C::kPoolBufs == 2 ? (it & 1) : 0) * kPoolStageAlloc);
+                if constexpr (kShareStage) ptx::bar_sync(kStageBar + cs.cg, 256);
+                else if constexpr (PP) ptx::bar_sync(kEpiBar + cs.cg, 128);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int rw = cs.row(h);
-                    if (rw >= 121) continue;
-                    const int cy_l = rw / 11, cx_l = rw - cy_l * 11;            // conv position inside the tile
-                    const int cy = ty * p.step_y + p.off_y + cy_l, cx = tx * p.step_x + p.off_x + cx_l;   // conv output coordinates
-                    const bool cvalid = cy >= 0 && cy < 88 && cx >= 0 && cx < 88;
-                    float* srow = stage + rw * kPoolPitch + 2 * cs.m;
-                    const float ninf = -3.0e38f;
+                for (int hf = 0; hf < NH; ++hf)
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {                               // columns 8j + 2m + {0, 1}
-                        float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
-                        if constexpr (C::kStack == 2) { a0 += acc[32 + 4 * j + 2 * h]; a1 += acc[32 + 4 * j + 2 * h + 1]; }
-                        *reinterpret_cast<float2*>(srow + 8 * j) = cvalid ? make_float2(a0, a1) : make_float2(ninf, ninf);
+                    for (int h = 0; h < 2; ++h) {
+                        const int rw = cs.row(half_of(hf), h);
+                        if (rw >= 121) continue;
+                        const int cy_l = rw / 11, cx_l = rw - cy_l * 11;            // conv position inside the tile
+                        const int cy = ty * p.step_y + p.off_y + cy_l, cx = tx * p.step_x + p.off_x + cx_l;   // conv output coordinates
+                        const bool cvalid = cy >= 0 && cy < 88 && cx >= 0 && cx < 88;
+                        float* srow = stage + rw * kPoolPitch + 2 * cs.m;
+                        const float ninf = -3.0e38f;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {                               // columns 8j + 2m + {0, 1}
+                            float a0 = acc[hf][4 * j + 2 * h], a1 = acc[hf][4 * j + 2 * h + 1];
+                            if constexpr (C::kStack == 2) { a0 += acc[hf][32 + 4 * j + 2 * h]; a1 += acc[hf][32 + 4 * j + 2 * h + 1]; }
+                            *reinterpret_cast<float2*>(srow + 8 * j) = cvalid ? make_float2(a0, a1) : make_float2(ninf, ninf);
+                        }
                     }
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");             // staging tile complete (consumer warpgroups only)
+                ptx::bar_sync(PP ? kEpiBar + cs.cg : kEpiBar, kEpiThreads);    // staging tile complete
 
-                const float* bias = p.img_wid ? p.gbias[p.img_wid[n0] * kLayersPerSet + L.li] : L.bias;
-                // 25 pooled pixels x 16 float4 channel groups = 400 vectors over 256 threads
-                for (int v = cs.ct; v < 400; v += 256) {
+                // 25 pooled pixels x 16 float4 channel groups = 400 vectors over the epilogue's threads
+                for (int v = et; v < 400; v += kEpiThreads) {
                     const int pp = v >> 4, c4 = (v & 15) * 4;
                     const int ppy = pp / 5, ppx = pp - ppy * 5;
                     const int oy = ty * 5 + ppy, ox = tx * 5 + ppx;     // pooled output coordinates
@@ -424,12 +529,18 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                             const float4 s4 = *reinterpret_cast<const float4*>(stage + ((2 * ppy + dy) * 11 + 2 * ppx + dx) * kPoolPitch + c4);
                             mx.x = fmaxf(mx.x, s4.x); mx.y = fmaxf(mx.y, s4.y); mx.z = fmaxf(mx.z, s4.z); mx.w = fmaxf(mx.w, s4.w);
                         }
-                    const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + c4));
-                    const float v4[4] = {selu_fast(mx.x + b4.x), selu_fast(mx.y + b4.y), selu_fast(mx.z + b4.z), selu_fast(mx.w + b4.w)};
+                    const float v4[4] = {selu_fast(mx.x + pb4.x), selu_fast(mx.y + pb4.y), selu_fast(mx.z + pb4.z), selu_fast(mx.w + pb4.w)};
                     S::encode(v4).store(L.out + S::addr((static_cast<size_t>(n0) * L.Ho + oy) * L.Wo + ox, L.out_c, L.out_coff + c4));
                 }
-                if (C::kPoolBufs == 1) asm volatile("bar.sync 1, 256;" ::: "memory");   // single staging buffer: readers done before the next tile writes
+                if constexpr (kShareStage) ptx::bar_arrive(kStageBar + (cs.cg ^ 1), 256);   // this warpgroup's readers are done
+                else if constexpr (!PP) { if (C::kPoolBufs == 1) ptx::bar_sync(kEpiBar, 256); }   // readers done before the next tile writes
             }
+            if (tstamp) tile_stamp(p.tile_trace, tile, 3);
+        }
+        if constexpr (PP) {
+            // no tile left to pass the turn (and the staging buffer) on to: the warpgroup whose turn it is takes it, so the named
+            // barriers end balanced
+            if ((it & 1) == cs.cg) { ptx::bar_sync(kTurnBar + cs.cg, 256); if constexpr (kShareStage) ptx::bar_sync(kStageBar + cs.cg, 256); }
         }
         if (stamp) { trace_stamp(p.trace, 4); trace_stamp(p.trace, 6); }
     }
@@ -454,19 +565,7 @@ template <int PREC> struct TCfg {
     static constexpr int kSmem = kAStages * kAUnit3 + kBStages * kBTile + ((kEpiBytes + 1023) & ~1023) + 1024 + 512;
     static_assert(kSmem <= 232448, "shared memory budget");
 };
-// registers per thread after setmaxnreg: the producer warpgroup gives up what the consumers' 128 accumulators need
-// (launch: 168 x 384 threads; after: 40 x 128 + 232 x 256 = the same 64,512)
-constexpr int kProducerRegs = 40;
-constexpr int kConsumerRegs = 232;
-constexpr int kTurnBar = 1;                    // named barrier kTurnBar + g: consumer warpgroup g may issue its unit's MMAs
 constexpr int kTaps3 = 9;                      // weight tiles per K chunk of a 3x3 conv (one per filter tap, both strides)
-
-// move a ring position (stage, phase) on by n stages
-__device__ __forceinline__ void ring_skip(int& stage, uint32_t& phase, int n, int stages) {
-    stage += n;
-    phase ^= static_cast<uint32_t>(stage / stages) & 1u;
-    stage %= stages;
-}
 
 struct UnitCoord { int l, img, tx, ty, n_tile, grp, c0, c1, piece, gidx; };
 // per-unit timeline (SE3TN_TRACE, small launches only): 5 stamps per work unit behind the trunk's per-CTA stamps:
@@ -947,15 +1046,19 @@ cudaError_t launch_resident_t(const ResidentParams& p, int num_sms, bool pdl, cu
     if ((KIND == KIND_STEM ? 7 : 9) * tiles_per_tap > C::kMaxWTiles) return cudaErrorInvalidValue;
     if (C::kStack == 2 && KIND == KIND_S1 && p.L.chunks != 2) return cudaErrorInvalidValue;    // a stacked tile row is exactly two 32-channel chunks
     if (p.L.cout != 64 || p.L.groups != 1 || p.L.n_tiles != 1 || p.m_tiles <= 0) return cudaErrorInvalidValue;
-    static size_t attr[64] = {};                   // the dynamic shared-memory limit is a per-device function attribute
-    cudaError_t e = set_smem(conv_resident_kernel<KIND, PREC>, C::kSmem, attr);
+    // Ping-pong only where some CTA has a second tile whose MMAs can run under its first tile's epilogue.  Where every CTA has
+    // one tile (n = 1: 81 stem tiles, 16 per 64-channel layer), the halves schedule runs that one epilogue on twice the threads.
+    const bool pp = p.m_tiles > num_sms;
+    void (*kernel)(ResidentParams) = pp ? conv_resident_kernel<KIND, PREC, true> : conv_resident_kernel<KIND, PREC, false>;
+    static size_t attr[2][64] = {};                // the dynamic shared-memory limit is a per-device function attribute
+    cudaError_t e = set_smem(kernel, C::kSmem, attr[pp]);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(std::min(p.m_tiles, num_sms)); cfg.blockDim = dim3(kThreads2); cfg.dynamicSmemBytes = C::kSmem; cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, conv_resident_kernel<KIND, PREC>, p);
+    return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 
 template <int PREC>

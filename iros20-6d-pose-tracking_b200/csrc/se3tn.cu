@@ -543,6 +543,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         else { rp.step_x = rp.step_y = 11; rp.off_x = rp.off_y = 0; }
         rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias;
         rp.trace = c->trace ? c->trace.get() + static_cast<size_t>(li) * 256 * 8 : nullptr;
+        rp.tile_trace = c->trace ? c->trace.get() + 14 * 256 * 8 + static_cast<size_t>(li) * SE3TN_TRACE_TILES * 4 : nullptr;
         { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, precision, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }

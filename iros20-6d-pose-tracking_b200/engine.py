@@ -453,7 +453,14 @@ class Engine:
 
     def get_trace(self):
         """(14, 256, 8) uint64 globaltimer stamps of the last forward's conv CTAs (needs SE3TN_TRACE=1 at Engine creation)."""
-        out = np.zeros((14, 256, 8), dtype=np.uint64)
+        return self._trace_words()[:14 * 256 * 8].reshape(14, 256, 8)
+
+    def get_tile_trace(self):
+        """(8, TRACE_TILES, 4) uint64 per-tile stamps of the last forward's 8 resident-weight conv launches (include/se3tn.h)."""
+        return self._trace_words()[14 * 256 * 8:].reshape(8, _lib.TRACE_TILES, 4)
+
+    def _trace_words(self):
+        out = np.zeros(14 * 256 * 8 + 8 * _lib.TRACE_TILES * 4, dtype=np.uint64)
         _lib.check(self.lib.se3tn_get_trace(self._ctx, out.ctypes.data_as(C.c_void_p)), self._ctx)
         return out
 

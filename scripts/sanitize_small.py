@@ -29,6 +29,12 @@ eng6 = pkg.Engine(max_batch=6); eng6.load_state_dict(synth.make_state_dict(0), 0
 A6, B6 = synth.tensor_pairs(6, seed=2); A6 = A6.cuda(); B6 = B6.cuda()
 for prec in ('bf16x3', 'tf32', 'bf16'):
     eng6.forward(A6, B6, precision=prec)
+# the resident launches run ping-pong where a CTA has more than one tile: the stems already do at n = 3 and 6, the 64-channel
+# layers (16 tiles per image) only from n = 9 on
+eng20 = pkg.Engine(max_batch=20); eng20.load_state_dict(synth.make_state_dict(0), 0)
+A20, B20 = synth.tensor_pairs(20, seed=3); A20 = A20.cuda(); B20 = B20.cuda()
+for prec in ('bf16x3', 'tf32', 'bf16'):
+    eng20.forward(A20, B20, precision=prec)
 m = torch.from_numpy(synth.model_points(500, 0)).cuda(); pr, gt = synth.pose_pairs(4, 0)
 add, adi = eng.add_adi(m, torch.from_numpy(pr).cuda(), torch.from_numpy(gt).cuda()); ap = eng.vocap(adi)
 torch.cuda.synchronize()
