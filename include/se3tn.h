@@ -157,14 +157,6 @@ int se3tn_track_batch(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* 
                       double trans_normalizer, double rot_normalizer, int precision,
                       float* out_trans, float* out_rot, double* poses_out, void* stream);
 
-/* a9, host side of the frame hand-over (reference predict.py:267-268 uploads whole tensors with .cuda()): copy only the
- * rows [y0, y1) x columns [x0, x1) of a HOST frame (rgb uint8 (H,W,3), depth uint16 (H,W); either may be NULL) into the
- * same rectangle of full-size DEVICE frame buffers.  K0 reads a frame only inside the tracks' crop windows, so a caller
- * that tracks a few objects uploads their bounding rectangle (a third of a 480x640 frame for one object) instead of 1.5 MB.
- * Two cudaMemcpy2DAsync on `stream`; pageable host memory makes them synchronous, as any such copy. */
-int se3tn_upload_frame_window(se3tn_ctx* ctx, const uint8_t* rgb_host, const uint16_t* depth_host, int H, int W,
-                              int y0, int y1, int x0, int x1, uint8_t* rgb_dev, uint16_t* depth_dev, void* stream);
-
 /* The one exchange step of the sharded path (SURVEY.md 8e): all-gather of the updated poses over an EXISTING NCCL
  * communicator, for hosts that drive libse3tn without torch.distributed (the Python layer uses
  * torch.distributed.all_gather_into_tensor, dist.py).  nccl_comm: the host's ncclComm_t; local_poses double

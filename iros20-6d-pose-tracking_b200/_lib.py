@@ -34,7 +34,6 @@ SIGNATURES = {
     'se3tn_add_adi': (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap': (_i, [_vp, _vp, _i, C.POINTER(_d), _vp]),
     'se3tn_allgather_poses': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
-    'se3tn_upload_frame_window': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),

@@ -1213,22 +1213,6 @@ int se3tn_vocap(se3tn_ctx* c, const double* errs, int n, double* out_ap, void* s
     return SE3TN_OK;
 }
 
-int se3tn_upload_frame_window(se3tn_ctx* c, const uint8_t* rgb_host, const uint16_t* depth_host, int H, int W,
-                              int y0, int y1, int x0, int x1, uint8_t* rgb_dev, uint16_t* depth_dev, void* stream) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (H <= 0 || W <= 0 || y0 < 0 || x0 < 0 || y1 > H || x1 > W || y0 > y1 || x0 > x1 || (rgb_host && !rgb_dev) || (depth_host && !depth_dev))
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_upload_frame_window: bad arguments");
-    if (y0 == y1 || x0 == x1) return SE3TN_OK;
-    DeviceGuard guard(c->device);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const size_t off = static_cast<size_t>(y0) * W + x0;
-    if (rgb_host) CU_TRY(c, cudaMemcpy2DAsync(rgb_dev + off * 3, static_cast<size_t>(W) * 3, rgb_host + off * 3, static_cast<size_t>(W) * 3,
-                                              static_cast<size_t>(x1 - x0) * 3, y1 - y0, cudaMemcpyHostToDevice, s));
-    if (depth_host) CU_TRY(c, cudaMemcpy2DAsync(depth_dev + off, static_cast<size_t>(W) * 2, depth_host + off, static_cast<size_t>(W) * 2,
-                                                static_cast<size_t>(x1 - x0) * 2, y1 - y0, cudaMemcpyHostToDevice, s));
-    return SE3TN_OK;
-}
-
 namespace {
 // crop window of one track in frame pixels: compute_bbox + crop_bbox's window (reference Utils.py:302-316, 324-327), the same
 // arithmetic as bbox.cuh on the device

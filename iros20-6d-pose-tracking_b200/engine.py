@@ -20,6 +20,10 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _hptr(a):
+    return a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
+
+
 def _stream(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -100,7 +104,7 @@ class Engine:
     def preprocess(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, weight_ids=None,
                    precision='bf16x3', want_tensors=False, want_crops=False):
         n = poses.shape[0]
-        self._check_frame(frame_rgb, frame_depth, rgbA, depthA, poses, object_width, n)
+        self._check_frame('preprocess', frame_rgb, frame_depth, poses, object_width, (rgbA, depthA), n)
         H, W = frame_depth.shape
         Kh = self._k4(K)
         outA = outB = crop_rgb = crop_depth = None
@@ -177,28 +181,8 @@ class Engine:
                     precision='bf16x3', out_poses=None, out_trans=None, out_rot=None, fill_depth=None):
         """n independent tracks of one frame: K0 -> conv stack -> K6, all enqueued on the current stream.  fill_depth: the
         observed depth is hole-filled inside the step first (depth_fill_spec); frame_depth itself is never written."""
-        n = poses.shape[0]
-        self._check_frame(frame_rgb, frame_depth, rgbA, depthA, poses, object_width, n)
-        fill = self.depth_fill_spec(fill_depth)
-        H, W = frame_depth.shape
-        Kh = self._k4(K)
-        out_poses = torch.empty_like(poses) if out_poses is None else out_poses
-        out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
-        out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
-        wh = None
-        if weight_ids_host is not None:
-            wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
-            if weight_ids_dev is None:
-                weight_ids_dev = torch.from_numpy(wh).to(self.device)
-        self._set_depth_fill(fill)
-        _lib.check(self.lib.se3tn_track_batch(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W,
-                                              Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width),
-                                              _ptr(rgbA), _ptr(depthA),
-                                              wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0),
-                                              _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer),
-                                              PREC[precision], _ptr(out_trans), _ptr(out_rot), _ptr(out_poses),
-                                              _stream(self.device)), self._ctx)
-        return out_poses, out_trans, out_rot
+        return self._track('track_batch', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
+                           rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth)
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
@@ -206,27 +190,33 @@ class Engine:
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised."""
+        return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
+                           trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
+                           fill_depth)
+
+    def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
+               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth):
+        """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
         n = poses.shape[0]
-        self._check_frame(frame_rgb, frame_depth, None, None, poses, object_width, n)
-        H, W = frame_depth.shape
-        Kh = self._k4(K)
-        rmode, rH, rW = self._render_mode(mode, image_hw)
+        self._check_frame(fn, frame_rgb, frame_depth, poses, object_width, A, n)
+        wh = self._host_ids(fn, weight_ids_host, n)
         fill = self.depth_fill_spec(fill_depth)
+        Kh = self._k4(K)
         out_poses = torch.empty_like(poses) if out_poses is None else out_poses
         out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
         out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
-        wh = None
-        if weight_ids_host is not None:
-            wh = np.ascontiguousarray(weight_ids_host, dtype=np.int32)
-            if weight_ids_dev is None:
-                weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        if wh is not None and weight_ids_dev is None:
+            weight_ids_dev = torch.from_numpy(wh).to(self.device)
         self._set_depth_fill(fill)
-        _lib.check(self.lib.se3tn_track_render(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W,
-                                               Kh.ctypes.data_as(C.c_void_p), _ptr(poses), _ptr(object_width), rmode, rH, rW,
-                                               wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0),
-                                               _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer),
-                                               PREC[precision], _ptr(out_trans), _ptr(out_rot), _ptr(out_poses),
-                                               _stream(self.device)), self._ctx)
+        H, W = frame_depth.shape
+        head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
+        tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
+                _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), _stream(self.device))
+        if render is None:
+            rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail)
+        else:
+            rc = self.lib.se3tn_track_render(*head, *render, *tail)
+        _lib.check(rc, self._ctx)
         return out_poses, out_trans, out_rot
 
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
@@ -235,41 +225,41 @@ class Engine:
         frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), poses float64 (n,4,4), object_width float64 (n), rgbA uint8
         (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous.  fill_depth as in
         track_batch: a live sensor's raw depth frame goes in as it is (the whole frame is uploaded then)."""
-        n = int(poses.shape[0])
-        wid = self._check_host('track_host', frame_rgb, frame_depth, poses, object_width, weight_ids, n,
-                               (('rgbA', rgbA, np.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', depthA, np.uint16, (n, IMAGE_SIZE, IMAGE_SIZE))))
-        fill = self.depth_fill_spec(fill_depth)
-        H, W = frame_depth.shape
-        Kh = self._k4(K)
-        out = np.empty((n, 4, 4), dtype=np.float64)
-        tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
-        ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
-        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
-        self._set_depth_fill(fill)
-        _lib.check(self.lib.se3tn_track_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
-                                             vp(rgbA), vp(depthA), vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
-                                             vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
-        return (out, tr, ro) if want_residuals else out
+        return self._track_host('track_host', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
+                                rot_normalizer, weight_ids, precision, want_residuals, fill_depth)
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                           weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None):
         """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
         without ids); mode / image_hw as in render()."""
+        return self._track_host('track_render_host', frame_rgb, frame_depth, K, poses, object_width, (),
+                                self._render_mode(mode, image_hw), trans_normalizer, rot_normalizer, weight_ids, precision,
+                                want_residuals, fill_depth)
+
+    def _track_host(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
+                    weight_ids, precision, want_residuals, fill_depth):
+        """track_host (A = (rgbA, depthA), render None) and track_render_host (A = (), render = _render_mode's triple)."""
         n = int(poses.shape[0])
-        wid = self._check_host('track_render_host', frame_rgb, frame_depth, poses, object_width, weight_ids, n, ())
-        H, W = frame_depth.shape
-        Kh = self._k4(K)
-        rmode, rH, rW = self._render_mode(mode, image_hw)
+        for name, a, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
+            if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
+                raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, dt, shape))
+        wid = self._host_ids(fn, weight_ids, n)
         fill = self.depth_fill_spec(fill_depth)
+        Kh = self._k4(K)
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
-        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
         self._set_depth_fill(fill)
-        _lib.check(self.lib.se3tn_track_render_host(self._ctx, vp(frame_rgb), vp(frame_depth), int(H), int(W), vp(Kh), vp(poses), vp(object_width),
-                                                    rmode, rH, rW, vp(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
-                                                    vp(out), vp(tr), vp(ro), _stream(self.device)), self._ctx)
+        H, W = frame_depth.shape
+        head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
+        tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
+                _stream(self.device))
+        if render is None:
+            rc = self.lib.se3tn_track_host(*head, *map(_hptr, A), *tail)
+        else:
+            rc = self.lib.se3tn_track_render_host(*head, *render, *tail)
+        _lib.check(rc, self._ctx)
         return (out, tr, ro) if want_residuals else out
 
     # ------------------------------------------------------------------ checkpoint validation
@@ -325,14 +315,6 @@ class Engine:
         _lib.check(self.lib.se3tn_pair_loss(self._ctx, _ptr(trans), _ptr(rot), _ptr(trans_label), _ptr(rot_label), n, _ptr(out_sums),
                                             _stream(self.device)), self._ctx)
         return out_sums
-
-    def upload_frame_window(self, rgb_host, depth_host, rgb_dev, depth_dev, y0, y1, x0, x1):
-        """Copy rows [y0,y1) x columns [x0,x1) of contiguous numpy frames (uint8 (H,W,3), uint16 (H,W); either may be None) into
-        full-size device frame buffers: K0 only reads a frame inside the tracks' crop windows."""
-        H, W = (depth_host if depth_host is not None else rgb_host).shape[:2]
-        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
-        _lib.check(self.lib.se3tn_upload_frame_window(self._ctx, vp(rgb_host), vp(depth_host), int(H), int(W),
-                                                      int(y0), int(y1), int(x0), int(x1), _ptr(rgb_dev), _ptr(depth_dev), _stream(self.device)), self._ctx)
 
     # ------------------------------------------------------------------ metrics (SURVEY 8f row 1)
     def add_adi(self, model_pts, pred, gt, want_add=True, want_adi=True):
@@ -478,33 +460,32 @@ class Engine:
             raise ValueError('expected a contiguous float32 CUDA tensor of shape (n,4,176,176), got %s %s' % (t.dtype, tuple(t.shape)))
 
     def _check_dev(self, name, t, dtype, shape):
-        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == self.device and t.dtype == dtype and t.is_contiguous()
-                and tuple(t.shape) == tuple(shape)):
+        if not (isinstance(t, torch.Tensor) and t.get_device() == self.device.index and t.dtype == dtype and t.is_contiguous()
+                and t.shape == tuple(shape)):
             raise ValueError('%s must be a contiguous %s CUDA tensor of shape %s on %s' % (name, dtype, tuple(shape), self.device))
 
-    def _check_frame(self, rgb, depth, rgbA, depthA, poses, ow, n):
-        """rgbA / depthA None: input A is rendered by the call, only the frame and the per-track arrays are checked."""
-        ok = (rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.is_contiguous() and rgb.dim() == 3 and rgb.shape[2] == 3 and
-              depth.is_cuda and depth.dtype == torch.uint16 and depth.is_contiguous() and depth.shape == rgb.shape[:2] and
-              (rgbA is None or (rgbA.is_cuda and rgbA.dtype == torch.uint8 and rgbA.is_contiguous() and tuple(rgbA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE, 3))) and
-              (depthA is None or (depthA.is_cuda and depthA.dtype == torch.uint16 and depthA.is_contiguous() and tuple(depthA.shape) == (n, IMAGE_SIZE, IMAGE_SIZE))) and
-              poses.is_cuda and poses.dtype == torch.float64 and poses.is_contiguous() and tuple(poses.shape) == (n, 4, 4) and
-              ow.is_cuda and ow.dtype == torch.float64 and ow.is_contiguous() and tuple(ow.shape) == (n,))
-        if not ok:
-            raise ValueError('bad frame/pose tensors: need uint8 (H,W,3), uint16 (H,W), uint8 (n,176,176,3), uint16 (n,176,176), '
-                             'float64 (n,4,4), float64 (n,), all contiguous CUDA tensors')
+    @staticmethod
+    def _track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
+        """(name, value, dtype name, shape) of each input of the tracking call fn; A is (rgbA, depthA), or () when the call
+        renders input A."""
+        hw = tuple(frame_depth.shape)
+        if len(hw) != 2:
+            raise ValueError('%s: frame_depth must be (H, W)' % fn)
+        rows = (('frame_rgb', frame_rgb, 'uint8', hw + (3,)), ('frame_depth', frame_depth, 'uint16', hw),
+                ('poses', poses, 'float64', (n, 4, 4)), ('object_width', object_width, 'float64', (n,)))
+        return rows + tuple(zip(('rgbA', 'depthA'), A, ('uint8', 'uint16'), ((n, IMAGE_SIZE, IMAGE_SIZE, 3), (n, IMAGE_SIZE, IMAGE_SIZE))))
+
+    def _check_frame(self, fn, frame_rgb, frame_depth, poses, object_width, A, n):
+        """The CUDA tensors of a tracking call.  A None input is passed on as a null pointer, which the library rejects."""
+        for name, t, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
+            if t is not None:
+                self._check_dev(name, t, getattr(torch, dt), shape)
         if n > self.max_batch:
             raise ValueError('n=%d exceeds max_batch=%d' % (n, self.max_batch))
 
     @staticmethod
-    def _check_host(fn, frame_rgb, frame_depth, poses, object_width, weight_ids, n, extra):
-        """Checks of the host-array entry points; returns weight_ids as a C-contiguous int32 array (or None)."""
-        for name, a, dt, shape in (('frame_rgb', frame_rgb, np.uint8, frame_depth.shape + (3,)), ('frame_depth', frame_depth, np.uint16, frame_depth.shape),
-                                   ('poses', poses, np.float64, (n, 4, 4)), ('object_width', object_width, np.float64, (n,))) + tuple(extra):
-            if not (isinstance(a, np.ndarray) and a.dtype == dt and tuple(a.shape) == tuple(shape) and a.flags['C_CONTIGUOUS']):
-                raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, np.dtype(dt).name, tuple(shape)))
-        if frame_depth.ndim != 2:
-            raise ValueError('%s: frame_depth must be (H, W)' % fn)
+    def _host_ids(fn, weight_ids, n):
+        """weight_ids as a C-contiguous int32 (n) host array, or None."""
         if weight_ids is None:
             return None
         wid = np.ascontiguousarray(weight_ids, dtype=np.int32)

@@ -12,7 +12,9 @@ Differences, all additive:
   * the second, visualisation-only render + cv2.imshow (predict.py:284-290) only happens with
     show=True.
   * on_track_batch(): N independent tracks of one frame in one batched launch sequence (the
-    reference is batch 1, F15).
+    reference is batch 1, F15).  Numpy frames and poses take the host route: one se3tn_track_host /
+    se3tn_track_render_host call that returns numpy poses.  Tensors and mixed inputs take the device
+    route: device tensors in, one se3tn_track_batch / se3tn_track_render step enqueued.
   * Tracker(..., fill_depth=True): on_track takes a live sensor's raw depth frame and hole-fills it
     inside the tracking step, as the reference's ROS node does with Utils.fill_depth before every
     on_track (predict_ros.py:38-41).
@@ -105,28 +107,6 @@ def _as_numpy_pose(p):
     return np.ascontiguousarray(p, dtype=np.float64)
 
 
-def crop_windows_union(poses, K, object_width, H, W, margin=2):
-    """Bounding rectangle (y0, y1, x0, x1), clipped to the frame, of the crop windows compute_bbox gives these poses (reference
-    Utils.py:302-316, same float64 arithmetic and np.round) plus a safety margin; None if a pose is degenerate (then upload everything)."""
-    import math
-    poses = np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4)
-    fx, fy, cx, cy = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
-    y0, y1, x0, x1 = H, 0, W, 0
-    for i in range(len(poses)):                    # plain Python floats: IEEE double like numpy's, round() is half-to-even like np.round
-        w = float(object_width if np.ndim(object_width) == 0 else object_width[i])
-        ox, oy, oz = float(poses[i, 0, 3]) * 1000.0, float(poses[i, 1, 3]) * 1000.0, float(poses[i, 2, 3]) * 1000.0
-        if oz == 0.0 or not all(math.isfinite(v) for v in (ox, oy, oz, w)):
-            return None
-        us = (round((ox - w / 2) * fx / oz + cx), round((ox + w / 2) * fx / oz + cx))
-        vs = (round((oy - w / 2) * fy / oz + cy), round((oy + w / 2) * fy / oz + cy))
-        y0 = min(y0, min(vs) - margin); y1 = max(y1, max(vs) + margin)
-        x0 = min(x0, min(us) - margin); x1 = max(x1, max(us) + margin)
-    y0, y1, x0, x1 = max(y0, 0), min(y1, H), max(x0, 0), min(x1, W)
-    if y1 <= y0 or x1 <= x0:
-        return (0, 0, 0, 0)                        # every window lies outside the frame: nothing to upload
-    return (y0, y1, x0, x1)
-
-
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
@@ -185,7 +165,6 @@ class Tracker:
                 renderer = None                                    # e.g. a vertices-only ply: fall through to the GL renderers
         self.renderer = renderer if renderer is not None else self._try_reference_renderer(model_path, cam_cfg)
         self._np_bufs = {}
-        self._pin_busy = False
         self.prev_rgb = None
         self.prev_depth = None
         self.frame_cnt = 0
@@ -275,128 +254,54 @@ class Tracker:
     def on_track_batch(self, prev_poses, current_rgb, current_depth, rgbA=None, depthA=None, weight_ids=None, object_width=None):
         """N independent tracks of ONE frame -> (N,4,4) float64.  rgbA / depthA None: rendered on the device by the CUDA
         rasteriser (needs a CudaRenderer; per-track models follow weight_ids), inside the tracking step when the renderer
-        allows it (_fused_renderer).
+        allows it (_fused_renderer).  The types of the inputs pick one of two routes:
 
-        numpy inputs   -> numpy result (synchronous, like the reference's on_track).
-        CUDA tensors   -> CUDA tensor, nothing is synchronised.
-        CPU tensors    -> CUDA tensor; the host->device copies run on a side stream into double-buffered
-                          staging, so the uploads of call k overlap the kernels of call k-1 (pinned memory
-                          makes them truly asynchronous).  Nothing is synchronised."""
-        dev = self.engine.device
-        as_numpy = not torch.is_tensor(prev_poses)
+        host    numpy frame and poses (ids and widths not tensors), input A numpy or drawn inside the step: one
+                Engine.track_host / track_render_host call stages the frame's crop-window rectangle, the poses and input A
+                through pinned memory and returns numpy poses (synchronous, like the reference's on_track).
+        device  everything else.  The inputs become device tensors, input A is rendered first when the step cannot draw it,
+                and one Engine.track_render / track_batch call is enqueued.
+                  CUDA tensors   are used as they are -> CUDA tensor, nothing is synchronised.
+                  CPU tensors    -> CUDA tensor; the host->device copies run on a side stream into double-buffered
+                                 staging, so the uploads of call k overlap the kernels of call k-1 (pinned memory
+                                 makes them truly asynchronous).  Nothing is synchronised.
+                  anything else  (numpy or mixed inputs): whole frames are copied into persistent device buffers; numpy
+                                 poses give a numpy result."""
         render = rgbA is None or depthA is None
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
-        if ((renderer is not None or (not render and all(isinstance(x, np.ndarray) for x in (rgbA, depthA))))
-                and all(isinstance(x, np.ndarray) for x in (current_rgb, current_depth))
-                and not torch.is_tensor(prev_poses) and not torch.is_tensor(weight_ids) and not torch.is_tensor(object_width)
-                and os.environ.get('SE3TN_HOST_CALL', '1') != '0'):
-            # numpy in, numpy out -- the reference's own calling pattern: ONE library call stages the crop-window rectangle of the
-            # frame, the poses and input A (unless the step renders it) through pinned memory, replays the step's graph and hands
-            # the poses back
+        is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
+        if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
+                and not any(torch.is_tensor(x) for x in (prev_poses, weight_ids, object_width))):
             c = lambda a, dt: a if (a.dtype == dt and a.flags['C_CONTIGUOUS']) else np.ascontiguousarray(a).astype(dt, copy=False)
-            poses_h = np.ascontiguousarray(prev_poses, dtype=np.float64).reshape(-1, 4, 4)
-            n = len(poses_h)
-            ow_h = np.full(n, float(self.object_width)) if object_width is None else np.ascontiguousarray(np.broadcast_to(np.asarray(object_width, dtype=np.float64), (n,)))
-            wh = None
-            if weight_ids is not None:
-                wh = np.ascontiguousarray(weight_ids, dtype=np.int32)
-            elif self.weight_id != 0:
-                wh = np.full(n, self.weight_id, dtype=np.int32)
+            poses = np.ascontiguousarray(prev_poses, dtype=np.float64).reshape(-1, 4, 4)
+            n = len(poses)
+            args = (c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses, self._widths(object_width, n))
+            kw = dict(weight_ids=self._weight_ids(weight_ids, n), precision=self.precision, fill_depth=self.fill_depth)
             if renderer is not None:
-                return self.engine.track_render_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h,
-                                                     self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw, fill_depth=self.fill_depth)
-            return self.engine.track_host(c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses_h, ow_h, c(rgbA, np.uint8), c(depthA, np.uint16),
-                                          self.trans_normalizer, self.rot_normalizer, weight_ids=wh, precision=self.precision,
-                                          fill_depth=self.fill_depth)
-        staged = not render and all(torch.is_tensor(x) and not x.is_cuda for x in (prev_poses, current_rgb, current_depth, rgbA, depthA))
+                return self.engine.track_render_host(*args, self.trans_normalizer, self.rot_normalizer, mode=renderer.mode,
+                                                     image_hw=renderer.image_hw, **kw)
+            return self.engine.track_host(*args, c(rgbA, np.uint8), c(depthA, np.uint16), self.trans_normalizer, self.rot_normalizer, **kw)
 
-        def up(x, dt, slot=None):
-            if torch.is_tensor(x):
-                return x.to(dev, dt).contiguous()
-            a = np.ascontiguousarray(x)
-            if dt == torch.uint16 and a.dtype != np.uint16:
-                a = a.astype(np.uint16)
-            src = torch.from_numpy(a)
-            if slot is None:
-                return src.to(dev).to(dt)
-            # numpy inputs land in persistent device buffers (one per argument and shape): the step's CUDA graph is keyed by its
-            # device pointers, so stable addresses mean every frame after the first is one graph launch
-            key = (slot, tuple(a.shape), dt)
-            buf = self._np_bufs.get(key)
-            if buf is None:
-                buf = self._np_bufs[key] = torch.empty(a.shape, dtype=dt, device=dev)
-            buf.copy_(src if src.dtype == dt else src.to(dt))
-            return buf
-
+        dev = self.engine.device
+        inputs = (prev_poses, current_rgb, current_depth) + ((None, None) if render else (rgbA, depthA))
+        staged = all(torch.is_tensor(x) and not x.is_cuda for x in inputs)
         if staged:
-            poses, rgb_d, depth_d, rgbA_d, depthA_d = self._stage_uploads(prev_poses, current_rgb, current_depth, rgbA, depthA)
+            poses, rgb_d, depth_d, rgbA_d, depthA_d = self._stage_uploads(*inputs)
         else:
-            poses = up(prev_poses, torch.float64, 'poses')
-            win = None
-            if (os.environ.get('SE3TN_WINDOW_UPLOAD', 'pinned') != 'off' and not torch.is_tensor(current_rgb) and not torch.is_tensor(current_depth) and not torch.is_tensor(prev_poses) and object_width is None
-                    and len(prev_poses) <= 4 and current_rgb.dtype == np.uint8 and current_depth.dtype == np.uint16
-                    and current_rgb.flags['C_CONTIGUOUS'] and current_depth.flags['C_CONTIGUOUS']):
-                # a few objects: K0 only reads the frame inside their crop windows -> upload that rectangle, not the whole 1.5 MB frame
-                win = crop_windows_union(prev_poses, self.K, self.object_width, current_depth.shape[0], current_depth.shape[1])
-            if win is not None and (win[1] - win[0]) * (win[3] - win[2]) * 2 < current_depth.size:
-                rk, dk = ('rgb', tuple(current_rgb.shape), torch.uint8), ('depth', tuple(current_depth.shape), torch.uint16)
-                for k2, dt in ((rk, torch.uint8), (dk, torch.uint16)):
-                    if k2 not in self._np_bufs:
-                        self._np_bufs[k2] = torch.zeros(k2[1], dtype=dt, device=dev)
-                rgb_d, depth_d = self._np_bufs[rk], self._np_bufs[dk]
-                # the fill reads the whole depth frame (the bilateral's range table is scaled by the whole image's min and max,
-                # extrapolate scans whole columns): then only rgb is windowed
-                dwin = (0, current_depth.shape[0], 0, current_depth.shape[1]) if Engine.depth_fill_spec(self.fill_depth)[0] else win
-                # through pinned staging (same geometry): a 2-D copy from pageable memory is staged row by row by the driver,
-                # from pinned memory it is one strided DMA
-                pk = ('pin', tuple(current_rgb.shape))
-                if os.environ.get('SE3TN_WINDOW_UPLOAD', 'pinned') == 'pageable':
-                    if dwin == win:
-                        self.engine.upload_frame_window(current_rgb, current_depth, rgb_d, depth_d, *win)
-                    else:
-                        self.engine.upload_frame_window(current_rgb, None, rgb_d, None, *win)
-                        self.engine.upload_frame_window(None, current_depth, None, depth_d, *dwin)
-                    pk = None
-                elif pk not in self._np_bufs:
-                    self._np_bufs[pk] = (torch.empty(current_rgb.shape, dtype=torch.uint8).pin_memory().numpy(),
-                                         torch.empty(current_depth.shape, dtype=torch.uint16).pin_memory().numpy())
-                if pk is not None:
-                    pin_rgb, pin_depth = self._np_bufs[pk]
-                    y0, y1, x0, x1 = win
-                    dy0, dy1, dx0, dx1 = dwin
-                    if self._pin_busy:
-                        torch.cuda.current_stream(dev).synchronize()          # the previous call's DMA may still be reading the staging
-                    np.copyto(pin_rgb[y0:y1, x0:x1], current_rgb[y0:y1, x0:x1]); np.copyto(pin_depth[dy0:dy1, dx0:dx1], current_depth[dy0:dy1, dx0:dx1])
-                    if dwin == win:
-                        self.engine.upload_frame_window(pin_rgb, pin_depth, rgb_d, depth_d, *win)
-                    else:
-                        self.engine.upload_frame_window(pin_rgb, None, rgb_d, None, *win)
-                        self.engine.upload_frame_window(None, pin_depth, None, depth_d, *dwin)
-                    self._pin_busy = not as_numpy
-            else:
-                rgb_d, depth_d = up(current_rgb, torch.uint8, 'rgb'), up(current_depth, torch.uint16, 'depth')
-            if not render:
-                rgbA_d, depthA_d = up(rgbA, torch.uint8, 'rgbA'), up(depthA, torch.uint16, 'depthA')
+            poses, rgb_d, depth_d, rgbA_d, depthA_d = map(self._to_device, inputs, ('poses', 'rgb', 'depth', 'rgbA', 'depthA'),
+                                                          (torch.float64, torch.uint8, torch.uint16, torch.uint8, torch.uint16))
         n = poses.shape[0]
+        wh = self._weight_ids(weight_ids, n)
+        wd = None if wh is None else self._resident(('wids', wh.tobytes()), lambda: wh)
         if object_width is None:
-            ow = self._np_bufs.get(('ow', n))
-            if ow is None:
-                ow = self._np_bufs[('ow', n)] = torch.full((n,), float(self.object_width), dtype=torch.float64, device=dev)
-        else:
-            ow = up(object_width, torch.float64, 'ow_arg')
+            ow = self._resident(('ow', n), lambda: self._widths(None, n))
+        else:                                         # widths passed in are refilled in place on every call, like the frame
+            ow = self._to_device(object_width if torch.is_tensor(object_width) else self._widths(object_width, n), 'ow_arg', torch.float64)
         if render and renderer is None:              # a renderer the step cannot stand in for draws input A first
-            mids = None
-            if weight_ids is not None:
-                mids = (weight_ids if torch.is_tensor(weight_ids) else torch.as_tensor(np.asarray(weight_ids))).to(dev, torch.int32)
-            rgbA_d, depthA_d = self.renderer.render_batch(poses, ow, mids)
-        wh = None
-        if weight_ids is not None:
-            wh = np.ascontiguousarray(weight_ids.cpu().numpy() if torch.is_tensor(weight_ids) else weight_ids, dtype=np.int32)
-        elif self.weight_id != 0:
-            wh = np.full(n, self.weight_id, dtype=np.int32)
+            rgbA_d, depthA_d = self.renderer.render_batch(poses, ow, None if weight_ids is None else wd)
+        as_numpy = not torch.is_tensor(prev_poses)
         outs = {}
         if as_numpy:                                  # results go back to the host: persistent output buffers keep the graph key stable too
             ob = self._np_bufs.get(('out', n))
@@ -404,24 +309,55 @@ class Tracker:
                 ob = self._np_bufs[('out', n)] = (torch.empty(n, 4, 4, dtype=torch.float64, device=dev),
                                                   torch.empty(n, 3, dtype=torch.float32, device=dev), torch.empty(n, 3, dtype=torch.float32, device=dev))
             outs = dict(out_poses=ob[0], out_trans=ob[1], out_rot=ob[2])
-        wd = None
-        if wh is not None:                            # device copy of the ids, cached by value
-            wk = ('wids', wh.tobytes())
-            wd = self._np_bufs.get(wk)
-            if wd is None:
-                wd = self._np_bufs[wk] = torch.from_numpy(wh).to(dev)
+        kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
         if renderer is not None:                      # input A is drawn inside the step, with the weight ids as mesh ids
             out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                 weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision,
-                                                 mode=renderer.mode, image_hw=renderer.image_hw, fill_depth=self.fill_depth, **outs)
+                                                 mode=renderer.mode, image_hw=renderer.image_hw, **kw)
         else:
             out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
-                                                self.trans_normalizer, self.rot_normalizer,
-                                                weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision,
-                                                fill_depth=self.fill_depth, **outs)
+                                                self.trans_normalizer, self.rot_normalizer, **kw)
         if staged:
             self._stage_done[self._stage_slot].record(torch.cuda.current_stream(dev))
         return out.cpu().numpy() if as_numpy else out
+
+    def _weight_ids(self, weight_ids, n):
+        """The tracks' weight ids as an int32 host array: the Tracker's weight set unless given, None for set 0 (a step
+        without ids uses set 0)."""
+        if weight_ids is None:
+            return np.full(n, self.weight_id, dtype=np.int32) if self.weight_id != 0 else None
+        return np.ascontiguousarray(weight_ids.cpu().numpy() if torch.is_tensor(weight_ids) else weight_ids, dtype=np.int32)
+
+    def _widths(self, object_width, n):
+        """The tracks' object widths as a float64 host array: the Tracker's object width unless given."""
+        return np.full(n, self.object_width if object_width is None else object_width, dtype=np.float64)
+
+    def _resident(self, key, make):
+        """A device copy of the small host array make() returns (weight ids, the default widths), made once per key and kept:
+        its stable address keeps the step's CUDA graph, and later calls copy nothing."""
+        t = self._np_bufs.get(key)
+        if t is None:
+            t = self._np_bufs[key] = torch.from_numpy(make()).to(self.engine.device)
+        return t
+
+    def _to_device(self, x, slot, dt):
+        """One input of the device route as a device tensor of dtype dt (None stays None).  A tensor is moved (a CUDA tensor
+        of that dtype is used as it is); anything else is copied whole into a persistent device buffer, one per argument and
+        shape: the step's CUDA graph is keyed by its device pointers, so stable addresses mean every frame after the first is
+        one graph launch."""
+        if x is None:
+            return None
+        if torch.is_tensor(x):
+            return x.to(self.engine.device, dt).contiguous()
+        a = np.ascontiguousarray(x)
+        if dt == torch.uint16 and a.dtype != np.uint16:
+            a = a.astype(np.uint16)
+        src = torch.from_numpy(a)
+        key = (slot, tuple(a.shape), dt)
+        buf = self._np_bufs.get(key)
+        if buf is None:
+            buf = self._np_bufs[key] = torch.empty(a.shape, dtype=dt, device=self.engine.device)
+        buf.copy_(src if src.dtype == dt else src.to(dt))
+        return buf
 
     # ------------------------------------------------------------------ pipelined uploads
     def _stage_uploads(self, *cpu_tensors):

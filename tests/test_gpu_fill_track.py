@@ -154,11 +154,11 @@ def _tracker(pkg, synth, tmp_path, engine=None, **kw):
     return trk
 
 
-def test_whole_frame_is_filled(pkg, synth, eng, tmp_path, monkeypatch):
+def test_whole_frame_is_filled(pkg, synth, eng, tmp_path):
     """One small crop window; a large patch at 60 m far outside it survives the hole filling and the median, so it sets the
     minimum of the median-filtered (inverted) image.  That stretches the bilateral's range table from about 1.5 m to about 60 m
-    and changes the filled depth inside the window.  The host entry points and the Tracker's window-upload branch must upload
-    the whole depth frame for the fill, over two frames that differ only outside the window."""
+    and changes the filled depth inside the window.  The host entry points and both of the Tracker's routes must fill the
+    whole depth frame, over two frames that differ only outside the window."""
     p = np.eye(4); p[:3, 3] = (0.0, 0.0, 1.5)                      # a 142-pixel window around the image centre
     c = Case(eng, synth, 1, seed=41, poses=p[None])
     far = c.depth.copy(); far[400:470, 10:80] = 60000
@@ -172,16 +172,15 @@ def test_whole_frame_is_filled(pkg, synth, eng, tmp_path, monkeypatch):
             want = _run(eng, entry, c, fl)
             got = _run(eng, entry, c, f, fill=True)
             assert _equal(got, want), entry
-    # Tracker.on_track_batch on numpy frames without the host entry points: the crop-window upload branch
-    monkeypatch.setenv('SE3TN_HOST_CALL', '0')
+    # Tracker.on_track_batch on numpy frames (the host route) and on CUDA tensors (the device route)
     trk = _tracker(pkg, synth, tmp_path, fill_depth=True)
     try:
         plain = _tracker(pkg, synth, tmp_path, engine=trk.engine)
-        for mode in ('pinned', 'pageable'):
-            monkeypatch.setenv('SE3TN_WINDOW_UPLOAD', mode)
-            for f, fl in zip(frames, filled):
-                want = plain.on_track_batch(p[None], c.rgb, fl)
-                assert np.array_equal(trk.on_track_batch(p[None], c.rgb, f), want), mode
+        T = lambda a: _dev(trk.engine, a)
+        for f, fl in zip(frames, filled):
+            assert np.array_equal(trk.on_track_batch(p[None], c.rgb, f), plain.on_track_batch(p[None], c.rgb, fl))
+            got = trk.on_track_batch(T(p[None]), T(c.rgb), T(f))
+            assert got.is_cuda and torch.equal(got, plain.on_track_batch(T(p[None]), T(c.rgb), T(fl)))
     finally:
         trk.engine.close()
 

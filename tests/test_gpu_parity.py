@@ -299,7 +299,7 @@ def test_on_track_end_to_end_vs_oracle(pkg, synth):
         assert staged.is_cuda and np.array_equal(staged.cpu().numpy(), batch)
 
 
-def test_track_host_one_call_equals_device_path(pkg, synth, eng, monkeypatch):
+def test_track_host_one_call_equals_device_path(pkg, synth, eng):
     """se3tn_track_host (numpy in / numpy out in ONE library call: pinned staging of the crop-window rectangle, graph replay, read
     back) runs the same kernels on the same bytes as se3tn_track_batch on device tensors: identical poses, for windows inside,
     across and outside the frame, several frame sizes, per-track weight sets and widths, and repeated calls (graph replay)."""
@@ -330,16 +330,15 @@ def test_track_host_one_call_equals_device_path(pkg, synth, eng, monkeypatch):
         big = 70
         eng.track_host(rgb, depth, synth.CAMERA_K, np.tile(poses[:1], (big, 1, 1)), np.full(big, 200.0), np.tile(rgbA[:1], (big, 1, 1, 1)),
                        np.tile(depthA[:1], (big, 1, 1)), TN, RN)
-    # the Tracker's numpy path is this call; SE3TN_HOST_CALL=0 keeps the tensor plumbing -- same poses either way
+    # the Tracker's numpy route is this call, its CUDA-tensor route is track_batch -- same poses either way
     info = {'resolution': 176, 'boundingbox': 10, 'object_width': 200.0,
             'camera': {'focalX': synth.CAMERA_K[0, 0], 'focalY': synth.CAMERA_K[1, 1], 'centerX': synth.CAMERA_K[0, 2],
                        'centerY': synth.CAMERA_K[1, 2], 'height': 480, 'width': 640}}
     trk = pkg.Tracker(info, mean, std, {'state_dict': synth.make_state_dict(0)}, model_path=None, engine=eng)
     rgb, depth, poses, rgbA, depthA = _frame_case(synth, 2, 5)
     a = trk.on_track_batch(poses, rgb, depth, rgbA, depthA)
-    monkeypatch.setenv('SE3TN_HOST_CALL', '0')
-    b = trk.on_track_batch(poses, rgb, depth, rgbA, depthA)
-    assert np.array_equal(a, b)
+    b = trk.on_track_batch(*map(t, (poses, rgb, depth, rgbA, depthA)))
+    assert b.is_cuda and np.array_equal(a, b.cpu().numpy())
 
 
 def test_track_batch_mixed_weight_sets(synth, eng):

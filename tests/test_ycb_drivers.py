@@ -83,24 +83,3 @@ def test_load_vertices_merges_duplicates_like_trimesh(pr, tmp_path):
     b = pr.PointCloud(pts).voxel_down_sample(0.005).points
     assert a.shape == b.shape and np.allclose(np.sort(a, 0), np.sort(b, 0))            # same voxels here; means of identical points are unchanged
 
-
-def test_crop_windows_union_covers_compute_bbox(pr):
-    """The few-object upload path sends only the bounding rectangle of the crop windows: it must contain every window the reference's
-    compute_bbox (oracle restatement) yields, clipped to the frame."""
-    import se3_oracle as O
-    synth = importlib.import_module('iros20-6d-pose-tracking_b200.synth')
-    K = synth.CAMERA_K
-    H, W = 480, 640
-    for seed in range(20):
-        poses = synth.raw_poses(3, seed=seed)
-        y0, y1, x0, x1 = pr.crop_windows_union(poses, K, 200.0, H, W)
-        for p in poses:
-            bb = O.compute_bbox(p, K, 200.0, scale=(1000, 1000, 1000))
-            top, bottom = max(bb[:, 0].min(), 0), min(bb[:, 0].max(), H)
-            left, right = max(bb[:, 1].min(), 0), min(bb[:, 1].max(), W)
-            if bottom > top and right > left:
-                assert y0 <= top and bottom <= y1 and x0 <= left and right <= x1
-    far = np.eye(4); far[:3, 3] = [5.0, 5.0, 0.5]                   # projects far outside the frame
-    assert pr.crop_windows_union(far[None], K, 200.0, H, W) == (0, 0, 0, 0)
-    bad = np.eye(4); bad[2, 3] = 0.0                                  # z = 0: no window
-    assert pr.crop_windows_union(bad[None], K, 200.0, H, W) is None
