@@ -149,7 +149,9 @@ int se3tn_so3_log(se3tn_ctx* ctx, const double* poses_a, const double* poses_b,
  * takes its weight tensor map / bias from per-set device tables.  Any id order is correct; keeping equal ids
  * contiguous (dist.shard_tracks does) avoids shared-memory weight reloads in the 64-channel layers.  In
  * SE3TN_PREC_FP32 each contiguous run of equal ids is one batched forward.
- * out_trans/out_rot float32 (n,3) device scratch the caller provides (also returned). */
+ * out_trans/out_rot float32 (n,3) device scratch the caller provides (also returned).
+ * poses_out may be poses_in: every read of a track's previous pose comes before its update is written, so tracks whose poses
+ * stay in one device array, updated in place frame after frame, keep the step's addresses and its CUDA graph. */
 int se3tn_track_batch(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                       const double* K, const double* poses_in, const double* object_width,
                       const uint8_t* rgbA, const uint16_t* depthA,
@@ -265,7 +267,7 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
  * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph (se3tn_last_step_was_graph);
  * SE3TN_PREC_FP32 renders and then runs its FFMA forwards without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
  * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
- * camera image size out of range is SE3TN_ERR_INVALID. */
+ * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch. */
 int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                        const double* K, const double* poses_in, const double* object_width,
                        int render_mode, int render_H, int render_W,

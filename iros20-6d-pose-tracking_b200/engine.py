@@ -189,7 +189,8 @@ class Engine:
                      out_poses=None, out_trans=None, out_rot=None, fill_depth=None):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
-        mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised."""
+        mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
+        out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h)."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
                            fill_depth)

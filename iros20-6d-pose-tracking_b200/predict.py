@@ -598,6 +598,19 @@ def predictSequenceYcb(ycb_dir, seq_id, class_id, dataset_info, images_mean, ima
     return pred_poses, adi_auc
 
 
+def _ycb_first_pose(ycb_dir, class_id, seq_id, gt_file0, initialize_method, keyframes_all, seqs):
+    """The pose a track of `class_id` starts sequence `seq_id` from (reference predict.py:376-390): the ground truth of its first
+    frame, PoseCNN's estimate at the sequence's first key frame, or PoseRBPF's first pose.  seqs: the class's test sequences."""
+    if initialize_method == 'posecnn':
+        seq_frame = '%04d/%06d' % (seq_id, 1)
+        return posecnn_pose('{}/YCB_Video_toolbox/results_PoseCNN_RSS2018/%06d.mat'.format(ycb_dir) % keyframes_all.index(seq_frame), class_id)
+    if initialize_method == 'poserbpf':
+        return poserbpf_pose(ycb_dir, class_id, seq_id, seqs)
+    if initialize_method == 'gt':
+        return np.loadtxt(gt_file0)
+    raise ValueError('initialize_method must be gt, posecnn or poserbpf')
+
+
 def getResultsYcb(ycb_dir, class_id, dataset_info, images_mean, images_std, ckpt_dir, model_path, outdir,
                   initialize_method='gt', tracker=None, max_frames=None, **tracker_kwargs):
     """Every YCB-Video TEST sequence (0048..0059) under <ycb_dir>/data_organized/ that contains `class_id`, tracked from its first
@@ -616,15 +629,7 @@ def getResultsYcb(ycb_dir, class_id, dataset_info, images_mean, images_std, ckpt
             continue
         seq_dir = os.path.join(gt_dir, '..')
         rgb_files, depth_files, gt_files = _ycb_sequence_files(seq_dir, class_id)
-        if initialize_method == 'posecnn':
-            seq_frame = '%04d/%06d' % (seq_id, 1)
-            prev_pose = posecnn_pose('{}/YCB_Video_toolbox/results_PoseCNN_RSS2018/%06d.mat'.format(ycb_dir) % keyframes_all.index(seq_frame), class_id)
-        elif initialize_method == 'poserbpf':
-            prev_pose = poserbpf_pose(ycb_dir, class_id, seq_id, seqs)
-        elif initialize_method == 'gt':
-            prev_pose = np.loadtxt(gt_files[0])
-        else:
-            raise ValueError('initialize_method must be gt, posecnn or poserbpf')
+        prev_pose = _ycb_first_pose(ycb_dir, class_id, seq_id, gt_files[0], initialize_method, keyframes_all, seqs)
         pred_poses = [prev_pose]
         n = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
         for i in range(1, n):
@@ -643,15 +648,219 @@ def getResultsYcb(ycb_dir, class_id, dataset_info, images_mean, images_std, ckpt
     return results
 
 
+# ----------------------------------------------------------------------------------------------------
+# Every class in one pass: the YCB-Video evaluation (the paper's Table I) as one run instead of one getResultsYcb run per class.
+# Each test sequence's requested classes are tracked together, one se3tn_track_render step per frame with one weight set and
+# mesh per class; each frame is decoded once.  The output tree is what eval_ycb.eval_all scores:
+#   <outdir>/<CADmodels folder of the class>/run/seq<id>/%07d.txt
+# Per-class configuration is four path templates with {class_id} and {class_name} (the CADmodels/ folder name) placeholders.
+# ----------------------------------------------------------------------------------------------------
+YCB_ALL_TEMPLATES = ('train_data_path', 'mean_std_path', 'ckpt_dir', 'model_path')
+YCB_ALL_RUN = 'run'
+
+
+def ycb_class_names(ycb_dir):
+    """The CADmodels/ folder names in sorted order: class id k is entry k - 1, as eval_ycb.py maps them."""
+    d = os.path.join(ycb_dir, 'CADmodels')
+    if not os.path.isdir(d):
+        raise FileNotFoundError('no CADmodels/ folder under %s: it names the classes' % ycb_dir)
+    return sorted(os.listdir(d))
+
+
+def ycb_all_res_dir(outdir, class_name):
+    """Where getResultsYcbAll writes a class's seq<id>/%07d.txt files: eval_ycb.eval_all takes the class folders in sorted order
+    as class ids 1, 2, ..., and the first folder inside each as its result folder."""
+    return os.path.join(outdir, class_name, YCB_ALL_RUN)
+
+
+def expand_class_paths(class_config, class_id, class_name):
+    """The four path templates of class_config for one class -> {train_data_path, mean_std_path, ckpt_dir, model_path}."""
+    out = {}
+    for key in YCB_ALL_TEMPLATES:
+        if key not in class_config:
+            raise ValueError('class_config needs a %r template' % key)
+        try:
+            out[key] = str(class_config[key]).format(class_id=class_id, class_name=class_name)
+        except (KeyError, IndexError, ValueError) as e:
+            raise ValueError('class_config[%r] = %r: the only placeholders are {class_id} and {class_name} (%s)'
+                             % (key, class_config[key], e)) from None
+    return out
+
+
+def _class_normalizer(class_config, key, class_id, default):
+    v = class_config.get(key, default)
+    if isinstance(v, dict) and class_id not in v:
+        raise ValueError('class_config[%r] has no value for class %d' % (key, class_id))
+    return float(v[class_id] if isinstance(v, dict) else v)
+
+
+def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
+    """The checked configuration of every requested class, before anything is loaded onto a device -> list (ascending class id)
+    of dicts: class_id, name, the expanded paths, dataset_info, mean, std, trans_normalizer, rot_normalizer.
+
+    class_config: the YCB_ALL_TEMPLATES path templates; optionally trans_normalizer / rot_normalizer (the Tracker's, default
+    0.03 m and 5 degrees as getResultsYcb uses them), each a number or a {class_id: number} mapping.  A missing file is a
+    FileNotFoundError naming the class and the path.  One step tracks every class of a frame, so the classes must share the
+    camera (K and image size), the resolution (176), the render mode, the two normalisers and the precision: a class that differs
+    from the first is a ValueError naming it."""
+    import yaml
+    from .engine import PREC
+    if precision not in PREC:
+        raise ValueError('unknown precision %r (one of %s)' % (precision, ', '.join(PREC)))
+    names = ycb_class_names(ycb_dir)
+    ids = sorted(set(int(c) for c in class_ids))
+    if not ids:
+        raise ValueError('no class ids given')
+    for c in ids:
+        if not 1 <= c <= len(names):
+            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
+    classes = []
+    for c in ids:
+        name = names[c - 1]
+        paths = expand_class_paths(class_config, c, name)
+        info_path = os.path.join(paths['train_data_path'], '../dataset_info.yml')
+        files = [('dataset_info.yml', info_path), ('mean', os.path.join(paths['mean_std_path'], 'mean.npy')),
+                 ('std', os.path.join(paths['mean_std_path'], 'std.npy')), ('checkpoint', paths['ckpt_dir']), ('mesh', paths['model_path'])]
+        for what, path in files:
+            if not os.path.isfile(path):
+                raise FileNotFoundError('class %d (%s): no %s file at %s' % (c, name, what, path))
+        with open(info_path, 'r') as ff:
+            info = yaml.safe_load(ff)
+        classes.append(dict(class_id=c, name=name, dataset_info=info, mean=np.load(files[1][1]), std=np.load(files[2][1]),
+                            trans_normalizer=_class_normalizer(class_config, 'trans_normalizer', c, 0.03),
+                            rot_normalizer=_class_normalizer(class_config, 'rot_normalizer', c, 5 * np.pi / 180), **paths))
+    first = classes[0]
+    shared = (('camera', lambda k: {key: float(v) for key, v in k['dataset_info']['camera'].items()}),
+              ('renderer', lambda k: k['dataset_info'].get('renderer') == 'pyrenderer'),
+              ('trans_normalizer', lambda k: k['trans_normalizer']), ('rot_normalizer', lambda k: k['rot_normalizer']))
+    for k in classes:
+        if k['dataset_info']['resolution'] != 176:
+            raise ValueError('class %d (%s): resolution %s; libse3tn is built for 176' % (k['class_id'], k['name'], k['dataset_info']['resolution']))
+        for what, get in shared:
+            if get(k) != get(first):
+                raise ValueError('class %d (%s): %s %r differs from class %d\'s %r; classes tracked in one step must share it'
+                                 % (k['class_id'], k['name'], what, get(k), first['class_id'], get(first)))
+    return classes
+
+
+def ycb_track_sets(ycb_dir, class_ids):
+    """{seq_id: [class ids]}, ascending: for every YCB-Video test sequence (0048..0059) under <ycb_dir>/data_organized/, the
+    requested classes its pose_gt/ lists -- the sequences a getResultsYcb run of each class visits."""
+    data_dir = '{}/data_organized/'.format(ycb_dir)
+    sets = {}
+    for c in sorted(set(int(c) for c in class_ids)):
+        for s in findClassContainedVideosYcb(c, data_dir, testset=True):
+            sets.setdefault(s, []).append(c)
+    return dict(sorted(sets.items()))
+
+
+def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None):
+    """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
+    writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
+
+    One Engine holds every class's weights, statistics and CUDA-renderer mesh under weight id = class id.  For each test sequence,
+    the tracks are its requested classes in ascending order, each started as getResultsYcb starts it.  Every frame is one
+    se3tn_track_render step for all of them: its colour and depth PNGs are decoded once, in a thread pool, into one of two pinned
+    staging sets (frame t+1 decodes while step t runs), and uploaded in stream order into one device frame.  The tracks' poses live
+    in one device tensor that every step updates in place (the step's graph key keeps its addresses, so every step after the
+    first of a sequence is a graph replay); after each step they are copied into a (frames, n, 4, 4) history on the device, which
+    comes back to the host once per sequence."""
+    from concurrent.futures import ThreadPoolExecutor
+    if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
+        raise ValueError('initialize_method must be gt, posecnn or poserbpf')
+    classes = ycb_all_classes(ycb_dir, class_ids, class_config, precision)
+    track_sets = ycb_track_sets(ycb_dir, [k['class_id'] for k in classes])
+    data_dir = '{}/data_organized/'.format(ycb_dir)
+    keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
+    eng = Engine(max_batch=max([len(v) for v in track_sets.values()] + [1]))
+    trackers = {}
+    for k in classes:
+        try:
+            trackers[k['class_id']] = Tracker(k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], model_path=k['model_path'],
+                                              engine=eng, weight_id=k['class_id'], precision=precision, renderer='cuda',
+                                              trans_normalizer=k['trans_normalizer'], rot_normalizer=k['rot_normalizer'])
+        except ValueError as e:
+            raise ValueError('class %d (%s): %s' % (k['class_id'], k['name'], e)) from e
+    name_of = {k['class_id']: k['name'] for k in classes}
+    trk0 = trackers[classes[0]['class_id']]
+    render = trk0.renderer
+    cam = trk0.dataset_info['camera']
+    dev = eng.device
+    pinned = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True)
+    host = [(pinned((cam['height'], cam['width'], 3), torch.uint8), pinned((cam['height'], cam['width']), torch.uint16)) for _ in range(2)]
+    rgb_d = torch.empty(host[0][0].shape, dtype=torch.uint8, device=dev)
+    depth_d = torch.empty(host[0][1].shape, dtype=torch.uint16, device=dev)
+    uploaded = [None, None]                                # event after the last upload from each staging set
+
+    def decode_into(dst, read, path):
+        img = read(path)
+        if img.shape != tuple(dst.shape):
+            raise ValueError('%s: %s, the camera image is %s (dataset_info.yml)' % (path, img.shape, tuple(dst.shape)))
+        dst.numpy()[...] = img
+
+    results = {k['class_id']: {} for k in classes}
+    with ThreadPoolExecutor(max_workers=2) as pool:
+        def submit(rgb_path, depth_path, slot):
+            if uploaded[slot] is not None:
+                uploaded[slot].synchronize()               # the staging set's previous upload has left it
+            return [pool.submit(decode_into, host[slot][0], read_rgb, rgb_path),
+                    pool.submit(decode_into, host[slot][1], read_depth, depth_path)]
+
+        for seq_id, cls in track_sets.items():
+            seq_dir = os.path.join(data_dir, '%04d' % seq_id)
+            files = {c: _ycb_sequence_files(seq_dir, c) for c in cls}
+            rgb_files, depth_files = files[cls[0]][0], files[cls[0]][1]
+            nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
+            init = [_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
+                                    sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]
+            n = len(cls)
+            ids = np.asarray(cls, dtype=np.int32)
+            ids_d = torch.from_numpy(ids).to(dev)
+            widths = torch.tensor([trackers[c].object_width for c in cls], dtype=torch.float64, device=dev)
+            poses = torch.from_numpy(np.stack(init).astype(np.float64)).to(dev)     # updated in place by every step
+            history = torch.empty((nf, n, 4, 4), dtype=torch.float64, device=dev)
+            history[0].copy_(poses)
+            out_trans = torch.empty((n, 3), dtype=torch.float32, device=dev)
+            out_rot = torch.empty((n, 3), dtype=torch.float32, device=dev)
+            pending = submit(rgb_files[1], depth_files[1], 1) if nf > 1 else None
+            for t in range(1, nf):
+                slot = t % 2
+                for f in pending:
+                    f.result()
+                rgb_d.copy_(host[slot][0], non_blocking=True)
+                depth_d.copy_(host[slot][1], non_blocking=True)
+                uploaded[slot] = torch.cuda.Event()
+                uploaded[slot].record()
+                eng.track_render(rgb_d, depth_d, trk0.K, poses, widths, trk0.trans_normalizer, trk0.rot_normalizer,
+                                 weight_ids_host=ids, weight_ids_dev=ids_d, precision=precision, mode=render.mode,
+                                 image_hw=render.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
+                history[t].copy_(poses)
+                if t + 1 < nf:
+                    pending = submit(rgb_files[t + 1], depth_files[t + 1], (t + 1) % 2)
+            tracked = history.cpu().numpy()
+            for j, c in enumerate(cls):
+                pred_poses = list(tracked[:, j])
+                while len(pred_poses) < len(rgb_files) and max_frames is None:      # predict.py:437-440
+                    pred_poses.append(pred_poses[-1])
+                sdir = os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq{}'.format(seq_id))
+                os.makedirs(sdir, exist_ok=True)
+                for i in range(len(pred_poses)):
+                    np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i])
+                results[c][seq_id] = np.array(pred_poses)
+    return results
+
+
 def main(argv=None):
     import argparse
     parser = argparse.ArgumentParser(description='headless se(3)-TrackNet sequence tracking on libse3tn (flags of the reference predict.py:626-641)')
-    parser.add_argument('--mode', default='ycbv', help='ycbv (one YCB-Video sequence) / ycbineoat / anything else: every YCB-Video test sequence of the class')
+    parser.add_argument('--mode', default='ycbv', help='ycbv (one YCB-Video sequence) / ycbineoat / ycbv_all (every class of --class_ids '
+                        'through every YCB-Video test sequence in one pass) / anything else: every YCB-Video test sequence of the class')
     parser.add_argument('--seq_id', default=None, type=int)
     parser.add_argument('--ycb_dir', default=None)
     parser.add_argument('--YCBInEOAT_dir', default=None)
     parser.add_argument('--train_data_path', required=True, help='dataset_info.yml is read from <train_data_path>/../')
     parser.add_argument('--class_id', default=-1, type=int, help='class id in YCB Video')
+    parser.add_argument('--class_ids', default=None, help='ycbv_all: comma-separated class ids, or all')
     parser.add_argument('--model_path', type=str, required=True, help='path to mesh (.ply with normals and vertex colours for the CUDA renderer)')
     parser.add_argument('--ckpt_dir', type=str, required=True)
     parser.add_argument('--mean_std_path', type=str, required=True)
@@ -659,7 +868,10 @@ def main(argv=None):
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
     parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt)')
     parser.add_argument('--max_frames', type=int, default=None)
+    parser.add_argument('--score', action='store_true', help='ycbv_all: score the output with eval_ycb and print its lines')
     args = parser.parse_args(argv)
+    if args.mode == 'ycbv_all':
+        return _main_ycbv_all(args)
     dataset_info, images_mean, images_std = load_run_config(args.train_data_path, args.mean_std_path)
     if args.mode == 'ycbineoat':
         if not args.YCBInEOAT_dir:
@@ -682,6 +894,36 @@ def main(argv=None):
     res = getResultsYcb(args.ycb_dir, args.class_id, dataset_info, images_mean, images_std, args.ckpt_dir, args.model_path, args.outdir,
                         initialize_method=args.init, max_frames=args.max_frames)
     print('tracked class %d through sequences %s -> %s' % (args.class_id, sorted(res), args.outdir))
+
+
+def _main_ycbv_all(args):
+    """--mode ycbv_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class path templates."""
+    import argparse
+    if not args.ycb_dir or not args.class_ids:
+        raise SystemExit('--mode ycbv_all needs --ycb_dir and --class_ids')
+    n_classes = len(ycb_class_names(args.ycb_dir))
+    if args.class_ids == 'all':
+        class_ids = list(range(1, n_classes + 1))
+    else:
+        try:
+            class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
+        except ValueError:
+            raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+    config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
+    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames)
+    for c in sorted(res):
+        print('tracked class %d through sequences %s' % (c, sorted(res[c])))
+    print('-> %s' % args.outdir)
+    if args.score:
+        from . import eval_ycb
+        names = ycb_class_names(args.ycb_dir)
+        if class_ids == list(range(1, 22)) and n_classes == 21:
+            eval_ycb.eval_all(argparse.Namespace(ycb_dir=args.ycb_dir, res_root=args.outdir))
+        else:                                                       # eval_all pools exactly the 21 classes: score each one
+            for c in class_ids:
+                eval_ycb.eval_one_class(argparse.Namespace(ycb_dir=args.ycb_dir, class_id=c,
+                                                           res_dir=ycb_all_res_dir(args.outdir, names[c - 1]) + '/'))
+    return res
 
 
 if __name__ == '__main__':

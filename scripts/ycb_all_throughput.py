@@ -1,0 +1,111 @@
+"""YCB-Video evaluation throughput: predict.getResultsYcbAll (every class of a test sequence in one step per frame, each frame
+decoded once) against the loop of per-class predict.getResultsYcb runs it replaces (one class per run, every frame decoded once
+per object, one synchronous n = 1 step per frame), over the same data set.  The two alternate `--rounds` times in one process,
+each call timed whole (engine set-up, weight and mesh upload, decoding, tracking, writing the pose files); the card's name and
+power limit are read in the same run.
+
+    python scripts/ycb_all_throughput.py [--frames 100] [--rounds 3] [--precision bf16x3]
+
+The data set is written to a temporary directory, seeded, and removed afterwards: test sequences 0048..0050 with 5 objects each,
+480 x 640 colour and depth PNGs, synthetic weights, statistics and meshes per class.  Rates: frames/s counts each sequence frame
+once; objects x frames/s counts each tracked object in each frame.
+"""
+import argparse, importlib, json, os, subprocess, sys, tempfile, time
+import cv2
+import numpy as np
+import torch
+import yaml
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
+PKG = 'iros20-6d-pose-tracking_b200'
+SEQS = {48: (1, 2, 3, 4, 5), 49: (2, 3, 4, 5, 6), 50: (1, 3, 5, 6, 7)}
+
+
+def smooth(rng, shape, lo, hi, dtype):
+    """A frame with some structure (a blurred random field plus noise), so the PNGs compress like camera images, not like noise."""
+    small = rng.uniform(lo, hi, (shape[0] // 16, shape[1] // 16) + shape[2:])
+    img = cv2.resize(small, (shape[1], shape[0]), interpolation=cv2.INTER_CUBIC) + rng.normal(0, (hi - lo) * 0.02, shape)
+    return np.clip(img, lo, hi).astype(dtype)
+
+
+def write_tree(tmp, frames, synth):
+    mio = importlib.import_module(PKG + '.mesh_io')
+    rng = np.random.default_rng(0)
+    ycb, cfg = os.path.join(tmp, 'ycb'), os.path.join(tmp, 'cfg')
+    classes = sorted(set(c for cls in SEQS.values() for c in cls))
+    K = synth.CAMERA_K
+    cam = {'focalX': float(K[0, 0]), 'focalY': float(K[1, 1]), 'centerX': float(K[0, 2]), 'centerY': float(K[1, 2]), 'height': 480, 'width': 640}
+    mean, std = synth.default_mean_std()
+    for c in classes:
+        d = os.path.join(cfg, 'c%d' % c)
+        os.makedirs(os.path.join(d, 'train'))
+        yaml.safe_dump({'resolution': 176, 'object_width': 150.0 + 10 * c, 'boundingbox': 10, 'camera': cam}, open(os.path.join(d, 'dataset_info.yml'), 'w'))
+        np.save(os.path.join(d, 'mean.npy'), mean + c); np.save(os.path.join(d, 'std.npy'), std)
+        torch.save({'epoch': 1, 'state_dict': synth.make_state_dict(c), 'best_prec': 0.0}, os.path.join(d, 'model_best_val.pth.tar'))
+        mio.save_ply_mesh(os.path.join(d, 'textured.ply'), synth.mesh(3, seed=c))
+    for k in range(1, 22):
+        os.makedirs(os.path.join(ycb, 'CADmodels', '%03d_obj' % k))
+    for seq, cls in SEQS.items():
+        base = os.path.join(ycb, 'data_organized', '%04d' % seq)
+        for sub in ['color', 'depth_filled'] + ['pose_gt/%d' % c for c in cls]:
+            os.makedirs(os.path.join(base, sub))
+        for i in range(frames):
+            cv2.imwrite(os.path.join(base, 'color', '%06d-color.png' % (i + 1)), smooth(rng, (480, 640, 3), 0, 255, np.uint8))
+            cv2.imwrite(os.path.join(base, 'depth_filled', '%06d-depth.png' % (i + 1)), smooth(rng, (480, 640), 400, 1500, np.uint16))
+        for c in cls:
+            p = synth.raw_poses(1, seed=10 * seq + c)[0]
+            for i in range(frames):
+                q = p.copy(); q[:3, 3] += 0.001 * i
+                np.savetxt(os.path.join(base, 'pose_gt', str(c), '%06d.txt' % (i + 1)), q)
+    templates = {'train_data_path': os.path.join(cfg, 'c{class_id}', 'train'), 'mean_std_path': os.path.join(cfg, 'c{class_id}'),
+                 'ckpt_dir': os.path.join(cfg, 'c{class_id}', 'model_best_val.pth.tar'),
+                 'model_path': os.path.join(cfg, 'c{class_id}', 'textured.ply')}
+    return ycb, templates, classes
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--frames', type=int, default=100, help='frames per sequence')
+    ap.add_argument('--rounds', type=int, default=3)
+    ap.add_argument('--precision', default='bf16x3')
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit('needs a CUDA device')
+    pkg = importlib.import_module(PKG)
+    pr = importlib.import_module(PKG + '.predict')
+    gpu = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                         capture_output=True, text=True).stdout.strip().splitlines()
+    with tempfile.TemporaryDirectory() as tmp:
+        ycb, templates, classes = write_tree(tmp, args.frames, pkg.synth)
+        seq_frames = len(SEQS) * args.frames
+        obj_frames = sum(len(cls) for cls in SEQS.values()) * args.frames
+
+        def one_pass(r):
+            pr.getResultsYcbAll(ycb, classes, templates, os.path.join(tmp, 'all%d' % r), precision=args.precision)
+
+        def per_class(r):
+            for k in pr.ycb_all_classes(ycb, classes, templates, args.precision):
+                pr.getResultsYcb(ycb, k['class_id'], k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], k['model_path'],
+                                 os.path.join(tmp, 'pc%d' % r, k['name']), precision=args.precision, max_batch=1)
+
+        times = {'one_pass': [], 'per_class': []}
+        for r in range(args.rounds + 1):                             # round 0 warms both up and is not counted
+            for name, fn in (('one_pass', one_pass), ('per_class', per_class)):
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                fn(r)
+                torch.cuda.synchronize()
+                if r > 0:
+                    times[name].append(time.perf_counter() - t0)
+    out = {'gpu': gpu, 'torch_device': torch.cuda.get_device_name(0), 'precision': args.precision, 'sequences': len(SEQS),
+           'objects_per_sequence': [len(c) for c in SEQS.values()], 'frames_per_sequence': args.frames, 'rounds': args.rounds}
+    for name, ts in times.items():
+        out[name] = {'seconds': [round(t, 3) for t in ts],
+                     'frames_per_s': [round(seq_frames / t, 1) for t in ts],
+                     'object_frames_per_s': [round(obj_frames / t, 1) for t in ts]}
+        print('%-9s frames/s %s   objects x frames/s %s' % (name, out[name]['frames_per_s'], out[name]['object_frames_per_s']))
+    print('card (name, power limit, max SM clock): %s' % gpu)
+    print(json.dumps(out))
+
+
+if __name__ == '__main__':
+    main()
