@@ -5,6 +5,7 @@
 #include "aux_kernels.h"
 #include "conv_common.h"
 #include "bbox.cuh"
+#include "launch.h"
 #include "ptx.cuh"
 #include "storage.cuh"
 #include <cfloat>
@@ -166,25 +167,13 @@ preprocess_kernel(PreprocessArgs a, int rows_per_cta)
 }
 
 
-static cudaError_t launch_pdl(const void* func, dim3 grid, dim3 block, void** args, cudaStream_t s) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelExC(&cfg, func, args);
-}
-
 cudaError_t launch_preprocess(const PreprocessArgs& a, int n, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     // rows per CTA: big strips amortise the per-CTA tables, small ones fill the machine when there are few tracks
     int rows = n >= 64 ? 88 : (n >= 32 ? 22 : 11);
     dim3 grid(kImg / rows, n);
-    PreprocessArgs aa = a;
-    void* args[] = {&aa, &rows};
-    if (rows == 88) return launch_pdl(reinterpret_cast<const void*>(preprocess_kernel<1024>), grid, dim3(1024), args, s);
-    return launch_pdl(reinterpret_cast<const void*>(preprocess_kernel<256>), grid, dim3(256), args, s);
+    if (rows == 88) return launch_kernel(preprocess_kernel<1024>, grid, dim3(1024), 0, s, true, a, rows);
+    return launch_kernel(preprocess_kernel<256>, grid, dim3(256), 0, s, true, a, rows);
 }
 
 // =============================================================================================
@@ -496,9 +485,8 @@ cudaError_t launch_head_pooled(const float* part, const float* fcw, const float*
     if (n_img <= 0) return cudaSuccess;
     if (loss.poses_a && (!loss.poses_b || !loss.sq)) return cudaErrorInvalidValue;
     const float4* p4 = reinterpret_cast<const float4*>(part);
-    LossArgs la = loss;
-    void* args[] = {&p4, &fcw, &fcb, &out_trans, &out_rot, &npix, &img_wid, &fc_table, &poses_in, &poses_out, &tn, &rn, &la, &zero_words, &n_zero};
-    return launch_pdl(reinterpret_cast<const void*>(head_pooled_kernel), dim3(n_img), dim3(256), args, s);
+    return launch_kernel(head_pooled_kernel, dim3(n_img), dim3(256), 0, s, true, p4, fcw, fcb, out_trans, out_rot, npix, img_wid, fc_table,
+                         poses_in, poses_out, tn, rn, loss, zero_words, n_zero);
 }
 
 // =============================================================================================
@@ -580,8 +568,7 @@ cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, floa
                         int n_img, int npix, cudaStream_t s) {
     if (n_img <= 0) return cudaSuccess;
     const float4* x4 = reinterpret_cast<const float4*>(x);
-    void* args[] = {&x4, &fcw, &fcb, &out_trans, &out_rot, &npix};
-    return launch_pdl(reinterpret_cast<const void*>(head_kernel), dim3(n_img, 2), dim3(512), args, s);
+    return launch_kernel(head_kernel, dim3(n_img, 2), dim3(512), 0, s, true, x4, fcw, fcb, out_trans, out_rot, npix);
 }
 
 // =============================================================================================
@@ -726,8 +713,7 @@ __global__ void pose_update_kernel(const double* poses_in, const float* __restri
 cudaError_t launch_pose_update(const double* poses_in, const float* trans, const float* rot, float tn, float rn,
                                double* poses_out, int n, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
-    void* args[] = {&poses_in, &trans, &rot, &tn, &rn, &poses_out, &n};
-    return launch_pdl(reinterpret_cast<const void*>(pose_update_kernel), dim3((n + 31) / 32), dim3(32), args, s);
+    return launch_kernel(pose_update_kernel, dim3((n + 31) / 32), dim3(32), 0, s, true, poses_in, trans, rot, tn, rn, poses_out, n);
 }
 
 // =============================================================================================

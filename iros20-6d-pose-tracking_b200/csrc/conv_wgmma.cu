@@ -3,11 +3,9 @@
 //
 // Common to both kernels
 //   * M tile = an 11x11 pixel box of one image (121 of 128 rows; 44, 22 and 11 are multiples of 11), as two wgmma M = 64
-//     halves.  Ping-pong (both kernels): one consumer warpgroup owns both halves of a tile / work unit, the two warpgroups take
-//     alternate ones.  The resident kernel keeps the halves schedule (each consumer warpgroup one half of every tile) for
-//     launches where no CTA has a second tile.  Accumulators stay in registers.
-//   * A operand by TMA "units": one cp.async.bulk.tensor.4d per (128-byte channel chunk, filter COLUMN) whose box is
-//     two rows taller than the tile.  It lands as 143 rows x 128 B in the SWIZZLE_128B K-major layout wgmma reads, and
+//     halves.  Accumulators stay in registers.
+//   * A operand by TMA "units" (load_a_units): one cp.async.bulk.tensor.4d per (128-byte channel chunk, filter COLUMN) whose
+//     box is two rows taller than the tile.  It lands as 143 rows x 128 B in the SWIZZLE_128B K-major layout wgmma reads, and
 //     the three vertical taps of that column are the SAME tile read through descriptors whose start address is advanced
 //     by whole pixel rows (11 * 128 B; the swizzle is a function of absolute address bits) -- no data moves.
 //     Out-of-image coordinates are zero-filled by TMA = the conv padding.  Stride-2 convs: six units per chunk over four
@@ -15,8 +13,15 @@
 //     view; the 7 filter rows are row shifts 0/11/22/33.
 //   * warp roles (384 threads = 3 warpgroups): warp 0 activation TMA producer (+ work scheduler in the trunk kernel),
 //     warp 1 weight TMA producer, warps 2-3 idle; warpgroups 1 and 2 issue the MMAs and run the epilogue from registers.
-//     A consumer warpgroup keeps one MMA group in flight and hands an operand stage back once the group after it has been
-//     issued (wgmma.wait_group 1).
+//     Operands pass through mbarrier rings (Ring).  A consumer warpgroup keeps one MMA group in flight and hands an operand
+//     stage back once the group after it has been issued (wgmma.wait_group 1).
+//   * ping-pong (the trunk always, the resident kernel in launches with more tiles than SMs): consumer warpgroup g owns the
+//     CTA's tiles / work units it % 2 == g, both 64-row halves, and issues each MMA step once per half, in the same K order
+//     as with one warpgroup per half: bit-identical results.  The two take turns issuing MMAs (Turn): a warpgroup starts its
+//     tile's MMAs once the other has ISSUED all of its previous tile's, so one warpgroup's epilogue runs under the other's
+//     MMAs.  Both walk every operand ring; the one that does not own a tile steps its positions past the tile's stages.
+//   * registers: a whole-tile accumulator takes up to 128 registers per consumer thread; setmaxnreg moves them from the
+//     producer warpgroup (168 at launch -> 40) to the consumers (-> 232).
 //   * PREC (an SE3TN_PREC_* value) selects arithmetic and storage (storage.cuh): TF32 (4 x k8 tf32 MMAs per chunk-tap),
 //     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product).
 //   * programmatic dependent launch: every CTA signals launch_dependents at entry; only the threads that touch
@@ -31,23 +36,19 @@
 //   * in the bf16 hi/lo modes the weight halves are STACKED along N: rows [w_hi ; w_lo] -> one N = 128 MMA forms
 //     a_hi*w_hi and a_hi*w_lo, one N = 64 MMA adds a_lo*w_hi into the first half, the epilogue sums the two column halves
 //     (4 instead of 6 MMAs per chunk-tap; the stem's [w_hi|w_hi ; w_lo|0] rows give all three products in one N = 128 MMA
-//     per K step).
+//     per K step).  The accumulator is then 128 registers, otherwise 64.
 //   * 64-channel layers keep their weight ROWS permuted (column 8j + 2m + e of a 32-column block carries channel
 //     8m + 2j + e, se3tn.cu) so that in the wgmma accumulator fragment each thread owns 8 consecutive channels of a pixel:
 //     16-byte pieces, no staging.
 //   * stem: fused MaxPool2d(3,2,1): the M tile is the 11x11 block of conv outputs that feeds a 5x5 block of pooled
 //     outputs; max -> +bias -> SELU (monotone, so they commute) on 1/4.84 of the values; the 88x88x64 conv output never
 //     reaches HBM.  The fp32 sums are staged in shared memory for the 3x3 max.
-//   * ping-pong (launches with more tiles than SMs): consumer warpgroup g owns the tiles it % 2 == g of the CTA's range and
-//     issues each MMA step once per 64-row half into acc[2][kAcc], in the same K order as the halves schedule: bit-identical.
-//     A named-barrier pair passes the MMA turn as in the trunk; the warpgroup that does not own a tile steps its A ring
-//     position past the tile's chunks x NU stages (a_empty: one arrival).  Both warpgroups track the weight generation, and
-//     at a weight-set switch each arrives on b_empty once its own MMAs on the old weights have retired.  The stem's epilogue
-//     runs on the owning 128 threads (warpgroup-local named barriers); in bf16 / bf16x3 its one staging buffer (a second
-//     does not fit next to the resident weights) is handed between the warpgroups by a second named-barrier pair, in tf32
-//     warpgroup g keeps buffer g.  The stem's bias is loaded before the MMAs.
-//   * registers: the whole-tile accumulator is 128 registers (bf16x3, the stems' stacked bf16) or 64; setmaxnreg moves them
-//     from the producer warpgroup (168 at launch -> 40) to the consumers (-> 232), as in the trunk.  In the 64-channel bf16x3
+//   * PP = false: the halves schedule (each consumer warpgroup one half of every tile) for launches where no CTA has a
+//     second tile.  PP = true: ping-pong; an A stage then has one reader (a_empty: one arrival).  Both warpgroups track the
+//     weight generation, and at a weight-set switch each arrives on b_empty once its own MMAs on the old weights have
+//     retired.  The stem's epilogue runs on the owning 128 threads (warpgroup-local named barriers); in bf16 / bf16x3 its
+//     one staging buffer (a second does not fit next to the resident weights) passes between the warpgroups as a second
+//     Turn, in tf32 warpgroup g keeps buffer g.  The stem's bias is loaded before the MMAs.  In the 64-channel bf16x3
 //     layers the second half's residual loads wait until the first half's epilogue has freed its accumulator registers.
 //
 // conv_trunk_kernel<PREC>  (Cout >= 256: convAB1, convAB2.{conv1,conv2}, {trans,rot}_conv1, {trans,rot}_conv2.{conv1,conv2})
@@ -55,20 +56,15 @@
 //     SM pulls the next unit from a global counter (layer-major, image-major order) when its producer has issued the last
 //     loads of the current one, and a unit of layer l first waits until done[l-1][image] says that image's previous-layer
 //     output is complete (release/acquire at gpu scope; the waits point backwards in the pull order and all CTAs are
-//     co-resident, so the schedule cannot deadlock).
-//   * ping-pong: consumer warpgroup g owns every other unit the CTA pulls (both warpgroups walk the unit ring; the other
-//     one only steps its operand ring positions past the unit's stages).  A pair of named barriers passes the turn to issue
-//     MMAs: a warpgroup starts its unit's MMAs once the other has ISSUED all of its previous unit's, so one warpgroup's
-//     epilogue runs under the other's MMAs.  Each MMA step is issued once per 64-row half, in the same K order as with one
-//     warpgroup per half: bit-identical results.
-//   * registers: the 128 x 128 fp32 accumulator is 128 registers per consumer thread.  setmaxnreg moves them from the
-//     producer warpgroup (168 at launch -> 40) to the consumers (-> 232).
+//     co-resident, so the schedule cannot deadlock).  Every role walks the same ring of pulled units.
+//   * the 128 x 128 fp32 accumulator is 128 registers per consumer thread.
 //   * weights stream through a 6-stage ring of {32 words, 128 rows} tiles fed by their own producer warp.
 //   * epilogue: each warp post-processes 32 rows (a 16-row slice of each half, one after the other); every 16-row x 32-column
 //     accumulator block is transposed through a per-warp shared-memory tile so every global load / store instruction covers
 //     whole lines; the last layer reduces its 121 rows to per-slice column sums instead (AdaptiveAvgPool2d(1) fused; eight
 //     16-row slices, fixed order -> deterministic).
 #include "conv_common.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include "storage.cuh"
 #include <algorithm>
@@ -80,15 +76,14 @@ constexpr int kThreads2 = 384;                 // warpgroup 0: warp 0 A-TMA, war
 constexpr int kPoolPitch = 68;                 // floats per staged conv position (64 + 4: bank spread)
 constexpr int kPoolStageBytes = 121 * kPoolPitch * 4;
 constexpr int kPoolStageAlloc = (kPoolStageBytes + 1023) & ~1023;
-constexpr int kAUnit3 = 19 * 1024;             // 3x3: (22 + 128) rows * 128 B = 19,200
-constexpr int kAUnitStem = 21 * 1024;          // stem: (33 + 128) rows * 128 B = 20,608
 constexpr int kWgRowBytes = 64 * kChunkBytes;  // the second 64-row half of a tile starts 64 rows into an A unit
 
 // Compile-time unit / tap structure per conv kind, so the MMA issue loop is straight-line code with immediate row
-// shifts / weight-tile indices, and the TMA producer's box coordinates are immediates too.
+// shifts / weight-tile indices, and the TMA producer's box coordinates are immediates too.  kAUnit: bytes of an A ring stage.
 template <int KIND> struct KTab;
 template <> struct KTab<KIND_S1> {            // 3x3 stride 1: unit = filter column s, taps = filter rows r
     static constexpr int NU = 3;
+    static constexpr int kAUnit = 19 * 1024;   // (22 + 128) rows * 128 B = 19,200
     __host__ __device__ static constexpr int ntaps(int) { return 3; }
     __host__ __device__ static constexpr int wtap(int u, int k) { return k * 3 + u; }
     __host__ __device__ static constexpr int amap(int) { return 0; }
@@ -98,6 +93,7 @@ template <> struct KTab<KIND_S1> {            // 3x3 stride 1: unit = filter col
 };
 template <> struct KTab<KIND_S2> {            // 3x3 stride 2: per column s an even-row unit (r=1) and an odd-row unit (r=0,2)
     static constexpr int NU = 6;
+    static constexpr int kAUnit = 19 * 1024;   // as stride 1: the trunk's A ring serves both
     __host__ __device__ static constexpr int ntaps(int u) { return (u & 1) ? 2 : 1; }
     __host__ __device__ static constexpr int wtap(int u, int k) { return (u & 1) ? (k == 0 ? (u >> 1) : 6 + (u >> 1)) : 3 + (u >> 1); }
     // iy = 2*oy + dy: dy = -1 -> odd row oy-1; dy = 0 -> even row oy; dy = +1 -> odd row oy; columns likewise
@@ -108,6 +104,7 @@ template <> struct KTab<KIND_S2> {            // 3x3 stride 2: per column s an e
 };
 template <> struct KTab<KIND_STEM> {          // 7x7 stride 2 stem: even input rows (r=0,2,4,6), odd input rows (r=1,3,5)
     static constexpr int NU = 2;
+    static constexpr int kAUnit = 21 * 1024;   // (33 + 128) rows * 128 B = 20,608
     __host__ __device__ static constexpr int ntaps(int u) { return u == 0 ? 4 : 3; }
     __host__ __device__ static constexpr int wtap(int u, int k) { return 2 * k + u; }
     __host__ __device__ static constexpr int amap(int u) { return u; }
@@ -168,11 +165,68 @@ constexpr int kTurnBar = 1;                    // kTurnBar + g: consumer warpgro
 constexpr int kStageBar = 3;                   // kStageBar + g: consumer warpgroup g may write the stem's single staging buffer
 constexpr int kEpiBar = 5;                     // kEpiBar + g: the 128 threads of warpgroup g (halves schedule: kEpiBar, all 256)
 
-// move a ring position (stage, phase) on by n stages
-__device__ __forceinline__ void ring_skip(int& stage, uint32_t& phase, int n, int stages) {
-    stage += n;
-    phase ^= static_cast<uint32_t>(stage / stages) & 1u;
-    stage %= stages;
+// Position in a ring of N stages, each with a full and an empty mbarrier; phase flips at every wrap.  The producer waits on
+// empty[stage] with producer_parity() (its first pass goes straight through), a consumer on full[stage] with consumer_parity().
+// A consumer that leaves some stages to another consumer still moves its position past them (skip).
+template <int N> struct Ring {
+    uint32_t phase = 0;
+    int stage = 0;
+    __device__ __forceinline__ void next() { if (++stage == N) { stage = 0; phase ^= 1; } }
+    __device__ __forceinline__ void skip(int n) {
+        stage += n;
+        phase ^= static_cast<uint32_t>(stage / N) & 1u;
+        stage %= N;
+    }
+    __device__ __forceinline__ uint32_t producer_parity() const { return phase ^ 1; }
+    __device__ __forceinline__ uint32_t consumer_parity() const { return phase; }
+};
+
+// Turn-taking of the two consumer warpgroups on the named-barrier pair base + {0, 1}: barrier base + g gives warpgroup g the
+// turn.  A turn is one bar.arrive by the warpgroup that passes it and one bar.sync by the one that takes it.  Warpgroup 0 has
+// the first turn (begin).  After the last turn has been passed the warpgroup it went to takes it (end), so that neither
+// barrier is left with a pending arrival when the CTA exits.
+struct Turn {
+    int base, g;                               // barrier pair, this consumer warpgroup (0 or 1)
+    __device__ __forceinline__ void begin() const { if (g == 1) ptx::bar_arrive(base, 256); }
+    __device__ __forceinline__ void wait() const { ptx::bar_sync(base + g, 256); }
+    __device__ __forceinline__ void pass() const { ptx::bar_arrive(base + (g ^ 1), 256); }
+    __device__ __forceinline__ bool mine(int t) const { return (t & 1) == g; }           // turns alternate, from warpgroup 0
+    __device__ __forceinline__ void end(int turns) const { if (mine(turns)) wait(); }      // turns: number of turns passed so far
+};
+
+// TMA loads of a tile's A units (producer thread): chunks [c0, c1) x KT::NU filter-column units, one A ring stage each.
+// (ox, oy): the tile's box origin in A-map coordinates; cbase: first channel word of the conv group; img: the image.
+template <int KIND, int N>
+__device__ __forceinline__ void load_a_units(const LayerDesc& L, int ox, int oy, int cbase, int img, int c0, int c1,
+                                             uint8_t* sA, uint64_t* a_full, uint64_t* a_empty, Ring<N>& ring)
+{
+    using KT = KTab<KIND>;
+    for (int ch = c0; ch < c1; ++ch) {
+#pragma unroll
+        for (int u = 0; u < KT::NU; ++u) {
+            ptx::mbar_wait(&a_empty[ring.stage], ring.producer_parity());
+            ptx::mbar_arrive_expect_tx(&a_full[ring.stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
+            ptx::tma_load_4d(sA + ring.stage * KT::kAUnit, &L.amap[KT::amap(u)], &a_full[ring.stage],
+                             cbase + ch * 32, ox + KT::c1(u), oy + KT::c2(u), img);
+            ring.next();
+        }
+    }
+}
+
+// The MMAs of one 128-byte K chunk: four K steps of 32 bytes (tf32 k8 with PREC == SE3TN_PREC_TF32, bf16 k16 in the bf16
+// modes) at N = 64 or 128.  a_lo / b_lo: low descriptor words (+2 per K step).  fresh == 0: the first step overwrites acc.
+template <int PREC, int N>
+__device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t fresh) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t a = mk_desc(a_lo + 2 * kk), b = mk_desc(b_lo + 2 * kk);
+        const uint32_t f = fresh | (kk ? 1u : 0u);
+        if constexpr (PREC == SE3TN_PREC_TF32) {
+            if constexpr (N == 64) ptx::wgmma_tf32_n64(acc, a, b, f); else ptx::wgmma_tf32_n128(acc, a, b, f);
+        } else {
+            if constexpr (N == 64) ptx::wgmma_bf16_n64(acc, a, b, f); else ptx::wgmma_bf16_n128(acc, a, b, f);
+        }
+    }
 }
 
 // ================================================================================================================
@@ -184,12 +238,11 @@ template <int KIND, int PREC> struct RCfg {
     // STACK: hi / lo weight rows stacked along N (header comment) for layers whose input is in the bf16x3 format
     static constexpr int kStack = ((POOL ? stem_input_prec(PREC) : PREC) == SE3TN_PREC_BF16X3) ? 2 : 1;
     static constexpr int kBTile = BN * kStack * kChunkBytes;
-    static constexpr int kAUnit = POOL ? kAUnitStem : kAUnit3;
     static constexpr int kAStages = POOL ? (PREC == SE3TN_PREC_TF32 ? 4 : 3) : (PREC == SE3TN_PREC_BF16 ? 6 : 4);
     static constexpr int kPoolBufs = POOL ? (PREC == SE3TN_PREC_TF32 ? 2 : 1) : 0;
     static constexpr int kAcc = BN * kStack / 2;                    // accumulator registers per thread (N / 2)
     static constexpr int kMaxWTiles = POOL ? 7 : ((PREC == SE3TN_PREC_TF32) ? 18 : 9);
-    static constexpr int kSmem = kAStages * kAUnit + kMaxWTiles * kBTile + kPoolBufs * kPoolStageAlloc + 1024 + 512;
+    static constexpr int kSmem = kAStages * KTab<KIND>::kAUnit + kMaxWTiles * kBTile + kPoolBufs * kPoolStageAlloc + 1024 + 512;
     static_assert(kSmem <= 232448, "shared memory budget");
 };
 
@@ -208,14 +261,7 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
         uint32_t b_lo;
         if (C::kStack == 2) b_lo = desc_lo(sB + KT::wtap(u, k) * C::kBTile) + ch * 4;   // chunk ch sits 64 bytes (4 x 16 B) further along K
         else                b_lo = desc_lo(sB + (KT::wtap(u, k) * tiles_per_tap + ch) * C::kBTile);
-        if constexpr (PREC == SE3TN_PREC_TF32) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) ptx::wgmma_tf32_n64(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
-        } else if constexpr (C::POOL) {
-            // stem window = 8 pixels x [hi4|lo4] against rows [w_hi|w_hi ; w_lo|0]: all three products in one N = 128 MMA per K step
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) ptx::wgmma_bf16_n128(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
-        } else if constexpr (C::kStack == 2) {
+        if constexpr (C::kStack == 2 && !C::POOL) {
             // chunk = [32 hi | 32 lo] (A); weight rows [w_hi ; w_lo]: a_hi x both (N = 128), then a_lo x w_hi (N = 64, columns 0-63)
 #pragma unroll
             for (int sl = 0; sl < 2; ++sl) {
@@ -223,9 +269,9 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
                 ptx::wgmma_bf16_n64(acc_lo32(acc), mk_desc(a_lo + 4 + 2 * sl), mk_desc(b_lo + 2 * sl), 1u);
             }
         } else {
-            // SE3TN_PREC_BF16: chunk = 64 bf16 channels: four K = 16 steps
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) ptx::wgmma_bf16_n64(acc, mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
+            // tf32, bf16, and the stem's bf16 modes: window = 8 pixels x [hi4|lo4] against rows [w_hi|w_hi ; w_lo|0], all three
+            // products in one N = 128 MMA per K step
+            mma_chunk<PREC, C::BN * C::kStack>(acc, a_lo, b_lo, fresh);
         }
         fresh = 1u;
     }
@@ -249,7 +295,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
     // K tiles of the resident weight matrix: STACK keeps all chunks of a tap in one 128-row tile, otherwise one tile per (tap, chunk)
     const int tiles_per_tap = (C::kStack == 2) ? 1 : chunks;
     uint8_t* sA = smem;                                                 // [kAStages][unit]
-    uint8_t* sB = sA + C::kAStages * C::kAUnit;                         // [num_taps * tiles_per_tap][BN*kStack rows x 128 B]
+    uint8_t* sB = sA + C::kAStages * KT::kAUnit;                        // [num_taps * tiles_per_tap][BN*kStack rows x 128 B]
     uint8_t* sP = sB + C::kMaxWTiles * C::kBTile;                       // pool staging (stem only)
     uint64_t* bars = reinterpret_cast<uint64_t*>(sP + C::kPoolBufs * kPoolStageAlloc);
     uint64_t* a_full = bars;                       // [kAStages]
@@ -285,21 +331,11 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
             // ============================== A producer ================================
             if (lane == 0) {
                 ptx::grid_dep_wait();                   // activations come from the previous kernel
-                int stage = 0; uint32_t phase = 0;
+                Ring<C::kAStages> ring;
                 for (int tile = w_begin; tile < w_end; ++tile) {
                     const int n0 = img_of(tile), r = tile % tiles_img;
                     const int ty = r / L.tiles_x, tx = r - ty * L.tiles_x;
-                    const int ox = tx * p.step_x + p.off_x, oy = ty * p.step_y + p.off_y;
-                    for (int ch = 0; ch < chunks; ++ch) {
-#pragma unroll
-                        for (int u = 0; u < KT::NU; ++u) {
-                            ptx::mbar_wait(&a_empty[stage], phase ^ 1);
-                            ptx::mbar_arrive_expect_tx(&a_full[stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
-                            ptx::tma_load_4d(sA + stage * C::kAUnit, &L.amap[KT::amap(u)], &a_full[stage],
-                                             ch * 32, ox + KT::c1(u), oy + KT::c2(u), n0);
-                            if (++stage == C::kAStages) { stage = 0; phase ^= 1; }
-                        }
-                    }
+                    load_a_units<KIND>(L, tx * p.step_x + p.off_x, ty * p.step_y + p.off_y, 0, n0, 0, chunks, sA, a_full, a_empty, ring);
                 }
             }
         } else if (warp == 1) {
@@ -336,23 +372,24 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
         constexpr int kEpiThreads = PP ? 128 : 256;                 // threads that run one tile's epilogue
         const int et = PP ? (cs.ct & 127) : cs.ct;                  // this thread's index among them
         auto half_of = [&](int hf) { return PP ? hf : cs.cg; };     // 64-row half of the tile in accumulator acc[hf]
-        int astage = 0; uint32_t aphase = 0;
+        Ring<C::kAStages> a_ring;
         int w_cur = -2; uint32_t w_gen = 0;        // weight set currently in shared memory
+        const Turn turn{kTurnBar, cs.cg}, stage_turn{kStageBar, cs.cg};   // one turn per tile of the CTA (PP)
         if constexpr (PP) {
-            // the first MMA turn (and the stem's staging buffer) is warpgroup 0's
-            if (cs.cg == 1) { ptx::bar_arrive(kTurnBar, 256); if constexpr (kShareStage) ptx::bar_arrive(kStageBar, 256); }
+            turn.begin();
+            if constexpr (kShareStage) stage_turn.begin();
         }
         int it = 0;
         for (int tile = w_begin; tile < w_end; ++tile, ++it) {
             const int wid = wid_of(tile);
             const bool new_w = (wid != w_cur);     // wait for each unit's weights at its first use below
             const bool w_last = tile + 1 < w_end && wid_of(tile + 1) != wid;   // the loader replaces these weights after this tile
-            if (PP && (it & 1) != cs.cg) {
+            if (PP && !turn.mine(it)) {
                 // the other warpgroup's tile: step this warpgroup's A ring position past its stages.  Keep the weight generation
                 // in step, and take part in the hand-back of the weights as below: this warpgroup's MMAs on them retired with its
                 // previous tile.  Waiting for a new generation first keeps this warpgroup's arrival for the next switch after
                 // the loader has seen both arrivals for this one.
-                ring_skip(astage, aphase, chunks * KT::NU, C::kAStages);
+                a_ring.skip(chunks * KT::NU);
                 if (new_w) {
 #pragma unroll
                     for (int u = 0; u < KT::NU; ++u) ptx::mbar_wait(&b_full[u], w_gen & 1);
@@ -404,7 +441,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
             for (int hf = 0; hf < NH; ++hf)
 #pragma unroll
                 for (int i = 0; i < C::kAcc; ++i) acc[hf][i] = 0.f;
-            if constexpr (PP) ptx::bar_sync(kTurnBar + cs.cg, 256);    // the other warpgroup has issued all MMAs of its previous tile
+            if constexpr (PP) turn.wait();          // the other warpgroup has issued all MMAs of its previous tile
             uint32_t fresh = 0;                     // 0 until the first MMA of this tile has been issued
             int pend = -1;                          // A stage of the previous MMA group, released once that group has completed
             for (int ch = 0; ch < chunks; ++ch) {
@@ -414,14 +451,14 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                         ptx::mbar_wait(&b_full[u], w_gen & 1);
                         if (it == 0 && u == 0 && stamp) trace_stamp(p.trace, 2);
                     }
-                    ptx::mbar_wait(&a_full[astage], aphase);
+                    ptx::mbar_wait(&a_full[a_ring.stage], a_ring.consumer_parity());
                     if (ch == 0 && u == 0) {
                         if (it == 0 && stamp) trace_stamp(p.trace, 3);
                         if (tstamp) tile_stamp(p.tile_trace, tile, 0);
                     }
                     ptx::wgmma_fence();
                     // each MMA step once per 64-row half, every half's accumulator in the same K order
-                    const uint32_t a_unit_lo = desc_lo(sA + astage * C::kAUnit);
+                    const uint32_t a_unit_lo = desc_lo(sA + a_ring.stage * KT::kAUnit);
 #pragma unroll
                     for (int hf = 0; hf < NH; ++hf) {
                         uint32_t f = fresh;
@@ -431,11 +468,11 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                     ptx::wgmma_commit();
                     ptx::wgmma_wait<1>();
                     if (pend >= 0 && cs.leader()) ptx::mbar_arrive(&a_empty[pend]);
-                    pend = astage;
-                    if (++astage == C::kAStages) { astage = 0; aphase ^= 1; }
+                    pend = a_ring.stage;
+                    a_ring.next();
                 }
             }
-            if constexpr (PP) ptx::bar_arrive(kTurnBar + (cs.cg ^ 1), 256);   // all of this tile's MMAs are issued: the other's turn
+            if constexpr (PP) turn.pass();          // all of this tile's MMAs are issued
             ptx::wgmma_wait<0>();
 #pragma unroll
             for (int hf = 0; hf < NH; ++hf) ptx::wgmma_reg_fence(acc[hf]);
@@ -490,10 +527,10 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                 }
             } else {
                 // ---- stem: conv tile 11x11 -> 5x5 max-pooled outputs (MaxPool2d(3,2,1), -inf padding) ----
-                // Ping-pong: with one staging buffer the two warpgroups' epilogues take turns on it (kStageBar); with two, tile
+                // Ping-pong: with one staging buffer the two warpgroups' epilogues take turns on it (stage_turn); with two, tile
                 // it % 2 == g always uses buffer g, and this warpgroup's readers of two tiles ago must be done before it writes.
                 float* stage = reinterpret_cast<float*>(sP + (C::kPoolBufs == 2 ? (it & 1) : 0) * kPoolStageAlloc);
-                if constexpr (kShareStage) ptx::bar_sync(kStageBar + cs.cg, 256);
+                if constexpr (kShareStage) stage_turn.wait();
                 else if constexpr (PP) ptx::bar_sync(kEpiBar + cs.cg, 128);
 #pragma unroll
                 for (int hf = 0; hf < NH; ++hf)
@@ -532,15 +569,14 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                     const float v4[4] = {selu_fast(mx.x + pb4.x), selu_fast(mx.y + pb4.y), selu_fast(mx.z + pb4.z), selu_fast(mx.w + pb4.w)};
                     S::encode(v4).store(L.out + S::addr((static_cast<size_t>(n0) * L.Ho + oy) * L.Wo + ox, L.out_c, L.out_coff + c4));
                 }
-                if constexpr (kShareStage) ptx::bar_arrive(kStageBar + (cs.cg ^ 1), 256);   // this warpgroup's readers are done
+                if constexpr (kShareStage) stage_turn.pass();   // this warpgroup's readers are done
                 else if constexpr (!PP) { if (C::kPoolBufs == 1) ptx::bar_sync(kEpiBar, 256); }   // readers done before the next tile writes
             }
             if (tstamp) tile_stamp(p.tile_trace, tile, 3);
         }
         if constexpr (PP) {
-            // no tile left to pass the turn (and the staging buffer) on to: the warpgroup whose turn it is takes it, so the named
-            // barriers end balanced
-            if ((it & 1) == cs.cg) { ptx::bar_sync(kTurnBar + cs.cg, 256); if constexpr (kShareStage) ptx::bar_sync(kStageBar + cs.cg, 256); }
+            turn.end(it);
+            if constexpr (kShareStage) stage_turn.end(it);
         }
         if (stamp) { trace_stamp(p.trace, 4); trace_stamp(p.trace, 6); }
     }
@@ -562,7 +598,9 @@ template <int PREC> struct TCfg {
     static constexpr int kEpiWarpBytes = 16 * kEpiPitch * 4 + 128;      // 16 rows + 32-entry pixel-index table
     static constexpr int kEpiBytes = 8 * kEpiWarpBytes;
     static constexpr int kSched = 4;                                    // work-unit ring between the scheduler (A producer) and the other roles
-    static constexpr int kSmem = kAStages * kAUnit3 + kBStages * kBTile + ((kEpiBytes + 1023) & ~1023) + 1024 + 512;
+    static constexpr int kAUnit = KTab<KIND_S1>::kAUnit;               // one A ring for both 3x3 kinds
+    static_assert(kAUnit == KTab<KIND_S2>::kAUnit, "A ring stage size");
+    static constexpr int kSmem = kAStages * kAUnit + kBStages * kBTile + ((kEpiBytes + 1023) & ~1023) + 1024 + 512;
     static_assert(kSmem <= 232448, "shared memory budget");
 };
 constexpr int kTaps3 = 9;                      // weight tiles per K chunk of a 3x3 conv (one per filter tap, both strides)
@@ -603,29 +641,10 @@ __device__ __forceinline__ UnitCoord decode_unit(const TrunkParams& p, int u) {
     return c;
 }
 
-// activation loads of one work unit (A producer thread)
-template <int KIND>
-__device__ __forceinline__ void trunk_load_unit(const LayerDesc& L, const UnitCoord& c, uint8_t* sA, uint64_t* a_full, uint64_t* a_empty,
-                                                int& stage, uint32_t& phase, int n_stages)
-{
-    using KT = KTab<KIND>;
-    const int cbase = c.grp * L.in_gstride_words;
-    const int ox = c.tx * 11, oy = c.ty * 11;
-    for (int ch = c.c0; ch < c.c1; ++ch) {
-#pragma unroll
-        for (int u = 0; u < KT::NU; ++u) {
-            ptx::mbar_wait(&a_empty[stage], phase ^ 1);
-            ptx::mbar_arrive_expect_tx(&a_full[stage], static_cast<uint32_t>(KT::rows(u)) * kChunkBytes);
-            ptx::tma_load_4d(sA + stage * kAUnit3, &L.amap[KT::amap(u)], &a_full[stage], cbase + ch * 32, ox + KT::c1(u), oy + KT::c2(u), c.img);
-            if (++stage == n_stages) { stage = 0; phase ^= 1; }
-        }
-    }
-}
-
 // weight-tile loads of one work unit (B producer thread)
 template <int KIND, int PREC>
 __device__ __forceinline__ void trunk_load_weights(const LayerDesc& L, const CUtensorMap* bm, const UnitCoord& c, uint8_t* sB,
-                                                   uint64_t* b_full, uint64_t* b_empty, int& stage, uint32_t& phase)
+                                                   uint64_t* b_full, uint64_t* b_empty, Ring<TCfg<PREC>::kBStages>& ring)
 {
     using KT = KTab<KIND>;
     using C = TCfg<PREC>;
@@ -635,24 +654,22 @@ __device__ __forceinline__ void trunk_load_weights(const LayerDesc& L, const CUt
         for (int u = 0; u < KT::NU; ++u) {
 #pragma unroll
             for (int k = 0; k < KT::ntaps(u); ++k) {
-                ptx::mbar_wait(&b_empty[stage], phase ^ 1);
-                ptx::mbar_arrive_expect_tx(&b_full[stage], C::kBTile);
-                ptx::tma_load_2d(sB + stage * C::kBTile, bm, &b_full[stage], KT::wtap(u, k) * L.cin_words + ch * 32, wrow);
-                if (++stage == C::kBStages) { stage = 0; phase ^= 1; }
+                ptx::mbar_wait(&b_empty[ring.stage], ring.producer_parity());
+                ptx::mbar_arrive_expect_tx(&b_full[ring.stage], C::kBTile);
+                ptx::tma_load_2d(sB + ring.stage * C::kBTile, bm, &b_full[ring.stage], KT::wtap(u, k) * L.cin_words + ch * 32, wrow);
+                ring.next();
             }
         }
     }
 }
 
 // MMAs of one work unit (one consumer warpgroup, all 128 rows: each MMA step is issued once per 64-row half, into that half's
-// accumulator).  The warpgroup first waits for its turn: the other consumer warpgroup has issued every MMA of the CTA's previous
-// unit; once this unit's last MMA is issued it passes the turn back, and its MMAs run while the other warpgroup's epilogue does.
-// One MMA group per weight tile; a group's weight stage (and, after the last tap of a filter column, its A stage) is handed back
-// once the next group has been issued and the group has completed.
+// accumulator), issued in the warpgroup's turn.  One MMA group per weight tile; a group's weight stage (and, after the last tap
+// of a filter column, its A stage) is handed back once the next group has been issued and the group has completed.
 template <int KIND, int PREC>
-__device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc], const Consumer& cs, int chunks, uint8_t* sA, uint8_t* sB,
-                                               uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty,
-                                               int& astage, uint32_t& aphase, int& bstage, uint32_t& bphase,
+__device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc], const Consumer& cs, const Turn& turn, int chunks,
+                                               uint8_t* sA, uint8_t* sB, uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full,
+                                               uint64_t* b_empty, Ring<TCfg<PREC>::kAStages>& a_ring, Ring<TCfg<PREC>::kBStages>& b_ring,
                                                unsigned long long* trace, bool first_unit, unsigned long long* ustamp)
 {
     using KT = KTab<KIND>;
@@ -660,28 +677,24 @@ __device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc]
     const bool stamp = cs.leader();
     uint32_t fresh = 0;
     int pend_b = -1, pend_a = -1;
-    ptx::bar_sync(kTurnBar + cs.cg, 256);
+    turn.wait();
     for (int ch = 0; ch < chunks; ++ch) {
 #pragma unroll
         for (int u = 0; u < KT::NU; ++u) {
-            ptx::mbar_wait(&a_full[astage], aphase);
+            ptx::mbar_wait(&a_full[a_ring.stage], a_ring.consumer_parity());
             if (first_unit && ch == 0 && u == 0 && stamp) trace_stamp(trace, 3);
             if (ustamp && ch == 0 && u == 0 && stamp) *ustamp = gtimer();
-            const uint32_t a_unit_lo = desc_lo(sA + astage * kAUnit3);
+            const uint32_t a_unit_lo = desc_lo(sA + a_ring.stage * C::kAUnit);
 #pragma unroll
             for (int k = 0; k < KT::ntaps(u); ++k) {
-                ptx::mbar_wait(&b_full[bstage], bphase);
+                ptx::mbar_wait(&b_full[b_ring.stage], b_ring.consumer_parity());
                 if (first_unit && ch == 0 && u == 0 && k == 0 && stamp) trace_stamp(trace, 2);
-                const uint32_t b_lo = desc_lo(sB + bstage * C::kBTile);
+                const uint32_t b_lo = desc_lo(sB + b_ring.stage * C::kBTile);
                 ptx::wgmma_fence();
 #pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
                     const uint32_t a_lo = a_unit_lo + hf * (kWgRowBytes >> 4) + k * kRowShift * (kChunkBytes >> 4);
-                    if constexpr (PREC == SE3TN_PREC_TF32) {
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)
-                            ptx::wgmma_tf32_n128(acc[hf], mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
-                    } else if constexpr (PREC == SE3TN_PREC_BF16X3) {
+                    if constexpr (PREC == SE3TN_PREC_BF16X3) {
                         // chunk = [32 hi | 32 lo] bf16 (A) x [32 w_hi | 32 w_lo] (B); offsets in 16-byte units
                         constexpr int AO[6] = {0, 2, 4, 6, 0, 2};      // hi, hi, lo, lo, hi, hi
                         constexpr int BO[6] = {0, 2, 0, 2, 4, 6};      // w_hi x4,        w_lo x2
@@ -689,9 +702,7 @@ __device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc]
                         for (int i = 0; i < 6; ++i)
                             ptx::wgmma_bf16_n128(acc[hf], mk_desc(a_lo + AO[i]), mk_desc(b_lo + BO[i]), fresh | (i ? 1u : 0u));
                     } else {
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)
-                            ptx::wgmma_bf16_n128(acc[hf], mk_desc(a_lo + 2 * kk), mk_desc(b_lo + 2 * kk), fresh | (kk ? 1u : 0u));
+                        mma_chunk<PREC, C::BN>(acc[hf], a_lo, b_lo, fresh);
                     }
                 }
                 ptx::wgmma_commit();
@@ -700,15 +711,15 @@ __device__ __forceinline__ void trunk_mma_unit(float (&acc)[2][TCfg<PREC>::kAcc]
                     if (pend_b >= 0) ptx::mbar_arrive(&b_empty[pend_b]);
                     if (pend_a >= 0) ptx::mbar_arrive(&a_empty[pend_a]);
                 }
-                pend_b = bstage;
-                pend_a = (k + 1 == KT::ntaps(u)) ? astage : -1;
+                pend_b = b_ring.stage;
+                pend_a = (k + 1 == KT::ntaps(u)) ? a_ring.stage : -1;
                 fresh = 1u;
-                if (++bstage == C::kBStages) { bstage = 0; bphase ^= 1; }
+                b_ring.next();
             }
-            if (++astage == C::kAStages) { astage = 0; aphase ^= 1; }
+            a_ring.next();
         }
     }
-    ptx::bar_arrive(kTurnBar + (cs.cg ^ 1), 256);
+    turn.pass();
     ptx::wgmma_wait<0>();
     ptx::wgmma_reg_fence(acc[0]);
     ptx::wgmma_reg_fence(acc[1]);
@@ -727,7 +738,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;                                                 // [kAStages][unit]
-    uint8_t* sB = sA + C::kAStages * kAUnit3;                           // [kBStages][128 rows x 128 B]
+    uint8_t* sB = sA + C::kAStages * C::kAUnit;                         // [kBStages][128 rows x 128 B]
     uint8_t* sT = sB + C::kBStages * C::kBTile;                         // epilogue transpose tiles
     uint64_t* bars = reinterpret_cast<uint64_t*>(sT + ((C::kEpiBytes + 1023) & ~1023));
     uint64_t* a_full = bars;                       // [kAStages]
@@ -756,14 +767,14 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
     if (threadIdx.x == 0) trace_stamp(p.trace, 1);
 
     // every consumer role walks the same ring of work units
-    int sslot = 0; uint32_t sphase = 0;
+    Ring<C::kSched> sring;
     auto next_unit = [&](bool whole_warp) -> int {  // a consumer role's next work unit: called by a whole warp, or by lane 0 alone
-        ptx::mbar_wait(&sched_full[sslot], sphase);
+        ptx::mbar_wait(&sched_full[sring.stage], sring.consumer_parity());
         int u = 0;
-        if (lane == 0) u = sched_slot[sslot];       // read by the one thread that hands the slot back (a direct mbarrier edge to the writer)
+        if (lane == 0) u = sched_slot[sring.stage];   // read by the one thread that hands the slot back (a direct mbarrier edge to the writer)
         if (whole_warp) u = __shfl_sync(0xffffffffu, u, 0);
-        if (lane == 0) ptx::mbar_arrive(&sched_empty[sslot]);
-        if (++sslot == C::kSched) { sslot = 0; sphase ^= 1; }
+        if (lane == 0) ptx::mbar_arrive(&sched_empty[sring.stage]);
+        sring.next();
         return u;
     };
 
@@ -775,18 +786,18 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                 for (int l = 0; l < p.n_layers; ++l)    // every layer brings its own tensor maps: fetch the descriptors now, not at each layer's first load
                     for (int m = 0; m < (p.layer[l].kind == KIND_S2 ? 4 : 1); ++m) ptx::prefetch_tmap(&p.layer[l].amap[m]);
                 ptx::grid_dep_wait();                   // the first layer's input comes from the previous kernel
-                int stage = 0; uint32_t phase = 0;
-                int ps = 0; uint32_t pph = 0;
+                Ring<C::kAStages> a_ring;
+                Ring<C::kSched> slot;
                 // latency mode: the pieces of a unit (consecutive indices) must sit on DIFFERENT CTAs, because a piece's epilogue waits for
                 // the others' partial sums -- units are dealt round robin (index i goes to CTA i mod grid; every wait then points at a
                 // smaller index or at a piece whose CTA only has smaller indices left to finish: no cycle).  Throughput mode: first come, first served.
                 const bool dealt = p.ksplit > 1;
                 int u = dealt ? static_cast<int>(blockIdx.x) : static_cast<int>(atomicAdd(p.sched, 1u));
                 for (;;) {
-                    ptx::mbar_wait(&sched_empty[ps], pph ^ 1);
-                    sched_slot[ps] = u;
-                    ptx::mbar_arrive(&sched_full[ps]);  // release: the slot write is visible to the waiters
-                    if (++ps == C::kSched) { ps = 0; pph ^= 1; }
+                    ptx::mbar_wait(&sched_empty[slot.stage], slot.producer_parity());
+                    sched_slot[slot.stage] = u;
+                    ptx::mbar_arrive(&sched_full[slot.stage]);  // release: the slot write is visible to the waiters
+                    slot.next();
                     if (u >= p.total_units) break;
                     const UnitCoord c = decode_unit(p, u);
                     const LayerDesc& L = p.layer[c.l];
@@ -803,8 +814,9 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                         ptx::fence_proxy_async_all();   // the TMA (async proxy) reads below must observe what the acquire made visible
                     }
                     unit_stamp(p, u, 0);
-                    if (L.kind == KIND_S1) trunk_load_unit<KIND_S1>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
-                    else                   trunk_load_unit<KIND_S2>(L, c, sA, a_full, a_empty, stage, phase, C::kAStages);
+                    const int cbase = c.grp * L.in_gstride_words;
+                    if (L.kind == KIND_S1) load_a_units<KIND_S1>(L, c.tx * 11, c.ty * 11, cbase, c.img, c.c0, c.c1, sA, a_full, a_empty, a_ring);
+                    else                   load_a_units<KIND_S2>(L, c.tx * 11, c.ty * 11, cbase, c.img, c.c0, c.c1, sA, a_full, a_empty, a_ring);
                     u = dealt ? u + static_cast<int>(gridDim.x) : static_cast<int>(atomicAdd(p.sched, 1u));   // pull the next unit only now: look-ahead = the A pipeline depth
                 }
             }
@@ -812,15 +824,15 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
             // ============================== B producer ================================
             if (lane == 0) {
                 if (!p.img_wid) for (int l = 0; l < p.n_layers; ++l) ptx::prefetch_tmap(&p.layer[l].bmap);
-                int stage = 0; uint32_t phase = 0;
+                Ring<C::kBStages> b_ring;
                 for (;;) {
                     const int u = next_unit(false);
                     if (u >= p.total_units) break;
                     const UnitCoord c = decode_unit(p, u);
                     const LayerDesc& L = p.layer[c.l];
                     const CUtensorMap* bm = p.img_wid ? p.gbmaps + p.img_wid[c.img] * kLayersPerSet + L.li : &L.bmap;
-                    if (L.kind == KIND_S1) trunk_load_weights<KIND_S1, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
-                    else                   trunk_load_weights<KIND_S2, PREC>(L, bm, c, sB, b_full, b_empty, stage, phase);
+                    if (L.kind == KIND_S1) trunk_load_weights<KIND_S1, PREC>(L, bm, c, sB, b_full, b_empty, b_ring);
+                    else                   trunk_load_weights<KIND_S2, PREC>(L, bm, c, sB, b_full, b_empty, b_ring);
                 }
             }
         }
@@ -835,26 +847,22 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
         float (*stg)[C::kEpiPitch] = reinterpret_cast<float (*)[C::kEpiPitch]>(sT + cs.ew * C::kEpiWarpBytes);
         int* rowtab = reinterpret_cast<int*>(sT + cs.ew * C::kEpiWarpBytes + 16 * C::kEpiPitch * 4);
         const int grp = lane & 7, sub = lane >> 3;  // lane = (16-byte column group, pixel within a group of 4)
-        int astage = 0; uint32_t aphase = 0;
-        int bstage = 0; uint32_t bphase = 0;
-        // Ping-pong: warpgroup it % 2 owns the CTA's it-th unit, and the two take turns issuing MMAs (trunk_mma_unit), so one
-        // warpgroup's epilogue runs under the other's MMAs.  The first turn is warpgroup 0's.
-        if (cs.cg == 1) ptx::bar_arrive(kTurnBar, 256);
+        Ring<C::kAStages> a_ring;
+        Ring<C::kBStages> b_ring;
+        // Ping-pong: warpgroup it % 2 owns the CTA's it-th unit and issues its MMAs in turn it.
+        const Turn turn{kTurnBar, cs.cg};
+        turn.begin();
         for (int it = 0;; ++it) {
             const int u = next_unit(true);
-            const bool mine = (it & 1) == cs.cg;
-            if (u >= p.total_units) {
-                // no unit left to pass the turn on to: the warpgroup whose turn it is takes it, so both barriers end balanced
-                if (mine) ptx::bar_sync(kTurnBar + cs.cg, 256);
-                break;
-            }
+            const bool mine = turn.mine(it);
+            if (u >= p.total_units) { turn.end(it); break; }
             const UnitCoord c = decode_unit(p, u);
             const LayerDesc& L = p.layer[c.l];
             const int chunks = L.chunks / p.ksplit;          // K chunks of this piece (the host makes chunks divisible)
             if (!mine) {
                 // the other warpgroup's unit: step this warpgroup's operand ring positions past the stages it occupies
-                ring_skip(astage, aphase, chunks * (L.kind == KIND_S1 ? KTab<KIND_S1>::NU : KTab<KIND_S2>::NU), C::kAStages);
-                ring_skip(bstage, bphase, chunks * kTaps3, C::kBStages);
+                a_ring.skip(chunks * (L.kind == KIND_S1 ? KTab<KIND_S1>::NU : KTab<KIND_S2>::NU));
+                b_ring.skip(chunks * kTaps3);
                 continue;
             }
             {
@@ -877,8 +885,8 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
 #pragma unroll
             for (int i = 0; i < C::kAcc; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
             unsigned long long* ust = (p.trace && u < 2048) ? p.trace + 256 * 8 + u * 5 + 1 : nullptr;
-            if (L.kind == KIND_S1) trunk_mma_unit<KIND_S1, PREC>(acc, cs, chunks, sA, sB, a_full, a_empty, b_full, b_empty, astage, aphase, bstage, bphase, p.trace, it == 0, ust);
-            else                   trunk_mma_unit<KIND_S2, PREC>(acc, cs, chunks, sA, sB, a_full, a_empty, b_full, b_empty, astage, aphase, bstage, bphase, p.trace, it == 0, ust);
+            if (L.kind == KIND_S1) trunk_mma_unit<KIND_S1, PREC>(acc, cs, turn, chunks, sA, sB, a_full, a_empty, b_full, b_empty, a_ring, b_ring, p.trace, it == 0, ust);
+            else                   trunk_mma_unit<KIND_S2, PREC>(acc, cs, turn, chunks, sA, sB, a_full, a_empty, b_full, b_empty, a_ring, b_ring, p.trace, it == 0, ust);
             if (cs.leader()) { unit_stamp(p, u, 2); unit_stamp(p, u, 3); if (it == 0) trace_stamp(p.trace, 5); }
             int pix[2][4];                                       // pixels this lane post-processes: rows 4k + sub of each 16-row slice
 #pragma unroll
@@ -1027,18 +1035,6 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-template <typename K>
-cudaError_t set_smem(K kernel, size_t smem, size_t* cache) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    if (smem > cache[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-        if (e != cudaSuccess) return e;
-        cache[dev] = smem;
-    }
-    return cudaSuccess;
-}
-
 template <int KIND, int PREC>
 cudaError_t launch_resident_t(const ResidentParams& p, int num_sms, bool pdl, cudaStream_t stream) {
     using C = RCfg<KIND, PREC>;
@@ -1049,16 +1045,11 @@ cudaError_t launch_resident_t(const ResidentParams& p, int num_sms, bool pdl, cu
     // Ping-pong only where some CTA has a second tile whose MMAs can run under its first tile's epilogue.  Where every CTA has
     // one tile (n = 1: 81 stem tiles, 16 per 64-channel layer), the halves schedule runs that one epilogue on twice the threads.
     const bool pp = p.m_tiles > num_sms;
-    void (*kernel)(ResidentParams) = pp ? conv_resident_kernel<KIND, PREC, true> : conv_resident_kernel<KIND, PREC, false>;
-    static size_t attr[2][64] = {};                // the dynamic shared-memory limit is a per-device function attribute
-    cudaError_t e = set_smem(kernel, C::kSmem, attr[pp]);
+    const cudaError_t e = pp ? set_max_dynamic_smem<conv_resident_kernel<KIND, PREC, true>>(C::kSmem)
+                             : set_max_dynamic_smem<conv_resident_kernel<KIND, PREC, false>>(C::kSmem);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(std::min(p.m_tiles, num_sms)); cfg.blockDim = dim3(kThreads2); cfg.dynamicSmemBytes = C::kSmem; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, p);
+    return launch_kernel(pp ? conv_resident_kernel<KIND, PREC, true> : conv_resident_kernel<KIND, PREC, false>,
+                         dim3(std::min(p.m_tiles, num_sms)), dim3(kThreads2), C::kSmem, stream, pdl, p);
 }
 
 template <int PREC>
@@ -1073,16 +1064,10 @@ cudaError_t launch_trunk_t(const TrunkParams& p, int num_sms, bool pdl, cudaStre
         if (L.dep_layer >= l) return cudaErrorInvalidValue;                                    // dependencies point backwards in the pull order
         if (L.chunks % p.ksplit) return cudaErrorInvalidValue;
     }
-    static size_t attr[64] = {};
-    cudaError_t e = set_smem(conv_trunk_kernel<PREC>, C::kSmem, attr);
+    const cudaError_t e = set_max_dynamic_smem<conv_trunk_kernel<PREC>>(C::kSmem);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
     // all CTAs must be co-resident (one per SM): the dependency waits rely on it
-    cfg.gridDim = dim3(std::min(p.total_units, num_sms)); cfg.blockDim = dim3(kThreads2); cfg.dynamicSmemBytes = C::kSmem; cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, conv_trunk_kernel<PREC>, p);
+    return launch_kernel(conv_trunk_kernel<PREC>, dim3(std::min(p.total_units, num_sms)), dim3(kThreads2), C::kSmem, stream, pdl, p);
 }
 
 }  // namespace

@@ -28,6 +28,7 @@
 // homogeneous path below (straddler_*), which yields the fragments GL's polygon clipping would.  Scope limit: float32 depth buffer.
 #include "render.h"
 #include "bbox.cuh"
+#include "launch.h"
 #include "ptx.cuh"
 #include <climits>
 
@@ -546,26 +547,12 @@ size_t render_projected_bytes_per_vertex() { return sizeof(PVtx); }
 cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     const size_t smem = static_cast<size_t>(kBandRows) * kRS * sizeof(unsigned long long);
-    static bool attr_set_dev[64] = {};                       // per-device function attribute
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    bool& attr_set = attr_set_dev[dev];
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(render_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    if (!a.projected || !a.uniforms || a.max_nv <= 0) return cudaErrorInvalidValue;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n); cfg.blockDim = dim3(kProjThreads); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, render_project_kernel, a);
+    cudaError_t e = set_max_dynamic_smem<render_kernel>(smem);
     if (e != cudaSuccess) return e;
-    cfg.gridDim = dim3(kBands, n); cfg.blockDim = dim3(kRenderThreads); cfg.dynamicSmemBytes = smem;
-    return cudaLaunchKernelEx(&cfg, render_kernel, a);
+    if (!a.projected || !a.uniforms || a.max_nv <= 0) return cudaErrorInvalidValue;
+    e = launch_kernel(render_project_kernel, dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n), dim3(kProjThreads), 0, s, true, a);
+    if (e != cudaSuccess) return e;
+    return launch_kernel(render_kernel, dim3(kBands, n), dim3(kRenderThreads), smem, s, true, a);
 }
 
 }  // namespace se3tn
