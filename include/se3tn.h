@@ -182,6 +182,25 @@ int se3tn_add_adi(se3tn_ctx* ctx, const double* model_pts, int m, const double* 
  * (the reference raises IndexError there). */
 int se3tn_vocap(se3tn_ctx* ctx, const double* errs, int n, double* out_ap, void* stream);
 
+/* Utils.add / Utils.adi for the poses of several objects in ONE launch, as eval_ycbineoat.py's eval_all scores a whole data set
+ * (reference eval_ycbineoat.py:75-93, one Utils.add + Utils.adi call per pose there).  pts double (M,3) device: the model points
+ * of n_sets objects, concatenated; set_offsets int32 (n_sets+1) HOST: object s owns points [set_offsets[s], set_offsets[s+1]);
+ * pose_set int32 (n) HOST: the object of each pose; pred / gt double (n,16), out_add / out_adi double (n), device, either output
+ * may be NULL (not both unless n == 0).  Each pose's values are bit-identical to se3tn_add_adi on that pose and its object's points.  SE3TN_ERR_INVALID
+ * unless set_offsets starts at 0, increases strictly (no empty set) and ends at M, and every id is in [0, n_sets); nothing is
+ * queued then.  The offsets and ids are staged through context-owned device memory, which grows with n and n_sets and is
+ * shared with se3tn_vocap_sets: the metric calls of one context go on one stream, or the caller orders them. */
+int se3tn_add_adi_sets(se3tn_ctx* ctx, const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* pose_set,
+                       const double* pred, const double* gt, int n, double* out_add, double* out_adi, void* stream);
+
+/* VOCap of each object's errors and of all of them in one call (reference eval_ycbineoat.py:95-109, which calls eval_ycb.py:45-64
+ * once per object and once on the pooled errors).  errs double (n) and err_set int32 (n) device, any order -> out_ap double
+ * (n_sets+1) HOST: the AP of set 0, ..., set n_sets-1, then of all n errors.  Each value is bit-identical to se3tn_vocap on the
+ * same errors; a set with no error below 0.1 m, or none at all, gets 0.  Synchronises the stream.  An id outside [0, n_sets) is
+ * SE3TN_ERR_INVALID (found on the device, so the call has run).  Scratch as se3tn_add_adi_sets: context-owned, grown only when a
+ * call needs more, so a run of calls allocates nothing once the largest has been seen. */
+int se3tn_vocap_sets(se3tn_ctx* ctx, const double* errs, const int32_t* err_set, int n, int n_sets, double* out_ap, void* stream);
+
 /* ---- input A: the rendered previous view (SURVEY.md 8(f) "next" row 2) ------------------------------------- */
 
 /* The CAD model the renderer draws: what VispyRenderer.__init__ uploads as vertex / index buffers (reference
@@ -355,6 +374,9 @@ int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
  * se3tn_last_step_was_graph: 1 if the last track_batch / track_render / eval_pairs call was a graph launch. */
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);
+
+/* Bytes of device scratch the context holds for se3tn_add_adi_sets / se3tn_vocap_sets (0 before the first call). */
+size_t se3tn_metrics_scratch_bytes(se3tn_ctx* ctx);
 
 #ifdef __cplusplus
 }

@@ -33,6 +33,8 @@ SIGNATURES = {
     'se3tn_track_batch': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_add_adi': (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap': (_i, [_vp, _vp, _i, C.POINTER(_d), _vp]),
+    'se3tn_add_adi_sets': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    'se3tn_vocap_sets': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     'se3tn_allgather_poses': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
@@ -49,6 +51,7 @@ SIGNATURES = {
     'se3tn_last_launch_count': (_i, [_vp]),
     'se3tn_get_trace': (_i, [_vp, _vp]),
     'se3tn_last_step_was_graph': (_i, [_vp]),
+    'se3tn_metrics_scratch_bytes': (_sz, [_vp]),
     'se3tn_set_profiling': (_i, [_vp, _i]),
     'se3tn_get_profile': (_i, [_vp, _vp]),
 }

@@ -9,6 +9,7 @@
 #include "metrics.h"
 #include "ptx.cuh"
 #include <cub/cub.cuh>
+#include <algorithm>
 
 namespace se3tn {
 
@@ -32,15 +33,16 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
     return s;                       // valid in thread 0
 }
 
-__global__ void __launch_bounds__(kMetricThreads)
-add_adi_kernel(const double* __restrict__ model, int m, const double* __restrict__ pred, const double* __restrict__ gt,
-               double* __restrict__ out_add, double* __restrict__ out_adi)
+// ADD / ADD-S of one (pred, gt) pair of 4x4 poses against m model points, computed by one CTA of kMetricThreads threads.  Both
+// metric kernels run this body, so a pose scored against its own point set gives the same bits in either.
+__device__ __forceinline__ void score_pose(const double* __restrict__ model, int m, const double* __restrict__ pred16,
+                                           const double* __restrict__ gt16, double* __restrict__ out_add,
+                                           double* __restrict__ out_adi, int pose)
 {
     __shared__ double sp[kPredTile * 3];
     __shared__ double red[kMetricThreads / 32];
     __shared__ double Tp[12], Tg[12];
-    const int pose = blockIdx.x;
-    if (threadIdx.x < 12) { Tp[threadIdx.x] = pred[pose * 16 + threadIdx.x]; Tg[threadIdx.x] = gt[pose * 16 + threadIdx.x]; }
+    if (threadIdx.x < 12) { Tp[threadIdx.x] = pred16[threadIdx.x]; Tg[threadIdx.x] = gt16[threadIdx.x]; }
     __syncthreads();
     double sum_add = 0, sum_adi = 0;
     for (int base = 0; base < m; base += kMetricThreads) {
@@ -84,9 +86,30 @@ add_adi_kernel(const double* __restrict__ model, int m, const double* __restrict
     }
 }
 
-// errs sorted ascending; ap = 10 * [ sum_j (r_j - r_{j-1}) * j/n  +  (0.1 - r_c) * c/n ],  r_0 = 0, c = #(r < 0.1)
-__global__ void __launch_bounds__(1024)
-vocap_kernel(const double* __restrict__ rec, int n, double* __restrict__ out)
+__global__ void __launch_bounds__(kMetricThreads)
+add_adi_kernel(const double* __restrict__ model, int m, const double* __restrict__ pred, const double* __restrict__ gt,
+               double* __restrict__ out_add, double* __restrict__ out_adi)
+{
+    const int pose = blockIdx.x;
+    score_pose(model, m, pred + pose * 16, gt + pose * 16, out_add, out_adi, pose);
+}
+
+// One CTA per pose; pose p is scored against points [offsets[s], offsets[s+1]) of the table, s = pose_set[p].
+__global__ void __launch_bounds__(kMetricThreads)
+add_adi_sets_kernel(const double* __restrict__ pts, const int* __restrict__ offsets, const int* __restrict__ pose_set,
+                    const double* __restrict__ pred, const double* __restrict__ gt, double* __restrict__ out_add,
+                    double* __restrict__ out_adi)
+{
+    const int pose = blockIdx.x;
+    const int s = pose_set[pose], first = offsets[s];
+    score_pose(pts + static_cast<size_t>(first) * 3, offsets[s + 1] - first, pred + pose * 16, gt + pose * 16, out_add, out_adi, pose);
+}
+
+// errs sorted ascending; ap = 10 * [ sum_j (r_j - r_{j-1}) * j/n  +  (0.1 - r_c) * c/n ],  r_0 = 0, c = #(r < 0.1).
+// One CTA of kVocapThreads threads; the additions happen in an order fixed by n alone.
+constexpr int kVocapThreads = 1024;
+
+__device__ __forceinline__ void vocap_block(const double* __restrict__ rec, int n, double* __restrict__ out)
 {
     __shared__ double red[32];
     __shared__ int s_c;
@@ -112,12 +135,46 @@ vocap_kernel(const double* __restrict__ rec, int n, double* __restrict__ out)
         out[0] = c > 0 ? tot * 10.0 : 0.0;
     }
 }
+
+__global__ void __launch_bounds__(kVocapThreads)
+vocap_kernel(const double* __restrict__ rec, int n, double* __restrict__ out)
+{
+    vocap_block(rec, n, out);
+}
+
+// CTA s < n_sets: the AP of segment s of seg_sorted (each segment sorted); CTA n_sets: the AP of all_sorted (all n errors).
+__global__ void __launch_bounds__(kVocapThreads)
+vocap_sets_kernel(const double* __restrict__ seg_sorted, const int* __restrict__ offsets, int n_sets,
+                  const double* __restrict__ all_sorted, int n, double* __restrict__ out)
+{
+    const int s = blockIdx.x;
+    if (s < n_sets) vocap_block(seg_sorted + offsets[s], offsets[s + 1] - offsets[s], out + s);
+    else vocap_block(all_sorted, n, out + n_sets);
+}
+
+// counts[s] = #(set[i] == s); an id outside [0, n_sets) sets *bad instead.  counts has n_sets + 1 zeroed entries (the last
+// stays 0, so an exclusive scan over all of them ends in the total).
+__global__ void count_sets_kernel(const int* __restrict__ set, int n, int n_sets, int* __restrict__ counts, int* __restrict__ bad)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int s = set[i];
+        if (s >= 0 && s < n_sets) atomicAdd(&counts[s], 1);
+        else atomicOr(bad, 1);
+    }
+}
 }  // namespace
 
 cudaError_t launch_add_adi(const double* model, int m, const double* pred, const double* gt, int n,
                            double* out_add, double* out_adi, cudaStream_t s) {
     if (n <= 0 || m <= 0) return cudaSuccess;
     add_adi_kernel<<<n, kMetricThreads, 0, s>>>(model, m, pred, gt, out_add, out_adi);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_add_adi_sets(const double* pts, const int* offsets, const int* pose_set, const double* pred, const double* gt,
+                                int n, double* out_add, double* out_adi, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    add_adi_sets_kernel<<<n, kMetricThreads, 0, s>>>(pts, offsets, pose_set, pred, gt, out_add, out_adi);
     return cudaGetLastError();
 }
 
@@ -131,13 +188,82 @@ cudaError_t vocap(const double* errs, int n, double* out_host, cudaStream_t s) {
     if ((e = cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1)) != cudaSuccess) { cudaFree(sorted); cudaFree(d_out); return e; }
     e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, errs, sorted, n, 0, 64, s);
     if (e == cudaSuccess) {
-        vocap_kernel<<<1, 1024, 0, s>>>(sorted, n, d_out);
+        vocap_kernel<<<1, kVocapThreads, 0, s>>>(sorted, n, d_out);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d_out, sizeof(double), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     cudaFree(tmp); cudaFree(sorted); cudaFree(d_out);
     return e;
+}
+
+
+namespace {
+inline size_t up256(size_t v) { return (v + 255) & ~size_t(255); }
+
+// The scratch of vocap_sets, carved in this order: grouped ids | grouped errors | segments sorted | all sorted | counts (n_sets + 1)
+// then the bad-id flag | offsets (n_sets + 1) | APs (n_sets + 1) | cub temporary storage.
+struct VocapSetsLayout {
+    size_t keys, grouped, seg_sorted, all_sorted, counts, offsets, out, temp, temp_bytes, total;
+};
+
+cudaError_t vocap_sets_layout(int n, int n_sets, VocapSetsLayout& L) {
+    size_t a = 0, b = 0, c = 0, d = 0;
+    const int* ki = nullptr; int* ko = nullptr; const double* vi = nullptr; double* vo = nullptr;
+    cudaError_t e;
+    if ((e = cub::DeviceRadixSort::SortPairs(nullptr, a, ki, ko, vi, vo, n, 0, 32)) != cudaSuccess) return e;
+    if ((e = cub::DeviceScan::ExclusiveSum(nullptr, b, ki, ko, n_sets + 1)) != cudaSuccess) return e;
+    if ((e = cub::DeviceSegmentedRadixSort::SortKeys(nullptr, c, vi, vo, n, n_sets, ki, ki + 1, 0, 64)) != cudaSuccess) return e;
+    if ((e = cub::DeviceRadixSort::SortKeys(nullptr, d, vi, vo, n, 0, 64)) != cudaSuccess) return e;
+    const size_t nd = up256(sizeof(double) * n), ni = up256(sizeof(int) * n), sets = static_cast<size_t>(n_sets) + 1;
+    L.keys = 0; L.grouped = ni; L.seg_sorted = L.grouped + nd; L.all_sorted = L.seg_sorted + nd;
+    L.counts = L.all_sorted + nd; L.offsets = L.counts + up256(sizeof(int) * (sets + 1));
+    L.out = L.offsets + up256(sizeof(int) * sets); L.temp = L.out + up256(sizeof(double) * sets);
+    L.temp_bytes = std::max(std::max(a, b), std::max(c, d));
+    L.total = L.temp + up256(L.temp_bytes ? L.temp_bytes : 1);
+    return cudaSuccess;
+}
+}  // namespace
+
+cudaError_t vocap_sets_scratch_bytes(int n, int n_sets, size_t* bytes) {
+    VocapSetsLayout L;
+    const cudaError_t e = vocap_sets_layout(n, n_sets, L);
+    if (e == cudaSuccess) *bytes = L.total;
+    return e;
+}
+
+cudaError_t vocap_sets(const double* errs, const int* err_set, int n, int n_sets, uint8_t* scratch, double* out_host, int* bad_host,
+                       cudaStream_t s) {
+    VocapSetsLayout L;
+    cudaError_t e = vocap_sets_layout(n, n_sets, L);
+    if (e != cudaSuccess) return e;
+    int* keys = reinterpret_cast<int*>(scratch + L.keys);
+    double* grouped = reinterpret_cast<double*>(scratch + L.grouped);
+    double* seg_sorted = reinterpret_cast<double*>(scratch + L.seg_sorted);
+    double* all_sorted = reinterpret_cast<double*>(scratch + L.all_sorted);
+    int* counts = reinterpret_cast<int*>(scratch + L.counts);
+    int* bad = counts + n_sets + 1;
+    int* offsets = reinterpret_cast<int*>(scratch + L.offsets);
+    double* out = reinterpret_cast<double*>(scratch + L.out);
+    void* temp = scratch + L.temp;
+    size_t tb = L.temp_bytes;
+    // group the errors by set (a stable sort on the ids), count each set, and turn the counts into segment offsets
+    if ((e = cub::DeviceRadixSort::SortPairs(temp, tb, err_set, keys, errs, grouped, n, 0, 32, s)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(counts, 0, sizeof(int) * (n_sets + 2), s)) != cudaSuccess) return e;
+    count_sets_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, s>>>(err_set, n, n_sets, counts, bad);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    tb = L.temp_bytes;
+    if ((e = cub::DeviceScan::ExclusiveSum(temp, tb, counts, offsets, n_sets + 1, s)) != cudaSuccess) return e;
+    // each segment sorted on its own, and all errors sorted together, as se3tn_vocap sorts them
+    tb = L.temp_bytes;
+    if ((e = cub::DeviceSegmentedRadixSort::SortKeys(temp, tb, grouped, seg_sorted, n, n_sets, offsets, offsets + 1, 0, 64, s)) != cudaSuccess) return e;
+    tb = L.temp_bytes;
+    if ((e = cub::DeviceRadixSort::SortKeys(temp, tb, errs, all_sorted, n, 0, 64, s)) != cudaSuccess) return e;
+    vocap_sets_kernel<<<n_sets + 1, kVocapThreads, 0, s>>>(seg_sorted, offsets, n_sets, all_sorted, n, out);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(out_host, out, sizeof(double) * (n_sets + 1), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
+    return cudaStreamSynchronize(s);
 }
 
 }  // namespace se3tn

@@ -198,6 +198,7 @@ struct se3tn_ctx {
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
     DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
     DevBuf<float> loss_sq; size_t loss_sq_floats = 0;   // se3tn_eval_pairs' loss terms when the caller wants none back: max_batch x 6 (allocated on first use)
+    DevBuf<uint8_t> metrics; size_t metrics_bytes = 0;   // se3tn_add_adi_sets' staged offsets and ids, or se3tn_vocap_sets' scratch (grows on demand)
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
     // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
     struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
@@ -1212,6 +1213,50 @@ int se3tn_vocap(se3tn_ctx* c, const double* errs, int n, double* out_ap, void* s
     CU_TRY(c, vocap(errs, n, out_ap, static_cast<cudaStream_t>(stream)));
     return SE3TN_OK;
 }
+
+int se3tn_add_adi_sets(se3tn_ctx* c, const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* pose_set,
+                       const double* pred, const double* gt, int n, double* out_add, double* out_adi, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!pts || !set_offsets || M <= 0 || n_sets <= 0 || n < 0 || (n > 0 && (!pose_set || !pred || !gt || (!out_add && !out_adi))))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: null/invalid argument");
+    if (set_offsets[0] != 0 || set_offsets[n_sets] != M)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: set_offsets must start at 0 and end at M = " + std::to_string(M));
+    for (int s = 0; s < n_sets; ++s)
+        if (set_offsets[s + 1] <= set_offsets[s])
+            return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: set " + std::to_string(s) + " is empty or its offsets decrease");
+    for (int i = 0; i < n; ++i)
+        if (pose_set[i] < 0 || pose_set[i] >= n_sets)
+            return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: pose " + std::to_string(i) + " has set id " + std::to_string(pose_set[i]) +
+                                              " outside [0, " + std::to_string(n_sets) + ")");
+    if (n == 0) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const size_t off_bytes = align256(sizeof(int32_t) * (static_cast<size_t>(n_sets) + 1));
+    CU_TRY(c, grow(c->metrics, c->metrics_bytes, off_bytes + sizeof(int32_t) * static_cast<size_t>(n)));
+    int32_t* d_off = reinterpret_cast<int32_t*>(c->metrics.get());
+    int32_t* d_set = reinterpret_cast<int32_t*>(c->metrics.get() + off_bytes);
+    CU_TRY(c, cudaMemcpyAsync(d_off, set_offsets, sizeof(int32_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
+    CU_TRY(c, cudaMemcpyAsync(d_set, pose_set, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+    CU_TRY(c, launch_add_adi_sets(pts, d_off, d_set, pred, gt, n, out_add, out_adi, s));
+    return SE3TN_OK;
+}
+
+int se3tn_vocap_sets(se3tn_ctx* c, const double* errs, const int32_t* err_set, int n, int n_sets, double* out_ap, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!out_ap || n < 0 || n_sets <= 0 || (n > 0 && (!errs || !err_set))) return fail(c, SE3TN_ERR_INVALID, "se3tn_vocap_sets: null/invalid argument");
+    if (n == 0) { std::fill(out_ap, out_ap + n_sets + 1, 0.0); return SE3TN_OK; }
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    size_t bytes = 0;
+    CU_TRY(c, vocap_sets_scratch_bytes(n, n_sets, &bytes));
+    CU_TRY(c, grow(c->metrics, c->metrics_bytes, bytes));
+    int bad = 0;
+    CU_TRY(c, vocap_sets(errs, err_set, n, n_sets, c->metrics.get(), out_ap, &bad, s));
+    if (bad) return fail(c, SE3TN_ERR_INVALID, "se3tn_vocap_sets: a set id is outside [0, " + std::to_string(n_sets) + ")");
+    return SE3TN_OK;
+}
+
+size_t se3tn_metrics_scratch_bytes(se3tn_ctx* c) { return c ? c->metrics_bytes : 0; }
 
 namespace {
 // crop window of one track in frame pixels: compute_bbox + crop_bbox's window (reference Utils.py:302-316, 324-327), the same

@@ -333,6 +333,50 @@ class Engine:
         _lib.check(self.lib.se3tn_vocap(self._ctx, _ptr(errs), int(errs.numel()), C.byref(ap), _stream(self.device)), self._ctx)
         return ap.value
 
+    def add_adi_sets(self, points, pose_set, pred, gt, set_offsets=None, want_add=True, want_adi=True):
+        """add_adi for the poses of several objects in one launch (se3tn_add_adi_sets).  points: a list of each object's (m_s,3)
+        float64 model points (numpy arrays or tensors), or one float64 CUDA table (M,3) with set_offsets (S+1) int32 giving each
+        object's rows.  pose_set (n) int32: the object of each pose; pred / gt float64 CUDA tensors (n,4,4).
+        -> (out_add, out_adi) float64 CUDA tensors (n), bit-identical to add_adi on each pose's own points."""
+        if torch.is_tensor(points):
+            table = points
+            if set_offsets is None:
+                raise ValueError('add_adi_sets: a point table needs set_offsets')
+        else:
+            sets = [np.asarray(p.cpu().numpy() if torch.is_tensor(p) else p, dtype=np.float64).reshape(-1, 3) for p in points]
+            set_offsets = np.cumsum([0] + [len(p) for p in sets])
+            table = torch.from_numpy(np.ascontiguousarray(np.concatenate(sets) if sets else np.zeros((0, 3)))).to(self.device)
+        offs = np.ascontiguousarray(set_offsets, dtype=np.int32)
+        ids = np.ascontiguousarray(pose_set.cpu().numpy() if torch.is_tensor(pose_set) else pose_set, dtype=np.int32).reshape(-1)
+        n = int(ids.shape[0])
+        if offs.ndim != 1 or offs.shape[0] < 2:
+            raise ValueError('add_adi_sets: set_offsets must hold S+1 >= 2 offsets')
+        self._check_dev('points', table, torch.float64, (table.shape[0], 3))
+        self._check_dev('pred', pred, torch.float64, (n, 4, 4))
+        self._check_dev('gt', gt, torch.float64, (n, 4, 4))
+        out_add = torch.empty(n, dtype=torch.float64, device=self.device) if want_add else None
+        out_adi = torch.empty(n, dtype=torch.float64, device=self.device) if want_adi else None
+        _lib.check(self.lib.se3tn_add_adi_sets(self._ctx, _ptr(table), int(table.shape[0]), _hptr(offs), int(offs.shape[0]) - 1, _hptr(ids),
+                                               _ptr(pred), _ptr(gt), n, _ptr(out_add), _ptr(out_adi), _stream(self.device)), self._ctx)
+        return out_add, out_adi
+
+    def vocap_sets(self, errs, err_set, n_sets):
+        """VOCap of each set's errors and of all of them (se3tn_vocap_sets): errs float64 CUDA tensor (n), err_set (n) int32
+        set ids in [0, n_sets) -> float64 numpy (n_sets+1,): one AP per set, then the pooled AP, each as vocap() computes it."""
+        n = int(errs.numel())
+        self._check_dev('errs', errs, torch.float64, (n,))
+        ids = err_set.to(self.device, torch.int32).contiguous() if torch.is_tensor(err_set) else \
+            torch.from_numpy(np.ascontiguousarray(err_set, dtype=np.int32)).to(self.device)
+        if ids.shape != (n,):
+            raise ValueError('vocap_sets: err_set must have one id per error')
+        out = np.zeros(int(n_sets) + 1, dtype=np.float64)
+        _lib.check(self.lib.se3tn_vocap_sets(self._ctx, _ptr(errs), _ptr(ids), n, int(n_sets), _hptr(out), _stream(self.device)), self._ctx)
+        return out
+
+    def metrics_scratch_bytes(self):
+        """Device bytes the context holds for add_adi_sets / vocap_sets."""
+        return int(self.lib.se3tn_metrics_scratch_bytes(self._ctx))
+
     # ------------------------------------------------------------------ input A renderer (SURVEY 8f row 2)
     def set_mesh(self, mesh, mesh_id=0):
         """Upload a CAD model (dict pos float32 (nv,3), nrm float32 (nv,3), col uint8 (nv,3), faces int32 (nf,3)) -- the

@@ -673,18 +673,58 @@ def ycb_all_res_dir(outdir, class_name):
     return os.path.join(outdir, class_name, YCB_ALL_RUN)
 
 
-def expand_class_paths(class_config, class_id, class_name):
-    """The four path templates of class_config for one class -> {train_data_path, mean_std_path, ckpt_dir, model_path}."""
+def _expand_templates(config, config_name, **placeholders):
+    """The four YCB_ALL_TEMPLATES path templates of config with the given placeholders filled in."""
     out = {}
     for key in YCB_ALL_TEMPLATES:
-        if key not in class_config:
-            raise ValueError('class_config needs a %r template' % key)
+        if key not in config:
+            raise ValueError('%s needs a %r template' % (config_name, key))
         try:
-            out[key] = str(class_config[key]).format(class_id=class_id, class_name=class_name)
+            out[key] = str(config[key]).format(**placeholders)
         except (KeyError, IndexError, ValueError) as e:
-            raise ValueError('class_config[%r] = %r: the only placeholders are {class_id} and {class_name} (%s)'
-                             % (key, class_config[key], e)) from None
+            raise ValueError('%s[%r] = %r: the only placeholders are %s (%s)' % (config_name, key, config[key],
+                             ' and '.join('{%s}' % p for p in placeholders), e)) from None
     return out
+
+
+def expand_class_paths(class_config, class_id, class_name):
+    """The four path templates of class_config for one class -> {train_data_path, mean_std_path, ckpt_dir, model_path}."""
+    return _expand_templates(class_config, 'class_config', class_id=class_id, class_name=class_name)
+
+
+def _load_run_files(label, paths):
+    """dataset_info.yml, mean and std of expanded paths, after checking that every file the run reads exists: a missing one is a
+    FileNotFoundError naming `label` and the path.  -> dict of dataset_info, mean, std and the paths."""
+    import yaml
+    info_path = os.path.join(paths['train_data_path'], '../dataset_info.yml')
+    files = [('dataset_info.yml', info_path), ('mean', os.path.join(paths['mean_std_path'], 'mean.npy')),
+             ('std', os.path.join(paths['mean_std_path'], 'std.npy')), ('checkpoint', paths['ckpt_dir']), ('mesh', paths['model_path'])]
+    for what, path in files:
+        if not os.path.isfile(path):
+            raise FileNotFoundError('%s: no %s file at %s' % (label, what, path))
+    with open(info_path, 'r') as ff:
+        info = yaml.safe_load(ff)
+    return dict(dataset_info=info, mean=np.load(files[1][1]), std=np.load(files[2][1]), **paths)
+
+
+def _check_shared(entries, label, short, shared, why):
+    """Every entry at the resolution libse3tn is built for, and equal to the first in each (name, getter) of `shared`; otherwise a
+    ValueError naming the entry (label(entry)) and the first (short(entry))."""
+    first = entries[0]
+    for k in entries:
+        if k['dataset_info']['resolution'] != 176:
+            raise ValueError('%s: resolution %s; libse3tn is built for 176' % (label(k), k['dataset_info']['resolution']))
+        for what, get in shared:
+            if get(k) != get(first):
+                raise ValueError('%s: %s %r differs from %s\'s %r; %s' % (label(k), what, get(k), short(first), get(first), why))
+
+
+def _camera(k):
+    return {key: float(v) for key, v in k['dataset_info']['camera'].items()}
+
+
+def _pyrender(k):
+    return k['dataset_info'].get('renderer') == 'pyrenderer'
 
 
 def _class_normalizer(class_config, key, class_id, default):
@@ -703,7 +743,6 @@ def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     FileNotFoundError naming the class and the path.  One step tracks every class of a frame, so the classes must share the
     camera (K and image size), the resolution (176), the render mode, the two normalisers and the precision: a class that differs
     from the first is a ValueError naming it."""
-    import yaml
     from .engine import PREC
     if precision not in PREC:
         raise ValueError('unknown precision %r (one of %s)' % (precision, ', '.join(PREC)))
@@ -717,29 +756,14 @@ def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     classes = []
     for c in ids:
         name = names[c - 1]
-        paths = expand_class_paths(class_config, c, name)
-        info_path = os.path.join(paths['train_data_path'], '../dataset_info.yml')
-        files = [('dataset_info.yml', info_path), ('mean', os.path.join(paths['mean_std_path'], 'mean.npy')),
-                 ('std', os.path.join(paths['mean_std_path'], 'std.npy')), ('checkpoint', paths['ckpt_dir']), ('mesh', paths['model_path'])]
-        for what, path in files:
-            if not os.path.isfile(path):
-                raise FileNotFoundError('class %d (%s): no %s file at %s' % (c, name, what, path))
-        with open(info_path, 'r') as ff:
-            info = yaml.safe_load(ff)
-        classes.append(dict(class_id=c, name=name, dataset_info=info, mean=np.load(files[1][1]), std=np.load(files[2][1]),
+        k = _load_run_files('class %d (%s)' % (c, name), expand_class_paths(class_config, c, name))
+        classes.append(dict(k, class_id=c, name=name,
                             trans_normalizer=_class_normalizer(class_config, 'trans_normalizer', c, 0.03),
-                            rot_normalizer=_class_normalizer(class_config, 'rot_normalizer', c, 5 * np.pi / 180), **paths))
-    first = classes[0]
-    shared = (('camera', lambda k: {key: float(v) for key, v in k['dataset_info']['camera'].items()}),
-              ('renderer', lambda k: k['dataset_info'].get('renderer') == 'pyrenderer'),
-              ('trans_normalizer', lambda k: k['trans_normalizer']), ('rot_normalizer', lambda k: k['rot_normalizer']))
-    for k in classes:
-        if k['dataset_info']['resolution'] != 176:
-            raise ValueError('class %d (%s): resolution %s; libse3tn is built for 176' % (k['class_id'], k['name'], k['dataset_info']['resolution']))
-        for what, get in shared:
-            if get(k) != get(first):
-                raise ValueError('class %d (%s): %s %r differs from class %d\'s %r; classes tracked in one step must share it'
-                                 % (k['class_id'], k['name'], what, get(k), first['class_id'], get(first)))
+                            rot_normalizer=_class_normalizer(class_config, 'rot_normalizer', c, 5 * np.pi / 180)))
+    _check_shared(classes, lambda k: 'class %d (%s)' % (k['class_id'], k['name']), lambda k: 'class %d' % k['class_id'],
+                  (('camera', _camera), ('renderer', _pyrender),
+                   ('trans_normalizer', lambda k: k['trans_normalizer']), ('rot_normalizer', lambda k: k['rot_normalizer'])),
+                  'classes tracked in one step must share it')
     return classes
 
 
@@ -850,11 +874,172 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     return results
 
 
+# ----------------------------------------------------------------------------------------------------
+# Every YCBInEOAT video in one pass: the paper's Table II as one run instead of one predictSequenceYcbInEOAT run per video.  One
+# Engine holds each object's weights, statistics and mesh; each frame is one n = 1 se3tn_track_render step, decoded ahead by a
+# thread pool.  The output tree is what eval_ycbineoat.eval_all scores:  <outdir>/<video>/%07d.txt
+# Per-object configuration is the four YCB_ALL_TEMPLATES path templates with {object} (a name of eval_ycbineoat.OBJECTS) and,
+# with ycb_dir, {class_name} (the CADmodels/ folder of the object) placeholders.
+# ----------------------------------------------------------------------------------------------------
+YCBINEOAT_TRANS_NORMALIZER, YCBINEOAT_ROT_NORMALIZER = 0.03, 30 * np.pi / 180       # predict.py:586-587
+
+
+def ycbineoat_videos(root):
+    """[(video folder name, object)], sorted by name: every folder under root with rgb/, depth_filled/ and annotated_poses/
+    (.tar.gz entries skipped).  A video folder that names no object is a ValueError naming it."""
+    from .eval_ycbineoat import OBJECTS, video_object
+    videos = []
+    for name in sorted(os.listdir(root)):
+        d = os.path.join(root, name)
+        if '.tar.gz' in name or not all(os.path.isdir(os.path.join(d, sub)) for sub in ('rgb', 'depth_filled', 'annotated_poses')):
+            continue
+        obj = video_object(name)
+        if obj is None:
+            raise ValueError('video folder %s names none of the objects %s' % (d, OBJECTS))
+        videos.append((name, obj))
+    return videos
+
+
+def ycbineoat_class_name(ycb_dir, obj):
+    """The CADmodels/ folder of an object: the first, in sorted order, whose name contains it."""
+    for name in ycb_class_names(ycb_dir):
+        if obj in name:
+            return name
+    raise FileNotFoundError('object %s: no CADmodels/ folder under %s contains its name' % (obj, ycb_dir))
+
+
+def expand_object_paths(object_config, obj, class_name=None):
+    """The four path templates of object_config for one object -> {train_data_path, mean_std_path, ckpt_dir, model_path}."""
+    ph = dict(object=obj) if class_name is None else dict(object=obj, class_name=class_name)
+    return _expand_templates(object_config, 'object_config', **ph)
+
+
+def ycbineoat_objects(objects, object_config, ycb_dir=None, precision='bf16x3'):
+    """The checked configuration of each object, before anything is loaded onto a device -> {object: dict of the expanded paths,
+    dataset_info, mean, std}.  A missing file is a FileNotFoundError naming the object and the path.  The frames of all videos go
+    through one set of buffers, so the objects must share the camera and the render mode."""
+    from .engine import PREC
+    if precision not in PREC:
+        raise ValueError('unknown precision %r (one of %s)' % (precision, ', '.join(PREC)))
+    out = {}
+    for obj in objects:
+        cname = ycbineoat_class_name(ycb_dir, obj) if ycb_dir else None
+        out[obj] = dict(_load_run_files('object %s' % obj, expand_object_paths(object_config, obj, cname)), object=obj)
+    if out:
+        _check_shared(list(out.values()), lambda k: 'object %s' % k['object'], lambda k: 'object %s' % k['object'],
+                      (('camera', _camera), ('renderer', _pyrender)), 'all videos are tracked through one set of frame buffers')
+    return out
+
+
+def write_video_poses(outdir, video, poses):
+    """<outdir>/<video>/%07d.txt, one np.savetxt pose per frame: what eval_ycbineoat.eval_all reads with res_dir = outdir + '/'."""
+    vdir = os.path.join(outdir, video)
+    os.makedirs(vdir, exist_ok=True)
+    for i in range(len(poses)):
+        np.savetxt(os.path.join(vdir, '%07d.txt' % i), poses[i])
+
+
+def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None):
+    """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
+    <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
+
+    Videos and objects as ycbineoat_videos and ycbineoat_objects find and check them.  One Engine holds each object's weights,
+    statistics and CUDA-renderer mesh once, under one weight id per object.  Each video starts from its annotated_poses[0] and is
+    tracked from frame 0 with the reference's normalisers (0.03 m, 30 degrees), one n = 1 se3tn_track_render step per frame.  The
+    pose lives in one device tensor that every step updates in place, and the frame in one device buffer, so every step after an
+    object's first replays its CUDA graph; a device history of the poses comes back to the host once per video.  A thread pool
+    decodes up to decode_ahead frames ahead, across video boundaries, into a ring of that many pinned staging sets."""
+    from collections import deque
+    from concurrent.futures import ThreadPoolExecutor
+    from .eval_ycbineoat import OBJECTS
+    decode_ahead = int(decode_ahead)
+    if decode_ahead < 1:
+        raise ValueError('decode_ahead must be at least 1')
+    videos = ycbineoat_videos(ycbineoat_dir)
+    files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
+    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, precision)
+    eng = Engine(max_batch=1)
+    trackers = {}
+    for obj, k in objects.items():
+        try:
+            trackers[obj] = Tracker(k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], model_path=k['model_path'], engine=eng,
+                                    weight_id=OBJECTS.index(obj), precision=precision, renderer='cuda',
+                                    trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER)
+        except ValueError as e:
+            raise ValueError('object %s: %s' % (obj, e)) from e
+    dev = eng.device
+    # per object: the step's ids and width, kept on the device so the step's addresses stay the same from video to video
+    ids = {o: np.array([OBJECTS.index(o)], dtype=np.int32) for o in trackers}
+    ids_d = {o: torch.from_numpy(ids[o]).to(dev) for o in trackers}
+    widths = {o: torch.tensor([trackers[o].object_width], dtype=torch.float64, device=dev) for o in trackers}
+    poses = torch.empty((1, 4, 4), dtype=torch.float64, device=dev)
+    out_trans = torch.empty((1, 3), dtype=torch.float32, device=dev)
+    out_rot = torch.empty((1, 3), dtype=torch.float32, device=dev)
+    frames = []                                            # (video, object, frame index, frames of the video)
+    for v, obj in videos:
+        nf = len(files[v][0]) if max_frames is None else min(max_frames, len(files[v][0]))
+        frames += [(v, obj, t, nf) for t in range(nf)]
+    results = {}
+    if not frames:
+        return results
+    cam = next(iter(trackers.values())).dataset_info['camera']
+    pinned = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True)
+    host = [(pinned((cam['height'], cam['width'], 3), torch.uint8), pinned((cam['height'], cam['width']), torch.uint16))
+            for _ in range(decode_ahead)]
+    rgb_d = torch.empty(host[0][0].shape, dtype=torch.uint8, device=dev)
+    depth_d = torch.empty(host[0][1].shape, dtype=torch.uint16, device=dev)
+    uploaded = [None] * decode_ahead                       # event after the last upload from each staging set
+
+    def decode_into(dst, read, path):
+        img = read(path)
+        if img.shape != tuple(dst.shape):
+            raise ValueError('%s: %s, the camera image is %s (dataset_info.yml)' % (path, img.shape, tuple(dst.shape)))
+        dst.numpy()[...] = img
+
+    with ThreadPoolExecutor(max_workers=2 * decode_ahead) as pool:
+        pending = deque()
+
+        def submit(k):                                     # frame k decodes into staging set k % decode_ahead
+            v, _, t, _ = frames[k]
+            slot = k % decode_ahead
+            if uploaded[slot] is not None:
+                uploaded[slot].synchronize()               # the staging set's previous upload has left it
+            pending.append([pool.submit(decode_into, host[slot][0], read_rgb, files[v][0][t]),
+                            pool.submit(decode_into, host[slot][1], read_depth, files[v][1][t])])
+
+        for k in range(min(decode_ahead, len(frames))):
+            submit(k)
+        history = None
+        for k, (v, obj, t, nf) in enumerate(frames):
+            if k > 0 and k + decode_ahead - 1 < len(frames):
+                submit(k + decode_ahead - 1)               # into the staging set frame k - 1 was uploaded from
+            for f in pending.popleft():
+                f.result()
+            slot = k % decode_ahead
+            rgb_d.copy_(host[slot][0], non_blocking=True)
+            depth_d.copy_(host[slot][1], non_blocking=True)
+            uploaded[slot] = torch.cuda.Event()
+            uploaded[slot].record()
+            if t == 0:
+                poses.copy_(torch.from_numpy(np.loadtxt(files[v][2][0]).reshape(1, 4, 4)))
+                history = torch.empty((nf, 1, 4, 4), dtype=torch.float64, device=dev)
+            trk = trackers[obj]
+            eng.track_render(rgb_d, depth_d, trk.K, poses, widths[obj], trk.trans_normalizer, trk.rot_normalizer,
+                             weight_ids_host=ids[obj], weight_ids_dev=ids_d[obj], precision=precision, mode=trk.renderer.mode,
+                             image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
+            history[t].copy_(poses)
+            if t == nf - 1:
+                results[v] = history[:, 0].cpu().numpy()
+                write_video_poses(outdir, v, results[v])
+    return results
+
+
 def main(argv=None):
     import argparse
     parser = argparse.ArgumentParser(description='headless se(3)-TrackNet sequence tracking on libse3tn (flags of the reference predict.py:626-641)')
     parser.add_argument('--mode', default='ycbv', help='ycbv (one YCB-Video sequence) / ycbineoat / ycbv_all (every class of --class_ids '
-                        'through every YCB-Video test sequence in one pass) / anything else: every YCB-Video test sequence of the class')
+                        'through every YCB-Video test sequence in one pass) / ycbineoat_all (every video under --YCBInEOAT_dir in one '
+                        'pass) / anything else: every YCB-Video test sequence of the class')
     parser.add_argument('--seq_id', default=None, type=int)
     parser.add_argument('--ycb_dir', default=None)
     parser.add_argument('--YCBInEOAT_dir', default=None)
@@ -868,10 +1053,14 @@ def main(argv=None):
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
     parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt)')
     parser.add_argument('--max_frames', type=int, default=None)
-    parser.add_argument('--score', action='store_true', help='ycbv_all: score the output with eval_ycb and print its lines')
+    parser.add_argument('--score', action='store_true', help='ycbv_all / ycbineoat_all: score the output with eval_ycb / '
+                        'eval_ycbineoat and print its lines')
+    parser.add_argument('--decode_ahead', type=int, default=4, help='ycbineoat_all: frames decoded ahead of the tracking step')
     args = parser.parse_args(argv)
     if args.mode == 'ycbv_all':
         return _main_ycbv_all(args)
+    if args.mode == 'ycbineoat_all':
+        return _main_ycbineoat_all(args)
     dataset_info, images_mean, images_std = load_run_config(args.train_data_path, args.mean_std_path)
     if args.mode == 'ycbineoat':
         if not args.YCBInEOAT_dir:
@@ -923,6 +1112,25 @@ def _main_ycbv_all(args):
             for c in class_ids:
                 eval_ycb.eval_one_class(argparse.Namespace(ycb_dir=args.ycb_dir, class_id=c,
                                                            res_dir=ycb_all_res_dir(args.outdir, names[c - 1]) + '/'))
+    return res
+
+
+def _main_ycbineoat_all(args):
+    """--mode ycbineoat_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-object path templates."""
+    import argparse
+    if not args.YCBInEOAT_dir:
+        raise SystemExit('--mode ycbineoat_all needs --YCBInEOAT_dir')
+    if args.score and not args.ycb_dir:
+        raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
+    config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
+    res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
+                              ycb_dir=args.ycb_dir)
+    for v in res:
+        print('tracked %s: %d frames' % (v, len(res[v])))
+    print('-> %s' % args.outdir)
+    if args.score:
+        from . import eval_ycbineoat
+        eval_ycbineoat.eval_all(argparse.Namespace(YCBInEOAT_dir=args.YCBInEOAT_dir, ycb_dir=args.ycb_dir, res_dir=args.outdir.rstrip('/') + '/'))
     return res
 
 
