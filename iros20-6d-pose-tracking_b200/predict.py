@@ -19,6 +19,7 @@ Differences, all additive:
     inside the tracking step, as the reference's ROS node does with Utils.fill_depth before every
     on_track (predict_ros.py:38-41).
 """
+import contextlib
 import os
 import numpy as np
 import torch
@@ -27,6 +28,7 @@ from .engine import Engine
 from .cuda_renderer import CudaRenderer
 from .se3_tracknet import Se3TrackNet
 from .datasets import TrackDataset
+from .staging import StagingRing
 from . import Utils as U
 
 
@@ -409,6 +411,15 @@ def read_depth(path):
     return d.astype(np.uint16)
 
 
+def _decode_into(host, name, read, path):
+    """A StagingRing job: read(path) (read_rgb or read_depth) into the pinned camera image host[name]."""
+    img = read(path)
+    dst = host[name]
+    if img.shape != tuple(dst.shape):
+        raise ValueError('%s: %s, the camera image is %s (dataset_info.yml)' % (path, img.shape, tuple(dst.shape)))
+    dst.numpy()[...] = img
+
+
 def sequence_files(test_data_path):
     """(rgb files, depth files, ground-truth pose files), each sorted (predict.py:584-590)."""
     import glob
@@ -778,99 +789,98 @@ def ycb_track_sets(ycb_dir, class_ids):
     return dict(sorted(sets.items()))
 
 
+def _one_pass_trackers(entries, precision, max_batch):
+    """One Engine of max_batch tracks per step and {weight id: Tracker} on it for [(weight id, label, checked configuration)]: the
+    configuration's files and normalisers, the CUDA renderer.  A ValueError is relabelled with the class or object it is about."""
+    eng = Engine(max_batch=max_batch)
+    trackers = {}
+    for wid, label, k in entries:
+        try:
+            trackers[wid] = Tracker(k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], model_path=k['model_path'], engine=eng,
+                                    weight_id=wid, precision=precision, renderer='cuda',
+                                    trans_normalizer=k['trans_normalizer'], rot_normalizer=k['rot_normalizer'])
+        except ValueError as e:
+            raise ValueError('%s: %s' % (label, e)) from e
+    return eng, trackers
+
+
+def _track_sequences(eng, trackers, sequences, precision, depth, workers):
+    """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
+    files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode.
+    Yields each sequence's (frames, n, 4, 4) numpy poses, the poses after each frame, as soon as the sequence ends.
+
+    Every frame is one se3tn_track_render step for the sequence's n tracks.  The frames of all sequences decode ahead, across
+    sequence boundaries, through one StagingRing of `depth` sets (`workers` threads) into its one device frame.  The step's other
+    device arguments are kept: the ids and widths per distinct weight-id tuple, and per n the pose tensor every step updates in
+    place and the step's outputs.  So every step after a track set's first replays the step's CUDA graph, across sequences too.
+    After each step the poses are copied into a device history, which comes back to the host once per sequence."""
+    if not sequences:
+        return
+    dev = eng.device
+    cam = trackers[sequences[0][2][0]].dataset_info['camera']
+    ring = StagingRing({'rgb': ((cam['height'], cam['width'], 3), torch.uint8), 'depth': ((cam['height'], cam['width']), torch.uint16)},
+                       depth, dev)
+    frames = [[(_decode_into, 'rgb', read_rgb, r), (_decode_into, 'depth', read_depth, d)]
+              for rgb_files, depth_files, _, _ in sequences for r, d in zip(rgb_files, depth_files)]
+    by_ids, by_n = {}, {}
+    with contextlib.closing(ring.uploads(frames, workers)) as uploads:
+        for rgb_files, _, ids, init in sequences:
+            n = len(ids)
+            if ids not in by_ids:
+                wh = np.asarray(ids, dtype=np.int32)
+                by_ids[ids] = (wh, torch.from_numpy(wh).to(dev),
+                               torch.tensor([trackers[w].object_width for w in ids], dtype=torch.float64, device=dev))
+            if n not in by_n:
+                by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
+                           torch.empty((n, 3), dtype=torch.float32, device=dev))
+            wh, wd, widths = by_ids[ids]
+            poses, out_trans, out_rot = by_n[n]
+            poses.copy_(torch.from_numpy(init))
+            history = torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev)
+            trk = trackers[ids[0]]
+            for t in range(len(rgb_files)):
+                next(uploads)
+                eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
+                                 weight_ids_host=wh, weight_ids_dev=wd, precision=precision, mode=trk.renderer.mode,
+                                 image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
+                history[t].copy_(poses)
+            yield history.cpu().numpy()
+
+
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
     One Engine holds every class's weights, statistics and CUDA-renderer mesh under weight id = class id.  For each test sequence,
-    the tracks are its requested classes in ascending order, each started as getResultsYcb starts it.  Every frame is one
-    se3tn_track_render step for all of them: its colour and depth PNGs are decoded once, in a thread pool, into one of two pinned
-    staging sets (frame t+1 decodes while step t runs), and uploaded in stream order into one device frame.  The tracks' poses live
-    in one device tensor that every step updates in place (the step's graph key keeps its addresses, so every step after the
-    first of a sequence is a graph replay); after each step they are copied into a (frames, n, 4, 4) history on the device, which
-    comes back to the host once per sequence."""
-    from concurrent.futures import ThreadPoolExecutor
+    the tracks are its requested classes in ascending order, each started as getResultsYcb starts it, and every frame after the
+    first is one se3tn_track_render step for all of them (_track_sequences: each frame decoded once, two frames ahead)."""
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     classes = ycb_all_classes(ycb_dir, class_ids, class_config, precision)
     track_sets = ycb_track_sets(ycb_dir, [k['class_id'] for k in classes])
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
-    eng = Engine(max_batch=max([len(v) for v in track_sets.values()] + [1]))
-    trackers = {}
-    for k in classes:
-        try:
-            trackers[k['class_id']] = Tracker(k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], model_path=k['model_path'],
-                                              engine=eng, weight_id=k['class_id'], precision=precision, renderer='cuda',
-                                              trans_normalizer=k['trans_normalizer'], rot_normalizer=k['rot_normalizer'])
-        except ValueError as e:
-            raise ValueError('class %d (%s): %s' % (k['class_id'], k['name'], e)) from e
+    sequences = []
+    for seq_id, cls in track_sets.items():
+        files = {c: _ycb_sequence_files(os.path.join(data_dir, '%04d' % seq_id), c) for c in cls}
+        rgb_files, depth_files, _ = files[cls[0]]
+        nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
+        init = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
+                                         sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]).astype(np.float64)
+        sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
+    eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], precision,
+                                       max([len(v) for v in track_sets.values()] + [1]))
     name_of = {k['class_id']: k['name'] for k in classes}
-    trk0 = trackers[classes[0]['class_id']]
-    render = trk0.renderer
-    cam = trk0.dataset_info['camera']
-    dev = eng.device
-    pinned = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True)
-    host = [(pinned((cam['height'], cam['width'], 3), torch.uint8), pinned((cam['height'], cam['width']), torch.uint16)) for _ in range(2)]
-    rgb_d = torch.empty(host[0][0].shape, dtype=torch.uint8, device=dev)
-    depth_d = torch.empty(host[0][1].shape, dtype=torch.uint16, device=dev)
-    uploaded = [None, None]                                # event after the last upload from each staging set
-
-    def decode_into(dst, read, path):
-        img = read(path)
-        if img.shape != tuple(dst.shape):
-            raise ValueError('%s: %s, the camera image is %s (dataset_info.yml)' % (path, img.shape, tuple(dst.shape)))
-        dst.numpy()[...] = img
-
     results = {k['class_id']: {} for k in classes}
-    with ThreadPoolExecutor(max_workers=2) as pool:
-        def submit(rgb_path, depth_path, slot):
-            if uploaded[slot] is not None:
-                uploaded[slot].synchronize()               # the staging set's previous upload has left it
-            return [pool.submit(decode_into, host[slot][0], read_rgb, rgb_path),
-                    pool.submit(decode_into, host[slot][1], read_depth, depth_path)]
-
-        for seq_id, cls in track_sets.items():
-            seq_dir = os.path.join(data_dir, '%04d' % seq_id)
-            files = {c: _ycb_sequence_files(seq_dir, c) for c in cls}
-            rgb_files, depth_files = files[cls[0]][0], files[cls[0]][1]
-            nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
-            init = [_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
-                                    sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]
-            n = len(cls)
-            ids = np.asarray(cls, dtype=np.int32)
-            ids_d = torch.from_numpy(ids).to(dev)
-            widths = torch.tensor([trackers[c].object_width for c in cls], dtype=torch.float64, device=dev)
-            poses = torch.from_numpy(np.stack(init).astype(np.float64)).to(dev)     # updated in place by every step
-            history = torch.empty((nf, n, 4, 4), dtype=torch.float64, device=dev)
-            history[0].copy_(poses)
-            out_trans = torch.empty((n, 3), dtype=torch.float32, device=dev)
-            out_rot = torch.empty((n, 3), dtype=torch.float32, device=dev)
-            pending = submit(rgb_files[1], depth_files[1], 1) if nf > 1 else None
-            for t in range(1, nf):
-                slot = t % 2
-                for f in pending:
-                    f.result()
-                rgb_d.copy_(host[slot][0], non_blocking=True)
-                depth_d.copy_(host[slot][1], non_blocking=True)
-                uploaded[slot] = torch.cuda.Event()
-                uploaded[slot].record()
-                eng.track_render(rgb_d, depth_d, trk0.K, poses, widths, trk0.trans_normalizer, trk0.rot_normalizer,
-                                 weight_ids_host=ids, weight_ids_dev=ids_d, precision=precision, mode=render.mode,
-                                 image_hw=render.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
-                history[t].copy_(poses)
-                if t + 1 < nf:
-                    pending = submit(rgb_files[t + 1], depth_files[t + 1], (t + 1) % 2)
-            tracked = history.cpu().numpy()
-            for j, c in enumerate(cls):
-                pred_poses = list(tracked[:, j])
-                while len(pred_poses) < len(rgb_files) and max_frames is None:      # predict.py:437-440
-                    pred_poses.append(pred_poses[-1])
-                sdir = os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq{}'.format(seq_id))
-                os.makedirs(sdir, exist_ok=True)
-                for i in range(len(pred_poses)):
-                    np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i])
-                results[c][seq_id] = np.array(pred_poses)
+    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, precision, 2, 2), track_sets.items(),
+                                                       sequences):
+        pred_poses = np.concatenate([init[None], tracked])           # row 0: the start pose, as in getResultsYcb
+        for j, c in enumerate(cls):
+            sdir = os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq{}'.format(seq_id))
+            os.makedirs(sdir, exist_ok=True)
+            for i in range(len(pred_poses)):
+                np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
+            results[c][seq_id] = pred_poses[:, j]
     return results
 
 
@@ -945,12 +955,9 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
 
     Videos and objects as ycbineoat_videos and ycbineoat_objects find and check them.  One Engine holds each object's weights,
     statistics and CUDA-renderer mesh once, under one weight id per object.  Each video starts from its annotated_poses[0] and is
-    tracked from frame 0 with the reference's normalisers (0.03 m, 30 degrees), one n = 1 se3tn_track_render step per frame.  The
-    pose lives in one device tensor that every step updates in place, and the frame in one device buffer, so every step after an
-    object's first replays its CUDA graph; a device history of the poses comes back to the host once per video.  A thread pool
-    decodes up to decode_ahead frames ahead, across video boundaries, into a ring of that many pinned staging sets."""
-    from collections import deque
-    from concurrent.futures import ThreadPoolExecutor
+    tracked from frame 0 with the reference's normalisers (0.03 m, 30 degrees), one n = 1 se3tn_track_render step per frame, so
+    every step after an object's first replays its CUDA graph (_track_sequences).  A thread pool decodes up to decode_ahead
+    frames ahead, across video boundaries, into a ring of that many pinned staging sets."""
     from .eval_ycbineoat import OBJECTS
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
@@ -958,79 +965,19 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     videos = ycbineoat_videos(ycbineoat_dir)
     files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
     objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, precision)
-    eng = Engine(max_batch=1)
-    trackers = {}
-    for obj, k in objects.items():
-        try:
-            trackers[obj] = Tracker(k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], model_path=k['model_path'], engine=eng,
-                                    weight_id=OBJECTS.index(obj), precision=precision, renderer='cuda',
-                                    trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER)
-        except ValueError as e:
-            raise ValueError('object %s: %s' % (obj, e)) from e
-    dev = eng.device
-    # per object: the step's ids and width, kept on the device so the step's addresses stay the same from video to video
-    ids = {o: np.array([OBJECTS.index(o)], dtype=np.int32) for o in trackers}
-    ids_d = {o: torch.from_numpy(ids[o]).to(dev) for o in trackers}
-    widths = {o: torch.tensor([trackers[o].object_width], dtype=torch.float64, device=dev) for o in trackers}
-    poses = torch.empty((1, 4, 4), dtype=torch.float64, device=dev)
-    out_trans = torch.empty((1, 3), dtype=torch.float32, device=dev)
-    out_rot = torch.empty((1, 3), dtype=torch.float32, device=dev)
-    frames = []                                            # (video, object, frame index, frames of the video)
+    eng, trackers = _one_pass_trackers([(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER,
+                                                                                 rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
+                                        for o, k in objects.items()], precision, 1)
+    sequences = {}
     for v, obj in videos:
-        nf = len(files[v][0]) if max_frames is None else min(max_frames, len(files[v][0]))
-        frames += [(v, obj, t, nf) for t in range(nf)]
+        rgb_files, depth_files, gt_files = files[v]
+        nf = len(rgb_files) if max_frames is None else min(max_frames, len(rgb_files))
+        if nf > 0:
+            sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
     results = {}
-    if not frames:
-        return results
-    cam = next(iter(trackers.values())).dataset_info['camera']
-    pinned = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True)
-    host = [(pinned((cam['height'], cam['width'], 3), torch.uint8), pinned((cam['height'], cam['width']), torch.uint16))
-            for _ in range(decode_ahead)]
-    rgb_d = torch.empty(host[0][0].shape, dtype=torch.uint8, device=dev)
-    depth_d = torch.empty(host[0][1].shape, dtype=torch.uint16, device=dev)
-    uploaded = [None] * decode_ahead                       # event after the last upload from each staging set
-
-    def decode_into(dst, read, path):
-        img = read(path)
-        if img.shape != tuple(dst.shape):
-            raise ValueError('%s: %s, the camera image is %s (dataset_info.yml)' % (path, img.shape, tuple(dst.shape)))
-        dst.numpy()[...] = img
-
-    with ThreadPoolExecutor(max_workers=2 * decode_ahead) as pool:
-        pending = deque()
-
-        def submit(k):                                     # frame k decodes into staging set k % decode_ahead
-            v, _, t, _ = frames[k]
-            slot = k % decode_ahead
-            if uploaded[slot] is not None:
-                uploaded[slot].synchronize()               # the staging set's previous upload has left it
-            pending.append([pool.submit(decode_into, host[slot][0], read_rgb, files[v][0][t]),
-                            pool.submit(decode_into, host[slot][1], read_depth, files[v][1][t])])
-
-        for k in range(min(decode_ahead, len(frames))):
-            submit(k)
-        history = None
-        for k, (v, obj, t, nf) in enumerate(frames):
-            if k > 0 and k + decode_ahead - 1 < len(frames):
-                submit(k + decode_ahead - 1)               # into the staging set frame k - 1 was uploaded from
-            for f in pending.popleft():
-                f.result()
-            slot = k % decode_ahead
-            rgb_d.copy_(host[slot][0], non_blocking=True)
-            depth_d.copy_(host[slot][1], non_blocking=True)
-            uploaded[slot] = torch.cuda.Event()
-            uploaded[slot].record()
-            if t == 0:
-                poses.copy_(torch.from_numpy(np.loadtxt(files[v][2][0]).reshape(1, 4, 4)))
-                history = torch.empty((nf, 1, 4, 4), dtype=torch.float64, device=dev)
-            trk = trackers[obj]
-            eng.track_render(rgb_d, depth_d, trk.K, poses, widths[obj], trk.trans_normalizer, trk.rot_normalizer,
-                             weight_ids_host=ids[obj], weight_ids_dev=ids_d[obj], precision=precision, mode=trk.renderer.mode,
-                             image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
-            history[t].copy_(poses)
-            if t == nf - 1:
-                results[v] = history[:, 0].cpu().numpy()
-                write_video_poses(outdir, v, results[v])
+    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), precision, decode_ahead, 2 * decode_ahead), sequences):
+        results[v] = tracked[:, 0]
+        write_video_poses(outdir, v, results[v])
     return results
 
 

@@ -5,22 +5,23 @@ Training (Problem.train, Problem.loop, the optimiser) is out of scope and raises
 validate() returns the reference's number -- the mean over the loader's batches of each batch's nn.MSELoss, translation and
 rotation, weighted by config['loss_weights'] -- but does not iterate the DataLoader.  It reads the dataset's file list and runs
 each batch through se3tn_eval_pairs (Engine.eval_pairs): processData's post-transforms, the network and the loss terms in one
-step on the device.  PNGs are decoded in a thread pool (cv2 releases the GIL) straight into one of two pinned staging buffers,
-so decoding step k+1 overlaps step k on the GPU.  A batch larger than the engine's max_batch runs as several steps whose sums
+step on the device.  PNGs are decoded in a thread pool (cv2 releases the GIL) straight into a StagingRing of two pinned
+staging sets, so decoding step k+1 overlaps step k on the GPU.  A batch larger than the engine's max_batch runs as several steps whose sums
 are added in order.  The pairs are taken in file order (the reference's validation loader does not shuffle, train.py:143-149).
 
     python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
                                  [--precision bf16x3|tf32|bf16|fp32|all] [--batch_size 200]
 """
 import argparse
+import contextlib
 import os
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from .datasets import TrackDataset, read_pair, resize_pair
 from .engine import PREC, IMAGE_SIZE
+from .staging import StagingRing
 
 
 class Problem:
@@ -109,14 +110,11 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
     dev = eng.device
     img = (IMAGE_SIZE, IMAGE_SIZE)
 
-    def pinned(shape, dt):
-        return torch.empty(shape, dtype=dt, pin_memory=True)
-
-    # two pinned staging sets (decode k+1 while step k runs), one device set (the uploads are ordered with the steps on the stream)
-    host = [dict(rgbA=pinned((cap,) + img + (3,), torch.uint8), depthA=pinned((cap,) + img, torch.uint16),
-                 rgbB=pinned((cap,) + img + (3,), torch.uint8), depthB=pinned((cap,) + img, torch.uint16),
-                 poses=pinned((cap, 2, 4, 4), torch.float64)) for _ in range(2)]
-    d = {k: torch.empty(v.shape, dtype=v.dtype, device=dev) for k, v in host[0].items()}
+    # the pinned sets decode step k+1 while step k runs; the one device set is what the steps read (uploads ordered on the stream)
+    ring = StagingRing(dict(rgbA=((cap,) + img + (3,), torch.uint8), depthA=((cap,) + img, torch.uint16),
+                            rgbB=((cap,) + img + (3,), torch.uint8), depthB=((cap,) + img, torch.uint16),
+                            poses=((cap, 2, 4, 4), torch.float64)), 2, dev)
+    d = ring.dev
     A_in_cam, B_in_cam = torch.empty(cap, 4, 4, dtype=torch.float64, device=dev), torch.empty(cap, 4, 4, dtype=torch.float64, device=dev)
     out_trans, out_rot = torch.empty(cap, 3, dtype=torch.float32, device=dev), torch.empty(cap, 3, dtype=torch.float32, device=dev)
     out_sums = torch.empty(2, dtype=torch.float32, device=dev)
@@ -124,13 +122,11 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
     preds = torch.empty(len(files), 6, dtype=torch.float32, device=dev) if keep_predictions else None
     ids_host = np.full(cap, wid, dtype=np.int32) if wid != 0 else None
     ids_dev = torch.from_numpy(ids_host).to(dev) if ids_host is not None else None
-    uploaded = [None, None]                                # event after the last upload from each staging set
     tn, rn = dataset.trans_normalizer, dataset.rot_normalizer
 
-    def decode_into(slot, j, path):
-        """One pair into row j of staging set `slot`; a pair stored at another size comes back whole for the device resize."""
+    def decode_into(h, j, path):
+        """One pair into row j of staging set h; a pair stored at another size comes back whole for the device resize."""
         p = read_pair(path)
-        h = host[slot]
         h['poses'].numpy()[j, 0] = p['A_in_cam']; h['poses'].numpy()[j, 1] = p['B_in_cam']
         if p['rgbB'].shape[0] != res:
             return p
@@ -141,28 +137,17 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
             h[k].numpy()[j] = p[k]
         return None
 
-    with ThreadPoolExecutor(max_workers=workers or min(16, os.cpu_count() or 4)) as pool:
-        def submit(k):
-            slot = k % 2
-            if uploaded[slot] is not None:
-                uploaded[slot].synchronize()               # the staging set's previous upload has left it
+    items = [[(decode_into, j, files[s + j]) for j in range(e - s)] for _, s, e in steps]
+    rows = [e - s for _, s, e in steps]
+    with contextlib.closing(ring.uploads(items, workers or min(16, os.cpu_count() or 4), rows)) as uploads:
+        for k, decoded in enumerate(uploads):
             _, s, e = steps[k]
-            return [pool.submit(decode_into, slot, j, files[s + j]) for j in range(e - s)]
-
-        pending = submit(0)
-        for k, (b, s, e) in enumerate(steps):
-            n, slot = e - s, k % 2
-            odd = [(j, f.result()) for j, f in enumerate(pending)]
-            odd = [(j, p) for j, p in odd if p is not None]
-            h = host[slot]
-            for key in ('rgbA', 'depthA', 'rgbB', 'depthB', 'poses'):
-                d[key][:n].copy_(h[key][:n], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
-            uploaded[slot] = ev
+            n = e - s
             A_in_cam[:n].copy_(d['poses'][:n, 0]); B_in_cam[:n].copy_(d['poses'][:n, 1])
-            for j, p in odd:                               # datasets.py:95-104 on the device
-                rA, dA, rB, dB, seg = resize_pair(eng, p, res)
+            for j, p in enumerate(decoded):
+                if p is None:
+                    continue
+                rA, dA, rB, dB, seg = resize_pair(eng, p, res)          # datasets.py:95-104 on the device
                 mask_sum = int((seg if seg is not None else (dB > 100)).sum().item())
                 if mask_sum <= 0:
                     raise AssertionError('%s: the pair has an empty maskB (datasets.py:104)' % files[s + j])
@@ -174,8 +159,6 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
             all_sums[k].copy_(out_sums)
             if preds is not None:
                 preds[s:e, :3].copy_(out_trans[:n]); preds[s:e, 3:].copy_(out_rot[:n])
-            if k + 1 < len(steps):
-                pending = submit(k + 1)                    # decode the next step while this one runs
     step_sums = all_sums.cpu().numpy()
     bt, br = batch_means(step_sums, steps)
     return dict(trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
