@@ -201,6 +201,34 @@ int se3tn_add_adi_sets(se3tn_ctx* ctx, const double* pts, int M, const int32_t* 
  * call needs more, so a run of calls allocates nothing once the largest has been seen. */
 int se3tn_vocap_sets(se3tn_ctx* ctx, const double* errs, const int32_t* err_set, int n, int n_sets, double* out_ap, void* stream);
 
+/* ---- result videos: each track's model points drawn over its frame (not on the per-frame tracking path) ------------------------- */
+
+/* The frames of the reference's result videos (getResultsYcb, predict.py:424-433; predictSequenceYcb / predictSequenceYcbInEOAT,
+ * predict.py:549-560, 612-624) for n tracks of one frame:  model = copy.deepcopy(tracker.object_cloud); model.transform(pose);
+ * uvs = project_points(model.points, K); cur_bgr = cvtColor(rgb, RGB2BGR); putText(cur_bgr, "frame:..", (W//2, H-50), ...,
+ * color=(255,0,0)); for each uv: circle(cur_bgr, uv, radius=1, color=(0,255,255), thickness=-1); resize(cur_bgr, (W//2, H//2)).
+ *   frame_rgb uint8 (H,W,3) device, H and W even; K HOST fx fy cx cy; poses double (n,16) device.
+ *   pts double (M,3) device, set_offsets int32 (n_sets+1) HOST and track_set int32 (n) HOST: track i draws points
+ *   [set_offsets[s], set_offsets[s+1]) of pts, s = track_set[i], each moved as x' = ((R00 x + R01 y) + R02 z) + t0 (fp64, no
+ *   FMA) and projected as u = (x' fx) / z' + cx, v = (y' fy) / z' + cy, rounded half to even.  A point whose u or v is not finite
+ *   or beyond +-2^30 is not drawn; a point behind the camera is drawn where it lands.  Each point sets the 5 pixels (u, v),
+ *   (u+-1, v), (u, v+-1) that cv2.circle(radius=1, thickness=-1) sets, clipped to the frame.
+ *   label_mask uint8 (label_h, W) device, or NULL for no label: rows [label_y0, label_y0 + label_h) of the frame, non-zero where
+ *   cv2.putText sets a pixel; those pixels take (255,0,0) under or over the points, as label_order says.
+ *   out_bgr uint8 (n, H/2, W/2, 3) device: each track's BGR image, halved as cv2.resize(INTER_LINEAR) halves it, which at an exact
+ *   factor of 2 is (a + b + c + d + 2) >> 2 over each 2 x 2 block.
+ * Plain stream launches, not part of any track step.  SE3TN_ERR_INVALID, with nothing queued, for an odd H or W, label rows
+ * outside the frame, or offsets and ids that se3tn_add_adi_sets would refuse.  The offsets, ids and n one-bit-per-pixel dot masks
+ * (n x H x W / 8 bytes) live in the metrics scratch of se3tn_add_adi_sets, on the same terms. */
+#define SE3TN_LABEL_UNDER_POINTS 0   /* getResultsYcb, predict.py:427-431 */
+#define SE3TN_LABEL_OVER_POINTS  1   /* predictSequenceYcb / YcbInEOAT, predict.py:553-556, 615-618 */
+int se3tn_draw_tracks(se3tn_ctx* ctx, const uint8_t* frame_rgb, int H, int W, const double* K,
+                      const double* poses, int n,
+                      const double* pts, int M, const int32_t* set_offsets, int n_sets,
+                      const int32_t* track_set,
+                      const uint8_t* label_mask, int label_y0, int label_h, int label_order,
+                      uint8_t* out_bgr, void* stream);
+
 /* ---- input A: the rendered previous view (SURVEY.md 8(f) "next" row 2) ------------------------------------- */
 
 /* The CAD model the renderer draws: what VispyRenderer.__init__ uploads as vertex / index buffers (reference
@@ -375,7 +403,8 @@ int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);
 
-/* Bytes of device scratch the context holds for se3tn_add_adi_sets / se3tn_vocap_sets (0 before the first call). */
+/* Bytes of device scratch the context holds for se3tn_add_adi_sets / se3tn_vocap_sets / se3tn_draw_tracks (0 before the first
+ * call). */
 size_t se3tn_metrics_scratch_bytes(se3tn_ctx* ctx);
 
 #ifdef __cplusplus

@@ -8,6 +8,7 @@ LIB_PATH = os.path.join(_HERE, 'libse3tn.so')
 OK, ERR_INVALID, ERR_CUDA, ERR_NOMEM, ERR_STATE, ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5
 PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16 = 0, 1, 2, 3
 RENDER_VISPY, RENDER_PYRENDER = 0, 1
+LABEL_UNDER_POINTS, LABEL_OVER_POINTS = 0, 1
 WEIGHT_BLOB_FLOATS = 13528326
 PROFILE_SLOTS = 22
 TRACE_TILES = 5184
@@ -35,6 +36,7 @@ SIGNATURES = {
     'se3tn_vocap': (_i, [_vp, _vp, _i, C.POINTER(_d), _vp]),
     'se3tn_add_adi_sets': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap_sets': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
+    'se3tn_draw_tracks': (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     'se3tn_allgather_poses': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),

@@ -4,6 +4,7 @@
 #include "conv_common.h"
 #include "aux_kernels.h"
 #include "metrics.h"
+#include "overlay.h"
 #include "render.h"
 #include <dlfcn.h>
 #include "depth_fill.h"
@@ -1214,30 +1215,79 @@ int se3tn_vocap(se3tn_ctx* c, const double* errs, int n, double* out_ap, void* s
     return SE3TN_OK;
 }
 
+namespace {
+// A point table's set offsets (host, n_sets + 1) and the set id (host) of each of n items: SE3TN_ERR_INVALID unless the offsets
+// start at 0, increase strictly and end at M, and every id is in [0, n_sets).
+int check_sets(se3tn_ctx* c, const char* fn, int M, const int32_t* set_offsets, int n_sets, const int32_t* ids, int n, const char* item) {
+    const std::string f(fn);
+    if (set_offsets[0] != 0 || set_offsets[n_sets] != M)
+        return fail(c, SE3TN_ERR_INVALID, f + ": set_offsets must start at 0 and end at M = " + std::to_string(M));
+    for (int s = 0; s < n_sets; ++s)
+        if (set_offsets[s + 1] <= set_offsets[s])
+            return fail(c, SE3TN_ERR_INVALID, f + ": set " + std::to_string(s) + " is empty or its offsets decrease");
+    for (int i = 0; i < n; ++i)
+        if (ids[i] < 0 || ids[i] >= n_sets)
+            return fail(c, SE3TN_ERR_INVALID, f + ": " + item + " " + std::to_string(i) + " has set id " + std::to_string(ids[i]) +
+                                              " outside [0, " + std::to_string(n_sets) + ")");
+    return SE3TN_OK;
+}
+
+// Grows the metrics scratch to hold the checked offsets and ids and `extra` more bytes after them, and queues the upload of the
+// offsets and ids on s.  -> their device copies and the extra bytes (256-byte aligned).
+int stage_sets(se3tn_ctx* c, const int32_t* set_offsets, int n_sets, const int32_t* ids, int n, size_t extra, cudaStream_t s,
+               int32_t** d_off, int32_t** d_ids, uint8_t** d_extra) {
+    const size_t off_bytes = align256(sizeof(int32_t) * (static_cast<size_t>(n_sets) + 1));
+    const size_t id_bytes = align256(sizeof(int32_t) * static_cast<size_t>(n));
+    CU_TRY(c, grow(c->metrics, c->metrics_bytes, off_bytes + id_bytes + extra));
+    *d_off = reinterpret_cast<int32_t*>(c->metrics.get());
+    *d_ids = reinterpret_cast<int32_t*>(c->metrics.get() + off_bytes);
+    *d_extra = c->metrics.get() + off_bytes + id_bytes;
+    CU_TRY(c, cudaMemcpyAsync(*d_off, set_offsets, sizeof(int32_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
+    CU_TRY(c, cudaMemcpyAsync(*d_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+    return SE3TN_OK;
+}
+}  // namespace
+
 int se3tn_add_adi_sets(se3tn_ctx* c, const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* pose_set,
                        const double* pred, const double* gt, int n, double* out_add, double* out_adi, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!pts || !set_offsets || M <= 0 || n_sets <= 0 || n < 0 || (n > 0 && (!pose_set || !pred || !gt || (!out_add && !out_adi))))
         return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: null/invalid argument");
-    if (set_offsets[0] != 0 || set_offsets[n_sets] != M)
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: set_offsets must start at 0 and end at M = " + std::to_string(M));
-    for (int s = 0; s < n_sets; ++s)
-        if (set_offsets[s + 1] <= set_offsets[s])
-            return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: set " + std::to_string(s) + " is empty or its offsets decrease");
-    for (int i = 0; i < n; ++i)
-        if (pose_set[i] < 0 || pose_set[i] >= n_sets)
-            return fail(c, SE3TN_ERR_INVALID, "se3tn_add_adi_sets: pose " + std::to_string(i) + " has set id " + std::to_string(pose_set[i]) +
-                                              " outside [0, " + std::to_string(n_sets) + ")");
-    if (n == 0) return SE3TN_OK;
+    int rc = check_sets(c, "se3tn_add_adi_sets", M, set_offsets, n_sets, pose_set, n, "pose");
+    if (rc || n == 0) return rc;
     DeviceGuard guard(c->device);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const size_t off_bytes = align256(sizeof(int32_t) * (static_cast<size_t>(n_sets) + 1));
-    CU_TRY(c, grow(c->metrics, c->metrics_bytes, off_bytes + sizeof(int32_t) * static_cast<size_t>(n)));
-    int32_t* d_off = reinterpret_cast<int32_t*>(c->metrics.get());
-    int32_t* d_set = reinterpret_cast<int32_t*>(c->metrics.get() + off_bytes);
-    CU_TRY(c, cudaMemcpyAsync(d_off, set_offsets, sizeof(int32_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
-    CU_TRY(c, cudaMemcpyAsync(d_set, pose_set, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+    int32_t *d_off, *d_set; uint8_t* unused;
+    if ((rc = stage_sets(c, set_offsets, n_sets, pose_set, n, 0, s, &d_off, &d_set, &unused))) return rc;
     CU_TRY(c, launch_add_adi_sets(pts, d_off, d_set, pred, gt, n, out_add, out_adi, s));
+    return SE3TN_OK;
+}
+
+int se3tn_draw_tracks(se3tn_ctx* c, const uint8_t* frame_rgb, int H, int W, const double* K, const double* poses, int n,
+                      const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* track_set,
+                      const uint8_t* label_mask, int label_y0, int label_h, int label_order, uint8_t* out_bgr, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !K || !pts || !set_offsets || M <= 0 || n_sets <= 0 || n < 0 || (n > 0 && (!poses || !track_set || !out_bgr)))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_draw_tracks: null/invalid argument");
+    if (H <= 0 || W <= 0 || H % 2 || W % 2 || H > (1 << 15) || W > (1 << 15))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_draw_tracks: the frame must have an even height and width in [2, 32768], not " +
+                                          std::to_string(H) + " x " + std::to_string(W));
+    if (label_order != SE3TN_LABEL_UNDER_POINTS && label_order != SE3TN_LABEL_OVER_POINTS)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_draw_tracks: unknown label_order");
+    if (label_mask && (label_y0 < 0 || label_h <= 0 || label_y0 > H - label_h))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_draw_tracks: label rows [" + std::to_string(label_y0) + ", " +
+                                          std::to_string(static_cast<long long>(label_y0) + label_h) + ") outside the frame");
+    int rc = check_sets(c, "se3tn_draw_tracks", M, set_offsets, n_sets, track_set, n, "track");
+    if (rc || n == 0) return rc;
+    int max_m = 0;
+    for (int i = 0; i < n; ++i) max_m = std::max(max_m, set_offsets[track_set[i] + 1] - set_offsets[track_set[i]]);
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    int32_t *d_off, *d_set; uint8_t* masks;
+    if ((rc = stage_sets(c, set_offsets, n_sets, track_set, n, sizeof(uint32_t) * overlay_mask_words(H, W) * n, s, &d_off, &d_set, &masks)))
+        return rc;
+    CU_TRY(c, launch_draw_tracks(frame_rgb, H, W, K, poses, n, pts, d_off, d_set, max_m, label_mask, label_y0, label_h,
+                                 label_order == SE3TN_LABEL_OVER_POINTS, reinterpret_cast<uint32_t*>(masks), out_bgr, s));
     return SE3TN_OK;
 }
 

@@ -14,6 +14,7 @@ from .weights import pack_state_dict
 
 PREC = {'tf32': _lib.PREC_TF32, 'fp32': _lib.PREC_FP32, 'bf16x3': _lib.PREC_BF16X3, 'bf16': _lib.PREC_BF16}
 IMAGE_SIZE = 176
+LABEL_ORDER = {'under': _lib.LABEL_UNDER_POINTS, 'over': _lib.LABEL_OVER_POINTS}
 
 
 def _ptr(t):
@@ -374,8 +375,39 @@ class Engine:
         return out
 
     def metrics_scratch_bytes(self):
-        """Device bytes the context holds for add_adi_sets / vocap_sets."""
+        """Device bytes the context holds for add_adi_sets / vocap_sets / draw_tracks."""
         return int(self.lib.se3tn_metrics_scratch_bytes(self._ctx))
+
+    # ------------------------------------------------------------------ result videos
+    def draw_tracks(self, frame_rgb, K, poses, points, set_offsets, track_set, label=None, label_order='under', out=None):
+        """Each track's model points drawn over one frame, as the reference's result videos draw them (se3tn_draw_tracks).
+        frame_rgb uint8 CUDA (H,W,3), H and W even; K 3x3 or (fx,fy,cx,cy); poses float64 CUDA (n,4,4); points float64 CUDA (M,3),
+        set_offsets (S+1) and track_set (n) int32 host arrays: track i draws points [set_offsets[s], set_offsets[s+1]), s =
+        track_set[i].  label: None or (y0, mask), mask a uint8 CUDA (rows, W) strip from row y0 that is non-zero where the
+        label's pixels are (label_strip renders one); label_order 'under' (getResultsYcb) or 'over' (predictSequenceYcb /
+        YcbInEOAT) the points.  -> uint8 CUDA (n, H/2, W/2, 3) BGR images (into `out` when given), queued on the current stream."""
+        H, W = int(frame_rgb.shape[0]), int(frame_rgb.shape[1])
+        offs = np.ascontiguousarray(set_offsets, dtype=np.int32).reshape(-1)
+        ids = np.ascontiguousarray(track_set, dtype=np.int32).reshape(-1)
+        n = int(ids.shape[0])
+        if offs.shape[0] < 2:
+            raise ValueError('draw_tracks: set_offsets must hold S+1 >= 2 offsets')
+        if label_order not in LABEL_ORDER:
+            raise ValueError('draw_tracks: label_order must be one of %s' % ', '.join(LABEL_ORDER))
+        self._check_dev('frame_rgb', frame_rgb, torch.uint8, (H, W, 3))
+        self._check_dev('poses', poses, torch.float64, (n, 4, 4))
+        self._check_dev('points', points, torch.float64, (points.shape[0], 3))
+        y0, mask = (0, None) if label is None else (int(label[0]), label[1])
+        if mask is not None:
+            self._check_dev('label mask', mask, torch.uint8, (mask.shape[0], W))
+        if out is None:
+            out = torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=self.device)
+        self._check_dev('out', out, torch.uint8, (n, H // 2, W // 2, 3))
+        _lib.check(self.lib.se3tn_draw_tracks(self._ctx, _ptr(frame_rgb), H, W, _hptr(self._k4(K)), _ptr(poses), n,
+                                              _ptr(points), int(points.shape[0]), _hptr(offs), int(offs.shape[0]) - 1, _hptr(ids),
+                                              _ptr(mask), y0, 0 if mask is None else int(mask.shape[0]), LABEL_ORDER[label_order],
+                                              _ptr(out), _stream(self.device)), self._ctx)
+        return out
 
     # ------------------------------------------------------------------ input A renderer (SURVEY 8f row 2)
     def set_mesh(self, mesh, mesh_id=0):

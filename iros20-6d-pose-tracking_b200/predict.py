@@ -28,7 +28,7 @@ from .engine import Engine
 from .cuda_renderer import CudaRenderer
 from .se3_tracknet import Se3TrackNet
 from .datasets import TrackDataset
-from .staging import StagingRing
+from .staging import StagingRing, VideoSink
 from . import Utils as U
 
 
@@ -420,6 +420,31 @@ def _decode_into(host, name, read, path):
     dst.numpy()[...] = img
 
 
+# The result videos' frame label: cv2.putText(img, text, (W//2, H-50), FONT_HERSHEY_SIMPLEX, fontScale=1, thickness=4)
+# (predict.py:428, 556, 618).  "frame:0" ... "frame:9999999" set pixels in rows H-73 ... H-48 only, so the label is kept as the
+# full-width strip of rows [H - LABEL_TOP, H - LABEL_BOTTOM).
+LABEL_TOP, LABEL_BOTTOM = 80, 40
+
+
+def label_strip(text, H, W, out=None):
+    """(y0, mask): the pixels of the result videos' label `text` on an H x W frame, as a uint8 (LABEL_TOP - LABEL_BOTTOM, W) mask
+    (255 where cv2.putText sets a pixel, 0 elsewhere; LINE_8 draws no anti-aliased edge) of the rows from y0 = H - LABEL_TOP.
+    Written into `out` when given.  Engine.draw_tracks takes it as its label."""
+    import cv2
+    if H < LABEL_TOP:
+        raise ValueError('a labelled video frame needs at least %d rows, not %d' % (LABEL_TOP, H))
+    y0 = H - LABEL_TOP
+    mask = np.zeros((LABEL_TOP - LABEL_BOTTOM, W), dtype=np.uint8) if out is None else out
+    mask[...] = 0
+    cv2.putText(mask, text, (W // 2, H - 50 - y0), cv2.FONT_HERSHEY_SIMPLEX, fontScale=1, thickness=4, color=255)
+    return y0, mask
+
+
+def _label_into(host, text, H, W):
+    """A StagingRing job: the label strip of `text` into the pinned host['label']."""
+    label_strip(text, H, W, host['label'].numpy())
+
+
 def sequence_files(test_data_path):
     """(rgb files, depth files, ground-truth pose files), each sorted (predict.py:584-590)."""
     import glob
@@ -804,7 +829,7 @@ def _one_pass_trackers(entries, precision, max_batch):
     return eng, trackers
 
 
-def _track_sequences(eng, trackers, sequences, precision, depth, workers):
+def _track_sequences(eng, trackers, sequences, precision, depth, workers, video=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode.
     Yields each sequence's (frames, n, 4, 4) numpy poses, the poses after each frame, as soon as the sequence ends.
@@ -813,18 +838,39 @@ def _track_sequences(eng, trackers, sequences, precision, depth, workers):
     sequence boundaries, through one StagingRing of `depth` sets (`workers` threads) into its one device frame.  The step's other
     device arguments are kept: the ids and widths per distinct weight-id tuple, and per n the pose tensor every step updates in
     place and the step's outputs.  So every step after a track set's first replays the step's CUDA graph, across sequences too.
-    After each step the poses are copied into a device history, which comes back to the host once per sequence."""
+    After each step the poses are copied into a device history, which comes back to the host once per sequence.
+
+    video: None, or (label order, [(paths, labels)] per sequence): paths holds one mp4 path per track, labels one text per frame.
+    Then each frame's decode jobs also render its label strip into the ring, and after each step Engine.draw_tracks draws every
+    track's Tracker.object_cloud points at its new pose over the device frame (the point sets uploaded once, as one table), and a
+    VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed."""
     if not sequences:
         return
     dev = eng.device
     cam = trackers[sequences[0][2][0]].dataset_info['camera']
-    ring = StagingRing({'rgb': ((cam['height'], cam['width'], 3), torch.uint8), 'depth': ((cam['height'], cam['width']), torch.uint16)},
-                       depth, dev)
-    frames = [[(_decode_into, 'rgb', read_rgb, r), (_decode_into, 'depth', read_depth, d)]
-              for rgb_files, depth_files, _, _ in sequences for r, d in zip(rgb_files, depth_files)]
-    by_ids, by_n = {}, {}
-    with contextlib.closing(ring.uploads(frames, workers)) as uploads:
-        for rgb_files, _, ids, init in sequences:
+    H, W = int(cam['height']), int(cam['width'])
+    spec = {'rgb': ((H, W, 3), torch.uint8), 'depth': ((H, W), torch.uint16)}
+    if video is not None:
+        spec['label'] = ((LABEL_TOP - LABEL_BOTTOM, W), torch.uint8)
+    ring = StagingRing(spec, depth, dev)
+    frames = []
+    for k, (rgb_files, depth_files, _, _) in enumerate(sequences):
+        for t, (r, d) in enumerate(zip(rgb_files, depth_files)):
+            jobs = [(_decode_into, 'rgb', read_rgb, r), (_decode_into, 'depth', read_depth, d)]
+            if video is not None:
+                jobs.append((_label_into, video[1][k][1][t], H, W))
+            frames.append(jobs)
+    with contextlib.ExitStack() as stack:
+        if video is not None:
+            wids = sorted(set(w for s in sequences for w in s[2]))
+            set_of = {w: j for j, w in enumerate(wids)}
+            clouds = [np.asarray(trackers[w].object_cloud.points, dtype=np.float64).reshape(-1, 3) for w in wids]
+            offsets = np.cumsum([0] + [len(p) for p in clouds]).astype(np.int32)
+            table = torch.from_numpy(np.ascontiguousarray(np.concatenate(clouds))).to(dev)
+            sink = stack.enter_context(contextlib.closing(VideoSink((max(len(s[2]) for s in sequences), H // 2, W // 2, 3), depth, dev)))
+        uploads = stack.enter_context(contextlib.closing(ring.uploads(frames, workers)))
+        by_ids, by_n = {}, {}
+        for k, (rgb_files, _, ids, init) in enumerate(sequences):
             n = len(ids)
             if ids not in by_ids:
                 wh = np.asarray(ids, dtype=np.int32)
@@ -832,28 +878,39 @@ def _track_sequences(eng, trackers, sequences, precision, depth, workers):
                                torch.tensor([trackers[w].object_width for w in ids], dtype=torch.float64, device=dev))
             if n not in by_n:
                 by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
-                           torch.empty((n, 3), dtype=torch.float32, device=dev))
+                           torch.empty((n, 3), dtype=torch.float32, device=dev),
+                           None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
             wh, wd, widths = by_ids[ids]
-            poses, out_trans, out_rot = by_n[n]
+            poses, out_trans, out_rot, drawn = by_n[n]
             poses.copy_(torch.from_numpy(init))
             history = torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev)
             trk = trackers[ids[0]]
+            track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
                 eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                  weight_ids_host=wh, weight_ids_dev=wd, precision=precision, mode=trk.renderer.mode,
                                  image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
                 history[t].copy_(poses)
+                if video is not None:
+                    eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
+                                    label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
+                    sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
             yield history.cpu().numpy()
 
 
-def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None):
+def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
+                     video=False):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
     One Engine holds every class's weights, statistics and CUDA-renderer mesh under weight id = class id.  For each test sequence,
     the tracks are its requested classes in ascending order, each started as getResultsYcb starts it, and every frame after the
-    first is one se3tn_track_render step for all of them (_track_sequences: each frame decoded once, two frames ahead)."""
+    first is one se3tn_track_render step for all of them (_track_sequences: each frame decoded once, two frames ahead).
+
+    video: also write the result video a per-class run writes next to its seq<id>/ (predict.py:403, 424-435): <outdir>/<class
+    folder>/run/seq<id>.mp4, one half-size frame per tracked frame (none for the start pose), the class's model points drawn at
+    their tracked pose over the frame, under the label 'frame:<i+1>' of frame i.  The drawing runs on the device."""
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     classes = ycb_all_classes(ycb_dir, class_ids, class_config, precision)
@@ -871,9 +928,15 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], precision,
                                        max([len(v) for v in track_sets.values()] + [1]))
     name_of = {k['class_id']: k['name'] for k in classes}
+    drawn = None
+    if video:
+        drawn = ('under', [([os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
+                            ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)])
+        for c in name_of.values():
+            os.makedirs(ycb_all_res_dir(outdir, c), exist_ok=True)
     results = {k['class_id']: {} for k in classes}
-    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, precision, 2, 2), track_sets.items(),
-                                                       sequences):
+    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, precision, 2, 2, drawn),
+                                                       track_sets.items(), sequences):
         pred_poses = np.concatenate([init[None], tracked])           # row 0: the start pose, as in getResultsYcb
         for j, c in enumerate(cls):
             sdir = os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq{}'.format(seq_id))
@@ -949,7 +1012,8 @@ def write_video_poses(outdir, video, poses):
         np.savetxt(os.path.join(vdir, '%07d.txt' % i), poses[i])
 
 
-def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None):
+def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
+                        video=False):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -957,7 +1021,12 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     statistics and CUDA-renderer mesh once, under one weight id per object.  Each video starts from its annotated_poses[0] and is
     tracked from frame 0 with the reference's normalisers (0.03 m, 30 degrees), one n = 1 se3tn_track_render step per frame, so
     every step after an object's first replays its CUDA graph (_track_sequences).  A thread pool decodes up to decode_ahead
-    frames ahead, across video boundaries, into a ring of that many pinned staging sets."""
+    frames ahead, across video boundaries, into a ring of that many pinned staging sets.
+
+    video: also write <outdir>/<video>.mp4, a headless stand-in for the window predictSequenceYcbInEOAT shows (predict.py:612-624;
+    the reference itself writes no file there): per frame i, the object's model points drawn at the tracked pose over the frame
+    with the label 'frame:<i>' over them, at half size.  The drawing runs on the device.  eval_ycbineoat lists the .mp4 files
+    among the result folders and finds no pose file in them, so the scores are unchanged."""
     from .eval_ycbineoat import OBJECTS
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
@@ -974,8 +1043,13 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
         nf = len(rgb_files) if max_frames is None else min(max_frames, len(rgb_files))
         if nf > 0:
             sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
+    drawn = None
+    if video:
+        os.makedirs(outdir, exist_ok=True)
+        drawn = ('over', [([os.path.join(outdir, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()])
     results = {}
-    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), precision, decode_ahead, 2 * decode_ahead), sequences):
+    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), precision, decode_ahead, 2 * decode_ahead, drawn),
+                          sequences):
         results[v] = tracked[:, 0]
         write_video_poses(outdir, v, results[v])
     return results
@@ -1003,6 +1077,8 @@ def main(argv=None):
     parser.add_argument('--score', action='store_true', help='ycbv_all / ycbineoat_all: score the output with eval_ycb / '
                         'eval_ycbineoat and print its lines')
     parser.add_argument('--decode_ahead', type=int, default=4, help='ycbineoat_all: frames decoded ahead of the tracking step')
+    parser.add_argument('--video', action='store_true', help='ycbv_all / ycbineoat_all: also write the result videos, each track\'s '
+                        'model points drawn over its frames on the device (<class folder>/run/seq<id>.mp4 / <video>.mp4)')
     args = parser.parse_args(argv)
     if args.mode == 'ycbv_all':
         return _main_ycbv_all(args)
@@ -1032,6 +1108,11 @@ def main(argv=None):
     print('tracked class %d through sequences %s -> %s' % (args.class_id, sorted(res), args.outdir))
 
 
+def _video_kw(args):
+    """The drivers' video argument: passed only when --video asks for the videos, so a run without it makes the same call."""
+    return {'video': True} if args.video else {}
+
+
 def _main_ycbv_all(args):
     """--mode ycbv_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class path templates."""
     import argparse
@@ -1046,7 +1127,8 @@ def _main_ycbv_all(args):
         except ValueError:
             raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames)
+    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames,
+                           **_video_kw(args))
     for c in sorted(res):
         print('tracked class %d through sequences %s' % (c, sorted(res[c])))
     print('-> %s' % args.outdir)
@@ -1071,7 +1153,7 @@ def _main_ycbineoat_all(args):
         raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
     res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
-                              ycb_dir=args.ycb_dir)
+                              ycb_dir=args.ycb_dir, **_video_kw(args))
     for v in res:
         print('tracked %s: %d frames' % (v, len(res[v])))
     print('-> %s' % args.outdir)

@@ -4,13 +4,19 @@ per object, one synchronous n = 1 step per frame), over the same data set.  The 
 each call timed whole (engine set-up, weight and mesh upload, decoding, tracking, writing the pose files); the card's name and
 power limit are read in the same run.
 
-    python scripts/ycb_all_throughput.py [--frames 100] [--rounds 3] [--precision bf16x3]
+    python scripts/ycb_all_throughput.py [--frames 100] [--rounds 3] [--precision bf16x3] [--video]
+
+--video times three legs instead, alternating in the same way: getResultsYcbAll without videos; with video=True (every track
+drawn on the device, written by the video sink); and without videos followed by the reference's own way of making them (the CPU
+oracle's cv2 drawing of every track in every frame on the host, encoding on a writer thread), from frames decoded before the
+timer starts.  It reports the model point counts drawn.
 
 The data set is written to a temporary directory, seeded, and removed afterwards: test sequences 0048..0050 with 5 objects each,
 480 x 640 colour and depth PNGs, synthetic weights, statistics and meshes per class.  Rates: frames/s counts each sequence frame
 once; objects x frames/s counts each tracked object in each frame.
 """
 import argparse, importlib, json, os, subprocess, sys, tempfile, time
+from concurrent.futures import ThreadPoolExecutor
 import cv2
 import numpy as np
 import torch
@@ -67,6 +73,7 @@ def main():
     ap.add_argument('--frames', type=int, default=100, help='frames per sequence')
     ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--precision', default='bf16x3')
+    ap.add_argument('--video', action='store_true', help='time the result videos: device drawing against host drawing')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('needs a CUDA device')
@@ -87,9 +94,41 @@ def main():
                 pr.getResultsYcb(ycb, k['class_id'], k['dataset_info'], k['mean'], k['std'], k['ckpt_dir'], k['model_path'],
                                  os.path.join(tmp, 'pc%d' % r, k['name']), precision=args.precision, max_batch=1)
 
-        times = {'one_pass': [], 'per_class': []}
-        for r in range(args.rounds + 1):                             # round 0 warms both up and is not counted
-            for name, fn in (('one_pass', one_pass), ('per_class', per_class)):
+        def one_pass_video(r):
+            pr.getResultsYcbAll(ycb, classes, templates, os.path.join(tmp, 'vid%d' % r), precision=args.precision, video=True)
+
+        points, frames_rgb = {}, {}
+        if args.video:
+            sys.path.insert(0, os.path.join(ROOT, 'oracle'))
+            import overlay_oracle as OV
+            points = {c: pr.PointCloud(pr.load_vertices(templates['model_path'].format(class_id=c))).voxel_down_sample(voxel_size=0.005).points
+                      for c in classes}
+            frames_rgb = {seq: [pr.read_rgb(os.path.join(ycb, 'data_organized', '%04d' % seq, 'color', '%06d-color.png' % (i + 1)))
+                                for i in range(args.frames)] for seq in SEQS}
+
+        def one_pass_host_video(r):
+            out = os.path.join(tmp, 'host%d' % r)
+            res = pr.getResultsYcbAll(ycb, classes, templates, out, precision=args.precision)
+            names = pr.ycb_class_names(ycb)
+            jobs = []
+            with ThreadPoolExecutor(max_workers=1) as writer:
+                for seq, cls in SEQS.items():
+                    vids = [cv2.VideoWriter(os.path.join(pr.ycb_all_res_dir(out, names[c - 1]), 'seq%d.mp4' % seq),
+                                            cv2.VideoWriter_fourcc(*'mp4v'), 30, (320, 240)) for c in cls]
+                    for i in range(1, args.frames):
+                        drawn = [OV.draw_track(frames_rgb[seq][i], synth_K, res[c][seq][i], points[c], 'frame:%d' % (i + 1), 'under')
+                                 for c in cls]
+                        jobs.append(writer.submit(lambda d=drawn, v=vids: [w.write(f) for w, f in zip(v, d)]))
+                    jobs.append(writer.submit(lambda v=vids: [w.release() for w in v]))
+            for j in jobs:
+                j.result()
+
+        synth_K = pkg.synth.CAMERA_K
+        legs = ((('one_pass', one_pass), ('one_pass_video', one_pass_video), ('one_pass_host_video', one_pass_host_video)) if args.video
+                else (('one_pass', one_pass), ('per_class', per_class)))
+        times = {name: [] for name, _ in legs}
+        for r in range(args.rounds + 1):                             # round 0 warms every leg up and is not counted
+            for name, fn in legs:
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
                 fn(r)
@@ -98,11 +137,14 @@ def main():
                     times[name].append(time.perf_counter() - t0)
     out = {'gpu': gpu, 'torch_device': torch.cuda.get_device_name(0), 'precision': args.precision, 'sequences': len(SEQS),
            'objects_per_sequence': [len(c) for c in SEQS.values()], 'frames_per_sequence': args.frames, 'rounds': args.rounds}
+    if points:
+        out['model_points'] = {c: len(p) for c, p in points.items()}
     for name, ts in times.items():
         out[name] = {'seconds': [round(t, 3) for t in ts],
                      'frames_per_s': [round(seq_frames / t, 1) for t in ts],
                      'object_frames_per_s': [round(obj_frames / t, 1) for t in ts]}
-        print('%-9s frames/s %s   objects x frames/s %s' % (name, out[name]['frames_per_s'], out[name]['object_frames_per_s']))
+        print('%-19s frames/s %s (%.1f-%.1f)   objects x frames/s %s' % (name, out[name]['frames_per_s'], min(out[name]['frames_per_s']),
+                                                                         max(out[name]['frames_per_s']), out[name]['object_frames_per_s']))
     print('card (name, power limit, max SM clock): %s' % gpu)
     print(json.dumps(out))
 
