@@ -2,26 +2,17 @@
 operation run in fp64 on the CPU (oracle/layer_ref.py), and the layer's stored output compared element by element against
 a bound derived from the mode's arithmetic -- in every precision mode and at the batch shapes the kernels split on.
 
-Before each call every conv output buffer (P1A ... H2; also Y1A / Y1B and H3 in the fp32 mode) is filled with 0xFF bytes,
-a NaN in every storage format, through the debug_buffer view into the Engine's own workspace.  After the call each checked
-element must have been overwritten (NaN fails the gate) and every image outside [first, first + n) must still hold the
-poison byte for byte.  The stem inputs X0A / X0B are never poisoned: their halo is the conv padding.
-
-Each case checks the 14 layers plus the head on a sample of its images (first, last and two picked with a seed); `-s`
-prints a per-layer table of the worst ratio of each gate (gate 1 elementwise worst case, gate 2 RMS; both pass at <= 1).
+Poisoning, the images checked and the per-layer tables `-s` prints: tests/layer_harness.py.
 """
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
-import layer_ref as R
+from layer_harness import run_case, track_inputs
 
 pytestmark = pytest.mark.gpu
 
 TN, RN = 0.03, 5 * np.pi / 180
-CONV_OUT = ['P1A', 'P1B', 'T1', 'T2', 'U', 'CAT', 'F1', 'T4', 'F2', 'H1', 'H2']
-FP32_OUT = ['Y1A', 'Y1B', 'H3']
 
 
 def _make_engine(pkg, synth, max_batch):
@@ -46,143 +37,6 @@ def blobs(pkg, synth):
     from importlib import import_module
     pack = import_module(pkg.__name__ + '.weights').pack_state_dict
     return {0: pack(synth.make_state_dict(0)), 1: pack(synth.make_state_dict(1))}
-
-
-def _bytes(eng, buf):
-    """The whole debug_buffer allocation of `buf` (max_batch images at 4 bytes per channel) as a uint8 view."""
-    return eng.debug_buffer(R.BUF_ID[buf], eng.max_batch).view(torch.uint8).reshape(-1)
-
-
-def _out_bufs(prec):
-    return CONV_OUT + (FP32_OUT if prec == 'fp32' else [])
-
-
-def poison(eng, prec):
-    for buf in _out_bufs(prec):
-        _bytes(eng, buf).fill_(0xFF)
-
-
-def check_poison_outside(eng, prec, first, n):
-    """Images outside [first, first + n) -- and, in the 2-byte bf16 mode, the allocation's unused second half -- still hold
-    the poison, byte for byte."""
-    bad = []
-    for buf in _out_bufs(prec):
-        nb = R.image_bytes(buf, R.buf_format(buf, prec))
-        u = _bytes(eng, buf)
-        for part in (u[:first * nb], u[(first + n) * nb:]):
-            if part.numel() and not bool((part == 0xFF).all()):
-                bad.append(buf)
-    assert not bad, 'written outside images [%d, %d): %s' % (first, first + n, bad)
-
-
-def sample_images(first, n, seed):
-    if n <= 4:
-        return list(range(first, first + n))
-    rng = np.random.default_rng(seed)
-    mid = rng.choice(np.arange(first + 1, first + n - 1), size=2, replace=False)
-    return sorted({first, first + n - 1, *(int(i) for i in mid)})
-
-
-def check_image(raw, prec, blob, ksplit, six):
-    """All 14 layers and the head of one image.  raw(buf) -> that image's bytes of buffer buf; blob: the image's fp32
-    weight blob; six: the (6,) trans ++ rot the call returned for it.  -> [(layer name, GateResult)]."""
-    D = {}
-
-    def dec(buf):
-        if buf not in D:
-            D[buf] = R.decode(raw(buf), buf, R.buf_format(buf, prec))
-        return D[buf]
-
-    W = lambda li: R.layer_weights(blob, li)
-    rows = []
-
-    def one(li, out_value, res=None, **kw):
-        L = R.LAYERS[li]
-        w, b = W(li)
-        ref = R.layer_ref(li, prec, dec(L.inp), w, b, res=dec(res) if res else None, ksplit=ksplit, **kw)
-        rows.append((L.name, R.gate(out_value, ref)))
-        return ref
-
-    cat = dec('CAT').value                          # convA2.conv2 writes channels 0-63, convB3.conv2 64-127
-    # stems: the tensor-core modes store the fused max-pool, the fp32 mode the conv (Y1) and then a separate max-pool
-    for li, y1, p1 in ((0, 'Y1A', 'P1A'), (1, 'Y1B', 'P1B')):
-        if prec == 'fp32':
-            one(li, dec(y1).value, pool=False)
-            pooled = F.max_pool2d(torch.from_numpy(dec(y1).value)[None], 3, 2, 1)[0].numpy()
-            same = np.array_equal(pooled, dec(p1).value, equal_nan=False)
-            rows.append(('maxpool %s -> %s (bit-exact)' % (y1, p1), R.GateResult(0.0 if same else np.inf, 0.0, same, pooled.size)))
-        else:
-            one(li, dec(p1).value)
-    one(2, dec('T1').value)
-    one(3, cat[:64], res='P1A')
-    # convB2.conv1's output T2 is overwritten by convB3.conv1: check convB2.conv2 through both layers from P1B
-    w4, b4 = W(4); w5, b5 = W(5)
-    _, r5 = R.chained_ref(4, prec, dec('P1B'), w4, b4, w5, b5, res2=dec('P1B'), ksplit=ksplit)
-    rows.append((R.LAYERS[4].name + ' + conv2', R.gate(dec('U').value, r5)))
-    one(6, dec('T2').value)
-    one(7, cat[64:], res='U')
-    one(8, dec('F1').value)
-    one(9, dec('T4').value)
-    one(10, dec('F2').value, res='F1')
-    one(11, dec('H1').value)
-    one(12, dec('H2').value)
-    fcw, fcb = R.fc_weights(blob)
-    if prec == 'fp32':
-        one(13, dec('H3').value, res='H1')
-        h3 = torch.from_numpy(dec('H3').value).double()
-        out, bound = R.head_ref(h3, torch.zeros_like(h3), fcw, fcb, R.C_POOL_FP32)
-    else:
-        # H3 is never stored: the average pool is fused into the last conv's epilogue.  Check that layer through the head.
-        w, b = W(13)
-        ref = R.layer_ref(13, prec, dec('H2'), w, b, res=dec('H1'), ksplit=ksplit, out_fmt='fp32')
-        out, bound = R.head_ref(ref.y, ref.bound(), fcw, fcb, R.C_POOL_TC)
-    d = torch.as_tensor(np.asarray(six, dtype=np.float64))
-    finite = bool(torch.isfinite(d).all())
-    rows.append(('head (trans, rot)', R.GateResult(float(((d - out).abs() / bound).max()) if finite else np.inf, 0.0, finite, 6)))
-    return rows
-
-
-def report(label, per_image):
-    """Per-layer table of the worst ratio of each gate over the sampled images; asserts every row passed."""
-    names = [n for n, _ in per_image[0][1]]
-    print('\n%s  (images %s)' % (label, [i for i, _ in per_image]))
-    print('  %-34s %10s %10s' % ('layer', 'gate 1', 'gate 2'))
-    failed = []
-    for k, name in enumerate(names):
-        gs = [rows[k][1] for _, rows in per_image]
-        worst, rms = max(g.worst for g in gs), max(g.rms for g in gs)
-        print('  %-34s %10.3g %10.3g%s' % (name, worst, rms, '' if all(g.ok for g in gs) else '   FAIL'))
-        failed += ['%s image %d: %r at %s' % (name, i, rows[k][1], rows[k][1].where) for i, rows in per_image if not rows[k][1].ok]
-    assert not failed, '\n'.join(failed)
-
-
-def run_case(eng, prec, first, n, call, wids, blobs, label, seed=0):
-    """Poison, run `call` (-> trans (n,3), rot (n,3), feature or None), check the untouched images, then every layer of
-    the sampled ones.  wids: weight-set id per image of the call."""
-    poison(eng, prec)
-    trans, rot, feat = call()
-    torch.cuda.synchronize()
-    check_poison_outside(eng, prec, first, n)
-    six = torch.cat((trans, rot), 1).cpu().numpy()
-    ks = R.trunk_ksplit(n, prec)
-    if feat is not None:                           # the feature output is the F2 buffer through launch_nhwc_to_nchw, bit for bit
-        nb = R.image_bytes('F2', prec)
-        f2 = _bytes(eng, 'F2')[first * nb:(first + n) * nb].cpu().numpy()
-        fc = feat.cpu().numpy()
-        for j in range(n):
-            assert np.array_equal(R.decode(f2[j * nb:(j + 1) * nb], 'F2', prec).value, fc[j]), 'feature %d != decoded F2' % j
-    per_image = []
-    for i in sample_images(first, n, seed):
-        cache = {}
-
-        def raw(buf, i=i):
-            nb = R.image_bytes(buf, R.buf_format(buf, prec))
-            if buf not in cache:
-                cache[buf] = _bytes(eng, buf)[i * nb:(i + 1) * nb].cpu().numpy()
-            return cache[buf]
-
-        per_image.append((i, check_image(raw, prec, blobs[int(wids[i - first])], ks, six[i - first])))
-    report('%s, %s, n = %d%s (ksplit %d)' % (label, prec, n, ', first = %d' % first if first else '', ks), per_image)
 
 
 # ------------------------------------------------------------------------------------------- Engine.forward
@@ -232,20 +86,13 @@ def test_forward_preprocessed_offset(synth, eng, blobs, prec):
 
 
 # ------------------------------------------------------------------------------------------- track_batch
-def _track_inputs(synth, n, seed):
-    rgb, depth = synth.raw_frame(seed)
-    poses = synth.raw_poses(n, seed=seed)
-    rgbA, depthA = synth.rendered_views(n, poses, seed=seed)
-    return rgb, depth, poses, rgbA, depthA
-
-
 @pytest.mark.parametrize('prec', ['bf16x3', 'bf16'])
 def test_track_batch_per_image_weights(synth, eng, blobs, prec):
     """A raw-regime frame (normalised magnitudes up to ~40), 37 tracks with weight ids alternating 0 / 1: per-image weight
     maps and biases (gbmaps / gbias) in the resident and trunk kernels; the reference uses each image's own set.  In bf16x3
     a second call with new poses replays the step's CUDA graph and must write the same buffers correctly."""
     n = 37
-    rgb, depth, poses, rgbA, depthA = _track_inputs(synth, n, 5)
+    rgb, depth, poses, rgbA, depthA = track_inputs(synth, n, 5)
     dev = eng.device
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     wid = np.arange(n, dtype=np.int32) % 2
@@ -269,7 +116,7 @@ def test_track_batch_per_image_weights(synth, eng, blobs, prec):
 def test_track_batch_fp32_runs(synth, eng, blobs):
     """fp32: one FFMA forward per run of equal ids ([0, 0], [1, 1, 1], [0]): the direct path at nonzero `first`."""
     n = 6
-    rgb, depth, poses, rgbA, depthA = _track_inputs(synth, n, 8)
+    rgb, depth, poses, rgbA, depthA = track_inputs(synth, n, 8)
     dev = eng.device
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     wid = np.array([0, 0, 1, 1, 1, 0], dtype=np.int32)

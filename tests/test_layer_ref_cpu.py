@@ -266,3 +266,19 @@ def test_chained_bound_accepts_stand_in():
         g2 = R.gate(stand_in(5, prec, t2d, w2, b2, res=x), r2)
         print('chained %s: conv1 %r, conv2 %r' % (prec, g1, g2))
         assert g1.ok and g2.ok
+
+
+def test_sample_images_sees_two_weight_sets():
+    """The device tests' image sample (tests/layer_harness.py): with weight ids given it holds the first image's id and another
+    one whenever the call has another; without a second id in the call it is the plain seeded sample."""
+    from layer_harness import sample_images
+    for seed in range(20):
+        plain = sample_images(3, 12, seed)
+        assert sample_images(3, 12, seed, [5] * 12) == plain and len(plain) == 4 and {3, 14} <= set(plain)
+        for j in range(1, 11):                       # one image of another id, anywhere between the first and the last
+            ids = [5] * 12
+            ids[j] = 2
+            got = sample_images(3, 12, seed, ids)
+            assert 3 + j in got and {3, 14} <= set(got) and set(got) <= set(range(3, 15)), (seed, j, got)
+            if 3 + j in plain:
+                assert got == plain
