@@ -37,8 +37,20 @@ enum {
     SE3TN_PREC_FP32 = 1,    /* plain FFMA direct convolution, no operand rounding (cross-check mode)         */
     SE3TN_PREC_BF16X3 = 2,  /* wgmma bf16 on bf16 hi/lo splits, 3 products per MAC: ~2^-16 relative
                                error (fp32-faithful for the gate) at 1.5x the tensor time of TF32            */
-    SE3TN_PREC_BF16 = 3     /* wgmma bf16, bf16 operands, 1 product per MAC (BASELINE configs[2])     */
+    SE3TN_PREC_BF16 = 3,    /* wgmma bf16, bf16 operands, 1 product per MAC (BASELINE configs[2])     */
+    SE3TN_PREC_FP8 = 4      /* the stems and 64-channel layers as SE3TN_PREC_BF16; the six trunk layers (convAB1 ...
+                               {trans,rot}_conv2.conv2) on wgmma e4m3 with e4m3 activations and weights and
+                               power-of-two scales.  Needs a weight set's activation scales (se3tn_calibrate_fp8 or
+                               se3tn_set_fp8_scales).  Lossy: see DESIGN.md §2 for its measured error             */
 };
+
+/* SE3TN_PREC_FP8's activation scales, one per e4m3 tensor, in this order: CAT (convAB1's input), F1, T4, F2, then
+ * H1 of the trans head, H1 of the rot head, H2 of the trans head, H2 of the rot head.  A stored e4m3 code q means
+ * q * s.  Every scale is a power of two. */
+#define SE3TN_FP8_SCALES 8
+/* Headroom H of se3tn_calibrate_fp8: s = 2^ceil(log2(max|x| * H / 448)), so the calibration's largest value lands at
+ * or below 448 / H (scripts/fp8_study.py: H = 1 ... 8 move the 6-vector's worst error by under 4 %; 2 is the lowest). */
+#define SE3TN_FP8_HEADROOM 2
 
 #define SE3TN_IMAGE_SIZE 176           /* reference dataset_info.yml:15 `resolution`          */
 #define SE3TN_WEIGHT_BLOB_FLOATS 13528326u  /* see se3tn_load_weights                          */
@@ -77,6 +89,18 @@ int se3tn_load_weights(se3tn_ctx* ctx, int weight_id, const float* blob, size_t 
  * A's 4 channels then B's.  `is_f64` selects the arithmetic of the normalisation so that it
  * reproduces numpy's for float32 resp. float64 mean/std arrays (data_augmentation.py:159-163). */
 int se3tn_set_stats(se3tn_ctx* ctx, int weight_id, const void* mean8, const void* std8, int is_f64);
+
+/* SE3TN_PREC_FP8's activation scales of weight set `weight_id` (SE3TN_FP8_SCALES values, the order above).
+ * se3tn_calibrate_fp8 runs the SE3TN_PREC_BF16X3 forward of the set on n normalised pairs A, B (as se3tn_forward
+ * takes them; n <= max_batch), reduces max|x| over each e4m3 tensor as stored, and sets s = 2^ceil(log2(max|x| *
+ * SE3TN_FP8_HEADROOM / 448)) (1 where max|x| is 0).  It synchronises the device.
+ * se3tn_set_fp8_scales sets saved ones: non-finite, non-positive or non-power-of-two values return SE3TN_ERR_INVALID.
+ * se3tn_get_fp8_scales copies them out; a set without scales returns SE3TN_ERR_STATE.
+ * The scales live at fixed device addresses: a captured step replays with the values set last.  An SE3TN_PREC_FP8
+ * step for a set without scales returns SE3TN_ERR_STATE and launches nothing; se3tn_load_weights drops a set's scales. */
+int se3tn_calibrate_fp8(se3tn_ctx* ctx, int weight_id, const float* A, const float* B, int n, void* stream);
+int se3tn_set_fp8_scales(se3tn_ctx* ctx, int weight_id, const float* scales, int n_scales);
+int se3tn_get_fp8_scales(se3tn_ctx* ctx, int weight_id, float* scales, int n_scales);
 
 /* ---- the hot path ---------------------------------------------------------------------------- */
 

@@ -6,7 +6,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libse3tn.so')
 
 OK, ERR_INVALID, ERR_CUDA, ERR_NOMEM, ERR_STATE, ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5
-PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16 = 0, 1, 2, 3
+PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16, PREC_FP8 = 0, 1, 2, 3, 4
+FP8_SCALES = 8
 RENDER_VISPY, RENDER_PYRENDER = 0, 1
 LABEL_UNDER_POINTS, LABEL_OVER_POINTS = 0, 1
 WEIGHT_BLOB_FLOATS = 13528326
@@ -23,6 +24,9 @@ SIGNATURES = {
     'se3tn_last_error': (C.c_char_p, [_vp]),
     'se3tn_load_weights': (_i, [_vp, _i, _vp, _sz]),
     'se3tn_set_stats': (_i, [_vp, _i, _vp, _vp, _i]),
+    'se3tn_calibrate_fp8': (_i, [_vp, _i, _vp, _vp, _i, _vp]),
+    'se3tn_set_fp8_scales': (_i, [_vp, _i, _vp, _i]),
+    'se3tn_get_fp8_scales': (_i, [_vp, _i, _vp, _i]),
     'se3tn_preprocess': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_normalize': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     'se3tn_compute_bbox': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),

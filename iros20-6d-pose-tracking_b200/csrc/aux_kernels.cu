@@ -577,7 +577,7 @@ cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, floa
 // in: the storage format of PREC (storage.cuh), C % 4 == 0.  One CTA transposes 32 pixels x 32 channels.
 template <int PREC>
 __global__ void __launch_bounds__(256)
-nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int HW, int C)
+nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int HW, int C, const float* __restrict__ fp8_scale)
 {
     using R = Raw<PREC, 4>;
     __shared__ float tile[32][33];
@@ -593,6 +593,11 @@ nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int
 #pragma unroll
             for (int q = 0; q < R::kPieces; ++q) r.set(q, *R::at(src, q));
             Storage<PREC>::decode(r, v);
+            if constexpr (PREC == SE3TN_PREC_FP8) {
+                const float sc = *fp8_scale;           // a power of two: exact
+#pragma unroll
+                for (int e = 0; e < 4; ++e) v[e] *= sc;
+            }
         }
 #pragma unroll
         for (int e = 0; e < 4; ++e) tile[j][4 * g + e] = v[e];
@@ -605,16 +610,20 @@ nhwc_to_nchw_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int
     }
 }
 
-cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s) {
+cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s,
+                                const float* fp8_scale) {
     if (n_img <= 0) return cudaSuccess;
     if (C % 4) return cudaErrorInvalidValue;
     dim3 grid((HW + 31) / 32, (C + 31) / 32, n_img);
     const uint8_t* src = static_cast<const uint8_t*>(in);
     switch (precision) {
         case SE3TN_PREC_FP32:            // plain fp32 words decode like tf32 ones
-        case SE3TN_PREC_TF32:   nhwc_to_nchw_kernel<SE3TN_PREC_TF32><<<grid, 256, 0, s>>>(src, out, HW, C); break;
-        case SE3TN_PREC_BF16X3: nhwc_to_nchw_kernel<SE3TN_PREC_BF16X3><<<grid, 256, 0, s>>>(src, out, HW, C); break;
-        case SE3TN_PREC_BF16:   nhwc_to_nchw_kernel<SE3TN_PREC_BF16><<<grid, 256, 0, s>>>(src, out, HW, C); break;
+        case SE3TN_PREC_TF32:   nhwc_to_nchw_kernel<SE3TN_PREC_TF32><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
+        case SE3TN_PREC_BF16X3: nhwc_to_nchw_kernel<SE3TN_PREC_BF16X3><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
+        case SE3TN_PREC_BF16:   nhwc_to_nchw_kernel<SE3TN_PREC_BF16><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
+        case SE3TN_PREC_FP8:
+            if (!fp8_scale) return cudaErrorInvalidValue;
+            nhwc_to_nchw_kernel<SE3TN_PREC_FP8><<<grid, 256, 0, s>>>(src, out, HW, C, fp8_scale); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
@@ -644,6 +653,78 @@ cudaError_t launch_encode_weights(int precision, const float* src, void* dst, in
         case SE3TN_PREC_BF16:   encode_weights_kernel<SE3TN_PREC_BF16><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
         default: return cudaErrorInvalidValue;
     }
+    return cudaGetLastError();
+}
+
+// SE3TN_PREC_FP8 weights: one CTA per row.  s_w = 2^ceil(log2(max|w| / 448)) (pow2_scale), codes e4m3(w / s_w).
+__device__ __forceinline__ float pow2_scale_dev(float amax) {
+    if (!(amax > 0.f)) return 1.f;
+    int ex;
+    const float m = frexpf(amax, &ex);            // amax = m 2^ex, m in [0.5, 1); 448 = 0.875 2^9
+    return ldexpf(1.f, ex - 9 + (m > 0.875f ? 1 : 0));
+}
+__global__ void __launch_bounds__(256)
+encode_weights_fp8_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, float* __restrict__ row_scale, int ktot)
+{
+    __shared__ float red[8];
+    const int row = blockIdx.x;
+    const float* w = src + static_cast<size_t>(row) * ktot;
+    float m = 0.f;
+    for (int k = threadIdx.x; k < ktot; k += 256) m = fmaxf(m, fabsf(w[k]));
+#pragma unroll
+    for (int off = 16; off; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    m = red[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
+    const float sw = pow2_scale_dev(m), inv = 1.f / sw;
+    if (threadIdx.x == 0) row_scale[row] = sw;
+    using S = Storage<SE3TN_PREC_FP8>;
+    for (int k = 4 * threadIdx.x; k < ktot; k += 4 * 256) {
+        const float v[4] = {w[k] * inv, w[k + 1] * inv, w[k + 2] * inv, w[k + 3] * inv};
+        S::encode(v).store(dst + S::addr(row, ktot, k));
+    }
+}
+cudaError_t launch_encode_weights_fp8(const float* src, void* dst, float* row_scale, int rows, int ktot, cudaStream_t s) {
+    if (rows <= 0 || ktot <= 0 || ktot % 128) return cudaErrorInvalidValue;
+    encode_weights_fp8_kernel<<<rows, 256, 0, s>>>(src, static_cast<uint8_t*>(dst), row_scale, ktot);
+    return cudaGetLastError();
+}
+
+// max|x| of bf16x3 tensors as stored: one grid row per tensor, atomicMax on the fp32 bits (non-negative floats order as
+// their bits; NaN's bits exceed +inf's, so a NaN shows as a non-finite maximum)
+__global__ void __launch_bounds__(256) amax_bf16x3_kernel(AmaxArgs a, unsigned* __restrict__ amax_bits)
+{
+    const AmaxArgs::Tensor t = a.t[blockIdx.y];
+    const int groups = t.nc / 4;
+    const size_t total = static_cast<size_t>(a.n) * t.pixels * groups;
+    using S = Storage<SE3TN_PREC_BF16X3>;
+    using R = Raw<SE3TN_PREC_BF16X3, 4>;
+    float m = 0.f;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const size_t pix = i / groups;
+        const int c = t.c0 + 4 * static_cast<int>(i - pix * groups);
+        const uint8_t* p = t.buf + S::addr(pix, t.C, c);
+        R r;
+#pragma unroll
+        for (int q = 0; q < R::kPieces; ++q) r.set(q, *R::at(p, q));
+        float v[4];
+        S::decode(r, v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) m = (fabsf(v[e]) > m || v[e] != v[e]) ? fabsf(v[e]) : m;
+    }
+#pragma unroll
+    for (int off = 16; off; off >>= 1) {
+        const float o = __shfl_xor_sync(0xffffffffu, m, off);
+        m = (o > m || o != o) ? o : m;
+    }
+    if ((threadIdx.x & 31) == 0) atomicMax(amax_bits + blockIdx.y, __float_as_uint(m));
+}
+cudaError_t launch_amax_bf16x3(const AmaxArgs& a, unsigned* amax_bits, cudaStream_t s) {
+    if (a.n_tensors <= 0 || a.n_tensors > AmaxArgs::kMax || a.n <= 0) return cudaErrorInvalidValue;
+    for (int i = 0; i < a.n_tensors; ++i) if (a.t[i].nc % 4 || a.t[i].c0 % 4) return cudaErrorInvalidValue;
+    amax_bf16x3_kernel<<<dim3(132, a.n_tensors), 256, 0, s>>>(a, amax_bits);
     return cudaGetLastError();
 }
 

@@ -64,10 +64,23 @@ cudaError_t launch_pair_loss(const float* trans, const float* rot, const double*
                              const LossArgs& loss, int n, float* sums, cudaStream_t s);
 cudaError_t launch_head(const float* x, const float* fcw, const float* fcb, float* out_trans, float* out_rot,
                         int n_img, int npix, cudaStream_t s);
-// `in` points at the first image, in the activation format of `precision` (SE3TN_PREC_*)
-cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s);
+// `in` points at the first image, in the activation format of `precision` (SE3TN_PREC_*); SE3TN_PREC_FP8: fp8_scale (device)
+// is the tensor's scale
+cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, int C, int precision, cudaStream_t s,
+                                const float* fp8_scale = nullptr);
 // fp32 weight matrix [rows][ktot] -> the weight format of a tensor-core precision (storage.cuh)
 cudaError_t launch_encode_weights(int precision, const float* src, void* dst, int rows, int ktot, cudaStream_t s);
+// SE3TN_PREC_FP8 weights: e4m3 codes of w / s_w[row] (K-major, ktot bytes per row) and the per-row power-of-two scales
+// s_w[row] = 2^ceil(log2(max_k |w[row][k]| / 448)), 1 for an all-zero row
+cudaError_t launch_encode_weights_fp8(const float* src, void* dst, float* row_scale, int rows, int ktot, cudaStream_t s);
+// max|x| over images [0, n) of up to kMax bf16x3-format NHWC tensors (channels [c0, c0 + nc) of C): amax_bits[i] receives
+// tensor i's maximum as fp32 bits through atomicMax (the caller zeroes them first)
+struct AmaxArgs {
+    static constexpr int kMax = 8;
+    struct Tensor { const uint8_t* buf; int pixels, C, c0, nc; } t[kMax];
+    int n_tensors, n;
+};
+cudaError_t launch_amax_bf16x3(const AmaxArgs& a, unsigned* amax_bits, cudaStream_t s);
 cudaError_t launch_permute_rows64(const float* src /*[64][ktot]*/, float* dst, int ktot, cudaStream_t s);
 cudaError_t launch_split_stack_weights(const float* src, void* dst /*[128][9*32 | 7*32 words]*/, bool stem, cudaStream_t s);
 cudaError_t launch_pose_update(const double* poses_in, const float* trans, const float* rot, float tn, float rn,

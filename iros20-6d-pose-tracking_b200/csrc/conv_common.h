@@ -83,6 +83,10 @@ struct LayerDesc {
     int out_c, out_coff;   // channels per pixel of the output buffer, channel offset of this layer's channel 0
     int res_c;             // channels per pixel of the residual buffer
     int li;                // row of the per-set tables (layer index)
+    // SE3TN_PREC_FP8 (a weight set's fp8 block, kFp8BlockFloats: scales, then per-layer mul tables): scale indices of the
+    // e4m3 output and residual (-1: not e4m3), plus ch / q_grp_ch when q_grp_ch > 0 (the heads' per-group scales); offset
+    // of this layer's mul[co] = s_in * s_w[co] table
+    int q_out, q_res, q_grp_ch, fp8_mul;
     // trunk scheduling
     int unit_base;         // first global work-unit index of this layer (units are K-split pieces when TrunkParams::ksplit > 1)
     int base_unit0;        // index of this layer's first UNSPLIT unit among all unsplit units of the launch (split-K scratch / counters)
@@ -92,6 +96,12 @@ struct LayerDesc {
 };
 
 constexpr int kTrunkMaxLayers = 6;
+
+// A weight set's SE3TN_PREC_FP8 block (floats): the SE3TN_FP8_SCALES activation scales (padded to 16 floats), then per trunk
+// layer its mul[co] = s_in(co) * s_w[co], rows 256, 256, 256, 1024, 1024, 1024.  At a fixed device address for the set's life.
+constexpr int kFp8MulBase = 16;
+constexpr int kFp8TrunkRows[kTrunkMaxLayers] = {256, 256, 256, 1024, 1024, 1024};
+constexpr int kFp8BlockFloats = kFp8MulBase + 256 * 3 + 1024 * 3;
 
 struct TrunkParams {
     LayerDesc layer[kTrunkMaxLayers];
@@ -110,6 +120,8 @@ struct TrunkParams {
     int ksplit;
     float* partial;                // [unsplit unit][piece][4 warp slices][64-row half][32-column block][float4 0..3][lane]
     unsigned* slice_cnt;           // [unsplit unit][4 warp slices] number of pieces that have dumped the slice (zeroed before the launch)
+    const float* fp8;              // SE3TN_PREC_FP8: the fp8 block of the single set
+    const float* const* gfp8;      // SE3TN_PREC_FP8, multi-set: fp8 block per set id
 };
 
 struct ResidentParams {
@@ -120,6 +132,8 @@ struct ResidentParams {
     const int* img_wid;
     const CUtensorMap* gbmaps;
     const float* const* gbias;
+    const float* fp8;              // SE3TN_PREC_FP8 (the layers that write CAT in e4m3): as TrunkParams
+    const float* const* gfp8;
     unsigned long long* trace;
     unsigned long long* tile_trace;    // SE3TN_TRACE: this launch's [SE3TN_TRACE_TILES][4] per-tile stamps (include/se3tn.h)
 };

@@ -23,7 +23,9 @@
 //   * registers: a whole-tile accumulator takes up to 128 registers per consumer thread; setmaxnreg moves them from the
 //     producer warpgroup (168 at launch -> 40) to the consumers (-> 232).
 //   * PREC (an SE3TN_PREC_* value) selects arithmetic and storage (storage.cuh): TF32 (4 x k8 tf32 MMAs per chunk-tap),
-//     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product).
+//     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product), FP8 (the
+//     trunk on e4m3 codes, 4 x k32 MMAs per chunk-tap; epilogue acc * mul[co] + bias (+ residual code * s_res), then the
+//     code of y / s_out; in the resident kernel FP8 means the bf16 layer that writes CAT as e4m3).
 //   * programmatic dependent launch: every CTA signals launch_dependents at entry; only the threads that touch
 //     activations execute griddepcontrol.wait, so barrier init and the weight TMA run under the previous kernel's tail.
 //   * per-object weights (reference README.md:132: one checkpoint per object class): with img_wid every work unit takes
@@ -214,7 +216,8 @@ __device__ __forceinline__ void load_a_units(const LayerDesc& L, int ox, int oy,
 }
 
 // The MMAs of one 128-byte K chunk: four K steps of 32 bytes (tf32 k8 with PREC == SE3TN_PREC_TF32, bf16 k16 in the bf16
-// modes) at N = 64 or 128.  a_lo / b_lo: low descriptor words (+2 per K step).  fresh == 0: the first step overwrites acc.
+// modes, e4m3 k32 in SE3TN_PREC_FP8 (trunk only, N = 128)) at N = 64 or 128.  a_lo / b_lo: low descriptor words (+2 per K
+// step).  fresh == 0: the first step overwrites acc.
 template <int PREC, int N>
 __device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t fresh) {
 #pragma unroll
@@ -223,6 +226,9 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a_lo, ui
         const uint32_t f = fresh | (kk ? 1u : 0u);
         if constexpr (PREC == SE3TN_PREC_TF32) {
             if constexpr (N == 64) ptx::wgmma_tf32_n64(acc, a, b, f); else ptx::wgmma_tf32_n128(acc, a, b, f);
+        } else if constexpr (PREC == SE3TN_PREC_FP8) {
+            static_assert(N == 128, "e4m3 MMAs only in the trunk");
+            ptx::wgmma_e4m3_n128(acc, a, b, f);
         } else {
             if constexpr (N == 64) ptx::wgmma_bf16_n64(acc, a, b, f); else ptx::wgmma_bf16_n128(acc, a, b, f);
         }
@@ -279,11 +285,15 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
 
 // PP: ping-pong schedule (consumer warpgroup g owns the CTA's tiles it % 2 == g, both 64-row halves); otherwise the halves
 // schedule (each consumer warpgroup owns one half of every tile), for launches where no CTA has a second tile to overlap with.
+// PREC == SE3TN_PREC_FP8: a 64-channel layer that writes CAT: bf16 operands and arithmetic (AP), the output encoded to e4m3
+// with CAT's scale in the epilogue.
 template <int KIND, int PREC, bool PP>
 __global__ void __launch_bounds__(kThreads2, 1)
 conv_resident_kernel(const __grid_constant__ ResidentParams p)
 {
-    using C = RCfg<KIND, PREC>;
+    constexpr int AP = resident_prec(PREC);                             // operand format and arithmetic
+    static_assert(PREC != SE3TN_PREC_FP8 || KIND == KIND_S1, "e4m3 output: the 64-channel layers only");
+    using C = RCfg<KIND, AP>;
     using KT = KTab<KIND>;
     constexpr bool POOL = C::POOL;
     constexpr int NH = PP ? 2 : 1;                                      // 64-row halves of a tile one consumer warpgroup computes
@@ -365,7 +375,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
         // ============================== MMA + epilogue (two warpgroups) ==========================
         ptx::setmaxnreg_inc<kConsumerRegs>();
         ptx::grid_dep_wait();                       // residual reads / output writes must follow the previous kernel
-        using S = Storage<PREC>;
+        using S = Storage<AP>;
         const Consumer cs;
         const bool stamp = threadIdx.x == 128;
         const bool tstamp = cs.leader() && (PP || cs.cg == 0);     // per-tile stamps (tile_stamp)
@@ -407,7 +417,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
             // the second half's once the first half's accumulator registers are free (0 spills; their latency then overlaps
             // the first half's epilogue and the other warpgroup's MMAs).
             constexpr int kPreRes = (PP && C::kStack == 2) ? 1 : NH;
-            size_t rpix[NH][2]; bool rvalid[NH][2]; Raw<PREC, 8> rres[NH][2][2];
+            size_t rpix[NH][2]; bool rvalid[NH][2]; Raw<AP, 8> rres[NH][2][2];
             auto load_res = [&](int hf) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -418,11 +428,11 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                     rpix[hf][h] = (static_cast<size_t>(n0) * L.Ho + y) * L.Wo + x;
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        rres[hf][h][b] = Raw<PREC, 8>{};
+                        rres[hf][h][b] = Raw<AP, 8>{};
                         if (L.res && rvalid[hf][h]) {
                             const uint8_t* rp = L.res + S::addr(rpix[hf][h], L.res_c, 32 * b + 8 * cs.m);
 #pragma unroll
-                            for (int q = 0; q < Raw<PREC, 8>::kPieces; ++q) rres[hf][h][b].set(q, __ldg(Raw<PREC, 8>::at(rp, q)));
+                            for (int q = 0; q < Raw<AP, 8>::kPieces; ++q) rres[hf][h][b].set(q, __ldg(Raw<AP, 8>::at(rp, q)));
                         }
                     }
                 }
@@ -462,7 +472,7 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
 #pragma unroll
                     for (int hf = 0; hf < NH; ++hf) {
                         uint32_t f = fresh;
-                        resident_mma_unit<KIND, PREC>(acc[hf], a_unit_lo + half_of(hf) * (kWgRowBytes >> 4), sB, u, ch, tiles_per_tap, f);
+                        resident_mma_unit<KIND, AP>(acc[hf], a_unit_lo + half_of(hf) * (kWgRowBytes >> 4), sB, u, ch, tiles_per_tap, f);
                     }
                     fresh = 1u;
                     ptx::wgmma_commit();
@@ -491,6 +501,8 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                 // Fragment register 16b + 4jj + 2h + e = row cs.row(half, h), column 32b + 8jj + 2m + e, which carries channel
                 // 32b + 8m + 2jj + e (permuted weight rows): the thread owns 8 CONSECUTIVE channels of each of its pixels per
                 // 32-column block.
+                float inv_out = 1.f;                // SE3TN_PREC_FP8: 1 / CAT's scale (a power of two: exact)
+                if constexpr (PREC == SE3TN_PREC_FP8) inv_out = 1.f / __ldg((p.img_wid ? p.gfp8[p.img_wid[n0]] : p.fp8) + L.q_out);
 #pragma unroll
                 for (int hf = 0; hf < NH; ++hf) {
                     if (hf >= kPreRes) load_res(hf);
@@ -521,7 +533,14 @@ conv_resident_kernel(const __grid_constant__ ResidentParams p)
                             }
 #pragma unroll
                             for (int e = 0; e < 8; ++e) v[e] = act_apply(v[e], L.act);
-                            S::encode(v).store(L.out + S::addr(rpix[hf][h], L.out_c, L.out_coff + ch0));
+                            if constexpr (PREC == SE3TN_PREC_FP8) {
+                                using S8 = Storage<SE3TN_PREC_FP8>;
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) v[e] *= inv_out;
+                                S8::encode(v).store(L.out + S8::addr(rpix[hf][h], L.out_c, L.out_coff + ch0));
+                            } else {
+                                S::encode(v).store(L.out + S::addr(rpix[hf][h], L.out_c, L.out_coff + ch0));
+                            }
                         }
                     }
                 }
@@ -880,6 +899,16 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
             float4 b4[BN / 32];                                  // bias of the four 32-column blocks: loads in flight during the MMAs
 #pragma unroll
             for (int bi = 0; bi < BN / 32; ++bi) b4[bi] = __ldg(reinterpret_cast<const float4*>(bias_base + ch0 + 32 * bi + grp * 4));
+            // SE3TN_PREC_FP8: y = acc * mul[co] + bias (+ residual code * its scale), then the output code = y / s_out.  A unit's
+            // 128 channels lie in one head group, so the two scales are the unit's.  Powers of two: both multiplies are exact.
+            const float* q8 = nullptr;
+            float s_res = 1.f, inv_out = 1.f;
+            if constexpr (PREC == SE3TN_PREC_FP8) {
+                q8 = p.img_wid ? p.gfp8[p.img_wid[c.img]] : p.fp8;
+                const int qg = L.q_grp_ch ? ch0 / L.q_grp_ch : 0;
+                if (L.q_res >= 0) s_res = __ldg(q8 + L.q_res + qg);
+                if (L.q_out >= 0) inv_out = 1.f / __ldg(q8 + L.q_out + qg);
+            }
 
             float acc[2][C::kAcc];                               // tile rows [0, 64) and [64, 128)
 #pragma unroll
@@ -982,18 +1011,26 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
 #pragma unroll
                         for (int h = 0; h < 2; ++h)
                             *reinterpret_cast<float2*>(&stg[cs.R + 8 * h][8 * jj + 2 * cs.m]) = make_float2(acc[hf][16 * bi + 4 * jj + 2 * h], acc[hf][16 * bi + 4 * jj + 2 * h + 1]);
+                    float4 m4 = make_float4(1.f, 1.f, 1.f, 1.f);
+                    if constexpr (PREC == SE3TN_PREC_FP8) m4 = __ldg(reinterpret_cast<const float4*>(q8 + L.fp8_mul + chan + grp * 4));
                     __syncwarp();
                     float4 a4[4];
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
                         a4[k] = *reinterpret_cast<const float4*>(&stg[4 * k + sub][grp * 4]);
-                        a4[k].x += b4[bi].x; a4[k].y += b4[bi].y; a4[k].z += b4[bi].z; a4[k].w += b4[bi].w;
+                        if constexpr (PREC == SE3TN_PREC_FP8) {
+                            a4[k].x = a4[k].x * m4.x + b4[bi].x; a4[k].y = a4[k].y * m4.y + b4[bi].y;
+                            a4[k].z = a4[k].z * m4.z + b4[bi].z; a4[k].w = a4[k].w * m4.w + b4[bi].w;
+                        } else {
+                            a4[k].x += b4[bi].x; a4[k].y += b4[bi].y; a4[k].z += b4[bi].z; a4[k].w += b4[bi].w;
+                        }
                     }
                     if (L.res) {
 #pragma unroll
                         for (int k = 0; k < 4; ++k) {
                             float r[4];
                             S::decode(rr[k], r);
+                            if constexpr (PREC == SE3TN_PREC_FP8) { r[0] *= s_res; r[1] *= s_res; r[2] *= s_res; r[3] *= s_res; }
                             a4[k].x += r[0]; a4[k].y += r[1]; a4[k].z += r[2]; a4[k].w += r[3];
                         }
                     }
@@ -1004,6 +1041,7 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
                         o.x = act_apply(o.x, L.act); o.y = act_apply(o.y, L.act); o.z = act_apply(o.z, L.act); o.w = act_apply(o.w, L.act);
                         if (pix[hf][k] < 0) continue;
                         if (L.pool_part) { psum.x += o.x; psum.y += o.y; psum.z += o.z; psum.w += o.w; continue; }
+                        if constexpr (PREC == SE3TN_PREC_FP8) { o.x *= inv_out; o.y *= inv_out; o.z *= inv_out; o.w *= inv_out; }
                         const float o4[4] = {o.x, o.y, o.z, o.w};
                         S::encode(o4).store(L.out + S::addr(pix[hf][k], L.out_c, L.out_coff + chan + grp * 4));
                     }
@@ -1037,7 +1075,8 @@ conv_trunk_kernel(const __grid_constant__ TrunkParams p)
 // ---------------------------------------------------------------------------------------------------------------
 template <int KIND, int PREC>
 cudaError_t launch_resident_t(const ResidentParams& p, int num_sms, bool pdl, cudaStream_t stream) {
-    using C = RCfg<KIND, PREC>;
+    using C = RCfg<KIND, resident_prec(PREC)>;
+    if (PREC == SE3TN_PREC_FP8 && ((!p.fp8 && !p.gfp8) || p.L.q_out < 0)) return cudaErrorInvalidValue;
     const int tiles_per_tap = (C::kStack == 2) ? 1 : p.L.chunks;
     if ((KIND == KIND_STEM ? 7 : 9) * tiles_per_tap > C::kMaxWTiles) return cudaErrorInvalidValue;
     if (C::kStack == 2 && KIND == KIND_S1 && p.L.chunks != 2) return cudaErrorInvalidValue;    // a stacked tile row is exactly two 32-channel chunks
@@ -1057,6 +1096,7 @@ cudaError_t launch_trunk_t(const TrunkParams& p, int num_sms, bool pdl, cudaStre
     using C = TCfg<PREC>;
     if (p.n_layers < 1 || p.n_layers > kTrunkMaxLayers || p.total_units <= 0 || !p.sched) return cudaErrorInvalidValue;
     if (p.ksplit < 1 || (p.ksplit > 1 && (!p.partial || !p.slice_cnt || p.ksplit > kSplitK))) return cudaErrorInvalidValue;
+    if (PREC == SE3TN_PREC_FP8 && !p.fp8 && !p.gfp8) return cudaErrorInvalidValue;
     for (int l = 0; l < p.n_layers; ++l) {
         const LayerDesc& L = p.layer[l];
         if ((L.kind != KIND_S1 && L.kind != KIND_S2) || L.cout % C::BN || L.n_tiles != L.cout / C::BN) return cudaErrorInvalidValue;
@@ -1084,6 +1124,7 @@ cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, in
             case SE3TN_PREC_TF32:   return launch_resident_t<KIND_S1, SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
             case SE3TN_PREC_BF16X3: return launch_resident_t<KIND_S1, SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
             case SE3TN_PREC_BF16:   return launch_resident_t<KIND_S1, SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_FP8:    return launch_resident_t<KIND_S1, SE3TN_PREC_FP8>(p, num_sms, pdl, stream);   // bf16, e4m3 output
         }
     }
     return cudaErrorInvalidValue;
@@ -1094,6 +1135,7 @@ cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int num_sms, bool 
         case SE3TN_PREC_TF32:   return launch_trunk_t<SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
         case SE3TN_PREC_BF16X3: return launch_trunk_t<SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
         case SE3TN_PREC_BF16:   return launch_trunk_t<SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
+        case SE3TN_PREC_FP8:    return launch_trunk_t<SE3TN_PREC_FP8>(p, num_sms, pdl, stream);
     }
     return cudaErrorInvalidValue;
 }

@@ -89,8 +89,31 @@ size_t blob_floats() {
 }
 
 // Per-precision state is indexed by the SE3TN_PREC_* value; the fp32 FFMA mode has no entry of its own there.
-constexpr int kNumPrecs = 4;
-constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16};
+constexpr int kNumPrecs = 5;
+constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16};   // every layer's weights in that format
+constexpr int kWgmmaPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16, SE3TN_PREC_FP8};   // per-set weight-map tables
+
+// SE3TN_PREC_FP8 scale indices (include/se3tn.h order) of trunk layer l's input, output and residual (-1: none).  H1 and H2
+// (indices 4 and 6) have one scale per 512-channel head group: + ch / 512.
+constexpr int kFp8In[6] = {0, 1, 2, 3, 4, 6}, kFp8Out[6] = {1, 2, 3, 4, 6, -1}, kFp8Res[6] = {-1, -1, 1, -1, -1, 4};
+constexpr int kFp8HeadCh = 512;
+inline bool fp8_in_grouped(int l) { return kFp8In[l] >= 4; }
+inline bool fp8_out_grouped(int l) { return l >= 3; }          // H1, H2, and the last layer's residual H1
+inline int fp8_mul_off(int l) { int o = kFp8MulBase; for (int i = 0; i < l; ++i) o += kFp8TrunkRows[i]; return o; }
+constexpr int kFp8WRows = 256 * 3 + 1024 * 3;                   // trunk weight rows: one s_w each
+
+// 2^ceil(log2(amax / 448)), 1 for amax == 0 (aux_kernels.cu pow2_scale_dev, exactly)
+float pow2_scale(double amax) {
+    if (!(amax > 0.0)) return 1.f;
+    int ex;
+    const double m = std::frexp(amax, &ex);
+    return std::ldexp(1.f, ex - 9 + (m > 0.875 ? 1 : 0));
+}
+bool is_pow2_scale(float s) {
+    if (!(std::isfinite(s) && s > 0.f) || !std::isnormal(s)) return false;
+    int ex;
+    return std::frexp(s, &ex) == 0.5f;
+}
 
 // Owned CUDA resources, released with their owner (every entry point makes the context's device current first).
 struct CudaRelease {
@@ -135,6 +158,9 @@ struct DeviceWeights {
     size_t w_off[14], b_off[14];
     size_t fc_off;
     CUtensorMap bmap[kNumPrecs][kLayersPerSet];   // the weight map the kernel of each layer wants, per precision
+    DevBuf<float> fp8;              // SE3TN_PREC_FP8 block (conv_common.h kFp8BlockFloats): activation scales, mul tables
+    DevBuf<float> fp8_sw;           // the trunk's per-row weight scales s_w, layer after layer
+    std::vector<float> fp8_sw_host;  // the same on the host (the mul tables are formed here)
 };
 
 struct WeightSet {
@@ -143,6 +169,8 @@ struct WeightSet {
     double mean64[8], std64[8];
     int stats_f64 = 0;
     bool has_stats = false;
+    float fp8_scales[SE3TN_FP8_SCALES];   // SE3TN_PREC_FP8 activation scales, valid with has_fp8 (dropped by a reload)
+    bool has_fp8 = false;
 };
 
 // One CAD model of the rasteriser in device memory; view() is the kernels' non-owning MeshDev.
@@ -192,7 +220,9 @@ struct se3tn_ctx {
     DevBuf<uint8_t> own_workspace;   // set only when the library allocated the workspace
     float* buf[B_COUNT] = {};
     CUtensorMap amap4[14][4];        // activation views, 4 bytes per channel (TF32 / BF16X3; also the stems' input in every mode)
-    CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16, layers 2..13)
+    CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16, layers 2..13; PREC_FP8, layers 2..7)
+    CUtensorMap amap1[14][4];        // activation views, 1 byte per channel (PREC_FP8, trunk layers 8..13)
+    DevBuf<float> fp8_scratch;       // se3tn_calibrate_fp8: 8 maxima (as bits), then trans / rot of max_batch pairs (first use)
     int pdl = 1;                     // SE3TN_PDL=0 disables programmatic dependent launch between the kernels of a step
     std::map<int, Mesh> meshes;      // CAD models of the rasteriser, keyed by mesh id
     DevBuf<MeshDev> d_meshes; int mesh_rows = 0; bool meshes_dirty = false;   // device table of their views, rebuilt when a model changes
@@ -216,6 +246,7 @@ struct se3tn_ctx {
     // per-weight-set device tables for multi-set launches, rebuilt when a set is (re)loaded: entry [wid*14 + layer]
     DevBuf<CUtensorMap> d_bmaps[kNumPrecs];   // per tensor-core precision
     DevBuf<const float*> d_bias, d_fc;        // d_fc[wid] -> [6][512] weights then [6] biases
+    DevBuf<const float*> d_fp8;               // d_fp8[wid] -> the set's SE3TN_PREC_FP8 block
     int table_rows = 0; bool tables_dirty = true;
     int launches = 0;
     bool profiling = false;
@@ -317,6 +348,7 @@ int build_activation_maps(se3tn_ctx* c, int bpc, CUtensorMap (*out)[4]) {
         const LayerSpec& L = kLayers[li];
         const uint8_t* base = reinterpret_cast<const uint8_t*>(c->buf[L.in]);
         char what[64];
+        if (bpc == 1 && li < kFirstTrunkLayer) continue;   // e4m3 activations: the trunk's inputs only
         if (L.kind == K_STEM) {
             if (bpc != 4) continue;
             // even / odd input-row views of the zero-padded NHWC4 stem input; x is the overlapping
@@ -384,8 +416,8 @@ void fill_layer_desc(const se3tn_ctx* c, const DeviceWeights& w, int li, int pre
     const int row = li;                            // row of the per-set tables
     memset(&d, 0, sizeof d);
     const bool stem = (L.kind == K_STEM);
-    const int bpc = prec_bytes_per_channel(stem ? stem_input_prec(precision) : precision);   // of this layer's input
-    const CUtensorMap (*amaps)[4] = bpc == 2 ? c->amap2 : c->amap4;
+    const int bpc = prec_bytes_per_channel(layer_input_prec(li, precision));   // of this layer's input
+    const CUtensorMap (*amaps)[4] = bpc == 1 ? c->amap1 : (bpc == 2 ? c->amap2 : c->amap4);
     for (int m = 0; m < 4; ++m) d.amap[m] = amaps[li][m];
     d.bmap = w.bmap[precision][row];
     d.bias = w.blob.get() + w.b_off[li];
@@ -406,6 +438,15 @@ void fill_layer_desc(const se3tn_ctx* c, const DeviceWeights& w, int li, int pre
     d.act = L.act; d.li = row;
     d.units_per_image = d.tiles_x * d.tiles_y * d.n_tiles * d.groups;
     d.dep_layer = -1; d.dep_target = 0; d.unit_base = 0;
+    d.q_out = d.q_res = -1; d.q_grp_ch = 0; d.fp8_mul = 0;
+    if (precision == SE3TN_PREC_FP8) {
+        if (li >= kFirstTrunkLayer) {
+            const int l = li - kFirstTrunkLayer;
+            d.q_out = kFp8Out[l]; d.q_res = kFp8Res[l]; d.q_grp_ch = fp8_out_grouped(l) ? kFp8HeadCh : 0; d.fp8_mul = fp8_mul_off(l);
+        } else if (L.out == B_CAT) {
+            d.q_out = 0;                           // the two layers that write CAT encode it to e4m3 themselves
+        }
+    }
 }
 
 int sync_stats(se3tn_ctx* c, cudaStream_t s) {
@@ -449,31 +490,34 @@ int sync_tables(se3tn_ctx* c, cudaStream_t s) {
     const int rows = max_id + 1;
     CU_TRY(c, cudaStreamSynchronize(s));
     if (rows > c->table_rows) {                    // grow: the old tables stay in place until all new ones exist
-        DevBuf<CUtensorMap> maps[kNumPrecs]; DevBuf<const float*> bias, fc;
-        for (int p : kTensorPrecs) CU_TRY(c, dev_alloc(maps[p], rows * kLayersPerSet));
+        DevBuf<CUtensorMap> maps[kNumPrecs]; DevBuf<const float*> bias, fc, fp8;
+        for (int p : kWgmmaPrecs) CU_TRY(c, dev_alloc(maps[p], rows * kLayersPerSet));
         CU_TRY(c, dev_alloc(bias, rows * kLayersPerSet));
         CU_TRY(c, dev_alloc(fc, rows));
-        for (int p : kTensorPrecs) c->d_bmaps[p] = std::move(maps[p]);
-        c->d_bias = std::move(bias); c->d_fc = std::move(fc);
+        CU_TRY(c, dev_alloc(fp8, rows));
+        for (int p : kWgmmaPrecs) c->d_bmaps[p] = std::move(maps[p]);
+        c->d_bias = std::move(bias); c->d_fc = std::move(fc); c->d_fp8 = std::move(fp8);
         c->table_rows = rows;
     }
     const size_t entries = static_cast<size_t>(rows) * kLayersPerSet;
     std::vector<CUtensorMap> maps(kNumPrecs * entries);    // [precision][entry], zeroed for ids without weights
-    std::vector<const float*> bias(entries, nullptr), fc(rows, nullptr);
+    std::vector<const float*> bias(entries, nullptr), fc(rows, nullptr), fp8(rows, nullptr);
     for (auto& kv : c->weights) {
         if (!kv.second.dev || kv.first < 0) continue;
         const DeviceWeights& w = *kv.second.dev;
         for (int li = 0; li < kLayersPerSet; ++li) {
             const size_t e = static_cast<size_t>(kv.first) * kLayersPerSet + li;
-            for (int p : kTensorPrecs) maps[p * entries + e] = w.bmap[p][li];
+            for (int p : kWgmmaPrecs) maps[p * entries + e] = w.bmap[p][li];
             bias[e] = w.blob.get() + w.b_off[li];
         }
         fc[kv.first] = w.blob.get() + w.fc_off;
+        fp8[kv.first] = w.fp8.get();
     }
-    for (int p : kTensorPrecs)
+    for (int p : kWgmmaPrecs)
         CU_TRY(c, cudaMemcpy(c->d_bmaps[p].get(), &maps[p * entries], entries * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
     CU_TRY(c, cudaMemcpy(c->d_bias.get(), bias.data(), bias.size() * sizeof(float*), cudaMemcpyHostToDevice));
     CU_TRY(c, cudaMemcpy(c->d_fc.get(), fc.data(), fc.size() * sizeof(float*), cudaMemcpyHostToDevice));
+    CU_TRY(c, cudaMemcpy(c->d_fp8.get(), fp8.data(), fp8.size() * sizeof(float*), cudaMemcpyHostToDevice));
     c->tables_dirty = false;
     return SE3TN_OK;
 }
@@ -509,7 +553,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     auto it = c->weights.find(weight_id);
     if (it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(weight_id) + " not loaded");
     const DeviceWeights& w = *it->second.dev;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
     const bool tensor = precision != SE3TN_PREC_FP32;
     auto bufp = [&](Buf b) { return c->buf[b] + kBufFloats[b] * static_cast<size_t>(first); };
     const float* fcw = w.blob.get() + w.fc_off;
@@ -535,6 +579,9 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     // ---- tensor-core modes: 8 resident-weight launches + 1 trunk launch + head ----
     const CUtensorMap* gbmaps = img_wid ? c->d_bmaps[precision].get() : nullptr;
     const float* const* gbias = img_wid ? c->d_bias.get() : nullptr;
+    const bool fp8 = precision == SE3TN_PREC_FP8;
+    const float* fp8_block = fp8 ? w.fp8.get() : nullptr;
+    const float* const* gfp8 = fp8 && img_wid ? c->d_fp8.get() : nullptr;
     if (c->sched_dirty) { CU_TRY(c, cudaMemsetAsync(c->sched.get(), 0, trunk_sched_words(c->max_batch) * sizeof(unsigned), s)); c->sched_dirty = false; }
     for (int li = 0; li < kFirstTrunkLayer; ++li) {
         ResidentParams rp;
@@ -543,10 +590,12 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         rp.m_tiles = n * rp.L.tiles_x * rp.L.tiles_y;
         if (kLayers[li].kind == K_STEM) { rp.step_x = rp.step_y = 10; rp.off_x = rp.off_y = -1; }   // 11x11 conv outputs from (10*t - 1): the 5x5 pooled block's window
         else { rp.step_x = rp.step_y = 11; rp.off_x = rp.off_y = 0; }
-        rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias;
+        rp.img_wid = img_wid; rp.gbmaps = gbmaps; rp.gbias = gbias; rp.fp8 = fp8_block; rp.gfp8 = gfp8;
+        // SE3TN_PREC_FP8: the stems and 64-channel layers are the bf16 mode's, but the two that write CAT encode it to e4m3
+        const int lp = fp8 && kLayers[li].out != B_CAT ? SE3TN_PREC_BF16 : precision;
         rp.trace = c->trace ? c->trace.get() + static_cast<size_t>(li) * 256 * 8 : nullptr;
         rp.tile_trace = c->trace ? c->trace.get() + 14 * 256 * 8 + static_cast<size_t>(li) * SE3TN_TRACE_TILES * 4 : nullptr;
-        { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, precision, c->num_sms, c->pdl != 0, s)); }
+        { ProfScope ps(c, li, s); CU_TRY(c, launch_conv_resident(rp, rp.L.kind, lp, c->num_sms, c->pdl != 0, s)); }
         ++c->launches;
     }
     {
@@ -558,7 +607,8 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         int ksplit = (n <= kSplitMaxImages) ? kSplitK : 1;
         for (int l = 0; l < 14 - kFirstTrunkLayer; ++l) {
             fill_layer_desc(c, w, kFirstTrunkLayer + l, precision, tp.layer[l]);
-            while (tp.layer[l].chunks % ksplit) ksplit /= 2;       // 2-byte storage: convAB1 has only two 128-byte chunks per pixel
+            while (tp.layer[l].chunks % ksplit) ksplit /= 2;       // 2-byte storage: convAB1 has only two 128-byte chunks per pixel,
+                                                                   // 1-byte (fp8) one: no latency mode there
         }
         int base = 0, base0 = 0;
         for (int l = 0; l < 14 - kFirstTrunkLayer; ++l) {
@@ -575,7 +625,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
         tp.layer[5].pool_part = c->pool_part.get();   // AdaptiveAvgPool2d(1) fused into the last conv's epilogue (indexed by absolute image)
         tp.n_layers = 6; tp.total_units = base;
         tp.img_first = first; tp.n_img = n; tp.max_batch = c->max_batch;
-        tp.sched = c->sched.get(); tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias;
+        tp.sched = c->sched.get(); tp.img_wid = img_wid; tp.gbmaps = gbmaps; tp.gbias = gbias; tp.fp8 = fp8_block; tp.gfp8 = gfp8;
         tp.trace = c->trace ? c->trace.get() + static_cast<size_t>(kFirstTrunkLayer) * 256 * 8 : nullptr;
         c->sched_dirty = true;                     // cleared again by the head kernel below
         { ProfScope ps(c, kFirstTrunkLayer, s); CU_TRY(c, launch_conv_trunk(tp, precision, c->num_sms, c->pdl != 0, s)); }
@@ -591,7 +641,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     }
     ++c->launches;
     if (out_feature) { CU_TRY(c, launch_nhwc_to_nchw(reinterpret_cast<const uint8_t*>(c->buf[B_F2]) + static_cast<size_t>(first) * 22 * 22 * 256 * prec_bytes_per_channel(precision), out_feature, n, 22 * 22, 256,
-                                                       precision, s)); ++c->launches; }
+                                                       precision, s, fp8 ? fp8_block + kFp8In[3] : nullptr)); ++c->launches; }   // F2's scale
     return SE3TN_OK;
 }
 
@@ -625,6 +675,9 @@ int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
     const size_t floats = blob_floats();
     CU_TRY(c, dev_alloc(w.blob, floats));
     for (int p : kTensorPrecs) CU_TRY(c, dev_alloc(w.conv[p], floats * prec_bytes_per_channel(p)));
+    CU_TRY(c, dev_alloc(w.conv[SE3TN_PREC_FP8], floats));
+    CU_TRY(c, dev_alloc(w.fp8, kFp8BlockFloats));
+    CU_TRY(c, dev_alloc(w.fp8_sw, kFp8WRows));
     CU_TRY(c, dev_alloc(w.stack, 8 * 128 * 288 * sizeof(float)));
     CU_TRY(c, dev_alloc(w.perm, 6 * 64 * 576));
     DevBuf<float> perm_tmp;                        // one 64-channel layer's fp32 weights with permuted rows
@@ -648,6 +701,11 @@ int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
                 CU_TRY(c, launch_encode_weights(p, wsrc, conv_dst(p), rows, ktot, 0));
                 if (!rc) rc = make_map2(c, &w.bmap[p][li], conv_dst(p), ktot * prec_bytes_per_channel(p) / 4, rows, L.block_n, what);
             }
+            // e4m3 with a power-of-two scale per row (SE3TN_PREC_FP8)
+            int sw_off = 0;
+            for (int l = 0; l < li - kFirstTrunkLayer; ++l) sw_off += kFp8TrunkRows[l];
+            CU_TRY(c, launch_encode_weights_fp8(wsrc, conv_dst(SE3TN_PREC_FP8), w.fp8_sw.get() + sw_off, rows, ktot, 0));
+            if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_FP8][li], conv_dst(SE3TN_PREC_FP8), ktot / 4, rows, L.block_n, what);
         } else {
             // resident-weight layers.  Stems keep the natural row order; the 64-channel 3x3 layers use the row order of the
             // accumulator fragment (all precisions).  BF16X3: hi / lo rows stacked along N.
@@ -669,11 +727,46 @@ int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
                 CU_TRY(c, launch_encode_weights(SE3TN_PREC_BF16, wsrc, conv_dst(SE3TN_PREC_BF16), 64, ktot, 0));   // permuted rows
                 if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_BF16][li], conv_dst(SE3TN_PREC_BF16), 288, 64, 64, what);
             }
+            w.bmap[SE3TN_PREC_FP8][li] = w.bmap[resident_prec(SE3TN_PREC_FP8)][li];   // SE3TN_PREC_FP8 runs these as bf16
         }
         if (rc) return rc;
     }
     w.fc_off = off;
     CU_TRY(c, cudaDeviceSynchronize());            // a kernel that failed above fails the load
+    w.fp8_sw_host.resize(kFp8WRows);
+    CU_TRY(c, cudaMemcpy(w.fp8_sw_host.data(), w.fp8_sw.get(), kFp8WRows * sizeof(float), cudaMemcpyDeviceToHost));
+    CU_TRY(c, cudaMemset(w.fp8.get(), 0, kFp8BlockFloats * sizeof(float)));   // no scales yet (WeightSet::has_fp8)
+    CU_TRY(c, cudaDeviceSynchronize());
+    return SE3TN_OK;
+}
+
+// A set's SE3TN_PREC_FP8 block from its activation scales: the scales, and mul[co] = s_in(co) * s_w[co] per trunk layer
+// (powers of two: exact).  The block keeps its address, so captured steps read the new values.  The device is synchronised
+// first: no queued step reads the block while it changes.
+int upload_fp8(se3tn_ctx* c, WeightSet& ws, const float* scales) {
+    const DeviceWeights& w = *ws.dev;
+    std::vector<float> blk(kFp8BlockFloats, 0.f);
+    for (int i = 0; i < SE3TN_FP8_SCALES; ++i) blk[i] = scales[i];
+    int sw = 0;
+    for (int l = 0; l < kTrunkMaxLayers; ++l) {
+        float* mul = blk.data() + fp8_mul_off(l);
+        for (int co = 0; co < kFp8TrunkRows[l]; ++co)
+            mul[co] = scales[kFp8In[l] + (fp8_in_grouped(l) ? co / kFp8HeadCh : 0)] * w.fp8_sw_host[sw + co];
+        sw += kFp8TrunkRows[l];
+    }
+    CU_TRY(c, cudaDeviceSynchronize());
+    CU_TRY(c, cudaMemcpy(w.fp8.get(), blk.data(), blk.size() * sizeof(float), cudaMemcpyHostToDevice));
+    memcpy(ws.fp8_scales, scales, sizeof ws.fp8_scales);
+    ws.has_fp8 = true;
+    return SE3TN_OK;
+}
+
+// An SE3TN_PREC_FP8 step needs the activation scales of every set it uses
+int check_fp8(se3tn_ctx* c, const char* fn, int wid) {
+    auto it = c->weights.find(wid);
+    if (it != c->weights.end() && it->second.dev && !it->second.has_fp8)
+        return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": weight set " + std::to_string(wid) +
+                                         " has no fp8 activation scales (se3tn_calibrate_fp8 / se3tn_set_fp8_scales)");
     return SE3TN_OK;
 }
 
@@ -743,6 +836,7 @@ int se3tn_create(int device, int max_batch, void* workspace, se3tn_ctx** out) {
     }
     int rc = build_activation_maps(c, 4, c->amap4);
     if (!rc) rc = build_activation_maps(c, 2, c->amap2);
+    if (!rc) rc = build_activation_maps(c, 1, c->amap1);
     if (rc) return fail(nullptr, rc, c->err);
     // the memsets above ran on the NULL stream: later launches may use non-blocking streams, which do not wait for it
     e = cudaDeviceSynchronize();
@@ -767,6 +861,7 @@ int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_
     // the id counts as loaded only once every form of the new weights is ready: a failed load leaves it not loaded
     WeightSet& ws = c->weights[weight_id];
     ws.dev.reset();
+    ws.has_fp8 = false;                            // fp8 activation scales belong to the weights they were calibrated on
     c->tables_dirty = true;
     c->graphs.clear();                             // captured steps hold the old tensor maps / table pointers
     std::unique_ptr<DeviceWeights> w(new DeviceWeights());
@@ -856,6 +951,7 @@ int se3tn_forward(se3tn_ctx* c, int weight_id, const float* A, const float* B, i
     if (!A || !B || !out_trans || !out_rot) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward: null argument");
     if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward: n exceeds max_batch");
     if (n == 0) return SE3TN_OK;
+    if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, "se3tn_forward", weight_id); if (rc) return rc; }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     c->launches = 0;
@@ -872,8 +968,71 @@ int se3tn_forward_preprocessed(se3tn_ctx* c, int weight_id, int first, int n,
     if (!out_trans || !out_rot) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward_preprocessed: null argument");
     if (first < 0 || n < 0 || first + n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward_preprocessed: range exceeds max_batch");
     if (n == 0) return SE3TN_OK;
+    if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, "se3tn_forward_preprocessed", weight_id); if (rc) return rc; }
     DeviceGuard guard(c->device);
     return run_network(c, weight_id, first, n, precision, out_trans, out_rot, out_feature, static_cast<cudaStream_t>(stream));
+}
+
+int se3tn_set_fp8_scales(se3tn_ctx* c, int weight_id, const float* scales, int n_scales) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!scales || n_scales != SE3TN_FP8_SCALES) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_fp8_scales: need SE3TN_FP8_SCALES scales");
+    auto it = c->weights.find(weight_id);
+    if (weight_id < 0 || it == c->weights.end() || !it->second.dev)
+        return fail(c, SE3TN_ERR_STATE, "se3tn_set_fp8_scales: weight set " + std::to_string(weight_id) + " not loaded");
+    for (int i = 0; i < SE3TN_FP8_SCALES; ++i)
+        if (!is_pow2_scale(scales[i]))
+            return fail(c, SE3TN_ERR_INVALID, "se3tn_set_fp8_scales: scale " + std::to_string(i) + " (" + std::to_string(scales[i]) +
+                                              ") is not a finite positive power of two");
+    DeviceGuard guard(c->device);
+    return upload_fp8(c, it->second, scales);
+}
+
+int se3tn_get_fp8_scales(se3tn_ctx* c, int weight_id, float* scales, int n_scales) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!scales || n_scales != SE3TN_FP8_SCALES) return fail(c, SE3TN_ERR_INVALID, "se3tn_get_fp8_scales: need room for SE3TN_FP8_SCALES scales");
+    auto it = c->weights.find(weight_id);
+    if (weight_id < 0 || it == c->weights.end() || !it->second.dev || !it->second.has_fp8)
+        return fail(c, SE3TN_ERR_STATE, "se3tn_get_fp8_scales: weight set " + std::to_string(weight_id) + " has no fp8 activation scales");
+    memcpy(scales, it->second.fp8_scales, sizeof(float) * SE3TN_FP8_SCALES);
+    return SE3TN_OK;
+}
+
+int se3tn_calibrate_fp8(se3tn_ctx* c, int weight_id, const float* A, const float* B, int n, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!A || !B || n <= 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_calibrate_fp8: null input or n outside [1, max_batch]");
+    auto it = c->weights.find(weight_id);
+    if (weight_id < 0 || it == c->weights.end() || !it->second.dev)
+        return fail(c, SE3TN_ERR_STATE, "se3tn_calibrate_fp8: weight set " + std::to_string(weight_id) + " not loaded");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DeviceGuard guard(c->device);
+    const size_t scratch = 16 + 6 * static_cast<size_t>(c->max_batch);
+    if (!c->fp8_scratch) CU_TRY(c, dev_alloc(c->fp8_scratch, scratch));
+    unsigned* amax = reinterpret_cast<unsigned*>(c->fp8_scratch.get());
+    float* tr = c->fp8_scratch.get() + 16;
+    // the bf16x3 forward leaves every e4m3 tensor of the mode in the buffers, stored in bf16x3
+    int rc = se3tn_forward(c, weight_id, A, B, n, tr, tr + 3 * c->max_batch, nullptr, SE3TN_PREC_BF16X3, stream);
+    if (rc) return rc;
+    AmaxArgs a{};
+    auto tensor = [&](int i, Buf b, int pixels, int C, int c0, int nc) { a.t[i] = {reinterpret_cast<const uint8_t*>(c->buf[b]), pixels, C, c0, nc}; };
+    tensor(0, B_CAT, 44 * 44, 128, 0, 128);
+    tensor(1, B_F1, 22 * 22, 256, 0, 256); tensor(2, B_T4, 22 * 22, 256, 0, 256); tensor(3, B_F2, 22 * 22, 256, 0, 256);
+    for (int g = 0; g < 2; ++g) {
+        tensor(4 + g, B_H1, 11 * 11, 1024, g * kFp8HeadCh, kFp8HeadCh);
+        tensor(6 + g, B_H2, 11 * 11, 1024, g * kFp8HeadCh, kFp8HeadCh);
+    }
+    a.n_tensors = SE3TN_FP8_SCALES; a.n = n;
+    CU_TRY(c, cudaMemsetAsync(amax, 0, SE3TN_FP8_SCALES * sizeof(unsigned), s));
+    CU_TRY(c, launch_amax_bf16x3(a, amax, s));
+    unsigned bits[SE3TN_FP8_SCALES];
+    CU_TRY(c, cudaMemcpyAsync(bits, amax, sizeof bits, cudaMemcpyDeviceToHost, s));
+    CU_TRY(c, cudaStreamSynchronize(s));
+    float scales[SE3TN_FP8_SCALES];
+    for (int i = 0; i < SE3TN_FP8_SCALES; ++i) {
+        float m; memcpy(&m, &bits[i], sizeof m);
+        if (!std::isfinite(m)) return fail(c, SE3TN_ERR_INVALID, "se3tn_calibrate_fp8: the activations of tensor " + std::to_string(i) + " are not finite");
+        scales[i] = pow2_scale(static_cast<double>(m) * SE3TN_FP8_HEADROOM);
+    }
+    return upload_fp8(c, it->second, scales);
 }
 
 int se3tn_pose_update(se3tn_ctx* c, const double* poses_in, const float* trans, const float* rot,
@@ -915,7 +1074,8 @@ int render_spec(se3tn_ctx* c, const char* fn, int mode, int H, int W, RenderSpec
 // (se3tn_set_stats is per weight id), so that the preprocess kernel never normalises with another set's (or no) statistics.
 // A step that renders input A also needs a model for every id: the rasteriser would otherwise draw model 0 in its place.
 // *multi: the tracks use more than one weight set.
-int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int32_t* wid_dev, int n, bool render, bool* multi) {
+int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int32_t* wid_dev, int n, bool render, bool* multi,
+               int precision) {
     if ((wid_host == nullptr) != (wid_dev == nullptr))
         return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
     if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": n exceeds max_batch");
@@ -927,6 +1087,7 @@ int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int3
         if (!it->second.has_stats) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(wid) + " has no mean/std (se3tn_set_stats)");
         if (render && !c->meshes.count(wid))
             return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": id " + std::to_string(wid) + " (track " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
+        if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, fn, wid); if (rc) return rc; }
         if (wid != (wid_host ? wid_host[0] : 0)) *multi = true;
         if (!wid_host) break;                       // all tracks use set 0
     }
@@ -1120,12 +1281,12 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
     if (!c) return SE3TN_ERR_INVALID;
     if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
     bool multi = false;
-    const int rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi);
+    const int rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
     if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || !rgbA || !depthA || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null argument or empty frame");
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
     DeviceGuard guard(c->device);
     Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
     st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
@@ -1148,10 +1309,10 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
     int rc = render_spec(c, "se3tn_track_render", render_mode, render_H, render_W, r);
     if (rc) return rc;
     bool multi = false;
-    rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi);
+    rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
     DeviceGuard guard(c->device);
     Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
     st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
@@ -1168,9 +1329,9 @@ int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, 
     if (!c) return SE3TN_ERR_INVALID;
     if (!rgbA || !depthA || !rgbB || !depthB || !A_in_cam || !B_in_cam) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null input");
     if (!out_trans || !out_rot || !out_sums) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null output");
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
     bool multi = false;
-    int rc = check_step(c, "se3tn_eval_pairs", weight_ids_host, weight_ids_dev, n, false, &multi);
+    int rc = check_step(c, "se3tn_eval_pairs", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
     if (n == 0) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: n == 0 (the loss of no pairs is undefined)");
     DeviceGuard guard(c->device);
@@ -1331,10 +1492,10 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
     bool multi = false;
-    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi);   // before anything is staged or copied
+    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);   // before anything is staged or copied
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_BF16) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
     DeviceGuard guard(c->device);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     auto& io = c->hio;

@@ -5,6 +5,10 @@
 //   SE3TN_PREC_BF16X3 : 4 bytes per channel, x = hi + lo as two bf16; per 32-channel (128-byte) chunk [32 x hi | 32 x lo],
 //                       so channel c's lo half sits 64 bytes behind its hi half.
 //   SE3TN_PREC_BF16   : 2 bytes per channel, plain bf16, 64 channels per 128-byte chunk.
+//   SE3TN_PREC_FP8    : 1 byte per channel, e4m3 (cvt.rn.satfinite: |x| > 448 saturates), 128 channels per 128-byte chunk.
+//                       Only the trunk's tensors (and CAT) are in this format; the mode's other layers store bf16
+//                       (resident_prec).  A code means code * s with a power-of-two scale s per tensor (activations) or
+//                       per row (weights); encode / decode here work on the unscaled codes, their callers scale.
 // Weight matrices use the same formats with a K-major row as the "pixel" and K as the channel.
 //
 // The helpers below are conversions, adds and address arithmetic only (no multiply-add), so they compile to the same
@@ -17,15 +21,38 @@
 #include <cstring>
 #include <type_traits>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 namespace se3tn {
 
-__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == SE3TN_PREC_BF16 ? 2 : 4; }
+__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == SE3TN_PREC_FP8 ? 1 : (prec == SE3TN_PREC_BF16 ? 2 : 4); }
 
 // The stem INPUT (4 channels, 16 bytes per pixel in every mode) has a format of its own: tf32 words in SE3TN_PREC_TF32, and in
-// both bf16 modes the bf16x3 split of the 4 channels as [2 words hi | 2 words lo] (no 64-byte gap), raw fp32 in SE3TN_PREC_FP32.
-// So the stems of both bf16 modes run the bf16x3 arithmetic: stacked hi / lo weight rows (conv_wgmma.cu RCfg::kStack).
-__host__ __device__ constexpr int stem_input_prec(int prec) { return prec == SE3TN_PREC_BF16 ? SE3TN_PREC_BF16X3 : prec; }
+// the bf16 and fp8 modes the bf16x3 split of the 4 channels as [2 words hi | 2 words lo] (no 64-byte gap), raw fp32 in
+// SE3TN_PREC_FP32.  So the stems of those modes run the bf16x3 arithmetic: stacked hi / lo weight rows (conv_wgmma.cu RCfg::kStack).
+__host__ __device__ constexpr int stem_input_prec(int prec) {
+    return (prec == SE3TN_PREC_BF16 || prec == SE3TN_PREC_FP8) ? SE3TN_PREC_BF16X3 : prec;
+}
+// The format and arithmetic of the stems and 64-channel layers (conv_resident_kernel) in mode prec: SE3TN_PREC_FP8 runs them
+// as SE3TN_PREC_BF16 (a 64-channel e4m3 pixel is half a SWIZZLE_128B row).
+__host__ __device__ constexpr int resident_prec(int prec) { return prec == SE3TN_PREC_FP8 ? SE3TN_PREC_BF16 : prec; }
+// Format of the input of layer li (0..13; 8 on: the trunk) in mode prec (the stems: stem_input_prec)
+__host__ __device__ constexpr int layer_input_prec(int li, int prec) {
+    return li < 2 ? stem_input_prec(prec) : (li < 8 ? resident_prec(prec) : prec);
+}
+
+// e4m3: element 0 in the low byte.  Saturating (satfinite: +-inf -> +-448), NaN stays NaN.
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+    uint16_t lo, hi;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));   // first source -> upper byte
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
+    return static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+}
+__device__ __forceinline__ float2 unpack_e4m3x2(uint16_t v) {   // exact: every e4m3 value is an f16 value
+    uint32_t h;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(v));
+    return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
 
 // The one hi / lo split: fp32 -> (bf16 hi, bf16 lo) with x ~= hi + lo, two values per 32-bit word (element 0 in the low half)
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -51,7 +78,7 @@ template <int PREC, int N> struct Raw {
     static constexpr int kPieces = kHiLo ? 2 : (kWords > 4 ? kWords / 4 : 1);
     static constexpr int kPieceWords = kWords / kPieces;
     static constexpr int kStride = kHiLo ? 64 : 16;
-    using Piece = std::conditional_t<kPieceWords == 4, uint4, uint2>;
+    using Piece = std::conditional_t<kPieceWords == 4, uint4, std::conditional_t<kPieceWords == 2, uint2, uint32_t>>;
     uint32_t w[kWords];
     __device__ __forceinline__ static const Piece* at(const uint8_t* p, int q) { return reinterpret_cast<const Piece*>(p + q * kStride); }
     __device__ __forceinline__ Piece get(int q) const { Piece v; memcpy(&v, w + q * kPieceWords, sizeof v); return v; }
@@ -63,7 +90,8 @@ template <int PREC, int N> struct Raw {
 };
 
 template <int PREC> struct Storage {
-    static_assert(PREC == SE3TN_PREC_TF32 || PREC == SE3TN_PREC_BF16X3 || PREC == SE3TN_PREC_BF16, "tensor-core precision");
+    static_assert(PREC == SE3TN_PREC_TF32 || PREC == SE3TN_PREC_BF16X3 || PREC == SE3TN_PREC_BF16 || PREC == SE3TN_PREC_FP8,
+                  "tensor-core precision");
     static constexpr int kBytes = prec_bytes_per_channel(PREC);     // per channel
     static constexpr bool kHiLo = PREC == SE3TN_PREC_BF16X3;
 
@@ -82,6 +110,9 @@ template <int PREC> struct Storage {
         } else if constexpr (kHiLo) {
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) split2(v[2 * i], v[2 * i + 1], r.w[i], r.w[N / 2 + i]);
+        } else if constexpr (PREC == SE3TN_PREC_FP8) {
+#pragma unroll
+            for (int i = 0; i < N / 4; ++i) r.w[i] = pack_e4m3x4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
         } else {
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) r.w[i] = pack_bf16(v[2 * i], v[2 * i + 1]);
@@ -93,6 +124,12 @@ template <int PREC> struct Storage {
         if constexpr (PREC == SE3TN_PREC_TF32) {
 #pragma unroll
             for (int i = 0; i < N; ++i) v[i] = __uint_as_float(r.w[i]);
+        } else if constexpr (PREC == SE3TN_PREC_FP8) {
+#pragma unroll
+            for (int i = 0; i < N / 4; ++i) {
+                const float2 a = unpack_e4m3x2(static_cast<uint16_t>(r.w[i] & 0xFFFFu)), b = unpack_e4m3x2(static_cast<uint16_t>(r.w[i] >> 16));
+                v[4 * i] = a.x; v[4 * i + 1] = a.y; v[4 * i + 2] = b.x; v[4 * i + 3] = b.y;
+            }
         } else {
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) {

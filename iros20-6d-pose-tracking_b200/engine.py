@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from .weights import pack_state_dict
 
-PREC = {'tf32': _lib.PREC_TF32, 'fp32': _lib.PREC_FP32, 'bf16x3': _lib.PREC_BF16X3, 'bf16': _lib.PREC_BF16}
+PREC = {'tf32': _lib.PREC_TF32, 'fp32': _lib.PREC_FP32, 'bf16x3': _lib.PREC_BF16X3, 'bf16': _lib.PREC_BF16, 'fp8': _lib.PREC_FP8}
 IMAGE_SIZE = 176
 LABEL_ORDER = {'under': _lib.LABEL_UNDER_POINTS, 'over': _lib.LABEL_OVER_POINTS}
 
@@ -83,6 +83,78 @@ class Engine:
         _lib.check(self.lib.se3tn_set_stats(self._ctx, int(weight_id), mean.ctypes.data_as(C.c_void_p),
                                             std.ctypes.data_as(C.c_void_p), int(f64)), self._ctx)
         self._stats[int(weight_id)] = key
+
+    def calibrate_fp8(self, A, B, weight_id=0):
+        """The 'fp8' mode's activation scales of a weight set from normalised pairs A, B (float32 (n,4,176,176) CUDA tensors,
+        n <= max_batch): the set's bf16x3 forward on them, max|x| of every e4m3 tensor, s = 2^ceil(log2(max|x| * H / 448)).
+        -> the scales (float32 (8,), the se3tn.h order).  Synchronises the device."""
+        self._check_img(A); self._check_img(B)
+        n = A.shape[0]
+        if B.shape[0] != n:
+            raise ValueError('A and B batch sizes differ')
+        _lib.check(self.lib.se3tn_calibrate_fp8(self._ctx, int(weight_id), _ptr(A), _ptr(B), n, _stream(self.device)), self._ctx)
+        return self.fp8_scales(weight_id)
+
+    def calibrate_fp8_missing(self, A, B, weight_ids=None):
+        """The one place where the 'fp8' mode picks calibration pairs from data (Tracker, problems and the one-pass drivers
+        come through here): every weight set among the pairs' ids (weight_ids: host int array, None = all set 0) that has
+        no activation scales yet is calibrated on its own pairs of the normalised A, B (CUDA tensors).  Sets that have
+        scales keep them.  -> the ids calibrated."""
+        ids = np.zeros(A.shape[0], np.int32) if weight_ids is None else np.asarray(weight_ids, dtype=np.int32)
+        done = []
+        for w in sorted(set(ids.tolist())):
+            if self.fp8_scales(w) is not None:
+                continue
+            idx = torch.from_numpy(np.flatnonzero(ids == w)[:self.max_batch]).to(self.device)
+            self.calibrate_fp8(A.index_select(0, idx), B.index_select(0, idx), weight_id=w)
+            done.append(w)
+        return done
+
+    def calibrate_fp8_tracks(self, frame_rgb, frame_depth, K, poses, object_width, rgbA=None, depthA=None, weight_ids=None,
+                             fill_depth=None, render=None):
+        """calibrate_fp8_missing on the pairs a tracking step of these tracks would form (all CUDA tensors, as track_batch
+        takes them): input A as given, or drawn by the rasteriser when render = dict(mode, image_hw, mesh_ids); B cropped
+        from the frame (hole-filled first with fill_depth) at the previous pose.  Nothing runs when every set has scales."""
+        n = poses.shape[0]
+        ids = np.zeros(n, np.int32) if weight_ids is None else np.asarray(weight_ids, dtype=np.int32)
+        if all(self.fp8_scales(w) is not None for w in set(ids.tolist())):
+            return []
+        wd = torch.from_numpy(np.ascontiguousarray(ids)).to(self.device)
+        if rgbA is None or depthA is None:
+            rgbA, depthA = self.render(K, poses, object_width, mesh_ids=render['mesh_ids'], mode=render['mode'],
+                                       image_hw=render['image_hw'])
+        on, max_depth, extrapolate, blur = self.depth_fill_spec(fill_depth)
+        if on:
+            frame_depth = self.fill_depth(frame_depth, max_depth=max_depth, extrapolate=bool(extrapolate),
+                                          blur_type='gaussian' if blur else 'bilateral')
+        A, B, _, _ = self.preprocess(frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, weight_ids=wd, want_tensors=True)
+        return self.calibrate_fp8_missing(A, B, ids)
+
+    def calibrate_fp8_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, weight_ids=None):
+        """calibrate_fp8_missing on validation pairs as eval_pairs takes them (CUDA tensors)."""
+        n = A_in_cam.shape[0]
+        ids = np.zeros(n, np.int32) if weight_ids is None else np.asarray(weight_ids, dtype=np.int32)
+        if all(self.fp8_scales(w) is not None for w in set(ids.tolist())):
+            return []
+        wd = torch.from_numpy(np.ascontiguousarray(ids)).to(self.device)
+        A, B = self.normalize(rgbA, depthA, rgbB, depthB, A_in_cam, weight_ids=wd, want_tensors=True)
+        return self.calibrate_fp8_missing(A, B, ids)
+
+    def fp8_scales(self, weight_id=0):
+        """The 'fp8' activation scales of a weight set (float32 (8,)), or None when it has none."""
+        out = np.zeros(_lib.FP8_SCALES, dtype=np.float32)
+        rc = self.lib.se3tn_get_fp8_scales(self._ctx, int(weight_id), out.ctypes.data_as(C.c_void_p), out.size)
+        if rc == _lib.ERR_STATE:
+            return None
+        _lib.check(rc, self._ctx)
+        return out
+
+    def set_fp8_scales(self, scales, weight_id=0):
+        """Saved 'fp8' activation scales (8 powers of two, e.g. from fp8_scales) for a weight set."""
+        s = np.ascontiguousarray(scales, dtype=np.float32)
+        if s.shape != (_lib.FP8_SCALES,):
+            raise ValueError('fp8 scales must be a %d-vector' % _lib.FP8_SCALES)
+        _lib.check(self.lib.se3tn_set_fp8_scales(self._ctx, int(weight_id), s.ctypes.data_as(C.c_void_p), s.size), self._ctx)
 
     # ------------------------------------------------------------------ hot path
     def forward(self, A, B, weight_id=0, precision='bf16x3', want_feature=False):

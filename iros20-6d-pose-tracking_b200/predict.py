@@ -272,6 +272,8 @@ class Tracker:
         render = rgbA is None or depthA is None
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
+        if self.precision == 'fp8':
+            self._calibrate_fp8(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
@@ -328,6 +330,31 @@ class Tracker:
         if weight_ids is None:
             return np.full(n, self.weight_id, dtype=np.int32) if self.weight_id != 0 else None
         return np.ascontiguousarray(weight_ids.cpu().numpy() if torch.is_tensor(weight_ids) else weight_ids, dtype=np.int32)
+
+    def _calibrate_fp8(self, prev_poses, rgb, depth, rgbA, depthA, weight_ids, object_width):
+        """'fp8': the weight sets of this frame's tracks that have no activation scales yet are calibrated on their tracks of
+        this frame before the step runs (Engine.calibrate_fp8_tracks): input A as given or drawn by the rasteriser, B cropped
+        at the previous pose from the frame (hole-filled as the step fills it).  Sets that have scales are left alone."""
+        n = len(prev_poses)
+        wh = self._weight_ids(weight_ids, n)
+        ids = np.zeros(n, np.int32) if wh is None else wh
+        eng = self.engine
+        if all(eng.fp8_scales(w) is not None for w in set(ids.tolist())):
+            return
+        dev = eng.device
+        t = lambda x, dt: (x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x))).to(dev, dt).contiguous()
+        poses = t(prev_poses, torch.float64).reshape(-1, 4, 4)
+        ow = t(object_width if torch.is_tensor(object_width) else self._widths(object_width, n), torch.float64)
+        render = None
+        if rgbA is None or depthA is None:
+            r = self.renderer
+            mesh_ids = t(ids, torch.int32) if weight_ids is not None else torch.full((n,), r.mesh_id, dtype=torch.int32, device=dev)
+            render = dict(mode=r.mode, image_hw=r.image_hw, mesh_ids=mesh_ids)
+            rgbA = depthA = None
+        else:
+            rgbA, depthA = t(rgbA, torch.uint8), t(depthA, torch.uint16)
+        eng.calibrate_fp8_tracks(t(rgb, torch.uint8), t(depth, torch.uint16), self.K, poses, ow, rgbA, depthA, weight_ids=ids,
+                                 fill_depth=self.fill_depth, render=render)
 
     def _widths(self, object_width, n):
         """The tracks' object widths as a float64 host array: the Tracker's object width unless given."""
@@ -888,6 +915,9 @@ def _track_sequences(eng, trackers, sequences, precision, depth, workers, video=
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
+                if precision == 'fp8' and t == 0:      # each set is calibrated on the first frame of the first sequence that tracks it
+                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, weight_ids=wh,
+                                             render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
                 eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                  weight_ids_host=wh, weight_ids_dev=wd, precision=precision, mode=trk.renderer.mode,
                                  image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)

@@ -10,7 +10,7 @@ staging sets, so decoding step k+1 overlaps step k on the GPU.  A batch larger t
 are added in order.  The pairs are taken in file order (the reference's validation loader does not shuffle, train.py:143-149).
 
     python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
-                                 [--precision bf16x3|tf32|bf16|fp32|all] [--batch_size 200]
+                                 [--precision bf16x3|tf32|bf16|fp8|fp32|all] [--batch_size 200]
 """
 import argparse
 import contextlib
@@ -152,6 +152,9 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
                 if mask_sum <= 0:
                     raise AssertionError('%s: the pair has an empty maskB (datasets.py:104)' % files[s + j])
                 d['rgbA'][j].copy_(rA); d['depthA'][j].copy_(dA); d['rgbB'][j].copy_(rB); d['depthB'][j].copy_(dB)
+            if precision == 'fp8' and k == 0:              # the set's activation scales from the first validation batch
+                eng.calibrate_fp8_pairs(d['rgbA'][:n], d['depthA'][:n], d['rgbB'][:n], d['depthB'][:n], A_in_cam[:n],
+                                        ids_host[:n] if ids_host is not None else None)
             eng.eval_pairs(d['rgbA'][:n], d['depthA'][:n], d['rgbB'][:n], d['depthB'][:n], A_in_cam[:n], B_in_cam[:n], tn, rn,
                            weight_ids_host=ids_host[:n] if ids_host is not None else None,
                            weight_ids_dev=ids_dev[:n] if ids_dev is not None else None, precision=precision,
