@@ -38,10 +38,16 @@ enum {
     SE3TN_PREC_BF16X3 = 2,  /* wgmma bf16 on bf16 hi/lo splits, 3 products per MAC: ~2^-16 relative
                                error (fp32-faithful for the gate) at 1.5x the tensor time of TF32            */
     SE3TN_PREC_BF16 = 3,    /* wgmma bf16, bf16 operands, 1 product per MAC (BASELINE configs[2])     */
-    SE3TN_PREC_FP8 = 4      /* the stems and 64-channel layers as SE3TN_PREC_BF16; the six trunk layers (convAB1 ...
+    SE3TN_PREC_FP8 = 4,     /* the stems and 64-channel layers as SE3TN_PREC_BF16; the six trunk layers (convAB1 ...
                                {trans,rot}_conv2.conv2) on wgmma e4m3 with e4m3 activations and weights and
                                power-of-two scales.  Needs a weight set's activation scales (se3tn_calibrate_fp8 or
                                se3tn_set_fp8_scales).  Lossy: see DESIGN.md §2 for its measured error             */
+    SE3TN_PREC_FP16 = 5     /* wgmma f16 on IEEE fp16 activations (2 bytes per channel, laid out as SE3TN_PREC_BF16)
+                               and fp16 weights: the same 11-bit significand as tf32 at the 16-bit MMA rate.  The
+                               stems read the bf16x3 input and run the bf16x3 arithmetic, then store fp16.  Encoding
+                               rounds to nearest even and saturates |x| > 65504 to +-65504 (no inf).  No scales, no
+                               calibration.  A step refuses a weight set with a weight of layers 2-13 above 65504 in
+                               magnitude (SE3TN_ERR_STATE).  tf32's accuracy class: DESIGN.md §2                   */
 };
 
 /* SE3TN_PREC_FP8's activation scales, one per e4m3 tensor, in this order: CAT (convAB1's input), F1, T4, F2, then

@@ -6,7 +6,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libse3tn.so')
 
 OK, ERR_INVALID, ERR_CUDA, ERR_NOMEM, ERR_STATE, ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5
-PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16, PREC_FP8 = 0, 1, 2, 3, 4
+PREC_TF32, PREC_FP32, PREC_BF16X3, PREC_BF16, PREC_FP8, PREC_FP16 = 0, 1, 2, 3, 4, 5
 FP8_SCALES = 8
 RENDER_VISPY, RENDER_PYRENDER = 0, 1
 LABEL_UNDER_POINTS, LABEL_OVER_POINTS = 0, 1

@@ -621,6 +621,7 @@ cudaError_t launch_nhwc_to_nchw(const void* in, float* out, int n_img, int HW, i
         case SE3TN_PREC_TF32:   nhwc_to_nchw_kernel<SE3TN_PREC_TF32><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
         case SE3TN_PREC_BF16X3: nhwc_to_nchw_kernel<SE3TN_PREC_BF16X3><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
         case SE3TN_PREC_BF16:   nhwc_to_nchw_kernel<SE3TN_PREC_BF16><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
+        case SE3TN_PREC_FP16:   nhwc_to_nchw_kernel<SE3TN_PREC_FP16><<<grid, 256, 0, s>>>(src, out, HW, C, nullptr); break;
         case SE3TN_PREC_FP8:
             if (!fp8_scale) return cudaErrorInvalidValue;
             nhwc_to_nchw_kernel<SE3TN_PREC_FP8><<<grid, 256, 0, s>>>(src, out, HW, C, fp8_scale); break;
@@ -651,6 +652,7 @@ cudaError_t launch_encode_weights(int precision, const float* src, void* dst, in
         case SE3TN_PREC_TF32:   encode_weights_kernel<SE3TN_PREC_TF32><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
         case SE3TN_PREC_BF16X3: encode_weights_kernel<SE3TN_PREC_BF16X3><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
         case SE3TN_PREC_BF16:   encode_weights_kernel<SE3TN_PREC_BF16><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
+        case SE3TN_PREC_FP16:   encode_weights_kernel<SE3TN_PREC_FP16><<<blocks, 256, 0, s>>>(src, d, rows, ktot); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

@@ -25,7 +25,8 @@
 //   * PREC (an SE3TN_PREC_* value) selects arithmetic and storage (storage.cuh): TF32 (4 x k8 tf32 MMAs per chunk-tap),
 //     BF16X3 (x = hi + lo as two bf16, 3 products per MAC: fp32-faithful), BF16 (2-byte activations, 1 product), FP8 (the
 //     trunk on e4m3 codes, 4 x k32 MMAs per chunk-tap; epilogue acc * mul[co] + bias (+ residual code * s_res), then the
-//     code of y / s_out; in the resident kernel FP8 means the bf16 layer that writes CAT as e4m3).
+//     code of y / s_out; in the resident kernel FP8 means the bf16 layer that writes CAT as e4m3), FP16 (2-byte fp16
+//     activations and weights, 1 product, f16 k16 MMAs; its stems run the bf16x3 arithmetic and store fp16).
 //   * programmatic dependent launch: every CTA signals launch_dependents at entry; only the threads that touch
 //     activations execute griddepcontrol.wait, so barrier init and the weight TMA run under the previous kernel's tail.
 //   * per-object weights (reference README.md:132: one checkpoint per object class): with img_wid every work unit takes
@@ -216,8 +217,8 @@ __device__ __forceinline__ void load_a_units(const LayerDesc& L, int ox, int oy,
 }
 
 // The MMAs of one 128-byte K chunk: four K steps of 32 bytes (tf32 k8 with PREC == SE3TN_PREC_TF32, bf16 k16 in the bf16
-// modes, e4m3 k32 in SE3TN_PREC_FP8 (trunk only, N = 128)) at N = 64 or 128.  a_lo / b_lo: low descriptor words (+2 per K
-// step).  fresh == 0: the first step overwrites acc.
+// modes, f16 k16 in SE3TN_PREC_FP16, e4m3 k32 in SE3TN_PREC_FP8 (trunk only, N = 128)) at N = 64 or 128.  a_lo / b_lo: low
+// descriptor words (+2 per K step).  fresh == 0: the first step overwrites acc.
 template <int PREC, int N>
 __device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a_lo, uint32_t b_lo, uint32_t fresh) {
 #pragma unroll
@@ -229,6 +230,8 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[N / 2], uint32_t a_lo, ui
         } else if constexpr (PREC == SE3TN_PREC_FP8) {
             static_assert(N == 128, "e4m3 MMAs only in the trunk");
             ptx::wgmma_e4m3_n128(acc, a, b, f);
+        } else if constexpr (PREC == SE3TN_PREC_FP16) {
+            if constexpr (N == 64) ptx::wgmma_f16_n64(acc, a, b, f); else ptx::wgmma_f16_n128(acc, a, b, f);
         } else {
             if constexpr (N == 64) ptx::wgmma_bf16_n64(acc, a, b, f); else ptx::wgmma_bf16_n128(acc, a, b, f);
         }
@@ -244,7 +247,7 @@ template <int KIND, int PREC> struct RCfg {
     // STACK: hi / lo weight rows stacked along N (header comment) for layers whose input is in the bf16x3 format
     static constexpr int kStack = ((POOL ? stem_input_prec(PREC) : PREC) == SE3TN_PREC_BF16X3) ? 2 : 1;
     static constexpr int kBTile = BN * kStack * kChunkBytes;
-    static constexpr int kAStages = POOL ? (PREC == SE3TN_PREC_TF32 ? 4 : 3) : (PREC == SE3TN_PREC_BF16 ? 6 : 4);
+    static constexpr int kAStages = POOL ? (PREC == SE3TN_PREC_TF32 ? 4 : 3) : (prec_2byte(PREC) ? 6 : 4);
     static constexpr int kPoolBufs = POOL ? (PREC == SE3TN_PREC_TF32 ? 2 : 1) : 0;
     static constexpr int kAcc = BN * kStack / 2;                    // accumulator registers per thread (N / 2)
     static constexpr int kMaxWTiles = POOL ? 7 : ((PREC == SE3TN_PREC_TF32) ? 18 : 9);
@@ -275,9 +278,9 @@ __device__ __forceinline__ void resident_mma_unit(float (&acc)[RCfg<KIND, PREC>:
                 ptx::wgmma_bf16_n64(acc_lo32(acc), mk_desc(a_lo + 4 + 2 * sl), mk_desc(b_lo + 2 * sl), 1u);
             }
         } else {
-            // tf32, bf16, and the stem's bf16 modes: window = 8 pixels x [hi4|lo4] against rows [w_hi|w_hi ; w_lo|0], all three
-            // products in one N = 128 MMA per K step
-            mma_chunk<PREC, C::BN * C::kStack>(acc, a_lo, b_lo, fresh);
+            // tf32, bf16, fp16, and the stems of the modes with a bf16x3 input: window = 8 pixels x [hi4|lo4] against rows
+            // [w_hi|w_hi ; w_lo|0], all three products in one bf16 N = 128 MMA per K step
+            mma_chunk<C::POOL ? stem_input_prec(PREC) : PREC, C::BN * C::kStack>(acc, a_lo, b_lo, fresh);
         }
         fresh = 1u;
     }
@@ -1118,6 +1121,7 @@ cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, in
             case SE3TN_PREC_TF32:   return launch_resident_t<KIND_STEM, SE3TN_PREC_TF32>(p, num_sms, pdl, stream);
             case SE3TN_PREC_BF16X3: return launch_resident_t<KIND_STEM, SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
             case SE3TN_PREC_BF16:   return launch_resident_t<KIND_STEM, SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
+            case SE3TN_PREC_FP16:   return launch_resident_t<KIND_STEM, SE3TN_PREC_FP16>(p, num_sms, pdl, stream);   // bf16x3, fp16 output
         }
     } else if (kind == KIND_S1) {
         switch (prec) {
@@ -1125,6 +1129,7 @@ cudaError_t launch_conv_resident(const ResidentParams& p, int kind, int prec, in
             case SE3TN_PREC_BF16X3: return launch_resident_t<KIND_S1, SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
             case SE3TN_PREC_BF16:   return launch_resident_t<KIND_S1, SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
             case SE3TN_PREC_FP8:    return launch_resident_t<KIND_S1, SE3TN_PREC_FP8>(p, num_sms, pdl, stream);   // bf16, e4m3 output
+            case SE3TN_PREC_FP16:   return launch_resident_t<KIND_S1, SE3TN_PREC_FP16>(p, num_sms, pdl, stream);
         }
     }
     return cudaErrorInvalidValue;
@@ -1136,6 +1141,7 @@ cudaError_t launch_conv_trunk(const TrunkParams& p, int prec, int num_sms, bool 
         case SE3TN_PREC_BF16X3: return launch_trunk_t<SE3TN_PREC_BF16X3>(p, num_sms, pdl, stream);
         case SE3TN_PREC_BF16:   return launch_trunk_t<SE3TN_PREC_BF16>(p, num_sms, pdl, stream);
         case SE3TN_PREC_FP8:    return launch_trunk_t<SE3TN_PREC_FP8>(p, num_sms, pdl, stream);
+        case SE3TN_PREC_FP16:   return launch_trunk_t<SE3TN_PREC_FP16>(p, num_sms, pdl, stream);
     }
     return cudaErrorInvalidValue;
 }

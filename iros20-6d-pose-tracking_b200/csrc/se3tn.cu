@@ -89,9 +89,10 @@ size_t blob_floats() {
 }
 
 // Per-precision state is indexed by the SE3TN_PREC_* value; the fp32 FFMA mode has no entry of its own there.
-constexpr int kNumPrecs = 5;
-constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16};   // every layer's weights in that format
-constexpr int kWgmmaPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16, SE3TN_PREC_FP8};   // per-set weight-map tables
+constexpr int kNumPrecs = 6;
+constexpr int kTensorPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16, SE3TN_PREC_FP16};   // every layer's weights in that format
+constexpr int kWgmmaPrecs[] = {SE3TN_PREC_TF32, SE3TN_PREC_BF16X3, SE3TN_PREC_BF16, SE3TN_PREC_FP8, SE3TN_PREC_FP16};   // per-set weight-map tables
+constexpr float kFp16Max = 65504.f;   // the largest finite fp16 value (SE3TN_PREC_FP16 saturates there)
 
 // SE3TN_PREC_FP8 scale indices (include/se3tn.h order) of trunk layer l's input, output and residual (-1: none).  H1 and H2
 // (indices 4 and 6) have one scale per 512-channel head group: + ch / 512.
@@ -171,6 +172,7 @@ struct WeightSet {
     bool has_stats = false;
     float fp8_scales[SE3TN_FP8_SCALES];   // SE3TN_PREC_FP8 activation scales, valid with has_fp8 (dropped by a reload)
     bool has_fp8 = false;
+    bool fp16_fits = false;               // every conv weight SE3TN_PREC_FP16 holds in fp16 is within its range (set by a load)
 };
 
 // One CAD model of the rasteriser in device memory; view() is the kernels' non-owning MeshDev.
@@ -220,7 +222,7 @@ struct se3tn_ctx {
     DevBuf<uint8_t> own_workspace;   // set only when the library allocated the workspace
     float* buf[B_COUNT] = {};
     CUtensorMap amap4[14][4];        // activation views, 4 bytes per channel (TF32 / BF16X3; also the stems' input in every mode)
-    CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16, layers 2..13; PREC_FP8, layers 2..7)
+    CUtensorMap amap2[14][4];        // activation views, 2 bytes per channel (PREC_BF16 / PREC_FP16, layers 2..13; PREC_FP8, layers 2..7)
     CUtensorMap amap1[14][4];        // activation views, 1 byte per channel (PREC_FP8, trunk layers 8..13)
     DevBuf<float> fp8_scratch;       // se3tn_calibrate_fp8: 8 maxima (as bits), then trans / rot of max_batch pairs (first use)
     int pdl = 1;                     // SE3TN_PDL=0 disables programmatic dependent launch between the kernels of a step
@@ -553,7 +555,7 @@ int run_network(se3tn_ctx* c, int weight_id, int first, int n, int precision,
     auto it = c->weights.find(weight_id);
     if (it == c->weights.end() || !it->second.dev) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(weight_id) + " not loaded");
     const DeviceWeights& w = *it->second.dev;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "unknown precision");
     const bool tensor = precision != SE3TN_PREC_FP32;
     auto bufp = [&](Buf b) { return c->buf[b] + kBufFloats[b] * static_cast<size_t>(first); };
     const float* fcw = w.blob.get() + w.fc_off;
@@ -722,10 +724,12 @@ int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
             uint8_t* sdst = w.stack.get() + static_cast<size_t>(li) * 128 * 288 * sizeof(float);
             CU_TRY(c, launch_split_stack_weights(wsrc, sdst, stem, 0));
             if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_BF16X3][li], sdst, stem ? 224 : 288, 128, 128, what);
-            if (stem) w.bmap[SE3TN_PREC_BF16][li] = w.bmap[stem_input_prec(SE3TN_PREC_BF16)][li];   // the stem's input format decides
-            else {
-                CU_TRY(c, launch_encode_weights(SE3TN_PREC_BF16, wsrc, conv_dst(SE3TN_PREC_BF16), 64, ktot, 0));   // permuted rows
-                if (!rc) rc = make_map2(c, &w.bmap[SE3TN_PREC_BF16][li], conv_dst(SE3TN_PREC_BF16), 288, 64, 64, what);
+            for (int p : {SE3TN_PREC_BF16, SE3TN_PREC_FP16}) {   // the 2-byte formats
+                if (stem) w.bmap[p][li] = w.bmap[stem_input_prec(p)][li];   // the stem's input format decides
+                else {
+                    CU_TRY(c, launch_encode_weights(p, wsrc, conv_dst(p), 64, ktot, 0));   // permuted rows
+                    if (!rc) rc = make_map2(c, &w.bmap[p][li], conv_dst(p), 288, 64, 64, what);
+                }
             }
             w.bmap[SE3TN_PREC_FP8][li] = w.bmap[resident_prec(SE3TN_PREC_FP8)][li];   // SE3TN_PREC_FP8 runs these as bf16
         }
@@ -761,12 +765,30 @@ int upload_fp8(se3tn_ctx* c, WeightSet& ws, const float* scales) {
     return SE3TN_OK;
 }
 
-// An SE3TN_PREC_FP8 step needs the activation scales of every set it uses
-int check_fp8(se3tn_ctx* c, const char* fn, int wid) {
+// Whether every conv weight that SE3TN_PREC_FP16 holds in fp16 (layers 2-13; the stems hold bf16x3) is within fp16's range
+bool fp16_weights_fit(const float* blob) {
+    size_t off = 0;
+    for (const LayerSpec& L : kLayers) {
+        const size_t nw = static_cast<size_t>(layer_rows(L)) * layer_ktot(L);
+        if (L.kind != K_STEM)
+            for (size_t i = 0; i < nw; ++i)
+                if (std::fabs(blob[off + i]) > kFp16Max) return false;
+        off += nw + layer_rows(L);
+    }
+    return true;
+}
+
+// What a step in `precision` needs of every set it uses besides its weights: SE3TN_PREC_FP8 the set's activation scales,
+// SE3TN_PREC_FP16 conv weights within fp16's range (a checkpoint's weights are not saturated silently)
+int check_prec(se3tn_ctx* c, const char* fn, int wid, int precision) {
     auto it = c->weights.find(wid);
-    if (it != c->weights.end() && it->second.dev && !it->second.has_fp8)
+    if (it == c->weights.end() || !it->second.dev) return SE3TN_OK;
+    if (precision == SE3TN_PREC_FP8 && !it->second.has_fp8)
         return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": weight set " + std::to_string(wid) +
                                          " has no fp8 activation scales (se3tn_calibrate_fp8 / se3tn_set_fp8_scales)");
+    if (precision == SE3TN_PREC_FP16 && !it->second.fp16_fits)
+        return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": weight set " + std::to_string(wid) +
+                                         " has a conv weight above 65504 in magnitude, outside fp16's range");
     return SE3TN_OK;
 }
 
@@ -862,6 +884,7 @@ int se3tn_load_weights(se3tn_ctx* c, int weight_id, const float* blob, size_t n_
     WeightSet& ws = c->weights[weight_id];
     ws.dev.reset();
     ws.has_fp8 = false;                            // fp8 activation scales belong to the weights they were calibrated on
+    ws.fp16_fits = fp16_weights_fit(blob);
     c->tables_dirty = true;
     c->graphs.clear();                             // captured steps hold the old tensor maps / table pointers
     std::unique_ptr<DeviceWeights> w(new DeviceWeights());
@@ -951,7 +974,7 @@ int se3tn_forward(se3tn_ctx* c, int weight_id, const float* A, const float* B, i
     if (!A || !B || !out_trans || !out_rot) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward: null argument");
     if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward: n exceeds max_batch");
     if (n == 0) return SE3TN_OK;
-    if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, "se3tn_forward", weight_id); if (rc) return rc; }
+    { const int rc = check_prec(c, "se3tn_forward", weight_id, precision); if (rc) return rc; }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     DeviceGuard guard(c->device);
     c->launches = 0;
@@ -968,7 +991,7 @@ int se3tn_forward_preprocessed(se3tn_ctx* c, int weight_id, int first, int n,
     if (!out_trans || !out_rot) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward_preprocessed: null argument");
     if (first < 0 || n < 0 || first + n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_forward_preprocessed: range exceeds max_batch");
     if (n == 0) return SE3TN_OK;
-    if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, "se3tn_forward_preprocessed", weight_id); if (rc) return rc; }
+    { const int rc = check_prec(c, "se3tn_forward_preprocessed", weight_id, precision); if (rc) return rc; }
     DeviceGuard guard(c->device);
     return run_network(c, weight_id, first, n, precision, out_trans, out_rot, out_feature, static_cast<cudaStream_t>(stream));
 }
@@ -1087,7 +1110,7 @@ int check_step(se3tn_ctx* c, const char* fn, const int32_t* wid_host, const int3
         if (!it->second.has_stats) return fail(c, SE3TN_ERR_STATE, "weight set " + std::to_string(wid) + " has no mean/std (se3tn_set_stats)");
         if (render && !c->meshes.count(wid))
             return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": id " + std::to_string(wid) + " (track " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
-        if (precision == SE3TN_PREC_FP8) { const int rc = check_fp8(c, fn, wid); if (rc) return rc; }
+        { const int rc = check_prec(c, fn, wid, precision); if (rc) return rc; }
         if (wid != (wid_host ? wid_host[0] : 0)) *multi = true;
         if (!wid_host) break;                       // all tracks use set 0
     }
@@ -1286,7 +1309,7 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
     if (n == 0) return SE3TN_OK;
     if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || !rgbA || !depthA || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null argument or empty frame");
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
     DeviceGuard guard(c->device);
     Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
     st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
@@ -1312,7 +1335,7 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
     rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
     DeviceGuard guard(c->device);
     Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
     st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
@@ -1329,7 +1352,7 @@ int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, 
     if (!c) return SE3TN_ERR_INVALID;
     if (!rgbA || !depthA || !rgbB || !depthB || !A_in_cam || !B_in_cam) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null input");
     if (!out_trans || !out_rot || !out_sums) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null output");
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
     bool multi = false;
     int rc = check_step(c, "se3tn_eval_pairs", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
@@ -1495,7 +1518,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);   // before anything is staged or copied
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP8) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
     DeviceGuard guard(c->device);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     auto& io = c->hio;

@@ -9,6 +9,8 @@
 //                       Only the trunk's tensors (and CAT) are in this format; the mode's other layers store bf16
 //                       (resident_prec).  A code means code * s with a power-of-two scale s per tensor (activations) or
 //                       per row (weights); encode / decode here work on the unscaled codes, their callers scale.
+//   SE3TN_PREC_FP16   : 2 bytes per channel, IEEE fp16 (cvt.rn.satfinite: |x| > 65504 saturates to +-65504), laid out as
+//                       SE3TN_PREC_BF16.  Decoding is exact.
 // Weight matrices use the same formats with a K-major row as the "pixel" and K as the channel.
 //
 // The helpers below are conversions, adds and address arithmetic only (no multiply-add), so they compile to the same
@@ -25,13 +27,15 @@
 
 namespace se3tn {
 
-__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == SE3TN_PREC_FP8 ? 1 : (prec == SE3TN_PREC_BF16 ? 2 : 4); }
+// The 2-byte formats (bf16, fp16): 64 channels per 128-byte chunk, one k16 MMA per 32-byte K step
+__host__ __device__ constexpr bool prec_2byte(int prec) { return prec == SE3TN_PREC_BF16 || prec == SE3TN_PREC_FP16; }
+__host__ __device__ constexpr int prec_bytes_per_channel(int prec) { return prec == SE3TN_PREC_FP8 ? 1 : (prec_2byte(prec) ? 2 : 4); }
 
 // The stem INPUT (4 channels, 16 bytes per pixel in every mode) has a format of its own: tf32 words in SE3TN_PREC_TF32, and in
-// the bf16 and fp8 modes the bf16x3 split of the 4 channels as [2 words hi | 2 words lo] (no 64-byte gap), raw fp32 in
+// the bf16, fp16 and fp8 modes the bf16x3 split of the 4 channels as [2 words hi | 2 words lo] (no 64-byte gap), raw fp32 in
 // SE3TN_PREC_FP32.  So the stems of those modes run the bf16x3 arithmetic: stacked hi / lo weight rows (conv_wgmma.cu RCfg::kStack).
 __host__ __device__ constexpr int stem_input_prec(int prec) {
-    return (prec == SE3TN_PREC_BF16 || prec == SE3TN_PREC_FP8) ? SE3TN_PREC_BF16X3 : prec;
+    return (prec_2byte(prec) || prec == SE3TN_PREC_FP8) ? SE3TN_PREC_BF16X3 : prec;
 }
 // The format and arithmetic of the stems and 64-channel layers (conv_resident_kernel) in mode prec: SE3TN_PREC_FP8 runs them
 // as SE3TN_PREC_BF16 (a 64-channel e4m3 pixel is half a SWIZZLE_128B row).
@@ -66,6 +70,15 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<const uint32_t*>(&h);
 }
+// fp16: element 0 in the low half.  Saturating (satfinite: +-inf -> +-65504), NaN stays NaN.
+__device__ __forceinline__ uint32_t pack_f16(float a, float b) {
+    uint32_t h;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(b), "f"(a));   // first source -> upper half
+    return h;
+}
+__device__ __forceinline__ float2 unpack_f16x2(uint32_t w) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&w));
+}
 __device__ __forceinline__ float2 unpack2(uint32_t w) {
     return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
 }
@@ -90,8 +103,8 @@ template <int PREC, int N> struct Raw {
 };
 
 template <int PREC> struct Storage {
-    static_assert(PREC == SE3TN_PREC_TF32 || PREC == SE3TN_PREC_BF16X3 || PREC == SE3TN_PREC_BF16 || PREC == SE3TN_PREC_FP8,
-                  "tensor-core precision");
+    static_assert(PREC == SE3TN_PREC_TF32 || PREC == SE3TN_PREC_BF16X3 || PREC == SE3TN_PREC_BF16 || PREC == SE3TN_PREC_FP8 ||
+                  PREC == SE3TN_PREC_FP16, "tensor-core precision");
     static constexpr int kBytes = prec_bytes_per_channel(PREC);     // per channel
     static constexpr bool kHiLo = PREC == SE3TN_PREC_BF16X3;
 
@@ -113,6 +126,9 @@ template <int PREC> struct Storage {
         } else if constexpr (PREC == SE3TN_PREC_FP8) {
 #pragma unroll
             for (int i = 0; i < N / 4; ++i) r.w[i] = pack_e4m3x4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+        } else if constexpr (PREC == SE3TN_PREC_FP16) {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) r.w[i] = pack_f16(v[2 * i], v[2 * i + 1]);
         } else {
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) r.w[i] = pack_bf16(v[2 * i], v[2 * i + 1]);
@@ -129,6 +145,12 @@ template <int PREC> struct Storage {
             for (int i = 0; i < N / 4; ++i) {
                 const float2 a = unpack_e4m3x2(static_cast<uint16_t>(r.w[i] & 0xFFFFu)), b = unpack_e4m3x2(static_cast<uint16_t>(r.w[i] >> 16));
                 v[4 * i] = a.x; v[4 * i + 1] = a.y; v[4 * i + 2] = b.x; v[4 * i + 3] = b.y;
+            }
+        } else if constexpr (PREC == SE3TN_PREC_FP16) {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) {
+                const float2 h = unpack_f16x2(r.w[i]);
+                v[2 * i] = h.x; v[2 * i + 1] = h.y;
             }
         } else {
 #pragma unroll

@@ -12,7 +12,8 @@ import torch
 from . import _lib
 from .weights import pack_state_dict
 
-PREC = {'tf32': _lib.PREC_TF32, 'fp32': _lib.PREC_FP32, 'bf16x3': _lib.PREC_BF16X3, 'bf16': _lib.PREC_BF16, 'fp8': _lib.PREC_FP8}
+PREC = {'tf32': _lib.PREC_TF32, 'fp32': _lib.PREC_FP32, 'bf16x3': _lib.PREC_BF16X3, 'bf16': _lib.PREC_BF16, 'fp8': _lib.PREC_FP8,
+        'fp16': _lib.PREC_FP16}
 IMAGE_SIZE = 176
 LABEL_ORDER = {'under': _lib.LABEL_UNDER_POINTS, 'over': _lib.LABEL_OVER_POINTS}
 

@@ -797,6 +797,11 @@ def _class_normalizer(class_config, key, class_id, default):
     return float(v[class_id] if isinstance(v, dict) else v)
 
 
+# The modes the one-pass YCB-Video driver offers: every mode but 'fp16', which its callers have treated as an unknown name
+# since before the mode existed.  The YCBInEOAT driver, the Tracker and the Engine take every mode of engine.PREC.
+YCB_ALL_PRECISIONS = ('bf16x3', 'tf32', 'bf16', 'fp8', 'fp32')
+
+
 def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     """The checked configuration of every requested class, before anything is loaded onto a device -> list (ascending class id)
     of dicts: class_id, name, the expanded paths, dataset_info, mean, std, trans_normalizer, rot_normalizer.
@@ -806,9 +811,8 @@ def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     FileNotFoundError naming the class and the path.  One step tracks every class of a frame, so the classes must share the
     camera (K and image size), the resolution (176), the render mode, the two normalisers and the precision: a class that differs
     from the first is a ValueError naming it."""
-    from .engine import PREC
-    if precision not in PREC:
-        raise ValueError('unknown precision %r (one of %s)' % (precision, ', '.join(PREC)))
+    if precision not in YCB_ALL_PRECISIONS:
+        raise ValueError('precision %r is not a mode of the one-pass YCB-Video driver (one of %s)' % (precision, ', '.join(YCB_ALL_PRECISIONS)))
     names = ycb_class_names(ycb_dir)
     ids = sorted(set(int(c) for c in class_ids))
     if not ids:

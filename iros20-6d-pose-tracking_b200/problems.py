@@ -10,7 +10,7 @@ staging sets, so decoding step k+1 overlaps step k on the GPU.  A batch larger t
 are added in order.  The pairs are taken in file order (the reference's validation loader does not shuffle, train.py:143-149).
 
     python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
-                                 [--precision bf16x3|tf32|bf16|fp8|fp32|all] [--batch_size 200]
+                                 [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200]
 """
 import argparse
 import contextlib

@@ -1,5 +1,8 @@
 """Precision study (CPU, not product code): exact emulation of TF32 / 3-product operand rounding per layer group on the
-raw-regime inputs, against the fp32 oracle -- the evidence behind the bf16x3 default (DESIGN.md section 2).  Run from the repo root."""
+raw-regime inputs, against the fp32 oracle -- the evidence behind the bf16x3 default (DESIGN.md section 2).  Run from the repo root.
+    python scripts/precision_raw.py          the per-layer-group study (6 tracks of frame seed 6)
+    python scripts/precision_raw.py --fp16   the fp16 mode (precision_study.run_fp16) on the 64 tracks of frame seed 11, half on
+                                             each weight seed, as tests/test_gpu_fp16.py runs them"""
 import importlib, sys, numpy as np, torch, torch.nn.functional as F
 sys.path.insert(0,'.'); sys.path.insert(0,'oracle')
 synth = importlib.import_module('iros20-6d-pose-tracking_b200.synth')
@@ -44,6 +47,24 @@ def run(sd, A, B, modes):
         x = cbr(ab,h+'_conv1',2,1,'head'); x = block(x,h+'_conv2','head')
         x = x.mean((2,3)); outs.append(torch.tanh(F.linear(x, sd[h+'_out.0.weight'], sd[h+'_out.0.bias'])))
     return torch.cat(outs,1)
+
+def fp16_raw(n=64, seed=11):
+    from precision_study import run_fp16
+    rgb, depth = synth.raw_frame(seed); poses = synth.raw_poses(n, seed=seed); rgbA, depthA = synth.rendered_views(n, poses, seed=seed)
+    mean, std = synth.default_mean_std(); stats = {0: (mean, std), 1: (mean + 1.5, std * 1.25)}
+    wid = np.repeat([0, 1], n // 2)
+    for w in (0, 1):
+        sd = synth.make_state_dict(w); sel = np.nonzero(wid == w)[0]
+        ds = [O.on_track(sd, poses[i], rgb, depth, rgbA[i], depthA[i], synth.CAMERA_K, 200.0, *stats[w], return_all=True)[1] for i in sel]
+        A = torch.from_numpy(np.stack([d['dataA'] for d in ds])).float(); B = torch.from_numpy(np.stack([d['dataB'] for d in ds])).float()
+        ref = torch.from_numpy(np.stack([np.concatenate([d['trans'], d['rot']]) for d in ds]))
+        with torch.no_grad(): out = run_fp16(sd, A, B)
+        err = (out.double() - ref).abs(); tol = 1e-4 + 1e-3 * ref.abs()
+        print('fp16, raw regime, weight seed %d (%d tracks): max abs err %.3e  max err/tol %.3f  input absmax %.1f'
+              % (w, len(sel), err.max().item(), (err / tol).max().item(), max(A.abs().max().item(), B.abs().max().item())))
+
+if '--fp16' in sys.argv:
+    fp16_raw(); sys.exit(0)
 
 n=6
 rgb, depth = synth.raw_frame(6); poses = synth.raw_poses(n, seed=6); rgbA, depthA = synth.rendered_views(n, poses, seed=6)
