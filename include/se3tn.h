@@ -393,6 +393,41 @@ int se3tn_eval_pairs(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA
 int se3tn_pair_loss(se3tn_ctx* ctx, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,
                     float* out_sums, void* stream);
 
+/* ---- held-out pairs from annotated frames: ProducerPurturb.generate (reference produce_train_pair_data.py:86-141) ------------- */
+
+/* crop_bbox with its segmentation plane (reference Utils.py:320-359 with seg): rgb and depth exactly as se3tn_crop_bbox cuts them, and
+ * seg uint8 (H,W) device through the same window and nearest-neighbour mapping, zero outside the image, never masked (Utils.py:346-349).
+ * class_ids NULL: crop_seg uint8 (n,out_h,out_w) receives the labels.  class_ids int32 (n) device: crop_seg receives (label == class id)
+ * as 0 / 1 and seg_count int32 (n) device (nullable) the number of ones.  One launch. */
+int se3tn_crop_bbox_seg(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W,
+                        const int32_t* bbox, const int32_t* class_ids, int n, int out_h, int out_w,
+                        uint8_t* crop_rgb, uint16_t* crop_depth, uint8_t* crop_seg, int32_t* seg_count, void* stream);
+
+/* The two counts of the generator's visibility check (produce_train_pair_data.py:97-104) for m rows (pose, mesh id, class id) of one
+ * frame:  out_visible[i] = #(seg == class_ids[i]) over the whole H x W seg frame (uint8, device);  out_covered[i] = the pixels of mesh
+ * i's render at poses[i] over the whole H x W camera image in the SE3TN_RENDER_PYRENDER mode whose float32 linearised depth is > 0.1f
+ * (np.sum(depth > 0.1) of Renderer.render's depth).  K HOST fx fy cx cy; poses double (m,16), class_ids int32 (m), outputs int32 (m),
+ * device; mesh_ids_host / mesh_ids_dev int32 (m) (both NULL: mesh 0).  Plain stream launches (memsets + 3 kernels), not captured.  The
+ * nearest-z planes (m x H x W words) are context-owned scratch that only grows.  Ids are checked on the host before anything is
+ * queued: a missing mesh is SE3TN_ERR_STATE, m > max_batch SE3TN_ERR_INVALID.  The host then applies the reference's thresholds. */
+int se3tn_visibility(se3tn_ctx* ctx, const uint8_t* seg, int H, int W, const double* K, const double* poses,
+                     const int32_t* mesh_ids_host, const int32_t* mesh_ids_dev, const int32_t* class_ids, int m,
+                     int32_t* out_visible, int32_t* out_covered, void* stream);
+
+/* One step of ProducerPurturb.generate for n perturbed samples of one frame (produce_train_pair_data.py:118-128): compute_bbox of each
+ * A_in_cam (object_width[i] mm, scale 1000), render A of mesh i at A_in_cam in the SE3TN_RENDER_PYRENDER mode over the H x W camera
+ * image and crop it (what se3tn_render_ex gives), then crop B, its depth and its seg out of the frame through the same window
+ * (se3tn_crop_bbox_seg with the class ids).  frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), seg uint8 (H,W), A_in_cam double (n,16),
+ * object_width double (n), class_ids int32 (n), device; K HOST.  Outputs, device: rgbA, rgbB uint8 (n,176,176,3), depthA, depthB
+ * uint16 (n,176,176), segB uint8 (n,176,176) 0 / 1 as the generator writes it, seg_count int32 (n) = #(segB == 1).  bbox + render (2) +
+ * crop = 4 launches, captured as one CUDA graph keyed like the track steps (se3tn_last_step_was_graph).  Errors as se3tn_track_render:
+ * ids checked on the host before anything is queued, a missing mesh is SE3TN_ERR_STATE, n > max_batch SE3TN_ERR_INVALID. */
+int se3tn_perturb_pairs(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W,
+                        const double* K, const double* A_in_cam, const double* object_width,
+                        const int32_t* mesh_ids_host, const int32_t* mesh_ids_dev, const int32_t* class_ids, int n,
+                        uint8_t* rgbA, uint16_t* depthA, uint8_t* rgbB, uint16_t* depthB, uint8_t* segB, int32_t* seg_count,
+                        void* stream);
+
 /* ---- introspection (tests / profiling) -------------------------------------------------------- */
 
 /* Device pointer + per-image float count of an internal NHWC activation buffer.
@@ -429,7 +464,8 @@ int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
  * depth-fill setting (se3tn_set_depth_fill), and the address of every device array, in or out.  A replay reads what those
  * arrays hold at the time, and a call's host ids only decide the first id and the mix.  SE3TN_GRAPH=0 in the environment,
  * an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
- * se3tn_last_step_was_graph: 1 if the last track_batch / track_render / eval_pairs call was a graph launch. */
+ * se3tn_perturb_pairs steps are captured and keyed the same way.
+ * se3tn_last_step_was_graph: 1 if the last track_batch / track_render / eval_pairs / perturb_pairs call was a graph launch. */
 int se3tn_last_step_was_graph(se3tn_ctx* ctx);
 int se3tn_last_launch_count(se3tn_ctx* ctx);
 

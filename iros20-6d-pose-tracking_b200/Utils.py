@@ -2,10 +2,14 @@
 GPU through libse3tn (numpy in / numpy out like the originals):
 
   compute_bbox               reference Utils.py:302-316
-  crop_bbox                  reference Utils.py:320-359
+  crop_bbox                  reference Utils.py:320-359 (with or without the seg plane)
   normalize_rotation_matrix  reference Utils.py:363-367 (9 flops: stays numpy)
   add / adi                  reference Utils.py:72-98 (ADD, ADD-S); `model` is anything with `.points` or an (m,3) array
+  random_direction / random_gaussian_magnitude   reference Utils.py:372-404 (host RNG draws: stay on the host, same order)
 """
+import math
+import random
+
 import numpy as np
 import torch
 
@@ -35,15 +39,58 @@ def compute_bbox(pose, K, scale_size=230, scale=(1, 1, 1)):
 
 
 def crop_bbox(color, depth, boundingbox, output_size=(100, 100), seg=None):
-    if seg is not None:
-        raise NotImplementedError('seg crops are only used by the training data generator (out of scope)')
+    """-> (rgb, depth), or (rgb, depth, seg) when seg (uint8 (H,W) labels) is given: the labels cropped through the same window
+    and nearest mapping, zero outside the image (Utils.py:346-349)."""
     eng = _eng()
     rgb = torch.from_numpy(np.ascontiguousarray(color, dtype=np.uint8)).to(eng.device)
     d = torch.from_numpy(np.ascontiguousarray(depth).astype(np.uint16)).to(eng.device)
     bb = torch.from_numpy(np.ascontiguousarray(boundingbox, dtype=np.int32).reshape(1, 4, 2)).to(eng.device)
-    # cv2.resize takes (width, height)
-    crgb, cdepth = eng.crop_bbox(rgb, d, bb, out_hw=(int(output_size[1]), int(output_size[0])))
-    return crgb[0].cpu().numpy(), cdepth[0].cpu().numpy()
+    out_hw = (int(output_size[1]), int(output_size[0]))            # cv2.resize takes (width, height)
+    if seg is None:
+        crgb, cdepth = eng.crop_bbox(rgb, d, bb, out_hw=out_hw)
+        return crgb[0].cpu().numpy(), cdepth[0].cpu().numpy()
+    seg = np.asarray(seg)
+    if seg.dtype != np.uint8:
+        raise ValueError('seg must be a uint8 label image (the reference crops it into a uint8 canvas, Utils.py:331)')
+    s = torch.from_numpy(np.ascontiguousarray(seg)).to(eng.device)
+    crgb, cdepth, cseg, _ = eng.crop_bbox_seg(rgb, d, s, bb, out_hw=out_hw)
+    return crgb[0].cpu().numpy(), cdepth[0].cpu().numpy(), cseg[0].cpu().numpy()
+
+
+def random_direction():
+    """Utils.py:394-404: a uniform direction on the unit sphere from two random.uniform draws (theta, then phi)."""
+    theta = random.uniform(0, 1) * math.pi * 2
+    phi = math.acos((2 * (random.uniform(0, 1))) - 1)
+    p = np.zeros(3)
+    p[0] = 1 * math.sin(phi) * math.cos(theta)
+    p[1] = 1 * math.sin(phi) * math.sin(theta)
+    p[2] = 1 * math.cos(phi)
+    return p
+
+
+def random_gaussian_magnitude(max_T, max_R):
+    """Utils.py:372-390, in the reference's draw order: translation direction (random), its magnitude (np.random.normal, redrawn
+    until |m| <= max_T), rotation direction (random), its magnitude in degrees (redrawn until |m| <= max_R), R = cv2.Rodrigues.
+    Host only: after random.seed(s); np.random.seed(s) it returns the reference's matrices bit for bit."""
+    import cv2
+    direction_T = random_direction()
+    while 1:
+        magn_T = np.random.normal(0, max_T)
+        if abs(magn_T) <= max_T:
+            break
+    T = direction_T * magn_T
+    direction_R = random_direction()
+    direction_R = direction_R / np.linalg.norm(direction_R)
+    while 1:
+        magn_R = np.random.normal(0, max_R)
+        if abs(magn_R) <= max_R:
+            break
+    rod = direction_R * magn_R / 180.0 * np.pi
+    R = cv2.Rodrigues(rod)[0].reshape(3, 3).copy()
+    pose = np.eye(4)
+    pose[:3, :3] = R
+    pose[:3, 3] = T.copy()
+    return pose
 
 
 def normalize_rotation_matrix(R):

@@ -53,6 +53,9 @@ SIGNATURES = {
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'se3tn_eval_pairs': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_pair_loss': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
+    'se3tn_crop_bbox_seg': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_visibility': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    'se3tn_perturb_pairs': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_debug_buffer': (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_sz)]),
     'se3tn_last_launch_count': (_i, [_vp]),
     'se3tn_get_trace': (_i, [_vp, _vp]),

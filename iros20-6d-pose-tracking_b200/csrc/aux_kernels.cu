@@ -245,6 +245,69 @@ cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, i
     return cudaGetLastError();
 }
 
+// crop_bbox with its segmentation plane (reference Utils.py:320-359 with seg, produce_train_pair_data.py:125-139): rgb and depth
+// exactly as crop_kernel cuts them, and the seg plane through the same window and nearest mapping -- zero outside the image,
+// never masked (Utils.py:346-349).  One CTA per sample.  class_ids null: crop_seg receives the label values.  class_ids given:
+// crop_seg receives (seg == class id) as 0 / 1, what the generator writes to disk, and count[i] the number of such pixels,
+// reduced in the CTA (np.sum(segB == class_id), produce_train_pair_data.py:128).
+constexpr int kCropSegThreads = 1024;
+__global__ void __launch_bounds__(kCropSegThreads)
+crop_seg_kernel(const uint8_t* __restrict__ frame_rgb, const uint16_t* __restrict__ frame_depth, const uint8_t* __restrict__ seg,
+                int H, int W, const int* __restrict__ bbox, const int* __restrict__ class_ids, int out_h, int out_w,
+                uint8_t* __restrict__ crop_rgb, uint16_t* __restrict__ crop_depth, uint8_t* __restrict__ crop_seg, int* __restrict__ count)
+{
+    ptx::grid_dep_wait();                                   // the bbox comes from bbox_kernel (a step may chain them)
+    const int n = blockIdx.x;
+    const int* bb = bbox + n * 8;
+    const int top = min(min(bb[0], bb[2]), min(bb[4], bb[6])), bottom = max(max(bb[0], bb[2]), max(bb[4], bb[6]));
+    const int left = min(min(bb[1], bb[3]), min(bb[5], bb[7])), right = max(max(bb[1], bb[3]), max(bb[5], bb[7]));
+    const int ch = bottom - top, cw = right - left;
+    const int cid = class_ids ? class_ids[n] : 0;
+    const double ifx = cw > 0 ? 1.0 / (static_cast<double>(out_w) / cw) : 0.0;
+    const double ify = ch > 0 ? 1.0 / (static_cast<double>(out_h) / ch) : 0.0;
+    int hits = 0;
+    for (int pix = threadIdx.x; pix < out_h * out_w; pix += blockDim.x) {
+        const int y = pix / out_w, x = pix - y * out_w;
+        unsigned r = 0, g = 0, b = 0, d = 0, sv = 0;
+        if (ch > 0 && cw > 0) {
+            int sx = static_cast<int>(floor(x * ifx)); if (sx > cw - 1) sx = cw - 1;
+            int sy = static_cast<int>(floor(y * ify)); if (sy > ch - 1) sy = ch - 1;
+            const int fy_ = top + sy, fx_ = left + sx;
+            if (fy_ >= 0 && fy_ < H && fx_ >= 0 && fx_ < W) {
+                const size_t fo = static_cast<size_t>(fy_) * W + fx_;
+                r = frame_rgb[fo * 3]; g = frame_rgb[fo * 3 + 1]; b = frame_rgb[fo * 3 + 2];
+                d = frame_depth[fo]; sv = seg[fo];
+            }
+        }
+        if (class_ids) {                                    // zero outside the image compares as label 0, as in the reference
+            sv = static_cast<int>(sv) == cid ? 1u : 0u;
+            hits += static_cast<int>(sv);
+        }
+        const size_t o = static_cast<size_t>(n) * out_h * out_w + pix;
+        crop_rgb[o * 3] = r; crop_rgb[o * 3 + 1] = g; crop_rgb[o * 3 + 2] = b;
+        crop_depth[o] = static_cast<uint16_t>(d);
+        crop_seg[o] = static_cast<uint8_t>(sv);
+    }
+    if (!count) return;
+    __shared__ int s_hits[kCropSegThreads / 32];
+    for (int o = 16; o > 0; o >>= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
+    if ((threadIdx.x & 31) == 0) s_hits[threadIdx.x >> 5] = hits;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int w = 0; w < kCropSegThreads / 32; ++w) t += s_hits[w];
+        count[n] = t;
+    }
+}
+
+cudaError_t launch_crop_seg(const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const int* bbox,
+                            const int* class_ids, int n, int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth,
+                            uint8_t* crop_seg, int* count, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    return launch_kernel(crop_seg_kernel, dim3(n), dim3(kCropSegThreads), 0, s, false, frame_rgb, frame_depth, seg, H, W, bbox,
+                         class_ids, out_h, out_w, crop_rgb, crop_depth, crop_seg, count);
+}
+
 // =============================================================================================
 // NCHW float32 (N,4,176,176) -> zero-padded NHWC4 stem input (for Se3TrackNet.forward(A, B))
 // =============================================================================================

@@ -48,6 +48,11 @@ cudaError_t launch_bbox(const double* poses, const double* K4, const double* wid
                         int* out, int n, cudaStream_t s);
 cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const int* bbox, int n,
                         int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth, cudaStream_t s);
+// crop_bbox with the seg plane (uint8 (H,W) labels): class_ids null -> crop_seg holds the labels; class_ids (n) given -> crop_seg
+// holds (label == class id) as 0 / 1 and count (n, nullable) the number of ones.  One CTA per sample.
+cudaError_t launch_crop_seg(const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const int* bbox,
+                            const int* class_ids, int n, int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth,
+                            uint8_t* crop_seg, int* count, cudaStream_t s);
 cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s);
 cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int Win, int C, cudaStream_t s);
 // poses_in non-null: also the pose update of every track (K6 fused into K4); loss.poses_a non-null: also the loss terms of every pair;

@@ -291,10 +291,11 @@ __device__ void make_uniforms(const RenderArgs& a, int n, int nf, Uniforms& u) {
         }
         const double nr = 0.1, fr = 2.0;
         u.mode = a.mode;
-        if (a.mode == 1) {
-            // the whole camera image is the viewport (pyrender IntrinsicsCamera, offscreen_renderer.py:52-53); crop_bbox's window
-            // (predict.py:211: scale (1000, 1000, 1000), no y flip) selects the samples
-            bbox_window(pose, a.fx, a.fy, a.cx, a.cy, a.object_width[n], 1000.0, 1000.0, 1000.0, top, left, ch, cw);
+        if (a.mode != 0) {
+            // the whole camera image is the viewport (pyrender IntrinsicsCamera, offscreen_renderer.py:52-53).  Mode 1: crop_bbox's
+            // window (predict.py:211: scale (1000, 1000, 1000), no y flip) selects the samples; mode 2 (the coverage pass) has none
+            if (a.mode == 1) bbox_window(pose, a.fx, a.fy, a.cx, a.cy, a.object_width[n], 1000.0, 1000.0, 1000.0, top, left, ch, cw);
+            else top = left = 0, ch = a.vh, cw = a.vw;
             u.valid = (cw > 0 && ch > 0 && nf > 0 && a.vw > 0 && a.vh > 0) ? 1 : 0;
             u.vw = a.vw; u.vh = a.vh; u.hx = a.vw * 0.5; u.hy = a.vh * 0.5;
             u.top = top; u.left = left; u.ch = ch; u.cw = cw;
@@ -539,6 +540,142 @@ render_kernel(RenderArgs a)
         a.depth[o] = static_cast<uint16_t>(mm);
     }
 }
+
+// ---------------- coverage: the nearest depth of every pixel of the WHOLE camera image (pyrender mode, uniforms of mode 2) ----------------
+// What np.sum(depth > 0.1) needs of Renderer.render's depth (produce_train_pair_data.py:101-102): only the nearest fragment of each
+// pixel, so no triangle index is kept -- zmin[j][i] = min over fragments of the float32 window-z bits (positive floats order as their
+// bits; -0.0 never wins, as it never wins the 64-bit keys of render_kernel or of the oracle).  Same set-up, edge functions, top-left
+// rule, depth clip and near-plane path as render_kernel; one thread per triangle, boxes above kBigBox pixels walked by the warp.
+constexpr int kCoverThreads = 256;
+constexpr unsigned kCoverClear = 0x7F7F7F7Fu;         // cudaMemset byte 0x7F: above every z in [0, 1)
+
+__device__ __forceinline__ void cover_pixel(const Tri& T, const EdgeSet& E, double inv_area, int i, int j, bool tl0, bool tl1, bool tl2,
+                                            unsigned* zmin, int vw) {
+    const double cx = static_cast<double>(i * kSub + kHalf), cy = static_cast<double>(j * kSub + kHalf);
+    double e0, e1, e2;
+    edges(E, cx, cy, e0, e1, e2);
+    if (!((e0 > 0 || (e0 == 0 && tl0)) && (e1 > 0 || (e1 == 0 && tl1)) && (e2 > 0 || (e2 == 0 && tl2)))) return;
+    const double l0 = e0 * inv_area, l1 = e1 * inv_area, l2 = e2 * inv_area;
+    const double z = (l0 * T.z0 + l1 * T.z1) + l2 * T.z2;
+    const float z32 = static_cast<float>(z);
+    if (!(z32 >= 0.f && z32 < 1.f)) return;
+    atomicMin(&zmin[static_cast<size_t>(j) * vw + i], __float_as_uint(z32));
+}
+
+__device__ __noinline__ void cover_straddler(const Uniforms& u, const MeshDev& m, int t, int lane, unsigned* zmin) {
+    Strad S;
+    straddler_setup(u, m, t, S);
+    if (!S.ok) return;
+    const int bw = S.ib - S.ia + 1, cnt = bw * (S.jb - S.ja + 1);
+    for (int k = lane; k < cnt; k += 32) {
+        const int i = S.ia + k % bw, j = S.ja + k / bw;
+        double b0, b1, b2;
+        straddler_weights(S, i, j, u.vw, u.vh, b0, b1, b2);
+        if (!(b0 >= 0.0 && b1 >= 0.0 && b2 >= 0.0)) continue;
+        const double zc = (b0 * S.z[0] + b1 * S.z[1]) + b2 * S.z[2], wc = (b0 * S.w[0] + b1 * S.w[1]) + b2 * S.w[2];
+        const float z32 = static_cast<float>((zc / wc + 1.0) * 0.5);
+        if (!(z32 >= 0.f && z32 < 1.f)) continue;
+        atomicMin(&zmin[static_cast<size_t>(j) * u.vw + i], __float_as_uint(z32));
+    }
+}
+
+// grid (triangle blocks, n): zmin (n, vh, vw), window rows bottom-up
+__global__ void __launch_bounds__(kCoverThreads)
+coverage_kernel(RenderArgs a, unsigned* __restrict__ zmin_all)
+{
+    __shared__ Uniforms u;
+    const int n = blockIdx.y;
+    ptx::grid_dep_wait();                                    // projected vertices + uniforms come from render_project_kernel
+    int mid = a.mesh_ids ? a.mesh_ids[n] : 0;
+    if (mid < 0 || mid >= a.n_meshes) mid = 0;
+    const MeshDev m = a.meshes[mid];
+    if (static_cast<int>(blockIdx.x * blockDim.x) >= m.nf) return;      // whole CTA past this model's triangles
+    if (threadIdx.x < sizeof(Uniforms) / sizeof(double))
+        reinterpret_cast<double*>(&u)[threadIdx.x] = reinterpret_cast<const double*>(a.uniforms + static_cast<size_t>(n) * sizeof(Uniforms))[threadIdx.x];
+    __syncthreads();
+    if (!u.valid) return;
+    const PVtx* __restrict__ pv = reinterpret_cast<const PVtx*>(a.projected) + static_cast<size_t>(n) * a.max_nv;
+    unsigned* zmin = zmin_all + static_cast<size_t>(n) * u.vw * u.vh;
+    const int lane = threadIdx.x & 31;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    bool big = false, strad = false;
+    if (t < m.nf) {
+        const unsigned i0 = m.faces[3 * t], i1 = m.faces[3 * t + 1], i2 = m.faces[3 * t + 2];
+        const bool idx_ok = i0 < static_cast<unsigned>(m.nv) && i1 < static_cast<unsigned>(m.nv) && i2 < static_cast<unsigned>(m.nv);
+        strad = idx_ok && (pv[i0].X == INT_MIN || pv[i1].X == INT_MIN || pv[i2].X == INT_MIN);
+        const Tri T = (idx_ok && !strad) ? setup(pv, m, t) : Tri{};
+        if (idx_ok && !strad && T.ok) {
+            const long long mnx = min(T.x0, min(T.x1, T.x2)), mxx = max(T.x0, max(T.x1, T.x2));
+            const long long mny = min(T.y0, min(T.y1, T.y2)), mxy = max(T.y0, max(T.y1, T.y2));
+            const int ia = static_cast<int>(max(0ll, floor_div(mnx - kHalf + kSub - 1, kSub))), ib = static_cast<int>(min(static_cast<long long>(u.vw - 1), floor_div(mxx - kHalf, kSub)));
+            const int ja = static_cast<int>(max(0ll, floor_div(mny - kHalf + kSub - 1, kSub))), jb = static_cast<int>(min(static_cast<long long>(u.vh - 1), floor_div(mxy - kHalf, kSub)));
+            if (ia <= ib && ja <= jb) {
+                if (static_cast<long long>(ib - ia + 1) * (jb - ja + 1) > kBigBox) big = true;
+                else {
+                    const bool tl0 = top_left(T.x2 - T.x1, T.y2 - T.y1), tl1 = top_left(T.x0 - T.x2, T.y0 - T.y2), tl2 = top_left(T.x1 - T.x0, T.y1 - T.y0);
+                    const double inv_area = 1.0 / static_cast<double>(T.area2);
+                    const EdgeSet E = edge_set(T);
+                    for (int j = ja; j <= jb; ++j)
+                        for (int i = ia; i <= ib; ++i) cover_pixel(T, E, inv_area, i, j, tl0, tl1, tl2, zmin, u.vw);
+                }
+            }
+        }
+    }
+    unsigned bigmask = __ballot_sync(0xffffffffu, big);
+    while (bigmask) {                                        // large triangles: the whole warp walks the bounding box
+        const int src = __ffs(bigmask) - 1; bigmask &= bigmask - 1;
+        const int tb = __shfl_sync(0xffffffffu, t, src);
+        const Tri T = setup(pv, m, tb);
+        const long long mnx = min(T.x0, min(T.x1, T.x2)), mxx = max(T.x0, max(T.x1, T.x2));
+        const long long mny = min(T.y0, min(T.y1, T.y2)), mxy = max(T.y0, max(T.y1, T.y2));
+        const int ia = static_cast<int>(max(0ll, floor_div(mnx - kHalf + kSub - 1, kSub))), ib = static_cast<int>(min(static_cast<long long>(u.vw - 1), floor_div(mxx - kHalf, kSub)));
+        const int ja = static_cast<int>(max(0ll, floor_div(mny - kHalf + kSub - 1, kSub))), jb = static_cast<int>(min(static_cast<long long>(u.vh - 1), floor_div(mxy - kHalf, kSub)));
+        const bool tl0 = top_left(T.x2 - T.x1, T.y2 - T.y1), tl1 = top_left(T.x0 - T.x2, T.y0 - T.y2), tl2 = top_left(T.x1 - T.x0, T.y1 - T.y0);
+        const double inv_area = 1.0 / static_cast<double>(T.area2);
+        const EdgeSet E = edge_set(T);
+        const int bw = ib - ia + 1, cnt = bw * (jb - ja + 1);
+        for (int k = lane; k < cnt; k += 32) cover_pixel(T, E, inv_area, ia + k % bw, ja + k / bw, tl0, tl1, tl2, zmin, u.vw);
+    }
+    unsigned smask = __ballot_sync(0xffffffffu, strad);
+    while (smask) {                                          // near-plane straddlers (rare): the whole warp, homogeneous weights
+        const int src = __ffs(smask) - 1; smask &= smask - 1;
+        cover_straddler(u, m, __shfl_sync(0xffffffffu, t, src), lane, zmin);
+    }
+}
+
+// Per row: visible = #(seg == class id) over the H x W frame, covered = #(linearised float32 depth of zmin > 0.1f).  One CTA
+// strip of pixels per row, a block reduction, one atomicAdd per CTA into the zeroed counts (integer: any order is exact).
+constexpr int kCountThreads = 256, kCountBlocks = 64;
+__global__ void __launch_bounds__(kCountThreads)
+coverage_count_kernel(const uint8_t* __restrict__ seg, const int* __restrict__ class_ids, const unsigned* __restrict__ zmin_all,
+                      int HW, int* __restrict__ visible, int* __restrict__ covered)
+{
+    const int n = blockIdx.y;
+    const int cid = class_ids[n];
+    const unsigned* zmin = zmin_all + static_cast<size_t>(n) * HW;
+    const float zn = 0.1f, zf = 2.0f;
+    int cv = 0, cc = 0;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+        cv += static_cast<int>(seg[p]) == cid;
+        const unsigned zb = zmin[p];
+        if (zb != kCoverClear) {
+            // offscreen_renderer.py -> pyrender's float32 linearisation, as render_kernel's mode 1 and render_full_frame_unlit
+            const float zndc = __fsub_rn(__fmul_rn(2.0f, __uint_as_float(zb)), 1.0f);
+            const float den = __fsub_rn(__fadd_rn(zf, zn), __fmul_rn(zndc, __fsub_rn(zf, zn)));
+            const float metres = __fdiv_rn(__fmul_rn(__fmul_rn(2.0f, zn), zf), den);
+            cc += metres > 0.1f;
+        }
+    }
+    __shared__ int s_v[kCountThreads / 32], s_c[kCountThreads / 32];
+    for (int o = 16; o > 0; o >>= 1) { cv += __shfl_xor_sync(0xffffffffu, cv, o); cc += __shfl_xor_sync(0xffffffffu, cc, o); }
+    if ((threadIdx.x & 31) == 0) { s_v[threadIdx.x >> 5] = cv; s_c[threadIdx.x >> 5] = cc; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int v = 0, c = 0;
+        for (int w = 0; w < kCountThreads / 32; ++w) { v += s_v[w]; c += s_c[w]; }
+        atomicAdd(&visible[n], v); atomicAdd(&covered[n], c);
+    }
+}
 }  // namespace
 
 size_t render_uniform_bytes() { return sizeof(Uniforms); }
@@ -553,6 +690,24 @@ cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s) {
     e = launch_kernel(render_project_kernel, dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n), dim3(kProjThreads), 0, s, true, a);
     if (e != cudaSuccess) return e;
     return launch_kernel(render_kernel, dim3(kBands, n), dim3(kRenderThreads), smem, s, true, a);
+}
+
+cudaError_t launch_coverage(RenderArgs a, int n, int max_nf, const uint8_t* seg, const int* class_ids, unsigned* zmin,
+                            int* visible, int* covered, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    if (!a.projected || !a.uniforms || a.max_nv <= 0 || max_nf <= 0 || a.vw <= 0 || a.vh <= 0) return cudaErrorInvalidValue;
+    a.mode = 2; a.object_width = nullptr;
+    const size_t hw = static_cast<size_t>(a.vw) * a.vh;
+    cudaError_t e = cudaMemsetAsync(zmin, 0x7F, static_cast<size_t>(n) * hw * sizeof(unsigned), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(visible, 0, n * sizeof(int), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(covered, 0, n * sizeof(int), s);
+    if (e != cudaSuccess) return e;
+    e = launch_kernel(render_project_kernel, dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n), dim3(kProjThreads), 0, s, false, a);
+    if (e != cudaSuccess) return e;
+    e = launch_kernel(coverage_kernel, dim3((max_nf + kCoverThreads - 1) / kCoverThreads, n), dim3(kCoverThreads), 0, s, false, a, zmin);
+    if (e != cudaSuccess) return e;
+    return launch_kernel(coverage_count_kernel, dim3(kCountBlocks, n), dim3(kCountThreads), 0, s, false, seg, class_ids,
+                         static_cast<const unsigned*>(zmin), static_cast<int>(hw), visible, covered);
 }
 
 }  // namespace se3tn

@@ -28,4 +28,10 @@ struct RenderArgs {
 size_t render_uniform_bytes();
 size_t render_projected_bytes_per_vertex();
 cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s);
+// The visibility check of produce_train_pair_data.py:97-104 for n rows of one frame: each row's model rendered over the whole
+// vh x vw camera image in the pyrender mode (nearest float32 window z per pixel into zmin, n x vh x vw words of scratch), then
+// visible[i] = #(seg == class_ids[i]) and covered[i] = #(linearised depth > 0.1f).  class_ids, visible, covered device (n).
+// Memsets + 3 launches; `a.mode` and `a.object_width` are ignored.
+cudaError_t launch_coverage(RenderArgs a, int n, int max_nf, const uint8_t* seg, const int* class_ids, unsigned* zmin,
+                            int* visible, int* covered, cudaStream_t s);
 }  // namespace se3tn

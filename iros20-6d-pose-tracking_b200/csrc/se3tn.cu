@@ -197,18 +197,20 @@ struct F64Bits {   // a double held as its bits: a double member would make Step
 // Everything the kernels of one track or validation step are given that can differ from one call to the next.  Its bytes,
 // compared with memcmp, are the key of the step's CUDA graph (run_step), and step_launches takes its arguments from nowhere
 // else: an argument missing here could not be read by the launches, so a replayed graph never runs on stale ones.
+enum : uint8_t { kStepTrack = 0, kStepEval = 1, kStepPairs = 2 };   // StepKey::kind
 struct StepKey {
-    uint8_t eval, mixed;                       // a validation step (se3tn_eval_pairs); the tracks use more than one weight set
+    uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
     uint8_t fill, fill_extrapolate;            // c->depth_fill when a track step is built (zero in a validation step)
     int32_t fill_blur, n, precision, first_wid;      // first_wid: the first track's weight set
     int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
     F64Bits K[4], tn, rn, fill_max_depth;
     const uint8_t* frame_rgb; const uint16_t* frame_depth; const double* object_width;   // track step
     const double* poses_in;                    // track step: the previous poses; validation step: A_in_cam
-    const double* B_in_cam; const uint8_t* rgbB; const uint16_t* depthB;                 // validation step
-    const uint8_t* rgbA; const uint16_t* depthA; const int32_t* wid_dev;                  // wid_dev NULL: every track uses set 0
+    const double* B_in_cam; const uint8_t* rgbB; const uint16_t* depthB;                 // validation step: inputs; pair step: rgbB / depthB outputs
+    const uint8_t* rgbA; const uint16_t* depthA; const int32_t* wid_dev;                  // wid_dev NULL: every track uses set 0 (pair step: mesh ids)
     float* out_trans; float* out_rot; double* poses_out;                                  // poses_out: track step
     float* sq; double* labels; float* sums;                                               // validation step
+    const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -231,6 +233,8 @@ struct se3tn_ctx {
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
     DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
     DevBuf<float> loss_sq; size_t loss_sq_floats = 0;   // se3tn_eval_pairs' loss terms when the caller wants none back: max_batch x 6 (allocated on first use)
+    DevBuf<int> pair_bbox; int pair_bbox_ints = 0;     // se3tn_perturb_pairs' crop windows, max_batch x 8 (allocated on first use, never moved)
+    DevBuf<unsigned> cover_z; size_t cover_z_words = 0;   // se3tn_visibility's nearest-z planes, rows x H x W (grows on demand; never in a captured step)
     DevBuf<uint8_t> metrics; size_t metrics_bytes = 0;   // se3tn_add_adi_sets' staged offsets and ids, or se3tn_vocap_sets' scratch (grows on demand)
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
     // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
@@ -1195,6 +1199,18 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     const double K[4] = {st.K[0], st.K[1], st.K[2], st.K[3]};
     const bool fp32 = st.precision == SE3TN_PREC_FP32;
     int rc;
+    if (st.kind == kStepPairs) {                   // se3tn_perturb_pairs: compute_bbox -> render A (pyrender mode) -> crop B with its seg
+        const double scale[3] = {1000.0, 1000.0, 1000.0};     // produce_train_pair_data.py:118
+        CU_TRY(c, launch_bbox(st.poses_in, K, st.object_width, scale, c->pair_bbox.get(), st.n, s));
+        ++c->launches;
+        rc = queue_render(c, K, st.poses_in, st.object_width, st.wid_dev, st.n, SE3TN_RENDER_PYRENDER, st.H, st.W,
+                          const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s);
+        if (rc) return rc;
+        CU_TRY(c, launch_crop_seg(st.frame_rgb, st.frame_depth, st.seg, st.H, st.W, c->pair_bbox.get(), st.class_ids, st.n, kImg, kImg,
+                                  const_cast<uint8_t*>(st.rgbB), const_cast<uint16_t*>(st.depthB), st.segB, st.seg_count, s));
+        ++c->launches;
+        return SE3TN_OK;
+    }
     if (st.render_mode >= 0) {                     // track i draws mesh weight_ids[i] (0 without ids): one network and one model per object
         rc = queue_render(c, K, st.poses_in, st.object_width, st.wid_dev, st.n, st.render_mode, st.render_H, st.render_W,
                           const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s);
@@ -1217,7 +1233,7 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     PreprocessArgs a{};
     a.poses = st.poses_in; a.rgbA = st.rgbA; a.depthA = st.depthA; a.weight_ids = st.wid_dev; a.precision = st.precision;
     HeadArgs head;
-    if (!st.eval) {
+    if (st.kind == kStepTrack) {
         a.frame_rgb = st.frame_rgb; a.frame_depth = depth; a.H = st.H; a.W = st.W; a.object_width = st.object_width;
         a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
         head.pose_in = st.poses_in; head.pose_out = st.poses_out;
@@ -1229,7 +1245,7 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     }
     if ((rc = queue_preprocess(c, a, st.n, s))) return rc;
     if ((rc = run_tracks(c, st, head, s))) return rc;
-    if (!st.eval) {
+    if (st.kind == kStepTrack) {
         if (!fp32) return SE3TN_OK;                // the head kernel has updated the poses
         ProfScope ps(c, 18, s);
         CU_TRY(c, launch_pose_update(st.poses_in, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
@@ -1259,7 +1275,7 @@ int run_step(se3tn_ctx* c, const Step& st, cudaStream_t s) {
                 return SE3TN_OK;
             }
     // host-side refreshes: synchronous copies, which must not happen inside a capture
-    if ((rc = sync_stats(c, s))) return rc;
+    if (st.kind != kStepPairs && (rc = sync_stats(c, s))) return rc;     // a pair step runs no network
     if (st.mixed && (rc = sync_tables(c, s))) return rc;
     if (st.render_mode >= 0 && (rc = sync_meshes(c, s))) return rc;
     if (capture) {
@@ -1362,7 +1378,7 @@ int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, 
     // allocated once, at max_batch pairs: nothing queued uses it before, and captured steps keep its address after
     if (tensor && !out_sq) CU_TRY(c, grow(c->loss_sq, c->loss_sq_floats, static_cast<size_t>(c->max_batch) * 6));
     Step st{};
-    st.eval = 1; st.n = n; st.precision = precision; st.tn = tn; st.rn = rn; st.render_mode = -1;
+    st.kind = kStepEval; st.n = n; st.precision = precision; st.tn = tn; st.rn = rn; st.render_mode = -1;
     st.wid_host = weight_ids_host; st.first_wid = weight_ids_host ? weight_ids_host[0] : 0; st.mixed = multi;
     st.rgbA = rgbA; st.depthA = depthA; st.rgbB = rgbB; st.depthB = depthB; st.poses_in = A_in_cam; st.B_in_cam = B_in_cam;
     st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot;
@@ -1380,6 +1396,95 @@ int se3tn_pair_loss(se3tn_ctx* c, const float* trans, const float* rot, const do
     { ProfScope ps(c, 21, s); CU_TRY(c, launch_pair_loss(trans, rot, trans_label, rot_label, LossArgs{}, n, out_sums, s)); }
     ++c->launches;
     return SE3TN_OK;
+}
+
+int se3tn_crop_bbox_seg(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W,
+                        const int32_t* bbox, const int32_t* class_ids, int n, int out_h, int out_w,
+                        uint8_t* crop_rgb, uint16_t* crop_depth, uint8_t* crop_seg, int32_t* seg_count, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !seg || !bbox || !crop_rgb || !crop_depth || !crop_seg || H <= 0 || W <= 0 || out_h <= 0 ||
+        out_w <= 0 || n < 0 || (seg_count && !class_ids))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_crop_bbox_seg: null/invalid argument");
+    DeviceGuard guard(c->device);
+    CU_TRY(c, launch_crop_seg(frame_rgb, frame_depth, seg, H, W, bbox, class_ids, n, out_h, out_w, crop_rgb, crop_depth, crop_seg,
+                              seg_count, static_cast<cudaStream_t>(stream)));
+    return SE3TN_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// The mesh ids of a visibility or pair call, checked on the host before anything is queued: both or neither of the host and device
+// copies, n within max_batch, a model for every id.
+int check_meshes(se3tn_ctx* c, const char* fn, const int32_t* ids_host, const int32_t* ids_dev, int n) {
+    if ((ids_host == nullptr) != (ids_dev == nullptr))
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": mesh_ids_host and mesh_ids_dev must both be given or both NULL");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": n exceeds max_batch");
+    for (int i = 0; i < n; ++i) {
+        const int id = ids_host ? ids_host[i] : 0;
+        if (!c->meshes.count(id))
+            return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": mesh id " + std::to_string(id) + " (row " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
+        if (!ids_host) break;
+    }
+    return SE3TN_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int se3tn_visibility(se3tn_ctx* c, const uint8_t* seg, int H, int W, const double* K, const double* poses,
+                     const int32_t* mesh_ids_host, const int32_t* mesh_ids_dev, const int32_t* class_ids, int m,
+                     int32_t* out_visible, int32_t* out_covered, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!seg || !K || !poses || !class_ids || !out_visible || !out_covered || H <= 0 || W <= 0 || H > 65536 || W > 65536)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_visibility: null argument or frame size out of range");
+    int rc = check_meshes(c, "se3tn_visibility", mesh_ids_host, mesh_ids_dev, m);
+    if (rc) return rc;
+    if (m == 0) return SE3TN_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DeviceGuard guard(c->device);
+    if ((rc = sync_meshes(c, s))) return rc;
+    const size_t words = static_cast<size_t>(m) * H * W;
+    if (words > c->cover_z_words) {                 // the old planes may still be read by a queued call
+        CU_TRY(c, cudaStreamSynchronize(s));
+        CU_TRY(c, grow(c->cover_z, c->cover_z_words, words));
+    }
+    int max_nf = 0;
+    for (auto& kv : c->meshes) max_nf = std::max(max_nf, kv.second.nf);
+    RenderArgs a;
+    a.poses = poses; a.object_width = nullptr; a.mesh_ids = mesh_ids_dev; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
+    a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
+    a.rgb = nullptr; a.depth = nullptr; a.mode = 2; a.vw = W; a.vh = H;
+    a.projected = c->render_proj.get(); a.uniforms = c->render_unif.get(); a.max_nv = c->render_max_nv;
+    c->launches = 0;
+    { ProfScope ps(c, 20, s); CU_TRY(c, launch_coverage(a, m, max_nf, seg, class_ids, c->cover_z.get(), out_visible, out_covered, s)); }
+    c->launches = 3;
+    return SE3TN_OK;
+}
+
+int se3tn_perturb_pairs(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W,
+                        const double* K, const double* A_in_cam, const double* object_width,
+                        const int32_t* mesh_ids_host, const int32_t* mesh_ids_dev, const int32_t* class_ids, int n,
+                        uint8_t* rgbA, uint16_t* depthA, uint8_t* rgbB, uint16_t* depthB, uint8_t* segB, int32_t* seg_count,
+                        void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !seg || !K || !A_in_cam || !object_width || !class_ids || H <= 0 || W <= 0 || H > 65536 || W > 65536)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_perturb_pairs: null argument or frame size out of range");
+    if (!rgbA || !depthA || !rgbB || !depthB || !segB || !seg_count) return fail(c, SE3TN_ERR_INVALID, "se3tn_perturb_pairs: null output");
+    int rc = check_meshes(c, "se3tn_perturb_pairs", mesh_ids_host, mesh_ids_dev, n);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    // allocated once, at max_batch rows: captured steps keep its address after
+    CU_TRY(c, grow(c->pair_bbox, c->pair_bbox_ints, c->max_batch * 8));
+    Step st{};
+    st.kind = kStepPairs; st.n = n; st.H = H; st.W = W;
+    for (int i = 0; i < 4; ++i) st.K[i] = K[i];
+    st.render_mode = SE3TN_RENDER_PYRENDER; st.render_H = H; st.render_W = W;
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.seg = seg; st.poses_in = A_in_cam; st.object_width = object_width;
+    st.wid_dev = mesh_ids_dev; st.class_ids = class_ids;
+    st.rgbA = rgbA; st.depthA = depthA; st.rgbB = rgbB; st.depthB = depthB; st.segB = segB; st.seg_count = seg_count;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_add_adi(se3tn_ctx* c, const double* model_pts, int m, const double* pred, const double* gt, int n,

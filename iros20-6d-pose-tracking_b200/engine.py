@@ -506,6 +506,78 @@ class Engine:
                                             rmode, H, W, _ptr(rgb), _ptr(dep), _stream(self.device)), self._ctx)
         return rgb, dep
 
+    # ------------------------------------------------------------------ held-out pairs (produce_train_pair_data.py)
+    def crop_bbox_seg(self, frame_rgb, frame_depth, seg, bbox, out_hw=(IMAGE_SIZE, IMAGE_SIZE), class_ids=None):
+        """crop_bbox with the segmentation plane (se3tn_crop_bbox_seg): seg uint8 CUDA (H,W) -> (rgb, depth, seg, count).  Without
+        class_ids seg holds the labels and count is None; with class_ids (int32 CUDA (n)) seg is (label == class id) as 0 / 1 and
+        count (int32 (n)) the number of ones."""
+        n = int(bbox.shape[0])
+        H, W = frame_depth.shape
+        self._check_dev('seg', seg, torch.uint8, (H, W))
+        crop_rgb = torch.empty(n, out_hw[0], out_hw[1], 3, dtype=torch.uint8, device=self.device)
+        crop_depth = torch.empty(n, out_hw[0], out_hw[1], dtype=torch.uint16, device=self.device)
+        crop_seg = torch.empty(n, out_hw[0], out_hw[1], dtype=torch.uint8, device=self.device)
+        count = torch.empty(n, dtype=torch.int32, device=self.device) if class_ids is not None else None
+        _lib.check(self.lib.se3tn_crop_bbox_seg(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), _ptr(seg), H, W, _ptr(bbox), _ptr(class_ids),
+                                                n, int(out_hw[0]), int(out_hw[1]), _ptr(crop_rgb), _ptr(crop_depth), _ptr(crop_seg),
+                                                _ptr(count), _stream(self.device)), self._ctx)
+        return crop_rgb, crop_depth, crop_seg, count
+
+    def visibility(self, seg, K, poses, class_ids, mesh_ids=None, out_visible=None, out_covered=None):
+        """The visibility check's two counts for m rows of one frame (se3tn_visibility): seg uint8 CUDA (H,W), K 3x3 or (fx,fy,cx,cy),
+        poses float64 CUDA (m,4,4), class_ids int32 (m) (host or CUDA), mesh_ids int32 (m) host array or None (mesh 0).  The camera
+        image is the seg frame's size.  -> (visible, covered) int32 CUDA (m): #(seg == class id) and the pixels of the model's
+        full-image pyrender-mode render whose float32 depth is > 0.1."""
+        m = int(poses.shape[0])
+        H, W = seg.shape
+        self._check_dev('seg', seg, torch.uint8, (H, W))
+        self._check_dev('poses', poses, torch.float64, (m, 4, 4))
+        cid = self._dev_ids(class_ids, m)
+        mh = self._host_ids('visibility', mesh_ids, m)
+        md = torch.from_numpy(mh).to(self.device) if mh is not None else None
+        vis = torch.empty(m, dtype=torch.int32, device=self.device) if out_visible is None else out_visible
+        cov = torch.empty(m, dtype=torch.int32, device=self.device) if out_covered is None else out_covered
+        self._check_dev('out_visible', vis, torch.int32, (m,)); self._check_dev('out_covered', cov, torch.int32, (m,))
+        _lib.check(self.lib.se3tn_visibility(self._ctx, _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _ptr(poses), _hptr(mh), _ptr(md),
+                                             _ptr(cid), m, _ptr(vis), _ptr(cov), _stream(self.device)), self._ctx)
+        return vis, cov
+
+    def perturb_pairs(self, frame_rgb, frame_depth, seg, K, A_in_cam, object_width, class_ids, mesh_ids=None, mesh_ids_dev=None, out=None):
+        """One ProducerPurturb.generate step for n samples of one frame (se3tn_perturb_pairs): compute_bbox of each A_in_cam, A rendered
+        in the pyrender mode over the frame-sized camera image and cropped, B / depthB / segB cropped from the frame through the same
+        window.  frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), seg uint8 (H,W), A_in_cam float64 (n,4,4), object_width float64
+        (n), class_ids int32 (n): CUDA tensors; mesh_ids int32 host array (n) or None (mesh 0).  out: a dict of output tensors to
+        reuse (keeps the step's addresses, so its CUDA graph).  -> dict rgbA, depthA, rgbB, depthB, segB (0/1), count (int32 (n))."""
+        n = int(A_in_cam.shape[0])
+        H, W = frame_depth.shape
+        for name, t, dt, shape in (('frame_rgb', frame_rgb, torch.uint8, (H, W, 3)), ('frame_depth', frame_depth, torch.uint16, (H, W)),
+                                   ('seg', seg, torch.uint8, (H, W)), ('A_in_cam', A_in_cam, torch.float64, (n, 4, 4)),
+                                   ('object_width', object_width, torch.float64, (n,)), ('class_ids', class_ids, torch.int32, (n,))):
+            self._check_dev(name, t, dt, shape)
+        mh = self._host_ids('perturb_pairs', mesh_ids, n)
+        if mh is not None and mesh_ids_dev is None:
+            mesh_ids_dev = torch.from_numpy(mh).to(self.device)
+        img = (n, IMAGE_SIZE, IMAGE_SIZE)
+        spec = dict(rgbA=(img + (3,), torch.uint8), depthA=(img, torch.uint16), rgbB=(img + (3,), torch.uint8), depthB=(img, torch.uint16),
+                    segB=(img, torch.uint8), count=((n,), torch.int32))
+        out = dict(out) if out is not None else {}
+        for k, (shape, dt) in spec.items():
+            if k not in out:
+                out[k] = torch.empty(shape, dtype=dt, device=self.device)
+            self._check_dev('out[%r]' % k, out[k], dt, shape)
+        _lib.check(self.lib.se3tn_perturb_pairs(self._ctx, _ptr(frame_rgb), _ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)),
+                                                _ptr(A_in_cam), _ptr(object_width), _hptr(mh), _ptr(mesh_ids_dev), _ptr(class_ids), n,
+                                                *(_ptr(out[k]) for k in spec), _stream(self.device)), self._ctx)
+        return out
+
+    def _dev_ids(self, ids, n):
+        """int32 (n) ids as a contiguous CUDA tensor (host arrays are uploaded)."""
+        t = ids.to(self.device, torch.int32).contiguous() if torch.is_tensor(ids) else \
+            torch.from_numpy(np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)).to(self.device)
+        if t.shape != (n,):
+            raise ValueError('expected %d ids, got %s' % (n, tuple(t.shape)))
+        return t
+
     @staticmethod
     def _render_mode(mode, image_hw):
         """(SE3TN_RENDER_* value, H, W) of a render mode name and the camera image size it needs."""
