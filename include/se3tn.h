@@ -428,6 +428,29 @@ int se3tn_perturb_pairs(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t
                         uint8_t* rgbA, uint16_t* depthA, uint8_t* rgbB, uint16_t* depthB, uint8_t* segB, int32_t* seg_count,
                         void* stream);
 
+/* The generator's threshold on a sample's segB pixel count (produce_train_pair_data.py:128): a sample is kept when seg_count >= it. */
+#define SE3TN_PAIR_MIN_SEG 100
+
+/* The kept rows of a se3tn_perturb_pairs step appended to per-queue validation batches, with no host read in between.  Row i
+ * (rgbA, rgbB uint8 (n,176,176,3), depthA, depthB uint16 (n,176,176), seg_count int32 (n), A_in_cam, B_in_cam double (n,16), all
+ * device) is kept when seg_count[i] >= SE3TN_PAIR_MIN_SEG and goes to queue q = queue_ids[i], slot tails_dev[q] + (the kept rows of
+ * queue q before it), so each queue receives its rows in row order.  The queues are num_queues x cap rows in the layout
+ * se3tn_eval_pairs reads: q_rgbA, q_rgbB uint8 (num_queues,cap,176,176,3), q_depthA, q_depthB uint16 (num_queues,cap,176,176),
+ * q_A_in_cam, q_B_in_cam double (num_queues,cap,16), device; queue q's slot s is row q * cap + s.  tails_dev int32 (num_queues)
+ * device: each advanced by its queue's kept rows.  Rejected rows and every other slot are left as they were.
+ * One launch (16-byte copies; the CTA that finishes last advances the tails through a context-owned counter).  Checked on the host
+ * before anything is queued, all SE3TN_ERR_INVALID: a null pointer, a device pointer not 16-byte aligned, n > max_batch, a queue
+ * id outside [0, num_queues) (queue_ids_host, with its device copy queue_ids_dev), and a queue whose capacity cannot hold all the
+ * rows sent to it, kept or not: tails_host[q] + #(rows of q) > cap, where tails_host (HOST, num_queues) is what tails_dev holds when
+ * the append runs, or a bound above it (the tails last read back plus every row sent since).  On the device a row whose slot would reach cap is not
+ * written, but its tail still advances, so an overflow shows in the tails read back.  n == 0 queues nothing. */
+int se3tn_append_pairs(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                       const int32_t* seg_count, const double* A_in_cam, const double* B_in_cam,
+                       const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
+                       int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
+                       uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
+                       void* stream);
+
 /* ---- introspection (tests / profiling) -------------------------------------------------------- */
 
 /* Device pointer + per-image float count of an internal NHWC activation buffer.

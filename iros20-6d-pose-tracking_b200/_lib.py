@@ -13,6 +13,7 @@ LABEL_UNDER_POINTS, LABEL_OVER_POINTS = 0, 1
 WEIGHT_BLOB_FLOATS = 13528326
 PROFILE_SLOTS = 22
 TRACE_TILES = 5184
+PAIR_MIN_SEG = 100
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -56,6 +57,8 @@ SIGNATURES = {
     'se3tn_crop_bbox_seg': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_visibility': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_perturb_pairs': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_append_pairs': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp,
+                                _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_debug_buffer': (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_sz)]),
     'se3tn_last_launch_count': (_i, [_vp]),
     'se3tn_get_trace': (_i, [_vp, _vp]),

@@ -309,6 +309,71 @@ cudaError_t launch_crop_seg(const uint8_t* frame_rgb, const uint16_t* frame_dept
 }
 
 // =============================================================================================
+// se3tn_append_pairs: the kept rows of a pair step to the tails of their validation queues
+// =============================================================================================
+// Grid (kAppendSlices, n): CTA (x, i) copies slice x of row i's four planes in 16-byte words (consecutive threads, consecutive
+// words) and, in slice 0, its two poses.  Row i's slot is its queue's tail plus the kept rows of that queue before it, counted by
+// the whole CTA.  Every CTA reads the tail before it counts itself done on a.done; the CTA that counts last has seen every other
+// one read, so it alone adds each queue's kept rows to its tail, then clears the counter for the next launch.
+constexpr int kAppendThreads = 256, kAppendSlices = 8;
+constexpr int kRgbWords = kImg * kImg * 3 / 16, kDepthWords = kImg * kImg * 2 / 16, kPoseWords = 16 * 8 / 16;
+static_assert(kImg * kImg * 3 % 16 == 0 && kImg * kImg * 2 % 16 == 0, "a crop plane is a whole number of 16-byte words");
+
+__device__ __forceinline__ void copy_words(const void* src, void* dst, int words) {
+    const uint4* s = static_cast<const uint4*>(src);
+    uint4* d = static_cast<uint4*>(dst);
+    for (int v = blockIdx.x * kAppendThreads + threadIdx.x; v < words; v += kAppendSlices * kAppendThreads) d[v] = __ldg(s + v);
+}
+
+__global__ void __launch_bounds__(kAppendThreads) append_pairs_kernel(const AppendArgs a)
+{
+    const int i = blockIdx.y;
+    const int q = a.queue_ids[i];
+    int before = 0;
+    for (int j0 = 0; j0 < i; j0 += kAppendThreads) {
+        const int j = j0 + threadIdx.x;
+        before += __syncthreads_count(j < i && a.queue_ids[j] == q && a.count[j] >= a.min_count);
+    }
+    __shared__ int s_tail;
+    __shared__ bool s_last;
+    if (threadIdx.x == 0) s_tail = a.tails[q];
+    __syncthreads();
+    const int slot = s_tail + before;
+    if (a.count[i] >= a.min_count && slot < a.cap) {
+        const size_t src = static_cast<size_t>(i), dst = static_cast<size_t>(q) * a.cap + slot;
+        copy_words(a.rgbA + src * kRgbWords * 16, a.q_rgbA + dst * kRgbWords * 16, kRgbWords);
+        copy_words(a.rgbB + src * kRgbWords * 16, a.q_rgbB + dst * kRgbWords * 16, kRgbWords);
+        copy_words(a.depthA + src * kDepthWords * 8, a.q_depthA + dst * kDepthWords * 8, kDepthWords);
+        copy_words(a.depthB + src * kDepthWords * 8, a.q_depthB + dst * kDepthWords * 8, kDepthWords);
+        if (blockIdx.x == 0 && threadIdx.x < 2 * kPoseWords) {
+            const bool b = threadIdx.x >= kPoseWords;
+            const int w = threadIdx.x - (b ? kPoseWords : 0);
+            const uint4* s = reinterpret_cast<const uint4*>((b ? a.B_in_cam : a.A_in_cam) + src * 16);
+            reinterpret_cast<uint4*>((b ? a.q_B : a.q_A) + dst * 16)[w] = __ldg(s + w);
+        }
+    }
+    if (threadIdx.x == 0) {
+        __threadfence();
+        s_last = atomicAdd(a.done, 1u) == gridDim.x * gridDim.y - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (int r = threadIdx.x; r < a.num_queues; r += kAppendThreads) {
+        int kept = 0;
+        for (int j = 0; j < a.n; ++j) kept += a.queue_ids[j] == r && a.count[j] >= a.min_count;
+        if (kept) a.tails[r] += kept;
+    }
+    if (threadIdx.x == 0) *a.done = 0u;
+}
+
+cudaError_t launch_append_pairs(const AppendArgs& a, cudaStream_t s) {
+    if (a.n <= 0) return cudaSuccess;
+    append_pairs_kernel<<<dim3(kAppendSlices, a.n), kAppendThreads, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+// =============================================================================================
 // NCHW float32 (N,4,176,176) -> zero-padded NHWC4 stem input (for Se3TrackNet.forward(A, B))
 // =============================================================================================
 __global__ void __launch_bounds__(256)

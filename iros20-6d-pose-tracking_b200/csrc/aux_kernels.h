@@ -53,6 +53,16 @@ cudaError_t launch_crop(const uint8_t* frame_rgb, const uint16_t* frame_depth, i
 cudaError_t launch_crop_seg(const uint8_t* frame_rgb, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const int* bbox,
                             const int* class_ids, int n, int out_h, int out_w, uint8_t* crop_rgb, uint16_t* crop_depth,
                             uint8_t* crop_seg, int* count, cudaStream_t s);
+// se3tn_append_pairs: rows of a pair step with count >= min_count copied to their queue's tail (see include/se3tn.h)
+struct AppendArgs {
+    const uint8_t* rgbA; const uint16_t* depthA; const uint8_t* rgbB; const uint16_t* depthB;   // (n, 176, 176[, 3])
+    const int* count; const double* A_in_cam; const double* B_in_cam; const int* queue_ids;     // (n), (n,16), (n,16), (n)
+    int n, num_queues, cap, min_count;
+    int* tails;                    // (num_queues), advanced by the CTA that finishes last
+    unsigned* done;                // context-owned CTA counter, zero between launches
+    uint8_t* q_rgbA; uint16_t* q_depthA; uint8_t* q_rgbB; uint16_t* q_depthB; double* q_A; double* q_B;   // (num_queues * cap, ...)
+};
+cudaError_t launch_append_pairs(const AppendArgs& a, cudaStream_t s);
 cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s);
 cudaError_t launch_maxpool(const float* in, float* out, int n_img, int Hin, int Win, int C, cudaStream_t s);
 // poses_in non-null: also the pose update of every track (K6 fused into K4); loss.poses_a non-null: also the loss terms of every pair;

@@ -11,10 +11,16 @@ are added in order.  The pairs are taken in file order (the reference's validati
 
     python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
                                  [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200]
+    python -m <package>.problems --ycb_dir DIR --class_ids all|3,5 --ckpt_dir TPL --mean_std_path TPL --train_data_path TPL
+                                 --model_path TPL [--num_sample 10] [--seed 0] [--precision MODE|all] [--batch_size 200] [--max_batch 200]
+
+The second form scores every class's checkpoint on the perturbed pairs of the YCB-Video key frames in one pass (validate_ycbv):
+bit-identical to `produce_train_pair_data --mode ycbv` followed by the first form on each class's folder, without the files.
 """
 import argparse
 import contextlib
 import os
+import random
 
 import numpy as np
 import torch
@@ -168,17 +174,244 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
                 predictions=preds.cpu().numpy() if preds is not None else None)
 
 
+# ----------------------------------------------------------------------------------------------------
+# One pass over perturbed YCB-Video key frames: the pairs `produce_train_pair_data --mode ycbv` would write, scored as
+# `evaluate` scores each class's folder, without the files.
+# ----------------------------------------------------------------------------------------------------
+class PairQueues:
+    """Per-class device queues of kept pairs and the validation steps that drain them.
+
+    add() takes one frame's pair steps and appends each kept row to its class's queue on the device (Engine.append_pairs: one
+    launch per step, slots and tails computed there).  Before that it drains every queue the earlier frames filled: each full
+    batch (rows [0, batch_size)) runs in every mode, cut into steps as batch_plan cuts it, and the remaining rows move to the
+    front, so a class's full batches always read the same addresses and replay their CUDA graphs.  finish() drains the full
+    batches left and then each class's partial last batch, and returns the results.  A class's batches are thus the loader's
+    batches over its pairs in count order, and its step sums are added exactly as `evaluate` adds them.
+
+    The tails come back through a pinned copy queued after each append and waited for at the next add(); the frame loop's
+    visibility call has synchronised the stream by then, so the wait costs nothing.  Device memory: the queues hold
+    len(class_ids) x (batch_size + rows_per_frame) pairs of 176 x 176 x 10 bytes plus two float64 poses each, e.g. about 1.4 GB
+    for 21 classes, batch_size 200 and 10 samples per class and frame."""
+
+    PLANES = (('rgbA', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', torch.uint16, (IMAGE_SIZE, IMAGE_SIZE)),
+              ('rgbB', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthB', torch.uint16, (IMAGE_SIZE, IMAGE_SIZE)),
+              ('A_in_cam', torch.float64, (4, 4)), ('B_in_cam', torch.float64, (4, 4)))
+
+    def __init__(self, eng, normalizers, modes, batch_size, max_batch, rows_per_frame, keep_predictions=False):
+        """normalizers: {class id (the weight set and mesh id): (trans_normalizer, rot_normalizer)}.  rows_per_frame: the most
+        rows one frame sends to one class (num_sample).  max_batch: the most pairs per validation step."""
+        if batch_size <= 0 or max_batch <= 0 or rows_per_frame <= 0:
+            raise ValueError('batch_size, max_batch and rows_per_frame must be positive')
+        self.eng = eng
+        self.ids = sorted(normalizers)
+        self.qid = {c: q for q, c in enumerate(self.ids)}
+        self.normalizers = dict(normalizers)
+        self.modes = list(modes)
+        self.batch_size = int(batch_size)
+        self.step = min(int(max_batch), self.batch_size)
+        if self.step > eng.max_batch:
+            raise ValueError('validation steps of %d pairs need an Engine of max_batch >= %d (it has %d)' % (self.step, self.step, eng.max_batch))
+        self.cap = self.batch_size + int(rows_per_frame)
+        self.keep_predictions = keep_predictions
+        dev = eng.device
+        Q = len(self.ids)
+        self.queues = {k: torch.empty((Q, self.cap) + shape, dtype=dt, device=dev) for k, dt, shape in self.PLANES}
+        self.tails = np.zeros(Q, dtype=np.int32)            # host: exact after a read-back, then a bound as rows are sent
+        self.tails_dev = torch.zeros(Q, dtype=torch.int32, device=dev)
+        on_cuda = torch.device(dev).type == 'cuda'
+        self._tails_back = torch.zeros(Q, dtype=torch.int32, pin_memory=on_cuda)
+        self._back_done = torch.cuda.Event() if on_cuda else None
+        self._sent = False                                  # rows appended since the tails were last read back
+        self.out_trans = torch.empty(self.step, 3, dtype=torch.float32, device=dev)
+        self.out_rot = torch.empty(self.step, 3, dtype=torch.float32, device=dev)
+        self.out_sums = torch.empty(2, dtype=torch.float32, device=dev)
+        self.ids_host = {c: np.full(self.step, c, dtype=np.int32) for c in self.ids}
+        self.ids_dev = {c: torch.from_numpy(self.ids_host[c]).to(dev) for c in self.ids}
+        self.pairs = {c: 0 for c in self.ids}
+        self.sums = {c: {m: [] for m in self.modes} for c in self.ids}
+        self.preds = {c: {m: [] for m in self.modes} for c in self.ids}
+        self.calibrated = set()
+
+    def add(self, owners, chunks):
+        """One frame: owners [(class id, B_in_cam, [A_in_cam of its rows], first row)], chunks [(first row, perturb_pairs dict with
+        A_in_cam)] as produce_train_pair_data.ycbv_pair_steps yields them with on_device."""
+        self._drain(final=False)
+        row_q, row_B = [], []
+        for c, B, inside, _ in owners:
+            row_q += [self.qid[c]] * len(inside)
+            row_B += [B] * len(inside)
+        for i0, res in chunks:
+            n = int(res['A_in_cam'].shape[0])
+            qids = np.array(row_q[i0:i0 + n], dtype=np.int32)
+            B = torch.from_numpy(np.ascontiguousarray(np.stack(row_B[i0:i0 + n]), dtype=np.float64)).to(self.eng.device)
+            self.eng.append_pairs(res, res['A_in_cam'], B, qids, self.tails, self.tails_dev, self.queues)
+            self.tails += np.bincount(qids, minlength=len(self.ids)).astype(np.int32)
+            self._sent = True
+        if self._sent:
+            self._tails_back.copy_(self.tails_dev, non_blocking=True)
+            if self._back_done is not None:
+                self._back_done.record(torch.cuda.current_stream(self.eng.device))
+
+    def finish(self):
+        """Drain every queue, the partial last batches included -> {class id: {mode: dict}}: `evaluate`'s dict plus 'pairs'.  A
+        class without a kept pair has pairs 0, trans / rot None, empty batch losses and predictions None."""
+        self._drain(final=True)
+        out = {}
+        for c in self.ids:
+            n = self.pairs[c]
+            out[c] = {}
+            for m in self.modes:
+                if n == 0:
+                    out[c][m] = dict(pairs=0, trans=None, rot=None, batch_trans=np.zeros(0, np.float32), batch_rot=np.zeros(0, np.float32),
+                                     predictions=None)
+                    continue
+                steps = batch_plan(n, self.batch_size, self.step)
+                assert len(steps) == len(self.sums[c][m])
+                bt, br = batch_means(torch.stack(self.sums[c][m]).cpu().numpy(), steps)
+                preds = torch.cat(self.preds[c][m]).cpu().numpy() if self.keep_predictions else None
+                out[c][m] = dict(pairs=n, trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
+                                 predictions=preds)
+        return out
+
+    def _drain(self, final):
+        """Read the tails back, run every full batch (and with `final` every partial one), move the remainders to the front."""
+        if self._sent:
+            if self._back_done is not None:
+                self._back_done.synchronize()
+            self.tails[:] = self._tails_back.numpy()
+            self._sent = False
+            if (self.tails > self.cap).any():
+                raise RuntimeError('a pair queue overflowed: tails %s, capacity %d' % (self.tails.tolist(), self.cap))
+        moved = False
+        for q, c in enumerate(self.ids):
+            while self.tails[q] >= self.batch_size or (final and self.tails[q] > 0):
+                n = min(int(self.tails[q]), self.batch_size)
+                self._eval_batch(q, c, n)
+                rest = int(self.tails[q]) - n
+                for k, _, _ in self.PLANES:
+                    if rest:
+                        self.queues[k][q, :rest].copy_(self.queues[k][q, n:n + rest].clone())
+                self.tails[q] = rest
+                moved = True
+        if moved:
+            self.tails_dev.copy_(torch.from_numpy(self.tails))
+
+    def _eval_batch(self, q, c, n_rows):
+        """Rows [0, n_rows) of queue q as one loader batch, in every mode."""
+        tn, rn = self.normalizers[c]
+        d = self.queues
+        for m in self.modes:
+            for _, s, e in batch_plan(n_rows, self.batch_size, self.step):
+                n = e - s
+                pairs = [d[k][q, s:e] for k in ('rgbA', 'depthA', 'rgbB', 'depthB')]
+                if m == 'fp8' and c not in self.calibrated:      # the set's scales from its first step, as evaluate's k == 0
+                    self.eng.calibrate_fp8_pairs(*pairs, d['A_in_cam'][q, s:e], self.ids_host[c][:n])
+                    self.calibrated.add(c)
+                self.eng.eval_pairs(*pairs, d['A_in_cam'][q, s:e], d['B_in_cam'][q, s:e], tn, rn, weight_ids_host=self.ids_host[c][:n],
+                                    weight_ids_dev=self.ids_dev[c][:n], precision=m, out_trans=self.out_trans[:n],
+                                    out_rot=self.out_rot[:n], out_sums=self.out_sums)
+                self.sums[c][m].append(self.out_sums.clone())
+                if self.keep_predictions:
+                    self.preds[c][m].append(torch.cat((self.out_trans[:n], self.out_rot[:n]), 1))
+        self.pairs[c] += n_rows
+
+
+def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_size=200, max_batch=200, precisions=('bf16x3',),
+                  keep_predictions=False, decode_ahead=4, workers=None, engine=None):
+    """Problem.validate of every class on the perturbed pairs of the YCB-Video key frames, in one pass and without pair files.
+
+    For each class and mode the result is bit-identical to `produce_train_pair_data --mode ycbv` with the same seed and
+    num_sample followed by `evaluate` on that class's folder with the same batch_size and max_batch: the same pair count, per-batch
+    MSEs, means over batches and (keep_predictions) per-pair outputs.  The frame loop is the writer's own
+    (produce_train_pair_data.ycbv_pair_steps: the same draws in the same order, so random / np.random end in the same state),
+    and a class's kept pairs are batched in the order the writer numbers them; see PairQueues.
+
+    templates: ckpt_dir, mean_std_path, train_data_path and model_path with {class_id} / {class_name} placeholders, as
+    `predict --mode ycbv_all` takes them.  One Engine (engine, or one of max(min(max_batch, batch_size), classes x num_sample)
+    rows) holds every class's weights, statistics and mesh under id = class id.  Each class's loss uses its dataset_info.yml's
+    max_translation and max_rotation * pi / 180, as the loader's labels do.  fp8 calibrates each class on its first step.
+
+    -> {class id: {mode: evaluate's dict plus 'pairs'}}.  A class without a kept pair is reported with 0 pairs and no loss
+    (trans / rot None), where `evaluate` on its empty folder raises ValueError.  The queues take
+    classes x (batch_size + num_sample) x 176 x 176 x 10 bytes of device memory (about 1.4 GB for 21 classes at 200 and 10)."""
+    from .engine import Engine
+    from .predict import ycb_class_names, expand_class_paths, _load_run_files
+    from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
+    modes = list(precisions)
+    for m in modes:
+        PREC[m]                                             # an unknown mode fails here
+    names = ycb_class_names(ycb_dir)
+    ids = sorted(set(int(c) for c in class_ids))
+    if not ids:
+        raise ValueError('no class ids given')
+    runs = {}
+    for c in ids:
+        if not 1 <= c <= len(names):
+            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
+        runs[c] = _load_run_files('class %d (%s)' % (c, names[c - 1]), expand_class_paths(templates, c, names[c - 1]))
+        if int(runs[c]['dataset_info']['resolution']) != IMAGE_SIZE:
+            raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
+    step = min(int(max_batch), int(batch_size))
+    eng = engine if engine is not None else Engine(max_batch=max(step, len(ids) * int(num_sample)))
+    normalizers = {}
+    for c in ids:
+        info = runs[c]['dataset_info']
+        ckpt = torch.load(runs[c]['ckpt_dir'], map_location='cpu')
+        eng.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt, c)
+        eng.set_stats(np.asarray(runs[c]['mean']), np.asarray(runs[c]['std']), c)
+        normalizers[c] = (info['max_translation'], info['max_rotation'] * np.pi / 180)
+    _, producers = ycbv_producers(ycb_dir, ids, templates, eng, workers)
+    queues = PairQueues(eng, normalizers, modes, batch_size, step, num_sample, keep_predictions)
+    random.seed(seed); np.random.seed(seed)
+    jobs = ycbv_keyframe_jobs(ycb_dir, ids)
+    for owners, chunks in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True):
+        queues.add(owners, chunks)
+    return queues.finish()
+
+
+ALL_MODES = ['fp32', 'bf16x3', 'tf32', 'bf16']          # --precision all, fp32 first: the reference of "max |d6|"
+
+
+def _print_modes(modes, losses, w):
+    """The per-mode table: losses(m) -> evaluate's dict (with predictions when there is more than one mode)."""
+    print('%-8s %14s %14s %14s %s' % ('mode', 'trans loss', 'rot loss', 'total', 'max |d6| vs fp32' if len(modes) > 1 else ''))
+    ref = None
+    for m in modes:
+        r = losses(m)
+        dev6 = ''
+        if len(modes) > 1:
+            if ref is None:
+                ref = r['predictions']
+            dev6 = '%.3e' % float(np.abs(r['predictions'] - ref).max())
+        print('%-8s %14.8g %14.8g %14.8g %s' % (m, r['trans'], r['rot'], r['trans'] * w['trans'] + r['rot'] * w['rot'], dev6))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="Validation loss of a se(3)-TrackNet checkpoint on a folder of training pairs "
-                                             "(the reference's Problem.validate), per precision mode")
-    ap.add_argument('--val_dir', required=True, help='folder of *rgbA.png / rgbB / depthA / depthB / [segB] / meta.npz pairs')
-    ap.add_argument('--ckpt', required=True, help="checkpoint with a 'state_dict' (e.g. model_best_val.pth.tar)")
-    ap.add_argument('--mean_std_path', required=True, help='folder holding mean.npy and std.npy (train.py:124-125)')
-    ap.add_argument('--dataset_info', required=True, help='dataset_info.yml (resolution, max_translation, max_rotation)')
+                                             "(the reference's Problem.validate), per precision mode; or of every class's checkpoint "
+                                             "on the perturbed pairs of the YCB-Video key frames, in one pass without pair files")
+    src = ap.add_mutually_exclusive_group(required=True)
+    src.add_argument('--val_dir', help='folder of *rgbA.png / rgbB / depthA / depthB / [segB] / meta.npz pairs')
+    src.add_argument('--ycb_dir', help='YCB-Video root (data_organized/, image_sets/keyframe.txt, CADmodels/): score the pairs '
+                                       '`produce_train_pair_data --mode ycbv` would write, class by class, without writing them')
+    ap.add_argument('--ckpt', help="--val_dir: checkpoint with a 'state_dict' (e.g. model_best_val.pth.tar)")
+    ap.add_argument('--mean_std_path', help='folder holding mean.npy and std.npy (train.py:124-125); --ycb_dir: its path template')
+    ap.add_argument('--dataset_info', help='--val_dir: dataset_info.yml (resolution, max_translation, max_rotation)')
+    ap.add_argument('--class_ids', help='--ycb_dir: comma-separated class ids, or all')
+    ap.add_argument('--ckpt_dir', help='--ycb_dir: path template ({class_id}, {class_name}) of each class\'s checkpoint')
+    ap.add_argument('--train_data_path', help='--ycb_dir: path template; dataset_info.yml is read from its ../')
+    ap.add_argument('--model_path', help='--ycb_dir: path template of each class\'s mesh')
+    ap.add_argument('--num_sample', type=int, default=10, help='--ycb_dir: perturbations drawn per annotated class and key frame')
+    ap.add_argument('--seed', type=int, default=0, help='--ycb_dir: seed of random and np.random before the first draw')
     ap.add_argument('--precision', default='bf16x3', choices=sorted(PREC) + ['all'])
     ap.add_argument('--batch_size', type=int, default=200, help='the validation loader batch size (train.py:146)')
     ap.add_argument('--max_batch', type=int, default=200, help='pairs per device step (a larger batch runs as several steps)')
     args = ap.parse_args(argv)
+    modes = ALL_MODES if args.precision == 'all' else [args.precision]
+    if args.ycb_dir:
+        return _main_ycbv(ap, args, modes)
+    if not (args.ckpt and args.mean_std_path and args.dataset_info):
+        ap.error('--val_dir needs --ckpt, --mean_std_path and --dataset_info')
     import yaml
     from .se3_tracknet import Se3TrackNet
     with open(args.dataset_info) as f:
@@ -192,19 +425,36 @@ def main(argv=None):
     model = Se3TrackNet(image_size=int(info['resolution']), max_batch=min(args.max_batch, args.batch_size))
     model.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt)
     prob = Problem(model, None, loader, config={'loss_weights': {'trans': 1, 'rot': 1}})   # config.yml:13-15
-    modes = ['fp32', 'bf16x3', 'tf32', 'bf16'] if args.precision == 'all' else [args.precision]
     print('%d pairs, batch %d, %s' % (len(ds), args.batch_size, torch.cuda.get_device_name(model.engine.device)))
-    print('%-8s %14s %14s %14s %s' % ('mode', 'trans loss', 'rot loss', 'total', 'max |d6| vs fp32' if len(modes) > 1 else ''))
-    ref = None
-    for m in modes:
-        r = prob.validation_losses(m, keep_predictions=len(modes) > 1)
-        w = prob.loss_weights
-        dev6 = ''
-        if len(modes) > 1:
-            if ref is None:
-                ref = r['predictions']
-            dev6 = '%.3e' % float(np.abs(r['predictions'] - ref).max())
-        print('%-8s %14.8g %14.8g %14.8g %s' % (m, r['trans'], r['rot'], r['trans'] * w['trans'] + r['rot'] * w['rot'], dev6))
+    _print_modes(modes, lambda m: prob.validation_losses(m, keep_predictions=len(modes) > 1), prob.loss_weights)
+
+
+def _main_ycbv(ap, args, modes):
+    """--ycb_dir: validate_ycbv, then per class the table --val_dir prints."""
+    from .predict import ycb_class_names, YCB_ALL_TEMPLATES
+    if args.ckpt or args.dataset_info:
+        ap.error('--ycb_dir takes --ckpt_dir and --train_data_path templates, not --ckpt / --dataset_info')
+    if not args.class_ids or not all(getattr(args, k) for k in YCB_ALL_TEMPLATES):
+        ap.error('--ycb_dir needs --class_ids, --ckpt_dir, --mean_std_path, --train_data_path and --model_path')
+    names = ycb_class_names(args.ycb_dir)
+    if args.class_ids == 'all':
+        ids = list(range(1, len(names) + 1))
+    else:
+        try:
+            ids = sorted(set(int(c) for c in args.class_ids.split(',')))
+        except ValueError:
+            ap.error('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+    res = validate_ycbv(args.ycb_dir, ids, {k: getattr(args, k) for k in YCB_ALL_TEMPLATES}, num_sample=args.num_sample, seed=args.seed,
+                        batch_size=args.batch_size, max_batch=args.max_batch, precisions=modes, keep_predictions=len(modes) > 1)
+    device = torch.cuda.get_device_name(torch.cuda.current_device())
+    for c in ids:
+        n = res[c][modes[0]]['pairs']
+        print('class %d (%s): %d pairs, batch %d, %s' % (c, names[c - 1], n, args.batch_size, device))
+        if n == 0:
+            print('no kept pair: no loss')
+            continue
+        _print_modes(modes, lambda m: res[c][m], {'trans': 1, 'rot': 1})                        # config.yml:13-15
+    return res
 
 
 if __name__ == '__main__':

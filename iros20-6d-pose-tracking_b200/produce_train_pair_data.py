@@ -1,7 +1,8 @@
 """Drop-in for the reference's produce_train_pair_data.py: ProducerPurturb (reference produce_train_pair_data.py:58-141), which cuts
 perturbed (A, B) pairs out of annotated frames, completeBlender (:145-226), its driver over a Blender data set, and a YCB-Video
 mode that builds held-out pair folders from real key frames.  The folders are what TrackDataset and Problem.validate read
-(`python -m <package>.problems --val_dir ...`).
+(`python -m <package>.problems --val_dir ...`); `problems --ycb_dir` scores the same pairs in one pass without writing them,
+on the key-frame loop both share (ycbv_pair_steps).
 
 What runs where:
   * host (numpy, the reference's own arithmetic): the perturbations B_in_A (Utils.random_gaussian_magnitude, in the reference's
@@ -87,10 +88,12 @@ def visibility(engine, seg_dev, K32, rows):
     return np.concatenate(vis).astype(np.int64), np.concatenate(cov).astype(np.int64)
 
 
-def pair_step(engine, frame_dev, K32, rows):
+def pair_step(engine, frame_dev, K32, rows, on_device=False):
     """rows: [(A_in_cam, object width, mesh id, class id)] of one frame -> dict of host arrays rgbA, depthA, rgbB, depthB, segB,
-    count (one row each), through Engine.perturb_pairs in chunks of max_batch."""
+    count (one row each), through Engine.perturb_pairs in chunks of max_batch.  on_device: nothing is copied back; -> a list of
+    (first row, the chunk's perturb_pairs dict with its A_in_cam CUDA tensor added), one per chunk."""
     out = {k: [] for k in ('rgbA', 'depthA', 'rgbB', 'depthB', 'segB', 'count')}
+    chunks = []
     rgb, depth, seg = frame_dev
     dev = engine.device
     for i0 in range(0, len(rows), engine.max_batch):
@@ -99,8 +102,13 @@ def pair_step(engine, frame_dev, K32, rows):
         ow = torch.tensor([float(r[1]) for r in chunk], dtype=torch.float64, device=dev)
         cid = torch.tensor([int(r[3]) for r in chunk], dtype=torch.int32, device=dev)
         res = engine.perturb_pairs(rgb, depth, seg, K32.astype(np.float64), A, ow, cid, mesh_ids=np.array([r[2] for r in chunk], np.int32))
+        if on_device:
+            chunks.append((i0, dict(res, A_in_cam=A)))
+            continue
         for k in out:
             out[k].append(res[k].cpu().numpy())
+    if on_device:
+        return chunks
     return {k: np.concatenate(v) if v else None for k, v in out.items()}
 
 
@@ -300,33 +308,41 @@ def ycbv_keyframe_jobs(ycb_dir, class_ids):
     return jobs
 
 
-def produce_ycbv(ycb_dir, class_ids, templates, outdir, num_sample=10, seed=0, max_batch=64, decode_ahead=4, workers=None):
-    """The YCB-Video mode (see above).  templates: {'train_data_path', 'model_path'} with {class_id} / {class_name} placeholders, as
-    --mode ycbv_all takes them; dataset_info.yml is read from <train_data_path>/../.  -> {class id: pairs written}."""
+def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None):
+    """One check_vis ProducerPurturb per class on `eng`, its mesh under id = class id.  templates: {'train_data_path',
+    'model_path'} with {class_id} / {class_name} placeholders, as --mode ycbv_all takes them; dataset_info.yml is read from
+    <train_data_path>/../.  The classes of a frame share one step, so they must share the camera.  -> (CADmodels folder names,
+    {class id: producer})."""
     import yaml
-    from .predict import ycb_class_names, read_rgb, read_depth
-    from .staging import StagingRing
+    from .predict import ycb_class_names
     names = ycb_class_names(ycb_dir)
-    class_ids = sorted(set(int(c) for c in class_ids))
-    eng = Engine(max_batch=max_batch)
-    producers, outs = {}, {}
-    for c in class_ids:
+    producers = {}
+    for c in sorted(set(int(c) for c in class_ids)):
         if not 1 <= c <= len(names):
             raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
         paths = {k: str(templates[k]).format(class_id=c, class_name=names[c - 1]) for k in ('train_data_path', 'model_path')}
         with open(os.path.join(paths['train_data_path'], '../dataset_info.yml'), 'r') as ff:
             info = yaml.safe_load(ff)
         producers[c] = ProducerPurturb(info, check_vis=True, engine=eng, model=paths['model_path'], mesh_id=c, workers=workers)
-        outs[c] = os.path.join(outdir, names[c - 1], '')
-        os.makedirs(outs[c], exist_ok=True)
-    first = producers[class_ids[0]]
-    for c in class_ids:
-        if producers[c].dataset_info['camera'] != first.dataset_info['camera']:
-            raise ValueError('class %d: its camera differs from class %d\'s; the classes of a frame share one step' % (c, class_ids[0]))
+    first_id = min(producers)
+    for c, p in producers.items():
+        if p.dataset_info['camera'] != producers[first_id].dataset_info['camera']:
+            raise ValueError('class %d: its camera differs from class %d\'s; the classes of a frame share one step' % (c, first_id))
+    return names, producers
+
+
+def ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead=4, workers=None, on_device=False):
+    """The key-frame loop of the YCB-Video mode, shared by produce_ycbv (which writes the kept pairs) and problems.validate_ycbv
+    (which scores them).  jobs: ycbv_keyframe_jobs.  Per frame, decoded ahead through a StagingRing: one visibility call for all
+    its classes (it synchronises), then, per visible class in class order, `draw` of num_sample offsets, then one pair step for
+    every sample inside the image.  Yields, per frame with such a sample, (owners, res): owners [(class id, B_in_cam, [A_in_cam
+    of its rows], first row)] and res pair_step's result for the frame's rows (a list of device chunks with on_device).  A frame's
+    device buffers are refilled once the loop resumes, so what res holds is consumed (or queued on the stream) before that."""
+    from .predict import read_rgb, read_depth
+    from .staging import StagingRing
+    first = producers[min(producers)]
     H, W = int(first.dataset_info['camera']['height']), int(first.dataset_info['camera']['width'])
     K32 = first.cam_K
-    random.seed(seed); np.random.seed(seed)
-    jobs = ycbv_keyframe_jobs(ycb_dir, class_ids)
 
     def seg_into(h, path):
         s = cv2.imread(path, cv2.IMREAD_UNCHANGED)
@@ -340,21 +356,36 @@ def produce_ycbv(ycb_dir, class_ids, templates, outdir, num_sample=10, seed=0, m
     ring = StagingRing(dict(rgb=((H, W, 3), torch.uint8), depth=((H, W), torch.uint16), seg=((H, W), torch.uint8)), decode_ahead, eng.device)
     items = [[(into, 'rgb', read_rgb, j[0]), (into, 'depth', read_depth, j[1]), (seg_into, j[2])] for j in jobs]
     frame = (ring.dev['rgb'], ring.dev['depth'], ring.dev['seg'])
+    for k, _ in enumerate(ring.uploads(items, workers or min(16, os.cpu_count() or 4))):
+        rows = jobs[k][3]
+        vis, cov = visibility(eng, frame[2], K32, [(B, c, c) for c, B in rows])
+        step, owners = [], []
+        for (c, B), v, cv in zip(rows, vis, cov):
+            if not visible_enough(v, cv):
+                continue
+            inside = [A for A, ok in producers[c].draw(B, num_sample) if ok]
+            owners.append((c, B, inside, len(step)))
+            step += [(A, producers[c].object_width, c, c) for A in inside]
+        if not step:
+            continue
+        yield owners, pair_step(eng, frame, K32, step, on_device)
+
+
+def produce_ycbv(ycb_dir, class_ids, templates, outdir, num_sample=10, seed=0, max_batch=64, decode_ahead=4, workers=None):
+    """The YCB-Video mode (see above).  templates: {'train_data_path', 'model_path'} with {class_id} / {class_name} placeholders, as
+    --mode ycbv_all takes them; dataset_info.yml is read from <train_data_path>/../.  -> {class id: pairs written}."""
+    class_ids = sorted(set(int(c) for c in class_ids))
+    eng = Engine(max_batch=max_batch)
+    names, producers = ycbv_producers(ycb_dir, class_ids, templates, eng, workers)
+    outs = {}
+    for c in class_ids:
+        outs[c] = os.path.join(outdir, names[c - 1], '')
+        os.makedirs(outs[c], exist_ok=True)
+    random.seed(seed); np.random.seed(seed)
+    jobs = ycbv_keyframe_jobs(ycb_dir, class_ids)
     with ThreadPoolExecutor(max_workers=workers or min(16, os.cpu_count() or 4)) as pool:
         futures = []
-        for k, _ in enumerate(ring.uploads(items, workers or min(16, os.cpu_count() or 4))):
-            rows = jobs[k][3]
-            vis, cov = visibility(eng, frame[2], K32, [(B, c, c) for c, B in rows])
-            step, owners = [], []
-            for (c, B), v, cv in zip(rows, vis, cov):
-                if not visible_enough(v, cv):
-                    continue
-                inside = [A for A, ok in producers[c].draw(B, num_sample) if ok]
-                owners.append((c, B, inside, len(step)))
-                step += [(A, producers[c].object_width, c, c) for A in inside]
-            if not step:
-                continue
-            res = pair_step(eng, frame, K32, step)
+        for owners, res in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers):
             for c, B, inside, at in owners:
                 producers[c].keep(outs[c], B, inside, res, at, c, pool, futures)
             done = [f for f in futures if f.done()]
