@@ -14,7 +14,8 @@ Differences, all additive:
   * on_track_batch(): N independent tracks of one frame in one batched launch sequence (the
     reference is batch 1, F15).  Numpy frames and poses take the host route: one se3tn_track_host /
     se3tn_track_render_host call that returns numpy poses.  Tensors and mixed inputs take the device
-    route: device tensors in, one se3tn_track_batch / se3tn_track_render step enqueued.
+    route: CUDA tensors are used as they are, every other input is staged through one double-buffered
+    set, and one se3tn_track_batch / se3tn_track_render step is enqueued.
   * Tracker(..., fill_depth=True): on_track takes a live sensor's raw depth frame and hole-fills it
     inside the tracking step, as the reference's ROS node does with Utils.fill_depth before every
     on_track (predict_ros.py:38-41).
@@ -167,6 +168,10 @@ class Tracker:
                 renderer = None                                    # e.g. a vertices-only ply: fall through to the GL renderers
         self.renderer = renderer if renderer is not None else self._try_reference_renderer(model_path, cam_cfg)
         self._np_bufs = {}
+        self._copy_stream = torch.cuda.Stream(device=self.engine.device)      # _uploads: two staging slots, used alternately
+        self._stage_bufs = ({}, {})
+        self._stage_done = (torch.cuda.Event(), torch.cuda.Event())
+        self._stage_slot = 0
         self.prev_rgb = None
         self.prev_depth = None
         self.frame_cnt = 0
@@ -261,19 +266,15 @@ class Tracker:
         host    numpy frame and poses (ids and widths not tensors), input A numpy or drawn inside the step: one
                 Engine.track_host / track_render_host call stages the frame's crop-window rectangle, the poses and input A
                 through pinned memory and returns numpy poses (synchronous, like the reference's on_track).
-        device  everything else.  The inputs become device tensors, input A is rendered first when the step cannot draw it,
-                and one Engine.track_render / track_batch call is enqueued.
-                  CUDA tensors   are used as they are -> CUDA tensor, nothing is synchronised.
-                  CPU tensors    -> CUDA tensor; the host->device copies run on a side stream into double-buffered
-                                 staging, so the uploads of call k overlap the kernels of call k-1 (pinned memory
-                                 makes them truly asynchronous).  Nothing is synchronised.
-                  anything else  (numpy or mixed inputs): whole frames are copied into persistent device buffers; numpy
-                                 poses give a numpy result."""
+        device  everything else.  CUDA tensors are used as they are; every other input (numpy arrays, pageable or pinned
+                CPU tensors) is staged through one double-buffered set (_uploads).  Input A is rendered first when the step
+                cannot draw it, and one Engine.track_render / track_batch call is enqueued.  Tensor poses give a CUDA
+                tensor and nothing is synchronised; numpy poses give a numpy result.
+        A pageable input may be overwritten as soon as the call returns.  A pinned CPU tensor is read asynchronously: it must
+        stay unchanged until the current stream has run this call's step."""
         render = rgbA is None or depthA is None
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
-        if self.precision == 'fp8':
-            self._calibrate_fp8(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
@@ -281,47 +282,47 @@ class Tracker:
             c = lambda a, dt: a if (a.dtype == dt and a.flags['C_CONTIGUOUS']) else np.ascontiguousarray(a).astype(dt, copy=False)
             poses = np.ascontiguousarray(prev_poses, dtype=np.float64).reshape(-1, 4, 4)
             n = len(poses)
-            args = (c(current_rgb, np.uint8), c(current_depth, np.uint16), self.K, poses, self._widths(object_width, n))
-            kw = dict(weight_ids=self._weight_ids(weight_ids, n), precision=self.precision, fill_depth=self.fill_depth)
+            wh = self._weight_ids(weight_ids, n)
+            frame, ow = (c(current_rgb, np.uint8), c(current_depth, np.uint16)), self._widths(object_width, n)
+            A = () if renderer is not None else (c(rgbA, np.uint8), c(depthA, np.uint16))
+            if self._fp8_pending(wh):                 # the inputs go to the device only to calibrate
+                with self._uploads(poses, *frame, *(A or (None, None)), ow) as d:
+                    self._calibrate_fp8(weight_ids, wh, *d)
+            kw = dict(weight_ids=wh, precision=self.precision, fill_depth=self.fill_depth)
             if renderer is not None:
-                return self.engine.track_render_host(*args, self.trans_normalizer, self.rot_normalizer, mode=renderer.mode,
-                                                     image_hw=renderer.image_hw, **kw)
-            return self.engine.track_host(*args, c(rgbA, np.uint8), c(depthA, np.uint16), self.trans_normalizer, self.rot_normalizer, **kw)
+                return self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
+                                                     mode=renderer.mode, image_hw=renderer.image_hw, **kw)
+            return self.engine.track_host(*frame, self.K, poses, ow, *A, self.trans_normalizer, self.rot_normalizer, **kw)
 
         dev = self.engine.device
-        inputs = (prev_poses, current_rgb, current_depth) + ((None, None) if render else (rgbA, depthA))
-        staged = all(torch.is_tensor(x) and not x.is_cuda for x in inputs)
-        if staged:
-            poses, rgb_d, depth_d, rgbA_d, depthA_d = self._stage_uploads(*inputs)
-        else:
-            poses, rgb_d, depth_d, rgbA_d, depthA_d = map(self._to_device, inputs, ('poses', 'rgb', 'depth', 'rgbA', 'depthA'),
-                                                          (torch.float64, torch.uint8, torch.uint16, torch.uint8, torch.uint16))
-        n = poses.shape[0]
+        n = len(prev_poses)
         wh = self._weight_ids(weight_ids, n)
-        wd = None if wh is None else self._resident(('wids', wh.tobytes()), lambda: wh)
         if object_width is None:
             ow = self._resident(('ow', n), lambda: self._widths(None, n))
-        else:                                         # widths passed in are refilled in place on every call, like the frame
-            ow = self._to_device(object_width if torch.is_tensor(object_width) else self._widths(object_width, n), 'ow_arg', torch.float64)
-        if render and renderer is None:              # a renderer the step cannot stand in for draws input A first
-            rgbA_d, depthA_d = self.renderer.render_batch(poses, ow, None if weight_ids is None else wd)
-        as_numpy = not torch.is_tensor(prev_poses)
-        outs = {}
-        if as_numpy:                                  # results go back to the host: persistent output buffers keep the graph key stable too
-            ob = self._np_bufs.get(('out', n))
-            if ob is None:
-                ob = self._np_bufs[('out', n)] = (torch.empty(n, 4, 4, dtype=torch.float64, device=dev),
-                                                  torch.empty(n, 3, dtype=torch.float32, device=dev), torch.empty(n, 3, dtype=torch.float32, device=dev))
-            outs = dict(out_poses=ob[0], out_trans=ob[1], out_rot=ob[2])
-        kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
-        if renderer is not None:                      # input A is drawn inside the step, with the weight ids as mesh ids
-            out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                 mode=renderer.mode, image_hw=renderer.image_hw, **kw)
         else:
-            out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
-                                                self.trans_normalizer, self.rot_normalizer, **kw)
-        if staged:
-            self._stage_done[self._stage_slot].record(torch.cuda.current_stream(dev))
+            ow = object_width if torch.is_tensor(object_width) else self._widths(object_width, n)
+        with self._uploads(prev_poses, current_rgb, current_depth, *((None, None) if render else (rgbA, depthA)), ow) as d:
+            poses, rgb_d, depth_d, rgbA_d, depthA_d, ow = d
+            if self._fp8_pending(wh):
+                self._calibrate_fp8(weight_ids, wh, *d)
+            wd = None if wh is None else self._resident(('wids', wh.tobytes()), lambda: wh)
+            if render and renderer is None:          # a renderer the step cannot stand in for draws input A first
+                rgbA_d, depthA_d = self.renderer.render_batch(poses, ow, None if weight_ids is None else wd)
+            as_numpy = not torch.is_tensor(prev_poses)
+            outs = {}
+            if as_numpy:                              # results go back to the host: persistent output buffers keep the graph key stable too
+                ob = self._np_bufs.get(('out', n))
+                if ob is None:
+                    ob = self._np_bufs[('out', n)] = (torch.empty(n, 4, 4, dtype=torch.float64, device=dev),
+                                                      torch.empty(n, 3, dtype=torch.float32, device=dev), torch.empty(n, 3, dtype=torch.float32, device=dev))
+                outs = dict(out_poses=ob[0], out_trans=ob[1], out_rot=ob[2])
+            kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
+            if renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
+                out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
+                                                     mode=renderer.mode, image_hw=renderer.image_hw, **kw)
+            else:
+                out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
+                                                    self.trans_normalizer, self.rot_normalizer, **kw)
         return out.cpu().numpy() if as_numpy else out
 
     def _weight_ids(self, weight_ids, n):
@@ -331,30 +332,25 @@ class Tracker:
             return np.full(n, self.weight_id, dtype=np.int32) if self.weight_id != 0 else None
         return np.ascontiguousarray(weight_ids.cpu().numpy() if torch.is_tensor(weight_ids) else weight_ids, dtype=np.int32)
 
-    def _calibrate_fp8(self, prev_poses, rgb, depth, rgbA, depthA, weight_ids, object_width):
+    def _fp8_pending(self, wh):
+        """'fp8' and some weight set among the tracks' ids (wh as _weight_ids gives them) has no activation scales yet."""
+        return self.precision == 'fp8' and any(self.engine.fp8_scales(w) is None for w in set([0] if wh is None else wh.tolist()))
+
+    def _calibrate_fp8(self, weight_ids, wh, poses, rgb, depth, rgbA, depthA, ow):
         """'fp8': the weight sets of this frame's tracks that have no activation scales yet are calibrated on their tracks of
-        this frame before the step runs (Engine.calibrate_fp8_tracks): input A as given or drawn by the rasteriser, B cropped
-        at the previous pose from the frame (hole-filled as the step fills it).  Sets that have scales are left alone."""
-        n = len(prev_poses)
-        wh = self._weight_ids(weight_ids, n)
+        this frame before the step runs (Engine.calibrate_fp8_tracks), from the device inputs _uploads made: input A as given
+        or (rgbA None) drawn by the rasteriser, B cropped at the previous pose from the frame (hole-filled as the step fills
+        it).  Sets that have scales are left alone."""
+        n = poses.shape[0]
         ids = np.zeros(n, np.int32) if wh is None else wh
-        eng = self.engine
-        if all(eng.fp8_scales(w) is not None for w in set(ids.tolist())):
-            return
-        dev = eng.device
-        t = lambda x, dt: (x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x))).to(dev, dt).contiguous()
-        poses = t(prev_poses, torch.float64).reshape(-1, 4, 4)
-        ow = t(object_width if torch.is_tensor(object_width) else self._widths(object_width, n), torch.float64)
         render = None
-        if rgbA is None or depthA is None:
-            r = self.renderer
-            mesh_ids = t(ids, torch.int32) if weight_ids is not None else torch.full((n,), r.mesh_id, dtype=torch.int32, device=dev)
+        if rgbA is None:
+            r, dev = self.renderer, self.engine.device
+            mesh_ids = (torch.from_numpy(ids).to(dev) if weight_ids is not None
+                        else torch.full((n,), r.mesh_id, dtype=torch.int32, device=dev))
             render = dict(mode=r.mode, image_hw=r.image_hw, mesh_ids=mesh_ids)
-            rgbA = depthA = None
-        else:
-            rgbA, depthA = t(rgbA, torch.uint8), t(depthA, torch.uint16)
-        eng.calibrate_fp8_tracks(t(rgb, torch.uint8), t(depth, torch.uint16), self.K, poses, ow, rgbA, depthA, weight_ids=ids,
-                                 fill_depth=self.fill_depth, render=render)
+        self.engine.calibrate_fp8_tracks(rgb, depth, self.K, poses, ow, rgbA, depthA, weight_ids=ids, fill_depth=self.fill_depth,
+                                         render=render)
 
     def _widths(self, object_width, n):
         """The tracks' object widths as a float64 host array: the Tracker's object width unless given."""
@@ -368,51 +364,50 @@ class Tracker:
             t = self._np_bufs[key] = torch.from_numpy(make()).to(self.engine.device)
         return t
 
-    def _to_device(self, x, slot, dt):
-        """One input of the device route as a device tensor of dtype dt (None stays None).  A tensor is moved (a CUDA tensor
-        of that dtype is used as it is); anything else is copied whole into a persistent device buffer, one per argument and
-        shape: the step's CUDA graph is keyed by its device pointers, so stable addresses mean every frame after the first is
-        one graph launch."""
-        if x is None:
-            return None
-        if torch.is_tensor(x):
-            return x.to(self.engine.device, dt).contiguous()
-        a = np.ascontiguousarray(x)
-        if dt == torch.uint16 and a.dtype != np.uint16:
-            a = a.astype(np.uint16)
-        src = torch.from_numpy(a)
-        key = (slot, tuple(a.shape), dt)
-        buf = self._np_bufs.get(key)
-        if buf is None:
-            buf = self._np_bufs[key] = torch.empty(a.shape, dtype=dt, device=self.engine.device)
-        buf.copy_(src if src.dtype == dt else src.to(dt))
-        return buf
+    _UPLOADS = (('poses', torch.float64), ('rgb', torch.uint8), ('depth', torch.uint16), ('rgbA', torch.uint8),
+                ('depthA', torch.uint16), ('widths', torch.float64))
 
-    # ------------------------------------------------------------------ pipelined uploads
-    def _stage_uploads(self, *cpu_tensors):
-        """Copy host tensors into one of two device staging sets on a side stream."""
+    @contextlib.contextmanager
+    def _uploads(self, *inputs):
+        """The device route's inputs (poses, rgb, depth, rgbA, depthA, widths; None stays None) as device tensors, for the
+        with-block to read.  A CUDA tensor is used as it is (converted when its dtype or layout differ).  Any other input -- a
+        numpy array (depth coerced to uint16), a pageable or a pinned CPU tensor -- is copied into this call's slot of two
+        staging sets, used alternately.  A slot keeps one device buffer per argument, reallocated only when that argument's
+        shape changes: the step's CUDA graph is keyed by its device pointers, so stable addresses mean one graph launch per
+        frame.  The copies run non_blocking on the copy stream once the kernels that last read the slot are done, so the
+        uploads of call k overlap the kernels of call k-1, and the current stream waits for them.  A copy from pageable memory
+        has read its source when it returns; a pinned tensor is read asynchronously.  When the block exits, the slot's done
+        event is recorded on the current stream after every kernel the block enqueued."""
         dev = self.engine.device
-        if not hasattr(self, '_copy_stream'):
-            self._copy_stream = torch.cuda.Stream(device=dev)
-            self._stage_bufs = [None, None]
-            self._stage_done = [torch.cuda.Event(), torch.cuda.Event()]
-            self._stage_slot = 0
+        cur, cs = torch.cuda.current_stream(dev), self._copy_stream
         self._stage_slot ^= 1
-        slot = self._stage_slot
-        want = [(torch.float64, cpu_tensors[0]), (torch.uint8, cpu_tensors[1]), (torch.uint16, cpu_tensors[2]),
-                (torch.uint8, cpu_tensors[3]), (torch.uint16, cpu_tensors[4])]
-        bufs = self._stage_bufs[slot]
-        if bufs is None or any(b.shape != t.shape for b, (_, t) in zip(bufs, want)):
-            bufs = [torch.empty(t.shape, dtype=dt, device=dev) for dt, t in want]
-            self._stage_bufs[slot] = bufs
-        cs = self._copy_stream
-        cs.wait_event(self._stage_done[slot])            # the kernels that last read this staging set are done
-        with torch.cuda.stream(cs):
-            for b, (dt, t) in zip(bufs, want):
-                b.copy_(t if t.dtype == dt else t.to(dt), non_blocking=True)
-            ev = torch.cuda.Event(); ev.record(cs)
-        torch.cuda.current_stream(dev).wait_event(ev)
-        return bufs
+        bufs, done = self._stage_bufs[self._stage_slot], self._stage_done[self._stage_slot]
+        out, copies = [], []
+        for (name, dt), x in zip(self._UPLOADS, inputs):
+            if x is None or (torch.is_tensor(x) and x.is_cuda):
+                out.append(x if x is None else x.to(dev, dt).contiguous())
+                continue
+            if not torch.is_tensor(x):
+                a = np.ascontiguousarray(x)
+                x = torch.from_numpy(a.astype(np.uint16) if dt == torch.uint16 and a.dtype != np.uint16 else a)
+            src = x if x.dtype == dt else x.to(dt)
+            buf = bufs.get(name)
+            if buf is None or buf.shape != src.shape:
+                buf = bufs[name] = torch.empty(src.shape, dtype=dt, device=dev)
+                cs.wait_stream(cur)                  # a new buffer may reuse memory that kernels queued on cur still use
+            copies.append((buf, src))
+            out.append(buf)
+        if copies:
+            cs.wait_event(done)                      # the kernels that last read this slot are done
+            with torch.cuda.stream(cs):
+                for buf, src in copies:
+                    buf.copy_(src, non_blocking=True)
+            cur.wait_stream(cs)
+        try:
+            yield out
+        finally:
+            if copies:
+                done.record(cur)
 
 
 # ====================================================================================================
