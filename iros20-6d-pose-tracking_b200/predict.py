@@ -99,6 +99,11 @@ def _ply_vertices(model_path):
         return np.stack([data['x'], data['y'], data['z']], 1).astype(np.float64)
 
 
+def object_cloud(model_path):
+    """Tracker.object_cloud of a mesh file: its vertices down-sampled on a 5 mm voxel grid (reference predict.py:131-133)."""
+    return PointCloud(load_vertices(model_path)).voxel_down_sample(voxel_size=0.005)
+
+
 def compute_obj_max_width(points):
     """Convex-hull diameter in mm (reference Utils.py:101-105, 450-451)."""
     from scipy.spatial import ConvexHull, distance_matrix
@@ -125,7 +130,7 @@ class Tracker:
             raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
         self.object_cloud = None
         if model_path is not None:
-            self.object_cloud = PointCloud(load_vertices(model_path)).voxel_down_sample(voxel_size=0.005)
+            self.object_cloud = object_cloud(model_path)
         if 'object_width' not in dataset_info:
             if self.object_cloud is None:
                 raise ValueError("need model_path or dataset_info['object_width']")
@@ -795,6 +800,36 @@ def _class_normalizer(class_config, key, class_id, default):
 # The modes the one-pass YCB-Video driver offers: every mode but 'fp16', which its callers have treated as an unknown name
 # since before the mode existed.  The YCBInEOAT driver, the Tracker and the Engine take every mode of engine.PREC.
 YCB_ALL_PRECISIONS = ('bf16x3', 'tf32', 'bf16', 'fp8', 'fp32')
+# Every mode of engine.PREC, in the order a sweep of the YCBInEOAT driver lists them.
+PRECISIONS = ('bf16x3', 'tf32', 'bf16', 'fp16', 'fp8', 'fp32')
+
+
+def precision_modes(precision, modes):
+    """The modes a one-pass driver tracks in -> (modes tuple, sweep).  A single mode name gives ((name,), False) and is checked
+    where it always was; 'all' gives (modes, True); a sequence of names gives (those names, True).  In a sweep, a name not in
+    `modes`, a name listed twice and an empty sequence are a ValueError."""
+    if isinstance(precision, str) and precision != 'all':
+        return (precision,), False
+    got = tuple(modes) if isinstance(precision, str) else tuple(precision)
+    if not got:
+        raise ValueError('no precision mode given')
+    for m in got:
+        if m not in modes:
+            raise ValueError('precision %r is not a mode of this driver (one of %s)' % (m, ', '.join(modes)))
+    twice = sorted(set(m for m in got if got.count(m) > 1))
+    if twice:
+        raise ValueError('precision %s listed more than once' % ', '.join(twice))
+    return got, True
+
+
+def sweep_reference(modes):
+    """The mode a sweep's drift is measured from: 'fp32' if swept, else 'bf16x3' if swept, else the first mode listed."""
+    return 'fp32' if 'fp32' in modes else 'bf16x3' if 'bf16x3' in modes else modes[0]
+
+
+def precision_outdir(outdir, mode):
+    """Where a sweep writes mode `mode`'s output tree: <outdir>/<mode>/, what a single-mode run with that outdir writes."""
+    return os.path.join(outdir, mode)
 
 
 def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
@@ -855,21 +890,28 @@ def _one_pass_trackers(entries, precision, max_batch):
     return eng, trackers
 
 
-def _track_sequences(eng, trackers, sequences, precision, depth, workers, video=None):
+def _track_sequences(eng, trackers, sequences, precisions, depth, workers, video=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
-    files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode.
-    Yields each sequence's (frames, n, 4, 4) numpy poses, the poses after each frame, as soon as the sequence ends.
+    files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
+    precisions: the modes (a tuple) every frame is tracked in.  Yields each sequence's {mode: (frames, n, 4, 4) numpy poses}, the
+    poses after each frame, as soon as the sequence ends.
 
-    Every frame is one se3tn_track_render step for the sequence's n tracks.  The frames of all sequences decode ahead, across
-    sequence boundaries, through one StagingRing of `depth` sets (`workers` threads) into its one device frame.  The step's other
-    device arguments are kept: the ids and widths per distinct weight-id tuple, and per n the pose tensor every step updates in
-    place and the step's outputs.  So every step after a track set's first replays the step's CUDA graph, across sequences too.
-    After each step the poses are copied into a device history, which comes back to the host once per sequence.
+    Every frame is one se3tn_track_render step per mode for the sequence's n tracks, all reading the same device frame: the
+    frames of all sequences decode ahead, across sequence boundaries, through one StagingRing of `depth` sets (`workers` threads)
+    into its one device frame, so a frame is decoded once whatever the number of modes.  The steps' other device arguments are
+    kept: the ids and widths per distinct weight-id tuple, and per (mode, n) the pose tensor that mode's steps update in place and
+    their outputs.  So in each mode every step after a track set's first replays that mode's CUDA graph, across sequences too
+    ('fp32' steps are never captured).  With 'fp8' among the modes, each weight set is calibrated on the first frame of the first
+    sequence that tracks it, before that frame's steps.  After each step the mode's poses are copied into its device history,
+    which comes back to the host once per sequence.
 
     video: None, or (label order, [(paths, labels)] per sequence): paths holds one mp4 path per track, labels one text per frame.
     Then each frame's decode jobs also render its label strip into the ring, and after each step Engine.draw_tracks draws every
     track's Tracker.object_cloud points at its new pose over the device frame (the point sets uploaded once, as one table), and a
-    VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed."""
+    VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed.
+    Videos are drawn for one mode only."""
+    if video is not None and len(precisions) != 1:
+        raise ValueError('result videos are drawn for one precision mode, not %d' % len(precisions))
     if not sequences:
         return
     dev = eng.device
@@ -902,36 +944,44 @@ def _track_sequences(eng, trackers, sequences, precision, depth, workers, video=
                 wh = np.asarray(ids, dtype=np.int32)
                 by_ids[ids] = (wh, torch.from_numpy(wh).to(dev),
                                torch.tensor([trackers[w].object_width for w in ids], dtype=torch.float64, device=dev))
-            if n not in by_n:
-                by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
-                           torch.empty((n, 3), dtype=torch.float32, device=dev),
-                           None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
+            for m in precisions:
+                if (m, n) not in by_n:
+                    by_n[m, n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
+                                  torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
+                                  None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
+                by_n[m, n][0].copy_(torch.from_numpy(init))
             wh, wd, widths = by_ids[ids]
-            poses, out_trans, out_rot, drawn = by_n[n]
-            poses.copy_(torch.from_numpy(init))
-            history = torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev)
+            history = {m: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for m in precisions}
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
-                if precision == 'fp8' and t == 0:      # each set is calibrated on the first frame of the first sequence that tracks it
-                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, weight_ids=wh,
+                if 'fp8' in precisions and t == 0:     # each set is calibrated on the first frame of the first sequence that tracks it
+                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n['fp8', n][0], widths, weight_ids=wh,
                                              render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
-                eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
-                                 weight_ids_host=wh, weight_ids_dev=wd, precision=precision, mode=trk.renderer.mode,
-                                 image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
-                history[t].copy_(poses)
+                for m in precisions:
+                    poses, out_trans, out_rot, drawn = by_n[m, n]
+                    eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
+                                     weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
+                                     image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
+                    history[m][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
                                     label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
                     sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
-            yield history.cpu().numpy()
+            yield {m: h.cpu().numpy() for m, h in history.items()}
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
                      video=False):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
+
+    precision: one mode of YCB_ALL_PRECISIONS, or a sweep: a sequence of them or 'all' (all five).  'fp16' is refused here, alone
+    or in a sequence, while getResultsYcbInEOAT takes it.  A sweep tracks every frame in every mode (one step per mode, each frame
+    decoded once, every weight set loaded once) and returns {mode: what a run in that mode returns}; mode m writes its tree under
+    <outdir>/<m>/, file for file what a run in mode m with that outdir writes.  score_precisions scores it.  Unknown or repeated
+    modes, an empty sequence, and video=True with more than one mode are a ValueError before anything is loaded.
 
     One Engine holds every class's weights, statistics and CUDA-renderer mesh under weight id = class id.  For each test sequence,
     the tracks are its requested classes in ascending order, each started as getResultsYcb starts it, and every frame after the
@@ -940,9 +990,12 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     video: also write the result video a per-class run writes next to its seq<id>/ (predict.py:403, 424-435): <outdir>/<class
     folder>/run/seq<id>.mp4, one half-size frame per tracked frame (none for the start pose), the class's model points drawn at
     their tracked pose over the frame, under the label 'frame:<i+1>' of frame i.  The drawing runs on the device."""
+    modes, sweep = precision_modes(precision, YCB_ALL_PRECISIONS)
+    if video and len(modes) > 1:
+        raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
-    classes = ycb_all_classes(ycb_dir, class_ids, class_config, precision)
+    classes = ycb_all_classes(ycb_dir, class_ids, class_config, modes[0])
     track_sets = ycb_track_sets(ycb_dir, [k['class_id'] for k in classes])
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
@@ -954,26 +1007,28 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
         init = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
                                          sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]).astype(np.float64)
         sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
-    eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], precision,
+    eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], modes[0],
                                        max([len(v) for v in track_sets.values()] + [1]))
     name_of = {k['class_id']: k['name'] for k in classes}
+    root = {m: precision_outdir(outdir, m) if sweep else outdir for m in modes}
     drawn = None
     if video:
-        drawn = ('under', [([os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
+        drawn = ('under', [([os.path.join(ycb_all_res_dir(root[modes[0]], name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)])
         for c in name_of.values():
-            os.makedirs(ycb_all_res_dir(outdir, c), exist_ok=True)
-    results = {k['class_id']: {} for k in classes}
-    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, precision, 2, 2, drawn),
+            os.makedirs(ycb_all_res_dir(root[modes[0]], c), exist_ok=True)
+    results = {m: {k['class_id']: {} for k in classes} for m in modes}
+    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, modes, 2, 2, drawn),
                                                        track_sets.items(), sequences):
-        pred_poses = np.concatenate([init[None], tracked])           # row 0: the start pose, as in getResultsYcb
-        for j, c in enumerate(cls):
-            sdir = os.path.join(ycb_all_res_dir(outdir, name_of[c]), 'seq{}'.format(seq_id))
-            os.makedirs(sdir, exist_ok=True)
-            for i in range(len(pred_poses)):
-                np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
-            results[c][seq_id] = pred_poses[:, j]
-    return results
+        for m in modes:
+            pred_poses = np.concatenate([init[None], tracked[m]])    # row 0: the start pose, as in getResultsYcb
+            for j, c in enumerate(cls):
+                sdir = os.path.join(ycb_all_res_dir(root[m], name_of[c]), 'seq{}'.format(seq_id))
+                os.makedirs(sdir, exist_ok=True)
+                for i in range(len(pred_poses)):
+                    np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
+                results[m][c][seq_id] = pred_poses[:, j]
+    return results if sweep else results[modes[0]]
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1055,33 +1110,115 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     video: also write <outdir>/<video>.mp4, a headless stand-in for the window predictSequenceYcbInEOAT shows (predict.py:612-624;
     the reference itself writes no file there): per frame i, the object's model points drawn at the tracked pose over the frame
     with the label 'frame:<i>' over them, at half size.  The drawing runs on the device.  eval_ycbineoat lists the .mp4 files
-    among the result folders and finds no pose file in them, so the scores are unchanged."""
+    among the result folders and finds no pose file in them, so the scores are unchanged.
+
+    precision: one mode of engine.PREC, or a sweep: a sequence of them or 'all' (all six, PRECISIONS).  Unlike getResultsYcbAll,
+    which refuses 'fp16', every mode is taken here.  A sweep tracks every frame in every mode (one step per mode, each frame
+    decoded once, every weight set loaded once) and returns {mode: what a run in that mode returns}; mode m writes its tree under
+    <outdir>/<m>/, file for file what a run in mode m with that outdir writes.  score_precisions scores it.  Unknown or repeated
+    modes, an empty sequence, and video=True with more than one mode are a ValueError before anything is loaded."""
     from .eval_ycbineoat import OBJECTS
+    modes, sweep = precision_modes(precision, PRECISIONS)
+    if video and len(modes) > 1:
+        raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
     videos = ycbineoat_videos(ycbineoat_dir)
     files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
-    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, precision)
+    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, modes[0])
     eng, trackers = _one_pass_trackers([(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER,
                                                                                  rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
-                                        for o, k in objects.items()], precision, 1)
+                                        for o, k in objects.items()], modes[0], 1)
     sequences = {}
     for v, obj in videos:
         rgb_files, depth_files, gt_files = files[v]
         nf = len(rgb_files) if max_frames is None else min(max_frames, len(rgb_files))
         if nf > 0:
             sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
+    root = {m: precision_outdir(outdir, m) if sweep else outdir for m in modes}
     drawn = None
     if video:
-        os.makedirs(outdir, exist_ok=True)
-        drawn = ('over', [([os.path.join(outdir, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()])
-    results = {}
-    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), precision, decode_ahead, 2 * decode_ahead, drawn),
+        os.makedirs(root[modes[0]], exist_ok=True)
+        drawn = ('over', [([os.path.join(root[modes[0]], v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))])
+                          for v, s in sequences.items()])
+    results = {m: {} for m in modes}
+    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), modes, decode_ahead, 2 * decode_ahead, drawn),
                           sequences):
-        results[v] = tracked[:, 0]
-        write_video_poses(outdir, v, results[v])
-    return results
+        for m in modes:
+            results[m][v] = tracked[m][:, 0]
+            write_video_poses(root[m], v, results[m][v])
+    return results if sweep else results[modes[0]]
+
+
+def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
+    """What each mode of a precision sweep scores, and how far it drifts from the reference mode.  results: what getResultsYcbAll
+    (YCBInEOAT_dir None) or getResultsYcbInEOAT returned for a sweep, {mode: ...}; outdir, ycb_dir and config (the path
+    templates) those of the run.  -> (reference mode, {mode: {'add', 'adds', 'add_max', 'add_mean', 'adds_max', 'adds_mean'}}).
+
+    add / adds: the ADD and ADD-S AUCs (percent) of the mode's tree <outdir>/<mode>/ from the existing scorers, whose lines are
+    printed under a 'precision <mode>' header: eval_ycbineoat.eval_all; for YCB-Video eval_ycb.eval_all when all 21 classes were
+    tracked, else eval_ycb.eval_one_class per class, with the errors of all classes pooled through eval_ycb.VOCap.
+    add_* / adds_*: ADD and ADD-S between every pose the mode returned and the reference mode's pose of the same track and frame,
+    max and mean in mm, on each class's or object's Tracker.object_cloud points; one add_adi_sets launch per mode.  No ground
+    truth is involved, so it also shows where modes part ways on frames without annotations.  The reference is
+    sweep_reference(modes), whose own row is 0."""
+    import argparse
+    from .eval_ycbineoat import eval_all, video_object
+    modes = list(results)
+    ref = sweep_reference(modes)
+    if YCBInEOAT_dir is None:
+        names = ycb_class_names(ycb_dir)
+        keys = [(c, s) for c in sorted(results[ref]) for s in sorted(results[ref][c])]
+        poses_of = lambda m, key: results[m][key[0]][key[1]]
+        model_of = {key: expand_class_paths(config, key[0], names[key[0] - 1])['model_path'] for key in keys}
+    else:
+        keys = sorted(results[ref])
+        poses_of = lambda m, key: results[m][key]
+        model_of = {v: expand_object_paths(config, video_object(v), ycbineoat_class_name(ycb_dir, video_object(v)) if ycb_dir else None)
+                    ['model_path'] for v in keys}
+    paths = sorted(set(model_of.values()))
+    clouds = [object_cloud(p).points for p in paths]
+    pose_set = np.concatenate([np.full(len(poses_of(ref, k)), paths.index(model_of[k]), dtype=np.int32) for k in keys])
+    eng = U._eng()
+    stacked = lambda m: torch.from_numpy(np.ascontiguousarray(np.concatenate([poses_of(m, k) for k in keys]).reshape(-1, 4, 4),
+                                                              dtype=np.float64)).to(eng.device)
+    ref_poses = stacked(ref)
+    rows = {}
+    for m in modes:
+        print('precision %s' % m)
+        root = precision_outdir(outdir, m)
+        if YCBInEOAT_dir is None:
+            adds, add = _score_ycb_tree(ycb_dir, root, sorted(results[m]))
+        else:
+            _, adds, add, _ = eval_all(argparse.Namespace(YCBInEOAT_dir=YCBInEOAT_dir, ycb_dir=ycb_dir, res_dir=root + '/'))
+        d_add, d_adds = (d.cpu().numpy() * 1000 for d in eng.add_adi_sets(clouds, pose_set, stacked(m), ref_poses))
+        rows[m] = dict(add=add, adds=adds, add_max=float(d_add.max()), add_mean=float(d_add.mean()),
+                       adds_max=float(d_adds.max()), adds_mean=float(d_adds.mean()))
+    return ref, rows
+
+
+def _score_ycb_tree(ycb_dir, root, class_ids):
+    """eval_ycb's lines for a getResultsYcbAll tree under root -> (ADD-S AUC, ADD AUC) in percent: eval_all when the tree holds
+    all 21 classes (it pools exactly those), else eval_one_class per class, the errors of all of them pooled through VOCap."""
+    import argparse
+    from . import eval_ycb
+    names = ycb_class_names(ycb_dir)
+    if list(class_ids) == list(range(1, 22)) and len(names) == 21:
+        adi_auc, add_auc, _ = eval_ycb.eval_all(argparse.Namespace(ycb_dir=ycb_dir, res_root=root))
+        return adi_auc, add_auc
+    errs = [eval_ycb.eval_one_class(argparse.Namespace(ycb_dir=ycb_dir, class_id=c, res_dir=ycb_all_res_dir(root, names[c - 1]) + '/'))
+            for c in class_ids]
+    return (eval_ycb.VOCap(np.concatenate([e[0] for e in errs])) * 100, eval_ycb.VOCap(np.concatenate([e[1] for e in errs])) * 100)
+
+
+def print_precision_table(ref, rows):
+    """The table --score prints after a sweep's per-mode scores: one row per mode of score_precisions' result."""
+    print('precision sweep: AUCs in percent; drift from %s in mm (ADD / ADD-S to its pose of the same track and frame)' % ref)
+    print('%-8s %9s %9s %11s %11s %11s %11s' % ('mode', 'ADD', 'ADD-S', 'ADD max', 'ADD mean', 'ADD-S max', 'ADD-S mean'))
+    for m, r in rows.items():
+        print('%-8s %9.4f %9.4f %11.4g %11.4g %11.4g %11.4g' % (m, r['add'], r['adds'], r['add_max'], r['add_mean'], r['adds_max'],
+                                                               r['adds_mean']))
 
 
 def main(argv=None):
@@ -1108,17 +1245,22 @@ def main(argv=None):
     parser.add_argument('--decode_ahead', type=int, default=4, help='ycbineoat_all: frames decoded ahead of the tracking step')
     parser.add_argument('--video', action='store_true', help='ycbv_all / ycbineoat_all: also write the result videos, each track\'s '
                         'model points drawn over its frames on the device (<class folder>/run/seq<id>.mp4 / <video>.mp4)')
+    parser.add_argument('--precision', default=None, help='MODE|all|MODE,MODE,...: the precision mode (default bf16x3).  ycbv_all / '
+                        'ycbineoat_all also take a comma-separated list of modes or all: every frame is tracked in each mode, mode m '
+                        'written under <outdir>/<m>/, and --score prints each mode\'s scores and a table of their AUCs and drift')
     args = parser.parse_args(argv)
+    precision = cli_precision(args.precision, args.mode)
     if args.mode == 'ycbv_all':
-        return _main_ycbv_all(args)
+        return _main_ycbv_all(args, precision)
     if args.mode == 'ycbineoat_all':
-        return _main_ycbineoat_all(args)
+        return _main_ycbineoat_all(args, precision)
+    prec_kw = {} if precision is None else {'precision': precision}
     dataset_info, images_mean, images_std = load_run_config(args.train_data_path, args.mean_std_path)
     if args.mode == 'ycbineoat':
         if not args.YCBInEOAT_dir:
             raise SystemExit('--mode ycbineoat needs --YCBInEOAT_dir')
         poses = predictSequenceYcbInEOAT(args.YCBInEOAT_dir, dataset_info, images_mean, images_std, args.ckpt_dir, args.model_path,
-                                         args.outdir, max_frames=args.max_frames)
+                                         args.outdir, max_frames=args.max_frames, **prec_kw)
         print('wrote %d poses to %s' % (len(poses), args.outdir))
         return
     if not args.ycb_dir:
@@ -1129,12 +1271,33 @@ def main(argv=None):
         class_id = args.class_id if args.class_id is not None and args.class_id >= 0 else 4      # predict.py:450-452
         reinit = args.reinit_frames.split(',') if args.reinit_frames else None
         poses, auc = predictSequenceYcb(args.ycb_dir, args.seq_id, class_id, dataset_info, images_mean, images_std, args.ckpt_dir,
-                                        args.model_path, args.outdir, init=args.init, reinit_frames=reinit, max_frames=args.max_frames)
+                                        args.model_path, args.outdir, init=args.init, reinit_frames=reinit, max_frames=args.max_frames,
+                                        **prec_kw)
         print('reinit_frames {}, adi_auc {}'.format(reinit or '', auc))
         return
     res = getResultsYcb(args.ycb_dir, args.class_id, dataset_info, images_mean, images_std, args.ckpt_dir, args.model_path, args.outdir,
-                        initialize_method=args.init, max_frames=args.max_frames)
+                        initialize_method=args.init, max_frames=args.max_frames, **prec_kw)
     print('tracked class %d through sequences %s -> %s' % (args.class_id, sorted(res), args.outdir))
+
+
+def cli_precision(text, mode):
+    """--precision of `mode` -> None (not given: the drivers' default, bf16x3), a mode name, or for ycbv_all / ycbineoat_all a
+    list of names or 'all' (a sweep).  A name that is no mode, and a list or 'all' with any other mode, are a SystemExit; so is a
+    sweep its driver refuses (unknown or repeated modes, an empty list, 'fp16' with ycbv_all)."""
+    if text is None:
+        return None
+    if text != 'all' and ',' not in text:
+        if text not in PRECISIONS:
+            raise SystemExit('--precision %s: not a precision mode (one of %s)' % (text, ', '.join(PRECISIONS)))
+        return text
+    if mode not in ('ycbv_all', 'ycbineoat_all'):
+        raise SystemExit('--precision %s: a list of modes or all needs --mode ycbv_all or ycbineoat_all' % text)
+    precision = 'all' if text == 'all' else [m.strip() for m in text.split(',')]
+    try:
+        precision_modes(precision, YCB_ALL_PRECISIONS if mode == 'ycbv_all' else PRECISIONS)
+    except ValueError as e:
+        raise SystemExit('--precision %s: %s' % (text, e))
+    return precision
 
 
 def _video_kw(args):
@@ -1142,9 +1305,8 @@ def _video_kw(args):
     return {'video': True} if args.video else {}
 
 
-def _main_ycbv_all(args):
+def _main_ycbv_all(args, precision=None):
     """--mode ycbv_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class path templates."""
-    import argparse
     if not args.ycb_dir or not args.class_ids:
         raise SystemExit('--mode ycbv_all needs --ycb_dir and --class_ids')
     n_classes = len(ycb_class_names(args.ycb_dir))
@@ -1156,24 +1318,21 @@ def _main_ycbv_all(args):
         except ValueError:
             raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames,
-                           **_video_kw(args))
-    for c in sorted(res):
-        print('tracked class %d through sequences %s' % (c, sorted(res[c])))
+    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
+    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
+    sweep = precision is not None and precision_modes(precision, YCB_ALL_PRECISIONS)[1]
+    one = next(iter(res.values()), {}) if sweep else res
+    for c in sorted(one):
+        print('tracked class %d through sequences %s' % (c, sorted(one[c])))
     print('-> %s' % args.outdir)
-    if args.score:
-        from . import eval_ycb
-        names = ycb_class_names(args.ycb_dir)
-        if class_ids == list(range(1, 22)) and n_classes == 21:
-            eval_ycb.eval_all(argparse.Namespace(ycb_dir=args.ycb_dir, res_root=args.outdir))
-        else:                                                       # eval_all pools exactly the 21 classes: score each one
-            for c in class_ids:
-                eval_ycb.eval_one_class(argparse.Namespace(ycb_dir=args.ycb_dir, class_id=c,
-                                                           res_dir=ycb_all_res_dir(args.outdir, names[c - 1]) + '/'))
+    if args.score and sweep:
+        print_precision_table(*score_precisions(res, args.outdir, args.ycb_dir, config))
+    elif args.score:
+        _score_ycb_tree(args.ycb_dir, args.outdir, class_ids)
     return res
 
 
-def _main_ycbineoat_all(args):
+def _main_ycbineoat_all(args, precision=None):
     """--mode ycbineoat_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-object path templates."""
     import argparse
     if not args.YCBInEOAT_dir:
@@ -1181,12 +1340,17 @@ def _main_ycbineoat_all(args):
     if args.score and not args.ycb_dir:
         raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
+    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
     res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
-                              ycb_dir=args.ycb_dir, **_video_kw(args))
-    for v in res:
-        print('tracked %s: %d frames' % (v, len(res[v])))
+                              ycb_dir=args.ycb_dir, **kw)
+    sweep = precision is not None and precision_modes(precision, PRECISIONS)[1]
+    one = next(iter(res.values()), {}) if sweep else res
+    for v in one:
+        print('tracked %s: %d frames' % (v, len(one[v])))
     print('-> %s' % args.outdir)
-    if args.score:
+    if args.score and sweep:
+        print_precision_table(*score_precisions(res, args.outdir.rstrip('/'), args.ycb_dir, config, YCBInEOAT_dir=args.YCBInEOAT_dir))
+    elif args.score:
         from . import eval_ycbineoat
         eval_ycbineoat.eval_all(argparse.Namespace(YCBInEOAT_dir=args.YCBInEOAT_dir, ycb_dir=args.ycb_dir, res_dir=args.outdir.rstrip('/') + '/'))
     return res
