@@ -322,6 +322,24 @@ int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, 
  * sets the mode it wants before each track call. */
 int se3tn_set_depth_fill(se3tn_ctx* ctx, int enable, double max_depth, int extrapolate, int blur_type);
 
+/* Refine every track k times per frame inside each following se3tn_track_render / se3tn_track_render_host step on this
+ * context: the step is then exactly k successive single-round steps on the same frame (Tracker.on_track called k times,
+ * each from the pose the previous call returned), in one call and one CUDA graph.  One step is the optional depth fill
+ * (once per step, not per round), then k rounds of render (2 launches) -> K0 -> the 14 conv launches -> head / K6, each round
+ * drawing input A and cropping B at the pose the round before wrote.  Round 0 reads poses_in; every later round reads and
+ * writes poses_out in place, so poses_out == poses_in keeps working and the step's graph is replayed frame after frame.
+ * out_trans / out_rot hold the last round's network outputs; se3tn_last_launch_count counts fill + k x the launches of one
+ * round; profiling slots time the last round.  SE3TN_PREC_FP32 runs the rounds as plain launches.  k is part of what makes
+ * two steps the same (se3tn_last_step_was_graph).  k = 1 (the default) is the single-round step.  The host variant uploads the
+ * whole frame when k > 1 instead of the crop-window rectangle of the previous poses, since later rounds crop where the step
+ * moved the tracks.  se3tn_track_batch and se3tn_track_host take input A from the caller and cannot redraw it: with k > 1
+ * they return SE3TN_ERR_STATE and queue nothing.  k outside [1, SE3TN_MAX_REFINE_ITERATIONS] is SE3TN_ERR_INVALID and the
+ * setting is unchanged.  A context is single-threaded: a caller that shares one between trackers sets the k it wants before
+ * each track call.  Whether more rounds improve accuracy depends on the checkpoint; it has not been measured on trained
+ * weights. */
+#define SE3TN_MAX_REFINE_ITERATIONS 8
+int se3tn_set_refine_iterations(se3tn_ctx* ctx, int k);
+
 /* The reference's own calling pattern as ONE call (Tracker.on_track, predict.py:217-296: numpy arrays in, numpy pose out):
  * every pointer is HOST memory.  The frame's crop-window rectangle, the poses, widths, input A and the ids are staged
  * through context-owned pinned memory into context-owned device buffers (stable addresses, so the step's CUDA graph is
@@ -344,7 +362,8 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
  * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph (se3tn_last_step_was_graph);
  * SE3TN_PREC_FP32 renders and then runs its FFMA forwards without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
  * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
- * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch. */
+ * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch.  With
+ * se3tn_set_refine_iterations(k > 1) the step refines every track k times on this frame. */
 int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                        const double* K, const double* poses_in, const double* object_width,
                        int render_mode, int render_H, int render_W,
@@ -484,7 +503,8 @@ int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
  * graph the first time they see it and replay it afterwards -- one graph launch per step.  Two calls are the same step when
  * every value their kernels are given is the same: tracking or validation, n, precision, the frame's H and W, K, the two
  * normalizers, the first weight id and whether the ids use more than one set, the render mode and camera image size, the
- * depth-fill setting (se3tn_set_depth_fill), and the address of every device array, in or out.  A replay reads what those
+ * depth-fill setting (se3tn_set_depth_fill), the refinement count of a step that renders input A (se3tn_set_refine_iterations),
+ * and the address of every device array, in or out.  A replay reads what those
  * arrays hold at the time, and a call's host ids only decide the first id and the mix.  SE3TN_GRAPH=0 in the environment,
  * an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.
  * se3tn_perturb_pairs steps are captured and keyed the same way.

@@ -14,6 +14,7 @@ WEIGHT_BLOB_FLOATS = 13528326
 PROFILE_SLOTS = 22
 TRACE_TILES = 5184
 PAIR_MIN_SEG = 100
+MAX_REFINE_ITERATIONS = 8
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -49,6 +50,7 @@ SIGNATURES = {
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
     'se3tn_set_depth_fill': (_i, [_vp, _i, _d, _i, _i]),
+    'se3tn_set_refine_iterations': (_i, [_vp, _i]),
     'se3tn_set_mesh': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i]),
     'se3tn_render': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),

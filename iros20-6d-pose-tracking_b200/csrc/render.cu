@@ -336,7 +336,10 @@ render_project_kernel(RenderArgs a)
     __shared__ Uniforms u;
     ptx::grid_dep_launch();
     const int n = blockIdx.y;
-    ptx::grid_dep_wait();                                    // poses come from the previous step's pose update
+    // poses come from the previous step's pose update, or in a refinement round from the previous round's head, which this
+    // launch may start under: every read of them, and every write of `projected` / `uniforms` (which the previous round's
+    // render_kernel read), stays behind this wait
+    ptx::grid_dep_wait();
     int mid = a.mesh_ids ? a.mesh_ids[n] : 0;
     if (mid < 0 || mid >= a.n_meshes) mid = 0;
     const MeshDev m = a.meshes[mid];

@@ -201,7 +201,8 @@ enum : uint8_t { kStepTrack = 0, kStepEval = 1, kStepPairs = 2 };   // StepKey::
 struct StepKey {
     uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
     uint8_t fill, fill_extrapolate;            // c->depth_fill when a track step is built (zero in a validation step)
-    int32_t fill_blur, n, precision, first_wid;      // first_wid: the first track's weight set
+    uint16_t fill_blur, iterations;            // iterations: c->refine_iterations in a track step (zero in a validation step)
+    int32_t n, precision, first_wid;           // first_wid: the first track's weight set
     int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
     F64Bits K[4], tn, rn, fill_max_depth;
     const uint8_t* frame_rgb; const uint16_t* frame_depth; const double* object_width;   // track step
@@ -240,6 +241,7 @@ struct se3tn_ctx {
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
     // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
     struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
+    int refine_iterations = 1;       // se3tn_set_refine_iterations: render -> network -> pose update rounds of a track step that renders input A
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -1162,8 +1164,16 @@ Step track_step(const se3tn_ctx* c, int H, int W, const double* K, const int32_t
     st.wid_host = wid_host; st.first_wid = wid_host ? wid_host[0] : 0; st.mixed = mixed;
     st.render_mode = -1;
     const auto& f = c->depth_fill;                 // all zero when the fill is off (se3tn_set_depth_fill)
-    st.fill = f.on; st.fill_max_depth = f.max_depth; st.fill_extrapolate = f.extrapolate != 0; st.fill_blur = f.blur_type;
+    st.fill = f.on; st.fill_max_depth = f.max_depth; st.fill_extrapolate = f.extrapolate != 0; st.fill_blur = static_cast<uint16_t>(f.blur_type);
+    st.iterations = static_cast<uint16_t>(c->refine_iterations);
     return st;
+}
+
+// se3tn_track_batch / se3tn_track_host take input A from the caller: a later round could not redraw it at the refined pose.
+int check_single_round(se3tn_ctx* c, const char* fn) {
+    if (c->refine_iterations == 1) return SE3TN_OK;
+    return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": input A from the caller cannot be redrawn; refine iterations is " +
+                std::to_string(c->refine_iterations) + " (se3tn_set_refine_iterations), which needs se3tn_track_render[_host]");
 }
 
 // A track step that draws input A first.  It lands in context scratch for max_batch tracks, allocated by the first such step:
@@ -1194,7 +1204,10 @@ int run_tracks(se3tn_ctx* c, const Step& st, const HeadArgs& head, cudaStream_t 
 
 // The launches of one step on stream s, captured or not: render (if set) -> fill (if on) -> preprocess (track) or normalize
 // (validation) -> conv stack -> the fp32 pose update (track) or the loss (validation: pair_loss in fp32, the reduction of the
-// head's terms otherwise).  Arguments come from `st` alone, context state only as the graph cache's comment in se3tn_ctx lists.
+// head's terms otherwise).  A track step that renders input A repeats render -> preprocess -> conv stack -> pose update
+// st.iterations times on the same (filled) frame: round 0 reads poses_in, every later round reads and writes poses_out in place,
+// exactly as a chain of single-round steps would.  Arguments come from `st` alone, context state only as the graph cache's
+// comment in se3tn_ctx lists.
 int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     c->launches = 0;
     const double K[4] = {st.K[0], st.K[1], st.K[2], st.K[3]};
@@ -1232,30 +1245,45 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     // that launch has completed and its writes are visible: keep every read of input A and of the frame behind that wait.
     // The fill kernels themselves are plain launches, so the first one starts after the render has completed.
     PreprocessArgs a{};
-    a.poses = st.poses_in; a.rgbA = st.rgbA; a.depthA = st.depthA; a.weight_ids = st.wid_dev; a.precision = st.precision;
+    a.rgbA = st.rgbA; a.depthA = st.depthA; a.weight_ids = st.wid_dev; a.precision = st.precision;
     HeadArgs head;
     if (st.kind == kStepTrack) {
         a.frame_rgb = st.frame_rgb; a.frame_depth = depth; a.H = st.H; a.W = st.W; a.object_width = st.object_width;
         a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
-        head.pose_in = st.poses_in; head.pose_out = st.poses_out;
+        head.pose_out = st.poses_out;
         head.tn = static_cast<float>(st.tn); head.rn = static_cast<float>(st.rn);
     } else {                                       // both depths are offset by A's z (reference datasets.py:136 -> data_augmentation.py:134-144)
         a.frame_rgb = st.rgbB; a.frame_depth = st.depthB; a.H = kImg; a.W = kImg; a.b_precropped = 1;
         head.loss.poses_a = st.poses_in; head.loss.poses_b = st.B_in_cam; head.loss.tn = st.tn; head.loss.rn = st.rn;
         head.loss.sq = st.sq; head.loss.labels = st.labels;
     }
-    if ((rc = queue_preprocess(c, a, st.n, s))) return rc;
-    if ((rc = run_tracks(c, st, head, s))) return rc;
-    if (st.kind == kStepTrack) {
-        if (!fp32) return SE3TN_OK;                // the head kernel has updated the poses
-        ProfScope ps(c, 18, s);
-        CU_TRY(c, launch_pose_update(st.poses_in, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
-    } else {
-        ProfScope ps(c, 21, s);
-        if (fp32) CU_TRY(c, launch_pair_loss(st.out_trans, st.out_rot, nullptr, nullptr, head.loss, st.n, st.sums, s));
-        else CU_TRY(c, launch_loss_reduce(st.sq, st.n, st.sums, s));
+    const int rounds = st.kind == kStepTrack && st.render_mode >= 0 ? st.iterations : 1;
+    for (int round = 0; round < rounds; ++round) {
+        const double* poses = round == 0 ? st.poses_in : st.poses_out;
+        if (round > 0) {
+            // render_project_kernel (PDL) may start under the previous round's head / pose-update kernel, which writes these
+            // poses; it reads them, and writes the projected vertices the previous round's render_kernel read, only after its
+            // griddepcontrol.wait, which returns once that kernel -- and so, through each kernel's own wait, every earlier
+            // launch of the step -- has completed.
+            rc = queue_render(c, K, poses, st.object_width, st.wid_dev, st.n, st.render_mode, st.render_H, st.render_W,
+                              const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s);
+            if (rc) return rc;
+        }
+        a.poses = poses;
+        if (st.kind == kStepTrack) head.pose_in = poses;
+        if ((rc = queue_preprocess(c, a, st.n, s))) return rc;
+        if ((rc = run_tracks(c, st, head, s))) return rc;
+        if (st.kind == kStepTrack) {
+            if (!fp32) continue;                   // the head kernel has updated the poses
+            ProfScope ps(c, 18, s);
+            CU_TRY(c, launch_pose_update(poses, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
+        } else {
+            ProfScope ps(c, 21, s);
+            if (fp32) CU_TRY(c, launch_pair_loss(st.out_trans, st.out_rot, nullptr, nullptr, head.loss, st.n, st.sums, s));
+            else CU_TRY(c, launch_loss_reduce(st.sq, st.n, st.sums, s));
+        }
+        ++c->launches;
     }
-    ++c->launches;
     return SE3TN_OK;
 }
 
@@ -1321,7 +1349,9 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
     if (!c) return SE3TN_ERR_INVALID;
     if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
     bool multi = false;
-    const int rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
+    int rc = check_single_round(c, "se3tn_track_batch");
+    if (rc) return rc;
+    rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
     if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || !rgbA || !depthA || H <= 0 || W <= 0)
@@ -1714,7 +1744,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
         x0 = std::min(x0, std::max(left - 1, 0)); x1 = std::max(x1, std::min(left + cw + 1, W));
     }
     if (y1 <= y0 || x1 <= x0) { y0 = y1 = x0 = x1 = 0; }         // every window misses the frame: nothing of it is read
-    if (static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
+    // refinement rounds after the first crop at poses only the step computes: their windows are not known here
+    const bool whole_frame = c->refine_iterations > 1;
+    if (whole_frame || static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
     // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
     // median-filtered image, and extrapolate scans whole columns.  Then the whole depth frame goes up; rgb stays windowed.
@@ -1771,6 +1803,8 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !rgbA || !depthA || !poses_out || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_host: null argument or empty frame");
+    const int rc = check_single_round(c, "se3tn_track_host");
+    if (rc) return rc;
     return track_host_step(c, "se3tn_track_host", frame_rgb, frame_depth, H, W, K, poses, object_width, rgbA, depthA, nullptr,
                            weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, stream);
 }
@@ -1836,6 +1870,14 @@ int se3tn_set_depth_fill(se3tn_ctx* c, int enable, double max_depth, int extrapo
     const float md = static_cast<float>(max_depth);                // what the kernels compute with
     if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_depth_fill: max_depth must be finite and > 0");
     c->depth_fill = {true, max_depth, extrapolate != 0 ? 1 : 0, blur_type};
+    return SE3TN_OK;
+}
+
+int se3tn_set_refine_iterations(se3tn_ctx* c, int k) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (k < 1 || k > SE3TN_MAX_REFINE_ITERATIONS)
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_set_refine_iterations: k must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
+    c->refine_iterations = k;
     return SE3TN_OK;
 }
 

@@ -256,23 +256,26 @@ class Engine:
         """n independent tracks of one frame: K0 -> conv stack -> K6, all enqueued on the current stream.  fill_depth: the
         observed depth is hole-filled inside the step first (depth_fill_spec); frame_depth itself is never written."""
         return self._track('track_batch', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
-                           rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth)
+                           rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, 1)
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
-                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None):
+                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
-        out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h)."""
+        out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h).  iterations: k rounds
+        of render -> network -> pose update on this frame in the one step, exactly what k chained calls with iterations=1
+        compute (se3tn_set_refine_iterations, 1..8); out_trans / out_rot hold the last round's outputs."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
-                           fill_depth)
+                           fill_depth, iterations)
 
     def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth):
+               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations):
         """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
         n = poses.shape[0]
+        iterations = self.refine_iterations(iterations)
         self._check_frame(fn, frame_rgb, frame_depth, poses, object_width, A, n)
         wh = self._host_ids(fn, weight_ids_host, n)
         fill = self.depth_fill_spec(fill_depth)
@@ -283,6 +286,7 @@ class Engine:
         if wh is not None and weight_ids_dev is None:
             weight_ids_dev = torch.from_numpy(wh).to(self.device)
         self._set_depth_fill(fill)
+        self._set_refine(iterations)
         H, W = frame_depth.shape
         head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
         tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
@@ -301,21 +305,23 @@ class Engine:
         (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous.  fill_depth as in
         track_batch: a live sensor's raw depth frame goes in as it is (the whole frame is uploaded then)."""
         return self._track_host('track_host', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
-                                rot_normalizer, weight_ids, precision, want_residuals, fill_depth)
+                                rot_normalizer, weight_ids, precision, want_residuals, fill_depth, 1)
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
-                          weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None):
+                          weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None,
+                          iterations=1):
         """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
-        without ids); mode / image_hw as in render()."""
+        without ids); mode / image_hw as in render(); iterations as in track_render (k > 1 uploads the whole frame)."""
         return self._track_host('track_render_host', frame_rgb, frame_depth, K, poses, object_width, (),
                                 self._render_mode(mode, image_hw), trans_normalizer, rot_normalizer, weight_ids, precision,
-                                want_residuals, fill_depth)
+                                want_residuals, fill_depth, iterations)
 
     def _track_host(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-                    weight_ids, precision, want_residuals, fill_depth):
+                    weight_ids, precision, want_residuals, fill_depth, iterations):
         """track_host (A = (rgbA, depthA), render None) and track_render_host (A = (), render = _render_mode's triple)."""
         n = int(poses.shape[0])
+        iterations = self.refine_iterations(iterations)
         for name, a, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
             if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
                 raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, dt, shape))
@@ -326,6 +332,7 @@ class Engine:
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         self._set_depth_fill(fill)
+        self._set_refine(iterations)
         H, W = frame_depth.shape
         head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
         tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
@@ -665,6 +672,18 @@ class Engine:
     def _set_depth_fill(self, spec):
         """Every tracking call sets the context's fill mode it wants: Trackers that share an Engine keep their own."""
         _lib.check(self.lib.se3tn_set_depth_fill(self._ctx, int(spec[0]), float(spec[1]), int(spec[2]), int(spec[3])), self._ctx)
+
+    @staticmethod
+    def refine_iterations(k):
+        """The refinement count of a tracking call as an int: 1..MAX_REFINE_ITERATIONS (se3tn_set_refine_iterations), else a
+        ValueError."""
+        if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 1 <= k <= _lib.MAX_REFINE_ITERATIONS:
+            raise ValueError('iterations must be an integer in [1, %d], not %r' % (_lib.MAX_REFINE_ITERATIONS, k))
+        return int(k)
+
+    def _set_refine(self, k):
+        """Every tracking call sets the refinement count it wants, as it sets the fill mode: track_batch / track_host set 1."""
+        _lib.check(self.lib.se3tn_set_refine_iterations(self._ctx, int(k)), self._ctx)
 
     # ------------------------------------------------------------------ introspection
     def debug_buffer(self, buf_id, n):

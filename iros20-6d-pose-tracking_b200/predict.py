@@ -19,6 +19,8 @@ Differences, all additive:
   * Tracker(..., fill_depth=True): on_track takes a live sensor's raw depth frame and hole-fills it
     inside the tracking step, as the reference's ROS node does with Utils.fill_depth before every
     on_track (predict_ros.py:38-41).
+  * Tracker(..., iterations=k): each frame refines every track k times inside one tracking step, exactly as k chained on_track
+    calls would (the CUDA rasteriser draws input A at each round's pose).
 """
 import contextlib
 import os
@@ -31,6 +33,8 @@ from .se3_tracknet import Se3TrackNet
 from .datasets import TrackDataset
 from .staging import StagingRing, VideoSink
 from . import Utils as U
+
+_refine_iterations = Engine.refine_iterations      # the drivers check counts before any Engine exists
 
 
 class PointCloud:
@@ -118,11 +122,15 @@ def _as_numpy_pose(p):
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
-                 fill_depth=False):
+                 fill_depth=False, iterations=1):
         """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
         tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
-        / blur_type (Engine.depth_fill_spec)."""
+        / blur_type (Engine.depth_fill_spec).
+        iterations: on_track / on_track_batch refine every track k times on each frame, in one tracking step (Engine.track_render),
+        exactly as k chained calls with iterations=1 would.  k > 1 needs the CUDA rasteriser drawing input A inside the step: a
+        reference GL renderer is a ValueError here, and input A passed to a call is a ValueError there."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
+        self.iterations = Engine.refine_iterations(iterations)
         self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
@@ -172,6 +180,9 @@ class Tracker:
                     raise
                 renderer = None                                    # e.g. a vertices-only ply: fall through to the GL renderers
         self.renderer = renderer if renderer is not None else self._try_reference_renderer(model_path, cam_cfg)
+        if self.iterations > 1 and not isinstance(self.renderer, CudaRenderer):
+            raise ValueError('iterations=%d redraws input A every round inside the tracking step: it needs the CUDA renderer '
+                             '(renderer="cuda"), not %r' % (self.iterations, self.renderer))
         self._np_bufs = {}
         self._copy_stream = torch.cuda.Stream(device=self.engine.device)      # _uploads: two staging slots, used alternately
         self._stage_bufs = ({}, {})
@@ -242,9 +253,13 @@ class Tracker:
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
                  rgbA=None, depthA=None, show=False):
         """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose.  Without rgbA / depthA and with the
-        CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host)."""
+        CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host), and refined
+        Tracker.iterations times."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
-        if (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None:
+        fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
+        if self.iterations > 1 and not fused:
+            raise ValueError(self._refine_refusal(rgbA is not None or depthA is not None))
+        if fused:
             out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
         else:
             if rgbA is None or depthA is None:
@@ -281,6 +296,8 @@ class Tracker:
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
+        if self.iterations > 1 and renderer is None:
+            raise ValueError(self._refine_refusal(not render))
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
                 and not any(torch.is_tensor(x) for x in (prev_poses, weight_ids, object_width))):
@@ -296,7 +313,7 @@ class Tracker:
             kw = dict(weight_ids=wh, precision=self.precision, fill_depth=self.fill_depth)
             if renderer is not None:
                 return self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw, **kw)
+                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations, **kw)
             return self.engine.track_host(*frame, self.K, poses, ow, *A, self.trans_normalizer, self.rot_normalizer, **kw)
 
         dev = self.engine.device
@@ -324,11 +341,16 @@ class Tracker:
             kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
             if renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
                 out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw, **kw)
+                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations, **kw)
             else:
                 out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
                                                     self.trans_normalizer, self.rot_normalizer, **kw)
         return out.cpu().numpy() if as_numpy else out
+
+    def _refine_refusal(self, given):
+        """Why a call of a Tracker with iterations > 1 cannot run: input A given (given), or a renderer the step cannot stand in for."""
+        why = 'input A was passed in' if given else 'the renderer cannot draw input A inside the tracking step (_fused_renderer)'
+        return 'iterations=%d redraws input A at each refined pose, but %s' % (self.iterations, why)
 
     def _weight_ids(self, weight_ids, n):
         """The tracks' weight ids as an int32 host array: the Tracker's weight set unless given, None for set 0 (a step
@@ -832,6 +854,49 @@ def precision_outdir(outdir, mode):
     return os.path.join(outdir, mode)
 
 
+def refine_counts(iterations):
+    """The refinement counts a one-pass driver tracks with -> (counts tuple, sweep).  An integer k gives ((k,), False); a sequence
+    of them gives (those counts, True).  A count outside [1, 8] (Engine.refine_iterations), a count listed twice and an empty
+    sequence are a ValueError."""
+    if isinstance(iterations, (list, tuple)):
+        got = tuple(_refine_iterations(k) for k in iterations)
+        if not got:
+            raise ValueError('no iteration count given')
+        twice = sorted(set(k for k in got if got.count(k) > 1))
+        if twice:
+            raise ValueError('iterations %s listed more than once' % ', '.join(map(str, twice)))
+        return got, True
+    return (_refine_iterations(iterations),), False
+
+
+def iterations_outdir(outdir, k):
+    """Where a sweep of refinement counts writes count k's output tree: <outdir>/iter<k>/, what a run with that k and that outdir
+    writes (with <mode>/ below it when precision modes are swept too)."""
+    return os.path.join(outdir, 'iter%d' % k)
+
+
+def _sweep_variants(outdir, modes, sweep, counts, ksweep):
+    """The variants a one-pass driver tracks every frame in -> [(key, mode, k, output tree)].  The key is what _track_sequences
+    keys a variant by: the mode name when every count is 1 (the runs without refinement), else (mode, k)."""
+    plain = counts == (1,)
+    out = []
+    for k in counts:
+        base = iterations_outdir(outdir, k) if ksweep else outdir
+        for m in modes:
+            out.append((m if plain else (m, k), m, k, precision_outdir(base, m) if sweep else base))
+    return out
+
+
+def _sweep_results(results, variants, sweep, ksweep):
+    """A driver's return value from {variant key: what one variant's run returns}: that alone for one variant, {mode: ...} for a
+    precision sweep, {k: ...} for a sweep of counts, {k: {mode: ...}} for both."""
+    per_k = {}
+    for key, m, k, _ in variants:
+        per_k.setdefault(k, {})[m] = results[key]
+    per_k = {k: (v if sweep else next(iter(v.values()))) for k, v in per_k.items()}
+    return per_k if ksweep else next(iter(per_k.values()))
+
+
 def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     """The checked configuration of every requested class, before anything is loaded onto a device -> list (ascending class id)
     of dicts: class_id, name, the expanded paths, dataset_info, mean, std, trans_normalizer, rot_normalizer.
@@ -890,28 +955,31 @@ def _one_pass_trackers(entries, precision, max_batch):
     return eng, trackers
 
 
-def _track_sequences(eng, trackers, sequences, precisions, depth, workers, video=None):
+def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
-    precisions: the modes (a tuple) every frame is tracked in.  Yields each sequence's {mode: (frames, n, 4, 4) numpy poses}, the
-    poses after each frame, as soon as the sequence ends.
+    variants: what every frame is tracked in (a tuple), each a precision mode name (one round per step) or a (mode, k) pair (k
+    refinement rounds per step, Engine.track_render's iterations).  Yields each sequence's {variant: (frames, n, 4, 4) numpy
+    poses}, the poses after each frame, as soon as the sequence ends.
 
-    Every frame is one se3tn_track_render step per mode for the sequence's n tracks, all reading the same device frame: the
+    Every frame is one se3tn_track_render step per variant for the sequence's n tracks, all reading the same device frame: the
     frames of all sequences decode ahead, across sequence boundaries, through one StagingRing of `depth` sets (`workers` threads)
-    into its one device frame, so a frame is decoded once whatever the number of modes.  The steps' other device arguments are
-    kept: the ids and widths per distinct weight-id tuple, and per (mode, n) the pose tensor that mode's steps update in place and
-    their outputs.  So in each mode every step after a track set's first replays that mode's CUDA graph, across sequences too
-    ('fp32' steps are never captured).  With 'fp8' among the modes, each weight set is calibrated on the first frame of the first
-    sequence that tracks it, before that frame's steps.  After each step the mode's poses are copied into its device history,
-    which comes back to the host once per sequence.
+    into its one device frame, so a frame is decoded once whatever the number of variants.  The steps' other device arguments are
+    kept: the ids and widths per distinct weight-id tuple, and per (variant, n) the pose tensor that variant's steps update in place
+    and their outputs.  So in each variant every step after a track set's first replays that variant's CUDA graph, across
+    sequences too ('fp32' steps are never captured).  With 'fp8' among the modes, each weight set is calibrated on the first frame
+    of the first sequence that tracks it, before that frame's steps, at the sequence's initial poses.  After each step the
+    variant's poses are copied into its device history, which comes back to the host once per sequence.
 
     video: None, or (label order, [(paths, labels)] per sequence): paths holds one mp4 path per track, labels one text per frame.
     Then each frame's decode jobs also render its label strip into the ring, and after each step Engine.draw_tracks draws every
     track's Tracker.object_cloud points at its new pose over the device frame (the point sets uploaded once, as one table), and a
     VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed.
-    Videos are drawn for one mode only."""
-    if video is not None and len(precisions) != 1:
-        raise ValueError('result videos are drawn for one precision mode, not %d' % len(precisions))
+    Videos are drawn for one variant only."""
+    if video is not None and len(variants) != 1:
+        raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
+    mode_k = {v: (v, 1) if isinstance(v, str) else v for v in variants}
+    fp8 = next((v for v in variants if mode_k[v][0] == 'fp8'), None)
     if not sequences:
         return
     dev = eng.device
@@ -944,36 +1012,38 @@ def _track_sequences(eng, trackers, sequences, precisions, depth, workers, video
                 wh = np.asarray(ids, dtype=np.int32)
                 by_ids[ids] = (wh, torch.from_numpy(wh).to(dev),
                                torch.tensor([trackers[w].object_width for w in ids], dtype=torch.float64, device=dev))
-            for m in precisions:
-                if (m, n) not in by_n:
-                    by_n[m, n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
+            for v in variants:
+                if (v, n) not in by_n:
+                    by_n[v, n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
                                   torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
                                   None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
-                by_n[m, n][0].copy_(torch.from_numpy(init))
+                by_n[v, n][0].copy_(torch.from_numpy(init))
             wh, wd, widths = by_ids[ids]
-            history = {m: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for m in precisions}
+            history = {v: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for v in variants}
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
-                if 'fp8' in precisions and t == 0:     # each set is calibrated on the first frame of the first sequence that tracks it
-                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n['fp8', n][0], widths, weight_ids=wh,
+                if fp8 is not None and t == 0:         # each set is calibrated on the first frame of the first sequence that tracks it
+                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[fp8, n][0], widths, weight_ids=wh,
                                              render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
-                for m in precisions:
-                    poses, out_trans, out_rot, drawn = by_n[m, n]
+                for v in variants:
+                    m, rounds = mode_k[v]
+                    poses, out_trans, out_rot, drawn = by_n[v, n]
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
-                                     image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot)
-                    history[m][t].copy_(poses)
+                                     image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot,
+                                     iterations=rounds)
+                    history[v][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
                                     label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
                     sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
-            yield {m: h.cpu().numpy() for m, h in history.items()}
+            yield {v: h.cpu().numpy() for v, h in history.items()}
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False):
+                     video=False, iterations=1):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -989,10 +1059,19 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
 
     video: also write the result video a per-class run writes next to its seq<id>/ (predict.py:403, 424-435): <outdir>/<class
     folder>/run/seq<id>.mp4, one half-size frame per tracked frame (none for the start pose), the class's model points drawn at
-    their tracked pose over the frame, under the label 'frame:<i+1>' of frame i.  The drawing runs on the device."""
+    their tracked pose over the frame, under the label 'frame:<i+1>' of frame i.  The drawing runs on the device.
+
+    iterations: k, the refinement rounds of every step (Engine.track_render; 1, today's step, writes what a run without the
+    argument writes), or a sweep: a sequence of counts.  A sweep of counts tracks every frame once per (mode, k) and returns
+    {k: what a run with that k returns}; count k writes its tree under <outdir>/iter<k>/ (with <mode>/ below it when modes are
+    swept too), file for file what a run with that k and mode writes.  score_iterations scores it.  Counts outside [1, 8], repeated
+    counts, an empty sequence, and video=True with more than one variant are a ValueError before anything is loaded."""
     modes, sweep = precision_modes(precision, YCB_ALL_PRECISIONS)
     if video and len(modes) > 1:
         raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
+    counts, ksweep = refine_counts(iterations)
+    if video and len(counts) > 1:
+        raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     classes = ycb_all_classes(ycb_dir, class_ids, class_config, modes[0])
@@ -1010,25 +1089,27 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], modes[0],
                                        max([len(v) for v in track_sets.values()] + [1]))
     name_of = {k['class_id']: k['name'] for k in classes}
-    root = {m: precision_outdir(outdir, m) if sweep else outdir for m in modes}
+    variants = _sweep_variants(outdir, modes, sweep, counts, ksweep)
+    root = {v: r for v, _, _, r in variants}
+    keys = tuple(root)
     drawn = None
     if video:
-        drawn = ('under', [([os.path.join(ycb_all_res_dir(root[modes[0]], name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
+        drawn = ('under', [([os.path.join(ycb_all_res_dir(root[keys[0]], name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)])
         for c in name_of.values():
-            os.makedirs(ycb_all_res_dir(root[modes[0]], c), exist_ok=True)
-    results = {m: {k['class_id']: {} for k in classes} for m in modes}
-    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, modes, 2, 2, drawn),
+            os.makedirs(ycb_all_res_dir(root[keys[0]], c), exist_ok=True)
+    results = {v: {k['class_id']: {} for k in classes} for v in keys}
+    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, keys, 2, 2, drawn),
                                                        track_sets.items(), sequences):
-        for m in modes:
-            pred_poses = np.concatenate([init[None], tracked[m]])    # row 0: the start pose, as in getResultsYcb
+        for v in keys:
+            pred_poses = np.concatenate([init[None], tracked[v]])    # row 0: the start pose, as in getResultsYcb
             for j, c in enumerate(cls):
-                sdir = os.path.join(ycb_all_res_dir(root[m], name_of[c]), 'seq{}'.format(seq_id))
+                sdir = os.path.join(ycb_all_res_dir(root[v], name_of[c]), 'seq{}'.format(seq_id))
                 os.makedirs(sdir, exist_ok=True)
                 for i in range(len(pred_poses)):
                     np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
-                results[m][c][seq_id] = pred_poses[:, j]
-    return results if sweep else results[modes[0]]
+                results[v][c][seq_id] = pred_poses[:, j]
+    return _sweep_results(results, variants, sweep, ksweep)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1097,7 +1178,7 @@ def write_video_poses(outdir, video, poses):
 
 
 def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
-                        video=False):
+                        video=False, iterations=1):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -1116,11 +1197,17 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     which refuses 'fp16', every mode is taken here.  A sweep tracks every frame in every mode (one step per mode, each frame
     decoded once, every weight set loaded once) and returns {mode: what a run in that mode returns}; mode m writes its tree under
     <outdir>/<m>/, file for file what a run in mode m with that outdir writes.  score_precisions scores it.  Unknown or repeated
-    modes, an empty sequence, and video=True with more than one mode are a ValueError before anything is loaded."""
+    modes, an empty sequence, and video=True with more than one mode are a ValueError before anything is loaded.
+
+    iterations: k refinement rounds per step, or a sweep of counts, as in getResultsYcbAll: count k of a sweep writes under
+    <outdir>/iter<k>/ (then <mode>/ when modes are swept too)."""
     from .eval_ycbineoat import OBJECTS
     modes, sweep = precision_modes(precision, PRECISIONS)
     if video and len(modes) > 1:
         raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
+    counts, ksweep = refine_counts(iterations)
+    if video and len(counts) > 1:
+        raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
@@ -1136,19 +1223,21 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
         nf = len(rgb_files) if max_frames is None else min(max_frames, len(rgb_files))
         if nf > 0:
             sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
-    root = {m: precision_outdir(outdir, m) if sweep else outdir for m in modes}
+    variants = _sweep_variants(outdir, modes, sweep, counts, ksweep)
+    root = {key: r for key, _, _, r in variants}
+    keys = tuple(root)
     drawn = None
     if video:
-        os.makedirs(root[modes[0]], exist_ok=True)
-        drawn = ('over', [([os.path.join(root[modes[0]], v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))])
+        os.makedirs(root[keys[0]], exist_ok=True)
+        drawn = ('over', [([os.path.join(root[keys[0]], v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))])
                           for v, s in sequences.items()])
-    results = {m: {} for m in modes}
-    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), modes, decode_ahead, 2 * decode_ahead, drawn),
+    results = {key: {} for key in keys}
+    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn),
                           sequences):
-        for m in modes:
-            results[m][v] = tracked[m][:, 0]
-            write_video_poses(root[m], v, results[m][v])
-    return results if sweep else results[modes[0]]
+        for key in keys:
+            results[key][v] = tracked[key][:, 0]
+            write_video_poses(root[key], v, results[key][v])
+    return _sweep_results(results, variants, sweep, ksweep)
 
 
 def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
@@ -1163,10 +1252,31 @@ def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
     max and mean in mm, on each class's or object's Tracker.object_cloud points; one add_adi_sets launch per mode.  No ground
     truth is involved, so it also shows where modes part ways on frames without annotations.  The reference is
     sweep_reference(modes), whose own row is 0."""
+    modes = list(results)
+    ref = sweep_reference(modes)
+    return ref, _score_variants(results, {m: precision_outdir(outdir, m) for m in modes}, ref, 'precision %s', ycb_dir, config,
+                                YCBInEOAT_dir)
+
+
+def score_iterations(results, outdir, ycb_dir, config, YCBInEOAT_dir=None, precision='bf16x3'):
+    """score_precisions for a sweep of refinement counts: results what getResultsYcbAll / getResultsYcbInEOAT returned for
+    iterations=[k1, k2, ...] with this precision (a mode, or the modes of a precision sweep).  One row per variant, labelled by its
+    tree under outdir: 'iter<k>', or 'iter<k>/<mode>' when modes were swept too, each with its AUCs and its drift from the k = 1
+    tree of the sweep's reference mode (sweep_reference; the smallest k swept when 1 is not).  -> (reference label, rows)."""
+    sweep = precision_modes(precision, PRECISIONS)[1]
+    modes = list(next(iter(results.values()))) if sweep else [precision]
+    label = lambda k, m: os.path.relpath(precision_outdir(iterations_outdir(outdir, k), m) if sweep else iterations_outdir(outdir, k), outdir)
+    flat = {label(k, m): (res[m] if sweep else res) for k, res in results.items() for m in modes}
+    ref = label(1 if 1 in results else min(results), sweep_reference(modes))
+    return ref, _score_variants(flat, {v: os.path.join(outdir, v) for v in flat}, ref, 'variant %s', ycb_dir, config, YCBInEOAT_dir)
+
+
+def _score_variants(results, roots, ref, header, ycb_dir, config, YCBInEOAT_dir):
+    """The rows of score_precisions / score_iterations: results {label: what one variant's run returned}, roots {label: its tree},
+    ref the label drift is measured from; each variant's scorer lines are printed under header % label."""
     import argparse
     from .eval_ycbineoat import eval_all, video_object
     modes = list(results)
-    ref = sweep_reference(modes)
     if YCBInEOAT_dir is None:
         names = ycb_class_names(ycb_dir)
         keys = [(c, s) for c in sorted(results[ref]) for s in sorted(results[ref][c])]
@@ -1186,8 +1296,8 @@ def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
     ref_poses = stacked(ref)
     rows = {}
     for m in modes:
-        print('precision %s' % m)
-        root = precision_outdir(outdir, m)
+        print(header % m)
+        root = roots[m]
         if YCBInEOAT_dir is None:
             adds, add = _score_ycb_tree(ycb_dir, root, sorted(results[m]))
         else:
@@ -1195,7 +1305,7 @@ def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
         d_add, d_adds = (d.cpu().numpy() * 1000 for d in eng.add_adi_sets(clouds, pose_set, stacked(m), ref_poses))
         rows[m] = dict(add=add, adds=adds, add_max=float(d_add.max()), add_mean=float(d_add.mean()),
                        adds_max=float(d_adds.max()), adds_mean=float(d_adds.mean()))
-    return ref, rows
+    return rows
 
 
 def _score_ycb_tree(ycb_dir, root, class_ids):
@@ -1212,10 +1322,11 @@ def _score_ycb_tree(ycb_dir, root, class_ids):
     return (eval_ycb.VOCap(np.concatenate([e[0] for e in errs])) * 100, eval_ycb.VOCap(np.concatenate([e[1] for e in errs])) * 100)
 
 
-def print_precision_table(ref, rows):
-    """The table --score prints after a sweep's per-mode scores: one row per mode of score_precisions' result."""
-    print('precision sweep: AUCs in percent; drift from %s in mm (ADD / ADD-S to its pose of the same track and frame)' % ref)
-    print('%-8s %9s %9s %11s %11s %11s %11s' % ('mode', 'ADD', 'ADD-S', 'ADD max', 'ADD mean', 'ADD-S max', 'ADD-S mean'))
+def print_precision_table(ref, rows, sweep='precision sweep', column='mode'):
+    """The table --score prints after a sweep's per-mode scores: one row per mode of score_precisions' result (per variant of
+    score_iterations' with sweep='iteration sweep', column='variant')."""
+    print('%s: AUCs in percent; drift from %s in mm (ADD / ADD-S to its pose of the same track and frame)' % (sweep, ref))
+    print('%-8s %9s %9s %11s %11s %11s %11s' % (column, 'ADD', 'ADD-S', 'ADD max', 'ADD mean', 'ADD-S max', 'ADD-S mean'))
     for m, r in rows.items():
         print('%-8s %9.4f %9.4f %11.4g %11.4g %11.4g %11.4g' % (m, r['add'], r['adds'], r['add_max'], r['add_mean'], r['adds_max'],
                                                                r['adds_mean']))
@@ -1248,13 +1359,18 @@ def main(argv=None):
     parser.add_argument('--precision', default=None, help='MODE|all|MODE,MODE,...: the precision mode (default bf16x3).  ycbv_all / '
                         'ycbineoat_all also take a comma-separated list of modes or all: every frame is tracked in each mode, mode m '
                         'written under <outdir>/<m>/, and --score prints each mode\'s scores and a table of their AUCs and drift')
+    parser.add_argument('--iterations', default=None, help='K|K1,K2,...: refine every track K times per frame in one tracking step '
+                        '(1..8, default 1).  ycbv_all / ycbineoat_all also take a comma-separated list: every frame is tracked with '
+                        'each K, K\'s tree written under <outdir>/iter<K>/, and --score adds a table of each variant\'s AUCs and drift '
+                        'from K = 1')
     args = parser.parse_args(argv)
     precision = cli_precision(args.precision, args.mode)
+    iterations = cli_iterations(args.iterations, args.mode)
     if args.mode == 'ycbv_all':
-        return _main_ycbv_all(args, precision)
+        return _main_ycbv_all(args, precision, iterations)
     if args.mode == 'ycbineoat_all':
-        return _main_ycbineoat_all(args, precision)
-    prec_kw = {} if precision is None else {'precision': precision}
+        return _main_ycbineoat_all(args, precision, iterations)
+    prec_kw = dict({} if precision is None else {'precision': precision}, **({} if iterations is None else {'iterations': iterations}))
     dataset_info, images_mean, images_std = load_run_config(args.train_data_path, args.mean_std_path)
     if args.mode == 'ycbineoat':
         if not args.YCBInEOAT_dir:
@@ -1300,12 +1416,44 @@ def cli_precision(text, mode):
     return precision
 
 
+def cli_iterations(text, mode):
+    """--iterations of `mode` -> None (not given: one round per step), a count, or for ycbv_all / ycbineoat_all a list of counts
+    (a sweep).  A count outside [1, 8] or not an integer, and a list with any other mode, are a SystemExit; so is a list its
+    driver refuses (repeated counts, an empty entry)."""
+    if text is None:
+        return None
+    try:
+        if ',' not in text:
+            return _refine_iterations(int(text))
+        if mode not in ('ycbv_all', 'ycbineoat_all'):
+            raise SystemExit('--iterations %s: a list of counts needs --mode ycbv_all or ycbineoat_all' % text)
+        counts = [int(k) for k in text.split(',')]
+        refine_counts(counts)
+    except ValueError as e:
+        raise SystemExit('--iterations %s: %s' % (text, e))
+    return counts
+
+
+def _sweep_kw(args, precision, iterations):
+    """A one-pass driver's keyword arguments: video, precision and iterations, each passed only when given, so a run without them
+    makes the same call."""
+    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
+    return dict(kw, **({} if iterations is None else {'iterations': iterations}))
+
+
+def _one_run(res, precision, iterations, modes):
+    """What a one-pass driver returned for one variant (the first of a sweep): the printout lists its sequences."""
+    if isinstance(iterations, list):
+        res = next(iter(res.values()), {})
+    return next(iter(res.values()), {}) if precision is not None and precision_modes(precision, modes)[1] else res
+
+
 def _video_kw(args):
     """The drivers' video argument: passed only when --video asks for the videos, so a run without it makes the same call."""
     return {'video': True} if args.video else {}
 
 
-def _main_ycbv_all(args, precision=None):
+def _main_ycbv_all(args, precision=None, iterations=None):
     """--mode ycbv_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class path templates."""
     if not args.ycb_dir or not args.class_ids:
         raise SystemExit('--mode ycbv_all needs --ycb_dir and --class_ids')
@@ -1318,21 +1466,24 @@ def _main_ycbv_all(args, precision=None):
         except ValueError:
             raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
+    kw = _sweep_kw(args, precision, iterations)
     res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
     sweep = precision is not None and precision_modes(precision, YCB_ALL_PRECISIONS)[1]
-    one = next(iter(res.values()), {}) if sweep else res
+    one = _one_run(res, precision, iterations, YCB_ALL_PRECISIONS)
     for c in sorted(one):
         print('tracked class %d through sequences %s' % (c, sorted(one[c])))
     print('-> %s' % args.outdir)
-    if args.score and sweep:
+    if args.score and isinstance(iterations, list):
+        print_precision_table(*score_iterations(res, args.outdir, args.ycb_dir, config, precision=precision or 'bf16x3'),
+                              sweep='iteration sweep', column='variant')
+    elif args.score and sweep:
         print_precision_table(*score_precisions(res, args.outdir, args.ycb_dir, config))
     elif args.score:
         _score_ycb_tree(args.ycb_dir, args.outdir, class_ids)
     return res
 
 
-def _main_ycbineoat_all(args, precision=None):
+def _main_ycbineoat_all(args, precision=None, iterations=None):
     """--mode ycbineoat_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-object path templates."""
     import argparse
     if not args.YCBInEOAT_dir:
@@ -1340,15 +1491,18 @@ def _main_ycbineoat_all(args, precision=None):
     if args.score and not args.ycb_dir:
         raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
+    kw = _sweep_kw(args, precision, iterations)
     res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
                               ycb_dir=args.ycb_dir, **kw)
     sweep = precision is not None and precision_modes(precision, PRECISIONS)[1]
-    one = next(iter(res.values()), {}) if sweep else res
+    one = _one_run(res, precision, iterations, PRECISIONS)
     for v in one:
         print('tracked %s: %d frames' % (v, len(one[v])))
     print('-> %s' % args.outdir)
-    if args.score and sweep:
+    if args.score and isinstance(iterations, list):
+        print_precision_table(*score_iterations(res, args.outdir.rstrip('/'), args.ycb_dir, config, YCBInEOAT_dir=args.YCBInEOAT_dir,
+                                                precision=precision or 'bf16x3'), sweep='iteration sweep', column='variant')
+    elif args.score and sweep:
         print_precision_table(*score_precisions(res, args.outdir.rstrip('/'), args.ycb_dir, config, YCBInEOAT_dir=args.YCBInEOAT_dir))
     elif args.score:
         from . import eval_ycbineoat
