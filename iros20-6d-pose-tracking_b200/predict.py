@@ -940,10 +940,11 @@ def ycb_track_sets(ycb_dir, class_ids):
     return dict(sorted(sets.items()))
 
 
-def _one_pass_trackers(entries, precision, max_batch):
-    """One Engine of max_batch tracks per step and {weight id: Tracker} on it for [(weight id, label, checked configuration)]: the
-    configuration's files and normalisers, the CUDA renderer.  A ValueError is relabelled with the class or object it is about."""
-    eng = Engine(max_batch=max_batch)
+def _one_pass_trackers(entries, precision, max_batch, device=None):
+    """One Engine of max_batch tracks per step on `device` (None: the current device) and {weight id: Tracker} on it for
+    [(weight id, label, checked configuration)]: the configuration's files and normalisers, the CUDA renderer.  A ValueError is
+    relabelled with the class or object it is about."""
+    eng = Engine(max_batch=max_batch, device=device)
     trackers = {}
     for wid, label, k in entries:
         try:
@@ -1042,8 +1043,197 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
             yield {v: h.cpu().numpy() for v, h in history.items()}
 
 
+# ----------------------------------------------------------------------------------------------------
+# The one-pass drivers on several GPUs (gpus=N): whole sequences are shared out over N ranks, one spawned process per GPU, each
+# running _track_sequences on its share with its own Engine and Trackers and writing its sequences' files.  A sequence keeps its
+# tracks, so every step has the n of the single-GPU run and the same bits (the trunk's split-K latency mode for n <= 4 and its
+# throughput mode beyond are chosen by n).  The one state that passes between sequences is each weight set's fp8 calibration:
+# every rank calibrates a set on the frame a single-GPU run uses, the first frame of the set's first sequence in run order.
+# ----------------------------------------------------------------------------------------------------
+def check_gpus(gpus):
+    """The one-pass drivers' gpus argument -> int.  Below 1 is a ValueError; so is more than torch.cuda.device_count(), checked
+    only for more than one, so gpus=1 asks nothing of the device."""
+    if isinstance(gpus, bool) or int(gpus) != gpus:
+        raise ValueError('gpus must be an integer, not %r' % (gpus,))
+    gpus = int(gpus)
+    if gpus < 1:
+        raise ValueError('gpus must be at least 1, not %d' % gpus)
+    if gpus > 1 and gpus > torch.cuda.device_count():
+        raise ValueError('gpus=%d, but %d CUDA devices are visible' % (gpus, torch.cuda.device_count()))
+    return gpus
+
+
+def assign_ranks(costs, gpus):
+    """Sequences onto ranks, greedy longest first: sequence i (cost costs[i], its frame count) goes to the rank with the least
+    cost so far (among equals the one with the fewest sequences, then the lowest), the sequences taken by descending cost and then
+    in order.  -> one ascending list of sequence indices per rank, min(gpus, len(costs)) ranks, none empty, each sequence on
+    exactly one."""
+    n = min(int(gpus), len(costs))
+    loads, ranks = [0] * n, [[] for _ in range(n)]
+    for i in sorted(range(len(costs)), key=lambda i: (-costs[i], i)):
+        r = min(range(n), key=lambda r: (loads[r], len(ranks[r]), r))
+        ranks[r].append(i)
+        loads[r] += costs[i]
+    return [sorted(r) for r in ranks]
+
+
+def borrowed_calibrations(track_sets, mine):
+    """Where a rank that tracks sequences `mine` (indices into track_sets, each sequence's weight ids in run order) calibrates the
+    fp8 scales of weight sets it cannot calibrate itself -> {sequence index: [track indices]}.  A single-GPU run calibrates each set
+    on the first frame of the first sequence that tracks it, at that sequence's initial poses (_track_sequences).  When that
+    sequence is the rank's, its own loop does the same; for each other set the rank tracks, the entry names that sequence and the
+    tracks of the sets whose first sequence it is."""
+    first = {}
+    for k, ids in enumerate(track_sets):
+        for w in ids:
+            first.setdefault(w, k)
+    own = set(mine)
+    needed = set(w for k in mine for w in track_sets[k])
+    out = {}
+    for w in sorted(needed):
+        if first[w] not in own:
+            out.setdefault(first[w], set()).add(w)
+    return {k: [j for j, w in enumerate(track_sets[k]) if w in ws] for k, ws in sorted(out.items())}
+
+
+def _rank_devices(n):
+    """The CUDA device of each of n ranks: rank r runs on cuda:r of the visible devices."""
+    return list(range(n))
+
+
+def _calibrate_borrowed(eng, trackers, sequences, borrowed):
+    """The fp8 calibrations borrowed_calibrations names, in sequence order: each sequence's first frame decoded and calibrated at
+    the initial poses of the named tracks, as _track_sequences calibrates it (Engine.calibrate_fp8_tracks, input A drawn by the
+    rasteriser).  Calibration takes per-tensor maxima of each set's own tracks, so it gives the single-GPU run's scales."""
+    dev = eng.device
+    for k, tracks in borrowed.items():
+        rgb_files, depth_files, ids, init = sequences[k]
+        wh = np.asarray([ids[j] for j in tracks], dtype=np.int32)
+        trk = trackers[int(wh[0])]
+        wd = torch.from_numpy(wh).to(dev)
+        widths = torch.tensor([trackers[int(w)].object_width for w in wh], dtype=torch.float64, device=dev)
+        poses = torch.from_numpy(np.ascontiguousarray(init[tracks])).to(dev)
+        rgb = torch.from_numpy(read_rgb(rgb_files[0])).to(dev)
+        depth = torch.from_numpy(read_depth(depth_files[0])).to(dev)
+        eng.calibrate_fp8_tracks(rgb, depth, trk.K, poses, widths, weight_ids=wh,
+                                 render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
+
+
+def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
+               writes):
+    """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: its Engine and Trackers for the weight sets of
+    its sequences, the borrowed fp8 calibrations, then _track_sequences over sequences[mine] with writes[k] (fn, *args) called as
+    fn(*args, tracked) on each.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error',
+    traceback text) through conn."""
+    import traceback
+    try:
+        wids = set(w for k in mine for w in sequences[k][2])
+        torch.cuda.set_device(device)
+        eng, trackers = _one_pass_trackers([e for e in entries if e[0] in wids], precision, max_batch, device)
+        _calibrate_borrowed(eng, trackers, sequences, borrowed)
+        drawn = None if video is None else (video[0], [video[1][k] for k in mine])
+        out = {}
+        for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn), mine):
+            fn, *args = writes[k]
+            out[k] = fn(*args, tracked)
+        conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
+    except BaseException:
+        conn.send(('error', traceback.format_exc()))
+    finally:
+        conn.close()
+
+
+def _agree_fp8_scales(per_rank):
+    """The ranks' {weight id: fp8 scales or None} -> one such dict.  Ranks that both have scales for a set have the same ones:
+    otherwise a RuntimeError, since the poses would depend on how the sequences were shared out."""
+    out = {}
+    for r, scales in enumerate(per_rank):
+        for w, s in scales.items():
+            if s is None:
+                continue
+            if w in out and not np.array_equal(out[w][1], s):
+                raise RuntimeError('ranks %d and %d calibrated weight set %d differently: %s, %s' % (out[w][0], r, w, out[w][1], s))
+            out.setdefault(w, (r, s))
+    return {w: s for w, (_, s) in sorted(out.items())}
+
+
+def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes):
+    """_track_sequences over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
+    rank (as _rank_main runs it) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
+    frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
+    with its traceback; then, as on any other exit (KeyboardInterrupt included), every rank still running is terminated, and every
+    rank is joined before this returns or raises."""
+    import multiprocessing as mp
+    from multiprocessing.connection import wait
+    plan = assign_ranks([len(s[0]) for s in sequences], gpus)
+    fp8 = any((v if isinstance(v, str) else v[0]) == 'fp8' for v in variants)
+    track_sets = [s[2] for s in sequences]
+    devices = _rank_devices(len(plan))
+    ctx = mp.get_context('spawn')
+    procs, conns, done = [], [], False
+    try:
+        for r, mine in enumerate(plan):
+            recv, send = ctx.Pipe(duplex=False)
+            conns.append(recv)
+            borrowed = borrowed_calibrations(track_sets, mine) if fp8 else {}
+            p = ctx.Process(target=_rank_main, name='one-pass rank %d' % r, daemon=True,
+                            args=(send, r, devices[r], entries, precision, max_batch, sequences, mine, borrowed, variants, depth,
+                                  workers, video, writes))
+            try:
+                p.start()
+            finally:
+                send.close()                       # the child's end: once the child exits, recv sees EOF
+            procs.append(p)
+        results, scales, pending = {}, {}, dict(enumerate(conns))
+        while pending:
+            ready = wait(list(pending.values()) + [procs[r].sentinel for r in pending])
+            for r in [r for r, c in pending.items() if c in ready or procs[r].sentinel in ready]:
+                try:
+                    msg = pending[r].recv() if pending[r].poll() else None
+                except EOFError:
+                    msg = None
+                if msg is None:
+                    procs[r].join(5)
+                    raise RuntimeError('rank %d (cuda:%d) exited with code %s before sending its results'
+                                       % (r, devices[r], procs[r].exitcode))
+                if msg[0] == 'error':
+                    raise RuntimeError('rank %d (cuda:%d) failed:\n%s' % (r, devices[r], msg[1]))
+                results.update(msg[1])
+                scales[r] = msg[2]
+                del pending[r]
+        _agree_fp8_scales([scales[r] for r in range(len(plan))])
+        done = True
+    finally:
+        for p in procs:
+            if not done and p.is_alive():
+                p.terminate()
+        for p in procs:
+            p.join(60)
+            if p.is_alive():
+                p.kill()
+                p.join()
+        for c in conns:
+            c.close()
+    return [results[k] for k in range(len(sequences))]
+
+
+def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
+    """One test sequence's files of a getResultsYcbAll run: for each variant (dirs: {variant: {class id: result folder}}) and
+    class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  -> {variant: (frames, n, 4, 4) poses}."""
+    out = {}
+    for v, folder in dirs.items():
+        pred_poses = np.concatenate([init[None], tracked[v]])    # row 0: the start pose, as in getResultsYcb
+        for j, c in enumerate(cls):
+            sdir = os.path.join(folder[c], 'seq{}'.format(seq_id))
+            os.makedirs(sdir, exist_ok=True)
+            for i in range(len(pred_poses)):
+                np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
+        out[v] = pred_poses
+    return out
+
+
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1):
+                     video=False, iterations=1, gpus=1):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1065,7 +1255,16 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     argument writes), or a sweep: a sequence of counts.  A sweep of counts tracks every frame once per (mode, k) and returns
     {k: what a run with that k returns}; count k writes its tree under <outdir>/iter<k>/ (with <mode>/ below it when modes are
     swept too), file for file what a run with that k and mode writes.  score_iterations scores it.  Counts outside [1, 8], repeated
-    counts, an empty sequence, and video=True with more than one variant are a ValueError before anything is loaded."""
+    counts, an empty sequence, and video=True with more than one variant are a ValueError before anything is loaded.
+
+    gpus: the number of GPUs, one process each (1: this process alone).  With N > 1 the test sequences are shared out whole over
+    min(N, sequences) spawned ranks on cuda:0 .. cuda:N-1 (assign_ranks, on frame counts); each rank loads the weight sets of its
+    sequences, tracks them as above and writes their files and videos, every file the one a single-GPU run writes.  The return
+    value equals the single-GPU run's, bit for bit and in the same order, and so do the files; each fp8 set is calibrated on the
+    frame a single-GPU run calibrates it on (borrowed_calibrations).  gpus below 1 or above torch.cuda.device_count() is a
+    ValueError before anything is loaded, as is every other refusal; a rank that fails is a RuntimeError with its traceback,
+    raised after every rank has stopped (_track_on_ranks)."""
+    gpus = check_gpus(gpus)
     modes, sweep = precision_modes(precision, YCB_ALL_PRECISIONS)
     if video and len(modes) > 1:
         raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
@@ -1086,8 +1285,10 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
         init = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
                                          sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]).astype(np.float64)
         sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
-    eng, trackers = _one_pass_trackers([(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes], modes[0],
-                                       max([len(v) for v in track_sets.values()] + [1]))
+    entries = [(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes]
+    max_batch = max([len(v) for v in track_sets.values()] + [1])
+    if gpus == 1:
+        eng, trackers = _one_pass_trackers(entries, modes[0], max_batch)
     name_of = {k['class_id']: k['name'] for k in classes}
     variants = _sweep_variants(outdir, modes, sweep, counts, ksweep)
     root = {v: r for v, _, _, r in variants}
@@ -1098,17 +1299,18 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)])
         for c in name_of.values():
             os.makedirs(ycb_all_res_dir(root[keys[0]], c), exist_ok=True)
+    dirs = {v: {c: ycb_all_res_dir(root[v], name) for c, name in name_of.items()} for v in keys}
+    writes = [(_write_ycb_all_sequence, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
+    if gpus == 1:
+        written = (fn(*args, tracked) for tracked, (fn, *args) in zip(_track_sequences(eng, trackers, sequences, keys, 2, 2, drawn),
+                                                                      writes))
+    else:
+        written = _track_on_ranks(gpus, entries, modes[0], max_batch, sequences, keys, 2, 2, drawn, writes)
     results = {v: {k['class_id']: {} for k in classes} for v in keys}
-    for tracked, (seq_id, cls), (_, _, _, init) in zip(_track_sequences(eng, trackers, sequences, keys, 2, 2, drawn),
-                                                       track_sets.items(), sequences):
+    for pred_poses, (seq_id, cls) in zip(written, track_sets.items()):
         for v in keys:
-            pred_poses = np.concatenate([init[None], tracked[v]])    # row 0: the start pose, as in getResultsYcb
             for j, c in enumerate(cls):
-                sdir = os.path.join(ycb_all_res_dir(root[v], name_of[c]), 'seq{}'.format(seq_id))
-                os.makedirs(sdir, exist_ok=True)
-                for i in range(len(pred_poses)):
-                    np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
-                results[v][c][seq_id] = pred_poses[:, j]
+                results[v][c][seq_id] = pred_poses[v][:, j]
     return _sweep_results(results, variants, sweep, ksweep)
 
 
@@ -1177,8 +1379,18 @@ def write_video_poses(outdir, video, poses):
         np.savetxt(os.path.join(vdir, '%07d.txt' % i), poses[i])
 
 
+def _write_ycbineoat_video(roots, video, tracked):
+    """One video's files of a getResultsYcbInEOAT run: write_video_poses under each variant's tree (roots: {variant: tree}).
+    -> {variant: (frames, 4, 4) poses}."""
+    out = {}
+    for key, root in roots.items():
+        out[key] = tracked[key][:, 0]
+        write_video_poses(root, video, out[key])
+    return out
+
+
 def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
-                        video=False, iterations=1):
+                        video=False, iterations=1, gpus=1):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -1200,8 +1412,13 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     modes, an empty sequence, and video=True with more than one mode are a ValueError before anything is loaded.
 
     iterations: k refinement rounds per step, or a sweep of counts, as in getResultsYcbAll: count k of a sweep writes under
-    <outdir>/iter<k>/ (then <mode>/ when modes are swept too)."""
+    <outdir>/iter<k>/ (then <mode>/ when modes are swept too).
+
+    gpus: the number of GPUs, as in getResultsYcbAll: whole videos shared out over min(gpus, videos) ranks, each decoding
+    decode_ahead frames ahead of its own steps and writing its videos' files; the return value and the files equal the
+    single-GPU run's."""
     from .eval_ycbineoat import OBJECTS
+    gpus = check_gpus(gpus)
     modes, sweep = precision_modes(precision, PRECISIONS)
     if video and len(modes) > 1:
         raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
@@ -1214,9 +1431,10 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     videos = ycbineoat_videos(ycbineoat_dir)
     files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
     objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, modes[0])
-    eng, trackers = _one_pass_trackers([(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER,
-                                                                                 rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
-                                        for o, k in objects.items()], modes[0], 1)
+    entries = [(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
+               for o, k in objects.items()]
+    if gpus == 1:
+        eng, trackers = _one_pass_trackers(entries, modes[0], 1)
     sequences = {}
     for v, obj in videos:
         rgb_files, depth_files, gt_files = files[v]
@@ -1231,12 +1449,17 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
         os.makedirs(root[keys[0]], exist_ok=True)
         drawn = ('over', [([os.path.join(root[keys[0]], v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))])
                           for v, s in sequences.items()])
+    writes = [(_write_ycbineoat_video, root, v) for v in sequences]
+    if gpus == 1:
+        written = (fn(*args, tracked) for tracked, (fn, *args) in
+                   zip(_track_sequences(eng, trackers, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn), writes))
+    else:
+        written = _track_on_ranks(gpus, entries, modes[0], 1, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn,
+                                  writes)
     results = {key: {} for key in keys}
-    for tracked, v in zip(_track_sequences(eng, trackers, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn),
-                          sequences):
+    for poses, v in zip(written, sequences):
         for key in keys:
-            results[key][v] = tracked[key][:, 0]
-            write_video_poses(root[key], v, results[key][v])
+            results[key][v] = poses[key]
     return _sweep_results(results, variants, sweep, ksweep)
 
 
@@ -1363,7 +1586,13 @@ def main(argv=None):
                         '(1..8, default 1).  ycbv_all / ycbineoat_all also take a comma-separated list: every frame is tracked with '
                         'each K, K\'s tree written under <outdir>/iter<K>/, and --score adds a table of each variant\'s AUCs and drift '
                         'from K = 1')
+    parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
+                        'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
+    if args.gpus is not None and args.gpus < 1:
+        raise SystemExit('--gpus %d: the number of GPUs is at least 1' % args.gpus)
+    if args.gpus is not None and args.gpus > 1 and args.mode not in ('ycbv_all', 'ycbineoat_all'):
+        raise SystemExit('--gpus %d needs --mode ycbv_all or ycbineoat_all' % args.gpus)
     precision = cli_precision(args.precision, args.mode)
     iterations = cli_iterations(args.iterations, args.mode)
     if args.mode == 'ycbv_all':
@@ -1435,9 +1664,10 @@ def cli_iterations(text, mode):
 
 
 def _sweep_kw(args, precision, iterations):
-    """A one-pass driver's keyword arguments: video, precision and iterations, each passed only when given, so a run without them
-    makes the same call."""
+    """A one-pass driver's keyword arguments: video, precision, iterations and gpus, each passed only when given, so a run without
+    them makes the same call."""
     kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
+    kw.update({} if args.gpus is None else {'gpus': args.gpus})
     return dict(kw, **({} if iterations is None else {'iterations': iterations}))
 
 

@@ -33,11 +33,12 @@ def smooth(rng, shape, lo, hi, dtype):
     return np.clip(img, lo, hi).astype(dtype)
 
 
-def write_tree(tmp, frames, synth):
+def write_tree(tmp, frames, synth, seqs=SEQS):
+    """The data set of {sequence id: class ids} `seqs` under tmp -> (ycb dir, path templates, class ids)."""
     mio = importlib.import_module(PKG + '.mesh_io')
     rng = np.random.default_rng(0)
     ycb, cfg = os.path.join(tmp, 'ycb'), os.path.join(tmp, 'cfg')
-    classes = sorted(set(c for cls in SEQS.values() for c in cls))
+    classes = sorted(set(c for cls in seqs.values() for c in cls))
     K = synth.CAMERA_K
     cam = {'focalX': float(K[0, 0]), 'focalY': float(K[1, 1]), 'centerX': float(K[0, 2]), 'centerY': float(K[1, 2]), 'height': 480, 'width': 640}
     mean, std = synth.default_mean_std()
@@ -50,7 +51,7 @@ def write_tree(tmp, frames, synth):
         mio.save_ply_mesh(os.path.join(d, 'textured.ply'), synth.mesh(3, seed=c))
     for k in range(1, 22):
         os.makedirs(os.path.join(ycb, 'CADmodels', '%03d_obj' % k))
-    for seq, cls in SEQS.items():
+    for seq, cls in seqs.items():
         base = os.path.join(ycb, 'data_organized', '%04d' % seq)
         for sub in ['color', 'depth_filled'] + ['pose_gt/%d' % c for c in cls]:
             os.makedirs(os.path.join(base, sub))

@@ -34,7 +34,8 @@ def smooth(rng, shape, lo, hi, dtype):
     return np.clip(img, lo, hi).astype(dtype)
 
 
-def write_tree(tmp, frames, synth):
+def write_tree(tmp, frames, synth, videos=VIDEOS):
+    """The data set of {video folder: object} `videos` under tmp -> path templates."""
     mio = importlib.import_module(PKG + '.mesh_io')
     rng = np.random.default_rng(0)
     K = synth.CAMERA_K
@@ -49,7 +50,7 @@ def write_tree(tmp, frames, synth):
         mio.save_ply_mesh(os.path.join(d, 'textured.ply'), synth.mesh(3, seed=j + 1))
         os.makedirs(os.path.join(tmp, 'ycb', 'CADmodels', CAD[obj]))
         np.savetxt(os.path.join(tmp, 'ycb', 'CADmodels', CAD[obj], 'points.xyz'), synth.mesh(4, seed=j + 1)['pos'].astype(np.float64))
-    for v_i, v in enumerate(VIDEOS):
+    for v_i, v in enumerate(videos):
         base = os.path.join(tmp, 'data', v)
         for sub in ('rgb', 'depth_filled', 'annotated_poses'):
             os.makedirs(os.path.join(base, sub))
