@@ -412,6 +412,68 @@ int se3tn_eval_pairs(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA
 int se3tn_pair_loss(se3tn_ctx* ctx, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,
                     float* out_sums, void* stream);
 
+/* ---- validation under the reference's train-time augmentations (data_augmentation.py:48-121, 217-267) ----------------------- */
+
+/* The augmentation chain of the reference's train.py:85-92, in that order, on input B of each pair: HSVJitter, ChangeBright,
+ * GaussianNoise, GaussianBlur, BlackCover (any subset; each stage's flag is 0 or 1).  Every random value of pair i comes from
+ * Philox4x32-10 keyed by (seed, pair_index[i], draw slot) with the reference's distribution, so a pair's augmentation depends on
+ * (seed, pair index) alone; given the draws, the arithmetic is the reference classes' bit for bit (cv2 4.13 on x86-64 for the
+ * colour conversions and the blur).  DepthMissing, commented out in train.py, is refused (SE3TN_ERR_UNSUPPORTED). */
+typedef struct se3tn_augment {
+    uint64_t seed;
+    int32_t hsv_jitter, change_bright, gaussian_noise, gaussian_blur, black_cover, depth_missing;   /* stage flags */
+    double hsv_prob, hsv_noise[3];          /* HSVJitter(h_noise, s_noise, v_noise, prob): each channel's test, then U(-noise, noise) */
+    double bright_mag[2];                   /* ChangeBright(mag): always applied, U(mag[0], mag[1]) */
+    double noise_prob, noise_rgb, noise_depth;   /* GaussianNoise(rgb_noise, depth_noise, prob): std ~ U(0, noise), N(0, std) */
+    double blur_prob; int32_t blur_max_kernel, reserved;   /* GaussianBlur(max_kernel_size, prob): k = 2 randint(1, max//2 + 1) + 1 */
+    double cover_prob;                      /* BlackCover(prob) */
+} se3tn_augment;
+
+/* The per-pair draws, as se3tn_augment_draws writes them: SE3TN_AUG_PARAMS doubles per pair.
+ *   0 HSVJitter on, 1-3 its h / s / v branch outcomes (0 / 1), 4-6 their magnitudes, 7 ChangeBright on, 8 its factor,
+ *   9 / 10 GaussianNoise rgb branch / std, 11 / 12 depth branch / std, 13 / 14 GaussianBlur rgb branch / k, 15 / 16 depth branch / k,
+ *   17 BlackCover branch, 18 / 19 the accepted corner (u column, v row), 20 its quadrant (0 top left, 1 top right, 2 bottom left,
+ *   3 bottom right; -1: no cover), 21 corners drawn, 22 num_valid = sum of maskB's values, 23 maskB == 1 pixels left.
+ * A magnitude is drawn whether or not its branch is taken.  BlackCover draws at most SE3TN_AUG_MAX_CORNERS corners (the reference
+ * loops without end when no quadrant can keep half of num_valid); a pair that reaches the cap is left uncovered, quadrant -1. */
+#define SE3TN_AUG_PARAMS 24
+#define SE3TN_AUG_MAX_CORNERS 64
+
+/* se3tn_eval_pairs on augmented pairs: the first nine rows of arguments as se3tn_eval_pairs, then
+ *   segB uint8 (n,176,176) device, or NULL: BlackCover's maskB, or depthB > 100 without it (datasets.py:103-104)
+ *   pair_index int64 (n) device: each pair's index, the key of its draws (read on the device, so a graph replays across batches)
+ *   aug HOST: the chain; its values and whether segB is NULL join the step's key
+ *   out_rgbB uint8 (n,176,176,3), out_depthB uint16 (n,176,176) device, nullable: the augmented crops the step evaluated.
+ * Two more launches than se3tn_eval_pairs (the draws, then every stage in one pass over bands of rows) write the augmented B into
+ * out_rgbB / out_depthB or context-owned scratch (max_batch x 176 x 176 x 5 bytes, allocated by the first such call); the
+ * normalize launch reads it instead of rgbB / depthB, which are only read.  One CUDA graph, as se3tn_eval_pairs.  Refused on the
+ * host before anything is queued: everything se3tn_eval_pairs refuses, a NULL pair_index or aug, and a chain se3tn_augment_draws
+ * refuses, and out_rgbB / out_depthB overlapping an input or each other (the blur reads neighbouring rows of input B, so the
+ * augmentation cannot run in place). */
+int se3tn_eval_pairs_augmented(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                               const double* A_in_cam, const double* B_in_cam,
+                               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                               double trans_normalizer, double rot_normalizer, int precision,
+                               float* out_trans, float* out_rot, float* out_sq, double* out_labels, float* out_sums,
+                               const uint8_t* segB, const int64_t* pair_index, const se3tn_augment* aug,
+                               uint8_t* out_rgbB, uint16_t* out_depthB, void* stream);
+
+/* Exactly the draws se3tn_eval_pairs_augmented uses for pairs pair_index[0..n) (int64, device): out_params double
+ * (n, SE3TN_AUG_PARAMS) device; BlackCover's corner needs maskB: segB uint8 (n,176,176) or, NULL, depthB uint16 (n,176,176) > 100.
+ * out_noise_rgb double (n,176,176,3) and out_noise_depth double (n,176,176) device, nullable: GaussianNoise's N(0, std) fields at
+ * every element, whatever the branch and the mask.  Plain stream launches.  Refused on the host (SE3TN_ERR_INVALID unless noted):
+ * a NULL aug, pair_index, depthB or out_params, n <= 0 or n > max_batch, a stage flag other than 0 / 1, no stage enabled,
+ * depth_missing set (SE3TN_ERR_UNSUPPORTED), a probability outside [0, 1], blur_max_kernel / 2 outside {1, 2, 3} (k outside
+ * {3, 5, 7}), a non-finite magnitude or a negative noise magnitude, and an output overlapping an input or another output. */
+int se3tn_augment_draws(se3tn_ctx* ctx, const se3tn_augment* aug, const uint16_t* depthB, const uint8_t* segB, const int64_t* pair_index,
+                        int n, double* out_params, double* out_noise_rgb, double* out_noise_depth, void* stream);
+
+/* The augmented crops alone, as se3tn_eval_pairs_augmented forms them (its two augmentation launches): rgbB uint8 (n,176,176,3),
+ * depthB uint16 (n,176,176), segB as there, pair_index int64 (n), all device -> out_rgbB, out_depthB device (TrackDataset's
+ * augmented rgbB / depthB).  Plain stream launches; refusals as se3tn_augment_draws. */
+int se3tn_augment_crops(se3tn_ctx* ctx, const se3tn_augment* aug, const uint8_t* rgbB, const uint16_t* depthB, const uint8_t* segB,
+                        const int64_t* pair_index, int n, uint8_t* out_rgbB, uint16_t* out_depthB, void* stream);
+
 /* ---- held-out pairs from annotated frames: ProducerPurturb.generate (reference produce_train_pair_data.py:86-141) ------------- */
 
 /* crop_bbox with its segmentation plane (reference Utils.py:320-359 with seg): rgb and depth exactly as se3tn_crop_bbox cuts them, and

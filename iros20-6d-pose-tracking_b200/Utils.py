@@ -132,3 +132,15 @@ def fill_depth(depth, max_depth=2.0, extrapolate=False, blur_type='bilateral'):
     _, out_m = eng.fill_depth(torch.from_numpy(mm.astype(np.uint16)).to(eng.device), max_depth=max_depth, want_metres=True,
                               extrapolate=extrapolate, blur_type=blur_type)
     return out_m.cpu().numpy()
+
+
+class Compose(object):
+    """Utils.py:517-524: transforms applied in order.  A chain of data_augmentation's classes is what
+    TrackDataset(augmentations=...) takes; it runs on the device, not through this __call__."""
+    def __init__(self, transforms):
+        self.transforms = transforms
+
+    def __call__(self, img):
+        for t in self.transforms:
+            img = t(img)
+        return img

@@ -15,6 +15,8 @@ PROFILE_SLOTS = 22
 TRACE_TILES = 5184
 PAIR_MIN_SEG = 100
 MAX_REFINE_ITERATIONS = 8
+AUG_PARAMS = 24
+AUG_MAX_CORNERS = 64
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -56,6 +58,10 @@ SIGNATURES = {
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'se3tn_eval_pairs': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_pair_loss': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
+    'se3tn_eval_pairs_augmented': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                                        _vp, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_augment_draws': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    'se3tn_augment_crops': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_crop_bbox_seg': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_visibility': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_perturb_pairs': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -69,6 +75,16 @@ SIGNATURES = {
     'se3tn_set_profiling': (_i, [_vp, _i]),
     'se3tn_get_profile': (_i, [_vp, _vp]),
 }
+
+
+
+class Augment(C.Structure):
+    """se3tn_augment (include/se3tn.h)."""
+    _fields_ = [('seed', C.c_uint64), ('hsv_jitter', C.c_int32), ('change_bright', C.c_int32), ('gaussian_noise', C.c_int32),
+                ('gaussian_blur', C.c_int32), ('black_cover', C.c_int32), ('depth_missing', C.c_int32), ('hsv_prob', _d),
+                ('hsv_noise', _d * 3), ('bright_mag', _d * 2), ('noise_prob', _d), ('noise_rgb', _d), ('noise_depth', _d),
+                ('blur_prob', _d), ('blur_max_kernel', C.c_int32), ('reserved', C.c_int32), ('cover_prob', _d)]
+
 
 _lib = None
 

@@ -3,6 +3,7 @@
 #include "../../include/se3tn.h"
 #include "conv_common.h"
 #include "aux_kernels.h"
+#include "augment.h"
 #include "metrics.h"
 #include "overlay.h"
 #include "render.h"
@@ -15,6 +16,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <string>
@@ -198,6 +200,22 @@ struct F64Bits {   // a double held as its bits: a double member would make Step
 // compared with memcmp, are the key of the step's CUDA graph (run_step), and step_launches takes its arguments from nowhere
 // else: an argument missing here could not be read by the launches, so a replayed graph never runs on stale ones.
 enum : uint8_t { kStepTrack = 0, kStepEval = 1, kStepPairs = 2 };   // StepKey::kind
+// se3tn_eval_pairs_augmented's chain (se3tn_augment as the kernels take it); all zero in every other step
+struct AugKey {
+    uint64_t seed;
+    F64Bits hsv_prob, hsv_noise[3], bright_lo, bright_hi, noise_prob, noise_rgb, noise_depth, blur_prob, cover_prob;
+    int32_t stages;                            // bit 0 HSVJitter, 1 ChangeBright, 2 GaussianNoise, 3 GaussianBlur, 4 BlackCover; 0: none
+    int32_t blur_half_max;                     // max_kernel_size // 2
+    aug::Config config() const {
+        aug::Config c{};
+        c.seed = seed; c.hsv = stages & 1; c.bright = (stages >> 1) & 1; c.noise = (stages >> 2) & 1; c.blur = (stages >> 3) & 1;
+        c.cover = (stages >> 4) & 1; c.blur_half_max = blur_half_max;
+        c.hsv_prob = hsv_prob; for (int k = 0; k < 3; ++k) c.hsv_noise[k] = hsv_noise[k];
+        c.bright_lo = bright_lo; c.bright_hi = bright_hi; c.noise_prob = noise_prob; c.noise_rgb = noise_rgb; c.noise_depth = noise_depth;
+        c.blur_prob = blur_prob; c.cover_prob = cover_prob;
+        return c;
+    }
+};
 struct StepKey {
     uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
     uint8_t fill, fill_extrapolate;            // c->depth_fill when a track step is built (zero in a validation step)
@@ -205,6 +223,8 @@ struct StepKey {
     int32_t n, precision, first_wid;           // first_wid: the first track's weight set
     int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
     F64Bits K[4], tn, rn, fill_max_depth;
+    AugKey aug;                                // validation step: the augmentation of input B (aug.stages 0: none)
+    const uint8_t* aug_seg; const int64_t* pair_index; uint8_t* aug_rgb; uint16_t* aug_depth;   // its maskB (NULL: depthB > 100), keys, output
     const uint8_t* frame_rgb; const uint16_t* frame_depth; const double* object_width;   // track step
     const double* poses_in;                    // track step: the previous poses; validation step: A_in_cam
     const double* B_in_cam; const uint8_t* rgbB; const uint16_t* depthB;                 // validation step: inputs; pair step: rgbB / depthB outputs
@@ -234,6 +254,9 @@ struct se3tn_ctx {
     DevBuf<uint8_t> render_proj, render_unif; size_t render_proj_bytes = 0; int render_max_nv = 0;   // rasteriser workspace
     DevBuf<uint8_t> in_a; size_t in_a_bytes = 0;   // se3tn_track_render's input A, rgbA | depthA for max_batch tracks (allocated on first use)
     DevBuf<float> loss_sq; size_t loss_sq_floats = 0;   // se3tn_eval_pairs' loss terms when the caller wants none back: max_batch x 6 (allocated on first use)
+    // augmented validation steps: the draws (max_batch x SE3TN_AUG_PARAMS doubles), then augmented rgbB | depthB for max_batch
+    // pairs (allocated at that size by the first augmented call, never moved after)
+    DevBuf<uint8_t> aug; size_t aug_bytes = 0;
     DevBuf<int> pair_bbox; int pair_bbox_ints = 0;     // se3tn_perturb_pairs' crop windows, max_batch x 8 (allocated on first use, never moved)
     DevBuf<unsigned> cover_z; size_t cover_z_words = 0;   // se3tn_visibility's nearest-z planes, rows x H x W (grows on demand; never in a captured step)
     DevBuf<unsigned> append_done; int append_done_words = 0;   // se3tn_append_pairs' CTA counter, zero between launches (allocated on first use)
@@ -1202,6 +1225,71 @@ int run_tracks(se3tn_ctx* c, const Step& st, const HeadArgs& head, cudaStream_t 
     return SE3TN_OK;
 }
 
+// se3tn_eval_pairs_augmented's scratch: the draws, then augmented rgbB | depthB of max_batch pairs
+double* aug_params(se3tn_ctx* c) { return reinterpret_cast<double*>(c->aug.get()); }
+size_t aug_params_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * SE3TN_AUG_PARAMS * sizeof(double)); }
+uint8_t* aug_rgb(se3tn_ctx* c) { return c->aug.get() + aug_params_bytes(c->max_batch); }
+uint16_t* aug_depth(se3tn_ctx* c) {
+    return reinterpret_cast<uint16_t*>(aug_rgb(c) + align256(static_cast<size_t>(c->max_batch) * kImg * kImg * 3));
+}
+int reserve_aug(se3tn_ctx* c) {
+    const size_t img = static_cast<size_t>(c->max_batch) * kImg * kImg;
+    CU_TRY(c, grow(c->aug, c->aug_bytes, aug_params_bytes(c->max_batch) + align256(img * 3) + img * 2));
+    return SE3TN_OK;
+}
+
+// se3tn_augment checked and turned into a step's AugKey.  n: the pairs of the call (n > max_batch is refused).
+int check_augment(se3tn_ctx* c, const char* fn, const se3tn_augment* a, int n, AugKey* out) {
+    const std::string f(fn);
+    if (!a) return fail(c, SE3TN_ERR_INVALID, f + ": NULL augmentation");
+    if (a->depth_missing) return fail(c, SE3TN_ERR_UNSUPPORTED, f + ": DepthMissing is not supported (commented out in the reference's train.py)");
+    if (n <= 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n must be in [1, max_batch]");
+    const int32_t flags[5] = {a->hsv_jitter, a->change_bright, a->gaussian_noise, a->gaussian_blur, a->black_cover};
+    AugKey k{};
+    for (int i = 0; i < 5; ++i) {
+        if (flags[i] != 0 && flags[i] != 1) return fail(c, SE3TN_ERR_INVALID, f + ": stage flags must be 0 or 1");
+        k.stages |= flags[i] << i;
+    }
+    if (!k.stages) return fail(c, SE3TN_ERR_INVALID, f + ": no stage enabled (se3tn_eval_pairs evaluates the pairs as they are)");
+    const double probs[4] = {a->hsv_prob, a->noise_prob, a->blur_prob, a->cover_prob};
+    for (double p : probs)
+        if (!(p >= 0.0 && p <= 1.0)) return fail(c, SE3TN_ERR_INVALID, f + ": probabilities must lie in [0, 1]");
+    const double mags[5] = {a->hsv_noise[0], a->hsv_noise[1], a->hsv_noise[2], a->bright_mag[0], a->bright_mag[1]};
+    for (double m : mags)
+        if (!std::isfinite(m)) return fail(c, SE3TN_ERR_INVALID, f + ": magnitudes must be finite");
+    if (!(std::isfinite(a->noise_rgb) && std::isfinite(a->noise_depth) && a->noise_rgb >= 0.0 && a->noise_depth >= 0.0))
+        return fail(c, SE3TN_ERR_INVALID, f + ": noise magnitudes must be finite and >= 0");
+    const int half = a->blur_max_kernel / 2;
+    if (a->gaussian_blur && (a->blur_max_kernel < 0 || half < 1 || half > 3))
+        return fail(c, SE3TN_ERR_INVALID, f + ": blur_max_kernel " + std::to_string(a->blur_max_kernel) +
+                    " draws k outside {3, 5, 7}");
+    k.seed = a->seed;
+    k.hsv_prob = a->hsv_prob; for (int i = 0; i < 3; ++i) k.hsv_noise[i] = a->hsv_noise[i];
+    k.bright_lo = a->bright_mag[0]; k.bright_hi = a->bright_mag[1];
+    k.noise_prob = a->noise_prob; k.noise_rgb = a->noise_rgb; k.noise_depth = a->noise_depth;
+    k.blur_prob = a->blur_prob; k.cover_prob = a->cover_prob;
+    k.blur_half_max = a->gaussian_blur ? half : 0;
+    *out = k;
+    return SE3TN_OK;
+}
+
+// Every output of an augmentation call must be disjoint from its inputs: a CTA's reads of input B (the blur's halo rows) may come
+// after another CTA has written its own rows.  Pairs of (pointer, bytes).
+int check_disjoint(se3tn_ctx* c, const char* fn, std::initializer_list<std::pair<const void*, size_t>> outs,
+                   std::initializer_list<std::pair<const void*, size_t>> ins) {
+    auto overlap = [](const std::pair<const void*, size_t>& a, const std::pair<const void*, size_t>& b) {
+        const uintptr_t x = reinterpret_cast<uintptr_t>(a.first), y = reinterpret_cast<uintptr_t>(b.first);
+        return a.first && b.first && x < y + b.second && y < x + a.second;
+    };
+    for (auto o = outs.begin(); o != outs.end(); ++o) {
+        for (const auto& i : ins)
+            if (overlap(*o, i)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": an output overlaps an input (in-place augmentation is not supported)");
+        for (auto o2 = o + 1; o2 != outs.end(); ++o2)
+            if (overlap(*o, *o2)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": two outputs overlap");
+    }
+    return SE3TN_OK;
+}
+
 // The launches of one step on stream s, captured or not: render (if set) -> fill (if on) -> preprocess (track) or normalize
 // (validation) -> conv stack -> the fp32 pose update (track) or the loss (validation: pair_loss in fp32, the reduction of the
 // head's terms otherwise).  A track step that renders input A repeats render -> preprocess -> conv stack -> pose update
@@ -1254,6 +1342,14 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         head.tn = static_cast<float>(st.tn); head.rn = static_cast<float>(st.rn);
     } else {                                       // both depths are offset by A's z (reference datasets.py:136 -> data_augmentation.py:134-144)
         a.frame_rgb = st.rgbB; a.frame_depth = st.depthB; a.H = kImg; a.W = kImg; a.b_precropped = 1;
+        if (st.aug.stages) {                       // input B augmented first; the normalize launch waits for it (grid_dep_wait)
+            const aug::Config cfg = st.aug.config();
+            double* params = aug_params(c);
+            CU_TRY(c, launch_augment_draws(cfg, st.depthB, st.aug_seg, st.pair_index, st.n, params, s));
+            CU_TRY(c, launch_augment_pixels(cfg, st.rgbB, st.depthB, st.pair_index, params, st.n, st.aug_rgb, st.aug_depth, s));
+            c->launches += 2;
+            a.frame_rgb = st.aug_rgb; a.frame_depth = st.aug_depth;
+        }
         head.loss.poses_a = st.poses_in; head.loss.poses_b = st.B_in_cam; head.loss.tn = st.tn; head.loss.rn = st.rn;
         head.loss.sq = st.sq; head.loss.labels = st.labels;
     }
@@ -1336,6 +1432,39 @@ int run_step(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     return step_launches(c, st, s);
 }
 
+// se3tn_eval_pairs and se3tn_eval_pairs_augmented: `aug` carries the augmentation fields of the step (NULL: none).
+int eval_pairs_step(se3tn_ctx* c, const char* fn, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                    const double* A_in_cam, const double* B_in_cam, const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                    double tn, double rn, int precision, float* out_trans, float* out_rot, float* out_sq, double* out_labels,
+                    float* out_sums, const Step* aug, void* stream) {
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!rgbA || !depthA || !rgbB || !depthB || !A_in_cam || !B_in_cam) return fail(c, SE3TN_ERR_INVALID, f + ": null input");
+    if (!out_trans || !out_rot || !out_sums) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
+    bool multi = false;
+    int rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, false, &multi, precision);
+    if (rc) return rc;
+    if (n == 0) return fail(c, SE3TN_ERR_INVALID, f + ": n == 0 (the loss of no pairs is undefined)");
+    DeviceGuard guard(c->device);
+    const bool tensor = precision != SE3TN_PREC_FP32;
+    // allocated once, at max_batch pairs: nothing queued uses it before, and captured steps keep its address after
+    if (tensor && !out_sq) CU_TRY(c, grow(c->loss_sq, c->loss_sq_floats, static_cast<size_t>(c->max_batch) * 6));
+    Step st{};
+    if (aug) {
+        if ((rc = reserve_aug(c))) return rc;
+        st.aug = aug->aug; st.aug_seg = aug->aug_seg; st.pair_index = aug->pair_index;
+        st.aug_rgb = aug->aug_rgb ? aug->aug_rgb : aug_rgb(c);
+        st.aug_depth = aug->aug_depth ? aug->aug_depth : aug_depth(c);
+    }
+    st.kind = kStepEval; st.n = n; st.precision = precision; st.tn = tn; st.rn = rn; st.render_mode = -1;
+    st.wid_host = weight_ids_host; st.first_wid = weight_ids_host ? weight_ids_host[0] : 0; st.mixed = multi;
+    st.rgbA = rgbA; st.depthA = depthA; st.rgbB = rgbB; st.depthB = depthB; st.poses_in = A_in_cam; st.B_in_cam = B_in_cam;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot;
+    st.sq = out_sq ? out_sq : (tensor ? c->loss_sq.get() : nullptr); st.labels = out_labels; st.sums = out_sums;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1396,25 +1525,73 @@ int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, 
                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                      double tn, double rn, int precision,
                      float* out_trans, float* out_rot, float* out_sq, double* out_labels, float* out_sums, void* stream) {
+    return eval_pairs_step(c, "se3tn_eval_pairs", rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_host, weight_ids_dev, n, tn,
+                           rn, precision, out_trans, out_rot, out_sq, out_labels, out_sums, nullptr, stream);
+}
+
+int se3tn_eval_pairs_augmented(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                               const double* A_in_cam, const double* B_in_cam,
+                               const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                               double tn, double rn, int precision,
+                               float* out_trans, float* out_rot, float* out_sq, double* out_labels, float* out_sums,
+                               const uint8_t* segB, const int64_t* pair_index, const se3tn_augment* aug,
+                               uint8_t* out_rgbB, uint16_t* out_depthB, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
-    if (!rgbA || !depthA || !rgbB || !depthB || !A_in_cam || !B_in_cam) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null input");
-    if (!out_trans || !out_rot || !out_sums) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: null output");
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: unknown precision");
-    bool multi = false;
-    int rc = check_step(c, "se3tn_eval_pairs", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
-    if (rc) return rc;
-    if (n == 0) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs: n == 0 (the loss of no pairs is undefined)");
-    DeviceGuard guard(c->device);
-    const bool tensor = precision != SE3TN_PREC_FP32;
-    // allocated once, at max_batch pairs: nothing queued uses it before, and captured steps keep its address after
-    if (tensor && !out_sq) CU_TRY(c, grow(c->loss_sq, c->loss_sq_floats, static_cast<size_t>(c->max_batch) * 6));
+    if (!pair_index) return fail(c, SE3TN_ERR_INVALID, "se3tn_eval_pairs_augmented: NULL pair_index");
     Step st{};
-    st.kind = kStepEval; st.n = n; st.precision = precision; st.tn = tn; st.rn = rn; st.render_mode = -1;
-    st.wid_host = weight_ids_host; st.first_wid = weight_ids_host ? weight_ids_host[0] : 0; st.mixed = multi;
-    st.rgbA = rgbA; st.depthA = depthA; st.rgbB = rgbB; st.depthB = depthB; st.poses_in = A_in_cam; st.B_in_cam = B_in_cam;
-    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot;
-    st.sq = out_sq ? out_sq : (tensor ? c->loss_sq.get() : nullptr); st.labels = out_labels; st.sums = out_sums;
-    return run_step(c, st, static_cast<cudaStream_t>(stream));
+    int rc = check_augment(c, "se3tn_eval_pairs_augmented", aug, n, &st.aug);
+    if (rc) return rc;
+    const size_t px = static_cast<size_t>(n) * kImg * kImg;
+    if ((rc = check_disjoint(c, "se3tn_eval_pairs_augmented", {{out_rgbB, px * 3}, {out_depthB, px * 2}},
+                             {{rgbB, px * 3}, {depthB, px * 2}, {segB, px}, {pair_index, n * sizeof(int64_t)}})))
+        return rc;
+    st.aug_seg = segB; st.pair_index = pair_index; st.aug_rgb = out_rgbB; st.aug_depth = out_depthB;
+    return eval_pairs_step(c, "se3tn_eval_pairs_augmented", rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, weight_ids_host, weight_ids_dev,
+                           n, tn, rn, precision, out_trans, out_rot, out_sq, out_labels, out_sums, &st, stream);
+}
+
+int se3tn_augment_draws(se3tn_ctx* c, const se3tn_augment* aug, const uint16_t* depthB, const uint8_t* segB, const int64_t* pair_index,
+                        int n, double* out_params, double* out_noise_rgb, double* out_noise_depth, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    AugKey k;
+    int rc = check_augment(c, "se3tn_augment_draws", aug, n, &k);
+    if (rc) return rc;
+    if (!depthB || !pair_index || !out_params) return fail(c, SE3TN_ERR_INVALID, "se3tn_augment_draws: null argument");
+    const size_t px = static_cast<size_t>(n) * kImg * kImg;
+    if ((rc = check_disjoint(c, "se3tn_augment_draws", {{out_params, n * SE3TN_AUG_PARAMS * sizeof(double)}, {out_noise_rgb, px * 3 * sizeof(double)},
+                                                        {out_noise_depth, px * sizeof(double)}},
+                             {{depthB, px * 2}, {segB, px}, {pair_index, n * sizeof(int64_t)}})))
+        return rc;
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const aug::Config cfg = k.config();
+    c->launches = 0;
+    CU_TRY(c, launch_augment_draws(cfg, depthB, segB, pair_index, n, out_params, s));
+    CU_TRY(c, launch_augment_noise(cfg, pair_index, out_params, n, out_noise_rgb, out_noise_depth, s));
+    c->launches = out_noise_rgb || out_noise_depth ? 2 : 1;
+    return SE3TN_OK;
+}
+
+int se3tn_augment_crops(se3tn_ctx* c, const se3tn_augment* aug, const uint8_t* rgbB, const uint16_t* depthB, const uint8_t* segB,
+                        const int64_t* pair_index, int n, uint8_t* out_rgbB, uint16_t* out_depthB, void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    AugKey k;
+    int rc = check_augment(c, "se3tn_augment_crops", aug, n, &k);
+    if (rc) return rc;
+    if (!rgbB || !depthB || !pair_index || !out_rgbB || !out_depthB) return fail(c, SE3TN_ERR_INVALID, "se3tn_augment_crops: null argument");
+    const size_t px = static_cast<size_t>(n) * kImg * kImg;
+    if ((rc = check_disjoint(c, "se3tn_augment_crops", {{out_rgbB, px * 3}, {out_depthB, px * 2}},
+                             {{rgbB, px * 3}, {depthB, px * 2}, {segB, px}, {pair_index, n * sizeof(int64_t)}})))
+        return rc;
+    DeviceGuard guard(c->device);
+    if ((rc = reserve_aug(c))) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const aug::Config cfg = k.config();
+    c->launches = 0;
+    CU_TRY(c, launch_augment_draws(cfg, depthB, segB, pair_index, n, aug_params(c), s));
+    CU_TRY(c, launch_augment_pixels(cfg, rgbB, depthB, pair_index, aug_params(c), n, out_rgbB, out_depthB, s));
+    c->launches = 2;
+    return SE3TN_OK;
 }
 
 int se3tn_pair_loss(se3tn_ctx* c, const float* trans, const float* rot, const double* trans_label, const double* rot_label, int n,

@@ -2,9 +2,10 @@
 processData and processPredict (datasets.py:115-175) with the same signatures and return structure, executed by libse3tn
 kernels (K0 normalisation, K5 so(3) log, K6 pose update, the crop kernel's nearest-neighbour resize).
 
-Train-time transforms are out of scope: pretransforms / augmentations must be None, as Tracker passes them (predict.py:191).
-The reference's validation set is built WITH its random augmentations (train.py:132), so its validation loss is a random
-variable; here the loss is that of the clean pairs.
+pretransforms must be None, as Tracker passes them (predict.py:191).  augmentations may be None or a Utils.Compose of
+data_augmentation's classes in train.py:85-92's order (the reference builds its validation set with that chain, train.py:132):
+input B is then augmented on the device, every draw keyed by (augment_seed, the pair's index in the sorted file list), so the
+augmented loss is reproducible where the reference's is a random variable (DESIGN §9).
 
 One deliberate difference: the reference derives a pair's other file names by str.replace on the WHOLE path of its rgbA file
 (``path.replace('A', 'B')`` for rgbB, datasets.py:76), which also rewrites every 'A' in the directory names.  Here every
@@ -20,15 +21,18 @@ import torch
 class TrackDataset:
     def __init__(self, root, mode, images_mean, images_std, pretransforms=None, augmentations=None,
                  posttransforms=None, dataset_info=None, trans_normalizer=0.03, rot_normalizer=5 * np.pi / 180,
-                 engine=None, weight_id=0, precision='bf16x3'):
-        if pretransforms is not None or augmentations is not None:
-            raise NotImplementedError('train-time transforms are out of scope (inference passes None, predict.py:191)')
+                 engine=None, weight_id=0, precision='bf16x3', augment_seed=0):
+        if pretransforms is not None:
+            raise NotImplementedError('pretransforms are out of scope (inference passes None, predict.py:191)')
+        from .data_augmentation import chain_config
+        self.augment_seed = int(augment_seed)
+        self.augment = chain_config(augmentations, self.augment_seed) if augmentations is not None else None
         self.root = root
         self.mode = mode
         self.images_mean = np.asarray(images_mean)
         self.images_std = np.asarray(images_std)
         self.pretransforms = None
-        self.augmentations = None
+        self.augmentations = augmentations
         # The reference composes OffsetDepth -> NormalizeChannels -> ToTensor here; that chain is
         # what the K0 kernel implements, so the object passed in is only kept for introspection.
         self.posttransforms = posttransforms
@@ -65,8 +69,25 @@ class TrackDataset:
         if maskB is None:
             maskB = (depthB > 100).astype(np.uint8)
         assert np.sum(maskB) > 0, 'index={}'.format(index)
+        if self.augment is not None:
+            rgbB, depthB, maskB = self._augment_item(index, rgbB, depthB, maskB)
         data, target, rgbA, rgbB, maskA, maskB = self.processData(rgbA, depthA, p['A_in_cam'], rgbB, depthB, p['B_in_cam'], maskB)
         return data, target, p['A_in_cam'], p['B_in_cam'], rgbA, rgbB, maskA, maskB
+
+    def _augment_item(self, index, rgbB, depthB, maskB):
+        """The augmentation chain on one pair's B on the device (se3tn_augment_crops), BlackCover's corner applied to maskB too."""
+        eng = self.engine
+        dev = eng.device
+        seg = torch.from_numpy(segB_plane(maskB)[None]).to(dev)
+        dB, idx = self._u16(depthB, dev), torch.tensor([index], dtype=torch.int64, device=dev)
+        r, d = eng.augment_crops(self.augment, self._u8(rgbB, dev), dB, idx, segB=seg)
+        params, _, _ = eng.augment_draws(self.augment, dB, idx, segB=seg)
+        p = params[0].cpu().numpy()
+        maskB = np.array(maskB, copy=True)
+        if p[17] and p[20] >= 0:                         # the accepted cover: the quadrant of corner (u, v), include/se3tn.h
+            u, v, q = int(p[18]), int(p[19]), int(p[20])
+            maskB[(slice(None, v) if q < 2 else slice(v, None)), (slice(None, u) if q % 2 == 0 else slice(u, None))] = 0
+        return r[0].cpu().numpy(), d[0].cpu().numpy(), maskB
 
     @property
     def engine(self):
@@ -115,6 +136,17 @@ class TrackDataset:
     @staticmethod
     def _u16(a, dev):
         return torch.from_numpy(np.ascontiguousarray(a).astype(np.uint16)[None]).to(dev)
+
+
+def segB_plane(maskB):
+    """BlackCover's maskB as the device takes it: a uint8 image (segB, or depthB > 100 as uint8).  A 16-bit segB is refused: the
+    reference's cover test would compare its values before and after a uint8 cast."""
+    m = np.asarray(maskB)
+    if m.dtype == np.bool_:
+        m = m.astype(np.uint8)
+    if m.dtype != np.uint8 or m.shape != (176, 176):
+        raise ValueError('augmentation needs maskB as a uint8 176 x 176 image (segB or depthB > 100), not %s %s' % (m.dtype, m.shape))
+    return np.ascontiguousarray(m)
 
 
 def pair_paths(rgbA_path):

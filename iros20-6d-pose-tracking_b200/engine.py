@@ -347,12 +347,17 @@ class Engine:
     # ------------------------------------------------------------------ checkpoint validation
     def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
                    weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', want_terms=False, want_labels=False,
-                   out_trans=None, out_rot=None, out_sums=None, out_sq=None, out_labels=None):
+                   out_trans=None, out_rot=None, out_sums=None, out_sq=None, out_labels=None, augment=None, segB=None,
+                   pair_index=None, out_rgbB=None, out_depthB=None):
         """The loss of n ready-made pairs in one step (se3tn_eval_pairs): processData's post-transforms, the network in eval mode
         and Se3TrackNet.loss's terms, enqueued on the current stream.  rgbA / rgbB uint8 (n,176,176,3), depthA / depthB uint16
         (n,176,176), A_in_cam / B_in_cam float64 (n,4,4), all contiguous CUDA tensors.  -> (trans (n,3), rot (n,3), sums (2,)
         float32: the summed translation / rotation squared errors, sq (n,6) float32 or None, labels (n,6) float64 or None).
-        MSE = sums / (3 n).  Pass out_* tensors to keep the step's addresses, and so its CUDA graph, across calls."""
+        MSE = sums / (3 n).  Pass out_* tensors to keep the step's addresses, and so its CUDA graph, across calls.
+
+        augment: an se3tn_augment (augment_config) to evaluate input B under the reference's train-time augmentations
+        (se3tn_eval_pairs_augmented): pair_index int64 (n) CUDA tensor, each pair's index (the key of its draws), segB uint8
+        (n,176,176) CUDA tensor or None (maskB = depthB > 100); out_rgbB / out_depthB receive the augmented crops when given."""
         n = int(A_in_cam.shape[0])
         for name, t, dt, shape in (('rgbA', rgbA, torch.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)), ('rgbB', rgbB, torch.uint8, (n, IMAGE_SIZE, IMAGE_SIZE, 3)),
                                    ('depthA', depthA, torch.uint16, (n, IMAGE_SIZE, IMAGE_SIZE)), ('depthB', depthB, torch.uint16, (n, IMAGE_SIZE, IMAGE_SIZE)),
@@ -377,12 +382,76 @@ class Engine:
                 raise ValueError('eval_pairs: weight_ids_host must have one entry per pair')
             if weight_ids_dev is None:
                 weight_ids_dev = torch.from_numpy(wh).to(self.device)
-        _lib.check(self.lib.se3tn_eval_pairs(self._ctx, _ptr(rgbA), _ptr(depthA), _ptr(rgbB), _ptr(depthB), _ptr(A_in_cam), _ptr(B_in_cam),
-                                             wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0), _ptr(weight_ids_dev), n,
-                                             float(trans_normalizer), float(rot_normalizer), PREC[precision],
-                                             _ptr(out_trans), _ptr(out_rot), _ptr(out_sq), _ptr(out_labels), _ptr(out_sums),
-                                             _stream(self.device)), self._ctx)
+        args = (self._ctx, _ptr(rgbA), _ptr(depthA), _ptr(rgbB), _ptr(depthB), _ptr(A_in_cam), _ptr(B_in_cam),
+                wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0), _ptr(weight_ids_dev), n,
+                float(trans_normalizer), float(rot_normalizer), PREC[precision],
+                _ptr(out_trans), _ptr(out_rot), _ptr(out_sq), _ptr(out_labels), _ptr(out_sums))
+        if augment is None:
+            if segB is not None or pair_index is not None or out_rgbB is not None or out_depthB is not None:
+                raise ValueError('eval_pairs: segB, pair_index and out_rgbB / out_depthB go with augment')
+            _lib.check(self.lib.se3tn_eval_pairs(*args, _stream(self.device)), self._ctx)
+        else:
+            self._check_augment_inputs(n, segB, pair_index, out_rgbB=out_rgbB, out_depthB=out_depthB)
+            _lib.check(self.lib.se3tn_eval_pairs_augmented(*args, _ptr(segB), _ptr(pair_index), C.byref(augment), _ptr(out_rgbB),
+                                                           _ptr(out_depthB), _stream(self.device)), self._ctx)
         return out_trans, out_rot, out_sums, out_sq, out_labels
+
+    # ------------------------------------------------------------------ augmentation (se3tn_augment)
+    @staticmethod
+    def augment_config(seed=0, hsv=None, bright=None, noise=None, blur=None, cover=None):
+        """An se3tn_augment: each stage None (off) or a dict of its arguments -- hsv (h, s, v, prob), bright (lo, hi), noise
+        (rgb, depth, prob), blur (max_kernel, prob), cover (prob).  data_augmentation.chain_config builds it from the reference's
+        classes."""
+        a = _lib.Augment()
+        a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        if hsv is not None:
+            a.hsv_jitter = 1; a.hsv_prob = hsv['prob']
+            for k, c in enumerate('hsv'):
+                a.hsv_noise[k] = hsv[c]
+        if bright is not None:
+            a.change_bright = 1; a.bright_mag[0] = bright['lo']; a.bright_mag[1] = bright['hi']
+        if noise is not None:
+            a.gaussian_noise = 1; a.noise_rgb = noise['rgb']; a.noise_depth = noise['depth']; a.noise_prob = noise['prob']
+        if blur is not None:
+            a.gaussian_blur = 1; a.blur_max_kernel = int(blur['max_kernel']); a.blur_prob = blur['prob']
+        if cover is not None:
+            a.black_cover = 1; a.cover_prob = cover['prob']
+        return a
+
+    def augment_draws(self, augment, depthB, pair_index, segB=None, want_noise=False):
+        """The draws eval_pairs(augment=...) uses for these pairs (se3tn_augment_draws): depthB uint16 (n,176,176), pair_index
+        int64 (n), segB uint8 (n,176,176) or None, CUDA tensors -> (params float64 (n, AUG_PARAMS), noise_rgb float64 (n,176,176,3),
+        noise_depth float64 (n,176,176)), the noise fields None without want_noise."""
+        n = int(pair_index.shape[0])
+        self._check_augment_inputs(n, segB, pair_index, depthB=depthB)
+        params = torch.empty(n, _lib.AUG_PARAMS, dtype=torch.float64, device=self.device)
+        nr = torch.empty(n, IMAGE_SIZE, IMAGE_SIZE, 3, dtype=torch.float64, device=self.device) if want_noise else None
+        nd = torch.empty(n, IMAGE_SIZE, IMAGE_SIZE, dtype=torch.float64, device=self.device) if want_noise else None
+        _lib.check(self.lib.se3tn_augment_draws(self._ctx, C.byref(augment), _ptr(depthB), _ptr(segB), _ptr(pair_index), n, _ptr(params),
+                                                _ptr(nr), _ptr(nd), _stream(self.device)), self._ctx)
+        return params, nr, nd
+
+    def augment_crops(self, augment, rgbB, depthB, pair_index, segB=None, out_rgbB=None, out_depthB=None):
+        """The augmented input B of these pairs, as eval_pairs(augment=...) forms it (se3tn_augment_crops): CUDA tensors as
+        augment_draws plus rgbB uint8 (n,176,176,3) -> (rgbB, depthB) augmented."""
+        n = int(pair_index.shape[0])
+        out_rgbB = torch.empty(n, IMAGE_SIZE, IMAGE_SIZE, 3, dtype=torch.uint8, device=self.device) if out_rgbB is None else out_rgbB
+        out_depthB = torch.empty(n, IMAGE_SIZE, IMAGE_SIZE, dtype=torch.uint16, device=self.device) if out_depthB is None else out_depthB
+        self._check_augment_inputs(n, segB, pair_index, rgbB=rgbB, depthB=depthB, out_rgbB=out_rgbB, out_depthB=out_depthB)
+        _lib.check(self.lib.se3tn_augment_crops(self._ctx, C.byref(augment), _ptr(rgbB), _ptr(depthB), _ptr(segB), _ptr(pair_index), n,
+                                                _ptr(out_rgbB), _ptr(out_depthB), _stream(self.device)), self._ctx)
+        return out_rgbB, out_depthB
+
+    def _check_augment_inputs(self, n, segB, pair_index, **images):
+        img = (n, IMAGE_SIZE, IMAGE_SIZE)
+        if pair_index is None:
+            raise ValueError('augmentation needs pair_index: the int64 index of each pair, the key of its draws')
+        self._check_dev('pair_index', pair_index, torch.int64, (n,))
+        if segB is not None:
+            self._check_dev('segB', segB, torch.uint8, img)
+        for name, t in images.items():
+            if t is not None:
+                self._check_dev(name, t, torch.uint8 if 'rgb' in name else torch.uint16, img + ((3,) if 'rgb' in name else ()))
 
     def pair_loss(self, trans, rot, trans_label, rot_label, out_sums=None):
         """Se3TrackNet.loss's sums on existing predictions (se3tn_pair_loss): float32 (n,3) predictions, float64 (n,3) labels,

@@ -10,12 +10,17 @@ staging sets, so decoding step k+1 overlaps step k on the GPU.  A batch larger t
 are added in order.  The pairs are taken in file order (the reference's validation loader does not shuffle, train.py:143-149).
 
     python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
-                                 [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200]
+                                 [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200] [--augment config.yml [--seed S]]
     python -m <package>.problems --ycb_dir DIR --class_ids all|3,5 --ckpt_dir TPL --mean_std_path TPL --train_data_path TPL
                                  --model_path TPL [--num_sample 10] [--seed 0] [--precision MODE|all] [--batch_size 200] [--max_batch 200]
 
 The second form scores every class's checkpoint on the perturbed pairs of the YCB-Video key frames in one pass (validate_ycbv):
 bit-identical to `produce_train_pair_data --mode ycbv` followed by the first form on each class's folder, without the files.
+
+--augment evaluates the first form under the reference's train-time augmentations (train.py:85-92, built from config.yml's
+data_augmentation block), as the reference's own validation loss is computed: input B of every pair is augmented inside the
+validation step (se3tn_eval_pairs_augmented), each pair's draws keyed by (--seed, its index in the sorted file list), so every
+mode of --precision all sees the same augmented pairs.
 """
 import argparse
 import contextlib
@@ -25,7 +30,7 @@ import random
 import numpy as np
 import torch
 
-from .datasets import TrackDataset, read_pair, resize_pair
+from .datasets import TrackDataset, read_pair, resize_pair, segB_plane
 from .engine import PREC, IMAGE_SIZE
 from .staging import StagingRing
 
@@ -117,9 +122,12 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
     img = (IMAGE_SIZE, IMAGE_SIZE)
 
     # the pinned sets decode step k+1 while step k runs; the one device set is what the steps read (uploads ordered on the stream)
-    ring = StagingRing(dict(rgbA=((cap,) + img + (3,), torch.uint8), depthA=((cap,) + img, torch.uint16),
-                            rgbB=((cap,) + img + (3,), torch.uint8), depthB=((cap,) + img, torch.uint16),
-                            poses=((cap, 2, 4, 4), torch.float64)), 2, dev)
+    augment = getattr(dataset, 'augment', None)
+    planes = dict(rgbA=((cap,) + img + (3,), torch.uint8), depthA=((cap,) + img, torch.uint16),
+                  rgbB=((cap,) + img + (3,), torch.uint8), depthB=((cap,) + img, torch.uint16), poses=((cap, 2, 4, 4), torch.float64))
+    if augment is not None:                                 # BlackCover's maskB: segB, or depthB > 100 where a pair has none
+        planes['segB'] = ((cap,) + img, torch.uint8)
+    ring = StagingRing(planes, 2, dev)
     d = ring.dev
     A_in_cam, B_in_cam = torch.empty(cap, 4, 4, dtype=torch.float64, device=dev), torch.empty(cap, 4, 4, dtype=torch.float64, device=dev)
     out_trans, out_rot = torch.empty(cap, 3, dtype=torch.float32, device=dev), torch.empty(cap, 3, dtype=torch.float32, device=dev)
@@ -129,6 +137,9 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
     ids_host = np.full(cap, wid, dtype=np.int32) if wid != 0 else None
     ids_dev = torch.from_numpy(ids_host).to(dev) if ids_host is not None else None
     tn, rn = dataset.trans_normalizer, dataset.rot_normalizer
+    if augment is not None:                                 # each step's pair indices, copied into one buffer: one graph for every step
+        all_index = torch.arange(len(files), dtype=torch.int64, device=dev)
+        pair_index = torch.empty(cap, dtype=torch.int64, device=dev)
 
     def decode_into(h, j, path):
         """One pair into row j of staging set h; a pair stored at another size comes back whole for the device resize."""
@@ -141,6 +152,8 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
             raise AssertionError('%s: the pair has an empty maskB (datasets.py:104)' % path)
         for k in ('rgbA', 'depthA', 'rgbB', 'depthB'):
             h[k].numpy()[j] = p[k]
+        if augment is not None:
+            h['segB'].numpy()[j] = segB_plane(maskB)
         return None
 
     items = [[(decode_into, j, files[s + j]) for j in range(e - s)] for _, s, e in steps]
@@ -158,13 +171,23 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
                 if mask_sum <= 0:
                     raise AssertionError('%s: the pair has an empty maskB (datasets.py:104)' % files[s + j])
                 d['rgbA'][j].copy_(rA); d['depthA'][j].copy_(dA); d['rgbB'][j].copy_(rB); d['depthB'][j].copy_(dB)
+                if augment is not None:
+                    if seg is not None and seg.dtype != torch.uint8:
+                        raise ValueError('%s: augmentation needs segB as an 8-bit image, not %s' % (files[s + j], seg.dtype))
+                    d['segB'][j].copy_(seg if seg is not None else (dB.to(torch.int32) > 100).to(torch.uint8))
+            aug = {}
+            if augment is not None:
+                pair_index[:n].copy_(all_index[s:e])
+                aug = dict(augment=augment, segB=d['segB'][:n], pair_index=pair_index[:n])
             if precision == 'fp8' and k == 0:              # the set's activation scales from the first validation batch
-                eng.calibrate_fp8_pairs(d['rgbA'][:n], d['depthA'][:n], d['rgbB'][:n], d['depthB'][:n], A_in_cam[:n],
-                                        ids_host[:n] if ids_host is not None else None)
+                rB, dB = d['rgbB'][:n], d['depthB'][:n]
+                if augment is not None and eng.fp8_scales(wid) is None:   # as the steps will see it: input B augmented
+                    rB, dB = eng.augment_crops(augment, rB, dB, pair_index[:n], segB=d['segB'][:n])
+                eng.calibrate_fp8_pairs(d['rgbA'][:n], d['depthA'][:n], rB, dB, A_in_cam[:n], ids_host[:n] if ids_host is not None else None)
             eng.eval_pairs(d['rgbA'][:n], d['depthA'][:n], d['rgbB'][:n], d['depthB'][:n], A_in_cam[:n], B_in_cam[:n], tn, rn,
                            weight_ids_host=ids_host[:n] if ids_host is not None else None,
                            weight_ids_dev=ids_dev[:n] if ids_dev is not None else None, precision=precision,
-                           out_trans=out_trans[:n], out_rot=out_rot[:n], out_sums=out_sums)
+                           out_trans=out_trans[:n], out_rot=out_rot[:n], out_sums=out_sums, **aug)
             all_sums[k].copy_(out_sums)
             if preds is not None:
                 preds[s:e, :3].copy_(out_trans[:n]); preds[s:e, 3:].copy_(out_rot[:n])
@@ -402,13 +425,18 @@ def main(argv=None):
     ap.add_argument('--train_data_path', help='--ycb_dir: path template; dataset_info.yml is read from its ../')
     ap.add_argument('--model_path', help='--ycb_dir: path template of each class\'s mesh')
     ap.add_argument('--num_sample', type=int, default=10, help='--ycb_dir: perturbations drawn per annotated class and key frame')
-    ap.add_argument('--seed', type=int, default=0, help='--ycb_dir: seed of random and np.random before the first draw')
+    ap.add_argument('--seed', type=int, default=0, help='--ycb_dir: seed of random and np.random before the first draw; '
+                                                        '--augment: the seed of every pair\'s augmentation draws')
+    ap.add_argument('--augment', help="--val_dir: the reference's config.yml; its data_augmentation block builds train.py:85-92's "
+                                      "chain, applied to input B of every pair inside the validation step")
     ap.add_argument('--precision', default='bf16x3', choices=sorted(PREC) + ['all'])
     ap.add_argument('--batch_size', type=int, default=200, help='the validation loader batch size (train.py:146)')
     ap.add_argument('--max_batch', type=int, default=200, help='pairs per device step (a larger batch runs as several steps)')
     args = ap.parse_args(argv)
     modes = ALL_MODES if args.precision == 'all' else [args.precision]
     if args.ycb_dir:
+        if args.augment:
+            ap.error('--augment works with --val_dir only: the pairs of --ycb_dir are cut on the device without a segB for BlackCover')
         return _main_ycbv(ap, args, modes)
     if not (args.ckpt and args.mean_std_path and args.dataset_info):
         ap.error('--val_dir needs --ckpt, --mean_std_path and --dataset_info')
@@ -418,14 +446,20 @@ def main(argv=None):
         info = yaml.safe_load(f)
     mean = np.load(os.path.join(args.mean_std_path, 'mean.npy'))
     std = np.load(os.path.join(args.mean_std_path, 'std.npy'))
-    ds = TrackDataset(args.val_dir, 'val', mean, std, None, None, None, dataset_info=info,
-                      trans_normalizer=info['max_translation'], rot_normalizer=info['max_rotation'] * np.pi / 180)
+    augmentations = None
+    if args.augment:
+        from .data_augmentation import from_config
+        with open(args.augment) as f:
+            augmentations = from_config(yaml.safe_load(f))
+    ds = TrackDataset(args.val_dir, 'val', mean, std, None, augmentations, None, dataset_info=info,
+                      trans_normalizer=info['max_translation'], rot_normalizer=info['max_rotation'] * np.pi / 180, augment_seed=args.seed)
     loader = torch.utils.data.DataLoader(ds, batch_size=args.batch_size, shuffle=False, drop_last=False)
     ckpt = torch.load(args.ckpt, map_location='cpu')
     model = Se3TrackNet(image_size=int(info['resolution']), max_batch=min(args.max_batch, args.batch_size))
     model.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt)
     prob = Problem(model, None, loader, config={'loss_weights': {'trans': 1, 'rot': 1}})   # config.yml:13-15
-    print('%d pairs, batch %d, %s' % (len(ds), args.batch_size, torch.cuda.get_device_name(model.engine.device)))
+    print('%d pairs, batch %d, %s%s' % (len(ds), args.batch_size, torch.cuda.get_device_name(model.engine.device),
+                                        ", augmented (train.py's chain, seed %d)" % args.seed if args.augment else ''))
     _print_modes(modes, lambda m: prob.validation_losses(m, keep_predictions=len(modes) > 1), prob.loss_weights)
 
 
