@@ -1,4 +1,5 @@
-"""Device side of the per-layer check (oracle/layer_ref.py is the fp64 side), shared by the test files that run it.
+"""Device side of the per-layer check (oracle/layer_ref.py is the fp64 side, with oracle/fp16_ref.py and oracle/fp8_ref.py
+for those two modes' formats and layers), shared by the test files that run it, in all six precision modes.
 
 Before each call every conv output buffer (P1A ... H2; also Y1A / Y1B and H3 in the fp32 mode) is filled with 0xFF bytes,
 a NaN in every storage format, through the debug_buffer view into the Engine's own workspace.  After the call each checked
@@ -7,12 +8,14 @@ poison byte for byte.  The stem inputs X0A / X0B are never poisoned: their halo 
 
 Each case checks the 14 layers plus the head on a sample of its images (all of them up to 4; else first, last and two
 picked with a seed); `-s` prints a per-layer table of the worst ratio of each gate (gate 1 elementwise worst case, gate 2
-RMS; both pass at <= 1).
+RMS; both pass at <= 1).  In 'fp8' an image is checked with the activation scales of its own weight set.
 """
 import numpy as np
 import torch
 import torch.nn.functional as F
 
+import fp16_ref as H
+import fp8_ref as E
 import layer_ref as R
 
 CONV_OUT = ['P1A', 'P1B', 'T1', 'T2', 'U', 'CAT', 'F1', 'T4', 'F2', 'H1', 'H2']
@@ -28,6 +31,33 @@ def _out_bufs(prec):
     return CONV_OUT + (FP32_OUT if prec == 'fp32' else [])
 
 
+def image_bytes(buf, prec):
+    """Bytes one image of buffer `buf` occupies in mode prec: the buffer's image stride."""
+    if prec == 'fp16':
+        return H.image_bytes(buf)
+    if prec == 'fp8':
+        return E.image_bytes(buf)
+    return R.image_bytes(buf, R.buf_format(buf, prec))
+
+
+def decode(raw, buf, prec, scales=None):
+    """One image's bytes of buffer `buf` in mode prec -> layer_ref.Decoded; scales: the image's set's fp8 scales."""
+    if prec == 'fp16':
+        return H.decode(raw, buf)
+    if prec == 'fp8':
+        return E.decode(raw, buf, scales)
+    return R.decode(raw, buf, R.buf_format(buf, prec))
+
+
+def trunk_ksplit(n, prec):
+    """run_network's split-K choice for n images in mode prec."""
+    if prec == 'fp16':
+        return H.trunk_ksplit(n)
+    if prec == 'fp8':
+        return E.trunk_ksplit(n)
+    return R.trunk_ksplit(n, prec)
+
+
 def poison(eng, prec):
     for buf in _out_bufs(prec):
         buffer_bytes(eng, buf).fill_(0xFF)
@@ -38,7 +68,7 @@ def check_poison_outside(eng, prec, first, n):
     the poison, byte for byte."""
     bad = []
     for buf in _out_bufs(prec):
-        nb = R.image_bytes(buf, R.buf_format(buf, prec))
+        nb = image_bytes(buf, prec)
         u = buffer_bytes(eng, buf)
         for part in (u[:first * nb], u[(first + n) * nb:]):
             if part.numel() and not bool((part == 0xFF).all()):
@@ -62,23 +92,38 @@ def sample_images(first, n, seed, wids=None):
     return sorted({first, first + n - 1, *mid})
 
 
-def check_image(raw, prec, blob, ksplit, six):
-    """All 14 layers and the head of one image.  raw(buf) -> that image's bytes of buffer buf; blob: the image's fp32
-    weight blob; six: the (6,) trans ++ rot the call returned for it.  -> [(layer name, GateResult)]."""
+def _head_row(out, bound, six):
+    d = torch.as_tensor(np.asarray(six, dtype=np.float64))
+    finite = bool(torch.isfinite(d).all())
+    return ('head (trans, rot)', R.GateResult(float(((d - out).abs() / bound).max()) if finite else np.inf, 0.0, finite, 6))
+
+
+def check_image(raw, prec, blob, ksplit, six, scales=None):
+    """All 14 layers and the head of one image ('fp8': the layers fp8_ref checks).  raw(buf) -> that image's bytes of
+    buffer buf; blob: the image's fp32 weight blob; six: the (6,) trans ++ rot the call returned for it; scales: its set's
+    fp8 scales.  -> [(layer name, GateResult)]."""
     D = {}
 
     def dec(buf):
         if buf not in D:
-            D[buf] = R.decode(raw(buf), buf, R.buf_format(buf, prec))
+            D[buf] = decode(raw(buf), buf, prec, scales)
         return D[buf]
 
+    if prec == 'fp8':
+        return _check_image_fp8(dec, blob, scales, six)
+    if prec == 'fp16':
+        layer_ref = lambda li, x, w, b, **kw: H.layer_ref(li, x, w, b, **kw)
+        chained_ref = lambda li, x, *wb, **kw: H.chained_ref(li, x, *wb, **kw)
+    else:
+        layer_ref = lambda li, x, w, b, **kw: R.layer_ref(li, prec, x, w, b, **kw)
+        chained_ref = lambda li, x, *wb, **kw: R.chained_ref(li, prec, x, *wb, **kw)
     W = lambda li: R.layer_weights(blob, li)
     rows = []
 
     def one(li, out_value, res=None, **kw):
         L = R.LAYERS[li]
         w, b = W(li)
-        ref = R.layer_ref(li, prec, dec(L.inp), w, b, res=dec(res) if res else None, ksplit=ksplit, **kw)
+        ref = layer_ref(li, dec(L.inp), w, b, res=dec(res) if res else None, ksplit=ksplit, **kw)
         rows.append((L.name, R.gate(out_value, ref)))
         return ref
 
@@ -96,7 +141,7 @@ def check_image(raw, prec, blob, ksplit, six):
     one(3, cat[:64], res='P1A')
     # convB2.conv1's output T2 is overwritten by convB3.conv1: check convB2.conv2 through both layers from P1B
     w4, b4 = W(4); w5, b5 = W(5)
-    _, r5 = R.chained_ref(4, prec, dec('P1B'), w4, b4, w5, b5, res2=dec('P1B'), ksplit=ksplit)
+    _, r5 = chained_ref(4, dec('P1B'), w4, b4, w5, b5, res2=dec('P1B'), ksplit=ksplit)
     rows.append((R.LAYERS[4].name + ' + conv2', R.gate(dec('U').value, r5)))
     one(6, dec('T2').value)
     one(7, cat[64:], res='U')
@@ -113,11 +158,35 @@ def check_image(raw, prec, blob, ksplit, six):
     else:
         # H3 is never stored: the average pool is fused into the last conv's epilogue.  Check that layer through the head.
         w, b = W(13)
-        ref = R.layer_ref(13, prec, dec('H2'), w, b, res=dec('H1'), ksplit=ksplit, out_fmt='fp32')
+        ref = layer_ref(13, dec('H2'), w, b, res=dec('H1'), ksplit=ksplit, out_fmt='fp32')
         out, bound = R.head_ref(ref.y, ref.bound(), fcw, fcb, R.C_POOL_TC)
-    d = torch.as_tensor(np.asarray(six, dtype=np.float64))
-    finite = bool(torch.isfinite(d).all())
-    rows.append(('head (trans, rot)', R.GateResult(float(((d - out).abs() / bound).max()) if finite else np.inf, 0.0, finite, 6)))
+    rows.append(_head_row(out, bound, six))
+    return rows
+
+
+def _check_image_fp8(dec, blob, scales, six):
+    """The e4m3-written layers (the CAT writers and the six trunk layers) and the head of one image, plus the bf16 layers
+    that feed them."""
+    rows = []
+    cat = dec('CAT').value
+    for li in (0, 1, 2, 6):                         # the bf16 mode's layers, as they are
+        L = R.LAYERS[li]
+        w, b = R.layer_weights(blob, li)
+        out = dec({0: 'P1A', 1: 'P1B'}.get(li, L.out)).value
+        rows.append((L.name + ' (bf16)', R.gate(out, R.layer_ref(li, 'bf16', dec(L.inp), w, b))))
+    for li, part, res in ((3, cat[:64], 'P1A'), (7, cat[64:], 'U')):
+        w, b = R.layer_weights(blob, li)
+        rows.append((R.LAYERS[li].name + ' -> CAT e4m3', R.gate(part, E.layer_ref(li, dec(R.LAYERS[li].inp), w, b, scales, res=dec(res)))))
+    for li in range(8, 13):
+        L = R.LAYERS[li]
+        w, b = R.layer_weights(blob, li)
+        ref = E.layer_ref(li, dec(L.inp), w, b, scales, res=dec(L.res) if L.res else None)
+        rows.append((L.name, R.gate(dec(L.out).value, ref)))
+    w, b = R.layer_weights(blob, 13)                # H3 is never stored: the last layer through the head
+    ref = E.layer_ref(13, dec('H2'), w, b, scales, res=dec('H1'))
+    fcw, fcb = R.fc_weights(blob)
+    out, bound = R.head_ref(ref.y, ref.bound(), fcw, fcb, R.C_POOL_TC)
+    rows.append(_head_row(out, bound, six))
     return rows
 
 
@@ -137,30 +206,34 @@ def report(label, per_image):
 
 def run_case(eng, prec, first, n, call, wids, blobs, label, seed=0):
     """Poison, run `call` (-> trans (n,3), rot (n,3), feature or None), check the untouched images, then every layer of
-    the sampled ones.  wids: weight-set id per image of the call; blobs[id]: that set's fp32 weight blob."""
+    the sampled ones.  wids: weight-set id per image of the call; blobs[id]: that set's fp32 weight blob.  'fp8': each image
+    is decoded with eng.fp8_scales of its own set."""
     poison(eng, prec)
     trans, rot, feat = call()
     torch.cuda.synchronize()
     check_poison_outside(eng, prec, first, n)
+    scales = {int(w): eng.fp8_scales(int(w)) if prec == 'fp8' else None for w in wids}
     six = torch.cat((trans, rot), 1).cpu().numpy()
-    ks = R.trunk_ksplit(n, prec)
+    ks = trunk_ksplit(n, prec)
     if feat is not None:                           # the feature output is the F2 buffer through launch_nhwc_to_nchw, bit for bit
-        nb = R.image_bytes('F2', prec)
+        nb = image_bytes('F2', prec)
         f2 = buffer_bytes(eng, 'F2')[first * nb:(first + n) * nb].cpu().numpy()
         fc = feat.cpu().numpy()
         for j in range(n):
-            assert np.array_equal(R.decode(f2[j * nb:(j + 1) * nb], 'F2', prec).value, fc[j]), 'feature %d != decoded F2' % j
+            s = scales[int(wids[j])]
+            assert np.array_equal(decode(f2[j * nb:(j + 1) * nb], 'F2', prec, s).value, fc[j]), 'feature %d != decoded F2' % j
     per_image = []
     for i in sample_images(first, n, seed, wids):
         cache = {}
 
         def raw(buf, i=i):
-            nb = R.image_bytes(buf, R.buf_format(buf, prec))
+            nb = image_bytes(buf, prec)
             if buf not in cache:
                 cache[buf] = buffer_bytes(eng, buf)[i * nb:(i + 1) * nb].cpu().numpy()
             return cache[buf]
 
-        per_image.append((i, check_image(raw, prec, blobs[int(wids[i - first])], ks, six[i - first])))
+        w = int(wids[i - first])
+        per_image.append((i, check_image(raw, prec, blobs[w], ks, six[i - first], scales[w])))
     report('%s, %s, n = %d%s (ksplit %d)' % (label, prec, n, ', first = %d' % first if first else '', ks), per_image)
 
 
@@ -170,3 +243,17 @@ def track_inputs(synth, n, seed):
     poses = synth.raw_poses(n, seed=seed)
     rgbA, depthA = synth.rendered_views(n, poses, seed=seed)
     return rgb, depth, poses, rgbA, depthA
+
+
+def distinct_fp8_scales(eng, calibrated):
+    """Give every weight id of `calibrated` ({id < 256: its calibrated fp8 scales}) its own scale vector: the elementwise
+    maximum of the calibrated ones, doubled on e4m3 tensor k where bit k of the id is set.  Calibration rounds each scale
+    to a power of two, so sets of similar weights may share scales, and a kernel that read another image's set's scales
+    would then pass.  The maximum keeps every set's headroom and a larger scale only coarsens the quantisation; the
+    references read the engine's scales.  -> {id: the scales set}"""
+    base = np.max(np.stack([np.asarray(s, np.float32) for s in calibrated.values()]), axis=0)
+    out = {}
+    for w in calibrated:
+        out[w] = (base * 2.0 ** ((w >> np.arange(len(E.SCALE_NAMES))) & 1)).astype(np.float32)
+        eng.set_fp8_scales(out[w], w)
+    return out

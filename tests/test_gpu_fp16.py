@@ -2,8 +2,8 @@
 (oracle/fp16_ref.py), the latency mode's independence of n and of the other tracks' sets, the end-to-end 6-vector against
 the fp32 reference, saturation, and the refusal of a weight set outside fp16's range.
 
-Poisoning, image sampling and the per-layer tables `-s` prints come from tests/layer_harness.py; the fp16 formats (2 bytes
-per channel, so an image stride half of the 4-byte modes') and the per-layer references are here.
+The per-layer check (poisoning, image sampling, the tables `-s` prints) is tests/layer_harness.py's in the fp16 formats:
+2 bytes per channel, so an image stride half of the 4-byte modes'.
 """
 import ctypes
 import os
@@ -15,7 +15,7 @@ import torch
 import fp16_ref as H
 import layer_ref as R
 import se3_oracle as O
-from layer_harness import CONV_OUT, buffer_bytes, poison, report, sample_images, track_inputs
+from layer_harness import CONV_OUT, buffer_bytes, check_poison_outside, poison, run_case, track_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -47,87 +47,6 @@ def blobs(pkg, synth):
     return {0: pack(synth.make_state_dict(0)), 1: pack(synth.make_state_dict(1))}
 
 
-# ------------------------------------------------------------------------------------------- fp16 harness
-def check_poison_outside(eng, first, n):
-    bad = []
-    for buf in CONV_OUT:
-        nb = H.image_bytes(buf)
-        u = buffer_bytes(eng, buf)
-        for part in (u[:first * nb], u[(first + n) * nb:]):
-            if part.numel() and not bool((part == 0xFF).all()):
-                bad.append(buf)
-    assert not bad, 'written outside images [%d, %d): %s' % (first, first + n, bad)
-
-
-def check_image(raw, blob, ksplit, six):
-    """All 14 layers and the head of one image (layer_harness.check_image in the fp16 formats)."""
-    D = {}
-
-    def dec(buf):
-        if buf not in D:
-            D[buf] = H.decode(raw(buf), buf)
-        return D[buf]
-
-    W = lambda li: R.layer_weights(blob, li)
-    rows = []
-
-    def one(li, out_value, res=None):
-        w, b = W(li)
-        ref = H.layer_ref(li, dec(R.LAYERS[li].inp), w, b, res=dec(res) if res else None, ksplit=ksplit)
-        rows.append((R.LAYERS[li].name, R.gate(out_value, ref)))
-
-    cat = dec('CAT').value
-    one(0, dec('P1A').value)
-    one(1, dec('P1B').value)
-    one(2, dec('T1').value)
-    one(3, cat[:64], res='P1A')
-    w4, b4 = W(4); w5, b5 = W(5)
-    _, r5 = H.chained_ref(4, dec('P1B'), w4, b4, w5, b5, res2=dec('P1B'), ksplit=ksplit)
-    rows.append((R.LAYERS[4].name + ' + conv2', R.gate(dec('U').value, r5)))
-    one(6, dec('T2').value)
-    one(7, cat[64:], res='U')
-    one(8, dec('F1').value)
-    one(9, dec('T4').value)
-    one(10, dec('F2').value, res='F1')
-    one(11, dec('H1').value)
-    one(12, dec('H2').value)
-    w, b = W(13)                                      # H3 is never stored: the last layer through the head
-    ref = H.layer_ref(13, dec('H2'), w, b, res=dec('H1'), ksplit=ksplit, out_fmt='fp32')
-    fcw, fcb = R.fc_weights(blob)
-    out, bound = R.head_ref(ref.y, ref.bound(), fcw, fcb, R.C_POOL_TC)
-    d = torch.as_tensor(np.asarray(six, dtype=np.float64))
-    finite = bool(torch.isfinite(d).all())
-    rows.append(('head (trans, rot)', R.GateResult(float(((d - out).abs() / bound).max()) if finite else np.inf, 0.0, finite, 6)))
-    return rows
-
-
-def run_case(eng, first, n, call, wids, blobs, label, seed=0):
-    poison(eng, 'fp16')
-    trans, rot, feat = call()
-    torch.cuda.synchronize()
-    check_poison_outside(eng, first, n)
-    six = torch.cat((trans, rot), 1).cpu().numpy()
-    ks = H.trunk_ksplit(n)
-    if feat is not None:                              # the feature output is F2 through launch_nhwc_to_nchw, bit for bit
-        nb = H.image_bytes('F2')
-        f2 = buffer_bytes(eng, 'F2')[first * nb:(first + n) * nb].cpu().numpy()
-        fc = feat.cpu().numpy()
-        for j in range(n):
-            assert np.array_equal(H.decode(f2[j * nb:(j + 1) * nb], 'F2').value, fc[j]), 'feature %d != decoded F2' % j
-    per_image = []
-    for i in sample_images(first, n, seed, wids):
-        cache = {}
-
-        def raw(buf, i=i):
-            nb = H.image_bytes(buf)
-            if buf not in cache:
-                cache[buf] = buffer_bytes(eng, buf)[i * nb:(i + 1) * nb].cpu().numpy()
-            return cache[buf]
-
-        per_image.append((i, check_image(raw, blobs[int(wids[i - first])], ks, six[i - first])))
-    report('%s, fp16, n = %d%s (ksplit %d)' % (label, n, ', first = %d' % first if first else '', ks), per_image)
-
-
 def _t(eng):
     return lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(eng.device)
 
@@ -139,7 +58,7 @@ def test_fp16_forward_layers(synth, eng, blobs, n):
     CTA; 64: the full batch."""
     A, B = synth.tensor_pairs(n, seed=40 + n)
     Ad, Bd = A.to(eng.device), B.to(eng.device)
-    run_case(eng, 0, n, lambda: eng.forward(Ad, Bd, weight_id=0, precision='fp16', want_feature=True), [0] * n, blobs, 'forward', seed=n)
+    run_case(eng, 'fp16', 0, n, lambda: eng.forward(Ad, Bd, weight_id=0, precision='fp16', want_feature=True), [0] * n, blobs, 'forward', seed=n)
 
 
 def test_fp16_forward_many_waves(pkg, synth, blobs):
@@ -148,7 +67,7 @@ def test_fp16_forward_many_waves(pkg, synth, blobs):
     try:
         A, B = synth.tensor_pairs(250, seed=7)
         Ad, Bd = A.to(e.device), B.to(e.device)
-        run_case(e, 0, 250, lambda: e.forward(Ad, Bd, weight_id=0, precision='fp16'), [0] * 250, blobs, 'forward (max_batch 256)')
+        run_case(e, 'fp16', 0, 250, lambda: e.forward(Ad, Bd, weight_id=0, precision='fp16'), [0] * 250, blobs, 'forward (max_batch 256)')
     finally:
         e.close()
 
@@ -166,7 +85,7 @@ def test_fp16_forward_preprocessed_offset(synth, eng, blobs):
         eng.normalize(t(rgbA), t(depthA), t(rgbB), t(depthB), t(poses), precision='fp16', want_tensors=False)
         return eng.forward_preprocessed(3, weight_id=0, first=5, precision='fp16')
 
-    run_case(eng, 5, 3, call, [0] * 3, blobs, 'forward_preprocessed')
+    run_case(eng, 'fp16', 5, 3, call, [0] * 3, blobs, 'forward_preprocessed')
 
 
 def test_fp16_track_batch_per_image_weights(synth, eng, blobs):
@@ -185,9 +104,9 @@ def test_fp16_track_batch_per_image_weights(synth, eng, blobs):
                         precision='fp16', out_poses=out_p, out_trans=out_t, out_rot=out_r)
         return out_t, out_r, None
 
-    run_case(eng, 0, n, call, wid, blobs, 'track_batch, ids 0/1', seed=1)
+    run_case(eng, 'fp16', 0, n, call, wid, blobs, 'track_batch, ids 0/1', seed=1)
     P.copy_(t(synth.raw_poses(n, seed=6)))            # same addresses: the second call replays the captured graph
-    run_case(eng, 0, n, call, wid, blobs, 'track_batch graph replay, new poses', seed=2)
+    run_case(eng, 'fp16', 0, n, call, wid, blobs, 'track_batch graph replay, new poses', seed=2)
     assert eng.last_step_was_graph()
 
 
@@ -348,7 +267,7 @@ def test_fp16_refuses_weights_outside_its_range(pkg, synth):
                           weight_ids_host=wid, weight_ids_dev=t(wid), precision='fp16')
         assert ex.value.code == L.ERR_STATE and 'weight set 2' in str(ex.value)
         torch.cuda.synchronize()
-        check_poison_outside(e, 0, 0)                  # nothing was launched
+        check_poison_outside(e, 'fp16', 0, 0)          # nothing was launched
         tr, ro, _ = e.forward(Ad, Bd, weight_id=2, precision='bf16x3')
         assert bool(torch.isfinite(tr).all()) and bool(torch.isfinite(ro).all())
         tr, ro, _ = e.forward(Ad, Bd, weight_id=1, precision='fp16')

@@ -1,8 +1,8 @@
 """The 'fp8' mode on the H100: every e4m3-written layer checked ALONE against an fp64 conv of its own stored input
 (oracle/fp8_ref.py), the calibration against the bf16x3 buffers it reads, and the mode's state rules.
 
-Poisoning, image sampling and the per-layer tables `-s` prints come from tests/layer_harness.py; the fp8 formats of the
-buffers (bf16 up to U, e4m3 from CAT to H2) and the per-layer references are here.
+The per-layer check (poisoning, image sampling, the tables `-s` prints) is tests/layer_harness.py's in the fp8 formats of
+the buffers: bf16 up to U, e4m3 from CAT to H2.
 """
 import numpy as np
 import pytest
@@ -10,7 +10,7 @@ import torch
 
 import fp8_ref as E
 import layer_ref as R
-from layer_harness import CONV_OUT, buffer_bytes, report, sample_images, track_inputs
+from layer_harness import buffer_bytes, check_poison_outside, poison, run_case, track_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -41,86 +41,6 @@ def blobs(pkg, synth):
     return {0: pack(synth.make_state_dict(0)), 1: pack(synth.make_state_dict(1))}
 
 
-# ------------------------------------------------------------------------------------------- fp8-only harness
-def poison(eng):
-    for buf in CONV_OUT:
-        buffer_bytes(eng, buf).fill_(0xFF)
-
-
-def check_poison_outside(eng, first, n):
-    bad = []
-    for buf in CONV_OUT:
-        nb = E.image_bytes(buf)
-        u = buffer_bytes(eng, buf)
-        for part in (u[:first * nb], u[(first + n) * nb:]):
-            if part.numel() and not bool((part == 0xFF).all()):
-                bad.append(buf)
-    assert not bad, 'written outside images [%d, %d): %s' % (first, first + n, bad)
-
-
-def check_image(raw, blob, scales, six):
-    """The e4m3-written layers (the CAT writers and the six trunk layers) and the head of one image, plus the bf16 layers
-    that feed them.  -> [(layer name, GateResult)]"""
-    D = {}
-
-    def dec(buf):
-        if buf not in D:
-            D[buf] = E.decode(raw(buf), buf, scales)
-        return D[buf]
-
-    rows = []
-    cat = dec('CAT').value
-    for li in (0, 1, 2, 6):                           # the bf16 mode's layers, as they are
-        L = R.LAYERS[li]
-        w, b = R.layer_weights(blob, li)
-        out = dec({0: 'P1A', 1: 'P1B'}.get(li, L.out)).value
-        rows.append((L.name + ' (bf16)', R.gate(out, R.layer_ref(li, 'bf16', dec(L.inp), w, b))))
-    for li, part, res in ((3, cat[:64], 'P1A'), (7, cat[64:], 'U')):
-        w, b = R.layer_weights(blob, li)
-        rows.append((R.LAYERS[li].name + ' -> CAT e4m3', R.gate(part, E.layer_ref(li, dec(R.LAYERS[li].inp), w, b, scales, res=dec(res)))))
-    for li in range(8, 13):
-        L = R.LAYERS[li]
-        w, b = R.layer_weights(blob, li)
-        ref = E.layer_ref(li, dec(L.inp), w, b, scales, res=dec(L.res) if L.res else None)
-        rows.append((L.name, R.gate(dec(L.out).value, ref)))
-    w, b = R.layer_weights(blob, 13)                  # H3 is never stored: the last layer through the head
-    ref = E.layer_ref(13, dec('H2'), w, b, scales, res=dec('H1'))
-    fcw, fcb = R.fc_weights(blob)
-    out, bound = R.head_ref(ref.y, ref.bound(), fcw, fcb, R.C_POOL_TC)
-    d = torch.as_tensor(np.asarray(six, dtype=np.float64))
-    finite = bool(torch.isfinite(d).all())
-    rows.append(('head (trans, rot)', R.GateResult(float(((d - out).abs() / bound).max()) if finite else np.inf, 0.0, finite, 6)))
-    return rows
-
-
-def run_case(eng, first, n, call, wids, blobs, label, seed=0):
-    poison(eng)
-    trans, rot, feat = call()
-    torch.cuda.synchronize()
-    check_poison_outside(eng, first, n)
-    scales = {w: eng.fp8_scales(w) for w in set(int(x) for x in wids)}
-    six = torch.cat((trans, rot), 1).cpu().numpy()
-    if feat is not None:                              # F2 through launch_nhwc_to_nchw: code * s_F2, bit for bit
-        nb = E.image_bytes('F2')
-        f2 = buffer_bytes(eng, 'F2')[first * nb:(first + n) * nb].cpu().numpy()
-        fc = feat.cpu().numpy()
-        for j in range(n):
-            assert np.array_equal(E.decode(f2[j * nb:(j + 1) * nb], 'F2', scales[int(wids[j])]).value, fc[j]), 'feature %d' % j
-    per_image = []
-    for i in sample_images(first, n, seed, wids):
-        cache = {}
-
-        def raw(buf, i=i):
-            nb = E.image_bytes(buf)
-            if buf not in cache:
-                cache[buf] = buffer_bytes(eng, buf)[i * nb:(i + 1) * nb].cpu().numpy()
-            return cache[buf]
-
-        wid = int(wids[i - first])
-        per_image.append((i, check_image(raw, blobs[wid], scales[wid], six[i - first])))
-    report('%s, fp8, n = %d (ksplit %d)' % (label, n, E.trunk_ksplit(n)), per_image)
-
-
 # ------------------------------------------------------------------------------------------- layers
 @pytest.mark.parametrize('n', [1, 3, 4, 5, 13, 64])
 def test_fp8_forward_layers(synth, eng, blobs, n):
@@ -129,7 +49,7 @@ def test_fp8_forward_layers(synth, eng, blobs, n):
     A, B = synth.tensor_pairs(n, seed=40 + n)
     Ad, Bd = A.to(eng.device), B.to(eng.device)
     eng.calibrate_fp8(Ad, Bd, weight_id=0)
-    run_case(eng, 0, n, lambda: eng.forward(Ad, Bd, weight_id=0, precision='fp8', want_feature=True), [0] * n, blobs, 'forward', seed=n)
+    run_case(eng, 'fp8', 0, n, lambda: eng.forward(Ad, Bd, weight_id=0, precision='fp8', want_feature=True), [0] * n, blobs, 'forward', seed=n)
 
 
 def test_fp8_forward_many_waves(pkg, synth, blobs):
@@ -139,7 +59,7 @@ def test_fp8_forward_many_waves(pkg, synth, blobs):
         A, B = synth.tensor_pairs(250, seed=7)
         Ad, Bd = A.to(e.device), B.to(e.device)
         e.calibrate_fp8(Ad, Bd, weight_id=0)
-        run_case(e, 0, 250, lambda: e.forward(Ad, Bd, weight_id=0, precision='fp8'), [0] * 250, blobs, 'forward (max_batch 256)')
+        run_case(e, 'fp8', 0, 250, lambda: e.forward(Ad, Bd, weight_id=0, precision='fp8'), [0] * 250, blobs, 'forward (max_batch 256)')
     finally:
         e.close()
 
@@ -171,9 +91,9 @@ def test_fp8_track_batch_per_image_weights(synth, eng, blobs):
                         precision='fp8', out_poses=out_p, out_trans=out_t, out_rot=out_r)
         return out_t, out_r, None
 
-    run_case(eng, 0, n, call, wid, blobs, 'track_batch, ids 0/1', seed=1)
+    run_case(eng, 'fp8', 0, n, call, wid, blobs, 'track_batch, ids 0/1', seed=1)
     P.copy_(t(synth.raw_poses(n, seed=6)))
-    run_case(eng, 0, n, call, wid, blobs, 'track_batch graph replay, new poses', seed=2)
+    run_case(eng, 'fp8', 0, n, call, wid, blobs, 'track_batch graph replay, new poses', seed=2)
     assert eng.last_step_was_graph()
 
 
@@ -207,7 +127,7 @@ def test_fp8_state_rules(pkg, synth, blobs):
         Ad, Bd = A.to(e.device), B.to(e.device)
         assert e.fp8_scales(0) is None
         # no scales: SE3TN_ERR_STATE naming the id, nothing launched (the poisoned buffers stay)
-        poison(e)
+        poison(e, 'fp8')
         with pytest.raises(L.Se3tnError) as ex:
             e.forward(Ad, Bd, weight_id=0, precision='fp8')
         assert ex.value.code == L.ERR_STATE and 'weight set 0' in str(ex.value)
@@ -215,13 +135,13 @@ def test_fp8_state_rules(pkg, synth, blobs):
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(e.device)
         wid = np.array([1, 0, 1], np.int32)
         e.calibrate_fp8(Ad, Bd, weight_id=1)
-        poison(e)
+        poison(e, 'fp8')
         with pytest.raises(L.Se3tnError) as ex:
             e.track_batch(t(rgb), t(depth), synth.CAMERA_K, t(poses), t(np.full(n, 200.0)), t(rgbA), t(depthA), TN, RN,
                           weight_ids_host=wid, weight_ids_dev=t(wid), precision='fp8')
         assert ex.value.code == L.ERR_STATE and 'weight set 0' in str(ex.value)
         torch.cuda.synchronize()
-        check_poison_outside(e, 0, 0)
+        check_poison_outside(e, 'fp8', 0, 0)
         # set / get round-trip; invalid scales refused and the old ones kept
         s = np.array([2.0 ** k for k in (-3, 0, 1, 2, -1, 3, 0, 4)], np.float32)
         e.set_fp8_scales(s, 0)

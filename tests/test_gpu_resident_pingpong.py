@@ -3,10 +3,15 @@
 64 tracks of one frame, track i on weight set (i // 3) % 2: the set changes every 3 images, so inside the contiguous tile range of
 many CTAs (stems: 81 tiles per image, ~39 per CTA; 64-channel layers: 16 per image, ~8 per CTA), and the changes land on tiles
 of either consumer warpgroup of the ping-pong schedule.  Each track's network output must equal, bit for bit, that of the same
-64 tracks run with one weight set for all of them (the single-set launches, where no weights are reloaded)."""
+64 tracks run with one weight set for all of them (the single-set launches, where no weights are reloaded).
+
+In fp8 the two sets also get different activation scales (layer_harness.distinct_fp8_scales): the writers of CAT take the
+scale of every tile's own set, so a set switch between two tiles of one CTA must switch the scale too."""
 import numpy as np
 import pytest
 import torch
+
+from layer_harness import distinct_fp8_scales
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +30,7 @@ def eng(pkg, synth):
     e.close()
 
 
-@pytest.mark.parametrize('prec', ['bf16x3', 'tf32', 'bf16'])
+@pytest.mark.parametrize('prec', ['bf16x3', 'tf32', 'bf16', 'fp16', 'fp8'])
 def test_weight_switch_inside_cta_ranges(synth, eng, prec):
     dev = eng.device
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
@@ -42,6 +47,10 @@ def test_weight_switch_inside_cta_ranges(synth, eng, prec):
         return torch.cat([out_t, out_r], 1).cpu().numpy()
 
     mixed_ids = (np.arange(N, dtype=np.int32) // 3) % 2
+    if prec == 'fp8':
+        eng.calibrate_fp8_tracks(fr, fd, synth.CAMERA_K, P, ow, A_, dA, weight_ids=mixed_ids)
+        distinct_fp8_scales(eng, {w: eng.fp8_scales(w) for w in (0, 1)})
+        assert not np.array_equal(eng.fp8_scales(0), eng.fp8_scales(1))
     mixed = run(mixed_ids)
     single = {w: run(np.full(N, w, dtype=np.int32)) for w in (0, 1)}
     assert not np.array_equal(single[0], single[1])      # the two sets give different outputs: a wrong set would show
