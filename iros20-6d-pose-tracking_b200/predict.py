@@ -22,6 +22,7 @@ Differences, all additive:
   * Tracker(..., iterations=k): each frame refines every track k times inside one tracking step, exactly as k chained on_track
     calls would (the CUDA rasteriser draws input A at each round's pose).
 """
+import collections
 import contextlib
 import os
 import numpy as np
@@ -752,6 +753,18 @@ def ycb_class_names(ycb_dir):
     return sorted(os.listdir(d))
 
 
+def ycb_classes(ycb_dir, class_ids):
+    """[(class id, CADmodels/ folder name)] of class_ids, ascending and without repeats.  An id outside [1, the number of
+    CADmodels/ folders] is a ValueError."""
+    names = ycb_class_names(ycb_dir)
+    out = []
+    for c in sorted(set(int(c) for c in class_ids)):
+        if not 1 <= c <= len(names):
+            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
+        out.append((c, names[c - 1]))
+    return out
+
+
 def ycb_all_res_dir(outdir, class_name):
     """Where getResultsYcbAll writes a class's seq<id>/%07d.txt files: eval_ycb.eval_all takes the class folders in sorted order
     as class ids 1, 2, ..., and the first folder inside each as its result folder."""
@@ -876,23 +889,21 @@ def iterations_outdir(outdir, k):
 
 
 def _sweep_variants(outdir, modes, sweep, counts, ksweep):
-    """The variants a one-pass driver tracks every frame in -> [(key, mode, k, output tree)].  The key is what _track_sequences
-    keys a variant by: the mode name when every count is 1 (the runs without refinement), else (mode, k)."""
-    plain = counts == (1,)
+    """The variants a one-pass driver tracks every frame in -> [(mode, k, output tree)].  A variant is keyed by (mode, k)."""
     out = []
     for k in counts:
         base = iterations_outdir(outdir, k) if ksweep else outdir
         for m in modes:
-            out.append((m if plain else (m, k), m, k, precision_outdir(base, m) if sweep else base))
+            out.append((m, k, precision_outdir(base, m) if sweep else base))
     return out
 
 
 def _sweep_results(results, variants, sweep, ksweep):
-    """A driver's return value from {variant key: what one variant's run returns}: that alone for one variant, {mode: ...} for a
+    """A driver's return value from {(mode, k): what one variant's run returns}: that alone for one variant, {mode: ...} for a
     precision sweep, {k: ...} for a sweep of counts, {k: {mode: ...}} for both."""
     per_k = {}
-    for key, m, k, _ in variants:
-        per_k.setdefault(k, {})[m] = results[key]
+    for m, k, _ in variants:
+        per_k.setdefault(k, {})[m] = results[m, k]
     per_k = {k: (v if sweep else next(iter(v.values()))) for k, v in per_k.items()}
     return per_k if ksweep else next(iter(per_k.values()))
 
@@ -908,16 +919,11 @@ def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
     from the first is a ValueError naming it."""
     if precision not in YCB_ALL_PRECISIONS:
         raise ValueError('precision %r is not a mode of the one-pass YCB-Video driver (one of %s)' % (precision, ', '.join(YCB_ALL_PRECISIONS)))
-    names = ycb_class_names(ycb_dir)
-    ids = sorted(set(int(c) for c in class_ids))
+    ids = ycb_classes(ycb_dir, class_ids)
     if not ids:
         raise ValueError('no class ids given')
-    for c in ids:
-        if not 1 <= c <= len(names):
-            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
     classes = []
-    for c in ids:
-        name = names[c - 1]
+    for c, name in ids:
         k = _load_run_files('class %d (%s)' % (c, name), expand_class_paths(class_config, c, name))
         classes.append(dict(k, class_id=c, name=name,
                             trans_normalizer=_class_normalizer(class_config, 'trans_normalizer', c, 0.03),
@@ -940,11 +946,11 @@ def ycb_track_sets(ycb_dir, class_ids):
     return dict(sorted(sets.items()))
 
 
-def _one_pass_trackers(entries, precision, max_batch, device=None):
-    """One Engine of max_batch tracks per step on `device` (None: the current device) and {weight id: Tracker} on it for
+def _one_pass_trackers(entries, precision, max_batch):
+    """One Engine of max_batch tracks per step on the current device and {weight id: Tracker} on it for
     [(weight id, label, checked configuration)]: the configuration's files and normalisers, the CUDA renderer.  A ValueError is
     relabelled with the class or object it is about."""
-    eng = Engine(max_batch=max_batch, device=device)
+    eng = Engine(max_batch=max_batch)
     trackers = {}
     for wid, label, k in entries:
         try:
@@ -959,9 +965,9 @@ def _one_pass_trackers(entries, precision, max_batch, device=None):
 def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
-    variants: what every frame is tracked in (a tuple), each a precision mode name (one round per step) or a (mode, k) pair (k
-    refinement rounds per step, Engine.track_render's iterations).  Yields each sequence's {variant: (frames, n, 4, 4) numpy
-    poses}, the poses after each frame, as soon as the sequence ends.
+    variants: what every frame is tracked in (a tuple), each a (mode, k) pair: precision mode and k refinement rounds per step
+    (Engine.track_render's iterations).  Yields each sequence's {variant: (frames, n, 4, 4) numpy poses}, the poses after each
+    frame, as soon as the sequence ends.
 
     Every frame is one se3tn_track_render step per variant for the sequence's n tracks, all reading the same device frame: the
     frames of all sequences decode ahead, across sequence boundaries, through one StagingRing of `depth` sets (`workers` threads)
@@ -979,8 +985,7 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     Videos are drawn for one variant only."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
-    mode_k = {v: (v, 1) if isinstance(v, str) else v for v in variants}
-    fp8 = next((v for v in variants if mode_k[v][0] == 'fp8'), None)
+    fp8 = next((v for v in variants if v[0] == 'fp8'), None)
     if not sequences:
         return
     dev = eng.device
@@ -1029,7 +1034,7 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                     eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[fp8, n][0], widths, weight_ids=wh,
                                              render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
                 for v in variants:
-                    m, rounds = mode_k[v]
+                    m, rounds = v
                     poses, out_trans, out_rot, drawn = by_n[v, n]
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
@@ -1105,11 +1110,10 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
     """The fp8 calibrations borrowed_calibrations names, in sequence order: each sequence's first frame decoded and calibrated at
     the initial poses of the named tracks, as _track_sequences calibrates it (Engine.calibrate_fp8_tracks, input A drawn by the
     rasteriser).  Calibration takes per-tensor maxima of each set's own tracks, so it gives the single-GPU run's scales."""
-    dev = eng.device
     for k, tracks in borrowed.items():
         rgb_files, depth_files, ids, init = sequences[k]
         wh = np.asarray([ids[j] for j in tracks], dtype=np.int32)
-        trk = trackers[int(wh[0])]
+        trk, dev = trackers[int(wh[0])], eng.device
         wd = torch.from_numpy(wh).to(dev)
         widths = torch.tensor([trackers[int(w)].object_width for w in wh], dtype=torch.float64, device=dev)
         poses = torch.from_numpy(np.ascontiguousarray(init[tracks])).to(dev)
@@ -1119,23 +1123,36 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
                                  render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
 
 
+def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes):
+    """One process's share of a one-pass run, sequences[k] for k in mine: the Engine and Trackers of `entries`
+    (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
+    share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
+    [(paths, labels)] per sequence, folders to make once the trackers exist).  -> (Engine, {k: what writes[k] returned})."""
+    eng, trackers = _one_pass_trackers(entries, precision, max_batch)
+    _calibrate_borrowed(eng, trackers, sequences, borrowed)
+    drawn = None
+    if video is not None:
+        for d in video[2]:
+            os.makedirs(d, exist_ok=True)
+        drawn = (video[0], [video[1][k] for k in mine])
+    out = {}
+    for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn), mine):
+        fn, *args = writes[k]
+        out[k] = fn(*args, tracked)
+    return eng, out
+
+
 def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
                writes):
-    """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: its Engine and Trackers for the weight sets of
-    its sequences, the borrowed fp8 calibrations, then _track_sequences over sequences[mine] with writes[k] (fn, *args) called as
-    fn(*args, tracked) on each.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error',
-    traceback text) through conn."""
+    """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: _track_share with the weight sets of its
+    sequences.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error', traceback text) through
+    conn."""
     import traceback
     try:
         wids = set(w for k in mine for w in sequences[k][2])
         torch.cuda.set_device(device)
-        eng, trackers = _one_pass_trackers([e for e in entries if e[0] in wids], precision, max_batch, device)
-        _calibrate_borrowed(eng, trackers, sequences, borrowed)
-        drawn = None if video is None else (video[0], [video[1][k] for k in mine])
-        out = {}
-        for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn), mine):
-            fn, *args = writes[k]
-            out[k] = fn(*args, tracked)
+        eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
+                                depth, workers, video, writes)
         conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
     except BaseException:
         conn.send(('error', traceback.format_exc()))
@@ -1158,15 +1175,15 @@ def _agree_fp8_scales(per_rank):
 
 
 def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes):
-    """_track_sequences over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
-    rank (as _rank_main runs it) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
+    """_track_share over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
+    rank (_rank_main) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
     frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
     with its traceback; then, as on any other exit (KeyboardInterrupt included), every rank still running is terminated, and every
     rank is joined before this returns or raises."""
     import multiprocessing as mp
     from multiprocessing.connection import wait
     plan = assign_ranks([len(s[0]) for s in sequences], gpus)
-    fp8 = any((v if isinstance(v, str) else v[0]) == 'fp8' for v in variants)
+    fp8 = any(v[0] == 'fp8' for v in variants)
     track_sets = [s[2] for s in sequences]
     devices = _rank_devices(len(plan))
     ctx = mp.get_context('spawn')
@@ -1217,6 +1234,40 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
     return [results[k] for k in range(len(sequences))]
 
 
+# What a one-pass driver's shared front hands its back: the GPU count, the first mode (the Trackers' precision, which
+# ycb_all_classes / ycbineoat_objects check), the variants (_sweep_variants) and whether modes and counts are swept.
+_OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep')
+
+
+def _one_pass_front(outdir, gpus, precision, modes, video, iterations):
+    """The checks both one-pass drivers make first, in this order, before anything is read: gpus (check_gpus), the precision
+    modes among `modes` (precision_modes), one mode with video, the refinement counts (refine_counts), one count with video.
+    -> _OnePass."""
+    gpus = check_gpus(gpus)
+    modes, sweep = precision_modes(precision, modes)
+    if video and len(modes) > 1:
+        raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
+    counts, ksweep = refine_counts(iterations)
+    if video and len(counts) > 1:
+        raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
+    return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep), sweep, ksweep)
+
+
+def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect):
+    """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
+    (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
+    sequence k's poses.  -> the driver's return value: _sweep_results of {(mode, k): collect(written, (mode, k))}, written being
+    [what writes[k] returned] in sequence order."""
+    keys = tuple((m, k) for m, k, _ in run.variants)
+    if run.gpus == 1:
+        _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
+                              writes)
+        written = [out[k] for k in range(len(sequences))]
+    else:
+        written = _track_on_ranks(run.gpus, entries, run.precision, max_batch, sequences, keys, depth, workers, video, writes)
+    return _sweep_results({key: collect(written, key) for key in keys}, run.variants, run.sweep, run.ksweep)
+
+
 def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
     """One test sequence's files of a getResultsYcbAll run: for each variant (dirs: {variant: {class id: result folder}}) and
     class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  -> {variant: (frames, n, 4, 4) poses}."""
@@ -1264,16 +1315,10 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     frame a single-GPU run calibrates it on (borrowed_calibrations).  gpus below 1 or above torch.cuda.device_count() is a
     ValueError before anything is loaded, as is every other refusal; a rank that fails is a RuntimeError with its traceback,
     raised after every rank has stopped (_track_on_ranks)."""
-    gpus = check_gpus(gpus)
-    modes, sweep = precision_modes(precision, YCB_ALL_PRECISIONS)
-    if video and len(modes) > 1:
-        raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
-    counts, ksweep = refine_counts(iterations)
-    if video and len(counts) > 1:
-        raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
+    run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
-    classes = ycb_all_classes(ycb_dir, class_ids, class_config, modes[0])
+    classes = ycb_all_classes(ycb_dir, class_ids, class_config, run.precision)
     track_sets = ycb_track_sets(ycb_dir, [k['class_id'] for k in classes])
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
@@ -1287,31 +1332,23 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
         sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
     entries = [(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes]
     max_batch = max([len(v) for v in track_sets.values()] + [1])
-    if gpus == 1:
-        eng, trackers = _one_pass_trackers(entries, modes[0], max_batch)
     name_of = {k['class_id']: k['name'] for k in classes}
-    variants = _sweep_variants(outdir, modes, sweep, counts, ksweep)
-    root = {v: r for v, _, _, r in variants}
-    keys = tuple(root)
     drawn = None
     if video:
-        drawn = ('under', [([os.path.join(ycb_all_res_dir(root[keys[0]], name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
-                            ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)])
-        for c in name_of.values():
-            os.makedirs(ycb_all_res_dir(root[keys[0]], c), exist_ok=True)
-    dirs = {v: {c: ycb_all_res_dir(root[v], name) for c, name in name_of.items()} for v in keys}
+        tree = run.variants[0][2]
+        drawn = ('under', [([os.path.join(ycb_all_res_dir(tree, name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
+                            ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)],
+                 [ycb_all_res_dir(tree, c) for c in name_of.values()])
+    dirs = {(m, k): {c: ycb_all_res_dir(tree, name) for c, name in name_of.items()} for m, k, tree in run.variants}
     writes = [(_write_ycb_all_sequence, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
-    if gpus == 1:
-        written = (fn(*args, tracked) for tracked, (fn, *args) in zip(_track_sequences(eng, trackers, sequences, keys, 2, 2, drawn),
-                                                                      writes))
-    else:
-        written = _track_on_ranks(gpus, entries, modes[0], max_batch, sequences, keys, 2, 2, drawn, writes)
-    results = {v: {k['class_id']: {} for k in classes} for v in keys}
-    for pred_poses, (seq_id, cls) in zip(written, track_sets.items()):
-        for v in keys:
+
+    def collect(written, key):
+        out = {c: {} for c in name_of}
+        for pred_poses, (seq_id, cls) in zip(written, track_sets.items()):
             for j, c in enumerate(cls):
-                results[v][c][seq_id] = pred_poses[v][:, j]
-    return _sweep_results(results, variants, sweep, ksweep)
+                out[c][seq_id] = pred_poses[key][:, j]
+        return out
+    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1418,49 +1455,30 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     decode_ahead frames ahead of its own steps and writing its videos' files; the return value and the files equal the
     single-GPU run's."""
     from .eval_ycbineoat import OBJECTS
-    gpus = check_gpus(gpus)
-    modes, sweep = precision_modes(precision, PRECISIONS)
-    if video and len(modes) > 1:
-        raise ValueError('video=True draws the result videos of one precision mode, not of %d' % len(modes))
-    counts, ksweep = refine_counts(iterations)
-    if video and len(counts) > 1:
-        raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
+    run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
     videos = ycbineoat_videos(ycbineoat_dir)
     files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
-    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, modes[0])
+    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, run.precision)
     entries = [(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
                for o, k in objects.items()]
-    if gpus == 1:
-        eng, trackers = _one_pass_trackers(entries, modes[0], 1)
     sequences = {}
     for v, obj in videos:
         rgb_files, depth_files, gt_files = files[v]
         nf = len(rgb_files) if max_frames is None else min(max_frames, len(rgb_files))
         if nf > 0:
             sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
-    variants = _sweep_variants(outdir, modes, sweep, counts, ksweep)
-    root = {key: r for key, _, _, r in variants}
-    keys = tuple(root)
     drawn = None
     if video:
-        os.makedirs(root[keys[0]], exist_ok=True)
-        drawn = ('over', [([os.path.join(root[keys[0]], v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))])
-                          for v, s in sequences.items()])
-    writes = [(_write_ycbineoat_video, root, v) for v in sequences]
-    if gpus == 1:
-        written = (fn(*args, tracked) for tracked, (fn, *args) in
-                   zip(_track_sequences(eng, trackers, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn), writes))
-    else:
-        written = _track_on_ranks(gpus, entries, modes[0], 1, list(sequences.values()), keys, decode_ahead, 2 * decode_ahead, drawn,
-                                  writes)
-    results = {key: {} for key in keys}
-    for poses, v in zip(written, sequences):
-        for key in keys:
-            results[key][v] = poses[key]
-    return _sweep_results(results, variants, sweep, ksweep)
+        tree = run.variants[0][2]
+        drawn = ('over', [([os.path.join(tree, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()],
+                 [tree])
+    trees = {(m, k): tree for m, k, tree in run.variants}
+    writes = [(_write_ycbineoat_video, trees, v) for v in sequences]
+    return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
+                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)})
 
 
 def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
@@ -1595,10 +1613,8 @@ def main(argv=None):
         raise SystemExit('--gpus %d needs --mode ycbv_all or ycbineoat_all' % args.gpus)
     precision = cli_precision(args.precision, args.mode)
     iterations = cli_iterations(args.iterations, args.mode)
-    if args.mode == 'ycbv_all':
-        return _main_ycbv_all(args, precision, iterations)
-    if args.mode == 'ycbineoat_all':
-        return _main_ycbineoat_all(args, precision, iterations)
+    if args.mode in ('ycbv_all', 'ycbineoat_all'):
+        return _main_one_pass(args, precision, iterations)
     prec_kw = dict({} if precision is None else {'precision': precision}, **({} if iterations is None else {'iterations': iterations}))
     dataset_info, images_mean, images_std = load_run_config(args.train_data_path, args.mean_std_path)
     if args.mode == 'ycbineoat':
@@ -1663,80 +1679,55 @@ def cli_iterations(text, mode):
     return counts
 
 
-def _sweep_kw(args, precision, iterations):
-    """A one-pass driver's keyword arguments: video, precision, iterations and gpus, each passed only when given, so a run without
-    them makes the same call."""
-    kw = dict(_video_kw(args), **({} if precision is None else {'precision': precision}))
-    kw.update({} if args.gpus is None else {'gpus': args.gpus})
-    return dict(kw, **({} if iterations is None else {'iterations': iterations}))
-
-
-def _one_run(res, precision, iterations, modes):
-    """What a one-pass driver returned for one variant (the first of a sweep): the printout lists its sequences."""
-    if isinstance(iterations, list):
-        res = next(iter(res.values()), {})
-    return next(iter(res.values()), {}) if precision is not None and precision_modes(precision, modes)[1] else res
-
-
-def _video_kw(args):
-    """The drivers' video argument: passed only when --video asks for the videos, so a run without it makes the same call."""
-    return {'video': True} if args.video else {}
-
-
-def _main_ycbv_all(args, precision=None, iterations=None):
-    """--mode ycbv_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class path templates."""
-    if not args.ycb_dir or not args.class_ids:
-        raise SystemExit('--mode ycbv_all needs --ycb_dir and --class_ids')
-    n_classes = len(ycb_class_names(args.ycb_dir))
-    if args.class_ids == 'all':
-        class_ids = list(range(1, n_classes + 1))
-    else:
-        try:
-            class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
-        except ValueError:
-            raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
-    config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    kw = _sweep_kw(args, precision, iterations)
-    res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
-    sweep = precision is not None and precision_modes(precision, YCB_ALL_PRECISIONS)[1]
-    one = _one_run(res, precision, iterations, YCB_ALL_PRECISIONS)
-    for c in sorted(one):
-        print('tracked class %d through sequences %s' % (c, sorted(one[c])))
-    print('-> %s' % args.outdir)
-    if args.score and isinstance(iterations, list):
-        print_precision_table(*score_iterations(res, args.outdir, args.ycb_dir, config, precision=precision or 'bf16x3'),
-                              sweep='iteration sweep', column='variant')
-    elif args.score and sweep:
-        print_precision_table(*score_precisions(res, args.outdir, args.ycb_dir, config))
-    elif args.score:
-        _score_ycb_tree(args.ycb_dir, args.outdir, class_ids)
-    return res
-
-
-def _main_ycbineoat_all(args, precision=None, iterations=None):
-    """--mode ycbineoat_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-object path templates."""
+def _main_one_pass(args, precision=None, iterations=None):
+    """--mode ycbv_all / ycbineoat_all: --train_data_path, --mean_std_path, --ckpt_dir and --model_path are the per-class /
+    per-object path templates.  --video, --precision, --gpus and --iterations are passed to the driver only when given, so a run
+    without them makes the same call."""
     import argparse
-    if not args.YCBInEOAT_dir:
+    ycbv = args.mode == 'ycbv_all'
+    if ycbv and (not args.ycb_dir or not args.class_ids):
+        raise SystemExit('--mode ycbv_all needs --ycb_dir and --class_ids')
+    if not ycbv and not args.YCBInEOAT_dir:
         raise SystemExit('--mode ycbineoat_all needs --YCBInEOAT_dir')
-    if args.score and not args.ycb_dir:
+    if not ycbv and args.score and not args.ycb_dir:
         raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
-    kw = _sweep_kw(args, precision, iterations)
-    res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
-                              ycb_dir=args.ycb_dir, **kw)
+    kw = {key: v for key, v in (('video', args.video or None), ('precision', precision), ('gpus', args.gpus),
+                                ('iterations', iterations)) if v is not None}
+    if ycbv:
+        if args.class_ids == 'all':
+            class_ids = list(range(1, len(ycb_class_names(args.ycb_dir)) + 1))
+        else:
+            try:
+                class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
+            except ValueError:
+                raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+        res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
+        outdir, eoat = args.outdir, {}
+    else:
+        res = getResultsYcbInEOAT(args.YCBInEOAT_dir, config, args.outdir, max_frames=args.max_frames, decode_ahead=args.decode_ahead,
+                                  ycb_dir=args.ycb_dir, **kw)
+        outdir, eoat = args.outdir.rstrip('/'), dict(YCBInEOAT_dir=args.YCBInEOAT_dir)
     sweep = precision is not None and precision_modes(precision, PRECISIONS)[1]
-    one = _one_run(res, precision, iterations, PRECISIONS)
-    for v in one:
-        print('tracked %s: %d frames' % (v, len(one[v])))
+    one = next(iter(res.values()), {}) if isinstance(iterations, list) else res       # the printout lists the first variant's run
+    one = next(iter(one.values()), {}) if sweep else one
+    if ycbv:
+        for c in sorted(one):
+            print('tracked class %d through sequences %s' % (c, sorted(one[c])))
+    else:
+        for v in one:
+            print('tracked %s: %d frames' % (v, len(one[v])))
     print('-> %s' % args.outdir)
     if args.score and isinstance(iterations, list):
-        print_precision_table(*score_iterations(res, args.outdir.rstrip('/'), args.ycb_dir, config, YCBInEOAT_dir=args.YCBInEOAT_dir,
-                                                precision=precision or 'bf16x3'), sweep='iteration sweep', column='variant')
+        print_precision_table(*score_iterations(res, outdir, args.ycb_dir, config, precision=precision or 'bf16x3', **eoat),
+                              sweep='iteration sweep', column='variant')
     elif args.score and sweep:
-        print_precision_table(*score_precisions(res, args.outdir.rstrip('/'), args.ycb_dir, config, YCBInEOAT_dir=args.YCBInEOAT_dir))
+        print_precision_table(*score_precisions(res, outdir, args.ycb_dir, config, **eoat))
+    elif args.score and ycbv:
+        _score_ycb_tree(args.ycb_dir, outdir, class_ids)
     elif args.score:
         from . import eval_ycbineoat
-        eval_ycbineoat.eval_all(argparse.Namespace(YCBInEOAT_dir=args.YCBInEOAT_dir, ycb_dir=args.ycb_dir, res_dir=args.outdir.rstrip('/') + '/'))
+        eval_ycbineoat.eval_all(argparse.Namespace(YCBInEOAT_dir=args.YCBInEOAT_dir, ycb_dir=args.ycb_dir, res_dir=outdir + '/'))
     return res
 
 

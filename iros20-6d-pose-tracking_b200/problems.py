@@ -358,20 +358,18 @@ def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_si
     (trans / rot None), where `evaluate` on its empty folder raises ValueError.  The queues take
     classes x (batch_size + num_sample) x 176 x 176 x 10 bytes of device memory (about 1.4 GB for 21 classes at 200 and 10)."""
     from .engine import Engine
-    from .predict import ycb_class_names, expand_class_paths, _load_run_files
+    from .predict import ycb_classes, expand_class_paths, _load_run_files
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
     modes = list(precisions)
     for m in modes:
         PREC[m]                                             # an unknown mode fails here
-    names = ycb_class_names(ycb_dir)
-    ids = sorted(set(int(c) for c in class_ids))
-    if not ids:
+    classes = ycb_classes(ycb_dir, class_ids)
+    if not classes:
         raise ValueError('no class ids given')
+    ids = [c for c, _ in classes]
     runs = {}
-    for c in ids:
-        if not 1 <= c <= len(names):
-            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
-        runs[c] = _load_run_files('class %d (%s)' % (c, names[c - 1]), expand_class_paths(templates, c, names[c - 1]))
+    for c, name in classes:
+        runs[c] = _load_run_files('class %d (%s)' % (c, name), expand_class_paths(templates, c, name))
         if int(runs[c]['dataset_info']['resolution']) != IMAGE_SIZE:
             raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
     step = min(int(max_batch), int(batch_size))

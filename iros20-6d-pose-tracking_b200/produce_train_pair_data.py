@@ -314,13 +314,11 @@ def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None):
     <train_data_path>/../.  The classes of a frame share one step, so they must share the camera.  -> (CADmodels folder names,
     {class id: producer})."""
     import yaml
-    from .predict import ycb_class_names
+    from .predict import ycb_class_names, ycb_classes
     names = ycb_class_names(ycb_dir)
     producers = {}
-    for c in sorted(set(int(c) for c in class_ids)):
-        if not 1 <= c <= len(names):
-            raise ValueError('class %d: CADmodels/ under %s has %d classes' % (c, ycb_dir, len(names)))
-        paths = {k: str(templates[k]).format(class_id=c, class_name=names[c - 1]) for k in ('train_data_path', 'model_path')}
+    for c, name in ycb_classes(ycb_dir, class_ids):
+        paths = {k: str(templates[k]).format(class_id=c, class_name=name) for k in ('train_data_path', 'model_path')}
         with open(os.path.join(paths['train_data_path'], '../dataset_info.yml'), 'r') as ff:
             info = yaml.safe_load(ff)
         producers[c] = ProducerPurturb(info, check_vis=True, engine=eng, model=paths['model_path'], mesh_id=c, workers=workers)

@@ -38,17 +38,17 @@ def test_tree_paths(pr, tmp_path):
     out = str(tmp_path / 'o')
     assert pr.iterations_outdir(out, 2) == os.path.join(out, 'iter2')
     v = pr._sweep_variants(out, ('bf16x3',), False, (1,), False)
-    assert v == [('bf16x3', 'bf16x3', 1, out)]                      # today's key and tree
+    assert v == [('bf16x3', 1, out)]                                # today's tree
     v = pr._sweep_variants(out, ('bf16x3',), False, (3,), False)
-    assert v == [(('bf16x3', 3), 'bf16x3', 3, out)]
+    assert v == [('bf16x3', 3, out)]
     v = pr._sweep_variants(out, ('fp8', 'fp32'), True, (1, 2), True)
     assert [r for *_, r in v] == [os.path.join(out, 'iter1', 'fp8'), os.path.join(out, 'iter1', 'fp32'),
                                   os.path.join(out, 'iter2', 'fp8'), os.path.join(out, 'iter2', 'fp32')]
-    assert [key for key, *_ in v] == [('fp8', 1), ('fp32', 1), ('fp8', 2), ('fp32', 2)]
-    res = {key: m + str(k) for key, m, k, _ in v}
+    assert [(m, k) for m, k, _ in v] == [('fp8', 1), ('fp32', 1), ('fp8', 2), ('fp32', 2)]
+    res = {(m, k): m + str(k) for m, k, _ in v}
     assert pr._sweep_results(res, v, True, True) == {1: {'fp8': 'fp81', 'fp32': 'fp321'}, 2: {'fp8': 'fp82', 'fp32': 'fp322'}}
     v = pr._sweep_variants(out, ('fp8',), False, (2, 1), True)
-    assert pr._sweep_results({key: k for key, _, k, _ in v}, v, False, True) == {2: 2, 1: 1}
+    assert pr._sweep_results({(m, k): k for m, k, _ in v}, v, False, True) == {2: 2, 1: 1}
 
 
 def test_cli_parses_iterations(pr):
@@ -107,9 +107,8 @@ def fake_loop(pr, monkeypatch, seen):
         seen.append(variants)
         for j, (rgb_files, _, ids, init) in enumerate(sequences):
             out = {}
-            for v in variants:
-                m, k = (v, 1) if isinstance(v, str) else v
-                out[v] = np.stack([init + 0.001 * (t + 1) * (pr.PRECISIONS.index(m) + 1) + 0.1 * k + j for t in range(len(rgb_files))])
+            for m, k in variants:
+                out[m, k] = np.stack([init + 0.001 * (t + 1) * (pr.PRECISIONS.index(m) + 1) + 0.1 * k + j for t in range(len(rgb_files))])
             yield out
     monkeypatch.setattr(pr, '_track_sequences', loop)
 
@@ -144,7 +143,7 @@ def test_layout_of_counts_and_modes(pr, tmp_path, monkeypatch):
     for k in (1, 2):
         for m in ('fp8', 'bf16x3'):
             one = run('%s%d' % (m, k), precision=m, iterations=k)
-            assert seen[-1] == ((m,) if k == 1 else ((m, k),))
+            assert seen[-1] == ((m, k),)
             assert all(np.array_equal(one[v], both[k][m][v]) for v in one)
             files = tree_files(str(tmp_path / ('%s%d' % (m, k))))
             assert files == tree_files(str(tmp_path / 'both' / ('iter%d' % k) / m)) and len(files) == 5
@@ -152,4 +151,4 @@ def test_layout_of_counts_and_modes(pr, tmp_path, monkeypatch):
     assert list(counts) == [2, 1] and sorted(os.listdir(tmp_path / 'counts')) == ['iter1', 'iter2']
     assert tree_files(str(tmp_path / 'counts' / 'iter1')) == tree_files(str(tmp_path / 'fp81'))
     run('default', precision='fp8')
-    assert seen[-1] == ('fp8',) and tree_files(str(tmp_path / 'default')) == tree_files(str(tmp_path / 'fp81'))
+    assert seen[-1] == (('fp8', 1),) and tree_files(str(tmp_path / 'default')) == tree_files(str(tmp_path / 'fp81'))
