@@ -57,7 +57,7 @@ preprocess_kernel(PreprocessArgs a, int rows_per_cta)
     __shared__ float s_lut[6][256];
     __shared__ float s_dlut[2][kDepthN];
     __shared__ float s_dinv[2];                    // normalised value of an invalid depth (2000)
-    __shared__ short s_sx[kImg], s_sy[kPreRowsMax];
+    __shared__ int s_sx[kImg], s_sy[kPreRowsMax];        // int: a window may be up to 2e9 px wide (bbox_window), far past 16 bits
     __shared__ int s_win[4];
     const int wi = a.weight_ids ? min(max(a.weight_ids[n], 0), a.stats_rows - 1) : 0;   // ids without statistics are rejected on the host where it can see them; never index past the table
     if (threadIdx.x < 256) {
@@ -92,11 +92,11 @@ preprocess_kernel(PreprocessArgs a, int rows_per_cta)
         // cv2 resizeNN index: floor(dst * ifx), ifx = 1/(dsize/ssize) in double, clamped to ssize-1
         const double ifx = (cw > 0) ? 1.0 / (static_cast<double>(kImg) / cw) : 0.0;
         const double ify = (ch > 0) ? 1.0 / (static_cast<double>(kImg) / ch) : 0.0;
-        if (threadIdx.x < kImg) { int sx = static_cast<int>(floor(threadIdx.x * ifx)); if (sx > cw - 1) sx = cw - 1; s_sx[threadIdx.x] = static_cast<short>(sx); }
+        if (threadIdx.x < kImg) { int sx = static_cast<int>(floor(threadIdx.x * ifx)); if (sx > cw - 1) sx = cw - 1; s_sx[threadIdx.x] = sx; }
         constexpr int kSyFirst = THREADS == 256 ? 192 : 256;     // threads that fill the row table (the column table takes 0..175)
         if (threadIdx.x >= kSyFirst && threadIdx.x < kSyFirst + rows_per_cta) {
             const int y = row0 + threadIdx.x - kSyFirst;
-            int sy = static_cast<int>(floor(y * ify)); if (sy > ch - 1) sy = ch - 1; s_sy[threadIdx.x - kSyFirst] = static_cast<short>(sy);
+            int sy = static_cast<int>(floor(y * ify)); if (sy > ch - 1) sy = ch - 1; s_sy[threadIdx.x - kSyFirst] = sy;
         }
     }
     __syncthreads();

@@ -15,7 +15,9 @@ wenbowen123/iros20-6d-pose-tracking @ 18dc5bac):
   normalize_channels           data_augmentation.py:154-164   (NormalizeChannels)
   to_tensor                    data_augmentation.py:179-189   (ToTensor)
   process_data                 datasets.py:115-156            (TrackDataset.processData)
+  crop_bbox_indexed            Utils.py:320-359 through cv2's nearest-neighbour index formula (no canvas)
   process_predict              datasets.py:159-175            (TrackDataset.processPredict)
+  process_predict_exact        datasets.py:159-175 with its float32 roundings and the product's association pinned
   forward                      se3_tracknet.py:81-112 + network_modules.py:59-66,86-120
   on_track                     predict.py:217-296 (render_window output taken as an input)
   add / adi                    Utils.py:72-98     (ADD, ADD-S; scipy cKDTree for the nearest neighbour)
@@ -104,6 +106,28 @@ def crop_bbox(color, depth, boundingbox, output_size=(100, 100)):
     return rgb_out * (rgb_out != 0), z_out * (z_out != 0)
 
 
+def crop_bbox_indexed(color, depth, boundingbox, output_size=(100, 100)):
+    """crop_bbox without the canvas, for windows too large to allocate one (tens of thousands of pixels a side when the
+    object is millimetres from the camera).  cv2's INTER_NEAREST takes output pixel (y, x) from canvas pixel
+    (min(floor(y * (1 / (dh / h))), h - 1), min(floor(x * (1 / (dw / w))), w - 1)), the factors in float64; the canvas
+    pixel is frame pixel (top + sy, left + sx), zero outside the frame.  An empty window (object_width 0) gives zeros:
+    that is what the crop kernels cut, while the reference's cv2.resize refuses an empty canvas."""
+    top, left, crop_h, crop_w = crop_window(boundingbox)
+    out_w, out_h = output_size
+    H, W = color.shape[:2]
+    rgb = np.zeros((out_h, out_w, 3), dtype=color.dtype)
+    z = np.zeros((out_h, out_w), dtype=depth.dtype)
+    if crop_h <= 0 or crop_w <= 0:
+        return rgb, z
+    sy = np.minimum(np.floor(np.arange(out_h) * (1.0 / (out_h / crop_h))).astype(np.int64), crop_h - 1)
+    sx = np.minimum(np.floor(np.arange(out_w) * (1.0 / (out_w / crop_w))).astype(np.int64), crop_w - 1)
+    fy, fx = top + sy, left + sx
+    iy, ix = np.nonzero((fy >= 0) & (fy < H))[0], np.nonzero((fx >= 0) & (fx < W))[0]
+    rgb[np.ix_(iy, ix)] = color[np.ix_(fy[iy], fx[ix])]
+    z[np.ix_(iy, ix)] = depth[np.ix_(fy[iy], fx[ix])]
+    return rgb, z
+
+
 def normalize_rotation_matrix(R):
     """Utils.py:363-367 (in place, column-normalise)."""
     R[:, 0] = R[:, 0] / np.linalg.norm(R[:, 0])
@@ -190,6 +214,33 @@ def process_predict(A_in_cam, predB, trans_normalizer=0.03, rot_normalizer=5 * n
     A2B = cv2.Rodrigues(rot_pred)[0].reshape(3, 3)
     B_in_cam[:3, :3] = A2B.dot(A_in_cam[:3, :3])
     return B_in_cam
+
+
+def pose_compose_exact(A_in_cam, R, t):
+    """B = [R . A_R | float64(t) + A_t] for a batch (n,4,4), (n,3,3), (n,3): each product entry in scalar float64 as
+    (r0 a0 + r1 a1) + r2 a2, every operation rounded on its own (numpy ufuncs; np.dot may fuse or reorder in BLAS)."""
+    A = np.asarray(A_in_cam, dtype=np.float64)
+    R = np.asarray(R, dtype=np.float64)
+    B = np.zeros_like(A)
+    for r in range(3):
+        for c in range(3):
+            B[:, r, c] = (R[:, r, 0] * A[:, 0, c] + R[:, r, 1] * A[:, 1, c]) + R[:, r, 2] * A[:, 2, c]
+    B[:, :3, 3] = np.asarray(t).astype(np.float64) + A[:, :3, 3]
+    B[:, 3, 3] = 1.0
+    return B
+
+
+def process_predict_exact(A_in_cam, trans, rot, trans_normalizer=0.03, rot_normalizer=5 * np.pi / 180):
+    """process_predict for a batch, every rounding pinned: the dtype chain of datasets.py:159-175 (F9 / F10) with the
+    rotation product in the association the pose update uses.
+      trans_pred = float32 trans * float32(tn)               (float32 array times a Python float stays float32)
+      R32        = cv2.Rodrigues(float32 rot * float32(rn))  (float32 in, float32 out: OpenCV's float64 result rounded)
+      B          = pose_compose_exact(A, R32, trans_pred)"""
+    t32 = np.asarray(trans, dtype=np.float32) * np.float32(trans_normalizer)
+    r32 = np.asarray(rot, dtype=np.float32) * np.float32(rot_normalizer)
+    R32 = np.stack([cv2.Rodrigues(r)[0] for r in r32])
+    assert t32.dtype == np.float32 and R32.dtype == np.float32
+    return pose_compose_exact(A_in_cam, R32, t32)
 
 
 # ----------------------------------------------------------------------------
