@@ -91,6 +91,11 @@ const char* se3tn_last_error(se3tn_ctx* ctx);
  * Replaces: Se3TrackNet.load_state_dict (reference predict.py:151-155). */
 int se3tn_load_weights(se3tn_ctx* ctx, int weight_id, const float* blob, size_t n_floats);
 
+/* Device bytes one loaded weight set holds: the blob in fp32 and the conv weights in every storage format (storage.cuh), the
+ * fp8 tables and the resident layers' stacked and permuted rows.  Weight ids are any int >= 0; the context's per-id tables
+ * take one small row per id up to the largest. */
+size_t se3tn_weight_set_bytes(void);
+
 /* Per-object channel statistics (reference predict.py:657-658 mean.npy/std.npy): 8 values each,
  * A's 4 channels then B's.  `is_f64` selects the arithmetic of the normalisation so that it
  * reproduces numpy's for float32 resp. float64 mean/std arrays (data_augmentation.py:159-163). */

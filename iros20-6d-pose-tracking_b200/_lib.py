@@ -23,6 +23,7 @@ _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 # name -> (restype, argtypes); mirrors include/se3tn.h one to one
 SIGNATURES = {
     'se3tn_workspace_bytes': (_sz, [_i]),
+    'se3tn_weight_set_bytes': (_sz, []),
     'se3tn_create': (_i, [_i, _i, _vp, C.POINTER(_vp)]),
     'se3tn_destroy': (None, [_vp]),
     'se3tn_last_error': (C.c_char_p, [_vp]),

@@ -702,7 +702,19 @@ int queue_render(se3tn_ctx* c, const double* K, const double* poses, const doubl
     return SE3TN_OK;
 }
 
+constexpr size_t kStackBytes = 8 * 128 * 288 * sizeof(float);   // DeviceWeights::stack
+constexpr size_t kPermFloats = 6 * 64 * 576;                     // DeviceWeights::perm
+
+// Device bytes of the DeviceWeights prepare_weights builds: what one loaded weight set holds.
+size_t weight_set_bytes() {
+    const size_t floats = blob_floats();
+    size_t bytes = floats * sizeof(float) + floats;                // the fp32 blob, the fp8 conv weights
+    for (int p : kTensorPrecs) bytes += floats * prec_bytes_per_channel(p);
+    return bytes + (kFp8BlockFloats + kFp8WRows + kPermFloats) * sizeof(float) + kStackBytes;
+}
+
 // Every form of a weight blob the kernels read, built into `w` (which owns all of it, so a failure leaves nothing behind).
+// Its allocations are the ones weight_set_bytes counts.
 int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
     const size_t floats = blob_floats();
     CU_TRY(c, dev_alloc(w.blob, floats));
@@ -710,8 +722,8 @@ int prepare_weights(se3tn_ctx* c, DeviceWeights& w, const float* blob) {
     CU_TRY(c, dev_alloc(w.conv[SE3TN_PREC_FP8], floats));
     CU_TRY(c, dev_alloc(w.fp8, kFp8BlockFloats));
     CU_TRY(c, dev_alloc(w.fp8_sw, kFp8WRows));
-    CU_TRY(c, dev_alloc(w.stack, 8 * 128 * 288 * sizeof(float)));
-    CU_TRY(c, dev_alloc(w.perm, 6 * 64 * 576));
+    CU_TRY(c, dev_alloc(w.stack, kStackBytes));
+    CU_TRY(c, dev_alloc(w.perm, kPermFloats));
     DevBuf<float> perm_tmp;                        // one 64-channel layer's fp32 weights with permuted rows
     CU_TRY(c, dev_alloc(perm_tmp, 64 * 576));
     CU_TRY(c, cudaDeviceSynchronize());
@@ -833,6 +845,8 @@ size_t se3tn_workspace_bytes(int max_batch) {
     if (max_batch <= 0) return 0;
     return workspace_floats(max_batch) * sizeof(float);
 }
+
+size_t se3tn_weight_set_bytes(void) { return weight_set_bytes(); }
 
 const char* se3tn_last_error(se3tn_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 

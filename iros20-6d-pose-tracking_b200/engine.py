@@ -30,6 +30,18 @@ def _stream(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def check_weight_sets_fit(n_sets, device=None, what='weight sets'):
+    """A ValueError, with the numbers, unless n_sets weight sets (se3tn_weight_set_bytes each: every storage format a set is
+    kept in) fit in the free memory of CUDA device `device` (default: the current one).  Called before any set is loaded."""
+    each = int(_lib.load().se3tn_weight_set_bytes())
+    dev = torch.cuda.current_device() if device is None else int(device)
+    free = int(torch.cuda.mem_get_info(dev)[0])
+    if n_sets * each > free:
+        raise ValueError('%d %s need %.2f GB of device memory (%.1f MB each, in every storage format), but cuda:%d has %.2f GB free'
+                         % (n_sets, what, n_sets * each / 1e9, each / 1e6, dev, free / 1e9))
+    return each
+
+
 class Engine:
     def __init__(self, max_batch=64, device=None):
         if not torch.cuda.is_available():

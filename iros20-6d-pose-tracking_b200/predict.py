@@ -28,7 +28,7 @@ import os
 import numpy as np
 import torch
 
-from .engine import Engine
+from .engine import Engine, check_weight_sets_fit
 from .cuda_renderer import CudaRenderer
 from .se3_tracknet import Se3TrackNet
 from .datasets import TrackDataset
@@ -888,24 +888,86 @@ def iterations_outdir(outdir, k):
     return os.path.join(outdir, 'iter%d' % k)
 
 
-def _sweep_variants(outdir, modes, sweep, counts, ksweep):
-    """The variants a one-pass driver tracks every frame in -> [(mode, k, output tree)].  A variant is keyed by (mode, k)."""
+def checkpoint_outdir(outdir, i):
+    """Where a run over several checkpoints writes checkpoint i's output tree: <outdir>/ckpt<i>/, what a run of checkpoint i
+    alone with that outdir writes (with iter<k>/ and <mode>/ below it when those are swept too)."""
+    return os.path.join(outdir, 'ckpt%d' % i)
+
+
+# Several checkpoints in one run: checkpoint i's weight set of the class or object of weight id w is w + CKPT_ID_STRIDE * i.  The
+# context takes any id >= 0 (its per-id tables grow to the largest); the stride keeps the checkpoints' ids apart, so a run over
+# several checkpoints takes base ids below it.
+CKPT_ID_STRIDE = 32
+
+
+def checkpoint_list(ckpts, mean_std_paths, ckpt_name='ckpt_dir', stats_name='mean_std_path'):
+    """The checkpoints of a run -> [(checkpoint, mean_std_path)]: ckpts one path (or template) or a list of them, mean_std_paths
+    one folder shared by all or one per checkpoint (train.py writes mean / std per training run).  An empty list or entry, a
+    checkpoint listed twice and any other number of mean_std_paths are a ValueError naming the argument."""
+    ckpts = [ckpts] if isinstance(ckpts, str) else list(ckpts)
+    stats = [mean_std_paths] if isinstance(mean_std_paths, str) else list(mean_std_paths)
+    if not ckpts or not all(ckpts):
+        raise ValueError('%s: an empty checkpoint entry' % ckpt_name)
+    if not stats or not all(stats):
+        raise ValueError('%s: an empty entry' % stats_name)
+    twice = sorted(set(c for c in ckpts if ckpts.count(c) > 1))
+    if twice:
+        raise ValueError('%s: checkpoint %s listed more than once' % (ckpt_name, ', '.join(twice)))
+    if len(stats) not in (1, len(ckpts)):
+        raise ValueError('%s: %d entries for %d checkpoints; give one, shared by all, or one per checkpoint'
+                         % (stats_name, len(stats), len(ckpts)))
+    return list(zip(ckpts, stats * len(ckpts) if len(stats) == 1 else stats))
+
+
+def checkpoint_configs(config):
+    """A one-pass driver's path templates with ckpt_dir (and mean_std_path) as lists -> one config per checkpoint, each with a
+    single ckpt_dir and mean_std_path (checkpoint_list's rules).  Plain strings give [config] unchanged."""
+    if 'ckpt_dir' not in config or 'mean_std_path' not in config:
+        return [config]
+    if isinstance(config['ckpt_dir'], str) and isinstance(config['mean_std_path'], str):
+        return [config]
+    return [dict(config, ckpt_dir=c, mean_std_path=m) for c, m in checkpoint_list(config['ckpt_dir'], config['mean_std_path'])]
+
+
+def _check_checkpoint_ids(base_ids, ckpts, what):
+    """With several checkpoints, every base weight id below CKPT_ID_STRIDE: otherwise a ValueError naming it."""
+    for w in base_ids:
+        if ckpts > 1 and not 0 <= w < CKPT_ID_STRIDE:
+            raise ValueError('%s %d: with %d checkpoints the weight ids are %s id + %d x checkpoint index, so the %s ids stop at %d'
+                             % (what, w, ckpts, what, CKPT_ID_STRIDE, what, CKPT_ID_STRIDE - 1))
+
+
+def _sweep_variants(outdir, modes, sweep, counts, ksweep, ckpts=1):
+    """The variants a one-pass driver tracks every frame in -> [(mode, k, output tree)] with one checkpoint, [(mode, k,
+    checkpoint index, output tree)] with several: each entry is a variant's key followed by its tree.  With one checkpoint the
+    tree has no ckpt<i>/ level."""
     out = []
-    for k in counts:
-        base = iterations_outdir(outdir, k) if ksweep else outdir
-        for m in modes:
-            out.append((m, k, precision_outdir(base, m) if sweep else base))
+    for c in range(ckpts):
+        root = checkpoint_outdir(outdir, c) if ckpts > 1 else outdir
+        for k in counts:
+            base = iterations_outdir(root, k) if ksweep else root
+            for m in modes:
+                out.append((m, k) + ((c,) if ckpts > 1 else ()) + (precision_outdir(base, m) if sweep else base,))
     return out
 
 
+def _variant_checkpoint(key):
+    """The checkpoint index of a variant key: (mode, k) is checkpoint 0 of a one-checkpoint run, (mode, k, i) checkpoint i."""
+    return key[2] if len(key) > 2 else 0
+
+
 def _sweep_results(results, variants, sweep, ksweep):
-    """A driver's return value from {(mode, k): what one variant's run returns}: that alone for one variant, {mode: ...} for a
-    precision sweep, {k: ...} for a sweep of counts, {k: {mode: ...}} for both."""
-    per_k = {}
-    for m, k, _ in variants:
-        per_k.setdefault(k, {})[m] = results[m, k]
-    per_k = {k: (v if sweep else next(iter(v.values()))) for k, v in per_k.items()}
-    return per_k if ksweep else next(iter(per_k.values()))
+    """A driver's return value from {variant key: what one variant's run returns}: per checkpoint, that alone for one variant,
+    {mode: ...} for a precision sweep, {k: ...} for a sweep of counts, {k: {mode: ...}} for both; {checkpoint index: that}
+    with more than one checkpoint."""
+    per_c = {}
+    for v in variants:
+        m, k = v[:2]
+        per_c.setdefault(_variant_checkpoint(v[:-1]), {}).setdefault(k, {})[m] = results[v[:-1]]
+    for c, per_k in per_c.items():
+        per_k = {k: (v if sweep else next(iter(v.values()))) for k, v in per_k.items()}
+        per_c[c] = per_k if ksweep else next(iter(per_k.values()))
+    return per_c if len(per_c) > 1 else per_c[0]
 
 
 def ycb_all_classes(ycb_dir, class_ids, class_config, precision='bf16x3'):
@@ -965,8 +1027,8 @@ def _one_pass_trackers(entries, precision, max_batch):
 def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
-    variants: what every frame is tracked in (a tuple), each a (mode, k) pair: precision mode and k refinement rounds per step
-    (Engine.track_render's iterations).  Yields each sequence's {variant: (frames, n, 4, 4) numpy poses}, the poses after each
+    variants: what every frame is tracked in (a tuple) as _sweep_variants keys them, (mode, k) or (mode, k, c): precision mode, k
+    refinement rounds per step (Engine.track_render's iterations) and the weight sets of checkpoint c (ids + CKPT_ID_STRIDE * c).  Yields each sequence's {variant: (frames, n, 4, 4) numpy poses}, the poses after each
     frame, as soon as the sequence ends.
 
     Every frame is one se3tn_track_render step per variant for the sequence's n tracks, all reading the same device frame: the
@@ -974,8 +1036,9 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     into its one device frame, so a frame is decoded once whatever the number of variants.  The steps' other device arguments are
     kept: the ids and widths per distinct weight-id tuple, and per (variant, n) the pose tensor that variant's steps update in place
     and their outputs.  So in each variant every step after a track set's first replays that variant's CUDA graph, across
-    sequences too ('fp32' steps are never captured).  With 'fp8' among the modes, each weight set is calibrated on the first frame
-    of the first sequence that tracks it, before that frame's steps, at the sequence's initial poses.  After each step the
+    sequences too ('fp32' steps are never captured).  Each checkpoint steps in the sequence's n, as a run of it alone does, so
+    every variant keeps that run's bits.  With 'fp8' among the modes, each weight set is calibrated on the first frame of the first
+    sequence that tracks it, before that frame's steps, at the sequence's initial poses.  After each step the
     variant's poses are copied into its device history, which comes back to the host once per sequence.
 
     video: None, or (label order, [(paths, labels)] per sequence): paths holds one mp4 path per track, labels one text per frame.
@@ -985,7 +1048,10 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     Videos are drawn for one variant only."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
-    fp8 = next((v for v in variants if v[0] == 'fp8'), None)
+    fp8 = {}                                               # checkpoint index -> its first fp8 variant
+    for v in variants:
+        if v[0] == 'fp8':
+            fp8.setdefault(_variant_checkpoint(v), v)
     if not sequences:
         return
     dev = eng.device
@@ -1014,27 +1080,29 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
         by_ids, by_n = {}, {}
         for k, (rgb_files, _, ids, init) in enumerate(sequences):
             n = len(ids)
-            if ids not in by_ids:
-                wh = np.asarray(ids, dtype=np.int32)
-                by_ids[ids] = (wh, torch.from_numpy(wh).to(dev),
-                               torch.tensor([trackers[w].object_width for w in ids], dtype=torch.float64, device=dev))
+            for c in _checkpoints(variants):
+                if (ids, c) not in by_ids:
+                    wh = np.asarray(ids, dtype=np.int32) + CKPT_ID_STRIDE * c
+                    by_ids[ids, c] = (wh, torch.from_numpy(wh).to(dev),
+                                      torch.tensor([trackers[int(w)].object_width for w in wh], dtype=torch.float64, device=dev))
             for v in variants:
                 if (v, n) not in by_n:
                     by_n[v, n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
                                   torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
                                   None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
                 by_n[v, n][0].copy_(torch.from_numpy(init))
-            wh, wd, widths = by_ids[ids]
             history = {v: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for v in variants}
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
-                if fp8 is not None and t == 0:         # each set is calibrated on the first frame of the first sequence that tracks it
-                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[fp8, n][0], widths, weight_ids=wh,
+                for c, v in (fp8.items() if t == 0 else ()):   # each set calibrated on the first frame of its first sequence
+                    wh, wd, widths = by_ids[ids, c]
+                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[v, n][0], widths, weight_ids=wh,
                                              render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
                 for v in variants:
-                    m, rounds = v
+                    m, rounds = v[:2]
+                    wh, wd, widths = by_ids[ids, _variant_checkpoint(v)]
                     poses, out_trans, out_rot, drawn = by_n[v, n]
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
@@ -1106,6 +1174,16 @@ def _rank_devices(n):
     return list(range(n))
 
 
+def _checkpoints(variants):
+    """The checkpoint indices of a run's variant keys, ascending."""
+    return sorted(set(_variant_checkpoint(v) for v in variants))
+
+
+def _checkpoint_sequences(sequences, c):
+    """sequences with every track's weight id moved to checkpoint c's set."""
+    return sequences if c == 0 else [(r, d, tuple(w + CKPT_ID_STRIDE * c for w in ids), init) for r, d, ids, init in sequences]
+
+
 def _calibrate_borrowed(eng, trackers, sequences, borrowed):
     """The fp8 calibrations borrowed_calibrations names, in sequence order: each sequence's first frame decoded and calibrated at
     the initial poses of the named tracks, as _track_sequences calibrates it (Engine.calibrate_fp8_tracks, input A drawn by the
@@ -1129,7 +1207,8 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
     share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
     [(paths, labels)] per sequence, folders to make once the trackers exist).  -> (Engine, {k: what writes[k] returned})."""
     eng, trackers = _one_pass_trackers(entries, precision, max_batch)
-    _calibrate_borrowed(eng, trackers, sequences, borrowed)
+    for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
+        _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
     drawn = None
     if video is not None:
         for d in video[2]:
@@ -1149,7 +1228,7 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
     conn."""
     import traceback
     try:
-        wids = set(w for k in mine for w in sequences[k][2])
+        wids = _rank_weight_ids(sequences, mine, variants)
         torch.cuda.set_device(device)
         eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
                                 depth, workers, video, writes)
@@ -1158,6 +1237,11 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
         conn.send(('error', traceback.format_exc()))
     finally:
         conn.close()
+
+
+def _rank_weight_ids(sequences, mine, variants):
+    """The weight sets a rank tracking sequences `mine` loads: every checkpoint's set of each of their tracks."""
+    return set(w + CKPT_ID_STRIDE * c for k in mine for w in sequences[k][2] for c in _checkpoints(variants))
 
 
 def _agree_fp8_scales(per_rank):
@@ -1186,6 +1270,9 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
     fp8 = any(v[0] == 'fp8' for v in variants)
     track_sets = [s[2] for s in sequences]
     devices = _rank_devices(len(plan))
+    if len(_checkpoints(variants)) > 1:
+        for r, mine in enumerate(plan):
+            check_weight_sets_fit(len(_rank_weight_ids(sequences, mine, variants)), devices[r], 'weight sets (checkpoints x classes)')
     ctx = mp.get_context('spawn')
     procs, conns, done = [], [], False
     try:
@@ -1236,13 +1323,13 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
 
 # What a one-pass driver's shared front hands its back: the GPU count, the first mode (the Trackers' precision, which
 # ycb_all_classes / ycbineoat_objects check), the variants (_sweep_variants) and whether modes and counts are swept.
-_OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep')
+_OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep configs')
 
 
-def _one_pass_front(outdir, gpus, precision, modes, video, iterations):
+def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
     """The checks both one-pass drivers make first, in this order, before anything is read: gpus (check_gpus), the precision
-    modes among `modes` (precision_modes), one mode with video, the refinement counts (refine_counts), one count with video.
-    -> _OnePass."""
+    modes among `modes` (precision_modes), one mode with video, the refinement counts (refine_counts), one count with video, the
+    checkpoints of config's ckpt_dir / mean_std_path lists (checkpoint_configs), one checkpoint with video.  -> _OnePass."""
     gpus = check_gpus(gpus)
     modes, sweep = precision_modes(precision, modes)
     if video and len(modes) > 1:
@@ -1250,15 +1337,21 @@ def _one_pass_front(outdir, gpus, precision, modes, video, iterations):
     counts, ksweep = refine_counts(iterations)
     if video and len(counts) > 1:
         raise ValueError('video=True draws the result videos of one iteration count, not of %d' % len(counts))
-    return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep), sweep, ksweep)
+    configs = checkpoint_configs(config)
+    if video and len(configs) > 1:
+        raise ValueError('video=True draws the result videos of one checkpoint, not of %d' % len(configs))
+    return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs)
 
 
 def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect):
     """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
     (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
-    sequence k's poses.  -> the driver's return value: _sweep_results of {(mode, k): collect(written, (mode, k))}, written being
-    [what writes[k] returned] in sequence order."""
-    keys = tuple((m, k) for m, k, _ in run.variants)
+    sequence k's poses.  With several checkpoints, a run whose weight sets do not fit in free device memory is refused first
+    (check_weight_sets_fit; per rank on several GPUs).  -> the driver's return value: _sweep_results of {variant:
+    collect(written, variant)}, written being [what writes[k] returned] in sequence order."""
+    keys = tuple(v[:-1] for v in run.variants)
+    if run.gpus == 1 and len(run.configs) > 1:
+        check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
     if run.gpus == 1:
         _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
                               writes)
@@ -1266,6 +1359,11 @@ def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, wr
     else:
         written = _track_on_ranks(run.gpus, entries, run.precision, max_batch, sequences, keys, depth, workers, video, writes)
     return _sweep_results({key: collect(written, key) for key in keys}, run.variants, run.sweep, run.ksweep)
+
+
+def _ckpt_label(i, run):
+    """' checkpoint <i>' in the labels of a run over several checkpoints, '' with one."""
+    return ' checkpoint %d' % i if len(run.configs) > 1 else ''
 
 
 def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
@@ -1314,11 +1412,18 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     value equals the single-GPU run's, bit for bit and in the same order, and so do the files; each fp8 set is calibrated on the
     frame a single-GPU run calibrates it on (borrowed_calibrations).  gpus below 1 or above torch.cuda.device_count() is a
     ValueError before anything is loaded, as is every other refusal; a rank that fails is a RuntimeError with its traceback,
-    raised after every rank has stopped (_track_on_ranks)."""
-    run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations)
+    raised after every rank has stopped (_track_on_ranks).
+
+    class_config['ckpt_dir'] (and 'mean_std_path') may be lists of templates, one per checkpoint (checkpoint_configs): every
+    frame is then tracked once per (checkpoint, mode, k), checkpoint i's sets under weight id class id + 32 i, its tree under
+    <outdir>/ckpt<i>/ file for file what a run of it alone writes, and the return value is {i: what that run returns}.
+    score_checkpoints scores it.  video=True takes one checkpoint; weight sets beyond the device's free memory are refused."""
+    run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
-    classes = ycb_all_classes(ycb_dir, class_ids, class_config, run.precision)
+    _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
+    per_ckpt = [ycb_all_classes(ycb_dir, class_ids, cfg, run.precision) for cfg in run.configs]
+    classes = per_ckpt[0]
     track_sets = ycb_track_sets(ycb_dir, [k['class_id'] for k in classes])
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
@@ -1330,16 +1435,17 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
         init = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
                                          sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]).astype(np.float64)
         sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
-    entries = [(k['class_id'], 'class %d (%s)' % (k['class_id'], k['name']), k) for k in classes]
+    entries = [(k['class_id'] + CKPT_ID_STRIDE * i, 'class %d (%s)' % (k['class_id'], k['name']) + _ckpt_label(i, run), k)
+               for i, cl in enumerate(per_ckpt) for k in cl]
     max_batch = max([len(v) for v in track_sets.values()] + [1])
     name_of = {k['class_id']: k['name'] for k in classes}
     drawn = None
     if video:
-        tree = run.variants[0][2]
+        tree = run.variants[0][-1]
         drawn = ('under', [([os.path.join(ycb_all_res_dir(tree, name_of[c]), 'seq%d.mp4' % seq_id) for c in cls],
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)],
                  [ycb_all_res_dir(tree, c) for c in name_of.values()])
-    dirs = {(m, k): {c: ycb_all_res_dir(tree, name) for c, name in name_of.items()} for m, k, tree in run.variants}
+    dirs = {v[:-1]: {c: ycb_all_res_dir(v[-1], name) for c, name in name_of.items()} for v in run.variants}
     writes = [(_write_ycb_all_sequence, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
 
     def collect(written, key):
@@ -1453,17 +1559,22 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
 
     gpus: the number of GPUs, as in getResultsYcbAll: whole videos shared out over min(gpus, videos) ranks, each decoding
     decode_ahead frames ahead of its own steps and writing its videos' files; the return value and the files equal the
-    single-GPU run's."""
+    single-GPU run's.
+
+    object_config['ckpt_dir'] (and 'mean_std_path') may be lists of templates, one per checkpoint, as in getResultsYcbAll:
+    checkpoint i's sets under weight id object index + 32 i, its tree under <outdir>/ckpt<i>/."""
     from .eval_ycbineoat import OBJECTS
-    run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations)
+    run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
     videos = ycbineoat_videos(ycbineoat_dir)
     files = {v: sequence_files(os.path.join(ycbineoat_dir, v)) for v, _ in videos}
-    objects = ycbineoat_objects([o for o in OBJECTS if any(o == ob for _, ob in videos)], object_config, ycb_dir, run.precision)
-    entries = [(OBJECTS.index(o), 'object %s' % o, dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
-               for o, k in objects.items()]
+    used = [o for o in OBJECTS if any(o == ob for _, ob in videos)]
+    _check_checkpoint_ids([OBJECTS.index(o) for o in used], len(run.configs), 'object')
+    entries = [(OBJECTS.index(o) + CKPT_ID_STRIDE * i, 'object %s' % o + _ckpt_label(i, run),
+                dict(k, trans_normalizer=YCBINEOAT_TRANS_NORMALIZER, rot_normalizer=YCBINEOAT_ROT_NORMALIZER))
+               for i, cfg in enumerate(run.configs) for o, k in ycbineoat_objects(used, cfg, ycb_dir, run.precision).items()]
     sequences = {}
     for v, obj in videos:
         rgb_files, depth_files, gt_files = files[v]
@@ -1472,10 +1583,10 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
             sequences[v] = (rgb_files[:nf], depth_files[:nf], (OBJECTS.index(obj),), np.loadtxt(gt_files[0]).reshape(1, 4, 4))
     drawn = None
     if video:
-        tree = run.variants[0][2]
+        tree = run.variants[0][-1]
         drawn = ('over', [([os.path.join(tree, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()],
                  [tree])
-    trees = {(m, k): tree for m, k, tree in run.variants}
+    trees = {v[:-1]: v[-1] for v in run.variants}
     writes = [(_write_ycbineoat_video, trees, v) for v in sequences]
     return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
                           lambda written, key: {v: w[key] for v, w in zip(sequences, written)})
@@ -1510,6 +1621,49 @@ def score_iterations(results, outdir, ycb_dir, config, YCBInEOAT_dir=None, preci
     flat = {label(k, m): (res[m] if sweep else res) for k, res in results.items() for m in modes}
     ref = label(1 if 1 in results else min(results), sweep_reference(modes))
     return ref, _score_variants(flat, {v: os.path.join(outdir, v) for v in flat}, ref, 'variant %s', ycb_dir, config, YCBInEOAT_dir)
+
+
+def score_checkpoints(results, outdir, ycb_dir, config, YCBInEOAT_dir=None, precision='bf16x3', iterations=1):
+    """score_precisions for a run over several checkpoints: results what getResultsYcbAll / getResultsYcbInEOAT returned,
+    {checkpoint index: ...}, for this precision (a mode or a sweep) and iterations (a count or a sweep); config the run's
+    templates (ckpt_dir / mean_std_path lists).  One row per variant, labelled by its tree under outdir ('ckpt<i>', then
+    '/iter<k>' and '/<mode>' when those were swept), each with its AUCs and its drift from checkpoint 0 in the sweep's reference
+    mode (sweep_reference) and k (1, or the smallest swept).  -> (reference label, rows)."""
+    sweep = precision_modes(precision, PRECISIONS)[1]
+    counts, ksweep = refine_counts(iterations)
+    one = results[0][counts[0]] if ksweep else results[0]
+    modes = tuple(one) if sweep else (precision,)
+    variants = _sweep_variants(outdir, modes, sweep, counts, ksweep, len(results))
+    flat, roots = {}, {}
+    for m, k, c, tree in variants:
+        label = os.path.relpath(tree, outdir)
+        r = results[c][k] if ksweep else results[c]
+        flat[label], roots[label] = (r[m] if sweep else r), tree
+    k0 = 1 if 1 in counts else min(counts)
+    ref = next(os.path.relpath(t, outdir) for m, k, c, t in variants if c == 0 and m == sweep_reference(modes) and k == k0)
+    return ref, _score_variants(flat, roots, ref, 'variant %s', ycb_dir, checkpoint_configs(config)[0], YCBInEOAT_dir)
+
+
+def best_checkpoints(rows):
+    """{variant below ckpt<i>/ ('' when only checkpoints vary): (checkpoint index, its ADD-S AUC)}, the checkpoint with the highest
+    ADD-S AUC among the rows of score_checkpoints, the first listed among equals."""
+    from .problems import best_checkpoint
+    groups = {}
+    for label, r in rows.items():
+        head, _, sub = label.partition('/')
+        groups.setdefault(sub, []).append((int(head[len('ckpt'):]), r['adds']))
+    out = {}
+    for sub, got in groups.items():
+        b = best_checkpoint([-a for _, a in got])
+        out[sub] = got[b]
+    return out
+
+
+def print_best_checkpoints(rows, ckpts):
+    """After score_checkpoints' table: one line per mode (and k) naming the checkpoint with the highest ADD-S AUC."""
+    ckpts = [ckpts] if isinstance(ckpts, str) else list(ckpts)
+    for sub, (i, adds) in best_checkpoints(rows).items():
+        print('best%s: checkpoint %d (%s), ADD-S %.4f' % (' ' + sub if sub else '', i, ckpts[i], adds))
 
 
 def _score_variants(results, roots, ref, header, ycb_dir, config, YCBInEOAT_dir):
@@ -1692,6 +1846,13 @@ def _main_one_pass(args, precision=None, iterations=None):
     if not ycbv and args.score and not args.ycb_dir:
         raise SystemExit('--score needs --ycb_dir (the model points eval_ycbineoat reads)')
     config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
+    for key in ('ckpt_dir', 'mean_std_path'):                   # template lists: one pass over several checkpoints
+        if ',' in config[key]:
+            config[key] = config[key].split(',')
+    try:
+        ckpts = len(checkpoint_configs(config))
+    except ValueError as e:
+        raise SystemExit('--%s: %s' % ('ckpt_dir / --mean_std_path', e))
     kw = {key: v for key, v in (('video', args.video or None), ('precision', precision), ('gpus', args.gpus),
                                 ('iterations', iterations)) if v is not None}
     if ycbv:
@@ -1709,7 +1870,8 @@ def _main_one_pass(args, precision=None, iterations=None):
                                   ycb_dir=args.ycb_dir, **kw)
         outdir, eoat = args.outdir.rstrip('/'), dict(YCBInEOAT_dir=args.YCBInEOAT_dir)
     sweep = precision is not None and precision_modes(precision, PRECISIONS)[1]
-    one = next(iter(res.values()), {}) if isinstance(iterations, list) else res       # the printout lists the first variant's run
+    one = res[0] if ckpts > 1 else res
+    one = next(iter(one.values()), {}) if isinstance(iterations, list) else one      # the printout lists the first variant's run
     one = next(iter(one.values()), {}) if sweep else one
     if ycbv:
         for c in sorted(one):
@@ -1718,7 +1880,12 @@ def _main_one_pass(args, precision=None, iterations=None):
         for v in one:
             print('tracked %s: %d frames' % (v, len(one[v])))
     print('-> %s' % args.outdir)
-    if args.score and isinstance(iterations, list):
+    if args.score and ckpts > 1:
+        ref, rows = score_checkpoints(res, outdir, args.ycb_dir, config, precision=precision or 'bf16x3',
+                                      iterations=iterations or 1, **eoat)
+        print_precision_table(ref, rows, sweep='checkpoint sweep', column='variant')
+        print_best_checkpoints(rows, config['ckpt_dir'])
+    elif args.score and isinstance(iterations, list):
         print_precision_table(*score_iterations(res, outdir, args.ycb_dir, config, precision=precision or 'bf16x3', **eoat),
                               sweep='iteration sweep', column='variant')
     elif args.score and sweep:

@@ -9,13 +9,17 @@ step on the device.  PNGs are decoded in a thread pool (cv2 releases the GIL) st
 staging sets, so decoding step k+1 overlaps step k on the GPU.  A batch larger than the engine's max_batch runs as several steps whose sums
 are added in order.  The pairs are taken in file order (the reference's validation loader does not shuffle, train.py:143-149).
 
-    python -m <package>.problems --val_dir DIR --ckpt model_best_val.pth.tar --mean_std_path DIR --dataset_info dataset_info.yml
+    python -m <package>.problems --val_dir DIR --ckpt CKPT[,CKPT...] --mean_std_path DIR[,DIR...] --dataset_info dataset_info.yml
                                  [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200] [--augment config.yml [--seed S]]
     python -m <package>.problems --ycb_dir DIR --class_ids all|3,5 --ckpt_dir TPL --mean_std_path TPL --train_data_path TPL
                                  --model_path TPL [--num_sample 10] [--seed 0] [--precision MODE|all] [--batch_size 200] [--max_batch 200]
 
 The second form scores every class's checkpoint on the perturbed pairs of the YCB-Video key frames in one pass (validate_ycbv):
 bit-identical to `produce_train_pair_data --mode ycbv` followed by the first form on each class's folder, without the files.
+
+Both forms take several checkpoints, comma-separated, with one statistics folder shared by all or one per checkpoint: the pairs
+are decoded (or cut) once and every step runs once per checkpoint and mode, each result what a run of that checkpoint alone
+gives; the table then names, per mode, the checkpoint with the lowest total loss.
 
 --augment evaluates the first form under the reference's train-time augmentations (train.py:85-92, built from config.yml's
 data_augmentation block), as the reference's own validation loss is computed: input B of every pair is augmented inside the
@@ -31,7 +35,8 @@ import numpy as np
 import torch
 
 from .datasets import TrackDataset, read_pair, resize_pair, segB_plane
-from .engine import PREC, IMAGE_SIZE
+from .engine import PREC, IMAGE_SIZE, check_weight_sets_fit
+from .predict import CKPT_ID_STRIDE
 from .staging import StagingRing
 
 
@@ -102,17 +107,37 @@ def _mean_over_batches(x):
     return float(np.array([float(v) for v in x]).mean())
 
 
-def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', keep_predictions=False, workers=None):
-    """The validation pass of `model` (the Se3TrackNet drop-in) over `dataset`'s pairs; see the module docstring."""
-    eng = model.engine
-    if not model._loaded:
-        model._upload()
-    wid = int(model.weight_id)
-    eng.set_stats(np.asarray(dataset.images_mean), np.asarray(dataset.images_std), wid)
+def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', keep_predictions=False, workers=None, stats=None):
+    """The validation pass of `model` (the Se3TrackNet drop-in) over `dataset`'s pairs; see the module docstring.
+
+    The list form compares checkpoints in one pass: `model` a list of Se3TrackNet on one Engine under distinct weight ids and / or
+    `precision` a list of modes.  Each step's pairs are decoded once (and with --augment, input B augmented once, by
+    se3tn_augment_crops) and then run once per variant (model index, mode), each on its own weight set and step sums, so every
+    variant's result is bit for bit what a one-model call gives.  stats: [(mean, std)] per model, default the dataset's for all
+    (train.py writes mean / std per training run).  fp8 calibrates each model's set on the first step as its steps see it.
+    -> {(model index, mode): the one-model call's dict}.  The one-model call returns that dict alone."""
+    many = isinstance(model, (list, tuple)) or isinstance(precision, (list, tuple))
+    models = list(model) if isinstance(model, (list, tuple)) else [model]
+    modes = list(precision) if isinstance(precision, (list, tuple)) else [precision]
+    if not models or not modes:
+        raise ValueError('evaluate needs at least one model and one precision mode')
+    for m in modes:
+        PREC[m]                                             # an unknown mode fails here
+    eng = models[0].engine
+    wids = [int(mdl.weight_id) for mdl in models]
+    if any(mdl.engine is not eng for mdl in models) or len(set(wids)) != len(wids):
+        raise ValueError('the models of one pass share one Engine under distinct weight ids (got ids %s)' % wids)
+    if stats is None:
+        stats = [(dataset.images_mean, dataset.images_std)] * len(models)
+    if len(stats) != len(models):
+        raise ValueError('%d (mean, std) pairs for %d models' % (len(stats), len(models)))
+    for mdl, wid, (mean, std) in zip(models, wids, stats):
+        if not mdl._loaded:
+            mdl._upload()
+        eng.set_stats(np.asarray(mean), np.asarray(std), wid)
     res = int(dataset.dataset_info['resolution']) if dataset.dataset_info is not None else IMAGE_SIZE
     if res != IMAGE_SIZE:
         raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
-    PREC[precision]                                         # an unknown mode fails here
     files = list(dataset.rgbA_files)
     cap = eng.max_batch
     steps = batch_plan(len(files), batch_size, cap, drop_last)
@@ -120,6 +145,7 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
         raise ValueError('no validation batch: %d pairs under %r' % (len(files), dataset.root))
     dev = eng.device
     img = (IMAGE_SIZE, IMAGE_SIZE)
+    variants = [(i, m) for i in range(len(models)) for m in modes]
 
     # the pinned sets decode step k+1 while step k runs; the one device set is what the steps read (uploads ordered on the stream)
     augment = getattr(dataset, 'augment', None)
@@ -132,14 +158,14 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
     A_in_cam, B_in_cam = torch.empty(cap, 4, 4, dtype=torch.float64, device=dev), torch.empty(cap, 4, 4, dtype=torch.float64, device=dev)
     out_trans, out_rot = torch.empty(cap, 3, dtype=torch.float32, device=dev), torch.empty(cap, 3, dtype=torch.float32, device=dev)
     out_sums = torch.empty(2, dtype=torch.float32, device=dev)
-    all_sums = torch.empty(len(steps), 2, dtype=torch.float32, device=dev)
-    preds = torch.empty(len(files), 6, dtype=torch.float32, device=dev) if keep_predictions else None
-    ids_host = np.full(cap, wid, dtype=np.int32) if wid != 0 else None
-    ids_dev = torch.from_numpy(ids_host).to(dev) if ids_host is not None else None
+    all_sums = {v: torch.empty(len(steps), 2, dtype=torch.float32, device=dev) for v in variants}
+    preds = {v: torch.empty(len(files), 6, dtype=torch.float32, device=dev) for v in variants} if keep_predictions else None
+    ids_host = [np.full(cap, w, dtype=np.int32) if w != 0 else None for w in wids]
+    ids_dev = [torch.from_numpy(h).to(dev) if h is not None else None for h in ids_host]
     tn, rn = dataset.trans_normalizer, dataset.rot_normalizer
-    if augment is not None:                                 # each step's pair indices, copied into one buffer: one graph for every step
+    if augment is not None:                                 # input B augmented once per step, read by every variant
         all_index = torch.arange(len(files), dtype=torch.int64, device=dev)
-        pair_index = torch.empty(cap, dtype=torch.int64, device=dev)
+        aug_rgbB, aug_depthB = torch.empty((cap,) + img + (3,), dtype=torch.uint8, device=dev), torch.empty((cap,) + img, dtype=torch.uint16, device=dev)
 
     def decode_into(h, j, path):
         """One pair into row j of staging set h; a pair stored at another size comes back whole for the device resize."""
@@ -175,26 +201,26 @@ def evaluate(model, dataset, batch_size, drop_last=False, precision='bf16x3', ke
                     if seg is not None and seg.dtype != torch.uint8:
                         raise ValueError('%s: augmentation needs segB as an 8-bit image, not %s' % (files[s + j], seg.dtype))
                     d['segB'][j].copy_(seg if seg is not None else (dB.to(torch.int32) > 100).to(torch.uint8))
-            aug = {}
-            if augment is not None:
-                pair_index[:n].copy_(all_index[s:e])
-                aug = dict(augment=augment, segB=d['segB'][:n], pair_index=pair_index[:n])
-            if precision == 'fp8' and k == 0:              # the set's activation scales from the first validation batch
-                rB, dB = d['rgbB'][:n], d['depthB'][:n]
-                if augment is not None and eng.fp8_scales(wid) is None:   # as the steps will see it: input B augmented
-                    rB, dB = eng.augment_crops(augment, rB, dB, pair_index[:n], segB=d['segB'][:n])
-                eng.calibrate_fp8_pairs(d['rgbA'][:n], d['depthA'][:n], rB, dB, A_in_cam[:n], ids_host[:n] if ids_host is not None else None)
-            eng.eval_pairs(d['rgbA'][:n], d['depthA'][:n], d['rgbB'][:n], d['depthB'][:n], A_in_cam[:n], B_in_cam[:n], tn, rn,
-                           weight_ids_host=ids_host[:n] if ids_host is not None else None,
-                           weight_ids_dev=ids_dev[:n] if ids_dev is not None else None, precision=precision,
-                           out_trans=out_trans[:n], out_rot=out_rot[:n], out_sums=out_sums, **aug)
-            all_sums[k].copy_(out_sums)
-            if preds is not None:
-                preds[s:e, :3].copy_(out_trans[:n]); preds[s:e, 3:].copy_(out_rot[:n])
-    step_sums = all_sums.cpu().numpy()
-    bt, br = batch_means(step_sums, steps)
-    return dict(trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
-                predictions=preds.cpu().numpy() if preds is not None else None)
+            rB, dB = d['rgbB'][:n], d['depthB'][:n]
+            if augment is not None:                         # what se3tn_eval_pairs_augmented evaluates, formed once
+                rB, dB = eng.augment_crops(augment, rB, dB, all_index[s:e], segB=d['segB'][:n], out_rgbB=aug_rgbB[:n],
+                                           out_depthB=aug_depthB[:n])
+            for i, m in variants:
+                wh = ids_host[i][:n] if ids_host[i] is not None else None
+                if m == 'fp8' and k == 0:                   # the set's activation scales from the first batch, as the steps see it
+                    eng.calibrate_fp8_pairs(d['rgbA'][:n], d['depthA'][:n], rB, dB, A_in_cam[:n], wh)
+                eng.eval_pairs(d['rgbA'][:n], d['depthA'][:n], rB, dB, A_in_cam[:n], B_in_cam[:n], tn, rn, weight_ids_host=wh,
+                               weight_ids_dev=ids_dev[i][:n] if ids_dev[i] is not None else None, precision=m,
+                               out_trans=out_trans[:n], out_rot=out_rot[:n], out_sums=out_sums)
+                all_sums[i, m][k].copy_(out_sums)
+                if preds is not None:
+                    preds[i, m][s:e, :3].copy_(out_trans[:n]); preds[i, m][s:e, 3:].copy_(out_rot[:n])
+    out = {}
+    for v in variants:
+        bt, br = batch_means(all_sums[v].cpu().numpy(), steps)
+        out[v] = dict(trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
+                      predictions=preds[v].cpu().numpy() if preds is not None else None)
+    return out if many else out[0, modes[0]]
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -220,9 +246,11 @@ class PairQueues:
               ('rgbB', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthB', torch.uint16, (IMAGE_SIZE, IMAGE_SIZE)),
               ('A_in_cam', torch.float64, (4, 4)), ('B_in_cam', torch.float64, (4, 4)))
 
-    def __init__(self, eng, normalizers, modes, batch_size, max_batch, rows_per_frame, keep_predictions=False):
+    def __init__(self, eng, normalizers, modes, batch_size, max_batch, rows_per_frame, keep_predictions=False, ckpts=1):
         """normalizers: {class id (the weight set and mesh id): (trans_normalizer, rot_normalizer)}.  rows_per_frame: the most
-        rows one frame sends to one class (num_sample).  max_batch: the most pairs per validation step."""
+        rows one frame sends to one class (num_sample).  max_batch: the most pairs per validation step.  ckpts: the number of
+        checkpoints; checkpoint i's set of class c is weight id c + CKPT_ID_STRIDE * i, and every batch runs once per checkpoint
+        and mode."""
         if batch_size <= 0 or max_batch <= 0 or rows_per_frame <= 0:
             raise ValueError('batch_size, max_batch and rows_per_frame must be positive')
         self.eng = eng
@@ -248,11 +276,13 @@ class PairQueues:
         self.out_trans = torch.empty(self.step, 3, dtype=torch.float32, device=dev)
         self.out_rot = torch.empty(self.step, 3, dtype=torch.float32, device=dev)
         self.out_sums = torch.empty(2, dtype=torch.float32, device=dev)
-        self.ids_host = {c: np.full(self.step, c, dtype=np.int32) for c in self.ids}
-        self.ids_dev = {c: torch.from_numpy(self.ids_host[c]).to(dev) for c in self.ids}
+        self.variants = [(i, m) for i in range(int(ckpts)) for m in self.modes]
+        wids = [c + CKPT_ID_STRIDE * i for c in self.ids for i in range(int(ckpts))]
+        self.ids_host = {w: np.full(self.step, w, dtype=np.int32) for w in wids}
+        self.ids_dev = {w: torch.from_numpy(self.ids_host[w]).to(dev) for w in wids}
         self.pairs = {c: 0 for c in self.ids}
-        self.sums = {c: {m: [] for m in self.modes} for c in self.ids}
-        self.preds = {c: {m: [] for m in self.modes} for c in self.ids}
+        self.sums = {c: {v: [] for v in self.variants} for c in self.ids}
+        self.preds = {c: {v: [] for v in self.variants} for c in self.ids}
         self.calibrated = set()
 
     def add(self, owners, chunks):
@@ -276,25 +306,26 @@ class PairQueues:
                 self._back_done.record(torch.cuda.current_stream(self.eng.device))
 
     def finish(self):
-        """Drain every queue, the partial last batches included -> {class id: {mode: dict}}: `evaluate`'s dict plus 'pairs'.  A
-        class without a kept pair has pairs 0, trans / rot None, empty batch losses and predictions None."""
+        """Drain every queue, the partial last batches included -> {class id: {mode: dict}}: `evaluate`'s dict plus 'pairs'; with
+        several checkpoints {checkpoint index: that}.  A class without a kept pair has pairs 0, trans / rot None, empty batch
+        losses and predictions None."""
         self._drain(final=True)
         out = {}
         for c in self.ids:
             n = self.pairs[c]
-            out[c] = {}
-            for m in self.modes:
+            for i, m in self.variants:
+                o = out.setdefault(i, {}).setdefault(c, {})
                 if n == 0:
-                    out[c][m] = dict(pairs=0, trans=None, rot=None, batch_trans=np.zeros(0, np.float32), batch_rot=np.zeros(0, np.float32),
+                    o[m] = dict(pairs=0, trans=None, rot=None, batch_trans=np.zeros(0, np.float32), batch_rot=np.zeros(0, np.float32),
                                      predictions=None)
                     continue
                 steps = batch_plan(n, self.batch_size, self.step)
-                assert len(steps) == len(self.sums[c][m])
-                bt, br = batch_means(torch.stack(self.sums[c][m]).cpu().numpy(), steps)
-                preds = torch.cat(self.preds[c][m]).cpu().numpy() if self.keep_predictions else None
-                out[c][m] = dict(pairs=n, trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
+                assert len(steps) == len(self.sums[c][i, m])
+                bt, br = batch_means(torch.stack(self.sums[c][i, m]).cpu().numpy(), steps)
+                preds = torch.cat(self.preds[c][i, m]).cpu().numpy() if self.keep_predictions else None
+                o[m] = dict(pairs=n, trans=_mean_over_batches(bt), rot=_mean_over_batches(br), batch_trans=bt, batch_rot=br,
                                  predictions=preds)
-        return out
+        return out if len(out) > 1 else out[0]
 
     def _drain(self, final):
         """Read the tails back, run every full batch (and with `final` every partial one), move the remainders to the front."""
@@ -320,22 +351,23 @@ class PairQueues:
             self.tails_dev.copy_(torch.from_numpy(self.tails))
 
     def _eval_batch(self, q, c, n_rows):
-        """Rows [0, n_rows) of queue q as one loader batch, in every mode."""
+        """Rows [0, n_rows) of queue q as one loader batch, in every checkpoint and mode."""
         tn, rn = self.normalizers[c]
         d = self.queues
-        for m in self.modes:
+        for i, m in self.variants:
+            w = c + CKPT_ID_STRIDE * i
             for _, s, e in batch_plan(n_rows, self.batch_size, self.step):
                 n = e - s
                 pairs = [d[k][q, s:e] for k in ('rgbA', 'depthA', 'rgbB', 'depthB')]
-                if m == 'fp8' and c not in self.calibrated:      # the set's scales from its first step, as evaluate's k == 0
-                    self.eng.calibrate_fp8_pairs(*pairs, d['A_in_cam'][q, s:e], self.ids_host[c][:n])
-                    self.calibrated.add(c)
-                self.eng.eval_pairs(*pairs, d['A_in_cam'][q, s:e], d['B_in_cam'][q, s:e], tn, rn, weight_ids_host=self.ids_host[c][:n],
-                                    weight_ids_dev=self.ids_dev[c][:n], precision=m, out_trans=self.out_trans[:n],
+                if m == 'fp8' and w not in self.calibrated:      # the set's scales from its first step, as evaluate's k == 0
+                    self.eng.calibrate_fp8_pairs(*pairs, d['A_in_cam'][q, s:e], self.ids_host[w][:n])
+                    self.calibrated.add(w)
+                self.eng.eval_pairs(*pairs, d['A_in_cam'][q, s:e], d['B_in_cam'][q, s:e], tn, rn, weight_ids_host=self.ids_host[w][:n],
+                                    weight_ids_dev=self.ids_dev[w][:n], precision=m, out_trans=self.out_trans[:n],
                                     out_rot=self.out_rot[:n], out_sums=self.out_sums)
-                self.sums[c][m].append(self.out_sums.clone())
+                self.sums[c][i, m].append(self.out_sums.clone())
                 if self.keep_predictions:
-                    self.preds[c][m].append(torch.cat((self.out_trans[:n], self.out_rot[:n]), 1))
+                    self.preds[c][i, m].append(torch.cat((self.out_trans[:n], self.out_rot[:n]), 1))
         self.pairs[c] += n_rows
 
 
@@ -354,35 +386,44 @@ def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_si
     rows) holds every class's weights, statistics and mesh under id = class id.  Each class's loss uses its dataset_info.yml's
     max_translation and max_rotation * pi / 180, as the loader's labels do.  fp8 calibrates each class on its first step.
 
-    -> {class id: {mode: evaluate's dict plus 'pairs'}}.  A class without a kept pair is reported with 0 pairs and no loss
+    templates may give ckpt_dir (and mean_std_path) as lists, one entry per checkpoint (mean_std_path: one shared, or one per
+    checkpoint): checkpoint i's set of class c is weight id c + 32 i.  The pairs are cut and queued once per class, and every
+    batch runs once per checkpoint and mode, so each checkpoint's result is what a run of it alone returns.
+
+    -> {class id: {mode: evaluate's dict plus 'pairs'}}; with several checkpoints {checkpoint index: that}.  A class without a kept pair is reported with 0 pairs and no loss
     (trans / rot None), where `evaluate` on its empty folder raises ValueError.  The queues take
     classes x (batch_size + num_sample) x 176 x 176 x 10 bytes of device memory (about 1.4 GB for 21 classes at 200 and 10)."""
     from .engine import Engine
-    from .predict import ycb_classes, expand_class_paths, _load_run_files
+    from .predict import ycb_classes, expand_class_paths, _load_run_files, checkpoint_configs, _check_checkpoint_ids
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
     modes = list(precisions)
     for m in modes:
         PREC[m]                                             # an unknown mode fails here
+    configs = checkpoint_configs(templates)
     classes = ycb_classes(ycb_dir, class_ids)
     if not classes:
         raise ValueError('no class ids given')
     ids = [c for c, _ in classes]
+    _check_checkpoint_ids(ids, len(configs), 'class')
     runs = {}
-    for c, name in classes:
-        runs[c] = _load_run_files('class %d (%s)' % (c, name), expand_class_paths(templates, c, name))
-        if int(runs[c]['dataset_info']['resolution']) != IMAGE_SIZE:
-            raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
+    for i, cfg in enumerate(configs):
+        for c, name in classes:
+            runs[c, i] = _load_run_files('class %d (%s)' % (c, name), expand_class_paths(cfg, c, name))
+            if int(runs[c, i]['dataset_info']['resolution']) != IMAGE_SIZE:
+                raise NotImplementedError('libse3tn is built for the reference resolution of 176 (dataset_info.yml:15)')
+    if len(configs) > 1:
+        check_weight_sets_fit(len(runs), what='weight sets (checkpoints x classes)')
     step = min(int(max_batch), int(batch_size))
     eng = engine if engine is not None else Engine(max_batch=max(step, len(ids) * int(num_sample)))
     normalizers = {}
-    for c in ids:
-        info = runs[c]['dataset_info']
-        ckpt = torch.load(runs[c]['ckpt_dir'], map_location='cpu')
-        eng.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt, c)
-        eng.set_stats(np.asarray(runs[c]['mean']), np.asarray(runs[c]['std']), c)
+    for (c, i), run in runs.items():
+        info = runs[c, 0]['dataset_info']
+        ckpt = torch.load(run['ckpt_dir'], map_location='cpu')
+        eng.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt, c + CKPT_ID_STRIDE * i)
+        eng.set_stats(np.asarray(run['mean']), np.asarray(run['std']), c + CKPT_ID_STRIDE * i)
         normalizers[c] = (info['max_translation'], info['max_rotation'] * np.pi / 180)
-    _, producers = ycbv_producers(ycb_dir, ids, templates, eng, workers)
-    queues = PairQueues(eng, normalizers, modes, batch_size, step, num_sample, keep_predictions)
+    _, producers = ycbv_producers(ycb_dir, ids, configs[0], eng, workers)
+    queues = PairQueues(eng, normalizers, modes, batch_size, step, num_sample, keep_predictions, len(configs))
     random.seed(seed); np.random.seed(seed)
     jobs = ycbv_keyframe_jobs(ycb_dir, ids)
     for owners, chunks in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True):
@@ -440,30 +481,69 @@ def main(argv=None):
         ap.error('--val_dir needs --ckpt, --mean_std_path and --dataset_info')
     import yaml
     from .se3_tracknet import Se3TrackNet
+    from .predict import checkpoint_list
+    try:
+        runs = checkpoint_list(args.ckpt.split(','), args.mean_std_path.split(','), '--ckpt', '--mean_std_path')
+    except ValueError as e:
+        ap.error(str(e))
+    if len(runs) > 1:
+        check_weight_sets_fit(len(runs), what='checkpoints')
     with open(args.dataset_info) as f:
         info = yaml.safe_load(f)
-    mean = np.load(os.path.join(args.mean_std_path, 'mean.npy'))
-    std = np.load(os.path.join(args.mean_std_path, 'std.npy'))
+    stats = [(np.load(os.path.join(d, 'mean.npy')), np.load(os.path.join(d, 'std.npy'))) for _, d in runs]
     augmentations = None
     if args.augment:
         from .data_augmentation import from_config
         with open(args.augment) as f:
             augmentations = from_config(yaml.safe_load(f))
-    ds = TrackDataset(args.val_dir, 'val', mean, std, None, augmentations, None, dataset_info=info,
+    ds = TrackDataset(args.val_dir, 'val', stats[0][0], stats[0][1], None, augmentations, None, dataset_info=info,
                       trans_normalizer=info['max_translation'], rot_normalizer=info['max_rotation'] * np.pi / 180, augment_seed=args.seed)
-    loader = torch.utils.data.DataLoader(ds, batch_size=args.batch_size, shuffle=False, drop_last=False)
-    ckpt = torch.load(args.ckpt, map_location='cpu')
-    model = Se3TrackNet(image_size=int(info['resolution']), max_batch=min(args.max_batch, args.batch_size))
-    model.load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt)
-    prob = Problem(model, None, loader, config={'loss_weights': {'trans': 1, 'rot': 1}})   # config.yml:13-15
-    print('%d pairs, batch %d, %s%s' % (len(ds), args.batch_size, torch.cuda.get_device_name(model.engine.device),
+    models = []
+    for i, (path, _) in enumerate(runs):
+        ckpt = torch.load(path, map_location='cpu')
+        models.append(Se3TrackNet(image_size=int(info['resolution']), max_batch=min(args.max_batch, args.batch_size),
+                                  engine=models[0].engine if models else None, weight_id=i))
+        models[-1].load_state_dict(ckpt['state_dict'] if 'state_dict' in ckpt else ckpt)
+    w = {'trans': 1, 'rot': 1}                                                          # config.yml:13-15
+    print('%d pairs, batch %d, %s%s' % (len(ds), args.batch_size, torch.cuda.get_device_name(models[0].engine.device),
                                         ", augmented (train.py's chain, seed %d)" % args.seed if args.augment else ''))
-    _print_modes(modes, lambda m: prob.validation_losses(m, keep_predictions=len(modes) > 1), prob.loss_weights)
+    res = evaluate(models, ds, args.batch_size, False, modes, keep_predictions=len(modes) > 1, stats=stats)
+    _print_checkpoints([p for p, _ in runs], modes, res, w)
+    return res
+
+
+def best_checkpoint(totals):
+    """The index of the lowest of `totals`, the first listed among equals: Problem.loop keeps a checkpoint only when its
+    validation loss is strictly below the best so far (problems.py:146-151)."""
+    best = 0
+    for i, t in enumerate(totals):
+        if t < totals[best]:
+            best = i
+    return best
+
+
+def _print_checkpoints(names, modes, res, w):
+    """The table of one pass over several checkpoints (res: {(checkpoint index, mode): evaluate's dict}): one row per checkpoint
+    and mode as _print_modes lays them out, max |d6| measured within each checkpoint from its first mode; then per mode the
+    checkpoint Problem.loop would keep (best_checkpoint).  A single checkpoint prints _print_modes' table alone."""
+    if len(names) == 1:
+        _print_modes(modes, lambda m: res[0, m], w)
+        return
+    total = lambda r: r['trans'] * w['trans'] + r['rot'] * w['rot']
+    print('%-5s %-8s %14s %14s %14s %s' % ('ckpt', 'mode', 'trans loss', 'rot loss', 'total', 'max |d6| vs %s' % modes[0] if len(modes) > 1 else ''))
+    for i in range(len(names)):
+        for m in modes:
+            r = res[i, m]
+            dev6 = '%.3e' % float(np.abs(r['predictions'] - res[i, modes[0]]['predictions']).max()) if len(modes) > 1 else ''
+            print('%-5d %-8s %14.8g %14.8g %14.8g %s' % (i, m, r['trans'], r['rot'], total(r), dev6))
+    for m in modes:
+        b = best_checkpoint([total(res[i, m]) for i in range(len(names))])
+        print('best %s: checkpoint %d (%s), total %.8g' % (m, b, names[b], total(res[b, m])))
 
 
 def _main_ycbv(ap, args, modes):
     """--ycb_dir: validate_ycbv, then per class the table --val_dir prints."""
-    from .predict import ycb_class_names, YCB_ALL_TEMPLATES
+    from .predict import ycb_class_names, YCB_ALL_TEMPLATES, checkpoint_configs
     if args.ckpt or args.dataset_info:
         ap.error('--ycb_dir takes --ckpt_dir and --train_data_path templates, not --ckpt / --dataset_info')
     if not args.class_ids or not all(getattr(args, k) for k in YCB_ALL_TEMPLATES):
@@ -476,16 +556,26 @@ def _main_ycbv(ap, args, modes):
             ids = sorted(set(int(c) for c in args.class_ids.split(',')))
         except ValueError:
             ap.error('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
-    res = validate_ycbv(args.ycb_dir, ids, {k: getattr(args, k) for k in YCB_ALL_TEMPLATES}, num_sample=args.num_sample, seed=args.seed,
-                        batch_size=args.batch_size, max_batch=args.max_batch, precisions=modes, keep_predictions=len(modes) > 1)
+    templates = {k: getattr(args, k) for k in YCB_ALL_TEMPLATES}
+    for key in ('ckpt_dir', 'mean_std_path'):                   # template lists: one pass over several checkpoints
+        if ',' in templates[key]:
+            templates[key] = templates[key].split(',')
+    try:
+        ckpts = [cfg['ckpt_dir'] for cfg in checkpoint_configs(templates)]
+    except ValueError as e:
+        ap.error(str(e))
+    res = validate_ycbv(args.ycb_dir, ids, templates, num_sample=args.num_sample, seed=args.seed, batch_size=args.batch_size,
+                        max_batch=args.max_batch, precisions=modes, keep_predictions=len(modes) > 1)
+    per_ckpt = [res[i] for i in range(len(ckpts))] if len(ckpts) > 1 else [res]
     device = torch.cuda.get_device_name(torch.cuda.current_device())
     for c in ids:
-        n = res[c][modes[0]]['pairs']
+        n = per_ckpt[0][c][modes[0]]['pairs']
         print('class %d (%s): %d pairs, batch %d, %s' % (c, names[c - 1], n, args.batch_size, device))
         if n == 0:
             print('no kept pair: no loss')
             continue
-        _print_modes(modes, lambda m: res[c][m], {'trans': 1, 'rot': 1})                        # config.yml:13-15
+        _print_checkpoints(ckpts, modes, {(i, m): r[c][m] for i, r in enumerate(per_ckpt) for m in modes},
+                           {'trans': 1, 'rot': 1})                                      # config.yml:13-15
     return res
 
 
