@@ -537,6 +537,17 @@ int se3tn_append_pairs(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* dept
                        uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
                        void* stream);
 
+/* se3tn_append_pairs with a fifth plane: segB uint8 (n,176,176) device, as se3tn_perturb_pairs writes it, goes with its row to
+ * q_segB uint8 (num_queues,cap,176,176) device, slot q * cap + s like the other planes (BlackCover's mask when the queued pairs
+ * are augmented).  The same single launch, copies and checks; segB and q_segB must also be non-null and 16-byte aligned.
+ * se3tn_append_pairs' four planes, poses and tails come out byte for byte as it writes them. */
+int se3tn_append_pairs_seg(se3tn_ctx* ctx, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                           const int32_t* seg_count, const double* A_in_cam, const double* B_in_cam,
+                           const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
+                           int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
+                           uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
+                           const uint8_t* segB, uint8_t* q_segB, void* stream);
+
 /* ---- introspection (tests / profiling) -------------------------------------------------------- */
 
 /* Device pointer + per-image float count of an internal NHWC activation buffer.

@@ -68,6 +68,8 @@ SIGNATURES = {
     'se3tn_perturb_pairs': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_append_pairs': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp,
                                 _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_append_pairs_seg': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_debug_buffer': (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_sz)]),
     'se3tn_last_launch_count': (_i, [_vp]),
     'se3tn_get_trace': (_i, [_vp, _vp]),

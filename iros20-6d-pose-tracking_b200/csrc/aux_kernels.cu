@@ -311,13 +311,13 @@ cudaError_t launch_crop_seg(const uint8_t* frame_rgb, const uint16_t* frame_dept
 // =============================================================================================
 // se3tn_append_pairs: the kept rows of a pair step to the tails of their validation queues
 // =============================================================================================
-// Grid (kAppendSlices, n): CTA (x, i) copies slice x of row i's four planes in 16-byte words (consecutive threads, consecutive
-// words) and, in slice 0, its two poses.  Row i's slot is its queue's tail plus the kept rows of that queue before it, counted by
-// the whole CTA.  Every CTA reads the tail before it counts itself done on a.done; the CTA that counts last has seen every other
-// one read, so it alone adds each queue's kept rows to its tail, then clears the counter for the next launch.
+// Grid (kAppendSlices, n): CTA (x, i) copies slice x of row i's four planes (five with a.segB) in 16-byte words (consecutive
+// threads, consecutive words) and, in slice 0, its two poses.  Row i's slot is its queue's tail plus the kept rows of that queue
+// before it, counted by the whole CTA.  Every CTA reads the tail before it counts itself done on a.done; the CTA that counts last
+// has seen every other one read, so it alone adds each queue's kept rows to its tail, then clears the counter for the next launch.
 constexpr int kAppendThreads = 256, kAppendSlices = 8;
-constexpr int kRgbWords = kImg * kImg * 3 / 16, kDepthWords = kImg * kImg * 2 / 16, kPoseWords = 16 * 8 / 16;
-static_assert(kImg * kImg * 3 % 16 == 0 && kImg * kImg * 2 % 16 == 0, "a crop plane is a whole number of 16-byte words");
+constexpr int kRgbWords = kImg * kImg * 3 / 16, kDepthWords = kImg * kImg * 2 / 16, kSegWords = kImg * kImg / 16, kPoseWords = 16 * 8 / 16;
+static_assert(kImg * kImg % 16 == 0, "a crop plane is a whole number of 16-byte words");
 
 __device__ __forceinline__ void copy_words(const void* src, void* dst, int words) {
     const uint4* s = static_cast<const uint4*>(src);
@@ -345,6 +345,7 @@ __global__ void __launch_bounds__(kAppendThreads) append_pairs_kernel(const Appe
         copy_words(a.rgbB + src * kRgbWords * 16, a.q_rgbB + dst * kRgbWords * 16, kRgbWords);
         copy_words(a.depthA + src * kDepthWords * 8, a.q_depthA + dst * kDepthWords * 8, kDepthWords);
         copy_words(a.depthB + src * kDepthWords * 8, a.q_depthB + dst * kDepthWords * 8, kDepthWords);
+        if (a.segB) copy_words(a.segB + src * kSegWords * 16, a.q_segB + dst * kSegWords * 16, kSegWords);
         if (blockIdx.x == 0 && threadIdx.x < 2 * kPoseWords) {
             const bool b = threadIdx.x >= kPoseWords;
             const int w = threadIdx.x - (b ? kPoseWords : 0);

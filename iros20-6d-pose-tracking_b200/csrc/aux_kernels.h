@@ -61,6 +61,7 @@ struct AppendArgs {
     int* tails;                    // (num_queues), advanced by the CTA that finishes last
     unsigned* done;                // context-owned CTA counter, zero between launches
     uint8_t* q_rgbA; uint16_t* q_depthA; uint8_t* q_rgbB; uint16_t* q_depthB; double* q_A; double* q_B;   // (num_queues * cap, ...)
+    const uint8_t* segB; uint8_t* q_segB;   // optional fifth plane, (n, 176, 176) -> (num_queues * cap, 176, 176); null: not copied
 };
 cudaError_t launch_append_pairs(const AppendArgs& a, cudaStream_t s);
 cudaError_t launch_nchw_to_stem(const float* src, float* dst, int n, int precision, cudaStream_t s);

@@ -1709,31 +1709,34 @@ int se3tn_perturb_pairs(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* 
     return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
-int se3tn_append_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
-                       const int32_t* seg_count, const double* A_in_cam, const double* B_in_cam,
-                       const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
-                       int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
-                       uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
-                       void* stream) {
+// se3tn_append_pairs (with_seg false: segB / q_segB are ignored and the kernel copies four planes) and se3tn_append_pairs_seg
+static int append_pairs(se3tn_ctx* c, const char* fn, bool with_seg, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB,
+                        const uint16_t* depthB, const uint8_t* segB, const int32_t* seg_count, const double* A_in_cam,
+                        const double* B_in_cam, const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
+                        int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
+                        uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, uint8_t* q_segB,
+                        double* q_A_in_cam, double* q_B_in_cam, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
-    const void* words[] = {rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, q_rgbA, q_depthA, q_rgbB, q_depthB, q_A_in_cam, q_B_in_cam};
+    const std::string name(fn);
+    const void* words[] = {rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, q_rgbA, q_depthA, q_rgbB, q_depthB, q_A_in_cam, q_B_in_cam,
+                           with_seg ? segB : rgbA, with_seg ? q_segB : rgbA};
     for (const void* p : words)
         if (!p || reinterpret_cast<uintptr_t>(p) % 16)
-            return fail(c, SE3TN_ERR_INVALID, "se3tn_append_pairs: a pair or queue array is null or not 16-byte aligned");
+            return fail(c, SE3TN_ERR_INVALID, name + ": a pair or queue array is null or not 16-byte aligned");
     if (!seg_count || !queue_ids_host || !queue_ids_dev || !tails_host || !tails_dev || n < 0 || num_queues <= 0 || cap <= 0)
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_append_pairs: null/invalid argument");
-    if (n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, "se3tn_append_pairs: n exceeds max_batch");
+        return fail(c, SE3TN_ERR_INVALID, name + ": null/invalid argument");
+    if (n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, name + ": n exceeds max_batch");
     std::vector<int> rows(num_queues, 0);
     for (int i = 0; i < n; ++i) {
         const int q = queue_ids_host[i];
         if (q < 0 || q >= num_queues)
-            return fail(c, SE3TN_ERR_INVALID, "se3tn_append_pairs: row " + std::to_string(i) + " has queue id " + std::to_string(q) +
+            return fail(c, SE3TN_ERR_INVALID, name + ": row " + std::to_string(i) + " has queue id " + std::to_string(q) +
                                               ", outside [0, " + std::to_string(num_queues) + ")");
         ++rows[q];
     }
     for (int q = 0; q < num_queues; ++q)
         if (tails_host[q] < 0 || static_cast<long long>(tails_host[q]) + rows[q] > cap)
-            return fail(c, SE3TN_ERR_INVALID, "se3tn_append_pairs: queue " + std::to_string(q) + " holds " + std::to_string(tails_host[q]) +
+            return fail(c, SE3TN_ERR_INVALID, name + ": queue " + std::to_string(q) + " holds " + std::to_string(tails_host[q]) +
                                               " of " + std::to_string(cap) + " rows and cannot take " + std::to_string(rows[q]) + " more");
     if (n == 0) return SE3TN_OK;
     DeviceGuard guard(c->device);
@@ -1742,16 +1745,39 @@ int se3tn_append_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA
         CU_TRY(c, grow(c->append_done, c->append_done_words, 1));
         CU_TRY(c, cudaMemsetAsync(c->append_done.get(), 0, sizeof(unsigned), s));
     }
-    AppendArgs a;
+    AppendArgs a{};
     a.rgbA = rgbA; a.depthA = depthA; a.rgbB = rgbB; a.depthB = depthB;
     a.count = seg_count; a.A_in_cam = A_in_cam; a.B_in_cam = B_in_cam; a.queue_ids = queue_ids_dev;
     a.n = n; a.num_queues = num_queues; a.cap = cap; a.min_count = SE3TN_PAIR_MIN_SEG;
     a.tails = tails_dev; a.done = c->append_done.get();
     a.q_rgbA = q_rgbA; a.q_depthA = q_depthA; a.q_rgbB = q_rgbB; a.q_depthB = q_depthB; a.q_A = q_A_in_cam; a.q_B = q_B_in_cam;
+    if (with_seg) a.segB = segB, a.q_segB = q_segB;
     c->launches = 0;
     CU_TRY(c, launch_append_pairs(a, s));
     c->launches = 1;
     return SE3TN_OK;
+}
+
+int se3tn_append_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                       const int32_t* seg_count, const double* A_in_cam, const double* B_in_cam,
+                       const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
+                       int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
+                       uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
+                       void* stream) {
+    return append_pairs(c, "se3tn_append_pairs", false, rgbA, depthA, rgbB, depthB, nullptr, seg_count, A_in_cam, B_in_cam, queue_ids_host,
+                        queue_ids_dev, n, num_queues, cap, tails_host, tails_dev, q_rgbA, q_depthA, q_rgbB, q_depthB, nullptr,
+                        q_A_in_cam, q_B_in_cam, stream);
+}
+
+int se3tn_append_pairs_seg(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
+                           const int32_t* seg_count, const double* A_in_cam, const double* B_in_cam,
+                           const int32_t* queue_ids_host, const int32_t* queue_ids_dev, int n,
+                           int num_queues, int cap, const int32_t* tails_host, int32_t* tails_dev,
+                           uint8_t* q_rgbA, uint16_t* q_depthA, uint8_t* q_rgbB, uint16_t* q_depthB, double* q_A_in_cam, double* q_B_in_cam,
+                           const uint8_t* segB, uint8_t* q_segB, void* stream) {
+    return append_pairs(c, "se3tn_append_pairs_seg", true, rgbA, depthA, rgbB, depthB, segB, seg_count, A_in_cam, B_in_cam, queue_ids_host,
+                        queue_ids_dev, n, num_queues, cap, tails_host, tails_dev, q_rgbA, q_depthA, q_rgbB, q_depthB, q_segB,
+                        q_A_in_cam, q_B_in_cam, stream);
 }
 
 int se3tn_add_adi(se3tn_ctx* c, const double* model_pts, int m, const double* pred, const double* gt, int n,

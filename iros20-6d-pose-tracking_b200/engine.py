@@ -664,17 +664,21 @@ class Engine:
         queue_ids int32 host array (n), uploaded unless queue_ids_dev is given; tails_host int32 host array (Q): what tails_dev
         (int32 CUDA (Q)) holds when the append runs, read only by the capacity check; queues: dict rgbA, depthA, rgbB, depthB,
         A_in_cam, B_in_cam of CUDA tensors (Q, cap, ...) in eval_pairs' layout.  A row is kept when its count reaches
-        _lib.PAIR_MIN_SEG; tails_dev advances on the device."""
+        _lib.PAIR_MIN_SEG; tails_dev advances on the device.  When queues also holds 'segB' (uint8 (Q, cap, 176, 176)), each kept
+        row's pairs['segB'] goes with it, in the same launch (se3tn_append_pairs_seg)."""
         n = int(A_in_cam.shape[0])
         Q, cap = int(queues['rgbA'].shape[0]), int(queues['rgbA'].shape[1])
         img = (IMAGE_SIZE, IMAGE_SIZE)
+        seg = 'segB' in queues
         for name, t, dt, shape in (('rgbA', pairs['rgbA'], torch.uint8, (n,) + img + (3,)), ('depthA', pairs['depthA'], torch.uint16, (n,) + img),
                                    ('rgbB', pairs['rgbB'], torch.uint8, (n,) + img + (3,)), ('depthB', pairs['depthB'], torch.uint16, (n,) + img),
                                    ('count', pairs['count'], torch.int32, (n,)), ('A_in_cam', A_in_cam, torch.float64, (n, 4, 4)),
-                                   ('B_in_cam', B_in_cam, torch.float64, (n, 4, 4)), ('tails_dev', tails_dev, torch.int32, (Q,))):
+                                   ('B_in_cam', B_in_cam, torch.float64, (n, 4, 4)), ('tails_dev', tails_dev, torch.int32, (Q,))) + \
+                ((('segB', pairs.get('segB'), torch.uint8, (n,) + img),) if seg else ()):
             self._check_dev(name, t, dt, shape)
         for name, dt, shape in (('rgbA', torch.uint8, img + (3,)), ('depthA', torch.uint16, img), ('rgbB', torch.uint8, img + (3,)),
-                                ('depthB', torch.uint16, img), ('A_in_cam', torch.float64, (4, 4)), ('B_in_cam', torch.float64, (4, 4))):
+                                ('depthB', torch.uint16, img), ('A_in_cam', torch.float64, (4, 4)), ('B_in_cam', torch.float64, (4, 4))) + \
+                ((('segB', torch.uint8, img),) if seg else ()):
             self._check_dev('queues[%r]' % name, queues[name], dt, (Q, cap) + shape)
         qh = self._host_ids('append_pairs', queue_ids, n)
         th = np.ascontiguousarray(tails_host, dtype=np.int32)
@@ -682,10 +686,13 @@ class Engine:
             raise ValueError('append_pairs: tails_host must have one entry per queue')
         if queue_ids_dev is None:
             queue_ids_dev = torch.from_numpy(qh).to(self.device)
-        _lib.check(self.lib.se3tn_append_pairs(self._ctx, *(_ptr(pairs[k]) for k in ('rgbA', 'depthA', 'rgbB', 'depthB', 'count')),
-                                               _ptr(A_in_cam), _ptr(B_in_cam), _hptr(qh), _ptr(queue_ids_dev), n, Q, cap, _hptr(th),
-                                               _ptr(tails_dev), *(_ptr(queues[k]) for k in ('rgbA', 'depthA', 'rgbB', 'depthB', 'A_in_cam', 'B_in_cam')),
-                                               _stream(self.device)), self._ctx)
+        args = (self._ctx, *(_ptr(pairs[k]) for k in ('rgbA', 'depthA', 'rgbB', 'depthB', 'count')), _ptr(A_in_cam), _ptr(B_in_cam),
+                _hptr(qh), _ptr(queue_ids_dev), n, Q, cap, _hptr(th), _ptr(tails_dev),
+                *(_ptr(queues[k]) for k in ('rgbA', 'depthA', 'rgbB', 'depthB', 'A_in_cam', 'B_in_cam')))
+        if seg:
+            _lib.check(self.lib.se3tn_append_pairs_seg(*args, _ptr(pairs['segB']), _ptr(queues['segB']), _stream(self.device)), self._ctx)
+        else:
+            _lib.check(self.lib.se3tn_append_pairs(*args, _stream(self.device)), self._ctx)
 
     def _dev_ids(self, ids, n):
         """int32 (n) ids as a contiguous CUDA tensor (host arrays are uploaded)."""

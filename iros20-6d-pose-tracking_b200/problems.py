@@ -13,6 +13,7 @@ are added in order.  The pairs are taken in file order (the reference's validati
                                  [--precision bf16x3|tf32|bf16|fp16|fp8|fp32|all] [--batch_size 200] [--augment config.yml [--seed S]]
     python -m <package>.problems --ycb_dir DIR --class_ids all|3,5 --ckpt_dir TPL --mean_std_path TPL --train_data_path TPL
                                  --model_path TPL [--num_sample 10] [--seed 0] [--precision MODE|all] [--batch_size 200] [--max_batch 200]
+                                 [--augment config.yml]
 
 The second form scores every class's checkpoint on the perturbed pairs of the YCB-Video key frames in one pass (validate_ycbv):
 bit-identical to `produce_train_pair_data --mode ycbv` followed by the first form on each class's folder, without the files.
@@ -21,10 +22,12 @@ Both forms take several checkpoints, comma-separated, with one statistics folder
 are decoded (or cut) once and every step runs once per checkpoint and mode, each result what a run of that checkpoint alone
 gives; the table then names, per mode, the checkpoint with the lowest total loss.
 
---augment evaluates the first form under the reference's train-time augmentations (train.py:85-92, built from config.yml's
-data_augmentation block), as the reference's own validation loss is computed: input B of every pair is augmented inside the
-validation step (se3tn_eval_pairs_augmented), each pair's draws keyed by (--seed, its index in the sorted file list), so every
-mode of --precision all sees the same augmented pairs.
+--augment evaluates either form under the reference's train-time augmentations (train.py:85-92, built from config.yml's
+data_augmentation block), as the reference's own validation loss is computed: input B of every pair is augmented once per step
+(se3tn_augment_crops), each pair's draws keyed by (--seed, its index in the sorted file list), so every checkpoint and every
+mode of --precision all sees the same augmented pairs.  With --ycb_dir, --seed seeds both the perturbations and the
+augmentation, and a pair's index is that of the file `produce_train_pair_data --mode ycbv --seed S` would write for it: the
+result is `--val_dir <class folder> --augment config.yml --seed S` on that folder, bit for bit.
 """
 import argparse
 import contextlib
@@ -237,20 +240,27 @@ class PairQueues:
     batches left and then each class's partial last batch, and returns the results.  A class's batches are thus the loader's
     batches over its pairs in count order, and its step sums are added exactly as `evaluate` adds them.
 
+    With `augment` (a se3tn_augment, as data_augmentation.chain_config builds it) the queues also carry each row's segB, and a
+    batch's input B is augmented once, before any variant runs (se3tn_augment_crops in steps of at most max_batch rows, BlackCover's
+    mask the queued segB), into a batch-sized buffer that every variant and fp8 calibration then reads.  Row r of a class's batch
+    is keyed by its index in the class's count order, the index of its file in the folder `--mode ycbv` writes, so the draws are
+    those `evaluate` makes on that folder.  The buffer is allocated once: later batches keep its addresses and their graphs.
+
     The tails come back through a pinned copy queued after each append and waited for at the next add(); the frame loop's
     visibility call has synchronised the stream by then, so the wait costs nothing.  Device memory: the queues hold
-    len(class_ids) x (batch_size + rows_per_frame) pairs of 176 x 176 x 10 bytes plus two float64 poses each, e.g. about 1.4 GB
-    for 21 classes, batch_size 200 and 10 samples per class and frame."""
+    len(class_ids) x (batch_size + rows_per_frame) pairs of 176 x 176 x 10 bytes (11 with augment) plus two float64 poses each,
+    e.g. about 1.4 GB (1.5 GB) for 21 classes, batch_size 200 and 10 samples per class and frame; augment adds
+    batch_size x 176 x 176 x 5 bytes for the augmented batch."""
 
     PLANES = (('rgbA', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthA', torch.uint16, (IMAGE_SIZE, IMAGE_SIZE)),
               ('rgbB', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE, 3)), ('depthB', torch.uint16, (IMAGE_SIZE, IMAGE_SIZE)),
               ('A_in_cam', torch.float64, (4, 4)), ('B_in_cam', torch.float64, (4, 4)))
 
-    def __init__(self, eng, normalizers, modes, batch_size, max_batch, rows_per_frame, keep_predictions=False, ckpts=1):
+    def __init__(self, eng, normalizers, modes, batch_size, max_batch, rows_per_frame, keep_predictions=False, ckpts=1, augment=None):
         """normalizers: {class id (the weight set and mesh id): (trans_normalizer, rot_normalizer)}.  rows_per_frame: the most
         rows one frame sends to one class (num_sample).  max_batch: the most pairs per validation step.  ckpts: the number of
         checkpoints; checkpoint i's set of class c is weight id c + CKPT_ID_STRIDE * i, and every batch runs once per checkpoint
-        and mode."""
+        and mode.  augment: the se3tn_augment applied to input B of every pair, or None."""
         if batch_size <= 0 or max_batch <= 0 or rows_per_frame <= 0:
             raise ValueError('batch_size, max_batch and rows_per_frame must be positive')
         self.eng = eng
@@ -266,7 +276,12 @@ class PairQueues:
         self.keep_predictions = keep_predictions
         dev = eng.device
         Q = len(self.ids)
-        self.queues = {k: torch.empty((Q, self.cap) + shape, dtype=dt, device=dev) for k, dt, shape in self.PLANES}
+        self.augment = augment
+        planes = self.PLANES + ((('segB', torch.uint8, (IMAGE_SIZE, IMAGE_SIZE)),) if augment is not None else ())
+        self.queues = {k: torch.empty((Q, self.cap) + shape, dtype=dt, device=dev) for k, dt, shape in planes}
+        if augment is not None:                             # one batch's augmented input B, read by every variant
+            self.aug_rgbB = torch.empty((self.batch_size, IMAGE_SIZE, IMAGE_SIZE, 3), dtype=torch.uint8, device=dev)
+            self.aug_depthB = torch.empty((self.batch_size, IMAGE_SIZE, IMAGE_SIZE), dtype=torch.uint16, device=dev)
         self.tails = np.zeros(Q, dtype=np.int32)            # host: exact after a read-back, then a bound as rows are sent
         self.tails_dev = torch.zeros(Q, dtype=torch.int32, device=dev)
         on_cuda = torch.device(dev).type == 'cuda'
@@ -342,7 +357,7 @@ class PairQueues:
                 n = min(int(self.tails[q]), self.batch_size)
                 self._eval_batch(q, c, n)
                 rest = int(self.tails[q]) - n
-                for k, _, _ in self.PLANES:
+                for k in self.queues:
                     if rest:
                         self.queues[k][q, :rest].copy_(self.queues[k][q, n:n + rest].clone())
                 self.tails[q] = rest
@@ -354,11 +369,20 @@ class PairQueues:
         """Rows [0, n_rows) of queue q as one loader batch, in every checkpoint and mode."""
         tn, rn = self.normalizers[c]
         d = self.queues
+        plan = batch_plan(n_rows, self.batch_size, self.step)
+        rgbB, depthB = d['rgbB'][q], d['depthB'][q]
+        if self.augment is not None:                        # evaluate's augmented input B, formed once for every variant
+            first = self.pairs[c]
+            for _, s, e in plan:
+                index = torch.arange(first + s, first + e, dtype=torch.int64, device=self.eng.device)
+                self.eng.augment_crops(self.augment, rgbB[s:e], depthB[s:e], index, segB=d['segB'][q, s:e],
+                                       out_rgbB=self.aug_rgbB[s:e], out_depthB=self.aug_depthB[s:e])
+            rgbB, depthB = self.aug_rgbB, self.aug_depthB
         for i, m in self.variants:
             w = c + CKPT_ID_STRIDE * i
-            for _, s, e in batch_plan(n_rows, self.batch_size, self.step):
+            for _, s, e in plan:
                 n = e - s
-                pairs = [d[k][q, s:e] for k in ('rgbA', 'depthA', 'rgbB', 'depthB')]
+                pairs = [d['rgbA'][q, s:e], d['depthA'][q, s:e], rgbB[s:e], depthB[s:e]]
                 if m == 'fp8' and w not in self.calibrated:      # the set's scales from its first step, as evaluate's k == 0
                     self.eng.calibrate_fp8_pairs(*pairs, d['A_in_cam'][q, s:e], self.ids_host[w][:n])
                     self.calibrated.add(w)
@@ -372,7 +396,7 @@ class PairQueues:
 
 
 def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_size=200, max_batch=200, precisions=('bf16x3',),
-                  keep_predictions=False, decode_ahead=4, workers=None, engine=None):
+                  keep_predictions=False, decode_ahead=4, workers=None, engine=None, augmentations=None, augment_seed=None):
     """Problem.validate of every class on the perturbed pairs of the YCB-Video key frames, in one pass and without pair files.
 
     For each class and mode the result is bit-identical to `produce_train_pair_data --mode ycbv` with the same seed and
@@ -390,13 +414,20 @@ def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_si
     checkpoint): checkpoint i's set of class c is weight id c + 32 i.  The pairs are cut and queued once per class, and every
     batch runs once per checkpoint and mode, so each checkpoint's result is what a run of it alone returns.
 
+    augmentations: train.py:85-92's chain (a Utils.Compose, as data_augmentation.from_config builds it), applied to input B of
+    every pair with draws keyed by (augment_seed, default seed, the pair's index in its class's count order).  Each class's
+    result is then bit-identical to `evaluate` on its folder through TrackDataset(augmentations=..., augment_seed=...).
+
     -> {class id: {mode: evaluate's dict plus 'pairs'}}; with several checkpoints {checkpoint index: that}.  A class without a kept pair is reported with 0 pairs and no loss
     (trans / rot None), where `evaluate` on its empty folder raises ValueError.  The queues take
-    classes x (batch_size + num_sample) x 176 x 176 x 10 bytes of device memory (about 1.4 GB for 21 classes at 200 and 10)."""
+    classes x (batch_size + num_sample) x 176 x 176 x 10 bytes of device memory (about 1.4 GB for 21 classes at 200 and 10);
+    with augmentations 11 bytes (about 1.5 GB) plus batch_size x 176 x 176 x 5 bytes for the augmented batch."""
     from .engine import Engine
     from .predict import ycb_classes, expand_class_paths, _load_run_files, checkpoint_configs, _check_checkpoint_ids
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
+    from .data_augmentation import chain_config
     modes = list(precisions)
+    augment = chain_config(augmentations, seed if augment_seed is None else augment_seed) if augmentations is not None else None
     for m in modes:
         PREC[m]                                             # an unknown mode fails here
     configs = checkpoint_configs(templates)
@@ -423,7 +454,7 @@ def validate_ycbv(ycb_dir, class_ids, templates, num_sample=10, seed=0, batch_si
         eng.set_stats(np.asarray(run['mean']), np.asarray(run['std']), c + CKPT_ID_STRIDE * i)
         normalizers[c] = (info['max_translation'], info['max_rotation'] * np.pi / 180)
     _, producers = ycbv_producers(ycb_dir, ids, configs[0], eng, workers)
-    queues = PairQueues(eng, normalizers, modes, batch_size, step, num_sample, keep_predictions, len(configs))
+    queues = PairQueues(eng, normalizers, modes, batch_size, step, num_sample, keep_predictions, len(configs), augment)
     random.seed(seed); np.random.seed(seed)
     jobs = ycbv_keyframe_jobs(ycb_dir, ids)
     for owners, chunks in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True):
@@ -466,16 +497,14 @@ def main(argv=None):
     ap.add_argument('--num_sample', type=int, default=10, help='--ycb_dir: perturbations drawn per annotated class and key frame')
     ap.add_argument('--seed', type=int, default=0, help='--ycb_dir: seed of random and np.random before the first draw; '
                                                         '--augment: the seed of every pair\'s augmentation draws')
-    ap.add_argument('--augment', help="--val_dir: the reference's config.yml; its data_augmentation block builds train.py:85-92's "
-                                      "chain, applied to input B of every pair inside the validation step")
+    ap.add_argument('--augment', help="the reference's config.yml; its data_augmentation block builds train.py:85-92's chain, "
+                                      "applied to input B of every pair before the validation step")
     ap.add_argument('--precision', default='bf16x3', choices=sorted(PREC) + ['all'])
     ap.add_argument('--batch_size', type=int, default=200, help='the validation loader batch size (train.py:146)')
     ap.add_argument('--max_batch', type=int, default=200, help='pairs per device step (a larger batch runs as several steps)')
     args = ap.parse_args(argv)
     modes = ALL_MODES if args.precision == 'all' else [args.precision]
     if args.ycb_dir:
-        if args.augment:
-            ap.error('--augment works with --val_dir only: the pairs of --ycb_dir are cut on the device without a segB for BlackCover')
         return _main_ycbv(ap, args, modes)
     if not (args.ckpt and args.mean_std_path and args.dataset_info):
         ap.error('--val_dir needs --ckpt, --mean_std_path and --dataset_info')
@@ -491,11 +520,7 @@ def main(argv=None):
     with open(args.dataset_info) as f:
         info = yaml.safe_load(f)
     stats = [(np.load(os.path.join(d, 'mean.npy')), np.load(os.path.join(d, 'std.npy'))) for _, d in runs]
-    augmentations = None
-    if args.augment:
-        from .data_augmentation import from_config
-        with open(args.augment) as f:
-            augmentations = from_config(yaml.safe_load(f))
+    augmentations = _augmentations(args.augment)
     ds = TrackDataset(args.val_dir, 'val', stats[0][0], stats[0][1], None, augmentations, None, dataset_info=info,
                       trans_normalizer=info['max_translation'], rot_normalizer=info['max_rotation'] * np.pi / 180, augment_seed=args.seed)
     models = []
@@ -510,6 +535,16 @@ def main(argv=None):
     res = evaluate(models, ds, args.batch_size, False, modes, keep_predictions=len(modes) > 1, stats=stats)
     _print_checkpoints([p for p, _ in runs], modes, res, w)
     return res
+
+
+def _augmentations(path):
+    """--augment: train.py:85-92's chain from config.yml, or None without the option."""
+    if not path:
+        return None
+    import yaml
+    from .data_augmentation import from_config
+    with open(path) as f:
+        return from_config(yaml.safe_load(f))
 
 
 def best_checkpoint(totals):
@@ -547,7 +582,8 @@ def _main_ycbv(ap, args, modes):
     if args.ckpt or args.dataset_info:
         ap.error('--ycb_dir takes --ckpt_dir and --train_data_path templates, not --ckpt / --dataset_info')
     if not args.class_ids or not all(getattr(args, k) for k in YCB_ALL_TEMPLATES):
-        ap.error('--ycb_dir needs --class_ids, --ckpt_dir, --mean_std_path, --train_data_path and --model_path')
+        need = '--ycb_dir needs --class_ids, --ckpt_dir, --mean_std_path, --train_data_path and --model_path'
+        ap.error('--augment works with --val_dir only or with a whole --ycb_dir run: ' + need if args.augment else need)
     names = ycb_class_names(args.ycb_dir)
     if args.class_ids == 'all':
         ids = list(range(1, len(names) + 1))
@@ -564,13 +600,16 @@ def _main_ycbv(ap, args, modes):
         ckpts = [cfg['ckpt_dir'] for cfg in checkpoint_configs(templates)]
     except ValueError as e:
         ap.error(str(e))
+    augmentations = _augmentations(args.augment)
     res = validate_ycbv(args.ycb_dir, ids, templates, num_sample=args.num_sample, seed=args.seed, batch_size=args.batch_size,
-                        max_batch=args.max_batch, precisions=modes, keep_predictions=len(modes) > 1)
+                        max_batch=args.max_batch, precisions=modes, keep_predictions=len(modes) > 1, augmentations=augmentations,
+                        augment_seed=args.seed)
     per_ckpt = [res[i] for i in range(len(ckpts))] if len(ckpts) > 1 else [res]
     device = torch.cuda.get_device_name(torch.cuda.current_device())
     for c in ids:
         n = per_ckpt[0][c][modes[0]]['pairs']
-        print('class %d (%s): %d pairs, batch %d, %s' % (c, names[c - 1], n, args.batch_size, device))
+        print('class %d (%s): %d pairs, batch %d, %s%s' % (c, names[c - 1], n, args.batch_size, device,
+                                                        ", augmented (train.py's chain, seed %d)" % args.seed if args.augment else ''))
         if n == 0:
             print('no kept pair: no loss')
             continue
