@@ -236,6 +236,18 @@ int se3tn_add_adi_sets(se3tn_ctx* ctx, const double* pts, int M, const int32_t* 
  * call needs more, so a run of calls allocates nothing once the largest has been seen. */
 int se3tn_vocap_sets(se3tn_ctx* ctx, const double* errs, const int32_t* err_set, int n, int n_sets, double* out_ap, void* stream);
 
+/* Pose errors of several objects' poses in ONE launch, arguments as se3tn_add_adi_sets (pts, set_offsets, pose_set, pred, gt) plus:
+ *   keep uint8 (n) device or NULL (every row kept): a row whose byte is 0 is not scored.
+ *   out_errors double (n,4) device: per row the translation error |t - t_gt| in mm, the rotation geodesic angle in degrees
+ *     acos(clamp((tr(R^T R_gt) - 1) / 2, -1, 1)) (the trace summed in row-major order), ADD and ADD-S; NaN in all four for a row
+ *     that is not kept.  ADD / ADD-S are bit-identical to se3tn_add_adi_sets on the same rows (the same per-pose body).
+ *   out_set int32 (n) device or NULL: each kept row's set id, -1 for a row that is not kept, so the caller can leave those rows out
+ *     of se3tn_vocap_sets (or of anything else) without reading the mask on the host first.
+ * Refusals and scratch as se3tn_add_adi_sets (every id is checked, kept or not); one launch, plain stream order. */
+int se3tn_pose_errors_sets(se3tn_ctx* ctx, const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* pose_set,
+                           const double* pred, const double* gt, const uint8_t* keep, int n, double* out_errors, int32_t* out_set,
+                           void* stream);
+
 /* ---- result videos: each track's model points drawn over its frame (not on the per-frame tracking path) ------------------------- */
 
 /* The frames of the reference's result videos (getResultsYcb, predict.py:424-433; predictSequenceYcb / predictSequenceYcbInEOAT,
@@ -341,7 +353,8 @@ int se3tn_set_depth_fill(se3tn_ctx* ctx, int enable, double max_depth, int extra
  * they return SE3TN_ERR_STATE and queue nothing.  k outside [1, SE3TN_MAX_REFINE_ITERATIONS] is SE3TN_ERR_INVALID and the
  * setting is unchanged.  A context is single-threaded: a caller that shares one between trackers sets the k it wants before
  * each track call.  Whether more rounds improve accuracy depends on the checkpoint; it has not been measured on trained
- * weights. */
+ * weights.  se3tn_track_render_rounds returns every round's poses from one step, and `predict --mode ycbv_recover` scores them
+ * against the annotations of the YCB-Video key frames (README). */
 #define SE3TN_MAX_REFINE_ITERATIONS 8
 int se3tn_set_refine_iterations(se3tn_ctx* ctx, int k);
 
@@ -375,6 +388,20 @@ int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t*
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double trans_normalizer, double rot_normalizer, int precision,
                        float* out_trans, float* out_rot, double* poses_out, void* stream);
+
+/* se3tn_track_render plus one device output: round_poses double (k, n, 16), k = se3tn_set_refine_iterations' count, where slot
+ * r - 1 receives every track's pose after round r, r = 1 .. k, bit for bit what an r-round step leaves in poses_out (slot k - 1
+ * equals poses_out).  After each round the step copies poses_out there (a device-to-device copy inside the step's CUDA graph;
+ * SE3TN_PREC_FP32 queues it between its plain launches); se3tn_last_launch_count counts kernels only, so it reads as for
+ * se3tn_track_render.  round_poses is part of the step's key: a step with it and one without are two graphs, and both compute
+ * the same poses_out.  Refused as se3tn_track_render refuses, and SE3TN_ERR_INVALID with nothing queued for a NULL round_poses
+ * or one that overlaps poses_in or poses_out. */
+int se3tn_track_render_rounds(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                              const double* K, const double* poses_in, const double* object_width,
+                              int render_mode, int render_H, int render_W,
+                              const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                              double trans_normalizer, double rot_normalizer, int precision,
+                              float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream);
 
 /* se3tn_track_render with every pointer in HOST memory, the reference's own calling pattern with rendering included: the
  * frame's crop-window rectangle, the poses, widths and ids go through se3tn_track_host's pinned staging (one copy in, one

@@ -44,11 +44,14 @@ SIGNATURES = {
     'se3tn_add_adi': (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap': (_i, [_vp, _vp, _i, C.POINTER(_d), _vp]),
     'se3tn_add_adi_sets': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    'se3tn_pose_errors_sets': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap_sets': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     'se3tn_draw_tracks': (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     'se3tn_allgather_poses': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
+    'se3tn_track_render_rounds': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
+                                       _vp]),
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),

@@ -33,11 +33,11 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
     return s;                       // valid in thread 0
 }
 
-// ADD / ADD-S of one (pred, gt) pair of 4x4 poses against m model points, computed by one CTA of kMetricThreads threads.  Both
-// metric kernels run this body, so a pose scored against its own point set gives the same bits in either.
+// ADD / ADD-S of one (pred, gt) pair of 4x4 poses against m model points, computed by one CTA of kMetricThreads threads; the
+// values are valid in thread 0 (ADD-S only with want_adi).  Every metric kernel runs this body, so a pose scored against its own
+// point set gives the same bits in each.
 __device__ __forceinline__ void score_pose(const double* __restrict__ model, int m, const double* __restrict__ pred16,
-                                           const double* __restrict__ gt16, double* __restrict__ out_add,
-                                           double* __restrict__ out_adi, int pose)
+                                           const double* __restrict__ gt16, bool want_adi, double& add, double& adi)
 {
     __shared__ double sp[kPredTile * 3];
     __shared__ double red[kMetricThreads / 32];
@@ -57,7 +57,7 @@ __device__ __forceinline__ void score_pose(const double* __restrict__ model, int
             const double dx = px - gx, dy = py - gy, dz = pz - gz;
             sum_add += sqrt(dx * dx + dy * dy + dz * dz);
         }
-        if (out_adi) {
+        if (want_adi) {
             double best = 1.0e300;
             for (int t0 = 0; t0 < m; t0 += kPredTile) {
                 __syncthreads();
@@ -78,12 +78,8 @@ __device__ __forceinline__ void score_pose(const double* __restrict__ model, int
             if (have) sum_adi += sqrt(best);
         }
     }
-    const double a = block_sum(sum_add, red);
-    if (threadIdx.x == 0 && out_add) out_add[pose] = a / m;
-    if (out_adi) {
-        const double b = block_sum(sum_adi, red);
-        if (threadIdx.x == 0) out_adi[pose] = b / m;
-    }
+    add = block_sum(sum_add, red) / m;
+    if (want_adi) adi = block_sum(sum_adi, red) / m;
 }
 
 __global__ void __launch_bounds__(kMetricThreads)
@@ -91,7 +87,12 @@ add_adi_kernel(const double* __restrict__ model, int m, const double* __restrict
                double* __restrict__ out_add, double* __restrict__ out_adi)
 {
     const int pose = blockIdx.x;
-    score_pose(model, m, pred + pose * 16, gt + pose * 16, out_add, out_adi, pose);
+    double a, b;
+    score_pose(model, m, pred + pose * 16, gt + pose * 16, out_adi != nullptr, a, b);
+    if (threadIdx.x == 0) {
+        if (out_add) out_add[pose] = a;
+        if (out_adi) out_adi[pose] = b;
+    }
 }
 
 // One CTA per pose; pose p is scored against points [offsets[s], offsets[s+1]) of the table, s = pose_set[p].
@@ -102,7 +103,46 @@ add_adi_sets_kernel(const double* __restrict__ pts, const int* __restrict__ offs
 {
     const int pose = blockIdx.x;
     const int s = pose_set[pose], first = offsets[s];
-    score_pose(pts + static_cast<size_t>(first) * 3, offsets[s + 1] - first, pred + pose * 16, gt + pose * 16, out_add, out_adi, pose);
+    double a, b;
+    score_pose(pts + static_cast<size_t>(first) * 3, offsets[s + 1] - first, pred + pose * 16, gt + pose * 16, out_adi != nullptr, a, b);
+    if (threadIdx.x == 0) {
+        if (out_add) out_add[pose] = a;
+        if (out_adi) out_adi[pose] = b;
+    }
+}
+
+// One CTA per row: out[row] = translation error (mm), rotation geodesic angle (degrees), ADD, ADD-S of pred against gt, the two
+// metrics from score_pose on the row's point set.  keep (nullable): a row whose byte is 0 is not scored; its four values are NaN and
+// its out_set entry is -1, every other row's out_set entry its set id.
+__global__ void __launch_bounds__(kMetricThreads)
+pose_errors_sets_kernel(const double* __restrict__ pts, const int* __restrict__ offsets, const int* __restrict__ pose_set,
+                        const double* __restrict__ pred, const double* __restrict__ gt, const uint8_t* __restrict__ keep,
+                        double* __restrict__ out, int* __restrict__ out_set)
+{
+    const int row = blockIdx.x;
+    const int s = pose_set[row];
+    if (keep && !keep[row]) {
+        if (threadIdx.x < 4) out[row * 4 + threadIdx.x] = __longlong_as_double(0x7ff8000000000000ll);
+        if (threadIdx.x == 0 && out_set) out_set[row] = -1;
+        return;
+    }
+    const int first = offsets[s];
+    const double* P = pred + row * 16;
+    const double* G = gt + row * 16;
+    double a, b;
+    score_pose(pts + static_cast<size_t>(first) * 3, offsets[s + 1] - first, P, G, true, a, b);
+    if (threadIdx.x == 0) {
+        const double dx = P[3] - G[3], dy = P[7] - G[7], dz = P[11] - G[11];
+        double tr = 0;                                  // tr(R^T R_gt) = sum_ij R_ij R_gt_ij, row-major order
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) tr += P[i * 4 + j] * G[i * 4 + j];
+        const double cosang = fmin(1.0, fmax(-1.0, (tr - 1.0) / 2.0));
+        out[row * 4 + 0] = sqrt(dx * dx + dy * dy + dz * dz) * 1000.0;
+        out[row * 4 + 1] = acos(cosang) * (180.0 / 3.14159265358979323846);
+        out[row * 4 + 2] = a;
+        out[row * 4 + 3] = b;
+        if (out_set) out_set[row] = s;
+    }
 }
 
 // errs sorted ascending; ap = 10 * [ sum_j (r_j - r_{j-1}) * j/n  +  (0.1 - r_c) * c/n ],  r_0 = 0, c = #(r < 0.1).
@@ -175,6 +215,13 @@ cudaError_t launch_add_adi_sets(const double* pts, const int* offsets, const int
                                 int n, double* out_add, double* out_adi, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     add_adi_sets_kernel<<<n, kMetricThreads, 0, s>>>(pts, offsets, pose_set, pred, gt, out_add, out_adi);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pose_errors_sets(const double* pts, const int* offsets, const int* pose_set, const double* pred, const double* gt,
+                                    const uint8_t* keep, int n, double* out, int* out_set, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    pose_errors_sets_kernel<<<n, kMetricThreads, 0, s>>>(pts, offsets, pose_set, pred, gt, keep, out, out_set);
     return cudaGetLastError();
 }
 

@@ -232,6 +232,7 @@ struct StepKey {
     float* out_trans; float* out_rot; double* poses_out;                                  // poses_out: track step
     float* sq; double* labels; float* sums;                                               // validation step
     const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
+    double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render_rounds) or NULL
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -1384,9 +1385,16 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         if ((rc = queue_preprocess(c, a, st.n, s))) return rc;
         if ((rc = run_tracks(c, st, head, s))) return rc;
         if (st.kind == kStepTrack) {
-            if (!fp32) continue;                   // the head kernel has updated the poses
-            ProfScope ps(c, 18, s);
-            CU_TRY(c, launch_pose_update(poses, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
+            if (fp32) {                            // otherwise the head kernel has updated the poses
+                ProfScope ps(c, 18, s);
+                CU_TRY(c, launch_pose_update(poses, st.out_trans, st.out_rot, head.tn, head.rn, st.poses_out, st.n, s));
+                ++c->launches;
+            }
+            // the poses after round + 1, what a (round + 1)-round step leaves in poses_out; the next round's render waits for the copy
+            if (st.round_poses)
+                CU_TRY(c, cudaMemcpyAsync(st.round_poses + static_cast<size_t>(round) * st.n * 16, st.poses_out,
+                                          sizeof(double) * 16 * static_cast<size_t>(st.n), cudaMemcpyDeviceToDevice, s));
+            continue;
         } else {
             ProfScope ps(c, 21, s);
             if (fp32) CU_TRY(c, launch_pair_loss(st.out_trans, st.out_rot, nullptr, nullptr, head.loss, st.n, st.sums, s));
@@ -1479,6 +1487,41 @@ int eval_pairs_step(se3tn_ctx* c, const char* fn, const uint8_t* rgbA, const uin
     return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
+// se3tn_track_render, and with round_poses (k x n x 16 doubles, k = c->refine_iterations) se3tn_track_render_rounds.
+int track_render_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                      const double* K, const double* poses_in, const double* object_width, int render_mode, int render_H, int render_W,
+                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, double tn, double rn, int precision,
+                      float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream) {
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    bool multi = false;
+    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
+    if (round_poses) {                             // the copies must not write the poses a later round reads
+        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
+        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * c->refine_iterations;
+        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
+            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
+            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
+        }
+    }
+    DeviceGuard guard(c->device);
+    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    st.round_poses = round_poses;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1514,24 +1557,21 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double tn, double rn, int precision,
                        float* out_trans, float* out_rot, double* poses_out, void* stream) {
+    return track_render_step(c, "se3tn_track_render", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
+                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, nullptr, stream);
+}
+
+int se3tn_track_render_rounds(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                              const double* K, const double* poses_in, const double* object_width,
+                              int render_mode, int render_H, int render_W,
+                              const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                              double tn, double rn, int precision,
+                              float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: null argument or empty frame");
-    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: null output");
-    RenderSpec r;
-    int rc = render_spec(c, "se3tn_track_render", render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    bool multi = false;
-    rc = check_step(c, "se3tn_track_render", weight_ids_host, weight_ids_dev, n, true, &multi, precision);
-    if (rc) return rc;
-    if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render: unknown precision");
-    DeviceGuard guard(c->device);
-    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
-    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
-    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
-    if ((rc = render_into_scratch(c, r, st))) return rc;
-    return run_step(c, st, static_cast<cudaStream_t>(stream));
+    if (!round_poses) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render_rounds: null round_poses");
+    return track_render_step(c, "se3tn_track_render_rounds", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode,
+                             render_H, render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out,
+                             round_poses, stream);
 }
 
 int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
@@ -1842,6 +1882,22 @@ int se3tn_add_adi_sets(se3tn_ctx* c, const double* pts, int M, const int32_t* se
     int32_t *d_off, *d_set; uint8_t* unused;
     if ((rc = stage_sets(c, set_offsets, n_sets, pose_set, n, 0, s, &d_off, &d_set, &unused))) return rc;
     CU_TRY(c, launch_add_adi_sets(pts, d_off, d_set, pred, gt, n, out_add, out_adi, s));
+    return SE3TN_OK;
+}
+
+int se3tn_pose_errors_sets(se3tn_ctx* c, const double* pts, int M, const int32_t* set_offsets, int n_sets, const int32_t* pose_set,
+                           const double* pred, const double* gt, const uint8_t* keep, int n, double* out_errors, int32_t* out_set,
+                           void* stream) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!pts || !set_offsets || M <= 0 || n_sets <= 0 || n < 0 || (n > 0 && (!pose_set || !pred || !gt || !out_errors)))
+        return fail(c, SE3TN_ERR_INVALID, "se3tn_pose_errors_sets: null/invalid argument");
+    int rc = check_sets(c, "se3tn_pose_errors_sets", M, set_offsets, n_sets, pose_set, n, "pose");
+    if (rc || n == 0) return rc;
+    DeviceGuard guard(c->device);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    int32_t *d_off, *d_set; uint8_t* unused;
+    if ((rc = stage_sets(c, set_offsets, n_sets, pose_set, n, 0, s, &d_off, &d_set, &unused))) return rc;
+    CU_TRY(c, launch_pose_errors_sets(pts, d_off, d_set, pred, gt, keep, n, out_errors, out_set, s));
     return SE3TN_OK;
 }
 

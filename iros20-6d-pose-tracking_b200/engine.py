@@ -272,19 +272,21 @@ class Engine:
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
-                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1):
+                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1, out_rounds=None):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
         out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h).  iterations: k rounds
         of render -> network -> pose update on this frame in the one step, exactly what k chained calls with iterations=1
-        compute (se3tn_set_refine_iterations, 1..8); out_trans / out_rot hold the last round's outputs."""
+        compute (se3tn_set_refine_iterations, 1..8); out_trans / out_rot hold the last round's outputs.  out_rounds: a float64
+        CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_render_rounds): entry r - 1 is
+        what a call with iterations=r returns.  The step with it is a CUDA graph of its own."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
-                           fill_depth, iterations)
+                           fill_depth, iterations, out_rounds)
 
     def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations):
+               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, out_rounds=None):
         """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
         n = poses.shape[0]
         iterations = self.refine_iterations(iterations)
@@ -297,6 +299,8 @@ class Engine:
         out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
         if wh is not None and weight_ids_dev is None:
             weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        if out_rounds is not None:
+            self._check_dev('out_rounds', out_rounds, torch.float64, (iterations, n, 4, 4))
         self._set_depth_fill(fill)
         self._set_refine(iterations)
         H, W = frame_depth.shape
@@ -305,6 +309,8 @@ class Engine:
                 _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), _stream(self.device))
         if render is None:
             rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail)
+        elif out_rounds is not None:
+            rc = self.lib.se3tn_track_render_rounds(*head, *render, *tail[:-1], _ptr(out_rounds), tail[-1])
         else:
             rc = self.lib.se3tn_track_render(*head, *render, *tail)
         _lib.check(rc, self._ctx)
@@ -500,20 +506,8 @@ class Engine:
         float64 model points (numpy arrays or tensors), or one float64 CUDA table (M,3) with set_offsets (S+1) int32 giving each
         object's rows.  pose_set (n) int32: the object of each pose; pred / gt float64 CUDA tensors (n,4,4).
         -> (out_add, out_adi) float64 CUDA tensors (n), bit-identical to add_adi on each pose's own points."""
-        if torch.is_tensor(points):
-            table = points
-            if set_offsets is None:
-                raise ValueError('add_adi_sets: a point table needs set_offsets')
-        else:
-            sets = [np.asarray(p.cpu().numpy() if torch.is_tensor(p) else p, dtype=np.float64).reshape(-1, 3) for p in points]
-            set_offsets = np.cumsum([0] + [len(p) for p in sets])
-            table = torch.from_numpy(np.ascontiguousarray(np.concatenate(sets) if sets else np.zeros((0, 3)))).to(self.device)
-        offs = np.ascontiguousarray(set_offsets, dtype=np.int32)
-        ids = np.ascontiguousarray(pose_set.cpu().numpy() if torch.is_tensor(pose_set) else pose_set, dtype=np.int32).reshape(-1)
+        table, offs, ids = self._point_sets('add_adi_sets', points, set_offsets, pose_set)
         n = int(ids.shape[0])
-        if offs.ndim != 1 or offs.shape[0] < 2:
-            raise ValueError('add_adi_sets: set_offsets must hold S+1 >= 2 offsets')
-        self._check_dev('points', table, torch.float64, (table.shape[0], 3))
         self._check_dev('pred', pred, torch.float64, (n, 4, 4))
         self._check_dev('gt', gt, torch.float64, (n, 4, 4))
         out_add = torch.empty(n, dtype=torch.float64, device=self.device) if want_add else None
@@ -521,6 +515,24 @@ class Engine:
         _lib.check(self.lib.se3tn_add_adi_sets(self._ctx, _ptr(table), int(table.shape[0]), _hptr(offs), int(offs.shape[0]) - 1, _hptr(ids),
                                                _ptr(pred), _ptr(gt), n, _ptr(out_add), _ptr(out_adi), _stream(self.device)), self._ctx)
         return out_add, out_adi
+
+    def pose_errors_sets(self, points, pose_set, pred, gt, set_offsets=None, keep=None):
+        """Translation error (mm), rotation angle (degrees), ADD and ADD-S of n poses in one launch (se3tn_pose_errors_sets).
+        points / set_offsets / pose_set / pred / gt as add_adi_sets takes them; keep: None or a uint8 CUDA tensor (n), a 0 row
+        left unscored.  -> (errors float64 CUDA (n, 4), set ids int32 CUDA (n): a kept row's pose_set entry, -1 for the others);
+        a row that is not kept has NaN errors.  ADD / ADD-S are add_adi_sets' values bit for bit."""
+        table, offs, ids = self._point_sets('pose_errors_sets', points, set_offsets, pose_set)
+        n = int(ids.shape[0])
+        self._check_dev('pred', pred, torch.float64, (n, 4, 4))
+        self._check_dev('gt', gt, torch.float64, (n, 4, 4))
+        if keep is not None:
+            self._check_dev('keep', keep, torch.uint8, (n,))
+        out = torch.empty((n, 4), dtype=torch.float64, device=self.device)
+        out_set = torch.empty(n, dtype=torch.int32, device=self.device)
+        _lib.check(self.lib.se3tn_pose_errors_sets(self._ctx, _ptr(table), int(table.shape[0]), _hptr(offs), int(offs.shape[0]) - 1,
+                                                   _hptr(ids), _ptr(pred), _ptr(gt), _ptr(keep), n, _ptr(out), _ptr(out_set),
+                                                   _stream(self.device)), self._ctx)
+        return out, out_set
 
     def vocap_sets(self, errs, err_set, n_sets):
         """VOCap of each set's errors and of all of them (se3tn_vocap_sets): errs float64 CUDA tensor (n), err_set (n) int32
@@ -534,6 +546,24 @@ class Engine:
         out = np.zeros(int(n_sets) + 1, dtype=np.float64)
         _lib.check(self.lib.se3tn_vocap_sets(self._ctx, _ptr(errs), _ptr(ids), n, int(n_sets), _hptr(out), _stream(self.device)), self._ctx)
         return out
+
+    def _point_sets(self, fn, points, set_offsets, pose_set):
+        """add_adi_sets' points / set_offsets / pose_set -> (float64 CUDA table (M,3), int32 offsets (S+1), int32 ids (n)), host
+        arrays for the offsets and ids."""
+        if torch.is_tensor(points):
+            table = points
+            if set_offsets is None:
+                raise ValueError('%s: a point table needs set_offsets' % fn)
+        else:
+            sets = [np.asarray(p.cpu().numpy() if torch.is_tensor(p) else p, dtype=np.float64).reshape(-1, 3) for p in points]
+            set_offsets = np.cumsum([0] + [len(p) for p in sets])
+            table = torch.from_numpy(np.ascontiguousarray(np.concatenate(sets) if sets else np.zeros((0, 3)))).to(self.device)
+        offs = np.ascontiguousarray(set_offsets, dtype=np.int32)
+        ids = np.ascontiguousarray(pose_set.cpu().numpy() if torch.is_tensor(pose_set) else pose_set, dtype=np.int32).reshape(-1)
+        if offs.ndim != 1 or offs.shape[0] < 2:
+            raise ValueError('%s: set_offsets must hold S+1 >= 2 offsets' % fn)
+        self._check_dev('points', table, torch.float64, (table.shape[0], 3))
+        return table, offs, ids
 
     def metrics_scratch_bytes(self):
         """Device bytes the context holds for add_adi_sets / vocap_sets / draw_tracks."""

@@ -25,6 +25,7 @@ Differences, all additive:
 import collections
 import contextlib
 import os
+import random
 import numpy as np
 import torch
 
@@ -1592,6 +1593,222 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
                           lambda written, key: {v: w[key] for v, w in zip(sequences, written)})
 
 
+# ----------------------------------------------------------------------------------------------------
+# Pose recovery from perturbed starts on the YCB-Video key frames (--mode ycbv_recover): the perturbed poses `produce_train_pair_data
+# --mode ycbv` keeps (ProducerPurturb.generate: "sample various purturbation around for evaluating the mean error") become track
+# starts on their own key frame, K refinement rounds run in one tracking step, and every round's pose is scored against the
+# annotation: translation / rotation error, ADD, ADD-S and their VOCap AUCs, per class and pooled.
+# ----------------------------------------------------------------------------------------------------
+RECOVER_GPUS_REFUSAL = ('ycbv_recover runs on one GPU: the perturbations of a key frame are drawn after every earlier frame\'s '
+                        'visibility check, so the frames cannot be shared out')
+
+
+def recover_front(precision='bf16x3', iterations=1, gpus=1):
+    """The argument checks of recoverYcbKeyframes, before anything is read -> (modes, K).  precision: a mode of YCB_ALL_PRECISIONS,
+    'all' or a list of them ('fp16' refused, as in ycbv_all); iterations: one K in [1, 8]; gpus: 1 (RECOVER_GPUS_REFUSAL).  Every
+    refusal is a ValueError."""
+    if gpus != 1:
+        raise ValueError(RECOVER_GPUS_REFUSAL)
+    modes, _ = precision_modes(precision, YCB_ALL_PRECISIONS)
+    if modes[0] not in YCB_ALL_PRECISIONS:
+        raise ValueError('precision %r is not a mode of ycbv_recover (one of %s)' % (modes[0], ', '.join(YCB_ALL_PRECISIONS)))
+    if isinstance(iterations, (list, tuple)) or isinstance(iterations, bool):
+        raise ValueError('ycbv_recover takes one iteration count K (every round 1..K is scored), not %r' % (iterations,))
+    return modes, _refine_iterations(iterations)
+
+
+def pair_mesh_base(class_ids, ckpts):
+    """The mesh id of class 0's producer mesh in a ycbv_recover run: CKPT_ID_STRIDE x ckpts, above the weight ids c + 32 i of every
+    checkpoint i < ckpts, under which the tracking meshes live.  A producer mesh id base + c that is also a weight id is a
+    ValueError."""
+    base = CKPT_ID_STRIDE * int(ckpts)
+    weights = {int(c) + CKPT_ID_STRIDE * i for c in class_ids for i in range(int(ckpts))}
+    clash = sorted(base + int(c) for c in class_ids if base + int(c) in weights)
+    if clash:
+        raise ValueError('producer mesh ids %s (%d + class id) are also weight ids of the tracking meshes; class ids must stay below %d'
+                         % (', '.join(map(str, clash)), base, CKPT_ID_STRIDE))
+    return base
+
+
+def pair_model_template(class_config):
+    """The producers' mesh template: class_config['pair_model_path'], else model_path with .ply -> .obj, as ProducerPurturb picks
+    it (produce_train_pair_data.py:76)."""
+    return class_config.get('pair_model_path') or str(class_config['model_path']).replace('.ply', '.obj')
+
+
+def pose_errors_np(pred, gt):
+    """se3tn_pose_errors_sets' translation error (mm) and rotation angle (degrees) in numpy fp64: pred, gt (n, 4, 4) -> (n, 2)."""
+    pred = np.asarray(pred, np.float64).reshape(-1, 4, 4)
+    gt = np.asarray(gt, np.float64).reshape(-1, 4, 4)
+    d = pred[:, :3, 3] - gt[:, :3, 3]
+    trans = np.sqrt(d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2]) * 1000.0
+    tr = np.zeros(len(pred))
+    for i in range(3):
+        for j in range(3):
+            tr = tr + pred[:, i, j] * gt[:, i, j]
+    rot = np.degrees(np.arccos(np.clip((tr - 1.0) / 2.0, -1.0, 1.0)))
+    return np.stack([trans, rot], 1)
+
+
+def _recover_summary(errors, add_auc, adds_auc):
+    """One table row's values from (rows, 4) errors (mm, degrees, ADD, ADD-S) and the two AUCs; None values with no row."""
+    n = int(errors.shape[0])
+    if n == 0:
+        return dict(rows=0, add_auc=None, adds_auc=None, rot_mean=None, rot_median=None, trans_mean=None, trans_median=None)
+    return dict(rows=n, add_auc=float(add_auc), adds_auc=float(adds_auc), rot_mean=float(np.mean(errors[:, 1])),
+                rot_median=float(np.median(errors[:, 1])), trans_mean=float(np.mean(errors[:, 0])), trans_median=float(np.median(errors[:, 0])))
+
+
+def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0, precision='bf16x3', iterations=1, max_frames=None,
+                        decode_ahead=4, workers=None, gpus=1):
+    """Pose recovery from perturbed starts on the YCB-Video key frames, every class in one pass.
+
+    The frame loop is `produce_train_pair_data --mode ycbv`'s own (ycbv_pair_steps, random / np.random seeded with `seed`): the same
+    visibility check, draws, centre test and pair step, so a class's kept rows are the pairs that mode writes with this seed and
+    num_sample, in its order, with its A_in_cam / B_in_cam, and the RNG ends in the same state.  The producers draw the mesh of
+    class_config['pair_model_path'] (default model_path with .ply -> .obj, pair_model_template) under mesh ids pair_mesh_base(...)
+    + class id; the tracks draw model_path under their weight ids.
+
+    Each frame's rows (the samples inside the image, classes in order) are n tracks of one se3tn_track_render_rounds step per
+    variant, started at their A_in_cam on the ring's device frame, with their class's weight set, statistics, mesh and
+    Tracker.object_width, refined K times; a row whose segB count is below 100 (the writer drops it) is tracked but not scored:
+    the counts stay on the device as the keep mask of se3tn_pose_errors_sets.  After the last frame every round r = 0 (the start)
+    .. K of every row is scored against B_in_cam in one launch per round and variant, against the tracking mesh's points
+    (Tracker.object_cloud), and se3tn_vocap_sets gives the per-class and pooled ADD / ADD-S AUCs.
+
+    class_config: the ycbv_all templates (YCB_ALL_TEMPLATES, optional normalisers), refused as ycb_all_classes refuses them;
+    ckpt_dir / mean_std_path may be lists (checkpoint i's set of class c is weight id c + 32 i).  precision: one mode, 'all' or a
+    list (recover_front); iterations: one K in 1..8; gpus: 1.  Every frame is decoded and cut once, then stepped once per
+    (checkpoint, mode); fp8 calibrates each set on its own rows of the first frame that has any (Engine.calibrate_fp8_tracks).
+    Each variant's numbers are those of a run with that checkpoint and mode alone.  max_frames: the first key frames only.
+
+    -> {variant: {class id: dict, ..., 'all': dict}}, variant (mode, K) with one checkpoint, (mode, K, checkpoint index) with several.
+    Each dict: rows, A_in_cam / B_in_cam (rows, 4, 4), poses (K, rows, 4, 4) after each round, errors (K + 1, rows, 4) (translation
+    mm, rotation degrees, ADD m, ADD-S m; index 0 the start), and summary: K + 1 dicts of _recover_summary (AUCs in [0, 1])."""
+    from . import _lib
+    from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
+    modes, K = recover_front(precision, iterations, gpus)
+    configs = checkpoint_configs(class_config)
+    ids = [c for c, _ in ycb_classes(ycb_dir, class_ids)]
+    if not ids:
+        raise ValueError('no class ids given')
+    _check_checkpoint_ids(ids, len(configs), 'class')
+    base = pair_mesh_base(ids, len(configs))
+    per_ckpt = [ycb_all_classes(ycb_dir, ids, cfg, modes[0]) for cfg in configs]
+    pair_tpl = dict(train_data_path=class_config['train_data_path'], model_path=pair_model_template(class_config))
+    entries = [(k['class_id'] + CKPT_ID_STRIDE * i, 'class %d (%s)' % (k['class_id'], k['name']) + (' checkpoint %d' % i if len(configs) > 1 else ''), k)
+               for i, cl in enumerate(per_ckpt) for k in cl]
+    if len(configs) > 1:
+        check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
+    eng, trackers = _one_pass_trackers(entries, modes[0], max(1, len(ids) * int(num_sample)))
+    _, producers = ycbv_producers(ycb_dir, ids, pair_tpl, eng, workers, mesh_base=base)
+    variants = [(m, K) + ((i,) if len(configs) > 1 else ()) for i in range(len(configs)) for m in modes]
+    dev = eng.device
+    set_of = {c: j for j, c in enumerate(ids)}
+    random.seed(seed); np.random.seed(seed)
+    jobs = ycbv_keyframe_jobs(ycb_dir, ids)
+    if max_frames is not None:
+        jobs = jobs[:int(max_frames)]
+    trk = trackers[entries[0][0]]
+    render = dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw)
+    starts, counts, row_set, row_B, rounds = [], [], [], [], {v: [] for v in variants}
+    by_n, by_cls = {}, {}
+    for owners, chunks, (rgb, depth) in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True,
+                                                        with_frame=True):
+        cls = tuple(c for c, _, inside, _ in owners for _ in inside)
+        n = len(cls)
+        if n not in by_n:                                  # per n: the start poses and each variant's outputs, at fixed addresses
+            by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
+                       {v: (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
+                            torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((K, n, 4, 4), dtype=torch.float64, device=dev))
+                        for v in variants})
+        start, outs = by_n[n]
+        start.copy_(torch.cat([r['A_in_cam'] for _, r in chunks]))
+        counts.append(torch.cat([r['count'] for _, r in chunks]))
+        starts.append(start.clone())
+        row_set += [set_of[c] for c in cls]
+        row_B += [B for c, B, inside, _ in owners for _ in inside]
+        for v in variants:
+            i = _variant_checkpoint(v)
+            if (cls, i) not in by_cls:
+                wh = np.asarray(cls, dtype=np.int32) + CKPT_ID_STRIDE * i
+                by_cls[cls, i] = (wh, torch.from_numpy(wh).to(dev),
+                                  torch.tensor([trackers[int(w)].object_width for w in wh], dtype=torch.float64, device=dev))
+            wh, wd, widths = by_cls[cls, i]
+            if v[0] == 'fp8':                              # sets without scales: calibrated on their own rows of this frame
+                eng.calibrate_fp8_tracks(rgb, depth, trk.K, start, widths, weight_ids=wh, render=dict(render, mesh_ids=wd))
+            poses, out_trans, out_rot, out_rounds = outs[v]
+            eng.track_render(rgb, depth, trk.K, start, widths, trk.trans_normalizer, trk.rot_normalizer, weight_ids_host=wh,
+                             weight_ids_dev=wd, precision=v[0], mode=render['mode'], image_hw=render['image_hw'], out_poses=poses,
+                             out_trans=out_trans, out_rot=out_rot, iterations=K, out_rounds=out_rounds)
+            rounds[v].append(out_rounds.clone())
+    return _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG)
+
+
+def _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, min_seg):
+    """recoverYcbKeyframes' scoring, after the last frame: every round of every row in one se3tn_pose_errors_sets launch per round
+    and variant (rows whose count is below min_seg masked), one read-back, then se3tn_vocap_sets per round and metric."""
+    dev = eng.device
+    N = len(row_set)
+    S = len(ids)
+    clouds = [np.asarray(trackers[c].object_cloud.points, dtype=np.float64).reshape(-1, 3) for c in ids]
+    offsets = np.cumsum([0] + [len(p) for p in clouds]).astype(np.int32)
+    table = torch.from_numpy(np.ascontiguousarray(np.concatenate(clouds))).to(dev)
+    pose_set = np.asarray(row_set, dtype=np.int32)
+    if N:
+        A = torch.cat(starts)
+        B = torch.from_numpy(np.ascontiguousarray(np.stack(row_B), dtype=np.float64)).to(dev)
+        keep = (torch.cat(counts) >= min_seg).to(torch.uint8)
+        err0, kept_set = eng.pose_errors_sets(table, pose_set, A, B, offsets, keep)
+        per_v = {v: torch.cat(rounds[v], 1) for v in variants}
+        errs = {v: torch.stack([err0] + [eng.pose_errors_sets(table, pose_set, per_v[v][r], B, offsets, keep)[0] for r in range(K)])
+                for v in variants}
+        kept = (kept_set >= 0).cpu().numpy()
+    else:
+        kept = np.zeros(0, bool)
+    kidx = torch.from_numpy(np.flatnonzero(kept)).to(dev)
+    kset = pose_set[kept]
+    A_h = A.index_select(0, kidx).cpu().numpy() if N else np.zeros((0, 4, 4))
+    B_h = B.index_select(0, kidx).cpu().numpy() if N else np.zeros((0, 4, 4))
+    out = {}
+    for v in variants:
+        E = errs[v].index_select(1, kidx) if N else torch.zeros((K + 1, 0, 4), dtype=torch.float64, device=dev)
+        P = per_v[v].index_select(1, kidx).cpu().numpy() if N else np.zeros((K, 0, 4, 4))
+        aucs = [(eng.vocap_sets(E[r, :, 2].contiguous(), kset, S), eng.vocap_sets(E[r, :, 3].contiguous(), kset, S)) for r in range(K + 1)]
+        Eh = E.cpu().numpy()
+        res = {}
+        for j, c in enumerate(ids + ['all']):
+            rows = np.flatnonzero(kset == j) if c != 'all' else np.arange(len(kset))
+            res[c] = dict(rows=len(rows), A_in_cam=A_h[rows], B_in_cam=B_h[rows], poses=P[:, rows], errors=Eh[:, rows],
+                          summary=[_recover_summary(Eh[r, rows], aucs[r][0][j], aucs[r][1][j]) for r in range(K + 1)])
+        out[v] = res
+    return out
+
+
+def print_recover_tables(results, names):
+    """recoverYcbKeyframes' tables: one per class (names: {class id: label}), then the pooled one; a row per (checkpoint, mode,
+    round), round 0 (the perturbed start, the same in every variant) printed once.  AUCs in percent, errors in degrees and mm."""
+    variants = list(results)
+    first = results[variants[0]]
+    head = '%-5s %-8s %5s %6s %8s %8s %9s %9s %9s %9s' % ('ckpt', 'mode', 'round', 'rows', 'ADD', 'ADD-S', 'rot mean', 'rot med',
+                                                       'trans mean', 'trans med')
+
+    def line(ckpt, mode, r, s):
+        if s['rows'] == 0:
+            return '%-5s %-8s %5d %6d' % (ckpt, mode, r, 0)
+        return '%-5s %-8s %5d %6d %8.3f %8.3f %9.4g %9.4g %9.4g %9.4g' % (ckpt, mode, r, s['rows'], 100 * s['add_auc'], 100 * s['adds_auc'],
+                                                                       s['rot_mean'], s['rot_median'], s['trans_mean'], s['trans_median'])
+    for c in first:
+        label = 'all classes' if c == 'all' else 'class %d (%s)' % (c, names.get(c, c))
+        print('%s: %d rows; AUCs in percent (VOCap, 0.1 m), rotation in degrees, translation in mm' % (label, first[c]['rows']))
+        print(head)
+        print(line('-', 'start', 0, first[c]['summary'][0]))
+        for v in variants:
+            s = results[v][c]['summary']
+            for r in range(1, len(s)):
+                print(line(str(_variant_checkpoint(v)), v[0], r, s[r]))
+
+
 def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
     """What each mode of a precision sweep scores, and how far it drifts from the reference mode.  results: what getResultsYcbAll
     (YCBInEOAT_dir None) or getResultsYcbInEOAT returned for a sweep, {mode: ...}; outdir, ycb_dir and config (the path
@@ -1732,7 +1949,8 @@ def main(argv=None):
     parser = argparse.ArgumentParser(description='headless se(3)-TrackNet sequence tracking on libse3tn (flags of the reference predict.py:626-641)')
     parser.add_argument('--mode', default='ycbv', help='ycbv (one YCB-Video sequence) / ycbineoat / ycbv_all (every class of --class_ids '
                         'through every YCB-Video test sequence in one pass) / ycbineoat_all (every video under --YCBInEOAT_dir in one '
-                        'pass) / anything else: every YCB-Video test sequence of the class')
+                        'pass) / ycbv_recover (score refinement from the perturbed starts of the YCB-Video key frames, every class of '
+                        '--class_ids in one pass; nothing is written) / anything else: every YCB-Video test sequence of the class')
     parser.add_argument('--seq_id', default=None, type=int)
     parser.add_argument('--ycb_dir', default=None)
     parser.add_argument('--YCBInEOAT_dir', default=None)
@@ -1742,7 +1960,11 @@ def main(argv=None):
     parser.add_argument('--model_path', type=str, required=True, help='path to mesh (.ply with normals and vertex colours for the CUDA renderer)')
     parser.add_argument('--ckpt_dir', type=str, required=True)
     parser.add_argument('--mean_std_path', type=str, required=True)
-    parser.add_argument('--outdir', type=str, required=True)
+    parser.add_argument('--outdir', type=str, default=None, help='required by every mode but ycbv_recover')
+    parser.add_argument('--pair_model_path', default=None, help='ycbv_recover: path template of the mesh the perturbed pairs are '
+                        'cut with (default --model_path with .ply -> .obj, as ProducerPurturb picks it)')
+    parser.add_argument('--num_sample', type=int, default=10, help='ycbv_recover: perturbations drawn per annotated class and key frame')
+    parser.add_argument('--seed', type=int, default=0, help='ycbv_recover: seed of random and np.random before the first draw')
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
     parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt)')
     parser.add_argument('--max_frames', type=int, default=None)
@@ -1761,6 +1983,10 @@ def main(argv=None):
     parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
                         'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
+    if args.mode == 'ycbv_recover':
+        return _main_recover(args)
+    if args.outdir is None:
+        parser.error('the following arguments are required: --outdir')
     if args.gpus is not None and args.gpus < 1:
         raise SystemExit('--gpus %d: the number of GPUs is at least 1' % args.gpus)
     if args.gpus is not None and args.gpus > 1 and args.mode not in ('ycbv_all', 'ycbineoat_all'):
@@ -1805,11 +2031,11 @@ def cli_precision(text, mode):
         if text not in PRECISIONS:
             raise SystemExit('--precision %s: not a precision mode (one of %s)' % (text, ', '.join(PRECISIONS)))
         return text
-    if mode not in ('ycbv_all', 'ycbineoat_all'):
-        raise SystemExit('--precision %s: a list of modes or all needs --mode ycbv_all or ycbineoat_all' % text)
+    if mode not in ('ycbv_all', 'ycbineoat_all', 'ycbv_recover'):
+        raise SystemExit('--precision %s: a list of modes or all needs --mode ycbv_all or ycbineoat_all, or ycbv_recover' % text)
     precision = 'all' if text == 'all' else [m.strip() for m in text.split(',')]
     try:
-        precision_modes(precision, YCB_ALL_PRECISIONS if mode == 'ycbv_all' else PRECISIONS)
+        precision_modes(precision, YCB_ALL_PRECISIONS if mode in ('ycbv_all', 'ycbv_recover') else PRECISIONS)
     except ValueError as e:
         raise SystemExit('--precision %s: %s' % (text, e))
     return precision
@@ -1831,6 +2057,60 @@ def cli_iterations(text, mode):
     except ValueError as e:
         raise SystemExit('--iterations %s: %s' % (text, e))
     return counts
+
+
+def cli_recover(args):
+    """--mode ycbv_recover's arguments -> (class ids, class_config, keyword arguments of recoverYcbKeyframes); every refusal
+    recover_front makes, a missing argument and an unreadable --class_ids are a SystemExit, before anything is read but the
+    CADmodels/ names."""
+    if not args.ycb_dir or not args.class_ids:
+        raise SystemExit('--mode ycbv_recover needs --ycb_dir and --class_ids')
+    if args.gpus is not None and args.gpus != 1:
+        raise SystemExit('--gpus %d: %s' % (args.gpus, RECOVER_GPUS_REFUSAL))
+    precision = cli_precision(args.precision, args.mode)
+    iterations = cli_iterations(args.iterations, args.mode)
+    try:
+        recover_front(precision or 'bf16x3', iterations or 1)
+    except ValueError as e:
+        raise SystemExit('--precision / --iterations: %s' % e)
+    config = {key: getattr(args, key) for key in YCB_ALL_TEMPLATES}
+    if args.pair_model_path:
+        config['pair_model_path'] = args.pair_model_path
+    for key in ('ckpt_dir', 'mean_std_path'):
+        if ',' in config[key]:
+            config[key] = config[key].split(',')
+    try:
+        checkpoint_configs(config)
+    except ValueError as e:
+        raise SystemExit('--ckpt_dir / --mean_std_path: %s' % e)
+    if args.class_ids == 'all':
+        class_ids = list(range(1, len(ycb_class_names(args.ycb_dir)) + 1))
+    else:
+        try:
+            class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
+        except ValueError:
+            raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+    try:
+        pair_mesh_base(class_ids, len(checkpoint_configs(config)))
+    except ValueError as e:
+        raise SystemExit('--class_ids: %s' % e)
+    kw = dict(num_sample=args.num_sample, seed=args.seed, precision=precision or 'bf16x3', iterations=iterations or 1,
+              max_frames=args.max_frames)
+    return class_ids, config, kw
+
+
+def _main_recover(args):
+    """--mode ycbv_recover: recoverYcbKeyframes, then its tables (print_recover_tables)."""
+    class_ids, config, kw = cli_recover(args)
+    try:
+        res = recoverYcbKeyframes(args.ycb_dir, class_ids, config, **kw)
+    except ValueError as e:
+        raise SystemExit(str(e))
+    names = ycb_class_names(args.ycb_dir)
+    print('ycbv_recover: num_sample %d, seed %d, K = %d, %s' % (kw['num_sample'], kw['seed'], kw['iterations'],
+                                                               torch.cuda.get_device_name(torch.cuda.current_device())))
+    print_recover_tables(res, {c: names[c - 1] for c in class_ids})
+    return res
 
 
 def _main_one_pass(args, precision=None, iterations=None):

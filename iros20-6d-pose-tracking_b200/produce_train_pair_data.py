@@ -308,8 +308,9 @@ def ycbv_keyframe_jobs(ycb_dir, class_ids):
     return jobs
 
 
-def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None):
-    """One check_vis ProducerPurturb per class on `eng`, its mesh under id = class id.  templates: {'train_data_path',
+def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None, mesh_base=0):
+    """One check_vis ProducerPurturb per class on `eng`, its mesh under id = mesh_base + class id (mesh_base > 0 keeps the
+    producers' meshes apart from the tracking meshes a step draws under the weight ids).  templates: {'train_data_path',
     'model_path'} with {class_id} / {class_name} placeholders, as --mode ycbv_all takes them; dataset_info.yml is read from
     <train_data_path>/../.  The classes of a frame share one step, so they must share the camera.  -> (CADmodels folder names,
     {class id: producer})."""
@@ -321,7 +322,7 @@ def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None):
         paths = {k: str(templates[k]).format(class_id=c, class_name=name) for k in ('train_data_path', 'model_path')}
         with open(os.path.join(paths['train_data_path'], '../dataset_info.yml'), 'r') as ff:
             info = yaml.safe_load(ff)
-        producers[c] = ProducerPurturb(info, check_vis=True, engine=eng, model=paths['model_path'], mesh_id=c, workers=workers)
+        producers[c] = ProducerPurturb(info, check_vis=True, engine=eng, model=paths['model_path'], mesh_id=mesh_base + c, workers=workers)
     first_id = min(producers)
     for c, p in producers.items():
         if p.dataset_info['camera'] != producers[first_id].dataset_info['camera']:
@@ -329,13 +330,14 @@ def ycbv_producers(ycb_dir, class_ids, templates, eng, workers=None):
     return names, producers
 
 
-def ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead=4, workers=None, on_device=False):
+def ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead=4, workers=None, on_device=False, with_frame=False):
     """The key-frame loop of the YCB-Video mode, shared by produce_ycbv (which writes the kept pairs) and problems.validate_ycbv
     (which scores them).  jobs: ycbv_keyframe_jobs.  Per frame, decoded ahead through a StagingRing: one visibility call for all
     its classes (it synchronises), then, per visible class in class order, `draw` of num_sample offsets, then one pair step for
     every sample inside the image.  Yields, per frame with such a sample, (owners, res): owners [(class id, B_in_cam, [A_in_cam
     of its rows], first row)] and res pair_step's result for the frame's rows (a list of device chunks with on_device).  A frame's
-    device buffers are refilled once the loop resumes, so what res holds is consumed (or queued on the stream) before that."""
+    device buffers are refilled once the loop resumes, so what res holds is consumed (or queued on the stream) before that.
+    with_frame: yields (owners, res, (rgb, depth)) instead, the frame's device planes (the ring's: the same tensors every frame)."""
     from .predict import read_rgb, read_depth
     from .staging import StagingRing
     first = producers[min(producers)]
@@ -356,17 +358,18 @@ def ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead=4, workers=No
     frame = (ring.dev['rgb'], ring.dev['depth'], ring.dev['seg'])
     for k, _ in enumerate(ring.uploads(items, workers or min(16, os.cpu_count() or 4))):
         rows = jobs[k][3]
-        vis, cov = visibility(eng, frame[2], K32, [(B, c, c) for c, B in rows])
+        vis, cov = visibility(eng, frame[2], K32, [(B, producers[c].mesh_id, c) for c, B in rows])
         step, owners = [], []
         for (c, B), v, cv in zip(rows, vis, cov):
             if not visible_enough(v, cv):
                 continue
             inside = [A for A, ok in producers[c].draw(B, num_sample) if ok]
             owners.append((c, B, inside, len(step)))
-            step += [(A, producers[c].object_width, c, c) for A in inside]
+            step += [(A, producers[c].object_width, producers[c].mesh_id, c) for A in inside]
         if not step:
             continue
-        yield owners, pair_step(eng, frame, K32, step, on_device)
+        res = pair_step(eng, frame, K32, step, on_device)
+        yield (owners, res, frame[:2]) if with_frame else (owners, res)
 
 
 def produce_ycbv(ycb_dir, class_ids, templates, outdir, num_sample=10, seed=0, max_batch=64, decode_ahead=4, workers=None):
