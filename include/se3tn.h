@@ -358,6 +358,39 @@ int se3tn_set_depth_fill(se3tn_ctx* ctx, int enable, double max_depth, int extra
 #define SE3TN_MAX_REFINE_ITERATIONS 8
 int se3tn_set_refine_iterations(se3tn_ctx* ctx, int k);
 
+/* Check how well every track fits its frame inside each following se3tn_track_render / _rounds / _render_host step on this
+ * context: after the last round the step draws each track's model at poses_out (the same mesh, mode, camera size and object
+ * width as the rounds, depth only, into scratch of its own: the step's input A keeps the last round's) and compares the
+ * rendered depth R with the observed depth O in the crop window of poses_out, cropped exactly as K0 crops input B
+ * (se3tn_compute_bbox's window, se3tn_crop_bbox's nearest mapping, 0 outside the image; the filled frame when the step fills
+ * the depth).  R and O are uint16 mm before any clipping.  Track i's row, SE3TN_FIT_COLS int32 over its 176 x 176 pixels:
+ *   0 model     #(R > 0)
+ *   1 observed  #(R > 0, O > 0)
+ *   2 inlier    #(R > 0, O > 0, |O - R| <= tau_mm)
+ *   3 front     #(R > 0, O > 0, O < R - tau_mm)   something in front of the model: occlusion
+ *   4 behind    #(R > 0, O > 0, O > R + tau_mm)   the object is not where the model is
+ *   5 residual  sum of |O - R| over the inliers, mm
+ * observed = inlier + front + behind.  The rows are exact integers, independent of the order of the reduction.  The fit adds
+ * 3 launches (render 2, fit 1; se3tn_last_launch_count) and no profiling slot; it is captured in the step's CUDA graph
+ * (SE3TN_PREC_FP32 queues it as plain launches), and tau_mm is part of what makes two steps the same.  The step's poses,
+ * out_trans, out_rot and round_poses are bit for bit those of the step without it.  Device routes: the rows land in a
+ * context-owned device buffer (max_batch x SE3TN_FIT_COLS int32, allocated by the first enable, never moved), whose address
+ * se3tn_fit_rows gives; the next step overwrites them.  se3tn_track_render_host uploads the whole depth frame while the check
+ * is on (the window of poses_out is not known before the step; rgb stays windowed) and brings the n rows back in its one copy out, into pinned
+ * memory se3tn_fit_rows_host points at, valid until the next host step.  enable = 0 (the default) turns the check off;
+ * tau_mm is then ignored.  tau_mm outside [1, 1000] is SE3TN_ERR_INVALID and the setting is unchanged.  While it is on,
+ * se3tn_track_batch and se3tn_track_host return SE3TN_ERR_STATE and queue nothing: they take input A from the caller, and a
+ * weight id need not have a mesh.  A context is single-threaded: a caller that shares one between trackers sets the check
+ * it wants before each track call.  How well the rows predict tracking failure has not been measured on a trained
+ * checkpoint or real data (`predict --fit --score` reports it per run, README). */
+#define SE3TN_FIT_COLS 6
+int se3tn_set_fit_check(se3tn_ctx* ctx, int enable, int tau_mm);
+/* *rows = the device rows of the fit check (max_batch x SE3TN_FIT_COLS int32).  SE3TN_ERR_STATE before the first enable. */
+int se3tn_fit_rows(se3tn_ctx* ctx, const int32_t** rows);
+/* *rows = the n x SE3TN_FIT_COLS rows of the last se3tn_track_render_host step, in pinned host memory.  SE3TN_ERR_STATE when
+ * that step ran no fit check or failed. */
+int se3tn_fit_rows_host(se3tn_ctx* ctx, const int32_t** rows);
+
 /* The reference's own calling pattern as ONE call (Tracker.on_track, predict.py:217-296: numpy arrays in, numpy pose out):
  * every pointer is HOST memory.  The frame's crop-window rectangle, the poses, widths, input A and the ids are staged
  * through context-owned pinned memory into context-owned device buffers (stable addresses, so the step's CUDA graph is
@@ -603,12 +636,14 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
 /* Number of kernels the last forward / track_batch / track_render / eval_pairs / pair_loss call on this context launched (for a
- * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill).
+ * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill,
+ * and a step with the fit check its 3, se3tn_set_fit_check).
  * se3tn_track_batch, se3tn_track_render, their _host variants and se3tn_eval_pairs capture each distinct step into a CUDA
  * graph the first time they see it and replay it afterwards -- one graph launch per step.  Two calls are the same step when
  * every value their kernels are given is the same: tracking or validation, n, precision, the frame's H and W, K, the two
  * normalizers, the first weight id and whether the ids use more than one set, the render mode and camera image size, the
- * depth-fill setting (se3tn_set_depth_fill), the refinement count of a step that renders input A (se3tn_set_refine_iterations),
+ * depth-fill setting (se3tn_set_depth_fill), the refinement count and fit check of a step that renders input A
+ * (se3tn_set_refine_iterations, se3tn_set_fit_check),
  * and the address of every device array, in or out.  A replay reads what those
  * arrays hold at the time, and a call's host ids only decide the first id and the mix.  SE3TN_GRAPH=0 in the environment,
  * an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.

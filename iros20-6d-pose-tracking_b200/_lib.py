@@ -15,6 +15,7 @@ PROFILE_SLOTS = 22
 TRACE_TILES = 5184
 PAIR_MIN_SEG = 100
 MAX_REFINE_ITERATIONS = 8
+FIT_COLS = 6
 AUG_PARAMS = 24
 AUG_MAX_CORNERS = 64
 
@@ -57,6 +58,9 @@ SIGNATURES = {
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
     'se3tn_set_depth_fill': (_i, [_vp, _i, _d, _i, _i]),
     'se3tn_set_refine_iterations': (_i, [_vp, _i]),
+    'se3tn_set_fit_check': (_i, [_vp, _i, _i]),
+    'se3tn_fit_rows': (_i, [_vp, C.POINTER(_vp)]),
+    'se3tn_fit_rows_host': (_i, [_vp, C.POINTER(_vp)]),
     'se3tn_set_mesh': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i]),
     'se3tn_render': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),

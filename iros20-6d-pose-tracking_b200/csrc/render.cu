@@ -539,7 +539,7 @@ render_kernel(RenderArgs a)
         }
         const int orow = u.mode == 1 ? (kRS - 1 - j) : j;         // mode 1: rows were walked bottom-up, the image is stored top-down
         const size_t o = (static_cast<size_t>(n) * kRS + orow) * kRS + i;
-        a.rgb[o * 3] = static_cast<uint8_t>(r8); a.rgb[o * 3 + 1] = static_cast<uint8_t>(g8); a.rgb[o * 3 + 2] = static_cast<uint8_t>(b8);
+        if (a.rgb) { a.rgb[o * 3] = static_cast<uint8_t>(r8); a.rgb[o * 3 + 1] = static_cast<uint8_t>(g8); a.rgb[o * 3 + 2] = static_cast<uint8_t>(b8); }
         a.depth[o] = static_cast<uint16_t>(mm);
     }
 }

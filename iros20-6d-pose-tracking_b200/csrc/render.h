@@ -22,7 +22,7 @@ struct RenderArgs {
     int max_nv;                    // vertex count of the largest model
     int mode;                      // 0: vispy-style (lit, the crop window is the viewport); 1: pyrender-style (unlit full camera image vw x vh, then crop_bbox)
     int vw, vh;                    // mode 1: camera image size
-    uint8_t* rgb;                  // [n][176][176][3]
+    uint8_t* rgb;                  // [n][176][176][3], or null: depth only (the fit check of a track step)
     uint16_t* depth;               // [n][176][176] mm, 0 = background
 };
 size_t render_uniform_bytes();

@@ -9,6 +9,7 @@
 #include "render.h"
 #include <dlfcn.h>
 #include "depth_fill.h"
+#include "fit.h"
 #include "storage.cuh"
 
 #include <algorithm>
@@ -222,6 +223,7 @@ struct StepKey {
     uint16_t fill_blur, iterations;            // iterations: c->refine_iterations in a track step (zero in a validation step)
     int32_t n, precision, first_wid;           // first_wid: the first track's weight set
     int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
+    int32_t fit_tau, fit_pad;                  // track step that renders input A: c->fit_tau (0: no fit check); fit_pad is always 0
     F64Bits K[4], tn, rn, fill_max_depth;
     AugKey aug;                                // validation step: the augmentation of input B (aug.stages 0: none)
     const uint8_t* aug_seg; const int64_t* pair_index; uint8_t* aug_rgb; uint16_t* aug_depth;   // its maskB (NULL: depthB > 100), keys, output
@@ -233,6 +235,7 @@ struct StepKey {
     float* sq; double* labels; float* sums;                                               // validation step
     const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
     double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render_rounds) or NULL
+    int32_t* fit_rows;                         // fit_tau > 0: the rows of the fit check, n x kFitCols
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -266,6 +269,11 @@ struct se3tn_ctx {
     // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
     struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
     int refine_iterations = 1;       // se3tn_set_refine_iterations: render -> network -> pose update rounds of a track step that renders input A
+    // se3tn_set_fit_check: tau in mm, 0 off.  The block holds the device route's rows (max_batch x kFitCols int32), then the fit's
+    // rendered depth for max_batch tracks; allocated by the first enable, never moved after (captured steps hold both addresses)
+    int fit_tau = 0;
+    DevBuf<uint8_t> fit; size_t fit_bytes = 0;
+    const int32_t* fit_rows_host = nullptr;   // the last fitting host step's rows, inside hio.pin (se3tn_fit_rows_host)
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -287,6 +295,7 @@ struct se3tn_ctx {
     // state whose every change drops these graphs (or that is fixed for the context's life: workspace, scheduler, activation
     // tensor maps): the weight sets and their device tables (se3tn_load_weights), the statistics (se3tn_set_stats), the meshes
     // and rasteriser workspace (se3tn_set_mesh), the depth-fill block (reserve_fill) and the host-IO buffers (track_host_step).
+    // The fit check's block never moves once allocated (se3tn_set_fit_check).
     int use_graphs = 1;              // SE3TN_GRAPH=0: plain stream launches; set to 0 at run time if capture is not possible
     bool last_was_graph = false;
     struct StepGraph { StepKey key; Handle<cudaGraphExec_t> exec; int launches; unsigned long long last_use; };
@@ -690,14 +699,20 @@ int queue_preprocess(se3tn_ctx* c, PreprocessArgs a, int n, cudaStream_t s) {
     return SE3TN_OK;
 }
 
-int queue_render(se3tn_ctx* c, const double* K, const double* poses, const double* object_width, const int32_t* mesh_ids, int n,
-                 int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA, cudaStream_t s) {
+RenderArgs render_args(const se3tn_ctx* c, const double* K, const double* poses, const double* object_width, const int32_t* mesh_ids,
+                       int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA) {
     RenderArgs a;
     a.poses = poses; a.object_width = object_width; a.mesh_ids = mesh_ids; a.meshes = c->d_meshes.get(); a.n_meshes = c->mesh_rows;
     a.fx = K[0]; a.fy = K[1]; a.cx = K[2]; a.cy = K[3];
     a.rgb = rgbA; a.depth = depthA;
     a.mode = mode == SE3TN_RENDER_PYRENDER ? 1 : 0; a.vw = W; a.vh = H;
     a.projected = c->render_proj.get(); a.uniforms = c->render_unif.get(); a.max_nv = c->render_max_nv;
+    return a;
+}
+
+int queue_render(se3tn_ctx* c, const double* K, const double* poses, const double* object_width, const int32_t* mesh_ids, int n,
+                 int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA, cudaStream_t s) {
+    const RenderArgs a = render_args(c, K, poses, object_width, mesh_ids, mode, H, W, rgbA, depthA);
     { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s)); }
     c->launches += 2;
     return SE3TN_OK;
@@ -1207,20 +1222,31 @@ Step track_step(const se3tn_ctx* c, int H, int W, const double* K, const int32_t
     return st;
 }
 
-// se3tn_track_batch / se3tn_track_host take input A from the caller: a later round could not redraw it at the refined pose.
+// se3tn_track_batch / se3tn_track_host take input A from the caller: a later round could not redraw it at the refined pose,
+// and the fit check could not draw a model the weight id need not have.
 int check_single_round(se3tn_ctx* c, const char* fn) {
+    if (c->fit_tau)
+        return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": input A from the caller; the fit check (se3tn_set_fit_check) draws "
+                    "each track's model and needs se3tn_track_render[_host]");
     if (c->refine_iterations == 1) return SE3TN_OK;
     return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": input A from the caller cannot be redrawn; refine iterations is " +
                 std::to_string(c->refine_iterations) + " (se3tn_set_refine_iterations), which needs se3tn_track_render[_host]");
 }
 
+// The fit check's block (se3tn_set_fit_check): the device route's rows, then the fit's rendered depth of max_batch tracks.
+size_t fit_rows_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kFitCols * sizeof(int32_t)); }
+int32_t* fit_rows(se3tn_ctx* c) { return reinterpret_cast<int32_t*>(c->fit.get()); }
+uint16_t* fit_depth(se3tn_ctx* c) { return reinterpret_cast<uint16_t*>(c->fit.get() + fit_rows_bytes(c->max_batch)); }
+
 // A track step that draws input A first.  It lands in context scratch for max_batch tracks, allocated by the first such step:
-// its address never changes after, so captured steps stay valid.
+// its address never changes after, so captured steps stay valid.  With the fit check on, the step also runs the fit into the
+// context's rows (the host route points them at its own output block).
 int render_into_scratch(se3tn_ctx* c, const RenderSpec& r, Step& st) {
     const size_t img = static_cast<size_t>(kImg) * kImg, rgb_bytes = align256(static_cast<size_t>(c->max_batch) * img * 3);
     CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
     st.render_mode = r.mode; st.render_H = r.H; st.render_W = r.W;
     st.rgbA = c->in_a.get(); st.depthA = reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes);
+    if (c->fit_tau) { st.fit_tau = c->fit_tau; st.fit_rows = fit_rows(c); }
     return SE3TN_OK;
 }
 
@@ -1309,8 +1335,9 @@ int check_disjoint(se3tn_ctx* c, const char* fn, std::initializer_list<std::pair
 // (validation) -> conv stack -> the fp32 pose update (track) or the loss (validation: pair_loss in fp32, the reduction of the
 // head's terms otherwise).  A track step that renders input A repeats render -> preprocess -> conv stack -> pose update
 // st.iterations times on the same (filled) frame: round 0 reads poses_in, every later round reads and writes poses_out in place,
-// exactly as a chain of single-round steps would.  Arguments come from `st` alone, context state only as the graph cache's
-// comment in se3tn_ctx lists.
+// exactly as a chain of single-round steps would.  With st.fit_tau, the fit check follows the last round: render (depth only)
+// at poses_out -> fit_kernel, which writes st.fit_rows and nothing the rounds read.  Arguments come from `st` alone, context
+// state only as the graph cache's comment in se3tn_ctx lists.
 int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
     c->launches = 0;
     const double K[4] = {st.K[0], st.K[1], st.K[2], st.K[3]};
@@ -1400,6 +1427,21 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
             if (fp32) CU_TRY(c, launch_pair_loss(st.out_trans, st.out_rot, nullptr, nullptr, head.loss, st.n, st.sums, s));
             else CU_TRY(c, launch_loss_reduce(st.sq, st.n, st.sums, s));
         }
+        ++c->launches;
+    }
+    if (st.fit_tau) {
+        // the fit check at poses_out: render_project_kernel (PDL) reads the poses the last round's head / pose update wrote only
+        // after its griddepcontrol.wait, as a later round's render does, and fit_kernel reads the depth drawn here, the poses and
+        // the frame only after its own.  Depth only, into the fit's scratch: the step's input A keeps the last round's.  No
+        // profiling slot: slot 20 keeps timing the last round's render.
+        const RenderArgs ra = render_args(c, K, st.poses_out, st.object_width, st.wid_dev, st.render_mode, st.render_H, st.render_W,
+                                          nullptr, fit_depth(c));
+        CU_TRY(c, launch_render(ra, st.n, s));
+        c->launches += 2;
+        FitArgs fa;
+        fa.poses = st.poses_out; fa.object_width = st.object_width; fa.fx = K[0]; fa.fy = K[1]; fa.cx = K[2]; fa.cy = K[3];
+        fa.frame_depth = depth; fa.H = st.H; fa.W = st.W; fa.rendered = fit_depth(c); fa.tau = st.fit_tau; fa.rows = st.fit_rows;
+        CU_TRY(c, launch_fit(fa, st.n, s));
         ++c->launches;
     }
     return SE3TN_OK;
@@ -1968,6 +2010,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
+    c->fit_rows_host = nullptr;                    // the pinned block may move below
     bool multi = false;
     int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);   // before anything is staged or copied
     if (rc) return rc;
@@ -1981,9 +2024,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (io.H != H || io.W != W || io.n_cap < n) {
         CU_TRY(c, cudaStreamSynchronize(s));
         const int cap = std::max(n, io.n_cap);
-        const size_t per = 128 + 8 + img * 3 + img * 2 + 4 + 128 + 12 + 12;
+        const size_t per = 128 + 8 + img * 3 + img * 2 + 4 + 128 + 12 + 12 + 4 * kFitCols;
         c->graphs.clear();                                       // before the buffers are replaced: captured steps hold their addresses
-        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 8 * 256));
+        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 9 * 256));
         CU_TRY(c, grow(io.pin, io.pin_bytes, px * 5 + per * cap + 4096));
         CU_TRY(c, cudaMemsetAsync(io.dev.get(), 0, io.dev_bytes, s));   // on the caller's stream, ahead of the copies below; frame pixels outside the uploaded windows are never read, keep them defined
         io.H = H; io.W = W; io.n_cap = cap;
@@ -1996,7 +2039,8 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     const size_t nn = static_cast<size_t>(n), a_img = render ? 0 : img;
     const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * a_img * 3),
                  o_wid = o_depthA + align256(nn * a_img * 2), in_bytes = o_wid + align256(nn * 4);
-    const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), out_bytes = o_ro + align256(nn * 12);
+    const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), o_fit = o_ro + align256(nn * 12);
+    const size_t out_bytes = c->fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
     double* d_ow = reinterpret_cast<double*>(d_in + o_ow);
@@ -2007,6 +2051,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     double* d_out = reinterpret_cast<double*>(d_res);
     float* d_tr = reinterpret_cast<float*>(d_res + o_tr);
     float* d_ro = reinterpret_cast<float*>(d_res + o_ro);
+    int32_t* d_fit = reinterpret_cast<int32_t*>(d_res + o_fit);
     // ---- the part of the frame the tracks' crop windows touch (K0 reads nothing else) ----
     int y0 = H, y1 = 0, x0 = W, x1 = 0;
     for (int i = 0; i < n; ++i) {
@@ -2022,8 +2067,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (whole_frame || static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
     // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
-    // median-filtered image, and extrapolate scans whole columns.  Then the whole depth frame goes up; rgb stays windowed.
-    const bool whole_depth = c->depth_fill.on;
+    // median-filtered image, and extrapolate scans whole columns.  The fit check crops the depth at the windows of the poses the
+    // step computes.  Then the whole depth frame goes up; rgb stays windowed.
+    const bool whole_depth = c->depth_fill.on || c->fit_tau;
     uint8_t* hp = io.pin.get();
     const int wh = y1 - y0, ww = x1 - x0;
     if (wh > 0 && ww > 0) {
@@ -2058,10 +2104,12 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     st.rgbA = d_rgbA; st.depthA = d_depthA; st.wid_dev = weight_ids ? d_wid : nullptr;
     st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
     if (render && (rc = render_into_scratch(c, *render, st))) return rc;
+    if (st.fit_tau) st.fit_rows = d_fit;
     if ((rc = run_step(c, st, s))) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
-    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
+    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
+    if (st.fit_tau) c->fit_rows_host = reinterpret_cast<const int32_t*>(ho + o_fit);
     memcpy(poses_out, ho, nn * 128);
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
@@ -2151,6 +2199,34 @@ int se3tn_set_refine_iterations(se3tn_ctx* c, int k) {
     if (k < 1 || k > SE3TN_MAX_REFINE_ITERATIONS)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_set_refine_iterations: k must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
     c->refine_iterations = k;
+    return SE3TN_OK;
+}
+
+int se3tn_set_fit_check(se3tn_ctx* c, int enable, int tau_mm) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!enable) { c->fit_tau = 0; return SE3TN_OK; }
+    if (tau_mm < 1 || tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_fit_check: tau_mm must be in [1, 1000]");
+    if (!c->fit) {                                 // once, at its full size: steps captured after keep its addresses
+        DeviceGuard guard(c->device);
+        CU_TRY(c, grow(c->fit, c->fit_bytes, fit_rows_bytes(c->max_batch) + static_cast<size_t>(c->max_batch) * kImg * kImg * sizeof(uint16_t)));
+    }
+    c->fit_tau = tau_mm;
+    return SE3TN_OK;
+}
+
+int se3tn_fit_rows(se3tn_ctx* c, const int32_t** rows) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!rows) return fail(c, SE3TN_ERR_INVALID, "se3tn_fit_rows: null argument");
+    if (!c->fit) return fail(c, SE3TN_ERR_STATE, "se3tn_fit_rows: the fit check was never enabled (se3tn_set_fit_check)");
+    *rows = fit_rows(c);
+    return SE3TN_OK;
+}
+
+int se3tn_fit_rows_host(se3tn_ctx* c, const int32_t** rows) {
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!rows) return fail(c, SE3TN_ERR_INVALID, "se3tn_fit_rows_host: null argument");
+    if (!c->fit_rows_host) return fail(c, SE3TN_ERR_STATE, "se3tn_fit_rows_host: the last host step ran no fit check");
+    *rows = c->fit_rows_host;
     return SE3TN_OK;
 }
 

@@ -68,6 +68,7 @@ class Engine:
             torch.cuda.synchronize(self.device)
             self.lib.se3tn_destroy(self._ctx)
             self._ctx = None
+            self._fit_rows = None
 
     def __del__(self):
         try:
@@ -272,7 +273,8 @@ class Engine:
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
-                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1, out_rounds=None):
+                     out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1, out_rounds=None,
+                     fit=None, out_fit=None):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
@@ -280,16 +282,21 @@ class Engine:
         of render -> network -> pose update on this frame in the one step, exactly what k chained calls with iterations=1
         compute (se3tn_set_refine_iterations, 1..8); out_trans / out_rot hold the last round's outputs.  out_rounds: a float64
         CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_render_rounds): entry r - 1 is
-        what a call with iterations=r returns.  The step with it is a CUDA graph of its own."""
+        what a call with iterations=r returns.  The step with it is a CUDA graph of its own.  fit: tau in mm (fit_spec) turns
+        on the fit check of the step (se3tn_set_fit_check): every track's model is drawn at its new pose and compared with the
+        observed depth, and the call returns a fourth value, out_fit: an int32 CUDA tensor (n, 6) of the rows (model, observed,
+        inlier, front, behind, residual), allocated when None and filled on the current stream."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
-                           fill_depth, iterations, out_rounds)
+                           fill_depth, iterations, out_rounds, fit, out_fit)
 
     def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, out_rounds=None):
+               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, out_rounds=None,
+               fit=None, out_fit=None):
         """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
         n = poses.shape[0]
         iterations = self.refine_iterations(iterations)
+        tau = self.fit_spec(fit)
         self._check_frame(fn, frame_rgb, frame_depth, poses, object_width, A, n)
         wh = self._host_ids(fn, weight_ids_host, n)
         fill = self.depth_fill_spec(fill_depth)
@@ -301,8 +308,12 @@ class Engine:
             weight_ids_dev = torch.from_numpy(wh).to(self.device)
         if out_rounds is not None:
             self._check_dev('out_rounds', out_rounds, torch.float64, (iterations, n, 4, 4))
+        if tau:
+            out_fit = torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=self.device) if out_fit is None else out_fit
+            self._check_dev('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS))
         self._set_depth_fill(fill)
         self._set_refine(iterations)
+        self._set_fit(tau)
         H, W = frame_depth.shape
         head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
         tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
@@ -314,7 +325,10 @@ class Engine:
         else:
             rc = self.lib.se3tn_track_render(*head, *render, *tail)
         _lib.check(rc, self._ctx)
-        return out_poses, out_trans, out_rot
+        if not tau:
+            return out_poses, out_trans, out_rot
+        out_fit.copy_(self._fit_rows_view()[:n])         # the next step overwrites the context's rows
+        return out_poses, out_trans, out_rot, out_fit
 
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
                    weight_ids=None, precision='bf16x3', want_residuals=False, fill_depth=None):
@@ -327,19 +341,22 @@ class Engine:
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                           weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None,
-                          iterations=1):
+                          iterations=1, fit=None):
         """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
-        without ids); mode / image_hw as in render(); iterations as in track_render (k > 1 uploads the whole frame)."""
+        without ids); mode / image_hw as in render(); iterations as in track_render (k > 1 uploads the whole frame).  fit as in
+        track_render (the whole depth frame is uploaded then): the fit rows come last in what the call returns, an int32 numpy
+        array (n, 6)."""
         return self._track_host('track_render_host', frame_rgb, frame_depth, K, poses, object_width, (),
                                 self._render_mode(mode, image_hw), trans_normalizer, rot_normalizer, weight_ids, precision,
-                                want_residuals, fill_depth, iterations)
+                                want_residuals, fill_depth, iterations, fit)
 
     def _track_host(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-                    weight_ids, precision, want_residuals, fill_depth, iterations):
+                    weight_ids, precision, want_residuals, fill_depth, iterations, fit=None):
         """track_host (A = (rgbA, depthA), render None) and track_render_host (A = (), render = _render_mode's triple)."""
         n = int(poses.shape[0])
         iterations = self.refine_iterations(iterations)
+        tau = self.fit_spec(fit)
         for name, a, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
             if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
                 raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, dt, shape))
@@ -351,6 +368,7 @@ class Engine:
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         self._set_depth_fill(fill)
         self._set_refine(iterations)
+        self._set_fit(tau)
         H, W = frame_depth.shape
         head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
         tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
@@ -360,7 +378,12 @@ class Engine:
         else:
             rc = self.lib.se3tn_track_render_host(*head, *render, *tail)
         _lib.check(rc, self._ctx)
-        return (out, tr, ro) if want_residuals else out
+        res = (out, tr, ro) if want_residuals else (out,)
+        if tau:
+            p = C.c_void_p()
+            _lib.check(self.lib.se3tn_fit_rows_host(self._ctx, C.byref(p)), self._ctx)
+            res += (np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int32)), shape=(n, _lib.FIT_COLS)).copy(),)
+        return res if len(res) > 1 else out
 
     # ------------------------------------------------------------------ checkpoint validation
     def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
@@ -802,6 +825,33 @@ class Engine:
     def _set_refine(self, k):
         """Every tracking call sets the refinement count it wants, as it sets the fill mode: track_batch / track_host set 1."""
         _lib.check(self.lib.se3tn_set_refine_iterations(self._ctx, int(k)), self._ctx)
+
+    @staticmethod
+    def fit_spec(fit):
+        """The fit check of a tracking call as se3tn_set_fit_check's tau in mm: None -> 0 (off), an integer in [1, 1000] -> itself,
+        else a ValueError."""
+        if fit is None:
+            return 0
+        if isinstance(fit, (bool, np.bool_)) or not isinstance(fit, (int, np.integer)) or not 1 <= fit <= 1000:
+            raise ValueError('fit must be None or an integer tau in mm in [1, 1000], not %r' % (fit,))
+        return int(fit)
+
+    def _set_fit(self, tau):
+        """Every tracking call sets the fit check it wants, as it sets the fill mode: track_batch / track_host turn it off."""
+        _lib.check(self.lib.se3tn_set_fit_check(self._ctx, int(tau > 0), int(tau) if tau else 1), self._ctx)
+
+    def _fit_rows_view(self):
+        """An int32 CUDA tensor (max_batch, 6) over the context's fit rows (se3tn_fit_rows; the address never changes)."""
+        if getattr(self, '_fit_rows', None) is None:
+            p = C.c_void_p()
+            _lib.check(self.lib.se3tn_fit_rows(self._ctx, C.byref(p)), self._ctx)
+            shape = (self.max_batch, _lib.FIT_COLS)
+
+            class _Rows:                                 # a borrowed device array: no stream, so torch adds no synchronisation
+                __cuda_array_interface__ = {'shape': shape, 'typestr': '<i4', 'data': (p.value, False), 'version': 2}
+            with torch.cuda.device(self.device):
+                self._fit_rows = torch.as_tensor(_Rows(), device=self.device)
+        return self._fit_rows
 
     # ------------------------------------------------------------------ introspection
     def debug_buffer(self, buf_id, n):

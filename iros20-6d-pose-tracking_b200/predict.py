@@ -37,6 +37,25 @@ from .staging import StagingRing, VideoSink
 from . import Utils as U
 
 _refine_iterations = Engine.refine_iterations      # the drivers check counts before any Engine exists
+_fit_spec = Engine.fit_spec                         # and the fit check's tau
+# Tracker(fit=True)'s tau: a starting guess for a sensor's depth noise at a metre or so, not measured on a real sensor
+FIT_TAU_DEFAULT = 10
+
+
+def fit_fractions(rows):
+    """The derived numbers of fit-check rows (Engine.track_render's fit; (..., 6) int32: model, observed, inlier, front, behind,
+    residual) -> dict of float64 arrays of the leading shape: 'inlier' inlier / model, 'front' front / model, 'behind' behind / model,
+    'residual' residual / inlier in mm (the mean inlier residual).  Each is 0 where its denominator is 0.  Rows of -1 (a frame
+    that was not tracked) give NaN."""
+    r = rows.cpu().numpy() if torch.is_tensor(rows) else np.asarray(rows)
+    r = r.astype(np.float64)
+    div = lambda a, b: np.divide(a, b, out=np.zeros_like(a), where=b > 0)
+    out = {'inlier': div(r[..., 2], r[..., 0]), 'front': div(r[..., 3], r[..., 0]), 'behind': div(r[..., 4], r[..., 0]),
+           'residual': div(r[..., 5], r[..., 2])}
+    untracked = (r == -1).all(axis=-1)
+    for v in out.values():
+        v[untracked] = np.nan
+    return out
 
 
 class PointCloud:
@@ -124,15 +143,21 @@ def _as_numpy_pose(p):
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
-                 fill_depth=False, iterations=1):
+                 fill_depth=False, iterations=1, fit=None):
         """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
         tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
         / blur_type (Engine.depth_fill_spec).
         iterations: on_track / on_track_batch refine every track k times on each frame, in one tracking step (Engine.track_render),
         exactly as k chained calls with iterations=1 would.  k > 1 needs the CUDA rasteriser drawing input A inside the step: a
-        reference GL renderer is a ValueError here, and input A passed to a call is a ValueError there."""
+        reference GL renderer is a ValueError here, and input A passed to a call is a ValueError there.
+        fit: the fit check of every tracking step (Engine.track_render's fit): None / False off, True FIT_TAU_DEFAULT mm, or tau in
+        mm (1..1000).  on_track / on_track_batch then leave the frame's rows (model, observed, inlier, front, behind, residual per
+        track) in last_fit: numpy on the host route, an int32 CUDA tensor on the device route; fit_fractions turns them into
+        fractions.  Like iterations > 1 it needs the CUDA rasteriser drawing input A inside the step."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
         self.iterations = Engine.refine_iterations(iterations)
+        self.fit = Engine.fit_spec(FIT_TAU_DEFAULT if fit is True else (None if fit is False else fit)) or None
+        self.last_fit = None
         self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
@@ -185,6 +210,9 @@ class Tracker:
         if self.iterations > 1 and not isinstance(self.renderer, CudaRenderer):
             raise ValueError('iterations=%d redraws input A every round inside the tracking step: it needs the CUDA renderer '
                              '(renderer="cuda"), not %r' % (self.iterations, self.renderer))
+        if self.fit and not isinstance(self.renderer, CudaRenderer):
+            raise ValueError('fit=%d draws every model at its new pose inside the tracking step: it needs the CUDA renderer '
+                             '(renderer="cuda"), not %r' % (self.fit, self.renderer))
         self._np_bufs = {}
         self._copy_stream = torch.cuda.Stream(device=self.engine.device)      # _uploads: two staging slots, used alternately
         self._stage_bufs = ({}, {})
@@ -259,7 +287,7 @@ class Tracker:
         Tracker.iterations times."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
-        if self.iterations > 1 and not fused:
+        if (self.iterations > 1 or self.fit) and not fused:
             raise ValueError(self._refine_refusal(rgbA is not None or depthA is not None))
         if fused:
             out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
@@ -298,8 +326,9 @@ class Tracker:
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
-        if self.iterations > 1 and renderer is None:
+        if (self.iterations > 1 or self.fit) and renderer is None:
             raise ValueError(self._refine_refusal(not render))
+        self.last_fit = None
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
                 and not any(torch.is_tensor(x) for x in (prev_poses, weight_ids, object_width))):
@@ -314,8 +343,12 @@ class Tracker:
                     self._calibrate_fp8(weight_ids, wh, *d)
             kw = dict(weight_ids=wh, precision=self.precision, fill_depth=self.fill_depth)
             if renderer is not None:
-                return self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations, **kw)
+                out = self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
+                                                    mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
+                                                    fit=self.fit, **kw)
+                if self.fit:
+                    out, self.last_fit = out
+                return out
             return self.engine.track_host(*frame, self.K, poses, ow, *A, self.trans_normalizer, self.rot_normalizer, **kw)
 
         dev = self.engine.device
@@ -342,17 +375,24 @@ class Tracker:
                 outs = dict(out_poses=ob[0], out_trans=ob[1], out_rot=ob[2])
             kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
             if renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
-                out, _, _ = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
-                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations, **kw)
+                res = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
+                                               mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
+                                               fit=self.fit, **kw)
+                out = res[0]
+                if self.fit:
+                    self.last_fit = res[3]
             else:
                 out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
                                                     self.trans_normalizer, self.rot_normalizer, **kw)
         return out.cpu().numpy() if as_numpy else out
 
     def _refine_refusal(self, given):
-        """Why a call of a Tracker with iterations > 1 cannot run: input A given (given), or a renderer the step cannot stand in for."""
+        """Why a call of a Tracker with iterations > 1 or a fit check cannot run: input A given (given), or a renderer the step
+        cannot stand in for."""
         why = 'input A was passed in' if given else 'the renderer cannot draw input A inside the tracking step (_fused_renderer)'
-        return 'iterations=%d redraws input A at each refined pose, but %s' % (self.iterations, why)
+        needs = (['iterations=%d redraws input A at each refined pose' % self.iterations] if self.iterations > 1 else []) + \
+                (['fit=%d draws every model at its new pose' % self.fit] if self.fit else [])
+        return '%s, but %s' % (' and '.join(needs), why)
 
     def _weight_ids(self, weight_ids, n):
         """The tracks' weight ids as an int32 host array: the Tracker's weight set unless given, None for set 0 (a step
@@ -1025,7 +1065,7 @@ def _one_pass_trackers(entries, precision, max_batch):
     return eng, trackers
 
 
-def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None):
+def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
     variants: what every frame is tracked in (a tuple) as _sweep_variants keys them, (mode, k) or (mode, k, c): precision mode, k
@@ -1046,7 +1086,10 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     Then each frame's decode jobs also render its label strip into the ring, and after each step Engine.draw_tracks draws every
     track's Tracker.object_cloud points at its new pose over the device frame (the point sets uploaded once, as one table), and a
     VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed.
-    Videos are drawn for one variant only."""
+    Videos are drawn for one variant only.
+
+    fit: tau in mm turns on every step's fit check (Engine.track_render's fit); each sequence's yield is then a pair, the poses
+    as above and {variant: (frames, n, 6) int32 numpy rows}, row t the fit of the step that wrote pose t."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
     fp8 = {}                                               # checkpoint index -> its first fp8 variant
@@ -1093,6 +1136,7 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                                   None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
                 by_n[v, n][0].copy_(torch.from_numpy(init))
             history = {v: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for v in variants}
+            fit_rows = {v: torch.empty((len(rgb_files), n, 6), dtype=torch.int32, device=dev) for v in variants} if fit else None
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
@@ -1108,13 +1152,14 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
                                      image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot,
-                                     iterations=rounds)
+                                     iterations=rounds, **({'fit': fit, 'out_fit': fit_rows[v][t]} if fit else {}))
                     history[v][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
                                     label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
                     sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
-            yield {v: h.cpu().numpy() for v, h in history.items()}
+            tracked = {v: h.cpu().numpy() for v, h in history.items()}
+            yield (tracked, {v: r.cpu().numpy() for v, r in fit_rows.items()}) if fit else tracked
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1202,11 +1247,12 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
                                  render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
 
 
-def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes):
+def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0):
     """One process's share of a one-pass run, sequences[k] for k in mine: the Engine and Trackers of `entries`
     (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
     share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
-    [(paths, labels)] per sequence, folders to make once the trackers exist).  -> (Engine, {k: what writes[k] returned})."""
+    [(paths, labels)] per sequence, folders to make once the trackers exist).  fit: _track_sequences' fit (then writes[k] gets
+    its (poses, fit rows) pair).  -> (Engine, {k: what writes[k] returned})."""
     eng, trackers = _one_pass_trackers(entries, precision, max_batch)
     for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
         _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
@@ -1216,14 +1262,15 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
             os.makedirs(d, exist_ok=True)
         drawn = (video[0], [video[1][k] for k in mine])
     out = {}
-    for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn), mine):
+    fit_kw = {'fit': fit} if fit else {}
+    for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn, **fit_kw), mine):
         fn, *args = writes[k]
         out[k] = fn(*args, tracked)
     return eng, out
 
 
 def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
-               writes):
+               writes, fit=0):
     """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: _track_share with the weight sets of its
     sequences.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error', traceback text) through
     conn."""
@@ -1232,7 +1279,7 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
         wids = _rank_weight_ids(sequences, mine, variants)
         torch.cuda.set_device(device)
         eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
-                                depth, workers, video, writes)
+                                depth, workers, video, writes, fit)
         conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
     except BaseException:
         conn.send(('error', traceback.format_exc()))
@@ -1259,7 +1306,7 @@ def _agree_fp8_scales(per_rank):
     return {w: s for w, (_, s) in sorted(out.items())}
 
 
-def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes):
+def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0):
     """_track_share over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
     rank (_rank_main) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
     frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
@@ -1283,7 +1330,7 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
             borrowed = borrowed_calibrations(track_sets, mine) if fp8 else {}
             p = ctx.Process(target=_rank_main, name='one-pass rank %d' % r, daemon=True,
                             args=(send, r, devices[r], entries, precision, max_batch, sequences, mine, borrowed, variants, depth,
-                                  workers, video, writes))
+                                  workers, video, writes, fit))
             try:
                 p.start()
             finally:
@@ -1322,6 +1369,24 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
     return [results[k] for k in range(len(sequences))]
 
 
+# The fit check in the one-pass drivers: FIT_FILE beside each sequence's pose files.  Not a .txt (eval_ycb globs **/*.txt under a
+# tree) and never at a tree's root (eval_ycbineoat takes every root entry for a video folder).
+FIT_FILE = 'fit.npy'
+# --score's fit table: a frame whose ADD-S is at least this far from the annotation counts as lost (a fixed bound, not an option)
+FIT_LOST_ADDS = 0.02
+
+
+def _driver_fit(fit):
+    """The drivers' fit argument -> tau in mm, 0 for None (Engine.fit_spec; checked before anything is read)."""
+    return _fit_spec(fit)
+
+
+def write_fit_rows(folder, rows):
+    """<folder>/FIT_FILE: the fit rows of a sequence as int32 (frames, 6)."""
+    os.makedirs(folder, exist_ok=True)
+    np.save(os.path.join(folder, FIT_FILE), np.ascontiguousarray(rows, dtype=np.int32))
+
+
 # What a one-pass driver's shared front hands its back: the GPU count, the first mode (the Trackers' precision, which
 # ycb_all_classes / ycbineoat_objects check), the variants (_sweep_variants) and whether modes and counts are swept.
 _OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep configs')
@@ -1344,21 +1409,24 @@ def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
     return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs)
 
 
-def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect):
+def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0):
     """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
     (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
     sequence k's poses.  With several checkpoints, a run whose weight sets do not fit in free device memory is refused first
     (check_weight_sets_fit; per rank on several GPUs).  -> the driver's return value: _sweep_results of {variant:
-    collect(written, variant)}, written being [what writes[k] returned] in sequence order."""
+    collect(written, variant)}, written being [what writes[k] returned] in sequence order.  fit: every step's fit check
+    (_track_sequences), writes[k] then taking the (poses, fit rows) pair."""
     keys = tuple(v[:-1] for v in run.variants)
     if run.gpus == 1 and len(run.configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
+    fit_kw = {'fit': fit} if fit else {}
     if run.gpus == 1:
         _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
-                              writes)
+                              writes, **fit_kw)
         written = [out[k] for k in range(len(sequences))]
     else:
-        written = _track_on_ranks(run.gpus, entries, run.precision, max_batch, sequences, keys, depth, workers, video, writes)
+        written = _track_on_ranks(run.gpus, entries, run.precision, max_batch, sequences, keys, depth, workers, video, writes,
+                                  **fit_kw)
     return _sweep_results({key: collect(written, key) for key in keys}, run.variants, run.sweep, run.ksweep)
 
 
@@ -1382,8 +1450,19 @@ def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
     return out
 
 
+def _write_ycb_all_sequence_fit(dirs, seq_id, cls, init, tracked):
+    """_write_ycb_all_sequence with the fit check: tracked is (poses, fit rows); each class's seq<id>/ also gets FIT_FILE, one
+    row per pose file, row 0 (the start pose, not tracked) all -1."""
+    poses, rows = tracked
+    out = _write_ycb_all_sequence(dirs, seq_id, cls, init, poses)
+    for v, folder in dirs.items():
+        for j, c in enumerate(cls):
+            write_fit_rows(os.path.join(folder[c], 'seq{}'.format(seq_id)), np.concatenate([np.full((1, 6), -1, np.int32), rows[v][:, j]]))
+    return out
+
+
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1):
+                     video=False, iterations=1, gpus=1, fit=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1418,8 +1497,13 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     class_config['ckpt_dir'] (and 'mean_std_path') may be lists of templates, one per checkpoint (checkpoint_configs): every
     frame is then tracked once per (checkpoint, mode, k), checkpoint i's sets under weight id class id + 32 i, its tree under
     <outdir>/ckpt<i>/ file for file what a run of it alone writes, and the return value is {i: what that run returns}.
-    score_checkpoints scores it.  video=True takes one checkpoint; weight sets beyond the device's free memory are refused."""
+    score_checkpoints scores it.  video=True takes one checkpoint; weight sets beyond the device's free memory are refused.
+
+    fit: tau in mm turns on every step's fit check (Engine.track_render's fit): each class's seq<id>/ of every tree also gets
+    FIT_FILE, int32 (pose files, 6), row i the fit of the step that wrote pose i, row 0 -1.  The pose files and the return value
+    are what the run without it gives.  score_fit reads it."""
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
+    fit = _driver_fit(fit)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
@@ -1447,7 +1531,8 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)],
                  [ycb_all_res_dir(tree, c) for c in name_of.values()])
     dirs = {v[:-1]: {c: ycb_all_res_dir(v[-1], name) for c, name in name_of.items()} for v in run.variants}
-    writes = [(_write_ycb_all_sequence, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
+    writer = _write_ycb_all_sequence_fit if fit else _write_ycb_all_sequence
+    writes = [(writer, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
 
     def collect(written, key):
         out = {c: {} for c in name_of}
@@ -1455,7 +1540,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
             for j, c in enumerate(cls):
                 out[c][seq_id] = pred_poses[key][:, j]
         return out
-    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect)
+    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect, fit)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1533,8 +1618,18 @@ def _write_ycbineoat_video(roots, video, tracked):
     return out
 
 
+def _write_ycbineoat_video_fit(roots, video, tracked):
+    """_write_ycbineoat_video with the fit check: tracked is (poses, fit rows); <tree>/<video>/ also gets FIT_FILE, one row per
+    pose file (every frame is tracked)."""
+    poses, rows = tracked
+    out = _write_ycbineoat_video(roots, video, poses)
+    for key, root in roots.items():
+        write_fit_rows(os.path.join(root, video), rows[key][:, 0])
+    return out
+
+
 def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
-                        video=False, iterations=1, gpus=1):
+                        video=False, iterations=1, gpus=1, fit=None):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -1563,9 +1658,12 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     single-GPU run's.
 
     object_config['ckpt_dir'] (and 'mean_std_path') may be lists of templates, one per checkpoint, as in getResultsYcbAll:
-    checkpoint i's sets under weight id object index + 32 i, its tree under <outdir>/ckpt<i>/."""
+    checkpoint i's sets under weight id object index + 32 i, its tree under <outdir>/ckpt<i>/.
+
+    fit: as in getResultsYcbAll; <tree>/<video>/FIT_FILE has one row per pose file, frame 0 included (it is tracked)."""
     from .eval_ycbineoat import OBJECTS
     run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config)
+    fit = _driver_fit(fit)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
@@ -1588,9 +1686,9 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
         drawn = ('over', [([os.path.join(tree, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()],
                  [tree])
     trees = {v[:-1]: v[-1] for v in run.variants}
-    writes = [(_write_ycbineoat_video, trees, v) for v in sequences]
+    writes = [(_write_ycbineoat_video_fit if fit else _write_ycbineoat_video, trees, v) for v in sequences]
     return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
-                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)})
+                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)}, fit)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1934,6 +2032,89 @@ def _score_ycb_tree(ycb_dir, root, class_ids):
     return (eval_ycb.VOCap(np.concatenate([e[0] for e in errs])) * 100, eval_ycb.VOCap(np.concatenate([e[1] for e in errs])) * 100)
 
 
+def roc_auc(score, positive):
+    """Area under the ROC curve of `score` as a detector of `positive` (bool): the chance that a random positive scores above a
+    random negative, ties counting half.  NaN without positives or without negatives."""
+    score, positive = np.asarray(score, np.float64), np.asarray(positive, bool)
+    npos, nneg = int(positive.sum()), int((~positive).sum())
+    if npos == 0 or nneg == 0:
+        return float('nan')
+    _, inv, counts = np.unique(score, return_inverse=True, return_counts=True)
+    ranks = (np.cumsum(counts) - (counts - 1) / 2.0)[inv]          # 1-based ranks, ties averaged
+    return float((ranks[positive].sum() - npos * (npos + 1) / 2.0) / (npos * nneg))
+
+
+def _fit_frames(root, ycb_dir, YCBInEOAT_dir=None, class_ids=None):
+    """The frames the tree's scorer scores that a step tracked, from the pose files and each folder's FIT_FILE -> (ADD-S in m,
+    fit rows (frames, 6)).  YCB-Video (class_ids): eval_ycb.eval_one_class's key frames of every class; YCBInEOAT: every frame
+    eval_ycbineoat.eval_all scores.  ADD-S is computed as those scorers compute it, on the same points and annotations."""
+    import glob
+    from . import eval_ycb, eval_ycbineoat
+    eng = U._eng()
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(np.stack(a).reshape(-1, 4, 4), dtype=np.float64)).to(eng.device)
+    adds, rows = [], []
+
+    def add(points, preds, gts, fit):
+        if preds:
+            adds.append(eng.add_adi(torch.from_numpy(np.ascontiguousarray(points)).to(eng.device), t(preds), t(gts))[1].cpu().numpy())
+            rows.append(np.stack(fit))
+    if YCBInEOAT_dir is None:
+        names = ycb_class_names(ycb_dir)
+        model_files = sorted(glob.glob('{}/CADmodels/**/points.xyz'.format(ycb_dir), recursive=True))
+        with open('{}/YCB_Video_toolbox/keyframe.txt'.format(ycb_dir)) as ff:
+            keyframes = set(line.rstrip() for line in ff.readlines())
+        for c in class_ids:
+            res_dir = ycb_all_res_dir(root, names[c - 1]) + '/'
+            preds, gts, fit, loaded = [], [], [], {}
+            for pose_file in sorted(glob.glob(res_dir + '**/*.txt', recursive=True)):
+                seq_dir = os.path.dirname(pose_file)
+                seq_id = int(pose_file.replace(res_dir, '').split('/')[0].replace('seq', ''))
+                i = int(os.path.basename(pose_file).split('.')[0])
+                if '%04d/%06d' % (seq_id, i + 1) not in keyframes:
+                    continue
+                r = loaded.setdefault(seq_dir, np.load(os.path.join(seq_dir, FIT_FILE)))[i]
+                if (r == -1).all():                      # the start pose: no step tracked it
+                    continue
+                preds.append(np.loadtxt(pose_file)); fit.append(r)
+                gts.append(np.loadtxt('{}/data_organized/%04d/pose_gt/{}/%06d.txt'.format(ycb_dir, c) % (seq_id, i + 1)))
+            add(eval_ycb._read_points(model_files[c - 1]), preds, gts, fit)
+    else:
+        models = eval_ycbineoat.model_points(ycb_dir)
+        for folder in sorted(os.listdir(root)):
+            d = os.path.join(root, folder)
+            if not os.path.isfile(os.path.join(d, FIT_FILE)):
+                continue
+            r = np.load(os.path.join(d, FIT_FILE))
+            pred_files = sorted(glob.glob(d + '/*.txt'))
+            gt_files = sorted(glob.glob(os.path.join(YCBInEOAT_dir, folder, 'annotated_poses', '*.txt')))
+            add(models[eval_ycbineoat.video_object(folder)], [np.loadtxt(f) for f in pred_files],
+                [np.loadtxt(f) for f in gt_files[:len(pred_files)]], list(r[:len(pred_files)]))
+    if not adds:
+        return np.zeros(0), np.zeros((0, 6), np.int32)
+    return np.concatenate(adds), np.concatenate(rows)
+
+
+def score_fit(root, ycb_dir, YCBInEOAT_dir=None, class_ids=None):
+    """How well the fit check flags lost frames in one variant's tree (a run with fit): over the frames _fit_frames finds, a frame
+    is lost when its ADD-S is at least FIT_LOST_ADDS (2 cm).  -> {'frames', 'lost' (share), 'inlier_lost' / 'inlier_kept' (mean
+    inlier fraction of the lost frames / of the rest, NaN for none), 'auc' (ROC AUC of 1 - inlier fraction as a detector of
+    the lost frames)}."""
+    adds, rows = _fit_frames(root, ycb_dir, YCBInEOAT_dir, class_ids)
+    lost = adds >= FIT_LOST_ADDS
+    inl = fit_fractions(rows)['inlier']
+    mean = lambda a: float(a.mean()) if len(a) else float('nan')
+    return dict(frames=int(len(adds)), lost=mean(lost.astype(np.float64)), inlier_lost=mean(inl[lost]), inlier_kept=mean(inl[~lost]),
+                auc=roc_auc(1.0 - inl, lost))
+
+
+def print_fit_table(rows):
+    """--score's table for a run with --fit: one row per variant tree of score_fit's result."""
+    print('fit check: frames with ADD-S >= %g cm count as lost; inlier fraction = inlier / model pixels' % (FIT_LOST_ADDS * 100))
+    print('%-16s %8s %8s %12s %12s %8s' % ('variant', 'frames', 'lost', 'inlier lost', 'inlier kept', 'ROC AUC'))
+    for label, r in rows.items():
+        print('%-16s %8d %8.4f %12.4f %12.4f %8.4f' % (label, r['frames'], r['lost'], r['inlier_lost'], r['inlier_kept'], r['auc']))
+
+
 def print_precision_table(ref, rows, sweep='precision sweep', column='mode'):
     """The table --score prints after a sweep's per-mode scores: one row per mode of score_precisions' result (per variant of
     score_iterations' with sweep='iteration sweep', column='variant')."""
@@ -1980,9 +2161,18 @@ def main(argv=None):
                         '(1..8, default 1).  ycbv_all / ycbineoat_all also take a comma-separated list: every frame is tracked with '
                         'each K, K\'s tree written under <outdir>/iter<K>/, and --score adds a table of each variant\'s AUCs and drift '
                         'from K = 1')
+    parser.add_argument('--fit', type=int, default=None, help='ycbv_all / ycbineoat_all: check every step\'s fit, tau in mm '
+                        '(1..1000): each sequence folder gets fit.npy beside its pose files, and --score adds the fit table')
     parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
                         'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
+    if args.fit is not None:
+        if args.mode not in ('ycbv_all', 'ycbineoat_all'):
+            raise SystemExit('--fit needs --mode ycbv_all or ycbineoat_all; --mode %s does not check the fit' % args.mode)
+        try:
+            _fit_spec(args.fit)
+        except ValueError as e:
+            raise SystemExit('--fit %d: %s' % (args.fit, e))
     if args.mode == 'ycbv_recover':
         return _main_recover(args)
     if args.outdir is None:
@@ -2134,7 +2324,7 @@ def _main_one_pass(args, precision=None, iterations=None):
     except ValueError as e:
         raise SystemExit('--%s: %s' % ('ckpt_dir / --mean_std_path', e))
     kw = {key: v for key, v in (('video', args.video or None), ('precision', precision), ('gpus', args.gpus),
-                                ('iterations', iterations)) if v is not None}
+                                ('iterations', iterations), ('fit', getattr(args, 'fit', None))) if v is not None}
     if ycbv:
         if args.class_ids == 'all':
             class_ids = list(range(1, len(ycb_class_names(args.ycb_dir)) + 1))
@@ -2175,6 +2365,12 @@ def _main_one_pass(args, precision=None, iterations=None):
     elif args.score:
         from . import eval_ycbineoat
         eval_ycbineoat.eval_all(argparse.Namespace(YCBInEOAT_dir=args.YCBInEOAT_dir, ycb_dir=args.ycb_dir, res_dir=outdir + '/'))
+    if args.score and getattr(args, 'fit', None):
+        modes, msweep = precision_modes(precision or 'bf16x3', YCB_ALL_PRECISIONS if ycbv else PRECISIONS)
+        counts, ksweep = refine_counts(iterations or 1)
+        trees = [v[-1] for v in _sweep_variants(outdir, modes, msweep, counts, ksweep, ckpts)]
+        print_fit_table({os.path.relpath(tr, outdir): score_fit(tr, args.ycb_dir, args.YCBInEOAT_dir if not ycbv else None,
+                                                                 class_ids if ycbv else None) for tr in trees})
     return res
 
 
