@@ -20,6 +20,7 @@ extern "C" {
 #endif
 
 typedef struct se3tn_ctx se3tn_ctx;
+typedef struct se3tn_track_opts se3tn_track_opts;   /* a tracking call's options (defined below) */
 
 enum {
     SE3TN_OK = 0,
@@ -186,13 +187,14 @@ int se3tn_so3_log(se3tn_ctx* ctx, const double* poses_a, const double* poses_b,
  * SE3TN_PREC_FP32 each contiguous run of equal ids is one batched forward.
  * out_trans/out_rot float32 (n,3) device scratch the caller provides (also returned).
  * poses_out may be poses_in: every read of a track's previous pose comes before its update is written, so tracks whose poses
- * stay in one device array, updated in place frame after frame, keep the step's addresses and its CUDA graph. */
+ * stay in one device array, updated in place frame after frame, keep the step's addresses and its CUDA graph.
+ * opts: the call's se3tn_track_opts, or NULL for the defaults (see there). */
 int se3tn_track_batch(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                       const double* K, const double* poses_in, const double* object_width,
                       const uint8_t* rgbA, const uint16_t* depthA,
                       const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                       double trans_normalizer, double rot_normalizer, int precision,
-                      float* out_trans, float* out_rot, double* poses_out, void* stream);
+                      float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, void* stream);
 
 /* The one exchange step of the sharded path (SURVEY.md 8e): all-gather of the updated poses over an EXISTING NCCL
  * communicator, for hosts that drive libse3tn without torch.distributed (the Python layer uses
@@ -325,45 +327,42 @@ enum { SE3TN_BLUR_BILATERAL = 0, SE3TN_BLUR_GAUSSIAN = 1 };
 int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, double max_depth, int extrapolate, int blur_type,
                         uint16_t* out_mm, float* out_m, void* stream);
 
-/* Fill the observed depth inside every following track step on this context (se3tn_track_batch, _render, _host,
- * _render_host): fill_depth(frame_depth) exactly as se3tn_fill_depth_ex computes it, with the same kernels, into context-owned
- * scratch, then K0 reads the filled frame.  A live sensor's raw depth image goes straight into the step, as the reference's
- * ROS node does with fill_depth before on_track (predict_ros.py:38-41: max_depth 2.0, extrapolate 0, bilateral).
- * enable = 0 (the default) restores the plain behaviour; the other arguments are then ignored.  The caller's frame_depth is
- * never written.  The fill adds its launches to the step (8 bilateral, 6 gaussian, 3 more with extrapolate; see
- * se3tn_last_launch_count), and its setting is part of what makes two steps the same (se3tn_last_step_was_graph); no
- * profiling slot times it.  The host variants upload the whole depth frame instead of the crop-window rectangle, since the fill reads every pixel.  The scratch holds
- * 2 x H x W floats plus the filled H x W uint16 frame and grows with the frame; growing it, here or in se3tn_fill_depth[_ex],
- * drops the context's captured steps.  SE3TN_ERR_INVALID for an unknown blur_type or a max_depth that is not finite and > 0
- * (as a float); the setting is then unchanged.  A context is single-threaded: a caller that shares one between trackers
- * sets the mode it wants before each track call. */
-int se3tn_set_depth_fill(se3tn_ctx* ctx, int enable, double max_depth, int extrapolate, int blur_type);
-
-/* Refine every track k times per frame inside each following se3tn_track_render / se3tn_track_render_host step on this
- * context: the step is then exactly k successive single-round steps on the same frame (Tracker.on_track called k times,
- * each from the pose the previous call returned), in one call and one CUDA graph.  One step is the optional depth fill
- * (once per step, not per round), then k rounds of render (2 launches) -> K0 -> the 14 conv launches -> head / K6, each round
- * drawing input A and cropping B at the pose the round before wrote.  Round 0 reads poses_in; every later round reads and
- * writes poses_out in place, so poses_out == poses_in keeps working and the step's graph is replayed frame after frame.
- * out_trans / out_rot hold the last round's network outputs; se3tn_last_launch_count counts fill + k x the launches of one
- * round; profiling slots time the last round.  SE3TN_PREC_FP32 runs the rounds as plain launches.  k is part of what makes
- * two steps the same (se3tn_last_step_was_graph).  k = 1 (the default) is the single-round step.  The host variant uploads the
- * whole frame when k > 1 instead of the crop-window rectangle of the previous poses, since later rounds crop where the step
- * moved the tracks.  se3tn_track_batch and se3tn_track_host take input A from the caller and cannot redraw it: with k > 1
- * they return SE3TN_ERR_STATE and queue nothing.  k outside [1, SE3TN_MAX_REFINE_ITERATIONS] is SE3TN_ERR_INVALID and the
- * setting is unchanged.  A context is single-threaded: a caller that shares one between trackers sets the k it wants before
- * each track call.  Whether more rounds improve accuracy depends on the checkpoint; it has not been measured on trained
- * weights.  se3tn_track_render_rounds returns every round's poses from one step, and `predict --mode ycbv_recover` scores them
- * against the annotations of the YCB-Video key frames (README). */
-#define SE3TN_MAX_REFINE_ITERATIONS 8
-int se3tn_set_refine_iterations(se3tn_ctx* ctx, int k);
-
-/* Check how well every track fits its frame inside each following se3tn_track_render / _rounds / _render_host step on this
- * context: after the last round the step draws each track's model at poses_out (the same mesh, mode, camera size and object
- * width as the rounds, depth only, into scratch of its own: the step's input A keeps the last round's) and compares the
- * rendered depth R with the observed depth O in the crop window of poses_out, cropped exactly as K0 crops input B
- * (se3tn_compute_bbox's window, se3tn_crop_bbox's nearest mapping, 0 outside the image; the filled frame when the step fills
- * the depth).  R and O are uint16 mm before any clipping.  Track i's row, SE3TN_FIT_COLS int32 over its 176 x 176 pixels:
+/* Options of one tracking call (se3tn_track_batch, _render, _host, _render_host), passed by pointer; NULL means the defaults: no
+ * fill, one round, no fit check.  Every field is part of what makes two steps the same (se3tn_last_step_was_graph).  The call
+ * reads nothing of it after it returns, and the context keeps no option from one call to the next.  Refused with
+ * SE3TN_ERR_INVALID, the field named and nothing queued: a value outside the ranges below, reserved != 0, and, in
+ * se3tn_track_batch / se3tn_track_host, iterations != 1 or fit_tau_mm != 0 (they take input A from the caller: a later round
+ * cannot redraw it, and a weight id need not have a mesh for the fit check to draw).
+ *
+ * fill_depth != 0: fill the observed depth inside the step: fill_depth(frame_depth) exactly as se3tn_fill_depth_ex computes it
+ * with fill_max_depth, fill_extrapolate (0 or not) and fill_blur (SE3TN_BLUR_*), with the same kernels, into context-owned
+ * scratch, then K0 reads the filled frame.  A live sensor's raw depth image goes straight into the step, as the reference's ROS
+ * node does with fill_depth before on_track (predict_ros.py:38-41: max_depth 2.0, extrapolate 0, bilateral).  fill_depth = 0:
+ * the plain behaviour; the other fill fields are then ignored.  The caller's frame_depth is never written.  The fill adds its
+ * launches to the step (8 bilateral, 6 gaussian, 3 more with extrapolate; see se3tn_last_launch_count), and no profiling slot
+ * times it.  The host calls upload the whole depth frame instead of the crop-window rectangle, since the fill reads every pixel.
+ * The scratch holds 2 x H x W floats plus the filled H x W uint16 frame and grows with the frame; growing it, here or in
+ * se3tn_fill_depth[_ex], drops the context's captured steps.  fill_max_depth must be finite and > 0 as a float.
+ *
+ * iterations = k in [1, SE3TN_MAX_REFINE_ITERATIONS]: refine every track k times on this frame (se3tn_track_render[_host]): the
+ * step is then exactly k successive single-round steps on the same frame (Tracker.on_track called k times, each from the pose
+ * the previous call returned), in one call and one CUDA graph.  One step is the optional depth fill (once per step, not per
+ * round), then k rounds of render (2 launches) -> K0 -> the 14 conv launches -> head / K6, each round drawing input A and
+ * cropping B at the pose the round before wrote.  Round 0 reads poses_in; every later round reads and writes poses_out in place,
+ * so poses_out == poses_in keeps working and the step's graph is replayed frame after frame.  out_trans / out_rot hold the last
+ * round's network outputs; se3tn_last_launch_count counts fill + k x the launches of one round; profiling slots time the last
+ * round.  SE3TN_PREC_FP32 runs the rounds as plain launches.  k = 1 is the single-round step.  se3tn_track_render_host uploads
+ * the whole frame when k > 1 instead of the crop-window rectangle of the previous poses, since later rounds crop where the step
+ * moved the tracks.  Whether more rounds improve accuracy depends on the checkpoint; it has not been measured on trained
+ * weights.  se3tn_track_render's round_poses returns every round's poses from one step, and `predict --mode ycbv_recover`
+ * scores them against the annotations of the YCB-Video key frames (README).
+ *
+ * fit_tau_mm = tau in [1, 1000]: check how well every track fits its frame (se3tn_track_render[_host]); 0 turns the check off.
+ * After the last round the step draws each track's model at poses_out (the same mesh, mode, camera size and object width as the
+ * rounds, depth only, into scratch of its own: the step's input A keeps the last round's) and compares the rendered depth R with
+ * the observed depth O in the crop window of poses_out, cropped exactly as K0 crops input B (se3tn_compute_bbox's window,
+ * se3tn_crop_bbox's nearest mapping, 0 outside the image; the filled frame when the step fills the depth).  R and O are uint16
+ * mm before any clipping.  Track i's row, SE3TN_FIT_COLS int32 over its 176 x 176 pixels:
  *   0 model     #(R > 0)
  *   1 observed  #(R > 0, O > 0)
  *   2 inlier    #(R > 0, O > 0, |O - R| <= tau_mm)
@@ -372,24 +371,24 @@ int se3tn_set_refine_iterations(se3tn_ctx* ctx, int k);
  *   5 residual  sum of |O - R| over the inliers, mm
  * observed = inlier + front + behind.  The rows are exact integers, independent of the order of the reduction.  The fit adds
  * 3 launches (render 2, fit 1; se3tn_last_launch_count) and no profiling slot; it is captured in the step's CUDA graph
- * (SE3TN_PREC_FP32 queues it as plain launches), and tau_mm is part of what makes two steps the same.  The step's poses,
- * out_trans, out_rot and round_poses are bit for bit those of the step without it.  Device routes: the rows land in a
- * context-owned device buffer (max_batch x SE3TN_FIT_COLS int32, allocated by the first enable, never moved), whose address
- * se3tn_fit_rows gives; the next step overwrites them.  se3tn_track_render_host uploads the whole depth frame while the check
- * is on (the window of poses_out is not known before the step; rgb stays windowed) and brings the n rows back in its one copy out, into pinned
- * memory se3tn_fit_rows_host points at, valid until the next host step.  enable = 0 (the default) turns the check off;
- * tau_mm is then ignored.  tau_mm outside [1, 1000] is SE3TN_ERR_INVALID and the setting is unchanged.  While it is on,
- * se3tn_track_batch and se3tn_track_host return SE3TN_ERR_STATE and queue nothing: they take input A from the caller, and a
- * weight id need not have a mesh.  A context is single-threaded: a caller that shares one between trackers sets the check
- * it wants before each track call.  How well the rows predict tracking failure has not been measured on a trained
- * checkpoint or real data (`predict --fit --score` reports it per run, README). */
+ * (SE3TN_PREC_FP32 queues it as plain launches).  The step's poses, out_trans, out_rot and round_poses are bit for bit those of
+ * the step without it.  se3tn_track_render: the rows land in a context-owned device buffer (max_batch x SE3TN_FIT_COLS int32,
+ * allocated by the first step with the check on, never moved), whose address se3tn_fit_rows gives; the next step overwrites
+ * them.  se3tn_track_render_host uploads the whole depth frame while the check is on (the window of poses_out is not known
+ * before the step; rgb stays windowed) and brings the n rows back in its one copy out, into its out_fit.  How well the rows
+ * predict tracking failure has not been measured on a trained checkpoint or real data (`predict --fit --score` reports it per
+ * run, README). */
+#define SE3TN_MAX_REFINE_ITERATIONS 8
 #define SE3TN_FIT_COLS 6
-int se3tn_set_fit_check(se3tn_ctx* ctx, int enable, int tau_mm);
-/* *rows = the device rows of the fit check (max_batch x SE3TN_FIT_COLS int32).  SE3TN_ERR_STATE before the first enable. */
+struct se3tn_track_opts {
+    int32_t fill_depth, fill_extrapolate, fill_blur, iterations;   /* fill_blur: SE3TN_BLUR_*; iterations 1..SE3TN_MAX_REFINE_ITERATIONS */
+    double fill_max_depth;                                          /* metres; finite and > 0 as a float when fill_depth */
+    int32_t fit_tau_mm, reserved;                                   /* fit_tau_mm 0: off, else 1..1000; reserved 0 */
+};                                                                  /* 32 bytes, no padding */
+
+/* *rows = the device rows of the fit check (max_batch x SE3TN_FIT_COLS int32).  SE3TN_ERR_STATE before the first step with the
+ * check on. */
 int se3tn_fit_rows(se3tn_ctx* ctx, const int32_t** rows);
-/* *rows = the n x SE3TN_FIT_COLS rows of the last se3tn_track_render_host step, in pinned host memory.  SE3TN_ERR_STATE when
- * that step ran no fit check or failed. */
-int se3tn_fit_rows_host(se3tn_ctx* ctx, const int32_t** rows);
 
 /* The reference's own calling pattern as ONE call (Tracker.on_track, predict.py:217-296: numpy arrays in, numpy pose out):
  * every pointer is HOST memory.  The frame's crop-window rectangle, the poses, widths, input A and the ids are staged
@@ -401,7 +400,7 @@ int se3tn_fit_rows_host(se3tn_ctx* ctx, const int32_t** rows);
 int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                      const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA,
                      const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
-                     double* poses_out, float* out_trans, float* out_rot, void* stream);
+                     double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, void* stream);
 
 /* ---- tracking from the previous poses and the frame alone: input A rendered inside the step ------------------------- */
 
@@ -413,38 +412,34 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
  * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph (se3tn_last_step_was_graph);
  * SE3TN_PREC_FP32 renders and then runs its FFMA forwards without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
  * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
- * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch.  With
- * se3tn_set_refine_iterations(k > 1) the step refines every track k times on this frame. */
+ * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch.  With opts->iterations
+ * k > 1 the step refines every track k times on this frame.
+ * round_poses: NULL, or a device output double (k, n, 16), k = opts->iterations (1 without opts), where slot r - 1 receives every
+ * track's pose after round r, r = 1 .. k, bit for bit what an r-round step leaves in poses_out (slot k - 1 equals poses_out).
+ * After each round the step copies poses_out there (a device-to-device copy inside the step's CUDA graph; SE3TN_PREC_FP32 queues
+ * it between its plain launches); se3tn_last_launch_count counts kernels only, so it reads as without it.  round_poses is part
+ * of the step's key: a step with it and one without are two graphs, and both compute the same poses_out.  SE3TN_ERR_INVALID
+ * with nothing queued for a round_poses that overlaps poses_in or poses_out. */
 int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                        const double* K, const double* poses_in, const double* object_width,
                        int render_mode, int render_H, int render_W,
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double trans_normalizer, double rot_normalizer, int precision,
-                       float* out_trans, float* out_rot, double* poses_out, void* stream);
-
-/* se3tn_track_render plus one device output: round_poses double (k, n, 16), k = se3tn_set_refine_iterations' count, where slot
- * r - 1 receives every track's pose after round r, r = 1 .. k, bit for bit what an r-round step leaves in poses_out (slot k - 1
- * equals poses_out).  After each round the step copies poses_out there (a device-to-device copy inside the step's CUDA graph;
- * SE3TN_PREC_FP32 queues it between its plain launches); se3tn_last_launch_count counts kernels only, so it reads as for
- * se3tn_track_render.  round_poses is part of the step's key: a step with it and one without are two graphs, and both compute
- * the same poses_out.  Refused as se3tn_track_render refuses, and SE3TN_ERR_INVALID with nothing queued for a NULL round_poses
- * or one that overlaps poses_in or poses_out. */
-int se3tn_track_render_rounds(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                              const double* K, const double* poses_in, const double* object_width,
-                              int render_mode, int render_H, int render_W,
-                              const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                              double trans_normalizer, double rot_normalizer, int precision,
-                              float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream);
+                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                       void* stream);
 
 /* se3tn_track_render with every pointer in HOST memory, the reference's own calling pattern with rendering included: the
  * frame's crop-window rectangle, the poses, widths and ids go through se3tn_track_host's pinned staging (one copy in, one
  * copy out, stable device addresses so the step's graph is replayed); input A is rendered on the device and never crosses
  * the bus.  Synchronises `stream`.  Arguments as se3tn_track_host without rgbA / depthA, plus the render arguments of
- * se3tn_track_render; weight_ids int32 (n) or NULL (all tracks use set 0 and mesh 0).  Errors as se3tn_track_render. */
+ * se3tn_track_render; weight_ids int32 (n) or NULL (all tracks use set 0 and mesh 0).  out_fit int32 (n, SE3TN_FIT_COLS) HOST:
+ * the fit check's rows, required when opts->fit_tau_mm is set and NULL otherwise (SE3TN_ERR_INVALID, nothing queued).  Errors
+ * as se3tn_track_render. */
 int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                             const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
                             const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
-                            double* poses_out, float* out_trans, float* out_rot, void* stream);
+                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                            void* stream);
 
 /* ---- checkpoint validation: the loss of ready-made training pairs ---------------------------------------------------- */
 
@@ -636,14 +631,13 @@ int se3tn_get_profile(se3tn_ctx* ctx, float* ms);
 int se3tn_get_trace(se3tn_ctx* ctx, unsigned long long* out);
 
 /* Number of kernels the last forward / track_batch / track_render / eval_pairs / pair_loss call on this context launched (for a
- * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, se3tn_set_depth_fill,
- * and a step with the fit check its 3, se3tn_set_fit_check).
+ * replayed CUDA graph: the kernels inside it; a step that fills the depth counts the fill's launches, and a step with the fit
+ * check its 3: se3tn_track_opts).
  * se3tn_track_batch, se3tn_track_render, their _host variants and se3tn_eval_pairs capture each distinct step into a CUDA
  * graph the first time they see it and replay it afterwards -- one graph launch per step.  Two calls are the same step when
  * every value their kernels are given is the same: tracking or validation, n, precision, the frame's H and W, K, the two
  * normalizers, the first weight id and whether the ids use more than one set, the render mode and camera image size, the
- * depth-fill setting (se3tn_set_depth_fill), the refinement count and fit check of a step that renders input A
- * (se3tn_set_refine_iterations, se3tn_set_fit_check),
+ * depth fill, the refinement count and fit check of a step that renders input A (se3tn_track_opts),
  * and the address of every device array, in or out.  A replay reads what those
  * arrays hold at the time, and a call's host ids only decide the first id and the mix.  SE3TN_GRAPH=0 in the environment,
  * an enabled profiler or SE3TN_PREC_FP32 use plain stream launches.

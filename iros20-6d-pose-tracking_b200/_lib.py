@@ -41,7 +41,7 @@ SIGNATURES = {
     'se3tn_forward_preprocessed': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     'se3tn_pose_update': (_i, [_vp, _vp, _vp, _vp, _d, _d, _vp, _i, _vp]),
     'se3tn_so3_log': (_i, [_vp, _vp, _vp, _d, _d, _vp, _vp, _i, _vp]),
-    'se3tn_track_batch': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
+    'se3tn_track_batch': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_add_adi': (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_vocap': (_i, [_vp, _vp, _i, C.POINTER(_d), _vp]),
     'se3tn_add_adi_sets': (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
@@ -49,18 +49,14 @@ SIGNATURES = {
     'se3tn_vocap_sets': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     'se3tn_draw_tracks': (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     'se3tn_allgather_poses': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
-    'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
-    'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
-    'se3tn_track_render_rounds': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
-                                       _vp]),
-    'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp]),
+    'se3tn_track_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_track_render': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                                _vp]),
+    'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                                     _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
-    'se3tn_set_depth_fill': (_i, [_vp, _i, _d, _i, _i]),
-    'se3tn_set_refine_iterations': (_i, [_vp, _i]),
-    'se3tn_set_fit_check': (_i, [_vp, _i, _i]),
     'se3tn_fit_rows': (_i, [_vp, C.POINTER(_vp)]),
-    'se3tn_fit_rows_host': (_i, [_vp, C.POINTER(_vp)]),
     'se3tn_set_mesh': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i]),
     'se3tn_render': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'se3tn_render_ex': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
@@ -94,6 +90,12 @@ class Augment(C.Structure):
                 ('gaussian_blur', C.c_int32), ('black_cover', C.c_int32), ('depth_missing', C.c_int32), ('hsv_prob', _d),
                 ('hsv_noise', _d * 3), ('bright_mag', _d * 2), ('noise_prob', _d), ('noise_rgb', _d), ('noise_depth', _d),
                 ('blur_prob', _d), ('blur_max_kernel', C.c_int32), ('reserved', C.c_int32), ('cover_prob', _d)]
+
+
+class TrackOpts(C.Structure):
+    """se3tn_track_opts (include/se3tn.h)."""
+    _fields_ = [('fill_depth', C.c_int32), ('fill_extrapolate', C.c_int32), ('fill_blur', C.c_int32), ('iterations', C.c_int32),
+                ('fill_max_depth', _d), ('fit_tau_mm', C.c_int32), ('reserved', C.c_int32)]
 
 
 _lib = None

@@ -11,7 +11,7 @@
 // accumulation whose order OpenCV's SIMD code does not expose, so the final metres agree to ~5e-7 and the uint16 millimetres
 // to +-1 on the rare pixel that sits on a truncation boundary (tests state both tolerances).
 // One thread per pixel, seven small launches per frame (1.2 MB images, L2 resident); latency matters here, not bandwidth.
-// Every kernel executes griddepcontrol.launch_dependents at entry: inside a track step that fills the frame (se3tn_set_depth_fill)
+// Every kernel executes griddepcontrol.launch_dependents at entry: inside a track step that fills the frame (se3tn_track_opts)
 // the next launch is preprocess_kernel, launched with programmatic dependent launch, which then becomes resident under the
 // last fill kernel's tail and reads the filled frame only after its griddepcontrol.wait.  No fill kernel is itself launched
 // with that attribute, so each one starts after the previous launch in the stream has completed.

@@ -1,4 +1,4 @@
-// The fit check of a track step (se3tn_set_fit_check): after the last round, every track's model is drawn at its new pose
+// The fit check of a track step (se3tn_track_opts): after the last round, every track's model is drawn at its new pose
 // (render_kernel, depth only) and compared pixel by pixel with the observed depth in the crop window of that pose -- the
 // window K0 would crop input B from in the next frame's step: bbox_window (bbox.cuh) and cv2's nearest source index
 // floor(dst * (1 / (176 / size))), clamped, 0 outside the frame.  R is the rendered depth, O the raw observed uint16 mm (the

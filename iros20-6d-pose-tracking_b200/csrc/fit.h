@@ -3,7 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 namespace se3tn {
-constexpr int kFitCols = 6;              // model, observed, inlier, front, behind, residual (include/se3tn.h, se3tn_set_fit_check)
+constexpr int kFitCols = 6;              // model, observed, inlier, front, behind, residual (include/se3tn.h, se3tn_track_opts)
 struct FitArgs {
     const double* poses;                 // [n][16] the step's poses_out
     const double* object_width;          // [n] mm

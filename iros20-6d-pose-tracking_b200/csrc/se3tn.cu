@@ -219,11 +219,11 @@ struct AugKey {
 };
 struct StepKey {
     uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
-    uint8_t fill, fill_extrapolate;            // c->depth_fill when a track step is built (zero in a validation step)
-    uint16_t fill_blur, iterations;            // iterations: c->refine_iterations in a track step (zero in a validation step)
+    uint8_t fill, fill_extrapolate;            // track step: its se3tn_track_opts fill, all zero when off (zero in a validation step)
+    uint16_t fill_blur, iterations;            // iterations: the track step's rounds, 1 without opts (zero in a validation step)
     int32_t n, precision, first_wid;           // first_wid: the first track's weight set
     int32_t H, W, render_mode, render_H, render_W;   // the frame; input A drawn in the step (SE3TN_RENDER_*, camera size) or -1, 0, 0
-    int32_t fit_tau, fit_pad;                  // track step that renders input A: c->fit_tau (0: no fit check); fit_pad is always 0
+    int32_t fit_tau, fit_pad;                  // track step that renders input A: opts->fit_tau_mm (0: no fit check); fit_pad is always 0
     F64Bits K[4], tn, rn, fill_max_depth;
     AugKey aug;                                // validation step: the augmentation of input B (aug.stages 0: none)
     const uint8_t* aug_seg; const int64_t* pair_index; uint8_t* aug_rgb; uint16_t* aug_depth;   // its maskB (NULL: depthB > 100), keys, output
@@ -234,7 +234,7 @@ struct StepKey {
     float* out_trans; float* out_rot; double* poses_out;                                  // poses_out: track step
     float* sq; double* labels; float* sums;                                               // validation step
     const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
-    double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render_rounds) or NULL
+    double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render) or NULL
     int32_t* fit_rows;                         // fit_tau > 0: the rows of the fit check, n x kFitCols
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
@@ -266,14 +266,9 @@ struct se3tn_ctx {
     DevBuf<unsigned> append_done; int append_done_words = 0;   // se3tn_append_pairs' CTA counter, zero between launches (allocated on first use)
     DevBuf<uint8_t> metrics; size_t metrics_bytes = 0;   // se3tn_add_adi_sets' staged offsets and ids, or se3tn_vocap_sets' scratch (grows on demand)
     DevBuf<uint8_t> fill; size_t fill_bytes = 0;   // depth hole-filling scratch a | b | lut | minmax in one block, then the filled frame of a track step that fills, so all exist or none (grows on demand)
-    // se3tn_set_depth_fill: every track step runs fill_depth(frame_depth) into the fill block and K0 reads the filled frame
-    struct DepthFill { bool on = false; double max_depth = 0.0; int extrapolate = 0, blur_type = SE3TN_BLUR_BILATERAL; } depth_fill;
-    int refine_iterations = 1;       // se3tn_set_refine_iterations: render -> network -> pose update rounds of a track step that renders input A
-    // se3tn_set_fit_check: tau in mm, 0 off.  The block holds the device route's rows (max_batch x kFitCols int32), then the fit's
-    // rendered depth for max_batch tracks; allocated by the first enable, never moved after (captured steps hold both addresses)
-    int fit_tau = 0;
+    // the fit check's block: the device route's rows (max_batch x kFitCols int32), then the fit's rendered depth for max_batch
+    // tracks; allocated by the first step with the check on, never moved after (captured steps hold both addresses)
     DevBuf<uint8_t> fit; size_t fit_bytes = 0;
-    const int32_t* fit_rows_host = nullptr;   // the last fitting host step's rows, inside hio.pin (se3tn_fit_rows_host)
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -295,7 +290,7 @@ struct se3tn_ctx {
     // state whose every change drops these graphs (or that is fixed for the context's life: workspace, scheduler, activation
     // tensor maps): the weight sets and their device tables (se3tn_load_weights), the statistics (se3tn_set_stats), the meshes
     // and rasteriser workspace (se3tn_set_mesh), the depth-fill block (reserve_fill) and the host-IO buffers (track_host_step).
-    // The fit check's block never moves once allocated (se3tn_set_fit_check).
+    // The fit check's block never moves once allocated (render_into_scratch).
     int use_graphs = 1;              // SE3TN_GRAPH=0: plain stream launches; set to 0 at run time if capture is not possible
     bool last_was_graph = false;
     struct StepGraph { StepKey key; Handle<cudaGraphExec_t> exec; int launches; unsigned long long last_use; };
@@ -1206,47 +1201,66 @@ uint16_t* filled_frame(se3tn_ctx* c, int H, int W) { return reinterpret_cast<uin
 // and the fp32 mode's runs of equal ids, which are never captured.
 struct Step : StepKey { const int32_t* wid_host; };
 
-// What every track step takes from its scalar arguments, its ids (checked by check_step: `mixed`) and the context's depth-fill
-// setting; the caller adds the device pointers.
-Step track_step(const se3tn_ctx* c, int H, int W, const double* K, const int32_t* wid_host, bool mixed, int n,
-                double tn, double rn, int precision) {
-    Step st{};
+// A tracking call's se3tn_track_opts (NULL: the defaults) checked and written into its step: the fill, the rounds and the fit
+// check, so the key holds them.  renders: the step draws input A.  se3tn_track_batch / se3tn_track_host take input A from the
+// caller: a later round could not redraw it at the refined pose, and the fit check could not draw a model the weight id need
+// not have.  Refused before anything is queued.
+static_assert(sizeof(se3tn_track_opts) == 32, "se3tn_track_opts is 32 bytes without padding: _lib.TrackOpts mirrors it");
+int track_opts(se3tn_ctx* c, const char* fn, const se3tn_track_opts* o, bool renders, Step& st) {
+    st.iterations = 1;
+    if (!o) return SE3TN_OK;
+    const std::string f(fn);
+    if (o->fill_depth) {                           // off: the fill fields stay zero, whatever the caller left in them
+        if (o->fill_blur != SE3TN_BLUR_BILATERAL && o->fill_blur != SE3TN_BLUR_GAUSSIAN)
+            return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_blur is " + std::to_string(o->fill_blur) + ", not an SE3TN_BLUR_*");
+        const float md = static_cast<float>(o->fill_max_depth);   // what the kernels compute with
+        if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_max_depth must be finite and > 0");
+        st.fill = 1; st.fill_max_depth = o->fill_max_depth; st.fill_extrapolate = o->fill_extrapolate != 0;
+        st.fill_blur = static_cast<uint16_t>(o->fill_blur);
+    }
+    if (o->iterations < 1 || o->iterations > SE3TN_MAX_REFINE_ITERATIONS)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
+    if (o->fit_tau_mm < 0 || o->fit_tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be 0 or in [1, 1000]");
+    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
+    if (!renders && o->iterations != 1)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations is " + std::to_string(o->iterations) + "; input A from the caller "
+                    "cannot be redrawn, which needs se3tn_track_render[_host]");
+    if (!renders && o->fit_tau_mm)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm is set; input A from the caller, and the fit check draws each "
+                    "track's model, which needs se3tn_track_render[_host]");
+    st.iterations = static_cast<uint16_t>(o->iterations);
+    st.fit_tau = o->fit_tau_mm;
+    return SE3TN_OK;
+}
+
+// What every track step takes from its scalar arguments and its ids (checked by check_step: `mixed`), added to what track_opts
+// wrote; the caller adds the device pointers.
+void track_step(Step& st, int H, int W, const double* K, const int32_t* wid_host, bool mixed, int n, double tn, double rn, int precision) {
     st.n = n; st.precision = precision; st.H = H; st.W = W;
     for (int i = 0; i < 4; ++i) st.K[i] = K[i];
     st.tn = tn; st.rn = rn;
     st.wid_host = wid_host; st.first_wid = wid_host ? wid_host[0] : 0; st.mixed = mixed;
     st.render_mode = -1;
-    const auto& f = c->depth_fill;                 // all zero when the fill is off (se3tn_set_depth_fill)
-    st.fill = f.on; st.fill_max_depth = f.max_depth; st.fill_extrapolate = f.extrapolate != 0; st.fill_blur = static_cast<uint16_t>(f.blur_type);
-    st.iterations = static_cast<uint16_t>(c->refine_iterations);
-    return st;
 }
 
-// se3tn_track_batch / se3tn_track_host take input A from the caller: a later round could not redraw it at the refined pose,
-// and the fit check could not draw a model the weight id need not have.
-int check_single_round(se3tn_ctx* c, const char* fn) {
-    if (c->fit_tau)
-        return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": input A from the caller; the fit check (se3tn_set_fit_check) draws "
-                    "each track's model and needs se3tn_track_render[_host]");
-    if (c->refine_iterations == 1) return SE3TN_OK;
-    return fail(c, SE3TN_ERR_STATE, std::string(fn) + ": input A from the caller cannot be redrawn; refine iterations is " +
-                std::to_string(c->refine_iterations) + " (se3tn_set_refine_iterations), which needs se3tn_track_render[_host]");
-}
-
-// The fit check's block (se3tn_set_fit_check): the device route's rows, then the fit's rendered depth of max_batch tracks.
+// The fit check's block: the device route's rows, then the fit's rendered depth of max_batch tracks.
 size_t fit_rows_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kFitCols * sizeof(int32_t)); }
 int32_t* fit_rows(se3tn_ctx* c) { return reinterpret_cast<int32_t*>(c->fit.get()); }
 uint16_t* fit_depth(se3tn_ctx* c) { return reinterpret_cast<uint16_t*>(c->fit.get() + fit_rows_bytes(c->max_batch)); }
 
 // A track step that draws input A first.  It lands in context scratch for max_batch tracks, allocated by the first such step:
 // its address never changes after, so captured steps stay valid.  With the fit check on, the step also runs the fit into the
-// context's rows (the host route points them at its own output block).
+// context's rows (the host route points them at its own output block); their block is allocated the same way, by the first step
+// with the check on.
 int render_into_scratch(se3tn_ctx* c, const RenderSpec& r, Step& st) {
     const size_t img = static_cast<size_t>(kImg) * kImg, rgb_bytes = align256(static_cast<size_t>(c->max_batch) * img * 3);
     CU_TRY(c, grow(c->in_a, c->in_a_bytes, rgb_bytes + static_cast<size_t>(c->max_batch) * img * 2));
     st.render_mode = r.mode; st.render_H = r.H; st.render_W = r.W;
     st.rgbA = c->in_a.get(); st.depthA = reinterpret_cast<uint16_t*>(c->in_a.get() + rgb_bytes);
-    if (c->fit_tau) { st.fit_tau = c->fit_tau; st.fit_rows = fit_rows(c); }
+    if (st.fit_tau) {
+        CU_TRY(c, grow(c->fit, c->fit_bytes, fit_rows_bytes(c->max_batch) + static_cast<size_t>(c->max_batch) * img * sizeof(uint16_t)));
+        st.fit_rows = fit_rows(c);
+    }
     return SE3TN_OK;
 }
 
@@ -1529,41 +1543,6 @@ int eval_pairs_step(se3tn_ctx* c, const char* fn, const uint8_t* rgbA, const uin
     return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
-// se3tn_track_render, and with round_poses (k x n x 16 doubles, k = c->refine_iterations) se3tn_track_render_rounds.
-int track_render_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                      const double* K, const double* poses_in, const double* object_width, int render_mode, int render_H, int render_W,
-                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, double tn, double rn, int precision,
-                      float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream) {
-    const std::string f(fn);
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
-    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
-    RenderSpec r;
-    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    bool multi = false;
-    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
-    if (rc) return rc;
-    if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
-    if (round_poses) {                             // the copies must not write the poses a later round reads
-        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
-        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * c->refine_iterations;
-        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
-            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
-            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
-        }
-    }
-    DeviceGuard guard(c->device);
-    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
-    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
-    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
-    st.round_poses = round_poses;
-    if ((rc = render_into_scratch(c, r, st))) return rc;
-    return run_step(c, st, static_cast<cudaStream_t>(stream));
-}
-
 }  // namespace
 
 extern "C" {
@@ -1573,11 +1552,12 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
                       const uint8_t* rgbA, const uint16_t* depthA,
                       const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                       double tn, double rn, int precision,
-                      float* out_trans, float* out_rot, double* poses_out, void* stream) {
+                      float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
     bool multi = false;
-    int rc = check_single_round(c, "se3tn_track_batch");
+    Step st{};
+    int rc = track_opts(c, "se3tn_track_batch", opts, false, st);
     if (rc) return rc;
     rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
@@ -1586,7 +1566,7 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null argument or empty frame");
     if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: unknown precision");
     DeviceGuard guard(c->device);
-    Step st = track_step(c, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
     st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
     st.rgbA = rgbA; st.depthA = depthA; st.wid_dev = weight_ids_dev;
     st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
@@ -1598,22 +1578,39 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
                        int render_mode, int render_H, int render_W,
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double tn, double rn, int precision,
-                       float* out_trans, float* out_rot, double* poses_out, void* stream) {
-    return track_render_step(c, "se3tn_track_render", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
-                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, nullptr, stream);
-}
-
-int se3tn_track_render_rounds(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                              const double* K, const double* poses_in, const double* object_width,
-                              int render_mode, int render_H, int render_W,
-                              const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                              double tn, double rn, int precision,
-                              float* out_trans, float* out_rot, double* poses_out, double* round_poses, void* stream) {
+                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                       void* stream) {
+    const char* fn = "se3tn_track_render";
+    const std::string f(fn);
     if (!c) return SE3TN_ERR_INVALID;
-    if (!round_poses) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render_rounds: null round_poses");
-    return track_render_step(c, "se3tn_track_render_rounds", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode,
-                             render_H, render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out,
-                             round_poses, stream);
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    Step st{};
+    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
+    bool multi = false;
+    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
+    if (round_poses) {                             // the copies must not write the poses a later round reads
+        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
+        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * st.iterations;
+        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
+            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
+            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
+        }
+    }
+    DeviceGuard guard(c->device);
+    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    st.round_poses = round_poses;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
 int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
@@ -2009,10 +2006,14 @@ inline void host_crop_window(const double* pose, const double* K, double width, 
 int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                    double* poses_out, float* out_trans, float* out_rot, void* stream) {
-    c->fit_rows_host = nullptr;                    // the pinned block may move below
+                    double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit, void* stream) {
     bool multi = false;
-    int rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);   // before anything is staged or copied
+    Step st{};                                     // options and ids are checked before anything is staged or copied
+    int rc = track_opts(c, fn, opts, render != nullptr, st);
+    if (rc) return rc;
+    if (!st.fit_tau != !out_fit)
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": out_fit is required with opts->fit_tau_mm and must be NULL without it");
+    rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
     if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": unknown precision");
@@ -2040,7 +2041,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * a_img * 3),
                  o_wid = o_depthA + align256(nn * a_img * 2), in_bytes = o_wid + align256(nn * 4);
     const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), o_fit = o_ro + align256(nn * 12);
-    const size_t out_bytes = c->fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
+    const size_t out_bytes = st.fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
     double* d_ow = reinterpret_cast<double*>(d_in + o_ow);
@@ -2063,13 +2064,13 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     }
     if (y1 <= y0 || x1 <= x0) { y0 = y1 = x0 = x1 = 0; }         // every window misses the frame: nothing of it is read
     // refinement rounds after the first crop at poses only the step computes: their windows are not known here
-    const bool whole_frame = c->refine_iterations > 1;
+    const bool whole_frame = st.iterations > 1;
     if (whole_frame || static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
     // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
     // median-filtered image, and extrapolate scans whole columns.  The fit check crops the depth at the windows of the poses the
     // step computes.  Then the whole depth frame goes up; rgb stays windowed.
-    const bool whole_depth = c->depth_fill.on || c->fit_tau;
+    const bool whole_depth = st.fill || st.fit_tau;
     uint8_t* hp = io.pin.get();
     const int wh = y1 - y0, ww = x1 - x0;
     if (wh > 0 && ww > 0) {
@@ -2099,7 +2100,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (weight_ids) memcpy(hp + o_wid, weight_ids, nn * 4);
     CU_TRY(c, cudaMemcpyAsync(d_in, hp, weight_ids ? in_bytes : o_wid, cudaMemcpyHostToDevice, s));
     hp += in_bytes;
-    Step st = track_step(c, H, W, K, weight_ids, multi, n, tn, rn, precision);
+    track_step(st, H, W, K, weight_ids, multi, n, tn, rn, precision);
     st.frame_rgb = d_rgb; st.frame_depth = d_depth; st.poses_in = d_poses; st.object_width = d_ow;
     st.rgbA = d_rgbA; st.depthA = d_depthA; st.wid_dev = weight_ids ? d_wid : nullptr;
     st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
@@ -2109,10 +2110,10 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
     CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
-    if (st.fit_tau) c->fit_rows_host = reinterpret_cast<const int32_t*>(ho + o_fit);
     memcpy(poses_out, ho, nn * 128);
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
+    if (out_fit) memcpy(out_fit, ho + o_fit, nn * 4 * kFitCols);
     return SE3TN_OK;
 }
 }  // namespace
@@ -2120,20 +2121,19 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
 int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                      const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA,
                      const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                     double* poses_out, float* out_trans, float* out_rot, void* stream) {
+                     double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !rgbA || !depthA || !poses_out || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_host: null argument or empty frame");
-    const int rc = check_single_round(c, "se3tn_track_host");
-    if (rc) return rc;
     return track_host_step(c, "se3tn_track_host", frame_rgb, frame_depth, H, W, K, poses, object_width, rgbA, depthA, nullptr,
-                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, stream);
+                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, nullptr, stream);
 }
 
 int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                             const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
                             const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                            double* poses_out, float* out_trans, float* out_rot, void* stream) {
+                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                            void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render_host: null argument or empty frame");
@@ -2141,7 +2141,7 @@ int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16
     const int rc = render_spec(c, "se3tn_track_render_host", render_mode, render_H, render_W, r);
     if (rc) return rc;
     return track_host_step(c, "se3tn_track_render_host", frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r,
-                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, stream);
+                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, out_fit, stream);
 }
 
 int se3tn_allgather_poses(se3tn_ctx* c, void* nccl_comm, const double* local_poses, double* all_poses, int n_local, void* stream) {
@@ -2184,49 +2184,11 @@ int se3tn_fill_depth(se3tn_ctx* c, const uint16_t* depth_mm, int H, int W, doubl
     return se3tn_fill_depth_ex(c, depth_mm, H, W, max_depth, 0, SE3TN_BLUR_BILATERAL, out_mm, out_m, stream);
 }
 
-int se3tn_set_depth_fill(se3tn_ctx* c, int enable, double max_depth, int extrapolate, int blur_type) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!enable) { c->depth_fill = {}; return SE3TN_OK; }
-    if (blur_type != SE3TN_BLUR_BILATERAL && blur_type != SE3TN_BLUR_GAUSSIAN) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_depth_fill: unknown blur_type");
-    const float md = static_cast<float>(max_depth);                // what the kernels compute with
-    if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_depth_fill: max_depth must be finite and > 0");
-    c->depth_fill = {true, max_depth, extrapolate != 0 ? 1 : 0, blur_type};
-    return SE3TN_OK;
-}
-
-int se3tn_set_refine_iterations(se3tn_ctx* c, int k) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (k < 1 || k > SE3TN_MAX_REFINE_ITERATIONS)
-        return fail(c, SE3TN_ERR_INVALID, "se3tn_set_refine_iterations: k must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
-    c->refine_iterations = k;
-    return SE3TN_OK;
-}
-
-int se3tn_set_fit_check(se3tn_ctx* c, int enable, int tau_mm) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!enable) { c->fit_tau = 0; return SE3TN_OK; }
-    if (tau_mm < 1 || tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, "se3tn_set_fit_check: tau_mm must be in [1, 1000]");
-    if (!c->fit) {                                 // once, at its full size: steps captured after keep its addresses
-        DeviceGuard guard(c->device);
-        CU_TRY(c, grow(c->fit, c->fit_bytes, fit_rows_bytes(c->max_batch) + static_cast<size_t>(c->max_batch) * kImg * kImg * sizeof(uint16_t)));
-    }
-    c->fit_tau = tau_mm;
-    return SE3TN_OK;
-}
-
 int se3tn_fit_rows(se3tn_ctx* c, const int32_t** rows) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!rows) return fail(c, SE3TN_ERR_INVALID, "se3tn_fit_rows: null argument");
-    if (!c->fit) return fail(c, SE3TN_ERR_STATE, "se3tn_fit_rows: the fit check was never enabled (se3tn_set_fit_check)");
+    if (!c->fit) return fail(c, SE3TN_ERR_STATE, "se3tn_fit_rows: no step has run the fit check yet");
     *rows = fit_rows(c);
-    return SE3TN_OK;
-}
-
-int se3tn_fit_rows_host(se3tn_ctx* c, const int32_t** rows) {
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!rows) return fail(c, SE3TN_ERR_INVALID, "se3tn_fit_rows_host: null argument");
-    if (!c->fit_rows_host) return fail(c, SE3TN_ERR_STATE, "se3tn_fit_rows_host: the last host step ran no fit check");
-    *rows = c->fit_rows_host;
     return SE3TN_OK;
 }
 

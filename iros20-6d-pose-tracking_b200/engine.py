@@ -280,12 +280,12 @@ class Engine:
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
         out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h).  iterations: k rounds
         of render -> network -> pose update on this frame in the one step, exactly what k chained calls with iterations=1
-        compute (se3tn_set_refine_iterations, 1..8); out_trans / out_rot hold the last round's outputs.  out_rounds: a float64
-        CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_render_rounds): entry r - 1 is
-        what a call with iterations=r returns.  The step with it is a CUDA graph of its own.  fit: tau in mm (fit_spec) turns
-        on the fit check of the step (se3tn_set_fit_check): every track's model is drawn at its new pose and compared with the
-        observed depth, and the call returns a fourth value, out_fit: an int32 CUDA tensor (n, 6) of the rows (model, observed,
-        inlier, front, behind, residual), allocated when None and filled on the current stream."""
+        compute (se3tn_track_opts.iterations, 1..8); out_trans / out_rot hold the last round's outputs.  out_rounds: a float64
+        CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_render's round_poses): entry
+        r - 1 is what a call with iterations=r returns.  The step with it is a CUDA graph of its own.  fit: tau in mm (fit_spec)
+        turns on the fit check of the step (se3tn_track_opts.fit_tau_mm): every track's model is drawn at its new pose and
+        compared with the observed depth, and the call returns a fourth value, out_fit: an int32 CUDA tensor (n, 6) of the rows
+        (model, observed, inlier, front, behind, residual), allocated when None and filled on the current stream."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
                            fill_depth, iterations, out_rounds, fit, out_fit)
@@ -311,19 +311,14 @@ class Engine:
         if tau:
             out_fit = torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=self.device) if out_fit is None else out_fit
             self._check_dev('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS))
-        self._set_depth_fill(fill)
-        self._set_refine(iterations)
-        self._set_fit(tau)
         H, W = frame_depth.shape
         head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
         tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
-                _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), _stream(self.device))
+                _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), self._track_opts(fill, iterations, tau))
         if render is None:
-            rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail)
-        elif out_rounds is not None:
-            rc = self.lib.se3tn_track_render_rounds(*head, *render, *tail[:-1], _ptr(out_rounds), tail[-1])
+            rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail, _stream(self.device))
         else:
-            rc = self.lib.se3tn_track_render(*head, *render, *tail)
+            rc = self.lib.se3tn_track_render(*head, *render, *tail, _ptr(out_rounds), _stream(self.device))
         _lib.check(rc, self._ctx)
         if not tau:
             return out_poses, out_trans, out_rot
@@ -366,23 +361,19 @@ class Engine:
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
-        self._set_depth_fill(fill)
-        self._set_refine(iterations)
-        self._set_fit(tau)
+        fit_rows = np.empty((n, _lib.FIT_COLS), dtype=np.int32) if tau else None
         H, W = frame_depth.shape
         head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
         tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
-                _stream(self.device))
+                self._track_opts(fill, iterations, tau))
         if render is None:
-            rc = self.lib.se3tn_track_host(*head, *map(_hptr, A), *tail)
+            rc = self.lib.se3tn_track_host(*head, *map(_hptr, A), *tail, _stream(self.device))
         else:
-            rc = self.lib.se3tn_track_render_host(*head, *render, *tail)
+            rc = self.lib.se3tn_track_render_host(*head, *render, *tail, _hptr(fit_rows), _stream(self.device))
         _lib.check(rc, self._ctx)
         res = (out, tr, ro) if want_residuals else (out,)
         if tau:
-            p = C.c_void_p()
-            _lib.check(self.lib.se3tn_fit_rows_host(self._ctx, C.byref(p)), self._ctx)
-            res += (np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int32)), shape=(n, _lib.FIT_COLS)).copy(),)
+            res += (fit_rows,)
         return res if len(res) > 1 else out
 
     # ------------------------------------------------------------------ checkpoint validation
@@ -794,7 +785,7 @@ class Engine:
 
     @staticmethod
     def depth_fill_spec(fill_depth):
-        """(enable, max_depth, extrapolate, blur_type) for se3tn_set_depth_fill from the tracking calls' fill_depth argument:
+        """(enable, max_depth, extrapolate, blur_type), se3tn_track_opts' fill, from the tracking calls' fill_depth argument:
         None / False: the frame's depth is used as it is.  True: fill_depth as the reference's ROS node calls it before every
         on_track (predict_ros.py:38-41: max_depth 2.0 m, no extrapolation, bilateral).  A dict with any of max_depth /
         extrapolate / blur_type: those arguments of fill_depth, the rest as with True."""
@@ -810,25 +801,17 @@ class Engine:
             raise ValueError('max_depth must be finite and > 0')
         return (1, max_depth, int(bool(fill_depth.get('extrapolate', False))), 1 if blur_type == 'gaussian' else 0)
 
-    def _set_depth_fill(self, spec):
-        """Every tracking call sets the context's fill mode it wants: Trackers that share an Engine keep their own."""
-        _lib.check(self.lib.se3tn_set_depth_fill(self._ctx, int(spec[0]), float(spec[1]), int(spec[2]), int(spec[3])), self._ctx)
-
     @staticmethod
     def refine_iterations(k):
-        """The refinement count of a tracking call as an int: 1..MAX_REFINE_ITERATIONS (se3tn_set_refine_iterations), else a
+        """The refinement count of a tracking call as an int: 1..MAX_REFINE_ITERATIONS (se3tn_track_opts.iterations), else a
         ValueError."""
         if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 1 <= k <= _lib.MAX_REFINE_ITERATIONS:
             raise ValueError('iterations must be an integer in [1, %d], not %r' % (_lib.MAX_REFINE_ITERATIONS, k))
         return int(k)
 
-    def _set_refine(self, k):
-        """Every tracking call sets the refinement count it wants, as it sets the fill mode: track_batch / track_host set 1."""
-        _lib.check(self.lib.se3tn_set_refine_iterations(self._ctx, int(k)), self._ctx)
-
     @staticmethod
     def fit_spec(fit):
-        """The fit check of a tracking call as se3tn_set_fit_check's tau in mm: None -> 0 (off), an integer in [1, 1000] -> itself,
+        """The fit check of a tracking call as se3tn_track_opts' fit_tau_mm: None -> 0 (off), an integer in [1, 1000] -> itself,
         else a ValueError."""
         if fit is None:
             return 0
@@ -836,9 +819,13 @@ class Engine:
             raise ValueError('fit must be None or an integer tau in mm in [1, 1000], not %r' % (fit,))
         return int(fit)
 
-    def _set_fit(self, tau):
-        """Every tracking call sets the fit check it wants, as it sets the fill mode: track_batch / track_host turn it off."""
-        _lib.check(self.lib.se3tn_set_fit_check(self._ctx, int(tau > 0), int(tau) if tau else 1), self._ctx)
+    @staticmethod
+    def _track_opts(fill, iterations, tau):
+        """The se3tn_track_opts of one tracking call, by reference: depth_fill_spec's tuple, the refinement count and the fit
+        check's tau.  Every call passes all of them, so Trackers that share an Engine each get their own."""
+        on, max_depth, extrapolate, blur = fill
+        return C.byref(_lib.TrackOpts(fill_depth=on, fill_extrapolate=extrapolate, fill_blur=blur, iterations=iterations,
+                                      fill_max_depth=max_depth, fit_tau_mm=tau))
 
     def _fit_rows_view(self):
         """An int32 CUDA tensor (max_batch, 6) over the context's fit rows (se3tn_fit_rows; the address never changes)."""

@@ -1767,7 +1767,7 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
     class_config['pair_model_path'] (default model_path with .ply -> .obj, pair_model_template) under mesh ids pair_mesh_base(...)
     + class id; the tracks draw model_path under their weight ids.
 
-    Each frame's rows (the samples inside the image, classes in order) are n tracks of one se3tn_track_render_rounds step per
+    Each frame's rows (the samples inside the image, classes in order) are n tracks of one se3tn_track_render step (round_poses) per
     variant, started at their A_in_cam on the ring's device frame, with their class's weight set, statistics, mesh and
     Tracker.object_width, refined K times; a row whose segB count is below 100 (the writer drops it) is tracked but not scored:
     the counts stay on the device as the keep mask of se3tn_pose_errors_sets.  After the last frame every round r = 0 (the start)

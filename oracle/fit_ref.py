@@ -1,4 +1,4 @@
-"""The fit check's rows (se3tn_set_fit_check, include/se3tn.h) restated in numpy.
+"""The fit check's rows (se3tn_track_opts.fit_tau_mm, include/se3tn.h) restated in numpy.
 
 R: rendered depth of the model at the step's new pose, O: observed depth cropped at that pose's window (crop_bbox of the frame,
 or of the filled frame), both uint16 mm of shape (..., 176, 176); tau: integer mm.  Per image, over the pixels with R > 0:

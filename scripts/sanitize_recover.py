@@ -1,5 +1,5 @@
 """One pose-recovery step with the round output and one se3tn_pose_errors_sets call with a keep mask, for compute-sanitizer
-(memcheck / racecheck): k = 3 rounds recorded by se3tn_track_render_rounds in a graph (bf16x3) and as plain launches (fp32).
+(memcheck / racecheck): k = 3 rounds recorded by se3tn_track_render's round_poses in a graph (bf16x3) and as plain launches (fp32).
 
     compute-sanitizer --tool memcheck python scripts/sanitize_recover.py
 """

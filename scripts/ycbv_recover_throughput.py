@@ -1,7 +1,7 @@
 """Pose recovery on perturbed YCB-Video key frames (predict.recoverYcbKeyframes), on the synthetic layout of
 perturbed_validate_throughput.build_layout (480 x 640 key frames, its classes, one checkpoint each):
 
-  * rounds in one step: one pass at K = 4, every frame one se3tn_track_render_rounds step that records rounds 1..4;
+  * rounds in one step: one pass at K = 4, every frame one se3tn_track_render step that records rounds 1..4;
   * separate steps: the passes at K = 1, 2, 3 and 4, the 1 + 2 + 3 + 4 = 10 rounds per frame a sweep of K costs without the
     round output.
 

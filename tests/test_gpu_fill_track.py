@@ -1,4 +1,4 @@
-"""Raw sensor depth in, hole-filled inside the tracking step (se3tn_set_depth_fill, Engine track calls' fill_depth=,
+"""Raw sensor depth in, hole-filled inside the tracking step (se3tn_track_opts' fill, Engine track calls' fill_depth=,
 Tracker(fill_depth=)): every step must give the same bits as Engine.fill_depth on the whole frame followed by the same entry
 point with the fill off, whatever the graph cache, the upload window or a Tracker sharing the Engine did before."""
 import ctypes as C
@@ -251,12 +251,12 @@ def test_raw_depth_is_not_written(synth, eng):
         assert torch.equal(c.D, keep_t) and np.array_equal(c.depth, keep_a), entry
 
 
-def _raw_track_batch(e, c, outs):
+def _raw_track_batch(e, c, outs, opts=None):
     K4 = e._k4(K)
     vp = lambda t: C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
     return e.lib.se3tn_track_batch(e._ctx, vp(c.R), vp(c.D), 480, 640, K4.ctypes.data_as(C.c_void_p), vp(c.P), vp(c.ow), vp(c.ra), vp(c.da),
                                    C.c_void_p(0), C.c_void_p(0), c.n, TN, RN, 2, vp(outs[1]), vp(outs[2]), vp(outs[0]),
-                                   C.c_void_p(torch.cuda.current_stream(e.device).cuda_stream))
+                                   None if opts is None else C.byref(opts), C.c_void_p(torch.cuda.current_stream(e.device).cuda_stream))
 
 
 def test_errors_and_fill_off(pkg, synth, eng):
@@ -276,14 +276,22 @@ def test_errors_and_fill_off(pkg, synth, eng):
         assert eng.last_launch_count() == before and all(torch.isnan(x).all() for x in o), b
         with pytest.raises(ValueError):
             pkg.Tracker({}, None, None, None, fill_depth=b)
-    # ... and in C, where a rejected call leaves the setting as it was
-    assert lib.OK == eng.lib.se3tn_set_depth_fill(eng._ctx, 1, 2.0, 0, 0)
-    for args in ((1, 2.0, 0, 7), (1, 0.0, 0, 0), (1, -1.0, 0, 0), (1, float('nan'), 0, 0), (1, float('inf'), 0, 1), (1, 1e300, 1, 0)):
-        assert eng.lib.se3tn_set_depth_fill(eng._ctx, *args) == lib.ERR_INVALID, args
+    # ... and in C, where a rejected call launches nothing, writes nothing and names the field
+    before = eng.last_launch_count()
+    for (max_depth, extrapolate, blur), field in (((2.0, 0, 7), b'fill_blur'), ((0.0, 0, 0), b'fill_max_depth'),
+                                                  ((-1.0, 0, 0), b'fill_max_depth'), ((float('nan'), 0, 0), b'fill_max_depth'),
+                                                  ((float('inf'), 0, 1), b'fill_max_depth'), ((1e300, 1, 0), b'fill_max_depth')):
+        o = nan_outs()
+        opts = lib.TrackOpts(fill_depth=1, fill_max_depth=max_depth, fill_extrapolate=extrapolate, fill_blur=blur, iterations=1)
+        assert _raw_track_batch(eng, c, o, opts) == lib.ERR_INVALID, (max_depth, extrapolate, blur)
+        assert field in eng.lib.se3tn_last_error(eng._ctx)
+        torch.cuda.synchronize()
+        assert all(torch.isnan(x).all() for x in o)
+    assert eng.last_launch_count() == before
     o = nan_outs()
-    assert _raw_track_batch(eng, c, o) == lib.OK
+    assert _raw_track_batch(eng, c, o, lib.TrackOpts(fill_depth=1, fill_max_depth=2.0, iterations=1)) == lib.OK
     assert _equal([x.cpu().numpy() for x in o], want_fill)
-    # fill off: the same bits and launches as a context on which the fill was never set
+    # fill off: the same bits and launches as a fresh context's step without options
     fresh = _make_engine(pkg, synth)
     try:
         cf = Case(fresh, synth, 5, seed=59)

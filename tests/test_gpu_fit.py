@@ -1,7 +1,8 @@
-"""The fit check of a tracking step (se3tn_set_fit_check, Engine.track_render(fit=), Tracker(fit=), the drivers' fit=): every row
+"""The fit check of a tracking step (se3tn_track_opts.fit_tau_mm, Engine.track_render(fit=), Tracker(fit=), the drivers' fit=): every row
 equals oracle/fit_ref.py on the model rendered at the step's new poses and the observed depth crop_bbox cuts at their windows, in
 every precision, render mode, batch shape, round count and route; the step's other outputs keep their bits; the graph key,
 launch count and refusals follow include/se3tn.h; and the rows mean what their names say on hand-made frames."""
+import ctypes as C
 import importlib
 import os
 import sys
@@ -9,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 from test_gpu_precision_sweep import eoat, ycbv, pr      # the synthetic layouts of the driver tests  # noqa: F401
-from test_gpu_refine import _raw_track_batch, _raw_track_host, _tracker
+from test_gpu_refine import _raw_track_batch, _raw_track_host, _raw_track_render, _tracker
 
 pytestmark = pytest.mark.gpu
 PKG = 'iros20-6d-pose-tracking_b200'
@@ -189,6 +190,14 @@ def test_meaning_with_a_zero_head(synth, eng):
         assert rows[0, 2] == rows[0, 0] and rows[0, 5] == 0 and rows[0, 1] == rows[0, 0]
 
 
+def _raw_track_render_host(e, c, out, opts, out_fit):
+    Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
+    h = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+    return e.lib.se3tn_track_render_host(e._ctx, h(c.rgb), h(c.depth), HW[0], HW[1], h(Kh), h(c.poses), h(np.full(c.n, 200.0)), 0, 0, 0,
+                                         h(c.wid), c.n, TN, RN, 2, h(out[0]), h(out[1]), h(out[2]), C.byref(opts), h(out_fit),
+                                         C.c_void_p(0))
+
+
 def test_refusals(synth, eng):
     L = importlib.import_module(PKG + '._lib')
     c = Case(eng, synth, 4, seed=45)
@@ -196,33 +205,35 @@ def test_refusals(synth, eng):
     dev_out = lambda: (torch.full((4, 4, 4), float('nan'), dtype=torch.float64, device=eng.device),
                        torch.full((4, 3), float('nan'), device=eng.device), torch.full((4, 3), float('nan'), device=eng.device))
     host_out = lambda: (np.full((4, 4, 4), np.nan), np.full((4, 3), np.nan, np.float32), np.full((4, 3), np.nan, np.float32))
-    try:
-        eng.lib.se3tn_set_refine_iterations(eng._ctx, 1)
-        eng.lib.se3tn_set_depth_fill(eng._ctx, 0, 0.0, 0, 0)
-        assert eng.lib.se3tn_set_fit_check(eng._ctx, 0, 1) == L.OK     # whatever the tests before left on the context
-        for bad in (0, 1001, -5):                                   # off stays off: track_batch still runs
-            assert eng.lib.se3tn_set_fit_check(eng._ctx, 1, bad) == L.ERR_INVALID
-        out = dev_out()
-        assert _raw_track_batch(eng, c, ra, da, out) == L.OK
+    refused = lambda rc, field: rc == L.ERR_INVALID and field in eng.lib.se3tn_last_error(eng._ctx)
+    out = dev_out()
+    assert _raw_track_batch(eng, c, ra, da, out, L.TrackOpts(iterations=1, fit_tau_mm=0)) == L.OK     # off: track_batch runs
+    torch.cuda.synchronize()
+    assert torch.isfinite(out[0]).all()
+    launches = eng.last_launch_count()
+    for bad in (1001, -5, 12):              # out of range for every call; on at all for the two calls that take input A
+        opts = L.TrackOpts(iterations=1, fit_tau_mm=bad)
+        out, hout, rout, rhout, rows = dev_out(), host_out(), dev_out(), host_out(), np.full((4, L.FIT_COLS), -1, np.int32)
+        assert refused(_raw_track_batch(eng, c, ra, da, out, opts), b'fit_tau_mm'), bad
+        assert refused(_raw_track_host(eng, c, ra.cpu().numpy(), da.cpu().numpy(), hout, opts), b'fit_tau_mm'), bad
+        if bad != 12:
+            assert refused(_raw_track_render(eng, c, c.P, rout, opts), b'fit_tau_mm'), bad
+            assert refused(_raw_track_render_host(eng, c, rhout, opts, rows), b'fit_tau_mm'), bad
         torch.cuda.synchronize()
-        assert torch.isfinite(out[0]).all()
-        assert eng.lib.se3tn_set_fit_check(eng._ctx, 1, 12) == L.OK
-        for bad in (0, 1001):                                       # on stays on: both entry points that take input A refuse
-            assert eng.lib.se3tn_set_fit_check(eng._ctx, 1, bad) == L.ERR_INVALID
-        out, hout = dev_out(), host_out()
-        assert _raw_track_batch(eng, c, ra, da, out) == L.ERR_STATE
-        assert _raw_track_host(eng, c, ra.cpu().numpy(), da.cpu().numpy(), hout) == L.ERR_STATE
-        assert b'se3tn_set_fit_check' in eng.lib.se3tn_last_error(eng._ctx)
-        torch.cuda.synchronize()
-        assert all(torch.isnan(x).all() for x in out) and all(np.isnan(x).all() for x in hout)
-    finally:
-        eng.lib.se3tn_set_fit_check(eng._ctx, 0, 1)
+        assert all(torch.isnan(x).all() for x in out + rout) and all(np.isnan(x).all() for x in hout + rhout), bad
+        assert (rows == -1).all(), bad
+    # the host route's rows: out_fit is required while the check is on, and must be NULL while it is off
+    hout, rows = host_out(), np.full((4, L.FIT_COLS), -1, np.int32)
+    assert refused(_raw_track_render_host(eng, c, hout, L.TrackOpts(iterations=1, fit_tau_mm=12), None), b'out_fit')
+    assert refused(_raw_track_render_host(eng, c, hout, L.TrackOpts(iterations=1, fit_tau_mm=0), rows), b'out_fit')
+    assert all(np.isnan(x).all() for x in hout) and (rows == -1).all()
+    assert eng.last_launch_count() == launches
     for bad in (0, 1001, 2.0, True, '10'):
         with pytest.raises(ValueError, match='fit'):
             eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, fit=bad)
     with pytest.raises(ValueError, match='out_fit'):
         eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, fit=10, out_fit=torch.empty(4, 5, dtype=torch.int32, device=eng.device))
-    eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, fit=10)          # the Engine's own track_batch turns the check off first
+    eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, fit=10)          # leaves nothing on the context for the next track_batch
     eng.track_batch(c.R, c.D, K, c.P, c.ow, ra, da, TN, RN)
 
 

@@ -1,4 +1,4 @@
-"""Refinement rounds inside one tracking step (se3tn_set_refine_iterations, Engine.track_render(iterations=k), Tracker(iterations=k),
+"""Refinement rounds inside one tracking step (se3tn_track_opts.iterations, Engine.track_render(iterations=k), Tracker(iterations=k),
 the one-pass drivers' iterations=): a k-round step must give the bits of k chained single-round steps on the same device frame,
 whatever the render mode, depth fill, precision, batch size or mix of weight sets; the host call those of the device call; and the
 graph key, launch count and refusals must follow include/se3tn.h."""
@@ -145,19 +145,31 @@ def test_k_back_to_one_is_a_context_that_never_set_it(pkg, synth, eng):
         fresh.close()
 
 
-def _raw_track_batch(e, c, ra, da, out):
+def _byref(opts):
+    return None if opts is None else C.byref(opts)
+
+
+def _raw_track_batch(e, c, ra, da, out, opts=None):
     Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
     p = lambda t: C.c_void_p(t.data_ptr())
     return e.lib.se3tn_track_batch(e._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(c.P), p(c.ow), p(ra), p(da),
                                    c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, 2, p(out[1]), p(out[2]), p(out[0]),
-                                   C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                   _byref(opts), C.c_void_p(torch.cuda.current_stream().cuda_stream))
 
 
-def _raw_track_host(e, c, ra, da, out):
+def _raw_track_host(e, c, ra, da, out, opts=None):
     Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
     h = lambda a: a.ctypes.data_as(C.c_void_p)
     return e.lib.se3tn_track_host(e._ctx, h(c.rgb), h(c.depth), HW[0], HW[1], h(Kh), h(c.poses), h(np.full(c.n, 200.0)), h(ra), h(da),
-                                  h(c.wid), c.n, TN, RN, 2, h(out[0]), h(out[1]), h(out[2]), C.c_void_p(0))
+                                  h(c.wid), c.n, TN, RN, 2, h(out[0]), h(out[1]), h(out[2]), _byref(opts), C.c_void_p(0))
+
+
+def _raw_track_render(e, c, P, out, opts=None, rounds=None):
+    Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
+    p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    return e.lib.se3tn_track_render(e._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(P), p(c.ow), 0, 0, 0,
+                                    c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, 2, p(out[1]), p(out[2]), p(out[0]),
+                                    _byref(opts), p(rounds), C.c_void_p(torch.cuda.current_stream().cuda_stream))
 
 
 def test_refusals(synth, eng):
@@ -167,28 +179,34 @@ def test_refusals(synth, eng):
     dev_out = lambda: (torch.full((4, 4, 4), float('nan'), dtype=torch.float64, device=eng.device),
                        torch.full((4, 3), float('nan'), device=eng.device), torch.full((4, 3), float('nan'), device=eng.device))
     host_out = lambda: (np.full((4, 4, 4), np.nan), np.full((4, 3), np.nan, np.float32), np.full((4, 3), np.nan, np.float32))
-    try:
-        for bad in (0, 9, -1):                                      # default k = 1 stays: track_batch still runs
-            assert eng.lib.se3tn_set_refine_iterations(eng._ctx, bad) == L.ERR_INVALID
-        out = dev_out()
-        assert _raw_track_batch(eng, c, ra, da, out) == L.OK
+    refused = lambda rc, field: rc == L.ERR_INVALID and field in eng.lib.se3tn_last_error(eng._ctx)
+    out = dev_out()
+    assert _raw_track_batch(eng, c, ra, da, out, L.TrackOpts(iterations=1)) == L.OK     # k = 1: track_batch runs
+    torch.cuda.synchronize()
+    assert torch.isfinite(out[0]).all()
+    launches = eng.last_launch_count()
+    for bad in (0, 9, -1, 2, 3):              # out of range for every call; k > 1 for the two calls that take input A
+        opts = L.TrackOpts(iterations=bad)
+        out, hout, rout = dev_out(), host_out(), dev_out()
+        assert refused(_raw_track_batch(eng, c, ra, da, out, opts), b'iterations'), bad
+        assert refused(_raw_track_host(eng, c, ra.cpu().numpy(), da.cpu().numpy(), hout, opts), b'iterations'), bad
+        if bad not in (2, 3):
+            assert refused(_raw_track_render(eng, c, c.P, rout, opts), b'iterations'), bad
         torch.cuda.synchronize()
-        assert torch.isfinite(out[0]).all()
-        assert eng.lib.se3tn_set_refine_iterations(eng._ctx, 3) == L.OK
-        for bad in (0, 9):                                          # k = 3 stays: both entry points that take input A refuse
-            assert eng.lib.se3tn_set_refine_iterations(eng._ctx, bad) == L.ERR_INVALID
-        out, hout = dev_out(), host_out()
-        assert _raw_track_batch(eng, c, ra, da, out) == L.ERR_STATE
-        assert _raw_track_host(eng, c, ra.cpu().numpy(), da.cpu().numpy(), hout) == L.ERR_STATE
-        assert b'se3tn_set_refine_iterations' in eng.lib.se3tn_last_error(eng._ctx)
-        torch.cuda.synchronize()
-        assert all(torch.isnan(x).all() for x in out) and all(np.isnan(x).all() for x in hout)
-    finally:
-        eng.lib.se3tn_set_refine_iterations(eng._ctx, 1)
+        assert all(torch.isnan(x).all() for x in out + rout) and all(np.isnan(x).all() for x in hout), bad
+    # round_poses must not overlap the poses a later round reads: over poses_out, then over poses_in
+    rounds = torch.full((3, 4, 4, 4), float('nan'), dtype=torch.float64, device=eng.device)
+    out = dev_out()
+    assert refused(_raw_track_render(eng, c, c.P, (rounds[2],) + out[1:], L.TrackOpts(iterations=3), rounds), b'round_poses')
+    rounds[0].copy_(c.P)
+    assert refused(_raw_track_render(eng, c, rounds[0], out, L.TrackOpts(iterations=3), rounds), b'round_poses')
+    torch.cuda.synchronize()
+    assert all(torch.isnan(x).all() for x in out) and torch.isnan(rounds[1:]).all()
+    assert eng.last_launch_count() == launches
     for bad in (0, 9, 2.0, True):
         with pytest.raises(ValueError, match='iterations'):
             eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, iterations=bad)
-    # the Engine's own track_batch sets k = 1 first, whatever a track_render call left on the context
+    # a track_render call with k = 3 leaves nothing on the context that the Engine's own track_batch would have to undo
     eng.track_render(c.R, c.D, K, c.P, c.ow, TN, RN, iterations=3)
     eng.track_batch(c.R, c.D, K, c.P, c.ow, ra, da, TN, RN)
 

@@ -190,7 +190,8 @@ def _raw_track_render(eng, R, D, P, ow, mode, rh, rw, wid, n, outs):
     vp = lambda t: C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
     return eng.lib.se3tn_track_render(eng._ctx, vp(R), vp(D), R.shape[0], R.shape[1], K4.ctypes.data_as(C.c_void_p), vp(P), vp(ow), mode, rh, rw,
                                       wh.ctypes.data_as(C.c_void_p) if wh is not None else C.c_void_p(0), vp(wd), n, TN, RN, 2,
-                                      vp(outs[1]), vp(outs[2]), vp(outs[0]), C.c_void_p(torch.cuda.current_stream(eng.device).cuda_stream))
+                                      vp(outs[1]), vp(outs[2]), vp(outs[0]), None, None,
+                                      C.c_void_p(torch.cuda.current_stream(eng.device).cuda_stream))
 
 
 def test_errors_launch_nothing_and_leave_the_context_usable(pkg, synth, eng):

@@ -1,4 +1,4 @@
-"""Pose recovery from perturbed starts on the YCB-Video key frames (predict.recoverYcbKeyframes, se3tn_track_render_rounds,
+"""Pose recovery from perturbed starts on the YCB-Video key frames (predict.recoverYcbKeyframes, se3tn_track_render's round_poses,
 se3tn_pose_errors_sets) on a synthetic layout of 120 x 160 frames and three classes with their own checkpoints, statistics and
 normalisers:
 

@@ -1,4 +1,4 @@
-"""Host logic of refinement rounds (se3tn_set_refine_iterations through Engine / Tracker / the one-pass drivers' iterations= and
+"""Host logic of refinement rounds (se3tn_track_opts.iterations through Engine / Tracker / the one-pass drivers' iterations= and
 predict --iterations): which counts are taken, what is refused before anything reaches a device, and where each variant's tree goes.
 CPU only; the tracked poses are checked on the GPU (test_gpu_refine.py)."""
 import importlib, os, re
