@@ -441,6 +441,79 @@ int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint
                             double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
                             void* stream);
 
+/* ---- multi-hypothesis tracking: several starts per track, the one whose model fits the frame best kept ---------------- */
+
+/* A track that has slipped further than the network was trained to correct stays lost: the network pulls a pose back from
+ * perturbations up to dataset_info's max_translation / max_rotation (reference produce_train_pair_data.py:90-110).  A hypothesis
+ * step looks around the previous pose instead of only at it.  For each of n tracks it
+ *   1. draws S - 1 start poses around the previous pose P: hypothesis h >= 1 is P . inv(D), D = random_gaussian_magnitude(
+ *      max_translation, max_rotation_deg) (reference Utils.py:372-404), composed as produce_train_pair_data.py:110 composes a
+ *      training pair (A_in_cam = B_in_cam . inv(B_in_A)); hypothesis 0 is P itself;
+ *   2. refines all n x S starts as one n x S-track se3tn_track_render step (the options' fill, k rounds and fit check);
+ *   3. keeps, per track, the hypothesis whose fit row has the highest inlier fraction inlier / model (compared exactly as int64
+ *      cross products; model = 0 ranks last), then the lowest mean inlier residual residual / inlier (inlier = 0 ranks last),
+ *      then the lowest h.  A frame without depth leaves every inlier count at 0 and keeps hypothesis 0 as long as hypothesis 0's
+ *      model covers a pixel of its window (model > 0); when it covers none, the first h >= 1 whose model does wins.
+ * Rows are track-major: track i's hypothesis h is row i S + h of every n x S array.  Draws: Philox4x32-10 (the generator of
+ * se3tn_augment), key = seed, counter = (draw_keys[i] low word, high word, h, slot).  Each of the translation and the rotation
+ * takes a direction from random_direction (theta = 2 pi U, phi = acos(2 U - 1)) and a magnitude from N(0, max), redrawn until
+ * |m| <= max as the reference does, at most 64 times; a magnitude that never lands inside (probability ~1e-32) is clamped to +-max.
+ * The rotation is cv2.Rodrigues of axis / |axis| * m / 180 * pi in fp64.  The draws depend on (seed, draw key, h) alone: not on
+ * n, the precision, the route or anything else in the step.  S = 1 draws nothing and is se3tn_track_render's step bit for bit.
+ * Whether more hypotheses track better on a trained checkpoint has not been measured (README). */
+#define SE3TN_MAX_HYPOTHESES 32
+#define SE3TN_HYP_DRAWS 8     /* se3tn_draw_hypotheses' out_draws columns (below) */
+typedef struct se3tn_hypothesis_opts {
+    int32_t hypotheses, reserved;                  /* S in [1, SE3TN_MAX_HYPOTHESES]; reserved 0                            */
+    int64_t seed;                                  /* the Philox key                                                         */
+    double max_translation, max_rotation_deg;      /* metres, finite, in (0, 1]; degrees, in (0, 180]                        */
+} se3tn_hypothesis_opts;                           /* 32 bytes, no padding                                                   */
+
+/* se3tn_track_render with S hypotheses per track, in one call and one CUDA graph.  Arguments as se3tn_track_render, plus:
+ *   draw_keys int64 (n) device: each track's draw key, read on the device, so one captured step replays frame after frame with
+ *     fresh draws when the caller writes new keys into the same array; may be NULL when S = 1
+ *   hyp: the hypothesis options (HOST, read during the call only)
+ *   out_choice int32 (n) device: the hypothesis each track kept
+ *   out_fit int32 (n, SE3TN_FIT_COLS) device: the kept rows; se3tn_fit_rows then holds all n x S rows of the step
+ *   hyp_poses double (n, S, 16) device or NULL: every hypothesis after the last round
+ *   round_poses double (k, n, S, 16) device or NULL: every round of every hypothesis, as se3tn_track_render's
+ * poses_out[i], out_trans[i], out_rot[i] are hypothesis out_choice[i]'s.  opts->fit_tau_mm is required (the choice ranks its
+ * rows).  poses_in is read only by the expansion, the step's first launch, so poses_out may be poses_in.  The n x S starts, ids,
+ * widths and network outputs live in context scratch (max_batch rows, allocated by the first call, never moved).  The step is the
+ * expansion, then the n x S-track se3tn_track_render step's launches (its first render waits for the expansion to complete), then
+ * the choice: se3tn_last_launch_count is that step's + 2.  The hypothesis options and every pointer are part of the step's key.
+ * The n x S step picks its split-K regime by n x S (n <= 4 is the latency mode), so hypothesis 0 matches a plain n-track step bit
+ * for bit only when both land in the same regime.  Refused with SE3TN_ERR_INVALID, the field named and nothing queued: what
+ * se3tn_track_render refuses, S, max_translation or max_rotation_deg out of range, hyp->reserved != 0, n x S > max_batch, fit off,
+ * draw_keys NULL with S > 1, and any output overlapping poses_in (except poses_out == poses_in), draw_keys or another output.  Ids
+ * without weights, statistics or a mesh are SE3TN_ERR_STATE, as in se3tn_track_render. */
+int se3tn_track_hypotheses(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                           const double* K, const double* poses_in, const double* object_width,
+                           int render_mode, int render_H, int render_W,
+                           const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                           double trans_normalizer, double rot_normalizer, int precision,
+                           float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                           const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, int32_t* out_fit,
+                           double* hyp_poses, void* stream);
+
+/* se3tn_track_hypotheses with every pointer in HOST memory, through se3tn_track_render_host's pinned staging: the draw keys go
+ * up with the poses in the one copy in; the poses, out_trans / out_rot (nullable), out_fit (n, SE3TN_FIT_COLS, required) and
+ * out_choice (n, required) come back in the one copy out.  The whole frame is uploaded when S > 1 (the starts' crop windows are
+ * drawn on the device).  Synchronises `stream`.  Errors as se3tn_track_hypotheses. */
+int se3tn_track_hypotheses_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                                const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                                const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
+                                double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                                const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, void* stream);
+
+/* The expansion alone, as se3tn_track_hypotheses' first launch forms it: poses_in double (n,16), draw_keys int64 (n) (NULL when
+ * S = 1) -> out_poses double (n, S, 16), all device.  out_draws double (n, S, SE3TN_HYP_DRAWS) device or NULL: per row the
+ * translation direction's U_theta, U_phi, the rotation axis' U_theta, U_phi, the accepted magnitudes m_T (m) and m_R (degrees),
+ * and the N(0, max) draws each took (1..64); all 0 in hypothesis 0's rows.  One plain launch.  Refused (SE3TN_ERR_INVALID,
+ * nothing queued): hyp out of range, n x S > max_batch, draw_keys NULL with S > 1, an output overlapping an input or the other. */
+int se3tn_draw_hypotheses(se3tn_ctx* ctx, const double* poses_in, const int64_t* draw_keys, int n, const se3tn_hypothesis_opts* hyp,
+                          double* out_poses, double* out_draws, void* stream);
+
 /* ---- checkpoint validation: the loss of ready-made training pairs ---------------------------------------------------- */
 
 /* Problem.validate's per-batch work (reference problems.py:106-132) as ONE step: for n pairs as TrackDataset.__getitem__ reads

@@ -18,6 +18,8 @@ MAX_REFINE_ITERATIONS = 8
 FIT_COLS = 6
 AUG_PARAMS = 24
 AUG_MAX_CORNERS = 64
+MAX_HYPOTHESES = 32
+HYP_DRAWS = 8
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -54,6 +56,11 @@ SIGNATURES = {
                                 _vp]),
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                      _vp]),
+    'se3tn_track_hypotheses': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_track_hypotheses_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
     'se3tn_fit_rows': (_i, [_vp, C.POINTER(_vp)]),
@@ -96,6 +103,12 @@ class TrackOpts(C.Structure):
     """se3tn_track_opts (include/se3tn.h)."""
     _fields_ = [('fill_depth', C.c_int32), ('fill_extrapolate', C.c_int32), ('fill_blur', C.c_int32), ('iterations', C.c_int32),
                 ('fill_max_depth', _d), ('fit_tau_mm', C.c_int32), ('reserved', C.c_int32)]
+
+
+class HypothesisOpts(C.Structure):
+    """se3tn_hypothesis_opts (include/se3tn.h)."""
+    _fields_ = [('hypotheses', C.c_int32), ('reserved', C.c_int32), ('seed', C.c_int64), ('max_translation', _d),
+                ('max_rotation_deg', _d)]
 
 
 _lib = None

@@ -4,6 +4,7 @@
 // whose rounding matters is spelt with an explicit round-to-nearest intrinsic on the device (nvcc would contract a * b + c).
 #pragma once
 #include <cstdint>
+#include "philox.cuh"
 #ifndef __CUDACC__
 #include <cmath>
 #define AUG_HD inline
@@ -147,24 +148,10 @@ AUG_HD uint8_t blur_round8(uint32_t acc) { return static_cast<uint8_t>((acc + (1
 AUG_HD uint16_t blur_round16(uint64_t acc) { return static_cast<uint16_t>((acc + (1ull << 31)) >> 32); }
 
 // ---------------------------------------------------------------------------------------------------- draws
-// Philox4x32-10 (Salmon et al., SC'11): counter (pair index low, high, stream, slot), key = the seed's two words.
-struct U4 { uint32_t x, y, z, w; };
-AUG_HD uint32_t mulhilo(uint32_t a, uint32_t b, uint32_t* hi) {
-    const uint64_t p = static_cast<uint64_t>(a) * b;
-    *hi = static_cast<uint32_t>(p >> 32);
-    return static_cast<uint32_t>(p);
-}
-AUG_HD U4 philox(U4 c, uint32_t k0, uint32_t k1) {
-    for (int r = 0; r < 10; ++r) {
-        uint32_t hi0, hi1;
-        const uint32_t lo0 = mulhilo(0xD2511F53u, c.x, &hi0), lo1 = mulhilo(0xCD9E8D57u, c.z, &hi1);
-        c = {hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0};
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return c;
-}
-// a uniform double in [0, 1) with 53 random bits, as numpy forms one from two 32-bit words
-AUG_HD double u53(uint32_t a, uint32_t b) { return ((a >> 5) * 67108864.0 + (b >> 6)) * (1.0 / 9007199254740992.0); }
+// Philox4x32-10 (philox.cuh): counter (pair index low, high, stream, slot), key = the seed's two words.
+using rng::U4;
+using rng::philox;
+using rng::u53;
 
 enum Stream : uint32_t { kScalars = 0, kNoiseRgb = 1, kNoiseDepth = 2 };
 AUG_HD U4 draw_words(const Config& c, int64_t pair, uint32_t stream, uint32_t slot) {
@@ -230,13 +217,7 @@ AUG_HD int quadrant(int row, int col, int u, int v) { return (row >= v ? 2 : 0) 
 // N(0, std) of element e of a noise field (stream kNoiseRgb: (176,176,3) in HWC order, kNoiseDepth: (176,176)).  Elements 2j and
 // 2j + 1 are the two Box-Muller normals of Philox slot j.  Device only: the host never forms the noise, it is handed the fields.
 __device__ __forceinline__ double gaussian(const Config& c, int64_t pair, uint32_t stream, uint32_t e, double stddev) {
-    const U4 w = draw_words(c, pair, stream, e >> 1);
-    const double u1 = 1.0 - u53(w.x, w.y);          // (0, 1]
-    const double u2 = u53(w.z, w.w);
-    double s, co;
-    sincospi(2.0 * u2, &s, &co);
-    const double r = sqrt(dmul(-2.0, log(u1)));
-    return dmul(stddev, dmul(r, (e & 1) ? s : co));
+    return dmul(stddev, rng::box_muller(draw_words(c, pair, stream, e >> 1), e & 1));
 }
 #endif
 

@@ -684,13 +684,13 @@ coverage_count_kernel(const uint8_t* __restrict__ seg, const int* __restrict__ c
 size_t render_uniform_bytes() { return sizeof(Uniforms); }
 size_t render_projected_bytes_per_vertex() { return sizeof(PVtx); }
 
-cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s) {
+cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s, bool pdl) {
     if (n <= 0) return cudaSuccess;
     const size_t smem = static_cast<size_t>(kBandRows) * kRS * sizeof(unsigned long long);
     cudaError_t e = set_max_dynamic_smem<render_kernel>(smem);
     if (e != cudaSuccess) return e;
     if (!a.projected || !a.uniforms || a.max_nv <= 0) return cudaErrorInvalidValue;
-    e = launch_kernel(render_project_kernel, dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n), dim3(kProjThreads), 0, s, true, a);
+    e = launch_kernel(render_project_kernel, dim3((a.max_nv + kProjThreads - 1) / kProjThreads, n), dim3(kProjThreads), 0, s, pdl, a);
     if (e != cudaSuccess) return e;
     return launch_kernel(render_kernel, dim3(kBands, n), dim3(kRenderThreads), smem, s, true, a);
 }

@@ -27,7 +27,9 @@ struct RenderArgs {
 };
 size_t render_uniform_bytes();
 size_t render_projected_bytes_per_vertex();
-cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s);
+// pdl = false: the projection starts only once the launch before it has completed (a step whose first kernel writes the poses,
+// ids and widths that kernels after the render read before their griddepcontrol.wait).
+cudaError_t launch_render(const RenderArgs& a, int n, cudaStream_t s, bool pdl = true);
 // The visibility check of produce_train_pair_data.py:97-104 for n rows of one frame: each row's model rendered over the whole
 // vh x vw camera image in the pyrender mode (nearest float32 window z per pixel into zmin, n x vh x vw words of scratch), then
 // visible[i] = #(seg == class_ids[i]) and covered[i] = #(linearised depth > 0.1f).  class_ids, visible, covered device (n).

@@ -10,6 +10,7 @@
 #include <dlfcn.h>
 #include "depth_fill.h"
 #include "fit.h"
+#include "hypotheses.h"
 #include "storage.cuh"
 
 #include <algorithm>
@@ -217,6 +218,15 @@ struct AugKey {
         return c;
     }
 };
+// se3tn_track_hypotheses' expansion and choice; all zero in every other step.  The step's own tracks (StepKey::n = n x S) are the
+// expanded rows in context scratch; these are the caller's n tracks and the call's results.
+struct HypKey {
+    int32_t S, pad;                            // hypotheses per track (0: not a hypothesis step); pad is always 0
+    uint64_t seed;
+    F64Bits max_t, max_r;                      // metres, degrees
+    const double* poses_in; const int64_t* keys; const int32_t* wid_in; const double* width_in;
+    double* poses_out; float* trans_out; float* rot_out; int32_t* choice; int32_t* fit_out;
+};
 struct StepKey {
     uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
     uint8_t fill, fill_extrapolate;            // track step: its se3tn_track_opts fill, all zero when off (zero in a validation step)
@@ -236,6 +246,7 @@ struct StepKey {
     const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
     double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render) or NULL
     int32_t* fit_rows;                         // fit_tau > 0: the rows of the fit check, n x kFitCols
+    HypKey hyp;                                // track step of se3tn_track_hypotheses[_host]
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -269,6 +280,9 @@ struct se3tn_ctx {
     // the fit check's block: the device route's rows (max_batch x kFitCols int32), then the fit's rendered depth for max_batch
     // tracks; allocated by the first step with the check on, never moved after (captured steps hold both addresses)
     DevBuf<uint8_t> fit; size_t fit_bytes = 0;
+    // se3tn_track_hypotheses' expanded tracks: poses (max_batch x 16), widths, ids, network outputs (max_batch x 3 each); allocated
+    // by the first hypothesis step, never moved after
+    DevBuf<uint8_t> hyp; size_t hyp_bytes = 0;
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -706,9 +720,9 @@ RenderArgs render_args(const se3tn_ctx* c, const double* K, const double* poses,
 }
 
 int queue_render(se3tn_ctx* c, const double* K, const double* poses, const double* object_width, const int32_t* mesh_ids, int n,
-                 int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA, cudaStream_t s) {
+                 int mode, int H, int W, uint8_t* rgbA, uint16_t* depthA, cudaStream_t s, bool pdl = true) {
     const RenderArgs a = render_args(c, K, poses, object_width, mesh_ids, mode, H, W, rgbA, depthA);
-    { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s)); }
+    { ProfScope ps(c, 20, s); CU_TRY(c, launch_render(a, n, s, pdl)); }
     c->launches += 2;
     return SE3TN_OK;
 }
@@ -1264,6 +1278,69 @@ int render_into_scratch(se3tn_ctx* c, const RenderSpec& r, Step& st) {
     return SE3TN_OK;
 }
 
+// se3tn_track_hypotheses' scratch: the expanded tracks' poses | widths | ids | trans | rot, max_batch rows each.
+struct HypScratch { double* poses; double* width; int32_t* wid; float* trans; float* rot; };
+int reserve_hyp(se3tn_ctx* c, HypScratch* x) {
+    const size_t mb = static_cast<size_t>(c->max_batch);
+    const size_t o_w = align256(mb * 16 * sizeof(double)), o_id = o_w + align256(mb * sizeof(double)),
+                 o_tr = o_id + align256(mb * sizeof(int32_t)), o_ro = o_tr + align256(mb * 3 * sizeof(float));
+    CU_TRY(c, grow(c->hyp, c->hyp_bytes, o_ro + mb * 3 * sizeof(float)));
+    uint8_t* b = c->hyp.get();
+    *x = {reinterpret_cast<double*>(b), reinterpret_cast<double*>(b + o_w), reinterpret_cast<int32_t*>(b + o_id),
+          reinterpret_cast<float*>(b + o_tr), reinterpret_cast<float*>(b + o_ro)};
+    return SE3TN_OK;
+}
+
+static_assert(sizeof(se3tn_hypothesis_opts) == 32, "se3tn_hypothesis_opts is 32 bytes without padding: _lib.HypothesisOpts mirrors it");
+static_assert(kHypDraws == SE3TN_HYP_DRAWS, "se3tn_draw_hypotheses' out_draws columns");
+// se3tn_hypothesis_opts checked for n tracks and written into st.hyp's scalars.  step: a tracking call, whose choice needs the
+// fit check's rows (st holds its se3tn_track_opts already).  Refused before anything is queued.
+int hypothesis_opts(se3tn_ctx* c, const char* fn, const se3tn_hypothesis_opts* h, const int64_t* keys, int n, bool step, Step& st) {
+    const std::string f(fn);
+    if (!h) return fail(c, SE3TN_ERR_INVALID, f + ": hyp is NULL");
+    if (h->hypotheses < 1 || h->hypotheses > SE3TN_MAX_HYPOTHESES)
+        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->hypotheses is " + std::to_string(h->hypotheses) + ", not in [1, " +
+                    std::to_string(SE3TN_MAX_HYPOTHESES) + "]");
+    if (h->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": hyp->reserved must be 0");
+    if (!(std::isfinite(h->max_translation) && h->max_translation > 0.0 && h->max_translation <= 1.0))
+        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->max_translation must be finite and in (0, 1] m");
+    if (!(h->max_rotation_deg > 0.0 && h->max_rotation_deg <= 180.0))
+        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->max_rotation_deg must be in (0, 180]");
+    if (n < 0 || static_cast<long long>(n) * h->hypotheses > c->max_batch)
+        return fail(c, SE3TN_ERR_INVALID, f + ": n x hyp->hypotheses = " + std::to_string(static_cast<long long>(n) * h->hypotheses) +
+                    " exceeds max_batch " + std::to_string(c->max_batch));
+    if (step && !st.fit_tau)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be set: the choice ranks the hypotheses by the fit check's rows");
+    if (h->hypotheses > 1 && !keys) return fail(c, SE3TN_ERR_INVALID, f + ": draw_keys is NULL with hyp->hypotheses > 1");
+    st.hyp.S = h->hypotheses; st.hyp.seed = static_cast<uint64_t>(h->seed);
+    st.hyp.max_t = h->max_translation; st.hyp.max_r = h->max_rotation_deg; st.hyp.keys = keys;
+    return SE3TN_OK;
+}
+
+int run_step(se3tn_ctx* c, const Step& st, cudaStream_t s);
+
+// A checked hypothesis step over device arrays: st holds the options and, in st.hyp, the caller's n tracks and outputs.  The
+// step's own n x S tracks are the context's scratch (their poses in hyp_poses when the caller wants them); the host ids are
+// repeated as the rows repeat them, for first_wid and the fp32 mode's runs of equal ids.
+int run_hypotheses(se3tn_ctx* c, Step& st, const RenderSpec& r, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                   const double* K, const int32_t* wid_host, bool multi, int n, double tn, double rn, int precision,
+                   double* hyp_poses, double* round_poses, cudaStream_t s) {
+    HypScratch x;
+    int rc = reserve_hyp(c, &x);
+    if (rc) return rc;
+    const int S = st.hyp.S;
+    std::vector<int32_t> ids(wid_host ? static_cast<size_t>(n) * S : 0);
+    for (size_t row = 0; row < ids.size(); ++row) ids[row] = wid_host[row / S];
+    track_step(st, H, W, K, wid_host ? ids.data() : nullptr, multi, n * S, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth;
+    st.poses_out = hyp_poses ? hyp_poses : x.poses;         // every round refines the expanded starts in place
+    st.poses_in = st.poses_out;
+    st.object_width = x.width; st.wid_dev = st.hyp.wid_in ? x.wid : nullptr;
+    st.out_trans = x.trans; st.out_rot = x.rot; st.round_poses = round_poses;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, s);
+}
+
 // The conv stack over a step's n tracks.  Tensor-core modes: one forward in which every track picks its own weight set when the
 // ids are mixed, its head doing `head` too.  fp32: one FFMA forward per run of equal ids, `head` left to the caller.
 int run_tracks(se3tn_ctx* c, const Step& st, const HeadArgs& head, cudaStream_t s) {
@@ -1331,14 +1408,14 @@ int check_augment(se3tn_ctx* c, const char* fn, const se3tn_augment* a, int n, A
 // Every output of an augmentation call must be disjoint from its inputs: a CTA's reads of input B (the blur's halo rows) may come
 // after another CTA has written its own rows.  Pairs of (pointer, bytes).
 int check_disjoint(se3tn_ctx* c, const char* fn, std::initializer_list<std::pair<const void*, size_t>> outs,
-                   std::initializer_list<std::pair<const void*, size_t>> ins) {
+                   std::initializer_list<std::pair<const void*, size_t>> ins, const char* why = "in-place augmentation is not supported") {
     auto overlap = [](const std::pair<const void*, size_t>& a, const std::pair<const void*, size_t>& b) {
         const uintptr_t x = reinterpret_cast<uintptr_t>(a.first), y = reinterpret_cast<uintptr_t>(b.first);
         return a.first && b.first && x < y + b.second && y < x + a.second;
     };
     for (auto o = outs.begin(); o != outs.end(); ++o) {
         for (const auto& i : ins)
-            if (overlap(*o, i)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": an output overlaps an input (in-place augmentation is not supported)");
+            if (overlap(*o, i)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": an output overlaps an input (" + why + ")");
         for (auto o2 = o + 1; o2 != outs.end(); ++o2)
             if (overlap(*o, *o2)) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": two outputs overlap");
     }
@@ -1369,9 +1446,19 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         ++c->launches;
         return SE3TN_OK;
     }
+    if (st.hyp.S) {                                // se3tn_track_hypotheses: the n x S starts, ids and widths every later launch reads
+        HypArgs h{};
+        h.poses_in = st.hyp.poses_in; h.keys = st.hyp.keys; h.n = st.n / st.hyp.S; h.S = st.hyp.S; h.seed = st.hyp.seed;
+        h.max_t = st.hyp.max_t; h.max_r_deg = st.hyp.max_r; h.wid_in = st.hyp.wid_in; h.width_in = st.hyp.width_in;
+        h.poses = const_cast<double*>(st.poses_in); h.wid = const_cast<int32_t*>(st.wid_dev); h.width = const_cast<double*>(st.object_width);
+        CU_TRY(c, launch_hypotheses(h, s));
+        ++c->launches;
+    }
     if (st.render_mode >= 0) {                     // track i draws mesh weight_ids[i] (0 without ids): one network and one model per object
+        // after the expansion, a plain launch: preprocess_kernel reads the ids before its griddepcontrol.wait, and the chain of
+        // PDL launches behind this render starts only once the expansion has completed
         rc = queue_render(c, K, st.poses_in, st.object_width, st.wid_dev, st.n, st.render_mode, st.render_H, st.render_W,
-                          const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s);
+                          const_cast<uint8_t*>(st.rgbA), const_cast<uint16_t*>(st.depthA), s, st.hyp.S == 0);
         if (rc) return rc;
     }
     const uint16_t* depth = st.frame_depth;
@@ -1456,6 +1543,14 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         fa.poses = st.poses_out; fa.object_width = st.object_width; fa.fx = K[0]; fa.fy = K[1]; fa.cx = K[2]; fa.cy = K[3];
         fa.frame_depth = depth; fa.H = st.H; fa.W = st.W; fa.rendered = fit_depth(c); fa.tau = st.fit_tau; fa.rows = st.fit_rows;
         CU_TRY(c, launch_fit(fa, st.n, s));
+        ++c->launches;
+    }
+    if (st.hyp.S) {                                // the choice: a plain launch, after fit_kernel has completed
+        SelectArgs sa{};
+        sa.n = st.n / st.hyp.S; sa.S = st.hyp.S; sa.rows = st.fit_rows; sa.poses = st.poses_out; sa.trans = st.out_trans; sa.rot = st.out_rot;
+        sa.poses_out = st.hyp.poses_out; sa.trans_out = st.hyp.trans_out; sa.rot_out = st.hyp.rot_out; sa.choice = st.hyp.choice;
+        sa.fit_out = st.hyp.fit_out;
+        CU_TRY(c, launch_select(sa, s));
         ++c->launches;
     }
     return SE3TN_OK;
@@ -1611,6 +1706,64 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
     st.round_poses = round_poses;
     if ((rc = render_into_scratch(c, r, st))) return rc;
     return run_step(c, st, static_cast<cudaStream_t>(stream));
+}
+
+int se3tn_track_hypotheses(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                           const double* K, const double* poses_in, const double* object_width,
+                           int render_mode, int render_H, int render_W,
+                           const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                           double tn, double rn, int precision,
+                           float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                           const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, int32_t* out_fit,
+                           double* hyp_poses, void* stream) {
+    const char* fn = "se3tn_track_hypotheses";
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
+    if (!out_trans || !out_rot || !poses_out || !out_choice || !out_fit) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    Step st{};
+    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
+    if ((rc = hypothesis_opts(c, fn, hyp, draw_keys, n, true, st))) return rc;
+    bool multi = false;
+    if ((rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision))) return rc;
+    if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
+    const size_t nn = static_cast<size_t>(n), rows = nn * st.hyp.S;
+    rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_trans, nn * 12}, {out_rot, nn * 12}, {out_choice, nn * 4},
+                                {out_fit, nn * 4 * kFitCols}, {hyp_poses, rows * 128}, {round_poses, st.iterations * rows * 128}},
+                        {{poses_out == poses_in ? nullptr : poses_in, nn * 128}, {draw_keys, nn * 8}},
+                        "the starts are drawn from poses_in and draw_keys; poses_out may be poses_in itself");
+    if (rc) return rc;
+    DeviceGuard guard(c->device);
+    st.hyp.poses_in = poses_in; st.hyp.wid_in = weight_ids_dev; st.hyp.width_in = object_width;
+    st.hyp.poses_out = poses_out; st.hyp.trans_out = out_trans; st.hyp.rot_out = out_rot; st.hyp.choice = out_choice; st.hyp.fit_out = out_fit;
+    return run_hypotheses(c, st, r, frame_rgb, frame_depth, H, W, K, weight_ids_host, multi, n, tn, rn, precision, hyp_poses, round_poses,
+                          static_cast<cudaStream_t>(stream));
+}
+
+int se3tn_draw_hypotheses(se3tn_ctx* c, const double* poses_in, const int64_t* draw_keys, int n, const se3tn_hypothesis_opts* hyp,
+                          double* out_poses, double* out_draws, void* stream) {
+    const char* fn = "se3tn_draw_hypotheses";
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!poses_in || !out_poses) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument");
+    Step st{};
+    int rc = hypothesis_opts(c, fn, hyp, draw_keys, n, false, st);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    const size_t nn = static_cast<size_t>(n), rows = nn * st.hyp.S;
+    rc = check_disjoint(c, fn, {{out_poses, rows * 128}, {out_draws, rows * 8 * kHypDraws}}, {{poses_in, nn * 128}, {draw_keys, nn * 8}},
+                        "the starts are drawn from poses_in and draw_keys");
+    if (rc) return rc;
+    DeviceGuard guard(c->device);
+    HypArgs h{};
+    h.poses_in = poses_in; h.keys = draw_keys; h.n = n; h.S = st.hyp.S; h.seed = st.hyp.seed; h.max_t = st.hyp.max_t;
+    h.max_r_deg = st.hyp.max_r; h.poses = out_poses; h.draws = out_draws;
+    CU_TRY(c, launch_hypotheses(h, static_cast<cudaStream_t>(stream)));
+    return SE3TN_OK;
 }
 
 int se3tn_eval_pairs(se3tn_ctx* c, const uint8_t* rgbA, const uint16_t* depthA, const uint8_t* rgbB, const uint16_t* depthB,
@@ -2006,11 +2159,13 @@ inline void host_crop_window(const double* pose, const double* K, double width, 
 int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                    double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit, void* stream) {
+                    double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit, void* stream,
+                    const int64_t* draw_keys = nullptr, const se3tn_hypothesis_opts* hyp = nullptr, int32_t* out_choice = nullptr) {
     bool multi = false;
     Step st{};                                     // options and ids are checked before anything is staged or copied
     int rc = track_opts(c, fn, opts, render != nullptr, st);
     if (rc) return rc;
+    if (hyp && (rc = hypothesis_opts(c, fn, hyp, draw_keys, n, true, st))) return rc;
     if (!st.fit_tau != !out_fit)
         return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": out_fit is required with opts->fit_tau_mm and must be NULL without it");
     rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);
@@ -2025,9 +2180,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (io.H != H || io.W != W || io.n_cap < n) {
         CU_TRY(c, cudaStreamSynchronize(s));
         const int cap = std::max(n, io.n_cap);
-        const size_t per = 128 + 8 + img * 3 + img * 2 + 4 + 128 + 12 + 12 + 4 * kFitCols;
+        const size_t per = 128 + 8 + img * 3 + img * 2 + 8 + 4 + 128 + 12 + 12 + 4 * kFitCols + 4;
         c->graphs.clear();                                       // before the buffers are replaced: captured steps hold their addresses
-        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 9 * 256));
+        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 11 * 256));
         CU_TRY(c, grow(io.pin, io.pin_bytes, px * 5 + per * cap + 4096));
         CU_TRY(c, cudaMemsetAsync(io.dev.get(), 0, io.dev_bytes, s));   // on the caller's stream, ahead of the copies below; frame pixels outside the uploaded windows are never read, keep them defined
         io.H = H; io.W = W; io.n_cap = cap;
@@ -2038,10 +2193,12 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     // the per-track arrays are packed by THIS call's n (a step's graph is keyed by n anyway), inputs first, outputs behind them:
     // one host -> device copy carries all inputs, one device -> host copy all outputs; input A takes no room when it is rendered
     const size_t nn = static_cast<size_t>(n), a_img = render ? 0 : img;
+    // a hypothesis step's draw keys go up with the poses, its choices come back behind the fit rows
     const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * a_img * 3),
-                 o_wid = o_depthA + align256(nn * a_img * 2), in_bytes = o_wid + align256(nn * 4);
+                 o_key = o_depthA + align256(nn * a_img * 2), o_wid = o_key + (hyp ? align256(nn * 8) : 0), in_bytes = o_wid + align256(nn * 4);
     const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), o_fit = o_ro + align256(nn * 12);
-    const size_t out_bytes = st.fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
+    const size_t o_choice = st.fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
+    const size_t out_bytes = hyp ? o_choice + align256(nn * 4) : o_choice;
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
     double* d_ow = reinterpret_cast<double*>(d_in + o_ow);
@@ -2053,6 +2210,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     float* d_tr = reinterpret_cast<float*>(d_res + o_tr);
     float* d_ro = reinterpret_cast<float*>(d_res + o_ro);
     int32_t* d_fit = reinterpret_cast<int32_t*>(d_res + o_fit);
+    int32_t* d_choice = reinterpret_cast<int32_t*>(d_res + o_choice);
     // ---- the part of the frame the tracks' crop windows touch (K0 reads nothing else) ----
     int y0 = H, y1 = 0, x0 = W, x1 = 0;
     for (int i = 0; i < n; ++i) {
@@ -2063,8 +2221,8 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
         x0 = std::min(x0, std::max(left - 1, 0)); x1 = std::max(x1, std::min(left + cw + 1, W));
     }
     if (y1 <= y0 || x1 <= x0) { y0 = y1 = x0 = x1 = 0; }         // every window misses the frame: nothing of it is read
-    // refinement rounds after the first crop at poses only the step computes: their windows are not known here
-    const bool whole_frame = st.iterations > 1;
+    // refinement rounds after the first crop at poses only the step computes, and hypotheses' starts: their windows are not known here
+    const bool whole_frame = st.iterations > 1 || st.hyp.S > 1;
     if (whole_frame || static_cast<size_t>(y1 - y0) * (x1 - x0) * 2 >= px) { y0 = 0; y1 = H; x0 = 0; x1 = W; }
     // ---- stage through pinned memory, one asynchronous copy per array ----
     // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
@@ -2097,16 +2255,25 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
         memcpy(hp + o_rgbA, rgbA, nn * img * 3);
         memcpy(hp + o_depthA, depthA, nn * img * 2);
     }
+    if (hyp && draw_keys) memcpy(hp + o_key, draw_keys, nn * 8);
     if (weight_ids) memcpy(hp + o_wid, weight_ids, nn * 4);
     CU_TRY(c, cudaMemcpyAsync(d_in, hp, weight_ids ? in_bytes : o_wid, cudaMemcpyHostToDevice, s));
     hp += in_bytes;
-    track_step(st, H, W, K, weight_ids, multi, n, tn, rn, precision);
-    st.frame_rgb = d_rgb; st.frame_depth = d_depth; st.poses_in = d_poses; st.object_width = d_ow;
-    st.rgbA = d_rgbA; st.depthA = d_depthA; st.wid_dev = weight_ids ? d_wid : nullptr;
-    st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
-    if (render && (rc = render_into_scratch(c, *render, st))) return rc;
-    if (st.fit_tau) st.fit_rows = d_fit;
-    if ((rc = run_step(c, st, s))) return rc;
+    if (hyp) {                                   // the n x S rows' fit rows stay in the context's block; the chosen ones come back
+        st.hyp.poses_in = d_poses; st.hyp.keys = draw_keys ? reinterpret_cast<const int64_t*>(d_in + o_key) : nullptr;
+        st.hyp.wid_in = weight_ids ? d_wid : nullptr; st.hyp.width_in = d_ow;
+        st.hyp.poses_out = d_out; st.hyp.trans_out = d_tr; st.hyp.rot_out = d_ro; st.hyp.choice = d_choice; st.hyp.fit_out = d_fit;
+        rc = run_hypotheses(c, st, *render, d_rgb, d_depth, H, W, K, weight_ids, multi, n, tn, rn, precision, nullptr, nullptr, s);
+    } else {
+        track_step(st, H, W, K, weight_ids, multi, n, tn, rn, precision);
+        st.frame_rgb = d_rgb; st.frame_depth = d_depth; st.poses_in = d_poses; st.object_width = d_ow;
+        st.rgbA = d_rgbA; st.depthA = d_depthA; st.wid_dev = weight_ids ? d_wid : nullptr;
+        st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
+        if (render && (rc = render_into_scratch(c, *render, st))) return rc;
+        if (st.fit_tau) st.fit_rows = d_fit;
+        rc = run_step(c, st, s);
+    }
+    if (rc) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
     CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
@@ -2114,6 +2281,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
     if (out_fit) memcpy(out_fit, ho + o_fit, nn * 4 * kFitCols);
+    if (out_choice) memcpy(out_choice, ho + o_choice, nn * 4);
     return SE3TN_OK;
 }
 }  // namespace
@@ -2142,6 +2310,23 @@ int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16
     if (rc) return rc;
     return track_host_step(c, "se3tn_track_render_host", frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r,
                            weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, out_fit, stream);
+}
+
+int se3tn_track_hypotheses_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                                const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                                const int32_t* weight_ids, int n, double tn, double rn, int precision,
+                                double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                                const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, void* stream) {
+    const char* fn = "se3tn_track_hypotheses_host";
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument or empty frame");
+    if (!hyp || !out_choice) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": hyp and out_choice are required");
+    RenderSpec r;
+    const int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    return track_host_step(c, fn, frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r, weight_ids, n, tn, rn,
+                           precision, poses_out, out_trans, out_rot, opts, out_fit, stream, draw_keys, hyp, out_choice);
 }
 
 int se3tn_allgather_poses(se3tn_ctx* c, void* nccl_comm, const double* local_poses, double* all_poses, int n_local, void* stream) {

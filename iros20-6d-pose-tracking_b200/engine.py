@@ -376,6 +376,114 @@ class Engine:
             res += (fit_rows,)
         return res if len(res) > 1 else out
 
+    # ------------------------------------------------------------------ multi-hypothesis tracking
+    @staticmethod
+    def hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg):
+        """se3tn_hypothesis_opts of a hypothesis call: S in [1, MAX_HYPOTHESES], a 64-bit seed, the spread in metres (finite, in
+        (0, 1]) and degrees (in (0, 180]); else a ValueError."""
+        S = hypotheses
+        if isinstance(S, (bool, np.bool_)) or not isinstance(S, (int, np.integer)) or not 1 <= S <= _lib.MAX_HYPOTHESES:
+            raise ValueError('hypotheses must be an integer in [1, %d], not %r' % (_lib.MAX_HYPOTHESES, S))
+        if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)):
+            raise ValueError('seed must be an integer, not %r' % (seed,))
+        mt, mr = float(max_translation), float(max_rotation_deg)
+        if not (math.isfinite(mt) and 0 < mt <= 1):
+            raise ValueError('max_translation must be finite and in (0, 1] m, not %r' % (max_translation,))
+        if not 0 < mr <= 180:
+            raise ValueError('max_rotation_deg must be in (0, 180], not %r' % (max_rotation_deg,))
+        seed = int(seed) & ((1 << 64) - 1)
+        return _lib.HypothesisOpts(hypotheses=int(S), seed=seed - (1 << 64) if seed >= 1 << 63 else seed, max_translation=mt,
+                                   max_rotation_deg=mr)
+
+    def draw_hypotheses(self, poses, draw_keys, hypotheses, max_translation, max_rotation_deg, seed=0, want_draws=False):
+        """The starts a hypothesis step expands n tracks into (se3tn_draw_hypotheses): poses float64 (n,4,4) and draw_keys int64
+        (n) CUDA tensors (draw_keys may be None when hypotheses is 1) -> float64 (n,S,4,4) [, float64 (n,S,8) draws: the
+        translation's U_theta, U_phi, the rotation axis' U_theta, U_phi, m_T (m), m_R (degrees), tries_T, tries_R]."""
+        n = int(poses.shape[0])
+        hyp = self.hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg)
+        self._check_dev('poses', poses, torch.float64, (n, 4, 4))
+        if draw_keys is not None:
+            self._check_dev('draw_keys', draw_keys, torch.int64, (n,))
+        S = hyp.hypotheses
+        out = torch.empty(n, S, 4, 4, dtype=torch.float64, device=self.device)
+        draws = torch.empty(n, S, _lib.HYP_DRAWS, dtype=torch.float64, device=self.device) if want_draws else None
+        _lib.check(self.lib.se3tn_draw_hypotheses(self._ctx, _ptr(poses), _ptr(draw_keys), n, C.byref(hyp), _ptr(out), _ptr(draws),
+                                                  _stream(self.device)), self._ctx)
+        return (out, draws) if want_draws else out
+
+    def track_hypotheses(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer, draw_keys,
+                         hypotheses, max_translation, max_rotation_deg, seed=0, fit=None, weight_ids_host=None, weight_ids_dev=None,
+                         precision='bf16x3', mode='vispy', image_hw=None, out_poses=None, out_trans=None, out_rot=None,
+                         fill_depth=None, iterations=1, out_choice=None, out_fit=None, out_hyp_poses=None, out_rounds=None):
+        """track_render from S start hypotheses per track, keeping the one whose model fits the frame best
+        (se3tn_track_hypotheses), enqueued on the current stream.  draw_keys int64 (n) CUDA tensor: each track's draw key (None
+        only with hypotheses=1); the spread is max_translation m / max_rotation_deg degrees; fit: tau in mm, required (fit_spec).
+        -> (poses (n,4,4), choice int32 (n), fit rows int32 (n,6)), then out_hyp_poses (n,S,4,4) and out_rounds (k,n,S,4,4)
+        when given (float64 CUDA tensors: every hypothesis after the last round, and after every round).  out_poses may be
+        poses itself."""
+        n = int(poses.shape[0])
+        iterations = self.refine_iterations(iterations)
+        tau = self.fit_spec(fit)
+        hyp = self.hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg)
+        S = hyp.hypotheses
+        self._check_frame('track_hypotheses', frame_rgb, frame_depth, poses, object_width, (), n)
+        if n * S > self.max_batch:
+            raise ValueError('n x hypotheses = %d exceeds max_batch=%d' % (n * S, self.max_batch))
+        wh = self._host_ids('track_hypotheses', weight_ids_host, n)
+        if wh is not None and weight_ids_dev is None:
+            weight_ids_dev = torch.from_numpy(wh).to(self.device)
+        if draw_keys is not None:
+            self._check_dev('draw_keys', draw_keys, torch.int64, (n,))
+        new = lambda shape, dt: torch.empty(*shape, dtype=dt, device=self.device)
+        out_poses = new((n, 4, 4), torch.float64) if out_poses is None else out_poses
+        out_trans = new((n, 3), torch.float32) if out_trans is None else out_trans
+        out_rot = new((n, 3), torch.float32) if out_rot is None else out_rot
+        out_choice = new((n,), torch.int32) if out_choice is None else out_choice
+        out_fit = new((n, _lib.FIT_COLS), torch.int32) if out_fit is None else out_fit
+        for name, t, dt, shape in (('out_choice', out_choice, torch.int32, (n,)), ('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS)),
+                                   ('out_hyp_poses', out_hyp_poses, torch.float64, (n, S, 4, 4)),
+                                   ('out_rounds', out_rounds, torch.float64, (iterations, n, S, 4, 4))):
+            if t is not None:
+                self._check_dev(name, t, dt, shape)
+        H, W = frame_depth.shape
+        rc = self.lib.se3tn_track_hypotheses(
+            self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(self._k4(K)), _ptr(poses), _ptr(object_width),
+            *self._render_mode(mode, image_hw), _hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer),
+            PREC[precision], _ptr(out_trans), _ptr(out_rot), _ptr(out_poses),
+            self._track_opts(self.depth_fill_spec(fill_depth), iterations, tau), _ptr(out_rounds), _ptr(draw_keys), C.byref(hyp),
+            _ptr(out_choice), _ptr(out_fit), _ptr(out_hyp_poses), _stream(self.device))
+        _lib.check(rc, self._ctx)
+        return (out_poses, out_choice, out_fit) + tuple(t for t in (out_hyp_poses, out_rounds) if t is not None)
+
+    def track_hypotheses_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer, draw_keys,
+                              hypotheses, max_translation, max_rotation_deg, seed=0, fit=None, weight_ids=None, precision='bf16x3',
+                              mode='vispy', image_hw=None, fill_depth=None, iterations=1):
+        """track_hypotheses with numpy arrays in and out, synchronous (se3tn_track_hypotheses_host): arguments as
+        track_render_host, draw_keys int64 (n) numpy or None (hypotheses=1).  -> (poses (n,4,4), choice int32 (n), fit rows
+        int32 (n,6))."""
+        n = int(poses.shape[0])
+        iterations = self.refine_iterations(iterations)
+        tau = self.fit_spec(fit)
+        hyp = self.hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg)
+        for name, a, dt, shape in self._track_inputs('track_hypotheses_host', frame_rgb, frame_depth, poses, object_width, (), n):
+            if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
+                raise ValueError('track_hypotheses_host: %s must be a C-contiguous %s array of shape %s' % (name, dt, shape))
+        keys = None if draw_keys is None else np.ascontiguousarray(draw_keys, dtype=np.int64)
+        if keys is not None and keys.shape != (n,):
+            raise ValueError('track_hypotheses_host: draw_keys must have one entry per track')
+        wid = self._host_ids('track_hypotheses_host', weight_ids, n)
+        out = np.empty((n, 4, 4), dtype=np.float64)
+        choice = np.empty(n, dtype=np.int32)
+        rows = np.empty((n, _lib.FIT_COLS), dtype=np.int32)
+        H, W = frame_depth.shape
+        rc = self.lib.se3tn_track_hypotheses_host(
+            self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(self._k4(K)), _hptr(poses), _hptr(object_width),
+            *self._render_mode(mode, image_hw), _hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
+            _hptr(out), None, None, self._track_opts(self.depth_fill_spec(fill_depth), iterations, tau), _hptr(rows), _hptr(keys),
+            C.byref(hyp), _hptr(choice), _stream(self.device))
+        _lib.check(rc, self._ctx)
+        return out, choice, rows
+
     # ------------------------------------------------------------------ checkpoint validation
     def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
                    weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', want_terms=False, want_labels=False,

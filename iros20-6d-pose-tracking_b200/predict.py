@@ -29,6 +29,8 @@ import random
 import numpy as np
 import torch
 
+from . import _lib
+from . import engine as _engine            # the class itself: tests stand in for Engine, not for its static checks
 from .engine import Engine, check_weight_sets_fit
 from .cuda_renderer import CudaRenderer
 from .se3_tracknet import Se3TrackNet
@@ -143,7 +145,7 @@ def _as_numpy_pose(p):
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
-                 fill_depth=False, iterations=1, fit=None):
+                 fill_depth=False, iterations=1, fit=None, hypotheses=1, seed=0):
         """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
         tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
         / blur_type (Engine.depth_fill_spec).
@@ -153,11 +155,29 @@ class Tracker:
         fit: the fit check of every tracking step (Engine.track_render's fit): None / False off, True FIT_TAU_DEFAULT mm, or tau in
         mm (1..1000).  on_track / on_track_batch then leave the frame's rows (model, observed, inlier, front, behind, residual per
         track) in last_fit: numpy on the host route, an int32 CUDA tensor on the device route; fit_fractions turns them into
-        fractions.  Like iterations > 1 it needs the CUDA rasteriser drawing input A inside the step."""
+        fractions.  Like iterations > 1 it needs the CUDA rasteriser drawing input A inside the step.
+        hypotheses: S in [1, 32].  S > 1 tracks every track from S starts per frame, its previous pose and S - 1 poses drawn
+        around it with the spread the network's training pairs were drawn with (dataset_info['max_translation'] m,
+        ['max_rotation'] degrees), and keeps the one whose model fits the frame best (Engine.track_hypotheses).  It turns the fit
+        check on at FIT_TAU_DEFAULT mm when fit is not given, and needs the CUDA rasteriser as fit does.  last_fit then holds the
+        kept rows and last_choice the kept hypotheses.  Hypothesis h of track j in the Tracker's c-th call is drawn with key
+        (seed, c, j).  A Tracker that builds its Engine sizes it max_batch x S; a shared Engine must hold n x S tracks per call.
+        S = 1 is the plain step (last_choice stays None)."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
         self.iterations = Engine.refine_iterations(iterations)
+        self.hypotheses = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
+        self.seed = int(seed)
+        if self.hypotheses > 1 and fit is None:
+            fit = True
         self.fit = Engine.fit_spec(FIT_TAU_DEFAULT if fit is True else (None if fit is False else fit)) or None
+        if self.hypotheses > 1 and not self.fit:
+            raise ValueError('hypotheses=%d ranks the starts by the fit check: fit must not be off' % self.hypotheses)
+        self.spread = (float(dataset_info['max_translation']), float(dataset_info['max_rotation'])) if self.hypotheses > 1 else None
+        if self.spread:
+            _engine.Engine.hypothesis_spec(self.hypotheses, seed, *self.spread)
+        self._calls = 0                                    # the c of the draw keys (seed, c, j)
         self.last_fit = None
+        self.last_choice = None
         self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
@@ -182,7 +202,7 @@ class Tracker:
             checkpoint = ckpt_dir if 'state_dict' in ckpt_dir else {'state_dict': ckpt_dir}
         else:
             checkpoint = torch.load(ckpt_dir, map_location='cpu')
-        self.engine = engine if engine is not None else Engine(max_batch=max_batch)
+        self.engine = engine if engine is not None else Engine(max_batch=max_batch * self.hypotheses)
         self.weight_id = weight_id
         self.precision = precision
         self.model = Se3TrackNet(image_size=self.image_size[0], engine=self.engine, weight_id=weight_id, precision=precision)
@@ -329,6 +349,15 @@ class Tracker:
         if (self.iterations > 1 or self.fit) and renderer is None:
             raise ValueError(self._refine_refusal(not render))
         self.last_fit = None
+        self.last_choice = None
+        hyp = None
+        if self.hypotheses > 1:                       # (c << 32) + j: track j's draw key in this call
+            n_tracks = len(prev_poses)
+            if n_tracks * self.hypotheses > self.engine.max_batch:
+                raise ValueError('%d tracks x hypotheses=%d exceed the engine\'s max_batch=%d'
+                                 % (n_tracks, self.hypotheses, self.engine.max_batch))
+            keys = (np.int64(self._calls) << np.int64(32)) + np.arange(n_tracks, dtype=np.int64)
+            hyp = dict(hypotheses=self.hypotheses, max_translation=self.spread[0], max_rotation_deg=self.spread[1], seed=self.seed)
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
                 and not any(torch.is_tensor(x) for x in (prev_poses, weight_ids, object_width))):
@@ -342,6 +371,12 @@ class Tracker:
                 with self._uploads(poses, *frame, *(A or (None, None)), ow) as d:
                     self._calibrate_fp8(weight_ids, wh, *d)
             kw = dict(weight_ids=wh, precision=self.precision, fill_depth=self.fill_depth)
+            if hyp is not None:
+                out, self.last_choice, self.last_fit = self.engine.track_hypotheses_host(
+                    *frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer, keys, mode=renderer.mode,
+                    image_hw=renderer.image_hw, iterations=self.iterations, fit=self.fit, **hyp, **kw)
+                self._calls += 1                      # only a call that ran uses up its c
+                return out
             if renderer is not None:
                 out = self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
@@ -374,7 +409,18 @@ class Tracker:
                                                       torch.empty(n, 3, dtype=torch.float32, device=dev), torch.empty(n, 3, dtype=torch.float32, device=dev))
                 outs = dict(out_poses=ob[0], out_trans=ob[1], out_rot=ob[2])
             kw = dict(weight_ids_host=wh, weight_ids_dev=wd, precision=self.precision, fill_depth=self.fill_depth, **outs)
-            if renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
+            if hyp is not None:                       # keys, choice and rows in persistent buffers: one graph, frame after frame
+                kb = self._np_bufs.get(('hyp', n))
+                if kb is None:
+                    kb = self._np_bufs[('hyp', n)] = (torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                                                      torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=dev))
+                # formed on the device from the call count: no host copy, nothing waits for the previous step
+                torch.arange(n, dtype=torch.int64, device=dev, out=kb[0]).add_(self._calls << 32)
+                out, self.last_choice, self.last_fit = self.engine.track_hypotheses(
+                    rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer, kb[0], mode=renderer.mode,
+                    image_hw=renderer.image_hw, iterations=self.iterations, fit=self.fit, out_choice=kb[1], out_fit=kb[2], **hyp, **kw)
+                self._calls += 1
+            elif renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
                 res = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
                                                fit=self.fit, **kw)
@@ -1065,7 +1111,48 @@ def _one_pass_trackers(entries, precision, max_batch):
     return eng, trackers
 
 
-def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0):
+# Multi-hypothesis steps in the drivers (Tracker(hypotheses=S) per step): track j of a step draws its starts with a 64-bit key
+# that names where it is in the run, so a run keys its draws the same on one GPU or several.
+def hypothesis_key(a, b, c):
+    """The draw key (a << 40) + (b << 16) + c: (sequence index in the run's sorted list, frame index, track index) in the one-pass
+    drivers, (key-frame index, row, 0) in ycbv_recover.  a < 2^23, b < 2^24, c < 2^16."""
+    if not (0 <= a < 1 << 23 and 0 <= b < 1 << 24 and 0 <= c < 1 << 16):
+        raise ValueError('hypothesis key (%d, %d, %d) out of range' % (a, b, c))
+    return (a << 40) + (b << 16) + c
+
+
+def hypothesis_groups(trackers, wh):
+    """The tracks of one step grouped by the spread of their class's dataset_info ((max_translation m, max_rotation degrees), the
+    bounds its training pairs were drawn with): [(None or an int64 numpy index array, spread)].  One group of all tracks (None)
+    when every class shares one spread; otherwise the step runs once per spread on its tracks."""
+    spreads = [(float(trackers[int(w)].dataset_info['max_translation']), float(trackers[int(w)].dataset_info['max_rotation']))
+               for w in wh]
+    if len(set(spreads)) == 1:
+        return [(None, spreads[0])]
+    return [(np.asarray([j for j, sp in enumerate(spreads) if sp == g], dtype=np.int64), g) for g in sorted(set(spreads))]
+
+
+def hypothesis_step(eng, trk, rgb, depth, poses, widths, wh, wd, keys, groups, S, seed, tau, precision, iterations, outs):
+    """One driver step of S hypotheses per track (Engine.track_hypotheses) over the frame (rgb, depth), per spread group
+    (hypothesis_groups).  outs: out_poses (n,4,4), out_trans / out_rot (n,3), out_choice (n), out_fit (n,6), and optionally
+    out_hyp_poses (n,S,4,4) / out_rounds (k,n,S,4,4); the rows of each group land at their tracks.  poses may be out_poses."""
+    mode = dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw)
+    for idx, (mt, mr) in groups:
+        kw = dict(fit=tau, precision=precision, iterations=iterations, max_translation=mt, max_rotation_deg=mr, seed=seed, **mode)
+        if idx is None:
+            eng.track_hypotheses(rgb, depth, trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer, keys, S,
+                                 weight_ids_host=wh, weight_ids_dev=wd, **kw, **outs)
+            continue
+        di = torch.from_numpy(idx).to(eng.device)
+        sub = {k: (v.index_select(1, di) if k == 'out_rounds' else v.index_select(0, di)).contiguous() for k, v in outs.items()}
+        eng.track_hypotheses(rgb, depth, trk.K, poses.index_select(0, di).contiguous(), widths.index_select(0, di).contiguous(),
+                             trk.trans_normalizer, trk.rot_normalizer, keys.index_select(0, di).contiguous(), S,
+                             weight_ids_host=wh[idx], weight_ids_dev=wd.index_select(0, di).contiguous(), **kw, **sub)
+        for k, v in sub.items():
+            outs[k].index_copy_(1 if k == 'out_rounds' else 0, di, v)
+
+
+def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0, hyp=None, seq_index=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
     variants: what every frame is tracked in (a tuple) as _sweep_variants keys them, (mode, k) or (mode, k, c): precision mode, k
@@ -1089,7 +1176,12 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     Videos are drawn for one variant only.
 
     fit: tau in mm turns on every step's fit check (Engine.track_render's fit); each sequence's yield is then a pair, the poses
-    as above and {variant: (frames, n, 6) int32 numpy rows}, row t the fit of the step that wrote pose t."""
+    as above and {variant: (frames, n, 6) int32 numpy rows}, row t the fit of the step that wrote pose t.
+
+    hyp: None, or (S, seed) with S > 1: every step tracks S hypotheses per track (hypothesis_step, the spread of each class's
+    dataset_info; the fit check at `fit`, or FIT_TAU_DEFAULT without it), the poses and fit rows being the kept hypotheses'.
+    Track j of frame t of sequence k draws with hypothesis_key(seq_index[k], t, j); seq_index (default 0, 1, ...) is each
+    sequence's index in the run's sorted list, so a share of the sequences on one GPU draws what the whole run draws."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
     fp8 = {}                                               # checkpoint index -> its first fp8 variant
@@ -1122,6 +1214,11 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
             sink = stack.enter_context(contextlib.closing(VideoSink((max(len(s[2]) for s in sequences), H // 2, W // 2, 3), depth, dev)))
         uploads = stack.enter_context(contextlib.closing(ring.uploads(frames, workers)))
         by_ids, by_n = {}, {}
+        if hyp is not None:
+            S, seed = hyp
+            hyp_tau = fit or FIT_TAU_DEFAULT
+            seq_index = list(range(len(sequences))) if seq_index is None else list(seq_index)
+            hyp_out = {}                                   # per (variant, n): the keys, choices and fit rows, at fixed addresses
         for k, (rgb_files, _, ids, init) in enumerate(sequences):
             n = len(ids)
             for c in _checkpoints(variants):
@@ -1149,6 +1246,18 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                     m, rounds = v[:2]
                     wh, wd, widths = by_ids[ids, _variant_checkpoint(v)]
                     poses, out_trans, out_rot, drawn = by_n[v, n]
+                    if hyp is not None:
+                        if (v, n) not in hyp_out:
+                            hyp_out[v, n] = (torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                                             torch.empty((n, 6), dtype=torch.int32, device=dev))
+                        keys, choice, rows = hyp_out[v, n]
+                        keys.copy_(torch.arange(n, dtype=torch.int64, device=dev) + hypothesis_key(seq_index[k], t, 0))
+                        hypothesis_step(eng, trk, ring.dev['rgb'], ring.dev['depth'], poses, widths, wh, wd, keys,
+                                        hypothesis_groups(trackers, wh), S, seed, hyp_tau, m, rounds,
+                                        dict(out_poses=poses, out_trans=out_trans, out_rot=out_rot, out_choice=choice,
+                                             out_fit=fit_rows[v][t] if fit else rows))
+                        history[v][t].copy_(poses)
+                        continue
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
                                      image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot,
@@ -1247,13 +1356,14 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
                                  render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
 
 
-def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0):
+def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0, hyp=None):
     """One process's share of a one-pass run, sequences[k] for k in mine: the Engine and Trackers of `entries`
     (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
     share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
     [(paths, labels)] per sequence, folders to make once the trackers exist).  fit: _track_sequences' fit (then writes[k] gets
-    its (poses, fit rows) pair).  -> (Engine, {k: what writes[k] returned})."""
-    eng, trackers = _one_pass_trackers(entries, precision, max_batch)
+    its (poses, fit rows) pair).  hyp: _track_sequences' hyp (the Engine then holds max_batch x S tracks per step).
+    -> (Engine, {k: what writes[k] returned})."""
+    eng, trackers = _one_pass_trackers(entries, precision, max_batch * (hyp[0] if hyp else 1))
     for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
         _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
     drawn = None
@@ -1262,7 +1372,7 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
             os.makedirs(d, exist_ok=True)
         drawn = (video[0], [video[1][k] for k in mine])
     out = {}
-    fit_kw = {'fit': fit} if fit else {}
+    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp, 'seq_index': list(mine)} if hyp else {}))
     for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn, **fit_kw), mine):
         fn, *args = writes[k]
         out[k] = fn(*args, tracked)
@@ -1270,7 +1380,7 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
 
 
 def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
-               writes, fit=0):
+               writes, fit=0, hyp=None):
     """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: _track_share with the weight sets of its
     sequences.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error', traceback text) through
     conn."""
@@ -1279,7 +1389,7 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
         wids = _rank_weight_ids(sequences, mine, variants)
         torch.cuda.set_device(device)
         eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
-                                depth, workers, video, writes, fit)
+                                depth, workers, video, writes, fit, hyp)
         conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
     except BaseException:
         conn.send(('error', traceback.format_exc()))
@@ -1306,7 +1416,7 @@ def _agree_fp8_scales(per_rank):
     return {w: s for w, (_, s) in sorted(out.items())}
 
 
-def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0):
+def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0, hyp=None):
     """_track_share over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
     rank (_rank_main) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
     frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
@@ -1330,7 +1440,7 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
             borrowed = borrowed_calibrations(track_sets, mine) if fp8 else {}
             p = ctx.Process(target=_rank_main, name='one-pass rank %d' % r, daemon=True,
                             args=(send, r, devices[r], entries, precision, max_batch, sequences, mine, borrowed, variants, depth,
-                                  workers, video, writes, fit))
+                                  workers, video, writes, fit, hyp))
             try:
                 p.start()
             finally:
@@ -1376,6 +1486,21 @@ FIT_FILE = 'fit.npy'
 FIT_LOST_ADDS = 0.02
 
 
+def _driver_hypotheses(hypotheses, seed, entries):
+    """The drivers' hypotheses / seed -> None for 1, else (S, seed) for _track_sequences; a ValueError for S outside [1, 32], a
+    non-integer seed, or a class / object whose dataset_info spread (max_translation, max_rotation) se3tn_hypothesis_opts refuses."""
+    hyp = _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
+    if hyp.hypotheses == 1:
+        return None
+    for _, label, k in entries:
+        info = k['dataset_info']
+        try:
+            _engine.Engine.hypothesis_spec(hypotheses, seed, info['max_translation'], info['max_rotation'])
+        except (KeyError, TypeError, ValueError) as e:
+            raise ValueError('%s: dataset_info max_translation / max_rotation: %s' % (label, e)) from e
+    return int(hyp.hypotheses), int(seed)
+
+
 def _driver_fit(fit):
     """The drivers' fit argument -> tau in mm, 0 for None (Engine.fit_spec; checked before anything is read)."""
     return _fit_spec(fit)
@@ -1409,17 +1534,17 @@ def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
     return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs)
 
 
-def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0):
+def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0, hyp=None):
     """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
     (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
     sequence k's poses.  With several checkpoints, a run whose weight sets do not fit in free device memory is refused first
     (check_weight_sets_fit; per rank on several GPUs).  -> the driver's return value: _sweep_results of {variant:
     collect(written, variant)}, written being [what writes[k] returned] in sequence order.  fit: every step's fit check
-    (_track_sequences), writes[k] then taking the (poses, fit rows) pair."""
+    (_track_sequences), writes[k] then taking the (poses, fit rows) pair.  hyp: _track_sequences' hyp."""
     keys = tuple(v[:-1] for v in run.variants)
     if run.gpus == 1 and len(run.configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
-    fit_kw = {'fit': fit} if fit else {}
+    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp} if hyp else {}))
     if run.gpus == 1:
         _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
                               writes, **fit_kw)
@@ -1462,7 +1587,7 @@ def _write_ycb_all_sequence_fit(dirs, seq_id, cls, init, tracked):
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1, fit=None):
+                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1501,9 +1626,16 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
 
     fit: tau in mm turns on every step's fit check (Engine.track_render's fit): each class's seq<id>/ of every tree also gets
     FIT_FILE, int32 (pose files, 6), row i the fit of the step that wrote pose i, row 0 -1.  The pose files and the return value
-    are what the run without it gives.  score_fit reads it."""
+    are what the run without it gives.  score_fit reads it.
+
+    hypotheses: S in [1, 32].  S > 1 tracks every step from S start hypotheses per track around its previous pose, spread by its
+    class's dataset_info max_translation / max_rotation, and keeps the one that fits the frame best (Tracker(hypotheses=S),
+    _track_sequences' hyp); the pose files hold the kept poses and FIT_FILE, with fit, the kept rows.  Track j of frame t of
+    sequence k (the run's sorted list) draws with key hypothesis_key(k, t, j) and `seed`, on one GPU or several.  S = 1 is the
+    plain run, file for file."""
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
     fit = _driver_fit(fit)
+    _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
@@ -1540,7 +1672,8 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
             for j, c in enumerate(cls):
                 out[c][seq_id] = pred_poses[key][:, j]
         return out
-    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect, fit)
+    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect, fit,
+                          _driver_hypotheses(hypotheses, seed, entries))
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1629,7 +1762,7 @@ def _write_ycbineoat_video_fit(roots, video, tracked):
 
 
 def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
-                        video=False, iterations=1, gpus=1, fit=None):
+                        video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -1660,10 +1793,12 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     object_config['ckpt_dir'] (and 'mean_std_path') may be lists of templates, one per checkpoint, as in getResultsYcbAll:
     checkpoint i's sets under weight id object index + 32 i, its tree under <outdir>/ckpt<i>/.
 
-    fit: as in getResultsYcbAll; <tree>/<video>/FIT_FILE has one row per pose file, frame 0 included (it is tracked)."""
+    fit: as in getResultsYcbAll; <tree>/<video>/FIT_FILE has one row per pose file, frame 0 included (it is tracked).
+    hypotheses, seed: as in getResultsYcbAll, sequence k being the k-th video of the sorted list."""
     from .eval_ycbineoat import OBJECTS
     run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config)
     fit = _driver_fit(fit)
+    _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
@@ -1688,7 +1823,8 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     trees = {v[:-1]: v[-1] for v in run.variants}
     writes = [(_write_ycbineoat_video_fit if fit else _write_ycbineoat_video, trees, v) for v in sequences]
     return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
-                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)}, fit)
+                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)}, fit,
+                          _driver_hypotheses(hypotheses, seed, entries))
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1758,7 +1894,7 @@ def _recover_summary(errors, add_auc, adds_auc):
 
 
 def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0, precision='bf16x3', iterations=1, max_frames=None,
-                        decode_ahead=4, workers=None, gpus=1):
+                        decode_ahead=4, workers=None, gpus=1, hypotheses=1):
     """Pose recovery from perturbed starts on the YCB-Video key frames, every class in one pass.
 
     The frame loop is `produce_train_pair_data --mode ycbv`'s own (ycbv_pair_steps, random / np.random seeded with `seed`): the same
@@ -1782,10 +1918,18 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
 
     -> {variant: {class id: dict, ..., 'all': dict}}, variant (mode, K) with one checkpoint, (mode, K, checkpoint index) with several.
     Each dict: rows, A_in_cam / B_in_cam (rows, 4, 4), poses (K, rows, 4, 4) after each round, errors (K + 1, rows, 4) (translation
-    mm, rotation degrees, ADD m, ADD-S m; index 0 the start), and summary: K + 1 dicts of _recover_summary (AUCs in [0, 1])."""
+    mm, rotation degrees, ADD m, ADD-S m; index 0 the start), and summary: K + 1 dicts of _recover_summary (AUCs in [0, 1]).
+
+    hypotheses: S in [1, 32].  S > 1 makes every row's step track S hypotheses around its A_in_cam (hypothesis_step: the spread of
+    its class's dataset_info, the fit check at FIT_TAU_DEFAULT, row j of key frame f keyed hypothesis_key(f, j, 0) and `seed`).
+    poses / errors / summary are then hypothesis 0's rounds (an n x S-track step's), and each dict also has 'selected' (the fit's
+    choice) and 'best' (per row the hypothesis with the lowest ADD-S against B_in_cam, the bound any selection rule can reach),
+    each a dict of poses (rows, 4, 4), errors (rows, 4), summary (one _recover_summary), and 'choice' (rows,) for 'selected'
+    and 'best', all at round K."""
     from . import _lib
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
     modes, K = recover_front(precision, iterations, gpus)
+    S = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
     configs = checkpoint_configs(class_config)
     ids = [c for c, _ in ycb_classes(ycb_dir, class_ids)]
     if not ids:
@@ -1798,7 +1942,9 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
                for i, cl in enumerate(per_ckpt) for k in cl]
     if len(configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
-    eng, trackers = _one_pass_trackers(entries, modes[0], max(1, len(ids) * int(num_sample)))
+    if S > 1:
+        _driver_hypotheses(S, seed, entries)
+    eng, trackers = _one_pass_trackers(entries, modes[0], max(1, len(ids) * int(num_sample)) * S)
     _, producers = ycbv_producers(ycb_dir, ids, pair_tpl, eng, workers, mesh_base=base)
     variants = [(m, K) + ((i,) if len(configs) > 1 else ()) for i in range(len(configs)) for m in modes]
     dev = eng.device
@@ -1810,9 +1956,10 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
     trk = trackers[entries[0][0]]
     render = dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw)
     starts, counts, row_set, row_B, rounds = [], [], [], [], {v: [] for v in variants}
+    picked = {v: ([], [], []) for v in variants} if S > 1 else None     # per variant: selected poses, choices, every hypothesis
     by_n, by_cls = {}, {}
-    for owners, chunks, (rgb, depth) in ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True,
-                                                        with_frame=True):
+    for f, (owners, chunks, (rgb, depth)) in enumerate(ycbv_pair_steps(eng, producers, jobs, num_sample, decode_ahead, workers, on_device=True,
+                                                        with_frame=True)):
         cls = tuple(c for c, _, inside, _ in owners for _ in inside)
         n = len(cls)
         if n not in by_n:                                  # per n: the start poses and each variant's outputs, at fixed addresses
@@ -1820,7 +1967,12 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
                        {v: (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
                             torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((K, n, 4, 4), dtype=torch.float64, device=dev))
                         for v in variants})
-        start, outs = by_n[n]
+            if S > 1:
+                by_n[n] += ({v: (torch.empty(n, dtype=torch.int32, device=dev), torch.empty((n, 6), dtype=torch.int32, device=dev),
+                                 torch.empty((n, S, 4, 4), dtype=torch.float64, device=dev),
+                                 torch.empty((K, n, S, 4, 4), dtype=torch.float64, device=dev)) for v in variants},
+                            torch.empty(n, dtype=torch.int64, device=dev))
+        start, outs = by_n[n][:2]
         start.copy_(torch.cat([r['A_in_cam'] for _, r in chunks]))
         counts.append(torch.cat([r['count'] for _, r in chunks]))
         starts.append(start.clone())
@@ -1836,16 +1988,29 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
             if v[0] == 'fp8':                              # sets without scales: calibrated on their own rows of this frame
                 eng.calibrate_fp8_tracks(rgb, depth, trk.K, start, widths, weight_ids=wh, render=dict(render, mesh_ids=wd))
             poses, out_trans, out_rot, out_rounds = outs[v]
+            if S > 1:
+                choice, rows, hyp_poses, hyp_rounds = by_n[n][2][v]
+                keys = by_n[n][3]
+                keys.copy_(torch.arange(n, dtype=torch.int64, device=dev) * (1 << 16) + hypothesis_key(f, 0, 0))
+                hypothesis_step(eng, trk, rgb, depth, start, widths, wh, wd, keys, hypothesis_groups(trackers, wh), S, seed,
+                                FIT_TAU_DEFAULT, v[0], K, dict(out_poses=poses, out_trans=out_trans, out_rot=out_rot, out_choice=choice,
+                                                               out_fit=rows, out_hyp_poses=hyp_poses, out_rounds=hyp_rounds))
+                rounds[v].append(hyp_rounds[:, :, 0].clone())
+                for acc, t in zip(picked[v], (poses, choice, hyp_poses)):
+                    acc.append(t.clone())
+                continue
             eng.track_render(rgb, depth, trk.K, start, widths, trk.trans_normalizer, trk.rot_normalizer, weight_ids_host=wh,
                              weight_ids_dev=wd, precision=v[0], mode=render['mode'], image_hw=render['image_hw'], out_poses=poses,
                              out_trans=out_trans, out_rot=out_rot, iterations=K, out_rounds=out_rounds)
             rounds[v].append(out_rounds.clone())
-    return _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG)
+    return _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG, picked)
 
 
-def _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, min_seg):
+def _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, min_seg, picked=None):
     """recoverYcbKeyframes' scoring, after the last frame: every round of every row in one se3tn_pose_errors_sets launch per round
-    and variant (rows whose count is below min_seg masked), one read-back, then se3tn_vocap_sets per round and metric."""
+    and variant (rows whose count is below min_seg masked), one read-back, then se3tn_vocap_sets per round and metric.  picked:
+    None, or per variant the hypothesis steps' (selected poses, choices, every hypothesis's poses) per frame: the selected rows
+    and every hypothesis are scored the same way, and 'best' takes per row the hypothesis of lowest ADD-S."""
     dev = eng.device
     N = len(row_set)
     S = len(ids)
@@ -1874,12 +2039,40 @@ def _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, ro
         P = per_v[v].index_select(1, kidx).cpu().numpy() if N else np.zeros((K, 0, 4, 4))
         aucs = [(eng.vocap_sets(E[r, :, 2].contiguous(), kset, S), eng.vocap_sets(E[r, :, 3].contiguous(), kset, S)) for r in range(K + 1)]
         Eh = E.cpu().numpy()
+        extra = {}
+        if picked is not None:
+            extra = _score_hypotheses(eng, table, pose_set, offsets, B if N else None, keep if N else None, picked[v], kidx, kset, S)
         res = {}
         for j, c in enumerate(ids + ['all']):
             rows = np.flatnonzero(kset == j) if c != 'all' else np.arange(len(kset))
             res[c] = dict(rows=len(rows), A_in_cam=A_h[rows], B_in_cam=B_h[rows], poses=P[:, rows], errors=Eh[:, rows],
                           summary=[_recover_summary(Eh[r, rows], aucs[r][0][j], aucs[r][1][j]) for r in range(K + 1)])
+            for name, (Pk, Ek, ch, ap) in extra.items():
+                res[c][name] = dict(poses=Pk[rows], errors=Ek[rows], choice=ch[rows],
+                                    summary=_recover_summary(Ek[rows], ap[0][j], ap[1][j]))
         out[v] = res
+    return out
+
+
+def _score_hypotheses(eng, table, pose_set, offsets, B, keep, picked, kidx, kset, n_sets):
+    """recoverYcbKeyframes' two hypothesis rows for one variant: {'selected' | 'best': (poses, errors (rows, 4), choice,
+    (ADD AUCs, ADD-S AUCs))} over the kept rows, 'best' being per row the hypothesis of lowest ADD-S (the first on a tie)."""
+    if B is None:
+        z = (np.zeros((0, 4, 4)), np.zeros((0, 4)), np.zeros(0, np.int32), ([0.0] * (n_sets + 1), [0.0] * (n_sets + 1)))
+        return {'selected': z, 'best': z}
+    sel, choice, every = (torch.cat(x) for x in picked)
+    S = every.shape[1]
+    E_sel = eng.pose_errors_sets(table, pose_set, sel, B, offsets, keep)[0]
+    E_all = eng.pose_errors_sets(table, np.repeat(pose_set, S), every.reshape(-1, 4, 4).contiguous(), B.repeat_interleave(S, 0),
+                                 offsets, keep.repeat_interleave(S, 0))[0].reshape(-1, S, 4)
+    best = torch.nan_to_num(E_all[:, :, 3], nan=float('inf')).argmin(1)
+    rows = torch.arange(len(best), device=best.device)
+    E_best, P_best = E_all[rows, best], every[rows, best]
+    out = {}
+    for name, E, P, ch in (('selected', E_sel, sel, choice.long()), ('best', E_best, P_best, best)):
+        E = E.index_select(0, kidx)
+        ap = (eng.vocap_sets(E[:, 2].contiguous(), kset, n_sets), eng.vocap_sets(E[:, 3].contiguous(), kset, n_sets))
+        out[name] = (P.index_select(0, kidx).cpu().numpy(), E.cpu().numpy(), ch.index_select(0, kidx).cpu().numpy(), ap)
     return out
 
 
@@ -1905,6 +2098,9 @@ def print_recover_tables(results, names):
             s = results[v][c]['summary']
             for r in range(1, len(s)):
                 print(line(str(_variant_checkpoint(v)), v[0], r, s[r]))
+            for name, label in (('selected', 'selected'), ('best', 'best of S')):
+                if name in results[v][c]:
+                    print(line(str(_variant_checkpoint(v)), v[0], len(s) - 1, results[v][c][name]['summary']) + '  ' + label)
 
 
 def score_precisions(results, outdir, ycb_dir, config, YCBInEOAT_dir=None):
@@ -2145,7 +2341,10 @@ def main(argv=None):
     parser.add_argument('--pair_model_path', default=None, help='ycbv_recover: path template of the mesh the perturbed pairs are '
                         'cut with (default --model_path with .ply -> .obj, as ProducerPurturb picks it)')
     parser.add_argument('--num_sample', type=int, default=10, help='ycbv_recover: perturbations drawn per annotated class and key frame')
-    parser.add_argument('--seed', type=int, default=0, help='ycbv_recover: seed of random and np.random before the first draw')
+    parser.add_argument('--seed', type=int, default=0, help='ycbv_recover: seed of random and np.random before the first draw, and '
+                        'of the hypotheses\' draws; ycbv_all / ycbineoat_all: seed of the hypotheses\' draws')
+    parser.add_argument('--hypotheses', type=int, default=None, help='ycbv_all / ycbineoat_all / ycbv_recover: track every step from S '
+                        'start hypotheses per track (1..32, default 1) and keep the one whose model fits the frame best')
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
     parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt)')
     parser.add_argument('--max_frames', type=int, default=None)
@@ -2173,6 +2372,12 @@ def main(argv=None):
             _fit_spec(args.fit)
         except ValueError as e:
             raise SystemExit('--fit %d: %s' % (args.fit, e))
+    if args.hypotheses is not None:
+        if args.hypotheses != 1 and args.mode not in ('ycbv_all', 'ycbineoat_all', 'ycbv_recover'):
+            raise SystemExit('--hypotheses %d needs --mode ycbv_all, ycbineoat_all or ycbv_recover; --mode %s tracks one start per '
+                             'track' % (args.hypotheses, args.mode))
+        if not 1 <= args.hypotheses <= _lib.MAX_HYPOTHESES:
+            raise SystemExit('--hypotheses %d: must be in [1, %d]' % (args.hypotheses, _lib.MAX_HYPOTHESES))
     if args.mode == 'ycbv_recover':
         return _main_recover(args)
     if args.outdir is None:
@@ -2286,6 +2491,8 @@ def cli_recover(args):
         raise SystemExit('--class_ids: %s' % e)
     kw = dict(num_sample=args.num_sample, seed=args.seed, precision=precision or 'bf16x3', iterations=iterations or 1,
               max_frames=args.max_frames)
+    if getattr(args, 'hypotheses', None) is not None:
+        kw['hypotheses'] = args.hypotheses
     return class_ids, config, kw
 
 
@@ -2324,7 +2531,10 @@ def _main_one_pass(args, precision=None, iterations=None):
     except ValueError as e:
         raise SystemExit('--%s: %s' % ('ckpt_dir / --mean_std_path', e))
     kw = {key: v for key, v in (('video', args.video or None), ('precision', precision), ('gpus', args.gpus),
-                                ('iterations', iterations), ('fit', getattr(args, 'fit', None))) if v is not None}
+                                ('iterations', iterations), ('fit', getattr(args, 'fit', None)),
+                                ('hypotheses', getattr(args, 'hypotheses', None))) if v is not None}
+    if 'hypotheses' in kw:
+        kw['seed'] = args.seed
     if ycbv:
         if args.class_ids == 'all':
             class_ids = list(range(1, len(ycb_class_names(args.ycb_dir)) + 1))
