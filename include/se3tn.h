@@ -441,6 +441,62 @@ int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint
                             double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
                             void* stream);
 
+/* ---- depth refinement: point-to-plane ICP of every track against the observed depth, inside the tracking step ---------- */
+
+/* The network's correction is bounded (tanh x normaliser) and as precise as its checkpoint; the step already holds the (filled)
+ * observed depth, the crop windows and a rasteriser.  With ICP on, a render step runs, after the network's last round and before
+ * the fit check, M fixed iterations of projective point-to-plane ICP per track, each render (depth + triangle ids at poses_out,
+ * 2 launches) -> accumulate (1) -> solve (1), all on `stream` and inside the step's one CUDA graph:
+ *   association: every crop pixel u of the render in the crop window of the current pose (se3tn_compute_bbox's window,
+ *     se3tn_crop_bbox's nearest mapping, as the fit check takes it) whose triangle id is >= 0 reads frame pixel p; d_obs = the
+ *     frame's depth there (the filled frame when the step fills), skipped when 0 or p lies outside the frame.  The ray
+ *     r = K^-1 (p_x, p_y, 1) meets the plane of that triangle (unit normal n, posed by the current pose) at q; d_model = 1000 q_z.
+ *     Skipped when |n . r / |r|| < 0.1 (grazing) or d_model <= 0.  Inlier: |d_obs - d_model| <= tau_mm; o = r d_obs / 1000.
+ *   linear system: e = n . (q - o), J = [(q x n)^T, n^T] for the left increment xi = (w, v); per track the upper 21 entries of
+ *     J^T J, J^T e, sum e^2 and the inlier count, summed in a fixed order (bit-reproducible across runs and graph replays).
+ *   solve: Cholesky of J^T J in fp64.  count < min_inliers or a pivot <= 1e-12 x the largest diagonal entry: the pose stays bit
+ *     for bit.  Otherwise xi = -(J^T J)^-1 J^T e, R <- Exp(w) R, t <- Exp(w) t + v (Rodrigues), poses_out updated in place.
+ * Stats row per track, SE3TN_ICP_COLS doubles: inliers, rms_mm (point-to-plane, before the update), step_mm (how far the object's
+ * origin moved), step_deg (the rotation's angle); steps are 0 when the update was skipped.  There is no early exit: the launch
+ * count is the step's + 4 M.  The defaults the Python layer uses (tau 20 mm, min_inliers 100) are starting guesses, not tuned on
+ * a real sensor; whether ICP improves a trained checkpoint's accuracy has not been measured. */
+#define SE3TN_MAX_ICP_ITERATIONS 16
+#define SE3TN_ICP_COLS 4      /* inliers, rms_mm (point-to-plane, before the update), step_mm, step_deg (0 when skipped) */
+typedef struct se3tn_icp_opts {
+    int32_t iterations;       /* 1..SE3TN_MAX_ICP_ITERATIONS */
+    int32_t tau_mm;           /* association gate, 1..1000 */
+    int32_t min_inliers;      /* 6..176*176 */
+    int32_t reserved;         /* 0 */
+} se3tn_icp_opts;             /* 16 bytes, no padding */
+
+/* se3tn_track_render followed by M ICP iterations (above), then the fit check, if on, at the refined pose.  Arguments as
+ * se3tn_track_render, plus:
+ *   icp: the ICP options (HOST, read during the call only), or NULL: exactly se3tn_track_render (same graph, same bits)
+ *   icp_poses double (M, n, 16) device or NULL: slot m - 1 receives every pose after ICP iteration m (round_poses keeps
+ *     recording the network's rounds only)
+ *   out_icp double (n, SE3TN_ICP_COLS) device or NULL: the stats of the last iteration
+ * The ICP render takes context scratch of its own, allocated at max_batch tracks by the first ICP step and never moved:
+ * 176 x 176 x (4 bytes of triangle ids + 2 bytes of depth) per track, plus 256 bytes of sums (about 186 KB a track).
+ * Refused with SE3TN_ERR_INVALID, the field named and nothing queued: what se3tn_track_render refuses, icp fields out of range
+ * or reserved != 0, icp_poses or out_icp overlapping poses_in, poses_out, round_poses or each other, and scratch that cannot be
+ * allocated.  SE3TN_PREC_FP32 queues the same launches without a graph. */
+int se3tn_track_icp(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                    const double* K, const double* poses_in, const double* object_width,
+                    int render_mode, int render_H, int render_W,
+                    const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                    double trans_normalizer, double rot_normalizer, int precision,
+                    float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                    const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream);
+
+/* se3tn_track_render_host with ICP: arguments as se3tn_track_render_host, plus icp (NULL: se3tn_track_render_host exactly) and
+ * out_icp double (n, SE3TN_ICP_COLS) HOST or NULL, brought back in the call's one copy out.  The whole depth frame is uploaded
+ * while ICP is on.  Synchronises `stream`.  Errors as se3tn_track_icp. */
+int se3tn_track_icp_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                         const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                         const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
+                         double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                         const se3tn_icp_opts* icp, double* out_icp, void* stream);
+
 /* ---- multi-hypothesis tracking: several starts per track, the one whose model fits the frame best kept ---------------- */
 
 /* A track that has slipped further than the network was trained to correct stays lost: the network pulls a pose back from

@@ -20,6 +20,8 @@ AUG_PARAMS = 24
 AUG_MAX_CORNERS = 64
 MAX_HYPOTHESES = 32
 HYP_DRAWS = 8
+MAX_ICP_ITERATIONS = 16
+ICP_COLS = 4
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -60,6 +62,10 @@ SIGNATURES = {
                                     _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_track_hypotheses_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
                                          _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_track_icp': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                             _vp, _vp, _vp, _vp]),
+    'se3tn_track_icp_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                                  _vp, _vp, _vp]),
     'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
@@ -109,6 +115,11 @@ class HypothesisOpts(C.Structure):
     """se3tn_hypothesis_opts (include/se3tn.h)."""
     _fields_ = [('hypotheses', C.c_int32), ('reserved', C.c_int32), ('seed', C.c_int64), ('max_translation', _d),
                 ('max_rotation_deg', _d)]
+
+
+class IcpOpts(C.Structure):
+    """se3tn_icp_opts (include/se3tn.h)."""
+    _fields_ = [('iterations', C.c_int32), ('tau_mm', C.c_int32), ('min_inliers', C.c_int32), ('reserved', C.c_int32)]
 
 
 _lib = None

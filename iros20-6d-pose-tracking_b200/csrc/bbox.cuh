@@ -24,4 +24,13 @@ __device__ __forceinline__ void bbox_window(const double* pose, double fx, doubl
     ch = static_cast<int>(fmax(-lim, fmin(lim, vmax))) - top;
 }
 
+// The source row / column cv2 INTER_NEAREST reads for output pixel dst when `size` source pixels are resized to `out`:
+// floor(dst * (1 / (out / size))) in float64, clamped to size - 1 -- as the crop kernels cut B (no meaning for size <= 0).
+__device__ __forceinline__ int nearest_source(int dst, int out, int size)
+{
+    const double inv = size > 0 ? 1.0 / (static_cast<double>(out) / size) : 0.0;
+    const int s = static_cast<int>(floor(dst * inv));
+    return s > size - 1 ? size - 1 : s;
+}
+
 }  // namespace se3tn

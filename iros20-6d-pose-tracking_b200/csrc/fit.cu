@@ -42,13 +42,8 @@ fit_kernel(const FitArgs a)
     const int top = s_win[0], left = s_win[1], ch = s_win[2], cw = s_win[3];
     const bool inside = ch > 0 && cw > 0;
     // the nearest source indices exactly as preprocess_kernel computes them
-    const double ifx = cw > 0 ? 1.0 / (static_cast<double>(kImg) / cw) : 0.0;
-    const double ify = ch > 0 ? 1.0 / (static_cast<double>(kImg) / ch) : 0.0;
-    if (threadIdx.x < kImg) { int sx = static_cast<int>(floor(threadIdx.x * ifx)); if (sx > cw - 1) sx = cw - 1; s_sx[threadIdx.x] = sx; }
-    else if (threadIdx.x >= 256 && threadIdx.x < 256 + kFitRows) {
-        const int ly = threadIdx.x - 256;
-        int sy = static_cast<int>(floor((row0 + ly) * ify)); if (sy > ch - 1) sy = ch - 1; s_sy[ly] = sy;
-    }
+    if (threadIdx.x < kImg) s_sx[threadIdx.x] = nearest_source(threadIdx.x, kImg, cw);
+    else if (threadIdx.x >= 256 && threadIdx.x < 256 + kFitRows) s_sy[threadIdx.x - 256] = nearest_source(row0 + threadIdx.x - 256, kImg, ch);
     __syncthreads();
     const uint16_t* R = a.rendered + (static_cast<size_t>(n) * kImg + row0) * kImg;
     int model = 0, observed = 0, inlier = 0, front = 0, behind = 0, residual = 0;

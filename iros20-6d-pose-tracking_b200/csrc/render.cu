@@ -541,6 +541,7 @@ render_kernel(RenderArgs a)
         const size_t o = (static_cast<size_t>(n) * kRS + orow) * kRS + i;
         if (a.rgb) { a.rgb[o * 3] = static_cast<uint8_t>(r8); a.rgb[o * 3 + 1] = static_cast<uint8_t>(g8); a.rgb[o * 3 + 2] = static_cast<uint8_t>(b8); }
         a.depth[o] = static_cast<uint16_t>(mm);
+        if (a.tri) a.tri[o] = (u.valid && t != 0xFFFFFFFFu) ? static_cast<int32_t>(t) : -1;
     }
 }
 

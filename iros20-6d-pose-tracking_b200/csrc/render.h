@@ -24,6 +24,7 @@ struct RenderArgs {
     int vw, vh;                    // mode 1: camera image size
     uint8_t* rgb;                  // [n][176][176][3], or null: depth only (the fit check of a track step)
     uint16_t* depth;               // [n][176][176] mm, 0 = background
+    int32_t* tri = nullptr;        // [n][176][176] the triangle each pixel shows (depth's layout), -1 = background; or null
 };
 size_t render_uniform_bytes();
 size_t render_projected_bytes_per_vertex();

@@ -10,6 +10,7 @@
 #include <dlfcn.h>
 #include "depth_fill.h"
 #include "fit.h"
+#include "icp.h"
 #include "hypotheses.h"
 #include "storage.cuh"
 
@@ -227,6 +228,13 @@ struct HypKey {
     const double* poses_in; const int64_t* keys; const int32_t* wid_in; const double* width_in;
     double* poses_out; float* trans_out; float* rot_out; int32_t* choice; int32_t* fit_out;
 };
+// se3tn_track_icp[_host]'s depth refinement after the last round (se3tn_icp_opts); all zero when ICP is off, so every other
+// step's key keeps its bytes.
+struct IcpKey {
+    int32_t iterations, tau, min_inliers, pad; // iterations 0: no ICP; pad is always 0
+    double* poses;                             // icp_poses (M x n x 16) or NULL
+    double* stats;                             // out_icp (n x kIcpCols) or NULL
+};
 struct StepKey {
     uint8_t kind, mixed;                       // kStepTrack, kStepEval (se3tn_eval_pairs) or kStepPairs (se3tn_perturb_pairs); the tracks use more than one weight set
     uint8_t fill, fill_extrapolate;            // track step: its se3tn_track_opts fill, all zero when off (zero in a validation step)
@@ -247,6 +255,7 @@ struct StepKey {
     double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render) or NULL
     int32_t* fit_rows;                         // fit_tau > 0: the rows of the fit check, n x kFitCols
     HypKey hyp;                                // track step of se3tn_track_hypotheses[_host]
+    IcpKey icp;                                // track step of se3tn_track_icp[_host]
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -283,6 +292,9 @@ struct se3tn_ctx {
     // se3tn_track_hypotheses' expanded tracks: poses (max_batch x 16), widths, ids, network outputs (max_batch x 3 each); allocated
     // by the first hypothesis step, never moved after
     DevBuf<uint8_t> hyp; size_t hyp_bytes = 0;
+    // se3tn_track_icp's block: the sums (max_batch x kIcpSums doubles), then the ICP render's depth and triangle ids of
+    // max_batch tracks; allocated by the first ICP step, never moved after
+    DevBuf<uint8_t> icp; size_t icp_bytes = 0;
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -1291,6 +1303,38 @@ int reserve_hyp(se3tn_ctx* c, HypScratch* x) {
     return SE3TN_OK;
 }
 
+// se3tn_track_icp's block: sums | the ICP render's depth | its triangle ids, max_batch tracks each.
+size_t icp_sums_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kIcpSums * sizeof(double)); }
+size_t icp_depth_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kImg * kImg * sizeof(uint16_t)); }
+double* icp_sums(se3tn_ctx* c) { return reinterpret_cast<double*>(c->icp.get()); }
+uint16_t* icp_depth(se3tn_ctx* c) { return reinterpret_cast<uint16_t*>(c->icp.get() + icp_sums_bytes(c->max_batch)); }
+int32_t* icp_tri(se3tn_ctx* c) {
+    return reinterpret_cast<int32_t*>(c->icp.get() + icp_sums_bytes(c->max_batch) + icp_depth_bytes(c->max_batch));
+}
+
+static_assert(sizeof(se3tn_icp_opts) == 16, "se3tn_icp_opts is 16 bytes without padding: _lib.IcpOpts mirrors it");
+static_assert(kIcpCols == SE3TN_ICP_COLS, "se3tn_track_icp's out_icp columns");
+// se3tn_icp_opts (NULL: ICP off, st.icp stays zero) checked and written into st.icp, and the block allocated, all before
+// anything is queued: a block that cannot be allocated refuses the call and leaves the context as it was.
+int icp_opts(se3tn_ctx* c, const char* fn, const se3tn_icp_opts* o, Step& st) {
+    if (!o) return SE3TN_OK;
+    const std::string f(fn);
+    if (o->iterations < 1 || o->iterations > SE3TN_MAX_ICP_ITERATIONS)
+        return fail(c, SE3TN_ERR_INVALID, f + ": icp->iterations is " + std::to_string(o->iterations) + ", not in [1, " +
+                    std::to_string(SE3TN_MAX_ICP_ITERATIONS) + "]");
+    if (o->tau_mm < 1 || o->tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": icp->tau_mm must be in [1, 1000]");
+    if (o->min_inliers < 6 || o->min_inliers > kImg * kImg)
+        return fail(c, SE3TN_ERR_INVALID, f + ": icp->min_inliers must be in [6, " + std::to_string(kImg * kImg) + "]");
+    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": icp->reserved must be 0");
+    const size_t bytes = icp_sums_bytes(c->max_batch) + icp_depth_bytes(c->max_batch) + static_cast<size_t>(c->max_batch) * kImg * kImg * sizeof(int32_t);
+    if (grow(c->icp, c->icp_bytes, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, SE3TN_ERR_INVALID, f + ": icp: its scratch (" + std::to_string(bytes) + " bytes) cannot be allocated");
+    }
+    st.icp.iterations = o->iterations; st.icp.tau = o->tau_mm; st.icp.min_inliers = o->min_inliers;
+    return SE3TN_OK;
+}
+
 static_assert(sizeof(se3tn_hypothesis_opts) == 32, "se3tn_hypothesis_opts is 32 bytes without padding: _lib.HypothesisOpts mirrors it");
 static_assert(kHypDraws == SE3TN_HYP_DRAWS, "se3tn_draw_hypotheses' out_draws columns");
 // se3tn_hypothesis_opts checked for n tracks and written into st.hyp's scalars.  step: a tracking call, whose choice needs the
@@ -1530,6 +1574,27 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         }
         ++c->launches;
     }
+    if (st.icp.iterations) {
+        // M ICP iterations at poses_out, each render (depth + triangle ids, into the ICP block) -> accumulate -> solve, the solve
+        // updating poses_out in place.  Every launch is PDL: each reads what the launch before it wrote only after its
+        // griddepcontrol.wait, as the rounds' renders do.  The copies into icp_poses are ordered like round_poses'.
+        RenderArgs ra = render_args(c, K, st.poses_out, st.object_width, st.wid_dev, st.render_mode, st.render_H, st.render_W,
+                                    nullptr, icp_depth(c));
+        ra.tri = icp_tri(c);
+        IcpArgs ia{};
+        ia.poses = st.poses_out; ia.object_width = st.object_width; ia.mesh_ids = st.wid_dev; ia.meshes = c->d_meshes.get();
+        ia.n_meshes = c->mesh_rows; ia.fx = K[0]; ia.fy = K[1]; ia.cx = K[2]; ia.cy = K[3];
+        ia.frame_depth = depth; ia.H = st.H; ia.W = st.W; ia.tri = icp_tri(c); ia.tau = st.icp.tau; ia.min_inliers = st.icp.min_inliers;
+        ia.sums = icp_sums(c); ia.stats = st.icp.stats;
+        for (int it = 0; it < st.icp.iterations; ++it) {
+            CU_TRY(c, launch_render(ra, st.n, s));
+            CU_TRY(c, launch_icp(ia, st.n, s));
+            c->launches += 4;
+            if (st.icp.poses)
+                CU_TRY(c, cudaMemcpyAsync(st.icp.poses + static_cast<size_t>(it) * st.n * 16, st.poses_out,
+                                          sizeof(double) * 16 * static_cast<size_t>(st.n), cudaMemcpyDeviceToDevice, s));
+        }
+    }
     if (st.fit_tau) {
         // the fit check at poses_out: render_project_kernel (PDL) reads the poses the last round's head / pose update wrote only
         // after its griddepcontrol.wait, as a later round's render does, and fit_kernel reads the depth drawn here, the poses and
@@ -1638,6 +1703,56 @@ int eval_pairs_step(se3tn_ctx* c, const char* fn, const uint8_t* rgbA, const uin
     return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
+// se3tn_track_render and se3tn_track_icp: one step that draws input A, with ICP after the rounds when icp is set.
+int track_render_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                      const double* K, const double* poses_in, const double* object_width,
+                      int render_mode, int render_H, int render_W,
+                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                      double tn, double rn, int precision,
+                      float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                      const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream) {
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    Step st{};
+    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
+    bool multi = false;
+    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
+    if (rc) return rc;
+    if (n == 0) return SE3TN_OK;
+    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
+    if (round_poses) {                             // the copies must not write the poses a later round reads
+        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
+        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * st.iterations;
+        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
+            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
+            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
+        }
+    }
+    DeviceGuard guard(c->device);
+    if ((rc = icp_opts(c, fn, icp, st))) return rc;
+    if (icp) {
+        const size_t nn = static_cast<size_t>(n);
+        const char* why = "icp_poses and out_icp must not overlap poses_in, poses_out, round_poses or each other";
+        const std::pair<const void*, size_t> in = {poses_in, nn * 128}, out = {poses_out, nn * 128}, rounds = {round_poses, st.iterations * nn * 128};
+        rc = check_disjoint(c, fn, {{icp_poses, st.icp.iterations * nn * 128}}, {in, out, rounds, {out_icp, nn * kIcpCols * sizeof(double)}}, why);
+        if (!rc) rc = check_disjoint(c, fn, {{out_icp, nn * kIcpCols * sizeof(double)}}, {in, out, rounds}, why);
+        if (rc) return rc;
+    }
+    st.icp.poses = icp ? icp_poses : nullptr; st.icp.stats = icp ? out_icp : nullptr;
+    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    st.round_poses = round_poses;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, static_cast<cudaStream_t>(stream));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1675,37 +1790,21 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
                        double tn, double rn, int precision,
                        float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
                        void* stream) {
-    const char* fn = "se3tn_track_render";
-    const std::string f(fn);
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
-    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
-    RenderSpec r;
-    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    Step st{};
-    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
-    bool multi = false;
-    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
-    if (rc) return rc;
-    if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
-    if (round_poses) {                             // the copies must not write the poses a later round reads
-        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
-        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * st.iterations;
-        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
-            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
-            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
-        }
-    }
-    DeviceGuard guard(c->device);
-    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
-    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
-    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
-    st.round_poses = round_poses;
-    if ((rc = render_into_scratch(c, r, st))) return rc;
-    return run_step(c, st, static_cast<cudaStream_t>(stream));
+    return track_render_step(c, "se3tn_track_render", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
+                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, opts,
+                             round_poses, nullptr, nullptr, nullptr, stream);
+}
+
+int se3tn_track_icp(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
+                    const double* K, const double* poses_in, const double* object_width,
+                    int render_mode, int render_H, int render_W,
+                    const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
+                    double tn, double rn, int precision,
+                    float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
+                    const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream) {
+    return track_render_step(c, "se3tn_track_icp", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
+                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, opts,
+                             round_poses, icp, icp_poses, out_icp, stream);
 }
 
 int se3tn_track_hypotheses(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
@@ -2160,11 +2259,16 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
                     double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit, void* stream,
-                    const int64_t* draw_keys = nullptr, const se3tn_hypothesis_opts* hyp = nullptr, int32_t* out_choice = nullptr) {
+                    const int64_t* draw_keys = nullptr, const se3tn_hypothesis_opts* hyp = nullptr, int32_t* out_choice = nullptr,
+                    const se3tn_icp_opts* icp = nullptr, double* out_icp = nullptr) {
     bool multi = false;
     Step st{};                                     // options and ids are checked before anything is staged or copied
     int rc = track_opts(c, fn, opts, render != nullptr, st);
     if (rc) return rc;
+    if (icp) {                                     // the block is allocated on the context's device before anything is queued
+        DeviceGuard guard(c->device);
+        if ((rc = icp_opts(c, fn, icp, st))) return rc;
+    }
     if (hyp && (rc = hypothesis_opts(c, fn, hyp, draw_keys, n, true, st))) return rc;
     if (!st.fit_tau != !out_fit)
         return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": out_fit is required with opts->fit_tau_mm and must be NULL without it");
@@ -2180,9 +2284,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     if (io.H != H || io.W != W || io.n_cap < n) {
         CU_TRY(c, cudaStreamSynchronize(s));
         const int cap = std::max(n, io.n_cap);
-        const size_t per = 128 + 8 + img * 3 + img * 2 + 8 + 4 + 128 + 12 + 12 + 4 * kFitCols + 4;
+        const size_t per = 128 + 8 + img * 3 + img * 2 + 8 + 4 + 128 + 12 + 12 + 4 * kFitCols + 4 + 8 * kIcpCols;
         c->graphs.clear();                                       // before the buffers are replaced: captured steps hold their addresses
-        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 11 * 256));
+        CU_TRY(c, grow(io.dev, io.dev_bytes, align256(px * 3) + align256(px * 2) + align256(per * cap) + 12 * 256));
         CU_TRY(c, grow(io.pin, io.pin_bytes, px * 5 + per * cap + 4096));
         CU_TRY(c, cudaMemsetAsync(io.dev.get(), 0, io.dev_bytes, s));   // on the caller's stream, ahead of the copies below; frame pixels outside the uploaded windows are never read, keep them defined
         io.H = H; io.W = W; io.n_cap = cap;
@@ -2198,7 +2302,8 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
                  o_key = o_depthA + align256(nn * a_img * 2), o_wid = o_key + (hyp ? align256(nn * 8) : 0), in_bytes = o_wid + align256(nn * 4);
     const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), o_fit = o_ro + align256(nn * 12);
     const size_t o_choice = st.fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
-    const size_t out_bytes = hyp ? o_choice + align256(nn * 4) : o_choice;
+    const size_t o_icp = hyp ? o_choice + align256(nn * 4) : o_choice;      // ICP's stats rows come back last
+    const size_t out_bytes = st.icp.iterations ? o_icp + nn * 8 * kIcpCols : o_icp;
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
     double* d_ow = reinterpret_cast<double*>(d_in + o_ow);
@@ -2211,6 +2316,7 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     float* d_ro = reinterpret_cast<float*>(d_res + o_ro);
     int32_t* d_fit = reinterpret_cast<int32_t*>(d_res + o_fit);
     int32_t* d_choice = reinterpret_cast<int32_t*>(d_res + o_choice);
+    double* d_icp = reinterpret_cast<double*>(d_res + o_icp);
     // ---- the part of the frame the tracks' crop windows touch (K0 reads nothing else) ----
     int y0 = H, y1 = 0, x0 = W, x1 = 0;
     for (int i = 0; i < n; ++i) {
@@ -2227,8 +2333,9 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     // ---- stage through pinned memory, one asynchronous copy per array ----
     // A step that fills the depth reads all of it: OpenCV's bilateral range table is scaled by the min and max of the whole
     // median-filtered image, and extrapolate scans whole columns.  The fit check crops the depth at the windows of the poses the
-    // step computes.  Then the whole depth frame goes up; rgb stays windowed.
-    const bool whole_depth = st.fill || st.fit_tau;
+    // step computes, and ICP associates pixels in the windows of the poses it refines.  Then the whole depth frame goes up; rgb
+    // stays windowed.
+    const bool whole_depth = st.fill || st.fit_tau || st.icp.iterations;
     uint8_t* hp = io.pin.get();
     const int wh = y1 - y0, ww = x1 - x0;
     if (wh > 0 && ww > 0) {
@@ -2271,17 +2378,19 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
         st.out_trans = d_tr; st.out_rot = d_ro; st.poses_out = d_out;
         if (render && (rc = render_into_scratch(c, *render, st))) return rc;
         if (st.fit_tau) st.fit_rows = d_fit;
+        if (st.icp.iterations) st.icp.stats = d_icp;
         rc = run_step(c, st, s);
     }
     if (rc) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
-    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
+    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau || out_icp) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
     memcpy(poses_out, ho, nn * 128);
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
     if (out_fit) memcpy(out_fit, ho + o_fit, nn * 4 * kFitCols);
     if (out_choice) memcpy(out_choice, ho + o_choice, nn * 4);
+    if (out_icp) memcpy(out_icp, ho + o_icp, nn * 8 * kIcpCols);
     return SE3TN_OK;
 }
 }  // namespace
@@ -2310,6 +2419,23 @@ int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16
     if (rc) return rc;
     return track_host_step(c, "se3tn_track_render_host", frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r,
                            weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, out_fit, stream);
+}
+
+int se3tn_track_icp_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
+                         const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
+                         const int32_t* weight_ids, int n, double tn, double rn, int precision,
+                         double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
+                         const se3tn_icp_opts* icp, double* out_icp, void* stream) {
+    const char* fn = "se3tn_track_icp_host";
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument or empty frame");
+    RenderSpec r;
+    const int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    return track_host_step(c, fn, frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r, weight_ids, n, tn, rn,
+                           precision, poses_out, out_trans, out_rot, opts, out_fit, stream, nullptr, nullptr, nullptr, icp,
+                           icp ? out_icp : nullptr);
 }
 
 int se3tn_track_hypotheses_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,

@@ -69,6 +69,7 @@ class Engine:
             self.lib.se3tn_destroy(self._ctx)
             self._ctx = None
             self._fit_rows = None
+            self._icp_rows = None
 
     def __del__(self):
         try:
@@ -274,7 +275,7 @@ class Engine:
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
                      out_poses=None, out_trans=None, out_rot=None, fill_depth=None, iterations=1, out_rounds=None,
-                     fit=None, out_fit=None):
+                     fit=None, out_fit=None, icp=None, out_icp_poses=None, out_icp=None):
         """track_batch with input A rendered inside the step (se3tn_track_render): the models at `poses` are drawn, then
         K0 -> conv stack -> K6, all enqueued on the current stream.  Track i draws mesh weight_ids[i] (mesh 0 without ids).
         mode / image_hw as in render(), fill_depth as in track_batch.  CUDA tensors in and out; nothing is synchronised.
@@ -285,18 +286,26 @@ class Engine:
         r - 1 is what a call with iterations=r returns.  The step with it is a CUDA graph of its own.  fit: tau in mm (fit_spec)
         turns on the fit check of the step (se3tn_track_opts.fit_tau_mm): every track's model is drawn at its new pose and
         compared with the observed depth, and the call returns a fourth value, out_fit: an int32 CUDA tensor (n, 6) of the rows
-        (model, observed, inlier, front, behind, residual), allocated when None and filled on the current stream."""
+        (model, observed, inlier, front, behind, residual), allocated when None and filled on the current stream.  icp (icp_spec):
+        M iterations of point-to-plane ICP against the observed depth after the last round and before the fit check
+        (se3tn_track_icp); the call then also returns the last iteration's stats, a float64 CUDA tensor (n, 4) of inliers,
+        rms_mm, step_mm, step_deg, after the fit rows when the fit is on (out_icp, allocated when None; the step itself writes an
+        Engine-owned block, so its graph is replayed frame after frame).  out_icp_poses: a float64 CUDA tensor (M, n, 4, 4) that
+        receives the poses after every ICP iteration."""
         return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
                            trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
-                           fill_depth, iterations, out_rounds, fit, out_fit)
+                           fill_depth, iterations, out_rounds, fit, out_fit, icp, out_icp_poses, out_icp)
 
     def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
                weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, out_rounds=None,
-               fit=None, out_fit=None):
+               fit=None, out_fit=None, icp=None, out_icp_poses=None, out_icp=None):
         """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
         n = poses.shape[0]
         iterations = self.refine_iterations(iterations)
         tau = self.fit_spec(fit)
+        icp = self.icp_spec(icp)
+        if icp is None and out_icp_poses is not None:
+            raise ValueError('%s: out_icp_poses needs icp' % fn)
         self._check_frame(fn, frame_rgb, frame_depth, poses, object_width, A, n)
         wh = self._host_ids(fn, weight_ids_host, n)
         fill = self.depth_fill_spec(fill_depth)
@@ -311,19 +320,33 @@ class Engine:
         if tau:
             out_fit = torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=self.device) if out_fit is None else out_fit
             self._check_dev('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS))
+        if icp is not None:
+            out_icp = torch.empty(n, _lib.ICP_COLS, dtype=torch.float64, device=self.device) if out_icp is None else out_icp
+            self._check_dev('out_icp', out_icp, torch.float64, (n, _lib.ICP_COLS))
+            if getattr(self, '_icp_rows', None) is None:
+                self._icp_rows = torch.empty(self.max_batch, _lib.ICP_COLS, dtype=torch.float64, device=self.device)
+            if out_icp_poses is not None:
+                self._check_dev('out_icp_poses', out_icp_poses, torch.float64, (icp.iterations, n, 4, 4))
         H, W = frame_depth.shape
         head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
         tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
                 _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), self._track_opts(fill, iterations, tau))
         if render is None:
             rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail, _stream(self.device))
-        else:
+        elif icp is None:
             rc = self.lib.se3tn_track_render(*head, *render, *tail, _ptr(out_rounds), _stream(self.device))
+        else:
+            rc = self.lib.se3tn_track_icp(*head, *render, *tail, _ptr(out_rounds), C.byref(icp), _ptr(out_icp_poses),
+                                          _ptr(self._icp_rows), _stream(self.device))
         _lib.check(rc, self._ctx)
-        if not tau:
-            return out_poses, out_trans, out_rot
-        out_fit.copy_(self._fit_rows_view()[:n])         # the next step overwrites the context's rows
-        return out_poses, out_trans, out_rot, out_fit
+        res = (out_poses, out_trans, out_rot)
+        if tau:
+            out_fit.copy_(self._fit_rows_view()[:n])     # the next step overwrites the context's rows
+            res += (out_fit,)
+        if icp is not None:
+            out_icp.copy_(self._icp_rows[:n])            # the next ICP step overwrites the Engine's rows
+            res += (out_icp,)
+        return res
 
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
                    weight_ids=None, precision='bf16x3', want_residuals=False, fill_depth=None):
@@ -336,22 +359,24 @@ class Engine:
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                           weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None,
-                          iterations=1, fit=None):
+                          iterations=1, fit=None, icp=None):
         """track_host with input A rendered on the device inside the step (se3tn_track_render_host): the previous poses and
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
         without ids); mode / image_hw as in render(); iterations as in track_render (k > 1 uploads the whole frame).  fit as in
         track_render (the whole depth frame is uploaded then): the fit rows come last in what the call returns, an int32 numpy
-        array (n, 6)."""
+        array (n, 6).  icp as in track_render (se3tn_track_icp_host; the whole depth frame is uploaded then): its stats come last,
+        a float64 numpy array (n, 4)."""
         return self._track_host('track_render_host', frame_rgb, frame_depth, K, poses, object_width, (),
                                 self._render_mode(mode, image_hw), trans_normalizer, rot_normalizer, weight_ids, precision,
-                                want_residuals, fill_depth, iterations, fit)
+                                want_residuals, fill_depth, iterations, fit, icp)
 
     def _track_host(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-                    weight_ids, precision, want_residuals, fill_depth, iterations, fit=None):
+                    weight_ids, precision, want_residuals, fill_depth, iterations, fit=None, icp=None):
         """track_host (A = (rgbA, depthA), render None) and track_render_host (A = (), render = _render_mode's triple)."""
         n = int(poses.shape[0])
         iterations = self.refine_iterations(iterations)
         tau = self.fit_spec(fit)
+        icp = self.icp_spec(icp)
         for name, a, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
             if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
                 raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, dt, shape))
@@ -366,14 +391,20 @@ class Engine:
         head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
         tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
                 self._track_opts(fill, iterations, tau))
+        icp_rows = np.empty((n, _lib.ICP_COLS), dtype=np.float64) if icp is not None else None
         if render is None:
             rc = self.lib.se3tn_track_host(*head, *map(_hptr, A), *tail, _stream(self.device))
-        else:
+        elif icp is None:
             rc = self.lib.se3tn_track_render_host(*head, *render, *tail, _hptr(fit_rows), _stream(self.device))
+        else:
+            rc = self.lib.se3tn_track_icp_host(*head, *render, *tail, _hptr(fit_rows), C.byref(icp), _hptr(icp_rows),
+                                               _stream(self.device))
         _lib.check(rc, self._ctx)
         res = (out, tr, ro) if want_residuals else (out,)
         if tau:
             res += (fit_rows,)
+        if icp is not None:
+            res += (icp_rows,)
         return res if len(res) > 1 else out
 
     # ------------------------------------------------------------------ multi-hypothesis tracking
@@ -926,6 +957,31 @@ class Engine:
         if isinstance(fit, (bool, np.bool_)) or not isinstance(fit, (int, np.integer)) or not 1 <= fit <= 1000:
             raise ValueError('fit must be None or an integer tau in mm in [1, 1000], not %r' % (fit,))
         return int(fit)
+
+    # icp_spec's defaults for an integer M: starting guesses (a gate a little wider than a depth sensor's noise at a metre, and
+    # enough pixels for six unknowns to be well determined), not tuned on a real sensor or a trained checkpoint
+    ICP_TAU_DEFAULT = 20
+    ICP_MIN_INLIERS_DEFAULT = 100
+
+    @staticmethod
+    def icp_spec(icp):
+        """The depth refinement of a tracking call as se3tn_icp_opts, or None (off): None / 0 -> None; an integer M in
+        [1, MAX_ICP_ITERATIONS] -> M iterations at tau ICP_TAU_DEFAULT mm and min_inliers ICP_MIN_INLIERS_DEFAULT; a dict with
+        'iterations' and optional 'tau_mm' (1..1000) and 'min_inliers' (6..176*176) sets those fields.  Else a ValueError."""
+        if icp is None or (isinstance(icp, (int, np.integer)) and not isinstance(icp, (bool, np.bool_)) and icp == 0):
+            return None
+        spec = dict(icp) if isinstance(icp, dict) else {'iterations': icp}
+        unknown = set(spec) - {'iterations', 'tau_mm', 'min_inliers'}
+        if unknown:
+            raise ValueError('icp: unknown fields %s' % sorted(unknown))
+        spec.setdefault('tau_mm', Engine.ICP_TAU_DEFAULT)
+        spec.setdefault('min_inliers', Engine.ICP_MIN_INLIERS_DEFAULT)
+        limits = {'iterations': (1, _lib.MAX_ICP_ITERATIONS), 'tau_mm': (1, 1000), 'min_inliers': (6, IMAGE_SIZE * IMAGE_SIZE)}
+        for k, (lo, hi) in limits.items():
+            v = spec.get(k)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+                raise ValueError('icp %s must be an integer in [%d, %d], not %r' % (k, lo, hi, v))
+        return _lib.IcpOpts(iterations=int(spec['iterations']), tau_mm=int(spec['tau_mm']), min_inliers=int(spec['min_inliers']))
 
     @staticmethod
     def _track_opts(fill, iterations, tau):

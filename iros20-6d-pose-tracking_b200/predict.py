@@ -145,7 +145,7 @@ def _as_numpy_pose(p):
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
-                 fill_depth=False, iterations=1, fit=None, hypotheses=1, seed=0):
+                 fill_depth=False, iterations=1, fit=None, hypotheses=1, seed=0, icp=None):
         """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
         tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
         / blur_type (Engine.depth_fill_spec).
@@ -162,10 +162,19 @@ class Tracker:
         check on at FIT_TAU_DEFAULT mm when fit is not given, and needs the CUDA rasteriser as fit does.  last_fit then holds the
         kept rows and last_choice the kept hypotheses.  Hypothesis h of track j in the Tracker's c-th call is drawn with key
         (seed, c, j).  A Tracker that builds its Engine sizes it max_batch x S; a shared Engine must hold n x S tracks per call.
-        S = 1 is the plain step (last_choice stays None)."""
+        S = 1 is the plain step (last_choice stays None).
+        icp: depth refinement after the network's last round (Engine.track_render's icp): None / 0 off, M iterations of
+        point-to-plane ICP at Engine.icp_spec's default gate, or a dict of its fields.  on_track / on_track_batch then leave the
+        last iteration's stats (inliers, rms_mm, step_mm, step_deg per track) in last_icp: numpy on the host route, a float64
+        CUDA tensor on the device route.  Like fit it needs the CUDA rasteriser drawing input A inside the step; it is refused
+        with hypotheses > 1."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
         self.iterations = Engine.refine_iterations(iterations)
+        self.icp = icp if Engine.icp_spec(icp) is not None else None
+        self.last_icp = None
         self.hypotheses = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
+        if self.icp is not None and self.hypotheses > 1:
+            raise ValueError('icp=%r with hypotheses=%d: ICP inside hypothesis steps is not supported' % (icp, self.hypotheses))
         self.seed = int(seed)
         if self.hypotheses > 1 and fit is None:
             fit = True
@@ -233,6 +242,9 @@ class Tracker:
         if self.fit and not isinstance(self.renderer, CudaRenderer):
             raise ValueError('fit=%d draws every model at its new pose inside the tracking step: it needs the CUDA renderer '
                              '(renderer="cuda"), not %r' % (self.fit, self.renderer))
+        if self.icp is not None and not isinstance(self.renderer, CudaRenderer):
+            raise ValueError('icp=%r draws every model at its refined pose inside the tracking step: it needs the CUDA renderer '
+                             '(renderer="cuda"), not %r' % (self.icp, self.renderer))
         self._np_bufs = {}
         self._copy_stream = torch.cuda.Stream(device=self.engine.device)      # _uploads: two staging slots, used alternately
         self._stage_bufs = ({}, {})
@@ -307,7 +319,7 @@ class Tracker:
         Tracker.iterations times."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
-        if (self.iterations > 1 or self.fit) and not fused:
+        if (self.iterations > 1 or self.fit or self.icp is not None) and not fused:
             raise ValueError(self._refine_refusal(rgbA is not None or depthA is not None))
         if fused:
             out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
@@ -346,9 +358,10 @@ class Tracker:
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
-        if (self.iterations > 1 or self.fit) and renderer is None:
+        if (self.iterations > 1 or self.fit or self.icp is not None) and renderer is None:
             raise ValueError(self._refine_refusal(not render))
         self.last_fit = None
+        self.last_icp = None
         self.last_choice = None
         hyp = None
         if self.hypotheses > 1:                       # (c << 32) + j: track j's draw key in this call
@@ -380,7 +393,10 @@ class Tracker:
             if renderer is not None:
                 out = self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
-                                                    fit=self.fit, **kw)
+                                                    fit=self.fit, icp=self.icp, **kw)
+                if self.icp is not None:
+                    *out, self.last_icp = out
+                    out = out[0] if len(out) == 1 else tuple(out)
                 if self.fit:
                     out, self.last_fit = out
                 return out
@@ -423,10 +439,12 @@ class Tracker:
             elif renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
                 res = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
-                                               fit=self.fit, **kw)
+                                               fit=self.fit, icp=self.icp, **kw)
                 out = res[0]
                 if self.fit:
                     self.last_fit = res[3]
+                if self.icp is not None:
+                    self.last_icp = res[-1]
             else:
                 out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
                                                     self.trans_normalizer, self.rot_normalizer, **kw)
@@ -437,7 +455,8 @@ class Tracker:
         cannot stand in for."""
         why = 'input A was passed in' if given else 'the renderer cannot draw input A inside the tracking step (_fused_renderer)'
         needs = (['iterations=%d redraws input A at each refined pose' % self.iterations] if self.iterations > 1 else []) + \
-                (['fit=%d draws every model at its new pose' % self.fit] if self.fit else [])
+                (['fit=%d draws every model at its new pose' % self.fit] if self.fit else []) + \
+                (['icp=%r draws every model at its refined pose' % (self.icp,)] if self.icp is not None else [])
         return '%s, but %s' % (' and '.join(needs), why)
 
     def _weight_ids(self, weight_ids, n):
@@ -1152,7 +1171,7 @@ def hypothesis_step(eng, trk, rgb, depth, poses, widths, wh, wd, keys, groups, S
             outs[k].index_copy_(1 if k == 'out_rounds' else 0, di, v)
 
 
-def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0, hyp=None, seq_index=None):
+def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0, hyp=None, seq_index=None, icp=None):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
     variants: what every frame is tracked in (a tuple) as _sweep_variants keys them, (mode, k) or (mode, k, c): precision mode, k
@@ -1181,7 +1200,10 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     hyp: None, or (S, seed) with S > 1: every step tracks S hypotheses per track (hypothesis_step, the spread of each class's
     dataset_info; the fit check at `fit`, or FIT_TAU_DEFAULT without it), the poses and fit rows being the kept hypotheses'.
     Track j of frame t of sequence k draws with hypothesis_key(seq_index[k], t, j); seq_index (default 0, 1, ...) is each
-    sequence's index in the run's sorted list, so a share of the sequences on one GPU draws what the whole run draws."""
+    sequence's index in the run's sorted list, so a share of the sequences on one GPU draws what the whole run draws.
+
+    icp: None, or Engine.icp_spec's dict: every step refines its tracks with ICP after the last round (Engine.track_render's
+    icp); the poses and, with fit, the fit rows are those after ICP.  Not combined with hyp (_driver_icp refuses it)."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
     fp8 = {}                                               # checkpoint index -> its first fp8 variant
@@ -1261,7 +1283,8 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                     eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
                                      weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
                                      image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot,
-                                     iterations=rounds, **({'fit': fit, 'out_fit': fit_rows[v][t]} if fit else {}))
+                                     iterations=rounds, **({'fit': fit, 'out_fit': fit_rows[v][t]} if fit else {}),
+                                     **({'icp': icp} if icp else {}))
                     history[v][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
@@ -1356,13 +1379,14 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
                                  render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
 
 
-def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0, hyp=None):
+def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0, hyp=None,
+                 icp=None):
     """One process's share of a one-pass run, sequences[k] for k in mine: the Engine and Trackers of `entries`
     (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
     share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
     [(paths, labels)] per sequence, folders to make once the trackers exist).  fit: _track_sequences' fit (then writes[k] gets
-    its (poses, fit rows) pair).  hyp: _track_sequences' hyp (the Engine then holds max_batch x S tracks per step).
-    -> (Engine, {k: what writes[k] returned})."""
+    its (poses, fit rows) pair).  hyp: _track_sequences' hyp (the Engine then holds max_batch x S tracks per step).  icp:
+    _track_sequences' icp.  -> (Engine, {k: what writes[k] returned})."""
     eng, trackers = _one_pass_trackers(entries, precision, max_batch * (hyp[0] if hyp else 1))
     for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
         _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
@@ -1372,7 +1396,7 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
             os.makedirs(d, exist_ok=True)
         drawn = (video[0], [video[1][k] for k in mine])
     out = {}
-    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp, 'seq_index': list(mine)} if hyp else {}))
+    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp, 'seq_index': list(mine)} if hyp else {}), **({'icp': icp} if icp else {}))
     for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn, **fit_kw), mine):
         fn, *args = writes[k]
         out[k] = fn(*args, tracked)
@@ -1380,7 +1404,7 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
 
 
 def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
-               writes, fit=0, hyp=None):
+               writes, fit=0, hyp=None, icp=None):
     """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: _track_share with the weight sets of its
     sequences.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error', traceback text) through
     conn."""
@@ -1389,7 +1413,7 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
         wids = _rank_weight_ids(sequences, mine, variants)
         torch.cuda.set_device(device)
         eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
-                                depth, workers, video, writes, fit, hyp)
+                                depth, workers, video, writes, fit, hyp, icp)
         conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
     except BaseException:
         conn.send(('error', traceback.format_exc()))
@@ -1416,7 +1440,7 @@ def _agree_fp8_scales(per_rank):
     return {w: s for w, (_, s) in sorted(out.items())}
 
 
-def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0, hyp=None):
+def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0, hyp=None, icp=None):
     """_track_share over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
     rank (_rank_main) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
     frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
@@ -1440,7 +1464,7 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
             borrowed = borrowed_calibrations(track_sets, mine) if fp8 else {}
             p = ctx.Process(target=_rank_main, name='one-pass rank %d' % r, daemon=True,
                             args=(send, r, devices[r], entries, precision, max_batch, sequences, mine, borrowed, variants, depth,
-                                  workers, video, writes, fit, hyp))
+                                  workers, video, writes, fit, hyp, icp))
             try:
                 p.start()
             finally:
@@ -1484,6 +1508,21 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
 FIT_FILE = 'fit.npy'
 # --score's fit table: a frame whose ADD-S is at least this far from the annotation counts as lost (a fixed bound, not an option)
 FIT_LOST_ADDS = 0.02
+
+
+def _driver_icp(icp, icp_tau=None, hypotheses=1):
+    """The drivers' icp (M iterations, 0 / None: off) and icp_tau (the gate in mm, None: Engine.ICP_TAU_DEFAULT) -> None, or the
+    dict Engine.icp_spec takes; a ValueError for values it refuses, icp_tau without icp, or icp with hypotheses > 1 (ICP inside
+    hypothesis steps is not supported).  Checked before anything is read."""
+    if not icp:
+        if icp_tau is not None:
+            raise ValueError('icp_tau %r without icp: the gate of ICP iterations that do not run' % (icp_tau,))
+        return None
+    spec = {'iterations': icp} if icp_tau is None else {'iterations': icp, 'tau_mm': icp_tau}
+    _engine.Engine.icp_spec(spec)
+    if hypotheses != 1:
+        raise ValueError('icp %r with hypotheses %r: ICP inside hypothesis steps is not supported' % (icp, hypotheses))
+    return spec
 
 
 def _driver_hypotheses(hypotheses, seed, entries):
@@ -1534,17 +1573,17 @@ def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
     return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs)
 
 
-def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0, hyp=None):
+def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0, hyp=None, icp=None):
     """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
     (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
     sequence k's poses.  With several checkpoints, a run whose weight sets do not fit in free device memory is refused first
     (check_weight_sets_fit; per rank on several GPUs).  -> the driver's return value: _sweep_results of {variant:
     collect(written, variant)}, written being [what writes[k] returned] in sequence order.  fit: every step's fit check
-    (_track_sequences), writes[k] then taking the (poses, fit rows) pair.  hyp: _track_sequences' hyp."""
+    (_track_sequences), writes[k] then taking the (poses, fit rows) pair.  hyp, icp: _track_sequences' hyp and icp."""
     keys = tuple(v[:-1] for v in run.variants)
     if run.gpus == 1 and len(run.configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
-    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp} if hyp else {}))
+    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp} if hyp else {}), **({'icp': icp} if icp else {}))
     if run.gpus == 1:
         _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
                               writes, **fit_kw)
@@ -1587,7 +1626,7 @@ def _write_ycb_all_sequence_fit(dirs, seq_id, cls, init, tracked):
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0):
+                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1632,10 +1671,15 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     class's dataset_info max_translation / max_rotation, and keeps the one that fits the frame best (Tracker(hypotheses=S),
     _track_sequences' hyp); the pose files hold the kept poses and FIT_FILE, with fit, the kept rows.  Track j of frame t of
     sequence k (the run's sorted list) draws with key hypothesis_key(k, t, j) and `seed`, on one GPU or several.  S = 1 is the
-    plain run, file for file."""
+    plain run, file for file.
+
+    icp: M iterations of ICP after every step's last round (Engine.track_render's icp), at the gate icp_tau mm
+    (Engine.ICP_TAU_DEFAULT when None); the pose files hold the refined poses and FIT_FILE, with fit, the fit after ICP.  0 is the
+    plain run, file for file; several GPUs write the one-GPU trees.  Refused with hypotheses > 1 (_driver_icp)."""
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
     fit = _driver_fit(fit)
     _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
+    icp = _driver_icp(icp, icp_tau, hypotheses)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
         raise ValueError('initialize_method must be gt, posecnn or poserbpf')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
@@ -1673,7 +1717,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                 out[c][seq_id] = pred_poses[key][:, j]
         return out
     return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect, fit,
-                          _driver_hypotheses(hypotheses, seed, entries))
+                          _driver_hypotheses(hypotheses, seed, entries), icp)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1762,7 +1806,7 @@ def _write_ycbineoat_video_fit(roots, video, tracked):
 
 
 def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3', max_frames=None, decode_ahead=4, ycb_dir=None,
-                        video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0):
+                        video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None):
     """predictSequenceYcbInEOAT for every video under ycbineoat_dir in one pass -> {video: (frames,4,4) poses}, and
     <outdir>/<video>/%07d.txt for each frame, which eval_ycbineoat.eval_all scores with res_dir = outdir + '/'.
 
@@ -1794,11 +1838,13 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     checkpoint i's sets under weight id object index + 32 i, its tree under <outdir>/ckpt<i>/.
 
     fit: as in getResultsYcbAll; <tree>/<video>/FIT_FILE has one row per pose file, frame 0 included (it is tracked).
-    hypotheses, seed: as in getResultsYcbAll, sequence k being the k-th video of the sorted list."""
+    hypotheses, seed: as in getResultsYcbAll, sequence k being the k-th video of the sorted list.
+    icp, icp_tau: as in getResultsYcbAll."""
     from .eval_ycbineoat import OBJECTS
     run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config)
     fit = _driver_fit(fit)
     _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
+    icp = _driver_icp(icp, icp_tau, hypotheses)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
@@ -1824,7 +1870,7 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     writes = [(_write_ycbineoat_video_fit if fit else _write_ycbineoat_video, trees, v) for v in sequences]
     return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
                           lambda written, key: {v: w[key] for v, w in zip(sequences, written)}, fit,
-                          _driver_hypotheses(hypotheses, seed, entries))
+                          _driver_hypotheses(hypotheses, seed, entries), icp)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1894,7 +1940,7 @@ def _recover_summary(errors, add_auc, adds_auc):
 
 
 def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0, precision='bf16x3', iterations=1, max_frames=None,
-                        decode_ahead=4, workers=None, gpus=1, hypotheses=1):
+                        decode_ahead=4, workers=None, gpus=1, hypotheses=1, icp=0, icp_tau=None):
     """Pose recovery from perturbed starts on the YCB-Video key frames, every class in one pass.
 
     The frame loop is `produce_train_pair_data --mode ycbv`'s own (ycbv_pair_steps, random / np.random seeded with `seed`): the same
@@ -1925,11 +1971,18 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
     poses / errors / summary are then hypothesis 0's rounds (an n x S-track step's), and each dict also has 'selected' (the fit's
     choice) and 'best' (per row the hypothesis with the lowest ADD-S against B_in_cam, the bound any selection rule can reach),
     each a dict of poses (rows, 4, 4), errors (rows, 4), summary (one _recover_summary), and 'choice' (rows,) for 'selected'
-    and 'best', all at round K."""
+    and 'best', all at round K.
+
+    icp: M > 0 refines every row with M ICP iterations after round K in the same step (Engine.track_render's icp, gate icp_tau mm,
+    Engine.ICP_TAU_DEFAULT when None; refused with hypotheses > 1).  poses / errors / summary then run on past round K: entries
+    K + 1 .. K + M are the poses after ICP iterations 1 .. M (out_icp_poses), and each dict has 'icp': M.  Rounds 0 .. K are
+    those of the run without it, bit for bit."""
     from . import _lib
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
     modes, K = recover_front(precision, iterations, gpus)
     S = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
+    icp = _driver_icp(icp, icp_tau, hypotheses)
+    M = icp['iterations'] if icp else 0
     configs = checkpoint_configs(class_config)
     ids = [c for c, _ in ycb_classes(ycb_dir, class_ids)]
     if not ids:
@@ -1965,7 +2018,7 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
         if n not in by_n:                                  # per n: the start poses and each variant's outputs, at fixed addresses
             by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
                        {v: (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
-                            torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((K, n, 4, 4), dtype=torch.float64, device=dev))
+                            torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((K + M, n, 4, 4), dtype=torch.float64, device=dev))
                         for v in variants})
             if S > 1:
                 by_n[n] += ({v: (torch.empty(n, dtype=torch.int32, device=dev), torch.empty((n, 6), dtype=torch.int32, device=dev),
@@ -1999,11 +2052,18 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
                 for acc, t in zip(picked[v], (poses, choice, hyp_poses)):
                     acc.append(t.clone())
                 continue
+            # the network's rounds, then (with icp) the poses after each ICP iteration, in one (K + M, n) block
             eng.track_render(rgb, depth, trk.K, start, widths, trk.trans_normalizer, trk.rot_normalizer, weight_ids_host=wh,
                              weight_ids_dev=wd, precision=v[0], mode=render['mode'], image_hw=render['image_hw'], out_poses=poses,
-                             out_trans=out_trans, out_rot=out_rot, iterations=K, out_rounds=out_rounds)
+                             out_trans=out_trans, out_rot=out_rot, iterations=K, out_rounds=out_rounds[:K],
+                             **(dict(icp=icp, out_icp_poses=out_rounds[K:]) if icp else {}))
             rounds[v].append(out_rounds.clone())
-    return _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG, picked)
+    out = _score_recovery(eng, trackers, ids, variants, K + M, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG, picked)
+    if M:
+        for res in out.values():
+            for d in res.values():
+                d['icp'] = M
+    return out
 
 
 def _score_recovery(eng, trackers, ids, variants, K, starts, counts, row_set, row_B, rounds, min_seg, picked=None):
@@ -2086,8 +2146,8 @@ def print_recover_tables(results, names):
 
     def line(ckpt, mode, r, s):
         if s['rows'] == 0:
-            return '%-5s %-8s %5d %6d' % (ckpt, mode, r, 0)
-        return '%-5s %-8s %5d %6d %8.3f %8.3f %9.4g %9.4g %9.4g %9.4g' % (ckpt, mode, r, s['rows'], 100 * s['add_auc'], 100 * s['adds_auc'],
+            return '%-5s %-8s %5s %6d' % (ckpt, mode, r, 0)
+        return '%-5s %-8s %5s %6d %8.3f %8.3f %9.4g %9.4g %9.4g %9.4g' % (ckpt, mode, r, s['rows'], 100 * s['add_auc'], 100 * s['adds_auc'],
                                                                        s['rot_mean'], s['rot_median'], s['trans_mean'], s['trans_median'])
     for c in first:
         label = 'all classes' if c == 'all' else 'class %d (%s)' % (c, names.get(c, c))
@@ -2096,8 +2156,9 @@ def print_recover_tables(results, names):
         print(line('-', 'start', 0, first[c]['summary'][0]))
         for v in variants:
             s = results[v][c]['summary']
+            K = len(s) - 1 - results[v][c].get('icp', 0)                 # rows past round K: 'icp 1' .. 'icp M'
             for r in range(1, len(s)):
-                print(line(str(_variant_checkpoint(v)), v[0], r, s[r]))
+                print(line(str(_variant_checkpoint(v)), v[0], r if r <= K else 'icp %d' % (r - K), s[r]))
             for name, label in (('selected', 'selected'), ('best', 'best of S')):
                 if name in results[v][c]:
                     print(line(str(_variant_checkpoint(v)), v[0], len(s) - 1, results[v][c][name]['summary']) + '  ' + label)
@@ -2362,6 +2423,11 @@ def main(argv=None):
                         'from K = 1')
     parser.add_argument('--fit', type=int, default=None, help='ycbv_all / ycbineoat_all: check every step\'s fit, tau in mm '
                         '(1..1000): each sequence folder gets fit.npy beside its pose files, and --score adds the fit table')
+    parser.add_argument('--icp', type=int, default=None, help='ycbv_all / ycbineoat_all / ycbv_recover: refine every track with M '
+                        'iterations of point-to-plane ICP against the depth after the last round (0..16, default 0: off); '
+                        'ycbv_recover adds rows icp 1 .. icp M after round K')
+    parser.add_argument('--icp_tau', type=int, default=None, help='with --icp: the association gate in mm (1..1000, default %d, a '
+                        'starting guess)' % _engine.Engine.ICP_TAU_DEFAULT)
     parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
                         'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
@@ -2378,6 +2444,16 @@ def main(argv=None):
                              'track' % (args.hypotheses, args.mode))
         if not 1 <= args.hypotheses <= _lib.MAX_HYPOTHESES:
             raise SystemExit('--hypotheses %d: must be in [1, %d]' % (args.hypotheses, _lib.MAX_HYPOTHESES))
+    if args.icp is not None or args.icp_tau is not None:
+        if args.mode not in ('ycbv_all', 'ycbineoat_all', 'ycbv_recover'):
+            raise SystemExit('--icp / --icp_tau need --mode ycbv_all, ycbineoat_all or ycbv_recover; --mode %s does not refine '
+                             'with ICP' % args.mode)
+        if args.icp is not None and args.icp < 0:
+            raise SystemExit('--icp %d: must be in [0, %d]' % (args.icp, _lib.MAX_ICP_ITERATIONS))
+        try:
+            _driver_icp(args.icp, args.icp_tau, args.hypotheses if args.hypotheses is not None else 1)
+        except ValueError as e:
+            raise SystemExit('--icp %s --icp_tau %s: %s' % (args.icp, args.icp_tau, e))
     if args.mode == 'ycbv_recover':
         return _main_recover(args)
     if args.outdir is None:
@@ -2493,6 +2569,9 @@ def cli_recover(args):
               max_frames=args.max_frames)
     if getattr(args, 'hypotheses', None) is not None:
         kw['hypotheses'] = args.hypotheses
+    for key in ('icp', 'icp_tau'):
+        if getattr(args, key, None) is not None:
+            kw[key] = getattr(args, key)
     return class_ids, config, kw
 
 
@@ -2532,7 +2611,8 @@ def _main_one_pass(args, precision=None, iterations=None):
         raise SystemExit('--%s: %s' % ('ckpt_dir / --mean_std_path', e))
     kw = {key: v for key, v in (('video', args.video or None), ('precision', precision), ('gpus', args.gpus),
                                 ('iterations', iterations), ('fit', getattr(args, 'fit', None)),
-                                ('hypotheses', getattr(args, 'hypotheses', None))) if v is not None}
+                                ('hypotheses', getattr(args, 'hypotheses', None)), ('icp', getattr(args, 'icp', None)),
+                                ('icp_tau', getattr(args, 'icp_tau', None))) if v is not None}
     if 'hypotheses' in kw:
         kw['seed'] = args.seed
     if ycbv:
