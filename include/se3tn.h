@@ -327,12 +327,73 @@ enum { SE3TN_BLUR_BILATERAL = 0, SE3TN_BLUR_GAUSSIAN = 1 };
 int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, double max_depth, int extrapolate, int blur_type,
                         uint16_t* out_mm, float* out_m, void* stream);
 
+/* ---- depth refinement: point-to-plane ICP of every track against the observed depth, inside the tracking step ---------- */
+
+/* The network's correction is bounded (tanh x normaliser) and as precise as its checkpoint; the step already holds the (filled)
+ * observed depth, the crop windows and a rasteriser.  With ICP on (se3tn_track_opts.icp), a render step runs, after the network's
+ * last round and before the fit check, M fixed iterations of projective point-to-plane ICP per track, each render (depth +
+ * triangle ids at poses_out, 2 launches) -> accumulate (1) -> solve (1), all on `stream` and inside the step's one CUDA graph:
+ *   association: every crop pixel u of the render in the crop window of the current pose (se3tn_compute_bbox's window,
+ *     se3tn_crop_bbox's nearest mapping, as the fit check takes it) whose triangle id is >= 0 reads frame pixel p; d_obs = the
+ *     frame's depth there (the filled frame when the step fills), skipped when 0 or p lies outside the frame.  The ray
+ *     r = K^-1 (p_x, p_y, 1) meets the plane of that triangle (unit normal n, posed by the current pose) at q; d_model = 1000 q_z.
+ *     Skipped when |n . r / |r|| < 0.1 (grazing) or d_model <= 0.  Inlier: |d_obs - d_model| <= tau_mm; o = r d_obs / 1000.
+ *   linear system: e = n . (q - o), J = [(q x n)^T, n^T] for the left increment xi = (w, v); per track the upper 21 entries of
+ *     J^T J, J^T e, sum e^2 and the inlier count, summed in a fixed order (bit-reproducible across runs and graph replays).
+ *   solve: Cholesky of J^T J in fp64.  count < min_inliers or a pivot <= 1e-12 x the largest diagonal entry: the pose stays bit
+ *     for bit.  Otherwise xi = -(J^T J)^-1 J^T e, R <- Exp(w) R, t <- Exp(w) t + v (Rodrigues), poses_out updated in place.
+ * Stats row per track, SE3TN_ICP_COLS doubles: inliers, rms_mm (point-to-plane, before the update), step_mm (how far the object's
+ * origin moved), step_deg (the rotation's angle); steps are 0 when the update was skipped.  There is no early exit: the launch
+ * count is the step's + 4 M.  The ICP render takes context scratch of its own, allocated at max_batch tracks by the first ICP
+ * step and never moved: 176 x 176 x (4 bytes of triangle ids + 2 bytes of depth) per track, plus 256 bytes of sums (about
+ * 186 KB a track).  The defaults the Python layer uses (tau 20 mm, min_inliers 100) are starting guesses, not tuned on a real
+ * sensor; whether ICP improves a trained checkpoint's accuracy has not been measured. */
+#define SE3TN_MAX_ICP_ITERATIONS 16
+#define SE3TN_ICP_COLS 4      /* inliers, rms_mm (point-to-plane, before the update), step_mm, step_deg (0 when skipped) */
+typedef struct se3tn_icp_opts {
+    int32_t iterations;       /* 1..SE3TN_MAX_ICP_ITERATIONS */
+    int32_t tau_mm;           /* association gate, 1..1000 */
+    int32_t min_inliers;      /* 6..176*176 */
+    int32_t reserved;         /* 0 */
+} se3tn_icp_opts;             /* 16 bytes, no padding */
+
+/* ---- multi-hypothesis tracking: several starts per track, the one whose model fits the frame best kept ---------------- */
+
+/* A track that has slipped further than the network was trained to correct stays lost: the network pulls a pose back from
+ * perturbations up to dataset_info's max_translation / max_rotation (reference produce_train_pair_data.py:90-110).  A hypothesis
+ * step (se3tn_track_opts.hyp) looks around the previous pose instead of only at it.  For each of n tracks it
+ *   1. draws S - 1 start poses around the previous pose P: hypothesis h >= 1 is P . inv(D), D = random_gaussian_magnitude(
+ *      max_translation, max_rotation_deg) (reference Utils.py:372-404), composed as produce_train_pair_data.py:110 composes a
+ *      training pair (A_in_cam = B_in_cam . inv(B_in_A)); hypothesis 0 is P itself;
+ *   2. refines all n x S starts as one n x S-track render step (the options' fill, k rounds and fit check);
+ *   3. keeps, per track, the hypothesis whose fit row has the highest inlier fraction inlier / model (compared exactly as int64
+ *      cross products; model = 0 ranks last), then the lowest mean inlier residual residual / inlier (inlier = 0 ranks last),
+ *      then the lowest h.  A frame without depth leaves every inlier count at 0 and keeps hypothesis 0 as long as hypothesis 0's
+ *      model covers a pixel of its window (model > 0); when it covers none, the first h >= 1 whose model does wins.
+ * Rows are track-major: track i's hypothesis h is row i S + h of every n x S array.  Draws: Philox4x32-10 (the generator of
+ * se3tn_augment), key = seed, counter = (draw_keys[i] low word, high word, h, slot).  Each of the translation and the rotation
+ * takes a direction from random_direction (theta = 2 pi U, phi = acos(2 U - 1)) and a magnitude from N(0, max), redrawn until
+ * |m| <= max as the reference does, at most 64 times; a magnitude that never lands inside (probability ~1e-32) is clamped to +-max.
+ * The rotation is cv2.Rodrigues of axis / |axis| * m / 180 * pi in fp64.  The draws depend on (seed, draw key, h) alone: not on
+ * n, the precision, the route or anything else in the step.  S = 1 draws nothing and is the plain render step bit for bit.
+ * Whether more hypotheses track better on a trained checkpoint has not been measured (README). */
+#define SE3TN_MAX_HYPOTHESES 32
+#define SE3TN_HYP_DRAWS 8     /* se3tn_draw_hypotheses' out_draws columns (below) */
+typedef struct se3tn_hypothesis_opts {
+    int32_t hypotheses, reserved;                  /* S in [1, SE3TN_MAX_HYPOTHESES]; reserved 0                            */
+    int64_t seed;                                  /* the Philox key                                                         */
+    double max_translation, max_rotation_deg;      /* metres, finite, in (0, 1]; degrees, in (0, 180]                        */
+} se3tn_hypothesis_opts;                           /* 32 bytes, no padding                                                   */
+
+/* ---- a tracking call's options and optional per-step arrays --------------------------------------------------------- */
+
 /* Options of one tracking call (se3tn_track_batch, _render, _host, _render_host), passed by pointer; NULL means the defaults: no
- * fill, one round, no fit check.  Every field is part of what makes two steps the same (se3tn_last_step_was_graph).  The call
- * reads nothing of it after it returns, and the context keeps no option from one call to the next.  Refused with
- * SE3TN_ERR_INVALID, the field named and nothing queued: a value outside the ranges below, reserved != 0, and, in
- * se3tn_track_batch / se3tn_track_host, iterations != 1 or fit_tau_mm != 0 (they take input A from the caller: a later round
- * cannot redraw it, and a weight id need not have a mesh for the fit check to draw).
+ * fill, one round, no fit check, no ICP, no hypotheses.  Every field, and every field of what icp and hyp point to, is part of
+ * what makes two steps the same (se3tn_last_step_was_graph).  The call reads nothing of it after it returns, and the context
+ * keeps no option from one call to the next.  Refused with SE3TN_ERR_INVALID, the field named and nothing queued: a value
+ * outside the ranges below, reserved != 0, icp and hyp together (ICP inside a hypothesis step is not supported), and, in
+ * se3tn_track_batch / se3tn_track_host, iterations != 1, fit_tau_mm != 0, icp or hyp (they take input A from the caller: a later
+ * round, ICP or a hypothesis cannot redraw it, and a weight id need not have a mesh for the fit check or ICP to draw).
  *
  * fill_depth != 0: fill the observed depth inside the step: fill_depth(frame_depth) exactly as se3tn_fill_depth_ex computes it
  * with fill_max_depth, fill_extrapolate (0 or not) and fill_blur (SE3TN_BLUR_*), with the same kernels, into context-owned
@@ -358,11 +419,11 @@ int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, 
  * scores them against the annotations of the YCB-Video key frames (README).
  *
  * fit_tau_mm = tau in [1, 1000]: check how well every track fits its frame (se3tn_track_render[_host]); 0 turns the check off.
- * After the last round the step draws each track's model at poses_out (the same mesh, mode, camera size and object width as the
- * rounds, depth only, into scratch of its own: the step's input A keeps the last round's) and compares the rendered depth R with
- * the observed depth O in the crop window of poses_out, cropped exactly as K0 crops input B (se3tn_compute_bbox's window,
- * se3tn_crop_bbox's nearest mapping, 0 outside the image; the filled frame when the step fills the depth).  R and O are uint16
- * mm before any clipping.  Track i's row, SE3TN_FIT_COLS int32 over its 176 x 176 pixels:
+ * After the last round (and ICP) the step draws each track's model at poses_out (the same mesh, mode, camera size and object
+ * width as the rounds, depth only, into scratch of its own: the step's input A keeps the last round's) and compares the rendered
+ * depth R with the observed depth O in the crop window of poses_out, cropped exactly as K0 crops input B (se3tn_compute_bbox's
+ * window, se3tn_crop_bbox's nearest mapping, 0 outside the image; the filled frame when the step fills the depth).  R and O are
+ * uint16 mm before any clipping.  Track i's row, SE3TN_FIT_COLS int32 over its 176 x 176 pixels:
  *   0 model     #(R > 0)
  *   1 observed  #(R > 0, O > 0)
  *   2 inlier    #(R > 0, O > 0, |O - R| <= tau_mm)
@@ -377,14 +438,63 @@ int se3tn_fill_depth_ex(se3tn_ctx* ctx, const uint16_t* depth_mm, int H, int W, 
  * them.  se3tn_track_render_host uploads the whole depth frame while the check is on (the window of poses_out is not known
  * before the step; rgb stays windowed) and brings the n rows back in its one copy out, into its out_fit.  How well the rows
  * predict tracking failure has not been measured on a trained checkpoint or real data (`predict --fit --score` reports it per
- * run, README). */
+ * run, README).
+ *
+ * icp: NULL (ICP off: the step, its graph and its bits are those of a step that never mentions ICP), or the ICP options above
+ * (HOST, read during the call only).  The block is allocated by the call, before anything is queued; scratch that cannot be
+ * allocated is SE3TN_ERR_INVALID.  The host route uploads the whole depth frame while ICP is on.
+ *
+ * hyp: NULL (no expansion and no choice), or the hypothesis options above (HOST, read during the call only); hyp->hypotheses = 1
+ * is the S = 1 hypothesis step, which draws nothing.  A hypothesis step needs fit_tau_mm (the choice ranks the fit rows) and
+ * n x S <= max_batch.  It is the expansion, then the n x S-track render step's launches (its first render waits for the
+ * expansion to complete), then the choice: se3tn_last_launch_count is that step's + 2.  The n x S starts, ids, widths and network
+ * outputs live in context scratch (max_batch rows, allocated by the first call, never moved).  poses_out[i], out_trans[i] and
+ * out_rot[i] are hypothesis out_choice[i]'s; poses_in is read only by the expansion, the step's first launch, so poses_out may be
+ * poses_in.  The n x S step picks its split-K regime by n x S (n <= 4 is the latency mode), so hypothesis 0 matches a plain
+ * n-track step bit for bit only when both land in the same regime.  The host route uploads the whole frame when S > 1 (the
+ * starts' crop windows are drawn on the device). */
 #define SE3TN_MAX_REFINE_ITERATIONS 8
 #define SE3TN_FIT_COLS 6
 struct se3tn_track_opts {
     int32_t fill_depth, fill_extrapolate, fill_blur, iterations;   /* fill_blur: SE3TN_BLUR_*; iterations 1..SE3TN_MAX_REFINE_ITERATIONS */
     double fill_max_depth;                                          /* metres; finite and > 0 as a float when fill_depth */
     int32_t fit_tau_mm, reserved;                                   /* fit_tau_mm 0: off, else 1..1000; reserved 0 */
-};                                                                  /* 32 bytes, no padding */
+    const se3tn_icp_opts* icp;                                      /* NULL: no ICP */
+    const se3tn_hypothesis_opts* hyp;                               /* NULL: no expansion or choice */
+};                                                                  /* 48 bytes on LP64, no padding */
+
+/* The optional per-step arrays of se3tn_track_render (device pointers) and se3tn_track_render_host (host pointers), passed by
+ * pointer; NULL means every field is NULL.  Each field is taken only where the step's options use it; one given where they do
+ * not, or missing where they require it, is SE3TN_ERR_INVALID with the field named and nothing queued.  n tracks, k =
+ * opts->iterations, M = opts->icp->iterations, S = opts->hyp->hypotheses:
+ *   draw_keys    int64 (n), with hyp only; required when S > 1.  Each track's draw key.  On the device route it is read on the
+ *                device, so one captured step replays frame after frame with fresh draws when the caller writes new keys into the
+ *                same array; the host route sends it up with the poses.
+ *   round_poses  double (k, n, 16), device route only: slot r - 1 receives every track's pose after round r, r = 1 .. k, bit for
+ *                bit what an r-round step leaves in poses_out (slot k - 1 equals poses_out).  After each round the step copies
+ *                poses_out there (a device-to-device copy inside the step's CUDA graph; SE3TN_PREC_FP32 queues it between its
+ *                plain launches); se3tn_last_launch_count counts kernels only, so it reads as without it.  With hyp it is
+ *                (k, n, S, 16): every round of every hypothesis.  ICP's iterations are not recorded here.
+ *   hyp_poses    double (n, S, 16), with hyp on the device route only: every hypothesis after the last round.
+ *   icp_poses    double (M, n, 16), with icp on the device route only: slot m - 1 receives every pose after ICP iteration m.
+ *   out_fit      int32 (n, SE3TN_FIT_COLS).  Device route: with hyp only, and then required: the kept hypotheses' rows
+ *                (se3tn_fit_rows then holds all n x S rows of the step; without hyp the rows stay there alone).  Host route:
+ *                required exactly when opts->fit_tau_mm is set, brought back in the call's one copy out.
+ *   out_choice   int32 (n), with hyp only, and then required: the hypothesis each track kept.
+ *   out_icp      double (n, SE3TN_ICP_COLS), with icp only: the stats of the last ICP iteration.
+ * Every pointer is part of the step's key: a step with round_poses and one without are two graphs, and both compute the same
+ * poses_out.  Device route: SE3TN_ERR_INVALID, with nothing queued, for round_poses overlapping poses_in or poses_out; icp_poses
+ * and out_icp overlapping poses_in, poses_out, round_poses or each other; with hyp, any output overlapping poses_in (except
+ * poses_out == poses_in), draw_keys or another output. */
+typedef struct se3tn_track_arrays {
+    const int64_t* draw_keys;
+    double* round_poses;
+    double* hyp_poses;
+    double* icp_poses;
+    int32_t* out_fit;
+    int32_t* out_choice;
+    double* out_icp;
+} se3tn_track_arrays;
 
 /* *rows = the device rows of the fit check (max_batch x SE3TN_FIT_COLS int32).  SE3TN_ERR_STATE before the first step with the
  * check on. */
@@ -412,157 +522,30 @@ int se3tn_track_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* f
  * is render (2 launches) + the launches of se3tn_track_batch, captured as one CUDA graph (se3tn_last_step_was_graph);
  * SE3TN_PREC_FP32 renders and then runs its FFMA forwards without a graph.  Every id is checked on the host before anything is launched: an id without weights, statistics or a
  * mesh is SE3TN_ERR_STATE (the id is named; no other model is drawn in its place), n > max_batch, an unknown mode or a
- * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch.  With opts->iterations
- * k > 1 the step refines every track k times on this frame.
- * round_poses: NULL, or a device output double (k, n, 16), k = opts->iterations (1 without opts), where slot r - 1 receives every
- * track's pose after round r, r = 1 .. k, bit for bit what an r-round step leaves in poses_out (slot k - 1 equals poses_out).
- * After each round the step copies poses_out there (a device-to-device copy inside the step's CUDA graph; SE3TN_PREC_FP32 queues
- * it between its plain launches); se3tn_last_launch_count counts kernels only, so it reads as without it.  round_poses is part
- * of the step's key: a step with it and one without are two graphs, and both compute the same poses_out.  SE3TN_ERR_INVALID
- * with nothing queued for a round_poses that overlaps poses_in or poses_out. */
+ * camera image size out of range is SE3TN_ERR_INVALID.  poses_out may be poses_in, as in se3tn_track_batch.  opts selects the
+ * step's extras (k rounds, the fit check, ICP, hypotheses: se3tn_track_opts); arrays, in HOST memory, holds their optional
+ * device outputs (se3tn_track_arrays), or NULL; an arrays pointer into device memory is SE3TN_ERR_INVALID. */
 int se3tn_track_render(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
                        const double* K, const double* poses_in, const double* object_width,
                        int render_mode, int render_H, int render_W,
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double trans_normalizer, double rot_normalizer, int precision,
-                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                       void* stream);
+                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts,
+                       const se3tn_track_arrays* arrays, void* stream);
 
 /* se3tn_track_render with every pointer in HOST memory, the reference's own calling pattern with rendering included: the
  * frame's crop-window rectangle, the poses, widths and ids go through se3tn_track_host's pinned staging (one copy in, one
  * copy out, stable device addresses so the step's graph is replayed); input A is rendered on the device and never crosses
  * the bus.  Synchronises `stream`.  Arguments as se3tn_track_host without rgbA / depthA, plus the render arguments of
- * se3tn_track_render; weight_ids int32 (n) or NULL (all tracks use set 0 and mesh 0).  out_fit int32 (n, SE3TN_FIT_COLS) HOST:
- * the fit check's rows, required when opts->fit_tau_mm is set and NULL otherwise (SE3TN_ERR_INVALID, nothing queued).  Errors
- * as se3tn_track_render. */
+ * se3tn_track_render; weight_ids int32 (n) or NULL (all tracks use set 0 and mesh 0).  arrays: the optional HOST arrays of
+ * se3tn_track_arrays this route takes (draw_keys, out_fit, out_choice, out_icp), or NULL.  Errors as se3tn_track_render. */
 int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                             const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
                             const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
-                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                            void* stream);
+                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts,
+                            const se3tn_track_arrays* arrays, void* stream);
 
-/* ---- depth refinement: point-to-plane ICP of every track against the observed depth, inside the tracking step ---------- */
-
-/* The network's correction is bounded (tanh x normaliser) and as precise as its checkpoint; the step already holds the (filled)
- * observed depth, the crop windows and a rasteriser.  With ICP on, a render step runs, after the network's last round and before
- * the fit check, M fixed iterations of projective point-to-plane ICP per track, each render (depth + triangle ids at poses_out,
- * 2 launches) -> accumulate (1) -> solve (1), all on `stream` and inside the step's one CUDA graph:
- *   association: every crop pixel u of the render in the crop window of the current pose (se3tn_compute_bbox's window,
- *     se3tn_crop_bbox's nearest mapping, as the fit check takes it) whose triangle id is >= 0 reads frame pixel p; d_obs = the
- *     frame's depth there (the filled frame when the step fills), skipped when 0 or p lies outside the frame.  The ray
- *     r = K^-1 (p_x, p_y, 1) meets the plane of that triangle (unit normal n, posed by the current pose) at q; d_model = 1000 q_z.
- *     Skipped when |n . r / |r|| < 0.1 (grazing) or d_model <= 0.  Inlier: |d_obs - d_model| <= tau_mm; o = r d_obs / 1000.
- *   linear system: e = n . (q - o), J = [(q x n)^T, n^T] for the left increment xi = (w, v); per track the upper 21 entries of
- *     J^T J, J^T e, sum e^2 and the inlier count, summed in a fixed order (bit-reproducible across runs and graph replays).
- *   solve: Cholesky of J^T J in fp64.  count < min_inliers or a pivot <= 1e-12 x the largest diagonal entry: the pose stays bit
- *     for bit.  Otherwise xi = -(J^T J)^-1 J^T e, R <- Exp(w) R, t <- Exp(w) t + v (Rodrigues), poses_out updated in place.
- * Stats row per track, SE3TN_ICP_COLS doubles: inliers, rms_mm (point-to-plane, before the update), step_mm (how far the object's
- * origin moved), step_deg (the rotation's angle); steps are 0 when the update was skipped.  There is no early exit: the launch
- * count is the step's + 4 M.  The defaults the Python layer uses (tau 20 mm, min_inliers 100) are starting guesses, not tuned on
- * a real sensor; whether ICP improves a trained checkpoint's accuracy has not been measured. */
-#define SE3TN_MAX_ICP_ITERATIONS 16
-#define SE3TN_ICP_COLS 4      /* inliers, rms_mm (point-to-plane, before the update), step_mm, step_deg (0 when skipped) */
-typedef struct se3tn_icp_opts {
-    int32_t iterations;       /* 1..SE3TN_MAX_ICP_ITERATIONS */
-    int32_t tau_mm;           /* association gate, 1..1000 */
-    int32_t min_inliers;      /* 6..176*176 */
-    int32_t reserved;         /* 0 */
-} se3tn_icp_opts;             /* 16 bytes, no padding */
-
-/* se3tn_track_render followed by M ICP iterations (above), then the fit check, if on, at the refined pose.  Arguments as
- * se3tn_track_render, plus:
- *   icp: the ICP options (HOST, read during the call only), or NULL: exactly se3tn_track_render (same graph, same bits)
- *   icp_poses double (M, n, 16) device or NULL: slot m - 1 receives every pose after ICP iteration m (round_poses keeps
- *     recording the network's rounds only)
- *   out_icp double (n, SE3TN_ICP_COLS) device or NULL: the stats of the last iteration
- * The ICP render takes context scratch of its own, allocated at max_batch tracks by the first ICP step and never moved:
- * 176 x 176 x (4 bytes of triangle ids + 2 bytes of depth) per track, plus 256 bytes of sums (about 186 KB a track).
- * Refused with SE3TN_ERR_INVALID, the field named and nothing queued: what se3tn_track_render refuses, icp fields out of range
- * or reserved != 0, icp_poses or out_icp overlapping poses_in, poses_out, round_poses or each other, and scratch that cannot be
- * allocated.  SE3TN_PREC_FP32 queues the same launches without a graph. */
-int se3tn_track_icp(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                    const double* K, const double* poses_in, const double* object_width,
-                    int render_mode, int render_H, int render_W,
-                    const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                    double trans_normalizer, double rot_normalizer, int precision,
-                    float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                    const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream);
-
-/* se3tn_track_render_host with ICP: arguments as se3tn_track_render_host, plus icp (NULL: se3tn_track_render_host exactly) and
- * out_icp double (n, SE3TN_ICP_COLS) HOST or NULL, brought back in the call's one copy out.  The whole depth frame is uploaded
- * while ICP is on.  Synchronises `stream`.  Errors as se3tn_track_icp. */
-int se3tn_track_icp_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
-                         const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
-                         const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
-                         double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                         const se3tn_icp_opts* icp, double* out_icp, void* stream);
-
-/* ---- multi-hypothesis tracking: several starts per track, the one whose model fits the frame best kept ---------------- */
-
-/* A track that has slipped further than the network was trained to correct stays lost: the network pulls a pose back from
- * perturbations up to dataset_info's max_translation / max_rotation (reference produce_train_pair_data.py:90-110).  A hypothesis
- * step looks around the previous pose instead of only at it.  For each of n tracks it
- *   1. draws S - 1 start poses around the previous pose P: hypothesis h >= 1 is P . inv(D), D = random_gaussian_magnitude(
- *      max_translation, max_rotation_deg) (reference Utils.py:372-404), composed as produce_train_pair_data.py:110 composes a
- *      training pair (A_in_cam = B_in_cam . inv(B_in_A)); hypothesis 0 is P itself;
- *   2. refines all n x S starts as one n x S-track se3tn_track_render step (the options' fill, k rounds and fit check);
- *   3. keeps, per track, the hypothesis whose fit row has the highest inlier fraction inlier / model (compared exactly as int64
- *      cross products; model = 0 ranks last), then the lowest mean inlier residual residual / inlier (inlier = 0 ranks last),
- *      then the lowest h.  A frame without depth leaves every inlier count at 0 and keeps hypothesis 0 as long as hypothesis 0's
- *      model covers a pixel of its window (model > 0); when it covers none, the first h >= 1 whose model does wins.
- * Rows are track-major: track i's hypothesis h is row i S + h of every n x S array.  Draws: Philox4x32-10 (the generator of
- * se3tn_augment), key = seed, counter = (draw_keys[i] low word, high word, h, slot).  Each of the translation and the rotation
- * takes a direction from random_direction (theta = 2 pi U, phi = acos(2 U - 1)) and a magnitude from N(0, max), redrawn until
- * |m| <= max as the reference does, at most 64 times; a magnitude that never lands inside (probability ~1e-32) is clamped to +-max.
- * The rotation is cv2.Rodrigues of axis / |axis| * m / 180 * pi in fp64.  The draws depend on (seed, draw key, h) alone: not on
- * n, the precision, the route or anything else in the step.  S = 1 draws nothing and is se3tn_track_render's step bit for bit.
- * Whether more hypotheses track better on a trained checkpoint has not been measured (README). */
-#define SE3TN_MAX_HYPOTHESES 32
-#define SE3TN_HYP_DRAWS 8     /* se3tn_draw_hypotheses' out_draws columns (below) */
-typedef struct se3tn_hypothesis_opts {
-    int32_t hypotheses, reserved;                  /* S in [1, SE3TN_MAX_HYPOTHESES]; reserved 0                            */
-    int64_t seed;                                  /* the Philox key                                                         */
-    double max_translation, max_rotation_deg;      /* metres, finite, in (0, 1]; degrees, in (0, 180]                        */
-} se3tn_hypothesis_opts;                           /* 32 bytes, no padding                                                   */
-
-/* se3tn_track_render with S hypotheses per track, in one call and one CUDA graph.  Arguments as se3tn_track_render, plus:
- *   draw_keys int64 (n) device: each track's draw key, read on the device, so one captured step replays frame after frame with
- *     fresh draws when the caller writes new keys into the same array; may be NULL when S = 1
- *   hyp: the hypothesis options (HOST, read during the call only)
- *   out_choice int32 (n) device: the hypothesis each track kept
- *   out_fit int32 (n, SE3TN_FIT_COLS) device: the kept rows; se3tn_fit_rows then holds all n x S rows of the step
- *   hyp_poses double (n, S, 16) device or NULL: every hypothesis after the last round
- *   round_poses double (k, n, S, 16) device or NULL: every round of every hypothesis, as se3tn_track_render's
- * poses_out[i], out_trans[i], out_rot[i] are hypothesis out_choice[i]'s.  opts->fit_tau_mm is required (the choice ranks its
- * rows).  poses_in is read only by the expansion, the step's first launch, so poses_out may be poses_in.  The n x S starts, ids,
- * widths and network outputs live in context scratch (max_batch rows, allocated by the first call, never moved).  The step is the
- * expansion, then the n x S-track se3tn_track_render step's launches (its first render waits for the expansion to complete), then
- * the choice: se3tn_last_launch_count is that step's + 2.  The hypothesis options and every pointer are part of the step's key.
- * The n x S step picks its split-K regime by n x S (n <= 4 is the latency mode), so hypothesis 0 matches a plain n-track step bit
- * for bit only when both land in the same regime.  Refused with SE3TN_ERR_INVALID, the field named and nothing queued: what
- * se3tn_track_render refuses, S, max_translation or max_rotation_deg out of range, hyp->reserved != 0, n x S > max_batch, fit off,
- * draw_keys NULL with S > 1, and any output overlapping poses_in (except poses_out == poses_in), draw_keys or another output.  Ids
- * without weights, statistics or a mesh are SE3TN_ERR_STATE, as in se3tn_track_render. */
-int se3tn_track_hypotheses(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                           const double* K, const double* poses_in, const double* object_width,
-                           int render_mode, int render_H, int render_W,
-                           const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                           double trans_normalizer, double rot_normalizer, int precision,
-                           float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                           const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, int32_t* out_fit,
-                           double* hyp_poses, void* stream);
-
-/* se3tn_track_hypotheses with every pointer in HOST memory, through se3tn_track_render_host's pinned staging: the draw keys go
- * up with the poses in the one copy in; the poses, out_trans / out_rot (nullable), out_fit (n, SE3TN_FIT_COLS, required) and
- * out_choice (n, required) come back in the one copy out.  The whole frame is uploaded when S > 1 (the starts' crop windows are
- * drawn on the device).  Synchronises `stream`.  Errors as se3tn_track_hypotheses. */
-int se3tn_track_hypotheses_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
-                                const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
-                                const int32_t* weight_ids, int n, double trans_normalizer, double rot_normalizer, int precision,
-                                double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                                const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, void* stream);
-
-/* The expansion alone, as se3tn_track_hypotheses' first launch forms it: poses_in double (n,16), draw_keys int64 (n) (NULL when
+/* The expansion alone, as a hypothesis step's first launch forms it: poses_in double (n,16), draw_keys int64 (n) (NULL when
  * S = 1) -> out_poses double (n, S, 16), all device.  out_draws double (n, S, SE3TN_HYP_DRAWS) device or NULL: per row the
  * translation direction's U_theta, U_phi, the rotation axis' U_theta, U_phi, the accepted magnitudes m_T (m) and m_R (degrees),
  * and the N(0, max) draws each took (1..64); all 0 in hypothesis 0's rows.  One plain launch.  Refused (SE3TN_ERR_INVALID,

@@ -58,14 +58,6 @@ SIGNATURES = {
                                 _vp]),
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                      _vp]),
-    'se3tn_track_hypotheses': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
-                                    _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'se3tn_track_hypotheses_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp,
-                                         _vp, _vp, _vp, _vp, _vp]),
-    'se3tn_track_icp': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
-                             _vp, _vp, _vp, _vp]),
-    'se3tn_track_icp_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
-                                  _vp, _vp, _vp]),
     'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
@@ -105,12 +97,6 @@ class Augment(C.Structure):
                 ('blur_prob', _d), ('blur_max_kernel', C.c_int32), ('reserved', C.c_int32), ('cover_prob', _d)]
 
 
-class TrackOpts(C.Structure):
-    """se3tn_track_opts (include/se3tn.h)."""
-    _fields_ = [('fill_depth', C.c_int32), ('fill_extrapolate', C.c_int32), ('fill_blur', C.c_int32), ('iterations', C.c_int32),
-                ('fill_max_depth', _d), ('fit_tau_mm', C.c_int32), ('reserved', C.c_int32)]
-
-
 class HypothesisOpts(C.Structure):
     """se3tn_hypothesis_opts (include/se3tn.h)."""
     _fields_ = [('hypotheses', C.c_int32), ('reserved', C.c_int32), ('seed', C.c_int64), ('max_translation', _d),
@@ -120,6 +106,19 @@ class HypothesisOpts(C.Structure):
 class IcpOpts(C.Structure):
     """se3tn_icp_opts (include/se3tn.h)."""
     _fields_ = [('iterations', C.c_int32), ('tau_mm', C.c_int32), ('min_inliers', C.c_int32), ('reserved', C.c_int32)]
+
+
+class TrackOpts(C.Structure):
+    """se3tn_track_opts (include/se3tn.h)."""
+    _fields_ = [('fill_depth', C.c_int32), ('fill_extrapolate', C.c_int32), ('fill_blur', C.c_int32), ('iterations', C.c_int32),
+                ('fill_max_depth', _d), ('fit_tau_mm', C.c_int32), ('reserved', C.c_int32), ('icp', C.POINTER(IcpOpts)),
+                ('hyp', C.POINTER(HypothesisOpts))]
+
+
+class TrackArrays(C.Structure):
+    """se3tn_track_arrays (include/se3tn.h): device pointers for se3tn_track_render, host pointers for _render_host."""
+    _fields_ = [('draw_keys', _vp), ('round_poses', _vp), ('hyp_poses', _vp), ('icp_poses', _vp), ('out_fit', _vp),
+                ('out_choice', _vp), ('out_icp', _vp)]
 
 
 _lib = None

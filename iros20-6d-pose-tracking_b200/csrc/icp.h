@@ -1,4 +1,4 @@
-// Depth refinement of a track step (se3tn_track_icp): projective point-to-plane ICP of every track's model against the
+// Depth refinement of a render step (se3tn_track_opts.icp): projective point-to-plane ICP of every track's model against the
 // observed depth, one Gauss-Newton iteration per accumulate + solve pair (see icp.cu).
 #pragma once
 #include <cuda_runtime.h>

@@ -219,7 +219,7 @@ struct AugKey {
         return c;
     }
 };
-// se3tn_track_hypotheses' expansion and choice; all zero in every other step.  The step's own tracks (StepKey::n = n x S) are the
+// A hypothesis step's expansion and choice (se3tn_track_opts.hyp); all zero in every other step.  The step's own tracks (StepKey::n = n x S) are the
 // expanded rows in context scratch; these are the caller's n tracks and the call's results.
 struct HypKey {
     int32_t S, pad;                            // hypotheses per track (0: not a hypothesis step); pad is always 0
@@ -228,7 +228,7 @@ struct HypKey {
     const double* poses_in; const int64_t* keys; const int32_t* wid_in; const double* width_in;
     double* poses_out; float* trans_out; float* rot_out; int32_t* choice; int32_t* fit_out;
 };
-// se3tn_track_icp[_host]'s depth refinement after the last round (se3tn_icp_opts); all zero when ICP is off, so every other
+// A render step's depth refinement after the last round (se3tn_track_opts.icp); all zero when ICP is off, so every other
 // step's key keeps its bytes.
 struct IcpKey {
     int32_t iterations, tau, min_inliers, pad; // iterations 0: no ICP; pad is always 0
@@ -254,8 +254,8 @@ struct StepKey {
     const uint8_t* seg; const int32_t* class_ids; uint8_t* segB; int32_t* seg_count;      // pair step
     double* round_poses;                       // track step that renders input A: each round's poses (se3tn_track_render) or NULL
     int32_t* fit_rows;                         // fit_tau > 0: the rows of the fit check, n x kFitCols
-    HypKey hyp;                                // track step of se3tn_track_hypotheses[_host]
-    IcpKey icp;                                // track step of se3tn_track_icp[_host]
+    HypKey hyp;                                // track step with opts->hyp
+    IcpKey icp;                                // track step with opts->icp
 };
 static_assert(std::has_unique_object_representations_v<StepKey>, "a graph key is compared byte for byte: no padding, no floating point");
 
@@ -289,10 +289,10 @@ struct se3tn_ctx {
     // the fit check's block: the device route's rows (max_batch x kFitCols int32), then the fit's rendered depth for max_batch
     // tracks; allocated by the first step with the check on, never moved after (captured steps hold both addresses)
     DevBuf<uint8_t> fit; size_t fit_bytes = 0;
-    // se3tn_track_hypotheses' expanded tracks: poses (max_batch x 16), widths, ids, network outputs (max_batch x 3 each); allocated
+    // a hypothesis step's expanded tracks: poses (max_batch x 16), widths, ids, network outputs (max_batch x 3 each); allocated
     // by the first hypothesis step, never moved after
     DevBuf<uint8_t> hyp; size_t hyp_bytes = 0;
-    // se3tn_track_icp's block: the sums (max_batch x kIcpSums doubles), then the ICP render's depth and triangle ids of
+    // the ICP block: the sums (max_batch x kIcpSums doubles), then the ICP render's depth and triangle ids of
     // max_batch tracks; allocated by the first ICP step, never moved after
     DevBuf<uint8_t> icp; size_t icp_bytes = 0;
     DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
@@ -1227,38 +1227,6 @@ uint16_t* filled_frame(se3tn_ctx* c, int H, int W) { return reinterpret_cast<uin
 // and the fp32 mode's runs of equal ids, which are never captured.
 struct Step : StepKey { const int32_t* wid_host; };
 
-// A tracking call's se3tn_track_opts (NULL: the defaults) checked and written into its step: the fill, the rounds and the fit
-// check, so the key holds them.  renders: the step draws input A.  se3tn_track_batch / se3tn_track_host take input A from the
-// caller: a later round could not redraw it at the refined pose, and the fit check could not draw a model the weight id need
-// not have.  Refused before anything is queued.
-static_assert(sizeof(se3tn_track_opts) == 32, "se3tn_track_opts is 32 bytes without padding: _lib.TrackOpts mirrors it");
-int track_opts(se3tn_ctx* c, const char* fn, const se3tn_track_opts* o, bool renders, Step& st) {
-    st.iterations = 1;
-    if (!o) return SE3TN_OK;
-    const std::string f(fn);
-    if (o->fill_depth) {                           // off: the fill fields stay zero, whatever the caller left in them
-        if (o->fill_blur != SE3TN_BLUR_BILATERAL && o->fill_blur != SE3TN_BLUR_GAUSSIAN)
-            return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_blur is " + std::to_string(o->fill_blur) + ", not an SE3TN_BLUR_*");
-        const float md = static_cast<float>(o->fill_max_depth);   // what the kernels compute with
-        if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_max_depth must be finite and > 0");
-        st.fill = 1; st.fill_max_depth = o->fill_max_depth; st.fill_extrapolate = o->fill_extrapolate != 0;
-        st.fill_blur = static_cast<uint16_t>(o->fill_blur);
-    }
-    if (o->iterations < 1 || o->iterations > SE3TN_MAX_REFINE_ITERATIONS)
-        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
-    if (o->fit_tau_mm < 0 || o->fit_tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be 0 or in [1, 1000]");
-    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
-    if (!renders && o->iterations != 1)
-        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations is " + std::to_string(o->iterations) + "; input A from the caller "
-                    "cannot be redrawn, which needs se3tn_track_render[_host]");
-    if (!renders && o->fit_tau_mm)
-        return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm is set; input A from the caller, and the fit check draws each "
-                    "track's model, which needs se3tn_track_render[_host]");
-    st.iterations = static_cast<uint16_t>(o->iterations);
-    st.fit_tau = o->fit_tau_mm;
-    return SE3TN_OK;
-}
-
 // What every track step takes from its scalar arguments and its ids (checked by check_step: `mixed`), added to what track_opts
 // wrote; the caller adds the device pointers.
 void track_step(Step& st, int H, int W, const double* K, const int32_t* wid_host, bool mixed, int n, double tn, double rn, int precision) {
@@ -1290,7 +1258,7 @@ int render_into_scratch(se3tn_ctx* c, const RenderSpec& r, Step& st) {
     return SE3TN_OK;
 }
 
-// se3tn_track_hypotheses' scratch: the expanded tracks' poses | widths | ids | trans | rot, max_batch rows each.
+// A hypothesis step's scratch: the expanded tracks' poses | widths | ids | trans | rot, max_batch rows each.
 struct HypScratch { double* poses; double* width; int32_t* wid; float* trans; float* rot; };
 int reserve_hyp(se3tn_ctx* c, HypScratch* x) {
     const size_t mb = static_cast<size_t>(c->max_batch);
@@ -1303,7 +1271,7 @@ int reserve_hyp(se3tn_ctx* c, HypScratch* x) {
     return SE3TN_OK;
 }
 
-// se3tn_track_icp's block: sums | the ICP render's depth | its triangle ids, max_batch tracks each.
+// The ICP block: sums | the ICP render's depth | its triangle ids, max_batch tracks each.
 size_t icp_sums_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kIcpSums * sizeof(double)); }
 size_t icp_depth_bytes(int max_batch) { return align256(static_cast<size_t>(max_batch) * kImg * kImg * sizeof(uint16_t)); }
 double* icp_sums(se3tn_ctx* c) { return reinterpret_cast<double*>(c->icp.get()); }
@@ -1313,23 +1281,22 @@ int32_t* icp_tri(se3tn_ctx* c) {
 }
 
 static_assert(sizeof(se3tn_icp_opts) == 16, "se3tn_icp_opts is 16 bytes without padding: _lib.IcpOpts mirrors it");
-static_assert(kIcpCols == SE3TN_ICP_COLS, "se3tn_track_icp's out_icp columns");
-// se3tn_icp_opts (NULL: ICP off, st.icp stays zero) checked and written into st.icp, and the block allocated, all before
-// anything is queued: a block that cannot be allocated refuses the call and leaves the context as it was.
+static_assert(kIcpCols == SE3TN_ICP_COLS, "se3tn_track_arrays' out_icp columns");
+// opts->icp checked and written into st.icp, and the block allocated on the current device: a block that cannot be allocated
+// refuses the call and leaves the context as it was.
 int icp_opts(se3tn_ctx* c, const char* fn, const se3tn_icp_opts* o, Step& st) {
-    if (!o) return SE3TN_OK;
     const std::string f(fn);
     if (o->iterations < 1 || o->iterations > SE3TN_MAX_ICP_ITERATIONS)
-        return fail(c, SE3TN_ERR_INVALID, f + ": icp->iterations is " + std::to_string(o->iterations) + ", not in [1, " +
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp->iterations is " + std::to_string(o->iterations) + ", not in [1, " +
                     std::to_string(SE3TN_MAX_ICP_ITERATIONS) + "]");
-    if (o->tau_mm < 1 || o->tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": icp->tau_mm must be in [1, 1000]");
+    if (o->tau_mm < 1 || o->tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp->tau_mm must be in [1, 1000]");
     if (o->min_inliers < 6 || o->min_inliers > kImg * kImg)
-        return fail(c, SE3TN_ERR_INVALID, f + ": icp->min_inliers must be in [6, " + std::to_string(kImg * kImg) + "]");
-    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": icp->reserved must be 0");
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp->min_inliers must be in [6, " + std::to_string(kImg * kImg) + "]");
+    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp->reserved must be 0");
     const size_t bytes = icp_sums_bytes(c->max_batch) + icp_depth_bytes(c->max_batch) + static_cast<size_t>(c->max_batch) * kImg * kImg * sizeof(int32_t);
     if (grow(c->icp, c->icp_bytes, bytes) != cudaSuccess) {
         cudaGetLastError();
-        return fail(c, SE3TN_ERR_INVALID, f + ": icp: its scratch (" + std::to_string(bytes) + " bytes) cannot be allocated");
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp: its scratch (" + std::to_string(bytes) + " bytes) cannot be allocated");
     }
     st.icp.iterations = o->iterations; st.icp.tau = o->tau_mm; st.icp.min_inliers = o->min_inliers;
     return SE3TN_OK;
@@ -1337,28 +1304,71 @@ int icp_opts(se3tn_ctx* c, const char* fn, const se3tn_icp_opts* o, Step& st) {
 
 static_assert(sizeof(se3tn_hypothesis_opts) == 32, "se3tn_hypothesis_opts is 32 bytes without padding: _lib.HypothesisOpts mirrors it");
 static_assert(kHypDraws == SE3TN_HYP_DRAWS, "se3tn_draw_hypotheses' out_draws columns");
-// se3tn_hypothesis_opts checked for n tracks and written into st.hyp's scalars.  step: a tracking call, whose choice needs the
-// fit check's rows (st holds its se3tn_track_opts already).  Refused before anything is queued.
-int hypothesis_opts(se3tn_ctx* c, const char* fn, const se3tn_hypothesis_opts* h, const int64_t* keys, int n, bool step, Step& st) {
-    const std::string f(fn);
-    if (!h) return fail(c, SE3TN_ERR_INVALID, f + ": hyp is NULL");
+// The se3tn_hypothesis_opts `name` checked for n tracks and written into st.hyp's scalars.  Refused before anything is queued.
+int hypothesis_opts(se3tn_ctx* c, const char* fn, const char* name, const se3tn_hypothesis_opts* h, int n, Step& st) {
+    const std::string f = std::string(fn) + ": " + name;
+    if (!h) return fail(c, SE3TN_ERR_INVALID, f + " is NULL");
     if (h->hypotheses < 1 || h->hypotheses > SE3TN_MAX_HYPOTHESES)
-        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->hypotheses is " + std::to_string(h->hypotheses) + ", not in [1, " +
+        return fail(c, SE3TN_ERR_INVALID, f + "->hypotheses is " + std::to_string(h->hypotheses) + ", not in [1, " +
                     std::to_string(SE3TN_MAX_HYPOTHESES) + "]");
-    if (h->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": hyp->reserved must be 0");
+    if (h->reserved) return fail(c, SE3TN_ERR_INVALID, f + "->reserved must be 0");
     if (!(std::isfinite(h->max_translation) && h->max_translation > 0.0 && h->max_translation <= 1.0))
-        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->max_translation must be finite and in (0, 1] m");
+        return fail(c, SE3TN_ERR_INVALID, f + "->max_translation must be finite and in (0, 1] m");
     if (!(h->max_rotation_deg > 0.0 && h->max_rotation_deg <= 180.0))
-        return fail(c, SE3TN_ERR_INVALID, f + ": hyp->max_rotation_deg must be in (0, 180]");
+        return fail(c, SE3TN_ERR_INVALID, f + "->max_rotation_deg must be in (0, 180]");
     if (n < 0 || static_cast<long long>(n) * h->hypotheses > c->max_batch)
-        return fail(c, SE3TN_ERR_INVALID, f + ": n x hyp->hypotheses = " + std::to_string(static_cast<long long>(n) * h->hypotheses) +
+        return fail(c, SE3TN_ERR_INVALID, f + "->hypotheses x n = " + std::to_string(static_cast<long long>(n) * h->hypotheses) +
                     " exceeds max_batch " + std::to_string(c->max_batch));
-    if (step && !st.fit_tau)
-        return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be set: the choice ranks the hypotheses by the fit check's rows");
-    if (h->hypotheses > 1 && !keys) return fail(c, SE3TN_ERR_INVALID, f + ": draw_keys is NULL with hyp->hypotheses > 1");
     st.hyp.S = h->hypotheses; st.hyp.seed = static_cast<uint64_t>(h->seed);
-    st.hyp.max_t = h->max_translation; st.hyp.max_r = h->max_rotation_deg; st.hyp.keys = keys;
+    st.hyp.max_t = h->max_translation; st.hyp.max_r = h->max_rotation_deg;
     return SE3TN_OK;
+}
+
+// A tracking call's se3tn_track_opts (NULL: the defaults) checked and written into its step, so the key holds them: the fill,
+// the rounds, the fit check, ICP (its block allocated) and the hypotheses.  renders: the step draws input A; n: its tracks.
+// se3tn_track_batch / se3tn_track_host take input A from the caller: a later round, ICP or a hypothesis could not redraw it at
+// another pose, and the fit check and ICP could not draw a model the weight id need not have.  ICP inside a hypothesis step is
+// refused here, the one place that decides which extras a step runs.  Refused before anything is queued.
+static_assert(sizeof(se3tn_track_opts) == 48, "se3tn_track_opts is 48 bytes without padding: _lib.TrackOpts mirrors it");
+int track_opts(se3tn_ctx* c, const char* fn, const se3tn_track_opts* o, bool renders, int n, Step& st) {
+    st.iterations = 1;
+    if (!o) return SE3TN_OK;
+    const std::string f(fn);
+    if (o->fill_depth) {                           // off: the fill fields stay zero, whatever the caller left in them
+        if (o->fill_blur != SE3TN_BLUR_BILATERAL && o->fill_blur != SE3TN_BLUR_GAUSSIAN)
+            return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_blur is " + std::to_string(o->fill_blur) + ", not an SE3TN_BLUR_*");
+        const float md = static_cast<float>(o->fill_max_depth);   // what the kernels compute with
+        if (!(std::isfinite(md) && md > 0.f)) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fill_max_depth must be finite and > 0");
+        st.fill = 1; st.fill_max_depth = o->fill_max_depth; st.fill_extrapolate = o->fill_extrapolate != 0;
+        st.fill_blur = static_cast<uint16_t>(o->fill_blur);
+    }
+    if (o->iterations < 1 || o->iterations > SE3TN_MAX_REFINE_ITERATIONS)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations must be in [1, " + std::to_string(SE3TN_MAX_REFINE_ITERATIONS) + "]");
+    if (o->fit_tau_mm < 0 || o->fit_tau_mm > 1000) return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be 0 or in [1, 1000]");
+    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
+    if (!renders && o->iterations != 1)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->iterations is " + std::to_string(o->iterations) + "; input A from the caller "
+                    "cannot be redrawn, which needs se3tn_track_render[_host]");
+    if (!renders && o->fit_tau_mm)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm is set; input A from the caller, and the fit check draws each "
+                    "track's model, which needs se3tn_track_render[_host]");
+    if (!renders && (o->icp || o->hyp))
+        return fail(c, SE3TN_ERR_INVALID, f + (o->icp ? ": opts->icp" : ": opts->hyp") + " is set; input A from the caller cannot "
+                    "be redrawn, which needs se3tn_track_render[_host]");
+    if (o->icp && o->hyp)
+        return fail(c, SE3TN_ERR_INVALID, f + ": opts->icp and opts->hyp are both set; ICP inside a hypothesis step is not supported");
+    st.iterations = static_cast<uint16_t>(o->iterations);
+    st.fit_tau = o->fit_tau_mm;
+    if (o->hyp) {
+        const int rc = hypothesis_opts(c, fn, "opts->hyp", o->hyp, n, st);
+        if (rc) return rc;
+        if (!st.fit_tau)
+            return fail(c, SE3TN_ERR_INVALID, f + ": opts->fit_tau_mm must be set with opts->hyp: the choice ranks the hypotheses by "
+                        "the fit check's rows");
+    }
+    if (!o->icp) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    return icp_opts(c, fn, o->icp, st);
 }
 
 int run_step(se3tn_ctx* c, const Step& st, cudaStream_t s);
@@ -1490,7 +1500,7 @@ int step_launches(se3tn_ctx* c, const Step& st, cudaStream_t s) {
         ++c->launches;
         return SE3TN_OK;
     }
-    if (st.hyp.S) {                                // se3tn_track_hypotheses: the n x S starts, ids and widths every later launch reads
+    if (st.hyp.S) {                                // hypothesis step: the n x S starts, ids and widths every later launch reads
         HypArgs h{};
         h.poses_in = st.hyp.poses_in; h.keys = st.hyp.keys; h.n = st.n / st.hyp.S; h.S = st.hyp.S; h.seed = st.hyp.seed;
         h.max_t = st.hyp.max_t; h.max_r_deg = st.hyp.max_r; h.wid_in = st.hyp.wid_in; h.width_in = st.hyp.width_in;
@@ -1703,54 +1713,38 @@ int eval_pairs_step(se3tn_ctx* c, const char* fn, const uint8_t* rgbA, const uin
     return run_step(c, st, static_cast<cudaStream_t>(stream));
 }
 
-// se3tn_track_render and se3tn_track_icp: one step that draws input A, with ICP after the rounds when icp is set.
-int track_render_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                      const double* K, const double* poses_in, const double* object_width,
-                      int render_mode, int render_H, int render_W,
-                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                      double tn, double rn, int precision,
-                      float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                      const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream) {
-    const std::string f(fn);
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
-    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
-    RenderSpec r;
-    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    Step st{};
-    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
-    bool multi = false;
-    rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision);
-    if (rc) return rc;
-    if (n == 0) return SE3TN_OK;
-    if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
-    if (round_poses) {                             // the copies must not write the poses a later round reads
-        const uintptr_t r0 = reinterpret_cast<uintptr_t>(round_poses);
-        const uintptr_t r1 = r0 + sizeof(double) * 16 * static_cast<size_t>(n) * st.iterations;
-        for (const double* p : {poses_in, static_cast<const double*>(poses_out)}) {
-            const uintptr_t p0 = reinterpret_cast<uintptr_t>(p), p1 = p0 + sizeof(double) * 16 * static_cast<size_t>(n);
-            if (p0 < r1 && r0 < p1) return fail(c, SE3TN_ERR_INVALID, f + ": round_poses overlaps poses_in or poses_out");
-        }
+// A render step's se3tn_track_arrays checked against its options (st, from track_opts), before anything is queued: each field is
+// taken only where the options use it (host: the host route, which keeps no per-round, per-hypothesis or per-iteration poses).
+// On the device route the step's outputs must not overlap what it reads later or each other: round_poses the poses a later
+// round reads, icp_poses and out_icp those and each other, and a hypothesis step's outputs its inputs.
+int track_arrays(se3tn_ctx* c, const char* fn, const se3tn_track_arrays& a, const Step& st, bool host, int n,
+                 const double* poses_in, const double* poses_out, const float* out_trans, const float* out_rot) {
+    const bool hyp = st.hyp.S != 0, icp = st.icp.iterations != 0, fit_rows = host ? st.fit_tau != 0 : hyp;
+    const struct { const void* p; bool taken, required; const char* name; } fields[] = {
+        {a.out_fit, fit_rows, fit_rows, "out_fit"}, {a.out_choice, hyp, hyp, "out_choice"},
+        {a.draw_keys, hyp, hyp && st.hyp.S > 1, "draw_keys"}, {a.round_poses, !host, false, "round_poses"},
+        {a.hyp_poses, hyp && !host, false, "hyp_poses"}, {a.icp_poses, icp && !host, false, "icp_poses"},
+        {a.out_icp, icp, false, "out_icp"}};
+    for (const auto& x : fields) {
+        if (x.p && !x.taken)
+            return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": arrays->" + x.name + " is set, but this step does not take it");
+        if (!x.p && x.required)
+            return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": arrays->" + x.name + " is NULL, but this step's options need it");
     }
-    DeviceGuard guard(c->device);
-    if ((rc = icp_opts(c, fn, icp, st))) return rc;
-    if (icp) {
-        const size_t nn = static_cast<size_t>(n);
-        const char* why = "icp_poses and out_icp must not overlap poses_in, poses_out, round_poses or each other";
-        const std::pair<const void*, size_t> in = {poses_in, nn * 128}, out = {poses_out, nn * 128}, rounds = {round_poses, st.iterations * nn * 128};
-        rc = check_disjoint(c, fn, {{icp_poses, st.icp.iterations * nn * 128}}, {in, out, rounds, {out_icp, nn * kIcpCols * sizeof(double)}}, why);
-        if (!rc) rc = check_disjoint(c, fn, {{out_icp, nn * kIcpCols * sizeof(double)}}, {in, out, rounds}, why);
-        if (rc) return rc;
-    }
-    st.icp.poses = icp ? icp_poses : nullptr; st.icp.stats = icp ? out_icp : nullptr;
-    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
-    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
-    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
-    st.round_poses = round_poses;
-    if ((rc = render_into_scratch(c, r, st))) return rc;
-    return run_step(c, st, static_cast<cudaStream_t>(stream));
+    if (host || n <= 0) return SE3TN_OK;
+    const size_t nn = static_cast<size_t>(n), rows = nn * (hyp ? st.hyp.S : 1);
+    const std::pair<const void*, size_t> in = {poses_in, nn * 128}, out = {poses_out, nn * 128}, rounds = {a.round_poses, st.iterations * rows * 128};
+    if (hyp)
+        return check_disjoint(c, fn, {out, {out_trans, nn * 12}, {out_rot, nn * 12}, {a.out_choice, nn * 4}, {a.out_fit, nn * 4 * kFitCols},
+                                      {a.hyp_poses, rows * 128}, rounds},
+                              {{poses_out == poses_in ? nullptr : poses_in, nn * 128}, {a.draw_keys, nn * 8}},
+                              "the starts are drawn from poses_in and draw_keys; poses_out may be poses_in itself");
+    int rc = check_disjoint(c, fn, {rounds}, {in, out}, "round_poses must not overlap poses_in or poses_out: a later round reads them");
+    if (rc || !icp) return rc;
+    const char* why = "icp_poses and out_icp must not overlap poses_in, poses_out, round_poses or each other";
+    rc = check_disjoint(c, fn, {{a.icp_poses, st.icp.iterations * nn * 128}}, {in, out, rounds, {a.out_icp, nn * kIcpCols * sizeof(double)}}, why);
+    if (!rc) rc = check_disjoint(c, fn, {{a.out_icp, nn * kIcpCols * sizeof(double)}}, {in, out, rounds}, why);
+    return rc;
 }
 
 }  // namespace
@@ -1767,7 +1761,7 @@ int se3tn_track_batch(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fr
     if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, "se3tn_track_batch: null output");
     bool multi = false;
     Step st{};
-    int rc = track_opts(c, "se3tn_track_batch", opts, false, st);
+    int rc = track_opts(c, "se3tn_track_batch", opts, false, n, st);
     if (rc) return rc;
     rc = check_step(c, "se3tn_track_batch", weight_ids_host, weight_ids_dev, n, false, &multi, precision);
     if (rc) return rc;
@@ -1788,60 +1782,50 @@ int se3tn_track_render(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* f
                        int render_mode, int render_H, int render_W,
                        const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
                        double tn, double rn, int precision,
-                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                       void* stream) {
-    return track_render_step(c, "se3tn_track_render", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
-                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, opts,
-                             round_poses, nullptr, nullptr, nullptr, stream);
-}
-
-int se3tn_track_icp(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                    const double* K, const double* poses_in, const double* object_width,
-                    int render_mode, int render_H, int render_W,
-                    const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                    double tn, double rn, int precision,
-                    float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                    const se3tn_icp_opts* icp, double* icp_poses, double* out_icp, void* stream) {
-    return track_render_step(c, "se3tn_track_icp", frame_rgb, frame_depth, H, W, K, poses_in, object_width, render_mode, render_H,
-                             render_W, weight_ids_host, weight_ids_dev, n, tn, rn, precision, out_trans, out_rot, poses_out, opts,
-                             round_poses, icp, icp_poses, out_icp, stream);
-}
-
-int se3tn_track_hypotheses(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W,
-                           const double* K, const double* poses_in, const double* object_width,
-                           int render_mode, int render_H, int render_W,
-                           const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n,
-                           double tn, double rn, int precision,
-                           float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts, double* round_poses,
-                           const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, int32_t* out_fit,
-                           double* hyp_poses, void* stream) {
-    const char* fn = "se3tn_track_hypotheses";
+                       float* out_trans, float* out_rot, double* poses_out, const se3tn_track_opts* opts,
+                       const se3tn_track_arrays* arrays, void* stream) {
+    const char* fn = "se3tn_track_render";
     const std::string f(fn);
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_rgb || !frame_depth || !K || !poses_in || !object_width || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
-    if (!out_trans || !out_rot || !poses_out || !out_choice || !out_fit) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    if (!out_trans || !out_rot || !poses_out) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
     RenderSpec r;
     int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
     if (rc) return rc;
     Step st{};
-    if ((rc = track_opts(c, fn, opts, true, st))) return rc;
-    if ((rc = hypothesis_opts(c, fn, hyp, draw_keys, n, true, st))) return rc;
+    if ((rc = track_opts(c, fn, opts, true, n, st))) return rc;
     bool multi = false;
     if ((rc = check_step(c, fn, weight_ids_host, weight_ids_dev, n, true, &multi, precision))) return rc;
+    // The struct is read on the host.  A device pointer in its place (a caller built against a header whose se3tn_track_render
+    // took a device round_poses there) is refused rather than dereferenced.
+    if (arrays) {
+        cudaPointerAttributes where{};
+        if (cudaPointerGetAttributes(&where, arrays) != cudaSuccess) cudaGetLastError();   // unknown to the runtime: host memory
+        else if (where.type == cudaMemoryTypeDevice)
+            return fail(c, SE3TN_ERR_INVALID, f + ": arrays points to device memory; se3tn_track_arrays is HOST memory whose fields "
+                        "(round_poses and the other outputs) point to the device");
+    }
+    const se3tn_track_arrays a = arrays ? *arrays : se3tn_track_arrays{};
+    if ((rc = track_arrays(c, fn, a, st, false, n, poses_in, poses_out, out_trans, out_rot))) return rc;
     if (n == 0) return SE3TN_OK;
     if (precision < SE3TN_PREC_TF32 || precision > SE3TN_PREC_FP16) return fail(c, SE3TN_ERR_INVALID, f + ": unknown precision");
-    const size_t nn = static_cast<size_t>(n), rows = nn * st.hyp.S;
-    rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_trans, nn * 12}, {out_rot, nn * 12}, {out_choice, nn * 4},
-                                {out_fit, nn * 4 * kFitCols}, {hyp_poses, rows * 128}, {round_poses, st.iterations * rows * 128}},
-                        {{poses_out == poses_in ? nullptr : poses_in, nn * 128}, {draw_keys, nn * 8}},
-                        "the starts are drawn from poses_in and draw_keys; poses_out may be poses_in itself");
-    if (rc) return rc;
     DeviceGuard guard(c->device);
-    st.hyp.poses_in = poses_in; st.hyp.wid_in = weight_ids_dev; st.hyp.width_in = object_width;
-    st.hyp.poses_out = poses_out; st.hyp.trans_out = out_trans; st.hyp.rot_out = out_rot; st.hyp.choice = out_choice; st.hyp.fit_out = out_fit;
-    return run_hypotheses(c, st, r, frame_rgb, frame_depth, H, W, K, weight_ids_host, multi, n, tn, rn, precision, hyp_poses, round_poses,
-                          static_cast<cudaStream_t>(stream));
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (st.hyp.S) {
+        st.hyp.poses_in = poses_in; st.hyp.keys = a.draw_keys; st.hyp.wid_in = weight_ids_dev; st.hyp.width_in = object_width;
+        st.hyp.poses_out = poses_out; st.hyp.trans_out = out_trans; st.hyp.rot_out = out_rot; st.hyp.choice = a.out_choice;
+        st.hyp.fit_out = a.out_fit;
+        return run_hypotheses(c, st, r, frame_rgb, frame_depth, H, W, K, weight_ids_host, multi, n, tn, rn, precision, a.hyp_poses,
+                              a.round_poses, s);
+    }
+    st.icp.poses = a.icp_poses; st.icp.stats = a.out_icp;
+    track_step(st, H, W, K, weight_ids_host, multi, n, tn, rn, precision);
+    st.frame_rgb = frame_rgb; st.frame_depth = frame_depth; st.poses_in = poses_in; st.object_width = object_width;
+    st.wid_dev = weight_ids_dev; st.out_trans = out_trans; st.out_rot = out_rot; st.poses_out = poses_out;
+    st.round_poses = a.round_poses;
+    if ((rc = render_into_scratch(c, r, st))) return rc;
+    return run_step(c, st, s);
 }
 
 int se3tn_draw_hypotheses(se3tn_ctx* c, const double* poses_in, const int64_t* draw_keys, int n, const se3tn_hypothesis_opts* hyp,
@@ -1850,8 +1834,9 @@ int se3tn_draw_hypotheses(se3tn_ctx* c, const double* poses_in, const int64_t* d
     if (!c) return SE3TN_ERR_INVALID;
     if (!poses_in || !out_poses) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument");
     Step st{};
-    int rc = hypothesis_opts(c, fn, hyp, draw_keys, n, false, st);
+    int rc = hypothesis_opts(c, fn, "hyp", hyp, n, st);
     if (rc) return rc;
+    if (st.hyp.S > 1 && !draw_keys) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": draw_keys is NULL with hyp->hypotheses > 1");
     if (n == 0) return SE3TN_OK;
     const size_t nn = static_cast<size_t>(n), rows = nn * st.hyp.S;
     rc = check_disjoint(c, fn, {{out_poses, rows * 128}, {out_draws, rows * 8 * kHypDraws}}, {{poses_in, nn * 128}, {draw_keys, nn * 8}},
@@ -2258,20 +2243,14 @@ inline void host_crop_window(const double* pose, const double* K, double width, 
 int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                     const double* poses, const double* object_width, const uint8_t* rgbA, const uint16_t* depthA, const RenderSpec* render,
                     const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                    double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit, void* stream,
-                    const int64_t* draw_keys = nullptr, const se3tn_hypothesis_opts* hyp = nullptr, int32_t* out_choice = nullptr,
-                    const se3tn_icp_opts* icp = nullptr, double* out_icp = nullptr) {
+                    double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, const se3tn_track_arrays* arrays,
+                    void* stream) {
     bool multi = false;
-    Step st{};                                     // options and ids are checked before anything is staged or copied
-    int rc = track_opts(c, fn, opts, render != nullptr, st);
+    Step st{};                                     // options, arrays and ids are checked before anything is staged or copied
+    int rc = track_opts(c, fn, opts, render != nullptr, n, st);
     if (rc) return rc;
-    if (icp) {                                     // the block is allocated on the context's device before anything is queued
-        DeviceGuard guard(c->device);
-        if ((rc = icp_opts(c, fn, icp, st))) return rc;
-    }
-    if (hyp && (rc = hypothesis_opts(c, fn, hyp, draw_keys, n, true, st))) return rc;
-    if (!st.fit_tau != !out_fit)
-        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": out_fit is required with opts->fit_tau_mm and must be NULL without it");
+    const se3tn_track_arrays a = arrays ? *arrays : se3tn_track_arrays{};
+    if ((rc = track_arrays(c, fn, a, st, true, n, nullptr, nullptr, nullptr, nullptr))) return rc;
     rc = check_step(c, fn, weight_ids, weight_ids, n, render != nullptr, &multi, precision);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
@@ -2299,10 +2278,10 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     const size_t nn = static_cast<size_t>(n), a_img = render ? 0 : img;
     // a hypothesis step's draw keys go up with the poses, its choices come back behind the fit rows
     const size_t o_ow = align256(nn * 128), o_rgbA = o_ow + align256(nn * 8), o_depthA = o_rgbA + align256(nn * a_img * 3),
-                 o_key = o_depthA + align256(nn * a_img * 2), o_wid = o_key + (hyp ? align256(nn * 8) : 0), in_bytes = o_wid + align256(nn * 4);
+                 o_key = o_depthA + align256(nn * a_img * 2), o_wid = o_key + (st.hyp.S ? align256(nn * 8) : 0), in_bytes = o_wid + align256(nn * 4);
     const size_t o_tr = align256(nn * 128), o_ro = o_tr + align256(nn * 12), o_fit = o_ro + align256(nn * 12);
     const size_t o_choice = st.fit_tau ? o_fit + align256(nn * 4 * kFitCols) : o_fit;   // the fit check's rows come back too
-    const size_t o_icp = hyp ? o_choice + align256(nn * 4) : o_choice;      // ICP's stats rows come back last
+    const size_t o_icp = st.hyp.S ? o_choice + align256(nn * 4) : o_choice;      // ICP's stats rows come back last
     const size_t out_bytes = st.icp.iterations ? o_icp + nn * 8 * kIcpCols : o_icp;
     uint8_t* d_in = d;
     double* d_poses = reinterpret_cast<double*>(d_in);
@@ -2362,12 +2341,12 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
         memcpy(hp + o_rgbA, rgbA, nn * img * 3);
         memcpy(hp + o_depthA, depthA, nn * img * 2);
     }
-    if (hyp && draw_keys) memcpy(hp + o_key, draw_keys, nn * 8);
+    if (a.draw_keys) memcpy(hp + o_key, a.draw_keys, nn * 8);
     if (weight_ids) memcpy(hp + o_wid, weight_ids, nn * 4);
     CU_TRY(c, cudaMemcpyAsync(d_in, hp, weight_ids ? in_bytes : o_wid, cudaMemcpyHostToDevice, s));
     hp += in_bytes;
-    if (hyp) {                                   // the n x S rows' fit rows stay in the context's block; the chosen ones come back
-        st.hyp.poses_in = d_poses; st.hyp.keys = draw_keys ? reinterpret_cast<const int64_t*>(d_in + o_key) : nullptr;
+    if (st.hyp.S) {                              // the n x S rows' fit rows stay in the context's block; the chosen ones come back
+        st.hyp.poses_in = d_poses; st.hyp.keys = a.draw_keys ? reinterpret_cast<const int64_t*>(d_in + o_key) : nullptr;
         st.hyp.wid_in = weight_ids ? d_wid : nullptr; st.hyp.width_in = d_ow;
         st.hyp.poses_out = d_out; st.hyp.trans_out = d_tr; st.hyp.rot_out = d_ro; st.hyp.choice = d_choice; st.hyp.fit_out = d_fit;
         rc = run_hypotheses(c, st, *render, d_rgb, d_depth, H, W, K, weight_ids, multi, n, tn, rn, precision, nullptr, nullptr, s);
@@ -2383,14 +2362,14 @@ int track_host_step(se3tn_ctx* c, const char* fn, const uint8_t* frame_rgb, cons
     }
     if (rc) return rc;
     uint8_t* ho = hp;                                            // outputs come back through the same pinned block
-    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau || out_icp) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
+    CU_TRY(c, cudaMemcpyAsync(ho, d_res, (out_trans || out_rot || st.fit_tau || a.out_icp) ? out_bytes : nn * 128, cudaMemcpyDeviceToHost, s));
     CU_TRY(c, cudaStreamSynchronize(s));
     memcpy(poses_out, ho, nn * 128);
     if (out_trans) memcpy(out_trans, ho + o_tr, nn * 12);
     if (out_rot) memcpy(out_rot, ho + o_ro, nn * 12);
-    if (out_fit) memcpy(out_fit, ho + o_fit, nn * 4 * kFitCols);
-    if (out_choice) memcpy(out_choice, ho + o_choice, nn * 4);
-    if (out_icp) memcpy(out_icp, ho + o_icp, nn * 8 * kIcpCols);
+    if (a.out_fit) memcpy(a.out_fit, ho + o_fit, nn * 4 * kFitCols);
+    if (a.out_choice) memcpy(a.out_choice, ho + o_choice, nn * 4);
+    if (a.out_icp) memcpy(a.out_icp, ho + o_icp, nn * 8 * kIcpCols);
     return SE3TN_OK;
 }
 }  // namespace
@@ -2409,8 +2388,8 @@ int se3tn_track_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* fra
 int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
                             const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
                             const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                            void* stream) {
+                            double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts,
+                            const se3tn_track_arrays* arrays, void* stream) {
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_track_render_host: null argument or empty frame");
@@ -2418,41 +2397,7 @@ int se3tn_track_render_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16
     const int rc = render_spec(c, "se3tn_track_render_host", render_mode, render_H, render_W, r);
     if (rc) return rc;
     return track_host_step(c, "se3tn_track_render_host", frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r,
-                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, out_fit, stream);
-}
-
-int se3tn_track_icp_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
-                         const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
-                         const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                         double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                         const se3tn_icp_opts* icp, double* out_icp, void* stream) {
-    const char* fn = "se3tn_track_icp_host";
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument or empty frame");
-    RenderSpec r;
-    const int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    return track_host_step(c, fn, frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r, weight_ids, n, tn, rn,
-                           precision, poses_out, out_trans, out_rot, opts, out_fit, stream, nullptr, nullptr, nullptr, icp,
-                           icp ? out_icp : nullptr);
-}
-
-int se3tn_track_hypotheses_host(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* frame_depth, int H, int W, const double* K,
-                                const double* poses, const double* object_width, int render_mode, int render_H, int render_W,
-                                const int32_t* weight_ids, int n, double tn, double rn, int precision,
-                                double* poses_out, float* out_trans, float* out_rot, const se3tn_track_opts* opts, int32_t* out_fit,
-                                const int64_t* draw_keys, const se3tn_hypothesis_opts* hyp, int32_t* out_choice, void* stream) {
-    const char* fn = "se3tn_track_hypotheses_host";
-    if (!c) return SE3TN_ERR_INVALID;
-    if (!frame_rgb || !frame_depth || !K || !poses || !object_width || !poses_out || H <= 0 || W <= 0)
-        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": null argument or empty frame");
-    if (!hyp || !out_choice) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": hyp and out_choice are required");
-    RenderSpec r;
-    const int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    return track_host_step(c, fn, frame_rgb, frame_depth, H, W, K, poses, object_width, nullptr, nullptr, &r, weight_ids, n, tn, rn,
-                           precision, poses_out, out_trans, out_rot, opts, out_fit, stream, draw_keys, hyp, out_choice);
+                           weight_ids, n, tn, rn, precision, poses_out, out_trans, out_rot, opts, arrays, stream);
 }
 
 int se3tn_allgather_poses(se3tn_ctx* c, void* nccl_comm, const double* local_poses, double* all_poses, int n_local, void* stream) {

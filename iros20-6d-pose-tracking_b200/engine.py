@@ -26,6 +26,12 @@ def _hptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)
 
 
+def _track_arrays(ptr, **fields):
+    """An se3tn_track_arrays by reference: the given CUDA tensors (ptr=_ptr) or numpy arrays (ptr=_hptr); None and absent fields
+    are NULL."""
+    return C.byref(_lib.TrackArrays(**{k: ptr(v).value for k, v in fields.items()}))
+
+
 def _stream(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -270,7 +276,7 @@ class Engine:
         """n independent tracks of one frame: K0 -> conv stack -> K6, all enqueued on the current stream.  fill_depth: the
         observed depth is hole-filled inside the step first (depth_fill_spec); frame_depth itself is never written."""
         return self._track('track_batch', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
-                           rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, 1)
+                           rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, 1)[:3]
 
     def track_render(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                      weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', mode='vispy', image_hw=None,
@@ -282,24 +288,29 @@ class Engine:
         out_poses may be poses itself: the tracks' poses are then updated in place (include/se3tn.h).  iterations: k rounds
         of render -> network -> pose update on this frame in the one step, exactly what k chained calls with iterations=1
         compute (se3tn_track_opts.iterations, 1..8); out_trans / out_rot hold the last round's outputs.  out_rounds: a float64
-        CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_render's round_poses): entry
+        CUDA tensor (k, n, 4, 4) that receives every round's poses from the same step (se3tn_track_arrays.round_poses): entry
         r - 1 is what a call with iterations=r returns.  The step with it is a CUDA graph of its own.  fit: tau in mm (fit_spec)
         turns on the fit check of the step (se3tn_track_opts.fit_tau_mm): every track's model is drawn at its new pose and
         compared with the observed depth, and the call returns a fourth value, out_fit: an int32 CUDA tensor (n, 6) of the rows
         (model, observed, inlier, front, behind, residual), allocated when None and filled on the current stream.  icp (icp_spec):
         M iterations of point-to-plane ICP against the observed depth after the last round and before the fit check
-        (se3tn_track_icp); the call then also returns the last iteration's stats, a float64 CUDA tensor (n, 4) of inliers,
+        (se3tn_track_opts.icp); the call then also returns the last iteration's stats, a float64 CUDA tensor (n, 4) of inliers,
         rms_mm, step_mm, step_deg, after the fit rows when the fit is on (out_icp, allocated when None; the step itself writes an
         Engine-owned block, so its graph is replayed frame after frame).  out_icp_poses: a float64 CUDA tensor (M, n, 4, 4) that
         receives the poses after every ICP iteration."""
-        return self._track('track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
-                           trans_normalizer, rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot,
-                           fill_depth, iterations, out_rounds, fit, out_fit, icp, out_icp_poses, out_icp)
+        P, tr, ro, rows, stats, _ = self._track(
+            'track_render', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw), trans_normalizer,
+            rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, fit,
+            icp=icp, out_rounds=out_rounds, out_fit=out_fit, out_icp_poses=out_icp_poses, out_icp=out_icp)
+        return (P, tr, ro) + tuple(x for x in (rows, stats) if x is not None)
 
     def _track(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, out_rounds=None,
-               fit=None, out_fit=None, icp=None, out_icp_poses=None, out_icp=None):
-        """track_batch (A = (rgbA, depthA), render None) and track_render (A = (), render = _render_mode's triple)."""
+               weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, fit=None,
+               icp=None, hyp=None, draw_keys=None, out_rounds=None, out_fit=None, out_icp_poses=None, out_icp=None, out_choice=None,
+               out_hyp_poses=None):
+        """The device route of every tracking method, one C call: track_batch (A = (rgbA, depthA), render None), track_render
+        and track_hypotheses (A = (), render = _render_mode's triple; hyp: hypothesis_spec's options).  -> (poses, trans, rot,
+        fit rows, ICP stats, choice), each of the last three None when the step has none."""
         n = poses.shape[0]
         iterations = self.refine_iterations(iterations)
         tau = self.fit_spec(fit)
@@ -307,46 +318,47 @@ class Engine:
         if icp is None and out_icp_poses is not None:
             raise ValueError('%s: out_icp_poses needs icp' % fn)
         self._check_frame(fn, frame_rgb, frame_depth, poses, object_width, A, n)
+        S = 1 if hyp is None else hyp.hypotheses
+        if n * S > self.max_batch:
+            raise ValueError('n x hypotheses = %d exceeds max_batch=%d' % (n * S, self.max_batch))
         wh = self._host_ids(fn, weight_ids_host, n)
         fill = self.depth_fill_spec(fill_depth)
         Kh = self._k4(K)
+        new = lambda shape, dt, t: torch.empty(*shape, dtype=dt, device=self.device) if t is None else t
         out_poses = torch.empty_like(poses) if out_poses is None else out_poses
-        out_trans = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_trans is None else out_trans
-        out_rot = torch.empty(n, 3, dtype=torch.float32, device=self.device) if out_rot is None else out_rot
+        out_trans, out_rot = new((n, 3), torch.float32, out_trans), new((n, 3), torch.float32, out_rot)
         if wh is not None and weight_ids_dev is None:
             weight_ids_dev = torch.from_numpy(wh).to(self.device)
-        if out_rounds is not None:
-            self._check_dev('out_rounds', out_rounds, torch.float64, (iterations, n, 4, 4))
-        if tau:
-            out_fit = torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=self.device) if out_fit is None else out_fit
-            self._check_dev('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS))
-        if icp is not None:
-            out_icp = torch.empty(n, _lib.ICP_COLS, dtype=torch.float64, device=self.device) if out_icp is None else out_icp
-            self._check_dev('out_icp', out_icp, torch.float64, (n, _lib.ICP_COLS))
-            if getattr(self, '_icp_rows', None) is None:
-                self._icp_rows = torch.empty(self.max_batch, _lib.ICP_COLS, dtype=torch.float64, device=self.device)
-            if out_icp_poses is not None:
-                self._check_dev('out_icp_poses', out_icp_poses, torch.float64, (icp.iterations, n, 4, 4))
+        out_fit = new((n, _lib.FIT_COLS), torch.int32, out_fit) if tau or hyp is not None else None
+        out_choice = new((n,), torch.int32, out_choice) if hyp is not None else None
+        out_icp = new((n, _lib.ICP_COLS), torch.float64, out_icp) if icp is not None else None
+        if icp is not None and getattr(self, '_icp_rows', None) is None:
+            self._icp_rows = torch.empty(self.max_batch, _lib.ICP_COLS, dtype=torch.float64, device=self.device)
+        for name, t, dt, shape in (('draw_keys', draw_keys, torch.int64, (n,)),
+                                   ('out_rounds', out_rounds, torch.float64, (iterations, n) + (() if hyp is None else (S,)) + (4, 4)),
+                                   ('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS)), ('out_choice', out_choice, torch.int32, (n,)),
+                                   ('out_hyp_poses', out_hyp_poses, torch.float64, (n, S, 4, 4)),
+                                   ('out_icp', out_icp, torch.float64, (n, _lib.ICP_COLS)),
+                                   ('out_icp_poses', out_icp_poses, torch.float64, (0 if icp is None else icp.iterations, n, 4, 4))):
+            if t is not None:
+                self._check_dev(name, t, dt, shape)
         H, W = frame_depth.shape
         head = (self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(Kh), _ptr(poses), _ptr(object_width))
         tail = (_hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
-                _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), self._track_opts(fill, iterations, tau))
+                _ptr(out_trans), _ptr(out_rot), _ptr(out_poses), self._track_opts(fill, iterations, tau, icp, hyp))
         if render is None:
             rc = self.lib.se3tn_track_batch(*head, *map(_ptr, A), *tail, _stream(self.device))
-        elif icp is None:
-            rc = self.lib.se3tn_track_render(*head, *render, *tail, _ptr(out_rounds), _stream(self.device))
-        else:
-            rc = self.lib.se3tn_track_icp(*head, *render, *tail, _ptr(out_rounds), C.byref(icp), _ptr(out_icp_poses),
-                                          _ptr(self._icp_rows), _stream(self.device))
+        else:                                            # without hypotheses the step's fit rows stay in the context's block
+            arrays = _track_arrays(_ptr, draw_keys=draw_keys, round_poses=out_rounds, hyp_poses=out_hyp_poses,
+                                   icp_poses=out_icp_poses, out_fit=out_fit if hyp is not None else None, out_choice=out_choice,
+                                   out_icp=self._icp_rows if icp is not None else None)
+            rc = self.lib.se3tn_track_render(*head, *render, *tail, arrays, _stream(self.device))
         _lib.check(rc, self._ctx)
-        res = (out_poses, out_trans, out_rot)
-        if tau:
+        if tau and hyp is None:
             out_fit.copy_(self._fit_rows_view()[:n])     # the next step overwrites the context's rows
-            res += (out_fit,)
         if icp is not None:
             out_icp.copy_(self._icp_rows[:n])            # the next ICP step overwrites the Engine's rows
-            res += (out_icp,)
-        return res
+        return out_poses, out_trans, out_rot, out_fit, out_icp, out_choice
 
     def track_host(self, frame_rgb, frame_depth, K, poses, object_width, rgbA, depthA, trans_normalizer, rot_normalizer,
                    weight_ids=None, precision='bf16x3', want_residuals=False, fill_depth=None):
@@ -354,8 +366,9 @@ class Engine:
         frame_rgb uint8 (H,W,3), frame_depth uint16 (H,W), poses float64 (n,4,4), object_width float64 (n), rgbA uint8
         (n,176,176,3), depthA uint16 (n,176,176), weight_ids int32 (n) or None -- all C-contiguous.  fill_depth as in
         track_batch: a live sensor's raw depth frame goes in as it is (the whole frame is uploaded then)."""
-        return self._track_host('track_host', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None, trans_normalizer,
-                                rot_normalizer, weight_ids, precision, want_residuals, fill_depth, 1)
+        out, tr, ro, *_ = self._track_host('track_host', frame_rgb, frame_depth, K, poses, object_width, (rgbA, depthA), None,
+                                           trans_normalizer, rot_normalizer, weight_ids, precision, want_residuals, fill_depth, 1)
+        return (out, tr, ro) if want_residuals else out
 
     def track_render_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer,
                           weight_ids=None, precision='bf16x3', mode='vispy', image_hw=None, want_residuals=False, fill_depth=None,
@@ -364,15 +377,19 @@ class Engine:
         the frame are all it takes.  Arguments as track_host without rgbA / depthA; track i draws mesh weight_ids[i] (mesh 0
         without ids); mode / image_hw as in render(); iterations as in track_render (k > 1 uploads the whole frame).  fit as in
         track_render (the whole depth frame is uploaded then): the fit rows come last in what the call returns, an int32 numpy
-        array (n, 6).  icp as in track_render (se3tn_track_icp_host; the whole depth frame is uploaded then): its stats come last,
-        a float64 numpy array (n, 4)."""
-        return self._track_host('track_render_host', frame_rgb, frame_depth, K, poses, object_width, (),
-                                self._render_mode(mode, image_hw), trans_normalizer, rot_normalizer, weight_ids, precision,
-                                want_residuals, fill_depth, iterations, fit, icp)
+        array (n, 6).  icp as in track_render (the whole depth frame is uploaded then): its stats come last, a float64 numpy
+        array (n, 4)."""
+        out, tr, ro, rows, stats, _ = self._track_host(
+            'track_render_host', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
+            trans_normalizer, rot_normalizer, weight_ids, precision, want_residuals, fill_depth, iterations, fit, icp)
+        res = ((out, tr, ro) if want_residuals else (out,)) + tuple(x for x in (rows, stats) if x is not None)
+        return res if len(res) > 1 else out
 
     def _track_host(self, fn, frame_rgb, frame_depth, K, poses, object_width, A, render, trans_normalizer, rot_normalizer,
-                    weight_ids, precision, want_residuals, fill_depth, iterations, fit=None, icp=None):
-        """track_host (A = (rgbA, depthA), render None) and track_render_host (A = (), render = _render_mode's triple)."""
+                    weight_ids, precision, want_residuals, fill_depth, iterations, fit=None, icp=None, hyp=None, draw_keys=None):
+        """The host route of every tracking method, one C call: track_host (A = (rgbA, depthA), render None),
+        track_render_host and track_hypotheses_host (A = (), render = _render_mode's triple; hyp: hypothesis_spec's options).
+        -> (poses, trans, rot, fit rows, ICP stats, choice) as numpy arrays, each None when the call has none."""
         n = int(poses.shape[0])
         iterations = self.refine_iterations(iterations)
         tau = self.fit_spec(fit)
@@ -380,32 +397,30 @@ class Engine:
         for name, a, dt, shape in self._track_inputs(fn, frame_rgb, frame_depth, poses, object_width, A, n):
             if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
                 raise ValueError('%s: %s must be a C-contiguous %s array of shape %s' % (fn, name, dt, shape))
+        if draw_keys is not None:
+            draw_keys = np.ascontiguousarray(draw_keys, dtype=np.int64)
+            if draw_keys.shape != (n,):
+                raise ValueError('%s: draw_keys must have one entry per track' % fn)
         wid = self._host_ids(fn, weight_ids, n)
         fill = self.depth_fill_spec(fill_depth)
         Kh = self._k4(K)
         out = np.empty((n, 4, 4), dtype=np.float64)
         tr = np.empty((n, 3), dtype=np.float32) if want_residuals else None
         ro = np.empty((n, 3), dtype=np.float32) if want_residuals else None
-        fit_rows = np.empty((n, _lib.FIT_COLS), dtype=np.int32) if tau else None
+        rows = np.empty((n, _lib.FIT_COLS), dtype=np.int32) if tau else None
+        stats = np.empty((n, _lib.ICP_COLS), dtype=np.float64) if icp is not None else None
+        choice = np.empty(n, dtype=np.int32) if hyp is not None else None
         H, W = frame_depth.shape
         head = (self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(Kh), _hptr(poses), _hptr(object_width))
         tail = (_hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision], _hptr(out), _hptr(tr), _hptr(ro),
-                self._track_opts(fill, iterations, tau))
-        icp_rows = np.empty((n, _lib.ICP_COLS), dtype=np.float64) if icp is not None else None
+                self._track_opts(fill, iterations, tau, icp, hyp))
         if render is None:
             rc = self.lib.se3tn_track_host(*head, *map(_hptr, A), *tail, _stream(self.device))
-        elif icp is None:
-            rc = self.lib.se3tn_track_render_host(*head, *render, *tail, _hptr(fit_rows), _stream(self.device))
         else:
-            rc = self.lib.se3tn_track_icp_host(*head, *render, *tail, _hptr(fit_rows), C.byref(icp), _hptr(icp_rows),
-                                               _stream(self.device))
+            arrays = _track_arrays(_hptr, draw_keys=draw_keys, out_fit=rows, out_choice=choice, out_icp=stats)
+            rc = self.lib.se3tn_track_render_host(*head, *render, *tail, arrays, _stream(self.device))
         _lib.check(rc, self._ctx)
-        res = (out, tr, ro) if want_residuals else (out,)
-        if tau:
-            res += (fit_rows,)
-        if icp is not None:
-            res += (icp_rows,)
-        return res if len(res) > 1 else out
+        return out, tr, ro, rows, stats, choice
 
     # ------------------------------------------------------------------ multi-hypothesis tracking
     @staticmethod
@@ -447,72 +462,28 @@ class Engine:
                          precision='bf16x3', mode='vispy', image_hw=None, out_poses=None, out_trans=None, out_rot=None,
                          fill_depth=None, iterations=1, out_choice=None, out_fit=None, out_hyp_poses=None, out_rounds=None):
         """track_render from S start hypotheses per track, keeping the one whose model fits the frame best
-        (se3tn_track_hypotheses), enqueued on the current stream.  draw_keys int64 (n) CUDA tensor: each track's draw key (None
+        (se3tn_track_opts.hyp), enqueued on the current stream.  draw_keys int64 (n) CUDA tensor: each track's draw key (None
         only with hypotheses=1); the spread is max_translation m / max_rotation_deg degrees; fit: tau in mm, required (fit_spec).
         -> (poses (n,4,4), choice int32 (n), fit rows int32 (n,6)), then out_hyp_poses (n,S,4,4) and out_rounds (k,n,S,4,4)
         when given (float64 CUDA tensors: every hypothesis after the last round, and after every round).  out_poses may be
         poses itself."""
-        n = int(poses.shape[0])
-        iterations = self.refine_iterations(iterations)
-        tau = self.fit_spec(fit)
         hyp = self.hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg)
-        S = hyp.hypotheses
-        self._check_frame('track_hypotheses', frame_rgb, frame_depth, poses, object_width, (), n)
-        if n * S > self.max_batch:
-            raise ValueError('n x hypotheses = %d exceeds max_batch=%d' % (n * S, self.max_batch))
-        wh = self._host_ids('track_hypotheses', weight_ids_host, n)
-        if wh is not None and weight_ids_dev is None:
-            weight_ids_dev = torch.from_numpy(wh).to(self.device)
-        if draw_keys is not None:
-            self._check_dev('draw_keys', draw_keys, torch.int64, (n,))
-        new = lambda shape, dt: torch.empty(*shape, dtype=dt, device=self.device)
-        out_poses = new((n, 4, 4), torch.float64) if out_poses is None else out_poses
-        out_trans = new((n, 3), torch.float32) if out_trans is None else out_trans
-        out_rot = new((n, 3), torch.float32) if out_rot is None else out_rot
-        out_choice = new((n,), torch.int32) if out_choice is None else out_choice
-        out_fit = new((n, _lib.FIT_COLS), torch.int32) if out_fit is None else out_fit
-        for name, t, dt, shape in (('out_choice', out_choice, torch.int32, (n,)), ('out_fit', out_fit, torch.int32, (n, _lib.FIT_COLS)),
-                                   ('out_hyp_poses', out_hyp_poses, torch.float64, (n, S, 4, 4)),
-                                   ('out_rounds', out_rounds, torch.float64, (iterations, n, S, 4, 4))):
-            if t is not None:
-                self._check_dev(name, t, dt, shape)
-        H, W = frame_depth.shape
-        rc = self.lib.se3tn_track_hypotheses(
-            self._ctx, _ptr(frame_rgb), _ptr(frame_depth), H, W, _hptr(self._k4(K)), _ptr(poses), _ptr(object_width),
-            *self._render_mode(mode, image_hw), _hptr(wh), _ptr(weight_ids_dev), n, float(trans_normalizer), float(rot_normalizer),
-            PREC[precision], _ptr(out_trans), _ptr(out_rot), _ptr(out_poses),
-            self._track_opts(self.depth_fill_spec(fill_depth), iterations, tau), _ptr(out_rounds), _ptr(draw_keys), C.byref(hyp),
-            _ptr(out_choice), _ptr(out_fit), _ptr(out_hyp_poses), _stream(self.device))
-        _lib.check(rc, self._ctx)
-        return (out_poses, out_choice, out_fit) + tuple(t for t in (out_hyp_poses, out_rounds) if t is not None)
+        P, _, _, rows, _, choice = self._track(
+            'track_hypotheses', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw), trans_normalizer,
+            rot_normalizer, weight_ids_host, weight_ids_dev, precision, out_poses, out_trans, out_rot, fill_depth, iterations, fit,
+            hyp=hyp, draw_keys=draw_keys, out_rounds=out_rounds, out_fit=out_fit, out_choice=out_choice, out_hyp_poses=out_hyp_poses)
+        return (P, choice, rows) + tuple(t for t in (out_hyp_poses, out_rounds) if t is not None)
 
     def track_hypotheses_host(self, frame_rgb, frame_depth, K, poses, object_width, trans_normalizer, rot_normalizer, draw_keys,
                               hypotheses, max_translation, max_rotation_deg, seed=0, fit=None, weight_ids=None, precision='bf16x3',
                               mode='vispy', image_hw=None, fill_depth=None, iterations=1):
-        """track_hypotheses with numpy arrays in and out, synchronous (se3tn_track_hypotheses_host): arguments as
+        """track_hypotheses with numpy arrays in and out, synchronous (se3tn_track_render_host): arguments as
         track_render_host, draw_keys int64 (n) numpy or None (hypotheses=1).  -> (poses (n,4,4), choice int32 (n), fit rows
         int32 (n,6))."""
-        n = int(poses.shape[0])
-        iterations = self.refine_iterations(iterations)
-        tau = self.fit_spec(fit)
         hyp = self.hypothesis_spec(hypotheses, seed, max_translation, max_rotation_deg)
-        for name, a, dt, shape in self._track_inputs('track_hypotheses_host', frame_rgb, frame_depth, poses, object_width, (), n):
-            if not (isinstance(a, np.ndarray) and a.dtype == dt and a.shape == shape and a.flags['C_CONTIGUOUS']):
-                raise ValueError('track_hypotheses_host: %s must be a C-contiguous %s array of shape %s' % (name, dt, shape))
-        keys = None if draw_keys is None else np.ascontiguousarray(draw_keys, dtype=np.int64)
-        if keys is not None and keys.shape != (n,):
-            raise ValueError('track_hypotheses_host: draw_keys must have one entry per track')
-        wid = self._host_ids('track_hypotheses_host', weight_ids, n)
-        out = np.empty((n, 4, 4), dtype=np.float64)
-        choice = np.empty(n, dtype=np.int32)
-        rows = np.empty((n, _lib.FIT_COLS), dtype=np.int32)
-        H, W = frame_depth.shape
-        rc = self.lib.se3tn_track_hypotheses_host(
-            self._ctx, _hptr(frame_rgb), _hptr(frame_depth), H, W, _hptr(self._k4(K)), _hptr(poses), _hptr(object_width),
-            *self._render_mode(mode, image_hw), _hptr(wid), n, float(trans_normalizer), float(rot_normalizer), PREC[precision],
-            _hptr(out), None, None, self._track_opts(self.depth_fill_spec(fill_depth), iterations, tau), _hptr(rows), _hptr(keys),
-            C.byref(hyp), _hptr(choice), _stream(self.device))
-        _lib.check(rc, self._ctx)
+        out, _, _, rows, _, choice = self._track_host(
+            'track_hypotheses_host', frame_rgb, frame_depth, K, poses, object_width, (), self._render_mode(mode, image_hw),
+            trans_normalizer, rot_normalizer, weight_ids, precision, False, fill_depth, iterations, fit, hyp=hyp, draw_keys=draw_keys)
         return out, choice, rows
 
     # ------------------------------------------------------------------ checkpoint validation
@@ -984,12 +955,14 @@ class Engine:
         return _lib.IcpOpts(iterations=int(spec['iterations']), tau_mm=int(spec['tau_mm']), min_inliers=int(spec['min_inliers']))
 
     @staticmethod
-    def _track_opts(fill, iterations, tau):
-        """The se3tn_track_opts of one tracking call, by reference: depth_fill_spec's tuple, the refinement count and the fit
-        check's tau.  Every call passes all of them, so Trackers that share an Engine each get their own."""
+    def _track_opts(fill, iterations, tau, icp=None, hyp=None):
+        """The se3tn_track_opts of one tracking call, by reference: depth_fill_spec's tuple, the refinement count, the fit
+        check's tau, and icp_spec's and hypothesis_spec's options or None.  Every call passes all of them, so Trackers that
+        share an Engine each get their own.  The reference keeps the struct, and the struct the options it points to, alive."""
         on, max_depth, extrapolate, blur = fill
+        ref = lambda o: None if o is None else C.pointer(o)
         return C.byref(_lib.TrackOpts(fill_depth=on, fill_extrapolate=extrapolate, fill_blur=blur, iterations=iterations,
-                                      fill_max_depth=max_depth, fit_tau_mm=tau))
+                                      fill_max_depth=max_depth, fit_tau_mm=tau, icp=ref(icp), hyp=ref(hyp)))
 
     def _fit_rows_view(self):
         """An int32 CUDA tensor (max_batch, 6) over the context's fit rows (se3tn_fit_rows; the address never changes)."""

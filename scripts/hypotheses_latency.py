@@ -1,6 +1,6 @@
 """Per-frame time of multi-hypothesis tracking (Tracker(hypotheses=S)), bf16x3, S in {1, 4, 8, 16} x n in {1, 8} tracks x k in {1, 2}
-refinement rounds, through Tracker.on_track_batch on numpy inputs (the host route: one synchronous se3tn_track_hypotheses_host
-call per frame; S = 1 is the plain step with the fit check, se3tn_track_render_host).  For each (n, k) the Trackers of every S
+refinement rounds, through Tracker.on_track_batch on numpy inputs (the host route: one synchronous se3tn_track_render_host
+call per frame, with opts->hyp for S > 1; S = 1 is the plain step with the fit check).  For each (n, k) the Trackers of every S
 share one Engine and alternate frame by frame in one process, so all see the same card state.  The card's name and power limit
 are printed first: the numbers belong to them.
 

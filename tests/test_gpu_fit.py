@@ -193,9 +193,10 @@ def test_meaning_with_a_zero_head(synth, eng):
 def _raw_track_render_host(e, c, out, opts, out_fit):
     Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
     h = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+    arrays = importlib.import_module(PKG + '._lib').TrackArrays(out_fit=None if out_fit is None else out_fit.ctypes.data)
     return e.lib.se3tn_track_render_host(e._ctx, h(c.rgb), h(c.depth), HW[0], HW[1], h(Kh), h(c.poses), h(np.full(c.n, 200.0)), 0, 0, 0,
-                                         h(c.wid), c.n, TN, RN, 2, h(out[0]), h(out[1]), h(out[2]), C.byref(opts), h(out_fit),
-                                         C.c_void_p(0))
+                                         h(c.wid), c.n, TN, RN, 2, h(out[0]), h(out[1]), h(out[2]), C.byref(opts),
+                                         C.byref(arrays), C.c_void_p(0))
 
 
 def test_refusals(synth, eng):

@@ -1,7 +1,8 @@
-"""Multi-hypothesis tracking on the device (se3tn_track_hypotheses[_host], se3tn_draw_hypotheses, Engine.track_hypotheses,
+"""Multi-hypothesis tracking on the device (se3tn_track_opts.hyp, se3tn_draw_hypotheses, Engine.track_hypotheses,
 Tracker(hypotheses=)): the starts equal oracle/hypotheses_ref.py, every hypothesis is a plain track_render step over the expanded
 starts bit for bit, the choice follows the fit rule, S = 1 is the plain step, a zero head recovers the hypothesis the frame shows,
 one graph replays with fresh keys, and the refusals queue nothing."""
+import ctypes as C
 import importlib
 import os
 import sys
@@ -56,6 +57,31 @@ def keep_utils_engine():
 
 def _dev(e, a):
     return torch.from_numpy(np.ascontiguousarray(a)).to(e.device)
+
+
+def _addr(t):
+    return None if t is None else (t.data_ptr() if torch.is_tensor(t) else t.ctypes.data)
+
+
+def _raw_render(e, c, opts, arrays, poses_out, P=None, n=None, trans=None):
+    """se3tn_track_render on Case c's device frame and tracks with these options and arrays (a TrackArrays, or a raw address),
+    past Engine's own checks."""
+    E = importlib.import_module(PKG + '.engine')
+    n = c.n if n is None else n
+    trans = torch.empty(n, 3, device=e.device) if trans is None else trans
+    return e.lib.se3tn_track_render(
+        e._ctx, E._ptr(c.R), E._ptr(c.D), HW[0], HW[1], E._hptr(E.Engine._k4(K)), E._ptr(c.P if P is None else P), E._ptr(c.ow),
+        0, 0, 0, E._hptr(c.wid), E._ptr(c.wd), n, TN, RN, 2, E._ptr(trans), E._ptr(trans.clone()), E._ptr(poses_out),
+        C.byref(opts), arrays if isinstance(arrays, C.c_void_p) else C.byref(arrays), E._stream(e.device))
+
+
+def _raw_render_host(e, c, opts, arrays, poses_out):
+    """se3tn_track_render_host on Case c's host frame and tracks with these options and arrays."""
+    E = importlib.import_module(PKG + '.engine')
+    return e.lib.se3tn_track_render_host(
+        e._ctx, E._hptr(c.rgb), E._hptr(c.depth), HW[0], HW[1], E._hptr(E.Engine._k4(K)), E._hptr(c.poses),
+        E._hptr(np.full(c.n, 200.0)), 0, 0, 0, E._hptr(c.wid), c.n, TN, RN, 2, E._hptr(poses_out), None, None, C.byref(opts),
+        C.byref(arrays), E._stream(e.device))
 
 
 class Case:
@@ -229,16 +255,10 @@ def test_refusals_queue_nothing(synth, eng, pkg):
         a.update(over)
         hyp = L.HypothesisOpts(hypotheses=a['S'], reserved=a['reserved'], seed=a['seed'], max_translation=a['max_t'],
                                max_rotation_deg=a['max_r'])
-        E = pkg.Engine
-        tr = torch.empty(n, 3, device=eng.device)
-        ptr = importlib.import_module(PKG + '.engine')._ptr
-        hptr = importlib.import_module(PKG + '.engine')._hptr
-        rc = eng.lib.se3tn_track_hypotheses(
-            eng._ctx, ptr(c.R), ptr(c.D), HW[0], HW[1], hptr(E._k4(K)), ptr(a['P']), ptr(c.ow), 0, 0, 0, hptr(c.wid), ptr(c.wd),
-            a['n'], TN, RN, 2, ptr(tr), ptr(tr.clone()), ptr(a['poses_out']), E._track_opts((0, 0.0, 0, 0), 1, a['tau']), None,
-            ptr(a['keys']), importlib.import_module('ctypes').byref(hyp), ptr(outs['out_choice']), ptr(a['fit']), ptr(a['hyp_poses']),
-            importlib.import_module(PKG + '.engine')._stream(eng.device))
-        L.check(rc, eng._ctx)
+        arrays = L.TrackArrays(draw_keys=_addr(a['keys']), hyp_poses=_addr(a['hyp_poses']), out_fit=_addr(a['fit']),
+                               out_choice=_addr(outs['out_choice']))
+        L.check(_raw_render(eng, c, L.TrackOpts(iterations=1, fit_tau_mm=a['tau'], hyp=C.pointer(hyp)), arrays, a['poses_out'],
+                            P=a['P'], n=a['n']), eng._ctx)
 
     refused(lambda: raw(S=0), 'hyp->hypotheses')
     refused(lambda: raw(S=33), 'hyp->hypotheses')
@@ -262,6 +282,69 @@ def test_refusals_queue_nothing(synth, eng, pkg):
     torch.cuda.synchronize()
     for key, v in outs.items():
         assert torch.equal(v, snap[key]), key
+
+
+def test_option_and_array_refusals_queue_nothing(synth, eng):
+    """ICP inside a hypothesis step, and a se3tn_track_arrays field on a route or in a mode that does not take it (or missing
+    where the options need it): SE3TN_ERR_INVALID naming the field, with nothing written to any output."""
+    L = importlib.import_module(PKG + '._lib')
+    n = 3
+    c = Case(eng, synth, n, seed=81)
+    dev = dict(poses=torch.full_like(c.P, 7.0), choice=torch.full((n,), 9, dtype=torch.int32, device=eng.device),
+               fit=torch.full((n, 6), 9, dtype=torch.int32, device=eng.device), stats=torch.full((n, 4), 9.0, dtype=torch.float64,
+               device=eng.device), slots=torch.full((1, n, 4, 4), 9.0, dtype=torch.float64, device=eng.device),
+               hyps=torch.full((n, 4, 4, 4), 9.0, dtype=torch.float64, device=eng.device))
+    host = dict(poses=np.full((n, 4, 4), 7.0), choice=np.full(n, 9, np.int32), fit=np.full((n, 6), 9, np.int32),
+                stats=np.full((n, 4), 9.0), keys=np.arange(n, dtype=np.int64), slots=np.full((1, n, 4, 4), 9.0))
+    snap = [v.clone() for v in dev.values()] + [v.copy() for v in host.values()]
+    hyp = L.HypothesisOpts(hypotheses=4, seed=1, **SPREAD)
+    icp = L.IcpOpts(iterations=1, tau_mm=20, min_inliers=100)
+    opts = lambda **kw: L.TrackOpts(iterations=1, fit_tau_mm=TAU, **{k: C.pointer(v) for k, v in kw.items()})
+    with_hyp = dict(draw_keys=c.keys, out_fit=dev['fit'], out_choice=dev['choice'])
+    host_hyp = dict(draw_keys=host['keys'], out_fit=host['fit'], out_choice=host['choice'])
+    arrays = lambda **kw: L.TrackArrays(**{k: _addr(v) for k, v in kw.items()})
+    refused = lambda rc, field: rc == L.ERR_INVALID and field in eng.lib.se3tn_last_error(eng._ctx).decode()
+    cases = [                                            # (route, options, arrays, the field the error names)
+        ('dev', opts(icp=icp, hyp=hyp), arrays(**with_hyp), 'opts->icp and opts->hyp'),
+        ('host', opts(icp=icp, hyp=hyp), arrays(**host_hyp), 'opts->icp and opts->hyp'),
+        ('dev', opts(hyp=hyp), arrays(**with_hyp, icp_poses=dev['slots']), 'arrays->icp_poses'),
+        ('dev', opts(hyp=hyp), arrays(**with_hyp, out_icp=dev['stats']), 'arrays->out_icp'),
+        ('dev', opts(hyp=hyp), arrays(draw_keys=c.keys, out_fit=dev['fit']), 'arrays->out_choice'),
+        ('dev', opts(hyp=hyp), arrays(draw_keys=c.keys, out_choice=dev['choice']), 'arrays->out_fit'),
+        ('dev', opts(), arrays(out_fit=dev['fit']), 'arrays->out_fit'),
+        ('dev', opts(), arrays(out_choice=dev['choice']), 'arrays->out_choice'),
+        ('dev', opts(), arrays(draw_keys=c.keys), 'arrays->draw_keys'),
+        ('dev', opts(), arrays(hyp_poses=dev['hyps']), 'arrays->hyp_poses'),
+        ('dev', opts(icp=icp), arrays(out_fit=dev['fit']), 'arrays->out_fit'),
+        ('host', opts(hyp=hyp), arrays(**host_hyp, hyp_poses=host['slots']), 'arrays->hyp_poses'),
+        ('host', opts(), arrays(out_fit=host['fit'], round_poses=host['slots']), 'arrays->round_poses'),
+        ('host', opts(icp=icp), arrays(out_fit=host['fit'], icp_poses=host['slots']), 'arrays->icp_poses'),
+        ('host', opts(), arrays(out_fit=host['fit'], out_icp=host['stats']), 'arrays->out_icp'),
+        ('host', opts(), arrays(out_fit=host['fit'], out_choice=host['choice']), 'arrays->out_choice'),
+        ('host', opts(), arrays(out_fit=host['fit'], draw_keys=host['keys']), 'arrays->draw_keys'),
+    ]
+    for route, o, a, field in cases:
+        rc = _raw_render(eng, c, o, a, dev['poses']) if route == 'dev' else _raw_render_host(eng, c, o, a, host['poses'])
+        assert refused(rc, field), (route, field)
+    # the struct itself must be host memory: a device address in its place is refused, not read
+    assert refused(_raw_render(eng, c, opts(), C.c_void_p(dev['slots'].data_ptr()), dev['poses']), 'arrays points to device memory')
+    # input A from the caller: neither batch call takes ICP or hypotheses
+    E = importlib.import_module(PKG + '.engine')
+    ra = torch.zeros(n, 176, 176, 3, dtype=torch.uint8, device=eng.device)
+    da = torch.zeros(n, 176, 176, dtype=torch.uint16, device=eng.device)
+    tr = torch.empty(n, 3, device=eng.device)
+    for o, field in ((L.TrackOpts(iterations=1, icp=C.pointer(icp)), 'opts->icp'), (L.TrackOpts(iterations=1, hyp=C.pointer(hyp)), 'opts->hyp')):
+        rc = eng.lib.se3tn_track_batch(eng._ctx, E._ptr(c.R), E._ptr(c.D), HW[0], HW[1], E._hptr(E.Engine._k4(K)), E._ptr(c.P),
+                                       E._ptr(c.ow), E._ptr(ra), E._ptr(da), E._hptr(c.wid), E._ptr(c.wd), n, TN, RN, 2, E._ptr(tr),
+                                       E._ptr(tr.clone()), E._ptr(dev['poses']), C.byref(o), E._stream(eng.device))
+        assert refused(rc, field)
+        rc = eng.lib.se3tn_track_host(eng._ctx, E._hptr(c.rgb), E._hptr(c.depth), HW[0], HW[1], E._hptr(E.Engine._k4(K)),
+                                      E._hptr(c.poses), E._hptr(np.full(n, 200.0)), E._hptr(ra.cpu().numpy()), E._hptr(da.cpu().numpy()),
+                                      E._hptr(c.wid), n, TN, RN, 2, E._hptr(host['poses']), None, None, C.byref(o), E._stream(eng.device))
+        assert refused(rc, field)
+    torch.cuda.synchronize()
+    for want, got in zip(snap, list(dev.values()) + list(host.values())):
+        assert (torch.equal(want, got) if torch.is_tensor(want) else np.array_equal(want, got))
 
 
 def _tracker(pkg, synth, tmp_path, **kw):

@@ -1,4 +1,4 @@
-"""The depth refinement of a tracking step (se3tn_track_icp[_host], Engine.track_render(icp=), Tracker(icp=)): ICP off is
+"""The depth refinement of a tracking step (se3tn_track_opts.icp, Engine.track_render(icp=), Tracker(icp=)): ICP off is
 se3tn_track_render bit for bit; every iteration's pose equals oracle/icp_ref.py's from the same start and the inlier counts are
 exact; with a zero head, ICP alone carries perturbed starts back to the poses that drew a synthetic frame; degenerate tracks
 keep their poses; graph replay, launch counts and refusals follow include/se3tn.h; the Tracker's two routes agree."""
@@ -80,27 +80,38 @@ def _step(e, c, icp, prec='bf16x3', mode='vispy', fill=None, k=1, **kw):
                           image_hw=HW if mode == 'pyrender' else None, fill_depth=fill, iterations=k, icp=icp, **outs)
 
 
-def _raw_icp(e, c, out, opts=None, rounds=None, icp=None, icp_poses=None, out_icp=None, render=False):
+def _raw_icp(e, c, out, opts=None, rounds=None, icp=None, icp_poses=None, out_icp=None):
+    """se3tn_track_render with opts->icp = icp (None: NULL) and the step's arrays."""
     L = importlib.import_module(PKG + '._lib')
     Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
     p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
-    head = (e._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(c.P), p(c.ow), 0, 0, 0,
-            c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, L.PREC_BF16X3, p(out[1]), p(out[2]), p(out[0]),
-            None if opts is None else C.byref(opts), p(rounds))
-    s = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    if render:
-        return e.lib.se3tn_track_render(*head, s)
-    return e.lib.se3tn_track_icp(*head, None if icp is None else C.byref(icp), p(icp_poses), p(out_icp), s)
+    if opts is not None:
+        opts.icp = None if icp is None else C.pointer(icp)
+    arrays = L.TrackArrays(*(None if t is None else t.data_ptr() for t in (None, rounds, None, icp_poses, None, None, out_icp)))
+    return e.lib.se3tn_track_render(e._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(c.P), p(c.ow), 0, 0, 0,
+                                    c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, L.PREC_BF16X3, p(out[1]), p(out[2]),
+                                    p(out[0]), None if opts is None else C.byref(opts), C.byref(arrays),
+                                    C.c_void_p(torch.cuda.current_stream().cuda_stream))
 
 
 def test_icp_off_is_track_render(eng, scene):
     L = importlib.import_module(PKG + '._lib')
     c = Case(eng, scene, 5)
     res = []
-    for render in (True, False):
+    for explicit in (False, True):                   # opts without the pointer fields set, then opts->icp = NULL
         out = (_nan(eng, 5, 4, 4), _nan(eng, 5, 3, dtype=torch.float32), _nan(eng, 5, 3, dtype=torch.float32))
         rounds = _nan(eng, 2, 5, 4, 4)
-        assert _raw_icp(eng, c, out, L.TrackOpts(iterations=2, fit_tau_mm=15), rounds, render=render) == L.OK
+        opts = L.TrackOpts(iterations=2, fit_tau_mm=15)
+        if explicit:
+            assert _raw_icp(eng, c, out, opts, rounds, icp=None) == L.OK and not opts.icp
+        else:
+            arrays = L.TrackArrays(round_poses=rounds.data_ptr())
+            p = lambda t: C.c_void_p(t.data_ptr())
+            Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
+            assert eng.lib.se3tn_track_render(eng._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(c.P), p(c.ow),
+                                              0, 0, 0, c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, L.PREC_BF16X3,
+                                              p(out[1]), p(out[2]), p(out[0]), C.byref(opts), C.byref(arrays),
+                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)) == L.OK
         torch.cuda.synchronize()
         res.append((out, rounds, eng._fit_rows_view()[:5].clone(), eng.last_launch_count(), eng.last_step_was_graph()))
     (a, ra, fa, na, ga), (b, rb, fb, nb, gb) = res
@@ -209,9 +220,10 @@ def test_refusals(eng, scene):
         icp = L.IcpOpts(**dict(good, **{field: bad}))
         assert refused(_raw_icp(eng, c, out, opts, None, icp, slots, st), 'icp->' + field), (field, bad)
         host_poses, host_icp = np.full((4, 4, 4), np.nan), np.full((4, 4), np.nan)
-        rc = eng.lib.se3tn_track_icp_host(eng._ctx, hp(c.rgb), hp(c.depth), HW[0], HW[1], hp(Kh), hp(c.poses), hp(np.full(4, WIDTH)),
-                                          0, 0, 0, hp(c.wid), 4, TN, RN, L.PREC_BF16X3, hp(host_poses), None, None, C.byref(opts),
-                                          None, C.byref(icp), hp(host_icp), None)
+        opts.icp = C.pointer(icp)
+        rc = eng.lib.se3tn_track_render_host(eng._ctx, hp(c.rgb), hp(c.depth), HW[0], HW[1], hp(Kh), hp(c.poses),
+                                             hp(np.full(4, WIDTH)), 0, 0, 0, hp(c.wid), 4, TN, RN, L.PREC_BF16X3, hp(host_poses), None,
+                                             None, C.byref(opts), C.byref(L.TrackArrays(out_icp=host_icp.ctypes.data)), None)
         assert refused(rc, 'icp->' + field)
         torch.cuda.synchronize()
         assert all(torch.isnan(t).all() for t in out + (slots, st)) and np.isnan(host_poses).all() and np.isnan(host_icp).all()

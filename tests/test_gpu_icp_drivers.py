@@ -1,5 +1,5 @@
 """ICP in the drivers on the synthetic layouts of the driver tests: icp=0 writes the trees a run without it writes, icp=M writes
-the poses its ICP steps returned (one se3tn_track_icp step per frame, the fit rows after ICP), and ycbv_recover's icp rows follow
+the poses its ICP steps returned (one ICP step per frame, the fit rows after ICP), and ycbv_recover's icp rows follow
 round K with the round rows unchanged."""
 import numpy as np
 import pytest

@@ -167,9 +167,11 @@ def _raw_track_host(e, c, ra, da, out, opts=None):
 def _raw_track_render(e, c, P, out, opts=None, rounds=None):
     Kh = np.ascontiguousarray([K[0, 0], K[1, 1], K[0, 2], K[1, 2]])
     p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    arrays = importlib.import_module(PKG + '._lib').TrackArrays(round_poses=None if rounds is None else rounds.data_ptr())
     return e.lib.se3tn_track_render(e._ctx, p(c.R), p(c.D), HW[0], HW[1], Kh.ctypes.data_as(C.c_void_p), p(P), p(c.ow), 0, 0, 0,
                                     c.wid.ctypes.data_as(C.c_void_p), p(c.wd), c.n, TN, RN, 2, p(out[1]), p(out[2]), p(out[0]),
-                                    _byref(opts), p(rounds), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                    _byref(opts), C.byref(arrays),
+                                    C.c_void_p(torch.cuda.current_stream().cuda_stream))
 
 
 def test_refusals(synth, eng):

@@ -102,20 +102,10 @@ def test_hypothesis_opts_match_the_header():
 def test_hypothesis_calls_match_the_header():
     src = _header()
     L = importlib.import_module(PKG + '._lib')
-    tail = {'se3tn_track_hypotheses': ['const int64_t* draw_keys', 'const se3tn_hypothesis_opts* hyp', 'int32_t* out_choice',
-                                       'int32_t* out_fit', 'double* hyp_poses', 'void* stream'],
-            'se3tn_track_hypotheses_host': ['int32_t* out_fit', 'const int64_t* draw_keys', 'const se3tn_hypothesis_opts* hyp',
-                                            'int32_t* out_choice', 'void* stream'],
-            'se3tn_draw_hypotheses': ['const se3tn_hypothesis_opts* hyp', 'double* out_poses', 'double* out_draws', 'void* stream']}
-    base = {'se3tn_track_hypotheses': 'se3tn_track_render', 'se3tn_track_hypotheses_host': 'se3tn_track_render_host'}
-    decl = lambda name: [' '.join(p.split()) for p in re.search(r'\bint\s+%s\s*\(([^)]*)\)\s*;' % name, src).group(1).split(',')]
-    for name, last in tail.items():
-        params = decl(name)
-        assert params[-len(last):] == last, name
-        if name in base:                              # the track call's arguments first, in its order
-            assert params[:len(decl(base[name])) - 1] == decl(base[name])[:-1], name
-        res, args = L.SIGNATURES[name]
-        assert res is L._i and len(args) == len(params), name
+    params = [' '.join(p.split()) for p in re.search(r'\bint\s+se3tn_draw_hypotheses\s*\(([^)]*)\)\s*;', src).group(1).split(',')]
+    assert params[-4:] == ['const se3tn_hypothesis_opts* hyp', 'double* out_poses', 'double* out_draws', 'void* stream']
+    res, args = L.SIGNATURES['se3tn_draw_hypotheses']
+    assert res is L._i and len(args) == len(params)
 
 
 def test_hypothesis_spec_refusals():

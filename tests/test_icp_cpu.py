@@ -1,4 +1,4 @@
-"""The depth refinement without a GPU: se3tn_icp_opts in include/se3tn.h against _lib.IcpOpts and the two calls' bindings,
+"""The depth refinement without a GPU: se3tn_icp_opts in include/se3tn.h against _lib.IcpOpts,
 oracle/icp_ref.py's Jacobian against central finite differences, its convergence on synthetic frames (which sets the bounds the
 GPU test holds the kernels to), and Engine.icp_spec's parsing."""
 import ctypes as C
@@ -43,20 +43,6 @@ def test_icp_opts_matches_the_header():
     src = open(os.path.join(ROOT, 'include', 'se3tn.h')).read()
     assert int(re.search(r'#define SE3TN_MAX_ICP_ITERATIONS (\d+)', src).group(1)) == L.MAX_ICP_ITERATIONS
     assert int(re.search(r'#define SE3TN_ICP_COLS (\d+)', src).group(1)) == L.ICP_COLS
-
-
-@pytest.mark.parametrize('name, tail', [('se3tn_track_icp', ['const se3tn_icp_opts* icp', 'double* icp_poses', 'double* out_icp']),
-                                        ('se3tn_track_icp_host', ['const se3tn_icp_opts* icp', 'double* out_icp'])])
-def test_icp_calls_are_declared_and_bound(name, tail):
-    L = importlib.import_module(PKG + '._lib')
-    m = re.search(r'\bint\s+%s\s*\(([^)]*)\)\s*;' % name, _header())
-    assert m, name + ' is not declared'
-    params = [' '.join(p.split()) for p in m.group(1).split(',')]
-    base = re.search(r'\bint\s+%s\s*\(([^)]*)\)\s*;' % name.replace('_icp', '_render'), _header())
-    base = [' '.join(p.split()) for p in base.group(1).split(',')]
-    assert params == base[:-1] + tail + ['void* stream']           # the render call's arguments, then ICP's, then the stream
-    res, args = L.SIGNATURES[name]
-    assert res is L._i and len(args) == len(params) and args[:len(base) - 1] == L.SIGNATURES[name.replace('_icp', '_render')][1][:-1]
 
 
 def test_jacobian_matches_central_differences():
