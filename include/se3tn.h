@@ -553,6 +553,84 @@ int se3tn_track_render_host(se3tn_ctx* ctx, const uint8_t* frame_rgb, const uint
 int se3tn_draw_hypotheses(se3tn_ctx* ctx, const double* poses_in, const int64_t* draw_keys, int n, const se3tn_hypothesis_opts* hyp,
                           double* out_poses, double* out_draws, void* stream);
 
+/* ---- start poses from a mask and the depth frame: render-and-compare over a rotation grid ---------------------------- */
+
+/* Every tracking call refines a pose it is given.  se3tn_init_poses finds a first one, for n objects of one frame, from each
+ * object's segmentation label and the depth frame alone (no network weights).  The stages, on `stream`, in this order:
+ *   1. Mask statistics, per object i with label l_i, over the whole H x W frame: mask = #(seg == l_i), depth_px = #(seg == l_i,
+ *      depth > 0), sum_u / sum_v = the sums of the mask pixels' columns / rows, z_med = the lower median (sorted index
+ *      (depth_px - 1) / 2) of the mask's depths > 0, in mm.  Integer atomics and a 65536-bin histogram: exact and independent
+ *      of the order of the reduction.  t0 = z_med / 1000 * K^-1 (sum_u / mask, sum_v / mask, 1) in fp64, metres.  status 1: the
+ *      mask is empty; 2: depth_px < min_pixels.  (A status != 0 object is drawn at the placeholder t0 = (0, 0, 1).)
+ *   2. Rotation grid: candidate c = v R + r, V viewpoints x R in-plane angles.  d_v is the Fibonacci-sphere direction
+ *      z = 1 - (2 v + 1) / V, phi = v pi (3 - sqrt 5) in the object frame; R_c maps d_v to the camera's -z axis with the
+ *      object's +z as the up vector (+y when |d_v.z| > 0.99) and then turns about the camera's z axis by 2 pi r / R.  fp64;
+ *      every candidate sits at t0 (oracle/init_ref.py restates the formulas).
+ *   3. Render and score: the n V R candidates are drawn (depth only, render_mode as se3tn_render_ex, mesh weight_ids[i])
+ *      in chunks of max_batch rows, each chunk followed by a score launch: one 4-CTA cluster per row crops the observed depth O
+ *      and the mask M = (seg == l_i) at the row's own window (se3tn_compute_bbox's window, se3tn_crop_bbox's nearest mapping,
+ *      0 outside the frame) and counts, over the rendered depth R: model #(R>0), maskc #M, overlap #(R>0, M), pairs
+ *      #(R>0, M, O>0) with S = sum (O - R) over them; then delta = floor((2 S + pairs) / (2 pairs)) mm (0 without pairs) and
+ *      inlier #(R>0, M, O>0, |O - (R + delta)| <= tau_mm).
+ *      Rank: the higher inlier / union (union = model + maskc - overlap; union 0 scores 0) as int64 cross products, then the
+ *      higher overlap, then the lower candidate index.
+ *   4. Keep K: per object, the K best candidates in rank order (exact: the rows are integers).  A kept pose moves along its
+ *      ray by its row's delta: t = t0 (1 + delta / (1000 t0_z)).
+ *   5. Refine (icp != NULL): icp->iterations ICP iterations (se3tn_icp_opts, the tracking step's render with triangle ids and
+ *      accumulate / solve launches) on the n K kept poses as n K tracks, then each refined pose is rendered and scored as in
+ *      3 at its own window with delta fixed at 0, and the best of the K by the same rank is kept.  Without icp the result is
+ *      the top grid candidate.
+ *   6. poses_out double (n, 16) device: one pose per object, all NaN when its status is not 0.  out_rows int32 (n,
+ *      SE3TN_INIT_COLS) device: the kept candidate's score row
+ *        0 status  1 candidate (v R + r)  2 model  3 maskc  4 overlap  5 pairs  6 inlier  7 delta_mm (0 after ICP)
+ * Arguments: frame_depth uint16 (H, W) mm and seg uint8 (H, W), device, H W < 2^31; K HOST fx fy cx cy; labels HOST int32 (n), 1..255
+ * (objects may share a label); object_width double (n) mm, device; render_mode / render_H / render_W as se3tn_track_render;
+ * weight_ids_host / weight_ids_dev int32 (n), both or neither (mesh 0).  No CUDA graph: plain launches, no synchronisation,
+ * except that a call needing more scratch than the context's init block holds first synchronises `stream` and grows it (the
+ * block holds the histogram, 256 KB per object, the n V R grid poses, widths, ids and rows, and one chunk's rendered depth,
+ * max_batch x 176 x 176 x 2 bytes).  The ICP stage uses the tracking step's ICP block (allocated by the call when no step
+ * has), whose contents no step reads before writing, so tracking steps and their graphs are unaffected.
+ * se3tn_last_launch_count: 2 (mask) + 1 (grid) + 3 per chunk + 1 (keep) [+ 4 M + 3 with icp] + 1 (choose).
+ * Refused with SE3TN_ERR_INVALID, the field named and nothing queued: a NULL input or output, a value outside the ranges
+ * below, reserved != 0, keep > V R, n K > max_batch, a label outside 1..255, an ICP option out of range, and an output
+ * overlapping an input or another output.  An id without a mesh is SE3TN_ERR_STATE.  n = 0 queues nothing.
+ * The defaults of Engine.init_spec (V 300, R 24, K 8, tau 20 mm, min_pixels 100, 5 ICP iterations) are starting guesses: how
+ * well they do on real sensor data has not been measured (README). */
+#define SE3TN_INIT_COLS 8
+#define SE3TN_INIT_STATS 6
+#define SE3TN_MAX_INIT_KEEP 32
+typedef struct se3tn_init_opts {
+    int32_t viewpoints, inplane;                   /* V in [1, 4096], R in [1, 360], V R <= 65536                            */
+    int32_t keep, tau_mm;                          /* K in [1, SE3TN_MAX_INIT_KEEP], K <= V R, n K <= max_batch; [1, 1000]    */
+    int32_t min_pixels, reserved;                  /* [1, 176 * 176]; 0                                                      */
+    const se3tn_icp_opts* icp;                     /* NULL: the best grid candidate; else refine the K kept, rescore, keep the best */
+} se3tn_init_opts;                                 /* 32 bytes on LP64, no padding                                           */
+
+/* The optional device outputs of se3tn_init_poses, passed by pointer (HOST memory); NULL means every field is NULL.
+ *   stats       int64 (n, SE3TN_INIT_STATS): status, mask, depth_px, sum_u, sum_v, z_med
+ *   t0          double (n, 3): the start translation, metres
+ *   cand_rows   int32 (n, V R, SE3TN_INIT_COLS): every candidate's score row, candidate c of object i at row i V R + c
+ *   kept_rows   int32 (n, K, SE3TN_INIT_COLS): the K kept candidates' rows in rank order
+ *   kept_poses  double (n, K, 16): their grid poses, moved along the ray by delta
+ *   icp_poses   double (n, K, 16), with icp only: the kept poses after the ICP iterations
+ *   icp_rows    int32 (n, K, SE3TN_INIT_COLS), with icp only: their rows, scored at delta 0
+ *   icp_stats   double (n, K, SE3TN_ICP_COLS), with icp only: the last ICP iteration's stats of each kept pose */
+typedef struct se3tn_init_arrays {
+    int64_t* stats;
+    double* t0;
+    int32_t* cand_rows;
+    int32_t* kept_rows;
+    double* kept_poses;
+    double* icp_poses;
+    int32_t* icp_rows;
+    double* icp_stats;
+} se3tn_init_arrays;
+
+int se3tn_init_poses(se3tn_ctx* ctx, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const double* K,
+                     const int32_t* labels, const double* object_width, int render_mode, int render_H, int render_W,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
+                     double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream);
+
 /* ---- checkpoint validation: the loss of ready-made training pairs ---------------------------------------------------- */
 
 /* Problem.validate's per-batch work (reference problems.py:106-132) as ONE step: for n pairs as TrackDataset.__getitem__ reads

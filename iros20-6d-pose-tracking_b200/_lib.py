@@ -22,6 +22,9 @@ MAX_HYPOTHESES = 32
 HYP_DRAWS = 8
 MAX_ICP_ITERATIONS = 16
 ICP_COLS = 4
+INIT_COLS = 8
+INIT_STATS = 6
+MAX_INIT_KEEP = 32
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -59,6 +62,7 @@ SIGNATURES = {
     'se3tn_track_render_host': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _d, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                      _vp]),
     'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    'se3tn_init_poses': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
     'se3tn_fit_rows': (_i, [_vp, C.POINTER(_vp)]),
@@ -119,6 +123,18 @@ class TrackArrays(C.Structure):
     """se3tn_track_arrays (include/se3tn.h): device pointers for se3tn_track_render, host pointers for _render_host."""
     _fields_ = [('draw_keys', _vp), ('round_poses', _vp), ('hyp_poses', _vp), ('icp_poses', _vp), ('out_fit', _vp),
                 ('out_choice', _vp), ('out_icp', _vp)]
+
+
+class InitOpts(C.Structure):
+    """se3tn_init_opts (include/se3tn.h)."""
+    _fields_ = [('viewpoints', C.c_int32), ('inplane', C.c_int32), ('keep', C.c_int32), ('tau_mm', C.c_int32),
+                ('min_pixels', C.c_int32), ('reserved', C.c_int32), ('icp', C.POINTER(IcpOpts))]
+
+
+class InitArrays(C.Structure):
+    """se3tn_init_arrays (include/se3tn.h): device pointers, NULL where not wanted."""
+    _fields_ = [('stats', _vp), ('t0', _vp), ('cand_rows', _vp), ('kept_rows', _vp), ('kept_poses', _vp), ('icp_poses', _vp),
+                ('icp_rows', _vp), ('icp_stats', _vp)]
 
 
 _lib = None

@@ -12,6 +12,7 @@
 #include "fit.h"
 #include "icp.h"
 #include "hypotheses.h"
+#include "init.h"
 #include "storage.cuh"
 
 #include <algorithm>
@@ -295,7 +296,9 @@ struct se3tn_ctx {
     // the ICP block: the sums (max_batch x kIcpSums doubles), then the ICP render's depth and triangle ids of
     // max_batch tracks; allocated by the first ICP step, never moved after
     DevBuf<uint8_t> icp; size_t icp_bytes = 0;
-    DevBuf<float> pool_part;         // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
+    // se3tn_init_poses' scratch (InitLayout); grows on demand after a stream synchronisation, never captured in a graph
+    DevBuf<uint8_t> init; size_t init_bytes = 0;
+    DevBuf<float> pool_part;        // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
     bool sched_dirty = false;        // a step failed between the trunk launch and the head launch: clear before the next one
@@ -2537,6 +2540,194 @@ int se3tn_get_profile(se3tn_ctx* c, float* ms) {
         CU_TRY(c, cudaEventElapsedTime(&ms[i], c->ev[0][i].get(), c->ev[1][i].get()));
         c->ev_used[i] = false;
     }
+    return SE3TN_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// se3tn_init_poses' scratch for n objects, V R candidates each and K kept: offsets into the context's init block.
+struct InitLayout {
+    size_t labels, acc, hist, stats, t0, grid, width, ids, rows, depth, kept_rows, kept_poses, kept_width, kept_ids, icp_poses,
+           icp_rows, icp_stats, bytes;
+    InitLayout(size_t n, size_t VR, size_t K, size_t max_batch) {
+        size_t o = 0;
+        auto take = [&o](size_t b) { const size_t at = o; o += align256(b); return at; };
+        labels = take(n * sizeof(int32_t)); acc = take(n * kInitAcc * sizeof(unsigned long long));
+        hist = take(n * kInitBins * sizeof(unsigned)); stats = take(n * kInitStats * sizeof(long long)); t0 = take(n * 3 * sizeof(double));
+        grid = take(n * VR * 16 * sizeof(double)); width = take(n * VR * sizeof(double)); ids = take(n * VR * sizeof(int32_t));
+        rows = take(n * VR * kInitCols * sizeof(int32_t)); depth = take(max_batch * kImg * kImg * sizeof(uint16_t));
+        kept_rows = take(n * K * kInitCols * sizeof(int32_t)); kept_poses = take(n * K * 16 * sizeof(double));
+        kept_width = take(n * K * sizeof(double)); kept_ids = take(n * K * sizeof(int32_t));
+        icp_poses = take(n * K * 16 * sizeof(double)); icp_rows = take(n * K * kInitCols * sizeof(int32_t));
+        icp_stats = take(n * K * kIcpCols * sizeof(double));
+        bytes = o;
+    }
+};
+
+static_assert(sizeof(se3tn_init_opts) == 32, "se3tn_init_opts is 32 bytes without padding: _lib.InitOpts mirrors it");
+static_assert(kInitCols == SE3TN_INIT_COLS && kInitStats == SE3TN_INIT_STATS && kInitMaxKeep == SE3TN_MAX_INIT_KEEP, "include/se3tn.h");
+
+// opts checked for n objects (the ICP options and block by icp_opts).  Refused before anything is queued.
+int init_opts(se3tn_ctx* c, const char* fn, const se3tn_init_opts* o, int n, Step& st) {
+    const std::string f(fn);
+    if (!o) return fail(c, SE3TN_ERR_INVALID, f + ": opts is NULL");
+    auto range = [&](int v, int lo, int hi, const char* name) {
+        return v >= lo && v <= hi ? SE3TN_OK
+                                  : fail(c, SE3TN_ERR_INVALID, f + ": opts->" + name + " is " + std::to_string(v) + ", not in [" +
+                                                                   std::to_string(lo) + ", " + std::to_string(hi) + "]");
+    };
+    int rc;
+    if ((rc = range(o->viewpoints, 1, 4096, "viewpoints")) || (rc = range(o->inplane, 1, 360, "inplane")) ||
+        (rc = range(o->keep, 1, kInitMaxKeep, "keep")) || (rc = range(o->tau_mm, 1, 1000, "tau_mm")) ||
+        (rc = range(o->min_pixels, 1, kImg * kImg, "min_pixels")))
+        return rc;
+    if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
+    const long long VR = static_cast<long long>(o->viewpoints) * o->inplane;
+    if (VR > 65536) return fail(c, SE3TN_ERR_INVALID, f + ": opts->viewpoints x opts->inplane = " + std::to_string(VR) + " exceeds 65536");
+    if (o->keep > VR) return fail(c, SE3TN_ERR_INVALID, f + ": opts->keep exceeds the " + std::to_string(VR) + " candidates");
+    if (static_cast<long long>(n) * o->keep > c->max_batch)
+        return fail(c, SE3TN_ERR_INVALID, f + ": n x opts->keep = " + std::to_string(static_cast<long long>(n) * o->keep) +
+                    " exceeds max_batch " + std::to_string(c->max_batch));
+    if (!o->icp) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    return icp_opts(c, fn, o->icp, st);
+}
+}  // namespace
+
+extern "C" {
+
+int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const double* K,
+                     const int32_t* labels, const double* object_width, int render_mode, int render_H, int render_W,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
+                     double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream) {
+    const char* fn = "se3tn_init_poses";
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    // the mask pass counts pixels in 32 bits (mask_finish_kernel's scan): H x W stays below 2^31
+    if (!frame_depth || !seg || !K || !labels || !object_width || H <= 0 || W <= 0 || static_cast<long long>(H) * W >= (1LL << 31))
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or frame size out of range (H x W must be below 2^31)");
+    if (!poses_out || !out_rows) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    Step st{};
+    if ((rc = init_opts(c, fn, opts, n, st))) return rc;
+    const se3tn_init_arrays a = arrays ? *arrays : se3tn_init_arrays{};
+    const bool icp = opts->icp != nullptr;
+    const struct { const void* p; const char* name; } icp_only[] = {{a.icp_poses, "icp_poses"}, {a.icp_rows, "icp_rows"}, {a.icp_stats, "icp_stats"}};
+    for (const auto& x : icp_only)
+        if (x.p && !icp) return fail(c, SE3TN_ERR_INVALID, f + ": arrays->" + x.name + " is set, but opts->icp is NULL");
+    if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
+        return fail(c, SE3TN_ERR_INVALID, f + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
+    for (int i = 0; i < n; ++i) {
+        if (labels[i] < 1 || labels[i] > 255)
+            return fail(c, SE3TN_ERR_INVALID, f + ": labels[" + std::to_string(i) + "] is " + std::to_string(labels[i]) + ", not in [1, 255]");
+        const int id = weight_ids_host ? weight_ids_host[i] : 0;
+        if (!c->meshes.count(id))
+            return fail(c, SE3TN_ERR_STATE, f + ": id " + std::to_string(id) + " (object " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
+    }
+    const size_t nn = static_cast<size_t>(n), VR = static_cast<size_t>(opts->viewpoints) * opts->inplane, Kk = opts->keep;
+    const size_t nK = nn * Kk, px = static_cast<size_t>(H) * W;
+    rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_rows, nn * 4 * kInitCols}, {a.stats, nn * 8 * kInitStats}, {a.t0, nn * 24},
+                                {a.cand_rows, nn * VR * 4 * kInitCols}, {a.kept_rows, nK * 4 * kInitCols}, {a.kept_poses, nK * 128},
+                                {a.icp_poses, nK * 128}, {a.icp_rows, nK * 4 * kInitCols}, {a.icp_stats, nK * 8 * kIcpCols}},
+                        {{frame_depth, px * 2}, {seg, px}, {object_width, nn * 8}, {weight_ids_dev, nn * 4}},
+                        "the outputs must not overlap frame_depth, seg, object_width or weight_ids_dev");
+    if (rc || n == 0) return rc;
+
+    DeviceGuard guard(c->device);
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if ((rc = sync_meshes(c, s))) return rc;
+    const InitLayout L(nn, VR, Kk, static_cast<size_t>(c->max_batch));
+    if (L.bytes > c->init_bytes) {                       // the old block may still be read by a queued call
+        CU_TRY(c, cudaStreamSynchronize(s));
+        CU_TRY(c, grow(c->init, c->init_bytes, L.bytes));
+    }
+    uint8_t* b = c->init.get();
+    auto at = [b](size_t off) { return static_cast<void*>(b + off); };
+    int32_t* d_labels = static_cast<int32_t*>(at(L.labels));
+    long long* stats = a.stats ? reinterpret_cast<long long*>(a.stats) : static_cast<long long*>(at(L.stats));
+    double* t0 = a.t0 ? a.t0 : static_cast<double*>(at(L.t0));
+    double* grid = static_cast<double*>(at(L.grid));
+    double* gwidth = static_cast<double*>(at(L.width));
+    int32_t* gids = weight_ids_dev ? static_cast<int32_t*>(at(L.ids)) : nullptr;
+    int32_t* rows = a.cand_rows ? a.cand_rows : static_cast<int32_t*>(at(L.rows));
+    uint16_t* depth = static_cast<uint16_t*>(at(L.depth));
+    int32_t* kept_rows = a.kept_rows ? a.kept_rows : static_cast<int32_t*>(at(L.kept_rows));
+    double* kept_poses = a.kept_poses ? a.kept_poses : static_cast<double*>(at(L.kept_poses));
+    double* kept_width = static_cast<double*>(at(L.kept_width));
+    int32_t* kept_ids = weight_ids_dev ? static_cast<int32_t*>(at(L.kept_ids)) : nullptr;
+    double* icp_poses = a.icp_poses ? a.icp_poses : static_cast<double*>(at(L.icp_poses));
+    int32_t* icp_rows = a.icp_rows ? a.icp_rows : static_cast<int32_t*>(at(L.icp_rows));
+    double* icp_stats = a.icp_stats ? a.icp_stats : static_cast<double*>(at(L.icp_stats));
+    c->launches = 0;
+
+    // 1. mask statistics and t0
+    CU_TRY(c, cudaMemcpyAsync(d_labels, labels, nn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    MaskArgs ma{};
+    ma.depth = frame_depth; ma.seg = seg; ma.H = H; ma.W = W; ma.labels = d_labels; ma.n = n;
+    ma.acc = static_cast<unsigned long long*>(at(L.acc)); ma.hist = static_cast<unsigned*>(at(L.hist)); ma.min_pixels = opts->min_pixels;
+    ma.fx = K[0]; ma.fy = K[1]; ma.cx = K[2]; ma.cy = K[3]; ma.stats = stats; ma.t0 = t0;
+    CU_TRY(c, launch_mask_stats(ma, s));
+    c->launches += 2;
+    // 2. the rotation grid at t0
+    GridArgs ga{};
+    ga.n = n; ga.V = opts->viewpoints; ga.R = opts->inplane; ga.t0 = t0; ga.width_in = object_width; ga.ids_in = weight_ids_dev;
+    ga.poses = grid; ga.width = gwidth; ga.ids = gids;
+    CU_TRY(c, launch_grid(ga, s));
+    ++c->launches;
+    // 3. render and score in chunks of max_batch rows: each render waits (PDL) for the score before it, which read the chunk
+    // depth it overwrites
+    ScoreArgs sa{};
+    sa.object_width = gwidth; sa.fx = K[0]; sa.fy = K[1]; sa.cx = K[2]; sa.cy = K[3];
+    sa.frame_depth = frame_depth; sa.seg = seg; sa.H = H; sa.W = W; sa.rendered = depth; sa.labels = d_labels; sa.stats = stats;
+    sa.tau = opts->tau_mm;
+    const size_t total = nn * VR;
+    for (size_t g0 = 0; g0 < total; g0 += c->max_batch) {
+        const int m = static_cast<int>(std::min(total - g0, static_cast<size_t>(c->max_batch)));
+        const RenderArgs ra = render_args(c, K, grid + 16 * g0, gwidth + g0, gids ? gids + g0 : nullptr, r.mode, r.H, r.W, nullptr, depth);
+        CU_TRY(c, launch_render(ra, m, s));
+        sa.poses = grid; sa.row0 = static_cast<int>(g0); sa.per_object = static_cast<int>(VR); sa.rows = rows;
+        CU_TRY(c, launch_score(sa, m, s));
+        c->launches += 3;
+    }
+    // 4. keep the K best of each object
+    KeepArgs ka{};
+    ka.n = n; ka.per_object = static_cast<int>(VR); ka.K = opts->keep; ka.rows = rows; ka.poses = grid; ka.width_in = object_width;
+    ka.ids_in = weight_ids_dev; ka.kept_rows = kept_rows; ka.kept_poses = kept_poses; ka.kept_width = kept_width; ka.kept_ids = kept_ids;
+    CU_TRY(c, launch_keep(ka, s));
+    ++c->launches;
+    // 5. ICP on the n K kept poses as n K tracks, then each rescored where it landed
+    ChooseArgs ca{};
+    ca.n = n; ca.K = opts->keep; ca.rows = kept_rows; ca.poses = kept_poses; ca.stats = stats; ca.poses_out = poses_out; ca.rows_out = out_rows;
+    if (icp) {
+        const int nk = static_cast<int>(nK);
+        CU_TRY(c, cudaMemcpyAsync(icp_poses, kept_poses, nK * 16 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        RenderArgs ra = render_args(c, K, icp_poses, kept_width, kept_ids, r.mode, r.H, r.W, nullptr, icp_depth(c));
+        ra.tri = icp_tri(c);
+        IcpArgs ia{};
+        ia.poses = icp_poses; ia.object_width = kept_width; ia.mesh_ids = kept_ids; ia.meshes = c->d_meshes.get(); ia.n_meshes = c->mesh_rows;
+        ia.fx = K[0]; ia.fy = K[1]; ia.cx = K[2]; ia.cy = K[3]; ia.frame_depth = frame_depth; ia.H = H; ia.W = W; ia.tri = icp_tri(c);
+        ia.tau = st.icp.tau; ia.min_inliers = st.icp.min_inliers; ia.sums = icp_sums(c); ia.stats = icp_stats;
+        for (int it = 0; it < st.icp.iterations; ++it) {
+            CU_TRY(c, launch_render(ra, nk, s));
+            CU_TRY(c, launch_icp(ia, nk, s));
+            c->launches += 4;
+        }
+        const RenderArgs rs = render_args(c, K, icp_poses, kept_width, kept_ids, r.mode, r.H, r.W, nullptr, depth);
+        CU_TRY(c, launch_render(rs, nk, s));
+        ScoreArgs sr = sa;
+        sr.poses = icp_poses; sr.object_width = kept_width; sr.row0 = 0; sr.per_object = opts->keep; sr.cand_rows = kept_rows;
+        sr.fixed_delta = 1; sr.rows = icp_rows;
+        CU_TRY(c, launch_score(sr, nk, s));
+        c->launches += 3;
+        ca.rows = icp_rows; ca.poses = icp_poses;
+    }
+    // 6. the best of each object's K
+    CU_TRY(c, launch_choose(ca, s));
+    ++c->launches;
     return SE3TN_OK;
 }
 

@@ -487,6 +487,80 @@ class Engine:
         return out, choice, rows
 
     # ------------------------------------------------------------------ checkpoint validation
+    # init_spec's defaults: starting guesses, not tuned on a real sensor: 300 x 24 = 7,200 candidates about 12 x 15 degrees
+    # apart, the 8 best refined by 5 ICP iterations at icp_spec's gate, a 20 mm inlier gate, at least 100 mask pixels with depth
+    INIT_DEFAULTS = dict(viewpoints=300, inplane=24, keep=8, tau_mm=20, min_pixels=100, icp=5)
+    INIT_STATUS = {1: 'the mask is empty', 2: 'too few mask pixels have depth (min_pixels)'}
+    INIT_ARRAYS = ('stats', 't0', 'cand_rows', 'kept_rows', 'kept_poses', 'icp_poses', 'icp_rows', 'icp_stats')
+
+    @staticmethod
+    def init_spec(init=None):
+        """se3tn_init_opts from None (INIT_DEFAULTS) or a dict of any of viewpoints (1..4096), inplane (1..360; viewpoints x
+        inplane <= 65536), keep (1..MAX_INIT_KEEP), tau_mm (1..1000), min_pixels (1..176*176) and icp (icp_spec's argument;
+        None / 0: the best grid candidate without refinement); the rest from INIT_DEFAULTS.  Else a ValueError."""
+        spec = dict(Engine.INIT_DEFAULTS)
+        if init is not None:
+            if not isinstance(init, dict):
+                raise ValueError('init must be None or a dict, not %r' % (init,))
+            unknown = set(init) - set(spec)
+            if unknown:
+                raise ValueError('init: unknown fields %s' % sorted(unknown))
+            spec.update(init)
+        limits = {'viewpoints': (1, 4096), 'inplane': (1, 360), 'keep': (1, _lib.MAX_INIT_KEEP), 'tau_mm': (1, 1000),
+                  'min_pixels': (1, IMAGE_SIZE * IMAGE_SIZE)}
+        for k, (lo, hi) in limits.items():
+            v = spec[k]
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+                raise ValueError('init %s must be an integer in [%d, %d], not %r' % (k, lo, hi, v))
+        if spec['viewpoints'] * spec['inplane'] > 65536:
+            raise ValueError('init viewpoints x inplane = %d exceeds 65536' % (spec['viewpoints'] * spec['inplane']))
+        if spec['keep'] > spec['viewpoints'] * spec['inplane']:
+            raise ValueError('init keep=%d exceeds the %d candidates' % (spec['keep'], spec['viewpoints'] * spec['inplane']))
+        icp = Engine.icp_spec(spec['icp'])
+        return _lib.InitOpts(viewpoints=int(spec['viewpoints']), inplane=int(spec['inplane']), keep=int(spec['keep']),
+                             tau_mm=int(spec['tau_mm']), min_pixels=int(spec['min_pixels']), icp=None if icp is None else C.pointer(icp))
+
+    def init_poses(self, frame_depth, seg, K, labels, object_width, weight_ids=None, mode='vispy', image_hw=None, init=None, out=None):
+        """Start poses for n objects of one frame from their segmentation labels and the depth (se3tn_init_poses): a rotation
+        grid at each mask's centroid ray and median depth, rendered and scored against the depth and the mask, the best `keep`
+        refined by ICP.  frame_depth uint16 (H,W) mm and seg uint8 (H,W) CUDA tensors; K 3x3 or (fx,fy,cx,cy); labels (n) ints
+        in 1..255; object_width float64 CUDA (n) mm; weight_ids int32 (n) host array or None (mesh 0); mode / image_hw as in
+        render(); init: init_spec's argument.  out: a dict that may hold 'poses' (float64 (n,4,4)), 'rows' (int32 (n,8)) and any
+        of INIT_ARRAYS (include/se3tn.h's se3tn_init_arrays, shaped (n, ...)) as CUDA tensors to fill.  -> (poses float64 (n,4,4),
+        all NaN for an object whose status is not 0, rows int32 (n, INIT_COLS): status, candidate, model, maskc, overlap, pairs,
+        inlier, delta_mm), queued on the current stream."""
+        opts = self.init_spec(init)
+        lab = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+        n = int(lab.shape[0])
+        H, W = frame_depth.shape
+        self._check_dev('frame_depth', frame_depth, torch.uint16, (H, W))
+        self._check_dev('seg', seg, torch.uint8, (H, W))
+        self._check_dev('object_width', object_width, torch.float64, (n,))
+        wh = self._host_ids('init_poses', weight_ids, n)
+        wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
+        out = dict(out or {})
+        unknown = set(out) - {'poses', 'rows'} - set(self.INIT_ARRAYS)
+        if unknown:
+            raise ValueError('init_poses: unknown outputs %s' % sorted(unknown))
+        VR, Kk = opts.viewpoints * opts.inplane, opts.keep
+        shapes = dict(poses=((n, 4, 4), torch.float64), rows=((n, _lib.INIT_COLS), torch.int32),
+                      stats=((n, _lib.INIT_STATS), torch.int64), t0=((n, 3), torch.float64),
+                      cand_rows=((n, VR, _lib.INIT_COLS), torch.int32), kept_rows=((n, Kk, _lib.INIT_COLS), torch.int32),
+                      kept_poses=((n, Kk, 4, 4), torch.float64), icp_poses=((n, Kk, 4, 4), torch.float64),
+                      icp_rows=((n, Kk, _lib.INIT_COLS), torch.int32), icp_stats=((n, Kk, _lib.ICP_COLS), torch.float64))
+        for k in ('poses', 'rows'):
+            if out.get(k) is None:
+                out[k] = torch.empty(shapes[k][0], dtype=shapes[k][1], device=self.device)
+        for k, t in out.items():
+            if t is not None:
+                self._check_dev('out[%r]' % k, t, shapes[k][1], shapes[k][0])
+        arrays = _lib.InitArrays(**{k: _ptr(out.get(k)).value for k in self.INIT_ARRAYS})
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        _lib.check(self.lib.se3tn_init_poses(self._ctx, _ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _hptr(lab),
+                                             _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
+                                             _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
+        return out['poses'], out['rows']
+
     def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
                    weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', want_terms=False, want_labels=False,
                    out_trans=None, out_rot=None, out_sums=None, out_sq=None, out_labels=None, augment=None, segB=None,

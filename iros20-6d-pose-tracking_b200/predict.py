@@ -172,6 +172,7 @@ class Tracker:
         self.iterations = Engine.refine_iterations(iterations)
         self.icp = icp if Engine.icp_spec(icp) is not None else None
         self.last_icp = None
+        self.last_init = None
         self.hypotheses = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
         if self.icp is not None and self.hypotheses > 1:
             raise ValueError('icp=%r with hypotheses=%d: ICP inside hypothesis steps is not supported' % (icp, self.hypotheses))
@@ -310,6 +311,47 @@ class Tracker:
         if renderer_width and r.object_width != float(self.object_width):
             return None
         return r
+
+    # ------------------------------------------------------------------ a start without a pose
+    def initialize(self, depth, mask, label=1, **init):
+        """The start pose of this Tracker's object from its mask and the depth frame (Engine.init_poses), with the Tracker's
+        mesh, width and render mode.  depth: uint16 (H,W) mm, numpy or CUDA; mask: a bool (H,W) array (the object's pixels) or a
+        uint8 label image in which the object's pixels are `label`.  init: Engine.init_spec's fields.  A Tracker built with
+        fill_depth fills the depth first with the same settings, so the start is scored on the depth its steps see.  -> the 4x4
+        float64 start on_track takes; the kept score row (status, candidate, model, maskc, overlap, pairs, inlier, delta_mm) is
+        left in last_init.  A ValueError names the status when there is no start (an empty mask, too few pixels with depth)."""
+        r = self._fused_renderer()
+        if r is None:
+            raise ValueError('initialize draws the model on the device: it needs the CUDA renderer (renderer="cuda") on this '
+                             "Tracker's engine and camera, not %r" % (self.renderer,))
+        dev = self.engine.device
+        as_dev = lambda a, dt: a.to(dev, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
+        depth_d = as_dev(depth, np.uint16 if not torch.is_tensor(depth) else torch.uint16)
+        m = mask if torch.is_tensor(mask) else np.asarray(mask)
+        if torch.is_tensor(m) and m.dtype == torch.bool:
+            seg = m.to(dev).to(torch.uint8).contiguous() * int(label)
+        elif not torch.is_tensor(m) and m.dtype == np.bool_:
+            seg = torch.from_numpy(np.where(m, np.uint8(label), np.uint8(0))).to(dev)
+        else:
+            size = m.numel() if torch.is_tensor(m) else m.size
+            lo, hi = (int(m.min()), int(m.max())) if size else (0, 0)
+            if lo < 0 or hi > 255:
+                raise ValueError('initialize: a label image holds labels 0..255, not %d..%d' % (lo, hi))
+            seg = as_dev(m, np.uint8 if not torch.is_tensor(m) else torch.uint8)
+        if tuple(seg.shape) != tuple(depth_d.shape):
+            raise ValueError('initialize: mask %s and depth %s differ in shape' % (tuple(seg.shape), tuple(depth_d.shape)))
+        on, max_depth, extrapolate, blur = Engine.depth_fill_spec(self.fill_depth)
+        if on:
+            depth_d = self.engine.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
+        width = torch.full((1,), float(self.object_width), dtype=torch.float64, device=dev)
+        poses, rows = self.engine.init_poses(depth_d, seg, self.K, [int(label)], width,
+                                             weight_ids=None if r.mesh_id == 0 else [r.mesh_id], mode=r.mode, image_hw=r.image_hw,
+                                             init=init or None)
+        self.last_init = rows[0].cpu().numpy()
+        status = int(self.last_init[0])
+        if status:
+            raise ValueError('initialize: no start for label %d: %s (status %d)' % (label, Engine.INIT_STATUS.get(status, '?'), status))
+        return poses[0].cpu().numpy()
 
     # ------------------------------------------------------------------ the hot path
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
@@ -1625,8 +1667,66 @@ def _write_ycb_all_sequence_fit(dirs, seq_id, cls, init, tracked):
     return out
 
 
+# ----------------------------------------------------------------------------------------------------
+# Starts from the segmentation masks (Engine.init_poses): the one-pass YCB-Video driver's --init mask and --mode ycbv_init.  The
+# label of class c in a YCB-Video seg/ image is c itself.
+# ----------------------------------------------------------------------------------------------------
+def read_seg(path):
+    """A YCB-Video label image (seg/%06d-label.png) -> uint8 (H, W)."""
+    import cv2
+    s = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if s is None:
+        raise FileNotFoundError(path)
+    return np.ascontiguousarray(s if s.ndim == 2 else s[:, :, 0], dtype=np.uint8)
+
+
+def class_width(k):
+    """The object width a Tracker of checked configuration k draws with (Tracker.__init__'s rule), in mm."""
+    info = k['dataset_info']
+    if 'object_width' in info:
+        return float(info['object_width'])
+    w = compute_obj_max_width(np.asarray(object_cloud(k['model_path']).points))
+    return float(w + info['boundingbox'] / 100 * w)
+
+
+class MaskStarts:
+    """One Engine holding each class's CUDA-renderer mesh under its class id, for init calls of up to n_max classes of one frame
+    (max_batch n_max x keep).  classes: checked configurations (class_id, model_path, dataset_info), sharing camera and render
+    mode; init: Engine.init_spec's argument."""
+    def __init__(self, classes, n_max, init=None):
+        from .mesh_io import load_mesh
+        self.init = init
+        self.spec = Engine.init_spec(init)
+        self.eng = Engine(max_batch=max(1, n_max * self.spec.keep))
+        self.width = {}
+        for k in classes:
+            self.eng.set_mesh(load_mesh(k['model_path']), k['class_id'])
+            self.width[k['class_id']] = class_width(k)
+        cam = classes[0]['dataset_info']['camera']
+        self.K = np.array([[cam['focalX'], 0, cam['centerX']], [0, cam['focalY'], cam['centerY']], [0, 0, 1]], dtype=np.float64)
+        self.render = dict(mode='pyrender', image_hw=(int(cam['height']), int(cam['width']))) if _pyrender(classes[0]) else \
+            dict(mode='vispy', image_hw=None)
+
+    def __call__(self, depth, seg, cls, out=None):
+        """One init call for the classes cls (labels = ids = class ids) of one frame (uint16 depth, uint8 seg, numpy or CUDA) ->
+        (poses (n, 4, 4), rows (n, INIT_COLS)) CUDA tensors, and out filled (Engine.init_poses)."""
+        dev = self.eng.device
+        as_dev = lambda a: a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        ids = np.asarray(cls, dtype=np.int32)
+        widths = torch.tensor([self.width[int(c)] for c in cls], dtype=torch.float64, device=dev)
+        return self.eng.init_poses(as_dev(depth), as_dev(seg), self.K, ids, widths, weight_ids=ids, init=self.init, out=out, **self.render)
+
+    def close(self):
+        self.eng.close()
+
+
+def _mask_start_refusal(seq, c, name, status):
+    return ValueError('sequence %04d, class %d (%s): no start from its mask in the first frame: %s (status %d)'
+                      % (seq, c, name, Engine.INIT_STATUS.get(int(status), '?'), int(status)))
+
+
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None):
+                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None, init=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1675,13 +1775,22 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
 
     icp: M iterations of ICP after every step's last round (Engine.track_render's icp), at the gate icp_tau mm
     (Engine.ICP_TAU_DEFAULT when None); the pose files hold the refined poses and FIT_FILE, with fit, the fit after ICP.  0 is the
-    plain run, file for file; several GPUs write the one-GPU trees.  Refused with hypotheses > 1 (_driver_icp)."""
+    plain run, file for file; several GPUs write the one-GPU trees.  Refused with hypotheses > 1 (_driver_icp).
+
+    initialize_method='mask': each sequence's tracks start from one Engine.init_poses call on its first frame (depth_filled and
+    seg/ label image; each class's label is its class id; init: Engine.init_spec's argument), made in this process before any
+    tracking, so several GPUs write the one-GPU trees.  A class the call finds no start for (an empty mask, too few pixels with
+    depth) is a ValueError naming the sequence and the class.  init without 'mask' is a ValueError."""
+    if init is not None and initialize_method != 'mask':
+        raise ValueError("init options need initialize_method='mask', not %r" % (initialize_method,))
+    if initialize_method == 'mask':
+        Engine.init_spec(init)
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
     fit = _driver_fit(fit)
     _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
     icp = _driver_icp(icp, icp_tau, hypotheses)
-    if initialize_method not in ('gt', 'posecnn', 'poserbpf'):
-        raise ValueError('initialize_method must be gt, posecnn or poserbpf')
+    if initialize_method not in ('gt', 'posecnn', 'poserbpf', 'mask'):
+        raise ValueError('initialize_method must be gt, posecnn, poserbpf or mask')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
     per_ckpt = [ycb_all_classes(ycb_dir, class_ids, cfg, run.precision) for cfg in run.configs]
     classes = per_ckpt[0]
@@ -1689,13 +1798,31 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
     sequences = []
-    for seq_id, cls in track_sets.items():
-        files = {c: _ycb_sequence_files(os.path.join(data_dir, '%04d' % seq_id), c) for c in cls}
-        rgb_files, depth_files, _ = files[cls[0]]
-        nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
-        init = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
-                                         sorted(findClassContainedVideosYcb(c, data_dir, testset=True))) for c in cls]).astype(np.float64)
-        sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init))
+    starts = MaskStarts(classes, max([len(v) for v in track_sets.values()] + [1]), init) if initialize_method == 'mask' else None
+    try:
+        for seq_id, cls in track_sets.items():
+            files = {c: _ycb_sequence_files(os.path.join(data_dir, '%04d' % seq_id), c) for c in cls}
+            rgb_files, depth_files, _ = files[cls[0]]
+            nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
+            if starts is not None:
+                import glob
+                segs = sorted(glob.glob(os.path.join(data_dir, '%04d' % seq_id, 'seg', '*')))
+                if not segs:
+                    raise FileNotFoundError('--init mask: no seg/ label image under %s' % os.path.join(data_dir, '%04d' % seq_id))
+                P, rows = starts(read_depth(depth_files[0]), read_seg(segs[0]), cls)
+                P, rows = P.cpu().numpy(), rows.cpu().numpy()
+                for j, c in enumerate(cls):
+                    if rows[j, 0]:
+                        raise _mask_start_refusal(seq_id, c, [k['name'] for k in classes if k['class_id'] == c][0], rows[j, 0])
+                init_poses = P
+            else:
+                init_poses = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
+                                                       sorted(findClassContainedVideosYcb(c, data_dir, testset=True)))
+                                       for c in cls]).astype(np.float64)
+            sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init_poses))
+    finally:
+        if starts is not None:
+            starts.close()
     entries = [(k['class_id'] + CKPT_ID_STRIDE * i, 'class %d (%s)' % (k['class_id'], k['name']) + _ckpt_label(i, run), k)
                for i, cl in enumerate(per_ckpt) for k in cl]
     max_batch = max([len(v) for v in track_sets.values()] + [1])
@@ -2136,6 +2263,132 @@ def _score_hypotheses(eng, table, pose_set, offsets, B, keep, picked, kidx, kset
     return out
 
 
+def init_classes(ycb_dir, class_ids, class_config):
+    """--mode ycbv_init's classes: [dict class_id, name, dataset_info, model_path] from class_config's train_data_path (its
+    ../dataset_info.yml) and model_path templates; no checkpoint is read.  A missing file is a FileNotFoundError naming the class;
+    classes must share the camera and the render mode (one init call per frame draws all of them)."""
+    import yaml
+    classes = []
+    for c, name in ycb_classes(ycb_dir, class_ids):
+        label = 'class %d (%s)' % (c, name)
+        paths = {}
+        for key in ('train_data_path', 'model_path'):
+            if key not in class_config:
+                raise ValueError('class_config needs a %r template' % key)
+            paths[key] = str(class_config[key]).format(class_id=c, class_name=name)
+        info_path = os.path.join(paths['train_data_path'], '../dataset_info.yml')
+        for what, path in (('dataset_info.yml', info_path), ('mesh', paths['model_path'])):
+            if not os.path.isfile(path):
+                raise FileNotFoundError('%s: no %s file at %s' % (label, what, path))
+        with open(info_path, 'r') as ff:
+            classes.append(dict(class_id=c, name=name, dataset_info=yaml.safe_load(ff), model_path=paths['model_path']))
+    if not classes:
+        raise ValueError('no class ids given')
+    _check_shared(classes, lambda k: 'class %d (%s)' % (k['class_id'], k['name']), lambda k: 'class %d' % k['class_id'],
+                  (('camera', _camera), ('renderer', _pyrender)), 'classes started in one call must share it')
+    return classes
+
+
+INIT_ROWS = ('grid', 'icp', 'best of K')
+
+
+def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=None):
+    """Starts from the masks scored on the YCB-Video key frames: no checkpoint, no tracking.  The frames are the key frames of
+    ycbv_recover's loop (produce_train_pair_data.ycbv_keyframe_jobs: every key frame with an annotated requested class), each
+    with its depth_filled and seg/ images; each is one Engine.init_poses call (MaskStarts) for all its annotated classes, label =
+    class id.  Every row is scored against its pose_gt with se3tn_pose_errors_sets against the class's model points
+    (object_cloud), and se3tn_vocap_sets gives the per-class and pooled ADD / ADD-S AUCs.  Rows: 'grid' the top grid candidate,
+    'icp' the returned pose, 'best of K' per row the kept candidate (after ICP when init has it) of lowest ADD-S, which bounds
+    any final choice.  A row whose call reports status != 0 is counted as failed and not scored.  max_frames: the first key
+    frames only.
+
+    -> {class id: dict, ..., 'all': dict}; each dict: rows (scored), failed, gt (rows, 4, 4), and per row name of INIT_ROWS a
+    dict of poses (rows, 4, 4), errors (rows, 4) (translation mm, rotation degrees, ADD m, ADD-S m) and summary
+    (_recover_summary)."""
+    from .produce_train_pair_data import ycbv_keyframe_jobs
+    spec = Engine.init_spec(init)
+    classes = init_classes(ycb_dir, class_ids, class_config)
+    ids = [k['class_id'] for k in classes]
+    jobs = ycbv_keyframe_jobs(ycb_dir, ids)
+    if max_frames is not None:
+        jobs = jobs[:int(max_frames)]
+    starts = MaskStarts(classes, len(ids), init)
+    try:
+        eng, dev, Kk = starts.eng, starts.eng.device, spec.keep
+        set_of = {c: j for j, c in enumerate(ids)}
+        row_set, gts, status, grid, final, cands = [], [], [], [], [], []
+        for rgb_path, depth_path, seg_path, rows in jobs:
+            cls = [c for c, _ in rows]
+            n = len(cls)
+            out = dict(kept_poses=torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev))
+            if spec.icp:
+                out['icp_poses'] = torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev)
+            P, R = starts(read_depth(depth_path), read_seg(seg_path), cls, out=out)
+            row_set += [set_of[c] for c in cls]
+            gts += [B for _, B in rows]
+            status.append(R[:, 0].clone())
+            grid.append(out['kept_poses'][:, 0].clone())
+            final.append(P.clone())
+            cands.append((out['icp_poses'] if spec.icp else out['kept_poses']).clone())
+        N = len(row_set)
+        clouds = [np.asarray(object_cloud(k['model_path']).points, dtype=np.float64).reshape(-1, 3) for k in classes]
+        offsets = np.cumsum([0] + [len(p) for p in clouds]).astype(np.int32)
+        table = torch.from_numpy(np.ascontiguousarray(np.concatenate(clouds))).to(dev)
+        pose_set = np.asarray(row_set, dtype=np.int32)
+        ok = (torch.cat(status) == 0) if N else torch.zeros(0, dtype=torch.bool, device=dev)
+        kidx = torch.nonzero(ok).reshape(-1)
+        kset = pose_set[ok.cpu().numpy()]
+        B = torch.from_numpy(np.ascontiguousarray(np.stack(gts), dtype=np.float64)).to(dev) if N else None
+        keep = ok.to(torch.uint8)
+        scored = {}
+        if N:
+            for name, Pn in (('grid', torch.cat(grid)), ('icp', torch.cat(final))):
+                scored[name] = (Pn, eng.pose_errors_sets(table, pose_set, Pn, B, offsets, keep)[0])
+            every = torch.cat(cands)
+            E_all = eng.pose_errors_sets(table, np.repeat(pose_set, Kk), every.reshape(-1, 4, 4).contiguous(), B.repeat_interleave(Kk, 0),
+                                         offsets, keep.repeat_interleave(Kk, 0))[0].reshape(-1, Kk, 4)
+            best = torch.nan_to_num(E_all[:, :, 3], nan=float('inf')).argmin(1)
+            r = torch.arange(N, device=dev)
+            scored['best of K'] = (every[r, best], E_all[r, best])
+        res = {}
+        for name in INIT_ROWS:
+            if N:
+                Pn, En = (x.index_select(0, kidx) for x in scored[name])
+                ap = (eng.vocap_sets(En[:, 2].contiguous(), kset, len(ids)), eng.vocap_sets(En[:, 3].contiguous(), kset, len(ids)))
+                Pn, En = Pn.cpu().numpy(), En.cpu().numpy()
+            else:
+                Pn, En, ap = np.zeros((0, 4, 4)), np.zeros((0, 4)), ([0.0] * (len(ids) + 1),) * 2
+            for j, c in enumerate(ids + ['all']):
+                sel = np.flatnonzero(kset == j) if c != 'all' else np.arange(len(kset))
+                d = res.setdefault(c, dict(rows=len(sel), gt=(B.index_select(0, kidx).cpu().numpy()[sel] if N else np.zeros((0, 4, 4)))))
+                d[name] = dict(poses=Pn[sel], errors=En[sel], summary=_recover_summary(En[sel], ap[0][j], ap[1][j]))
+        failed = (~ok).cpu().numpy()
+        for j, c in enumerate(ids + ['all']):
+            res[c]['failed'] = int((failed & (pose_set == j)).sum()) if c != 'all' else int(failed.sum())
+        return res
+    finally:
+        starts.close()
+
+
+def print_init_tables(results, names):
+    """initYcbKeyframes' tables: one per class (names: {class id: label}), then the pooled one, in the columns of
+    print_recover_tables plus the failed rows; AUCs in percent, errors in degrees and mm."""
+    head = '%-10s %6s %6s %8s %8s %9s %9s %9s %9s' % ('start', 'rows', 'failed', 'ADD', 'ADD-S', 'rot mean', 'rot med', 'trans mean',
+                                                    'trans med')
+    for c, d in results.items():
+        label = 'all classes' if c == 'all' else 'class %d (%s)' % (c, names.get(c, c))
+        print('%s: %d rows scored, %d failed; AUCs in percent (VOCap, 0.1 m), rotation in degrees, translation in mm'
+              % (label, d['rows'], d['failed']))
+        print(head)
+        for name in INIT_ROWS:
+            s = d[name]['summary']
+            if s['rows'] == 0:
+                print('%-10s %6d %6d' % (name, 0, d['failed']))
+                continue
+            print('%-10s %6d %6d %8.3f %8.3f %9.4g %9.4g %9.4g %9.4g' % (name, s['rows'], d['failed'], 100 * s['add_auc'], 100 * s['adds_auc'],
+                                                                        s['rot_mean'], s['rot_median'], s['trans_mean'], s['trans_median']))
+
+
 def print_recover_tables(results, names):
     """recoverYcbKeyframes' tables: one per class (names: {class id: label}), then the pooled one; a row per (checkpoint, mode,
     round), round 0 (the perturbed start, the same in every variant) printed once.  AUCs in percent, errors in degrees and mm."""
@@ -2388,7 +2641,8 @@ def main(argv=None):
     parser.add_argument('--mode', default='ycbv', help='ycbv (one YCB-Video sequence) / ycbineoat / ycbv_all (every class of --class_ids '
                         'through every YCB-Video test sequence in one pass) / ycbineoat_all (every video under --YCBInEOAT_dir in one '
                         'pass) / ycbv_recover (score refinement from the perturbed starts of the YCB-Video key frames, every class of '
-                        '--class_ids in one pass; nothing is written) / anything else: every YCB-Video test sequence of the class')
+                        '--class_ids in one pass; nothing is written) / ycbv_init (score the starts Engine.init_poses finds from the masks of '
+                        'the YCB-Video key frames; no checkpoint) / anything else: every YCB-Video test sequence of the class')
     parser.add_argument('--seq_id', default=None, type=int)
     parser.add_argument('--ycb_dir', default=None)
     parser.add_argument('--YCBInEOAT_dir', default=None)
@@ -2396,8 +2650,8 @@ def main(argv=None):
     parser.add_argument('--class_id', default=-1, type=int, help='class id in YCB Video')
     parser.add_argument('--class_ids', default=None, help='ycbv_all: comma-separated class ids, or all')
     parser.add_argument('--model_path', type=str, required=True, help='path to mesh (.ply with normals and vertex colours for the CUDA renderer)')
-    parser.add_argument('--ckpt_dir', type=str, required=True)
-    parser.add_argument('--mean_std_path', type=str, required=True)
+    parser.add_argument('--ckpt_dir', type=str, default=None, help='required by every mode but ycbv_init')
+    parser.add_argument('--mean_std_path', type=str, default=None, help='required by every mode but ycbv_init')
     parser.add_argument('--outdir', type=str, default=None, help='required by every mode but ycbv_recover')
     parser.add_argument('--pair_model_path', default=None, help='ycbv_recover: path template of the mesh the perturbed pairs are '
                         'cut with (default --model_path with .ply -> .obj, as ProducerPurturb picks it)')
@@ -2407,7 +2661,16 @@ def main(argv=None):
     parser.add_argument('--hypotheses', type=int, default=None, help='ycbv_all / ycbineoat_all / ycbv_recover: track every step from S '
                         'start hypotheses per track (1..32, default 1) and keep the one whose model fits the frame best')
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
-    parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt)')
+    parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt); ycbv_all also mask: '
+                        'each sequence starts from Engine.init_poses on its first frame\'s depth and seg/ label image')
+    parser.add_argument('--init_viewpoints', type=int, default=None, help='--init mask / ycbv_init: grid viewpoints V (default %d)'
+                        % _engine.Engine.INIT_DEFAULTS['viewpoints'])
+    parser.add_argument('--init_inplane', type=int, default=None, help='--init mask / ycbv_init: in-plane angles R (default %d)'
+                        % _engine.Engine.INIT_DEFAULTS['inplane'])
+    parser.add_argument('--init_keep', type=int, default=None, help='--init mask / ycbv_init: candidates kept K (default %d)'
+                        % _engine.Engine.INIT_DEFAULTS['keep'])
+    parser.add_argument('--init_icp', type=int, default=None, help='--init mask / ycbv_init: ICP iterations on the kept candidates '
+                        '(0: none; default %d)' % _engine.Engine.INIT_DEFAULTS['icp'])
     parser.add_argument('--max_frames', type=int, default=None)
     parser.add_argument('--score', action='store_true', help='ycbv_all / ycbineoat_all: score the output with eval_ycb / '
                         'eval_ycbineoat and print its lines')
@@ -2431,6 +2694,12 @@ def main(argv=None):
     parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
                         'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
+    init = cli_init(args)
+    if args.mode == 'ycbv_init':
+        return _main_init(args, init)
+    missing = [f for f in ('--ckpt_dir', '--mean_std_path') if getattr(args, f[2:]) is None]
+    if missing:
+        parser.error('the following arguments are required: %s' % ', '.join(missing))
     if args.fit is not None:
         if args.mode not in ('ycbv_all', 'ycbineoat_all'):
             raise SystemExit('--fit needs --mode ycbv_all or ycbineoat_all; --mode %s does not check the fit' % args.mode)
@@ -2575,6 +2844,56 @@ def cli_recover(args):
     return class_ids, config, kw
 
 
+def cli_init(args):
+    """The start-from-mask options of the command line -> Engine.init_spec's dict (None: the defaults), also left in
+    args.init_spec.  --init mask needs --mode ycbv_all; the --init_* options need --init mask or --mode ycbv_init; the other
+    modes refuse --init mask and them; a value init_spec refuses is a SystemExit."""
+    flags = {'viewpoints': args.init_viewpoints, 'inplane': args.init_inplane, 'keep': args.init_keep, 'icp': args.init_icp}
+    given = {k: v for k, v in flags.items() if v is not None}
+    if args.init == 'mask' and args.mode != 'ycbv_all':
+        raise SystemExit('--init mask needs --mode ycbv_all; --mode %s does not start from masks (--mode ycbv_init scores the '
+                         'starts on the key frames)' % args.mode)
+    if given and args.mode != 'ycbv_init' and args.init != 'mask':
+        raise SystemExit('%s need --init mask (with --mode ycbv_all) or --mode ycbv_init' % ', '.join('--init_' + k for k in given))
+    spec = given or None
+    try:
+        _engine.Engine.init_spec(spec)
+    except ValueError as e:
+        raise SystemExit('--init_*: %s' % e)
+    args.init_spec = spec
+    return spec
+
+
+def _main_init(args, init):
+    """--mode ycbv_init: initYcbKeyframes, then its tables (print_init_tables).  Needs --ycb_dir, --class_ids, --train_data_path
+    and --model_path; takes no checkpoint, and refuses the tracking options."""
+    if not args.ycb_dir or not args.class_ids:
+        raise SystemExit('--mode ycbv_init needs --ycb_dir and --class_ids')
+    tracking = [f for f, v in (('--outdir', args.outdir), ('--precision', args.precision), ('--iterations', args.iterations),
+                               ('--fit', args.fit), ('--hypotheses', args.hypotheses), ('--icp', args.icp), ('--icp_tau', args.icp_tau),
+                               ('--gpus', args.gpus), ('--video', args.video or None), ('--score', args.score or None)) if v is not None]
+    if tracking:
+        raise SystemExit('%s: --mode ycbv_init scores starts, it does not track (--init_icp sets its ICP)' % ', '.join(tracking))
+    if args.class_ids == 'all':
+        class_ids = list(range(1, len(ycb_class_names(args.ycb_dir)) + 1))
+    else:
+        try:
+            class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
+        except ValueError:
+            raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+    config = dict(train_data_path=args.train_data_path, model_path=args.model_path)
+    try:
+        res = initYcbKeyframes(args.ycb_dir, class_ids, config, init=init, max_frames=args.max_frames)
+    except ValueError as e:
+        raise SystemExit(str(e))
+    names = ycb_class_names(args.ycb_dir)
+    spec = _engine.Engine.init_spec(init)
+    print('ycbv_init: V %d, R %d, K %d, ICP %d, %s' % (spec.viewpoints, spec.inplane, spec.keep, spec.icp.contents.iterations if spec.icp else 0,
+                                                       torch.cuda.get_device_name(torch.cuda.current_device())))
+    print_init_tables(res, {c: names[c - 1] for c in class_ids})
+    return res
+
+
 def _main_recover(args):
     """--mode ycbv_recover: recoverYcbKeyframes, then its tables (print_recover_tables)."""
     class_ids, config, kw = cli_recover(args)
@@ -2623,6 +2942,8 @@ def _main_one_pass(args, precision=None, iterations=None):
                 class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
             except ValueError:
                 raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
+        if args.init == 'mask':
+            kw['init'] = getattr(args, 'init_spec', None)
         res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
         outdir, eoat = args.outdir, {}
     else:
