@@ -39,9 +39,57 @@ from .staging import StagingRing, VideoSink
 from . import Utils as U
 
 _refine_iterations = Engine.refine_iterations      # the drivers check counts before any Engine exists
-_fit_spec = Engine.fit_spec                         # and the fit check's tau
 # Tracker(fit=True)'s tau: a starting guess for a sensor's depth noise at a metre or so, not measured on a real sensor
 FIT_TAU_DEFAULT = 10
+
+# The per-step options of a Tracker or a driver run, as step_options checks them: fit the tau in mm whose rows the caller keeps
+# (None: none), tau the step's fit check in mm (None: off), icp Engine.icp_spec's argument (None: off), hypotheses S and the seed
+# of their draws.  A tuple, so the spawned ranks of a multi-GPU run receive it in their process arguments.
+StepOptions = collections.namedtuple('StepOptions', 'fit tau icp hypotheses seed')
+
+
+def step_options(fit=None, hypotheses=1, seed=0, icp=None, icp_tau=None, fit_switch=False):
+    """The options of every tracking step -> StepOptions, or a ValueError, checked in this order:
+    fit       None or a tau in mm (Engine.fit_spec).  fit_switch (the Tracker's fit) also takes True, FIT_TAU_DEFAULT mm, and
+              False, off, which refuses hypotheses.
+    hypotheses  S, an integer in [1, MAX_HYPOTHESES]; seed an integer.
+    icp       None / 0 off, or M iterations or a dict (Engine.icp_spec); icp_tau the gate in mm, refused without icp.  ICP inside
+              hypothesis steps is not supported: refused with S > 1.
+    S > 1 ranks the starts by the fit check, so the step's tau is fit, or FIT_TAU_DEFAULT when fit is None."""
+    off = fit_switch and fit is False
+    if fit_switch and isinstance(fit, bool):
+        fit = FIT_TAU_DEFAULT if fit else None
+    fit = _engine.Engine.fit_spec(fit) or None
+    if isinstance(hypotheses, (bool, np.bool_)) or not isinstance(hypotheses, (int, np.integer)) or \
+            not 1 <= hypotheses <= _lib.MAX_HYPOTHESES:
+        raise ValueError('hypotheses must be an integer in [1, %d], not %r' % (_lib.MAX_HYPOTHESES, hypotheses))
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)):
+        raise ValueError('seed must be an integer, not %r' % (seed,))
+    if icp_tau is not None:
+        if not icp:
+            raise ValueError('icp_tau %r without icp: the gate of ICP iterations that do not run' % (icp_tau,))
+        icp = {'iterations': icp, 'tau_mm': icp_tau}
+    if _engine.Engine.icp_spec(icp) is None:
+        icp = None
+    elif hypotheses > 1:
+        raise ValueError('icp %r with hypotheses %d: ICP inside hypothesis steps is not supported' % (icp, hypotheses))
+    if off and hypotheses > 1:
+        raise ValueError('hypotheses=%d ranks the starts by the fit check: fit must not be off' % hypotheses)
+    return StepOptions(fit, fit or (FIT_TAU_DEFAULT if hypotheses > 1 else None), icp, int(hypotheses), int(seed))
+
+
+def hypothesis_spread(info, opts, label=None):
+    """The spread a class's start hypotheses are drawn with: its dataset_info's (max_translation m, max_rotation degrees), the
+    bounds its training pairs were drawn with; None when opts has no hypotheses.  A ValueError, prefixed with `label`, when either
+    is missing or Engine.hypothesis_spec refuses it."""
+    if opts.hypotheses == 1:
+        return None
+    try:
+        spread = float(info['max_translation']), float(info['max_rotation'])
+        _engine.Engine.hypothesis_spec(opts.hypotheses, opts.seed, *spread)
+    except (KeyError, TypeError, ValueError) as e:
+        raise ValueError('%sdataset_info max_translation / max_rotation: %s' % ('' if label is None else label + ': ', e)) from e
+    return spread
 
 
 def fit_fractions(rows):
@@ -167,27 +215,14 @@ class Tracker:
         point-to-plane ICP at Engine.icp_spec's default gate, or a dict of its fields.  on_track / on_track_batch then leave the
         last iteration's stats (inliers, rms_mm, step_mm, step_deg per track) in last_icp: numpy on the host route, a float64
         CUDA tensor on the device route.  Like fit it needs the CUDA rasteriser drawing input A inside the step; it is refused
-        with hypotheses > 1."""
+        with hypotheses > 1.  fit, hypotheses, seed and icp are checked by step_options and kept in opts."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
         self.iterations = Engine.refine_iterations(iterations)
-        self.icp = icp if Engine.icp_spec(icp) is not None else None
-        self.last_icp = None
-        self.last_init = None
-        self.hypotheses = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
-        if self.icp is not None and self.hypotheses > 1:
-            raise ValueError('icp=%r with hypotheses=%d: ICP inside hypothesis steps is not supported' % (icp, self.hypotheses))
-        self.seed = int(seed)
-        if self.hypotheses > 1 and fit is None:
-            fit = True
-        self.fit = Engine.fit_spec(FIT_TAU_DEFAULT if fit is True else (None if fit is False else fit)) or None
-        if self.hypotheses > 1 and not self.fit:
-            raise ValueError('hypotheses=%d ranks the starts by the fit check: fit must not be off' % self.hypotheses)
-        self.spread = (float(dataset_info['max_translation']), float(dataset_info['max_rotation'])) if self.hypotheses > 1 else None
-        if self.spread:
-            _engine.Engine.hypothesis_spec(self.hypotheses, seed, *self.spread)
+        self.opts = step_options(fit, hypotheses, seed, icp, fit_switch=True)
+        self.fit, self.icp, self.hypotheses, self.seed = self.opts.tau, self.opts.icp, self.opts.hypotheses, self.opts.seed
+        self.spread = hypothesis_spread(dataset_info, self.opts)
         self._calls = 0                                    # the c of the draw keys (seed, c, j)
-        self.last_fit = None
-        self.last_choice = None
+        self.last_fit = self.last_icp = self.last_choice = self.last_init = None
         self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
@@ -237,15 +272,8 @@ class Tracker:
                     raise
                 renderer = None                                    # e.g. a vertices-only ply: fall through to the GL renderers
         self.renderer = renderer if renderer is not None else self._try_reference_renderer(model_path, cam_cfg)
-        if self.iterations > 1 and not isinstance(self.renderer, CudaRenderer):
-            raise ValueError('iterations=%d redraws input A every round inside the tracking step: it needs the CUDA renderer '
-                             '(renderer="cuda"), not %r' % (self.iterations, self.renderer))
-        if self.fit and not isinstance(self.renderer, CudaRenderer):
-            raise ValueError('fit=%d draws every model at its new pose inside the tracking step: it needs the CUDA renderer '
-                             '(renderer="cuda"), not %r' % (self.fit, self.renderer))
-        if self.icp is not None and not isinstance(self.renderer, CudaRenderer):
-            raise ValueError('icp=%r draws every model at its refined pose inside the tracking step: it needs the CUDA renderer '
-                             '(renderer="cuda"), not %r' % (self.icp, self.renderer))
+        if not isinstance(self.renderer, CudaRenderer):
+            self._check_step_draws(why='it needs the CUDA renderer (renderer="cuda"), not %r' % (self.renderer,))
         self._np_bufs = {}
         self._copy_stream = torch.cuda.Stream(device=self.engine.device)      # _uploads: two staging slots, used alternately
         self._stage_bufs = ({}, {})
@@ -361,8 +389,8 @@ class Tracker:
         Tracker.iterations times."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
-        if (self.iterations > 1 or self.fit or self.icp is not None) and not fused:
-            raise ValueError(self._refine_refusal(rgbA is not None or depthA is not None))
+        if not fused:
+            self._check_step_draws(rgbA is not None or depthA is not None)
         if fused:
             out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
         else:
@@ -400,19 +428,17 @@ class Tracker:
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
         renderer = self._fused_renderer(weight_ids) if render else None      # None: render input A first, then track
-        if (self.iterations > 1 or self.fit or self.icp is not None) and renderer is None:
-            raise ValueError(self._refine_refusal(not render))
-        self.last_fit = None
-        self.last_icp = None
-        self.last_choice = None
-        hyp = None
-        if self.hypotheses > 1:                       # (c << 32) + j: track j's draw key in this call
+        if renderer is None:
+            self._check_step_draws(not render)
+        self.last_fit = self.last_icp = self.last_choice = None
+        opts, hyp = self.opts, None
+        if opts.hypotheses > 1:                       # (c << 32) + j: track j's draw key in this call
             n_tracks = len(prev_poses)
-            if n_tracks * self.hypotheses > self.engine.max_batch:
+            if n_tracks * opts.hypotheses > self.engine.max_batch:
                 raise ValueError('%d tracks x hypotheses=%d exceed the engine\'s max_batch=%d'
-                                 % (n_tracks, self.hypotheses, self.engine.max_batch))
+                                 % (n_tracks, opts.hypotheses, self.engine.max_batch))
             keys = (np.int64(self._calls) << np.int64(32)) + np.arange(n_tracks, dtype=np.int64)
-            hyp = dict(hypotheses=self.hypotheses, max_translation=self.spread[0], max_rotation_deg=self.spread[1], seed=self.seed)
+            hyp = dict(hypotheses=opts.hypotheses, max_translation=self.spread[0], max_rotation_deg=self.spread[1], seed=opts.seed)
         is_np = lambda *xs: all(isinstance(x, np.ndarray) for x in xs)
         if (is_np(current_rgb, current_depth) and (renderer is not None or is_np(rgbA, depthA))
                 and not any(torch.is_tensor(x) for x in (prev_poses, weight_ids, object_width))):
@@ -429,17 +455,17 @@ class Tracker:
             if hyp is not None:
                 out, self.last_choice, self.last_fit = self.engine.track_hypotheses_host(
                     *frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer, keys, mode=renderer.mode,
-                    image_hw=renderer.image_hw, iterations=self.iterations, fit=self.fit, **hyp, **kw)
+                    image_hw=renderer.image_hw, iterations=self.iterations, fit=opts.tau, **hyp, **kw)
                 self._calls += 1                      # only a call that ran uses up its c
                 return out
             if renderer is not None:
                 out = self.engine.track_render_host(*frame, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                     mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
-                                                    fit=self.fit, icp=self.icp, **kw)
-                if self.icp is not None:
+                                                    fit=opts.tau, icp=opts.icp, **kw)
+                if opts.icp is not None:
                     *out, self.last_icp = out
                     out = out[0] if len(out) == 1 else tuple(out)
-                if self.fit:
+                if opts.tau:
                     out, self.last_fit = out
                 return out
             return self.engine.track_host(*frame, self.K, poses, ow, *A, self.trans_normalizer, self.rot_normalizer, **kw)
@@ -476,30 +502,32 @@ class Tracker:
                 torch.arange(n, dtype=torch.int64, device=dev, out=kb[0]).add_(self._calls << 32)
                 out, self.last_choice, self.last_fit = self.engine.track_hypotheses(
                     rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer, kb[0], mode=renderer.mode,
-                    image_hw=renderer.image_hw, iterations=self.iterations, fit=self.fit, out_choice=kb[1], out_fit=kb[2], **hyp, **kw)
+                    image_hw=renderer.image_hw, iterations=self.iterations, fit=opts.tau, out_choice=kb[1], out_fit=kb[2], **hyp, **kw)
                 self._calls += 1
             elif renderer is not None:                  # input A is drawn inside the step, with the weight ids as mesh ids
                 res = self.engine.track_render(rgb_d, depth_d, self.K, poses, ow, self.trans_normalizer, self.rot_normalizer,
                                                mode=renderer.mode, image_hw=renderer.image_hw, iterations=self.iterations,
-                                               fit=self.fit, icp=self.icp, **kw)
+                                               fit=opts.tau, icp=opts.icp, **kw)
                 out = res[0]
-                if self.fit:
+                if opts.tau:
                     self.last_fit = res[3]
-                if self.icp is not None:
+                if opts.icp is not None:
                     self.last_icp = res[-1]
             else:
                 out, _, _ = self.engine.track_batch(rgb_d, depth_d, self.K, poses, ow, rgbA_d, depthA_d,
                                                     self.trans_normalizer, self.rot_normalizer, **kw)
         return out.cpu().numpy() if as_numpy else out
 
-    def _refine_refusal(self, given):
-        """Why a call of a Tracker with iterations > 1 or a fit check cannot run: input A given (given), or a renderer the step
-        cannot stand in for."""
-        why = 'input A was passed in' if given else 'the renderer cannot draw input A inside the tracking step (_fused_renderer)'
+    def _check_step_draws(self, given=False, why=None):
+        """A ValueError when iterations > 1, the fit check or ICP need the models drawn inside the tracking step and it cannot
+        draw them: why, or input A given (given), or a renderer the step cannot stand in for."""
+        if why is None:
+            why = 'input A was passed in' if given else 'the renderer cannot draw input A inside the tracking step (_fused_renderer)'
         needs = (['iterations=%d redraws input A at each refined pose' % self.iterations] if self.iterations > 1 else []) + \
-                (['fit=%d draws every model at its new pose' % self.fit] if self.fit else []) + \
-                (['icp=%r draws every model at its refined pose' % (self.icp,)] if self.icp is not None else [])
-        return '%s, but %s' % (' and '.join(needs), why)
+                (['fit=%d draws every model at its new pose' % self.opts.tau] if self.opts.tau else []) + \
+                (['icp=%r draws every model at its refined pose' % (self.opts.icp,)] if self.opts.icp is not None else [])
+        if needs:
+            raise ValueError('%s, but %s' % (' and '.join(needs), why))
 
     def _weight_ids(self, weight_ids, n):
         """The tracks' weight ids as an int32 host array: the Tracker's weight set unless given, None for set 0 (a step
@@ -1182,47 +1210,53 @@ def hypothesis_key(a, b, c):
     return (a << 40) + (b << 16) + c
 
 
-def hypothesis_groups(trackers, wh):
-    """The tracks of one step grouped by the spread of their class's dataset_info ((max_translation m, max_rotation degrees), the
-    bounds its training pairs were drawn with): [(None or an int64 numpy index array, spread)].  One group of all tracks (None)
-    when every class shares one spread; otherwise the step runs once per spread on its tracks."""
-    spreads = [(float(trackers[int(w)].dataset_info['max_translation']), float(trackers[int(w)].dataset_info['max_rotation']))
-               for w in wh]
+def hypothesis_groups(trackers, wh, opts):
+    """The tracks of one step grouped by the spread of their class (hypothesis_spread): [(None or an int64 numpy index array,
+    spread)].  One group of all tracks (None) when every class shares one spread; otherwise the step runs once per spread on its
+    tracks."""
+    spreads = [hypothesis_spread(trackers[int(w)].dataset_info, opts) for w in wh]
     if len(set(spreads)) == 1:
         return [(None, spreads[0])]
     return [(np.asarray([j for j, sp in enumerate(spreads) if sp == g], dtype=np.int64), g) for g in sorted(set(spreads))]
 
 
-def hypothesis_step(eng, trk, rgb, depth, poses, widths, wh, wd, keys, groups, S, seed, tau, precision, iterations, outs):
-    """One driver step of S hypotheses per track (Engine.track_hypotheses) over the frame (rgb, depth), per spread group
-    (hypothesis_groups).  outs: out_poses (n,4,4), out_trans / out_rot (n,3), out_choice (n), out_fit (n,6), and optionally
-    out_hyp_poses (n,S,4,4) / out_rounds (k,n,S,4,4); the rows of each group land at their tracks.  poses may be out_poses."""
-    mode = dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw)
-    for idx, (mt, mr) in groups:
-        kw = dict(fit=tau, precision=precision, iterations=iterations, max_translation=mt, max_rotation_deg=mr, seed=seed, **mode)
+def track_step(eng, trackers, trk, rgb, depth, poses, widths, wh, wd, keys, opts, precision, iterations, outs):
+    """One driver step of a variant for n tracks over the device frame (rgb, depth), with trk's camera, normalisers and render
+    mode.  Without hypotheses, one Engine.track_render with opts' fit check and ICP.  With S > 1, Engine.track_hypotheses with
+    the draw keys `keys` (int64 (n)), once per spread group (hypothesis_groups), the rows of each group landing at their tracks.
+    outs: out_poses (n,4,4), out_trans / out_rot (n,3), and as the step has them out_fit (n,6), out_choice (n), out_rounds
+    (k,n,4,4) / (k,n,S,4,4), out_hyp_poses (n,S,4,4), out_icp_poses (M,n,4,4).  poses may be out_poses."""
+    kw = dict(fit=opts.tau, precision=precision, iterations=iterations, mode=trk.renderer.mode, image_hw=trk.renderer.image_hw)
+    if opts.hypotheses == 1:
+        eng.track_render(rgb, depth, trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer, weight_ids_host=wh,
+                         weight_ids_dev=wd, icp=opts.icp, **kw, **outs)
+        return
+    for idx, (mt, mr) in hypothesis_groups(trackers, wh, opts):
+        hyp = dict(kw, max_translation=mt, max_rotation_deg=mr, seed=opts.seed)
         if idx is None:
-            eng.track_hypotheses(rgb, depth, trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer, keys, S,
-                                 weight_ids_host=wh, weight_ids_dev=wd, **kw, **outs)
+            eng.track_hypotheses(rgb, depth, trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer, keys, opts.hypotheses,
+                                 weight_ids_host=wh, weight_ids_dev=wd, **hyp, **outs)
             continue
         di = torch.from_numpy(idx).to(eng.device)
         sub = {k: (v.index_select(1, di) if k == 'out_rounds' else v.index_select(0, di)).contiguous() for k, v in outs.items()}
         eng.track_hypotheses(rgb, depth, trk.K, poses.index_select(0, di).contiguous(), widths.index_select(0, di).contiguous(),
-                             trk.trans_normalizer, trk.rot_normalizer, keys.index_select(0, di).contiguous(), S,
-                             weight_ids_host=wh[idx], weight_ids_dev=wd.index_select(0, di).contiguous(), **kw, **sub)
+                             trk.trans_normalizer, trk.rot_normalizer, keys.index_select(0, di).contiguous(), opts.hypotheses,
+                             weight_ids_host=wh[idx], weight_ids_dev=wd.index_select(0, di).contiguous(), **hyp, **sub)
         for k, v in sub.items():
             outs[k].index_copy_(1 if k == 'out_rounds' else 0, di, v)
 
 
-def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=None, fit=0, hyp=None, seq_index=None, icp=None):
+def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
     """The one-pass drivers' tracking loop.  sequences: [(rgb files, depth files, weight ids (tuple), initial poses (n,4,4))], the
     files those of the frames to track; trackers: {weight id: Tracker} on eng, sharing camera, normalisers and render mode;
     variants: what every frame is tracked in (a tuple) as _sweep_variants keys them, (mode, k) or (mode, k, c): precision mode, k
-    refinement rounds per step (Engine.track_render's iterations) and the weight sets of checkpoint c (ids + CKPT_ID_STRIDE * c).  Yields each sequence's {variant: (frames, n, 4, 4) numpy poses}, the poses after each
-    frame, as soon as the sequence ends.
+    refinement rounds per step (Engine.track_render's iterations) and the weight sets of checkpoint c (ids + CKPT_ID_STRIDE * c).
+    Yields each sequence's ({variant: (frames, n, 4, 4) numpy poses}, the poses after each frame, and its fit rows or None) as
+    soon as the sequence ends.
 
-    Every frame is one se3tn_track_render step per variant for the sequence's n tracks, all reading the same device frame: the
-    frames of all sequences decode ahead, across sequence boundaries, through one StagingRing of `depth` sets (`workers` threads)
-    into its one device frame, so a frame is decoded once whatever the number of variants.  The steps' other device arguments are
+    Every frame is one se3tn_track_render step per variant (track_step) for the sequence's n tracks, all reading the same device
+    frame: the frames of all sequences decode ahead, across sequence boundaries, through one StagingRing of `depth` sets (`workers`
+    threads) into its one device frame, so a frame is decoded once whatever the number of variants.  The steps' other device arguments are
     kept: the ids and widths per distinct weight-id tuple, and per (variant, n) the pose tensor that variant's steps update in place
     and their outputs.  So in each variant every step after a track set's first replays that variant's CUDA graph, across
     sequences too ('fp32' steps are never captured).  Each checkpoint steps in the sequence's n, as a run of it alone does, so
@@ -1236,16 +1270,11 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
     VideoSink of `depth` sets writes the half-size frames; every video is complete when the generator is exhausted or closed.
     Videos are drawn for one variant only.
 
-    fit: tau in mm turns on every step's fit check (Engine.track_render's fit); each sequence's yield is then a pair, the poses
-    as above and {variant: (frames, n, 6) int32 numpy rows}, row t the fit of the step that wrote pose t.
-
-    hyp: None, or (S, seed) with S > 1: every step tracks S hypotheses per track (hypothesis_step, the spread of each class's
-    dataset_info; the fit check at `fit`, or FIT_TAU_DEFAULT without it), the poses and fit rows being the kept hypotheses'.
-    Track j of frame t of sequence k draws with hypothesis_key(seq_index[k], t, j); seq_index (default 0, 1, ...) is each
-    sequence's index in the run's sorted list, so a share of the sequences on one GPU draws what the whole run draws.
-
-    icp: None, or Engine.icp_spec's dict: every step refines its tracks with ICP after the last round (Engine.track_render's
-    icp); the poses and, with fit, the fit rows are those after ICP.  Not combined with hyp (_driver_icp refuses it)."""
+    opts: step_options' value for every step.  With opts.fit, each sequence's fit rows are {variant: (frames, n, 6) int32 numpy
+    rows}, row t the fit of the step that wrote pose t.  With ICP the poses and fit rows are those after ICP.  With S > 1
+    hypotheses the poses and fit rows are the kept hypotheses', and track j of frame t of sequence k draws with
+    hypothesis_key(seq_index[k], t, j): seq_index is each sequence's index in the run's sorted list, so a share of the sequences
+    on one GPU draws what the whole run draws."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
     fp8 = {}                                               # checkpoint index -> its first fp8 variant
@@ -1278,11 +1307,6 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
             sink = stack.enter_context(contextlib.closing(VideoSink((max(len(s[2]) for s in sequences), H // 2, W // 2, 3), depth, dev)))
         uploads = stack.enter_context(contextlib.closing(ring.uploads(frames, workers)))
         by_ids, by_n = {}, {}
-        if hyp is not None:
-            S, seed = hyp
-            hyp_tau = fit or FIT_TAU_DEFAULT
-            seq_index = list(range(len(sequences))) if seq_index is None else list(seq_index)
-            hyp_out = {}                                   # per (variant, n): the keys, choices and fit rows, at fixed addresses
         for k, (rgb_files, _, ids, init) in enumerate(sequences):
             n = len(ids)
             for c in _checkpoints(variants):
@@ -1292,48 +1316,41 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video=N
                                       torch.tensor([trackers[int(w)].object_width for w in wh], dtype=torch.float64, device=dev))
             for v in variants:
                 if (v, n) not in by_n:
-                    by_n[v, n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
-                                  torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
-                                  None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
-                by_n[v, n][0].copy_(torch.from_numpy(init))
+                    outs = dict(out_poses=torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
+                                out_trans=torch.empty((n, 3), dtype=torch.float32, device=dev),
+                                out_rot=torch.empty((n, 3), dtype=torch.float32, device=dev))
+                    keys = None
+                    if opts.hypotheses > 1:                # the draw keys, choices and kept rows, at fixed addresses
+                        keys = torch.empty(n, dtype=torch.int64, device=dev)
+                        outs.update(out_choice=torch.empty(n, dtype=torch.int32, device=dev),
+                                    out_fit=torch.empty((n, 6), dtype=torch.int32, device=dev))
+                    by_n[v, n] = (outs, keys, None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
+                by_n[v, n][0]['out_poses'].copy_(torch.from_numpy(init))
             history = {v: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for v in variants}
-            fit_rows = {v: torch.empty((len(rgb_files), n, 6), dtype=torch.int32, device=dev) for v in variants} if fit else None
+            fit_rows = {v: torch.empty((len(rgb_files), n, 6), dtype=torch.int32, device=dev) for v in variants} if opts.fit else None
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
                 next(uploads)
                 for c, v in (fp8.items() if t == 0 else ()):   # each set calibrated on the first frame of its first sequence
                     wh, wd, widths = by_ids[ids, c]
-                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[v, n][0], widths, weight_ids=wh,
+                    eng.calibrate_fp8_tracks(ring.dev['rgb'], ring.dev['depth'], trk.K, by_n[v, n][0]['out_poses'], widths, weight_ids=wh,
                                              render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
                 for v in variants:
-                    m, rounds = v[:2]
                     wh, wd, widths = by_ids[ids, _variant_checkpoint(v)]
-                    poses, out_trans, out_rot, drawn = by_n[v, n]
-                    if hyp is not None:
-                        if (v, n) not in hyp_out:
-                            hyp_out[v, n] = (torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
-                                             torch.empty((n, 6), dtype=torch.int32, device=dev))
-                        keys, choice, rows = hyp_out[v, n]
+                    outs, keys, drawn = by_n[v, n]
+                    poses = outs['out_poses']
+                    if keys is not None:
                         keys.copy_(torch.arange(n, dtype=torch.int64, device=dev) + hypothesis_key(seq_index[k], t, 0))
-                        hypothesis_step(eng, trk, ring.dev['rgb'], ring.dev['depth'], poses, widths, wh, wd, keys,
-                                        hypothesis_groups(trackers, wh), S, seed, hyp_tau, m, rounds,
-                                        dict(out_poses=poses, out_trans=out_trans, out_rot=out_rot, out_choice=choice,
-                                             out_fit=fit_rows[v][t] if fit else rows))
-                        history[v][t].copy_(poses)
-                        continue
-                    eng.track_render(ring.dev['rgb'], ring.dev['depth'], trk.K, poses, widths, trk.trans_normalizer, trk.rot_normalizer,
-                                     weight_ids_host=wh, weight_ids_dev=wd, precision=m, mode=trk.renderer.mode,
-                                     image_hw=trk.renderer.image_hw, out_poses=poses, out_trans=out_trans, out_rot=out_rot,
-                                     iterations=rounds, **({'fit': fit, 'out_fit': fit_rows[v][t]} if fit else {}),
-                                     **({'icp': icp} if icp else {}))
+                    track_step(eng, trackers, trk, ring.dev['rgb'], ring.dev['depth'], poses, widths, wh, wd, keys, opts, v[0], v[1],
+                               dict(outs, out_fit=fit_rows[v][t]) if fit_rows else outs)
                     history[v][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
                                     label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
                     sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
-            tracked = {v: h.cpu().numpy() for v, h in history.items()}
-            yield (tracked, {v: r.cpu().numpy() for v, r in fit_rows.items()}) if fit else tracked
+            yield ({v: h.cpu().numpy() for v, h in history.items()},
+                   None if fit_rows is None else {v: r.cpu().numpy() for v, r in fit_rows.items()})
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1421,15 +1438,13 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
                                  render=dict(mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, mesh_ids=wd))
 
 
-def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, fit=0, hyp=None,
-                 icp=None):
+def _track_share(entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video, writes, opts):
     """One process's share of a one-pass run, sequences[k] for k in mine: the Engine and Trackers of `entries`
     (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
-    share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's poses.  video: None, or (label order,
-    [(paths, labels)] per sequence, folders to make once the trackers exist).  fit: _track_sequences' fit (then writes[k] gets
-    its (poses, fit rows) pair).  hyp: _track_sequences' hyp (the Engine then holds max_batch x S tracks per step).  icp:
-    _track_sequences' icp.  -> (Engine, {k: what writes[k] returned})."""
-    eng, trackers = _one_pass_trackers(entries, precision, max_batch * (hyp[0] if hyp else 1))
+    share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's (poses, fit rows or None).  video: None, or
+    (label order, [(paths, labels)] per sequence, folders to make once the trackers exist).  opts: _track_sequences' opts (the
+    Engine holds max_batch x S tracks per step).  -> (Engine, {k: what writes[k] returned})."""
+    eng, trackers = _one_pass_trackers(entries, precision, max_batch * opts.hypotheses)
     for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
         _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
     drawn = None
@@ -1438,15 +1453,15 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
             os.makedirs(d, exist_ok=True)
         drawn = (video[0], [video[1][k] for k in mine])
     out = {}
-    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp, 'seq_index': list(mine)} if hyp else {}), **({'icp': icp} if icp else {}))
-    for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn, **fit_kw), mine):
+    for tracked, k in zip(_track_sequences(eng, trackers, [sequences[k] for k in mine], variants, depth, workers, drawn, opts,
+                                           list(mine)), mine):
         fn, *args = writes[k]
         out[k] = fn(*args, tracked)
     return eng, out
 
 
 def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, mine, borrowed, variants, depth, workers, video,
-               writes, fit=0, hyp=None, icp=None):
+               writes, opts):
     """Rank `rank` of a multi-GPU one-pass run, in its own process on cuda:`device`: _track_share with the weight sets of its
     sequences.  Sends ('ok', {k: what writes[k] returned}, {weight id: fp8 scales or None}) or ('error', traceback text) through
     conn."""
@@ -1455,7 +1470,7 @@ def _rank_main(conn, rank, device, entries, precision, max_batch, sequences, min
         wids = _rank_weight_ids(sequences, mine, variants)
         torch.cuda.set_device(device)
         eng, out = _track_share([e for e in entries if e[0] in wids], precision, max_batch, sequences, mine, borrowed, variants,
-                                depth, workers, video, writes, fit, hyp, icp)
+                                depth, workers, video, writes, opts)
         conn.send(('ok', out, {w: eng.fp8_scales(w) for w in sorted(wids)}))
     except BaseException:
         conn.send(('error', traceback.format_exc()))
@@ -1482,7 +1497,7 @@ def _agree_fp8_scales(per_rank):
     return {w: s for w, (_, s) in sorted(out.items())}
 
 
-def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, fit=0, hyp=None, icp=None):
+def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, opts):
     """_track_share over `sequences` on min(gpus, len(sequences)) GPUs, with writes[k] applied to sequence k's poses on its
     rank (_rank_main) -> [what writes[k] returned], in sequence order.  Sequences are shared out by assign_ranks on their
     frame counts; rank r runs as a spawned process on _rank_devices()[r].  A rank that raises or dies is a RuntimeError naming it,
@@ -1506,7 +1521,7 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
             borrowed = borrowed_calibrations(track_sets, mine) if fp8 else {}
             p = ctx.Process(target=_rank_main, name='one-pass rank %d' % r, daemon=True,
                             args=(send, r, devices[r], entries, precision, max_batch, sequences, mine, borrowed, variants, depth,
-                                  workers, video, writes, fit, hyp, icp))
+                                  workers, video, writes, opts))
             try:
                 p.start()
             finally:
@@ -1552,41 +1567,6 @@ FIT_FILE = 'fit.npy'
 FIT_LOST_ADDS = 0.02
 
 
-def _driver_icp(icp, icp_tau=None, hypotheses=1):
-    """The drivers' icp (M iterations, 0 / None: off) and icp_tau (the gate in mm, None: Engine.ICP_TAU_DEFAULT) -> None, or the
-    dict Engine.icp_spec takes; a ValueError for values it refuses, icp_tau without icp, or icp with hypotheses > 1 (ICP inside
-    hypothesis steps is not supported).  Checked before anything is read."""
-    if not icp:
-        if icp_tau is not None:
-            raise ValueError('icp_tau %r without icp: the gate of ICP iterations that do not run' % (icp_tau,))
-        return None
-    spec = {'iterations': icp} if icp_tau is None else {'iterations': icp, 'tau_mm': icp_tau}
-    _engine.Engine.icp_spec(spec)
-    if hypotheses != 1:
-        raise ValueError('icp %r with hypotheses %r: ICP inside hypothesis steps is not supported' % (icp, hypotheses))
-    return spec
-
-
-def _driver_hypotheses(hypotheses, seed, entries):
-    """The drivers' hypotheses / seed -> None for 1, else (S, seed) for _track_sequences; a ValueError for S outside [1, 32], a
-    non-integer seed, or a class / object whose dataset_info spread (max_translation, max_rotation) se3tn_hypothesis_opts refuses."""
-    hyp = _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
-    if hyp.hypotheses == 1:
-        return None
-    for _, label, k in entries:
-        info = k['dataset_info']
-        try:
-            _engine.Engine.hypothesis_spec(hypotheses, seed, info['max_translation'], info['max_rotation'])
-        except (KeyError, TypeError, ValueError) as e:
-            raise ValueError('%s: dataset_info max_translation / max_rotation: %s' % (label, e)) from e
-    return int(hyp.hypotheses), int(seed)
-
-
-def _driver_fit(fit):
-    """The drivers' fit argument -> tau in mm, 0 for None (Engine.fit_spec; checked before anything is read)."""
-    return _fit_spec(fit)
-
-
 def write_fit_rows(folder, rows):
     """<folder>/FIT_FILE: the fit rows of a sequence as int32 (frames, 6)."""
     os.makedirs(folder, exist_ok=True)
@@ -1594,14 +1574,16 @@ def write_fit_rows(folder, rows):
 
 
 # What a one-pass driver's shared front hands its back: the GPU count, the first mode (the Trackers' precision, which
-# ycb_all_classes / ycbineoat_objects check), the variants (_sweep_variants) and whether modes and counts are swept.
-_OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep configs')
+# ycb_all_classes / ycbineoat_objects check), the variants (_sweep_variants), whether modes and counts are swept, the
+# checkpoints' configurations and the steps' options (step_options).
+_OnePass = collections.namedtuple('_OnePass', 'gpus precision variants sweep ksweep configs opts')
 
 
-def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
+def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config, **step):
     """The checks both one-pass drivers make first, in this order, before anything is read: gpus (check_gpus), the precision
     modes among `modes` (precision_modes), one mode with video, the refinement counts (refine_counts), one count with video, the
-    checkpoints of config's ckpt_dir / mean_std_path lists (checkpoint_configs), one checkpoint with video.  -> _OnePass."""
+    checkpoints of config's ckpt_dir / mean_std_path lists (checkpoint_configs), one checkpoint with video, then the steps'
+    fit, hypotheses and ICP (step_options of `step`).  -> _OnePass."""
     gpus = check_gpus(gpus)
     modes, sweep = precision_modes(precision, modes)
     if video and len(modes) > 1:
@@ -1612,27 +1594,29 @@ def _one_pass_front(outdir, gpus, precision, modes, video, iterations, config):
     configs = checkpoint_configs(config)
     if video and len(configs) > 1:
         raise ValueError('video=True draws the result videos of one checkpoint, not of %d' % len(configs))
-    return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs)
+    return _OnePass(gpus, modes[0], _sweep_variants(outdir, modes, sweep, counts, ksweep, len(configs)), sweep, ksweep, configs,
+                    step_options(**step))
 
 
-def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect, fit=0, hyp=None, icp=None):
-    """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass), in this process
-    (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k] applied to
-    sequence k's poses.  With several checkpoints, a run whose weight sets do not fit in free device memory is refused first
-    (check_weight_sets_fit; per rank on several GPUs).  -> the driver's return value: _sweep_results of {variant:
-    collect(written, variant)}, written being [what writes[k] returned] in sequence order.  fit: every step's fit check
-    (_track_sequences), writes[k] then taking the (poses, fit rows) pair.  hyp, icp: _track_sequences' hyp and icp."""
+def _one_pass_back(run, entries, max_batch, sequences, depth, workers, video, writes, collect):
+    """The shared end of both one-pass drivers: `sequences` tracked in every variant of run (an _OnePass) with run.opts, in this
+    process (_track_share over all of them, every entry loaded) or shared out over run.gpus ranks (_track_on_ranks), writes[k]
+    applied to sequence k's (poses, fit rows or None).  Every entry's hypothesis spread is checked first (hypothesis_spread), and
+    with several checkpoints a run whose weight sets do not fit in free device memory is refused (check_weight_sets_fit; per rank
+    on several GPUs).  -> the driver's return value: _sweep_results of {variant: collect(written, variant)}, written being [what
+    writes[k] returned] in sequence order."""
+    for _, label, k in entries:
+        hypothesis_spread(k['dataset_info'], run.opts, label)
     keys = tuple(v[:-1] for v in run.variants)
     if run.gpus == 1 and len(run.configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
-    fit_kw = dict({'fit': fit} if fit else {}, **({'hyp': hyp} if hyp else {}), **({'icp': icp} if icp else {}))
     if run.gpus == 1:
         _, out = _track_share(entries, run.precision, max_batch, sequences, range(len(sequences)), {}, keys, depth, workers, video,
-                              writes, **fit_kw)
+                              writes, run.opts)
         written = [out[k] for k in range(len(sequences))]
     else:
         written = _track_on_ranks(run.gpus, entries, run.precision, max_batch, sequences, keys, depth, workers, video, writes,
-                                  **fit_kw)
+                                  run.opts)
     return _sweep_results({key: collect(written, key) for key in keys}, run.variants, run.sweep, run.ksweep)
 
 
@@ -1643,27 +1627,20 @@ def _ckpt_label(i, run):
 
 def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
     """One test sequence's files of a getResultsYcbAll run: for each variant (dirs: {variant: {class id: result folder}}) and
-    class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  -> {variant: (frames, n, 4, 4) poses}."""
+    class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  tracked: (poses, fit rows or None); with rows, each seq<id>/ also
+    gets FIT_FILE, one row per pose file, row 0 (the start pose, not tracked) all -1.  -> {variant: (frames, n, 4, 4) poses}."""
+    poses, rows = tracked
     out = {}
     for v, folder in dirs.items():
-        pred_poses = np.concatenate([init[None], tracked[v]])    # row 0: the start pose, as in getResultsYcb
+        pred_poses = np.concatenate([init[None], poses[v]])      # row 0: the start pose, as in getResultsYcb
         for j, c in enumerate(cls):
             sdir = os.path.join(folder[c], 'seq{}'.format(seq_id))
             os.makedirs(sdir, exist_ok=True)
             for i in range(len(pred_poses)):
                 np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
+            if rows is not None:
+                write_fit_rows(sdir, np.concatenate([np.full((1, 6), -1, np.int32), rows[v][:, j]]))
         out[v] = pred_poses
-    return out
-
-
-def _write_ycb_all_sequence_fit(dirs, seq_id, cls, init, tracked):
-    """_write_ycb_all_sequence with the fit check: tracked is (poses, fit rows); each class's seq<id>/ also gets FIT_FILE, one
-    row per pose file, row 0 (the start pose, not tracked) all -1."""
-    poses, rows = tracked
-    out = _write_ycb_all_sequence(dirs, seq_id, cls, init, poses)
-    for v, folder in dirs.items():
-        for j, c in enumerate(cls):
-            write_fit_rows(os.path.join(folder[c], 'seq{}'.format(seq_id)), np.concatenate([np.full((1, 6), -1, np.int32), rows[v][:, j]]))
     return out
 
 
@@ -1775,7 +1752,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
 
     icp: M iterations of ICP after every step's last round (Engine.track_render's icp), at the gate icp_tau mm
     (Engine.ICP_TAU_DEFAULT when None); the pose files hold the refined poses and FIT_FILE, with fit, the fit after ICP.  0 is the
-    plain run, file for file; several GPUs write the one-GPU trees.  Refused with hypotheses > 1 (_driver_icp).
+    plain run, file for file; several GPUs write the one-GPU trees.  Refused with hypotheses > 1 (step_options).
 
     initialize_method='mask': each sequence's tracks start from one Engine.init_poses call on its first frame (depth_filled and
     seg/ label image; each class's label is its class id; init: Engine.init_spec's argument), made in this process before any
@@ -1785,10 +1762,8 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
         raise ValueError("init options need initialize_method='mask', not %r" % (initialize_method,))
     if initialize_method == 'mask':
         Engine.init_spec(init)
-    run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config)
-    fit = _driver_fit(fit)
-    _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
-    icp = _driver_icp(icp, icp_tau, hypotheses)
+    run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config, fit=fit,
+                          hypotheses=hypotheses, seed=seed, icp=icp, icp_tau=icp_tau)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf', 'mask'):
         raise ValueError('initialize_method must be gt, posecnn, poserbpf or mask')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
@@ -1834,8 +1809,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                             ['frame:%d' % (i + 1) for i in range(1, 1 + len(s[0]))]) for (seq_id, cls), s in zip(track_sets.items(), sequences)],
                  [ycb_all_res_dir(tree, c) for c in name_of.values()])
     dirs = {v[:-1]: {c: ycb_all_res_dir(v[-1], name) for c, name in name_of.items()} for v in run.variants}
-    writer = _write_ycb_all_sequence_fit if fit else _write_ycb_all_sequence
-    writes = [(writer, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
+    writes = [(_write_ycb_all_sequence, dirs, seq_id, tuple(cls), s[3]) for (seq_id, cls), s in zip(track_sets.items(), sequences)]
 
     def collect(written, key):
         out = {c: {} for c in name_of}
@@ -1843,8 +1817,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
             for j, c in enumerate(cls):
                 out[c][seq_id] = pred_poses[key][:, j]
         return out
-    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect, fit,
-                          _driver_hypotheses(hypotheses, seed, entries), icp)
+    return _one_pass_back(run, entries, max_batch, sequences, 2, 2, drawn, writes, collect)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1914,21 +1887,15 @@ def write_video_poses(outdir, video, poses):
 
 def _write_ycbineoat_video(roots, video, tracked):
     """One video's files of a getResultsYcbInEOAT run: write_video_poses under each variant's tree (roots: {variant: tree}).
-    -> {variant: (frames, 4, 4) poses}."""
+    tracked: (poses, fit rows or None); with rows, <tree>/<video>/ also gets FIT_FILE, one row per pose file (every frame is
+    tracked).  -> {variant: (frames, 4, 4) poses}."""
+    poses, rows = tracked
     out = {}
     for key, root in roots.items():
-        out[key] = tracked[key][:, 0]
+        out[key] = poses[key][:, 0]
         write_video_poses(root, video, out[key])
-    return out
-
-
-def _write_ycbineoat_video_fit(roots, video, tracked):
-    """_write_ycbineoat_video with the fit check: tracked is (poses, fit rows); <tree>/<video>/ also gets FIT_FILE, one row per
-    pose file (every frame is tracked)."""
-    poses, rows = tracked
-    out = _write_ycbineoat_video(roots, video, poses)
-    for key, root in roots.items():
-        write_fit_rows(os.path.join(root, video), rows[key][:, 0])
+        if rows is not None:
+            write_fit_rows(os.path.join(root, video), rows[key][:, 0])
     return out
 
 
@@ -1968,10 +1935,8 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
     hypotheses, seed: as in getResultsYcbAll, sequence k being the k-th video of the sorted list.
     icp, icp_tau: as in getResultsYcbAll."""
     from .eval_ycbineoat import OBJECTS
-    run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config)
-    fit = _driver_fit(fit)
-    _engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0)
-    icp = _driver_icp(icp, icp_tau, hypotheses)
+    run = _one_pass_front(outdir, gpus, precision, PRECISIONS, video, iterations, object_config, fit=fit, hypotheses=hypotheses,
+                          seed=seed, icp=icp, icp_tau=icp_tau)
     decode_ahead = int(decode_ahead)
     if decode_ahead < 1:
         raise ValueError('decode_ahead must be at least 1')
@@ -1994,10 +1959,9 @@ def getResultsYcbInEOAT(ycbineoat_dir, object_config, outdir, precision='bf16x3'
         drawn = ('over', [([os.path.join(tree, v + '.mp4')], ['frame:%d' % i for i in range(len(s[0]))]) for v, s in sequences.items()],
                  [tree])
     trees = {v[:-1]: v[-1] for v in run.variants}
-    writes = [(_write_ycbineoat_video_fit if fit else _write_ycbineoat_video, trees, v) for v in sequences]
+    writes = [(_write_ycbineoat_video, trees, v) for v in sequences]
     return _one_pass_back(run, entries, 1, list(sequences.values()), decode_ahead, 2 * decode_ahead, drawn, writes,
-                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)}, fit,
-                          _driver_hypotheses(hypotheses, seed, entries), icp)
+                          lambda written, key: {v: w[key] for v, w in zip(sequences, written)})
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -2093,8 +2057,8 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
     Each dict: rows, A_in_cam / B_in_cam (rows, 4, 4), poses (K, rows, 4, 4) after each round, errors (K + 1, rows, 4) (translation
     mm, rotation degrees, ADD m, ADD-S m; index 0 the start), and summary: K + 1 dicts of _recover_summary (AUCs in [0, 1]).
 
-    hypotheses: S in [1, 32].  S > 1 makes every row's step track S hypotheses around its A_in_cam (hypothesis_step: the spread of
-    its class's dataset_info, the fit check at FIT_TAU_DEFAULT, row j of key frame f keyed hypothesis_key(f, j, 0) and `seed`).
+    hypotheses: S in [1, 32].  S > 1 makes every row's step track S hypotheses around its A_in_cam (track_step: the spread of
+    its class's dataset_info, the fit check at step_options' tau, row j of key frame f keyed hypothesis_key(f, j, 0) and `seed`).
     poses / errors / summary are then hypothesis 0's rounds (an n x S-track step's), and each dict also has 'selected' (the fit's
     choice) and 'best' (per row the hypothesis with the lowest ADD-S against B_in_cam, the bound any selection rule can reach),
     each a dict of poses (rows, 4, 4), errors (rows, 4), summary (one _recover_summary), and 'choice' (rows,) for 'selected'
@@ -2107,9 +2071,8 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
     from . import _lib
     from .produce_train_pair_data import ycbv_producers, ycbv_pair_steps, ycbv_keyframe_jobs
     modes, K = recover_front(precision, iterations, gpus)
-    S = int(_engine.Engine.hypothesis_spec(hypotheses, seed, 0.01, 1.0).hypotheses)
-    icp = _driver_icp(icp, icp_tau, hypotheses)
-    M = icp['iterations'] if icp else 0
+    opts = step_options(hypotheses=hypotheses, seed=seed, icp=icp, icp_tau=icp_tau)
+    S, M = opts.hypotheses, 0 if opts.icp is None else _engine.Engine.icp_spec(opts.icp).iterations
     configs = checkpoint_configs(class_config)
     ids = [c for c, _ in ycb_classes(ycb_dir, class_ids)]
     if not ids:
@@ -2122,8 +2085,8 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
                for i, cl in enumerate(per_ckpt) for k in cl]
     if len(configs) > 1:
         check_weight_sets_fit(len(entries), what='weight sets (checkpoints x classes)')
-    if S > 1:
-        _driver_hypotheses(S, seed, entries)
+    for _, label, k in entries:
+        hypothesis_spread(k['dataset_info'], opts, label)
     eng, trackers = _one_pass_trackers(entries, modes[0], max(1, len(ids) * int(num_sample)) * S)
     _, producers = ycbv_producers(ycb_dir, ids, pair_tpl, eng, workers, mesh_base=base)
     variants = [(m, K) + ((i,) if len(configs) > 1 else ()) for i in range(len(configs)) for m in modes]
@@ -2142,17 +2105,24 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
                                                         with_frame=True)):
         cls = tuple(c for c, _, inside, _ in owners for _ in inside)
         n = len(cls)
-        if n not in by_n:                                  # per n: the start poses and each variant's outputs, at fixed addresses
-            by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
-                       {v: (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), torch.empty((n, 3), dtype=torch.float32, device=dev),
-                            torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((K + M, n, 4, 4), dtype=torch.float64, device=dev))
-                        for v in variants})
-            if S > 1:
-                by_n[n] += ({v: (torch.empty(n, dtype=torch.int32, device=dev), torch.empty((n, 6), dtype=torch.int32, device=dev),
-                                 torch.empty((n, S, 4, 4), dtype=torch.float64, device=dev),
-                                 torch.empty((K, n, S, 4, 4), dtype=torch.float64, device=dev)) for v in variants},
-                            torch.empty(n, dtype=torch.int64, device=dev))
-        start, outs = by_n[n][:2]
+        if n not in by_n:                                  # per n: the start poses, draw keys and each variant's outputs, at fixed addresses
+            outs = {}
+            for v in variants:
+                o = dict(out_poses=torch.empty((n, 4, 4), dtype=torch.float64, device=dev),
+                         out_trans=torch.empty((n, 3), dtype=torch.float32, device=dev),
+                         out_rot=torch.empty((n, 3), dtype=torch.float32, device=dev))
+                if S > 1:                                  # every hypothesis after each round; hypothesis 0's rounds are scored
+                    o.update(out_choice=torch.empty(n, dtype=torch.int32, device=dev), out_fit=torch.empty((n, 6), dtype=torch.int32, device=dev),
+                             out_hyp_poses=torch.empty((n, S, 4, 4), dtype=torch.float64, device=dev),
+                             out_rounds=torch.empty((K, n, S, 4, 4), dtype=torch.float64, device=dev))
+                    scored = o['out_rounds'][:, :, 0]
+                else:                                      # the network's rounds, then (with icp) the poses after each ICP iteration
+                    scored = torch.empty((K + M, n, 4, 4), dtype=torch.float64, device=dev)
+                    o.update(out_rounds=scored[:K], **({'out_icp_poses': scored[K:]} if M else {}))
+                outs[v] = (o, scored)
+            by_n[n] = (torch.empty((n, 4, 4), dtype=torch.float64, device=dev), outs,
+                       torch.empty(n, dtype=torch.int64, device=dev) if S > 1 else None)
+        start, outs, keys = by_n[n]
         start.copy_(torch.cat([r['A_in_cam'] for _, r in chunks]))
         counts.append(torch.cat([r['count'] for _, r in chunks]))
         starts.append(start.clone())
@@ -2167,24 +2137,14 @@ def recoverYcbKeyframes(ycb_dir, class_ids, class_config, num_sample=10, seed=0,
             wh, wd, widths = by_cls[cls, i]
             if v[0] == 'fp8':                              # sets without scales: calibrated on their own rows of this frame
                 eng.calibrate_fp8_tracks(rgb, depth, trk.K, start, widths, weight_ids=wh, render=dict(render, mesh_ids=wd))
-            poses, out_trans, out_rot, out_rounds = outs[v]
-            if S > 1:
-                choice, rows, hyp_poses, hyp_rounds = by_n[n][2][v]
-                keys = by_n[n][3]
+            o, scored = outs[v]
+            if keys is not None:
                 keys.copy_(torch.arange(n, dtype=torch.int64, device=dev) * (1 << 16) + hypothesis_key(f, 0, 0))
-                hypothesis_step(eng, trk, rgb, depth, start, widths, wh, wd, keys, hypothesis_groups(trackers, wh), S, seed,
-                                FIT_TAU_DEFAULT, v[0], K, dict(out_poses=poses, out_trans=out_trans, out_rot=out_rot, out_choice=choice,
-                                                               out_fit=rows, out_hyp_poses=hyp_poses, out_rounds=hyp_rounds))
-                rounds[v].append(hyp_rounds[:, :, 0].clone())
-                for acc, t in zip(picked[v], (poses, choice, hyp_poses)):
+            track_step(eng, trackers, trk, rgb, depth, start, widths, wh, wd, keys, opts, v[0], K, o)
+            rounds[v].append(scored.clone())
+            if picked is not None:
+                for acc, t in zip(picked[v], (o['out_poses'], o['out_choice'], o['out_hyp_poses'])):
                     acc.append(t.clone())
-                continue
-            # the network's rounds, then (with icp) the poses after each ICP iteration, in one (K + M, n) block
-            eng.track_render(rgb, depth, trk.K, start, widths, trk.trans_normalizer, trk.rot_normalizer, weight_ids_host=wh,
-                             weight_ids_dev=wd, precision=v[0], mode=render['mode'], image_hw=render['image_hw'], out_poses=poses,
-                             out_trans=out_trans, out_rot=out_rot, iterations=K, out_rounds=out_rounds[:K],
-                             **(dict(icp=icp, out_icp_poses=out_rounds[K:]) if icp else {}))
-            rounds[v].append(out_rounds.clone())
     out = _score_recovery(eng, trackers, ids, variants, K + M, starts, counts, row_set, row_B, rounds, _lib.PAIR_MIN_SEG, picked)
     if M:
         for res in out.values():
@@ -2704,23 +2664,23 @@ def main(argv=None):
         if args.mode not in ('ycbv_all', 'ycbineoat_all'):
             raise SystemExit('--fit needs --mode ycbv_all or ycbineoat_all; --mode %s does not check the fit' % args.mode)
         try:
-            _fit_spec(args.fit)
+            step_options(fit=args.fit)
         except ValueError as e:
             raise SystemExit('--fit %d: %s' % (args.fit, e))
     if args.hypotheses is not None:
         if args.hypotheses != 1 and args.mode not in ('ycbv_all', 'ycbineoat_all', 'ycbv_recover'):
             raise SystemExit('--hypotheses %d needs --mode ycbv_all, ycbineoat_all or ycbv_recover; --mode %s tracks one start per '
                              'track' % (args.hypotheses, args.mode))
-        if not 1 <= args.hypotheses <= _lib.MAX_HYPOTHESES:
+        try:
+            step_options(hypotheses=args.hypotheses)
+        except ValueError:
             raise SystemExit('--hypotheses %d: must be in [1, %d]' % (args.hypotheses, _lib.MAX_HYPOTHESES))
     if args.icp is not None or args.icp_tau is not None:
         if args.mode not in ('ycbv_all', 'ycbineoat_all', 'ycbv_recover'):
             raise SystemExit('--icp / --icp_tau need --mode ycbv_all, ycbineoat_all or ycbv_recover; --mode %s does not refine '
                              'with ICP' % args.mode)
-        if args.icp is not None and args.icp < 0:
-            raise SystemExit('--icp %d: must be in [0, %d]' % (args.icp, _lib.MAX_ICP_ITERATIONS))
         try:
-            _driver_icp(args.icp, args.icp_tau, args.hypotheses if args.hypotheses is not None else 1)
+            step_options(hypotheses=args.hypotheses or 1, icp=args.icp, icp_tau=args.icp_tau)
         except ValueError as e:
             raise SystemExit('--icp %s --icp_tau %s: %s' % (args.icp, args.icp_tau, e))
     if args.mode == 'ycbv_recover':

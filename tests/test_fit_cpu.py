@@ -1,7 +1,8 @@
-"""The fit check without a GPU: oracle/fit_ref.py on hand-made arrays, fit_fractions and roc_auc, the drivers' --fit parsing and
-refusals, and the FIT_FILE layout the drivers write (tracking faked)."""
+"""The fit check without a GPU: oracle/fit_ref.py on hand-made arrays, fit_fractions and roc_auc, step_options' fit and --fit
+parsing and refusals, and the FIT_FILE layout the drivers write (tracking faked)."""
 import importlib
 import os
+import pickle
 import sys
 import numpy as np
 import pytest
@@ -55,8 +56,20 @@ def test_fit_fractions_and_roc_auc(pr):
 def test_fit_argument(pr):
     for bad in (0, 1001, -1, 2.5, True, '10'):
         with pytest.raises(ValueError, match='fit'):
-            pr._driver_fit(bad)
-    assert pr._driver_fit(None) == 0 and pr._driver_fit(1000) == 1000 and pr._driver_fit(np.int64(7)) == 7
+            pr.step_options(fit=bad)
+    assert pr.step_options().fit is None and pr.step_options(fit=1000).fit == 1000 and pr.step_options(fit=np.int64(7)).fit == 7
+    # rows are kept for a given fit only; the check runs at it, or at FIT_TAU_DEFAULT when hypotheses rank the starts
+    assert pr.step_options(fit=7).tau == 7 and pr.step_options().tau is None
+    hyp = pr.step_options(hypotheses=4)
+    assert hyp.fit is None and hyp.tau == pr.FIT_TAU_DEFAULT and pr.step_options(fit=7, hypotheses=4).tau == 7
+    # the Tracker's switch: True is FIT_TAU_DEFAULT, False is off and refuses hypotheses
+    on = pr.step_options(fit=True, fit_switch=True)
+    assert on.fit == on.tau == pr.FIT_TAU_DEFAULT and pr.step_options(fit=False, fit_switch=True).tau is None
+    with pytest.raises(ValueError, match='fit must not be off'):
+        pr.step_options(fit=False, hypotheses=4, fit_switch=True)
+    with pytest.raises(ValueError, match='fit'):
+        pr.step_options(fit=np.bool_(True), fit_switch=True)
+    assert pickle.loads(pickle.dumps(hyp)) == hyp                   # the ranks of a multi-GPU run receive it pickled
 
 
 @pytest.mark.parametrize('mode', ['ycbv', 'ycbineoat', 'ycbv_recover'])
@@ -97,8 +110,8 @@ def test_fit_file_layout(pr, tmp_path):
     poses = {('bf16x3', 1): np.stack([init * (1 + 0.01 * t) for t in range(3)])}
     rows = {('bf16x3', 1): np.arange(3 * 2 * 6, dtype=np.int32).reshape(3, 2, 6)}
     dirs = lambda root: {('bf16x3', 1): {2: str(tmp_path / root / 'c2'), 5: str(tmp_path / root / 'c5')}}
-    a = pr._write_ycb_all_sequence(dirs('plain'), 48, (2, 5), init, poses)
-    b = pr._write_ycb_all_sequence_fit(dirs('fit'), 48, (2, 5), init, (poses, rows))
+    a = pr._write_ycb_all_sequence(dirs('plain'), 48, (2, 5), init, (poses, None))
+    b = pr._write_ycb_all_sequence(dirs('fit'), 48, (2, 5), init, (poses, rows))
     assert all(np.array_equal(a[k], b[k]) for k in a)
     for j, c in enumerate((2, 5)):
         sdir = tmp_path / 'fit' / ('c%d' % c) / 'seq48'
@@ -109,8 +122,12 @@ def test_fit_file_layout(pr, tmp_path):
         assert f.dtype == np.int32 and f.shape == (4, 6) and (f[0] == -1).all() and np.array_equal(f[1:], rows[('bf16x3', 1)][:, j])
     roots = {('bf16x3', 1): str(tmp_path / 'eoat')}
     one = {('bf16x3', 1): poses[('bf16x3', 1)][:, :1]}
-    out = pr._write_ycbineoat_video_fit(roots, 'bleach0', (one, {k: v[:, :1] for k, v in rows.items()}))
+    out = pr._write_ycbineoat_video(roots, 'bleach0', (one, {k: v[:, :1] for k, v in rows.items()}))
     assert np.array_equal(out[('bf16x3', 1)], one[('bf16x3', 1)][:, 0])
+    plain = pr._write_ycbineoat_video({('bf16x3', 1): str(tmp_path / 'eoat_plain')}, 'bleach0', (one, None))
+    assert np.array_equal(plain[('bf16x3', 1)], out[('bf16x3', 1)])
+    assert sorted(os.listdir(tmp_path / 'eoat_plain' / 'bleach0')) == sorted(x for x in os.listdir(tmp_path / 'eoat' / 'bleach0')
+                                                                           if x.endswith('.txt'))
     assert sorted(os.listdir(tmp_path / 'eoat')) == ['bleach0']                 # nothing at the tree's root
     f = np.load(str(tmp_path / 'eoat' / 'bleach0' / pr.FIT_FILE))
     assert np.array_equal(f, rows[('bf16x3', 1)][:, 0]) and len([x for x in os.listdir(tmp_path / 'eoat' / 'bleach0') if x.endswith('.txt')]) == 3
@@ -118,22 +135,24 @@ def test_fit_file_layout(pr, tmp_path):
 
 
 def test_drivers_pass_fit_through_the_sequence_loop(pr, tmp_path, monkeypatch):
-    """_one_pass_back with fit hands it to _track_sequences and writes[k] gets the (poses, rows) pair; without it the loop is
-    called exactly as before."""
+    """_one_pass_back hands the run's options to _track_sequences: with fit, a value whose fit is the given one, and writes[k]
+    gets the rows; without it, fit and the check off, and writes[k] gets None for rows."""
     calls = []
     monkeypatch.setattr(pr, '_one_pass_trackers', lambda entries, precision, max_batch, device=None: (None, {}))
     monkeypatch.setattr(pr, '_calibrate_borrowed', lambda *a: None)
 
-    def loop(eng, trackers, sequences, variants, depth, workers, video=None, **kw):
-        calls.append(kw)
+    def loop(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
+        calls.append(opts)
         for rgb_files, _, ids, init in sequences:
             poses = {v: np.stack([init] * len(rgb_files)) for v in variants}
-            yield (poses, {v: np.zeros((len(rgb_files), len(ids), 6), np.int32) for v in variants}) if kw else poses
+            yield poses, ({v: np.zeros((len(rgb_files), len(ids), 6), np.int32) for v in variants} if opts.fit else None)
     monkeypatch.setattr(pr, '_track_sequences', loop)
-    run = pr._OnePass(1, 'bf16x3', [('bf16x3', 1, str(tmp_path))], False, False, [{}])
+    run = lambda **step: pr._OnePass(1, 'bf16x3', [('bf16x3', 1, str(tmp_path))], False, False, [{}], pr.step_options(**step))
     seqs = [(['a', 'b'], ['a', 'b'], (0,), np.eye(4)[None])]
     got = []
-    pr._one_pass_back(run, [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w, fit=7)
-    assert calls[-1] == {'fit': 7} and isinstance(got[-1], tuple)
-    pr._one_pass_back(run, [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w)
-    assert calls[-1] == {} and isinstance(got[-1], dict)
+    pr._one_pass_back(run(fit=7), [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w)
+    assert calls[-1] == pr.step_options(fit=7) and calls[-1].fit == calls[-1].tau == 7
+    assert isinstance(got[-1], tuple) and got[-1][1] is not None
+    pr._one_pass_back(run(), [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w)
+    assert calls[-1] == pr.step_options() and calls[-1].fit is None and calls[-1].tau is None
+    assert isinstance(got[-1][0], dict) and got[-1][1] is None

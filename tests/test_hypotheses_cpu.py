@@ -166,13 +166,16 @@ def test_driver_hypothesis_keys_and_groups():
             pr.hypothesis_key(*bad)
     T = lambda t, r: type('T', (), {'dataset_info': {'max_translation': t, 'max_rotation': r}})()
     trk = {1: T(0.02, 15), 2: T(0.02, 15), 3: T(0.03, 5)}
-    assert pr.hypothesis_groups(trk, [1, 2]) == [(None, (0.02, 15.0))]
-    g = pr.hypothesis_groups(trk, [1, 3, 2])
+    opts = pr.step_options(hypotheses=4, seed=3)
+    assert (opts.hypotheses, opts.seed) == (4, 3)
+    assert pr.hypothesis_groups(trk, [1, 2], opts) == [(None, (0.02, 15.0))]
+    g = pr.hypothesis_groups(trk, [1, 3, 2], opts)
     assert [x[1] for x in g] == [(0.02, 15.0), (0.03, 5.0)] and g[0][0].tolist() == [0, 2] and g[1][0].tolist() == [1]
-    assert pr._driver_hypotheses(1, 0, []) is None
-    entries = [(1, 'class 1', {'dataset_info': {'max_translation': 0.02, 'max_rotation': 15}})]
-    assert pr._driver_hypotheses(4, 3, entries) == (4, 3)
-    with pytest.raises(ValueError, match='class 2'):
-        pr._driver_hypotheses(4, 3, entries + [(2, 'class 2', {'dataset_info': {}})])
-    with pytest.raises(ValueError):
-        pr._driver_hypotheses(33, 0, entries)
+    assert pr.hypothesis_spread({}, pr.step_options(seed=3)) is None          # S = 1 reads no spread
+    assert pr.hypothesis_spread({'max_translation': 0.02, 'max_rotation': 15}, opts, 'class 1') == (0.02, 15.0)
+    for info in ({}, {'max_translation': 0.02}, {'max_translation': 1.5, 'max_rotation': 15}, {'max_translation': 0.02, 'max_rotation': 0}):
+        with pytest.raises(ValueError, match='class 2: dataset_info max_translation / max_rotation'):
+            pr.hypothesis_spread(info, opts, 'class 2')
+    for bad in (dict(hypotheses=33), dict(hypotheses=0), dict(hypotheses=True), dict(hypotheses=2.0), dict(seed=0.5), dict(seed=True)):
+        with pytest.raises(ValueError, match='hypotheses|seed'):
+            pr.step_options(**bad)

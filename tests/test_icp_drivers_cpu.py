@@ -1,4 +1,4 @@
-"""ICP in the drivers without a GPU: _driver_icp's parsing and refusals, the CLI's --icp / --icp_tau (modes that refuse them,
+"""ICP in the drivers without a GPU: step_options' icp parsing and refusals, the CLI's --icp / --icp_tau (modes that refuse them,
 ranges, hypotheses), and that the one-pass loop and the CLI pass icp through unchanged, and not at all without it."""
 import importlib
 import numpy as np
@@ -14,11 +14,15 @@ def pr():
 
 
 def test_driver_icp(pr):
-    assert pr._driver_icp(0) is None and pr._driver_icp(None) is None
-    assert pr._driver_icp(3) == {'iterations': 3} and pr._driver_icp(2, 5) == {'iterations': 2, 'tau_mm': 5}
-    for args in ((17,), (-1,), (3, 0), (3, 1001), (0, 5), (3, None, 2)):
+    assert pr.step_options(icp=0).icp is None and pr.step_options(icp=None).icp is None
+    assert pr.step_options(icp=3).icp == 3 and pr.step_options(icp=2, icp_tau=5).icp == {'iterations': 2, 'tau_mm': 5}
+    assert pr.step_options(icp={'iterations': 2, 'min_inliers': 50}).icp == {'iterations': 2, 'min_inliers': 50}
+    for icp, tau, S in ((17, None, 1), (-1, None, 1), (3, 0, 1), (3, 1001, 1), (0, 5, 1), (3, None, 2), (2, 5, 4)):
         with pytest.raises(ValueError, match='icp'):
-            pr._driver_icp(*args)
+            pr.step_options(hypotheses=S, icp=icp, icp_tau=tau)
+    with pytest.raises(ValueError, match='ICP inside hypothesis steps is not supported'):
+        pr.step_options(hypotheses=4, icp=2)
+    assert pr.step_options(hypotheses=4, icp=0).icp is None
 
 
 @pytest.mark.parametrize('mode', ['ycbv', 'ycbineoat'])
@@ -66,17 +70,19 @@ def test_one_pass_loop_gets_icp(pr, monkeypatch, tmp_path):
     monkeypatch.setattr(pr, '_one_pass_trackers', lambda entries, precision, max_batch, device=None: (None, {}))
     monkeypatch.setattr(pr, '_calibrate_borrowed', lambda *a: None)
 
-    def loop(eng, trackers, sequences, variants, depth, workers, video=None, **kw):
-        calls.append(kw)
+    def loop(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
+        calls.append(opts)
         for rgb_files, _, ids, init in sequences:
-            yield {v: np.stack([init] * len(rgb_files)) for v in variants}
+            yield {v: np.stack([init] * len(rgb_files)) for v in variants}, None
     monkeypatch.setattr(pr, '_track_sequences', loop)
-    run = pr._OnePass(1, 'bf16x3', [('bf16x3', 1, str(tmp_path))], False, False, [{}])
+    run = lambda **step: pr._OnePass(1, 'bf16x3', [('bf16x3', 1, str(tmp_path))], False, False, [{}], pr.step_options(**step))
     seqs = [(['a', 'b'], ['a', 'b'], (0,), np.eye(4)[None])]
-    pr._one_pass_back(run, [], 1, seqs, 1, 1, None, [(lambda t: {},)], lambda w, k: w, icp={'iterations': 2})
-    assert calls[-1] == {'icp': {'iterations': 2}}
-    pr._one_pass_back(run, [], 1, seqs, 1, 1, None, [(lambda t: {},)], lambda w, k: w, icp=None)
-    assert calls[-1] == {}
+    got = []
+    pr._one_pass_back(run(icp=2, icp_tau=30), [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w)
+    assert calls[-1] == pr.step_options(icp=2, icp_tau=30) and calls[-1].icp == {'iterations': 2, 'tau_mm': 30}
+    assert calls[-1].fit is None and got[-1][1] is None
+    pr._one_pass_back(run(icp=None), [], 1, seqs, 1, 1, None, [(lambda t: got.append(t) or {},)], lambda w, k: w)
+    assert calls[-1] == pr.step_options() and calls[-1].icp is None and got[-1][1] is None
 
 
 def test_recover_table_labels_icp_rows(pr, capsys):

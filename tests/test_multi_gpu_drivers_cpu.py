@@ -165,18 +165,19 @@ def test_split_run_writes_and_returns_what_one_process_does(pr, tmp_path, monkey
     monkeypatch.setattr(torch.cuda, 'set_device', lambda d: None)
     monkeypatch.setattr(torch.cuda, 'device_count', lambda: 3)
 
-    def loop(eng, trackers, sequences, variants, depth, workers, video=None):
+    def loop(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
         for rgb_files, _, ids, init in sequences:
-            yield {v: np.stack([init * (1 + 0.01 * (t + 1)) + sum(ids) + len(str(v)) for t in range(len(rgb_files))]) for v in variants}
+            yield {v: np.stack([init * (1 + 0.01 * (t + 1)) + sum(ids) + len(str(v)) for t in range(len(rgb_files))]) for v in variants}, None
     monkeypatch.setattr(pr, '_track_sequences', loop)
 
-    def ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes):
+    def ranks(gpus, entries, precision, max_batch, sequences, variants, depth, workers, video, writes, opts):
         plan = pr.assign_ranks([len(s[0]) for s in sequences], gpus)
         results = {}
         for r in reversed(range(len(plan))):
             conn = Sent()
             borrowed = pr.borrowed_calibrations([s[2] for s in sequences], plan[r])
-            pr._rank_main(conn, r, 0, entries, precision, max_batch, sequences, plan[r], borrowed, variants, depth, workers, video, writes)
+            pr._rank_main(conn, r, 0, entries, precision, max_batch, sequences, plan[r], borrowed, variants, depth, workers, video, writes,
+                          opts)
             (kind, out, scales), = conn.msgs
             assert kind == 'ok' and sorted(out) == plan[r], conn.msgs
             results.update(out)
@@ -230,7 +231,7 @@ def test_split_run_writes_and_returns_what_one_process_does(pr, tmp_path, monkey
 def test_failing_ranks_raise_one_error_and_leave_no_process(pr):
     bad = [(['a.png'], ['a.png'], None, None)] * 3               # a weight-id tuple that is not one: each rank raises at once
     with pytest.raises(RuntimeError) as e:
-        pr._track_on_ranks(2, [], 'bf16x3', 1, bad, ('bf16x3',), 1, 1, None, [None] * 3)
+        pr._track_on_ranks(2, [], 'bf16x3', 1, bad, ('bf16x3',), 1, 1, None, [None] * 3, pr.step_options())
     msg = str(e.value)
     assert msg.startswith(('rank 0 (cuda:0) failed:', 'rank 1 (cuda:1) failed:')) and 'TypeError' in msg and 'Traceback' in msg, msg
     assert multiprocessing.active_children() == []

@@ -152,10 +152,10 @@ def fake_loop(pr, monkeypatch):
     """The drivers without a device: no trackers, and a tracking loop whose poses depend on the mode and the sequence only."""
     monkeypatch.setattr(pr, '_one_pass_trackers', lambda entries, precision, max_batch: (None, {}))
 
-    def loop(eng, trackers, sequences, variants, depth, workers, video=None):
+    def loop(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
         for k, (rgb_files, _, ids, init) in enumerate(sequences):
             yield {(m, i): np.stack([init + 0.001 * (t + 1) * (pr.PRECISIONS.index(m) + 1) + k for t in range(len(rgb_files))])
-                   for m, i in variants}
+                   for m, i in variants}, None
     monkeypatch.setattr(pr, '_track_sequences', loop)
 
 

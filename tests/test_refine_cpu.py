@@ -103,13 +103,13 @@ def fake_loop(pr, monkeypatch, seen):
     """The drivers without a device: poses that depend on the variant (mode and count) and the sequence only."""
     monkeypatch.setattr(pr, '_one_pass_trackers', lambda entries, precision, max_batch: (None, {}))
 
-    def loop(eng, trackers, sequences, variants, depth, workers, video=None):
+    def loop(eng, trackers, sequences, variants, depth, workers, video, opts, seq_index):
         seen.append(variants)
         for j, (rgb_files, _, ids, init) in enumerate(sequences):
             out = {}
             for m, k in variants:
                 out[m, k] = np.stack([init + 0.001 * (t + 1) * (pr.PRECISIONS.index(m) + 1) + 0.1 * k + j for t in range(len(rgb_files))])
-            yield out
+            yield out, None
     monkeypatch.setattr(pr, '_track_sequences', loop)
 
 
