@@ -527,6 +527,9 @@ render_kernel(RenderArgs a)
                 const double x0 = (-u.light[0]) - pos[0], x1 = (-u.light[1]) - pos[1], x2 = (-u.light[2]) - pos[2];
                 const double il = 1.0 / sqrt((x0 * x0 + x1 * x1) + x2 * x2);
                 const double d = (nrm[0] * (x0 * il) + nrm[1] * (x1 * il)) + nrm[2] * (x2 * il);
+                // fmax drops a NaN operand: a NaN Lambert term (a zero-length normal normalised to NaN) counts as 0, the fragment
+                // gets the ambient 0.65 alone.  GLSL leaves max() of a NaN undefined; NVIDIA's max instruction returns the other
+                // operand as fmax does.  oracle/se3_oracle.py (render_window) states the same rule
                 const double lightv = 0.4 * fmax(d, 0.0) + 0.65;
                 r8 = static_cast<unsigned>(rint(fmin(fmax(lightv * col[0], 0.0), 1.0) * 255.0));
                 g8 = static_cast<unsigned>(rint(fmin(fmax(lightv * col[1], 0.0), 1.0) * 255.0));

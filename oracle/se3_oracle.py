@@ -560,7 +560,9 @@ def render_window(ob2cam, K, object_width, mesh, size=176, uniforms=None):
         il = 1.0 / np.sqrt((x[0] * x[0] + x[1] * x[1]) + x[2] * x[2])
         L = [x[c] * il for c in range(3)]
         d = (nrm[0] * L[0] + nrm[1] * L[1]) + nrm[2] * L[2]
-        lightv = 0.4 * max(d, 0.0) + 0.65
+        # max(d, 0) as the GPU's max instruction and C's fmax take it: a NaN term (a zero-length normal that load_ply_mesh
+        # normalised to NaN) counts as 0, so the fragment gets the ambient 0.65 alone; Python's max would keep the NaN
+        lightv = 0.4 * (d if d > 0.0 else 0.0) + 0.65
         for c in range(3):
             rgb[j, i, c] = np.uint8(np.rint(min(max(lightv * col[c], 0.0), 1.0) * 255.0))
         d32 = np.uint32(key[j, i] >> np.uint64(32)).view(np.float32)

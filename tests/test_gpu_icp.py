@@ -151,6 +151,42 @@ def test_iterations_equal_the_oracle(eng, scene, prec, fill, mode):
         assert moved > 0
 
 
+@pytest.mark.parametrize('mode', ['vispy', 'pyrender'])
+def test_iterations_equal_the_oracle_on_a_dense_model(pkg, synth, scene, mode):
+    """test_iterations_equal_the_oracle's check with a level-6 model (81,920 faces): the triangle ids ICP reads come from
+    sub-pixel triangles, many per pixel, so they test the rasteriser's choice among them.  2 tracks, 2 iterations."""
+    M, n, DENSE = 2, 2, 5
+    mesh = synth.mesh(6, seed=6)
+    e = pkg.Engine(max_batch=8)
+    try:
+        mean, std = synth.default_mean_std()
+        e.load_state_dict(synth.make_state_dict(0), DENSE); e.set_stats(mean, std, DENSE); e.set_mesh(mesh, DENSE)
+        c = Case(e, scene, n, ids=DENSE)
+        rounds, slots = _nan(e, 1, n, 4, 4), _nan(e, M, n, 4, 4)
+        P, _, _, stats = _step(e, c, {'iterations': M, 'tau_mm': 20, 'min_inliers': 100}, mode=mode, out_rounds=rounds, out_icp_poses=slots)
+        torch.cuda.synchronize()
+        pre, slots, stats, P = rounds[0].cpu().numpy(), slots.cpu().numpy(), stats.cpu().numpy(), P.cpu().numpy()
+    finally:
+        e.close()
+    assert np.array_equal(slots[-1], P)
+    moved = 0
+    for i in range(n):
+        start = pre[i]
+        for m in range(M):
+            want, st, terms = icp_ref.iterate(start, K, WIDTH, mesh, scene['D'], 20, 100, mode, *HW)
+            got = slots[m, i]
+            if want is start:
+                assert np.array_equal(got, start), (i, m)
+            else:
+                moved += 1
+                assert np.abs(got[:3, 3] - want[:3, 3]).max() <= 1e-9, (i, m)
+                assert np.abs(got[:3, :3] - want[:3, :3]).max() <= 1e-9, (i, m)
+            if m == M - 1:
+                assert stats[i, 0] == st[0] == len(terms['e']), i
+            start = got
+    assert moved > 0
+
+
 @pytest.mark.parametrize('n', [1, 8])
 def test_zero_head_converges(synth, eng, scene, n):
     c = Case(eng, scene, n, ids=ZERO)

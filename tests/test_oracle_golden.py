@@ -189,7 +189,8 @@ def test_fill_depth_oracle_vs_reference(golden_dir):
 
 def _ray_cast_depth(mesh, pose, K, u, S=176):
     """Pinhole ray through every pixel centre of the crop window against the posed triangles (Moeller-Trumbore, float64);
-    -> camera-space depth (S, S), inf where nothing is hit between the near (0.1 m) and far (2 m) planes."""
+    -> camera-space depth (S, S), inf where nothing is hit between the near (0.1 m) and far (2 m) planes.  A triangle wholly in
+    front of the eye is tested against the rays of its projected box (one pixel of margin) only; any other against all rays."""
     cols = u['left'] + (np.arange(S) + 0.5) * (u['right'] - u['left']) / S
     # the window rows live in the y-flipped image v' = 2*cy - v (compute_bbox with scale -1000); array row 0 is v' = bottom
     vflip = u['bottom'] - (np.arange(S) + 0.5) * (u['bottom'] - u['top']) / S
@@ -197,20 +198,33 @@ def _ray_cast_depth(mesh, pose, K, u, S=176):
     dx = (cols - K[0, 2]) / K[0, 0]; dy = (rows - K[1, 2]) / K[1, 1]
     D = np.stack(np.broadcast_arrays(dx[None, :], dy[:, None], np.ones((S, S))), -1).reshape(-1, 3)     # ray directions, origin 0
     P = mesh['pos'].astype(np.float64) @ pose[:3, :3].T + pose[:3, 3]
+    with np.errstate(divide='ignore', invalid='ignore'):            # window column / row of each vertex (valid where z > 0)
+        pi = (K[0, 0] * P[:, 0] / P[:, 2] + K[0, 2] - u['left']) * S / (u['right'] - u['left']) - 0.5
+        pj = (K[1, 1] * P[:, 1] / P[:, 2] + K[1, 2] - 2 * K[1, 2] + u['bottom']) * S / (u['bottom'] - u['top']) - 0.5
+    everything = np.arange(S * S)
     best = np.full(len(D), np.inf)
     for f in mesh['faces']:
+        if (P[f, 2] > 1e-3).all():
+            ia, ib = max(0, int(np.floor(pi[f].min())) - 1), min(S - 1, int(np.ceil(pi[f].max())) + 1)
+            ja, jb = max(0, int(np.floor(pj[f].min())) - 1), min(S - 1, int(np.ceil(pj[f].max())) + 1)
+            if ia > ib or ja > jb:
+                continue
+            sel = (np.arange(ja, jb + 1)[:, None] * S + np.arange(ia, ib + 1)[None, :]).ravel()
+        else:
+            sel = everything
+        Ds = D[sel]
         v0, v1, v2 = P[f[0]], P[f[1]], P[f[2]]
         e1, e2 = v1 - v0, v2 - v0
-        pv = np.cross(D, e2); det = pv @ e1
+        pv = np.cross(Ds, e2); det = pv @ e1
         with np.errstate(divide='ignore', invalid='ignore'):
             inv = 1.0 / det
             tv = -v0
             uu = (pv @ tv) * inv
             qv = np.cross(tv, e1)
-            vv = (D @ qv) * inv
+            vv = (Ds @ qv) * inv
             t = (qv @ e2) * inv
         hit = (np.abs(det) > 1e-15) & (uu >= 0) & (vv >= 0) & (uu + vv <= 1) & (t > 0.1) & (t < 2.0)
-        best = np.where(hit & (t < best), t, best)
+        best[sel] = np.where(hit & (t < best[sel]), t, best[sel])
     return best.reshape(S, S)                                       # direction z-component is 1: t is the camera-space depth
 
 
@@ -227,13 +241,35 @@ def _assert_same_surface(dep, z, min_pixels):
 def test_render_oracle_vs_ray_casting(synth):
     """Independent geometric cross-check of the rasterisation restatement (no GL here): cast a pinhole ray through every pixel
     centre of the crop window and intersect it with the posed triangles.  The rasteriser must see the same surface: identical
-    coverage away from silhouette edges, depth within 1 mm (uint16 truncation + float32 z-buffer)."""
-    mesh = synth.mesh(1, seed=2)                                   # 80 faces
+    coverage away from silhouette edges, depth within 1 mm (uint16 truncation + float32 z-buffer).  An 80-face model with large
+    triangles, and a 20,480-face one (level 5) whose triangles are mostly below a pixel, as real models' are."""
     K = synth.CAMERA_K
     pose = synth.raw_poses(3, seed=21)[2]
     u = O.render_uniforms(pose, K, 200.0)
-    rgb, dep = O.render_window(pose, K, 200.0, mesh)
-    _assert_same_surface(dep, _ray_cast_depth(mesh, pose, K, u), 3000)
+    for level in (1, 5):
+        mesh = synth.mesh(level, seed=2)
+        rgb, dep = O.render_window(pose, K, 200.0, mesh)
+        _assert_same_surface(dep, _ray_cast_depth(mesh, pose, K, u), 3000)
+
+
+def test_render_oracle_nan_normals_count_as_zero_lambert(synth):
+    """A NaN vertex normal (what load_ply_mesh makes of a stored (0, 0, 0)) gives a NaN Lambert term, which counts as 0 as the
+    GPU's max instruction and fmax take it: all normals NaN draws exactly what all normals zero draws (n.l = 0), and a model
+    with some NaN normals casts no NaN to uint8 and shows no black fragment."""
+    import warnings
+    mesh = synth.mesh(2, seed=0)
+    pose = synth.raw_poses(3, seed=21)[2]
+    K = synth.CAMERA_K
+    nan_all, zero_all, some = dict(mesh), dict(mesh), dict(mesh)
+    nan_all['nrm'] = np.full_like(mesh['nrm'], np.nan); zero_all['nrm'] = np.zeros_like(mesh['nrm'])
+    some['nrm'] = mesh['nrm'].copy(); some['nrm'][::7] = np.nan
+    with warnings.catch_warnings():
+        warnings.simplefilter('error')                                 # an invalid cast would warn
+        a, b, c = (O.render_window(pose, K, 200.0, m) for m in (nan_all, zero_all, some))
+        plain = O.render_window(pose, K, 200.0, mesh)
+    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and np.array_equal(c[1], plain[1])
+    fg = c[1] > 0
+    assert fg.sum() > 2000 and (c[0][fg].max(-1) > 0).all() and (c[0] != plain[0]).any(-1).sum() > 100
 
 
 def _long_mesh(synth, level, seed, stretch=24.0):
