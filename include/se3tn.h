@@ -631,6 +631,70 @@ int se3tn_init_poses(se3tn_ctx* ctx, const uint16_t* frame_depth, const uint8_t*
                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
                      double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream);
 
+/* ---- re-initialisation: a start from the mask replaces a track the fit check finds lost ------------------------------ */
+
+/* Three calls connect the fit check (se3tn_track_opts.fit_tau_mm) to se3tn_init_poses.  Engine.reinit runs them after a
+ * tracking step; oracle/reinit_ref.py restates the rules in numpy.
+ *   Lost.     Track i is below in a step when 1000 inlier < below_permille model, compared as int64; a track with model = 0 is
+ *             below.  Each track has an int32 streak that persists across calls (the caller keeps it, zeroed at the start):
+ *             streak + 1 when below, 0 otherwise.  A track is lost when its streak reaches `after`.
+ *   Restart.  The lost tracks of a frame, in ascending track order, go through one se3tn_init_poses call, each with its own
+ *             label, mesh and width, on the depth the step saw (the filled frame when the step fills).
+ *   Accept.   A start replaces the tracked pose only when its init status is 0 and its fit row (se3tn_fit_poses: the step's
+ *             fit check at the start) ranks strictly above the tracked pose's row, in the hypothesis choice's order: the
+ *             higher inlier / model, then the lower residual / inlier, as int64 cross products (model = 0 or inlier = 0
+ *             ranks last; a tie is not above).  The pose and the fit row are then both the start's.
+ *   After an attempt the streak is 0 whatever the outcome, so a track is retried at most once every `after` frames.
+ * Event codes per track and step (int32): 0 not below; 1 below, no attempt (the streak is short of `after`, or the track is
+ * lost but no mask was given); 2 restarted, the pose is the start; 3 no start (init status != 0); 4 start rejected (it fits no
+ * better than the tracked pose).
+ * The defaults of Engine.reinit_spec / Tracker(reinit=) (below 0.5, after 3) are guesses, not tuned: `predict --fit --score`
+ * reports how well the inlier fraction separates lost from kept tracks on a data set, which is what to choose them by. */
+#define SE3TN_REINIT_NONE 0
+#define SE3TN_REINIT_BELOW 1
+#define SE3TN_REINIT_RESTARTED 2
+#define SE3TN_REINIT_NO_START 3
+#define SE3TN_REINIT_REJECTED 4
+typedef struct se3tn_reinit_opts {
+    int32_t below_permille, after;                 /* [1, 1000], [1, 1000]                                                   */
+    int32_t reserved[2];                           /* 0                                                                      */
+} se3tn_reinit_opts;                               /* 16 bytes, no padding                                                   */
+
+/* The loss rule over one step's fit rows, one launch of one CTA: fit_rows int32 (n, SE3TN_FIT_COLS), streak int32 (n) in /
+ * out, out_event int32 (n) (0 or 1 for every track), out_lost int32 (n + 1): the count of lost tracks, then their indices in
+ * ascending order (a block scan: the order never depends on scheduling); entries past the count are not written.  All device.
+ * Refused with SE3TN_ERR_INVALID, the field named and nothing queued: NULL arguments, n outside [0, max_batch], an option out
+ * of range, reserved != 0, and an output overlapping fit_rows or another output.  se3tn_last_launch_count: 1. */
+int se3tn_lost_tracks(se3tn_ctx* ctx, const int32_t* fit_rows, int n, const se3tn_reinit_opts* opts, int32_t* streak,
+                      int32_t* out_event, int32_t* out_lost, void* stream);
+
+/* The fit check of a tracking step (se3tn_track_opts.fit_tau_mm) at n given poses: each model is drawn (depth only, mesh
+ * weight_ids[i], render_mode / render_H / render_W as se3tn_track_render) and compared with frame_depth in the crop window of
+ * its pose.  Its rows equal, as exact integers, those a tracking step's fit check gives at the same poses on the same frame
+ * with the same tau, mode, meshes and widths.  A pose with a non-finite entry draws nothing: its row is all 0.
+ *   frame_depth uint16 (H, W) mm, poses double (n, 16), object_width double (n) mm, out_rows int32 (n, SE3TN_FIT_COLS): device;
+ *   K HOST fx fy cx cy; weight_ids_host / weight_ids_dev int32 (n), both or neither (mesh 0); fit_tau_mm in [1, 1000].
+ * Plain launches, no CUDA graph.  The rendered depth goes to scratch of the call's own (n x 176 x 176 x 2 bytes), which no
+ * tracking step reads or writes: a call needing more than it holds synchronises `stream` and grows it.  The fit check's
+ * rows (se3tn_fit_rows) and the step's input A are untouched.  se3tn_last_launch_count: 3 (render 2, fit 1).  Refused with
+ * SE3TN_ERR_INVALID, nothing queued: NULL arguments, n outside [0, max_batch], tau out of range, a bad render mode, out_rows
+ * overlapping an input; an id without a mesh is SE3TN_ERR_STATE. */
+int se3tn_fit_poses(se3tn_ctx* ctx, const uint16_t* frame_depth, int H, int W, const double* K, const double* poses,
+                    const double* object_width, int render_mode, int render_H, int render_W, const int32_t* weight_ids_host,
+                    const int32_t* weight_ids_dev, int n, int fit_tau_mm, int32_t* out_rows, void* stream);
+
+/* The accept rule for the starts of m lost tracks, one launch: start k belongs to track lost_idx[k] and comes with its init
+ * row (init_rows int32 (m, SE3TN_INIT_COLS), se3tn_init_poses' out_rows) and its fit row (start_fit int32 (m, SE3TN_FIT_COLS),
+ * se3tn_fit_poses at starts double (m, 16)).  In place over the n tracks: poses double (n, 16) and fit_rows int32 (n,
+ * SE3TN_FIT_COLS) take the start's pose and row on a restart; streak int32 (n) is 0 for each of the m tracks; out_event int32
+ * (n) is 2, 3 or 4 for each of them.  Tracks not in the list are not touched.  All device except lost_idx_host, a host copy
+ * of lost_idx_dev that the checks read (as se3tn_lost_tracks' out_lost gives it after a copy back).  Refused with
+ * SE3TN_ERR_INVALID, nothing queued: NULL arguments, n outside [0, max_batch], m outside [0, n], a lost index outside [0, n)
+ * or repeated, and an in-place output overlapping an input or another output.  se3tn_last_launch_count: 1 (0 when m = 0). */
+int se3tn_accept_starts(se3tn_ctx* ctx, const int32_t* lost_idx_host, const int32_t* lost_idx_dev, int m, const double* starts,
+                        const int32_t* init_rows, const int32_t* start_fit, int n, double* poses, int32_t* fit_rows, int32_t* streak,
+                        int32_t* out_event, void* stream);
+
 /* ---- checkpoint validation: the loss of ready-made training pairs ---------------------------------------------------- */
 
 /* Problem.validate's per-batch work (reference problems.py:106-132) as ONE step: for n pairs as TrackDataset.__getitem__ reads

@@ -25,6 +25,7 @@ ICP_COLS = 4
 INIT_COLS = 8
 INIT_STATS = 6
 MAX_INIT_KEEP = 32
+REINIT_NONE, REINIT_BELOW, REINIT_RESTARTED, REINIT_NO_START, REINIT_REJECTED = 0, 1, 2, 3, 4
 
 _vp, _i, _d, _sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
 
@@ -63,6 +64,9 @@ SIGNATURES = {
                                      _vp]),
     'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     'se3tn_init_poses': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_lost_tracks': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_fit_poses': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
+    'se3tn_accept_starts': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_fill_depth': (_i, [_vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     'se3tn_fill_depth_ex': (_i, [_vp, _vp, _i, _i, _d, _i, _i, _vp, _vp, _vp]),
     'se3tn_fit_rows': (_i, [_vp, C.POINTER(_vp)]),
@@ -135,6 +139,11 @@ class InitArrays(C.Structure):
     """se3tn_init_arrays (include/se3tn.h): device pointers, NULL where not wanted."""
     _fields_ = [('stats', _vp), ('t0', _vp), ('cand_rows', _vp), ('kept_rows', _vp), ('kept_poses', _vp), ('icp_poses', _vp),
                 ('icp_rows', _vp), ('icp_stats', _vp)]
+
+
+class ReinitOpts(C.Structure):
+    """se3tn_reinit_opts (include/se3tn.h)."""
+    _fields_ = [('below_permille', C.c_int32), ('after', C.c_int32), ('reserved', C.c_int32 * 2)]
 
 
 _lib = None

@@ -16,7 +16,7 @@ STAMP = os.path.join(HERE, 'libse3tn.stamp')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-I' + os.path.join(ROOT, 'include')]
 # aux_kernels.cu restates numpy/cv2 float arithmetic: no FMA contraction there.
-SOURCES = [('conv_wgmma.cu', []), ('conv_direct.cu', []), ('aux_kernels.cu', ['-fmad=false']), ('metrics.cu', ['-fmad=false']), ('render.cu', ['-fmad=false']), ('depth_fill.cu', ['-fmad=false']), ('overlay.cu', ['-fmad=false']), ('augment.cu', ['-fmad=false']), ('fit.cu', ['-fmad=false']), ('hypotheses.cu', ['-fmad=false']), ('icp.cu', ['-fmad=false']), ('init.cu', ['-fmad=false']), ('se3tn.cu', [])]
+SOURCES = [('conv_wgmma.cu', []), ('conv_direct.cu', []), ('aux_kernels.cu', ['-fmad=false']), ('metrics.cu', ['-fmad=false']), ('render.cu', ['-fmad=false']), ('depth_fill.cu', ['-fmad=false']), ('overlay.cu', ['-fmad=false']), ('augment.cu', ['-fmad=false']), ('fit.cu', ['-fmad=false']), ('hypotheses.cu', ['-fmad=false']), ('icp.cu', ['-fmad=false']), ('init.cu', ['-fmad=false']), ('reinit.cu', []), ('se3tn.cu', [])]
 
 
 def _nvcc():

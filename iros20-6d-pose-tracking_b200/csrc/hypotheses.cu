@@ -19,6 +19,7 @@
 // keeps hypothesis 0, unless hypothesis 0's model = 0 (nothing drawn in its window): then the first h >= 1 with model > 0 wins.
 #include "hypotheses.h"
 #include "fit.h"
+#include "fit_rank.cuh"
 #include "launch.h"
 #include "philox.cuh"
 #include <cfloat>
@@ -109,16 +110,6 @@ __global__ void __launch_bounds__(kHypThreads) hypotheses_kernel(const HypArgs a
     }
 }
 
-// true when fit row x ranks strictly above row y
-__device__ bool better(const int32_t* x, const int32_t* y) {
-    const long long xm = x[0], ym = y[0], xi = x[2], yi = y[2], xr = x[5], yr = y[5];
-    if ((xm == 0) != (ym == 0)) return ym == 0;
-    if (xm != 0 && xi * ym != yi * xm) return xi * ym > yi * xm;
-    if ((xi == 0) != (yi == 0)) return yi == 0;
-    if (xi != 0 && xr * yi != yr * xi) return xr * yi < yr * xi;
-    return false;
-}
-
 __global__ void __launch_bounds__(kHypThreads) select_kernel(const SelectArgs a)
 {
     const int i = blockIdx.x * kHypThreads + threadIdx.x;
@@ -126,7 +117,7 @@ __global__ void __launch_bounds__(kHypThreads) select_kernel(const SelectArgs a)
     const size_t base = static_cast<size_t>(i) * a.S;
     int best = 0;
     for (int h = 1; h < a.S; ++h)
-        if (better(a.rows + (base + h) * kFitCols, a.rows + (base + best) * kFitCols)) best = h;
+        if (fit_better(a.rows + (base + h) * kFitCols, a.rows + (base + best) * kFitCols)) best = h;
     const size_t r = base + best;
     for (int k = 0; k < 16; ++k) a.poses_out[16 * static_cast<size_t>(i) + k] = a.poses[16 * r + k];
     for (int k = 0; k < kFitCols; ++k) a.fit_out[kFitCols * static_cast<size_t>(i) + k] = a.rows[kFitCols * r + k];

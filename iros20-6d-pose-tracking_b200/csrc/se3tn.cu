@@ -13,6 +13,7 @@
 #include "icp.h"
 #include "hypotheses.h"
 #include "init.h"
+#include "reinit.h"
 #include "storage.cuh"
 
 #include <algorithm>
@@ -298,6 +299,8 @@ struct se3tn_ctx {
     DevBuf<uint8_t> icp; size_t icp_bytes = 0;
     // se3tn_init_poses' scratch (InitLayout); grows on demand after a stream synchronisation, never captured in a graph
     DevBuf<uint8_t> init; size_t init_bytes = 0;
+    // se3tn_fit_poses' rendered depth (n x 176 x 176 uint16); grows on demand after a stream synchronisation, never captured
+    DevBuf<uint8_t> fit_poses; size_t fit_poses_bytes = 0;
     DevBuf<float> pool_part;        // [max_batch][kPoolSlices][1024] column sums from the last conv's epilogue
     DevBuf<unsigned> sched;          // trunk kernel: next-unit counter + done[6][max_batch] + split-K slice counters; zero between steps (head_pooled_kernel clears it)
     DevBuf<float> partial;           // split-K scratch of the latency mode (n <= 4): trunk_partial_floats()
@@ -2728,6 +2731,119 @@ int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* s
     // 6. the best of each object's K
     CU_TRY(c, launch_choose(ca, s));
     ++c->launches;
+    return SE3TN_OK;
+}
+
+}  // extern "C"
+
+namespace {
+static_assert(sizeof(se3tn_reinit_opts) == 16, "se3tn_reinit_opts is 16 bytes without padding: _lib.ReinitOpts mirrors it");
+static_assert(kReinitNone == SE3TN_REINIT_NONE && kReinitBelow == SE3TN_REINIT_BELOW && kReinitRestarted == SE3TN_REINIT_RESTARTED &&
+              kReinitNoStart == SE3TN_REINIT_NO_START && kReinitRejected == SE3TN_REINIT_REJECTED, "include/se3tn.h");
+}  // namespace
+
+extern "C" {
+
+int se3tn_lost_tracks(se3tn_ctx* c, const int32_t* fit_rows, int n, const se3tn_reinit_opts* opts, int32_t* streak,
+                      int32_t* out_event, int32_t* out_lost, void* stream) {
+    const std::string f("se3tn_lost_tracks");
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!fit_rows || !opts || !streak || !out_event || !out_lost) return fail(c, SE3TN_ERR_INVALID, f + ": null argument");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    const struct { int v; const char* name; } fields[] = {{opts->below_permille, "below_permille"}, {opts->after, "after"}};
+    for (const auto& x : fields)
+        if (x.v < 1 || x.v > 1000)
+            return fail(c, SE3TN_ERR_INVALID, f + ": opts->" + x.name + " is " + std::to_string(x.v) + ", not in [1, 1000]");
+    if (opts->reserved[0] || opts->reserved[1]) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
+    const size_t nn = static_cast<size_t>(n);
+    const int rc = check_disjoint(c, f.c_str(), {{streak, nn * 4}, {out_event, nn * 4}, {out_lost, (nn + 1) * 4}},
+                                  {{fit_rows, nn * 4 * kFitCols}}, "the outputs must not overlap fit_rows");
+    if (rc) return rc;
+    DeviceGuard guard(c->device);
+    LostArgs a{};
+    a.fit_rows = fit_rows; a.n = n; a.below_permille = opts->below_permille; a.after = opts->after;
+    a.streak = streak; a.event = out_event; a.lost = out_lost;
+    CU_TRY(c, launch_lost(a, static_cast<cudaStream_t>(stream)));
+    c->launches = 1;
+    return SE3TN_OK;
+}
+
+int se3tn_fit_poses(se3tn_ctx* c, const uint16_t* frame_depth, int H, int W, const double* K, const double* poses,
+                    const double* object_width, int render_mode, int render_H, int render_W, const int32_t* weight_ids_host,
+                    const int32_t* weight_ids_dev, int n, int fit_tau_mm, int32_t* out_rows, void* stream) {
+    const char* fn = "se3tn_fit_poses";
+    const std::string f(fn);
+    if (!c) return SE3TN_ERR_INVALID;
+    if (!frame_depth || !K || !poses || !object_width || !out_rows || H <= 0 || W <= 0)
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    if (fit_tau_mm < 1 || fit_tau_mm > 1000)
+        return fail(c, SE3TN_ERR_INVALID, f + ": fit_tau_mm is " + std::to_string(fit_tau_mm) + ", not in [1, 1000]");
+    RenderSpec r;
+    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
+    if (rc) return rc;
+    if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
+        return fail(c, SE3TN_ERR_INVALID, f + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
+    for (int i = 0; i < n; ++i) {
+        const int id = weight_ids_host ? weight_ids_host[i] : 0;
+        if (!c->meshes.count(id))
+            return fail(c, SE3TN_ERR_STATE, f + ": id " + std::to_string(id) + " (pose " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
+    }
+    const size_t nn = static_cast<size_t>(n);
+    rc = check_disjoint(c, fn, {{out_rows, nn * 4 * kFitCols}},
+                        {{frame_depth, static_cast<size_t>(H) * W * 2}, {poses, nn * 128}, {object_width, nn * 8}, {weight_ids_dev, nn * 4}},
+                        "out_rows must not overlap an input");
+    if (rc || n == 0) return rc;
+    DeviceGuard guard(c->device);
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if ((rc = sync_meshes(c, s))) return rc;
+    const size_t bytes = nn * kImg * kImg * sizeof(uint16_t);
+    if (bytes > c->fit_poses_bytes) {                    // the old block may still be read by a queued call
+        CU_TRY(c, cudaStreamSynchronize(s));
+        CU_TRY(c, grow(c->fit_poses, c->fit_poses_bytes, bytes));
+    }
+    uint16_t* depth = reinterpret_cast<uint16_t*>(c->fit_poses.get());
+    // the step's fit check (step_launches), as plain launches at the given poses
+    const RenderArgs ra = render_args(c, K, poses, object_width, weight_ids_dev, r.mode, r.H, r.W, nullptr, depth);
+    CU_TRY(c, launch_render(ra, n, s, false));
+    FitArgs fa;
+    fa.poses = poses; fa.object_width = object_width; fa.fx = K[0]; fa.fy = K[1]; fa.cx = K[2]; fa.cy = K[3];
+    fa.frame_depth = frame_depth; fa.H = H; fa.W = W; fa.rendered = depth; fa.tau = fit_tau_mm; fa.rows = out_rows;
+    CU_TRY(c, launch_fit(fa, n, s));
+    c->launches = 3;
+    return SE3TN_OK;
+}
+
+int se3tn_accept_starts(se3tn_ctx* c, const int32_t* lost_idx_host, const int32_t* lost_idx_dev, int m, const double* starts,
+                        const int32_t* init_rows, const int32_t* start_fit, int n, double* poses, int32_t* fit_rows, int32_t* streak,
+                        int32_t* out_event, void* stream) {
+    const std::string f("se3tn_accept_starts");
+    if (!c) return SE3TN_ERR_INVALID;
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    if (m < 0 || m > n) return fail(c, SE3TN_ERR_INVALID, f + ": m is " + std::to_string(m) + ", not in [0, n]");
+    if (m > 0 && (!lost_idx_host || !lost_idx_dev || !starts || !init_rows || !start_fit || !poses || !fit_rows || !streak || !out_event))
+        return fail(c, SE3TN_ERR_INVALID, f + ": null argument");
+    std::vector<char> seen(static_cast<size_t>(n), 0);
+    for (int k = 0; k < m; ++k) {
+        const int i = lost_idx_host[k];
+        if (i < 0 || i >= n)
+            return fail(c, SE3TN_ERR_INVALID, f + ": lost_idx[" + std::to_string(k) + "] is " + std::to_string(i) + ", not in [0, n)");
+        if (seen[i]) return fail(c, SE3TN_ERR_INVALID, f + ": lost_idx[" + std::to_string(k) + "] repeats track " + std::to_string(i));
+        seen[i] = 1;
+    }
+    const size_t nn = static_cast<size_t>(n), mm = static_cast<size_t>(m);
+    const int rc = check_disjoint(c, f.c_str(), {{poses, nn * 128}, {fit_rows, nn * 4 * kFitCols}, {streak, nn * 4}, {out_event, nn * 4}},
+                                  {{lost_idx_dev, mm * 4}, {starts, mm * 128}, {init_rows, mm * 4 * kInitCols}, {start_fit, mm * 4 * kFitCols}},
+                                  "the in-place outputs must not overlap an input");
+    if (rc) return rc;
+    c->launches = 0;
+    if (m == 0) return SE3TN_OK;
+    DeviceGuard guard(c->device);
+    AcceptArgs a{};
+    a.lost_idx = lost_idx_dev; a.m = m; a.starts = starts; a.init_rows = init_rows; a.start_fit = start_fit;
+    a.poses = poses; a.fit_rows = fit_rows; a.streak = streak; a.event = out_event;
+    CU_TRY(c, launch_accept(a, static_cast<cudaStream_t>(stream)));
+    c->launches = 1;
     return SE3TN_OK;
 }
 

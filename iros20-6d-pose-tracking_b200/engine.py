@@ -5,6 +5,7 @@ torch.distributed -- all arithmetic happens inside libse3tn.so.  There is no CPU
 fallback: without a CUDA device and the built library every call raises.
 """
 import ctypes as C
+import decimal
 import math
 import numpy as np
 import torch
@@ -560,6 +561,127 @@ class Engine:
                                              _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
                                              _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
         return out['poses'], out['rows']
+
+    # ------------------------------------------------------------------ re-initialisation of lost tracks
+    # reinit_spec's defaults: guesses, not tuned -- `predict --fit --score` shows how well the inlier fraction separates lost
+    # from kept tracks on a data set, which is what to choose them by
+    REINIT_DEFAULTS = dict(below=0.5, after=3)
+
+    @staticmethod
+    def reinit_spec(below=0.5, after=3):
+        """se3tn_reinit_opts: below, the inlier fraction under which a track counts as below, in (0, 1] and exact in three
+        decimals (it is passed as permille: 0.5 -> 500; 0.1234 is a ValueError); after, the frames in a row below that make a
+        track lost, an integer in [1, 1000]."""
+        if isinstance(below, (bool, np.bool_)) or not isinstance(below, (int, float, np.integer, np.floating)):
+            raise ValueError('reinit below must be a number in (0, 1], not %r' % (below,))
+        try:
+            permille = decimal.Decimal(repr(float(below))) * 1000
+        except decimal.InvalidOperation:
+            raise ValueError('reinit below must be a number in (0, 1], not %r' % (below,)) from None
+        if not permille.is_finite() or permille != permille.to_integral_value() or not 1 <= permille <= 1000:
+            raise ValueError('reinit below must be in (0, 1] with at most three decimals (a whole permille), not %r' % (below,))
+        if isinstance(after, (bool, np.bool_)) or not isinstance(after, (int, np.integer)) or not 1 <= after <= 1000:
+            raise ValueError('reinit after must be an integer in [1, 1000], not %r' % (after,))
+        return _lib.ReinitOpts(below_permille=int(permille), after=int(after))
+
+    def lost_tracks(self, fit_rows, streak, below=0.5, after=3, out_event=None, out_lost=None):
+        """The loss rule over one step's fit rows (se3tn_lost_tracks), queued on the current stream: fit_rows int32 (n, 6) and
+        streak int32 (n) CUDA tensors, the streak updated in place.  -> (event int32 (n): 1 below, 0 not; lost int32 (n + 1):
+        the count of lost tracks, then their indices in ascending order)."""
+        opts = self.reinit_spec(below, after)
+        n = int(fit_rows.shape[0])
+        self._check_dev('fit_rows', fit_rows, torch.int32, (n, _lib.FIT_COLS))
+        self._check_dev('streak', streak, torch.int32, (n,))
+        out_event = torch.empty(n, dtype=torch.int32, device=self.device) if out_event is None else out_event
+        out_lost = torch.empty(n + 1, dtype=torch.int32, device=self.device) if out_lost is None else out_lost
+        self._check_dev('out_event', out_event, torch.int32, (n,))
+        self._check_dev('out_lost', out_lost, torch.int32, (n + 1,))
+        _lib.check(self.lib.se3tn_lost_tracks(self._ctx, _ptr(fit_rows), n, C.byref(opts), _ptr(streak), _ptr(out_event),
+                                              _ptr(out_lost), _stream(self.device)), self._ctx)
+        return out_event, out_lost
+
+    def fit_poses(self, frame_depth, K, poses, object_width, fit, weight_ids=None, mode='vispy', image_hw=None, out=None):
+        """The tracking step's fit check at given poses (se3tn_fit_poses), queued on the current stream: frame_depth uint16
+        (H,W) mm, poses float64 (n,4,4), object_width float64 (n) CUDA tensors; fit: tau in mm (fit_spec, required); weight_ids
+        int32 (n) host array or None (mesh 0); mode / image_hw as in render().  -> int32 (n, 6) rows (model, observed, inlier,
+        front, behind, residual), exactly those of a track_render step with the same fit at these poses on this frame."""
+        tau = self.fit_spec(fit)
+        if not tau:
+            raise ValueError('fit_poses: fit must be a tau in mm, not %r' % (fit,))
+        n = int(poses.shape[0])
+        H, W = frame_depth.shape
+        self._check_dev('frame_depth', frame_depth, torch.uint16, (H, W))
+        self._check_dev('poses', poses, torch.float64, (n, 4, 4))
+        self._check_dev('object_width', object_width, torch.float64, (n,))
+        wh = self._host_ids('fit_poses', weight_ids, n)
+        wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
+        out = torch.empty(n, _lib.FIT_COLS, dtype=torch.int32, device=self.device) if out is None else out
+        self._check_dev('out', out, torch.int32, (n, _lib.FIT_COLS))
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        _lib.check(self.lib.se3tn_fit_poses(self._ctx, _ptr(frame_depth), int(H), int(W), _hptr(self._k4(K)), _ptr(poses),
+                                            _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, int(tau), _ptr(out),
+                                            _stream(self.device)), self._ctx)
+        return out
+
+    def accept_starts(self, lost, starts, init_rows, start_fit, poses, fit_rows, streak, event):
+        """The accept rule for the starts of the lost tracks (se3tn_accept_starts), queued on the current stream: lost int32 (m)
+        host array of track indices; starts float64 (m,4,4), init_rows int32 (m, INIT_COLS), start_fit int32 (m, 6) CUDA
+        tensors.  poses float64 (n,4,4), fit_rows int32 (n,6), streak and event int32 (n) CUDA tensors are updated in place:
+        a restarted track takes its start's pose and row (event 2), a start without init status 0 is event 3, one that fits no
+        better event 4; the m streaks go back to 0."""
+        idx = np.ascontiguousarray(lost, dtype=np.int32).reshape(-1)
+        m, n = int(idx.shape[0]), int(poses.shape[0])
+        for name, t, dt, shape in (('starts', starts, torch.float64, (m, 4, 4)), ('init_rows', init_rows, torch.int32, (m, _lib.INIT_COLS)),
+                                   ('start_fit', start_fit, torch.int32, (m, _lib.FIT_COLS)), ('poses', poses, torch.float64, (n, 4, 4)),
+                                   ('fit_rows', fit_rows, torch.int32, (n, _lib.FIT_COLS)), ('streak', streak, torch.int32, (n,)),
+                                   ('event', event, torch.int32, (n,))):
+            self._check_dev(name, t, dt, shape)
+        idx_d = torch.from_numpy(idx).to(self.device)
+        _lib.check(self.lib.se3tn_accept_starts(self._ctx, _hptr(idx), _ptr(idx_d), m, _ptr(starts), _ptr(init_rows), _ptr(start_fit),
+                                                n, _ptr(poses), _ptr(fit_rows), _ptr(streak), _ptr(event), _stream(self.device)), self._ctx)
+
+    def reinit(self, frame_depth, seg, K, labels, object_width, poses, fit_rows, streak, fit, below=0.5, after=3, weight_ids=None,
+               mode='vispy', image_hw=None, init=None, fill_depth=None):
+        """Re-initialise the lost tracks of one tracking step from their masks (include/se3tn.h): the loss rule over the step's
+        fit rows (lost_tracks), the lost list copied back through pinned memory (one synchronisation of the current stream,
+        the call's only one), then, when some track is lost and seg is given, one init_poses call on the lost tracks in
+        ascending order, fit_poses at their starts and accept_starts.
+        poses float64 (n,4,4) and fit_rows int32 (n,6) CUDA tensors (the step's output and its fit rows) are updated in place;
+        streak int32 (n) CUDA tensor, the tracks' streaks, persists across calls (zeros at the start).  frame_depth uint16 (H,W)
+        mm and seg uint8 (H,W) label image (or None: no attempt) are CUDA tensors or numpy arrays, uploaded only when a track is
+        lost; fill_depth as in track_render: the depth is filled first, as the step filled it.  labels (n) ints in 1..255,
+        object_width float64 CUDA (n), weight_ids int32 (n) host array or None (mesh 0), mode / image_hw as in render(): the
+        step's.  fit: the step's tau in mm; init: init_spec's argument.  -> event int32 (n) CUDA tensor: 0 not below, 1 below and
+        no attempt, 2 restarted, 3 no start, 4 start rejected."""
+        tau = self.fit_spec(fit)
+        if not tau:
+            raise ValueError('reinit: fit must be the step\'s tau in mm, not %r' % (fit,))
+        n = int(poses.shape[0])
+        lab = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+        if lab.shape != (n,):
+            raise ValueError('reinit: %d labels for %d tracks' % (lab.shape[0], n))
+        wh = self._host_ids('reinit', weight_ids, n)
+        event, lost = self.lost_tracks(fit_rows, streak, below, after)
+        pin = getattr(self, '_reinit_pin', None)
+        if pin is None or pin.numel() < n + 1:
+            pin = self._reinit_pin = torch.empty(max(n, self.max_batch) + 1, dtype=torch.int32, pin_memory=True)
+        pin[:n + 1].copy_(lost, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        m = int(pin[0])
+        if m == 0 or seg is None:
+            return event
+        idx = pin[1:1 + m].numpy().copy()
+        as_dev = lambda a, dt: a.to(self.device, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
+        depth_d, seg_d = as_dev(frame_depth, torch.uint16), as_dev(seg, torch.uint8)
+        on, max_depth, extrapolate, blur = self.depth_fill_spec(fill_depth)
+        if on:
+            depth_d = self.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
+        sub_ids = None if wh is None else wh[idx]
+        width = object_width.index_select(0, lost[1:1 + m].long())
+        starts, init_rows = self.init_poses(depth_d, seg_d, K, lab[idx], width, weight_ids=sub_ids, mode=mode, image_hw=image_hw, init=init)
+        start_fit = self.fit_poses(depth_d, K, starts, width, tau, weight_ids=sub_ids, mode=mode, image_hw=image_hw)
+        self.accept_starts(idx, starts, init_rows, start_fit, poses, fit_rows, streak, event)
+        return event
 
     def eval_pairs(self, rgbA, depthA, rgbB, depthB, A_in_cam, B_in_cam, trans_normalizer, rot_normalizer,
                    weight_ids_host=None, weight_ids_dev=None, precision='bf16x3', want_terms=False, want_labels=False,

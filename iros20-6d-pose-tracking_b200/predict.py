@@ -44,18 +44,21 @@ FIT_TAU_DEFAULT = 10
 
 # The per-step options of a Tracker or a driver run, as step_options checks them: fit the tau in mm whose rows the caller keeps
 # (None: none), tau the step's fit check in mm (None: off), icp Engine.icp_spec's argument (None: off), hypotheses S and the seed
-# of their draws.  A tuple, so the spawned ranks of a multi-GPU run receive it in their process arguments.
-StepOptions = collections.namedtuple('StepOptions', 'fit tau icp hypotheses seed')
+# of their draws, reinit reinit_options' value (None: off).  A tuple, so the spawned ranks of a multi-GPU run receive it in their
+# process arguments.
+StepOptions = collections.namedtuple('StepOptions', 'fit tau icp hypotheses seed reinit', defaults=(None,))
 
 
-def step_options(fit=None, hypotheses=1, seed=0, icp=None, icp_tau=None, fit_switch=False):
+def step_options(fit=None, hypotheses=1, seed=0, icp=None, icp_tau=None, fit_switch=False, reinit=None):
     """The options of every tracking step -> StepOptions, or a ValueError, checked in this order:
     fit       None or a tau in mm (Engine.fit_spec).  fit_switch (the Tracker's fit) also takes True, FIT_TAU_DEFAULT mm, and
               False, off, which refuses hypotheses.
     hypotheses  S, an integer in [1, MAX_HYPOTHESES]; seed an integer.
     icp       None / 0 off, or M iterations or a dict (Engine.icp_spec); icp_tau the gate in mm, refused without icp.  ICP inside
               hypothesis steps is not supported: refused with S > 1.
-    S > 1 ranks the starts by the fit check, so the step's tau is fit, or FIT_TAU_DEFAULT when fit is None."""
+    S > 1 ranks the starts by the fit check, so the step's tau is fit, or FIT_TAU_DEFAULT when fit is None.
+    reinit    None off, or reinit_options' argument: re-initialise lost tracks after every step.  It ranks starts by the fit check
+              as hypotheses do: the step's tau is then fit or FIT_TAU_DEFAULT, and fit_switch's False is refused."""
     off = fit_switch and fit is False
     if fit_switch and isinstance(fit, bool):
         fit = FIT_TAU_DEFAULT if fit else None
@@ -75,7 +78,34 @@ def step_options(fit=None, hypotheses=1, seed=0, icp=None, icp_tau=None, fit_swi
         raise ValueError('icp %r with hypotheses %d: ICP inside hypothesis steps is not supported' % (icp, hypotheses))
     if off and hypotheses > 1:
         raise ValueError('hypotheses=%d ranks the starts by the fit check: fit must not be off' % hypotheses)
-    return StepOptions(fit, fit or (FIT_TAU_DEFAULT if hypotheses > 1 else None), icp, int(hypotheses), int(seed))
+    reinit = reinit_options(reinit)
+    if off and reinit is not None:
+        raise ValueError('reinit ranks a start against the tracked pose by the fit check: fit must not be off')
+    tau = fit or (FIT_TAU_DEFAULT if hypotheses > 1 or reinit is not None else None)
+    return StepOptions(fit, tau, icp, int(hypotheses), int(seed), reinit)
+
+
+def reinit_options(reinit):
+    """Tracker(reinit=)'s value -> None (off) or a dict {'below', 'after', 'init'}: below the inlier fraction and after the frames
+    in a row below it that make a track lost (Engine.reinit_spec; defaults Engine.REINIT_DEFAULTS), init Engine.init_spec's
+    fields for the restart (None: its defaults).  Anything else is a ValueError."""
+    if reinit is None:
+        return None
+    if not isinstance(reinit, dict):
+        raise ValueError('reinit must be None or a dict of below, after and init, not %r' % (reinit,))
+    unknown = set(reinit) - {'below', 'after', 'init'}
+    if unknown:
+        raise ValueError('reinit: unknown fields %s' % sorted(unknown))
+    spec = dict(_engine.Engine.REINIT_DEFAULTS, init=None)
+    spec.update(reinit)
+    _engine.Engine.reinit_spec(spec['below'], spec['after'])
+    _engine.Engine.init_spec(spec['init'])
+    return spec
+
+
+def reinit_keep(opts):
+    """The tracks per restarted track an Engine must hold for opts' re-initialisation (its init keep), 1 without it."""
+    return 1 if opts.reinit is None else Engine.init_spec(opts.reinit['init']).keep
 
 
 def hypothesis_spread(info, opts, label=None):
@@ -193,7 +223,7 @@ def _as_numpy_pose(p):
 class Tracker:
     def __init__(self, dataset_info, images_mean, images_std, ckpt_dir, model_path=None, trans_normalizer=0.03,
                  rot_normalizer=5 * np.pi / 180, engine=None, weight_id=0, renderer=None, precision='bf16x3', max_batch=64,
-                 fill_depth=False, iterations=1, fit=None, hypotheses=1, seed=0, icp=None):
+                 fill_depth=False, iterations=1, fit=None, hypotheses=1, seed=0, icp=None, reinit=None):
         """fill_depth: the depth frames given to on_track / on_track_batch are raw sensor frames, hole-filled inside every
         tracking step.  True is the reference ROS node's fill_depth(depth, max_depth=2.0); a dict sets max_depth / extrapolate
         / blur_type (Engine.depth_fill_spec).
@@ -215,14 +245,25 @@ class Tracker:
         point-to-plane ICP at Engine.icp_spec's default gate, or a dict of its fields.  on_track / on_track_batch then leave the
         last iteration's stats (inliers, rms_mm, step_mm, step_deg per track) in last_icp: numpy on the host route, a float64
         CUDA tensor on the device route.  Like fit it needs the CUDA rasteriser drawing input A inside the step; it is refused
-        with hypotheses > 1.  fit, hypotheses, seed and icp are checked by step_options and kept in opts."""
+        with hypotheses > 1.  fit, hypotheses, seed, icp and reinit are checked by step_options and kept in opts.
+        reinit: None off, or a dict {'below': f, 'after': L, 'init': {Engine.init_spec's fields}} (reinit_options): after every
+        step, a track whose inlier fraction stayed below f for L frames in a row is restarted from its mask
+        (Engine.reinit) when on_track / on_track_batch are given the frame's mask or label image, and the start replaces the
+        tracked pose only when it fits the frame better.  The event codes of the frame's tracks (0 not below, 1 below, 2
+        restarted, 3 no start, 4 start rejected) are left in last_reinit.  Each track index keeps its streak of frames below
+        across calls; a call with another number of tracks, or reset_reinit(), starts them from 0.  Like hypotheses it turns the
+        fit check on at FIT_TAU_DEFAULT mm when fit is not given, and needs the CUDA rasteriser; a Tracker that builds its
+        Engine sizes it for max_batch x init keep tracks, which one restart of every track needs.  Each frame with reinit on
+        synchronises once, to read which tracks are lost."""
         Engine.depth_fill_spec(fill_depth)                 # a bad value fails here, not at the first frame
         self.iterations = Engine.refine_iterations(iterations)
-        self.opts = step_options(fit, hypotheses, seed, icp, fit_switch=True)
+        self.opts = step_options(fit, hypotheses, seed, icp, fit_switch=True, reinit=reinit)
+        self.reinit = self.opts.reinit
+        self._streak = None                                # reinit: the tracks' streaks on the device, per track index
         self.fit, self.icp, self.hypotheses, self.seed = self.opts.tau, self.opts.icp, self.opts.hypotheses, self.opts.seed
         self.spread = hypothesis_spread(dataset_info, self.opts)
         self._calls = 0                                    # the c of the draw keys (seed, c, j)
-        self.last_fit = self.last_icp = self.last_choice = self.last_init = None
+        self.last_fit = self.last_icp = self.last_choice = self.last_init = self.last_reinit = None
         self.fill_depth = fill_depth
         self.dataset_info = dataset_info
         self.image_size = (dataset_info['resolution'], dataset_info['resolution'])
@@ -247,7 +288,11 @@ class Tracker:
             checkpoint = ckpt_dir if 'state_dict' in ckpt_dir else {'state_dict': ckpt_dir}
         else:
             checkpoint = torch.load(ckpt_dir, map_location='cpu')
-        self.engine = engine if engine is not None else Engine(max_batch=max_batch * self.hypotheses)
+        keep = reinit_keep(self.opts)
+        if engine is not None and self.reinit is not None and engine.max_batch < keep:
+            raise ValueError('reinit restarts a lost track with init keep=%d candidates, more than the engine\'s max_batch=%d'
+                             % (keep, engine.max_batch))
+        self.engine = engine if engine is not None else Engine(max_batch=max_batch * max(self.hypotheses, keep))
         self.weight_id = weight_id
         self.precision = precision
         self.model = Se3TrackNet(image_size=self.image_size[0], engine=self.engine, weight_id=weight_id, precision=precision)
@@ -383,22 +428,30 @@ class Tracker:
 
     # ------------------------------------------------------------------ the hot path
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
-                 rgbA=None, depthA=None, show=False):
+                 rgbA=None, depthA=None, show=False, mask=None, label=1):
         """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose.  Without rgbA / depthA and with the
         CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host), and refined
-        Tracker.iterations times."""
+        Tracker.iterations times.  mask: with reinit, the object's pixels of this frame, a bool (H,W) array or a uint8 label
+        image in which they are `label`; read only when the track is lost."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
+        seg = None
+        if mask is not None:
+            m = mask.cpu().numpy() if torch.is_tensor(mask) else np.asarray(mask)
+            if m.dtype not in (np.bool_, np.uint8):
+                raise ValueError('on_track: mask must be a bool mask or a uint8 label image, not %s' % m.dtype)
+            seg = np.where(m, np.uint8(label), np.uint8(0)) if m.dtype == np.bool_ else m
+        kw = {} if self.reinit is None else dict(seg=seg, labels=[int(label)])
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
         if not fused:
             self._check_step_draws(rgbA is not None or depthA is not None)
         if fused:
-            out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth)
+            out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth, **kw)
         else:
             if rgbA is None or depthA is None:
                 rgbA, depthA = self.render_window(A_in_cam)
             out = self.on_track_batch(A_in_cam[None], current_rgb, current_depth,
                                       np.ascontiguousarray(rgbA, dtype=np.uint8)[None],
-                                      np.ascontiguousarray(depthA).astype(np.uint16)[None])
+                                      np.ascontiguousarray(depthA).astype(np.uint16)[None], **kw)
         final_estimate = out[0]
         self.prev_rgb = current_rgb
         self.prev_depth = current_depth
@@ -410,7 +463,8 @@ class Tracker:
         self.frame_cnt += 1
         return final_estimate
 
-    def on_track_batch(self, prev_poses, current_rgb, current_depth, rgbA=None, depthA=None, weight_ids=None, object_width=None):
+    def on_track_batch(self, prev_poses, current_rgb, current_depth, rgbA=None, depthA=None, weight_ids=None, object_width=None,
+                       seg=None, labels=None):
         """N independent tracks of ONE frame -> (N,4,4) float64.  rgbA / depthA None: rendered on the device by the CUDA
         rasteriser (needs a CudaRenderer; per-track models follow weight_ids), inside the tracking step when the renderer
         allows it (_fused_renderer).  The types of the inputs pick one of two routes:
@@ -423,7 +477,55 @@ class Tracker:
                 cannot draw it, and one Engine.track_render / track_batch call is enqueued.  Tensor poses give a CUDA
                 tensor and nothing is synchronised; numpy poses give a numpy result.
         A pageable input may be overwritten as soon as the call returns.  A pinned CPU tensor is read asynchronously: it must
-        stay unchanged until the current stream has run this call's step."""
+        stay unchanged until the current stream has run this call's step.
+        seg / labels: with reinit, the frame's uint8 (H,W) label image (numpy or a tensor) and each track's label in it (ints
+        in 1..255; None with one track: 1), read only when a track is lost (_reinit).  Without seg no track is restarted."""
+        if self.reinit is None:
+            return self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
+        n = len(prev_poses)
+        if labels is None and seg is not None and n != 1:
+            raise ValueError('on_track_batch: seg needs labels, one per track')
+        lab = np.ascontiguousarray([1] * n if labels is None else labels, dtype=np.int64).reshape(-1)
+        if lab.shape != (n,) or (seg is not None and (lab.min() < 1 or lab.max() > 255)):
+            raise ValueError('on_track_batch: labels must be %d ints in 1..255, not %r' % (n, labels))
+        if seg is not None and seg.dtype not in (np.uint8, torch.uint8):
+            raise ValueError('on_track_batch: seg must be a uint8 label image, not %s' % seg.dtype)
+        if n * reinit_keep(self.opts) > self.engine.max_batch:     # checked before the step, which would update the streaks
+            raise ValueError('reinit: %d tracks x init keep=%d exceed the engine\'s max_batch=%d'
+                             % (n, reinit_keep(self.opts), self.engine.max_batch))
+        self.last_reinit = None
+        out = self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
+        return self._reinit(out, current_depth, seg, lab, weight_ids, object_width)
+
+    def reset_reinit(self):
+        """Start every track's streak of frames below the fit threshold from 0 (reinit), as at a new sequence."""
+        self._streak = None
+
+    def _reinit(self, out, depth, seg, labels, weight_ids, object_width):
+        """Engine.reinit after the step that gave `out` (a CUDA tensor, updated in place, or numpy, uploaded and brought back)
+        and last_fit, on the raw frame depth (filled as the step fills it), with the step's meshes, widths and render mode."""
+        dev, n = self.engine.device, len(out)
+        if self._streak is None or self._streak.numel() != n:
+            self._streak = torch.zeros(n, dtype=torch.int32, device=dev)
+        on_host = not torch.is_tensor(out)
+        poses = torch.from_numpy(np.ascontiguousarray(out)).to(dev) if on_host else out
+        rows = self.last_fit if torch.is_tensor(self.last_fit) else torch.from_numpy(np.ascontiguousarray(self.last_fit)).to(dev)
+        ow = object_width.to(dev, torch.float64).contiguous() if torch.is_tensor(object_width) else \
+            torch.from_numpy(self._widths(object_width, n)).to(dev)
+        r = self.renderer
+        event = self.engine.reinit(depth, seg, self.K, labels, ow, poses, rows, self._streak, self.opts.tau, self.reinit['below'],
+                                   self.reinit['after'], weight_ids=self._weight_ids(weight_ids, n), mode=r.mode, image_hw=r.image_hw,
+                                   init=self.reinit['init'], fill_depth=self.fill_depth)
+        if not on_host:
+            self.last_reinit = event
+            return out
+        self.last_reinit = event.cpu().numpy()
+        if not torch.is_tensor(self.last_fit):           # the host route's rows; the device route's were updated in place
+            self.last_fit = rows.cpu().numpy()
+        return poses.cpu().numpy()
+
+    def _track_step(self, prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width):
+        """on_track_batch's tracking step, without re-initialisation."""
         render = rgbA is None or depthA is None
         if render and not hasattr(self.renderer, 'render_batch'):
             raise RuntimeError('on_track_batch without rgbA/depthA needs the CUDA renderer (Tracker(renderer="cuda", model_path=*.ply))')
@@ -1274,7 +1376,13 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, 
     rows}, row t the fit of the step that wrote pose t.  With ICP the poses and fit rows are those after ICP.  With S > 1
     hypotheses the poses and fit rows are the kept hypotheses', and track j of frame t of sequence k draws with
     hypothesis_key(seq_index[k], t, j): seq_index is each sequence's index in the run's sorted list, so a share of the sequences
-    on one GPU draws what the whole run draws."""
+    on one GPU draws what the whole run draws.
+
+    opts.reinit (re-initialisation of lost tracks): each sequence is then a 5-tuple whose last entry is the label-image file of
+    every tracked frame, decoded through the same ring (its 'seg' field).  After each variant's step, Engine.reinit runs on that
+    variant's poses and fit rows, in place, before the history copy: the labels are the class ids, the meshes the weight ids, and
+    every (variant, sequence) has its own streaks, zero at the sequence's start.  The yield then has a third entry, {variant:
+    (frames, n) int32 event codes}, and the fit rows are those after the restarts (None unless opts.fit)."""
     if video is not None and len(variants) != 1:
         raise ValueError('result videos are drawn for one variant, not %d' % len(variants))
     fp8 = {}                                               # checkpoint index -> its first fp8 variant
@@ -1289,11 +1397,16 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, 
     spec = {'rgb': ((H, W, 3), torch.uint8), 'depth': ((H, W), torch.uint16)}
     if video is not None:
         spec['label'] = ((LABEL_TOP - LABEL_BOTTOM, W), torch.uint8)
+    reinit = opts.reinit
+    if reinit is not None:
+        spec['seg'] = ((H, W), torch.uint8)
     ring = StagingRing(spec, depth, dev)
     frames = []
-    for k, (rgb_files, depth_files, _, _) in enumerate(sequences):
+    for k, (rgb_files, depth_files) in enumerate(s[:2] for s in sequences):
         for t, (r, d) in enumerate(zip(rgb_files, depth_files)):
             jobs = [(_decode_into, 'rgb', read_rgb, r), (_decode_into, 'depth', read_depth, d)]
+            if reinit is not None:
+                jobs.append((_decode_into, 'seg', read_seg, sequences[k][4][t]))
             if video is not None:
                 jobs.append((_label_into, video[1][k][1][t], H, W))
             frames.append(jobs)
@@ -1307,7 +1420,7 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, 
             sink = stack.enter_context(contextlib.closing(VideoSink((max(len(s[2]) for s in sequences), H // 2, W // 2, 3), depth, dev)))
         uploads = stack.enter_context(contextlib.closing(ring.uploads(frames, workers)))
         by_ids, by_n = {}, {}
-        for k, (rgb_files, _, ids, init) in enumerate(sequences):
+        for k, (rgb_files, _, ids, init) in enumerate(s[:4] for s in sequences):
             n = len(ids)
             for c in _checkpoints(variants):
                 if (ids, c) not in by_ids:
@@ -1327,7 +1440,12 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, 
                     by_n[v, n] = (outs, keys, None if video is None else torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=dev))
                 by_n[v, n][0]['out_poses'].copy_(torch.from_numpy(init))
             history = {v: torch.empty((len(rgb_files), n, 4, 4), dtype=torch.float64, device=dev) for v in variants}
-            fit_rows = {v: torch.empty((len(rgb_files), n, 6), dtype=torch.int32, device=dev) for v in variants} if opts.fit else None
+            fit_rows = {v: torch.empty((len(rgb_files), n, 6), dtype=torch.int32, device=dev) for v in variants} \
+                if opts.fit or reinit is not None else None
+            if reinit is not None:                          # per variant: the streaks from 0, the event codes of every frame
+                streaks = {v: torch.zeros(n, dtype=torch.int32, device=dev) for v in variants}
+                events = {v: torch.empty((len(rgb_files), n), dtype=torch.int32, device=dev) for v in variants}
+                labels = np.asarray(ids, dtype=np.int32)
             trk = trackers[ids[0]]
             track_set = None if video is None else np.asarray([set_of[w] for w in ids], dtype=np.int32)
             for t in range(len(rgb_files)):
@@ -1344,13 +1462,18 @@ def _track_sequences(eng, trackers, sequences, variants, depth, workers, video, 
                         keys.copy_(torch.arange(n, dtype=torch.int64, device=dev) + hypothesis_key(seq_index[k], t, 0))
                     track_step(eng, trackers, trk, ring.dev['rgb'], ring.dev['depth'], poses, widths, wh, wd, keys, opts, v[0], v[1],
                                dict(outs, out_fit=fit_rows[v][t]) if fit_rows else outs)
+                    if reinit is not None:
+                        events[v][t].copy_(eng.reinit(ring.dev['depth'], ring.dev['seg'], trk.K, labels, widths, poses, fit_rows[v][t],
+                                                      streaks[v], opts.tau, reinit['below'], reinit['after'], weight_ids=wh,
+                                                      mode=trk.renderer.mode, image_hw=trk.renderer.image_hw, init=reinit['init']))
                     history[v][t].copy_(poses)
                 if video is not None:
                     eng.draw_tracks(ring.dev['rgb'], trk.K, poses, table, offsets, track_set,
                                     label=(H - LABEL_TOP, ring.dev['label']), label_order=video[0], out=drawn)
                     sink.put(drawn, video[1][k][0], last=t == len(rgb_files) - 1)
-            yield ({v: h.cpu().numpy() for v, h in history.items()},
-                   None if fit_rows is None else {v: r.cpu().numpy() for v, r in fit_rows.items()})
+            res = ({v: h.cpu().numpy() for v, h in history.items()},
+                   None if not opts.fit else {v: r.cpu().numpy() for v, r in fit_rows.items()})
+            yield res if reinit is None else res + ({v: e.cpu().numpy() for v, e in events.items()},)
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -1418,7 +1541,7 @@ def _checkpoints(variants):
 
 def _checkpoint_sequences(sequences, c):
     """sequences with every track's weight id moved to checkpoint c's set."""
-    return sequences if c == 0 else [(r, d, tuple(w + CKPT_ID_STRIDE * c for w in ids), init) for r, d, ids, init in sequences]
+    return sequences if c == 0 else [(s[0], s[1], tuple(w + CKPT_ID_STRIDE * c for w in s[2])) + tuple(s[3:]) for s in sequences]
 
 
 def _calibrate_borrowed(eng, trackers, sequences, borrowed):
@@ -1426,7 +1549,7 @@ def _calibrate_borrowed(eng, trackers, sequences, borrowed):
     the initial poses of the named tracks, as _track_sequences calibrates it (Engine.calibrate_fp8_tracks, input A drawn by the
     rasteriser).  Calibration takes per-tensor maxima of each set's own tracks, so it gives the single-GPU run's scales."""
     for k, tracks in borrowed.items():
-        rgb_files, depth_files, ids, init = sequences[k]
+        rgb_files, depth_files, ids, init = sequences[k][:4]
         wh = np.asarray([ids[j] for j in tracks], dtype=np.int32)
         trk, dev = trackers[int(wh[0])], eng.device
         wd = torch.from_numpy(wh).to(dev)
@@ -1443,8 +1566,8 @@ def _track_share(entries, precision, max_batch, sequences, mine, borrowed, varia
     (_one_pass_trackers), the fp8 calibrations borrowed from other shares (_calibrate_borrowed), then _track_sequences over the
     share with writes[k] (fn, *args) called as fn(*args, tracked) on sequence k's (poses, fit rows or None).  video: None, or
     (label order, [(paths, labels)] per sequence, folders to make once the trackers exist).  opts: _track_sequences' opts (the
-    Engine holds max_batch x S tracks per step).  -> (Engine, {k: what writes[k] returned})."""
-    eng, trackers = _one_pass_trackers(entries, precision, max_batch * opts.hypotheses)
+    Engine holds max_batch x S tracks per step, and max_batch x init keep with re-initialisation).  -> (Engine, {k: what writes[k] returned})."""
+    eng, trackers = _one_pass_trackers(entries, precision, max_batch * max(opts.hypotheses, reinit_keep(opts)))
     for c in _checkpoints(variants):                    # every checkpoint's sets, each on its own single-GPU frame
         _calibrate_borrowed(eng, trackers, _checkpoint_sequences(sequences, c), borrowed)
     drawn = None
@@ -1565,6 +1688,9 @@ def _track_on_ranks(gpus, entries, precision, max_batch, sequences, variants, de
 FIT_FILE = 'fit.npy'
 # --score's fit table: a frame whose ADD-S is at least this far from the annotation counts as lost (a fixed bound, not an option)
 FIT_LOST_ADDS = 0.02
+# Re-initialisation in the YCB-Video one-pass driver: REINIT_FILE beside each sequence's pose files, the event code of every
+# pose file's step (include/se3tn.h: 0 not below, 1 below, 2 restarted, 3 no start, 4 rejected), row 0 (the start pose) -1
+REINIT_FILE = 'reinit.npy'
 
 
 def write_fit_rows(folder, rows):
@@ -1627,9 +1753,11 @@ def _ckpt_label(i, run):
 
 def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
     """One test sequence's files of a getResultsYcbAll run: for each variant (dirs: {variant: {class id: result folder}}) and
-    class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  tracked: (poses, fit rows or None); with rows, each seq<id>/ also
-    gets FIT_FILE, one row per pose file, row 0 (the start pose, not tracked) all -1.  -> {variant: (frames, n, 4, 4) poses}."""
-    poses, rows = tracked
+    class, <folder>/seq<id>/%07d.txt, row 0 the start pose.  tracked: (poses, fit rows or None[, event codes]); with rows, each
+    seq<id>/ also gets FIT_FILE, one row per pose file, row 0 (the start pose, not tracked) all -1; with event codes (a run with
+    re-initialisation), REINIT_FILE, int32 (pose files,), row 0 -1.  -> {variant: (frames, n, 4, 4) poses}."""
+    poses, rows = tracked[:2]
+    events = tracked[2] if len(tracked) > 2 else None
     out = {}
     for v, folder in dirs.items():
         pred_poses = np.concatenate([init[None], poses[v]])      # row 0: the start pose, as in getResultsYcb
@@ -1640,6 +1768,8 @@ def _write_ycb_all_sequence(dirs, seq_id, cls, init, tracked):
                 np.savetxt(os.path.join(sdir, '%07d.txt' % i), pred_poses[i, j])
             if rows is not None:
                 write_fit_rows(sdir, np.concatenate([np.full((1, 6), -1, np.int32), rows[v][:, j]]))
+            if events is not None:
+                np.save(os.path.join(sdir, REINIT_FILE), np.concatenate([[-1], events[v][:, j]]).astype(np.int32))
         out[v] = pred_poses
     return out
 
@@ -1655,6 +1785,12 @@ def read_seg(path):
     if s is None:
         raise FileNotFoundError(path)
     return np.ascontiguousarray(s if s.ndim == 2 else s[:, :, 0], dtype=np.uint8)
+
+
+def ycb_label_file(color_file):
+    """The seg/ label image of a YCB-Video frame: <seq>/seg/%06d-label.png beside <seq>/color/%06d-color.png."""
+    seq_dir = os.path.dirname(os.path.dirname(color_file))
+    return os.path.join(seq_dir, 'seg', os.path.basename(color_file).split('-')[0] + '-label.png')
 
 
 def class_width(k):
@@ -1703,7 +1839,7 @@ def _mask_start_refusal(seq, c, name, status):
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None, init=None):
+                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None, init=None, reinit=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1757,13 +1893,22 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     initialize_method='mask': each sequence's tracks start from one Engine.init_poses call on its first frame (depth_filled and
     seg/ label image; each class's label is its class id; init: Engine.init_spec's argument), made in this process before any
     tracking, so several GPUs write the one-GPU trees.  A class the call finds no start for (an empty mask, too few pixels with
-    depth) is a ValueError naming the sequence and the class.  init without 'mask' is a ValueError."""
+    depth) is a ValueError naming the sequence and the class.  init without 'mask' is a ValueError.
+
+    reinit: None off, or {'below': f, 'after': L, 'init': Engine.init_spec's argument} (reinit_options): after every step, the
+    tracks whose inlier fraction stayed below f for L frames in a row are restarted from that frame's seg/%06d-label.png (the
+    label of class c is c) by Engine.reinit, and a start replaces the tracked pose only when it fits the frame better.  The pose
+    files, FIT_FILE and the video hold the poses after the restarts; each class's seq<id>/ also gets REINIT_FILE, the event code
+    of every pose file (row 0 -1).  Every variant, checkpoint and sequence has its own streaks, zero at the sequence's start.
+    It turns the fit check on at FIT_TAU_DEFAULT when fit is not given; the Engine then holds n_max x init keep tracks (the
+    steps' split-K regime depends on n alone, so their bits do not move).  Every tracked frame's label image must exist: a
+    missing one is a FileNotFoundError before anything is loaded.  Several GPUs write the one-GPU trees."""
     if init is not None and initialize_method != 'mask':
         raise ValueError("init options need initialize_method='mask', not %r" % (initialize_method,))
     if initialize_method == 'mask':
         Engine.init_spec(init)
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config, fit=fit,
-                          hypotheses=hypotheses, seed=seed, icp=icp, icp_tau=icp_tau)
+                          hypotheses=hypotheses, seed=seed, icp=icp, icp_tau=icp_tau, reinit=reinit)
     if initialize_method not in ('gt', 'posecnn', 'poserbpf', 'mask'):
         raise ValueError('initialize_method must be gt, posecnn, poserbpf or mask')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
@@ -1773,6 +1918,14 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     data_dir = '{}/data_organized/'.format(ycb_dir)
     keyframes_all = read_keyframes(ycb_dir) if initialize_method == 'posecnn' else []
     sequences = []
+    if run.opts.reinit is not None:                       # every tracked frame's label image, before anything is loaded
+        for seq_id, cls in track_sets.items():
+            rgb_files = _ycb_sequence_files(os.path.join(data_dir, '%04d' % seq_id), cls[0])[0]
+            nf = len(rgb_files) if max_frames is None else min(len(rgb_files), 1 + max_frames)
+            missing = [p for p in (ycb_label_file(r) for r in rgb_files[1:nf]) if not os.path.isfile(p)]
+            if missing:
+                raise FileNotFoundError('reinit: %d tracked frames of sequence %04d have no label image, the first %s'
+                                        % (len(missing), seq_id, missing[0]))
     starts = MaskStarts(classes, max([len(v) for v in track_sets.values()] + [1]), init) if initialize_method == 'mask' else None
     try:
         for seq_id, cls in track_sets.items():
@@ -1794,7 +1947,8 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                 init_poses = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
                                                        sorted(findClassContainedVideosYcb(c, data_dir, testset=True)))
                                        for c in cls]).astype(np.float64)
-            sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init_poses))
+            sequences.append((rgb_files[1:nf], depth_files[1:nf], tuple(cls), init_poses)
+                             + (() if run.opts.reinit is None else ([ycb_label_file(r) for r in rgb_files[1:nf]],)))
     finally:
         if starts is not None:
             starts.close()
@@ -2577,6 +2731,48 @@ def score_fit(root, ycb_dir, YCBInEOAT_dir=None, class_ids=None):
                 auc=roc_auc(1.0 - inl, lost))
 
 
+def score_reinit(root, ycb_dir, class_ids):
+    """What re-initialisation did in one variant's tree of a YCB-Video run with reinit, from each seq<id>/'s REINIT_FILE ->
+    {'tracked' frames (pose files a step wrote, over every class), 'below' (event != 0), 'attempts' (events 2, 3 and 4: every
+    frame has its mask here, so these are the lost frames),
+    'restarted', 'rejected', 'failed' (no start), 'restarts_near' (the share of restarted poses within FIT_LOST_ADDS ADD-S of
+    the annotation, on the class's points.xyz as eval_ycb reads them; NaN without restarts)}."""
+    import glob
+    from . import eval_ycb
+    eng = U._eng()
+    names = ycb_class_names(ycb_dir)
+    model_files = sorted(glob.glob('{}/CADmodels/**/points.xyz'.format(ycb_dir), recursive=True))
+    ev, near = [], []
+    for c in class_ids:
+        restarted, gts = [], []
+        for f in sorted(glob.glob(os.path.join(ycb_all_res_dir(root, names[c - 1]), 'seq*', REINIT_FILE))):
+            e = np.load(f)[1:]
+            ev.append(e)
+            seq_id = int(os.path.basename(os.path.dirname(f))[3:])
+            for i in np.nonzero(e == _lib.REINIT_RESTARTED)[0] + 1:
+                restarted.append(np.loadtxt(os.path.join(os.path.dirname(f), '%07d.txt' % i)))
+                gts.append(np.loadtxt('{}/data_organized/%04d/pose_gt/{}/%06d.txt'.format(ycb_dir, c) % (seq_id, i + 1)))
+        if restarted:
+            t = lambda a: torch.from_numpy(np.ascontiguousarray(np.stack(a), dtype=np.float64)).to(eng.device)
+            pts = torch.from_numpy(np.ascontiguousarray(eval_ycb._read_points(model_files[c - 1]))).to(eng.device)
+            near.append(eng.add_adi(pts, t(restarted), t(gts))[1].cpu().numpy() < FIT_LOST_ADDS)
+    e = np.concatenate(ev) if ev else np.zeros(0, np.int32)
+    near = np.concatenate(near) if near else np.zeros(0, bool)
+    count = lambda *codes: int(np.isin(e, codes).sum())
+    return dict(tracked=int(len(e)), below=int((e != 0).sum()), attempts=count(2, 3, 4), restarted=count(2), rejected=count(4),
+                failed=count(3), restarts_near=float(near.mean()) if len(near) else float('nan'))
+
+
+def print_reinit_table(rows):
+    """--score's table for a run with --reinit_below: one row per variant tree of score_reinit's result."""
+    print('re-initialisation: restarts near = the share of restarted poses within %g cm ADD-S of the annotation' % (FIT_LOST_ADDS * 100))
+    print('%-16s %8s %8s %8s %9s %8s %8s %14s' % ('variant', 'tracked', 'below', 'attempts', 'restarted', 'rejected', 'failed',
+                                                 'restarts near'))
+    for label, r in rows.items():
+        print('%-16s %8d %8d %8d %9d %8d %8d %14.4f' % (label, r['tracked'], r['below'], r['attempts'], r['restarted'], r['rejected'],
+                                                      r['failed'], r['restarts_near']))
+
+
 def print_fit_table(rows):
     """--score's table for a run with --fit: one row per variant tree of score_fit's result."""
     print('fit check: frames with ADD-S >= %g cm count as lost; inlier fraction = inlier / model pixels' % (FIT_LOST_ADDS * 100))
@@ -2631,6 +2827,12 @@ def main(argv=None):
                         % _engine.Engine.INIT_DEFAULTS['keep'])
     parser.add_argument('--init_icp', type=int, default=None, help='--init mask / ycbv_init: ICP iterations on the kept candidates '
                         '(0: none; default %d)' % _engine.Engine.INIT_DEFAULTS['icp'])
+    parser.add_argument('--reinit_below', type=float, default=None, help='ycbv_all: re-initialise a track from its frame\'s seg/ '
+                        'label image when its fit check\'s inlier fraction stays below F (0..1, three decimals) for --reinit_after '
+                        'frames; the --init_* options set the restart.  Each sequence folder gets reinit.npy, and --score adds its table.  '
+                        'Defaults are guesses: choose F with --fit --score')
+    parser.add_argument('--reinit_after', type=int, default=None, help='with --reinit_below: the frames in a row below F that make a '
+                        'track lost (1..1000, default %d)' % _engine.Engine.REINIT_DEFAULTS['after'])
     parser.add_argument('--max_frames', type=int, default=None)
     parser.add_argument('--score', action='store_true', help='ycbv_all / ycbineoat_all: score the output with eval_ycb / '
                         'eval_ycbineoat and print its lines')
@@ -2654,6 +2856,7 @@ def main(argv=None):
     parser.add_argument('--gpus', type=int, default=None, help='ycbv_all / ycbineoat_all: share the sequences out over N GPUs, '
                         'one process each (default 1); every file is the one a one-GPU run writes')
     args = parser.parse_args(argv)
+    cli_reinit(args)
     init = cli_init(args)
     if args.mode == 'ycbv_init':
         return _main_init(args, init)
@@ -2807,14 +3010,16 @@ def cli_recover(args):
 def cli_init(args):
     """The start-from-mask options of the command line -> Engine.init_spec's dict (None: the defaults), also left in
     args.init_spec.  --init mask needs --mode ycbv_all; the --init_* options need --init mask or --mode ycbv_init; the other
-    modes refuse --init mask and them; a value init_spec refuses is a SystemExit."""
+    modes refuse --init mask and them; --reinit_below (ycbv_all) also takes them, for its restarts; a value init_spec refuses is
+    a SystemExit."""
     flags = {'viewpoints': args.init_viewpoints, 'inplane': args.init_inplane, 'keep': args.init_keep, 'icp': args.init_icp}
     given = {k: v for k, v in flags.items() if v is not None}
     if args.init == 'mask' and args.mode != 'ycbv_all':
         raise SystemExit('--init mask needs --mode ycbv_all; --mode %s does not start from masks (--mode ycbv_init scores the '
                          'starts on the key frames)' % args.mode)
-    if given and args.mode != 'ycbv_init' and args.init != 'mask':
-        raise SystemExit('%s need --init mask (with --mode ycbv_all) or --mode ycbv_init' % ', '.join('--init_' + k for k in given))
+    if given and args.mode != 'ycbv_init' and args.init != 'mask' and args.reinit_below is None:
+        raise SystemExit('%s need --init mask (with --mode ycbv_all), --reinit_below or --mode ycbv_init'
+                         % ', '.join('--init_' + k for k in given))
     spec = given or None
     try:
         _engine.Engine.init_spec(spec)
@@ -2822,6 +3027,23 @@ def cli_init(args):
         raise SystemExit('--init_*: %s' % e)
     args.init_spec = spec
     return spec
+
+
+def cli_reinit(args):
+    """The re-initialisation options of the command line, checked before anything else: --reinit_below needs --mode ycbv_all
+    (the other modes' layouts have no per-frame masks, or they do not track a sequence), --reinit_after needs --reinit_below,
+    and values reinit_options refuses are a SystemExit."""
+    if args.reinit_after is not None and args.reinit_below is None:
+        raise SystemExit('--reinit_after needs --reinit_below')
+    if args.reinit_below is None:
+        return
+    if args.mode != 'ycbv_all':
+        raise SystemExit('--reinit_below needs --mode ycbv_all; --mode %s does not re-initialise tracks from per-frame masks' % args.mode)
+    try:
+        reinit_options({'below': args.reinit_below, 'after': _engine.Engine.REINIT_DEFAULTS['after'] if args.reinit_after is None
+                        else args.reinit_after})
+    except ValueError as e:
+        raise SystemExit('--reinit_below / --reinit_after: %s' % e)
 
 
 def _main_init(args, init):
@@ -2904,6 +3126,9 @@ def _main_one_pass(args, precision=None, iterations=None):
                 raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
         if args.init == 'mask':
             kw['init'] = getattr(args, 'init_spec', None)
+        if args.reinit_below is not None:
+            kw['reinit'] = dict(below=args.reinit_below, init=getattr(args, 'init_spec', None),
+                                **({} if args.reinit_after is None else {'after': args.reinit_after}))
         res = getResultsYcbAll(args.ycb_dir, class_ids, config, args.outdir, initialize_method=args.init, max_frames=args.max_frames, **kw)
         outdir, eoat = args.outdir, {}
     else:
@@ -2942,6 +3167,11 @@ def _main_one_pass(args, precision=None, iterations=None):
         trees = [v[-1] for v in _sweep_variants(outdir, modes, msweep, counts, ksweep, ckpts)]
         print_fit_table({os.path.relpath(tr, outdir): score_fit(tr, args.ycb_dir, args.YCBInEOAT_dir if not ycbv else None,
                                                                  class_ids if ycbv else None) for tr in trees})
+    if args.score and ycbv and args.reinit_below is not None:
+        modes, msweep = precision_modes(precision or 'bf16x3', YCB_ALL_PRECISIONS)
+        counts, ksweep = refine_counts(iterations or 1)
+        trees = [v[-1] for v in _sweep_variants(outdir, modes, msweep, counts, ksweep, ckpts)]
+        print_reinit_table({os.path.relpath(tr, outdir): score_reinit(tr, args.ycb_dir, class_ids) for tr in trees})
     return res
 
 
