@@ -631,6 +631,38 @@ int se3tn_init_poses(se3tn_ctx* ctx, const uint16_t* frame_depth, const uint8_t*
                      const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
                      double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream);
 
+/* ---- start poses from a 2D box and the depth frame ------------------------------------------------------------------ */
+
+/* se3tn_init_boxes starts n objects of one frame from 2D boxes, as a detector gives them, instead of labels.  A box is
+ * int32 (x0, y0, x1, y1) in frame pixels, half-open: the pixels with x0 <= u < x1 and y0 <= v < y1.  Boxes may overlap;
+ * each object owns its box's pixels whatever the other boxes hold.  The stages are those of se3tn_init_poses with:
+ *   1. Box statistics: the object's pixels are its box's pixels instead of seg == l_i.  stats keep their columns over them
+ *      (mask = the box's pixel count, sum_u / mask = (x0 + x1 - 1) / 2 exactly; z_med the lower median; status 1 / 2 as
+ *      before, an empty box (x1 == x0 or y1 == y0) gives status 1).  From the same histogram, D = `depths` depth candidates:
+ *      z_d = the sorted depth at index k_d = max(0, floor(((2 d + 1) depth_px - D) / (2 D))), d = 0 .. D-1, the quantiles
+ *      (2 d + 1) / 2 D of the box's depths (D = 1: the lower median), and t0_d = z_d / 1000 * K^-1 (u, v, 1) in fp64 on the
+ *      ray through the box centre.  A box holds background as well as the object, so one median may lie behind it: the D
+ *      depths let the score pick the one at which the silhouette fits.
+ *   2. Grid: candidate c = d V R + v R + r is the mask grid's rotation (v, r) at t0_d.  All D V R candidates of an object
+ *      compete in one ranking.
+ *   3. Score: the mask score, with M = "the crop pixel's source frame pixel lies in the object's box".  Counts, delta,
+ *      inlier and rank unchanged.
+ *   4-6. Keep, refine and choose unchanged (a kept pose moves along its own ray by delta).
+ * So for D = 1 and boxes that do not overlap, the call equals se3tn_init_poses on a label image in which each object's box
+ * pixels carry its own label, on every output, bit for bit.
+ * Arguments as se3tn_init_poses, with boxes HOST int32 (n, 4) in place of seg and labels (staged into the context's init
+ * block) and depths D in [1, 8].  Shapes that differ: arrays->t0 double (n, D, 3); arrays->cand_rows int32 (n, D V R,
+ * SE3TN_INIT_COLS), column 1 of a row is c above; keep <= D V R.  Refused with SE3TN_ERR_INVALID, the field named and nothing
+ * queued, as se3tn_init_poses, and: depths outside [1, 8]; a box with x0 < 0, y0 < 0, x1 > W, y1 > H, x1 < x0 or y1 < y0.  An
+ * id without a mesh is SE3TN_ERR_STATE.  Plain launches, no CUDA graph; the init block grows as se3tn_init_poses' (a call
+ * that needs more first synchronises `stream`), and tracking steps and their graphs are unaffected.
+ * se3tn_last_launch_count: 2 (box pass, depths) + 1 (grid) + 3 per chunk of the n D V R rows + 1 (keep) [+ 4 M + 3 with
+ * icp] + 1 (choose).  The Python default D = 4 (Engine.init_boxes) is a starting guess, like the other init defaults. */
+int se3tn_init_boxes(se3tn_ctx* ctx, const uint16_t* frame_depth, int H, int W, const double* K,
+                     const int32_t* boxes, int depths, const double* object_width, int render_mode, int render_H, int render_W,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
+                     double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream);
+
 /* ---- re-initialisation: a start from the mask replaces a track the fit check finds lost ------------------------------ */
 
 /* Three calls connect the fit check (se3tn_track_opts.fit_tau_mm) to se3tn_init_poses.  Engine.reinit runs them after a

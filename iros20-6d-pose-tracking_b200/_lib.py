@@ -64,6 +64,7 @@ SIGNATURES = {
                                      _vp]),
     'se3tn_draw_hypotheses': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     'se3tn_init_poses': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    'se3tn_init_boxes': (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_lost_tracks': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     'se3tn_fit_poses': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     'se3tn_accept_starts': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),

@@ -7,14 +7,18 @@
 //   only: the statistics are exact and do not depend on the order of the reduction.  status 1: mask = 0; 2: depth_px <
 //   min_pixels.  t0 = z_med / 1000 * ((u - cx) / fx, (v - cy) / fy, 1), (u, v) = (sum_u, sum_v) / mask, in fp64; an object
 //   with status != 0 gets the placeholder t0 = (0, 0, 1), which keeps every later launch on finite poses.
-// grid_kernel: candidate c = v R + r.  d_v = (sqrt(1 - z^2) cos phi, sqrt(1 - z^2) sin phi, z), z = 1 - (2 v + 1) / V,
+// box_pass_kernel (se3tn_init_boxes): the same statistics over the pixels of object i's half-open box (x0, y0, x1, y1)
+//   instead of seg == l_i, one grid slice per object.  mask_finish_kernel then also takes D depth candidates z_d = the sorted
+//   depth at index max(0, floor(((2 d + 1) depth_px - D) / (2 D))), d < D, with t0_d = z_d / 1000 K^-1 (u, v, 1): t0 is
+//   [n][D][3]; D = 1 is the lower median, the mask call's t0.
+// grid_kernel: candidate c = d V R + v R + r (d = 0 with a mask).  d_v = (sqrt(1 - z^2) cos phi, sqrt(1 - z^2) sin phi, z), z = 1 - (2 v + 1) / V,
 //   phi = v pi (3 - sqrt 5): a Fibonacci-sphere direction in the object frame.  The camera axes in object coordinates are
 //   z_c = -d_v, x_c = (z_c x up) / |z_c x up|, y_c = z_c x x_c with up = +z (+y when |d_v.z| > 0.99), so R_c = [x_c; y_c; z_c]
 //   maps d_v to the camera's -z axis; the candidate turns that about the camera's z axis by th = 2 pi r / R:
-//   rows (cos th x_c - sin th y_c, sin th x_c + cos th y_c, z_c).  Translation t0.  fp64, restated in oracle/init_ref.py.
+//   rows (cos th x_c - sin th y_c, sin th x_c + cos th y_c, z_c).  Translation t0_d.  fp64, restated in oracle/init_ref.py.
 // score_kernel: one 4-CTA cluster per rendered row, as fit_kernel: the crop window of the row's pose (bbox_window, cv2's
 //   nearest source index, 0 outside the frame) gives the observed depth O and the mask M = (seg == l_i) under each of the
-//   176 x 176 pixels of the rendered depth R.  model #(R>0), maskc #M, overlap #(R>0, M), pairs #(R>0, M, O>0) and
+//   176 x 176 pixels of the rendered depth R (with boxes, M = the source pixel lies in object i's box).  model #(R>0), maskc #M, overlap #(R>0, M), pairs #(R>0, M, O>0) and
 //   S = sum (O - R) over the pairs; after a cluster barrier delta = floor((2 S + pairs) / (2 pairs)) mm (0 without pairs,
 //   or when the row is scored where it is), then inlier #(R>0, M, O>0, |O - (R + delta)| <= tau).
 // keep_kernel: per object, the K best rows in rank order; the kept grid pose moves along its ray: t = t0 (1 + delta / (1000 t0_z)).
@@ -68,13 +72,47 @@ __global__ void __launch_bounds__(kMaskThreads) mask_pass_kernel(const MaskArgs 
         if (s_acc[k]) atomicAdd(a.acc + k, s_acc[k]);
 }
 
+// se3tn_init_boxes: blockIdx.y is the object, the x CTAs stride over its own box's pixels only (the same accumulators and
+// histogram as mask_pass_kernel)
+__global__ void __launch_bounds__(kMaskThreads) box_pass_kernel(const MaskArgs a)
+{
+    __shared__ unsigned long long s_acc[kInitAcc];
+    const int i = blockIdx.y;
+    const int x0 = a.boxes[4 * i], y0 = a.boxes[4 * i + 1], x1 = a.boxes[4 * i + 2], y1 = a.boxes[4 * i + 3];
+    if (threadIdx.x < kInitAcc) s_acc[threadIdx.x] = 0;
+    __syncthreads();
+    const long long bw = x1 - x0, total = bw * (y1 - y0);
+    unsigned* hist = a.hist + static_cast<size_t>(i) * kInitBins;
+    unsigned long long own[kInitAcc] = {0, 0, 0, 0};        // integer sums: exact in any order
+    for (long long p = blockIdx.x * static_cast<long long>(kMaskThreads) + threadIdx.x; p < total; p += static_cast<long long>(gridDim.x) * kMaskThreads) {
+        const long long v = y0 + p / bw, u = x0 + p % bw;
+        const int d = a.depth[v * a.W + u];
+        ++own[0]; own[2] += u; own[3] += v;
+        if (d > 0) {
+            ++own[1];
+            atomicAdd(hist + d, 1u);
+        }
+    }
+    for (int k = 0; k < kInitAcc; ++k)
+        if (own[k]) atomicAdd(s_acc + k, own[k]);
+    __syncthreads();
+    if (threadIdx.x < kInitAcc && s_acc[threadIdx.x]) atomicAdd(a.acc + i * kInitAcc + threadIdx.x, s_acc[threadIdx.x]);
+}
+
 constexpr int kFinishThreads = 1024, kBinsPerThread = kInitBins / kFinishThreads;
 static_assert(kInitBins % kFinishThreads == 0, "whole bins per thread");
+
+// The sorted index of depth candidate d of D among depth_px depths: the quantile (2 d + 1) / 2 D, floored and clamped at 0.
+// D = 1 gives the lower median (depth_px - 1) / 2.
+__device__ __forceinline__ unsigned long long quantile_index(int d, int D, unsigned long long depth_px) {
+    const long long num = static_cast<long long>(2 * d + 1) * static_cast<long long>(depth_px) - D;
+    return num < 0 ? 0ull : static_cast<unsigned long long>(num / (2 * D));
+}
 
 __global__ void __launch_bounds__(kFinishThreads) mask_finish_kernel(const MaskArgs a)
 {
     __shared__ unsigned s_scan[kFinishThreads];
-    __shared__ int s_med;
+    __shared__ int s_z[1 + kInitMaxDepths];                  // the lower median, then the D depth candidates
     const int i = blockIdx.x, t = threadIdx.x;
     const unsigned long long* acc = a.acc + i * kInitAcc;
     const unsigned long long mask = acc[0], depth_px = acc[1];
@@ -82,7 +120,7 @@ __global__ void __launch_bounds__(kFinishThreads) mask_finish_kernel(const MaskA
     unsigned own = 0;
     for (int b = 0; b < kBinsPerThread; ++b) own += h[b];
     s_scan[t] = own;
-    if (t == 0) s_med = 0;
+    if (t <= a.D) s_z[t] = 0;
     __syncthreads();
     for (int off = 1; off < kFinishThreads; off <<= 1) {     // inclusive Hillis-Steele scan
         const unsigned x = t >= off ? s_scan[t - off] : 0u;
@@ -91,13 +129,14 @@ __global__ void __launch_bounds__(kFinishThreads) mask_finish_kernel(const MaskA
         __syncthreads();
     }
     if (depth_px > 0) {
-        const unsigned long long k = (depth_px - 1) / 2;     // the lower median's sorted index
         const unsigned long long hi = s_scan[t], lo = hi - own;
-        if (k >= lo && k < hi) {
+        for (int q = 0; q <= a.D; ++q) {
+            const unsigned long long k = q == 0 ? (depth_px - 1) / 2 : quantile_index(q - 1, a.D, depth_px);   // sorted index
+            if (k < lo || k >= hi) continue;
             unsigned long long c = lo;
             for (int b = 0; b < kBinsPerThread; ++b) {
                 c += h[b];
-                if (k < c) { s_med = t * kBinsPerThread + b; break; }
+                if (k < c) { s_z[q] = t * kBinsPerThread + b; break; }
             }
         }
     }
@@ -106,14 +145,17 @@ __global__ void __launch_bounds__(kFinishThreads) mask_finish_kernel(const MaskA
     const int status = mask == 0 ? 1 : (depth_px < static_cast<unsigned long long>(a.min_pixels) ? 2 : 0);
     long long* st = a.stats + i * kInitStats;
     st[0] = status; st[1] = static_cast<long long>(mask); st[2] = static_cast<long long>(depth_px);
-    st[3] = static_cast<long long>(acc[2]); st[4] = static_cast<long long>(acc[3]); st[5] = s_med;
-    double* t0 = a.t0 + 3 * i;
-    if (status) { t0[0] = 0.0; t0[1] = 0.0; t0[2] = 1.0; return; }
+    st[3] = static_cast<long long>(acc[2]); st[4] = static_cast<long long>(acc[3]); st[5] = s_z[0];
     const double m = static_cast<double>(mask);
-    const double u = static_cast<double>(acc[2]) / m, v = static_cast<double>(acc[3]) / m, z = static_cast<double>(s_med) / 1000.0;
-    t0[0] = z * ((u - a.cx) / a.fx);
-    t0[1] = z * ((v - a.cy) / a.fy);
-    t0[2] = z;
+    const double u = static_cast<double>(acc[2]) / m, v = static_cast<double>(acc[3]) / m;
+    for (int d = 0; d < a.D; ++d) {
+        double* t0 = a.t0 + 3 * (static_cast<size_t>(i) * a.D + d);
+        if (status) { t0[0] = 0.0; t0[1] = 0.0; t0[2] = 1.0; continue; }
+        const double z = static_cast<double>(s_z[1 + d]) / 1000.0;
+        t0[0] = z * ((u - a.cx) / a.fx);
+        t0[1] = z * ((v - a.cy) / a.fy);
+        t0[2] = z;
+    }
 }
 
 // ---- rotation grid ------------------------------------------------------------------------------------------------------
@@ -121,10 +163,11 @@ constexpr int kGridThreads = 128;
 
 __global__ void __launch_bounds__(kGridThreads) grid_kernel(const GridArgs a)
 {
-    const int VR = a.V * a.R;
+    const int VR = a.V * a.R, per = a.D * VR;
     const long long g = static_cast<long long>(blockIdx.x) * kGridThreads + threadIdx.x;
-    if (g >= static_cast<long long>(a.n) * VR) return;
-    const int i = static_cast<int>(g / VR), c = static_cast<int>(g - static_cast<long long>(i) * VR), v = c / a.R, r = c - v * a.R;
+    if (g >= static_cast<long long>(a.n) * per) return;
+    const int i = static_cast<int>(g / per), cd = static_cast<int>(g - static_cast<long long>(i) * per), dz = cd / VR;
+    const int c = cd - dz * VR, v = c / a.R, r = c - v * a.R;
     const double z = 1.0 - (2.0 * v + 1.0) / a.V;
     const double rad = sqrt(1.0 - z * z);
     const double phi = v * (CUDART_PI * (3.0 - sqrt(5.0)));
@@ -138,7 +181,7 @@ __global__ void __launch_bounds__(kGridThreads) grid_kernel(const GridArgs a)
     const double th = (2.0 * CUDART_PI) * r / a.R;
     const double ct = cos(th), st = sin(th);
     double* P = a.poses + 16 * g;
-    const double* t0 = a.t0 + 3 * i;
+    const double* t0 = a.t0 + 3 * (static_cast<long long>(i) * a.D + dz);
     for (int k = 0; k < 3; ++k) {
         P[k] = ct * xc[k] - st * yc[k];
         P[4 + k] = st * xc[k] + ct * yc[k];
@@ -184,7 +227,9 @@ score_kernel(const ScoreArgs a)
     // the poses come from the grid or ICP, `rendered` from the render launched right before this one: every read stays
     // behind this wait
     ptx::grid_dep_wait();
-    const int label = a.labels[obj];
+    const int label = a.boxes ? 0 : a.labels[obj];
+    const int* box = a.boxes ? a.boxes + 4 * obj : nullptr;
+    const int bx0 = box ? box[0] : 0, by0 = box ? box[1] : 0, bx1 = box ? box[2] : 0, by1 = box ? box[3] : 0;
     if (threadIdx.x == 0) {
         int top, left, ch, cw;
         bbox_window(a.poses + 16 * g, a.fx, a.fy, a.cx, a.cy, a.object_width[g], 1000.0, 1000.0, 1000.0, top, left, ch, cw);
@@ -205,11 +250,17 @@ score_kernel(const ScoreArgs a)
         if (fy < 0 || fy >= a.H || fx < 0 || fx >= a.W) return -1;
         return static_cast<long long>(fy) * a.W + fx;
     };
+    // M of frame pixel q >= 0: its label, or with boxes whether it lies in the object's box (H x W < 2^31: q fits an int)
+    auto member = [&](long long q) -> bool {
+        if (!box) return a.seg[q] == label;
+        const int fy = static_cast<int>(q) / a.W, fx = static_cast<int>(q) - fy * a.W;
+        return fx >= bx0 && fx < bx1 && fy >= by0 && fy < by1;
+    };
     int model = 0, maskc = 0, overlap = 0, pairs = 0, sum = 0;     // sum: at most 16 pixels x 65535 per thread
     for (int p = threadIdx.x; p < kScoreRows * kImg; p += kScoreThreads) {
         const int rd = R[p];
         const long long q = source(p);
-        const bool m = q >= 0 && a.seg[q] == label;
+        const bool m = q >= 0 && member(q);
         model += rd > 0; maskc += m;
         if (!(rd > 0 && m)) continue;
         ++overlap;
@@ -249,7 +300,7 @@ score_kernel(const ScoreArgs a)
         const int rd = R[p];
         if (rd == 0) continue;
         const long long q = source(p);
-        if (q < 0 || a.seg[q] != label) continue;
+        if (q < 0 || !member(q)) continue;
         const int o = a.frame_depth[q];
         if (o == 0) continue;
         const long long e = static_cast<long long>(o) - (rd + delta);
@@ -337,10 +388,17 @@ __global__ void choose_kernel(const ChooseArgs a)
 
 cudaError_t launch_mask_stats(const MaskArgs& a, cudaStream_t s) {
     if (a.n <= 0) return cudaSuccess;
-    if (!a.depth || !a.seg || !a.labels || !a.acc || !a.hist || !a.stats || !a.t0 || a.H <= 0 || a.W <= 0) return cudaErrorInvalidValue;
+    if (!a.depth || !(a.boxes || (a.seg && a.labels)) || !a.acc || !a.hist || !a.stats || !a.t0 || a.H <= 0 || a.W <= 0 ||
+        a.D < 1 || a.D > kInitMaxDepths || (!a.boxes && a.D != 1) || a.box_px_max < 0)
+        return cudaErrorInvalidValue;
     cudaError_t e = cudaMemsetAsync(a.acc, 0, sizeof(unsigned long long) * kInitAcc * a.n, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.hist, 0, sizeof(unsigned) * kInitBins * static_cast<size_t>(a.n), s);
     if (e != cudaSuccess) return e;
+    if (a.boxes) {
+        const int blocks = static_cast<int>(std::max<long long>(1, std::min<long long>(kMaskBlocks, (a.box_px_max + kMaskThreads - 1) / kMaskThreads)));
+        if ((e = launch_kernel(box_pass_kernel, dim3(blocks, a.n), dim3(kMaskThreads), 0, s, false, a)) != cudaSuccess) return e;
+        return launch_kernel(mask_finish_kernel, dim3(a.n), dim3(kFinishThreads), 0, s, false, a);
+    }
     const size_t smem = static_cast<size_t>(a.n) * (kInitAcc * sizeof(unsigned long long) + sizeof(int));
     if ((e = set_max_dynamic_smem<mask_pass_kernel>(smem)) != cudaSuccess) return e;
     const long long px = static_cast<long long>(a.H) * a.W;
@@ -350,16 +408,16 @@ cudaError_t launch_mask_stats(const MaskArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_grid(const GridArgs& a, cudaStream_t s) {
-    const long long rows = static_cast<long long>(a.n) * a.V * a.R;
+    const long long rows = static_cast<long long>(a.n) * a.D * a.V * a.R;
     if (rows <= 0) return cudaSuccess;
-    if (!a.t0 || !a.width_in || !a.poses || !a.width || (a.ids && !a.ids_in)) return cudaErrorInvalidValue;
+    if (a.D < 1 || a.D > kInitMaxDepths || !a.t0 || !a.width_in || !a.poses || !a.width || (a.ids && !a.ids_in)) return cudaErrorInvalidValue;
     return launch_kernel(grid_kernel, dim3(static_cast<unsigned>((rows + kGridThreads - 1) / kGridThreads)), dim3(kGridThreads), 0, s,
                          false, a);
 }
 
 cudaError_t launch_score(const ScoreArgs& a, int chunk_rows, cudaStream_t s) {
     if (chunk_rows <= 0) return cudaSuccess;
-    if (!a.poses || !a.object_width || !a.frame_depth || !a.seg || !a.rendered || !a.labels || !a.stats || !a.rows ||
+    if (!a.poses || !a.object_width || !a.frame_depth || !(a.boxes || (a.seg && a.labels)) || !a.rendered || !a.stats || !a.rows ||
         a.per_object <= 0 || a.tau < 1 || a.tau > 1000)
         return cudaErrorInvalidValue;
     return launch_kernel(score_kernel, dim3(kScoreCtas, chunk_rows), dim3(kScoreThreads), 0, s, true, a);

@@ -2549,17 +2549,19 @@ int se3tn_get_profile(se3tn_ctx* c, float* ms) {
 }  // extern "C"
 
 namespace {
-// se3tn_init_poses' scratch for n objects, V R candidates each and K kept: offsets into the context's init block.
+// se3tn_init_poses' and se3tn_init_boxes' scratch for n objects, D depths, D V R candidates each and K kept: offsets into the
+// context's init block.  `labels` holds the n labels or the n boxes.
 struct InitLayout {
     size_t labels, acc, hist, stats, t0, grid, width, ids, rows, depth, kept_rows, kept_poses, kept_width, kept_ids, icp_poses,
            icp_rows, icp_stats, bytes;
-    InitLayout(size_t n, size_t VR, size_t K, size_t max_batch) {
+    InitLayout(size_t n, size_t D, size_t VR, size_t K, size_t max_batch) {
         size_t o = 0;
         auto take = [&o](size_t b) { const size_t at = o; o += align256(b); return at; };
-        labels = take(n * sizeof(int32_t)); acc = take(n * kInitAcc * sizeof(unsigned long long));
-        hist = take(n * kInitBins * sizeof(unsigned)); stats = take(n * kInitStats * sizeof(long long)); t0 = take(n * 3 * sizeof(double));
-        grid = take(n * VR * 16 * sizeof(double)); width = take(n * VR * sizeof(double)); ids = take(n * VR * sizeof(int32_t));
-        rows = take(n * VR * kInitCols * sizeof(int32_t)); depth = take(max_batch * kImg * kImg * sizeof(uint16_t));
+        labels = take(n * 4 * sizeof(int32_t)); acc = take(n * kInitAcc * sizeof(unsigned long long));
+        hist = take(n * kInitBins * sizeof(unsigned)); stats = take(n * kInitStats * sizeof(long long)); t0 = take(n * D * 3 * sizeof(double));
+        const size_t cand = D * VR;
+        grid = take(n * cand * 16 * sizeof(double)); width = take(n * cand * sizeof(double)); ids = take(n * cand * sizeof(int32_t));
+        rows = take(n * cand * kInitCols * sizeof(int32_t)); depth = take(max_batch * kImg * kImg * sizeof(uint16_t));
         kept_rows = take(n * K * kInitCols * sizeof(int32_t)); kept_poses = take(n * K * 16 * sizeof(double));
         kept_width = take(n * K * sizeof(double)); kept_ids = take(n * K * sizeof(int32_t));
         icp_poses = take(n * K * 16 * sizeof(double)); icp_rows = take(n * K * kInitCols * sizeof(int32_t));
@@ -2571,8 +2573,8 @@ struct InitLayout {
 static_assert(sizeof(se3tn_init_opts) == 32, "se3tn_init_opts is 32 bytes without padding: _lib.InitOpts mirrors it");
 static_assert(kInitCols == SE3TN_INIT_COLS && kInitStats == SE3TN_INIT_STATS && kInitMaxKeep == SE3TN_MAX_INIT_KEEP, "include/se3tn.h");
 
-// opts checked for n objects (the ICP options and block by icp_opts).  Refused before anything is queued.
-int init_opts(se3tn_ctx* c, const char* fn, const se3tn_init_opts* o, int n, Step& st) {
+// opts checked for n objects and D depths (the ICP options and block by icp_opts).  Refused before anything is queued.
+int init_opts(se3tn_ctx* c, const char* fn, const se3tn_init_opts* o, int n, int D, Step& st) {
     const std::string f(fn);
     if (!o) return fail(c, SE3TN_ERR_INVALID, f + ": opts is NULL");
     auto range = [&](int v, int lo, int hi, const char* name) {
@@ -2588,7 +2590,7 @@ int init_opts(se3tn_ctx* c, const char* fn, const se3tn_init_opts* o, int n, Ste
     if (o->reserved) return fail(c, SE3TN_ERR_INVALID, f + ": opts->reserved must be 0");
     const long long VR = static_cast<long long>(o->viewpoints) * o->inplane;
     if (VR > 65536) return fail(c, SE3TN_ERR_INVALID, f + ": opts->viewpoints x opts->inplane = " + std::to_string(VR) + " exceeds 65536");
-    if (o->keep > VR) return fail(c, SE3TN_ERR_INVALID, f + ": opts->keep exceeds the " + std::to_string(VR) + " candidates");
+    if (o->keep > D * VR) return fail(c, SE3TN_ERR_INVALID, f + ": opts->keep exceeds the " + std::to_string(D * VR) + " candidates");
     if (static_cast<long long>(n) * o->keep > c->max_batch)
         return fail(c, SE3TN_ERR_INVALID, f + ": n x opts->keep = " + std::to_string(static_cast<long long>(n) * o->keep) +
                     " exceeds max_batch " + std::to_string(c->max_batch));
@@ -2596,27 +2598,35 @@ int init_opts(se3tn_ctx* c, const char* fn, const se3tn_init_opts* o, int n, Ste
     DeviceGuard guard(c->device);
     return icp_opts(c, fn, o->icp, st);
 }
-}  // namespace
 
-extern "C" {
+// Where the pixels of the n objects come from: seg == labels[i] (se3tn_init_poses) or boxes[i] (se3tn_init_boxes, D depths).
+struct InitSource {
+    const uint8_t* seg; const int32_t* labels;          // HOST labels
+    const int32_t* boxes; int D;                        // HOST (n, 4); null with a mask, and D = 1
+};
 
-int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const double* K,
-                     const int32_t* labels, const double* object_width, int render_mode, int render_H, int render_W,
-                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
-                     double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream) {
-    const char* fn = "se3tn_init_poses";
+// The stages shared by se3tn_init_poses and se3tn_init_boxes: every check first (nothing queued on a refusal), then the
+// launches.  check_object(i) checks object i's label or box.
+template <class CheckObject>
+int init_run(se3tn_ctx* c, const char* fn, const uint16_t* frame_depth, int H, int W, const double* K, const InitSource& src,
+             const double* object_width, int render_mode, int render_H, int render_W, const int32_t* weight_ids_host,
+             const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts, double* poses_out, int32_t* out_rows,
+             const se3tn_init_arrays* arrays, void* stream, CheckObject check_object) {
     const std::string f(fn);
     if (!c) return SE3TN_ERR_INVALID;
     // the mask pass counts pixels in 32 bits (mask_finish_kernel's scan): H x W stays below 2^31
-    if (!frame_depth || !seg || !K || !labels || !object_width || H <= 0 || W <= 0 || static_cast<long long>(H) * W >= (1LL << 31))
+    if (!frame_depth || !(src.boxes || (src.seg && src.labels)) || !K || !object_width || H <= 0 || W <= 0 ||
+        static_cast<long long>(H) * W >= (1LL << 31))
         return fail(c, SE3TN_ERR_INVALID, f + ": null argument or frame size out of range (H x W must be below 2^31)");
     if (!poses_out || !out_rows) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
     if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    if (src.D < 1 || src.D > kInitMaxDepths)
+        return fail(c, SE3TN_ERR_INVALID, f + ": depths is " + std::to_string(src.D) + ", not in [1, " + std::to_string(kInitMaxDepths) + "]");
     RenderSpec r;
     int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
     if (rc) return rc;
     Step st{};
-    if ((rc = init_opts(c, fn, opts, n, st))) return rc;
+    if ((rc = init_opts(c, fn, opts, n, src.D, st))) return rc;
     const se3tn_init_arrays a = arrays ? *arrays : se3tn_init_arrays{};
     const bool icp = opts->icp != nullptr;
     const struct { const void* p; const char* name; } icp_only[] = {{a.icp_poses, "icp_poses"}, {a.icp_rows, "icp_rows"}, {a.icp_stats, "icp_stats"}};
@@ -2625,32 +2635,32 @@ int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* s
     if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
         return fail(c, SE3TN_ERR_INVALID, f + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
     for (int i = 0; i < n; ++i) {
-        if (labels[i] < 1 || labels[i] > 255)
-            return fail(c, SE3TN_ERR_INVALID, f + ": labels[" + std::to_string(i) + "] is " + std::to_string(labels[i]) + ", not in [1, 255]");
+        if ((rc = check_object(i))) return rc;
         const int id = weight_ids_host ? weight_ids_host[i] : 0;
         if (!c->meshes.count(id))
             return fail(c, SE3TN_ERR_STATE, f + ": id " + std::to_string(id) + " (object " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
     }
-    const size_t nn = static_cast<size_t>(n), VR = static_cast<size_t>(opts->viewpoints) * opts->inplane, Kk = opts->keep;
-    const size_t nK = nn * Kk, px = static_cast<size_t>(H) * W;
-    rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_rows, nn * 4 * kInitCols}, {a.stats, nn * 8 * kInitStats}, {a.t0, nn * 24},
-                                {a.cand_rows, nn * VR * 4 * kInitCols}, {a.kept_rows, nK * 4 * kInitCols}, {a.kept_poses, nK * 128},
+    const size_t nn = static_cast<size_t>(n), D = static_cast<size_t>(src.D), VR = static_cast<size_t>(opts->viewpoints) * opts->inplane;
+    const size_t DVR = D * VR, Kk = opts->keep, nK = nn * Kk, px = static_cast<size_t>(H) * W;
+    rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_rows, nn * 4 * kInitCols}, {a.stats, nn * 8 * kInitStats}, {a.t0, nn * D * 24},
+                                {a.cand_rows, nn * DVR * 4 * kInitCols}, {a.kept_rows, nK * 4 * kInitCols}, {a.kept_poses, nK * 128},
                                 {a.icp_poses, nK * 128}, {a.icp_rows, nK * 4 * kInitCols}, {a.icp_stats, nK * 8 * kIcpCols}},
-                        {{frame_depth, px * 2}, {seg, px}, {object_width, nn * 8}, {weight_ids_dev, nn * 4}},
-                        "the outputs must not overlap frame_depth, seg, object_width or weight_ids_dev");
+                        {{frame_depth, px * 2}, {src.seg, src.seg ? px : 0}, {object_width, nn * 8}, {weight_ids_dev, nn * 4}},
+                        src.boxes ? "the outputs must not overlap frame_depth, object_width or weight_ids_dev"
+                                  : "the outputs must not overlap frame_depth, seg, object_width or weight_ids_dev");
     if (rc || n == 0) return rc;
 
     DeviceGuard guard(c->device);
     const cudaStream_t s = static_cast<cudaStream_t>(stream);
     if ((rc = sync_meshes(c, s))) return rc;
-    const InitLayout L(nn, VR, Kk, static_cast<size_t>(c->max_batch));
+    const InitLayout L(nn, D, VR, Kk, static_cast<size_t>(c->max_batch));
     if (L.bytes > c->init_bytes) {                       // the old block may still be read by a queued call
         CU_TRY(c, cudaStreamSynchronize(s));
         CU_TRY(c, grow(c->init, c->init_bytes, L.bytes));
     }
     uint8_t* b = c->init.get();
     auto at = [b](size_t off) { return static_cast<void*>(b + off); };
-    int32_t* d_labels = static_cast<int32_t*>(at(L.labels));
+    int32_t* d_src = static_cast<int32_t*>(at(L.labels));   // the labels or the boxes
     long long* stats = a.stats ? reinterpret_cast<long long*>(a.stats) : static_cast<long long*>(at(L.stats));
     double* t0 = a.t0 ? a.t0 : static_cast<double*>(at(L.t0));
     double* grid = static_cast<double*>(at(L.grid));
@@ -2667,17 +2677,23 @@ int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* s
     double* icp_stats = a.icp_stats ? a.icp_stats : static_cast<double*>(at(L.icp_stats));
     c->launches = 0;
 
-    // 1. mask statistics and t0
-    CU_TRY(c, cudaMemcpyAsync(d_labels, labels, nn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    // 1. mask or box statistics and t0
+    const int32_t* d_labels = src.boxes ? nullptr : d_src;
+    const int32_t* d_boxes = src.boxes ? d_src : nullptr;
+    CU_TRY(c, cudaMemcpyAsync(d_src, src.boxes ? src.boxes : src.labels, nn * (src.boxes ? 4 : 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     MaskArgs ma{};
-    ma.depth = frame_depth; ma.seg = seg; ma.H = H; ma.W = W; ma.labels = d_labels; ma.n = n;
+    ma.depth = frame_depth; ma.seg = src.seg; ma.H = H; ma.W = W; ma.labels = d_labels; ma.boxes = d_boxes; ma.D = src.D; ma.n = n;
+    for (int i = 0; src.boxes && i < n; ++i) {
+        const int32_t* bx = src.boxes + 4 * i;
+        ma.box_px_max = std::max(ma.box_px_max, static_cast<long long>(bx[2] - bx[0]) * (bx[3] - bx[1]));
+    }
     ma.acc = static_cast<unsigned long long*>(at(L.acc)); ma.hist = static_cast<unsigned*>(at(L.hist)); ma.min_pixels = opts->min_pixels;
     ma.fx = K[0]; ma.fy = K[1]; ma.cx = K[2]; ma.cy = K[3]; ma.stats = stats; ma.t0 = t0;
     CU_TRY(c, launch_mask_stats(ma, s));
     c->launches += 2;
-    // 2. the rotation grid at t0
+    // 2. the rotation grid at each t0_d
     GridArgs ga{};
-    ga.n = n; ga.V = opts->viewpoints; ga.R = opts->inplane; ga.t0 = t0; ga.width_in = object_width; ga.ids_in = weight_ids_dev;
+    ga.n = n; ga.V = opts->viewpoints; ga.R = opts->inplane; ga.D = src.D; ga.t0 = t0; ga.width_in = object_width; ga.ids_in = weight_ids_dev;
     ga.poses = grid; ga.width = gwidth; ga.ids = gids;
     CU_TRY(c, launch_grid(ga, s));
     ++c->launches;
@@ -2685,20 +2701,20 @@ int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* s
     // depth it overwrites
     ScoreArgs sa{};
     sa.object_width = gwidth; sa.fx = K[0]; sa.fy = K[1]; sa.cx = K[2]; sa.cy = K[3];
-    sa.frame_depth = frame_depth; sa.seg = seg; sa.H = H; sa.W = W; sa.rendered = depth; sa.labels = d_labels; sa.stats = stats;
-    sa.tau = opts->tau_mm;
-    const size_t total = nn * VR;
+    sa.frame_depth = frame_depth; sa.seg = src.seg; sa.H = H; sa.W = W; sa.rendered = depth; sa.labels = d_labels; sa.boxes = d_boxes;
+    sa.stats = stats; sa.tau = opts->tau_mm;
+    const size_t total = nn * DVR;
     for (size_t g0 = 0; g0 < total; g0 += c->max_batch) {
         const int m = static_cast<int>(std::min(total - g0, static_cast<size_t>(c->max_batch)));
         const RenderArgs ra = render_args(c, K, grid + 16 * g0, gwidth + g0, gids ? gids + g0 : nullptr, r.mode, r.H, r.W, nullptr, depth);
         CU_TRY(c, launch_render(ra, m, s));
-        sa.poses = grid; sa.row0 = static_cast<int>(g0); sa.per_object = static_cast<int>(VR); sa.rows = rows;
+        sa.poses = grid; sa.row0 = static_cast<int>(g0); sa.per_object = static_cast<int>(DVR); sa.rows = rows;
         CU_TRY(c, launch_score(sa, m, s));
         c->launches += 3;
     }
     // 4. keep the K best of each object
     KeepArgs ka{};
-    ka.n = n; ka.per_object = static_cast<int>(VR); ka.K = opts->keep; ka.rows = rows; ka.poses = grid; ka.width_in = object_width;
+    ka.n = n; ka.per_object = static_cast<int>(DVR); ka.K = opts->keep; ka.rows = rows; ka.poses = grid; ka.width_in = object_width;
     ka.ids_in = weight_ids_dev; ka.kept_rows = kept_rows; ka.kept_poses = kept_poses; ka.kept_width = kept_width; ka.kept_ids = kept_ids;
     CU_TRY(c, launch_keep(ka, s));
     ++c->launches;
@@ -2732,6 +2748,40 @@ int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* s
     CU_TRY(c, launch_choose(ca, s));
     ++c->launches;
     return SE3TN_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int se3tn_init_poses(se3tn_ctx* c, const uint16_t* frame_depth, const uint8_t* seg, int H, int W, const double* K,
+                     const int32_t* labels, const double* object_width, int render_mode, int render_H, int render_W,
+                     const int32_t* weight_ids_host, const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts,
+                     double* poses_out, int32_t* out_rows, const se3tn_init_arrays* arrays, void* stream) {
+    const char* fn = "se3tn_init_poses";
+    const InitSource src{seg, labels, nullptr, 1};
+    return init_run(c, fn, frame_depth, H, W, K, src, object_width, render_mode, render_H, render_W, weight_ids_host, weight_ids_dev,
+                    n, opts, poses_out, out_rows, arrays, stream, [&](int i) -> int {
+                        if (labels[i] >= 1 && labels[i] <= 255) return SE3TN_OK;
+                        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": labels[" + std::to_string(i) + "] is " +
+                                                              std::to_string(labels[i]) + ", not in [1, 255]");
+                    });
+}
+
+int se3tn_init_boxes(se3tn_ctx* c, const uint16_t* frame_depth, int H, int W, const double* K, const int32_t* boxes, int depths,
+                     const double* object_width, int render_mode, int render_H, int render_W, const int32_t* weight_ids_host,
+                     const int32_t* weight_ids_dev, int n, const se3tn_init_opts* opts, double* poses_out, int32_t* out_rows,
+                     const se3tn_init_arrays* arrays, void* stream) {
+    const char* fn = "se3tn_init_boxes";
+    const InitSource src{nullptr, nullptr, boxes, depths};
+    return init_run(c, fn, frame_depth, H, W, K, src, object_width, render_mode, render_H, render_W, weight_ids_host, weight_ids_dev,
+                    n, opts, poses_out, out_rows, arrays, stream, [&](int i) -> int {
+                        const int32_t* b = boxes + 4 * i;
+                        if (b[0] >= 0 && b[1] >= 0 && b[2] <= W && b[3] <= H && b[2] >= b[0] && b[3] >= b[1]) return SE3TN_OK;
+                        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": boxes[" + std::to_string(i) + "] = (" +
+                                    std::to_string(b[0]) + ", " + std::to_string(b[1]) + ", " + std::to_string(b[2]) + ", " +
+                                    std::to_string(b[3]) + ") is not a box inside the frame (0 <= x0 <= x1 <= W = " + std::to_string(W) +
+                                    ", 0 <= y0 <= y1 <= H = " + std::to_string(H) + ")");
+                    });
 }
 
 }  // extern "C"

@@ -539,14 +539,24 @@ class Engine:
         self._check_dev('object_width', object_width, torch.float64, (n,))
         wh = self._host_ids('init_poses', weight_ids, n)
         wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
+        out, arrays = self._init_outputs('init_poses', n, opts, None, out)
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        _lib.check(self.lib.se3tn_init_poses(self._ctx, _ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _hptr(lab),
+                                             _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
+                                             _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
+        return out['poses'], out['rows']
+
+    def _init_outputs(self, fn, n, opts, D, out):
+        """out (init_poses' / init_boxes' argument) checked against the shapes of n objects with D depths (None: a mask, t0
+        (n, 3)), 'poses' and 'rows' allocated when missing.  -> (out dict, _lib.InitArrays)."""
         out = dict(out or {})
         unknown = set(out) - {'poses', 'rows'} - set(self.INIT_ARRAYS)
         if unknown:
-            raise ValueError('init_poses: unknown outputs %s' % sorted(unknown))
+            raise ValueError('%s: unknown outputs %s' % (fn, sorted(unknown)))
         VR, Kk = opts.viewpoints * opts.inplane, opts.keep
         shapes = dict(poses=((n, 4, 4), torch.float64), rows=((n, _lib.INIT_COLS), torch.int32),
-                      stats=((n, _lib.INIT_STATS), torch.int64), t0=((n, 3), torch.float64),
-                      cand_rows=((n, VR, _lib.INIT_COLS), torch.int32), kept_rows=((n, Kk, _lib.INIT_COLS), torch.int32),
+                      stats=((n, _lib.INIT_STATS), torch.int64), t0=((n, 3) if D is None else (n, D, 3), torch.float64),
+                      cand_rows=((n, (D or 1) * VR, _lib.INIT_COLS), torch.int32), kept_rows=((n, Kk, _lib.INIT_COLS), torch.int32),
                       kept_poses=((n, Kk, 4, 4), torch.float64), icp_poses=((n, Kk, 4, 4), torch.float64),
                       icp_rows=((n, Kk, _lib.INIT_COLS), torch.int32), icp_stats=((n, Kk, _lib.ICP_COLS), torch.float64))
         for k in ('poses', 'rows'):
@@ -555,9 +565,68 @@ class Engine:
         for k, t in out.items():
             if t is not None:
                 self._check_dev('out[%r]' % k, t, shapes[k][1], shapes[k][0])
-        arrays = _lib.InitArrays(**{k: _ptr(out.get(k)).value for k in self.INIT_ARRAYS})
+        return out, _lib.InitArrays(**{k: _ptr(out.get(k)).value for k in self.INIT_ARRAYS})
+
+    # init_boxes' default depth count: a starting guess, like INIT_DEFAULTS -- the quantiles 1/8, 3/8, 5/8 and 7/8 of the box's
+    # depths, so that one of them lies on the object when the background fills up to half of the box
+    INIT_BOX_DEPTHS = 4
+    MAX_INIT_DEPTHS = 8
+    INIT_BOX_STATUS = {1: 'the box is empty', 2: 'too few box pixels have depth (min_pixels)'}
+
+    @staticmethod
+    def depths_spec(depths):
+        """init_boxes' depth candidates D checked as an integer in [1, MAX_INIT_DEPTHS] -> int."""
+        if isinstance(depths, (bool, np.bool_)) or not isinstance(depths, (int, np.integer)) or not 1 <= depths <= Engine.MAX_INIT_DEPTHS:
+            raise ValueError('init depths must be an integer in [1, %d], not %r' % (Engine.MAX_INIT_DEPTHS, depths))
+        return int(depths)
+
+    @staticmethod
+    def box_spec(boxes, depths=INIT_BOX_DEPTHS):
+        """boxes (n, 4) integers (x0, y0, x1, y1), half-open, as a contiguous int32 array, and depths_spec(depths).  Float boxes
+        are a ValueError: round a detector's box with box_pixels first."""
+        depths = Engine.depths_spec(depths)
+        b = np.asarray(boxes)
+        if b.size and (b.dtype == np.bool_ or not np.issubdtype(b.dtype, np.integer)):
+            raise ValueError('boxes must be integers (x0, y0, x1, y1), not %s' % b.dtype)
+        if b.size % 4 or (b.size and b.shape[-1] != 4):
+            raise ValueError('boxes must be (n, 4), not %s' % (b.shape,))
+        if b.size and (b.min() < -2 ** 31 or b.max() >= 2 ** 31):
+            raise ValueError('boxes must fit int32')
+        return np.ascontiguousarray(b, dtype=np.int32).reshape(-1, 4), int(depths)
+
+    @staticmethod
+    def box_pixels(box, H, W):
+        """A detector's (x0, y0, x1, y1) in frame pixels, floats allowed, as the half-open integer box init_boxes takes: rounded
+        outwards (floor x0 / y0, ceil x1 / y1) and clipped to the H x W frame.  Non-finite values are a ValueError."""
+        b = np.asarray(box, dtype=np.float64).reshape(-1)
+        if b.shape != (4,) or not np.isfinite(b).all():
+            raise ValueError('box must be four finite numbers (x0, y0, x1, y1), not %r' % (box,))
+        x0, y0 = np.floor(b[0]), np.floor(b[1])
+        x1, y1 = np.ceil(b[2]), np.ceil(b[3])
+        clip = lambda v, hi: int(min(max(v, 0), hi))
+        x0, x1, y0, y1 = clip(x0, W), clip(x1, W), clip(y0, H), clip(y1, H)
+        return np.array([x0, y0, max(x0, x1), max(y0, y1)], np.int32)
+
+    def init_boxes(self, frame_depth, boxes, K, object_width, weight_ids=None, mode='vispy', image_hw=None, init=None,
+                   depths=INIT_BOX_DEPTHS, out=None):
+        """Start poses for n objects of one frame from 2D boxes and the depth (se3tn_init_boxes): init_poses' rule with each
+        object's pixels the box's, D = depths depth candidates along the ray through the box centre (the quantiles
+        (2 d + 1) / 2 D of the box's depths), and the D V R candidates of an object ranked together.  frame_depth uint16 (H,W)
+        mm CUDA tensor; boxes (n, 4) ints (x0, y0, x1, y1), half-open, inside the frame, may overlap; depths in [1,
+        MAX_INIT_DEPTHS]; the rest as init_poses.  out as init_poses', with t0 (n, D, 3) and cand_rows (n, D V R, INIT_COLS);
+        column 1 of a row is the candidate d V R + v R + r.  -> (poses float64 (n,4,4), NaN where the status is not 0 -- 1: the
+        box is empty, 2: too few of its pixels have depth --, rows int32 (n, INIT_COLS)), queued on the current stream."""
+        opts = self.init_spec(init)
+        b, D = self.box_spec(boxes, depths)
+        n = int(b.shape[0])
+        H, W = frame_depth.shape
+        self._check_dev('frame_depth', frame_depth, torch.uint16, (H, W))
+        self._check_dev('object_width', object_width, torch.float64, (n,))
+        wh = self._host_ids('init_boxes', weight_ids, n)
+        wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
+        out, arrays = self._init_outputs('init_boxes', n, opts, D, out)
         rmode, rH, rW = self._render_mode(mode, image_hw)
-        _lib.check(self.lib.se3tn_init_poses(self._ctx, _ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _hptr(lab),
+        _lib.check(self.lib.se3tn_init_boxes(self._ctx, _ptr(frame_depth), int(H), int(W), _hptr(self._k4(K)), _hptr(b), D,
                                              _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
                                              _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
         return out['poses'], out['rows']
@@ -641,7 +710,7 @@ class Engine:
                                                 n, _ptr(poses), _ptr(fit_rows), _ptr(streak), _ptr(event), _stream(self.device)), self._ctx)
 
     def reinit(self, frame_depth, seg, K, labels, object_width, poses, fit_rows, streak, fit, below=0.5, after=3, weight_ids=None,
-               mode='vispy', image_hw=None, init=None, fill_depth=None):
+               mode='vispy', image_hw=None, init=None, fill_depth=None, boxes=None, depths=INIT_BOX_DEPTHS):
         """Re-initialise the lost tracks of one tracking step from their masks (include/se3tn.h): the loss rule over the step's
         fit rows (lost_tracks), the lost list copied back through pinned memory (one synchronisation of the current stream,
         the call's only one), then, when some track is lost and seg is given, one init_poses call on the lost tracks in
@@ -651,14 +720,22 @@ class Engine:
         mm and seg uint8 (H,W) label image (or None: no attempt) are CUDA tensors or numpy arrays, uploaded only when a track is
         lost; fill_depth as in track_render: the depth is filled first, as the step filled it.  labels (n) ints in 1..255,
         object_width float64 CUDA (n), weight_ids int32 (n) host array or None (mesh 0), mode / image_hw as in render(): the
-        step's.  fit: the step's tau in mm; init: init_spec's argument.  -> event int32 (n) CUDA tensor: 0 not below, 1 below and
-        no attempt, 2 restarted, 3 no start, 4 start rejected."""
+        step's.  fit: the step's tau in mm; init: init_spec's argument.  boxes: instead of seg (at most one of the two), each
+        track's (x0, y0, x1, y1) box in this frame, ints (n, 4) as init_boxes takes them; the lost tracks' rows go through one
+        init_boxes call with `depths`, and labels may be None.  -> event int32 (n) CUDA tensor: 0 not below, 1 below and no
+        attempt, 2 restarted, 3 no start, 4 start rejected."""
         tau = self.fit_spec(fit)
         if not tau:
             raise ValueError('reinit: fit must be the step\'s tau in mm, not %r' % (fit,))
         n = int(poses.shape[0])
-        lab = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
-        if lab.shape != (n,):
+        if seg is not None and boxes is not None:
+            raise ValueError('reinit: give seg or boxes, not both')
+        if boxes is not None:
+            box, depths = self.box_spec(boxes, depths)
+            if box.shape != (n, 4):
+                raise ValueError('reinit: %d boxes for %d tracks' % (box.shape[0], n))
+        lab = None if boxes is not None and labels is None else np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+        if lab is not None and lab.shape != (n,):
             raise ValueError('reinit: %d labels for %d tracks' % (lab.shape[0], n))
         wh = self._host_ids('reinit', weight_ids, n)
         event, lost = self.lost_tracks(fit_rows, streak, below, after)
@@ -668,17 +745,22 @@ class Engine:
         pin[:n + 1].copy_(lost, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
         m = int(pin[0])
-        if m == 0 or seg is None:
+        if m == 0 or (seg is None and boxes is None):
             return event
         idx = pin[1:1 + m].numpy().copy()
         as_dev = lambda a, dt: a.to(self.device, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
-        depth_d, seg_d = as_dev(frame_depth, torch.uint16), as_dev(seg, torch.uint8)
+        depth_d = as_dev(frame_depth, torch.uint16)
         on, max_depth, extrapolate, blur = self.depth_fill_spec(fill_depth)
         if on:
             depth_d = self.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
         sub_ids = None if wh is None else wh[idx]
         width = object_width.index_select(0, lost[1:1 + m].long())
-        starts, init_rows = self.init_poses(depth_d, seg_d, K, lab[idx], width, weight_ids=sub_ids, mode=mode, image_hw=image_hw, init=init)
+        if boxes is not None:
+            starts, init_rows = self.init_boxes(depth_d, box[idx], K, width, weight_ids=sub_ids, mode=mode, image_hw=image_hw, init=init,
+                                                depths=depths)
+        else:
+            starts, init_rows = self.init_poses(depth_d, as_dev(seg, torch.uint8), K, lab[idx], width, weight_ids=sub_ids, mode=mode,
+                                                image_hw=image_hw, init=init)
         start_fit = self.fit_poses(depth_d, K, starts, width, tau, weight_ids=sub_ids, mode=mode, image_hw=image_hw)
         self.accept_starts(idx, starts, init_rows, start_fit, poses, fit_rows, streak, event)
         return event

@@ -386,13 +386,18 @@ class Tracker:
         return r
 
     # ------------------------------------------------------------------ a start without a pose
-    def initialize(self, depth, mask, label=1, **init):
-        """The start pose of this Tracker's object from its mask and the depth frame (Engine.init_poses), with the Tracker's
-        mesh, width and render mode.  depth: uint16 (H,W) mm, numpy or CUDA; mask: a bool (H,W) array (the object's pixels) or a
-        uint8 label image in which the object's pixels are `label`.  init: Engine.init_spec's fields.  A Tracker built with
-        fill_depth fills the depth first with the same settings, so the start is scored on the depth its steps see.  -> the 4x4
-        float64 start on_track takes; the kept score row (status, candidate, model, maskc, overlap, pairs, inlier, delta_mm) is
-        left in last_init.  A ValueError names the status when there is no start (an empty mask, too few pixels with depth)."""
+    def initialize(self, depth, mask=None, label=1, box=None, depths=Engine.INIT_BOX_DEPTHS, **init):
+        """The start pose of this Tracker's object from its mask or its 2D box and the depth frame (Engine.init_poses /
+        Engine.init_boxes), with the Tracker's mesh, width and render mode.  Exactly one of mask and box.  depth: uint16 (H,W)
+        mm, numpy or CUDA; mask: a bool (H,W) array (the object's pixels) or a uint8 label image in which the object's pixels
+        are `label`; box: a detector's (x0, y0, x1, y1) in frame pixels, floats allowed, rounded outwards (floor x0 / y0, ceil
+        x1 / y1) and clipped to the frame (Engine.box_pixels); depths: init_boxes' depth candidates.  init: Engine.init_spec's
+        fields.  A Tracker built with fill_depth fills the depth first with the same settings, so the start is scored on the
+        depth its steps see.  -> the 4x4 float64 start on_track takes; the kept score row (status, candidate, model, maskc,
+        overlap, pairs, inlier, delta_mm) is left in last_init.  A ValueError names the status when there is no start (an
+        empty mask or box, too few pixels with depth)."""
+        if (mask is None) == (box is None):
+            raise ValueError('initialize: give exactly one of mask and box')
         r = self._fused_renderer()
         if r is None:
             raise ValueError('initialize draws the model on the device: it needs the CUDA renderer (renderer="cuda") on this '
@@ -400,40 +405,52 @@ class Tracker:
         dev = self.engine.device
         as_dev = lambda a, dt: a.to(dev, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
         depth_d = as_dev(depth, np.uint16 if not torch.is_tensor(depth) else torch.uint16)
-        m = mask if torch.is_tensor(mask) else np.asarray(mask)
-        if torch.is_tensor(m) and m.dtype == torch.bool:
-            seg = m.to(dev).to(torch.uint8).contiguous() * int(label)
-        elif not torch.is_tensor(m) and m.dtype == np.bool_:
-            seg = torch.from_numpy(np.where(m, np.uint8(label), np.uint8(0))).to(dev)
+        if box is not None:
+            b = Engine.box_pixels(box, *depth_d.shape)
+            Engine.depths_spec(depths)
         else:
-            size = m.numel() if torch.is_tensor(m) else m.size
-            lo, hi = (int(m.min()), int(m.max())) if size else (0, 0)
-            if lo < 0 or hi > 255:
-                raise ValueError('initialize: a label image holds labels 0..255, not %d..%d' % (lo, hi))
-            seg = as_dev(m, np.uint8 if not torch.is_tensor(m) else torch.uint8)
-        if tuple(seg.shape) != tuple(depth_d.shape):
-            raise ValueError('initialize: mask %s and depth %s differ in shape' % (tuple(seg.shape), tuple(depth_d.shape)))
+            m = mask if torch.is_tensor(mask) else np.asarray(mask)
+            if torch.is_tensor(m) and m.dtype == torch.bool:
+                seg = m.to(dev).to(torch.uint8).contiguous() * int(label)
+            elif not torch.is_tensor(m) and m.dtype == np.bool_:
+                seg = torch.from_numpy(np.where(m, np.uint8(label), np.uint8(0))).to(dev)
+            else:
+                size = m.numel() if torch.is_tensor(m) else m.size
+                lo, hi = (int(m.min()), int(m.max())) if size else (0, 0)
+                if lo < 0 or hi > 255:
+                    raise ValueError('initialize: a label image holds labels 0..255, not %d..%d' % (lo, hi))
+                seg = as_dev(m, np.uint8 if not torch.is_tensor(m) else torch.uint8)
+            if tuple(seg.shape) != tuple(depth_d.shape):
+                raise ValueError('initialize: mask %s and depth %s differ in shape' % (tuple(seg.shape), tuple(depth_d.shape)))
         on, max_depth, extrapolate, blur = Engine.depth_fill_spec(self.fill_depth)
         if on:
             depth_d = self.engine.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
         width = torch.full((1,), float(self.object_width), dtype=torch.float64, device=dev)
-        poses, rows = self.engine.init_poses(depth_d, seg, self.K, [int(label)], width,
-                                             weight_ids=None if r.mesh_id == 0 else [r.mesh_id], mode=r.mode, image_hw=r.image_hw,
-                                             init=init or None)
+        common = dict(weight_ids=None if r.mesh_id == 0 else [r.mesh_id], mode=r.mode, image_hw=r.image_hw, init=init or None)
+        if box is not None:
+            poses, rows = self.engine.init_boxes(depth_d, b[None], self.K, width, depths=depths, **common)
+        else:
+            poses, rows = self.engine.init_poses(depth_d, seg, self.K, [int(label)], width, **common)
         self.last_init = rows[0].cpu().numpy()
         status = int(self.last_init[0])
         if status:
+            if box is not None:
+                raise ValueError('initialize: no start for box %s: %s (status %d)' % (tuple(int(x) for x in b),
+                                 Engine.INIT_BOX_STATUS.get(status, '?'), status))
             raise ValueError('initialize: no start for label %d: %s (status %d)' % (label, Engine.INIT_STATUS.get(status, '?'), status))
         return poses[0].cpu().numpy()
 
     # ------------------------------------------------------------------ the hot path
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
-                 rgbA=None, depthA=None, show=False, mask=None, label=1):
+                 rgbA=None, depthA=None, show=False, mask=None, label=1, box=None):
         """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose.  Without rgbA / depthA and with the
         CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host), and refined
         Tracker.iterations times.  mask: with reinit, the object's pixels of this frame, a bool (H,W) array or a uint8 label
-        image in which they are `label`; read only when the track is lost."""
+        image in which they are `label`; read only when the track is lost.  box: with reinit, instead of mask, the object's
+        (x0, y0, x1, y1) box in this frame (Tracker.initialize's rounding): a lost track restarts from it (Engine.init_boxes)."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
+        if mask is not None and box is not None:
+            raise ValueError('on_track: give mask or box, not both')
         seg = None
         if mask is not None:
             m = mask.cpu().numpy() if torch.is_tensor(mask) else np.asarray(mask)
@@ -441,6 +458,8 @@ class Tracker:
                 raise ValueError('on_track: mask must be a bool mask or a uint8 label image, not %s' % m.dtype)
             seg = np.where(m, np.uint8(label), np.uint8(0)) if m.dtype == np.bool_ else m
         kw = {} if self.reinit is None else dict(seg=seg, labels=[int(label)])
+        if self.reinit is not None and box is not None:
+            kw = dict(boxes=Engine.box_pixels(box, *np.shape(current_depth)[:2])[None])
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
         if not fused:
             self._check_step_draws(rgbA is not None or depthA is not None)
@@ -464,7 +483,7 @@ class Tracker:
         return final_estimate
 
     def on_track_batch(self, prev_poses, current_rgb, current_depth, rgbA=None, depthA=None, weight_ids=None, object_width=None,
-                       seg=None, labels=None):
+                       seg=None, labels=None, boxes=None):
         """N independent tracks of ONE frame -> (N,4,4) float64.  rgbA / depthA None: rendered on the device by the CUDA
         rasteriser (needs a CudaRenderer; per-track models follow weight_ids), inside the tracking step when the renderer
         allows it (_fused_renderer).  The types of the inputs pick one of two routes:
@@ -479,10 +498,18 @@ class Tracker:
         A pageable input may be overwritten as soon as the call returns.  A pinned CPU tensor is read asynchronously: it must
         stay unchanged until the current stream has run this call's step.
         seg / labels: with reinit, the frame's uint8 (H,W) label image (numpy or a tensor) and each track's label in it (ints
-        in 1..255; None with one track: 1), read only when a track is lost (_reinit).  Without seg no track is restarted."""
+        in 1..255; None with one track: 1), read only when a track is lost (_reinit).  boxes: instead of seg / labels, each
+        track's (x0, y0, x1, y1) box in this frame, ints (n, 4) (Engine.init_boxes).  Without seg or boxes no track is
+        restarted."""
         if self.reinit is None:
             return self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
         n = len(prev_poses)
+        if boxes is not None:
+            if seg is not None or labels is not None:
+                raise ValueError('on_track_batch: give seg / labels or boxes, not both')
+            box, _ = Engine.box_spec(boxes, Engine.INIT_BOX_DEPTHS)
+            if box.shape != (n, 4):
+                raise ValueError('on_track_batch: boxes must be (%d, 4), not %s' % (n, box.shape))
         if labels is None and seg is not None and n != 1:
             raise ValueError('on_track_batch: seg needs labels, one per track')
         lab = np.ascontiguousarray([1] * n if labels is None else labels, dtype=np.int64).reshape(-1)
@@ -495,13 +522,13 @@ class Tracker:
                              % (n, reinit_keep(self.opts), self.engine.max_batch))
         self.last_reinit = None
         out = self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
-        return self._reinit(out, current_depth, seg, lab, weight_ids, object_width)
+        return self._reinit(out, current_depth, seg, lab, weight_ids, object_width, None if boxes is None else box)
 
     def reset_reinit(self):
         """Start every track's streak of frames below the fit threshold from 0 (reinit), as at a new sequence."""
         self._streak = None
 
-    def _reinit(self, out, depth, seg, labels, weight_ids, object_width):
+    def _reinit(self, out, depth, seg, labels, weight_ids, object_width, boxes=None):
         """Engine.reinit after the step that gave `out` (a CUDA tensor, updated in place, or numpy, uploaded and brought back)
         and last_fit, on the raw frame depth (filled as the step fills it), with the step's meshes, widths and render mode."""
         dev, n = self.engine.device, len(out)
@@ -515,7 +542,7 @@ class Tracker:
         r = self.renderer
         event = self.engine.reinit(depth, seg, self.K, labels, ow, poses, rows, self._streak, self.opts.tau, self.reinit['below'],
                                    self.reinit['after'], weight_ids=self._weight_ids(weight_ids, n), mode=r.mode, image_hw=r.image_hw,
-                                   init=self.reinit['init'], fill_depth=self.fill_depth)
+                                   init=self.reinit['init'], fill_depth=self.fill_depth, boxes=boxes)
         if not on_host:
             self.last_reinit = event
             return out
@@ -1829,17 +1856,44 @@ class MaskStarts:
         widths = torch.tensor([self.width[int(c)] for c in cls], dtype=torch.float64, device=dev)
         return self.eng.init_poses(as_dev(depth), as_dev(seg), self.K, ids, widths, weight_ids=ids, init=self.init, out=out, **self.render)
 
+    def from_boxes(self, depth, seg, cls, depths=None, out=None):
+        """One init_boxes call for the classes cls of one frame, each class's box the tight box of its pixels in the uint8
+        label image seg (label_boxes: what a perfect detector gives; no pixels, an empty box and status 1) -> as __call__
+        (Engine.init_boxes with `depths`, None: Engine.INIT_BOX_DEPTHS)."""
+        dev = self.eng.device
+        ids = np.asarray(cls, dtype=np.int32)
+        widths = torch.tensor([self.width[int(c)] for c in cls], dtype=torch.float64, device=dev)
+        seg = seg.cpu().numpy() if torch.is_tensor(seg) else np.asarray(seg)
+        depth = depth if torch.is_tensor(depth) else torch.from_numpy(np.ascontiguousarray(depth)).to(dev)
+        return self.eng.init_boxes(depth, label_boxes(seg, cls), self.K, widths, weight_ids=ids, init=self.init, out=out,
+                                   depths=Engine.INIT_BOX_DEPTHS if depths is None else depths, **self.render)
+
     def close(self):
         self.eng.close()
 
 
-def _mask_start_refusal(seq, c, name, status):
-    return ValueError('sequence %04d, class %d (%s): no start from its mask in the first frame: %s (status %d)'
-                      % (seq, c, name, Engine.INIT_STATUS.get(int(status), '?'), int(status)))
+def label_boxes(seg, labels):
+    """The tight half-open box (min u, min v, max u + 1, max v + 1) of each label's pixels in a uint8 label image, (0, 0, 0, 0)
+    for a label without pixels -> int32 (n, 4)."""
+    seg = np.asarray(seg)
+    out = np.zeros((len(labels), 4), np.int32)
+    for j, c in enumerate(labels):
+        m = seg == int(c)
+        rows, cols = np.flatnonzero(m.any(axis=1)), np.flatnonzero(m.any(axis=0))
+        if len(rows):
+            out[j] = (cols[0], rows[0], cols[-1] + 1, rows[-1] + 1)
+    return out
+
+
+def _mask_start_refusal(seq, c, name, status, source='mask'):
+    return ValueError('sequence %04d, class %d (%s): no start from its %s in the first frame: %s (status %d)'
+                      % (seq, c, name, source, (Engine.INIT_BOX_STATUS if source == 'box' else Engine.INIT_STATUS).get(int(status), '?'),
+                         int(status)))
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
-                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None, init=None, reinit=None):
+                     video=False, iterations=1, gpus=1, fit=None, hypotheses=1, seed=0, icp=0, icp_tau=None, init=None, reinit=None,
+                     depths=None):
     """getResultsYcb for every class of `class_ids` in one pass -> {class_id: {seq_id: poses}}, and the files each per-class run
     writes, under <outdir>/<class folder>/run/ (see ycb_all_classes for class_config and the refusals).
 
@@ -1893,7 +1947,11 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     initialize_method='mask': each sequence's tracks start from one Engine.init_poses call on its first frame (depth_filled and
     seg/ label image; each class's label is its class id; init: Engine.init_spec's argument), made in this process before any
     tracking, so several GPUs write the one-GPU trees.  A class the call finds no start for (an empty mask, too few pixels with
-    depth) is a ValueError naming the sequence and the class.  init without 'mask' is a ValueError.
+    depth) is a ValueError naming the sequence and the class.  init without 'mask' or 'box' is a ValueError.
+
+    initialize_method='box': as 'mask', with one Engine.init_boxes call (depths: its D, None the default) whose boxes are each
+    class's tight box in that label image (label_boxes), a perfect detector's boxes; a class without pixels has an empty box
+    and no start.  depths without 'box' is a ValueError.
 
     reinit: None off, or {'below': f, 'after': L, 'init': Engine.init_spec's argument} (reinit_options): after every step, the
     tracks whose inlier fraction stayed below f for L frames in a row are restarted from that frame's seg/%06d-label.png (the
@@ -1903,14 +1961,18 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
     It turns the fit check on at FIT_TAU_DEFAULT when fit is not given; the Engine then holds n_max x init keep tracks (the
     steps' split-K regime depends on n alone, so their bits do not move).  Every tracked frame's label image must exist: a
     missing one is a FileNotFoundError before anything is loaded.  Several GPUs write the one-GPU trees."""
-    if init is not None and initialize_method != 'mask':
-        raise ValueError("init options need initialize_method='mask', not %r" % (initialize_method,))
-    if initialize_method == 'mask':
+    if init is not None and initialize_method not in ('mask', 'box'):
+        raise ValueError("init options need initialize_method='mask' or 'box', not %r" % (initialize_method,))
+    if depths is not None and initialize_method != 'box':
+        raise ValueError("depths needs initialize_method='box', not %r" % (initialize_method,))
+    if initialize_method in ('mask', 'box'):
         Engine.init_spec(init)
+    if initialize_method == 'box':
+        Engine.depths_spec(Engine.INIT_BOX_DEPTHS if depths is None else depths)
     run = _one_pass_front(outdir, gpus, precision, YCB_ALL_PRECISIONS, video, iterations, class_config, fit=fit,
                           hypotheses=hypotheses, seed=seed, icp=icp, icp_tau=icp_tau, reinit=reinit)
-    if initialize_method not in ('gt', 'posecnn', 'poserbpf', 'mask'):
-        raise ValueError('initialize_method must be gt, posecnn, poserbpf or mask')
+    if initialize_method not in ('gt', 'posecnn', 'poserbpf', 'mask', 'box'):
+        raise ValueError('initialize_method must be gt, posecnn, poserbpf, mask or box')
     _check_checkpoint_ids([c for c, _ in ycb_classes(ycb_dir, class_ids)], len(run.configs), 'class')
     per_ckpt = [ycb_all_classes(ycb_dir, class_ids, cfg, run.precision) for cfg in run.configs]
     classes = per_ckpt[0]
@@ -1926,7 +1988,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
             if missing:
                 raise FileNotFoundError('reinit: %d tracked frames of sequence %04d have no label image, the first %s'
                                         % (len(missing), seq_id, missing[0]))
-    starts = MaskStarts(classes, max([len(v) for v in track_sets.values()] + [1]), init) if initialize_method == 'mask' else None
+    starts = MaskStarts(classes, max([len(v) for v in track_sets.values()] + [1]), init) if initialize_method in ('mask', 'box') else None
     try:
         for seq_id, cls in track_sets.items():
             files = {c: _ycb_sequence_files(os.path.join(data_dir, '%04d' % seq_id), c) for c in cls}
@@ -1936,12 +1998,16 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                 import glob
                 segs = sorted(glob.glob(os.path.join(data_dir, '%04d' % seq_id, 'seg', '*')))
                 if not segs:
-                    raise FileNotFoundError('--init mask: no seg/ label image under %s' % os.path.join(data_dir, '%04d' % seq_id))
-                P, rows = starts(read_depth(depth_files[0]), read_seg(segs[0]), cls)
+                    raise FileNotFoundError('--init %s: no seg/ label image under %s' % (initialize_method, os.path.join(data_dir, '%04d' % seq_id)))
+                if initialize_method == 'box':
+                    P, rows = starts.from_boxes(read_depth(depth_files[0]), read_seg(segs[0]), cls, depths)
+                else:
+                    P, rows = starts(read_depth(depth_files[0]), read_seg(segs[0]), cls)
                 P, rows = P.cpu().numpy(), rows.cpu().numpy()
                 for j, c in enumerate(cls):
                     if rows[j, 0]:
-                        raise _mask_start_refusal(seq_id, c, [k['name'] for k in classes if k['class_id'] == c][0], rows[j, 0])
+                        raise _mask_start_refusal(seq_id, c, [k['name'] for k in classes if k['class_id'] == c][0], rows[j, 0],
+                                                  initialize_method)
                 init_poses = P
             else:
                 init_poses = np.stack([_ycb_first_pose(ycb_dir, c, seq_id, files[c][2][0], initialize_method, keyframes_all,
@@ -2406,7 +2472,7 @@ def init_classes(ycb_dir, class_ids, class_config):
 INIT_ROWS = ('grid', 'icp', 'best of K')
 
 
-def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=None):
+def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=None, box=False, depths=None):
     """Starts from the masks scored on the YCB-Video key frames: no checkpoint, no tracking.  The frames are the key frames of
     ycbv_recover's loop (produce_train_pair_data.ycbv_keyframe_jobs: every key frame with an annotated requested class), each
     with its depth_filled and seg/ images; each is one Engine.init_poses call (MaskStarts) for all its annotated classes, label =
@@ -2414,13 +2480,19 @@ def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=Non
     (object_cloud), and se3tn_vocap_sets gives the per-class and pooled ADD / ADD-S AUCs.  Rows: 'grid' the top grid candidate,
     'icp' the returned pose, 'best of K' per row the kept candidate (after ICP when init has it) of lowest ADD-S, which bounds
     any final choice.  A row whose call reports status != 0 is counted as failed and not scored.  max_frames: the first key
-    frames only.
+    frames only.  box: each call is Engine.init_boxes (MaskStarts.from_boxes, D = depths, None the default) with each class's
+    tight box in the key frame's label image, a perfect detector's boxes; a class without pixels gets an empty box and counts
+    as failed.  depths without box is a ValueError.
 
     -> {class id: dict, ..., 'all': dict}; each dict: rows (scored), failed, gt (rows, 4, 4), and per row name of INIT_ROWS a
     dict of poses (rows, 4, 4), errors (rows, 4) (translation mm, rotation degrees, ADD m, ADD-S m) and summary
     (_recover_summary)."""
     from .produce_train_pair_data import ycbv_keyframe_jobs
     spec = Engine.init_spec(init)
+    if depths is not None and not box:
+        raise ValueError('initYcbKeyframes: depths needs box=True')
+    if box:
+        Engine.depths_spec(Engine.INIT_BOX_DEPTHS if depths is None else depths)
     classes = init_classes(ycb_dir, class_ids, class_config)
     ids = [k['class_id'] for k in classes]
     jobs = ycbv_keyframe_jobs(ycb_dir, ids)
@@ -2437,7 +2509,10 @@ def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=Non
             out = dict(kept_poses=torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev))
             if spec.icp:
                 out['icp_poses'] = torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev)
-            P, R = starts(read_depth(depth_path), read_seg(seg_path), cls, out=out)
+            if box:
+                P, R = starts.from_boxes(read_depth(depth_path), read_seg(seg_path), cls, depths, out=out)
+            else:
+                P, R = starts(read_depth(depth_path), read_seg(seg_path), cls, out=out)
             row_set += [set_of[c] for c in cls]
             gts += [B for _, B in rows]
             status.append(R[:, 0].clone())
@@ -2818,7 +2893,10 @@ def main(argv=None):
                         'start hypotheses per track (1..32, default 1) and keep the one whose model fits the frame best')
     parser.add_argument('--reinit_frames', type=str, default=None, help='comma-separated %%04d/%%06d frames to re-initialise from PoseCNN')
     parser.add_argument('--init', default='gt', help='gt / posecnn / poserbpf (the reference hard-codes gt); ycbv_all also mask: '
-                        'each sequence starts from Engine.init_poses on its first frame\'s depth and seg/ label image')
+                        'each sequence starts from Engine.init_poses on its first frame\'s depth and seg/ label image; ycbv_all and '
+                        'ycbv_init also box: Engine.init_boxes with each class\'s tight box in that label image')
+    parser.add_argument('--init_depths', type=int, default=None, help='--init box: depth candidates D along each box\'s ray (1..%d, '
+                        'default %d)' % (_engine.Engine.MAX_INIT_DEPTHS, _engine.Engine.INIT_BOX_DEPTHS))
     parser.add_argument('--init_viewpoints', type=int, default=None, help='--init mask / ycbv_init: grid viewpoints V (default %d)'
                         % _engine.Engine.INIT_DEFAULTS['viewpoints'])
     parser.add_argument('--init_inplane', type=int, default=None, help='--init mask / ycbv_init: in-plane angles R (default %d)'
@@ -3014,10 +3092,22 @@ def cli_init(args):
     a SystemExit."""
     flags = {'viewpoints': args.init_viewpoints, 'inplane': args.init_inplane, 'keep': args.init_keep, 'icp': args.init_icp}
     given = {k: v for k, v in flags.items() if v is not None}
+    depths = getattr(args, 'init_depths', None)
+    if args.init == 'box' and args.mode not in ('ycbv_all', 'ycbv_init'):
+        raise SystemExit('--init box needs --mode ycbv_all or ycbv_init, not --mode %s' % args.mode)
+    if depths is not None and args.init != 'box':
+        raise SystemExit('--init_depths needs --init box')
+    if args.init == 'box' and args.reinit_below is not None:
+        raise SystemExit('--init box with --reinit_below: restarts inside the one-pass driver come from masks only')
+    if depths is not None:
+        try:
+            _engine.Engine.depths_spec(depths)
+        except ValueError as e:
+            raise SystemExit('--init_depths: %s' % e)
     if args.init == 'mask' and args.mode != 'ycbv_all':
         raise SystemExit('--init mask needs --mode ycbv_all; --mode %s does not start from masks (--mode ycbv_init scores the '
                          'starts on the key frames)' % args.mode)
-    if given and args.mode != 'ycbv_init' and args.init != 'mask' and args.reinit_below is None:
+    if given and args.mode != 'ycbv_init' and args.init not in ('mask', 'box') and args.reinit_below is None:
         raise SystemExit('%s need --init mask (with --mode ycbv_all), --reinit_below or --mode ycbv_init'
                          % ', '.join('--init_' + k for k in given))
     spec = given or None
@@ -3065,13 +3155,16 @@ def _main_init(args, init):
             raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
     config = dict(train_data_path=args.train_data_path, model_path=args.model_path)
     try:
-        res = initYcbKeyframes(args.ycb_dir, class_ids, config, init=init, max_frames=args.max_frames)
+        box = dict(box=True, depths=getattr(args, 'init_depths', None)) if args.init == 'box' else {}
+        res = initYcbKeyframes(args.ycb_dir, class_ids, config, init=init, max_frames=args.max_frames, **box)
     except ValueError as e:
         raise SystemExit(str(e))
     names = ycb_class_names(args.ycb_dir)
     spec = _engine.Engine.init_spec(init)
-    print('ycbv_init: V %d, R %d, K %d, ICP %d, %s' % (spec.viewpoints, spec.inplane, spec.keep, spec.icp.contents.iterations if spec.icp else 0,
-                                                       torch.cuda.get_device_name(torch.cuda.current_device())))
+    print('ycbv_init: V %d, R %d, K %d, ICP %d, %s%s' % (spec.viewpoints, spec.inplane, spec.keep, spec.icp.contents.iterations if spec.icp else 0,
+                                                         torch.cuda.get_device_name(torch.cuda.current_device()),
+                                                         ', boxes from the labels, D %d' % (getattr(args, 'init_depths', None) or _engine.Engine.INIT_BOX_DEPTHS)
+                                                         if args.init == 'box' else ''))
     print_init_tables(res, {c: names[c - 1] for c in class_ids})
     return res
 
@@ -3124,8 +3217,10 @@ def _main_one_pass(args, precision=None, iterations=None):
                 class_ids = sorted(set(int(c) for c in args.class_ids.split(',')))
             except ValueError:
                 raise SystemExit('--class_ids must be comma-separated integers or all, not %r' % args.class_ids)
-        if args.init == 'mask':
+        if args.init in ('mask', 'box'):
             kw['init'] = getattr(args, 'init_spec', None)
+        if args.init == 'box' and getattr(args, 'init_depths', None) is not None:
+            kw['depths'] = args.init_depths
         if args.reinit_below is not None:
             kw['reinit'] = dict(below=args.reinit_below, init=getattr(args, 'init_spec', None),
                                 **({} if args.reinit_after is None else {'after': args.reinit_after}))

@@ -1,6 +1,7 @@
 """Small start-pose calls for compute-sanitizer (memcheck / racecheck): se3tn_init_poses on a 120 x 160 frame with three objects
 (one whose mask runs over the frame's edge, one without depth under its mask, one label absent), both render modes, with and
-without ICP, several chunks per call (max_batch 4), and every optional output.
+without ICP, several chunks per call (max_batch 4), and every optional output; then se3tn_init_boxes on the same frame with
+overlapping boxes, a box on the frame's corner, one without depth and an empty one, at D = 1 and 3.
 
     compute-sanitizer --tool memcheck python scripts/sanitize_init.py
 """
@@ -33,6 +34,21 @@ for mode in ('vispy', 'pyrender'):
                            icp_rows=torch.empty(n, 2, 8, dtype=torch.int32, device='cuda'),
                            icp_stats=torch.empty(n, 2, 4, dtype=torch.float64, device='cuda'))
             P, R = eng.init_poses(D, S, K, labels, ow, mode=mode, image_hw=(120, 160) if mode == 'pyrender' else None, init=init, out=out)
+boxes = np.array([[50, 30, 110, 90], [60, 40, 100, 80], [130, 0, 160, 30], [10, 90, 30, 110], [5, 5, 5, 50]], np.int32)
+for mode in ('vispy', 'pyrender'):
+    for icp in (None, 2):
+        for sel, nd in (([0, 1], 1), ([2, 3], 3), ([4, 0], 3)):          # overlapping; corner and no depth; empty
+            init = dict(viewpoints=3, inplane=2, keep=2, min_pixels=10, icp=icp)
+            out = dict(stats=torch.empty(n, 6, dtype=torch.int64, device='cuda'), t0=torch.empty(n, nd, 3, dtype=torch.float64, device='cuda'),
+                       cand_rows=torch.empty(n, 6 * nd, 8, dtype=torch.int32, device='cuda'),
+                       kept_rows=torch.empty(n, 2, 8, dtype=torch.int32, device='cuda'),
+                       kept_poses=torch.empty(n, 2, 4, 4, dtype=torch.float64, device='cuda'))
+            if icp:
+                out.update(icp_poses=torch.empty(n, 2, 4, 4, dtype=torch.float64, device='cuda'),
+                           icp_rows=torch.empty(n, 2, 8, dtype=torch.int32, device='cuda'),
+                           icp_stats=torch.empty(n, 2, 4, dtype=torch.float64, device='cuda'))
+            Pb, Rb = eng.init_boxes(D, boxes[sel], K, ow, mode=mode, image_hw=(120, 160) if mode == 'pyrender' else None, init=init,
+                                    depths=nd, out=out)
 torch.cuda.synchronize()
-print('ok', R.cpu().numpy().tolist())
+print('ok', R.cpu().numpy().tolist(), Rb.cpu().numpy().tolist())
 eng.close()
