@@ -1958,12 +1958,12 @@ int se3tn_crop_bbox_seg(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* 
 }  // extern "C"
 
 namespace {
-// The mesh ids of a visibility or pair call, checked on the host before anything is queued: both or neither of the host and device
-// copies, n within max_batch, a model for every id.
-int check_meshes(se3tn_ctx* c, const char* fn, const int32_t* ids_host, const int32_t* ids_dev, int n) {
+// The mesh ids of a visibility, pair, init or fit_poses call, checked on the host before anything is queued: both or neither of
+// the host and device copies (ids_name: the arguments' stem, mesh_ids or weight_ids), n within max_batch, a model for every id.
+int check_meshes(se3tn_ctx* c, const char* fn, const char* ids_name, const int32_t* ids_host, const int32_t* ids_dev, int n) {
     if ((ids_host == nullptr) != (ids_dev == nullptr))
-        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": mesh_ids_host and mesh_ids_dev must both be given or both NULL");
-    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": n exceeds max_batch");
+        return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": " + ids_name + "_host and " + ids_name + "_dev must both be given or both NULL");
+    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, std::string(fn) + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
     for (int i = 0; i < n; ++i) {
         const int id = ids_host ? ids_host[i] : 0;
         if (!c->meshes.count(id))
@@ -1982,7 +1982,7 @@ int se3tn_visibility(se3tn_ctx* c, const uint8_t* seg, int H, int W, const doubl
     if (!c) return SE3TN_ERR_INVALID;
     if (!seg || !K || !poses || !class_ids || !out_visible || !out_covered || H <= 0 || W <= 0 || H > 65536 || W > 65536)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_visibility: null argument or frame size out of range");
-    int rc = check_meshes(c, "se3tn_visibility", mesh_ids_host, mesh_ids_dev, m);
+    int rc = check_meshes(c, "se3tn_visibility", "mesh_ids", mesh_ids_host, mesh_ids_dev, m);
     if (rc) return rc;
     if (m == 0) return SE3TN_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -2015,7 +2015,7 @@ int se3tn_perturb_pairs(se3tn_ctx* c, const uint8_t* frame_rgb, const uint16_t* 
     if (!frame_rgb || !frame_depth || !seg || !K || !A_in_cam || !object_width || !class_ids || H <= 0 || W <= 0 || H > 65536 || W > 65536)
         return fail(c, SE3TN_ERR_INVALID, "se3tn_perturb_pairs: null argument or frame size out of range");
     if (!rgbA || !depthA || !rgbB || !depthB || !segB || !seg_count) return fail(c, SE3TN_ERR_INVALID, "se3tn_perturb_pairs: null output");
-    int rc = check_meshes(c, "se3tn_perturb_pairs", mesh_ids_host, mesh_ids_dev, n);
+    int rc = check_meshes(c, "se3tn_perturb_pairs", "mesh_ids", mesh_ids_host, mesh_ids_dev, n);
     if (rc) return rc;
     if (n == 0) return SE3TN_OK;
     DeviceGuard guard(c->device);
@@ -2619,12 +2619,12 @@ int init_run(se3tn_ctx* c, const char* fn, const uint16_t* frame_depth, int H, i
         static_cast<long long>(H) * W >= (1LL << 31))
         return fail(c, SE3TN_ERR_INVALID, f + ": null argument or frame size out of range (H x W must be below 2^31)");
     if (!poses_out || !out_rows) return fail(c, SE3TN_ERR_INVALID, f + ": null output");
-    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    int rc = check_meshes(c, fn, "weight_ids", weight_ids_host, weight_ids_dev, n);
+    if (rc) return rc;
     if (src.D < 1 || src.D > kInitMaxDepths)
         return fail(c, SE3TN_ERR_INVALID, f + ": depths is " + std::to_string(src.D) + ", not in [1, " + std::to_string(kInitMaxDepths) + "]");
     RenderSpec r;
-    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
+    if ((rc = render_spec(c, fn, render_mode, render_H, render_W, r))) return rc;
     Step st{};
     if ((rc = init_opts(c, fn, opts, n, src.D, st))) return rc;
     const se3tn_init_arrays a = arrays ? *arrays : se3tn_init_arrays{};
@@ -2632,14 +2632,8 @@ int init_run(se3tn_ctx* c, const char* fn, const uint16_t* frame_depth, int H, i
     const struct { const void* p; const char* name; } icp_only[] = {{a.icp_poses, "icp_poses"}, {a.icp_rows, "icp_rows"}, {a.icp_stats, "icp_stats"}};
     for (const auto& x : icp_only)
         if (x.p && !icp) return fail(c, SE3TN_ERR_INVALID, f + ": arrays->" + x.name + " is set, but opts->icp is NULL");
-    if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
-        return fail(c, SE3TN_ERR_INVALID, f + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
-    for (int i = 0; i < n; ++i) {
+    for (int i = 0; i < n; ++i)
         if ((rc = check_object(i))) return rc;
-        const int id = weight_ids_host ? weight_ids_host[i] : 0;
-        if (!c->meshes.count(id))
-            return fail(c, SE3TN_ERR_STATE, f + ": id " + std::to_string(id) + " (object " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
-    }
     const size_t nn = static_cast<size_t>(n), D = static_cast<size_t>(src.D), VR = static_cast<size_t>(opts->viewpoints) * opts->inplane;
     const size_t DVR = D * VR, Kk = opts->keep, nK = nn * Kk, px = static_cast<size_t>(H) * W;
     rc = check_disjoint(c, fn, {{poses_out, nn * 128}, {out_rows, nn * 4 * kInitCols}, {a.stats, nn * 8 * kInitStats}, {a.t0, nn * D * 24},
@@ -2826,19 +2820,12 @@ int se3tn_fit_poses(se3tn_ctx* c, const uint16_t* frame_depth, int H, int W, con
     if (!c) return SE3TN_ERR_INVALID;
     if (!frame_depth || !K || !poses || !object_width || !out_rows || H <= 0 || W <= 0)
         return fail(c, SE3TN_ERR_INVALID, f + ": null argument or empty frame");
-    if (n < 0 || n > c->max_batch) return fail(c, SE3TN_ERR_INVALID, f + ": n is " + std::to_string(n) + ", not in [0, max_batch]");
+    int rc = check_meshes(c, fn, "weight_ids", weight_ids_host, weight_ids_dev, n);
+    if (rc) return rc;
     if (fit_tau_mm < 1 || fit_tau_mm > 1000)
         return fail(c, SE3TN_ERR_INVALID, f + ": fit_tau_mm is " + std::to_string(fit_tau_mm) + ", not in [1, 1000]");
     RenderSpec r;
-    int rc = render_spec(c, fn, render_mode, render_H, render_W, r);
-    if (rc) return rc;
-    if ((weight_ids_host == nullptr) != (weight_ids_dev == nullptr))
-        return fail(c, SE3TN_ERR_INVALID, f + ": weight_ids_host and weight_ids_dev must both be given or both NULL");
-    for (int i = 0; i < n; ++i) {
-        const int id = weight_ids_host ? weight_ids_host[i] : 0;
-        if (!c->meshes.count(id))
-            return fail(c, SE3TN_ERR_STATE, f + ": id " + std::to_string(id) + " (pose " + std::to_string(i) + ") has no mesh (se3tn_set_mesh)");
-    }
+    if ((rc = render_spec(c, fn, render_mode, render_H, render_W, r))) return rc;
     const size_t nn = static_cast<size_t>(n);
     rc = check_disjoint(c, fn, {{out_rows, nn * 4 * kFitCols}},
                         {{frame_depth, static_cast<size_t>(H) * W * 2}, {poses, nn * 128}, {object_width, nn * 8}, {weight_ids_dev, nn * 4}},

@@ -491,7 +491,7 @@ class Engine:
     # init_spec's defaults: starting guesses, not tuned on a real sensor: 300 x 24 = 7,200 candidates about 12 x 15 degrees
     # apart, the 8 best refined by 5 ICP iterations at icp_spec's gate, a 20 mm inlier gate, at least 100 mask pixels with depth
     INIT_DEFAULTS = dict(viewpoints=300, inplane=24, keep=8, tau_mm=20, min_pixels=100, icp=5)
-    INIT_STATUS = {1: 'the mask is empty', 2: 'too few mask pixels have depth (min_pixels)'}
+    INIT_STATUS = {1: 'the {} is empty', 2: 'too few {} pixels have depth (min_pixels)'}
     INIT_ARRAYS = ('stats', 't0', 'cand_rows', 'kept_rows', 'kept_poses', 'icp_poses', 'icp_rows', 'icp_stats')
 
     @staticmethod
@@ -530,25 +530,26 @@ class Engine:
         of INIT_ARRAYS (include/se3tn.h's se3tn_init_arrays, shaped (n, ...)) as CUDA tensors to fill.  -> (poses float64 (n,4,4),
         all NaN for an object whose status is not 0, rows int32 (n, INIT_COLS): status, candidate, model, maskc, overlap, pairs,
         inlier, delta_mm), queued on the current stream."""
+        return self._init('init_poses', frame_depth, K, object_width, weight_ids, mode, image_hw, init, out, seg, labels, None)
+
+    @staticmethod
+    def init_status(status, source):
+        """The text of an init row's status (INIT_STATUS) for a start from a 'mask' or a 'box'."""
+        return Engine.INIT_STATUS.get(int(status), '?').format(source)
+
+    def _init(self, fn, frame_depth, K, object_width, weight_ids, mode, image_hw, init, out, seg, rows, D):
+        """init_poses' and init_boxes' checks and their one library call.  A start from a label image: seg, its labels as rows
+        and D None; from boxes: seg None, and the boxes as rows and D as box_spec gives them."""
         opts = self.init_spec(init)
-        lab = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
-        n = int(lab.shape[0])
         H, W = frame_depth.shape
         self._check_dev('frame_depth', frame_depth, torch.uint16, (H, W))
-        self._check_dev('seg', seg, torch.uint8, (H, W))
+        if D is None:
+            rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1)
+            self._check_dev('seg', seg, torch.uint8, (H, W))
+        n = int(rows.shape[0])
         self._check_dev('object_width', object_width, torch.float64, (n,))
-        wh = self._host_ids('init_poses', weight_ids, n)
+        wh = self._host_ids(fn, weight_ids, n)
         wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
-        out, arrays = self._init_outputs('init_poses', n, opts, None, out)
-        rmode, rH, rW = self._render_mode(mode, image_hw)
-        _lib.check(self.lib.se3tn_init_poses(self._ctx, _ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _hptr(lab),
-                                             _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
-                                             _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
-        return out['poses'], out['rows']
-
-    def _init_outputs(self, fn, n, opts, D, out):
-        """out (init_poses' / init_boxes' argument) checked against the shapes of n objects with D depths (None: a mask, t0
-        (n, 3)), 'poses' and 'rows' allocated when missing.  -> (out dict, _lib.InitArrays)."""
         out = dict(out or {})
         unknown = set(out) - {'poses', 'rows'} - set(self.INIT_ARRAYS)
         if unknown:
@@ -565,13 +566,18 @@ class Engine:
         for k, t in out.items():
             if t is not None:
                 self._check_dev('out[%r]' % k, t, shapes[k][1], shapes[k][0])
-        return out, _lib.InitArrays(**{k: _ptr(out.get(k)).value for k in self.INIT_ARRAYS})
+        arrays = _lib.InitArrays(**{k: _ptr(out.get(k)).value for k in self.INIT_ARRAYS})
+        rmode, rH, rW = self._render_mode(mode, image_hw)
+        call, src = (self.lib.se3tn_init_poses, (_ptr(frame_depth), _ptr(seg), int(H), int(W), _hptr(self._k4(K)), _hptr(rows))) \
+            if D is None else (self.lib.se3tn_init_boxes, (_ptr(frame_depth), int(H), int(W), _hptr(self._k4(K)), _hptr(rows), D))
+        _lib.check(call(self._ctx, *src, _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
+                        _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
+        return out['poses'], out['rows']
 
     # init_boxes' default depth count: a starting guess, like INIT_DEFAULTS -- the quantiles 1/8, 3/8, 5/8 and 7/8 of the box's
     # depths, so that one of them lies on the object when the background fills up to half of the box
     INIT_BOX_DEPTHS = 4
     MAX_INIT_DEPTHS = 8
-    INIT_BOX_STATUS = {1: 'the box is empty', 2: 'too few box pixels have depth (min_pixels)'}
 
     @staticmethod
     def depths_spec(depths):
@@ -616,25 +622,30 @@ class Engine:
         MAX_INIT_DEPTHS]; the rest as init_poses.  out as init_poses', with t0 (n, D, 3) and cand_rows (n, D V R, INIT_COLS);
         column 1 of a row is the candidate d V R + v R + r.  -> (poses float64 (n,4,4), NaN where the status is not 0 -- 1: the
         box is empty, 2: too few of its pixels have depth --, rows int32 (n, INIT_COLS)), queued on the current stream."""
-        opts = self.init_spec(init)
-        b, D = self.box_spec(boxes, depths)
-        n = int(b.shape[0])
-        H, W = frame_depth.shape
-        self._check_dev('frame_depth', frame_depth, torch.uint16, (H, W))
-        self._check_dev('object_width', object_width, torch.float64, (n,))
-        wh = self._host_ids('init_boxes', weight_ids, n)
-        wd = torch.from_numpy(wh).to(self.device) if wh is not None else None
-        out, arrays = self._init_outputs('init_boxes', n, opts, D, out)
-        rmode, rH, rW = self._render_mode(mode, image_hw)
-        _lib.check(self.lib.se3tn_init_boxes(self._ctx, _ptr(frame_depth), int(H), int(W), _hptr(self._k4(K)), _hptr(b), D,
-                                             _ptr(object_width), rmode, rH, rW, _hptr(wh), _ptr(wd), n, C.byref(opts), _ptr(out['poses']),
-                                             _ptr(out['rows']), C.byref(arrays), _stream(self.device)), self._ctx)
-        return out['poses'], out['rows']
+        return self._init('init_boxes', frame_depth, K, object_width, weight_ids, mode, image_hw, init, out, None, *self.box_spec(boxes, depths))
 
     # ------------------------------------------------------------------ re-initialisation of lost tracks
     # reinit_spec's defaults: guesses, not tuned -- `predict --fit --score` shows how well the inlier fraction separates lost
     # from kept tracks on a data set, which is what to choose them by
     REINIT_DEFAULTS = dict(below=0.5, after=3)
+
+    @staticmethod
+    def reinit_source(fn, n, seg=None, labels=None, boxes=None, depths=INIT_BOX_DEPTHS):
+        """reinit's seg (uint8, numpy or a tensor) with labels (n ints in 1..255), or boxes and depths, for n tracks, checked ->
+        _init's seg, rows and D, a row per track: (seg as given, labels, None), (None, boxes, D), or all None without either."""
+        if seg is not None and boxes is not None:
+            raise ValueError('%s: give seg / labels or boxes, not both' % fn)
+        lab = np.ascontiguousarray([] if labels is None else labels, dtype=np.int64).reshape(-1)
+        if (seg is not None or labels is not None) and (lab.shape != (n,) or (seg is not None and n and (lab.min() < 1 or lab.max() > 255))):
+            raise ValueError('%s: labels must be %d ints in 1..255, not %r' % (fn, n, labels))
+        if boxes is not None:
+            b, D = Engine.box_spec(boxes, depths)
+            if b.shape != (n, 4):
+                raise ValueError('%s: boxes must be (%d, 4), not %s' % (fn, n, b.shape))
+            return None, b, D
+        if seg is not None and seg.dtype not in (np.uint8, torch.uint8):
+            raise ValueError('%s: seg must be a uint8 label image, not %s' % (fn, seg.dtype))
+        return seg, (None if seg is None else lab), None
 
     @staticmethod
     def reinit_spec(below=0.5, after=3):
@@ -728,15 +739,7 @@ class Engine:
         if not tau:
             raise ValueError('reinit: fit must be the step\'s tau in mm, not %r' % (fit,))
         n = int(poses.shape[0])
-        if seg is not None and boxes is not None:
-            raise ValueError('reinit: give seg or boxes, not both')
-        if boxes is not None:
-            box, depths = self.box_spec(boxes, depths)
-            if box.shape != (n, 4):
-                raise ValueError('reinit: %d boxes for %d tracks' % (box.shape[0], n))
-        lab = None if boxes is not None and labels is None else np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
-        if lab is not None and lab.shape != (n,):
-            raise ValueError('reinit: %d labels for %d tracks' % (lab.shape[0], n))
+        seg, rows, D = self.reinit_source('reinit', n, seg, labels, boxes, depths)
         wh = self._host_ids('reinit', weight_ids, n)
         event, lost = self.lost_tracks(fit_rows, streak, below, after)
         pin = getattr(self, '_reinit_pin', None)
@@ -745,7 +748,7 @@ class Engine:
         pin[:n + 1].copy_(lost, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
         m = int(pin[0])
-        if m == 0 or (seg is None and boxes is None):
+        if m == 0 or rows is None:
             return event
         idx = pin[1:1 + m].numpy().copy()
         as_dev = lambda a, dt: a.to(self.device, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
@@ -755,12 +758,8 @@ class Engine:
             depth_d = self.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
         sub_ids = None if wh is None else wh[idx]
         width = object_width.index_select(0, lost[1:1 + m].long())
-        if boxes is not None:
-            starts, init_rows = self.init_boxes(depth_d, box[idx], K, width, weight_ids=sub_ids, mode=mode, image_hw=image_hw, init=init,
-                                                depths=depths)
-        else:
-            starts, init_rows = self.init_poses(depth_d, as_dev(seg, torch.uint8), K, lab[idx], width, weight_ids=sub_ids, mode=mode,
-                                                image_hw=image_hw, init=init)
+        starts, init_rows = self._init('reinit', depth_d, K, width, sub_ids, mode, image_hw, init, None,
+                                       None if seg is None else as_dev(seg, torch.uint8), rows[idx], D)
         start_fit = self.fit_poses(depth_d, K, starts, width, tau, weight_ids=sub_ids, mode=mode, image_hw=image_hw)
         self.accept_starts(idx, starts, init_rows, start_fit, poses, fit_rows, streak, event)
         return event

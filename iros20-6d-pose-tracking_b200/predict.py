@@ -405,61 +405,58 @@ class Tracker:
         dev = self.engine.device
         as_dev = lambda a, dt: a.to(dev, dt).contiguous() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
         depth_d = as_dev(depth, np.uint16 if not torch.is_tensor(depth) else torch.uint16)
-        if box is not None:
-            b = Engine.box_pixels(box, *depth_d.shape)
-            Engine.depths_spec(depths)
-        else:
-            m = mask if torch.is_tensor(mask) else np.asarray(mask)
-            if torch.is_tensor(m) and m.dtype == torch.bool:
-                seg = m.to(dev).to(torch.uint8).contiguous() * int(label)
-            elif not torch.is_tensor(m) and m.dtype == np.bool_:
-                seg = torch.from_numpy(np.where(m, np.uint8(label), np.uint8(0))).to(dev)
-            else:
-                size = m.numel() if torch.is_tensor(m) else m.size
-                lo, hi = (int(m.min()), int(m.max())) if size else (0, 0)
-                if lo < 0 or hi > 255:
-                    raise ValueError('initialize: a label image holds labels 0..255, not %d..%d' % (lo, hi))
-                seg = as_dev(m, np.uint8 if not torch.is_tensor(m) else torch.uint8)
-            if tuple(seg.shape) != tuple(depth_d.shape):
-                raise ValueError('initialize: mask %s and depth %s differ in shape' % (tuple(seg.shape), tuple(depth_d.shape)))
+        seg, labels, boxes = self._object_pixels('initialize', mask, label, box, *depth_d.shape)
         on, max_depth, extrapolate, blur = Engine.depth_fill_spec(self.fill_depth)
         if on:
             depth_d = self.engine.fill_depth(depth_d, max_depth, extrapolate=bool(extrapolate), blur_type='gaussian' if blur else 'bilateral')
         width = torch.full((1,), float(self.object_width), dtype=torch.float64, device=dev)
         common = dict(weight_ids=None if r.mesh_id == 0 else [r.mesh_id], mode=r.mode, image_hw=r.image_hw, init=init or None)
-        if box is not None:
-            poses, rows = self.engine.init_boxes(depth_d, b[None], self.K, width, depths=depths, **common)
+        if boxes is None:
+            poses, rows = self.engine.init_poses(depth_d, as_dev(seg, seg.dtype), self.K, labels, width, **common)
         else:
-            poses, rows = self.engine.init_poses(depth_d, seg, self.K, [int(label)], width, **common)
+            poses, rows = self.engine.init_boxes(depth_d, boxes, self.K, width, depths=depths, **common)
         self.last_init = rows[0].cpu().numpy()
         status = int(self.last_init[0])
         if status:
-            if box is not None:
-                raise ValueError('initialize: no start for box %s: %s (status %d)' % (tuple(int(x) for x in b),
-                                 Engine.INIT_BOX_STATUS.get(status, '?'), status))
-            raise ValueError('initialize: no start for label %d: %s (status %d)' % (label, Engine.INIT_STATUS.get(status, '?'), status))
+            what, source = ('label %d' % label, 'mask') if boxes is None else ('box %s' % (tuple(int(x) for x in boxes[0]),), 'box')
+            raise ValueError('initialize: no start for %s: %s (status %d)' % (what, Engine.init_status(status, source), status))
         return poses[0].cpu().numpy()
+
+    @staticmethod
+    def _object_pixels(fn, mask, label, box, H, W):
+        """One object's pixels in an H x W frame as on_track_batch's seg, labels and boxes, nothing copied to the device: mask, a
+        bool (H,W) mask or an integer label image with labels 0..255 (numpy or a tensor), as a uint8 label image in which the
+        object is `label`; box, a detector's (x0, y0, x1, y1) as Engine.box_pixels rounds and clips it; neither, all None."""
+        if mask is not None and box is not None:
+            raise ValueError('%s: give mask or box, not both' % fn)
+        if mask is None:
+            return None, None, (None if box is None else Engine.box_pixels(box, H, W)[None])
+        m = mask if torch.is_tensor(mask) else np.asarray(mask)
+        if torch.is_tensor(m) and m.dtype == torch.bool:
+            seg = m.to(torch.uint8) * int(label)
+        elif not torch.is_tensor(m) and m.dtype == np.bool_:
+            seg = np.where(m, np.uint8(label), np.uint8(0))
+        else:
+            lo, hi = (int(m.min()), int(m.max())) if (m.numel() if torch.is_tensor(m) else m.size) else (0, 0)
+            if lo < 0 or hi > 255:
+                raise ValueError('%s: mask must be a bool mask or a uint8 label image (any integer type, labels 0..255), not %s '
+                                 'with labels %d..%d' % (fn, m.dtype, lo, hi))
+            seg = m.to(torch.uint8) if torch.is_tensor(m) else m.astype(np.uint8, copy=False)
+        if tuple(seg.shape) != (H, W):
+            raise ValueError('%s: mask %s and depth %s differ in shape' % (fn, tuple(seg.shape), (H, W)))
+        return seg, [int(label)], None
 
     # ------------------------------------------------------------------ the hot path
     def on_track(self, prev_pose, current_rgb, current_depth, gt_A_in_cam=None, gt_B_in_cam=None, debug=False, samples=1,
                  rgbA=None, depthA=None, show=False, mask=None, label=1, box=None):
         """One frame, one object (reference predict.py:217-296) -> new 4x4 float64 pose.  Without rgbA / depthA and with the
         CUDA rasteriser, input A is rendered inside the tracking step itself (se3tn_track_render_host), and refined
-        Tracker.iterations times.  mask: with reinit, the object's pixels of this frame, a bool (H,W) array or a uint8 label
-        image in which they are `label`; read only when the track is lost.  box: with reinit, instead of mask, the object's
+        Tracker.iterations times.  mask: with reinit, the object's pixels of this frame, a bool (H,W) array or a label image
+        in which they are `label`, as Tracker.initialize takes them; read only when the track is lost.  box: with reinit, instead of mask, the object's
         (x0, y0, x1, y1) box in this frame (Tracker.initialize's rounding): a lost track restarts from it (Engine.init_boxes)."""
         A_in_cam = _as_numpy_pose(prev_pose).copy()
-        if mask is not None and box is not None:
-            raise ValueError('on_track: give mask or box, not both')
-        seg = None
-        if mask is not None:
-            m = mask.cpu().numpy() if torch.is_tensor(mask) else np.asarray(mask)
-            if m.dtype not in (np.bool_, np.uint8):
-                raise ValueError('on_track: mask must be a bool mask or a uint8 label image, not %s' % m.dtype)
-            seg = np.where(m, np.uint8(label), np.uint8(0)) if m.dtype == np.bool_ else m
-        kw = {} if self.reinit is None else dict(seg=seg, labels=[int(label)])
-        if self.reinit is not None and box is not None:
-            kw = dict(boxes=Engine.box_pixels(box, *np.shape(current_depth)[:2])[None])
+        seg, labels, boxes = self._object_pixels('on_track', mask, label, box, *np.shape(current_depth)[:2])
+        kw = dict(seg=seg, labels=labels, boxes=boxes)                 # read by on_track_batch only with reinit
         fused = (rgbA is None or depthA is None) and self._fused_renderer(renderer_width=True) is not None
         if not fused:
             self._check_step_draws(rgbA is not None or depthA is not None)
@@ -504,31 +501,20 @@ class Tracker:
         if self.reinit is None:
             return self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
         n = len(prev_poses)
-        if boxes is not None:
-            if seg is not None or labels is not None:
-                raise ValueError('on_track_batch: give seg / labels or boxes, not both')
-            box, _ = Engine.box_spec(boxes, Engine.INIT_BOX_DEPTHS)
-            if box.shape != (n, 4):
-                raise ValueError('on_track_batch: boxes must be (%d, 4), not %s' % (n, box.shape))
-        if labels is None and seg is not None and n != 1:
-            raise ValueError('on_track_batch: seg needs labels, one per track')
-        lab = np.ascontiguousarray([1] * n if labels is None else labels, dtype=np.int64).reshape(-1)
-        if lab.shape != (n,) or (seg is not None and (lab.min() < 1 or lab.max() > 255)):
-            raise ValueError('on_track_batch: labels must be %d ints in 1..255, not %r' % (n, labels))
-        if seg is not None and seg.dtype not in (np.uint8, torch.uint8):
-            raise ValueError('on_track_batch: seg must be a uint8 label image, not %s' % seg.dtype)
+        labels = [1] if labels is None and n == 1 else labels
+        Engine.reinit_source('on_track_batch', n, seg, labels, boxes)
         if n * reinit_keep(self.opts) > self.engine.max_batch:     # checked before the step, which would update the streaks
             raise ValueError('reinit: %d tracks x init keep=%d exceed the engine\'s max_batch=%d'
                              % (n, reinit_keep(self.opts), self.engine.max_batch))
         self.last_reinit = None
         out = self._track_step(prev_poses, current_rgb, current_depth, rgbA, depthA, weight_ids, object_width)
-        return self._reinit(out, current_depth, seg, lab, weight_ids, object_width, None if boxes is None else box)
+        return self._reinit(out, current_depth, seg, labels, boxes, weight_ids, object_width)
 
     def reset_reinit(self):
         """Start every track's streak of frames below the fit threshold from 0 (reinit), as at a new sequence."""
         self._streak = None
 
-    def _reinit(self, out, depth, seg, labels, weight_ids, object_width, boxes=None):
+    def _reinit(self, out, depth, seg, labels, boxes, weight_ids, object_width):
         """Engine.reinit after the step that gave `out` (a CUDA tensor, updated in place, or numpy, uploaded and brought back)
         and last_fit, on the raw frame depth (filled as the step fills it), with the step's meshes, widths and render mode."""
         dev, n = self.engine.device, len(out)
@@ -1847,26 +1833,20 @@ class MaskStarts:
         self.render = dict(mode='pyrender', image_hw=(int(cam['height']), int(cam['width']))) if _pyrender(classes[0]) else \
             dict(mode='vispy', image_hw=None)
 
-    def __call__(self, depth, seg, cls, out=None):
+    def __call__(self, depth, seg, cls, box=False, depths=None, out=None):
         """One init call for the classes cls (labels = ids = class ids) of one frame (uint16 depth, uint8 seg, numpy or CUDA) ->
-        (poses (n, 4, 4), rows (n, INIT_COLS)) CUDA tensors, and out filled (Engine.init_poses)."""
+        (poses (n, 4, 4), rows (n, INIT_COLS)) CUDA tensors, and out filled: Engine.init_poses, or with box Engine.init_boxes
+        (D = depths, None: Engine.INIT_BOX_DEPTHS) on each class's tight box in seg (label_boxes: what a perfect detector
+        gives; no pixels, an empty box and status 1)."""
         dev = self.eng.device
         as_dev = lambda a: a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a)).to(dev)
         ids = np.asarray(cls, dtype=np.int32)
         widths = torch.tensor([self.width[int(c)] for c in cls], dtype=torch.float64, device=dev)
-        return self.eng.init_poses(as_dev(depth), as_dev(seg), self.K, ids, widths, weight_ids=ids, init=self.init, out=out, **self.render)
-
-    def from_boxes(self, depth, seg, cls, depths=None, out=None):
-        """One init_boxes call for the classes cls of one frame, each class's box the tight box of its pixels in the uint8
-        label image seg (label_boxes: what a perfect detector gives; no pixels, an empty box and status 1) -> as __call__
-        (Engine.init_boxes with `depths`, None: Engine.INIT_BOX_DEPTHS)."""
-        dev = self.eng.device
-        ids = np.asarray(cls, dtype=np.int32)
-        widths = torch.tensor([self.width[int(c)] for c in cls], dtype=torch.float64, device=dev)
-        seg = seg.cpu().numpy() if torch.is_tensor(seg) else np.asarray(seg)
-        depth = depth if torch.is_tensor(depth) else torch.from_numpy(np.ascontiguousarray(depth)).to(dev)
-        return self.eng.init_boxes(depth, label_boxes(seg, cls), self.K, widths, weight_ids=ids, init=self.init, out=out,
-                                   depths=Engine.INIT_BOX_DEPTHS if depths is None else depths, **self.render)
+        kw = dict(weight_ids=ids, init=self.init, out=out, **self.render)
+        if box:
+            boxes = label_boxes(seg.cpu().numpy() if torch.is_tensor(seg) else seg, cls)
+            return self.eng.init_boxes(as_dev(depth), boxes, self.K, widths, depths=Engine.INIT_BOX_DEPTHS if depths is None else depths, **kw)
+        return self.eng.init_poses(as_dev(depth), as_dev(seg), self.K, ids, widths, **kw)
 
     def close(self):
         self.eng.close()
@@ -1887,8 +1867,7 @@ def label_boxes(seg, labels):
 
 def _mask_start_refusal(seq, c, name, status, source='mask'):
     return ValueError('sequence %04d, class %d (%s): no start from its %s in the first frame: %s (status %d)'
-                      % (seq, c, name, source, (Engine.INIT_BOX_STATUS if source == 'box' else Engine.INIT_STATUS).get(int(status), '?'),
-                         int(status)))
+                      % (seq, c, name, source, Engine.init_status(status, source), int(status)))
 
 
 def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method='gt', precision='bf16x3', max_frames=None,
@@ -1999,10 +1978,7 @@ def getResultsYcbAll(ycb_dir, class_ids, class_config, outdir, initialize_method
                 segs = sorted(glob.glob(os.path.join(data_dir, '%04d' % seq_id, 'seg', '*')))
                 if not segs:
                     raise FileNotFoundError('--init %s: no seg/ label image under %s' % (initialize_method, os.path.join(data_dir, '%04d' % seq_id)))
-                if initialize_method == 'box':
-                    P, rows = starts.from_boxes(read_depth(depth_files[0]), read_seg(segs[0]), cls, depths)
-                else:
-                    P, rows = starts(read_depth(depth_files[0]), read_seg(segs[0]), cls)
+                P, rows = starts(read_depth(depth_files[0]), read_seg(segs[0]), cls, initialize_method == 'box', depths)
                 P, rows = P.cpu().numpy(), rows.cpu().numpy()
                 for j, c in enumerate(cls):
                     if rows[j, 0]:
@@ -2480,7 +2456,7 @@ def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=Non
     (object_cloud), and se3tn_vocap_sets gives the per-class and pooled ADD / ADD-S AUCs.  Rows: 'grid' the top grid candidate,
     'icp' the returned pose, 'best of K' per row the kept candidate (after ICP when init has it) of lowest ADD-S, which bounds
     any final choice.  A row whose call reports status != 0 is counted as failed and not scored.  max_frames: the first key
-    frames only.  box: each call is Engine.init_boxes (MaskStarts.from_boxes, D = depths, None the default) with each class's
+    frames only.  box: each call is Engine.init_boxes (MaskStarts with box, D = depths, None the default) with each class's
     tight box in the key frame's label image, a perfect detector's boxes; a class without pixels gets an empty box and counts
     as failed.  depths without box is a ValueError.
 
@@ -2509,10 +2485,7 @@ def initYcbKeyframes(ycb_dir, class_ids, class_config, init=None, max_frames=Non
             out = dict(kept_poses=torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev))
             if spec.icp:
                 out['icp_poses'] = torch.empty((n, Kk, 4, 4), dtype=torch.float64, device=dev)
-            if box:
-                P, R = starts.from_boxes(read_depth(depth_path), read_seg(seg_path), cls, depths, out=out)
-            else:
-                P, R = starts(read_depth(depth_path), read_seg(seg_path), cls, out=out)
+            P, R = starts(read_depth(depth_path), read_seg(seg_path), cls, box, depths, out=out)
             row_set += [set_of[c] for c in cls]
             gts += [B for _, B in rows]
             status.append(R[:, 0].clone())

@@ -338,6 +338,9 @@ def test_tracker_refuses_masks_and_engines_it_cannot_use(pkg, synth, jump, tmp_p
         trk.on_track_batch(gts.copy(), rgb, D, seg=S.astype(np.int32), labels=[1, 2])
     pose = trk.on_track(gts[1], rgb, D, mask=S == 2)              # a bool mask: the object's pixels under label 1
     assert trk.last_reinit[0] == R.RESTARTED and np.isfinite(pose).all()
+    pose = trk.on_track(gts[1], rgb, D, mask=S, label=2)          # a uint8 label image, then its int32 copy: the same restart
+    assert trk.last_reinit[0] == R.RESTARTED
+    assert np.array_equal(trk.on_track(gts[1], rgb, D, mask=S.astype(np.int32), label=2), pose) and trk.last_reinit[0] == R.RESTARTED
     # a shared Engine must hold n x init keep tracks: refused before the step, so the streaks do not move
     small = pkg.Engine(max_batch=8)
     try:
